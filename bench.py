@@ -1,8 +1,10 @@
 #!/usr/bin/env python
-"""bench.py — registrations/sec of the TEASER++ solve() hot path on B200 (BASELINE.json metric).
+"""bench.py — registrations/sec of the TEASER++ solve() hot path on H100 (BASELINE.json metric).
 
     python bench.py --gpus N --steps K --warmup W [--config C2]   # this repo's CUDA path
     python bench.py --impl reference --gpus N --steps K ...         # the reference algorithm on the host cores
+    --dump-outputs DIR   after the timed steps, write what the last timed step computed (rotation, translation,
+                         scale, clique sizes and clique index sets of every problem) as DIR/<name>.npy
 
 --config selects one of the BASELINE.json configurations (SURVEY §8d); the default, C2, is the one the metric is
 quoted on.  All use fixed scale (what every reference example uses) unless --estimate-scaling is given.
@@ -62,7 +64,7 @@ def bytes_graph(n):
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons during the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks / throttle reasons during the timed region (read-only queries)."""
 
     def __init__(self, index):
         self.index = index
@@ -216,6 +218,28 @@ def run_reference(args, rank, world):
     print(json.dumps(line), flush=True)
 
 
+def dump_outputs(out_dir, capi, sol_d, clq_d, B, budget=48 << 20):
+    """What tzr_solve_batch_dev handed back in the last timed step, per problem: the pose and scale (float64) and the
+    maximum clique (float32 indices, exact below 2^24; rows cut to the largest clique and padded with -1).  If the
+    cliques exceed `budget` bytes, a fixed seeded sample of problems is kept; clique_problem.npy lists which."""
+    import torch
+    os.makedirs(out_dir, exist_ok=True)
+    sols = np.frombuffer(sol_d.cpu().numpy().tobytes(), dtype=capi.SOLUTION_DTYPE)[:B]
+    size = sols["clique_size"].astype(np.int64)
+    width = max(int(size.max()), 1)
+    rows = np.arange(B)
+    if B * width * 4 > budget:
+        rows = np.sort(np.random.default_rng(0).choice(B, size=max(1, budget // (width * 4)), replace=False))
+    clq = clq_d[torch.as_tensor(rows, device=clq_d.device), :width].cpu().numpy().astype(np.float32)
+    clq[np.arange(width)[None, :] >= size[rows][:, None]] = -1.0
+    out = {"rotation": sols["rotation"].reshape(B, 3, 3).transpose(0, 2, 1),  # column-major record -> R[b] row-major
+           "translation": sols["translation"], "scale": sols["scale"], "valid": sols["valid"], "clique_size": size}
+    for name, arr in out.items():
+        np.save(os.path.join(out_dir, f"{name}.npy"), np.ascontiguousarray(arr, dtype=np.float64))
+    np.save(os.path.join(out_dir, "clique.npy"), clq)
+    np.save(os.path.join(out_dir, "clique_problem.npy"), rows.astype(np.float64))
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--gpus", type=int, default=1)
@@ -228,6 +252,8 @@ def main():
     ap.add_argument("--ref-problems-per-step", type=int, default=2)
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--parity-problems", type=int, default=16)
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the outputs of the last timed step as DIR/<name>.npy (float64; rank 0)")
     args = ap.parse_args()
     if CONFIGS[args.config].get("estimate_scaling"):
         args.estimate_scaling = True
@@ -242,7 +268,7 @@ def main():
     import torch
     import torch.distributed as dist
     if not torch.cuda.is_available():
-        raise SystemExit("bench.py: no CUDA device — the B200 path has no CPU fallback")
+        raise SystemExit("bench.py: no CUDA device — the GPU path has no CPU fallback")
     torch.cuda.set_device(local_rank)
     use_dist = world > 1
     if use_dist:
@@ -283,7 +309,7 @@ def main():
     ctx.set_flags(base_flags)
     stream = torch.cuda.Stream()
     ctx.set_stream(stream.cuda_stream)
-    # L2 flush between steps for working sets that would otherwise sit in the 126 MB L2
+    # L2 flush between steps for working sets that would otherwise sit in the 50 MB L2
     step_bytes = B * (48 * n + n * ((n + 127) // 128) * 16)
     flush = None
     if step_bytes < 512e6:
@@ -338,6 +364,8 @@ def main():
         ev_end.record(stream)
         ev_end.synchronize()
         t_dev = ev_begin.elapsed_time(ev_end)
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, capi, sol_d, clq_d, B)
     stage_sum, n_calls = ctx.stage_log_read()
     ctx.stage_log(False)
     barrier()
@@ -392,22 +420,19 @@ def main():
         value = global_batch * K / (t_dev_max * 1e-3)
         e2e = global_batch * K / (t_e2e_max * 1e-3)
         e2e_pg = global_batch * K / (t_pg_max * 1e-3)
+        # optional, not in git: {"hbm_gbs": <copy bandwidth measured on this machine>}
         peaks = {}
         try:
-            peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
-        except Exception:
+            with open(os.path.join(ROOT, "MEASURED_PEAKS.json")) as fh:
+                peaks = json.load(fh)
+        except (OSError, ValueError):
             pass
-        peak = float(peaks.get("hbm_gbs", 6650.0))
-        peak_kind = "measured (MEASURED_PEAKS.json hbm_gbs)" if "hbm_gbs" in peaks else "fallback 6.65 TB/s"
+        if isinstance(peaks, dict) and float(peaks.get("hbm_gbs") or 0) > 0:
+            peak, peak_kind = float(peaks["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
+        else:
+            peak, peak_kind = 3350.0, "H100 SXM data sheet HBM3 bandwidth (not a measured peak)"
         g_ms = stage_sum["graph"] / max(n_calls, 1)   # graph stage per step (operand tiles + graph kernels), CUDA events
         achieved = bytes_graph(n) * B / (g_ms * 1e-3) / 1e9
-        traffic = None
-        try:  # measured once with `ncu --set full`, scaled to this launch's batch
-            prof = json.load(open(os.path.join(ROOT, "profiles", "graph_kernel_traffic.json")))
-            if prof.get("n") == n:
-                traffic = prof.get("dram_bytes_per_problem") * B
-        except Exception:
-            pass
         kern = ("graph_tc_kernel (+ tc_prep_kernel, tc_patch_kernel)" if base_flags & 1024 else
                 "graph_strip3_kernel (+ tc_patch_kernel)" if base_flags & 2048 else "graph_strip2_kernel")
         line = {
@@ -419,7 +444,7 @@ def main():
                                             f"; {'total batch ' + str(global_batch) + ' sharded b mod G' if strong else 'batch ' + str(B) + ' problems/step/GPU'}"),
                 "name": cfg, "global_batch": global_batch,
                 "parallelism": f"batch sharded over {world} GPU(s), no collective",
-                "l2": (f"inputs larger than L2: {step_bytes / 1e6:.0f} MB of points + adjacency per step (L2 = 126 MB); no flush"
+                "l2": (f"inputs larger than L2: {step_bytes / 1e6:.0f} MB of points + adjacency per step (L2 = 50 MB); no flush"
                        if flush is None else
                        f"working set {step_bytes / 1e6:.0f} MB per step: 256 MB L2 flush between steps (its {t_flush / K:.3f} ms "
                        f"per step is subtracted from ms_per_step)"),
@@ -439,11 +464,11 @@ def main():
             "clocks": clocks,
             "roofline": {"bound": "hbm", "kernel": kern,
                          "achieved": achieved, "peak": peak,
-                         "unit": "GB/s", "frac": achieved / peak, "traffic": traffic, "peak_kind": peak_kind,
+                         "unit": "GB/s", "frac": achieved / peak, "peak_kind": peak_kind,
                          "algorithmic_bytes_per_launch": bytes_graph(n) * B, "kernel_ms": g_ms,
                          "note": "graph stage = O(N^2) pair classification; SURVEY §8d defines its roofline against HBM "
                                  "(algorithmic bytes: points in, packed bitset + degrees out).  The binding resource is "
-                                 "the per-pair arithmetic (issue 78 %, XU 64 %, FMA pipe 58 % in the ncu capture), not DRAM"},
+                                 "the per-pair arithmetic, not DRAM"},
             "stage_ms_per_step": {k_: v / max(n_calls, 1) for k_, v in stage_sum.items()},
             "counters": {"graph_exact_rechecks_per_problem": counters["filter_rechecks"] / B,
                          "clique_search_nodes_per_problem": counters["clique_nodes"] / B},

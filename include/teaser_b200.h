@@ -1,5 +1,5 @@
 /*
- * teaser_b200.h — C-ABI of the B200-native TEASER++ registration hot path.
+ * teaser_b200.h — C-ABI of the GPU-native TEASER++ registration hot path.
  *
  * This is the drop-in boundary: plain C, caller-owned buffers, no STL / Eigen / torch types.
  * The reference has no FFI layer of its own (SURVEY.md §8b); each entry point below names the
@@ -265,9 +265,9 @@ int tzr_solve_batch_multi(const int32_t* devices, int n_devices, const tzr_param
 /* Debug/verification switches: bit 0 (1) = force the pure-FP64 graph predicate (no FP32 filter),
  * bit 1 (2) = verify the FP32 / tensor-core filter against FP64 for every pair and count mismatches,
  * bit 2 (4) = count exact re-checks and clique search nodes, bit 8 (256) = degrees by a separate pass,
- * bit 10 (1024) = build the graph with the tensor-core kernel (tcgen05 Gram norms; bit-identical, measured slower than
- * the default CUDA-core kernel on B200: DESIGN.md 3.1), bit 9 (512) overrides it, bit 11 (2048) = the one-MUFU
- * CUDA-core variant (graph_strip3_kernel; bit-identical, FMA-pipe bound, 8 % slower), bit 13 (8192) = exact clique
+ * bit 10 (1024) = build the graph with the tensor-core kernel (wgmma Gram norms; bit-identical to the default CUDA-core
+ * kernel: DESIGN.md 3.1), bit 9 (512) overrides it, bit 11 (2048) = the one-MUFU
+ * CUDA-core variant (graph_strip3_kernel; bit-identical), bit 13 (8192) = exact clique
  * search without the singleton-class path of the colouring (A/B), bit 12 (4096) = without the block colour bound (only
  * present in builds with -DTZR_BLOCK_BOUND). */
 int tzr_ctx_set_flags(tzr_ctx* ctx, uint32_t flags);

@@ -1,7 +1,7 @@
 // TEST INFRASTRUCTURE ONLY — CPU restatement of teaser::FPFHEstimation::computeFPFHFeatures
 // (reference: teaser/src/fpfh.cc:15-43), which is a thin wrapper over PCL: NormalEstimationOMP with a radius search,
 // then FPFHEstimationOMP with a (larger) radius search on the same KD-tree.  PCL is a system dependency of the
-// reference (find_package(PCL 1.8), CMakeLists.txt) and is absent from this image and from /root/reference, so the
+// reference (find_package(PCL 1.8), CMakeLists.txt) and is not part of the reference tree, so the
 // algorithm below restates PCL's published sources (pcl/features/impl/normal_3d.hpp, feature.hpp
 // solvePlaneParameters, common/impl/centroid.hpp computeMeanAndCovarianceMatrix, common/impl/eigen.hpp
 // computeRoots/eigen33, features/src/pfh_tools.cpp computePairFeatures, features/impl/fpfh.hpp

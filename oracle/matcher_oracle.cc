@@ -4,7 +4,7 @@
 //
 // PARITY STATUS: **unpinned**.  The reference's two matcher tests (test/teaser/matcher-test.cc:17-78) feed FPFH
 // descriptors computed by PCL, and the nearest-neighbour search is FLANN's KDTreeSingleIndex (flann 1.9.x, a system
-// package the reference finds with find_package; neither PCL nor FLANN is in this image or in /root/reference).
+// package the reference finds with find_package; neither PCL nor FLANN is part of the reference tree).
 // What is restated here:
 //   * normalizePoints (matcher.cc:55-113): float arithmetic, sequential accumulation in index order;
 //   * advancedMatching (matcher.cc:114-297): larger cloud becomes "i"; NN of every j in the i-features; the reverse

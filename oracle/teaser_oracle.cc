@@ -6,21 +6,21 @@
 // this file.  The product path (teaser-plusplus_b200/csrc) never links, includes or
 // calls anything in oracle/.
 //
-// Parity status: the true reference cannot be compiled in this environment (Eigen, PMC,
-// tinyply are absent, no network).  This restatement is pinned against the reference's
-// own golden vectors (tests/golden/, copied data files from /root/reference/test/...):
+// Parity status: the true reference is not built alongside this project (it needs Eigen, PMC
+// and tinyply, fetched at configure time).  This restatement is pinned against the reference's
+// own golden vectors (tests/golden/, data files copied from the reference's test/...):
 // tls-test KATs, translation-solver KAT, rotation-solver KAT, scale-solver KATs, the
 // six benchmark_* end-to-end fixtures and the PMC toy graphs (tests/test_oracle_*.py).
 // The max-clique stage replaces the un-vendored, un-pinned PMC library
 // (https://github.com/jingnanshi/pmc.git, fetched at configure time with no tag by
-// /root/reference/teaser/CMakeLists.txt:6-8) by an own exact branch-and-bound that
+// the reference's teaser/CMakeLists.txt:6-8) by an own exact branch-and-bound that
 // follows PMC's published structure (k-core bound -> greedy heuristic -> k-core pruning
 // -> greedy-colouring branch and bound).  Its result is a *mathematically* maximum
 // clique; it equals PMC's answer as an index set whenever the maximum clique is unique.
 // At benchmark scale the reference's tests do not pin the clique: "parity unpinned" there.
 //
 // Every function cites the reference file:line it restates (paths relative to
-// /root/reference/).  Build: see oracle/Makefile
+// the reference repository).  Build: see oracle/Makefile
 //   g++ -O3 -DNDEBUG -fopenmp -ffp-contract=off  (mirrors the reference's Release flags,
 //   CMakeLists.txt:11-15; no -march=native => no FMA contraction, SURVEY Q6).
 // =============================================================================

@@ -1,4 +1,4 @@
-"""Exercise every kernel once on small inputs (meant to run under compute-sanitizer on the GPU box)."""
+"""Exercise every kernel once on small inputs (meant to run under compute-sanitizer)."""
 import importlib
 import os
 import sys
@@ -76,7 +76,7 @@ if "--no-cert" not in sys.argv:  # cuSOLVER's own kernels are slow under the san
     Wd = ctx.certifier_dual_projection(M0, th)
     r = ctx.certify(Rr, v1, v2, th, max_iterations=3)
     print("certify", mu, len(r["suboptimality_traj"]))
-# round 2: the tensor-core graph kernel (tcgen05 / TMA / mbarrier pipeline), the one-MUFU strip kernel, the re-check queue
+# round 2: the tensor-core graph kernel (wgmma / TMA / mbarrier pipeline), the one-MUFU strip kernel, the re-check queue
 for flags in (1024, 1024 | 2, 2048, 2048 | 2, 2048 | 1):
     ctx.set_flags(flags | 4)
     for cfg, n in (("C2", 300), ("C2cube", 200)):

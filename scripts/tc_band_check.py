@@ -6,12 +6,13 @@ import numpy as np, sys, importlib
 sys.path.insert(0, __import__("os").path.dirname(__import__("os").path.dirname(__import__("os").path.abspath(__file__))))
 synth=importlib.import_module("teaser-plusplus_b200.synth")
 u=2.0**-24
+KAPPA=64.0  # kTcKappa (csrc/tzr_internal.cuh)
 def f32(x): return np.asarray(x,dtype=np.float64).astype(np.float32).astype(np.float64)
 def check(src,dst,nb,mode,label,verbose=True):
     n=len(src); beta=2*nb
     mn=src.min(0);mx=src.max(0);Ds2=((mx-mn)**2).sum()
     mn=dst.min(0);mx=dst.max(0);Dd2=((mx-mn)**2).sum()
-    E=12*u*(Ds2+Dd2); b2=beta*beta;b4=b2*b2
+    E=KAPPA*u*(Ds2+Dd2); b2=beta*beta;b4=b2*b2
     lam=0.75*beta*np.sqrt(0.5*(Ds2+Dd2)); Smax=Ds2+Dd2+E
     kap=E/lam+8*u; c0=E*lam+E*E+2*b2*E+16*u*b2*Smax+8*u*b4+b4
     up=1+2.0**-20
@@ -22,7 +23,7 @@ def check(src,dst,nb,mode,label,verbose=True):
     a=((src[iu[0]]-src[iu[1]])**2).sum(1); b=((dst[iu[0]]-dst[iu[1]])**2).sum(1)
     exact=np.abs(np.sqrt(a)-np.sqrt(b))<=beta
     rng=np.random.default_rng(1)
-    ea=12*u*Ds2; eb=12*u*Dd2
+    ea=KAPPA*u*Ds2; eb=KAPPA*u*Dd2
     if mode=='rand': pa=rng.uniform(-1,1,a.shape)*ea; pb=rng.uniform(-1,1,a.shape)*eb
     elif mode=='pp': pa=ea;pb=-eb
     elif mode=='pm': pa=-ea;pb=eb

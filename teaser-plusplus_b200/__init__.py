@@ -1,4 +1,4 @@
-"""B200-native TEASER++ registration hot path (package directory `teaser-plusplus_b200`).
+"""GPU-native TEASER++ registration hot path (package directory `teaser-plusplus_b200`).
 
 Import with `importlib.import_module("teaser-plusplus_b200")` (the hyphen is part of the
 contractual directory name).  Sub-modules:

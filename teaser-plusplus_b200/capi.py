@@ -100,7 +100,7 @@ _SYMBOLS = [
 
 
 def build(verbose: bool = False):
-    """Compile csrc/*.cu for sm_100a with nvcc (cross-compiles without a GPU)."""
+    """Compile csrc/*.cu for sm_90a with nvcc (cross-compiles without a GPU)."""
     cmd = ["make", "-C", CSRC_DIR] + ([] if verbose else ["-s"])
     subprocess.check_call(cmd)
 

@@ -27,7 +27,7 @@ struct tzr_ctx {
   std::string last_error;
   int64_t launches = 0;
   uint32_t flags = 0;
-  int num_sms = 148;
+  int num_sms = 132;
   // device buffers (grow-only)
   DevBuf src, dst, sf, df, pk, opnd, tclist, gc, adj, deg, nedges, hclq, hsize, clq, L, alive, best_bits, alive_cnt, root_ctr, lock, flg, kfinal, tstart, stack, cv,
       centry, ps, pd, wgt, res, skey, sidx, sorted, rmask, tmask, sol, dbg, misc, sc_x, sc_r, sc_key, sc_idx, m_in, m_scratch, m_out, cert;
@@ -189,10 +189,10 @@ int setup_batch(tzr_ctx* ctx, int B, int n, bool own_points, Batch* out, bool co
   bt.exact_ctas = G;
   bt.max_depth = (int)depth;
   {
-    // problems under search at a time: their bitsets should stay in the L2 together (~48 MB of the 126 MB: the
+    // problems under search at a time: their bitsets should stay in the L2 together (~18 MB of the 50 MB: the
     // stacks, the other lane's graph kernel and the two L2 partitions take the rest)
     const size_t bits = n * W32 * sizeof(uint32_t);
-    const size_t conc = ((size_t)48 << 20) / std::max<size_t>(bits, 1);
+    const size_t conc = ((size_t)18 << 20) / std::max<size_t>(bits, 1);
     bt.exact_conc = (int)std::min<size_t>(std::max<size_t>(conc, 1), (size_t)B);
   }
   ENS(stack, warps * depth * level_bytes);
@@ -336,12 +336,12 @@ Batch sub_batch(const Batch& bt, int b0, int Bc) {
 }
 
 // Problems per pipeline chunk: small enough that a chunk's adjacency bitsets (written by the graph kernel, then
-// read by the degree / clique kernels) stay resident in the 126 MB L2 instead of making a round trip through HBM.
+// read by the degree / clique kernels) stay resident in the 50 MB L2 instead of making a round trip through HBM.
 int l2_chunk(const tzr_ctx* ctx, int B, int n, const tzr_params& p) {
   (void)ctx;
   // Optional sub-chunking of graph+degree so the degree pass reads the bitsets from L2 (TZR_L2_CHUNK_MB = MB of
   // adjacency per sub-chunk).  Off by default: with the v5 graph kernel the tail of each small launch costs more
-  // than the saved HBM read (measured r01: 84.5 K reg/s unchunked vs 78.1 K at 96 MB, profiles/README.md).
+  // than the saved HBM read.
   static const long long budget_mb = [] {
     const char* e = std::getenv("TZR_L2_CHUNK_MB");
     return e ? std::atoll(e) : 0LL;
@@ -524,7 +524,7 @@ const char* tzr_status_string(int s) {
   switch (s) {
     case TZR_OK: return "ok";
     case TZR_ERR_INVALID_ARG: return "invalid argument";
-    case TZR_ERR_NO_DEVICE: return "no usable CUDA device (the B200 path has no CPU fallback)";
+    case TZR_ERR_NO_DEVICE: return "no usable CUDA device (the GPU path has no CPU fallback)";
     case TZR_ERR_CUDA: return "CUDA error";
     case TZR_ERR_ALLOC: return "allocation failed";
     case TZR_ERR_UNSUPPORTED: return "unsupported parameter combination";

@@ -1,6 +1,6 @@
 // Stage 1 of solve(): TIMs + scale-consistency test + inlier graph, fused.
 //
-// Replaces (reference, /root/reference):
+// Replaces (reference):
 //   RobustRegistrationSolver::computeTIMs            teaser/src/registration.cc:512-551  (x2)
 //   ScaleInliersSelector::solveForScale              teaser/src/registration.cc:427-443
 //   inlier_graph_.addEdge loop                       teaser/src/registration.cc:614-619
@@ -168,7 +168,7 @@ __global__ void __launch_bounds__(256) prep_kernel(Batch bt) {
       const double kap = E / lam + 8.0 * u32;
       const double c0 = E * lam + E * E + 2.0 * b2 * E + 16.0 * u32 * b2 * Smax + 8.0 * u32 * b4 + b4;
       // When is the filter worth it (correctness never depends on this)?  beta <= D/8: the beta^4 floor of the band stays
-      // below ~1e-3 of the pairs (measured 3.5e-5 at C2's beta/D = 1/26, 7.8e-4 at 1/4); E / (0.75 D) <= beta / 64: the band in g = |sqrt a - sqrt b| is a small fraction of the
+      // below ~1e-3 of the pairs; E / (0.75 D) <= beta / 64: the band in g = |sqrt a - sqrt b| is a small fraction of the
       // threshold (fails when the noise bound is tiny against the extent of a cloud: beta/D below ~3e-4); b4 a normal float.
       const double Dmin = sqrt(fmin(Ds2, Dd2));
       const bool ok = !use64 && (bt.flags_dbg & 1024u) != 0 && (bt.flags_dbg & 512u) == 0 && Ds2 > 0 && Dd2 > 0 && Ds2 < 1e8 && Dd2 < 1e8 &&
@@ -582,14 +582,13 @@ __global__ void __launch_bounds__(kGraphThreads, kMinBlocks) graph_strip_kernel(
 #endif  // TZR_AB_KERNELS
 
 // ------------------------------------------------------------------------------------------------
-// graph strip kernel, packed-FP32 variant (default): identical decomposition and outputs as graph_strip_kernel,
-// but the twelve FP32 operations per pair run as sm_100 packed instructions (FADD2 / FMUL2 / FFMA2 via
-// __fadd2_rn / __fmul2_rn / __ffma2_rn: two pairs per instruction), because the scalar kernel is ISSUE-bound
-// (ncu: 75 % issue-active, FMA pipe 43 %): packing halves the FP32 issue slots at unchanged pipe work.  Every
-// component is the same IEEE operation as in the scalar kernel, so the classification (and delta) is unchanged.
-// The row point is stored negated and duplicated in shared memory ((-x,-x), ...) so that js - is is one FADD2.
+// graph strip kernel, paired-FP32 variant (default): identical decomposition and outputs as graph_strip_kernel, with
+// two pairs per 64-bit register pair: the twelve FP32 operations per pair run on (x, y) lanes that are loaded with
+// one 8-byte access and stay paired end to end, so no re-packing moves are needed.  Every component is the same IEEE
+// operation (explicit round-to-nearest, no contraction) as in the scalar kernel, so the classification (and delta) is
+// unchanged.  The row point is stored negated and duplicated in shared memory ((-x,-x), ...) so that js - is is one
+// paired add.
 // ------------------------------------------------------------------------------------------------
-// packed FP32x2 values live in 64-bit registers end to end (PTX *.f32x2), so no re-packing moves are needed
 typedef unsigned long long f32x2;
 __device__ __forceinline__ f32x2 pk2(float lo, float hi) {
   f32x2 r;
@@ -600,24 +599,29 @@ __device__ __forceinline__ void upk2(f32x2 v, float& lo, float& hi) {
   asm("mov.b64 {%0, %1}, %2;" : "=f"(lo), "=f"(hi) : "l"(v));
 }
 __device__ __forceinline__ f32x2 add2(f32x2 a, f32x2 b) {
-  f32x2 r;
-  asm("add.rn.f32x2 %0, %1, %2;" : "=l"(r) : "l"(a), "l"(b));
-  return r;
+  float a0, a1, b0, b1;
+  upk2(a, a0, a1);
+  upk2(b, b0, b1);
+  return pk2(__fadd_rn(a0, b0), __fadd_rn(a1, b1));
 }
 __device__ __forceinline__ f32x2 sub2(f32x2 a, f32x2 b) {
-  f32x2 r;
-  asm("sub.rn.f32x2 %0, %1, %2;" : "=l"(r) : "l"(a), "l"(b));
-  return r;
+  float a0, a1, b0, b1;
+  upk2(a, a0, a1);
+  upk2(b, b0, b1);
+  return pk2(__fsub_rn(a0, b0), __fsub_rn(a1, b1));
 }
 __device__ __forceinline__ f32x2 mul2(f32x2 a, f32x2 b) {
-  f32x2 r;
-  asm("mul.rn.f32x2 %0, %1, %2;" : "=l"(r) : "l"(a), "l"(b));
-  return r;
+  float a0, a1, b0, b1;
+  upk2(a, a0, a1);
+  upk2(b, b0, b1);
+  return pk2(__fmul_rn(a0, b0), __fmul_rn(a1, b1));
 }
 __device__ __forceinline__ f32x2 fma2(f32x2 a, f32x2 b, f32x2 c) {
-  f32x2 r;
-  asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(r) : "l"(a), "l"(b), "l"(c));
-  return r;
+  float a0, a1, b0, b1, c0, c1;
+  upk2(a, a0, a1);
+  upk2(b, b0, b1);
+  upk2(c, c0, c1);
+  return pk2(__fmaf_rn(a0, b0, c0), __fmaf_rn(a1, b1, c1));
 }
 
 struct __align__(16) IPointNeg2 {
@@ -1050,7 +1054,7 @@ void launch_prep(const Batch& bt, cudaStream_t st) { prep_kernel<<<bt.B, 256, 0,
 int launch_graph(const Batch& bt0, cudaStream_t st, int num_sms) {
   Batch bt = bt0;
   // default: CUDA-core strip kernel.  Debug flag 1024 routes every problem prep_kernel marked use_tc through the
-  // tensor-core kernel instead (bit-identical output, measured slower: DESIGN.md §3.1, profiles/r02_graph_tc_*)
+  // tensor-core kernel instead (bit-identical output: DESIGN.md §3.1)
   bt.tc_active = ((bt.flags_dbg & 1024u) && !(bt.flags_dbg & (8u | 16u | 32u | 64u | 128u | 256u | 512u))) ? 1 : 0;
   int launches = 1;  // the CUDA-core strip kernel below (grid covers every problem; TC problems return at once)
   if (bt.tc_active) launches += launch_graph_tc(bt, st, num_sms);
@@ -1069,7 +1073,7 @@ int launch_graph(const Batch& bt0, cudaStream_t st, int num_sms) {
   if (!bt.tc_active) cudaMemsetAsync(bt.tc_list_count, 0, sizeof(unsigned int), st);  // (launch_graph_tc zeroes it otherwise)
   bool v7 = false;
   if (bt.flags_dbg & 2048u) {  // v7 (one MUFU, sign-bit words, re-check queue): fewer instructions, but FMA-pipe bound
-    v7 = true;                 // on B200 and 8 % slower than the default (profiles/r02_graph_v7_vs_v6.md)
+    v7 = true;
     if (bt.flags_dbg & 2u)
       graph_strip3_kernel<true, 5><<<sgrid, kGraphThreads, 0, st>>>(bt);
     else
@@ -1080,16 +1084,16 @@ int launch_graph(const Batch& bt0, cudaStream_t st, int num_sms) {
     graph_strip_kernel<false, 6><<<sgrid, kGraphThreads, 0, st>>>(bt);
   else if (bt.flags_dbg & 32u)  // occupancy A/B: 5 CTAs/SM (96 registers)
     graph_strip_kernel<false, 5><<<sgrid, kGraphThreads, 0, st>>>(bt);
-  else if (bt.flags_dbg & 64u)  // scalar-FP32 strip kernel (A/B against the packed default)
+  else if (bt.flags_dbg & 64u)  // scalar-FP32 strip kernel (A/B against the paired default)
     graph_strip_kernel<false, 8><<<sgrid, kGraphThreads, 0, st>>>(bt);
-  else if (bt.flags_dbg & 128u)  // packed kernel at 6 CTAs/SM
+  else if (bt.flags_dbg & 128u)  // paired kernel at 6 CTAs/SM
     graph_strip2_kernel<false, 6, false><<<sgrid, kGraphThreads, 0, st>>>(bt);
 #endif
   else if (bt.flags_dbg & 2u)
     graph_strip2_kernel<true, 5, false><<<sgrid, kGraphThreads, 0, st>>>(bt);
   else if (bt.flags_dbg & 256u)  // degrees by the separate degree kernel (A/B against the fused default)
     graph_strip2_kernel<false, 8, false><<<sgrid, kGraphThreads, 0, st>>>(bt);
-  else  // default: packed FP32x2 strip kernel, 8 CTAs/SM, degrees fused
+  else  // default: paired-FP32 strip kernel, 8 CTAs/SM, degrees fused
     graph_strip2_kernel<false, 8, true><<<sgrid, kGraphThreads, 0, st>>>(bt);
   if (v7) {  // exact re-check of the pairs the strip kernel queued
     launch_graph_patch(bt, st, num_sms);

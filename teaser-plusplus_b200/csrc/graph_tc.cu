@@ -1,6 +1,6 @@
-// Stage 1 of solve() on the 5th-generation tensor cores: TIMs + scale-consistency test + inlier graph.
+// Stage 1 of solve() on the tensor cores (Hopper warpgroup MMA): TIMs + scale-consistency test + inlier graph.
 //
-// Replaces (reference, /root/reference), exactly like graph_build.cu:
+// Replaces (reference), exactly like graph_build.cu:
 //   RobustRegistrationSolver::computeTIMs            teaser/src/registration.cc:512-551  (x2)
 //   ScaleInliersSelector::solveForScale              teaser/src/registration.cc:427-443
 //   inlier_graph_.addEdge loop                       teaser/src/registration.cc:614-619
@@ -10,23 +10,22 @@
 //     a_ij = |s_i - s_j|^2 = n_i + n_j - 2 s_i.s_j      (and b_ij for the destination cloud)
 // is a K = 3 (+2 for the norms) contraction.  Every centred coordinate (and every norm) is split into three tf32
 // pieces h + m + l (11 significant bits each, so the split carries 33 bits of the FP64 value), and the products
-// hh', hm', mh', mm', hl', lh' plus the six norm pieces are laid out as a K = 24 tf32 GEMM (three K = 8 tcgen05.mma
-// steps per cloud): one 128x64 tile of a and of b lands in tensor memory per 6 MMAs, issued by one thread.  The
+// hh', hm', mh', mm', hl', lh' plus the six norm pieces are laid out as a K = 24 tf32 GEMM (three K = 8 wgmma steps
+// per cloud): one 128x64 tile of a and of b is computed by two consumer warpgroups (64 rows each) into registers.  The
 // operand tiles (tc_prep_kernel writes them once per problem in the exact shared-memory image the MMA descriptor
-// wants: no-swizzle K-major planes) are staged by the TMA engine (cp.async.bulk -> UBLKCP) into a shared-memory ring,
-// completion on mbarriers; the accumulators are double-buffered in TMEM so the MMAs of tile t+1 run under the
-// epilogue of tile t.
+// wants: no-swizzle K-major planes) are staged by the TMA engine (cp.async.bulk -> UBLKCP) into a shared-memory ring
+// by one producer warp, completion on mbarriers; two CTAs per SM overlap one CTA's MMAs with the other's epilogue.
 //
-// Epilogue (8 warps, tcgen05.ld 32 lanes x 16 columns): with t = a-b, s = a+b, g = |sqrt a - sqrt b|, w = (sqrt a + sqrt b)^2
+// Epilogue (in the MMA's register fragments): with t = a-b, s = a+b, g = |sqrt a - sqrt b|, w = (sqrt a + sqrt b)^2
 //     f = t^2 - 2 beta^2 s + beta^4 = (g^2 - beta^2)(w - beta^2)          edge  <=>  s <= beta^2  or  f <= 0
 // a polynomial in the tensor-core values: no square root, no division, and its error is a Lipschitz bound
-// (|f' - f| <= 2 E |t'| + E^2 + 2 beta^2 E for |a' - a| + |b' - b| <= E), so there are no guards for tiny norms.  Per pair,
-// packed two at a time: t, s, P = t^2 + beta^4, d = P - 2 beta^2 s, band = kap P + c0, d + band, d - band = 7 FP32
-// lane operations; the two sign bits are funnel-shifted into the words whi (surely an edge) and wlo (not surely a
-// non-edge) — no compare, no ballot, no MUFU.  whi is the tentative row word; wlo & ~whi are the pairs inside the error
-// band (prep_kernel, DESIGN.md §3.1: 3.5e-5 of the pairs on C2): they are queued and tc_patch_kernel re-evaluates them
-// with the reference's exact FP64 sequence.  The accumulator stage goes back to the MMA issuer as soon as the warp's
-// values sit in registers.
+// (|f' - f| <= 2 E |t'| + E^2 + 2 beta^2 E for |a' - a| + |b' - b| <= E), so there are no guards for tiny norms.  Per pair:
+// t, s, P = t^2 + beta^4, d = P - 2 beta^2 s, band = kap P + c0, d + band, d - band = 7 FP32 operations; the two sign
+// bits go into the words whi (surely an edge) and wlo (not surely a non-edge) — no compare, no MUFU.  The four lanes
+// that share a fragment row combine their bits so that each lane ends up owning one (row, 32-column) word.  whi is the
+// tentative row word; wlo & ~whi are the pairs inside the error band (prep_kernel, DESIGN.md §3.1): they are queued and
+// tc_patch_kernel re-evaluates them with the reference's exact FP64 sequence.  The transposed half of the bitset goes
+// through a small shared-memory buffer and a warp bit transpose.
 // Output (packed symmetric bitset, fused degrees) is bit-identical to graph_build.cu's and to the oracle's.
 #include "tc_ptx.cuh"
 #include "tzr_internal.cuh"
@@ -35,8 +34,8 @@ namespace tzr {
 
 using namespace tc;
 
-constexpr int kTcEpiWarps = 8;                        // warp w: TMEM lanes 32*(w&3).., columns 32*(w>>2)..
-constexpr int kTcThreads = 32 * (kTcEpiWarps + 1);    // + 1 producer warp (TMA + MMA issue by one elected lane)
+constexpr int kTcEpiWarps = 8;                        // two consumer warpgroups (MMA + epilogue): 64 rows of a tile each
+constexpr int kTcThreads = 32 * (kTcEpiWarps + 1);    // + 1 producer warp (TMA issue by one elected lane)
 constexpr int kTcN = 64;                              // columns of one tile (MMA N)
 constexpr int kTcPlaneA = 128 * 16;                   // A role: 128 rows x 4 tf32 per plane
 constexpr int kTcPlaneB = kTcN * 16;                  // B role: 64 rows x 4 tf32 per plane
@@ -44,7 +43,8 @@ constexpr int kTcCloudA = 6 * kTcPlaneA, kTcCloudB = 6 * kTcPlaneB;   // 6 plane
 constexpr int kTcTileA = 2 * kTcCloudA;               // src + dst: 24 KB per 128-row block
 constexpr int kTcTileB = 2 * kTcCloudB;               // 12 KB per 64-column block
 constexpr int kTcBStages = 4;
-constexpr int kTcSmemBytes = 2 * kTcTileA + kTcBStages * kTcTileB + 256;
+constexpr int kTcTrBytes = 2 * kTile * 2 * 4;         // row words of a tile for the transposed half, double-buffered
+constexpr int kTcSmemBytes = 2 * kTcTileA + kTcBStages * kTcTileB + 256 + kTcTrBytes;   // 98 KB: two CTAs per SM
 
 __host__ __device__ inline size_t tc_a_bytes(int n) { return (size_t)((n + 127) / 128) * kTcTileA; }
 // 64-column blocks per problem: the whole padded row pitch (2 per 128-block), so that every word of the bitset rows is
@@ -168,73 +168,48 @@ __host__ __device__ inline int tc_strips_per_problem(int n, int S) {
   return total;
 }
 
-// packed FP32x2 (two pairs per instruction; FADD2 / FMUL2 / FFMA2)
-typedef unsigned long long f32x2;
-__device__ __forceinline__ f32x2 pk2(uint32_t lo, uint32_t hi) {
-  f32x2 r;
-  asm("mov.b64 %0, {%1, %2};" : "=l"(r) : "r"(lo), "r"(hi));
-  return r;
-}
-__device__ __forceinline__ f32x2 pk2f(float lo, float hi) {
-  f32x2 r;
-  asm("mov.b64 %0, {%1, %2};" : "=l"(r) : "f"(lo), "f"(hi));
-  return r;
-}
-__device__ __forceinline__ void upk2(f32x2 v, float& lo, float& hi) {
-  asm("mov.b64 {%0, %1}, %2;" : "=f"(lo), "=f"(hi) : "l"(v));
-}
-__device__ __forceinline__ f32x2 add2(f32x2 a, f32x2 b) {
-  f32x2 r;
-  asm("add.rn.f32x2 %0, %1, %2;" : "=l"(r) : "l"(a), "l"(b));
-  return r;
-}
-__device__ __forceinline__ f32x2 sub2(f32x2 a, f32x2 b) {
-  f32x2 r;
-  asm("sub.rn.f32x2 %0, %1, %2;" : "=l"(r) : "l"(a), "l"(b));
-  return r;
-}
-__device__ __forceinline__ f32x2 mul2(f32x2 a, f32x2 b) {
-  f32x2 r;
-  asm("mul.rn.f32x2 %0, %1, %2;" : "=l"(r) : "l"(a), "l"(b));
-  return r;
-}
-__device__ __forceinline__ f32x2 fma2(f32x2 a, f32x2 b, f32x2 c) {
-  f32x2 r;
-  asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(r) : "l"(a), "l"(b), "l"(c));
-  return r;
-}
-__device__ __forceinline__ float sqrt_approx_tc(float x) {  // MUFU.SQRT, max relative error 2^-23 (inside the 24 u term)
-  float y;
-  asm("sqrt.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
-  return y;
-}
-
 struct TcConsts {
-  f32x2 nc2, b4, kap, c0;  // -2 beta^2, beta^4, band slope, band offset (prep_kernel; DESIGN.md §3.1)
+  float nc2, b4, kap, c0;  // -2 beta^2, beta^4, band slope, band offset (prep_kernel; DESIGN.md §3.1)
 };
 
-// 16 pairs (columns c0 .. c0+15 of the warp's 32; call with the upper half first).  Per pair, packed two at a time:
+// The pair test on the 32 accumulator values of this thread (d[4 i + 2 r + c] = row r0 + 8 r, column 8 i + 2 (lane % 4)
+// + c of the 64-column tile).  Per pair:
 //   t = a - b, s = a + b, P = t^2 + beta^4, d = P - 2 beta^2 s  [= (g^2 - beta^2)(w - beta^2)],  band = kap P + c0,
 //   d_hi = d + band  (sign bit 1: surely an edge),   d_lo = d - band  (sign bit 0: surely not an edge)
-// = 7 FP32 lane operations, no MUFU, no compare; the two sign bits are funnel-shifted into the words.
-__device__ __forceinline__ void tc_sweep16(const uint32_t (&ra)[16], const uint32_t (&rb)[16], const TcConsts& k,
-                                           uint32_t& whi, uint32_t& wlo) {
+// = 7 FP32 operations, no MUFU, no compare.  whi[r][h] / wlo[r][h] bit k: this lane's sign bits of column 32 h + k.
+__device__ __forceinline__ void tc_sweep(const float (&a)[32], const float (&b)[32], const TcConsts& k, int lane,
+                                         uint32_t (&whi)[2][2], uint32_t (&wlo)[2][2]) {
 #pragma unroll
-  for (int g = 7; g >= 0; --g) {
-    const f32x2 A = pk2(ra[2 * g], ra[2 * g + 1]), B = pk2(rb[2 * g], rb[2 * g + 1]);
-    const f32x2 t = sub2(A, B), s = add2(A, B);
-    const f32x2 P = fma2(t, t, k.b4);
-    const f32x2 d = fma2(s, k.nc2, P);
-    const f32x2 bd = fma2(P, k.kap, k.c0);
-    const f32x2 dh = add2(d, bd), dl = sub2(d, bd);
-    float h0, h1, l0, l1;
-    upk2(dh, h0, h1);
-    upk2(dl, l0, l1);
-    whi = __funnelshift_l(__float_as_uint(h1), whi, 1);
-    whi = __funnelshift_l(__float_as_uint(h0), whi, 1);
-    wlo = __funnelshift_l(__float_as_uint(l1), wlo, 1);
-    wlo = __funnelshift_l(__float_as_uint(l0), wlo, 1);
+  for (int r = 0; r < 2; ++r)
+#pragma unroll
+    for (int h = 0; h < 2; ++h) whi[r][h] = wlo[r][h] = 0u;
+#pragma unroll
+  for (int e = 0; e < 32; ++e) {
+    const int i = e >> 2, r = (e >> 1) & 1, pos = 8 * (i & 3) + (e & 1);
+    const float t = __fsub_rn(a[e], b[e]), s = __fadd_rn(a[e], b[e]);
+    const float P = __fmaf_rn(t, t, k.b4);
+    const float d = __fmaf_rn(s, k.nc2, P);
+    const float bd = __fmaf_rn(P, k.kap, k.c0);
+    whi[r][i >> 2] |= (__float_as_uint(__fadd_rn(d, bd)) >> 31) << pos;
+    wlo[r][i >> 2] |= (__float_as_uint(__fsub_rn(d, bd)) >> 31) << pos;
   }
+  const int sh = 2 * (lane & 3);
+#pragma unroll
+  for (int r = 0; r < 2; ++r)
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      whi[r][h] <<= sh;
+      wlo[r][h] <<= sh;
+    }
+}
+
+// The four lanes of a quad hold disjoint bits of the same four words (2 rows x 2 column halves).  Reduce-scatter in two
+// exchanges: lane (lane & 3) = 2 mr + mh ends up with the complete word of row r0 + 8 mr, column half mh.
+__device__ __forceinline__ uint32_t tc_quad_word(const uint32_t (&w)[2][2], int lane) {
+  const int mr = (lane >> 1) & 1, mh = lane & 1;
+  const uint32_t k0 = (mr ? w[1][0] : w[0][0]) | __shfl_xor_sync(0xffffffffu, mr ? w[0][0] : w[1][0], 2);
+  const uint32_t k1 = (mr ? w[1][1] : w[0][1]) | __shfl_xor_sync(0xffffffffu, mr ? w[0][1] : w[1][1], 2);
+  return (mh ? k1 : k0) | __shfl_xor_sync(0xffffffffu, mh ? k0 : k1, 1);
 }
 
 // 32x32 bit transpose across the lanes of a warp (lane l passes row l, receives column l)
@@ -256,19 +231,19 @@ __device__ __forceinline__ uint32_t tc_transpose32(uint32_t x, int lane) {
 // barrier slots in shared memory
 enum {
   kBarAFull = 0,                          // [2]  TMA -> MMA: A tile of the strip landed
-  kBarAEmpty = 2,                         // [2]  MMA commit -> TMA: the strip's A tile has been read for the last time
+  kBarAEmpty = 2,                         // [2]  consumer warps (8 arrivals) -> TMA: the strip's A tile was read for the last time
   kBarBFull = 4,                          // [kTcBStages]  TMA -> MMA
-  kBarBEmpty = kBarBFull + kTcBStages,    // [kTcBStages]  MMA commit -> TMA: stage may be overwritten
-  kBarTFull = kBarBEmpty + kTcBStages,    // [2]  MMA commit -> epilogue: accumulator stage ready
-  kBarTEmpty = kBarTFull + 2,             // [2]  epilogue (8 arrivals) -> MMA: accumulator stage drained
-  kNumBars = kBarTEmpty + 2
+  kBarBEmpty = kBarBFull + kTcBStages,    // [kTcBStages]  consumer warps (8 arrivals) -> TMA: stage may be overwritten
+  kNumBars = kBarBEmpty + kTcBStages
 };
 
+// 112 registers: two 288-thread CTAs per SM (64 512 of the 65 536 registers); the 64 accumulators of a thread fit without
+// spills (at the 96 registers a (288, 2) launch bound gives, ptxas spills).
 template <bool kVerify>
-__global__ void __launch_bounds__(kTcThreads, 2) graph_tc_kernel(Batch bt, int S, int spp, int total_items) {
+__global__ void __maxnreg__(112) graph_tc_kernel(Batch bt, int S, int spp, int total_items) {
   extern __shared__ __align__(1024) uint8_t smem[];
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + 2 * kTcTileA + kTcBStages * kTcTileB);
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + kNumBars);
+  uint32_t* s_tr = reinterpret_cast<uint32_t*>(smem + 2 * kTcTileA + kTcBStages * kTcTileB + 256);
   const uint32_t sA0 = smem_u32(smem), sB0 = smem_u32(smem + 2 * kTcTileA);
   const uint32_t bar0 = smem_u32(bars);
   auto bar = [&](int i) { return bar0 + 8u * (uint32_t)i; };
@@ -276,107 +251,56 @@ __global__ void __launch_bounds__(kTcThreads, 2) graph_tc_kernel(Batch bt, int S
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int n = bt.n;
   if (tid == 0) {
-    for (int i = 0; i < kNumBars; ++i) mbar_init(bar(i), i >= kBarTEmpty ? kTcEpiWarps : 1);
+    for (int i = 0; i < kNumBars; ++i)
+      mbar_init(bar(i), (i >= kBarBEmpty || (i >= kBarAEmpty && i < kBarBFull)) ? kTcEpiWarps : 1);
     mbar_fence_init();
   }
-  if (warp == kTcEpiWarps) tmem_alloc<256>(smem_u32(tmem_slot));
-  fence_before_sync();
   __syncthreads();
-  fence_after_sync();
-  const uint32_t tbase = *tmem_slot;  // accumulator stage s: a at columns 128 s .. +63, b at 128 s + 64 .. +63
 
   if (warp == kTcEpiWarps) {
-    // ================= producer: TMA loads (kTcBStages - 1 tiles ahead), MMA issue =================
+    // ================= producer: TMA loads, up to kTcBStages tiles and two strips ahead of the MMAs =================
     if (lane == 0) {
       const uint8_t* opnd = reinterpret_cast<const uint8_t*>(bt.opnd);
       const size_t per_problem = tc_a_bytes(n) + tc_b_bytes(n), a_bytes = tc_a_bytes(n);
-      TileIter ld, mm;
+      TileIter ld;
       ld.init(blockIdx.x, gridDim.x, total_items, spp, S, n);
-      mm.init(blockIdx.x, gridDim.x, total_items, spp, S, n);
-      uint32_t n_loaded = 0, n_strips_loaded = 0, n_mma = 0, n_strips = 0, ap = 0;
+      uint32_t n_loaded = 0, n_strips_loaded = 0;
       int tc_b = -1;
       bool tc_ok = false;
-      auto next_tc = [&](TileIter& t) {  // next tile of a problem that takes the tensor-core path
-        while (t.next()) {
-          if (t.b != tc_b) {
-            tc_b = t.b;
-            tc_ok = bt.gc[t.b].use_tc != 0;
-          }
-          if (tc_ok) return true;
+      while (ld.next()) {
+        if (ld.b != tc_b) {  // only tiles of problems that take the tensor-core path
+          tc_b = ld.b;
+          tc_ok = bt.gc[ld.b].use_tc != 0;
         }
-        return false;
-      };
-      auto issue_load = [&](const TileIter& t) {
+        if (!tc_ok) continue;
         const uint32_t st = n_loaded % kTcBStages, use = n_loaded / kTcBStages;
         if (use > 0) mbar_wait(bar(kBarBEmpty + st), (use - 1) & 1u);  // the MMAs that read this stage are complete
-        const uint8_t* pb = opnd + (size_t)t.b * per_problem;
-        if (t.first) {
+        const uint8_t* pb = opnd + (size_t)ld.b * per_problem;
+        if (ld.first) {
           // A buffer (strip index & 1): wait until the strip that used it two strips ago has been read completely
           const uint32_t a = n_strips_loaded & 1u;
           if (n_strips_loaded >= 2) mbar_wait(bar(kBarAEmpty + a), ((n_strips_loaded >> 1) - 1) & 1u);
           mbar_arrive_expect_tx(bar(kBarAFull + a), kTcTileA);
-          bulk_g2s(sA0 + a * kTcTileA, pb + (size_t)t.I * kTcTileA, kTcTileA, bar(kBarAFull + a));
+          bulk_g2s(sA0 + a * kTcTileA, pb + (size_t)ld.I * kTcTileA, kTcTileA, bar(kBarAFull + a));
           ++n_strips_loaded;
         }
         mbar_arrive_expect_tx(bar(kBarBFull + st), kTcTileB);
-        bulk_g2s(sB0 + st * kTcTileB, pb + a_bytes + (size_t)t.J * kTcTileB, kTcTileB, bar(kBarBFull + st));
+        bulk_g2s(sB0 + st * kTcTileB, pb + a_bytes + (size_t)ld.J * kTcTileB, kTcTileB, bar(kBarBFull + st));
         ++n_loaded;
-      };
-      const uint32_t idesc = make_idesc_tf32(128, kTcN);
-      // The loads run ahead of the MMAs by at most kTcBStages - 1 tiles and at most one strip: this thread issues both,
-      // so a load may only wait for commits of MMAs that have ALREADY been issued (B stage of tile n_loaded - kTcBStages,
-      // A buffer of the strip before the previous one) — otherwise it would wait for itself.
-      bool pend = next_tc(ld);
-      auto can_load = [&]() {
-        return pend && (n_loaded - n_mma) < (uint32_t)(kTcBStages - 1) && (!ld.first || n_strips >= n_strips_loaded);
-      };
-      while (can_load()) {
-        issue_load(ld);
-        pend = next_tc(ld);
-      }
-      while (next_tc(mm)) {
-        const uint32_t st = n_mma % kTcBStages, use = n_mma / kTcBStages;
-        const uint32_t ts = n_mma & 1u, tuse = n_mma >> 1;
-        if (mm.first) {
-          ap = n_strips & 1u;
-          mbar_wait(bar(kBarAFull + ap), (n_strips >> 1) & 1u);
-          ++n_strips;
-        }
-        mbar_wait(bar(kBarBFull + st), use & 1u);
-        if (tuse > 0) mbar_wait(bar(kBarTEmpty + ts), (tuse - 1) & 1u);  // the epilogue has drained this accumulator stage
-        fence_after_sync();
-        // K-major, no swizzle: leading byte offset = distance of the two 16-byte K-chunks (planes), stride byte offset
-        // = distance of consecutive 8-row groups (128 B)
-#pragma unroll
-        for (int cloud = 0; cloud < 2; ++cloud)
-#pragma unroll
-          for (int s = 0; s < 3; ++s) {
-            const uint64_t da = make_smem_desc(sA0 + ap * kTcTileA + cloud * kTcCloudA + s * 2 * kTcPlaneA, kTcPlaneA, 128);
-            const uint64_t db = make_smem_desc(sB0 + st * kTcTileB + cloud * kTcCloudB + s * 2 * kTcPlaneB, kTcPlaneB, 128);
-            mma_tf32(tbase + 128u * ts + (uint32_t)kTcN * cloud, da, db, idesc, s > 0);
-          }
-        mma_commit(bar(kBarBEmpty + st));
-        if (mm.last_of_strip()) mma_commit(bar(kBarAEmpty + ap));  // the strip's A tile has been read for the last time
-        mma_commit(bar(kBarTFull + ts));
-        ++n_mma;
-        while (can_load()) {
-          issue_load(ld);
-          pend = next_tc(ld);
-        }
       }
     }
     __syncwarp();
   } else {
-    // ================= epilogue warps =================
-    const int q = warp & 3, h = warp >> 2;
-    const uint32_t lane_base = (uint32_t)(32 * q) << 16;
+    // ================= consumers: warpgroup g = warp / 4 computes rows 64 g .. 64 g + 63 of the 128-row block =========
+    const int g = warp >> 2;
+    const int mr = (lane >> 1) & 1, h = lane & 1;
+    const int rloc = 64 * g + 16 * (warp & 3) + (lane >> 2) + 8 * mr;  // the row whose (32-column) word this lane owns
     TileIter ti;
     ti.init(blockIdx.x, gridDim.x, total_items, spp, S, n);
-    uint32_t n_t = 0;
+    uint32_t n_t = 0, n_strips = 0, n_tr = 0, ap = 0;
     int rdeg = 0;
     const int P32 = pitch32(n);
-    TcConsts kc;
-    kc.nc2 = kc.b4 = kc.kap = kc.c0 = pk2f(0.f, 0.f);
+    TcConsts kc{0.f, 0.f, 0.f, 0.f};
     const GraphConsts* gcp = bt.gc;
     bool use_tc = false;
     uint32_t* adj32 = nullptr;  // bitset of the strip's problem
@@ -384,47 +308,70 @@ __global__ void __launch_bounds__(kTcThreads, 2) graph_tc_kernel(Batch bt, int S
     int* degp = nullptr;
     int i = 0;
     bool row_ok = false, row_edge = false;
+    float acc[2][32];
+#pragma unroll
+    for (int e = 0; e < 32; ++e) acc[0][e] = acc[1][e] = 0.f;
     while (ti.next()) {
-      if (ti.first) {  // per strip, not per tile: the load sits on the critical path of the tile hand-off
+      if (ti.first) {  // per strip, not per tile
         gcp = bt.gc + ti.b;
         use_tc = gcp->use_tc != 0;
       }
       if (!use_tc) continue;
       const int I = ti.I, J = ti.J;
       if (ti.first) {
-        kc.nc2 = pk2f(-gcp->tc_c2, -gcp->tc_c2);
-        kc.b4 = pk2f(gcp->tc_b4, gcp->tc_b4);
-        kc.kap = pk2f(gcp->tc_kap, gcp->tc_kap);
-        kc.c0 = pk2f(gcp->tc_c0, gcp->tc_c0);
-        i = I * kTile + 32 * q + lane;
+        kc.nc2 = -gcp->tc_c2;
+        kc.b4 = gcp->tc_b4;
+        kc.kap = gcp->tc_kap;
+        kc.c0 = gcp->tc_c0;
+        i = I * kTile + rloc;
         adj32 = reinterpret_cast<uint32_t*>(bt.adj) + (size_t)ti.b * n * P32;
         rowp = adj32 + (size_t)i * P32;
         degp = bt.deg + (size_t)ti.b * n;
         row_ok = i < n;
         row_edge = I * kTile + kTile > n;  // some rows of the block lie past n
+        ap = n_strips & 1u;
+        mbar_wait(bar(kBarAFull + ap), (n_strips >> 1) & 1u);
+        ++n_strips;
       }
       const int j0 = J * kTcN + 32 * h;
-      const uint32_t ts = n_t & 1u;
-      mbar_wait(bar(kBarTFull + ts), (n_t >> 1) & 1u);
-      fence_after_sync();
-      const uint32_t ta = tbase + lane_base + 128u * ts + 32u * (uint32_t)h, tb = ta + (uint32_t)kTcN;
-      // ---- sweep: whi bit k = pair (i, j0+k) surely an edge, wlo bit k = not surely a non-edge.  The second half of the
-      // accumulators is in flight while the first is evaluated; the stage goes back to the MMA issuer as soon as the
-      // warp's 2 x 32 x 32 values sit in registers.
-      uint32_t whi = 0u, wlo = 0u;
+      const uint32_t st = n_t % kTcBStages, use = n_t / kTcBStages;
+      mbar_wait(bar(kBarBFull + st), use & 1u);
+      // ---- a and b of the 64 x 64 sub-tile: K-major, no swizzle: leading byte offset = distance of the two 16-byte
+      // K-chunks (planes), stride byte offset = distance of consecutive 8-row groups (128 B)
+#pragma unroll
+      for (int e = 0; e < 32; ++e) {
+        acc_fence(acc[0][e]);
+        acc_fence(acc[1][e]);
+      }
+      wgmma_fence();
+#pragma unroll
+      for (int cloud = 0; cloud < 2; ++cloud)
+#pragma unroll
+        for (int s = 0; s < 3; ++s) {
+          const uint64_t da = make_smem_desc(sA0 + ap * kTcTileA + cloud * kTcCloudA + s * 2 * kTcPlaneA + g * 64 * 16,
+                                             kTcPlaneA, 128);
+          const uint64_t db = make_smem_desc(sB0 + st * kTcTileB + cloud * kTcCloudB + s * 2 * kTcPlaneB, kTcPlaneB, 128);
+          wgmma_m64n64k8_tf32(acc[cloud], da, db, s > 0);
+        }
+      wgmma_commit();
+      wgmma_wait_all();
+#pragma unroll
+      for (int e = 0; e < 32; ++e) {
+        acc_fence(acc[0][e]);
+        acc_fence(acc[1][e]);
+      }
+      __syncwarp();
+      if (lane == 0) {  // this warp's reads of the B stage (and, at the end of a strip, of the A tile) are complete
+        mbar_arrive(bar(kBarBEmpty + st));
+        if (ti.last_of_strip()) mbar_arrive(bar(kBarAEmpty + ap));
+      }
+      // ---- sweep: whi bit k = pair (i, j0+k) surely an edge, wlo bit k = not surely a non-edge
+      uint32_t whi, wlo;
       {
-        uint32_t a1[16], b1[16], a0[16], b0[16];
-        tmem_ld16(ta + 16u, a1);
-        tmem_ld16(tb + 16u, b1);
-        tmem_wait_ld();
-        tmem_ld16(ta, a0);
-        tmem_ld16(tb, b0);
-        tc_sweep16(a1, b1, kc, whi, wlo);
-        tmem_wait_ld();
-        fence_before_sync();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(bar(kBarTEmpty + ts));
-        tc_sweep16(a0, b0, kc, whi, wlo);
+        uint32_t qh[2][2], ql[2][2];
+        tc_sweep(acc[0], acc[1], kc, lane, qh, ql);
+        whi = tc_quad_word(qh, lane);
+        wlo = tc_quad_word(ql, lane);
       }
       // validity of the pairs of this thread: columns < n, row < n, i != j (interior tiles: everything valid)
       uint32_t vmask = 0xffffffffu;
@@ -496,13 +443,18 @@ __global__ void __launch_bounds__(kTcThreads, 2) graph_tc_kernel(Batch bt, int S
       }
       rdeg += __popc(word);
       if (row_ok) rowp[2 * J + h] = word;
-      if (!diag) {  // transposed half: lane l holds column j0+l over rows I*128 + 32q .. +31
-        const uint32_t colw = tc_transpose32(word, lane);
-        const int jc = j0 + lane;
+      if (!diag) {  // transposed half: warp w transposes rows I*128 + 32 (w & 3) .. +31 of column half w >> 2
+        uint32_t* buf = s_tr + (n_tr & 1u) * (2 * kTile);
+        buf[2 * rloc + h] = word;
+        named_bar_sync(1, 32 * kTcEpiWarps);
+        const int q = warp & 3, hh = warp >> 2;
+        const uint32_t colw = tc_transpose32(buf[2 * (32 * q + lane) + hh], lane);
+        const int jc = J * kTcN + 32 * hh + lane;
         if (jc < n) {
           adj32[(size_t)jc * P32 + 4 * I + q] = colw;
           if (colw) atomicAdd(degp + jc, __popc(colw));
         }
+        ++n_tr;  // the next transposed tile uses the other buffer: its barrier orders these reads before the rewrite
       }
       if (ti.last_of_strip()) {
         if (row_ok && rdeg) atomicAdd(degp + i, rdeg);
@@ -511,9 +463,6 @@ __global__ void __launch_bounds__(kTcThreads, 2) graph_tc_kernel(Batch bt, int S
       ++n_t;
     }
   }
-  fence_before_sync();
-  __syncthreads();
-  if (warp == kTcEpiWarps) tmem_dealloc<256>(tbase);
 }
 
 // ------------------------------------------------------------------------------------------------

@@ -1028,9 +1028,7 @@ __device__ int node_colour(WarpCtx& c, int csz) {
 // blocks are different colours, so the sum over the blocks is a valid (weaker) colour bound: ~0.085 colours per vertex
 // at 15 % density and 128-vertex blocks against ~0.04 for the full greedy colouring — enough whenever
 // |P| is below ~12x the incumbent size, at a fraction of the row traffic and without the dependent round trips.
-// Measured on B200 (C3, one problem, scripts/gpu_r2_s2_clique_ab.sh): the search is FASTER without this bound (18.7 ms vs
-// 20.0 ms with the counters of debug flag 4 on), and inlined into the ~10 k-instruction search kernel the build faults
-// with "illegal instruction" at a warp collective (the kernel runs out of convergence-barrier registers; out of line it
+// It did not make the search faster, and inlined into the ~10 k-instruction search kernel it is fragile (out of line it
 // is correct).  So it is compiled only with EXTRA=-DTZR_BLOCK_BOUND, out of line, for A/B runs.
 #ifndef TZR_BLOCK_BOUND
 __device__ __forceinline__ bool node_block_bound(WarpCtx&, int) { return false; }
@@ -1398,8 +1396,7 @@ __device__ void exact_search_problem(const Batch& bt, WarpCtx& c, int b) {
 // starting at one of `exact_conc` evenly spaced problems, and on each problem that still has roots takes root vertices
 // from that problem's counter until they run out.  All warps of a start group therefore work on the same problem and
 // move on together: at most ~exact_conc adjacency bitsets are live at a time, chosen on the host so that they fit the
-// L2 (one 10k-vertex bitset is 12.5 MB; a chunk of eight of them under search at once ran at HBM speed, ~2.7x slower
-// per problem than one at a time).  Scratch (stack, clique, entry sizes) belongs to the warp, not to the problem.
+// L2 (one 10k-vertex bitset is 12.5 MB; bitsets that do not fit together are searched at HBM speed).  Scratch (stack, clique, entry sizes) belongs to the warp, not to the problem.
 __global__ void __launch_bounds__(kExactThreads, TZR_EXACT_MIN_BLOCKS) clique_exact_kernel(Batch bt) {
   const int n = bt.n, W = pitch32(n), B = bt.B;
   extern __shared__ __align__(16) unsigned char smem_raw[];

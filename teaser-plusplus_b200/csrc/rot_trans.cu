@@ -1,7 +1,7 @@
 // Stages 3 and 4 of solve(): GNC-TLS rotation and per-axis TLS translation; one CTA per problem,
 // all iterations on chip.
 //
-// Replaces (reference, /root/reference):
+// Replaces (reference):
 //   chain-TIM rebuild + de-scaling                       teaser/src/registration.cc:657-704
 //   GNCTLSRotationSolver::solveForRotation               teaser/src/registration.cc:764-866
 //   utils::svdRot (weighted 3x3 covariance + SVD)        teaser/include/teaser/utils.h:121-136
@@ -19,7 +19,7 @@ namespace tzr {
 
 namespace {
 
-constexpr int kRTThreads = 128;  // 128 regs x 128 threads: 4 CTAs/SM (256 threads: 2), measured 0.625 vs 0.655 ms per 1024 problems
+constexpr int kRTThreads = 128;  // 128 regs x 128 threads: 4 CTAs/SM (256 threads: 2)
 constexpr int kRTWarps = kRTThreads / 32;
 
 // ---- 3x3 helpers (column-major like Eigen::Matrix3d) -------------------------------------------

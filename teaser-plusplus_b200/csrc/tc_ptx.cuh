@@ -1,7 +1,7 @@
-// Thin inline-PTX wrappers for the sm_100a features the tensor-core graph kernel uses:
-// mbarrier, 1-D bulk async copy (TMA engine, SASS UBLKCP), TMEM allocation, tcgen05.mma (kind::tf32, SASS UTCHMMA),
-// tcgen05.commit, tcgen05.ld (SASS LDTM).  No CUTLASS dependency; field layouts follow the PTX ISA descriptor
-// tables (shared-memory matrix descriptor, instruction descriptor).
+// Thin inline-PTX wrappers for the sm_90a features the tensor-core graph kernel uses:
+// mbarrier, 1-D bulk async copy (TMA engine, SASS UBLKCP), warpgroup MMA (wgmma.mma_async kind tf32, SASS HGMMA) with
+// both operands in shared memory and the accumulators in registers.  No CUTLASS dependency; field layouts follow the
+// PTX ISA's shared-memory matrix descriptor table.
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -36,15 +36,10 @@ __device__ __forceinline__ bool mbar_try_wait(uint32_t bar, uint32_t parity) {
   return ok != 0;
 }
 // Spins until the phase with the given parity has completed.  try_wait suspends the thread in hardware for a
-// bounded time, so this is not a hot spin.  `guard` (optional, debug) bounds the number of polls.
+// bounded time, so this is not a hot spin.
 __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
   while (!mbar_try_wait(bar, parity)) {
   }
-}
-__device__ __forceinline__ bool mbar_wait_bounded(uint32_t bar, uint32_t parity, unsigned long long max_polls) {
-  for (unsigned long long it = 0; it < max_polls; ++it)
-    if (mbar_try_wait(bar, parity)) return true;
-  return false;
 }
 
 // ---- bulk async copy global -> shared (TMA engine), completion on an mbarrier ------------------------
@@ -54,43 +49,9 @@ __device__ __forceinline__ void bulk_g2s(uint32_t dst_smem, const void* src_gmem
                : "memory");
 }
 
-// ---- TMEM ---------------------------------------------------------------------------------------------
-template <int kCols>
-__device__ __forceinline__ void tmem_alloc(uint32_t dst_smem) {  // whole warp
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(dst_smem), "n"(kCols) : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-template <int kCols>
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr) {  // whole warp
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "n"(kCols) : "memory");
-}
-__device__ __forceinline__ void fence_before_sync() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void fence_after_sync() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tmem_wait_ld() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-
-// 32 lanes x 32 columns of 32-bit: thread t of the warp receives lane (base lane + t), columns [col, col+32).
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t (&r)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]),
-        "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]),
-        "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr)
-      : "memory");
-}
-
-// 32 lanes x 16 columns
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, uint32_t (&r)[16]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr)
-      : "memory");
+// ---- named barrier over a subset of the CTA's warps -------------------------------------------------
+__device__ __forceinline__ void named_bar_sync(uint32_t id, uint32_t threads) {
+  asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(threads) : "memory");
 }
 
 // ---- descriptors -----------------------------------------------------------------------------------
@@ -98,35 +59,38 @@ __device__ __forceinline__ void tmem_ld16(uint32_t taddr, uint32_t (&r)[16]) {
 // 16-byte core matrices (rows 16 B apart inside a core matrix);
 //   leading byte offset (bits 16-29, >>4) = distance between the two 16-byte K-chunks of one K=8 (tf32) step,
 //   stride  byte offset (bits 32-45, >>4) = distance between consecutive 8-row groups,
-//   bits 46-47 = 0b01 (sm_100 descriptor version), bits 61-63 = 0 (no swizzle).
+//   base offset (bits 49-51) = 0, layout type (bits 62-63) = 0 (no swizzle).
 __device__ __forceinline__ uint64_t make_smem_desc(uint32_t smem_addr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
   uint64_t d = 0;
   d |= (uint64_t)((smem_addr >> 4) & 0x3FFFu);
   d |= (uint64_t)((lbo_bytes >> 4) & 0x3FFFu) << 16;
   d |= (uint64_t)((sbo_bytes >> 4) & 0x3FFFu) << 32;
-  d |= (uint64_t)1 << 46;
   return d;
 }
-// Instruction descriptor for kind::tf32: D = F32 (bits 4-5 = 1), A = B = TF32 (bits 7-9, 10-12 = 2), both K-major
-// (bits 15, 16 = 0), N >> 3 at bits 17-22, M >> 4 at bits 24-28.
-__host__ __device__ constexpr uint32_t make_idesc_tf32(int M, int N) {
-  return (1u << 4) | (2u << 7) | (2u << 10) | ((uint32_t)(N >> 3) << 17) | ((uint32_t)(M >> 4) << 24);
-}
 
-// D[tmem] (+)= A[smem] * B[smem]^T, one K = 8 step of tf32; issued by ONE thread on behalf of the CTA.
-__device__ __forceinline__ void mma_tf32(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc, uint32_t idesc, bool accumulate) {
+// ---- warpgroup MMA ---------------------------------------------------------------------------------
+// Keeps the compiler from moving accesses of an accumulator register across the asynchronous MMA.
+__device__ __forceinline__ void acc_fence(float& r) { asm volatile("" : "+f"(r)::"memory"); }
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_wait_all() { asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory"); }
+
+// D (+)= A[smem] * B[smem]^T, one K = 8 step of tf32, M = 64 (this warpgroup's rows), N = 64; issued by all 128 threads
+// of the warpgroup.  Thread t holds D rows 16 (t/32) + (t%32)/4 (+8), columns 8 i + 2 (t%4) (+1): d[4i + 2r + c].
+__device__ __forceinline__ void wgmma_m64n64k8_tf32(float (&d)[32], uint64_t a_desc, uint64_t b_desc, bool accumulate) {
   const uint32_t acc = accumulate ? 1u : 0u;
   asm volatile(
       "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n\t}"
-      :
-      : "r"(d_tmem), "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(acc)
+      "setp.ne.b32 p, %34, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n64k8.f32.tf32.tf32 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, p, 1, 1;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]),
+        "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]),
+        "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]),
+        "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+      : "l"(a_desc), "l"(b_desc), "r"(acc)
       : "memory");
-}
-// Makes the mbarrier track completion of every tcgen05.mma this thread has issued so far (arrive::one when done).
-__device__ __forceinline__ void mma_commit(uint32_t bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
 }
 
 }  // namespace tc

@@ -1,4 +1,4 @@
-// B200 build of the reference's C++ quick-start (examples/teaser_cpp_ply/teaser_cpp_ply.cc): the solver-facing
+// GPU build of the reference's C++ quick-start (examples/teaser_cpp_ply/teaser_cpp_ply.cc): the solver-facing
 // lines (PLYReader, Params, constructor, solve, getSolution) are written exactly as a TEASER++ user writes them.
 //   usage: example_cpp_ply <bun_zipper_res3.ply>
 #include <chrono>

@@ -1,4 +1,4 @@
-"""B200 build of the reference's Python quick-start (examples/teaser_python_ply/teaser_python_ply.py): the
+"""GPU build of the reference's Python quick-start (examples/teaser_python_ply/teaser_python_ply.py): the
 `teaserpp_python` lines (Params, solver, solve, getSolution) are exactly what a TEASER++ user writes; only the PLY
 reader (open3d in the reference) is replaced by this repo's 20-line ASCII parser and the RNG is seeded.
 

@@ -1,5 +1,5 @@
 // Descriptor containers of the TEASER++ public API (mirrors teaser/include/teaser/fpfh.h:19-21 of the reference, where
-// FPFHCloud is pcl::PointCloud<pcl::FPFHSignature33>).  PCL is not a dependency of the B200 path: the two types below
+// FPFHCloud is pcl::PointCloud<pcl::FPFHSignature33>).  PCL is not a dependency of the GPU path: the two types below
 // have the layout the matcher needs (33 floats per point, `histogram` member like pcl::FPFHSignature33, a
 // std::vector-like cloud), so code that fills or iterates descriptors compiles unchanged.  FPFHEstimation keeps the
 // reference's computeFPFHFeatures / getNormals (fpfh.h:23-57); the work (PCL's NormalEstimationOMP + FPFHEstimationOMP

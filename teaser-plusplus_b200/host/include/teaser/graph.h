@@ -1,6 +1,6 @@
 // teaser::Graph / teaser::MaxCliqueSolver — the public graph façade of the reference
 // (teaser/include/teaser/graph.h:29-279), kept source compatible.  Graph is the same adjacency-list
-// container; MaxCliqueSolver::findMaxClique forwards to the B200 C-ABI (tzr_max_clique) instead of PMC.
+// container; MaxCliqueSolver::findMaxClique forwards to the GPU C-ABI (tzr_max_clique) instead of PMC.
 #pragma once
 #include <algorithm>
 #include <map>

@@ -1,4 +1,4 @@
-// teaser::RobustRegistrationSolver — the drop-in C++ surface of the B200 path.
+// teaser::RobustRegistrationSolver — the drop-in C++ surface of the GPU path.
 //
 // Source compatible with the reference header teaser/include/teaser/registration.h (class and member names,
 // Params fields and defaults, enum values, getters), but every computation is forwarded to the C-ABI
@@ -249,7 +249,7 @@ class RobustRegistrationSolver {
   void reset(const Params& params);
   Params getParams() { return params_; }
 
-  // B200 extras (not in the reference)
+  // GPU extras (not in the reference)
   // Many independent problems in one call: the batch is cut into shards and every shard is solved on its own GPU
   // (tzr_solve_batch_multi: one context + host thread per device inside the library, no collective) with this
   // solver's Params.  devices empty = every visible device.  cliques (optional) receives the sorted max-clique index

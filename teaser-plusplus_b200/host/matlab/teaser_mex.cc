@@ -1,4 +1,4 @@
-// MATLAB MEX entry point `teaser_solve_mex` for the B200 path — same positional contract as the reference's
+// MATLAB MEX entry point `teaser_solve_mex` for the GPU path — same positional contract as the reference's
 // matlab/teaser_mex.cc:19-38,99-244:
 //   [s, R, t, time_ms] = teaser_solve_mex(src(3xN), dst(3xN), cbar2, noise_bound, estimate_scaling(logical),
 //                                         rot_alg(0 GNC_TLS | 1 FGR | 2 QUATRO), rotation_gnc_factor,
@@ -45,7 +45,7 @@ void mexFunction(int nlhs, mxArray* plhs[], int nrhs, const mxArray* prhs[]) {
   }
   if (!g_ctx) {
     if (tzr_ctx_create(-1, &g_ctx) != TZR_OK)
-      mexErrMsgIdAndTxt("teaserSolve:noDevice", "No usable CUDA device (the B200 path has no CPU fallback).");
+      mexErrMsgIdAndTxt("teaserSolve:noDevice", "No usable CUDA device (the GPU path has no CPU fallback).");
     mexAtExit(release_ctx);
   }
   tzr_params p;

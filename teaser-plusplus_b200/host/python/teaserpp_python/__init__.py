@@ -1,4 +1,4 @@
-"""`teaserpp_python` for the B200-native path.
+"""`teaserpp_python` for the GPU-native path.
 
 Public surface = the reference package's (python/teaserpp_python/__init__.py): the pybind11 classes re-exported from
 `_teaserpp`, the v1.0 enum aliases on the solver / certifier classes, `RobustRegistrationSolverParams` (a named tuple

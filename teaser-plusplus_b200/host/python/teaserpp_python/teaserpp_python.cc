@@ -1,4 +1,4 @@
-// pybind11 module `teaserpp_python._teaserpp` for the B200 path.  Same module / class / method / property names
+// pybind11 module `teaserpp_python._teaserpp` for the GPU path.  Same module / class / method / property names
 // as the reference binding (python/teaserpp_python/teaserpp_python.cc:25-291) so existing Python callers keep
 // working; arrays cross the boundary as numpy (3,N) float64 exactly like the reference's pybind11/eigen.h casters
 // (copied if not Fortran-contiguous).  Fixes of the reference's copy-paste slips (SURVEY Q4): the dst_* properties
@@ -53,7 +53,7 @@ py::array_t<int> irow_to_numpy(const Eigen::Matrix<int, 1, Eigen::Dynamic>& m) {
 }  // namespace
 
 PYBIND11_MODULE(_teaserpp, m) {
-  m.doc() = "Python binding for TEASER++ (B200-native solve() path)";
+  m.doc() = "Python binding for TEASER++ (GPU-native solve() path)";
 
   py::class_<teaser::RegistrationSolution>(m, "RegistrationSolution")
       .def_readwrite("valid", &teaser::RegistrationSolution::valid)
@@ -114,7 +114,7 @@ PYBIND11_MODULE(_teaserpp, m) {
            })
       .def("solve_batch",
            [](Solver& s, const std::vector<ArrD>& src, const std::vector<ArrD>& dst, const std::vector<int>& devices) {
-             // B200 extra: many independent problems in one call, sharded over the GPUs of the node inside the library
+             // GPU extra: many independent problems in one call, sharded over the GPUs of the node inside the library
              std::vector<teaser::Mat3X> a, b;
              for (const auto& x : src) a.push_back(to_mat3x(x));
              for (const auto& x : dst) b.push_back(to_mat3x(x));
@@ -171,7 +171,7 @@ PYBIND11_MODULE(_teaserpp, m) {
       .def("getSrcTIMs", [](Solver& s) { return to_numpy(s.getSrcTIMs()); })
       .def_property_readonly("dst_tims", [](Solver& s) { return to_numpy(s.getDstTIMs()); })
       .def("getDstTIMs", [](Solver& s) { return to_numpy(s.getDstTIMs()); })
-      // B200 extras
+      // GPU extras
       .def("isMaxCliqueProvenOptimal", &Solver::isMaxCliqueProvenOptimal)
       .def("getNumInlierGraphEdges", &Solver::getNumInlierGraphEdges)
       .def("getGNCRotationIterations", &Solver::getGNCRotationIterations);

@@ -53,7 +53,7 @@ CertificationResult DRSCertifier::certify(const Eigen::Matrix3d& R_solution,
   tzr_certification_result r;
   const int rc = tzr_certify(ctx, &p, R_solution.data(), src.data(), dst.data(), theta.data(), n, &r,
                              out.suboptimality_traj.data(), cap);
-  if (rc != TZR_OK) fail("teaser::DRSCertifier (B200)", rc, ctx);
+  if (rc != TZR_OK) fail("teaser::DRSCertifier (GPU)", rc, ctx);
   out.suboptimality_traj.resize(r.n_iterations);
   out.is_optimal = r.is_optimal != 0;
   out.best_suboptimality = r.best_suboptimality;
@@ -86,7 +86,7 @@ void DRSCertifier::getOptimalDualProjection(const Eigen::MatrixXd& W,
   W_dual->resize(W.rows(), W.cols());
   tzr_ctx* ctx = b200_context();
   const int rc = tzr_certifier_dual_projection(ctx, W.data(), theta_prepended.data() + 1, n, W_dual->data());
-  if (rc != TZR_OK) fail("teaser::DRSCertifier::getOptimalDualProjection (B200)", rc, ctx);
+  if (rc != TZR_OK) fail("teaser::DRSCertifier::getOptimalDualProjection (GPU)", rc, ctx);
 }
 
 void DRSCertifier::getInitialMatrix(const Eigen::Matrix3d& R_solution,
@@ -100,7 +100,7 @@ void DRSCertifier::getInitialMatrix(const Eigen::Matrix3d& R_solution,
   const tzr_certifier_params p = to_c(params_);
   const int rc = tzr_certifier_initial_matrix(ctx, &p, R_solution.data(), src.data(), dst.data(), theta.data(), n,
                                               M_init->data(), mu);
-  if (rc != TZR_OK) fail("teaser::DRSCertifier::getInitialMatrix (B200)", rc, ctx);
+  if (rc != TZR_OK) fail("teaser::DRSCertifier::getInitialMatrix (GPU)", rc, ctx);
 }
 
 }  // namespace teaser

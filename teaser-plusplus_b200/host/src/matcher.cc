@@ -40,7 +40,7 @@ std::vector<std::pair<int, int>> Matcher::calculateCorrespondences(const PointCl
                                            tuple_scale, tuple_seed_, pairs.data(), static_cast<int64_t>(ns) + nd,
                                            &n_pairs, &global_scale_);
   if (rc != TZR_OK)
-    throw std::runtime_error(std::string("teaser::Matcher (B200): ") + tzr_status_string(rc) + " (" +
+    throw std::runtime_error(std::string("teaser::Matcher (GPU): ") + tzr_status_string(rc) + " (" +
                              tzr_last_error(ctx) + ")");
   tuple_seed_ += 0x9E3779B97F4A7C15ull;  // a fresh stream for the next call, like successive time(NULL) seeds
   corres_.reserve(static_cast<size_t>(n_pairs));
@@ -62,7 +62,7 @@ FPFHCloudPtr FPFHEstimation::computeFPFHFeatures(const PointCloud& input_cloud, 
   const int rc = tzr_compute_fpfh(ctx, &input_cloud[0].x, n, normal_search_radius, fpfh_search_radius,
                                   (*descriptors)[0].histogram, &normals_[0].normal_x);
   if (rc != TZR_OK)
-    throw std::runtime_error(std::string("teaser::FPFHEstimation (B200): ") + tzr_status_string(rc) + " (" +
+    throw std::runtime_error(std::string("teaser::FPFHEstimation (GPU): ") + tzr_status_string(rc) + " (" +
                              tzr_last_error(ctx) + ")");
   return descriptors;
 }

@@ -58,7 +58,7 @@ tzr_ctx* b200_context() {
   thread_local Holder h;
   if (!h.c) {
     int rc = tzr_ctx_create(-1, &h.c);
-    if (rc != TZR_OK) fail("teaser (B200): cannot create a CUDA context", rc, nullptr);
+    if (rc != TZR_OK) fail("teaser (GPU): cannot create a CUDA context", rc, nullptr);
   }
   return h.c;
 }

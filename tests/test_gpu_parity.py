@@ -1,4 +1,4 @@
-"""GPU parity tests (run on the B200 box: `pytest -m gpu`).  Every call goes through the C-ABI
+"""GPU parity tests (run on an H100: `pytest -m gpu`).  Every call goes through the C-ABI
 (libteaser_b200.so via ctypes); the oracle is the checker."""
 import importlib
 import os
