@@ -266,7 +266,8 @@ int tzr_solve_batch_multi(const int32_t* devices, int n_devices, const tzr_param
  * bit 1 (2) = verify the FP32 / tensor-core filter against FP64 for every pair and count mismatches,
  * bit 2 (4) = count exact re-checks and clique search nodes, bit 8 (256) = degrees by a separate pass,
  * bit 10 (1024) = build the graph with the tensor-core kernel (wgmma Gram norms; bit-identical to the default CUDA-core
- * kernel: DESIGN.md 3.1), bit 9 (512) overrides it, bit 11 (2048) = the one-MUFU
+ * kernel: DESIGN.md 3.1), bit 9 (512) = the square-root interval test for every problem (no Gram test, no tensor-core
+ * kernel; bit-identical), bit 11 (2048) = the one-MUFU
  * CUDA-core variant (graph_strip3_kernel; bit-identical), bit 13 (8192) = exact clique
  * search without the singleton-class path of the colouring (A/B), bit 12 (4096) = without the block colour bound (only
  * present in builds with -DTZR_BLOCK_BOUND). */

@@ -180,6 +180,23 @@ __global__ void __launch_bounds__(256) prep_kernel(Batch bt) {
       gc.tc_c0 = (float)(c0 * up);
       gc.tc_pad = 0.f;
       if (ok && bt.rechecks) atomicAdd(bt.mismatches + 7, 1ull);  // debug counter 7: problems on the tensor-core path
+      // ---- Gram-form test of graph_strip2_kernel (derivation in DESIGN.md §3.1).  a' = fl(N_i + N_j - 2 q_i.q_j) from the
+      // float copies q (|q| <= R, R^2 <= Ds2 / 4 about the box centre) is within 8 u R^2 (conversion) + 2 u R^2 (rounded
+      // norms) + 14 u R^2 (one FADD and three FMA roundings on partial sums of at most 2 R^2 and 4 R^2) of a; 28 u R^2 is
+      // used, the rest covers second-order terms and the reference's own FP64 rounding.  With E = ea + eb, k = E / lam,
+      // C = E lam + E^2 + 2 beta^2 E and 4 u (t^2 + |m| S + |c|) the FP32 evaluation error of fma(t, t, fma(s, m, c)):
+      //   t^2 + mhi s + chi <= 0  =>  (1 + k) t^2 - 2 beta^2 s + beta^4 + C <= 0  =>  f(a, b) <= 0           (edge)
+      //   t^2 + mlo s + clo >= 0  =>  (1 - k) t^2 - 2 beta^2 s - C > 0            =>  f(a, b) > beta^4      (s > beta^2: not)
+      const double gE = 7.0 * u32 * (Ds2 + Dd2), gk = gE / lam, gS = Ds2 + Dd2 + gE;
+      const double gC = gE * lam + gE * gE + 2.0 * b2 * gE;
+      gc.g_mhi = (float)(-2.0 * b2 * (1.0 - 4.0 * u32) / (1.0 + gk) * dn);
+      gc.g_chi = (float)(((b4 + gC) / (1.0 + gk) + 8.0 * u32 * b2 * gS) * up);
+      gc.g_mlo = (float)(-2.0 * b2 * (1.0 + 4.0 * u32) / (1.0 - gk) * up);
+      gc.g_clo = (float)(-(gC + 9.0 * u32 * b2 * gS) / (1.0 - gk) * up * up);
+      // conditioning guard (same form as use_tc's): beta <= D/8 keeps pairs with s <= beta^2 rare, 64 E <= 0.75 D beta keeps
+      // the band narrow against beta (and k <= 1/64).  C1 (outliers moved 5-10 extents away, beta/D ~ 1e-4) fails it.
+      gc.use_gram = (!use64 && (bt.flags_dbg & 512u) == 0 && Ds2 > 0 && Dd2 > 0 && Ds2 < 1e8 && Dd2 < 1e8 && b4 > 1e-30 &&
+                     isfinite(gE) && 8.0 * beta <= Dmin && 64.0 * gE <= 0.75 * Dmin * beta) ? 1 : 0;
     }
     bt.gc[b] = gc;
     bt.n_edges2[b] = 0ull;
@@ -192,11 +209,11 @@ __global__ void __launch_bounds__(256) prep_kernel(Batch bt) {
     a.x = (float)((src[3 * i + 0] - s_c[0]) * s_c[6]);
     a.y = (float)((src[3 * i + 1] - s_c[1]) * s_c[6]);
     a.z = (float)((src[3 * i + 2] - s_c[2]) * s_c[6]);
-    a.w = 0.f;
+    a.w = (float)((double)a.x * a.x + (double)a.y * a.y + (double)a.z * a.z);  // squares exact in FP64: one rounding
     c.x = (float)(dst[3 * i + 0] - s_c[3]);
     c.y = (float)(dst[3 * i + 1] - s_c[4]);
     c.z = (float)(dst[3 * i + 2] - s_c[5]);
-    c.w = 0.f;
+    c.w = (float)((double)c.x * c.x + (double)c.y * c.y + (double)c.z * c.z);
     sf[i] = a;
     df[i] = c;
     bt.deg[(size_t)b * n + i] = 0;  // accumulated by the graph kernel (fused-degree path)
@@ -630,28 +647,17 @@ struct __align__(16) IPointNeg2 {
   float4 c;  // (-dy,-dy,-dz,-dz)
 };
 
-// kFuseDeg: vertex degrees are accumulated here (row part: one atomic per row and strip; column part: one 32-lane
-// RED per transposed word) instead of a second pass over the B*n^2/8-byte bitset; deg[] is zeroed by prep_kernel.
-template <bool kVerify, int kMinBlocks, bool kFuseDeg>
-__global__ void __launch_bounds__(kGraphThreads, kMinBlocks) graph_strip2_kernel(Batch bt) {
-  const int b = blockIdx.y;
+// Interval test of graph_strip2_kernel, for the problems that fail the Gram test's conditioning guard (and for every
+// problem under debug flags 1 and 512).  kFuseDeg: vertex degrees are accumulated here (row part: one atomic per row and
+// strip; column part: one 32-lane RED per transposed word) instead of a second pass over the B*n^2/8-byte bitset; deg[] is
+// zeroed by prep_kernel.
+template <bool kVerify, bool kFuseDeg>
+__device__ __forceinline__ void strip_interval(const Batch& bt, const int b, const int I, const int J0, const int J1) {
   const int n = bt.n;
-  const int nt = (n + kTile - 1) / kTile;
-  int I = 0, p = blockIdx.x;
-  while (true) {
-    const int ng = (nt - I + kStripBlocks - 1) / kStripBlocks;
-    if (p < ng) break;
-    p -= ng;
-    ++I;
-  }
-  const int J0 = I + p * kStripBlocks;
-  const int J1 = min(nt, J0 + kStripBlocks);
-
   __shared__ IPointNeg2 s_ip[kTile];
   __shared__ __align__(16) uint32_t s_rw[kTile][4];
 
   const GraphConsts* gcp = bt.gc + b;
-  if (bt.tc_active && gcp->use_tc) return;  // built by graph_tc_kernel
   const float b1 = gcp->b1, b2 = gcp->b2;
   const double beta = gcp->beta;
   const bool scale_mode = bt.scale_mode != 0;
@@ -804,6 +810,192 @@ __global__ void __launch_bounds__(kGraphThreads, kMinBlocks) graph_strip2_kernel
     __syncwarp();
   }
   if (kFuseDeg && lane < nrows && rdeg) atomicAdd(degp + ibase + lane, rdeg);
+}
+
+// Gram test of graph_strip2_kernel (problems with gc.use_gram; DESIGN.md §3.1).  Per pair, on the centred float copies:
+//   a = fma(z_j, -2 z_i, fma(y_j, -2 y_i, fma(x_j, -2 x_i, N_i + N_j))), b the same on the destination cloud,
+//   t = a - b, s = a + b,  d_hi = fma(t, t, fma(s, mhi, chi)),  d_lo = fma(t, t, fma(s, mlo, clo))
+// = 14 FP32 operations and two funnel shifts that move the sign bits into the lane's column words: sign(d_hi) = 1 proves
+// an edge, sign(d_lo) = 0 a non-edge.  No square root, no compare, no vote.  Column points (x, y, z, N), (u, v, w, M) stay
+// in registers; row points are broadcast from a warp-private slice as (-2x, -2y, -2z, N), (-2u, -2v, -2w, M).  The
+// undecided pairs (lo & ~hi, a few per million) keep bit 0 and are queued for tc_patch_kernel; a full queue is evaluated
+// in place.  Row words come from the warp-shuffle bit transpose of the column words.
+template <bool kVerify, bool kFuseDeg>
+__device__ __forceinline__ void strip_gram(const Batch& bt, const int b, const int I, const int J0, const int J1) {
+  const int n = bt.n;
+  __shared__ float4 s_gr[2 * kTile];
+
+  const GraphConsts* gcp = bt.gc + b;
+  const float mhi = gcp->g_mhi, chi = gcp->g_chi, mlo = gcp->g_mlo, clo = gcp->g_clo;
+  const double beta = gcp->beta;
+  const bool scale_mode = bt.scale_mode != 0;
+  const double s_hat = scale_mode ? bt.sol[b].scale : 1.0;
+
+  const float4* sf = bt.sf + (size_t)b * n;
+  const float4* df = bt.df + (size_t)b * n;
+  const double* src = bt.src + (size_t)b * n * 3;
+  const double* dst = bt.dst + (size_t)b * n * 3;
+
+  const int tid = threadIdx.x, w = tid >> 5, lane = tid & 31;
+  const int ibase = I * kTile + 32 * w;
+  const int nrows = min(32, n - ibase);
+  if (nrows <= 0) return;
+  const float4 z4 = make_float4(0.f, 0.f, 0.f, 0.f);
+  {
+    const int i = ibase + lane;
+    const float4 s = (i < n) ? sf[i] : z4, d = (i < n) ? df[i] : z4;
+    s_gr[2 * tid] = make_float4(-2.f * s.x, -2.f * s.y, -2.f * s.z, s.w);
+    s_gr[2 * tid + 1] = make_float4(-2.f * d.x, -2.f * d.y, -2.f * d.z, d.w);
+  }
+  __syncwarp();
+  uint32_t* adj32 = reinterpret_cast<uint32_t*>(bt.adj) + (size_t)b * n * pitch32(n);
+  const int P32 = pitch32(n);
+  const uint32_t rmask = nrows >= 32 ? 0xffffffffu : ((1u << nrows) - 1u);
+  const float4* rows = s_gr + 2 * 32 * w;
+
+  int* degp = bt.deg + (size_t)b * n;
+  int rdeg = 0;
+  for (int J = J0; J < J1; ++J) {
+    const int jb = J * kTile + lane;
+    float4 cs[4], cd[4];
+    bool vj[4];
+#pragma unroll
+    for (int c = 0; c < 4; ++c) {
+      const int j = jb + 32 * c;
+      vj[c] = j < n;
+      cs[c] = vj[c] ? sf[j] : z4;
+      cd[c] = vj[c] ? df[j] : z4;
+    }
+    // column words of this lane: bit ii = pair (row ibase+ii, column jb + 32c); hi = surely an edge, lo = edge or undecided
+    uint32_t hi[4] = {0u, 0u, 0u, 0u}, lo[4] = {0u, 0u, 0u, 0u};
+    // rows are visited from the last to the first so that the funnel shift leaves row ii at bit ii
+#pragma unroll 4
+    for (int ii = 31; ii >= 0; --ii) {
+      const float4 rs = rows[2 * ii], rd = rows[2 * ii + 1];
+#pragma unroll
+      for (int c = 0; c < 4; ++c) {
+        float a = __fadd_rn(rs.w, cs[c].w);
+        a = __fmaf_rn(cs[c].x, rs.x, a);
+        a = __fmaf_rn(cs[c].y, rs.y, a);
+        a = __fmaf_rn(cs[c].z, rs.z, a);
+        float bb = __fadd_rn(rd.w, cd[c].w);
+        bb = __fmaf_rn(cd[c].x, rd.x, bb);
+        bb = __fmaf_rn(cd[c].y, rd.y, bb);
+        bb = __fmaf_rn(cd[c].z, rd.z, bb);
+        const float t = __fsub_rn(a, bb), s = __fadd_rn(a, bb);
+        const float dh = __fmaf_rn(t, t, __fmaf_rn(s, mhi, chi));
+        const float dl = __fmaf_rn(t, t, __fmaf_rn(s, mlo, clo));
+        hi[c] = __funnelshift_l(__float_as_uint(dh), hi[c], 1);
+        lo[c] = __funnelshift_l(__float_as_uint(dl), lo[c], 1);
+      }
+    }
+    // ---- validity (rows < n, columns < n, i != j), undecided pairs, tentative column words
+    uint32_t colw[4];
+    int nflag = 0;
+#pragma unroll
+    for (int c = 0; c < 4; ++c) {
+      uint32_t vm = vj[c] ? rmask : 0u;
+      if (I == J && c == w) vm &= ~(1u << lane);  // column 32c + lane of the diagonal block meets row 32w + lane
+      const uint32_t fm = lo[c] & ~hi[c] & vm;
+      colw[c] = hi[c] & vm;
+      if (kVerify) {  // every DECIDED pair is re-evaluated exactly; disagreements are counted (must stay 0)
+        uint32_t dm = vm & ~fm;
+        int bad = 0;
+        while (dm) {
+          const int ii = __ffs(dm) - 1;
+          dm &= dm - 1;
+          const int i = ibase + ii, j = jb + 32 * c;
+          const bool ex = scale_mode ? edge_exact_scale(src, dst, i, j, beta, s_hat) : edge_exact(src, dst, i, j, beta);
+          bad += (ex != (((colw[c] >> ii) & 1u) != 0u));
+        }
+        if (bad) atomicAdd(bt.mismatches, (unsigned long long)bad);
+      }
+      lo[c] = fm;  // re-used: undecided mask of column c
+      nflag += __popc(fm);
+    }
+    if (__any_sync(0xffffffffu, nflag != 0)) {
+      // ---- rare: queue the undecided pairs for tc_patch_kernel (their tentative bit is 0); queue full: exact here
+      int incl = nflag;
+#pragma unroll
+      for (int o = 1; o < 32; o <<= 1) {
+        const int v = __shfl_up_sync(0xffffffffu, incl, o);
+        if (lane >= o) incl += v;
+      }
+      const int total = __shfl_sync(0xffffffffu, incl, 31);
+      unsigned int base = 0;
+      if (lane == 0) base = atomicAdd(bt.tc_list_count, (unsigned int)total);
+      base = __shfl_sync(0xffffffffu, base, 0);
+      const bool queued = base + (unsigned int)total <= bt.tc_list_cap;
+      unsigned int pos = base + (unsigned int)(incl - nflag);
+      if (!queued)  // the first warp that does not fit leaves [base, cap) unwritten: void entries for the patch kernel
+        for (unsigned int q = base + (unsigned int)lane; q < bt.tc_list_cap; q += 32u) bt.tc_list[q] = make_uint2(0xffffffffu, 0u);
+      int nre = 0;
+#pragma unroll
+      for (int c = 0; c < 4; ++c) {
+        uint32_t fm = lo[c];
+        const int j = jb + 32 * c;
+        while (fm) {
+          const int ii = __ffs(fm) - 1;
+          fm &= fm - 1;
+          const int i = ibase + ii;
+          if (queued) {
+            // the patch kernel flips bit (i, j) and, off the diagonal block, its mirror; the diagonal block holds both
+            // orientations as separate pairs, each queued by the lane that owns its column
+            bt.tc_list[pos++] = make_uint2((unsigned int)b, ((unsigned int)i << 16) | (unsigned int)j);
+          } else {
+            const bool ex = scale_mode ? edge_exact_scale(src, dst, i, j, beta, s_hat) : edge_exact(src, dst, i, j, beta);
+            colw[c] |= (ex ? 1u : 0u) << ii;
+            ++nre;
+          }
+        }
+      }
+      if (bt.rechecks && !queued) {
+        nre = __reduce_add_sync(0xffffffffu, nre);
+        if (lane == 0 && nre) atomicAdd(bt.rechecks, (unsigned long long)nre);
+      }
+    }
+    // ---- row words (lane = row ibase + lane) by transposition; stores; fused degrees
+    uint32_t roww[4];
+#pragma unroll
+    for (int c = 0; c < 4; ++c) roww[c] = warp_transpose32(colw[c], lane);
+    if (lane < nrows)
+      *reinterpret_cast<uint4*>(adj32 + (size_t)(ibase + lane) * P32 + 4 * J) =
+          make_uint4(roww[0], roww[1], roww[2], roww[3]);
+    if (kFuseDeg) rdeg += __popc(roww[0]) + __popc(roww[1]) + __popc(roww[2]) + __popc(roww[3]);
+    if (I != J) {
+#pragma unroll
+      for (int c = 0; c < 4; ++c)
+        if (vj[c]) {
+          adj32[(size_t)(jb + 32 * c) * P32 + 4 * I + w] = colw[c];
+          if (kFuseDeg && colw[c]) atomicAdd(degp + jb + 32 * c, __popc(colw[c]));
+        }
+    }
+  }
+  if (kFuseDeg && lane < nrows && rdeg) atomicAdd(degp + ibase + lane, rdeg);
+}
+
+// graph strip kernel (default): one launch for the whole batch; each problem runs the Gram test or the interval test, as
+// prep_kernel chose (CTA-uniform: a strip belongs to one problem).  Undecided pairs of the Gram test are settled by
+// tc_patch_kernel afterwards (launch_graph).
+template <bool kVerify, int kMinBlocks, bool kFuseDeg>
+__global__ void __launch_bounds__(kGraphThreads, kMinBlocks) graph_strip2_kernel(Batch bt) {
+  const int b = blockIdx.y;
+  const int nt = (bt.n + kTile - 1) / kTile;
+  int I = 0, p = blockIdx.x;
+  while (true) {
+    const int ng = (nt - I + kStripBlocks - 1) / kStripBlocks;
+    if (p < ng) break;
+    p -= ng;
+    ++I;
+  }
+  const int J0 = I + p * kStripBlocks;
+  const int J1 = min(nt, J0 + kStripBlocks);
+  const GraphConsts* gcp = bt.gc + b;
+  if (bt.tc_active && gcp->use_tc) return;  // built by graph_tc_kernel
+  if (gcp->use_gram)
+    strip_gram<kVerify, kFuseDeg>(bt, b, I, J0, J1);
+  else
+    strip_interval<kVerify, kFuseDeg>(bt, b, I, J0, J1);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -1093,9 +1285,10 @@ int launch_graph(const Batch& bt0, cudaStream_t st, int num_sms) {
     graph_strip2_kernel<true, 5, false><<<sgrid, kGraphThreads, 0, st>>>(bt);
   else if (bt.flags_dbg & 256u)  // degrees by the separate degree kernel (A/B against the fused default)
     graph_strip2_kernel<false, 8, false><<<sgrid, kGraphThreads, 0, st>>>(bt);
-  else  // default: paired-FP32 strip kernel, 8 CTAs/SM, degrees fused
+  else  // default: Gram test (interval test where prep_kernel's guard fails), 8 CTAs/SM, degrees fused
     graph_strip2_kernel<false, 8, true><<<sgrid, kGraphThreads, 0, st>>>(bt);
-  if (v7) {  // exact re-check of the pairs the strip kernel queued
+  // exact re-check of the pairs the strip kernel queued (v7, or the Gram test: every problem unless debug flag 512)
+  if (v7 || !(bt.flags_dbg & 512u)) {
     launch_graph_patch(bt, st, num_sms);
     ++launches;
   }

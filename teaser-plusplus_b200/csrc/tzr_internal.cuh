@@ -55,6 +55,10 @@ struct GraphConsts {
   float tc_b4;    // beta^4
   float tc_kap, tc_c0;  // |d| <= kap (t^2 + beta^4) + c0 : undecided -> exact FP64 re-check   (t = a - b)
   float tc_pad;
+  // Gram-form test of graph_strip2_kernel (DESIGN.md §3.1): with a', b' the FP32 Gram-form squared norms, t = a' - b',
+  // s = a' + b':  t^2 + g_mhi s + g_chi <= 0 proves an edge, t^2 + g_mlo s + g_clo >= 0 proves a non-edge
+  int use_gram;   // 1: the conditioning guard holds, the strip kernel runs the Gram test; 0: the sqrt interval test (b1, b2)
+  float g_mhi, g_chi, g_mlo, g_clo;
 };
 
 // Everything the device kernels need to know about one batch (passed by value).
@@ -68,7 +72,7 @@ struct Batch {
   double beta;    // 2*noise_bound*sqrt(cbar2)  (registration.cc:438)
   const double* src;  // B*n*3
   const double* dst;  // B*n*3
-  float4* sf;     // B*n centred float copies (w unused)
+  float4* sf;     // B*n centred float copies; w = their squared norm, rounded to float (Gram-form test)
   float4* df;
   float* opnd;    // B * ceil(n/128) * 2 roles * 2 clouds * 6 planes * 128 rows * 4: tf32-split MMA operand tiles of the
                   // tensor-core graph kernel (graph_tc.cu), written by tc_prep_kernel
