@@ -270,7 +270,9 @@ int tzr_solve_batch_multi(const int32_t* devices, int n_devices, const tzr_param
  * kernel; bit-identical), bit 11 (2048) = the one-MUFU
  * CUDA-core variant (graph_strip3_kernel; bit-identical), bit 13 (8192) = exact clique
  * search without the singleton-class path of the colouring (A/B), bit 12 (4096) = without the block colour bound (only
- * present in builds with -DTZR_BLOCK_BOUND). */
+ * present in builds with -DTZR_BLOCK_BOUND), bit 14 (16384) = cap the graph kernels' re-check queue at 64 entries (the
+ * buffer keeps its full size), so that the queue-full path (pairs evaluated in place by the graph kernel) runs at test
+ * sizes; bit-identical. */
 int tzr_ctx_set_flags(tzr_ctx* ctx, uint32_t flags);
 int64_t tzr_ctx_filter_mismatches(tzr_ctx* ctx);
 /* Number of pairs of the most recent graph build that needed the exact FP64 re-check. */
@@ -279,7 +281,8 @@ int64_t tzr_ctx_filter_rechecks(tzr_ctx* ctx);
  * search nodes, [3] reduce rounds, [4] vertices scanned by reduce rounds, [5] colourings, [6] vertices coloured,
  * [7] problems whose graph was built by the tensor-core kernel, [8]-[10] clock cycles of the exact search in the root
  * colour bound / degree rules / colourings, [11] slowest root (ns << 16 | vertex), [12] summed root time (ns),
- * [13] roots above 1 ms, [14] roots closed by the block colour bound. */
+ * [13] roots above 1 ms, [14] roots closed by the block colour bound, [15] problems whose graph the default CUDA-core
+ * kernel built with the Gram-form test (not the interval test, the tensor-core kernel or the flag-2048 kernel). */
 int tzr_ctx_debug_counters(tzr_ctx* ctx, int64_t* out16);
 
 #ifdef __cplusplus

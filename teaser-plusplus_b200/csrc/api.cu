@@ -158,6 +158,9 @@ int setup_batch(tzr_ctx* ctx, int B, int n, bool own_points, Batch* out, bool co
   ENS(opnd, tc_operand_bytes(B, n));
   bt.tc_list_cap = (unsigned int)tc_list_entries(B, n);
   ENS(tclist, (size_t)bt.tc_list_cap * sizeof(uint2) + 256);
+  // debug flag 16384: a re-check queue of 64 entries (the buffer keeps its full size), so that the queue-full path of the
+  // graph kernels (void entries, in-place exact evaluation, the patch kernel's clamp) runs at test sizes
+  if (ctx->flags & 16384u) bt.tc_list_cap = std::min(bt.tc_list_cap, 64u);
   ENS(gc, (size_t)B * sizeof(GraphConsts));
   ENS(adj, Bn * pitch64(n) * sizeof(uint64_t));
   ENS(deg, Bn * sizeof(int32_t));
@@ -403,7 +406,6 @@ int run_pipeline(tzr_ctx* ctx, Batch& bt, const tzr_params& p, cudaEvent_t* ev, 
   }
   cudaEventRecord(ev[0], sg);
   init_solutions_kernel<<<(bt.B + 127) / 128, 128, 0, sg>>>(bt.sol, bt.B);
-  if (ctx->flags & 6u) cudaMemsetAsync((void*)ctx->dbg.p, 0, 16 * sizeof(unsigned long long), sg);
   ctx->launches += 1;
   if (bt.scale_mode) {  // before prep: the FP32 filter copies are pre-scaled by the estimate
     bt.beta = 2.0 * p.noise_bound * std::sqrt(p.cbar2);
@@ -473,6 +475,9 @@ int run_chunked(tzr_ctx* ctx, Batch& bt, const tzr_params& p, const std::vector<
     ctx->stage_ev.push_back(e);
   }
   const bool lanes = n_chunks > 1 && ctx->gstream && ctx->hstream && l2_chunk(ctx, bt.B, bt.n, p) >= bt.B;
+  // debug counters cover the whole call: zeroed once, ahead of every chunk on either lane (not per chunk, which would
+  // keep only the last chunk's counts)
+  if (ctx->flags & 6u) CK(cudaMemsetAsync((void*)ctx->dbg.p, 0, 16 * sizeof(unsigned long long), ctx->stream));
   if (lanes) {
     while ((int)ctx->gdone_ev.size() < n_chunks) {
       cudaEvent_t e;

@@ -35,6 +35,12 @@ __device__ __forceinline__ double warp_max(double v) {
   return v;
 }
 
+// launch_graph sends the problems prep_kernel marked use_tc to graph_tc_kernel only under debug flag 1024 without an A/B
+// flag (8-256) or the interval-test flag 512
+__host__ __device__ __forceinline__ bool tc_path_active(uint32_t flags) {
+  return (flags & 1024u) && !(flags & (8u | 16u | 32u | 64u | 128u | 256u | 512u));
+}
+
 __global__ void __launch_bounds__(256) prep_kernel(Batch bt) {
   const int b = blockIdx.x;
   const int n = bt.n;
@@ -197,6 +203,10 @@ __global__ void __launch_bounds__(256) prep_kernel(Batch bt) {
       // the band narrow against beta (and k <= 1/64).  C1 (outliers moved 5-10 extents away, beta/D ~ 1e-4) fails it.
       gc.use_gram = (!use64 && (bt.flags_dbg & 512u) == 0 && Ds2 > 0 && Dd2 > 0 && Ds2 < 1e8 && Dd2 < 1e8 && b4 > 1e-30 &&
                      isfinite(gE) && 8.0 * beta <= Dmin && 64.0 * gE <= 0.75 * Dmin * beta) ? 1 : 0;
+      // debug counter 15: problems graph_strip2_kernel builds with the Gram test (not those graph_tc_kernel or
+      // graph_strip3_kernel builds; launch_graph makes the same choice)
+      if (gc.use_gram && bt.rechecks && !(ok && tc_path_active(bt.flags_dbg)) && !(bt.flags_dbg & 2048u))
+        atomicAdd(bt.mismatches + 15, 1ull);
     }
     bt.gc[b] = gc;
     bt.n_edges2[b] = 0ull;
@@ -1247,7 +1257,7 @@ int launch_graph(const Batch& bt0, cudaStream_t st, int num_sms) {
   Batch bt = bt0;
   // default: CUDA-core strip kernel.  Debug flag 1024 routes every problem prep_kernel marked use_tc through the
   // tensor-core kernel instead (bit-identical output: DESIGN.md §3.1)
-  bt.tc_active = ((bt.flags_dbg & 1024u) && !(bt.flags_dbg & (8u | 16u | 32u | 64u | 128u | 256u | 512u))) ? 1 : 0;
+  bt.tc_active = tc_path_active(bt.flags_dbg) ? 1 : 0;
   int launches = 1;  // the CUDA-core strip kernel below (grid covers every problem; TC problems return at once)
   if (bt.tc_active) launches += launch_graph_tc(bt, st, num_sms);
   const int nt = (bt.n + kTile - 1) / kTile;
