@@ -116,9 +116,27 @@ int tzr_graph_build(tzr_ctx* ctx, const double* src_3xN, const double* dst_3xN, 
  * Replaces teaser::MaxCliqueSolver::findMaxClique (teaser/src/graph.cc:12-125) including the PMC
  * library calls it makes.  mode: 0 PMC_EXACT, 1 PMC_HEU, 2 KCORE_HEU.  clique: capacity n, returned
  * sorted ascending (solve() sorts it, registration.cc:636).  *proven_optimal: 1 / 2 / 0 with the meaning of
- * tzr_solution.clique_proven_optimal. */
+ * tzr_solution.clique_proven_optimal.  Input contract: the bitset must be symmetric; diagonal bits and bits at or beyond
+ * n in a row's last word are ignored (cleared on the device after the copy).  Entries of clique past *clique_size are
+ * set to -1.  This is tzr_max_clique_batch with B = 1. */
 int tzr_max_clique(tzr_ctx* ctx, const uint64_t* adj_bits, int n, int mode, double kcore_heuristic_threshold,
                    double time_limit_s, int32_t* clique, int32_t* clique_size, int32_t* proven_optimal);
+/* B independent problems of n vertices searched in one launch sequence.  adj_bits: B * n * tzr_words_per_row(n)
+ * uint64 (problem-major, same input contract as above).  cliques: B * n int32, row b sorted ascending, -1 past
+ * clique_sizes[b].  proven_optimal (B int32, may be NULL): as tzr_max_clique.  search_flags (B int32, may be NULL): the
+ * per-problem flags word the search ends with: 1 = result not proven (depth cap or budget hit), 2 = first-pass deadline
+ * (set while a problem is still open after the first pass; cleared when the second pass resumes it), 4 = closed by the
+ * vertex-cover LP bound, 8 = Nemhauser-Trotter reduction then a second pass that only accepts larger cliques; bits 8 and
+ * up hold the LP bound when 8 is set.  A result with proven_optimal 1 is the one tzr_max_clique gives for that problem
+ * alone. */
+int tzr_max_clique_batch(tzr_ctx* ctx, int B, int n, const uint64_t* adj_bits, int mode,
+                         double kcore_heuristic_threshold, double time_limit_s, int32_t* cliques, int32_t* clique_sizes,
+                         int32_t* proven_optimal, int32_t* search_flags);
+/* Diagnostics of the most recent tzr_max_clique(_batch) call on this context (TZR_ERR_INVALID_ARG once another call has
+ * reused the workspace).  geometry3: CTAs of the persistent exact-search grid, problems searched at a time (start groups
+ * of the sweep, sized so that their bitsets fit the L2), stack depth.  heuristic_best (B int32, may be NULL): per
+ * problem, the largest clique of the root-based greedy heuristic, before the peel kernel's second chance. */
+int tzr_ctx_clique_info(tzr_ctx* ctx, int32_t* geometry3, int32_t* heuristic_best);
 
 /* ---- stage 3: GNC-TLS rotation --------------------------------------------------------------
  * Replaces GNCTLSRotationSolver::solveForRotation (registration.cc:764-866) + utils::svdRot
@@ -272,7 +290,13 @@ int tzr_solve_batch_multi(const int32_t* devices, int n_devices, const tzr_param
  * search without the singleton-class path of the colouring (A/B), bit 12 (4096) = without the block colour bound (only
  * present in builds with -DTZR_BLOCK_BOUND), bit 14 (16384) = cap the graph kernels' re-check queue at 64 entries (the
  * buffer keeps its full size), so that the queue-full path (pairs evaluated in place by the graph kernel) runs at test
- * sizes; bit-identical. */
+ * sizes; bit-identical, bit 15 (32768) = a first exact clique pass of 1 ns (the second pass keeps the caller's whole
+ * budget), so that every problem that reaches the exact search goes through the vertex-cover LP kernel regardless of
+ * machine load (a problem whose whole first pass fits inside one %globaltimer tick, about 1 us or less, would still
+ * finish in it), bit 16 (65536) = an exact-search stack of 8 levels, so that the depth cap (result not proven) is
+ * reachable at test sizes, bit 17 (131072) = one exact pass with the caller's whole budget instead of 50 ms + LP bound
+ * + second pass, so that whether a canonical enumeration finishes does not depend on the wall clock (bit 15 wins when
+ * both are set).  Bits 15 to 17 change host code only. */
 int tzr_ctx_set_flags(tzr_ctx* ctx, uint32_t flags);
 int64_t tzr_ctx_filter_mismatches(tzr_ctx* ctx);
 /* Number of pairs of the most recent graph build that needed the exact FP64 re-check. */

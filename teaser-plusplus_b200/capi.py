@@ -90,12 +90,12 @@ class CertificationResult(C.Structure):
 _SYMBOLS = [
     "tzr_abi_version", "tzr_status_string", "tzr_last_error", "tzr_params_default", "tzr_ctx_create",
     "tzr_ctx_destroy", "tzr_ctx_set_stream", "tzr_ctx_synchronize", "tzr_ctx_kernel_launches", "tzr_words_per_row",
-    "tzr_graph_build", "tzr_max_clique", "tzr_gnc_tls_rotation", "tzr_rotation_solve", "tzr_tls_translation", "tzr_scalar_tls",
+    "tzr_graph_build", "tzr_max_clique", "tzr_max_clique_batch", "tzr_gnc_tls_rotation", "tzr_rotation_solve", "tzr_tls_translation", "tzr_scalar_tls",
     "tzr_solve", "tzr_solve_batch", "tzr_solve_batch_dev", "tzr_last_graph", "tzr_last_stage_ms",
     "tzr_ctx_set_flags", "tzr_ctx_filter_mismatches", "tzr_ctx_filter_rechecks", "tzr_ctx_debug_counters",
     "tzr_match_correspondences", "tzr_feature_nn", "tzr_compute_fpfh", "tzr_certifier_params_default", "tzr_certify",
     "tzr_certifier_initial_matrix", "tzr_certifier_dual_projection", "tzr_last_graph_info", "tzr_ctx_stage_log",
-    "tzr_ctx_stage_log_read", "tzr_solve_batch_multi",
+    "tzr_ctx_stage_log_read", "tzr_solve_batch_multi", "tzr_ctx_clique_info",
 ]
 
 
@@ -132,6 +132,8 @@ def lib():
     L.tzr_words_per_row.argtypes = [C.c_int]
     L.tzr_graph_build.argtypes = [vp, dp, dp, C.c_int, C.c_double, u64p, i32p, i64p]
     L.tzr_max_clique.argtypes = [vp, u64p, C.c_int, C.c_int, C.c_double, C.c_double, i32p, i32p, i32p]
+    L.tzr_max_clique_batch.argtypes = [vp, C.c_int, C.c_int, u64p, C.c_int, C.c_double, C.c_double, i32p, i32p, i32p,
+                                       i32p]
     L.tzr_gnc_tls_rotation.argtypes = [vp, dp, dp, C.c_int, C.c_double, C.c_double, C.c_uint64, C.c_double, dp, u8p,
                                        dp, i32p]
     L.tzr_rotation_solve.argtypes = [vp, C.c_int, dp, dp, C.c_int, C.c_double, C.c_double, C.c_uint64, C.c_double, dp,
@@ -155,6 +157,7 @@ def lib():
     L.tzr_ctx_filter_rechecks.argtypes = [vp]
     L.tzr_ctx_filter_rechecks.restype = C.c_int64
     L.tzr_ctx_debug_counters.argtypes = [vp, i64p]
+    L.tzr_ctx_clique_info.argtypes = [vp, i32p, i32p]
     fp = C.POINTER(C.c_float)
     L.tzr_match_correspondences.argtypes = [vp, fp, C.c_int, fp, C.c_int, fp, fp, C.c_int, C.c_int, C.c_int, C.c_int,
                                             C.c_float, C.c_uint64, i32p, C.c_int64, i64p, fp]
@@ -241,6 +244,13 @@ class Context:
                     # problems graph_strip2_kernel built with the Gram-form test (the rest: interval test or another kernel)
                     gram_problems=int(out[15]))
 
+    def clique_info(self, B: int):
+        """Geometry of the most recent max_clique(_batch) call and each problem's root-heuristic clique size."""
+        geom = np.zeros(3, dtype=np.int32)
+        heur = np.zeros(B, dtype=np.int32)
+        self._ck(lib().tzr_ctx_clique_info(self._h, _p(geom, C.c_int32), _p(heur, C.c_int32)))
+        return dict(exact_ctas=int(geom[0]), exact_conc=int(geom[1]), max_depth=int(geom[2]), heuristic_best=heur)
+
     def kernel_launches(self) -> int:
         return int(lib().tzr_ctx_kernel_launches(self._h))
 
@@ -290,6 +300,22 @@ class Context:
         self._ck(lib().tzr_max_clique(self._h, _p(bits, C.c_uint64), n, mode, kcore_thr, time_limit,
                                       _p(out, C.c_int32), C.byref(m), C.byref(proven)))
         return out[:m.value].copy(), bool(proven.value)
+
+    def max_clique_batch(self, bits, mode=0, kcore_thr=0.5, time_limit=3600.0):
+        """bits: (B, n, tzr_words_per_row(n)) uint64, one bitset per problem.  Returns (cliques: list of B sorted int32
+        arrays, proven: (B,) int32 codes as tzr_solution.clique_proven_optimal, search_flags: (B,) int32)."""
+        bits = np.ascontiguousarray(bits, dtype=np.uint64)
+        if bits.ndim != 3 or bits.shape[2] != lib().tzr_words_per_row(bits.shape[1]):
+            raise ValueError("bits must be (B, n, tzr_words_per_row(n)) uint64")
+        B, n = bits.shape[0], bits.shape[1]
+        out = np.zeros((B, n), dtype=np.int32)
+        sizes = np.zeros(B, dtype=np.int32)
+        proven = np.zeros(B, dtype=np.int32)
+        flags = np.zeros(B, dtype=np.int32)
+        self._ck(lib().tzr_max_clique_batch(self._h, B, n, _p(bits, C.c_uint64), mode, kcore_thr, time_limit,
+                                            _p(out, C.c_int32), _p(sizes, C.c_int32), _p(proven, C.c_int32),
+                                            _p(flags, C.c_int32)))
+        return [out[b, :sizes[b]].copy() for b in range(B)], proven, flags
 
     def gnc_tls_rotation(self, src, dst, noise_bound, gnc_factor=1.4, max_iterations=100, cost_threshold=1e-6):
         return self.rotation_solve(0, src, dst, noise_bound, gnc_factor, max_iterations, cost_threshold)

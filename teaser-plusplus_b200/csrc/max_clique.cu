@@ -1697,15 +1697,21 @@ void launch_clique(const Batch& bt, const tzr_params& p, int mode, cudaStream_t 
     // Nemhauser–Trotter bound / reduction for whatever ran into that deadline, then the rest of the caller's budget.
     constexpr unsigned long long kFirstPassNs = 50ull * 1000 * 1000;
     const unsigned long long total = bt.budget_ns;  // 0 = unlimited
+    // Debug flag 32768: a first pass of 1 ns, so that every problem that reaches the exact search goes through the LP
+    // kernel (unless its whole first pass fits in one %globaltimer tick); the second pass keeps the caller's whole
+    // budget.  Debug flag 131072: a single pass with the caller's whole budget (no 50 ms cap), so that whether a
+    // canonical enumeration finishes does not depend on the wall clock.
+    const bool short_first = (bt.flags_dbg & 32768u) != 0u;
+    const bool one_pass = !short_first && (bt.flags_dbg & 131072u) != 0u;
     const unsigned g3 = (unsigned)bt.exact_ctas;
     Batch p1 = b2;
-    p1.budget_ns = (total == 0ull || total > kFirstPassNs) ? kFirstPassNs : total;
+    p1.budget_ns = short_first ? 1ull : one_pass ? total : (total == 0ull || total > kFirstPassNs) ? kFirstPassNs : total;
     clique_exact_kernel<<<g3, kExactThreads, clique_exact_smem(n), st>>>(p1);
     clique_lp_kernel<<<bt.B, 32, 0, st>>>(b2);
     launches += 2;
-    if (total == 0ull || total > kFirstPassNs) {
+    if (!one_pass && (short_first || total == 0ull || total > kFirstPassNs)) {
       Batch p2 = b2;
-      p2.budget_ns = total ? total - kFirstPassNs : 0ull;
+      p2.budget_ns = short_first ? total : total ? total - kFirstPassNs : 0ull;
       clique_resume_kernel<<<(bt.B + 127) / 128, 128, 0, st>>>(b2);
       clique_exact_kernel<<<g3, kExactThreads, clique_exact_smem(n), st>>>(p2);
       launches += 2;

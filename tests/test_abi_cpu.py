@@ -30,6 +30,19 @@ def test_header_symbols_exported():
     assert set(capi._SYMBOLS) == names
 
 
+def test_max_clique_batch_signature():
+    """tzr_max_clique_batch is an added symbol (the ABI version stays 2) with the argument order the binding uses."""
+    _ensure_built()
+    hdr = re.sub(r"/\*.*?\*/", "", open(os.path.join(ROOT, "include", "teaser_b200.h")).read(), flags=re.S)
+    m = re.search(r"int\s+tzr_max_clique_batch\s*\(([^)]*)\)", hdr)
+    assert m, "tzr_max_clique_batch missing from the header"
+    args = [a.split()[-1].lstrip("*") for a in " ".join(m.group(1).split()).split(",")]
+    assert args == ["ctx", "B", "n", "adj_bits", "mode", "kcore_heuristic_threshold", "time_limit_s", "cliques",
+                    "clique_sizes", "proven_optimal", "search_flags"]
+    assert len(capi.lib().tzr_max_clique_batch.argtypes) == len(args)
+    assert capi.lib().tzr_abi_version() == 2
+
+
 def test_params_defaults_match_reference():
     _ensure_built()
     p = capi.default_params()
