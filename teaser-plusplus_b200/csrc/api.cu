@@ -30,7 +30,7 @@ struct tzr_ctx {
   int num_sms = 132;
   // device buffers (grow-only)
   DevBuf src, dst, sf, df, pk, opnd, tclist, gc, adj, deg, nedges, hclq, hsize, clq, L, alive, best_bits, alive_cnt, root_ctr, lock, flg, kfinal, tstart, stack, cv,
-      centry, ps, pd, wgt, res, skey, sidx, sorted, rmask, tmask, sol, dbg, misc, sc_x, sc_r, sc_key, sc_idx, m_in, m_scratch, m_out, cert;
+      centry, ps, pd, wgt, res, skey, sidx, sorted, rmask, tmask, sol, dbg, misc, sc, m_in, m_scratch, m_out, cert;
   // pinned host staging
   void* h_pin = nullptr;
   size_t h_pin_cap = 0;
@@ -121,12 +121,6 @@ void parallel_stage(char* dst_base, const double* const* bufs, int first, int co
   for (auto& x : th) x.join();
 }
 
-int next_pow2_host(int v) {
-  int p = 1;
-  while (p < v) p <<= 1;
-  return p;
-}
-
 // effective inlier selection mode (registration.cc:574-583)
 int effective_mode(const tzr_params& p) {
   int mode = p.inlier_selection_mode;
@@ -207,7 +201,7 @@ int setup_batch(tzr_ctx* ctx, int B, int n, bool own_points, Batch* out, bool co
   ENS(stack, warps * depth * level_bytes);
   ENS(cv, std::max(warps, (size_t)4 * B) * (size_t)n * sizeof(int32_t));
   ENS(centry, warps * depth * sizeof(int32_t));
-  bt.sort_cap = next_pow2_host(2 * n);
+  bt.sort_cap = next_pow2(2 * n);
   ENS(ps, Bn * 3 * sizeof(double));
   ENS(pd, Bn * 3 * sizeof(double));
   // rotation TIM capacity: n for CHAIN; for COMPLETE min(n(n-1)/2, what a 4 GiB budget allows)
@@ -390,51 +384,21 @@ int run_pipeline(tzr_ctx* ctx, Batch& bt, const tzr_params& p, cudaEvent_t* ev, 
   if (mode == 0 && p.max_clique_time_limit > 0 && p.max_clique_time_limit < 1e7)
     bt.budget_ns = (unsigned long long)(p.max_clique_time_limit * 1e9);
   // unknown scale (Params default): TLS over the K TIM ratios first (registration.cc:603 -> :410-425)
-  constexpr int kScaleSmallN = 256;  // single-CTA bitonic sort + sequential one-thread sweep below (bit-exact vs the
-                                     // reference's order; ~1 ms at 256), radix-sort + parallel-scan pipeline above
   bt.scale_mode = p.estimate_scaling ? 1 : 0;
-  double *scx = nullptr, *scr = nullptr, *sckey = nullptr;
-  int32_t* scidx = nullptr;
-  long long sc_npad = 0;
-  // debug flag 262144: the large path at every size (same results within the rounding of its summation tree)
-  const bool scale_large = bt.scale_mode && (bt.n > kScaleSmallN || (ctx->flags & 262144u));
   if (bt.scale_mode) {
-    const long long K = (long long)bt.n * (bt.n - 1) / 2;
-    int rc;
-    if (!scale_large) {
-      sc_npad = 1;
-      while (sc_npad < 2 * K) sc_npad <<= 1;
-      if ((rc = ensure(ctx, ctx->sc_x, (size_t)bt.B * K * 8 + 8)) != TZR_OK) return rc;
-      if ((rc = ensure(ctx, ctx->sc_r, (size_t)bt.B * K * 8 + 8)) != TZR_OK) return rc;
-      if ((rc = ensure(ctx, ctx->sc_key, (size_t)bt.B * sc_npad * 8)) != TZR_OK) return rc;
-      if ((rc = ensure(ctx, ctx->sc_idx, (size_t)bt.B * sc_npad * 4)) != TZR_OK) return rc;
-    } else {
-      if (2 * K >= (1LL << 31)) {
-        ctx->last_error = "estimate_scaling: 2K end points exceed 2^31";
-        return TZR_ERR_TOO_LARGE;
-      }
-      if ((rc = ensure(ctx, ctx->sc_x, (size_t)K * 8 + 8)) != TZR_OK) return rc;
-      if ((rc = ensure(ctx, ctx->sc_r, (size_t)K * 8 + 8)) != TZR_OK) return rc;
-      if ((rc = ensure(ctx, ctx->sc_key, scale_large_scratch_bytes(bt.n))) != TZR_OK) return rc;
+    const size_t bytes = scale_scratch_bytes(bt.B, bt.n, ctx->flags);
+    if (!bytes) {
+      ctx->last_error = "estimate_scaling: 2K end points exceed 2^31";
+      return TZR_ERR_TOO_LARGE;
     }
-    scx = (double*)ctx->sc_x.p;
-    scr = (double*)ctx->sc_r.p;
-    sckey = (double*)ctx->sc_key.p;
-    scidx = (int32_t*)ctx->sc_idx.p;
+    const int rc = ensure(ctx, ctx->sc, bytes);
+    if (rc != TZR_OK) return rc;
   }
   cudaEventRecord(ev[0], sg);
   init_solutions_kernel<<<(bt.B + 127) / 128, 128, 0, sg>>>(bt.sol, bt.B);
   ctx->launches += 1;
-  if (bt.scale_mode) {  // before prep: the FP32 filter copies are pre-scaled by the estimate
-    bt.beta = 2.0 * p.noise_bound * std::sqrt(p.cbar2);
-    if (scale_large) {
-      const int nl2 = launch_scale_estimation_large(bt, scx, scr, sckey, sg);
-      if (nl2 < 0) return TZR_ERR_TOO_LARGE;
-      ctx->launches += nl2;
-    } else {
-      ctx->launches += launch_scale_estimation(bt, scx, scr, sckey, scidx, sc_npad, sg);
-    }
-  }
+  // before prep: the FP32 filter copies are pre-scaled by the estimate
+  if (bt.scale_mode) ctx->launches += launch_scale_estimation(bt, ctx->flags, ctx->sc.p, sg);
   launch_prep(bt, sg);
   ctx->launches += 1;
   cudaEventRecord(ev[1], sg);
@@ -619,7 +583,7 @@ int tzr_ctx_destroy(tzr_ctx* ctx) {
                     &ctx->hclq, &ctx->hsize, &ctx->clq, &ctx->L, &ctx->alive, &ctx->best_bits, &ctx->alive_cnt, &ctx->root_ctr,
                     &ctx->lock, &ctx->flg, &ctx->kfinal, &ctx->tstart, &ctx->stack, &ctx->cv, &ctx->centry, &ctx->ps, &ctx->pd, &ctx->wgt,
                     &ctx->res, &ctx->skey, &ctx->sidx, &ctx->sorted, &ctx->rmask, &ctx->tmask, &ctx->sol, &ctx->dbg,
-                    &ctx->misc, &ctx->sc_x, &ctx->sc_r, &ctx->sc_key, &ctx->sc_idx, &ctx->m_in, &ctx->m_scratch, &ctx->m_out, &ctx->cert};
+                    &ctx->misc, &ctx->sc, &ctx->m_in, &ctx->m_scratch, &ctx->m_out, &ctx->cert};
   for (DevBuf* b : bufs)
     if (b->p) cudaFree(b->p);
   if (ctx->h_pin) cudaFreeHost(ctx->h_pin);
@@ -842,32 +806,22 @@ int tzr_tls_translation(tzr_ctx* ctx, const double* src, const double* dst, int 
   cudaSetDevice(ctx->device);
   cudaStream_t st = ctx->stream;
   const size_t pts = (size_t)m * 3 * sizeof(double);
-  const int npad = next_pow2_host(2 * m);
-  const size_t key_bytes = ((size_t)3 * npad + (size_t)3 * m) * sizeof(double);
-  const size_t idx_bytes = (size_t)3 * npad * sizeof(int32_t);
-  int rc = ensure(ctx, ctx->misc, 2 * pts + key_bytes + idx_bytes + (size_t)m + 64);
+  const size_t keys = (size_t)3 * next_pow2(2 * m);
+  // layout: src[3m] dst[3m] raw[3m] key[keys] t[4] idx[keys] mask[m]
+  const size_t bytes = 3 * pts + keys * sizeof(double) + 4 * sizeof(double) + keys * sizeof(int32_t) + (size_t)m;
+  int rc = ensure(ctx, ctx->misc, bytes);
   if (rc) return rc;
   double* d_src = (double*)ctx->misc.p;
   double* d_dst = d_src + (size_t)m * 3;
-  double* d_key = d_dst + (size_t)m * 3;
-  int32_t* d_idx = (int32_t*)(d_key + (size_t)3 * npad + (size_t)3 * m);
-  double* d_t = (double*)(d_idx + (size_t)3 * npad + ((3 * npad) & 1));
-  uint8_t* d_mask = (uint8_t*)(d_t + 4);
-  // the tail (d_t, d_mask) needs 4 doubles + m bytes more
-  rc = ensure(ctx, ctx->misc, (size_t)((char*)d_mask - (char*)ctx->misc.p) + (size_t)m + 64);
-  if (rc) return rc;
-  if ((double*)ctx->misc.p != d_src) {  // buffer moved on growth: recompute pointers
-    d_src = (double*)ctx->misc.p;
-    d_dst = d_src + (size_t)m * 3;
-    d_key = d_dst + (size_t)m * 3;
-    d_idx = (int32_t*)(d_key + (size_t)3 * npad + (size_t)3 * m);
-    d_t = (double*)(d_idx + (size_t)3 * npad + ((3 * npad) & 1));
-    d_mask = (uint8_t*)(d_t + 4);
-  }
+  double* d_raw = d_dst + (size_t)m * 3;
+  double* d_key = d_raw + (size_t)m * 3;
+  double* d_t = d_key + keys;
+  int32_t* d_idx = (int32_t*)(d_t + 4);
+  uint8_t* d_mask = (uint8_t*)(d_idx + keys);
   CK(cudaMemcpyAsync(d_src, src, pts, cudaMemcpyHostToDevice, st));
   CK(cudaMemcpyAsync(d_dst, dst, pts, cudaMemcpyHostToDevice, st));
   const double beta = noise_bound * std::sqrt(cbar2);  // registration.cc:459
-  launch_translation_only(d_src, d_dst, m, beta, d_key, d_idx, d_t, d_mask, st);
+  launch_translation_only(d_src, d_dst, m, beta, d_key, d_idx, d_raw, d_t, d_mask, st);
   ctx->launches += 1;
   rc = check_launch(ctx, "translation");
   if (rc) return rc;
@@ -884,31 +838,18 @@ int tzr_scalar_tls(tzr_ctx* ctx, const double* x, const double* ranges, int64_t 
   cudaSetDevice(ctx->device);
   cudaStream_t st = ctx->stream;
   const bool large = (ctx->flags & 262144u) != 0;  // debug flag: the unknown-scale stage's large path
-  int64_t npad = 1;
-  while (npad < 2 * m) npad <<= 1;
-  // layout: x[m] r[m] est[2] inliers[m, padded to 8 bytes] then the sort keys + payloads (or the large path's scratch)
-  const size_t head = 2 * (size_t)m * 8 + 16 + (((size_t)m + 7) & ~(size_t)7);
-  const size_t tail = large ? tls_large_scratch_bytes(m) + 256 : (size_t)npad * 8 + (size_t)npad * 4;
-  int rc = ensure(ctx, ctx->misc, head + tail + 64);
+  // layout: sort scratch (at the allocation's 256-byte alignment), x[m] r[m] est[2] inliers[m]
+  const size_t sort = (tls_scratch_bytes(m, 1, large) + 7) & ~(size_t)7;
+  int rc = ensure(ctx, ctx->misc, sort + 2 * (size_t)m * 8 + 16 + (size_t)m);
   if (rc) return rc;
-  double* d_x = (double*)ctx->misc.p;
+  void* d_sort = ctx->misc.p;
+  double* d_x = (double*)((char*)d_sort + sort);
   double* d_r = d_x + m;
   double* d_est = d_r + m;
   uint8_t* d_inl = (uint8_t*)(d_est + 2);
-  char* d_tail = (char*)ctx->misc.p + head;
   CK(cudaMemcpyAsync(d_x, x, (size_t)m * 8, cudaMemcpyHostToDevice, st));
   CK(cudaMemcpyAsync(d_r, ranges, (size_t)m * 8, cudaMemcpyHostToDevice, st));
-  if (large) {
-    void* scratch = (void*)(((uintptr_t)d_tail + 255) & ~(uintptr_t)255);
-    const int nl = launch_scalar_tls_large(d_x, d_r, m, scratch, d_est, d_inl, st);
-    if (nl < 0) return TZR_ERR_TOO_LARGE;
-    ctx->launches += nl;
-  } else {
-    double* d_key = (double*)d_tail;
-    int32_t* d_idx = (int32_t*)(d_key + npad);
-    launch_scalar_tls(d_x, d_r, m, d_key, d_idx, d_est, d_inl, st);
-    ctx->launches += 1;
-  }
+  ctx->launches += launch_scalar_tls(d_x, d_r, m, large, d_sort, d_est, d_inl, st);
   rc = check_launch(ctx, "scalar tls");
   if (rc) return rc;
   CK(cudaMemcpyAsync(estimate, d_est, sizeof(double), cudaMemcpyDeviceToHost, st));

@@ -406,6 +406,27 @@ __device__ void rotation_block(int alg, const TimSrc& ts, unsigned long long max
     gnc_tls_block(ts, alg == 2, max_iterations, cost_threshold, gnc_factor, noise_bound, wgt, mask, out, s_buf, s_R);
 }
 
+// ---- TLS translation (registration.cc:445-471), whole CTA ---------------------------------------------------------
+// raw: axis-major raw[ax*m + i]; key/idx: 3 * next_pow2(2m) entries.  s_t (shared, 3) receives the estimate of each
+// axis; mask[i] = measurement i is an inlier on all three axes.  Returns the number of inliers on every thread.
+__device__ int tls_translation(const double* __restrict__ raw, int m, double beta, double* key, int32_t* idx,
+                               uint8_t* __restrict__ mask, double* s_t, int* s_cnt) {
+  if (threadIdx.x == 0) *s_cnt = 0;
+  tls_block(raw, nullptr, beta, m, 3, key, idx, s_t);
+  int c = 0;
+  for (int i = threadIdx.x; i < m; i += kRTThreads) {
+    bool in = true;
+#pragma unroll
+    for (int ax = 0; ax < 3; ++ax) in = in && tls_inlier(raw[(size_t)ax * m + i], beta, s_t[ax]);  // :86, :469
+    mask[i] = in;
+    c += in;
+  }
+  c = __reduce_add_sync(0xffffffffu, c);
+  if ((threadIdx.x & 31) == 0 && c) atomicAdd(s_cnt, c);
+  __syncthreads();
+  return *s_cnt;
+}
+
 }  // namespace
 
 // =================================================================================================
@@ -536,10 +557,7 @@ __global__ void __launch_bounds__(kRTThreads) rot_trans_kernel(Batch bt, tzr_par
   rotation_block(p.rotation_estimation_algorithm, ts, p.rotation_max_iterations, p.rotation_cost_threshold,
                  p.rotation_gnc_factor, rot_nb, bt.wgt + (size_t)b * bt.rot_cap, rmask, g, s_buf, &s_R);
   __syncthreads();
-  if (tid == 0) {
-    s_cnt[0] = 0;
-    s_cnt[1] = 0;
-  }
+  if (tid == 0) s_cnt[0] = 0;
   __syncthreads();
   {
     int c = 0;
@@ -553,9 +571,6 @@ __global__ void __launch_bounds__(kRTThreads) rot_trans_kernel(Batch bt, tzr_par
 #pragma unroll
   for (int k = 0; k < 9; ++k) sR[k] = scale * R.a[k];
   double* raw = ps;  // reuse: axis-major raw[ax*m + i]
-  const int npad = next_pow2(2 * m);
-  double* key = bt.skey + (size_t)b * 3 * bt.sort_cap;  // per-axis capacity sort_cap >= npad
-  int32_t* idx = bt.sidx + (size_t)b * 3 * bt.sort_cap;
   __syncthreads();
   const double beta = p.noise_bound * sqrt(p.cbar2);
   // gather first (ps is overwritten by raw): compute into registers per i, then store
@@ -578,41 +593,10 @@ __global__ void __launch_bounds__(kRTThreads) rot_trans_kernel(Batch bt, tzr_par
     }
   }
   __syncthreads();
-  for (int t = tid; t < 3 * npad; t += kRTThreads) {
-    const int ax = t / npad, q = t - ax * npad;
-    double k;
-    int id;
-    if (q < 2 * m) {
-      k = tls_key(raw[(size_t)ax * m + (q >> 1)], beta, q);  // :36-37
-      id = q;
-    } else {
-      k = 1.0 / 0.0;
-      id = 0x7fffffff;
-    }
-    key[(size_t)ax * npad + q] = k;
-    idx[(size_t)ax * npad + q] = id;
-  }
-  __syncthreads();
-  bitonic_sort_block(key, idx, npad, 3);
-  if ((tid & 31) == 0 && (tid >> 5) < 3) {
-    const int ax = tid >> 5;
-    s_t[ax] = tls_sweep(raw + (size_t)ax * m, nullptr, beta, m, idx + (size_t)ax * npad);
-  }
-  __syncthreads();
-  uint8_t* tmask = bt.trans_mask + (size_t)b * n;
-  {
-    int c = 0;
-    for (int i = tid; i < m; i += kRTThreads) {
-      bool in = true;
-#pragma unroll
-      for (int ax = 0; ax < 3; ++ax) in = in && (fabs(raw[(size_t)ax * m + i] - s_t[ax]) <= beta);  // :86, :469
-      tmask[i] = in;
-      c += in;
-    }
-    c = __reduce_add_sync(0xffffffffu, c);
-    if ((tid & 31) == 0 && c) atomicAdd(&s_cnt[1], c);
-  }
-  __syncthreads();
+  // per-axis key capacity sort_cap = next_pow2(2n) >= next_pow2(2m)
+  const int n_trans = tls_translation(raw, m, beta, bt.skey + (size_t)b * 3 * bt.sort_cap,
+                                      bt.sidx + (size_t)b * 3 * bt.sort_cap, bt.trans_mask + (size_t)b * n, s_t,
+                                      &s_cnt[1]);
   if (tid == 0) {
 #pragma unroll
     for (int k = 0; k < 9; ++k) sol->rotation[k] = R.a[k];
@@ -622,7 +606,7 @@ __global__ void __launch_bounds__(kRTThreads) rot_trans_kernel(Batch bt, tzr_par
     sol->gnc_cost = g.cost;
     sol->gnc_iterations = g.iters;
     sol->n_rotation_inliers = s_cnt[0];
-    sol->n_translation_inliers = s_cnt[1];
+    sol->n_translation_inliers = n_trans;
     sol->valid = 1;
   }
 }
@@ -680,84 +664,17 @@ __global__ void __launch_bounds__(kRTThreads) translation_only_kernel(const doub
                                                                        double beta, double* key, int32_t* idx,
                                                                        double* raw, double* out_t, uint8_t* mask) {
   __shared__ double s_t[3];
-  const int tid = threadIdx.x;
-  const int npad = next_pow2(2 * m);
-  for (int i = tid; i < m; i += kRTThreads)
+  __shared__ int s_cnt;
+  for (int i = threadIdx.x; i < m; i += kRTThreads)
     for (int ax = 0; ax < 3; ++ax) raw[(size_t)ax * m + i] = dst[3 * (size_t)i + ax] - src[3 * (size_t)i + ax];  // :455
   __syncthreads();
-  for (int t = tid; t < 3 * npad; t += kRTThreads) {
-    const int ax = t / npad, q = t - ax * npad;
-    double k;
-    int id;
-    if (q < 2 * m) {
-      k = tls_key(raw[(size_t)ax * m + (q >> 1)], beta, q);
-      id = q;
-    } else {
-      k = 1.0 / 0.0;
-      id = 0x7fffffff;
-    }
-    key[(size_t)ax * npad + q] = k;
-    idx[(size_t)ax * npad + q] = id;
-  }
-  __syncthreads();
-  bitonic_sort_block(key, idx, npad, 3);
-  if ((tid & 31) == 0 && (tid >> 5) < 3) {
-    const int ax = tid >> 5;
-    s_t[ax] = tls_sweep(raw + (size_t)ax * m, nullptr, beta, m, idx + (size_t)ax * npad);
-  }
-  __syncthreads();
-  if (mask)
-    for (int i = tid; i < m; i += kRTThreads) {
-      bool in = true;
-      for (int ax = 0; ax < 3; ++ax) in = in && (fabs(raw[(size_t)ax * m + i] - s_t[ax]) <= beta);
-      mask[i] = in;
-    }
-  if (tid < 3) out_t[tid] = s_t[tid];
+  tls_translation(raw, m, beta, key, idx, mask, s_t, &s_cnt);
+  if (threadIdx.x < 3) out_t[threadIdx.x] = s_t[threadIdx.x];
 }
 
-void launch_translation_only(const double* src, const double* dst, int m, double beta, double* skey, int32_t* sidx,
-                             double* out_t, uint8_t* mask, cudaStream_t st) {
-  // layout of skey: [3*npad keys][3*m raw]
-  int npad = 1;
-  while (npad < 2 * m) npad <<= 1;
-  double* raw = skey + (size_t)3 * npad;
-  translation_only_kernel<<<1, kRTThreads, 0, st>>>(src, dst, m, beta, skey, sidx, raw, out_t, mask);
-}
-
-// generic scalar TLS with per-measurement ranges
-__global__ void __launch_bounds__(1024) scalar_tls_kernel(const double* x, const double* ranges, long long m,
-                                                           double* key, int32_t* idx, double* out_est,
-                                                           uint8_t* inliers) {
-  __shared__ double s_est;
-  const int tid = threadIdx.x;
-  long long npad = 1;
-  while (npad < 2 * m) npad <<= 1;
-  for (long long q = tid; q < npad; q += blockDim.x) {
-    double k;
-    int id;
-    if (q < 2 * m) {
-      k = tls_key(x[q >> 1], ranges[q >> 1], q);
-      id = (int)q;
-    } else {
-      k = 1.0 / 0.0;
-      id = 0x7fffffff;
-    }
-    key[q] = k;
-    idx[q] = id;
-  }
-  __syncthreads();
-  bitonic_sort_block(key, idx, (int)npad, 1);
-  if (tid == 0) s_est = tls_sweep(x, ranges, 0.0, m, idx);
-  __syncthreads();
-  const double est = s_est;
-  if (inliers)
-    for (long long i = tid; i < m; i += blockDim.x) inliers[i] = tls_kept(x[i], ranges[i]) && fabs(x[i] - est) <= ranges[i];
-  if (tid == 0) *out_est = est;
-}
-
-void launch_scalar_tls(const double* x, const double* ranges, long long m, double* skey, int32_t* sidx,
-                       double* out_est, uint8_t* inliers, cudaStream_t st) {
-  scalar_tls_kernel<<<1, 1024, 0, st>>>(x, ranges, m, skey, sidx, out_est, inliers);
+void launch_translation_only(const double* src, const double* dst, int m, double beta, double* key, int32_t* idx,
+                             double* raw, double* out_t, uint8_t* mask, cudaStream_t st) {
+  translation_only_kernel<<<1, kRTThreads, 0, st>>>(src, dst, m, beta, key, idx, raw, out_t, mask);
 }
 
 }  // namespace tzr

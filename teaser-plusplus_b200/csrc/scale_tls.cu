@@ -40,35 +40,26 @@ __global__ void __launch_bounds__(256) scale_pairs_kernel(Batch bt, double* X, d
   }
 }
 
+// small path: one CTA per problem (n <= kScaleSmallN, so K and its end-point count fit an int)
 __global__ void __launch_bounds__(1024) scale_tls_kernel(Batch bt, const double* X, const double* Rg, double* key,
-                                                          int32_t* idx, long long npad) {
+                                                          int32_t* idx) {
   const int b = blockIdx.x;
-  const int n = bt.n;
-  const long long K = (long long)n * (n - 1) / 2;
-  const double* x = X + (size_t)b * K;
-  const double* r = Rg + (size_t)b * K;
-  double* kk = key + (size_t)b * npad;
-  int32_t* ii = idx + (size_t)b * npad;
+  const int K = bt.n * (bt.n - 1) / 2;
+  const int npad = next_pow2(2 * K);
   __shared__ double s_est;
-  for (long long q = threadIdx.x; q < npad; q += blockDim.x) {
-    double k;
-    int id;
-    if (q < 2 * K) {
-      const long long t = q >> 1;
-      k = tls_key(x[t], r[t], q);  // registration.cc:36-37
-      id = (int)q;
-    } else {
-      k = 1.0 / 0.0;
-      id = 0x7fffffff;
-    }
-    kk[q] = k;
-    ii[q] = id;
-  }
-  __syncthreads();
-  bitonic_sort_block(kk, ii, (int)npad, 1);
-  if (threadIdx.x == 0) s_est = tls_sweep(x, r, 0.0, K, ii);
-  __syncthreads();
+  tls_block(X + (size_t)b * K, Rg + (size_t)b * K, 0.0, K, 1, key + (size_t)b * npad, idx + (size_t)b * npad, &s_est);
   if (threadIdx.x == 0) bt.sol[b].scale = s_est;
+}
+
+// tzr_scalar_tls on the small path: one CTA
+__global__ void __launch_bounds__(1024) scalar_tls_kernel(const double* x, const double* ranges, long long m,
+                                                           double* key, int32_t* idx, double* out_est,
+                                                           uint8_t* inliers) {
+  __shared__ double s_est;
+  tls_block(x, ranges, 0.0, (int)m, 1, key, idx, &s_est);
+  const double est = s_est;
+  for (long long i = threadIdx.x; i < m; i += blockDim.x) inliers[i] = tls_inlier(x[i], ranges[i], est);
+  if (threadIdx.x == 0) *out_est = est;
 }
 
 // ---------------------------------------------------------------------------------------------------------------
@@ -240,10 +231,8 @@ __global__ void final_argmin_kernel(const Best* tile_best, long long n_tiles, do
 __global__ void tls_inliers_kernel(const double* __restrict__ X, const double* __restrict__ Rg, long long K,
                                    const double* __restrict__ est, uint8_t* __restrict__ inliers) {
   const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-  if (i < K) inliers[i] = tls_kept(X[i], Rg[i]) && fabs(X[i] - *est) <= Rg[i];  // registration.cc:86
+  if (i < K) inliers[i] = tls_inlier(X[i], Rg[i], *est);
 }
-
-}  // namespace
 
 size_t tls_large_scratch_bytes(long long K) {
   const long long M = 2 * K;
@@ -255,11 +244,10 @@ size_t tls_large_scratch_bytes(long long K) {
 }
 
 // Scalar TLS over K measurements with the radix sort + tiled scans + first-minimum arg-min; writes the estimate to
-// *out (device).  scratch: tls_large_scratch_bytes(K) bytes.  Returns the number of launches (approximate: the radix
-// sort's internal kernels are counted as 8).
+// *out (device).  scratch: tls_large_scratch_bytes(K) bytes, 2K < 2^31.  Returns the number of launches (approximate:
+// the radix sort's internal kernels are counted as 8).
 int launch_tls_large(const double* X, const double* Rg, long long K, void* scratch, double* out, cudaStream_t st) {
   const long long M = 2 * K;
-  if (M >= (1LL << 31)) return -1;
   const long long n_tiles = (M + kTileElems - 1) / kTileElems;
   size_t temp = 0;
   cub::DeviceRadixSort::SortPairs(nullptr, temp, (const double*)nullptr, (double*)nullptr, (const int*)nullptr,
@@ -284,43 +272,70 @@ int launch_tls_large(const double* X, const double* Rg, long long K, void* scrat
   return 5 + 8;
 }
 
-size_t scale_large_scratch_bytes(int n) { return tls_large_scratch_bytes((long long)n * (n - 1) / 2); }
+constexpr int kScaleSmallN = 256;  // single-CTA bitonic sort + sequential one-thread sweep up to here (bit-exact vs the
+                                   // reference's order; ~1 ms at 256), radix-sort + parallel-scan pipeline above
+// debug flag 262144: the large path at every size (same results within the rounding of its summation tree)
+bool scale_large(int n, uint32_t flags) { return n > kScaleSmallN || (flags & 262144u); }
 
-// One problem at a time (the sort uses the whole GPU).  scratch: scale_large_scratch_bytes(n) bytes.
-int launch_scale_estimation_large(const Batch& bt, double* X, double* Rg, void* scratch, cudaStream_t st) {
-  const int n = bt.n;
+size_t align256(size_t v) { return (v + 255) & ~(size_t)255; }
+
+}  // namespace
+
+size_t tls_scratch_bytes(long long m, int count, bool large) {
+  if (2 * m >= (1LL << 31)) return 0;  // end-point payloads are ints
+  if (large) return tls_large_scratch_bytes(m);
+  return (size_t)count * next_pow2((int)(2 * m)) * (sizeof(double) + sizeof(int32_t));
+}
+
+// scratch: tls_scratch_bytes(m, 1, large) bytes (small path: the keys, then the payloads)
+int launch_scalar_tls(const double* x, const double* ranges, long long m, bool large, void* scratch, double* out_est,
+                      uint8_t* inliers, cudaStream_t st) {
+  if (!large) {
+    double* key = (double*)scratch;
+    scalar_tls_kernel<<<1, 1024, 0, st>>>(x, ranges, m, key, (int32_t*)(key + next_pow2((int)(2 * m))), out_est,
+                                          inliers);
+    return 1;
+  }
+  const int nl = launch_tls_large(x, ranges, m, scratch, out_est, st);
+  tls_inliers_kernel<<<(unsigned)((m + 255) / 256), 256, 0, st>>>(x, ranges, m, out_est, inliers);
+  return nl + 1;
+}
+
+// Layout: ratios X and ranges Rg (K doubles per problem), then the sort scratch (256-byte aligned).  The small path holds
+// every problem of the batch, the large path one problem at a time (its sort uses the whole GPU).
+size_t scale_scratch_bytes(int B, int n, uint32_t flags) {
+  const bool large = scale_large(n, flags);
   const long long K = (long long)n * (n - 1) / 2;
+  const int sets = large ? 1 : B;
+  const size_t sort = tls_scratch_bytes(K, sets, large);
+  return sort ? align256((size_t)sets * K * 16) + sort : 0;
+}
+
+int launch_scale_estimation(const Batch& bt, uint32_t flags, void* scratch, cudaStream_t st) {
+  const int n = bt.n;
   if (n < 2) return 0;
-  if (2 * K >= (1LL << 31)) return -1;
+  const bool large = scale_large(n, flags);
+  const long long K = (long long)n * (n - 1) / 2;
+  const int sets = large ? 1 : bt.B;
+  double* X = (double*)scratch;
+  double* Rg = X + (size_t)sets * K;
+  char* sort = (char*)scratch + align256((size_t)sets * K * 16);
+  if (!large) {
+    double* key = (double*)sort;
+    scale_pairs_kernel<<<dim3((unsigned)(n - 1), (unsigned)bt.B), 256, 0, st>>>(bt, X, Rg);
+    scale_tls_kernel<<<bt.B, 1024, 0, st>>>(bt, X, Rg, key, (int32_t*)(key + (size_t)bt.B * next_pow2((int)(2 * K))));
+    return 2;
+  }
   int launches = 0;
-  dim3 g1((unsigned)(n - 1), 1);
   for (int b = 0; b < bt.B; ++b) {
     Batch one = bt;  // view of problem b for the pairs kernel
     one.B = 1;
     one.src = bt.src + (size_t)b * n * 3;
     one.dst = bt.dst + (size_t)b * n * 3;
-    scale_pairs_kernel<<<g1, 256, 0, st>>>(one, X, Rg);
-    launches += 1 + launch_tls_large(X, Rg, K, scratch, &bt.sol[b].scale, st);
+    scale_pairs_kernel<<<(unsigned)(n - 1), 256, 0, st>>>(one, X, Rg);
+    launches += 1 + launch_tls_large(X, Rg, K, sort, &bt.sol[b].scale, st);
   }
   return launches;
-}
-
-// tzr_scalar_tls through the large path (debug flag 262144).  scratch: tls_large_scratch_bytes(m) bytes.
-int launch_scalar_tls_large(const double* x, const double* ranges, long long m, void* scratch, double* out_est,
-                            uint8_t* inliers, cudaStream_t st) {
-  const int nl = launch_tls_large(x, ranges, m, scratch, out_est, st);
-  if (nl < 0) return nl;
-  if (inliers) tls_inliers_kernel<<<(unsigned)((m + 255) / 256), 256, 0, st>>>(x, ranges, m, out_est, inliers);
-  return nl + 1;
-}
-
-int launch_scale_estimation(const Batch& bt, double* X, double* Rg, double* key, int32_t* idx, long long npad,
-                            cudaStream_t st) {
-  if (bt.n < 2) return 0;
-  dim3 g1((unsigned)(bt.n - 1), (unsigned)bt.B);
-  scale_pairs_kernel<<<g1, 256, 0, st>>>(bt, X, Rg);
-  scale_tls_kernel<<<bt.B, 1024, 0, st>>>(bt, X, Rg, key, idx, npad);
-  return 2;
 }
 
 }  // namespace tzr

@@ -90,12 +90,40 @@ __device__ double tls_sweep(const double* __restrict__ X, const double* __restri
   return best_xhat;
 }
 
-__device__ inline int next_pow2(int v) {
-  int p = 1;
-  while (p < v) p <<= 1;
-  return p;
+// Inlier flag of a measurement against the estimate (registration.cc:86); false for an excluded measurement.
+// By reference, so that operands in memory are read where the expression uses them (the range only for a finite value,
+// the estimate only for a kept measurement), as the inline expression did.
+__device__ __forceinline__ bool tls_inlier(const double& x, const double& r, const double& est) {
+  return tls_kept(x, r) && fabs(x - est) <= r;
 }
 
+// Scalar TLS of `nax` independent estimators in one CTA.  Estimator ax has the m measurements x[ax*m + i] with ranges
+// r[ax*m + i], or the constant range c_range when r is nullptr.  key/idx: nax * next_pow2(2m) entries of scratch.
+// The end points of each estimator are padded to a power of two with (+inf, 0x7fffffff), which sorts after every real
+// one, and sorted together; thread 32*ax then sweeps estimator ax.  On return est[ax] (shared memory) holds its estimate
+// on every thread.
+__device__ __forceinline__ void tls_block(const double* __restrict__ x, const double* __restrict__ r, double c_range,
+                                          int m, int nax, double* key, int* idx, double* est) {
+  const int npad = next_pow2(2 * m);
+  for (int t = threadIdx.x; t < nax * npad; t += blockDim.x) {
+    const int ax = t / npad, q = t - ax * npad;
+    if (q < 2 * m) {
+      const size_t i = (size_t)ax * m + (q >> 1);
+      key[t] = tls_key(x[i], r ? r[i] : c_range, q);  // registration.cc:36-37
+      idx[t] = q;
+    } else {
+      key[t] = 1.0 / 0.0;
+      idx[t] = 0x7fffffff;
+    }
+  }
+  __syncthreads();
+  bitonic_sort_block(key, idx, npad, nax);
+  if ((threadIdx.x & 31) == 0 && (threadIdx.x >> 5) < nax) {
+    const int ax = threadIdx.x >> 5;
+    est[ax] = tls_sweep(x + (size_t)ax * m, r ? r + (size_t)ax * m : nullptr, c_range, m, idx + (size_t)ax * npad);
+  }
+  __syncthreads();
+}
 
 }  // namespace
 }  // namespace tzr

@@ -20,6 +20,12 @@ __host__ __device__ inline int pitch64(int n) { return 2 * ((n + 127) / 128); }
 __host__ __device__ inline int pitch32(int n) { return 2 * pitch64(n); }
 __host__ __device__ inline int words64(int n) { return (n + 63) / 64; }
 __host__ __device__ inline int npad128(int n) { return 128 * ((n + 127) / 128); }
+// smallest power of two >= v: the padded end-point count of the bitonic TLS sort (tls_device.cuh)
+__host__ __device__ inline int next_pow2(int v) {
+  int p = 1;
+  while (p < v) p <<= 1;
+  return p;
+}
 
 constexpr int kTile = 128;          // graph tile edge (pairs per tile = 128*128)
 constexpr int kGraphThreads = 128;  // 4 warps, each owns a 32x128 sub-tile (4 pairs per lane per step)
@@ -170,13 +176,16 @@ void launch_graph_patch(const Batch& bt, cudaStream_t st, int num_sms);  // tc_p
 // bitset_only: the adjacency did not come from launch_graph (tzr_max_clique on a caller's bitset): always popcount
 void launch_degree(const Batch& bt, cudaStream_t st, bool bitset_only = false);
 void launch_clique(const Batch& bt, const tzr_params& p, int mode, cudaStream_t st, int* n_launches);
-int launch_scale_estimation(const Batch& bt, double* X, double* Rg, double* key, int32_t* idx, long long npad,
-                            cudaStream_t st);
-size_t scale_large_scratch_bytes(int n);
-int launch_scale_estimation_large(const Batch& bt, double* X, double* Rg, void* scratch, cudaStream_t st);
-size_t tls_large_scratch_bytes(long long K);
-int launch_scalar_tls_large(const double* x, const double* ranges, long long m, void* scratch, double* out_est,
-                            uint8_t* inliers, cudaStream_t st);
+// scale_tls.cu: the scalar TLS launches with per-measurement ranges (tzr_scalar_tls and the unknown-scale stage).
+// The small path sorts in one CTA per estimator (tls_block), the large path with a radix sort and tiled scans.
+// tls_scratch_bytes: sort scratch of `count` estimators over m measurements each; 0 when the 2m end points do not fit
+// the int payload (TZR_ERR_TOO_LARGE).  The large path runs one estimator at a time.
+size_t tls_scratch_bytes(long long m, int count, bool large);
+int launch_scalar_tls(const double* x, const double* ranges, long long m, bool large, void* scratch, double* out_est,
+                      uint8_t* inliers, cudaStream_t st);
+// Unknown-scale stage: TIM ratios, ranges and sort scratch of a batch (0: too large), and its launches.
+size_t scale_scratch_bytes(int B, int n, uint32_t flags);
+int launch_scale_estimation(const Batch& bt, uint32_t flags, void* scratch, cudaStream_t st);
 void launch_rot_trans(const Batch& bt, const tzr_params& p, int use_clique, cudaStream_t st);
 size_t clique_heur_smem(int n);
 size_t clique_peel_smem(int n);
@@ -187,10 +196,9 @@ int clique_exact_grid(int n, int num_sms);  // CTAs of the persistent exact-phas
 void launch_gnc_only(int alg, const double* src, const double* dst, int m, double noise_bound, double gnc_factor,
                      unsigned long long max_iter, double cost_thr, double* wgt, double* res, double* out_R,
                      uint8_t* mask, double* out_cost, int* out_iters, cudaStream_t st);
-void launch_translation_only(const double* src, const double* dst, int m, double beta, double* skey, int32_t* sidx,
-                             double* out_t, uint8_t* mask, cudaStream_t st);
-void launch_scalar_tls(const double* x, const double* ranges, long long m, double* skey, int32_t* sidx,
-                       double* out_est, uint8_t* inliers, cudaStream_t st);
+// key/idx: 3 * next_pow2(2m) entries, raw: 3m doubles
+void launch_translation_only(const double* src, const double* dst, int m, double beta, double* key, int32_t* idx,
+                             double* raw, double* out_t, uint8_t* mask, cudaStream_t st);
 
 // fpfh.cu (FPFHEstimation::computeFPFHFeatures, fpfh.cc:15-43)
 size_t fpfh_grid_scratch_bytes(int n);
