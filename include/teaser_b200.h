@@ -188,6 +188,31 @@ int tzr_match_correspondences(tzr_ctx* ctx, const float* src_pts, int ns, const 
 int tzr_compute_fpfh(tzr_ctx* ctx, const float* pts, int n, double normal_search_radius, double fpfh_search_radius,
                      float* fpfh_out, float* normals_out);
 
+/* ---- the front end over many clouds in one call ----------------------------------------------
+ * Host pointers, ragged sizes, synchronous like tzr_solve_batch; the number of kernel launches does not depend on B.
+ *
+ * Descriptors of B clouds: cloud b has n[b] >= 1 points at pts[b] (n[b] x 3 float).  fpfh_out[b]: n[b] x 33 floats.
+ * normals_out (may be NULL, or hold NULL entries): n[b] x 4 floats.  status (B int32, may be NULL): per cloud TZR_OK or
+ * TZR_ERR_TOO_LARGE (a point with more than 4096 neighbours).  Returns TZR_ERR_TOO_LARGE if any cloud overflowed; every
+ * other cloud's outputs are still written.  TZR_ERR_TOO_LARGE also when the batch holds more than 2^31 - 1 points.
+ * Per cloud, the outputs are bit-identical to tzr_compute_fpfh on that cloud alone. */
+int tzr_compute_fpfh_batch(tzr_ctx* ctx, int B, const int32_t* n, const float* const* pts,
+                           double normal_search_radius, double fpfh_search_radius, float* const* fpfh_out,
+                           float* const* normals_out, int32_t* status);
+
+/* Correspondences of B cloud pairs: pair b has ns[b] source points (src_pts[b], src_feat[b]) and nd[b] target points
+ * (dst_pts[b], dst_feat[b]); dim and the flags apply to every pair; tuple_seeds: B seeds.  pairs[b]: capacity[b] x 2
+ * int32 rows.  n_pairs[b] (B entries) is always set.  If some pair needs more than capacity[b] rows the call returns
+ * TZR_ERR_INVALID_ARG, and the pairs that fit are still written.  global_scale (B floats, may be NULL).
+ * TZR_ERR_TOO_LARGE when the batch holds more than 2^31 - 1 points.  Per pair, the outputs are bit-identical to
+ * tzr_match_correspondences with the same arguments and seed. */
+int tzr_match_correspondences_batch(tzr_ctx* ctx, int B, const int32_t* ns, const float* const* src_pts,
+                                    const int32_t* nd, const float* const* dst_pts, const float* const* src_feat,
+                                    const float* const* dst_feat, int dim, int use_absolute_scale, int use_crosscheck,
+                                    int use_tuple_test, float tuple_scale, const uint64_t* tuple_seeds,
+                                    int32_t* const* pairs, const int64_t* capacity, int64_t* n_pairs,
+                                    float* global_scale);
+
 /* The matcher's search primitive on its own (Matcher::searchKDTree with nn = 1, matcher.cc:314-335, for every
  * query row): nn_index[q] = argmin_i L2(query[q], db[i]), nn_dist[q] (optional) the squared distance. */
 int tzr_feature_nn(tzr_ctx* ctx, const float* query, int nq, const float* db, int ndb, int dim, int32_t* nn_index,

@@ -95,7 +95,8 @@ _SYMBOLS = [
     "tzr_ctx_set_flags", "tzr_ctx_filter_mismatches", "tzr_ctx_filter_rechecks", "tzr_ctx_debug_counters",
     "tzr_match_correspondences", "tzr_feature_nn", "tzr_compute_fpfh", "tzr_certifier_params_default", "tzr_certify",
     "tzr_certifier_initial_matrix", "tzr_certifier_dual_projection", "tzr_last_graph_info", "tzr_ctx_stage_log",
-    "tzr_ctx_stage_log_read", "tzr_solve_batch_multi", "tzr_ctx_clique_info",
+    "tzr_ctx_stage_log_read", "tzr_solve_batch_multi", "tzr_ctx_clique_info", "tzr_compute_fpfh_batch",
+    "tzr_match_correspondences_batch",
 ]
 
 
@@ -163,6 +164,10 @@ def lib():
                                             C.c_float, C.c_uint64, i32p, C.c_int64, i64p, fp]
     L.tzr_feature_nn.argtypes = [vp, fp, C.c_int, fp, C.c_int, C.c_int, i32p, fp]
     L.tzr_compute_fpfh.argtypes = [vp, fp, C.c_int, C.c_double, C.c_double, fp, fp]
+    fpp = C.POINTER(fp)
+    L.tzr_compute_fpfh_batch.argtypes = [vp, C.c_int, i32p, fpp, C.c_double, C.c_double, fpp, fpp, i32p]
+    L.tzr_match_correspondences_batch.argtypes = [vp, C.c_int, i32p, fpp, i32p, fpp, fpp, fpp, C.c_int, C.c_int,
+                                                  C.c_int, C.c_int, C.c_float, u64p, C.POINTER(i32p), i64p, i64p, fp]
     L.tzr_certifier_params_default.argtypes = [C.POINTER(CertifierParams)]
     L.tzr_certifier_params_default.restype = None
     L.tzr_certify.argtypes = [vp, C.POINTER(CertifierParams), dp, dp, dp, dp, C.c_int, C.POINTER(CertificationResult),
@@ -444,6 +449,77 @@ class Context:
         self._ck(lib().tzr_compute_fpfh(self._h, _p(p, C.c_float), p.shape[0], float(normal_search_radius),
                                         float(fpfh_search_radius), _p(out, C.c_float), _p(nor, C.c_float)))
         return (out, nor) if return_normals else out
+
+    def compute_fpfh_batch(self, pts_list, normal_search_radius=0.03, fpfh_search_radius=0.05, return_normals=False):
+        """compute_fpfh on every (n_b,3) cloud of the list in one call: a list of (n_b,33) descriptors (and a list of
+        (n_b,4) normals), each bit-identical to compute_fpfh on that cloud alone.  When a cloud has a point with more
+        than 4096 neighbours the TzrError carries `status` (per cloud 0 or the error code) and `result` (the outputs
+        of every cloud, written for the others)."""
+        pts = [np.ascontiguousarray(p, dtype=np.float32) for p in pts_list]
+        if not pts or any(p.ndim != 2 or p.shape[1] != 3 for p in pts):
+            raise TzrError("compute_fpfh_batch: a non-empty list of (n,3) clouds is required")
+        B = len(pts)
+        n = np.array([p.shape[0] for p in pts], dtype=np.int32)
+        outs = [np.zeros((p.shape[0], 33), dtype=np.float32) for p in pts]
+        nors = [np.zeros((p.shape[0], 4), dtype=np.float32) for p in pts] if return_normals else None
+        status = np.zeros(B, dtype=np.int32)
+        fp = C.POINTER(C.c_float)
+        arr = lambda xs: (fp * B)(*[_p(x, C.c_float) for x in xs])
+        rc = lib().tzr_compute_fpfh_batch(self._h, B, _p(n, C.c_int32), arr(pts), float(normal_search_radius),
+                                          float(fpfh_search_radius), arr(outs), arr(nors) if nors else None,
+                                          _p(status, C.c_int32))
+        result = (outs, nors) if return_normals else outs
+        try:
+            self._ck(rc)
+        except TzrError as e:
+            e.status, e.result = status, result
+            raise
+        return result
+
+    def match_correspondences_batch(self, src_pts, dst_pts, src_feat, dst_feat, use_absolute_scale=True,
+                                    use_crosscheck=True, use_tuple_test=True, tuple_scale=0.0, tuple_seeds=None,
+                                    return_scale=False, capacity=None):
+        """match_correspondences on B pairs in one call (lists of (n,3) points and (n,dim) features, one dim for all);
+        tuple_seeds: B seeds (default 0 each).  Returns a list of (m_b,2) int32 pair arrays (and a list of
+        global scales), each bit-identical to match_correspondences on that pair with its seed.  capacity (B row
+        counts, default ns + nd) bounds each output; when one is too small the TzrError carries `n_pairs` and
+        `result` (the pairs that fit, None for the others)."""
+        cast = lambda xs: [np.ascontiguousarray(x, dtype=np.float32) for x in xs]
+        sp, tp, sf, tf = cast(src_pts), cast(dst_pts), cast(src_feat), cast(dst_feat)
+        B = len(sp)
+        if B == 0 or not (len(tp) == len(sf) == len(tf) == B):
+            raise TzrError("match_correspondences_batch: four lists of the same non-zero length are required")
+        dim = sf[0].shape[1] if sf[0].ndim == 2 else -1
+        for a, b, fa, fb in zip(sp, tp, sf, tf):
+            if a.ndim != 2 or a.shape[1] != 3 or b.ndim != 2 or b.shape[1] != 3 or fa.shape != (a.shape[0], dim) or \
+                    fb.shape != (b.shape[0], dim):
+                raise TzrError("match_correspondences_batch: points must be (n,3) and features (n,dim) with one row "
+                               "per point and one dim for every pair")
+        ns = np.array([a.shape[0] for a in sp], dtype=np.int32)
+        nd = np.array([b.shape[0] for b in tp], dtype=np.int32)
+        cap = (ns.astype(np.int64) + nd) if capacity is None else np.ascontiguousarray(capacity, dtype=np.int64)
+        seeds = np.zeros(B, dtype=np.uint64) if tuple_seeds is None else \
+            np.ascontiguousarray([int(s) for s in tuple_seeds], dtype=np.uint64)
+        if cap.shape != (B,) or seeds.shape != (B,):
+            raise TzrError("match_correspondences_batch: capacity and tuple_seeds need one entry per pair")
+        pairs = [np.zeros((max(int(c), 1), 2), dtype=np.int32) for c in cap]
+        cnt = np.zeros(B, dtype=np.int64)
+        g = np.zeros(B, dtype=np.float32)
+        fp, i32p = C.POINTER(C.c_float), C.POINTER(C.c_int32)
+        arr = lambda xs: (fp * B)(*[_p(x, C.c_float) for x in xs])
+        rc = lib().tzr_match_correspondences_batch(
+            self._h, B, _p(ns, C.c_int32), arr(sp), _p(nd, C.c_int32), arr(tp), arr(sf), arr(tf), dim,
+            int(bool(use_absolute_scale)), int(bool(use_crosscheck)), int(bool(use_tuple_test)), float(tuple_scale),
+            _p(seeds, C.c_uint64), (i32p * B)(*[_p(p, C.c_int32) for p in pairs]), _p(cap, C.c_int64),
+            _p(cnt, C.c_int64), _p(g, C.c_float))
+        out = [p[:k].copy() if k <= c else None for p, k, c in zip(pairs, cnt, cap)]
+        scales = [float(x) for x in g]
+        try:
+            self._ck(rc)
+        except TzrError as e:
+            e.n_pairs, e.result = cnt, out
+            raise
+        return (out, scales) if return_scale else out
 
     def feature_nn(self, query, db):
         """Exact 1-NN (flann::L2<float> accumulation order, lowest index among ties) of every query row in db."""

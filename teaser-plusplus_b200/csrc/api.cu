@@ -102,23 +102,88 @@ int ensure_pinned(tzr_ctx* ctx, size_t bytes) {
   return TZR_OK;
 }
 
-// Copy `count` caller buffers of `per` bytes each into a contiguous pinned area with a few host threads (pageable
-// host memory cannot be DMA'd asynchronously; one thread moves ~10 GB/s, which is slower than the GPU consumes it).
-void parallel_stage(char* dst_base, const double* const* bufs, int first, int count, size_t per) {
-  const size_t total = per * (size_t)count;
+struct CopySpan {
+  void* dst;
+  const void* src;
+  size_t bytes;
+};
+
+// Host memcpy of every span with a few host threads, each taking a contiguous share of the bytes (pageable host memory
+// cannot be DMA'd asynchronously; one thread moves ~10 GB/s, which is slower than the GPU consumes it).
+void parallel_copy(const std::vector<CopySpan>& spans) {
+  size_t total = 0;
+  for (const CopySpan& s : spans) total += s.bytes;
   int T = (int)std::min<size_t>(8, total / ((size_t)4 << 20));
   const unsigned hw = std::thread::hardware_concurrency();
   if (hw && (unsigned)T > hw) T = (int)hw;
+  auto run = [&spans](size_t lo, size_t hi) {
+    size_t at = 0;
+    for (const CopySpan& s : spans) {
+      const size_t a = std::max(lo, at), b = std::min(hi, at + s.bytes);
+      if (a < b) memcpy((char*)s.dst + (a - at), (const char*)s.src + (a - at), b - a);
+      at += s.bytes;
+      if (at >= hi) break;
+    }
+  };
   if (T <= 1) {
-    for (int b = 0; b < count; ++b) memcpy(dst_base + per * b, bufs[first + b], per);
+    run(0, total);
     return;
   }
   std::vector<std::thread> th;
-  for (int t = 0; t < T; ++t)
-    th.emplace_back([=] {
-      for (int b = t; b < count; b += T) memcpy(dst_base + per * b, bufs[first + b], per);
-    });
+  for (int t = 0; t < T; ++t) th.emplace_back(run, total * t / T, total * (t + 1) / T);
   for (auto& x : th) x.join();
+}
+
+// Host -> device of spans whose dst lies in the pinned area h (mirrored at d); [tables, bytes) holds the library's own
+// tables.  A batch is gathered into the pinned area and copied once; a single cloud or pair goes straight from the
+// caller's memory, where the driver pipelines its own staging of pageable memory with the DMA, and the tables follow
+// in one pinned copy.
+cudaError_t stage_in(const std::vector<CopySpan>& spans, char* h, char* d, size_t tables, size_t bytes, bool direct,
+                     cudaStream_t st) {
+  if (!direct) {
+    parallel_copy(spans);
+    return cudaMemcpyAsync(d, h, bytes, cudaMemcpyHostToDevice, st);
+  }
+  std::vector<CopySpan> own;
+  for (const CopySpan& s : spans) {
+    const size_t off = (size_t)((char*)s.dst - h);
+    if (off >= tables) {
+      own.push_back(s);
+      continue;
+    }
+    const cudaError_t e = cudaMemcpyAsync(d + off, s.src, s.bytes, cudaMemcpyHostToDevice, st);
+    if (e != cudaSuccess) return e;
+  }
+  parallel_copy(own);
+  return cudaMemcpyAsync(d + tables, h + tables, bytes - tables, cudaMemcpyHostToDevice, st);
+}
+
+// Device -> host of spans whose src lies in the pinned area h (mirrored at d), then synchronise: one copy of `bytes`
+// and host copies for a batch, a copy per span (spans with dst == src land in the pinned area itself) for one cloud.
+cudaError_t stage_out(const std::vector<CopySpan>& spans, char* h, const char* d, size_t bytes, bool direct,
+                      cudaStream_t st) {
+  cudaError_t e = cudaSuccess;
+  if (!direct) {
+    e = cudaMemcpyAsync(h, d, bytes, cudaMemcpyDeviceToHost, st);
+  } else {
+    for (const CopySpan& s : spans)
+      if (e == cudaSuccess) e = cudaMemcpyAsync(s.dst, d + ((const char*)s.src - h), s.bytes, cudaMemcpyDeviceToHost, st);
+  }
+  if (e == cudaSuccess) e = cudaStreamSynchronize(st);
+  if (e == cudaSuccess && !direct) {
+    std::vector<CopySpan> host;
+    for (const CopySpan& s : spans)
+      if (s.dst != s.src) host.push_back(s);
+    parallel_copy(host);
+  }
+  return e;
+}
+
+// Copy `count` caller buffers of `per` bytes each into a contiguous pinned area.
+void parallel_stage(char* dst_base, const double* const* bufs, int first, int count, size_t per) {
+  std::vector<CopySpan> spans((size_t)count);
+  for (int b = 0; b < count; ++b) spans[b] = CopySpan{dst_base + per * b, bufs[first + b], per};
+  parallel_copy(spans);
 }
 
 // effective inlier selection mode (registration.cc:574-583)
@@ -497,6 +562,168 @@ int run_chunked(tzr_ctx* ctx, Batch& bt, const tzr_params& p, const std::vector<
   ctx->last = bt;
   ctx->have_last = true;
   ctx->last_has_graph = effective_mode(p) != 3;  // NONE: populateVertices is never called (registration.cc:607-650)
+  return TZR_OK;
+}
+
+size_t al256(size_t x) { return (x + 255) & ~(size_t)255; }
+
+// tzr_compute_fpfh(_batch): B clouds staged back to back in one pinned area, one H2D copy, the batched launches, one
+// D2H copy of [overflow flags | descriptors | normals], then the caller's buffers are filled from the pinned copy.
+int fpfh_run(tzr_ctx* ctx, int B, const int32_t* n, const float* const* pts, double normal_radius,
+             double fpfh_radius, float* const* fpfh_out, float* const* normals_out, int32_t* status) {
+  if (!ctx || B < 1 || !n || !pts || !fpfh_out || !(normal_radius > 0) || !(fpfh_radius > 0))
+    return TZR_ERR_INVALID_ARG;
+  bool want_normals = false;
+  for (int b = 0; b < B; ++b) {
+    if (n[b] <= 0 || !pts[b] || !fpfh_out[b]) return TZR_ERR_INVALID_ARG;
+    want_normals |= normals_out && normals_out[b];
+  }
+  std::vector<FpfhCloud> clouds((size_t)B);
+  FpfhPlan plan;
+  if (fpfh_plan(B, n, normal_radius, fpfh_radius, clouds.data(), &plan) != TZR_OK) {
+    ctx->last_error = "the batch's points do not fit 32-bit indices";
+    return TZR_ERR_TOO_LARGE;
+  }
+  cudaSetDevice(ctx->device);
+  cudaStream_t st = ctx->stream;
+  const size_t N = (size_t)plan.N;
+  const size_t pb = N * 12, cb = (size_t)B * sizeof(FpfhCloud), ob = (size_t)B * 4, hb = N * 33 * 4, nb = N * 16;
+  const size_t in_bytes = al256(pb) + cb, out_bytes = al256(ob) + al256(hb) + (want_normals ? nb : 0);
+  int rc;
+  if ((rc = ensure(ctx, ctx->m_in, in_bytes)) != TZR_OK) return rc;
+  if ((rc = ensure(ctx, ctx->m_scratch, al256(hb) + plan.grid_bytes)) != TZR_OK) return rc;
+  if ((rc = ensure(ctx, ctx->m_out, al256(ob) + al256(hb) + nb)) != TZR_OK) return rc;
+  if ((rc = ensure_pinned(ctx, al256(in_bytes) + out_bytes)) != TZR_OK) return rc;
+  char* h_in = (char*)ctx->h_pin;
+  char* h_out = h_in + al256(in_bytes);
+  std::vector<CopySpan> spans;
+  for (int b = 0; b < B; ++b) spans.push_back(CopySpan{h_in + (size_t)clouds[b].lo * 12, pts[b], (size_t)n[b] * 12});
+  spans.push_back(CopySpan{h_in + al256(pb), clouds.data(), cb});
+  char* d_in = (char*)ctx->m_in.p;
+  char* d_out = (char*)ctx->m_out.p;
+  CK(stage_in(spans, h_in, d_in, al256(pb), in_bytes, B == 1, st));
+  float* d_spfh = (float*)ctx->m_scratch.p;
+  void* d_grid = plan.grid_bytes ? (void*)((char*)ctx->m_scratch.p + al256(hb)) : nullptr;
+  int* d_overflow = (int*)d_out;
+  float* d_fpfh = (float*)(d_out + al256(ob));
+  float4* d_normals = (float4*)(d_out + al256(ob) + al256(hb));
+  ctx->launches += launch_fpfh(plan, (const float*)d_in, (FpfhCloud*)(d_in + al256(pb)), normal_radius, fpfh_radius,
+                               d_normals, d_spfh, d_fpfh, d_overflow, d_grid, st);
+  if ((rc = check_launch(ctx, "fpfh launch")) != TZR_OK) return rc;
+  spans.clear();
+  spans.push_back(CopySpan{h_out, h_out, ob});  // the overflow flags stay in the pinned area
+  for (int b = 0; b < B; ++b) {
+    const size_t lo = (size_t)clouds[b].lo;
+    spans.push_back(CopySpan{fpfh_out[b], h_out + al256(ob) + lo * 33 * 4, (size_t)n[b] * 33 * 4});
+    if (normals_out && normals_out[b])
+      spans.push_back(CopySpan{normals_out[b], h_out + al256(ob) + al256(hb) + lo * 16, (size_t)n[b] * 16});
+  }
+  CK(stage_out(spans, h_out, d_out, out_bytes, B == 1, st));
+  const int* overflow = (const int*)h_out;
+  bool any_overflow = false;
+  for (int b = 0; b < B; ++b) {
+    if (status) status[b] = overflow[b] ? TZR_ERR_TOO_LARGE : TZR_OK;
+    any_overflow |= overflow[b] != 0;
+  }
+  if (any_overflow) {
+    ctx->last_error = "a point has more than 4096 neighbours inside a search radius";
+    return TZR_ERR_TOO_LARGE;
+  }
+  return TZR_OK;
+}
+
+// tzr_match_correspondences(_batch): B pairs staged back to back in one pinned area with the pair table and the NN
+// work list, one H2D copy, the batched launches, one D2H copy of [counts | global scales | pairs].
+int match_run(tzr_ctx* ctx, int B, const int32_t* ns, const float* const* src_pts, const int32_t* nd,
+              const float* const* dst_pts, const float* const* src_feat, const float* const* dst_feat, int dim,
+              int use_absolute_scale, int use_crosscheck, int use_tuple_test, float tuple_scale,
+              const uint64_t* seeds, int32_t* const* pairs, const int64_t* capacity, int64_t* n_pairs,
+              float* global_scale) {
+  if (!ctx || B < 1 || !ns || !nd || !src_pts || !dst_pts || !src_feat || !dst_feat || !seeds || !pairs ||
+      !capacity || !n_pairs || dim < 1 || dim > kMatchMaxDim)
+    return TZR_ERR_INVALID_ARG;
+  for (int b = 0; b < B; ++b)
+    if (!src_pts[b] || !dst_pts[b] || !src_feat[b] || !dst_feat[b] || !pairs[b] || ns[b] <= 0 || nd[b] <= 0 ||
+        capacity[b] < 0)
+      return TZR_ERR_INVALID_ARG;
+  for (int b = 0; b < B; ++b)
+    if ((long long)ns[b] + nd[b] > (1ll << 30)) return TZR_ERR_TOO_LARGE;
+  std::vector<MatchPair> P;
+  std::vector<NnWork> W;
+  MatchPlan plan;
+  if (match_plan(B, ns, nd, seeds, ctx->num_sms, &P, &W, &plan) != TZR_OK) {
+    ctx->last_error = "the batch's points do not fit 32-bit indices";
+    return TZR_ERR_TOO_LARGE;
+  }
+  cudaSetDevice(ctx->device);
+  cudaStream_t st = ctx->stream;
+  const size_t C = (size_t)plan.NS + plan.ND;
+  const size_t psb = (size_t)plan.NS * 12, pdb = (size_t)plan.ND * 12, fsb = (size_t)plan.NS * dim * 4,
+               fdb = (size_t)plan.ND * dim * 4, tb = P.size() * sizeof(MatchPair), wb = W.size() * sizeof(NnWork);
+  const size_t o_dp = al256(psb), o_sf = o_dp + al256(pdb), o_df = o_sf + al256(fsb), o_t = o_df + al256(fdb),
+               o_w = o_t + al256(tb), in_bytes = o_w + wb;
+  const size_t o_g = (size_t)B * 4, o_pairs = al256((size_t)B * 8), out_bytes = o_pairs + C * 8;
+  int rc;
+  if ((rc = ensure(ctx, ctx->m_in, in_bytes)) != TZR_OK) return rc;
+  if ((rc = ensure(ctx, ctx->m_scratch, match_scratch_bytes(plan))) != TZR_OK) return rc;
+  if ((rc = ensure(ctx, ctx->m_out, out_bytes)) != TZR_OK) return rc;
+  if ((rc = ensure_pinned(ctx, al256(in_bytes) + out_bytes)) != TZR_OK) return rc;
+  char* h_in = (char*)ctx->h_pin;
+  char* h_out = h_in + al256(in_bytes);
+  std::vector<CopySpan> spans;
+  for (int b = 0; b < B; ++b) {
+    const size_t so = (size_t)P[b].s_off, dof = (size_t)P[b].d_off;
+    spans.push_back(CopySpan{h_in + so * 12, src_pts[b], (size_t)ns[b] * 12});
+    spans.push_back(CopySpan{h_in + o_dp + dof * 12, dst_pts[b], (size_t)nd[b] * 12});
+    spans.push_back(CopySpan{h_in + o_sf + so * dim * 4, src_feat[b], (size_t)ns[b] * dim * 4});
+    spans.push_back(CopySpan{h_in + o_df + dof * dim * 4, dst_feat[b], (size_t)nd[b] * dim * 4});
+  }
+  spans.push_back(CopySpan{h_in + o_t, P.data(), tb});
+  spans.push_back(CopySpan{h_in + o_w, W.data(), wb});
+  char* d_in = (char*)ctx->m_in.p;
+  char* d_out = (char*)ctx->m_out.p;
+  CK(stage_in(spans, h_in, d_in, o_t, in_bytes, B == 1, st));
+  const int nl = launch_match(plan, (const MatchPair*)(d_in + o_t), (const NnWork*)(d_in + o_w), (int)W.size(),
+                              (float*)d_in, (float*)(d_in + o_dp), (const float*)(d_in + o_sf),
+                              (const float*)(d_in + o_df), dim, use_absolute_scale, use_crosscheck, use_tuple_test,
+                              tuple_scale, ctx->m_scratch.p, (int32_t*)(d_out + o_pairs), (int*)d_out,
+                              (float*)(d_out + o_g), ctx->num_sms, st);
+  ctx->launches += nl;
+  if ((rc = check_launch(ctx, "matcher launch")) != TZR_OK) return rc;
+  struct {
+    int count;
+    float g;
+  } one;
+  if (B == 1) {  // one pair: its count and scale, then only the rows it has, straight into the caller's buffer
+    CK(cudaMemcpyAsync(&one, d_out, 8, cudaMemcpyDeviceToHost, st));
+    CK(cudaStreamSynchronize(st));
+    if (one.count > 0 && (int64_t)one.count <= capacity[0]) {
+      CK(cudaMemcpyAsync(pairs[0], d_out + o_pairs, (size_t)one.count * 8, cudaMemcpyDeviceToHost, st));
+      CK(cudaStreamSynchronize(st));
+    }
+  } else {
+    CK(cudaMemcpyAsync(h_out, d_out, out_bytes, cudaMemcpyDeviceToHost, st));
+    CK(cudaStreamSynchronize(st));
+  }
+  const int* counts = B == 1 ? &one.count : (const int*)h_out;
+  const float* g = B == 1 ? &one.g : (const float*)(h_out + o_g);
+  spans.clear();
+  bool too_small = false;
+  for (int b = 0; b < B; ++b) {
+    n_pairs[b] = counts[b];
+    if (global_scale) global_scale[b] = g[b];
+    if ((int64_t)counts[b] > capacity[b]) {
+      too_small = true;
+      continue;
+    }
+    const size_t slot = (size_t)P[b].s_off + P[b].d_off;
+    if (B > 1) spans.push_back(CopySpan{pairs[b], h_out + o_pairs + slot * 8, (size_t)counts[b] * 8});
+  }
+  parallel_copy(spans);
+  if (too_small) {
+    ctx->last_error = "pairs capacity too small";
+    return TZR_ERR_INVALID_ARG;
+  }
   return TZR_OK;
 }
 
@@ -1090,55 +1317,19 @@ int tzr_match_correspondences(tzr_ctx* ctx, const float* src_pts, int ns, const 
                               const float* src_feat, const float* dst_feat, int dim, int use_absolute_scale,
                               int use_crosscheck, int use_tuple_test, float tuple_scale, uint64_t tuple_seed,
                               int32_t* pairs, int64_t capacity, int64_t* n_pairs, float* global_scale) {
-  if (!ctx || !src_pts || !dst_pts || !src_feat || !dst_feat || !pairs || !n_pairs || ns <= 0 || nd <= 0 ||
-      dim < 1 || dim > kMatchMaxDim || capacity < 0)
-    return TZR_ERR_INVALID_ARG;
-  if ((long long)ns + nd > (1ll << 30)) return TZR_ERR_TOO_LARGE;
-  cudaSetDevice(ctx->device);
-  cudaStream_t st = ctx->stream;
-  const size_t pb_s = (size_t)ns * 3 * 4, pb_d = (size_t)nd * 3 * 4, fb_s = (size_t)ns * dim * 4,
-               fb_d = (size_t)nd * dim * 4;
-  auto al = [](size_t x) { return (x + 255) & ~(size_t)255; };
-  int rc;
-  if ((rc = ensure(ctx, ctx->m_in, al(pb_s) + al(pb_d) + al(fb_s) + al(fb_d))) != TZR_OK) return rc;
-  if ((rc = ensure(ctx, ctx->m_scratch, match_scratch_bytes(ns, nd))) != TZR_OK) return rc;
-  const size_t cap = (size_t)ns + nd;
-  if ((rc = ensure(ctx, ctx->m_out, cap * 8 + 256)) != TZR_OK) return rc;
-  char* in = (char*)ctx->m_in.p;
-  float* d_sp = (float*)in;
-  float* d_dp = (float*)(in + al(pb_s));
-  float* d_sf = (float*)(in + al(pb_s) + al(pb_d));
-  float* d_df = (float*)(in + al(pb_s) + al(pb_d) + al(fb_s));
-  int32_t* d_pairs = (int32_t*)ctx->m_out.p;
-  int* d_count = (int*)((char*)ctx->m_out.p + cap * 8);
-  float* d_g = (float*)(d_count + 1);
-  CK(cudaMemcpyAsync(d_sp, src_pts, pb_s, cudaMemcpyHostToDevice, st));
-  CK(cudaMemcpyAsync(d_dp, dst_pts, pb_d, cudaMemcpyHostToDevice, st));
-  CK(cudaMemcpyAsync(d_sf, src_feat, fb_s, cudaMemcpyHostToDevice, st));
-  CK(cudaMemcpyAsync(d_df, dst_feat, fb_d, cudaMemcpyHostToDevice, st));
-  const int nl = launch_match(d_sp, ns, d_dp, nd, d_sf, d_df, dim, use_absolute_scale, use_crosscheck,
-                              use_tuple_test, tuple_scale, tuple_seed, ctx->m_scratch.p, d_pairs, d_count, d_g,
-                              ctx->num_sms, st);
-  if (nl < 0) return nl;
-  ctx->launches += nl;
-  if ((rc = check_launch(ctx, "matcher launch")) != TZR_OK) return rc;
-  struct {
-    int count;
-    float g;
-  } tail;
-  CK(cudaMemcpyAsync(&tail, d_count, 8, cudaMemcpyDeviceToHost, st));
-  CK(cudaStreamSynchronize(st));
-  *n_pairs = tail.count;
-  if (global_scale) *global_scale = tail.g;
-  if ((int64_t)tail.count > capacity) {
-    ctx->last_error = "pairs capacity too small";
-    return TZR_ERR_INVALID_ARG;
-  }
-  if (tail.count > 0) {
-    CK(cudaMemcpyAsync(pairs, d_pairs, (size_t)tail.count * 8, cudaMemcpyDeviceToHost, st));
-    CK(cudaStreamSynchronize(st));
-  }
-  return TZR_OK;
+  const int32_t ns1 = ns, nd1 = nd;
+  return match_run(ctx, 1, &ns1, &src_pts, &nd1, &dst_pts, &src_feat, &dst_feat, dim, use_absolute_scale,
+                   use_crosscheck, use_tuple_test, tuple_scale, &tuple_seed, &pairs, &capacity, n_pairs, global_scale);
+}
+
+int tzr_match_correspondences_batch(tzr_ctx* ctx, int B, const int32_t* ns, const float* const* src_pts,
+                                    const int32_t* nd, const float* const* dst_pts, const float* const* src_feat,
+                                    const float* const* dst_feat, int dim, int use_absolute_scale, int use_crosscheck,
+                                    int use_tuple_test, float tuple_scale, const uint64_t* tuple_seeds,
+                                    int32_t* const* pairs, const int64_t* capacity, int64_t* n_pairs,
+                                    float* global_scale) {
+  return match_run(ctx, B, ns, src_pts, nd, dst_pts, src_feat, dst_feat, dim, use_absolute_scale, use_crosscheck,
+                   use_tuple_test, tuple_scale, tuple_seeds, pairs, capacity, n_pairs, global_scale);
 }
 
 void tzr_certifier_params_default(tzr_certifier_params* p) {
@@ -1192,37 +1383,14 @@ int tzr_certifier_dual_projection(tzr_ctx* ctx, const double* W, const double* t
 
 int tzr_compute_fpfh(tzr_ctx* ctx, const float* pts, int n, double normal_search_radius, double fpfh_search_radius,
                      float* fpfh_out, float* normals_out) {
-  if (!ctx || !pts || !fpfh_out || n <= 0 || !(normal_search_radius > 0) || !(fpfh_search_radius > 0))
-    return TZR_ERR_INVALID_ARG;
-  cudaSetDevice(ctx->device);
-  cudaStream_t st = ctx->stream;
-  auto al = [](size_t x) { return (x + 255) & ~(size_t)255; };
-  const size_t pb = (size_t)n * 12, nb = (size_t)n * 16, hb = (size_t)n * 33 * 4;
-  int rc;
-  if ((rc = ensure(ctx, ctx->m_in, al(pb))) != TZR_OK) return rc;
-  const size_t gb = fpfh_grid_scratch_bytes(n);
-  if ((rc = ensure(ctx, ctx->m_scratch, al(nb) + al(hb) + 256 + gb)) != TZR_OK) return rc;
-  if ((rc = ensure(ctx, ctx->m_out, al(hb))) != TZR_OK) return rc;
-  float* d_pts = (float*)ctx->m_in.p;
-  float4* d_normals = (float4*)ctx->m_scratch.p;
-  float* d_spfh = (float*)((char*)ctx->m_scratch.p + al(nb));
-  int* d_overflow = (int*)((char*)ctx->m_scratch.p + al(nb) + al(hb));
-  float* d_out = (float*)ctx->m_out.p;
-  CK(cudaMemcpyAsync(d_pts, pts, pb, cudaMemcpyHostToDevice, st));
-  void* d_grid = gb ? (void*)((char*)ctx->m_scratch.p + al(nb) + al(hb) + 256) : nullptr;
-  ctx->launches += launch_fpfh(d_pts, n, normal_search_radius, fpfh_search_radius, d_normals, d_spfh, d_out,
-                               d_overflow, d_grid, st);
-  if ((rc = check_launch(ctx, "fpfh launch")) != TZR_OK) return rc;
-  int overflow = 0;
-  CK(cudaMemcpyAsync(&overflow, d_overflow, sizeof(int), cudaMemcpyDeviceToHost, st));
-  CK(cudaMemcpyAsync(fpfh_out, d_out, hb, cudaMemcpyDeviceToHost, st));
-  if (normals_out) CK(cudaMemcpyAsync(normals_out, d_normals, nb, cudaMemcpyDeviceToHost, st));
-  CK(cudaStreamSynchronize(st));
-  if (overflow) {
-    ctx->last_error = "a point has more than 4096 neighbours inside a search radius";
-    return TZR_ERR_TOO_LARGE;
-  }
-  return TZR_OK;
+  const int32_t n1 = n;
+  return fpfh_run(ctx, 1, &n1, &pts, normal_search_radius, fpfh_search_radius, &fpfh_out, &normals_out, nullptr);
+}
+
+int tzr_compute_fpfh_batch(tzr_ctx* ctx, int B, const int32_t* n, const float* const* pts,
+                           double normal_search_radius, double fpfh_search_radius, float* const* fpfh_out,
+                           float* const* normals_out, int32_t* status) {
+  return fpfh_run(ctx, B, n, pts, normal_search_radius, fpfh_search_radius, fpfh_out, normals_out, status);
 }
 
 int tzr_feature_nn(tzr_ctx* ctx, const float* query, int nq, const float* db, int ndb, int dim, int32_t* nn_index,
@@ -1233,15 +1401,21 @@ int tzr_feature_nn(tzr_ctx* ctx, const float* query, int nq, const float* db, in
   cudaStream_t st = ctx->stream;
   auto al = [](size_t x) { return (x + 255) & ~(size_t)255; };
   const size_t qb = (size_t)nq * dim * 4, dbb = (size_t)ndb * dim * 4;
+  std::vector<NnWork> work;  // ~4 CTAs per SM
+  const long long tile_pairs = (long long)((nq + 63) / 64) * ((ndb + 63) / 64);
+  nn_work_append(&work, 0, 0, nq, 0, ndb, nn_tiles_per_seg(tile_pairs, 4 * ctx->num_sms));
+  const size_t wb = work.size() * sizeof(NnWork);
   int rc;
-  if ((rc = ensure(ctx, ctx->m_in, al(qb) + al(dbb))) != TZR_OK) return rc;
+  if ((rc = ensure(ctx, ctx->m_in, al(qb) + al(dbb) + wb)) != TZR_OK) return rc;
   if ((rc = ensure(ctx, ctx->m_out, (size_t)nq * 8)) != TZR_OK) return rc;
   float* d_q = (float*)ctx->m_in.p;
   float* d_db = (float*)((char*)ctx->m_in.p + al(qb));
+  NnWork* d_work = (NnWork*)((char*)ctx->m_in.p + al(qb) + al(dbb));
   unsigned long long* d_best = (unsigned long long*)ctx->m_out.p;
   CK(cudaMemcpyAsync(d_q, query, qb, cudaMemcpyHostToDevice, st));
   CK(cudaMemcpyAsync(d_db, db, dbb, cudaMemcpyHostToDevice, st));
-  ctx->launches += launch_feature_nn(d_q, nq, d_db, ndb, dim, d_best, ctx->num_sms, st);
+  CK(cudaMemcpyAsync(d_work, work.data(), wb, cudaMemcpyHostToDevice, st));
+  ctx->launches += launch_feature_nn(d_work, (int)work.size(), d_q, d_db, dim, d_best, nullptr, nq, st);
   if ((rc = check_launch(ctx, "feature nn launch")) != TZR_OK) return rc;
   std::vector<unsigned long long> h((size_t)nq);
   CK(cudaMemcpyAsync(h.data(), d_best, (size_t)nq * 8, cudaMemcpyDeviceToHost, st));

@@ -21,12 +21,17 @@
 // 3x3x3 cell neighbourhood and applies the SAME float distance test, so the neighbour sets — and everything downstream —
 // are identical to the brute-force ones (a point two cells away is farther than the radius by more than the float
 // error of the test; hash collisions only add candidates that fail it).
+//
+// Batches: every kernel runs over B clouds stored back to back (one CTA per point of the whole batch); a CTA finds its
+// cloud from the per-cloud FpfhCloud table and searches only inside it.  Each grid cloud owns the bucket range
+// [base, base + T_b); one radix sort on base + hash orders the points of all of them, and the table (origin, 1/h, mask,
+// base, brute-force fallback) stays on the device, so nothing is read back before the three descriptor kernels.  A
+// single cloud is the B = 1 case of the same launches.
 #include <math_constants.h>
 
 #include <cub/cub.cuh>
 
 #include <algorithm>
-#include <cstring>
 
 #include "tzr_internal.cuh"
 
@@ -213,17 +218,29 @@ __device__ bool pair_features(const float* p1, const float* n1, const float* p2,
   return true;
 }
 
-
 constexpr int kGridMinN = 4096;
 
-struct Grid {          // all-zero (n_sorted == 0) means brute force
-  const int* sorted;   // point indices sorted by bucket
-  const int* bstart;   // [T] first position of every bucket in sorted
-  const int* bend;     // [T] one past the last
+// the cloud of flat point p: the last c with clouds[c].lo <= p (every cloud has at least one point)
+__device__ __forceinline__ int cloud_of(const FpfhCloud* __restrict__ clouds, int B, int p) {
+  int lo = 0, hi = B - 1;
+  while (lo < hi) {
+    const int mid = (lo + hi + 1) >> 1;
+    if (clouds[mid].lo <= p) lo = mid;
+    else hi = mid - 1;
+  }
+  return lo;
+}
+
+struct Grid {           // the radius search of one cloud; n_sorted == 0 means brute force over [lo, lo + n)
+  const int* sorted;    // flat point indices of the batch sorted by bucket
+  const int* bstart;    // [buckets] first position of every bucket in sorted
+  const int* bend;      // [buckets] one past the last
+  int lo, n;
   int n_sorted;
-  unsigned int mask;   // T - 1
-  double ox, oy, oz;   // grid origin (bounding-box minimum)
-  double inv_h;        // 1 / cell edge
+  unsigned int mask;    // T_b - 1
+  unsigned int base;    // first bucket of the cloud
+  double ox, oy, oz;    // grid origin (bounding-box minimum)
+  double inv_h;         // 1 / cell edge
 };
 
 __device__ __forceinline__ unsigned int cell_hash(long long ix, long long iy, long long iz, unsigned int mask) {
@@ -249,52 +266,87 @@ __device__ __forceinline__ int f2ord(float f) {
 }
 __device__ __forceinline__ float ord2f(int i) { return __int_as_float(i >= 0 ? i : i ^ 0x7fffffff); }
 
-__global__ void bbox_min_kernel(const float* __restrict__ pts, int n, int* mins /*[3], init INT_MAX*/) {
+// The search of cloud c: the grid when the cloud has one and every finite point of it found a cell, else brute force.
+__device__ __forceinline__ Grid grid_of(const FpfhCloud& cl, const int* sorted, const int* bstart, const int* bend) {
+  Grid g{};
+  g.lo = cl.lo;
+  g.n = cl.n;
+  if (!cl.grid || cl.mins[3]) return g;
+  g.sorted = sorted;
+  g.bstart = bstart;
+  g.bend = bend;
+  g.n_sorted = cl.n;
+  g.mask = cl.mask;
+  g.base = cl.base;
+  g.ox = (double)ord2f(cl.mins[0]);
+  g.oy = (double)ord2f(cl.mins[1]);
+  g.oz = (double)ord2f(cl.mins[2]);
+  g.inv_h = cl.inv_h;
+  return g;
+}
+
+// per-cloud minimum of the grid clouds' points; a warp whose lanes share one cloud reduces before its atomics
+__global__ void bbox_min_kernel(const float* __restrict__ pts, int N, FpfhCloud* clouds, int B) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   int m[3] = {0x7fffffff, 0x7fffffff, 0x7fffffff};
-  if (i < n)
-    for (int k = 0; k < 3; ++k) {
-      const float v = pts[3 * (size_t)i + k];
-      if (v == v && fabsf(v) < 3.0e38f) m[k] = f2ord(v);
-    }
+  int c = -1;
+  if (i < N) {
+    c = cloud_of(clouds, B, i);
+    if (clouds[c].grid)
+      for (int k = 0; k < 3; ++k) {
+        const float v = pts[3 * (size_t)i + k];
+        if (v == v && fabsf(v) < 3.0e38f) m[k] = f2ord(v);
+      }
+  }
+  const bool uniform = __all_sync(0xffffffffu, c == __shfl_sync(0xffffffffu, c, 0));
   for (int k = 0; k < 3; ++k) {
-    for (int off = 16; off; off >>= 1) m[k] = min(m[k], __shfl_xor_sync(0xffffffffu, m[k], off));
-    if ((threadIdx.x & 31) == 0 && m[k] != 0x7fffffff) atomicMin(&mins[k], m[k]);
+    if (uniform)
+      for (int off = 16; off; off >>= 1) m[k] = min(m[k], __shfl_xor_sync(0xffffffffu, m[k], off));
+    if ((!uniform || (threadIdx.x & 31) == 0) && m[k] != 0x7fffffff) atomicMin(&clouds[c].mins[k], m[k]);
   }
 }
 
-__global__ void bucket_kernel(const float* __restrict__ pts, int n, const int* __restrict__ mins, double inv_h,
-                              unsigned int mask, unsigned int* __restrict__ keys, int* __restrict__ idx) {
+// key = the cloud's first bucket + cell hash; `buckets` (a bucket nobody visits) for non-finite points and for the
+// points of brute-force clouds
+__global__ void bucket_kernel(const float* __restrict__ pts, int N, FpfhCloud* clouds, int B, unsigned int buckets,
+                              unsigned int* __restrict__ keys, int* __restrict__ idx) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= n) return;
+  if (i >= N) return;
+  idx[i] = i;
+  const int c = cloud_of(clouds, B, i);
+  FpfhCloud& cl = clouds[c];
+  if (!cl.grid) {
+    keys[i] = buckets;
+    return;
+  }
   Grid g{};
-  g.ox = (double)ord2f(mins[0]);
-  g.oy = (double)ord2f(mins[1]);
-  g.oz = (double)ord2f(mins[2]);
-  g.inv_h = inv_h;
+  g.ox = (double)ord2f(cl.mins[0]);
+  g.oy = (double)ord2f(cl.mins[1]);
+  g.oz = (double)ord2f(cl.mins[2]);
+  g.inv_h = cl.inv_h;
   long long ix, iy, iz;
   const float x = pts[3 * (size_t)i], y = pts[3 * (size_t)i + 1], z = pts[3 * (size_t)i + 2];
   const bool ok = cell_of(g, x, y, z, &ix, &iy, &iz);
-  keys[i] = ok ? cell_hash(ix, iy, iz, mask) : (mask + 1u);  // non-finite points: a bucket nobody visits
-  idx[i] = i;
-  // a finite point the grid cannot index (extent / radius beyond 2^62 cells): tell the host to use brute force
+  keys[i] = ok ? cl.base + cell_hash(ix, iy, iz, cl.mask) : buckets;
+  // a finite point the grid cannot index (extent / radius beyond 2^62 cells): this cloud falls back to brute force
   if (!ok && x == x && y == y && z == z && fabsf(x) < 3.0e38f && fabsf(y) < 3.0e38f && fabsf(z) < 3.0e38f)
-    const_cast<int*>(mins)[3] = 1;
+    cl.mins[3] = 1;
 }
 
-__global__ void bucket_bounds_kernel(const unsigned int* __restrict__ keys, int n, unsigned int mask,
+__global__ void bucket_bounds_kernel(const unsigned int* __restrict__ keys, int n, unsigned int buckets,
                                      int* __restrict__ bstart, int* __restrict__ bend) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n) return;
   const unsigned int k = keys[i];
-  if (k > mask) return;
+  if (k >= buckets) return;
   if (i == 0 || keys[i - 1] != k) bstart[k] = i;
   if (i == n - 1 || keys[i + 1] != k) bend[k] = i + 1;
 }
 
-// Block-wide radius search of point q: keys[] (shared, kNbCap) receives (d2 bits << 32 | index) of every point with
-// d2 < r2, unordered.  Returns the count (may exceed kNbCap: overflow, caller flags it).  Contains __syncthreads.
-__device__ int collect_neighbors(const float* __restrict__ pts, int n, int q, float r2, unsigned long long* keys,
+// Block-wide radius search of point q inside its cloud: keys[] (shared, kNbCap) receives (d2 bits << 32 | index) of
+// every point with d2 < r2, unordered; indices are flat, so their order within the cloud is the cloud-local one.
+// Returns the count (may exceed kNbCap: overflow, caller flags it).  Contains __syncthreads.
+__device__ int collect_neighbors(const float* __restrict__ pts, int q, float r2, unsigned long long* keys,
                                  int* s_count, const Grid& g) {
   __shared__ int s_rs[28], s_re[28], s_pref[28];
   if (threadIdx.x == 0) *s_count = 0;
@@ -311,7 +363,7 @@ __device__ int collect_neighbors(const float* __restrict__ pts, int n, int q, fl
   };
   if (g.n_sorted == 0) {  // brute force
     __syncthreads();
-    for (int i = threadIdx.x; i < n; i += blockDim.x) test(i);
+    for (int i = g.lo + threadIdx.x; i < g.lo + g.n; i += blockDim.x) test(i);
     __syncthreads();
     return *s_count;
   }
@@ -326,8 +378,8 @@ __device__ int collect_neighbors(const float* __restrict__ pts, int n, int q, fl
       for (int u = 0; u < t; ++u)
         dup |= cell_hash(ix + (u % 3) - 1, iy + ((u / 3) % 3) - 1, iz + (u / 9) - 1, g.mask) == b;
       if (!dup) {
-        rs = g.bstart[b];
-        re = g.bend[b];
+        rs = g.bstart[g.base + b];
+        re = g.bend[g.base + b];
       }
     }
     s_rs[threadIdx.x] = rs;
@@ -376,16 +428,29 @@ __device__ void sort_keys(unsigned long long* keys, int count) {
     }
 }
 
-__global__ void __launch_bounds__(kFpfhThreads) normals_kernel(const float* __restrict__ pts, int n, float r2,
-                                                              float4* __restrict__ normals, int* overflow,
-                                                              Grid g) {
+// The arguments every descriptor kernel shares: the flat points, the cloud table and the batch's grid arrays.
+struct Clouds {
+  const float* pts;
+  const FpfhCloud* clouds;
+  int B;
+  const int* sorted;
+  const int* bstart;
+  const int* bend;
+  __device__ __forceinline__ int cloud(int p) const { return cloud_of(clouds, B, p); }
+  __device__ __forceinline__ Grid grid(int c) const { return grid_of(clouds[c], sorted, bstart, bend); }
+};
+
+__global__ void __launch_bounds__(kFpfhThreads) normals_kernel(Clouds cs, float r2, float4* __restrict__ normals,
+                                                              int* overflow) {
   __shared__ unsigned long long keys[kNbCap];
   __shared__ int s_count;
+  const float* __restrict__ pts = cs.pts;
   const int p = blockIdx.x;
-  const int cnt = collect_neighbors(pts, n, p, r2, keys, &s_count, g);
+  const int c = cs.cloud(p);
+  const int cnt = collect_neighbors(pts, p, r2, keys, &s_count, cs.grid(c));
   if (cnt > kNbCap) {
     if (threadIdx.x == 0) {
-      atomicExch(overflow, 1);
+      atomicExch(&overflow[c], 1);
       normals[p] = make_float4(CUDART_NAN_F, CUDART_NAN_F, CUDART_NAN_F, CUDART_NAN_F);
     }
     return;
@@ -444,17 +509,18 @@ __device__ __forceinline__ int bin11(double v) {  // static_cast<int>(floor(v)) 
   return (int)f;
 }
 
-__global__ void __launch_bounds__(kFpfhThreads) spfh_kernel(const float* __restrict__ pts,
-                                                           const float4* __restrict__ normals, int n, float r2,
-                                                           float* __restrict__ spfh, int* overflow, Grid g) {
+__global__ void __launch_bounds__(kFpfhThreads) spfh_kernel(Clouds cs, const float4* __restrict__ normals, float r2,
+                                                           float* __restrict__ spfh, int* overflow) {
   __shared__ unsigned long long keys[kNbCap];
   __shared__ int s_count;
   __shared__ int s_bins[33];
+  const float* __restrict__ pts = cs.pts;
   const int p = blockIdx.x;
+  const int c = cs.cloud(p);
   if (threadIdx.x < 33) s_bins[threadIdx.x] = 0;
-  const int cnt = collect_neighbors(pts, n, p, r2, keys, &s_count, g);  // its barriers also publish s_bins
+  const int cnt = collect_neighbors(pts, p, r2, keys, &s_count, cs.grid(c));  // its barriers also publish s_bins
   if (cnt > kNbCap) {
-    if (threadIdx.x == 0) atomicExch(overflow, 1);
+    if (threadIdx.x == 0) atomicExch(&overflow[c], 1);
     if (threadIdx.x < 33) spfh[(size_t)p * 33 + threadIdx.x] = 0.f;
     return;
   }
@@ -478,20 +544,20 @@ __global__ void __launch_bounds__(kFpfhThreads) spfh_kernel(const float* __restr
   if (threadIdx.x < 33) {
     const float hist_incr = 100.0f / (float)(cnt - 1);
     float v = 0.f;
-    for (int c = s_bins[threadIdx.x]; c > 0; --c) v += hist_incr;  // the reference's repeated `+= hist_incr`
+    for (int k = s_bins[threadIdx.x]; k > 0; --k) v += hist_incr;  // the reference's repeated `+= hist_incr`
     spfh[(size_t)p * 33 + threadIdx.x] = v;
   }
 }
 
-__global__ void __launch_bounds__(kFpfhThreads) fpfh_kernel(const float* __restrict__ pts,
-                                                           const float* __restrict__ spfh, int n, float r2,
-                                                           float* __restrict__ out, int* overflow, Grid g) {
+__global__ void __launch_bounds__(kFpfhThreads) fpfh_kernel(Clouds cs, const float* __restrict__ spfh, float r2,
+                                                           float* __restrict__ out, int* overflow) {
   __shared__ unsigned long long keys[kNbCap];
   __shared__ int s_count;
   const int p = blockIdx.x;
-  const int cnt = collect_neighbors(pts, n, p, r2, keys, &s_count, g);
+  const int c = cs.cloud(p);
+  const int cnt = collect_neighbors(cs.pts, p, r2, keys, &s_count, cs.grid(c));
   if (cnt > kNbCap) {
-    if (threadIdx.x == 0) atomicExch(overflow, 1);
+    if (threadIdx.x == 0) atomicExch(&overflow[c], 1);
     if (threadIdx.x < 33) out[(size_t)p * 33 + threadIdx.x] = 0.f;
     return;
   }
@@ -521,75 +587,87 @@ __global__ void __launch_bounds__(kFpfhThreads) fpfh_kernel(const float* __restr
   for (int k = 0; k < 11; ++k) out[(size_t)p * 33 + 11 * s + k] = acc[k] * sc;
 }
 
-}  // namespace
-
-size_t fpfh_grid_scratch_bytes(int n) {
-  if (n < kGridMinN) return 0;
-  unsigned int T = 1024;
-  while (T < 2u * (unsigned int)n) T <<= 1;
+size_t radix_bytes(int n, int bits) {
   size_t cub_bytes = 0;
   cub::DeviceRadixSort::SortPairs(nullptr, cub_bytes, (const unsigned int*)nullptr, (unsigned int*)nullptr,
-                                  (const int*)nullptr, (int*)nullptr, n);
-  return 4 * (size_t)n * 4 + 2 * (size_t)T * 4 + 64 + cub_bytes + 1024;
+                                  (const int*)nullptr, (int*)nullptr, n, 0, bits);
+  return cub_bytes;
 }
 
-// pts, normals (n float4), spfh (n x 33), out (n x 33), overflow (int, zeroed here), grid_scratch
-// (fpfh_grid_scratch_bytes(n) bytes, may be null below kGridMinN): device pointers.
-int launch_fpfh(const float* pts, int n, double normal_radius, double fpfh_radius, float4* normals, float* spfh,
-                float* out, int* overflow, void* grid_scratch, cudaStream_t st) {
+int key_bits(unsigned int buckets) {  // keys go up to `buckets` (the sentinel)
+  int bits = 1;
+  while (bits < 32 && (1ull << bits) <= buckets) ++bits;
+  return bits;
+}
+
+}  // namespace
+
+int fpfh_plan(int B, const int32_t* n, double normal_radius, double fpfh_radius, FpfhCloud* clouds, FpfhPlan* plan) {
+  const double h = std::max(normal_radius, fpfh_radius) * (1.0 + 1e-5);
+  long long lo = 0, buckets = 0;
+  bool any_grid = false;
+  for (int c = 0; c < B; ++c) {
+    FpfhCloud& cl = clouds[c];
+    cl = FpfhCloud{};
+    cl.lo = (int)lo;
+    cl.n = n[c];
+    cl.grid = n[c] >= kGridMinN;
+    cl.mins[0] = cl.mins[1] = cl.mins[2] = 0x7fffffff;
+    cl.mins[3] = 0;
+    cl.inv_h = 1.0 / h;
+    if (cl.grid) {
+      unsigned int T = 1024;
+      while (T < 2u * (unsigned int)n[c]) T <<= 1;
+      cl.mask = T - 1;
+      cl.base = (unsigned int)buckets;
+      buckets += T;
+      any_grid = true;
+    }
+    lo += n[c];
+  }
+  if (lo > 0x7fffffffll || buckets >= 0xffffffffll) return TZR_ERR_TOO_LARGE;
+  plan->B = B;
+  plan->N = (int)lo;
+  plan->any_grid = any_grid;
+  plan->buckets = (unsigned int)buckets;
+  plan->grid_bytes = any_grid ? 4 * (size_t)lo * 4 + 2 * (size_t)buckets * 4 +
+                                    radix_bytes(plan->N, key_bits(plan->buckets)) + 1024
+                              : 0;
+  return TZR_OK;
+}
+
+int launch_fpfh(const FpfhPlan& plan, const float* pts, FpfhCloud* clouds, double normal_radius, double fpfh_radius,
+                float4* normals, float* spfh, float* out, int* overflow, void* grid_scratch, cudaStream_t st) {
   const float r2n = (float)(normal_radius * normal_radius);
   const float r2f = (float)(fpfh_radius * fpfh_radius);
+  const int N = plan.N, B = plan.B;
   int nl = 0;
-  cudaMemsetAsync(overflow, 0, sizeof(int), st);
-  Grid g{};
-  if (n >= kGridMinN && grid_scratch) {
-    unsigned int T = 1024;
-    while (T < 2u * (unsigned int)n) T <<= 1;
+  cudaMemsetAsync(overflow, 0, (size_t)B * sizeof(int), st);
+  Clouds cs{pts, clouds, B, nullptr, nullptr, nullptr};
+  if (plan.any_grid) {
+    const unsigned int T = plan.buckets;
     char* w = (char*)grid_scratch;
-    unsigned int* keys = (unsigned int*)w;  w += (size_t)n * 4;
-    unsigned int* keys2 = (unsigned int*)w; w += (size_t)n * 4;
-    int* idx = (int*)w;                     w += (size_t)n * 4;
-    int* idx2 = (int*)w;                    w += (size_t)n * 4;
+    unsigned int* keys = (unsigned int*)w;  w += (size_t)N * 4;
+    unsigned int* keys2 = (unsigned int*)w; w += (size_t)N * 4;
+    int* idx = (int*)w;                     w += (size_t)N * 4;
+    int* idx2 = (int*)w;                    w += (size_t)N * 4;
     int* bstart = (int*)w;                  w += (size_t)T * 4;
     int* bend = (int*)w;                    w += (size_t)T * 4;
-    int* mins = (int*)w;                    w += 64;
-    size_t cub_bytes = 0;
-    cub::DeviceRadixSort::SortPairs(nullptr, cub_bytes, (const unsigned int*)nullptr, (unsigned int*)nullptr,
-                                    (const int*)nullptr, (int*)nullptr, n);
-    const double h = std::max(normal_radius, fpfh_radius) * (1.0 + 1e-5);
-    int bits = 1;
-    while ((1u << bits) <= T) ++bits;  // keys go up to T (the sentinel bucket)
-    const int init[4] = {0x7fffffff, 0x7fffffff, 0x7fffffff, 0};
-    cudaMemcpyAsync(mins, init, 16, cudaMemcpyHostToDevice, st);
+    const int bits = key_bits(T);
+    size_t cub_bytes = radix_bytes(N, bits);
     cudaMemsetAsync(bstart, 0, 2 * (size_t)T * 4, st);
-    bbox_min_kernel<<<(n + 255) / 256, 256, 0, st>>>(pts, n, mins);
-    bucket_kernel<<<(n + 255) / 256, 256, 0, st>>>(pts, n, mins, 1.0 / h, T - 1, keys, idx);
-    cub::DeviceRadixSort::SortPairs((void*)w, cub_bytes, keys, keys2, idx, idx2, n, 0, bits, st);
-    bucket_bounds_kernel<<<(n + 255) / 256, 256, 0, st>>>(keys2, n, T - 1, bstart, bend);
+    bbox_min_kernel<<<(N + 255) / 256, 256, 0, st>>>(pts, N, clouds, B);
+    bucket_kernel<<<(N + 255) / 256, 256, 0, st>>>(pts, N, clouds, B, T, keys, idx);
+    cub::DeviceRadixSort::SortPairs((void*)w, cub_bytes, keys, keys2, idx, idx2, N, 0, bits, st);
+    bucket_bounds_kernel<<<(N + 255) / 256, 256, 0, st>>>(keys2, N, T, bstart, bend);
     nl += 4;
-    // the Grid travels by value, so the origin has to be known on the host: one 12-byte read-back
-    int hm[4];
-    cudaMemcpyAsync(hm, mins, 16, cudaMemcpyDeviceToHost, st);
-    cudaStreamSynchronize(st);
-    auto dec = [](int i) {
-      const int b = i >= 0 ? i : i ^ 0x7fffffff;
-      float f;
-      memcpy(&f, &b, 4);
-      return (double)f;
-    };
-    g.sorted = idx2;
-    g.bstart = bstart;
-    g.bend = bend;
-    g.n_sorted = hm[3] ? 0 : n;  // 0 = brute force
-    g.mask = T - 1;
-    g.ox = dec(hm[0]);
-    g.oy = dec(hm[1]);
-    g.oz = dec(hm[2]);
-    g.inv_h = 1.0 / h;
+    cs.sorted = idx2;
+    cs.bstart = bstart;
+    cs.bend = bend;
   }
-  normals_kernel<<<n, kFpfhThreads, 0, st>>>(pts, n, r2n, normals, overflow, g);
-  spfh_kernel<<<n, kFpfhThreads, 0, st>>>(pts, normals, n, r2f, spfh, overflow, g);
-  fpfh_kernel<<<n, kFpfhThreads, 0, st>>>(pts, spfh, n, r2f, out, overflow, g);
+  normals_kernel<<<N, kFpfhThreads, 0, st>>>(cs, r2n, normals, overflow);
+  spfh_kernel<<<N, kFpfhThreads, 0, st>>>(cs, normals, r2f, spfh, overflow);
+  fpfh_kernel<<<N, kFpfhThreads, 0, st>>>(cs, spfh, r2f, out, overflow);
   return nl + 3;
 }
 

@@ -7,6 +7,7 @@
 #include <stdio.h>
 
 #include <string>
+#include <vector>
 
 #include "../../include/teaser_b200.h"
 
@@ -200,10 +201,28 @@ void launch_gnc_only(int alg, const double* src, const double* dst, int m, doubl
 void launch_translation_only(const double* src, const double* dst, int m, double beta, double* key, int32_t* idx,
                              double* raw, double* out_t, uint8_t* mask, cudaStream_t st);
 
-// fpfh.cu (FPFHEstimation::computeFPFHFeatures, fpfh.cc:15-43)
-size_t fpfh_grid_scratch_bytes(int n);
-int launch_fpfh(const float* pts, int n, double normal_radius, double fpfh_radius, float4* normals, float* spfh,
-                float* out, int* overflow, void* grid_scratch, cudaStream_t st);
+// fpfh.cu (FPFHEstimation::computeFPFHFeatures, fpfh.cc:15-43), over B clouds stored back to back
+struct FpfhCloud {     // one per cloud, filled by fpfh_plan, read by the kernels from device memory
+  int lo, n;           // first point of the cloud in the flat array, point count
+  int grid;            // 1: radius search through the hashed grid (n >= kGridMinN), 0: brute force
+  unsigned int mask;   // T_b - 1 (T_b buckets, a power of two)
+  unsigned int base;   // first bucket of the cloud in the batch's bucket range
+  int mins[4];         // bounding-box minimum (ordered-int floats; the grid origin); [3] = 1: the grid cannot index
+  double inv_h;        // 1 / cell edge
+};
+struct FpfhPlan {
+  int B = 0, N = 0;            // clouds, points in all of them
+  bool any_grid = false;
+  unsigned int buckets = 0;    // sum of T_b over the grid clouds (also the sentinel key of unsorted points)
+  size_t grid_bytes = 0;       // device scratch of the grid path (0 without grid clouds)
+};
+// Fills clouds[0..B) (host copy, to be staged to the device before launch_fpfh) and the plan.  TZR_ERR_TOO_LARGE when
+// the points or buckets of the batch do not fit 32-bit indices.
+int fpfh_plan(int B, const int32_t* n, double normal_radius, double fpfh_radius, FpfhCloud* clouds, FpfhPlan* plan);
+// pts (plan.N x 3), clouds (device copy of fpfh_plan's table), normals (N float4), spfh (N x 33), out (N x 33),
+// overflow (B ints, zeroed here), grid_scratch (plan.grid_bytes): device pointers.  Returns the launches.
+int launch_fpfh(const FpfhPlan& plan, const float* pts, FpfhCloud* clouds, double normal_radius, double fpfh_radius,
+                float4* normals, float* spfh, float* out, int* overflow, void* grid_scratch, cudaStream_t st);
 
 // certify.cu (DRSCertifier::certify, certification.cc:40-190); mode 0 certify, 1 initial matrix, 2 dual projection
 int certify_device(int mode, double noise_bound, double cbar2, double sub_optimality, double max_iterations,
@@ -213,13 +232,42 @@ int certify_device(int mode, double noise_bound, double cbar2, double sub_optima
                    size_t* scratch_cap, void** solver_handle, int64_t* launches, cudaStream_t st, std::string* err);
 void certify_release(void* solver_handle);
 
-// matcher.cu (Matcher::calculateCorrespondences, matcher.cc:21-337)
-int launch_feature_nn(const float* query, int nq, const float* db, int ndb, int dim, unsigned long long* best,
-                      int num_sms, cudaStream_t st);
-size_t match_scratch_bytes(int ns, int nd);
-int launch_match(float* src_pts, int ns, float* dst_pts, int nd, const float* src_feat, const float* dst_feat, int dim,
-                 int use_absolute_scale, int use_crosscheck, int use_tuple_test, float tuple_scale, uint64_t seed,
-                 void* scratch, int32_t* pairs, int* count, float* gscale, int num_sms, cudaStream_t st);
+// matcher.cu (Matcher::calculateCorrespondences, matcher.cc:21-337), over B cloud pairs stored back to back
+struct MatchPair {      // one per pair, device-resident
+  int s_off, ns;        // first row and rows of the source cloud in the flat source arrays
+  int d_off, nd;        // same for the target cloud; the pair's slots (ns + nd of them) start at s_off + d_off
+  uint64_t seed;        // tuple-test seed
+};
+struct NnWork {         // one CTA of the nearest-neighbour kernel: a query tile against one database segment
+  int dir;              // 0: query rows of feat_a, database rows of feat_b, result in best_a; 1: the reverse
+  int q0, q_end;        // query rows [q0, min(q0 + 64, q_end))
+  int db_lo;            // first row of the query's database cloud (reported indices are relative to it)
+  int seg_lo, seg_hi;   // database rows of this segment
+};
+struct MatchPlan {
+  int B = 0, NS = 0, ND = 0;   // pairs, source rows, target rows (slots: NS + ND)
+  int bits_a = 0, bits_b = 0, bits = 0;  // sort key: pair << (bits_a + bits_b) | source << bits_b | target
+  size_t cub_bytes = 0;
+};
+// Appends the NN work items of query rows [q_lo, q_lo + nq) against database rows [db_lo, db_lo + ndb); tiles_per_seg
+// database tiles of 64 rows per item.
+void nn_work_append(std::vector<NnWork>* work, int dir, int q_lo, int nq, int db_lo, int ndb, int tiles_per_seg);
+// database tiles per NN work item that spread `tile_pairs` (query tile x database tile products) over the GPU
+int nn_tiles_per_seg(long long tile_pairs, int num_sms);
+int launch_feature_nn(const NnWork* work, int n_work, const float* feat_a, const float* feat_b, int dim,
+                      unsigned long long* best_a, unsigned long long* best_b, long long n_best, cudaStream_t st);
+// Host tables of a batch: pairs (B entries, seeds[b]), NN work list of both directions; TZR_ERR_TOO_LARGE when the
+// sort key does not fit 64 bits.
+int match_plan(int B, const int32_t* ns, const int32_t* nd, const uint64_t* seeds, int num_sms,
+               std::vector<MatchPair>* pairs, std::vector<NnWork>* work, MatchPlan* plan);
+size_t match_scratch_bytes(const MatchPlan& plan);
+// All inputs device-resident (pairs/work: device copies of match_plan's tables); pts are normalised IN PLACE (pass
+// copies).  out_pairs: (NS + ND) x 2 int32, pair b's rows from slot s_off + d_off; counts, gscale: B each.
+// Returns the number of kernel launches.
+int launch_match(const MatchPlan& plan, const MatchPair* pairs, const NnWork* work, int n_work, float* src_pts,
+                 float* dst_pts, const float* src_feat, const float* dst_feat, int dim, int use_absolute_scale,
+                 int use_crosscheck, int use_tuple_test, float tuple_scale, void* scratch, int32_t* out_pairs,
+                 int* counts, float* gscale, int num_sms, cudaStream_t st);
 
 
 }  // namespace tzr

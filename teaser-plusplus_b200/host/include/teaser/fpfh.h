@@ -66,6 +66,14 @@ class FPFHEstimation {
   FPFHCloudPtr computeFPFHFeatures(const PointCloud& input_cloud, double normal_search_radius = 0.03,
                                    double fpfh_search_radius = 0.05);
 
+  /**
+   * computeFPFHFeatures on every cloud of the list in one device call; descriptors[b] is what computeFPFHFeatures
+   * returns for clouds[b], and getNormals() afterwards holds the last cloud's normals, as after consecutive calls.
+   */
+  std::vector<FPFHCloudPtr> computeFPFHFeaturesBatch(const std::vector<PointCloud>& clouds,
+                                                     double normal_search_radius = 0.03,
+                                                     double fpfh_search_radius = 0.05);
+
   /// The normal vectors of the input cloud that were used in the calculation of FPFH (fpfh.h:55).
   NormalCloud getNormals() { return normals_; }
 

@@ -34,6 +34,17 @@ class Matcher {
                                                             bool use_crosscheck = true, bool use_tuple_test = true,
                                                             float tuple_scale = 0);
 
+  /**
+   * calculateCorrespondences on B cloud pairs (source_points[b], target_points[b] and their descriptors) in one
+   * device call.  Pair b uses the tuple seed the b-th of B consecutive single calls would use, so the result, the
+   * seed afterwards and getGlobalScale() (the last non-empty pair's) are those of the B consecutive calls.
+   */
+  std::vector<std::vector<std::pair<int, int>>> calculateCorrespondencesBatch(
+      const std::vector<teaser::PointCloud>& source_points, const std::vector<teaser::PointCloud>& target_points,
+      const std::vector<teaser::FPFHCloudPtr>& source_features,
+      const std::vector<teaser::FPFHCloudPtr>& target_features, bool use_absolute_scale = true,
+      bool use_crosscheck = true, bool use_tuple_test = true, float tuple_scale = 0);
+
   /// The reference seeds the tuple test with time(NULL) (matcher.cc:225); here the seed is explicit and every call
   /// advances it, so two Matcher objects with the same seed produce the same sequence of results.
   void setTupleSeed(uint64_t seed) { tuple_seed_ = seed; }
