@@ -830,60 +830,25 @@ __device__ __forceinline__ void strip_interval(const Batch& bt, const int b, con
 // in registers; row points are broadcast from a warp-private slice as (-2x, -2y, -2z, N), (-2u, -2v, -2w, M).  The
 // undecided pairs (lo & ~hi, a few per million) keep bit 0 and are queued for tc_patch_kernel; a full queue is evaluated
 // in place.  Row words come from the warp-shuffle bit transpose of the column words.
-template <bool kVerify, bool kFuseDeg>
-__device__ __forceinline__ void strip_gram(const Batch& bt, const int b, const int I, const int J0, const int J1) {
-  const int n = bt.n;
-  __shared__ float4 s_gr[2 * kTile];
-
-  const GraphConsts* gcp = bt.gc + b;
-  const float mhi = gcp->g_mhi, chi = gcp->g_chi, mlo = gcp->g_mlo, clo = gcp->g_clo;
-  const double beta = gcp->beta;
-  const bool scale_mode = bt.scale_mode != 0;
-  const double s_hat = scale_mode ? bt.sol[b].scale : 1.0;
-
-  const float4* sf = bt.sf + (size_t)b * n;
-  const float4* df = bt.df + (size_t)b * n;
-  const double* src = bt.src + (size_t)b * n * 3;
-  const double* dst = bt.dst + (size_t)b * n * 3;
-
-  const int tid = threadIdx.x, w = tid >> 5, lane = tid & 31;
-  const int ibase = I * kTile + 32 * w;
-  const int nrows = min(32, n - ibase);
-  if (nrows <= 0) return;
-  const float4 z4 = make_float4(0.f, 0.f, 0.f, 0.f);
-  {
-    const int i = ibase + lane;
-    const float4 s = (i < n) ? sf[i] : z4, d = (i < n) ? df[i] : z4;
-    s_gr[2 * tid] = make_float4(-2.f * s.x, -2.f * s.y, -2.f * s.z, s.w);
-    s_gr[2 * tid + 1] = make_float4(-2.f * d.x, -2.f * d.y, -2.f * d.z, d.w);
-  }
-  __syncwarp();
-  uint32_t* adj32 = reinterpret_cast<uint32_t*>(bt.adj) + (size_t)b * n * pitch32(n);
-  const int P32 = pitch32(n);
-  const uint32_t rmask = nrows >= 32 ? 0xffffffffu : ((1u << nrows) - 1u);
-  const float4* rows = s_gr + 2 * 32 * w;
-
-  int* degp = bt.deg + (size_t)b * n;
-  int rdeg = 0;
-  for (int J = J0; J < J1; ++J) {
-    const int jb = J * kTile + lane;
-    float4 cs[4], cd[4];
-    bool vj[4];
+//
+// Gram sweep of rows [0, nr) (nr a multiple of 4) against the lane's first NC column points; column groups wholly past n
+// are not swept (their words stay 0).  Rows are visited from the last to the first so that the funnel shift leaves row ii
+// at bit ii.  Row ii-1 is loaded into registers of its own while row ii is evaluated, so neither load waits for the other
+// row's last read; rows[-2], rows[-1] exist (the slice starts 2 float4 into s_gr) and the last prefetch is not used.
+template <int NC>
+__device__ __forceinline__ void gram_sweep(const float4* rows, const int nr, const float4 (&cs)[4], const float4 (&cd)[4],
+                                           const float mhi, const float chi, const float mlo, const float clo,
+                                           uint32_t (&hi)[4], uint32_t (&lo)[4]) {
+  float4 ns = rows[2 * nr - 2], nd = rows[2 * nr - 1];
+  for (int g = nr / 4 - 1; g >= 0; --g) {
 #pragma unroll
-    for (int c = 0; c < 4; ++c) {
-      const int j = jb + 32 * c;
-      vj[c] = j < n;
-      cs[c] = vj[c] ? sf[j] : z4;
-      cd[c] = vj[c] ? df[j] : z4;
-    }
-    // column words of this lane: bit ii = pair (row ibase+ii, column jb + 32c); hi = surely an edge, lo = edge or undecided
-    uint32_t hi[4] = {0u, 0u, 0u, 0u}, lo[4] = {0u, 0u, 0u, 0u};
-    // rows are visited from the last to the first so that the funnel shift leaves row ii at bit ii
-#pragma unroll 4
-    for (int ii = 31; ii >= 0; --ii) {
-      const float4 rs = rows[2 * ii], rd = rows[2 * ii + 1];
+    for (int k = 3; k >= 0; --k) {
+      const int ii = 4 * g + k;
+      const float4 rs = ns, rd = nd;
+      ns = rows[2 * ii - 2];
+      nd = rows[2 * ii - 1];
 #pragma unroll
-      for (int c = 0; c < 4; ++c) {
+      for (int c = 0; c < NC; ++c) {
         float a = __fadd_rn(rs.w, cs[c].w);
         a = __fmaf_rn(cs[c].x, rs.x, a);
         a = __fmaf_rn(cs[c].y, rs.y, a);
@@ -899,90 +864,171 @@ __device__ __forceinline__ void strip_gram(const Batch& bt, const int b, const i
         lo[c] = __funnelshift_l(__float_as_uint(dl), lo[c], 1);
       }
     }
-    // ---- validity (rows < n, columns < n, i != j), undecided pairs, tentative column words
-    uint32_t colw[4];
-    int nflag = 0;
-#pragma unroll
-    for (int c = 0; c < 4; ++c) {
-      uint32_t vm = vj[c] ? rmask : 0u;
-      if (I == J && c == w) vm &= ~(1u << lane);  // column 32c + lane of the diagonal block meets row 32w + lane
-      const uint32_t fm = lo[c] & ~hi[c] & vm;
-      colw[c] = hi[c] & vm;
-      if (kVerify) {  // every DECIDED pair is re-evaluated exactly; disagreements are counted (must stay 0)
-        uint32_t dm = vm & ~fm;
-        int bad = 0;
-        while (dm) {
-          const int ii = __ffs(dm) - 1;
-          dm &= dm - 1;
-          const int i = ibase + ii, j = jb + 32 * c;
-          const bool ex = scale_mode ? edge_exact_scale(src, dst, i, j, beta, s_hat) : edge_exact(src, dst, i, j, beta);
-          bad += (ex != (((colw[c] >> ii) & 1u) != 0u));
-        }
-        if (bad) atomicAdd(bt.mismatches, (unsigned long long)bad);
-      }
-      lo[c] = fm;  // re-used: undecided mask of column c
-      nflag += __popc(fm);
-    }
-    if (__any_sync(0xffffffffu, nflag != 0)) {
-      // ---- rare: queue the undecided pairs for tc_patch_kernel (their tentative bit is 0); queue full: exact here
-      int incl = nflag;
-#pragma unroll
-      for (int o = 1; o < 32; o <<= 1) {
-        const int v = __shfl_up_sync(0xffffffffu, incl, o);
-        if (lane >= o) incl += v;
-      }
-      const int total = __shfl_sync(0xffffffffu, incl, 31);
-      unsigned int base = 0;
-      if (lane == 0) base = atomicAdd(bt.tc_list_count, (unsigned int)total);
-      base = __shfl_sync(0xffffffffu, base, 0);
-      const bool queued = base + (unsigned int)total <= bt.tc_list_cap;
-      unsigned int pos = base + (unsigned int)(incl - nflag);
-      if (!queued)  // the first warp that does not fit leaves [base, cap) unwritten: void entries for the patch kernel
-        for (unsigned int q = base + (unsigned int)lane; q < bt.tc_list_cap; q += 32u) bt.tc_list[q] = make_uint2(0xffffffffu, 0u);
-      int nre = 0;
+  }
+}
+
+// The mirror half of an off-diagonal block (column words, 4 B per column row and warp) is gathered in a CTA-shared slice
+// and leaves as one 16-byte store per column row, with one degree atomic per column row carrying the sum of the four
+// warps' popcounts.  Every warp of the CTA runs every block of the strip and reaches every barrier: a warp without rows
+// (only in the last row block) sweeps nothing and contributes zero words.
+template <bool kVerify, bool kFuseDeg>
+__device__ __forceinline__ void strip_gram(const Batch& bt, const int b, const int I, const int J0, const int J1) {
+  const int n = bt.n;
+  __shared__ float4 s_gr[2 + 2 * kTile];
+  __shared__ __align__(16) uint32_t s_mir[2][kTile][4];  // [block parity][column row][warp]
+
+  const GraphConsts* gcp = bt.gc + b;
+  const float mhi = gcp->g_mhi, chi = gcp->g_chi, mlo = gcp->g_mlo, clo = gcp->g_clo;
+  const double beta = gcp->beta;
+  const bool scale_mode = bt.scale_mode != 0;
+  const double s_hat = scale_mode ? bt.sol[b].scale : 1.0;
+
+  const float4* sf = bt.sf + (size_t)b * n;
+  const float4* df = bt.df + (size_t)b * n;
+  const double* src = bt.src + (size_t)b * n * 3;
+  const double* dst = bt.dst + (size_t)b * n * 3;
+
+  const int tid = threadIdx.x, w = tid >> 5, lane = tid & 31;
+  const int ibase = I * kTile + 32 * w;
+  const int nrows = max(0, min(32, n - ibase));  // 0 only in the last row block, whose one block is diagonal
+  const float4 z4 = make_float4(0.f, 0.f, 0.f, 0.f);
+  {
+    const int i = ibase + lane;
+    const float4 s = (i < n) ? sf[i] : z4, d = (i < n) ? df[i] : z4;
+    s_gr[2 + 2 * tid] = make_float4(-2.f * s.x, -2.f * s.y, -2.f * s.z, s.w);
+    s_gr[2 + 2 * tid + 1] = make_float4(-2.f * d.x, -2.f * d.y, -2.f * d.z, d.w);
+  }
+  __syncwarp();
+  uint32_t* adj32 = reinterpret_cast<uint32_t*>(bt.adj) + (size_t)b * n * pitch32(n);
+  const int P32 = pitch32(n);
+  const uint32_t rmask = nrows >= 32 ? 0xffffffffu : ((1u << nrows) - 1u);
+  const int nr = (nrows + 3) & ~3;  // rows swept: the rows below n, rounded up to the sweep's unroll
+  const float4* rows = s_gr + 2 + 2 * 32 * w;
+
+  int* degp = bt.deg + (size_t)b * n;
+  int rdeg = 0;
+  for (int J = J0; J < J1; ++J) {
+    const int jb = J * kTile + lane;
+    uint32_t colw[4] = {0u, 0u, 0u, 0u};
+    if (nrows > 0) {  // warp-uniform
+      float4 cs[4], cd[4];
+      bool vj[4];
 #pragma unroll
       for (int c = 0; c < 4; ++c) {
-        uint32_t fm = lo[c];
         const int j = jb + 32 * c;
-        while (fm) {
-          const int ii = __ffs(fm) - 1;
-          fm &= fm - 1;
-          const int i = ibase + ii;
-          if (queued) {
-            // the patch kernel flips bit (i, j) and, off the diagonal block, its mirror; the diagonal block holds both
-            // orientations as separate pairs, each queued by the lane that owns its column
-            bt.tc_list[pos++] = make_uint2((unsigned int)b, ((unsigned int)i << 16) | (unsigned int)j);
-          } else {
+        vj[c] = j < n;
+        cs[c] = vj[c] ? sf[j] : z4;
+        cd[c] = vj[c] ? df[j] : z4;
+      }
+      // column words of this lane: bit ii = pair (row ibase+ii, column jb + 32c); hi = surely an edge, lo = edge or
+      // undecided
+      uint32_t hi[4] = {0u, 0u, 0u, 0u}, lo[4] = {0u, 0u, 0u, 0u};
+      const int ncg = min(4, (n - J * kTile + 31) / 32);  // column groups with at least one point below n
+      if (ncg == 4)
+        gram_sweep<4>(rows, nr, cs, cd, mhi, chi, mlo, clo, hi, lo);
+      else if (ncg == 3)
+        gram_sweep<3>(rows, nr, cs, cd, mhi, chi, mlo, clo, hi, lo);
+      else if (ncg == 2)
+        gram_sweep<2>(rows, nr, cs, cd, mhi, chi, mlo, clo, hi, lo);
+      else
+        gram_sweep<1>(rows, nr, cs, cd, mhi, chi, mlo, clo, hi, lo);
+      // ---- validity (rows < n, columns < n, i != j), undecided pairs, tentative column words
+      int nflag = 0;
+#pragma unroll
+      for (int c = 0; c < 4; ++c) {
+        uint32_t vm = vj[c] ? rmask : 0u;
+        if (I == J && c == w) vm &= ~(1u << lane);  // column 32c + lane of the diagonal block meets row 32w + lane
+        const uint32_t fm = lo[c] & ~hi[c] & vm;
+        colw[c] = hi[c] & vm;
+        if (kVerify) {  // every DECIDED pair is re-evaluated exactly; disagreements are counted (must stay 0)
+          uint32_t dm = vm & ~fm;
+          int bad = 0;
+          while (dm) {
+            const int ii = __ffs(dm) - 1;
+            dm &= dm - 1;
+            const int i = ibase + ii, j = jb + 32 * c;
             const bool ex = scale_mode ? edge_exact_scale(src, dst, i, j, beta, s_hat) : edge_exact(src, dst, i, j, beta);
-            colw[c] |= (ex ? 1u : 0u) << ii;
-            ++nre;
+            bad += (ex != (((colw[c] >> ii) & 1u) != 0u));
+          }
+          if (bad) atomicAdd(bt.mismatches, (unsigned long long)bad);
+        }
+        lo[c] = fm;  // re-used: undecided mask of column c
+        nflag += __popc(fm);
+      }
+      if (__any_sync(0xffffffffu, nflag != 0)) {
+        // ---- rare: queue the undecided pairs for tc_patch_kernel (their tentative bit is 0); queue full: exact here
+        int incl = nflag;
+#pragma unroll
+        for (int o = 1; o < 32; o <<= 1) {
+          const int v = __shfl_up_sync(0xffffffffu, incl, o);
+          if (lane >= o) incl += v;
+        }
+        const int total = __shfl_sync(0xffffffffu, incl, 31);
+        unsigned int base = 0;
+        if (lane == 0) base = atomicAdd(bt.tc_list_count, (unsigned int)total);
+        base = __shfl_sync(0xffffffffu, base, 0);
+        const bool queued = base + (unsigned int)total <= bt.tc_list_cap;
+        unsigned int pos = base + (unsigned int)(incl - nflag);
+        if (!queued)  // the first warp that does not fit leaves [base, cap) unwritten: void entries for the patch kernel
+          for (unsigned int q = base + (unsigned int)lane; q < bt.tc_list_cap; q += 32u) bt.tc_list[q] = make_uint2(0xffffffffu, 0u);
+        int nre = 0;
+#pragma unroll
+        for (int c = 0; c < 4; ++c) {
+          uint32_t fm = lo[c];
+          const int j = jb + 32 * c;
+          while (fm) {
+            const int ii = __ffs(fm) - 1;
+            fm &= fm - 1;
+            const int i = ibase + ii;
+            if (queued) {
+              // the patch kernel flips bit (i, j) and, off the diagonal block, its mirror; the diagonal block holds both
+              // orientations as separate pairs, each queued by the lane that owns its column
+              bt.tc_list[pos++] = make_uint2((unsigned int)b, ((unsigned int)i << 16) | (unsigned int)j);
+            } else {
+              const bool ex = scale_mode ? edge_exact_scale(src, dst, i, j, beta, s_hat) : edge_exact(src, dst, i, j, beta);
+              colw[c] |= (ex ? 1u : 0u) << ii;
+              ++nre;
+            }
           }
         }
-      }
-      if (bt.rechecks && !queued) {
-        nre = __reduce_add_sync(0xffffffffu, nre);
-        if (lane == 0 && nre) atomicAdd(bt.rechecks, (unsigned long long)nre);
-      }
-    }
-    // ---- row words (lane = row ibase + lane) by transposition; stores; fused degrees
-    uint32_t roww[4];
-#pragma unroll
-    for (int c = 0; c < 4; ++c) roww[c] = warp_transpose32(colw[c], lane);
-    if (lane < nrows)
-      *reinterpret_cast<uint4*>(adj32 + (size_t)(ibase + lane) * P32 + 4 * J) =
-          make_uint4(roww[0], roww[1], roww[2], roww[3]);
-    if (kFuseDeg) rdeg += __popc(roww[0]) + __popc(roww[1]) + __popc(roww[2]) + __popc(roww[3]);
-    if (I != J) {
-#pragma unroll
-      for (int c = 0; c < 4; ++c)
-        if (vj[c]) {
-          adj32[(size_t)(jb + 32 * c) * P32 + 4 * I + w] = colw[c];
-          if (kFuseDeg && colw[c]) atomicAdd(degp + jb + 32 * c, __popc(colw[c]));
+        if (bt.rechecks && !queued) {
+          nre = __reduce_add_sync(0xffffffffu, nre);
+          if (lane == 0 && nre) atomicAdd(bt.rechecks, (unsigned long long)nre);
         }
+      }
+      // ---- row words (lane = row ibase + lane) by transposition; stores; fused degrees
+      uint32_t roww[4];
+#pragma unroll
+      for (int c = 0; c < 4; ++c) roww[c] = warp_transpose32(colw[c], lane);
+      if (lane < nrows)
+        *reinterpret_cast<uint4*>(adj32 + (size_t)(ibase + lane) * P32 + 4 * J) =
+            make_uint4(roww[0], roww[1], roww[2], roww[3]);
+      if (kFuseDeg) rdeg += __popc(roww[0]) + __popc(roww[1]) + __popc(roww[2]) + __popc(roww[3]);
+    }
+    // ---- mirror half (CTA-uniform: the diagonal block holds both orientations in its row words)
+    if (I != J) {
+      uint32_t(*mir)[4] = s_mir[J & 1];  // two slices: the barrier of block J+1 orders the reads of J before J+2's writes
+#pragma unroll
+      for (int c = 0; c < 4; ++c) mir[32 * c + lane][w] = colw[c];
+      __syncthreads();
+      const int j = J * kTile + tid;
+      if (j < n) {
+        const uint4 v = *reinterpret_cast<const uint4*>(&mir[tid][0]);
+        *reinterpret_cast<uint4*>(adj32 + (size_t)j * P32 + 4 * I) = v;
+        const int d = __popc(v.x) + __popc(v.y) + __popc(v.z) + __popc(v.w);
+        if (kFuseDeg && d) atomicAdd(degp + j, d);
+      }
     }
   }
   if (kFuseDeg && lane < nrows && rdeg) atomicAdd(degp + ibase + lane, rdeg);
 }
+
+// CTAs per SM the default strip kernel (and its separate-degree instance, flag 256) is compiled for: 6 (80 registers)
+// gives the Gram sweep room to keep the next row's loads and four columns' chains in flight (DESIGN.md §3.1; A/B builds:
+// make EXTRA=-DTZR_STRIP_MIN_BLOCKS=5 or 8)
+#ifndef TZR_STRIP_MIN_BLOCKS
+#define TZR_STRIP_MIN_BLOCKS 6
+#endif
 
 // graph strip kernel (default): one launch for the whole batch; each problem runs the Gram test or the interval test, as
 // prep_kernel chose (CTA-uniform: a strip belongs to one problem).  Undecided pairs of the Gram test are settled by
@@ -1294,9 +1340,9 @@ int launch_graph(const Batch& bt0, cudaStream_t st, int num_sms) {
   else if (bt.flags_dbg & 2u)
     graph_strip2_kernel<true, 5, false><<<sgrid, kGraphThreads, 0, st>>>(bt);
   else if (bt.flags_dbg & 256u)  // degrees by the separate degree kernel (A/B against the fused default)
-    graph_strip2_kernel<false, 8, false><<<sgrid, kGraphThreads, 0, st>>>(bt);
-  else  // default: Gram test (interval test where prep_kernel's guard fails), 8 CTAs/SM, degrees fused
-    graph_strip2_kernel<false, 8, true><<<sgrid, kGraphThreads, 0, st>>>(bt);
+    graph_strip2_kernel<false, TZR_STRIP_MIN_BLOCKS, false><<<sgrid, kGraphThreads, 0, st>>>(bt);
+  else  // default: Gram test (interval test where prep_kernel's guard fails), degrees fused
+    graph_strip2_kernel<false, TZR_STRIP_MIN_BLOCKS, true><<<sgrid, kGraphThreads, 0, st>>>(bt);
   // exact re-check of the pairs the strip kernel queued (v7, or the Gram test: every problem unless debug flag 512)
   if (v7 || !(bt.flags_dbg & 512u)) {
     launch_graph_patch(bt, st, num_sms);
