@@ -138,6 +138,25 @@ int tzr_max_clique_batch(tzr_ctx* ctx, int B, int n, const uint64_t* adj_bits, i
  * problem, the largest clique of the root-based greedy heuristic, before the peel kernel's second chance. */
 int tzr_ctx_clique_info(tzr_ctx* ctx, int32_t* geometry3, int32_t* heuristic_best);
 
+/* Per-problem size limit of this context: 32768 <= max_n <= 65536 (TZR_ERR_INVALID_ARG otherwise); the default is
+ * 32768.  It applies to tzr_graph_build, tzr_max_clique(_batch), tzr_solve, tzr_solve_batch, tzr_solve_batch_dev and
+ * tzr_last_graph; a larger problem is TZR_ERR_TOO_LARGE.  65536 is a hard bound: the graph kernels and the clique
+ * heuristic keep vertex indices in 16 bits.  tzr_solve_batch_multi keeps 32768 (its contexts are library-internal).
+ * Problems of more than 32768 vertices take the large clique route (DESIGN.md 3.2): the heuristic clique (size L) on
+ * the full graph, the (L-1)-core of the graph on the device, and the small route's exact search on that core compacted
+ * to at most 32768 vertices (the relabelling keeps the index order, so the canonical tie-break is unchanged).  A graph
+ * whose core keeps more than 32768 vertices (a dense graph, e.g. most vertices in one large inlier set) is not
+ * searched: it returns its heuristic clique, a valid clique with clique_proven_optimal = 0.  estimate_scaling = 1 needs
+ * the unknown-scale stage's scratch (tens of GB at these sizes) and is TZR_ERR_TOO_LARGE from n = 46341 (2K end points
+ * exceed 2^31).  A buffer that does not fit the device is TZR_ERR_ALLOC (tzr_last_error names the size). */
+int tzr_ctx_set_max_n(tzr_ctx* ctx, int max_n);
+/* Clique route of each problem of the most recent clique stage on this context (a solve or a max-clique call; B
+ * entries; TZR_ERR_INVALID_ARG once another call has reused the workspace): 0 = small route; k > 0 = large route with
+ * the core compacted to k vertices, where k equal to the clique size means the core was the clique itself (or a
+ * heuristic mode, or a clique of size <= 1) and no search ran; -1 = large route whose core kept more vertices than the
+ * cap, the heuristic clique is returned with clique_proven_optimal = 0 (search flags 1 | 16). */
+int tzr_ctx_clique_route(tzr_ctx* ctx, int32_t* per_problem);
+
 /* ---- stage 3: GNC-TLS rotation --------------------------------------------------------------
  * Replaces GNCTLSRotationSolver::solveForRotation (registration.cc:764-866) + utils::svdRot
  * (teaser/include/teaser/utils.h:121-136).  inlier_mask (m bytes) and the scalar outputs may be NULL. */
@@ -324,8 +343,10 @@ int tzr_solve_batch_multi(const int32_t* devices, int n_devices, const tzr_param
  * reachable at test sizes, bit 17 (131072) = one exact pass with the caller's whole budget instead of 50 ms + LP bound
  * + second pass, so that whether a canonical enumeration finishes does not depend on the wall clock (bit 15 wins when
  * both are set), bit 18 (262144) = the unknown-scale stage and tzr_scalar_tls through the large path (radix sort +
- * tiled scans) at every size instead of the bitonic sort + sequential sweep below 257 points.  Bits 15 to 18 change
- * host code only. */
+ * tiled scans) at every size instead of the bitonic sort + sequential sweep below 257 points, bit 19 (524288) = the
+ * large clique route at every n (tzr_ctx_clique_route), so that the two routes can be compared on the same graphs,
+ * bit 20 (1048576) = cap the large route's compacted core at 64 vertices instead of 32768, so that its "core too large"
+ * outcome is reachable at test sizes.  Bits 15 to 20 change host code only. */
 int tzr_ctx_set_flags(tzr_ctx* ctx, uint32_t flags);
 int64_t tzr_ctx_filter_mismatches(tzr_ctx* ctx);
 /* Number of pairs of the most recent graph build that needed the exact FP64 re-check. */

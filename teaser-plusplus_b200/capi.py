@@ -96,7 +96,7 @@ _SYMBOLS = [
     "tzr_match_correspondences", "tzr_feature_nn", "tzr_compute_fpfh", "tzr_certifier_params_default", "tzr_certify",
     "tzr_certifier_initial_matrix", "tzr_certifier_dual_projection", "tzr_last_graph_info", "tzr_ctx_stage_log",
     "tzr_ctx_stage_log_read", "tzr_solve_batch_multi", "tzr_ctx_clique_info", "tzr_compute_fpfh_batch",
-    "tzr_match_correspondences_batch",
+    "tzr_match_correspondences_batch", "tzr_ctx_set_max_n", "tzr_ctx_clique_route",
 ]
 
 
@@ -159,6 +159,8 @@ def lib():
     L.tzr_ctx_filter_rechecks.restype = C.c_int64
     L.tzr_ctx_debug_counters.argtypes = [vp, i64p]
     L.tzr_ctx_clique_info.argtypes = [vp, i32p, i32p]
+    L.tzr_ctx_set_max_n.argtypes = [vp, C.c_int]
+    L.tzr_ctx_clique_route.argtypes = [vp, i32p]
     fp = C.POINTER(C.c_float)
     L.tzr_match_correspondences.argtypes = [vp, fp, C.c_int, fp, C.c_int, fp, fp, C.c_int, C.c_int, C.c_int, C.c_int,
                                             C.c_float, C.c_uint64, i32p, C.c_int64, i64p, fp]
@@ -202,13 +204,20 @@ def _p(a, t):
 
 
 class Context:
-    """One CUDA device + stream + workspace (tzr_ctx)."""
+    """One CUDA device + stream + workspace (tzr_ctx).  max_n: per-problem size limit, 32768 (default) ... 65536
+    (tzr_ctx_set_max_n)."""
 
-    def __init__(self, device: int = -1):
+    def __init__(self, device: int = -1, max_n: int = 32768):
         self._h = C.c_void_p()
         rc = lib().tzr_ctx_create(device, C.byref(self._h))
         if rc != 0:
             raise TzrError(f"tzr_ctx_create failed: {lib().tzr_status_string(rc).decode()}")
+        if max_n != 32768:
+            try:
+                self.set_max_n(max_n)
+            except TzrError:
+                self.close()
+                raise
 
     def close(self):
         if self._h:
@@ -255,6 +264,18 @@ class Context:
         heur = np.zeros(B, dtype=np.int32)
         self._ck(lib().tzr_ctx_clique_info(self._h, _p(geom, C.c_int32), _p(heur, C.c_int32)))
         return dict(exact_ctas=int(geom[0]), exact_conc=int(geom[1]), max_depth=int(geom[2]), heuristic_best=heur)
+
+    def set_max_n(self, max_n: int):
+        """Per-problem size limit: 32768 <= max_n <= 65536; above 32768 the clique stage takes the large route."""
+        self._ck(lib().tzr_ctx_set_max_n(self._h, int(max_n)))
+
+    def clique_route(self, B: int):
+        """(B,) int32 clique route of each problem of the most recent clique stage: 0 small route, k > 0 large route
+        with the core compacted to k vertices (k = clique size: no search ran), -1 core above the cap (heuristic
+        clique, not proven)."""
+        out = np.zeros(B, dtype=np.int32)
+        self._ck(lib().tzr_ctx_clique_route(self._h, _p(out, C.c_int32)))
+        return out
 
     def kernel_launches(self) -> int:
         return int(lib().tzr_ctx_kernel_launches(self._h))

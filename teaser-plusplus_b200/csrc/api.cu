@@ -31,6 +31,9 @@ struct tzr_ctx {
   // device buffers (grow-only)
   DevBuf src, dst, sf, df, pk, opnd, tclist, gc, adj, deg, nedges, hclq, hsize, clq, L, alive, best_bits, alive_cnt, root_ctr, lock, flg, kfinal, tstart, stack, cv,
       centry, ps, pd, wgt, res, skey, sidx, sorted, rmask, tmask, sol, dbg, misc, sc, m_in, m_scratch, m_out, cert;
+  // large clique route (n > kMaxN or debug flag 524288): scratch on the full graph, and the compacted batch's buffers
+  DevBuf lg, cq;
+  int max_n = kMaxN;  // per-problem size limit of this context (tzr_ctx_set_max_n: kMaxN ... kMaxNLarge)
   // pinned host staging
   void* h_pin = nullptr;
   size_t h_pin_cap = 0;
@@ -58,6 +61,9 @@ struct tzr_ctx {
   // geometry of the most recent tzr_max_clique(_batch) call (tzr_ctx_clique_info); clique_B = 0 once the workspace is reused
   int clique_B = 0;
   int clique_geom[3] = {0, 0, 0};  // exact_ctas, exact_conc, max_depth
+  // clique route of every problem of the most recent clique stage (tzr_ctx_clique_route); route_B = 0 once reused
+  std::vector<int32_t> route;
+  int route_B = 0;
 };
 
 namespace {
@@ -81,7 +87,8 @@ int ensure(tzr_ctx* ctx, DevBuf& b, size_t bytes) {
   size_t want = bytes + bytes / 8 + 256;
   cudaError_t e = cudaMalloc(&b.p, want);
   if (e != cudaSuccess) {
-    ctx->last_error = std::string("cudaMalloc: ") + cudaGetErrorString(e);
+    cudaGetLastError();  // not sticky: keep it from surfacing as a launch error of a later call
+    ctx->last_error = std::string("cudaMalloc of ") + std::to_string(want) + " bytes: " + cudaGetErrorString(e);
     return TZR_ERR_ALLOC;
   }
   b.cap = want;
@@ -194,15 +201,47 @@ int effective_mode(const tzr_params& p) {
   return mode;
 }
 
+// Exact-phase geometry of a (B, n) batch: a persistent grid that fills the GPU, whose warps own the search scratch (any
+// problem): *ctas, *depth (stack levels per warp), *conc (problems searched at a time).
+void search_geometry(const tzr_ctx* ctx, int B, int n, int* ctas, int* depth_out, int* conc) {
+  int G = clique_exact_grid(n, ctx->num_sms);
+  {
+    const long long roots = ((long long)B * n + 7) / 8;  // never more warps than root vertices
+    if ((long long)G > roots) G = (int)std::max<long long>(1, roots);
+  }
+  const size_t warps = (size_t)G * 8;
+  const size_t level_bytes = (size_t)2 * pitch32(n) * sizeof(uint32_t);
+  size_t depth = ((size_t)4 << 30) / (warps * level_bytes);
+  if (depth > 512) depth = 512;
+  if (depth > (size_t)n) depth = (size_t)n;
+  if (depth < 16) depth = 16;
+  *ctas = G;
+  *depth_out = (int)depth;
+  // debug flag 65536: a search stack of 8 levels, so that the depth cap (result not proven) is reachable at test sizes
+  if (ctx->flags & 65536u) *depth_out = 8;
+  {
+    // problems under search at a time: their bitsets should stay in the L2 together (~18 MB of the 50 MB: the
+    // stacks, the other lane's graph kernel and the two L2 partitions take the rest)
+    const size_t bits = (size_t)n * pitch32(n) * sizeof(uint32_t);
+    const size_t c = ((size_t)18 << 20) / std::max<size_t>(bits, 1);
+    *conc = (int)std::min<size_t>(std::max<size_t>(c, 1), (size_t)B);
+  }
+}
+
 // Size the workspace for a (B, n) batch and fill the Batch descriptor (src/dst left to the caller).
 int setup_batch(tzr_ctx* ctx, int B, int n, bool own_points, Batch* out, bool complete_graph = false) {
   if (B <= 0 || n <= 0) return TZR_ERR_INVALID_ARG;
-  if (n > kMaxN) return TZR_ERR_TOO_LARGE;
+  if (n > ctx->max_n) {
+    ctx->last_error = "n = " + std::to_string(n) + " exceeds this context's limit of " + std::to_string(ctx->max_n) +
+                      " correspondences (tzr_ctx_set_max_n raises it to " + std::to_string(kMaxNLarge) + ")";
+    return TZR_ERR_TOO_LARGE;
+  }
   // the workspace is about to be re-used (and possibly re-allocated): the retained graph of the previous call is gone
   ctx->have_last = false;
   ctx->last_has_graph = false;
   ++ctx->generation;
   ctx->clique_B = 0;
+  ctx->route_B = 0;
   Batch bt{};
   bt.B = B;
   bt.n = n;
@@ -240,32 +279,15 @@ int setup_batch(tzr_ctx* ctx, int B, int n, bool own_points, Batch* out, bool co
   ENS(flg, (size_t)B * sizeof(int32_t));
   ENS(kfinal, (size_t)B * sizeof(int32_t));
   ENS(tstart, (size_t)B * sizeof(unsigned long long));
-  // exact phase geometry: a persistent grid that fills the GPU; its warps own the search scratch (any problem)
-  int G = clique_exact_grid(n, ctx->num_sms);
-  {
-    const long long roots = ((long long)B * n + 7) / 8;  // never more warps than root vertices
-    if ((long long)G > roots) G = (int)std::max<long long>(1, roots);
+  // exact phase: above kMaxN the search runs on the large route's compacted batch, which has its own scratch
+  if (n <= kMaxN) {
+    search_geometry(ctx, B, n, &bt.exact_ctas, &bt.max_depth, &bt.exact_conc);
+    const size_t warps = (size_t)bt.exact_ctas * 8;
+    const size_t level_bytes = (size_t)2 * W32 * sizeof(uint32_t);
+    ENS(stack, warps * bt.max_depth * level_bytes);
+    ENS(cv, std::max(warps, (size_t)4 * B) * (size_t)n * sizeof(int32_t));
+    ENS(centry, warps * bt.max_depth * sizeof(int32_t));
   }
-  const size_t warps = (size_t)G * 8;
-  const size_t level_bytes = (size_t)2 * W32 * sizeof(uint32_t);
-  size_t depth = ((size_t)4 << 30) / (warps * level_bytes);
-  if (depth > 512) depth = 512;
-  if (depth > (size_t)n) depth = (size_t)n;
-  if (depth < 16) depth = 16;
-  bt.exact_ctas = G;
-  bt.max_depth = (int)depth;
-  // debug flag 65536: a search stack of 8 levels, so that the depth cap (result not proven) is reachable at test sizes
-  if (ctx->flags & 65536u) bt.max_depth = 8;
-  {
-    // problems under search at a time: their bitsets should stay in the L2 together (~18 MB of the 50 MB: the
-    // stacks, the other lane's graph kernel and the two L2 partitions take the rest)
-    const size_t bits = n * W32 * sizeof(uint32_t);
-    const size_t conc = ((size_t)18 << 20) / std::max<size_t>(bits, 1);
-    bt.exact_conc = (int)std::min<size_t>(std::max<size_t>(conc, 1), (size_t)B);
-  }
-  ENS(stack, warps * depth * level_bytes);
-  ENS(cv, std::max(warps, (size_t)4 * B) * (size_t)n * sizeof(int32_t));
-  ENS(centry, warps * depth * sizeof(int32_t));
   bt.sort_cap = next_pow2(2 * n);
   ENS(ps, Bn * 3 * sizeof(double));
   ENS(pd, Bn * 3 * sizeof(double));
@@ -433,10 +455,116 @@ int l2_chunk(const tzr_ctx* ctx, int B, int n, const tzr_params& p) {
   return (int)c;
 }
 
+size_t al256(size_t x) { return (x + 255) & ~(size_t)255; }
+
+// Large clique route (DESIGN.md §3.2), taken when n > kMaxN or under debug flag 524288: the heuristic on the full graph,
+// its (L-1)-core on many CTAs, the cores compacted (order-preserving) into a batch of at most kMaxN vertices per problem
+// (64 under debug flag 1048576), the small route's peel and exact passes on that batch, the cliques mapped back.  One
+// host read-back: the core sizes, which size the compacted batch.  route: B entries as tzr_ctx_clique_route reports them.
+int run_clique_large(tzr_ctx* ctx, const Batch& bt, const tzr_params& p, int mode, cudaStream_t st, int* nl,
+                     int32_t* route) {
+  const int B = bt.B, n = bt.n;
+  const size_t Bn = (size_t)B * n;
+  size_t off = 0;
+  auto carve = [&off](size_t bytes) {
+    const size_t o = off;
+    off = al256(off + bytes);
+    return o;
+  };
+  const size_t o_lists = carve(Bn * kHeurRoots * 2 * sizeof(uint16_t)), o_chg = carve((size_t)B * kCoreRounds * 4),
+               o_n2o = carve(Bn * 4), o_o2n = carve(Bn * 4), o_cnt = carve((size_t)B * 4), o_route = carve((size_t)B * 4);
+  int rc = ensure(ctx, ctx->lg, off);
+  if (rc) return rc;
+  char* lg = (char*)ctx->lg.p;
+  int32_t* n2o = (int32_t*)(lg + o_n2o);
+  int32_t* o2n = (int32_t*)(lg + o_o2n);
+  int32_t* cnt_d = (int32_t*)(lg + o_cnt);
+  int32_t* route_d = (int32_t*)(lg + o_route);
+  launch_clique_large_front(bt, p, mode, (uint16_t*)(lg + o_lists), st, nl);
+  std::vector<int32_t> L(B), cnt(B, 0);
+  if (mode == 0) launch_core(bt, (int32_t*)(lg + o_chg), n2o, o2n, cnt_d, ctx->num_sms, st, nl);
+  CK(cudaMemcpyAsync(L.data(), bt.L, (size_t)B * 4, cudaMemcpyDeviceToHost, st));
+  if (mode == 0) CK(cudaMemcpyAsync(cnt.data(), cnt_d, (size_t)B * 4, cudaMemcpyDeviceToHost, st));
+  CK(cudaStreamSynchronize(st));
+  // heuristic modes, L <= 1 and the uniqueness shortcut (only the incumbent survives its own core bound): the result is
+  // final, reported as the clique size (at least 1)
+  const int cap = (ctx->flags & 1048576u) ? 64 : kMaxN;
+  std::vector<int32_t> search(B, 0);
+  int n2 = 0;
+  for (int b = 0; b < B; ++b) {
+    if (mode != 0 || L[b] <= 1 || cnt[b] == L[b]) {
+      route[b] = std::max(L[b], 1);
+    } else if (cnt[b] > cap) {
+      route[b] = -1;
+      search[b] = -1;
+    } else {
+      route[b] = cnt[b];
+      search[b] = 1;
+      n2 = std::max(n2, cnt[b]);
+    }
+  }
+  if (mode != 0) return TZR_OK;
+  CK(cudaMemcpyAsync(route_d, search.data(), (size_t)B * 4, cudaMemcpyHostToDevice, st));
+  Batch cb = bt;
+  if (n2 > 0) {
+    // the compacted batch: B problems of n2 vertices, its own clique state and exact-phase scratch
+    const size_t Bn2 = (size_t)B * n2;
+    const int W2 = pitch32(n2);
+    search_geometry(ctx, B, n2, &cb.exact_ctas, &cb.max_depth, &cb.exact_conc);
+    const size_t warps = (size_t)cb.exact_ctas * 8;
+    off = 0;
+    const size_t c_adj = carve(Bn2 * pitch64(n2) * 8), c_deg = carve(Bn2 * 4), c_ne = carve((size_t)B * 8),
+                 c_hclq = carve(Bn2 * kHeurRoots * 4), c_hsize = carve((size_t)B * kHeurRoots * 4), c_clq = carve(Bn2 * 4),
+                 c_L = carve((size_t)B * 4), c_alive = carve((size_t)B * W2 * 4), c_bb = carve((size_t)B * W2 * 4),
+                 c_acnt = carve((size_t)B * 4), c_rctr = carve((size_t)B * 4), c_lock = carve((size_t)B * 4),
+                 c_flg = carve((size_t)B * 4), c_ts = carve((size_t)B * 8),
+                 c_stack = carve(warps * cb.max_depth * 2 * W2 * 4),
+                 c_cv = carve(std::max(warps, (size_t)4 * B) * n2 * 4), c_centry = carve(warps * cb.max_depth * 4);
+    rc = ensure(ctx, ctx->cq, off);
+    if (rc) return rc;
+    char* q = (char*)ctx->cq.p;
+    cb.n = n2;
+    cb.adj = (uint64_t*)(q + c_adj);
+    cb.deg = (int32_t*)(q + c_deg);
+    cb.n_edges2 = (unsigned long long*)(q + c_ne);
+    cb.hclq = (int32_t*)(q + c_hclq);
+    cb.hsize = (int32_t*)(q + c_hsize);
+    cb.clq = (int32_t*)(q + c_clq);
+    cb.L = (int32_t*)(q + c_L);
+    cb.alive = (uint32_t*)(q + c_alive);
+    cb.best_bits = (uint32_t*)(q + c_bb);
+    cb.alive_cnt = (int32_t*)(q + c_acnt);
+    cb.root_ctr = (int32_t*)(q + c_rctr);
+    cb.lock = (int32_t*)(q + c_lock);
+    cb.flags = (int32_t*)(q + c_flg);
+    cb.t_start = (unsigned long long*)(q + c_ts);
+    cb.stack = (uint32_t*)(q + c_stack);
+    cb.cv = (int32_t*)(q + c_cv);
+    cb.centry = (int32_t*)(q + c_centry);
+    cb.kcore_final = nullptr;
+    launch_core_compact(bt, cb, n2o, o2n, cnt_d, route_d, st, nl);
+    CK(cudaMemsetAsync(cb.n_edges2, 0, (size_t)B * 8, st));
+    launch_degree(cb, st, true);
+    launch_clique_search(cb, st, nl);
+    *nl += 1;
+  }
+  launch_core_map_back(bt, cb, n2o, route_d, st, nl);
+  return TZR_OK;
+}
+
+// The clique stage of a batch: the small route (launch_clique) or the large one.  route: B entries (tzr_ctx_clique_route).
+int run_clique(tzr_ctx* ctx, const Batch& bt, const tzr_params& p, int mode, cudaStream_t st, int* nl, int32_t* route) {
+  if (bt.n > kMaxN || (ctx->flags & 524288u)) return run_clique_large(ctx, bt, p, mode, st, nl, route);
+  launch_clique(bt, p, mode, st, nl);
+  std::fill(route, route + bt.B, 0);
+  return TZR_OK;
+}
+
 // The fused device pipeline for one uniform batch.  src/dst must already be set in bt.
 // st: stream of the clique / rotation stages; sg: stream of prep + graph (== st for the single-lane form, otherwise
 // gdone is recorded on sg after the graph kernel and st waits for it).
-int run_pipeline(tzr_ctx* ctx, Batch& bt, const tzr_params& p, cudaEvent_t* ev, cudaStream_t st,
+// route: the batch's entries of ctx->route.
+int run_pipeline(tzr_ctx* ctx, Batch& bt, const tzr_params& p, cudaEvent_t* ev, cudaStream_t st, int32_t* route,
                  cudaStream_t sg = nullptr, cudaEvent_t gdone = nullptr) {
   if (!sg) sg = st;
   if (p.rotation_estimation_algorithm < 0 || p.rotation_estimation_algorithm > 2 || p.rotation_tim_graph < 0 ||
@@ -490,7 +618,8 @@ int run_pipeline(tzr_ctx* ctx, Batch& bt, const tzr_params& p, cudaEvent_t* ev, 
       nl += 2;
     }
     cudaEventRecord(ev[2], st);
-    launch_clique(bt, p, mode, st, &nl);
+    const int rc = run_clique(ctx, bt, p, mode, st, &nl, route);
+    if (rc) return rc;
   } else {
     if (sg != st) {
       cudaEventRecord(gdone, sg);
@@ -522,6 +651,7 @@ int run_chunked(tzr_ctx* ctx, Batch& bt, const tzr_params& p, const std::vector<
     ctx->stage_ev.push_back(e);
   }
   const bool lanes = n_chunks > 1 && ctx->gstream && ctx->hstream && l2_chunk(ctx, bt.B, bt.n, p) >= bt.B;
+  ctx->route.assign((size_t)bt.B, 0);
   // debug counters cover the whole call: zeroed once, ahead of every chunk on either lane (not per chunk, which would
   // keep only the last chunk's counts)
   if (ctx->flags & 6u) CK(cudaMemsetAsync((void*)ctx->dbg.p, 0, 16 * sizeof(unsigned long long), ctx->stream));
@@ -547,7 +677,8 @@ int run_chunked(tzr_ctx* ctx, Batch& bt, const tzr_params& p, const std::vector<
       if (cudaStreamWaitEvent(sg, ready[c], 0) != cudaSuccess) return TZR_ERR_CUDA;
     }
     Batch sb = (n_chunks > 1) ? sub_batch(bt, b0, Bc) : bt;
-    int rc = run_pipeline(ctx, sb, p, ctx->stage_ev.data() + 5 * (ctx->stage_first + c), st, sg, lanes ? ctx->gdone_ev[c] : nullptr);
+    int rc = run_pipeline(ctx, sb, p, ctx->stage_ev.data() + 5 * (ctx->stage_first + c), st, ctx->route.data() + b0, sg,
+                          lanes ? ctx->gdone_ev[c] : nullptr);
     if (rc) return rc;
     if (n_chunks == 1) bt = sb;  // keep fields filled in by run_pipeline (beta, scale_mode, ...)
   }
@@ -562,10 +693,9 @@ int run_chunked(tzr_ctx* ctx, Batch& bt, const tzr_params& p, const std::vector<
   ctx->last = bt;
   ctx->have_last = true;
   ctx->last_has_graph = effective_mode(p) != 3;  // NONE: populateVertices is never called (registration.cc:607-650)
+  ctx->route_B = ctx->last_has_graph ? bt.B : 0;
   return TZR_OK;
 }
-
-size_t al256(size_t x) { return (x + 255) & ~(size_t)255; }
 
 // tzr_compute_fpfh(_batch): B clouds staged back to back in one pinned area, one H2D copy, the batched launches, one
 // D2H copy of [overflow flags | descriptors | normals], then the caller's buffers are filled from the pinned copy.
@@ -810,7 +940,7 @@ int tzr_ctx_destroy(tzr_ctx* ctx) {
                     &ctx->hclq, &ctx->hsize, &ctx->clq, &ctx->L, &ctx->alive, &ctx->best_bits, &ctx->alive_cnt, &ctx->root_ctr,
                     &ctx->lock, &ctx->flg, &ctx->kfinal, &ctx->tstart, &ctx->stack, &ctx->cv, &ctx->centry, &ctx->ps, &ctx->pd, &ctx->wgt,
                     &ctx->res, &ctx->skey, &ctx->sidx, &ctx->sorted, &ctx->rmask, &ctx->tmask, &ctx->sol, &ctx->dbg,
-                    &ctx->misc, &ctx->sc, &ctx->m_in, &ctx->m_scratch, &ctx->m_out, &ctx->cert};
+                    &ctx->misc, &ctx->sc, &ctx->m_in, &ctx->m_scratch, &ctx->m_out, &ctx->cert, &ctx->lg, &ctx->cq};
   for (DevBuf* b : bufs)
     if (b->p) cudaFree(b->p);
   if (ctx->h_pin) cudaFreeHost(ctx->h_pin);
@@ -936,11 +1066,14 @@ int tzr_max_clique_batch(tzr_ctx* ctx, int B, int n, const uint64_t* adj_bits, i
   p.kcore_heuristic_threshold = kcore_thr;
   if (mode == 0 && time_limit_s > 0 && time_limit_s < 1e7) bt.budget_ns = (unsigned long long)(time_limit_s * 1e9);
   int nl = 2;
-  launch_clique(bt, p, mode, st, &nl);
+  ctx->route.assign((size_t)B, 0);
+  rc = run_clique(ctx, bt, p, mode, st, &nl, ctx->route.data());
   ctx->launches += nl;
+  if (rc) return rc;
   rc = check_launch(ctx, "max clique");
   if (rc) return rc;
   ctx->clique_B = B;
+  ctx->route_B = B;
   ctx->clique_geom[0] = bt.exact_ctas;
   ctx->clique_geom[1] = bt.exact_conc;
   ctx->clique_geom[2] = bt.max_depth;
@@ -978,6 +1111,18 @@ int tzr_ctx_clique_info(tzr_ctx* ctx, int32_t* geometry3, int32_t* heuristic_bes
     for (int b = 0; b < ctx->clique_B; ++b)
       heuristic_best[b] = *std::max_element(hs.begin() + (size_t)b * kHeurRoots, hs.begin() + (size_t)(b + 1) * kHeurRoots);
   }
+  return TZR_OK;
+}
+
+int tzr_ctx_set_max_n(tzr_ctx* ctx, int max_n) {
+  if (!ctx || max_n < kMaxN || max_n > kMaxNLarge) return TZR_ERR_INVALID_ARG;
+  ctx->max_n = max_n;
+  return TZR_OK;
+}
+
+int tzr_ctx_clique_route(tzr_ctx* ctx, int32_t* per_problem) {
+  if (!ctx || !per_problem || ctx->route_B <= 0) return TZR_ERR_INVALID_ARG;
+  std::copy(ctx->route.begin(), ctx->route.begin() + ctx->route_B, per_problem);
   return TZR_OK;
 }
 
@@ -1154,7 +1299,9 @@ static int solve_uniform_host(tzr_ctx* ctx, const tzr_params* params, int B, int
   // PCIe moves a problem ~3x faster than the kernels consume it, so only the first chunk's copy is exposed: it is
   // kept small (B/32) and the later chunks grow (3B/32, B/8, then B/4 each) to keep launch tails few.
   std::vector<int> bounds{0};
-  if (B >= 64 && !params->estimate_scaling) {
+  if (n > kMaxN) {  // one such problem fills the GPU (a 512 MiB bitset at n = 65536): one per chunk
+    for (int b = 1; b <= B; ++b) bounds.push_back(b);
+  } else if (B >= 64 && !params->estimate_scaling) {
     const int unit = std::max(8, B / 32);
     const int sizes[3] = {unit, 3 * unit, 4 * unit};
     for (int k = 0; bounds.back() < B; ++k) {

@@ -26,6 +26,8 @@
 //        The incumbent is shared through L[b] (atomic) + a spin lock for the vertex list/bitset.
 //
 // Bit-parallel integer work, L2-resident bitset: no tensor cores, no meaningful HBM roofline.
+#include <algorithm>
+
 #include "tzr_internal.cuh"
 
 namespace tzr {
@@ -136,18 +138,15 @@ __device__ int block_excl_scan(int v, int* s_tmp /* >= 34 */, int* total) {
 // =================================================================================================
 size_t clique_heur_smem(int n) { return (size_t)pitch32(n) * 4 + (size_t)n * 2 * 2 + 16; }
 
-__global__ void __launch_bounds__(kHeurThreads) clique_heur_kernel(Batch bt) {
-  const int r = blockIdx.x, b = blockIdx.y;
-  const int n = bt.n, W = pitch32(n);
-  extern __shared__ __align__(16) unsigned char smem_raw[];
-  uint32_t* P = reinterpret_cast<uint32_t*>(smem_raw);
-  uint16_t* list = reinterpret_cast<uint16_t*>(P + W);
-  uint16_t* dl = list + n;
-  __shared__ unsigned long long s_key[34];
-  __shared__ int s_scan[34];
-  __shared__ int s_chosen[kHeurRoots];
-  __shared__ int s_csz, s_nuni;
+namespace {
 
+// Body of K1 for root r of problem b.  P: the candidate bitset (shared memory); list / dl: the ordered candidate list
+// and in-P degrees (u16: vertex indices and degrees are below 2^16), in shared memory for clique_heur_kernel and in
+// global scratch for clique_heur_large_kernel (n > kMaxN: 4 n bytes do not fit the SM).  Inlined into both kernels.
+__device__ __forceinline__ void heur_body(const Batch& bt, int r, int b, uint32_t* P, uint16_t* list, uint16_t* dl,
+                                          unsigned long long* s_key, int* s_scan, int* s_chosen, int& s_csz,
+                                          int& s_nuni) {
+  const int n = bt.n, W = pitch32(n);
   if (bt.kcore_final && bt.kcore_final[b]) return;  // KCORE_HEU shortcut already produced the answer
   const int32_t* deg = bt.deg + (size_t)b * n;
   int32_t* C = bt.hclq + ((size_t)b * kHeurRoots + r) * n;
@@ -273,6 +272,40 @@ __global__ void __launch_bounds__(kHeurThreads) clique_heur_kernel(Batch bt) {
   }
   __syncthreads();
   if (tid == 0) bt.hsize[b * kHeurRoots + r] = s_csz;
+}
+
+}  // namespace
+
+__global__ void __launch_bounds__(kHeurThreads) clique_heur_kernel(Batch bt) {
+  const int r = blockIdx.x, b = blockIdx.y;
+  const int n = bt.n, W = pitch32(n);
+  extern __shared__ __align__(16) unsigned char smem_raw[];
+  uint32_t* P = reinterpret_cast<uint32_t*>(smem_raw);
+  uint16_t* list = reinterpret_cast<uint16_t*>(P + W);
+  uint16_t* dl = list + n;
+  __shared__ unsigned long long s_key[34];
+  __shared__ int s_scan[34];
+  __shared__ int s_chosen[kHeurRoots];
+  __shared__ int s_csz, s_nuni;
+  heur_body(bt, r, b, P, list, dl, s_key, s_scan, s_chosen, s_csz, s_nuni);
+}
+
+// K1 of the large route (n > kMaxN, or debug flag 524288): the same greedy with P in shared memory (W words) and the
+// candidate list / in-P degrees in `lists` (B * kHeurRoots * 2n u16 of global scratch, L2-resident).
+size_t clique_heur_large_smem(int n) { return (size_t)pitch32(n) * 4 + 16; }
+
+__global__ void __launch_bounds__(kHeurThreads) clique_heur_large_kernel(Batch bt, uint16_t* lists) {
+  const int r = blockIdx.x, b = blockIdx.y;
+  const int n = bt.n;
+  extern __shared__ __align__(16) unsigned char smem_raw[];
+  uint32_t* P = reinterpret_cast<uint32_t*>(smem_raw);
+  uint16_t* list = lists + ((size_t)b * kHeurRoots + r) * 2 * (size_t)n;
+  uint16_t* dl = list + n;
+  __shared__ unsigned long long s_key[34];
+  __shared__ int s_scan[34];
+  __shared__ int s_chosen[kHeurRoots];
+  __shared__ int s_csz, s_nuni;
+  heur_body(bt, r, b, P, list, dl, s_key, s_scan, s_chosen, s_csz, s_nuni);
 }
 
 // =================================================================================================
@@ -1650,6 +1683,181 @@ __global__ void clique_resume_kernel(Batch bt) {
   }
 }
 
+// =================================================================================================
+// Large route (DESIGN.md §3.2): the (L-1)-core of the full graph on many CTAs, its order-preserving compaction into a
+// graph of at most kMaxN vertices, and the way back.  L is the incumbent that clique_peel_kernel (mode 1) selected
+// from the heuristic cliques; every clique of size >= L lies inside the (L-1)-core.
+// =================================================================================================
+
+// alive0 = {v : deg[v] >= L - 1} (the first peel round, from the degrees the graph stage already has); zeroes the
+// per-round change counters.  Grid (ceil(W / 256), B).
+__global__ void __launch_bounds__(256) core_init_kernel(Batch bt, int32_t* chg) {
+  const int b = blockIdx.y, n = bt.n, W = pitch32(n);
+  const int x = blockIdx.x * 256 + threadIdx.x;
+  if (blockIdx.x == 0 && threadIdx.x < kCoreRounds) chg[b * kCoreRounds + threadIdx.x] = 0;
+  if (x >= W) return;
+  const int thr = bt.L[b] - 1;
+  const int32_t* deg = bt.deg + (size_t)b * n;
+  uint32_t m = 0u;
+  for (int k = 0; k < 32; ++k) {
+    const int v = x * 32 + k;
+    if (v < n && deg[v] >= thr) m |= 1u << k;
+  }
+  bt.alive[(size_t)b * W + x] = m;
+}
+
+// One peel round over every problem, one warp per alive word (grid-stride), four vertices at a time.  Degrees count
+// only the alive words of the set, and each row word is loaded only where the set has vertices.  The set is peeled in
+// place: a vertex whose degree inside some superset of the core is below L - 1 is not in the core, so concurrent
+// removals only speed convergence.  A round that removes nothing proves the set is the core; later rounds return at
+// once (chg[r - 1] == 0).  Grid (ctas, B).
+__global__ void __launch_bounds__(256) core_round_kernel(Batch bt, int32_t* chg, int r) {
+  const int b = blockIdx.y, n = bt.n, W = pitch32(n);
+  int32_t* cb = chg + b * kCoreRounds;
+  if (r > 0 && *(volatile int32_t*)(cb + r - 1) == 0) return;
+  const int thr = bt.L[b] - 1;
+  if (thr <= 0) return;  // L <= 1: nothing to peel
+  uint32_t* S = bt.alive + (size_t)b * W;
+  const int lane = threadIdx.x & 31;
+  const int gw = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5), nwarps = gridDim.x * (blockDim.x >> 5);
+  int removed = 0;
+  for (int x = gw; x < W; x += nwarps) {
+    uint32_t m = *(volatile uint32_t*)(S + x);
+    while (m) {
+      int u[4], bits[4], kc = 0;
+      while (m && kc < 4) {
+        bits[kc] = __ffs(m) - 1;
+        m &= m - 1;
+        u[kc] = x * 32 + bits[kc];
+        ++kc;
+      }
+      for (int q = kc; q < 4; ++q) u[q] = u[0];
+      const uint32_t* r0 = adj_row32(bt, b, u[0]);
+      const uint32_t* r1 = adj_row32(bt, b, u[1]);
+      const uint32_t* r2 = adj_row32(bt, b, u[2]);
+      const uint32_t* r3 = adj_row32(bt, b, u[3]);
+      int d0 = 0, d1 = 0, d2 = 0, d3 = 0;
+      for (int y = lane; y < W; y += 32) {
+        const uint32_t sw = S[y];
+        if (sw) {
+          d0 += __popc(r0[y] & sw);
+          d1 += __popc(r1[y] & sw);
+          d2 += __popc(r2[y] & sw);
+          d3 += __popc(r3[y] & sw);
+        }
+      }
+      const int d[4] = {__reduce_add_sync(0xffffffffu, d0), __reduce_add_sync(0xffffffffu, d1),
+                        __reduce_add_sync(0xffffffffu, d2), __reduce_add_sync(0xffffffffu, d3)};
+      uint32_t clr = 0u;
+#pragma unroll
+      for (int q = 0; q < 4; ++q)
+        if (q < kc && d[q] < thr) clr |= 1u << bits[q];
+      if (clr && lane == 0) {
+        atomicAnd(S + x, ~clr);
+        removed = 1;
+      }
+    }
+  }
+  if (removed) atomicAdd(cb + r, 1);
+}
+
+// Survivors in ascending order: new2old[0..cnt) and old2new[v] for every survivor; core_cnt[b] = cnt.  One CTA per
+// problem (a scan over W <= 2048 words).
+__global__ void __launch_bounds__(kPeelThreads) core_list_kernel(Batch bt, int32_t* new2old, int32_t* old2new,
+                                                                 int32_t* core_cnt) {
+  const int b = blockIdx.x, n = bt.n, W = pitch32(n);
+  const uint32_t* S = bt.alive + (size_t)b * W;
+  int32_t* n2o = new2old + (size_t)b * n;
+  int32_t* o2n = old2new + (size_t)b * n;
+  __shared__ int s_scan[34];
+  int base = 0;
+  for (int x0 = 0; x0 < W; x0 += blockDim.x) {
+    const int x = x0 + threadIdx.x;
+    uint32_t m = x < W ? S[x] : 0u;
+    int tot = 0;
+    int pos = base + block_excl_scan(__popc(m), s_scan, &tot);
+    while (m) {
+      const int v = x * 32 + __ffs(m) - 1;
+      m &= m - 1;
+      n2o[pos] = v;
+      o2n[v] = pos++;
+    }
+    base += tot;
+  }
+  if (threadIdx.x == 0) core_cnt[b] = base;
+}
+
+// Compacted bitset, one warp per row i of the compacted batch (n2 vertices, pitch32(n2) words, built in shared
+// memory): row i of a searched problem is adj[new2old[i]] & alive with every bit j moved to old2new[j], O(W + core
+// degree) per row; rows past the problem's core and every row of a problem that is not searched stay empty (isolated
+// padding vertices join no clique of size >= 2).  Grid (ceil(n2 / 8), B), 8 warps x pitch32(n2) words of shared memory.
+__global__ void __launch_bounds__(256) core_compact_kernel(Batch bt, Batch cb, const int32_t* new2old,
+                                                           const int32_t* old2new, const int32_t* core_cnt,
+                                                           const int32_t* route) {
+  const int b = blockIdx.y, n = bt.n, W = pitch32(n), n2 = cb.n, W2 = pitch32(n2);
+  extern __shared__ __align__(16) unsigned char smem_raw[];
+  const int wid = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  uint32_t* row = reinterpret_cast<uint32_t*>(smem_raw) + (size_t)wid * W2;
+  const int i = blockIdx.x * 8 + wid;
+  if (i >= n2) return;
+  for (int x = lane; x < W2; x += 32) row[x] = 0u;
+  __syncwarp();
+  if (route[b] > 0 && i < core_cnt[b]) {
+    const int v = new2old[(size_t)b * n + i];
+    const uint32_t* rv = adj_row32(bt, b, v);
+    const uint32_t* S = bt.alive + (size_t)b * W;
+    const int32_t* o2n = old2new + (size_t)b * n;
+    for (int x = lane; x < W; x += 32) {
+      uint32_t m = rv[x] & S[x];
+      while (m) {
+        const int j = o2n[x * 32 + __ffs(m) - 1];
+        m &= m - 1;
+        atomicOr(row + (j >> 5), 1u << (j & 31));
+      }
+    }
+  }
+  __syncwarp();
+  uint32_t* dst = reinterpret_cast<uint32_t*>(cb.adj) + ((size_t)b * n2 + i) * W2;
+  for (int x = lane; x < W2; x += 32) dst[x] = row[x];
+}
+
+// The full graph's incumbent (clq[0..L), heuristic order) becomes heuristic clique 0 of the compacted problem, so that
+// clique_peel_kernel starts from the incumbent the small route has at that point; problems that are not searched get
+// no candidate (L = 0: the compacted search leaves them alone).  One CTA per problem.
+__global__ void __launch_bounds__(256) core_plant_kernel(Batch bt, Batch cb, const int32_t* old2new,
+                                                         const int32_t* route) {
+  const int b = blockIdx.x;
+  const int L = route[b] > 0 ? bt.L[b] : 0;
+  if (threadIdx.x < kHeurRoots) cb.hsize[b * kHeurRoots + threadIdx.x] = threadIdx.x == 0 ? L : 0;
+  const int32_t* src = bt.clq + (size_t)b * bt.n;
+  const int32_t* o2n = old2new + (size_t)b * bt.n;
+  int32_t* dst = cb.hclq + (size_t)b * kHeurRoots * cb.n;
+  for (int k = threadIdx.x; k < L; k += blockDim.x) dst[k] = o2n[src[k]];
+}
+
+// Back to the full graph: a searched problem takes the compacted result (clique through new2old, the map is monotone,
+// so the canonical order carries over) and its search flags; a problem whose core exceeded the cap keeps its
+// heuristic clique, marked not proven (flags 1 | 16).  One CTA per problem.
+__global__ void __launch_bounds__(256) core_map_back_kernel(Batch bt, Batch cb, const int32_t* new2old,
+                                                            const int32_t* route) {
+  const int b = blockIdx.x;
+  const int rt = route[b];
+  if (rt < 0) {
+    if (threadIdx.x == 0) bt.flags[b] |= 1 | 16;
+    return;
+  }
+  if (rt == 0) return;
+  const int L = cb.L[b];
+  const int32_t* src = cb.clq + (size_t)b * cb.n;
+  const int32_t* n2o = new2old + (size_t)b * bt.n;
+  int32_t* dst = bt.clq + (size_t)b * bt.n;
+  for (int k = threadIdx.x; k < L; k += blockDim.x) dst[k] = n2o[src[k]];
+  if (threadIdx.x == 0) {
+    bt.L[b] = L;
+    bt.flags[b] = cb.flags[b];
+  }
+}
+
 namespace {
 void clique_set_attrs() {
   // per device: a process may hold contexts on several GPUs
@@ -1677,6 +1885,38 @@ int clique_exact_grid(int n, int num_sms) {
   return occ * num_sms;
 }
 
+namespace {
+// Exact phase after the peel kernel (mode 0), shared by both routes.  Returns the launches.
+int launch_exact_passes(const Batch& b2, cudaStream_t st) {
+  const int n = b2.n;
+  int launches = 0;
+  // Two passes: a short first one (every instance the canonical enumeration can finish does so here), then the
+  // Nemhauser–Trotter bound / reduction for whatever ran into that deadline, then the rest of the caller's budget.
+  constexpr unsigned long long kFirstPassNs = 50ull * 1000 * 1000;
+  const unsigned long long total = b2.budget_ns;  // 0 = unlimited
+  // Debug flag 32768: a first pass of 1 ns, so that every problem that reaches the exact search goes through the LP
+  // kernel (unless its whole first pass fits in one %globaltimer tick); the second pass keeps the caller's whole
+  // budget.  Debug flag 131072: a single pass with the caller's whole budget (no 50 ms cap), so that whether a
+  // canonical enumeration finishes does not depend on the wall clock.
+  const bool short_first = (b2.flags_dbg & 32768u) != 0u;
+  const bool one_pass = !short_first && (b2.flags_dbg & 131072u) != 0u;
+  const unsigned g3 = (unsigned)b2.exact_ctas;
+  Batch p1 = b2;
+  p1.budget_ns = short_first ? 1ull : one_pass ? total : (total == 0ull || total > kFirstPassNs) ? kFirstPassNs : total;
+  clique_exact_kernel<<<g3, kExactThreads, clique_exact_smem(n), st>>>(p1);
+  clique_lp_kernel<<<b2.B, 32, 0, st>>>(b2);
+  launches += 2;
+  if (!one_pass && (short_first || total == 0ull || total > kFirstPassNs)) {
+    Batch p2 = b2;
+    p2.budget_ns = short_first ? total : total ? total - kFirstPassNs : 0ull;
+    clique_resume_kernel<<<(b2.B + 127) / 128, 128, 0, st>>>(b2);
+    clique_exact_kernel<<<g3, kExactThreads, clique_exact_smem(n), st>>>(p2);
+    launches += 2;
+  }
+  return launches;
+}
+}  // namespace
+
 void launch_clique(const Batch& bt, const tzr_params& p, int mode, cudaStream_t st, int* n_launches) {
   const int n = bt.n;
   clique_set_attrs();
@@ -1692,32 +1932,63 @@ void launch_clique(const Batch& bt, const tzr_params& p, int mode, cudaStream_t 
   clique_heur_kernel<<<g1, kHeurThreads, clique_heur_smem(n), st>>>(b2);
   clique_peel_kernel<<<bt.B, kPeelThreads, clique_peel_smem(n), st>>>(b2, mode == 0 ? 0 : 1);
   launches += 2;
-  if (mode == 0) {
-    // Two passes: a short first one (every instance the canonical enumeration can finish does so here), then the
-    // Nemhauser–Trotter bound / reduction for whatever ran into that deadline, then the rest of the caller's budget.
-    constexpr unsigned long long kFirstPassNs = 50ull * 1000 * 1000;
-    const unsigned long long total = bt.budget_ns;  // 0 = unlimited
-    // Debug flag 32768: a first pass of 1 ns, so that every problem that reaches the exact search goes through the LP
-    // kernel (unless its whole first pass fits in one %globaltimer tick); the second pass keeps the caller's whole
-    // budget.  Debug flag 131072: a single pass with the caller's whole budget (no 50 ms cap), so that whether a
-    // canonical enumeration finishes does not depend on the wall clock.
-    const bool short_first = (bt.flags_dbg & 32768u) != 0u;
-    const bool one_pass = !short_first && (bt.flags_dbg & 131072u) != 0u;
-    const unsigned g3 = (unsigned)bt.exact_ctas;
-    Batch p1 = b2;
-    p1.budget_ns = short_first ? 1ull : one_pass ? total : (total == 0ull || total > kFirstPassNs) ? kFirstPassNs : total;
-    clique_exact_kernel<<<g3, kExactThreads, clique_exact_smem(n), st>>>(p1);
-    clique_lp_kernel<<<bt.B, 32, 0, st>>>(b2);
-    launches += 2;
-    if (!one_pass && (short_first || total == 0ull || total > kFirstPassNs)) {
-      Batch p2 = b2;
-      p2.budget_ns = short_first ? total : total ? total - kFirstPassNs : 0ull;
-      clique_resume_kernel<<<(bt.B + 127) / 128, 128, 0, st>>>(b2);
-      clique_exact_kernel<<<g3, kExactThreads, clique_exact_smem(n), st>>>(p2);
-      launches += 2;
-    }
-  }
+  if (mode == 0) launches += launch_exact_passes(b2, st);
   if (n_launches) *n_launches += launches;
+}
+
+void launch_clique_large_front(const Batch& bt, const tzr_params& p, int mode, uint16_t* lists, cudaStream_t st,
+                               int* n_launches) {
+  const int n = bt.n;
+  clique_set_attrs();
+  int launches = 0;
+  Batch b2 = bt;
+  if (mode == 2) {
+    clique_kcore_kernel<<<bt.B, kPeelThreads, clique_kcore_smem(n), st>>>(bt, p.kcore_heuristic_threshold);
+    ++launches;
+  } else {
+    b2.kcore_final = nullptr;
+  }
+  dim3 g1(kHeurRoots, (unsigned)bt.B);
+  clique_heur_large_kernel<<<g1, kHeurThreads, clique_heur_large_smem(n), st>>>(b2, lists);
+  // mode 1: selects the best heuristic clique into clq / L / best_bits and stops (no peel, no search)
+  clique_peel_kernel<<<bt.B, kPeelThreads, clique_peel_smem(n), st>>>(b2, 1);
+  launches += 2;
+  if (n_launches) *n_launches += launches;
+}
+
+void launch_core(const Batch& bt, int32_t* chg, int32_t* new2old, int32_t* old2new, int32_t* core_cnt, int num_sms,
+                 cudaStream_t st, int* n_launches) {
+  const int W = pitch32(bt.n);
+  core_init_kernel<<<dim3((unsigned)((W + 255) / 256), (unsigned)bt.B), 256, 0, st>>>(bt, chg);
+  const int per = std::max(1, std::min((W + 7) / 8, (2 * num_sms + bt.B - 1) / bt.B));
+  for (int r = 0; r < kCoreRounds; ++r) core_round_kernel<<<dim3((unsigned)per, (unsigned)bt.B), 256, 0, st>>>(bt, chg, r);
+  core_list_kernel<<<bt.B, kPeelThreads, 0, st>>>(bt, new2old, old2new, core_cnt);
+  if (n_launches) *n_launches += kCoreRounds + 2;
+}
+
+size_t core_compact_smem(int n2) { return (size_t)8 * pitch32(n2) * 4; }
+
+void launch_core_compact(const Batch& bt, const Batch& cb, const int32_t* new2old, const int32_t* old2new,
+                         const int32_t* core_cnt, const int32_t* route, cudaStream_t st, int* n_launches) {
+  core_compact_kernel<<<dim3((unsigned)((cb.n + 7) / 8), (unsigned)bt.B), 256, core_compact_smem(cb.n), st>>>(
+      bt, cb, new2old, old2new, core_cnt, route);
+  core_plant_kernel<<<bt.B, 256, 0, st>>>(bt, cb, old2new, route);
+  if (n_launches) *n_launches += 2;
+}
+
+void launch_clique_search(const Batch& cb, cudaStream_t st, int* n_launches) {
+  clique_set_attrs();
+  Batch b2 = cb;
+  b2.kcore_final = nullptr;
+  clique_peel_kernel<<<cb.B, kPeelThreads, clique_peel_smem(cb.n), st>>>(b2, 0);
+  const int launches = 1 + launch_exact_passes(b2, st);
+  if (n_launches) *n_launches += launches;
+}
+
+void launch_core_map_back(const Batch& bt, const Batch& cb, const int32_t* new2old, const int32_t* route,
+                          cudaStream_t st, int* n_launches) {
+  core_map_back_kernel<<<bt.B, 256, 0, st>>>(bt, cb, new2old, route);
+  if (n_launches) *n_launches += 1;
 }
 
 }  // namespace tzr

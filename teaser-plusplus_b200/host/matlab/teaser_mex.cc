@@ -46,6 +46,7 @@ void mexFunction(int nlhs, mxArray* plhs[], int nrhs, const mxArray* prhs[]) {
   if (!g_ctx) {
     if (tzr_ctx_create(-1, &g_ctx) != TZR_OK)
       mexErrMsgIdAndTxt("teaserSolve:noDevice", "No usable CUDA device (the GPU path has no CPU fallback).");
+    tzr_ctx_set_max_n(g_ctx, 65536);  // the reference has no size limit: up to 65536 correspondences
     mexAtExit(release_ctx);
   }
   tzr_params p;

@@ -61,6 +61,9 @@ tzr_ctx* b200_context() {
   if (!h.c) {
     int rc = tzr_ctx_create(-1, &h.c);
     if (rc != TZR_OK) fail("teaser (GPU): cannot create a CUDA context", rc, nullptr);
+    // the reference has no size limit: take the device's largest (65536 correspondences, large clique route)
+    rc = tzr_ctx_set_max_n(h.c, 65536);
+    if (rc != TZR_OK) fail("teaser (GPU): tzr_ctx_set_max_n", rc, h.c);
   }
   return h.c;
 }
