@@ -266,6 +266,28 @@ int tzr_certify(tzr_ctx* ctx, const tzr_certifier_params* params, const double* 
                 const double* dst_3xN, const double* theta, int n, tzr_certification_result* result, double* traj,
                 int traj_capacity);
 
+/* B certifications in one call: problem b has N[b] >= 1 measurements, its rotation at R_colmajor9xB + 9b (column-major),
+ * src_3xN[b] / dst_3xN[b] (3 x N[b] column-major) and theta[b] (N[b] doubles, +1 / -1); params apply to every problem.
+ * Host pointers, synchronous like tzr_compute_fpfh_batch.  results: B entries, each meaning what tzr_certify's result
+ * means for that problem alone (is_optimal, n_iterations, best_suboptimality).  traj (may be NULL, or hold NULL entries):
+ * traj[b] receives min(n_iterations, traj_capacity[b]) gaps; traj_capacity (B int32 >= 0) may be NULL when traj is
+ * (TZR_ERR_INVALID_ARG when traj is given without it).
+ * The problems run together: one launch sequence per iteration for the whole batch, one read-back of the active flags
+ * per iteration, the trajectories copied back once at the end.  Finished problems are skipped by every kernel and by the
+ * eigensolver.  The eigendecompositions of an iteration are one cusolverDnXsyevBatched call over the active problems'
+ * matrices padded to 4 max N + 4 with an identity block (DESIGN.md 3.9; once some problems have finished, the active
+ * ones are gathered into a compact batch first) while at least 8 problems are active, else one cusolverDnDsyevd per
+ * active problem; the loop is also taken
+ * when the batched symbol is missing, the batched call refuses the size, or debug flag 2097152 is set.
+ * tzr_ctx_kernel_launches counts every eigensolver call as one launch.  A batch that does not fit the device is cut into
+ * consecutive groups inside the call; the caller need not split it.  TZR_ERR_TOO_LARGE when some 4N[b]+4 exceeds 32768
+ * (no result written); TZR_ERR_ALLOC when a single problem's workspace does not fit the device (tzr_last_error names
+ * the size); TZR_ERR_UNSUPPORTED when cuSOLVER cannot be loaded. */
+int tzr_certify_batch(tzr_ctx* ctx, const tzr_certifier_params* params, int B, const int32_t* N,
+                      const double* R_colmajor9xB, const double* const* src_3xN, const double* const* dst_3xN,
+                      const double* const* theta, tzr_certification_result* results, double* const* traj,
+                      const int32_t* traj_capacity);
+
 /* Building blocks, exposed so that each can be checked against the reference's fixtures
  * (test/teaser/certification-test.cc:355-497):
  * tzr_certifier_initial_matrix: M_init = D^T Q_cost D - mu J - lambda_guess (certification.cc:60-100), dense
@@ -346,7 +368,9 @@ int tzr_solve_batch_multi(const int32_t* devices, int n_devices, const tzr_param
  * tiled scans) at every size instead of the bitonic sort + sequential sweep below 257 points, bit 19 (524288) = the
  * large clique route at every n (tzr_ctx_clique_route), so that the two routes can be compared on the same graphs,
  * bit 20 (1048576) = cap the large route's compacted core at 64 vertices instead of 32768, so that its "core too large"
- * outcome is reachable at test sizes.  Bits 15 to 20 change host code only. */
+ * outcome is reachable at test sizes, bit 21 (2097152) = tzr_certify_batch loops cusolverDnDsyevd over the active
+ * problems instead of one cusolverDnXsyevBatched call, so that the two eigen routes can be compared on the same batch.
+ * Bits 15 to 21 change host code only. */
 int tzr_ctx_set_flags(tzr_ctx* ctx, uint32_t flags);
 int64_t tzr_ctx_filter_mismatches(tzr_ctx* ctx);
 /* Number of pairs of the most recent graph build that needed the exact FP64 re-check. */

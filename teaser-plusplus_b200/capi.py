@@ -96,7 +96,7 @@ _SYMBOLS = [
     "tzr_match_correspondences", "tzr_feature_nn", "tzr_compute_fpfh", "tzr_certifier_params_default", "tzr_certify",
     "tzr_certifier_initial_matrix", "tzr_certifier_dual_projection", "tzr_last_graph_info", "tzr_ctx_stage_log",
     "tzr_ctx_stage_log_read", "tzr_solve_batch_multi", "tzr_ctx_clique_info", "tzr_compute_fpfh_batch",
-    "tzr_match_correspondences_batch", "tzr_ctx_set_max_n", "tzr_ctx_clique_route",
+    "tzr_match_correspondences_batch", "tzr_ctx_set_max_n", "tzr_ctx_clique_route", "tzr_certify_batch",
 ]
 
 
@@ -174,6 +174,8 @@ def lib():
     L.tzr_certifier_params_default.restype = None
     L.tzr_certify.argtypes = [vp, C.POINTER(CertifierParams), dp, dp, dp, dp, C.c_int, C.POINTER(CertificationResult),
                               dp, C.c_int]
+    L.tzr_certify_batch.argtypes = [vp, C.POINTER(CertifierParams), C.c_int, i32p, dp, C.POINTER(dp), C.POINTER(dp),
+                                    C.POINTER(dp), C.POINTER(CertificationResult), C.POINTER(dp), i32p]
     L.tzr_certifier_initial_matrix.argtypes = [vp, C.POINTER(CertifierParams), dp, dp, dp, dp, C.c_int, dp, dp]
     L.tzr_certifier_dual_projection.argtypes = [vp, dp, dp, C.c_int, dp]
     for s in _SYMBOLS:
@@ -412,6 +414,43 @@ class Context:
                                    _p(th, C.c_double), th.size, C.byref(res), _p(traj, C.c_double), cap))
         return dict(is_optimal=bool(res.is_optimal), best_suboptimality=res.best_suboptimality,
                     suboptimality_traj=traj[:res.n_iterations].copy())
+
+    @staticmethod
+    def _cert_batch_inputs(Rs, srcs, dsts, thetas):
+        """Validated, contiguous per-problem inputs of certify_batch (no device needed)."""
+        Rs, srcs, dsts, thetas = list(Rs), list(srcs), list(dsts), list(thetas)
+        B = len(Rs)
+        if B == 0 or not (len(srcs) == len(dsts) == len(thetas) == B):
+            raise TzrError("certify_batch: four lists of the same non-zero length are required")
+        probs = []
+        for b in range(B):
+            if np.asarray(Rs[b]).shape != (3, 3):
+                raise TzrError(f"certify_batch: rotation {b} must be (3,3)")
+            Rc, s, d, th = Context._cert_inputs(Rs[b], srcs[b], dsts[b], thetas[b])
+            if th.size == 0:
+                raise TzrError(f"certify_batch: problem {b} has no measurements")
+            probs.append((Rc, s, d, th))
+        return probs
+
+    def certify_batch(self, Rs, srcs, dsts, thetas, **params):
+        """certify on every problem of the lists in one call (tzr_certify_batch): Rs (3,3), srcs/dsts (3,N_b), thetas
+        (N_b,) +-1 or bool.  Returns a list of dicts shaped like certify's."""
+        probs = self._cert_batch_inputs(Rs, srcs, dsts, thetas)
+        p = self.certifier_params(**params)
+        B = len(probs)
+        R = np.ascontiguousarray(np.concatenate([pr[0].ravel() for pr in probs]))
+        N = np.array([pr[3].size for pr in probs], dtype=np.int32)
+        cap = int(max(1, np.ceil(p.max_iterations)))
+        trajs = [np.zeros(cap) for _ in range(B)]
+        caps = np.full(B, cap, dtype=np.int32)
+        res = (CertificationResult * B)()
+        dp = C.POINTER(C.c_double)
+        arr = lambda xs: (dp * B)(*[_p(x, C.c_double) for x in xs])
+        self._ck(lib().tzr_certify_batch(self._h, C.byref(p), B, _p(N, C.c_int32), _p(R, C.c_double),
+                                         arr([pr[1] for pr in probs]), arr([pr[2] for pr in probs]),
+                                         arr([pr[3] for pr in probs]), res, arr(trajs), _p(caps, C.c_int32)))
+        return [dict(is_optimal=bool(r.is_optimal), best_suboptimality=r.best_suboptimality,
+                     suboptimality_traj=t[:r.n_iterations].copy()) for r, t in zip(res, trajs)]
 
     def certifier_initial_matrix(self, R, src, dst, theta, **params):
         p = self.certifier_params(**params)

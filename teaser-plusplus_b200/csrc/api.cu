@@ -30,7 +30,8 @@ struct tzr_ctx {
   int num_sms = 132;
   // device buffers (grow-only)
   DevBuf src, dst, sf, df, pk, opnd, tclist, gc, adj, deg, nedges, hclq, hsize, clq, L, alive, best_bits, alive_cnt, root_ctr, lock, flg, kfinal, tstart, stack, cv,
-      centry, ps, pd, wgt, res, skey, sidx, sorted, rmask, tmask, sol, dbg, misc, sc, m_in, m_scratch, m_out, cert;
+      centry, ps, pd, wgt, res, skey, sidx, sorted, rmask, tmask, sol, dbg, misc, sc, m_in, m_scratch, m_out, cert,
+      certb;
   // large clique route (n > kMaxN or debug flag 524288): scratch on the full graph, and the compacted batch's buffers
   DevBuf lg, cq;
   int max_n = kMaxN;  // per-problem size limit of this context (tzr_ctx_set_max_n: kMaxN ... kMaxNLarge)
@@ -940,7 +941,7 @@ int tzr_ctx_destroy(tzr_ctx* ctx) {
                     &ctx->hclq, &ctx->hsize, &ctx->clq, &ctx->L, &ctx->alive, &ctx->best_bits, &ctx->alive_cnt, &ctx->root_ctr,
                     &ctx->lock, &ctx->flg, &ctx->kfinal, &ctx->tstart, &ctx->stack, &ctx->cv, &ctx->centry, &ctx->ps, &ctx->pd, &ctx->wgt,
                     &ctx->res, &ctx->skey, &ctx->sidx, &ctx->sorted, &ctx->rmask, &ctx->tmask, &ctx->sol, &ctx->dbg,
-                    &ctx->misc, &ctx->sc, &ctx->m_in, &ctx->m_scratch, &ctx->m_out, &ctx->cert, &ctx->lg, &ctx->cq};
+                    &ctx->misc, &ctx->sc, &ctx->m_in, &ctx->m_scratch, &ctx->m_out, &ctx->cert, &ctx->certb, &ctx->lg, &ctx->cq};
   for (DevBuf* b : bufs)
     if (b->p) cudaFree(b->p);
   if (ctx->h_pin) cudaFreeHost(ctx->h_pin);
@@ -1507,6 +1508,22 @@ int tzr_certify(tzr_ctx* ctx, const tzr_certifier_params* params, const double* 
   result->n_iterations = iters;
   result->best_suboptimality = best;
   return TZR_OK;
+}
+
+int tzr_certify_batch(tzr_ctx* ctx, const tzr_certifier_params* params, int B, const int32_t* N,
+                      const double* R_colmajor9xB, const double* const* src_3xN, const double* const* dst_3xN,
+                      const double* const* theta, tzr_certification_result* results, double* const* traj,
+                      const int32_t* traj_capacity) {
+  if (!ctx || !params || B <= 0 || !N || !R_colmajor9xB || !src_3xN || !dst_3xN || !theta || !results ||
+      (traj && !traj_capacity))
+    return TZR_ERR_INVALID_ARG;
+  for (int b = 0; b < B; ++b)
+    if (N[b] <= 0 || !src_3xN[b] || !dst_3xN[b] || !theta[b] || (traj_capacity && traj_capacity[b] < 0))
+      return TZR_ERR_INVALID_ARG;
+  cudaSetDevice(ctx->device);
+  return certify_batch_device(*params, B, N, R_colmajor9xB, src_3xN, dst_3xN, theta, results, traj, traj_capacity,
+                              (ctx->flags & 2097152u) != 0, &ctx->certb.p, &ctx->certb.cap, &ctx->solver_handle,
+                              &ctx->launches, ctx->stream, &ctx->last_error);
 }
 
 int tzr_certifier_initial_matrix(tzr_ctx* ctx, const tzr_certifier_params* params, const double* R_colmajor9,

@@ -39,6 +39,16 @@ struct Cusolver {
                                 const double*, int*) = nullptr;
   cusolverStatus_t (*syevd)(cusolverDnHandle_t, cusolverEigMode_t, cublasFillMode_t, int, double*, int, double*,
                             double*, int, int*) = nullptr;
+  // batched route of tzr_certify_batch (optional: without them the batch loops syevd)
+  cusolverStatus_t (*create_params)(cusolverDnParams_t*) = nullptr;
+  cusolverStatus_t (*destroy_params)(cusolverDnParams_t) = nullptr;
+  cusolverStatus_t (*syev_batched_buf)(cusolverDnHandle_t, cusolverDnParams_t, cusolverEigMode_t, cublasFillMode_t,
+                                       int64_t, cudaDataType, const void*, int64_t, cudaDataType, const void*,
+                                       cudaDataType, size_t*, size_t*, int64_t) = nullptr;
+  cusolverStatus_t (*syev_batched)(cusolverDnHandle_t, cusolverDnParams_t, cusolverEigMode_t, cublasFillMode_t,
+                                   int64_t, cudaDataType, void*, int64_t, cudaDataType, void*, cudaDataType, void*,
+                                   size_t, void*, size_t, int*, int64_t) = nullptr;
+  bool batched = false;
   bool ok = false;
   std::string err;
 };
@@ -60,6 +70,11 @@ Cusolver& cusolver() {
     s.set_stream = (decltype(s.set_stream))dlsym(s.lib, "cusolverDnSetStream");
     s.syevd_buf = (decltype(s.syevd_buf))dlsym(s.lib, "cusolverDnDsyevd_bufferSize");
     s.syevd = (decltype(s.syevd))dlsym(s.lib, "cusolverDnDsyevd");
+    s.create_params = (decltype(s.create_params))dlsym(s.lib, "cusolverDnCreateParams");
+    s.destroy_params = (decltype(s.destroy_params))dlsym(s.lib, "cusolverDnDestroyParams");
+    s.syev_batched_buf = (decltype(s.syev_batched_buf))dlsym(s.lib, "cusolverDnXsyevBatched_bufferSize");
+    s.syev_batched = (decltype(s.syev_batched))dlsym(s.lib, "cusolverDnXsyevBatched");
+    s.batched = s.create_params && s.destroy_params && s.syev_batched_buf && s.syev_batched;
     s.ok = s.create && s.destroy && s.set_stream && s.syevd_buf && s.syevd;
     if (!s.ok) s.err = "libcusolver lacks the Dsyevd entry points";
     return s;
@@ -101,12 +116,10 @@ __device__ __forceinline__ void hat(const double* u, double* H) {  // column-maj
 
 // per-k outputs, 16 doubles each (column-major 4x4): offA (rotated first-row/column block), diagB (rotated diagonal
 // block), lam (the un-negated "current_block" of getLambdaGuess); terms[k] = theta-weighted contribution to mu
-__global__ void cert_blocks_kernel(const double* __restrict__ src, const double* __restrict__ dst,
-                                   const double* __restrict__ theta, int N, const double* __restrict__ Rcm,
-                                   const double* __restrict__ q_xyzw, double nbs, double* offA, double* diagB,
-                                   double* lam, double* mu_terms) {
-  const int k = blockIdx.x * blockDim.x + threadIdx.x;
-  if (k >= N) return;
+__device__ __forceinline__ void cert_block(int k, const double* __restrict__ src, const double* __restrict__ dst,
+                                           const double* __restrict__ theta, const double* __restrict__ Rcm,
+                                           const double* __restrict__ q_xyzw, double nbs, double* offA, double* diagB,
+                                           double* lam, double* mu_terms) {
   const double v1[3] = {src[3 * k], src[3 * k + 1], src[3 * k + 2]};
   const double v2[3] = {dst[3 * k], dst[3 * k + 1], dst[3 * k + 2]};
   // P_k = reshape(P' vec(v2 v1'), [4,4]) (column-major vec and reshape, :268-271)
@@ -183,9 +196,18 @@ __global__ void cert_blocks_kernel(const double* __restrict__ src, const double*
   for (int e = 0; e < 16; ++e) lam[16 * (size_t)k + e] = blk[e];
 }
 
+__global__ void cert_blocks_kernel(const double* __restrict__ src, const double* __restrict__ dst,
+                                   const double* __restrict__ theta, int N, const double* __restrict__ Rcm,
+                                   const double* __restrict__ q_xyzw, double nbs, double* offA, double* diagB,
+                                   double* lam, double* mu_terms) {
+  const int k = blockIdx.x * blockDim.x + threadIdx.x;
+  if (k >= N) return;
+  cert_block(k, src, dst, theta, Rcm, q_xyzw, nbs, offA, diagB, lam, mu_terms);
+}
+
 // one CTA: top[16] = sum_k lam_k, *mu = sum_k mu_terms[k] (k ascending per thread, then a fixed tree: deterministic)
-__global__ void __launch_bounds__(256) cert_reduce_kernel(const double* lam, const double* mu_terms, int N,
-                                                         double* top, double* mu) {
+__device__ __forceinline__ void cert_reduce_cta(const double* lam, const double* mu_terms, int N, double* top,
+                                                double* mu) {
   __shared__ double sh[256];
   for (int e = 0; e <= 16; ++e) {
     double s = 0;
@@ -204,13 +226,14 @@ __global__ void __launch_bounds__(256) cert_reduce_kernel(const double* lam, con
   }
 }
 
+__global__ void __launch_bounds__(256) cert_reduce_kernel(const double* lam, const double* mu_terms, int N,
+                                                         double* top, double* mu) {
+  cert_reduce_cta(lam, mu_terms, N, top, mu);
+}
+
 // M_init = Q_bar - mu J_bar - lambda_bar_init, one thread per entry
-__global__ void cert_fill_kernel(int N, const double* offA, const double* diagB, const double* lam, const double* top,
-                                 const double* mu, double* M_init) {
-  const int n = 4 * N + 4;
-  const long long e = blockIdx.x * (long long)blockDim.x + threadIdx.x;
-  if (e >= (long long)n * n) return;
-  const int r = (int)(e % n), c = (int)(e / n);
+__device__ __forceinline__ double cert_fill_value(int r, int c, const double* offA, const double* diagB,
+                                                  const double* lam, const double* top, const double* mu) {
   const int bi = r >> 2, bj = c >> 2, lr = r & 3, lc = c & 3;
   double v = 0;
   if (bi == 0 && bj == 0) {
@@ -222,7 +245,15 @@ __global__ void cert_fill_kernel(int N, const double* offA, const double* diagB,
   } else if (bi == bj) {
     v = diagB[16 * (size_t)(bi - 1) + lr + 4 * lc] + lam[16 * (size_t)(bi - 1) + lr + 4 * lc];  // lambda = -blk
   }
-  M_init[e] = v;
+  return v;
+}
+
+__global__ void cert_fill_kernel(int N, const double* offA, const double* diagB, const double* lam, const double* top,
+                                 const double* mu, double* M_init) {
+  const int n = 4 * N + 4;
+  const long long e = blockIdx.x * (long long)blockDim.x + threadIdx.x;
+  if (e >= (long long)n * n) return;
+  M_init[e] = cert_fill_value((int)(e % n), (int)(e / n), offA, diagB, lam, top, mu);
 }
 
 __global__ void sym_kernel(const double* __restrict__ M, int n, double* __restrict__ B) {
@@ -310,11 +341,12 @@ __device__ __forceinline__ long long pair_id(int i, int j, int N1) {  // N1 = N 
 
 #define WAT(r, c) W[(size_t)(c) * n + (r)]
 
+// The bodies below take the leading dimension n of W / Wd as an argument: 4N+4 for tzr_certify, the padded size of a
+// certify batch (cbt_* kernels further down).
 // bW[p][0..2] = -th_ij C + D - E + th_ij F (:349-368)
-__global__ void dual_bw_kernel(const double* __restrict__ W, const double* __restrict__ thp, int N,
-                               double* __restrict__ bW) {
-  const int n = 4 * N + 4, N1 = N + 1;
-  const int j = blockIdx.x * blockDim.x + threadIdx.x, i = blockIdx.y;
+__device__ __forceinline__ void dual_bw_at(const double* __restrict__ W, int n, const double* __restrict__ thp, int N,
+                                           int i, int j, double* __restrict__ bW) {
+  const int N1 = N + 1;
   if (i >= N || j <= i || j >= N1) return;
   const double tij = thp[i] * thp[j];
   const long long p = pair_id(i, j, N1);
@@ -325,11 +357,15 @@ __global__ void dual_bw_kernel(const double* __restrict__ W, const double* __res
   }
 }
 
+__global__ void dual_bw_kernel(const double* __restrict__ W, const double* __restrict__ thp, int N,
+                               double* __restrict__ bW) {
+  dual_bw_at(W, 4 * N + 4, thp, N, blockIdx.y, blockIdx.x * blockDim.x + threadIdx.x, bW);
+}
+
 // D[v][c] = Rs[v][c] - Cs[v][c]: Rs[v] = sum_{j>v} th_j B[v,j], Cs[v] = sum_{i<v} th_i B[i,v]   (one thread per (v,c))
-__global__ void dual_sums_kernel(const double* __restrict__ bW, const double* __restrict__ thp, int N,
-                                 double* __restrict__ D) {
+__device__ __forceinline__ void dual_sums_at(const double* __restrict__ bW, const double* __restrict__ thp, int N,
+                                             int t, double* __restrict__ D) {
   const int N1 = N + 1;
-  const int t = blockIdx.x * blockDim.x + threadIdx.x;
   if (t >= 3 * N1) return;
   const int v = t / 3, c = t % 3;
   double rs = 0, cs = 0;
@@ -338,12 +374,16 @@ __global__ void dual_sums_kernel(const double* __restrict__ bW, const double* __
   D[t] = rs - cs;
 }
 
+__global__ void dual_sums_kernel(const double* __restrict__ bW, const double* __restrict__ thp, int N,
+                                 double* __restrict__ D) {
+  dual_sums_at(bW, thp, N, blockIdx.x * blockDim.x + threadIdx.x, D);
+}
+
 // off-diagonal blocks of W_dual (both triangles) (:381-415), A_inv applied in closed form
-__global__ void dual_off_kernel(const double* __restrict__ W, const double* __restrict__ thp,
-                                const double* __restrict__ bW, const double* __restrict__ D, int N,
-                                double* __restrict__ Wd) {
-  const int n = 4 * N + 4, N1 = N + 1;
-  const int j = blockIdx.x * blockDim.x + threadIdx.x, i = blockIdx.y;
+__device__ __forceinline__ void dual_off_at(const double* __restrict__ W, int n, const double* __restrict__ thp,
+                                            const double* __restrict__ bW, const double* __restrict__ D, int N, int i,
+                                            int j, double* __restrict__ Wd) {
+  const int N1 = N + 1;
   if (i >= N || j <= i || j >= N1) return;
   const double y = 1.0 / (2.0 * N + 6.0), x = (N + 1.0) * y;
   const long long p = pair_id(i, j, N1);
@@ -364,11 +404,17 @@ __global__ void dual_off_kernel(const double* __restrict__ W, const double* __re
     }
 }
 
+__global__ void dual_off_kernel(const double* __restrict__ W, const double* __restrict__ thp,
+                                const double* __restrict__ bW, const double* __restrict__ D, int N,
+                                double* __restrict__ Wd) {
+  dual_off_at(W, 4 * N + 4, thp, bW, D, N, blockIdx.y, blockIdx.x * blockDim.x + threadIdx.x, Wd);
+}
+
 // diagonal blocks (:419-434): one warp per block row; then diag3[i][9] holds the 3x3 corner for the mean
-__global__ void dual_diag_kernel(const double* __restrict__ W, const double* __restrict__ thp, int N,
-                                 double* __restrict__ Wd, double* __restrict__ diag3) {
-  const int n = 4 * N + 4, N1 = N + 1;
-  const int i = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5), lane = threadIdx.x & 31;
+__device__ __forceinline__ void dual_diag_at(const double* __restrict__ W, int n, const double* __restrict__ thp,
+                                             int N, int i, int lane, double* __restrict__ Wd,
+                                             double* __restrict__ diag3) {
+  const int N1 = N + 1;
   if (i >= N1) return;
   double rs[4] = {0, 0, 0, 0};
   for (int j = lane; j < N1; j += 32) {
@@ -392,12 +438,18 @@ __global__ void dual_diag_kernel(const double* __restrict__ W, const double* __r
   }
 }
 
+__global__ void dual_diag_kernel(const double* __restrict__ W, const double* __restrict__ thp, int N,
+                                 double* __restrict__ Wd, double* __restrict__ diag3) {
+  dual_diag_at(W, 4 * N + 4, thp, N, blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5), threadIdx.x & 31, Wd,
+               diag3);
+}
+
 // one CTA: mean of the 3x3 corners, subtracted from every diagonal block (:435-445)
-__global__ void __launch_bounds__(256) dual_mean_kernel(const double* __restrict__ diag3, int N,
-                                                       double* __restrict__ Wd) {
+__device__ __forceinline__ void dual_mean_cta(const double* __restrict__ diag3, int n, int N,
+                                              double* __restrict__ Wd) {
   __shared__ double sh[256];
   __shared__ double mean[9];
-  const int n = 4 * N + 4, N1 = N + 1;
+  const int N1 = N + 1;
   for (int e = 0; e < 9; ++e) {
     double s = 0;
     for (int i = threadIdx.x; i < N1; i += 256) s += diag3[9 * (size_t)i + e];
@@ -416,6 +468,11 @@ __global__ void __launch_bounds__(256) dual_mean_kernel(const double* __restrict
   }
 }
 
+__global__ void __launch_bounds__(256) dual_mean_kernel(const double* __restrict__ diag3, int N,
+                                                       double* __restrict__ Wd) {
+  dual_mean_cta(diag3, 4 * N + 4, N, Wd);
+}
+
 __global__ void affine_out_kernel(const double* __restrict__ Minit, const double* __restrict__ Wd, long long nn,
                                   double* __restrict__ Maff) {
   const long long e = blockIdx.x * (long long)blockDim.x + threadIdx.x;
@@ -429,6 +486,249 @@ __global__ void update_kernel(double* __restrict__ M, const double* __restrict__
 }
 
 inline int grid1(long long items, int threads) { return (int)((items + threads - 1) / threads); }
+
+// ---- certify batch (tzr_certify_batch): B problems in one launch sequence ----------------------------------------
+// Every problem's matrices are nmax x nmax (nmax = 4 max N + 4 of the group), column-major, leading dimension nmax, at
+// b * nmax^2; the real block is the top-left n x n.  Per-measurement arrays lie back to back (first measurement k_off),
+// block-row arrays likewise (first block row v_off = k_off + b).  Every kernel skips problems whose active flag is 0.
+struct CertBatchProb {
+  int N, n;            // measurements, 4N + 4
+  int k_off, v_off;    // first measurement; first block row (thp, D, diag3)
+  long long p_off;     // first block pair of bW
+  int active;          // 1 while the iteration runs
+  int iters;           // iterations done (length of the trajectory)
+  int first_pos;       // first eigen column with a positive eigenvalue
+  int pad;
+  double mu, best;
+};
+
+// Eigenvalue of the pad block (the identity times it) of a padded problem: block diagonal, so the padded matrix has the
+// real block's eigenpairs plus (kCertPad, e_k) with e_k zero on the real rows; see DESIGN.md 3.9.
+constexpr double kCertPad = 1.0;
+
+__global__ void cbt_blocks_kernel(const CertBatchProb* __restrict__ pr, const double* __restrict__ src,
+                                  const double* __restrict__ dst, const double* __restrict__ theta,
+                                  const double* __restrict__ R, const double* __restrict__ q, double nbs, double* offA,
+                                  double* diagB, double* lam, double* mu_terms) {
+  const CertBatchProb p = pr[blockIdx.y];
+  const int k = blockIdx.x * blockDim.x + threadIdx.x;
+  if (k >= p.N) return;
+  const size_t o = p.k_off;
+  cert_block(k, src + 3 * o, dst + 3 * o, theta + o, R + 9 * blockIdx.y, q + 4 * blockIdx.y, nbs, offA + 16 * o,
+             diagB + 16 * o, lam + 16 * o, mu_terms + o);
+}
+
+__global__ void __launch_bounds__(256) cbt_reduce_kernel(CertBatchProb* pr, const double* lam,
+                                                        const double* mu_terms, double* top) {
+  const int b = blockIdx.x;
+  const size_t o = pr[b].k_off;
+  __shared__ double mu;
+  cert_reduce_cta(lam + 16 * o, mu_terms + o, pr[b].N, top + 16 * b, &mu);
+  if (threadIdx.x == 0) pr[b].mu = mu;
+}
+
+// M_init of every problem; the pad region is zero
+__global__ void cbt_fill_kernel(const CertBatchProb* __restrict__ pr, int nmax, const double* offA,
+                                const double* diagB, const double* lam, const double* top, double* M_init) {
+  const int b = blockIdx.y;
+  const long long e = blockIdx.x * (long long)blockDim.x + threadIdx.x;
+  if (e >= (long long)nmax * nmax) return;
+  const CertBatchProb& p = pr[b];
+  const int r = (int)(e % nmax), c = (int)(e / nmax);
+  const size_t o = p.k_off;
+  M_init[(size_t)b * nmax * nmax + e] =
+      (r < p.n && c < p.n) ? cert_fill_value(r, c, offA + 16 * o, diagB + 16 * o, lam + 16 * o, top + 16 * b, &p.mu)
+                           : 0.0;
+}
+
+// B = (M + M^T) / 2 on the real block, kCertPad * I on the pad block
+__global__ void cbt_sym_kernel(const CertBatchProb* __restrict__ pr, int nmax, const double* __restrict__ M,
+                               double* __restrict__ Bm) {
+  const int b = blockIdx.y;
+  const long long e = blockIdx.x * (long long)blockDim.x + threadIdx.x;
+  if (e >= (long long)nmax * nmax || !pr[b].active) return;
+  const int n = pr[b].n;
+  const int r = (int)(e % nmax), c = (int)(e / nmax);
+  const size_t base = (size_t)b * nmax * nmax;
+  Bm[base + e] = (r < n && c < n) ? (M[base + e] + M[base + (size_t)r * nmax + c]) / 2 : (r == c ? kCertPad : 0.0);
+}
+
+// first eigen column with w > 0 (w ascending); ne_full: the eigensolver ran on the padded nmax (else on n)
+__global__ void cbt_first_pos_kernel(CertBatchProb* pr, int B, int nmax, int ne_full, const double* __restrict__ w) {
+  const int b = blockIdx.x * blockDim.x + threadIdx.x;
+  if (b >= B || !pr[b].active) return;
+  const double* wb = w + (size_t)b * nmax;
+  int lo = 0, hi = ne_full ? nmax : pr[b].n;
+  while (lo < hi) {
+    const int mid = (lo + hi) >> 1;
+    if (wb[mid] > 0) hi = mid;
+    else lo = mid + 1;
+  }
+  pr[b].first_pos = lo;
+}
+
+// C = V[:, k0:ne] diag(w[k0:ne]) V[:, k0:ne]^T on the real block, FP64 tensor cores (DMMA, mma.sync m8n8k4).  64 x 64
+// output tile per CTA, 8 warps of 32 x 16 (4 x 2 MMA tiles); k in slabs of 16 staged in shared memory, the eigenvalue
+// scaling applied to the A operand on the way in.  Row pitch 68 doubles: the fragment loads (row = k, 8 consecutive
+// columns per k) are conflict-free in each half-warp.
+constexpr int kPT = 64, kPK = 16, kPS = kPT + 4;
+__device__ __forceinline__ void dmma_m8n8k4(double& d0, double& d1, double a, double b) {
+  asm volatile("mma.sync.aligned.m8n8k4.row.col.f64.f64.f64.f64 {%0, %1}, {%2}, {%3}, {%0, %1};\n"
+               : "+d"(d0), "+d"(d1)
+               : "d"(a), "d"(b));
+}
+
+__global__ void __launch_bounds__(256) cbt_psd_kernel(const CertBatchProb* __restrict__ pr, int nmax, int ne_full,
+                                                     const double* __restrict__ V, const double* __restrict__ w,
+                                                     double* __restrict__ C) {
+  __shared__ double As[kPK][kPS], Bs[kPK][kPS];
+  const int b = blockIdx.z;
+  const int n = pr[b].n, r0 = blockIdx.x * kPT, c0 = blockIdx.y * kPT;
+  if (!pr[b].active || r0 >= n || c0 >= n) return;
+  const int ne = ne_full ? nmax : n, k0 = pr[b].first_pos;
+  const size_t base = (size_t)b * nmax * nmax;
+  V += base;
+  C += base;
+  w += (size_t)b * nmax;
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, gid = lane >> 2, tig = lane & 3;
+  const int wr = (warp & 1) * 32, wc = (warp >> 1) * 16;
+  double acc[4][2][2];
+#pragma unroll
+  for (int i = 0; i < 4; ++i)
+#pragma unroll
+    for (int j = 0; j < 2; ++j) acc[i][j][0] = acc[i][j][1] = 0;
+  for (int kb = k0; kb < ne; kb += kPK) {
+    for (int e = threadIdx.x; e < kPK * kPT; e += 256) {
+      const int kk = e / kPT, i = e % kPT;
+      const int k = kb + kk;
+      const double wk = k < ne ? w[k] : 0.0;
+      As[kk][i] = (k < ne && r0 + i < n && wk > 0) ? V[(size_t)k * nmax + r0 + i] * wk : 0.0;
+      Bs[kk][i] = (k < ne && c0 + i < n) ? V[(size_t)k * nmax + c0 + i] : 0.0;
+    }
+    __syncthreads();
+#pragma unroll
+    for (int kk = 0; kk < kPK; kk += 4) {
+      double a[4], bb[2];
+#pragma unroll
+      for (int i = 0; i < 4; ++i) a[i] = As[kk + tig][wr + 8 * i + gid];
+#pragma unroll
+      for (int j = 0; j < 2; ++j) bb[j] = Bs[kk + tig][wc + 8 * j + gid];
+#pragma unroll
+      for (int i = 0; i < 4; ++i)
+#pragma unroll
+        for (int j = 0; j < 2; ++j) dmma_m8n8k4(acc[i][j][0], acc[i][j][1], a[i], bb[j]);
+    }
+    __syncthreads();
+  }
+#pragma unroll
+  for (int i = 0; i < 4; ++i)
+#pragma unroll
+    for (int j = 0; j < 2; ++j)
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const int r = r0 + wr + 8 * i + gid, c = c0 + wc + 8 * j + 2 * tig + h;
+        if (r < n && c < n) C[(size_t)c * nmax + r] = acc[i][j][h];
+      }
+}
+
+// op 0: W = 2 Mpsd - M - Minit (affine-in), 1: Maff = Minit + Wd (affine-out), 2: M += gamma_tau (Maff - Mpsd)
+// (update); real block of every active problem
+__global__ void cbt_affine_kernel(const CertBatchProb* __restrict__ pr, int nmax, int op, const double* __restrict__ X,
+                                  const double* __restrict__ Y, double* __restrict__ Z, const double* __restrict__ Minit,
+                                  double gamma_tau) {
+  const int b = blockIdx.y;
+  const long long e = blockIdx.x * (long long)blockDim.x + threadIdx.x;
+  if (e >= (long long)nmax * nmax || !pr[b].active) return;
+  const int n = pr[b].n;
+  if ((int)(e % nmax) >= n || (int)(e / nmax) >= n) return;
+  const size_t i = (size_t)b * nmax * nmax + e;
+  if (op == 0) Z[i] = 2 * X[i] - Y[i] - Minit[i];
+  else if (op == 1) Z[i] = Minit[i] + X[i];
+  else Z[i] += gamma_tau * (X[i] - Y[i]);
+}
+
+__global__ void cbt_dual_bw_kernel(const CertBatchProb* __restrict__ pr, int nmax, const double* __restrict__ W,
+                                   const double* __restrict__ thp, double* __restrict__ bW) {
+  const CertBatchProb& p = pr[blockIdx.z];
+  if (!p.active) return;
+  dual_bw_at(W + (size_t)blockIdx.z * nmax * nmax, nmax, thp + p.v_off, p.N, blockIdx.y,
+             blockIdx.x * blockDim.x + threadIdx.x, bW + 3 * p.p_off);
+}
+
+__global__ void cbt_dual_sums_kernel(const CertBatchProb* __restrict__ pr, const double* __restrict__ bW,
+                                     const double* __restrict__ thp, double* __restrict__ D) {
+  const CertBatchProb& p = pr[blockIdx.y];
+  if (!p.active) return;
+  dual_sums_at(bW + 3 * p.p_off, thp + p.v_off, p.N, blockIdx.x * blockDim.x + threadIdx.x, D + 3 * (size_t)p.v_off);
+}
+
+__global__ void cbt_dual_off_kernel(const CertBatchProb* __restrict__ pr, int nmax, const double* __restrict__ W,
+                                    const double* __restrict__ thp, const double* __restrict__ bW,
+                                    const double* __restrict__ D, double* __restrict__ Wd) {
+  const CertBatchProb& p = pr[blockIdx.z];
+  if (!p.active) return;
+  const size_t base = (size_t)blockIdx.z * nmax * nmax;
+  dual_off_at(W + base, nmax, thp + p.v_off, bW + 3 * p.p_off, D + 3 * (size_t)p.v_off, p.N, blockIdx.y,
+              blockIdx.x * blockDim.x + threadIdx.x, Wd + base);
+}
+
+__global__ void cbt_dual_diag_kernel(const CertBatchProb* __restrict__ pr, int nmax, const double* __restrict__ W,
+                                     const double* __restrict__ thp, double* __restrict__ Wd,
+                                     double* __restrict__ diag3) {
+  const CertBatchProb& p = pr[blockIdx.y];
+  if (!p.active) return;
+  const size_t base = (size_t)blockIdx.y * nmax * nmax;
+  dual_diag_at(W + base, nmax, thp + p.v_off, p.N, blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5),
+               threadIdx.x & 31, Wd + base, diag3 + 9 * (size_t)p.v_off);
+}
+
+__global__ void __launch_bounds__(256) cbt_dual_mean_kernel(const CertBatchProb* __restrict__ pr, int nmax,
+                                                           const double* __restrict__ diag3, double* __restrict__ Wd) {
+  const CertBatchProb& p = pr[blockIdx.x];
+  if (!p.active) return;
+  dual_mean_cta(diag3 + 9 * (size_t)p.v_off, nmax, p.N, Wd + (size_t)blockIdx.x * nmax * nmax);
+}
+
+// Compact batch of the eigensolver once some problems have finished: slot s holds problem idx[s].  Gather copies the
+// matrices into the compact buffer; scatter copies back the eigenvalues, info and (vectors = 1) the eigenvectors.
+__global__ void cbt_gather_kernel(const int* __restrict__ idx, int nmax, const double* __restrict__ Bm,
+                                  double* __restrict__ Bc) {
+  const long long nn = (long long)nmax * nmax, e = blockIdx.x * (long long)blockDim.x + threadIdx.x;
+  if (e < nn) Bc[blockIdx.y * nn + e] = Bm[idx[blockIdx.y] * nn + e];
+}
+
+__global__ void cbt_scatter_kernel(const int* __restrict__ idx, int nmax, int vectors, const double* __restrict__ Bc,
+                                   const double* __restrict__ wc, const int* __restrict__ infoc, double* __restrict__ Bm,
+                                   double* __restrict__ w, int* __restrict__ info) {
+  const int s = blockIdx.y, b = idx[s];
+  const long long nn = (long long)nmax * nmax, e = blockIdx.x * (long long)blockDim.x + threadIdx.x;
+  if (vectors && e < nn) Bm[b * nn + e] = Bc[s * nn + e];
+  if (e < nmax) w[(size_t)b * nmax + e] = wc[(size_t)s * nmax + e];
+  if (e == 0) info[b] = infoc[s];
+}
+
+// certify_device's gap rule per active problem (info != 0 -> inf, min_eig > 0 -> 0, else -min_eig (N+1) / mu), the
+// trajectory entry, the best gap, and the stop rule (gap < sub_optimality or the iteration cap); active_out: the flags
+__global__ void cbt_gap_kernel(CertBatchProb* pr, int B, int nmax, const double* __restrict__ w,
+                               const int* __restrict__ info, int iter, double sub_optimality, double max_iterations,
+                               double* traj, int traj_cap, int* active_out) {
+  const int b = blockIdx.x * blockDim.x + threadIdx.x;
+  if (b >= B) return;
+  CertBatchProb& p = pr[b];
+  if (p.active) {
+    const double min_eig = w[(size_t)b * nmax];  // ascending: w[0] is the minimum
+    double gap;
+    if (info[b] != 0) gap = INFINITY;
+    else if (min_eig > 0) gap = 0;
+    else gap = (-min_eig * (p.N + 1)) / p.mu;
+    if (iter < traj_cap) traj[(size_t)b * traj_cap + iter] = gap;
+    p.iters = iter + 1;
+    if (gap < p.best) p.best = gap;
+    if (gap < sub_optimality || (double)(iter + 1) >= max_iterations) p.active = 0;
+  }
+  active_out[b] = p.active;
+}
+
 
 }  // namespace
 
@@ -489,6 +789,37 @@ static int launch_dual_projection(const CertWork& w, int N, cudaStream_t st) {
   return 5;
 }
 
+// quaternion of R (Eigen::Quaterniond(R).normalize(), :66-69) on the host: 20 flops
+static void quaternion_xyzw(const double* R_cm, double q[4]) {
+  const double* R = R_cm;  // column-major: R(r,c) = R[r + 3c]
+  auto Rm = [&](int r, int c) { return R[r + 3 * c]; };
+  const double t = Rm(0, 0) + Rm(1, 1) + Rm(2, 2);
+  double x, y, z, ww;
+  if (t > 0) {
+    double s = std::sqrt(t + 1.0);
+    ww = 0.5 * s;
+    s = 0.5 / s;
+    x = (Rm(2, 1) - Rm(1, 2)) * s;
+    y = (Rm(0, 2) - Rm(2, 0)) * s;
+    z = (Rm(1, 0) - Rm(0, 1)) * s;
+  } else {
+    int i = 0;
+    if (Rm(1, 1) > Rm(0, 0)) i = 1;
+    if (Rm(2, 2) > Rm(i, i)) i = 2;
+    const int j = (i + 1) % 3, k = (i + 2) % 3;
+    double s = std::sqrt(Rm(i, i) - Rm(j, j) - Rm(k, k) + 1.0);
+    double v[3];
+    v[i] = 0.5 * s;
+    s = 0.5 / s;
+    ww = (Rm(k, j) - Rm(j, k)) * s;
+    v[j] = (Rm(j, i) + Rm(i, j)) * s;
+    v[k] = (Rm(k, i) + Rm(i, k)) * s;
+    x = v[0]; y = v[1]; z = v[2];
+  }
+  const double nrm = std::sqrt(x * x + y * y + z * z + ww * ww);
+  q[0] = x / nrm; q[1] = y / nrm; q[2] = z / nrm; q[3] = ww / nrm;
+}
+
 // Returns TZR_OK or a negative status; err receives a message.  All pointers host.  mode: 0 full certify,
 // 1 initial matrix only (M_init_out n*n, mu_out), 2 dual projection only (W_in n*n -> Wd_out n*n; theta = N values).
 int certify_device(int mode, double noise_bound, double cbar2, double sub_optimality, double max_iterations,
@@ -541,37 +872,8 @@ int certify_device(int mode, double noise_bound, double cbar2, double sub_optima
     if (cudaStreamSynchronize(st) != cudaSuccess) return TZR_ERR_CUDA;
     return TZR_OK;
   }
-  // quaternion of R (Eigen::Quaterniond(R).normalize(), :66-69) on the host: 20 flops
   double q[4];
-  {
-    const double* R = R_cm;  // column-major: R(r,c) = R[r + 3c]
-    auto Rm = [&](int r, int c) { return R[r + 3 * c]; };
-    const double t = Rm(0, 0) + Rm(1, 1) + Rm(2, 2);
-    double x, y, z, ww;
-    if (t > 0) {
-      double s = std::sqrt(t + 1.0);
-      ww = 0.5 * s;
-      s = 0.5 / s;
-      x = (Rm(2, 1) - Rm(1, 2)) * s;
-      y = (Rm(0, 2) - Rm(2, 0)) * s;
-      z = (Rm(1, 0) - Rm(0, 1)) * s;
-    } else {
-      int i = 0;
-      if (Rm(1, 1) > Rm(0, 0)) i = 1;
-      if (Rm(2, 2) > Rm(i, i)) i = 2;
-      const int j = (i + 1) % 3, k = (i + 2) % 3;
-      double s = std::sqrt(Rm(i, i) - Rm(j, j) - Rm(k, k) + 1.0);
-      double v[3];
-      v[i] = 0.5 * s;
-      s = 0.5 / s;
-      ww = (Rm(k, j) - Rm(j, k)) * s;
-      v[j] = (Rm(j, i) + Rm(i, j)) * s;
-      v[k] = (Rm(k, i) + Rm(i, k)) * s;
-      x = v[0]; y = v[1]; z = v[2];
-    }
-    const double nrm = std::sqrt(x * x + y * y + z * z + ww * ww);
-    q[0] = x / nrm; q[1] = y / nrm; q[2] = z / nrm; q[3] = ww / nrm;
-  }
+  quaternion_xyzw(R_cm, q);
   cudaMemcpyAsync(w.src, src, 3 * (size_t)N * sizeof(double), cudaMemcpyHostToDevice, st);
   cudaMemcpyAsync(w.dst, dst, 3 * (size_t)N * sizeof(double), cudaMemcpyHostToDevice, st);
   cudaMemcpyAsync(w.theta, theta, (size_t)N * sizeof(double), cudaMemcpyHostToDevice, st);
@@ -643,6 +945,315 @@ int certify_device(int mode, double noise_bound, double cbar2, double sub_optima
   *best_subopt = best;
   *n_iters = iters;
   if (cudaStreamSynchronize(st) != cudaSuccess) return TZR_ERR_CUDA;
+  return TZR_OK;
+}
+
+// ---- tzr_certify_batch ---------------------------------------------------------------------------------------------
+// Fewest active problems for which an eigen step takes cusolverDnXsyevBatched; below, one cusolverDnDsyevd per active
+// problem.  The batched call has a large fixed cost: per DRS iteration (two eigen steps) 12-16 ms at n = 204 for 16
+// and for 64 problems, against 3.4 ms per problem on Dsyevd; 45 ms for 16 at n = 404 (7.3 per problem), 140 ms for 16
+// at n = 1004 (21 per problem).  That puts the crossover at about 5-7 problems; at 8 the batched call was faster at
+// every measured size (DESIGN.md 3.9).
+constexpr int kCertBatchedMinActive = 8;
+
+namespace {
+struct CertBatchWork {
+  double *src, *dst, *theta, *thp, *R, *q, *offA, *diagB, *lam, *mu_terms, *top, *bW, *D, *diag3, *w;
+  double *M_init, *M, *Bm, *M_psd, *W, *Wd, *M_aff, *traj, *wc;
+  CertBatchProb* pr;
+  int *info, *active, *infoc, *idx;
+  void* work;
+};
+
+// Device bytes of a group of G problems with K measurements, P block pairs, padded size nmax and T trajectory columns,
+// plus `work` bytes of eigensolver workspace; carve() of the same arguments lays them out.
+size_t cbt_carve(void* base, int G, long long K, long long P, int nmax, int T, size_t work, CertBatchWork* out) {
+  char* p = (char*)base;
+  auto take = [&](size_t bytes) {
+    void* r = p;
+    p += (bytes + 255) / 256 * 256;
+    return r;
+  };
+  const size_t V = (size_t)K + G, nn = (size_t)nmax * nmax, d = sizeof(double);
+  CertBatchWork w;
+  w.src = (double*)take(3 * K * d); w.dst = (double*)take(3 * K * d); w.theta = (double*)take(K * d);
+  w.thp = (double*)take(V * d); w.R = (double*)take(9 * (size_t)G * d); w.q = (double*)take(4 * (size_t)G * d);
+  w.offA = (double*)take(16 * K * d); w.diagB = (double*)take(16 * K * d); w.lam = (double*)take(16 * K * d);
+  w.mu_terms = (double*)take(K * d); w.top = (double*)take(16 * (size_t)G * d);
+  w.bW = (double*)take(3 * (size_t)P * d); w.D = (double*)take(3 * V * d); w.diag3 = (double*)take(9 * V * d);
+  w.w = (double*)take((size_t)G * nmax * d);
+  w.M_init = (double*)take(G * nn * d); w.M = (double*)take(G * nn * d); w.Bm = (double*)take(G * nn * d);
+  w.M_psd = (double*)take(G * nn * d); w.W = (double*)take(G * nn * d); w.Wd = (double*)take(G * nn * d);
+  w.M_aff = (double*)take(G * nn * d); w.traj = (double*)take((size_t)G * T * d);
+  w.pr = (CertBatchProb*)take(G * sizeof(CertBatchProb));
+  w.info = (int*)take(G * sizeof(int)); w.active = (int*)take(G * sizeof(int));
+  w.wc = (double*)take((size_t)G * nmax * d); w.infoc = (int*)take(G * sizeof(int)); w.idx = (int*)take(G * sizeof(int));
+  w.work = take(work);
+  if (out) *out = w;
+  return (size_t)(p - (char*)base);
+}
+}  // namespace
+
+int certify_batch_device(const tzr_certifier_params& prm, int B, const int32_t* N, const double* R_cm,
+                         const double* const* src, const double* const* dst, const double* const* theta,
+                         tzr_certification_result* results, double* const* traj, const int32_t* traj_cap,
+                         bool loop_eig, void** scratch, size_t* scratch_cap, void** solver_handle, int64_t* launches,
+                         cudaStream_t st, std::string* err) {
+  int nmax_all = 0;
+  for (int b = 0; b < B; ++b) {
+    if (4 * (size_t)N[b] + 4 > 32768) {
+      *err = "problem " + std::to_string(b) + ": 4N+4 = " + std::to_string(4 * (size_t)N[b] + 4) + " exceeds 32768";
+      return TZR_ERR_TOO_LARGE;
+    }
+    nmax_all = std::max(nmax_all, 4 * N[b] + 4);
+  }
+  Cusolver& cs = cusolver();
+  if (!cs.ok) {
+    *err = cs.err;
+    return TZR_ERR_UNSUPPORTED;
+  }
+  cusolverDnHandle_t& handle = *reinterpret_cast<cusolverDnHandle_t*>(solver_handle);  // owned by the context
+  if (!handle && cs.create(&handle) != CUSOLVER_STATUS_SUCCESS) {
+    *err = "cusolverDnCreate failed";
+    return TZR_ERR_CUDA;
+  }
+  cs.set_stream(handle, st);
+  cusolverDnParams_t sp = nullptr;
+  bool batched = !loop_eig && cs.batched && B > 1 && cs.create_params(&sp) == CUSOLVER_STATUS_SUCCESS;
+  struct ParamsGuard {
+    Cusolver& cs;
+    cusolverDnParams_t& p;
+    ~ParamsGuard() { if (p) cs.destroy_params(p); }
+  } guard{cs, sp};
+  // eigensolver workspace of `G` problems padded to `nmax`: (device bytes, host bytes); {0, 0} when the batched call
+  // refuses the size
+  auto batched_ws = [&](int nmax, int G, size_t* host) -> size_t {
+    size_t dmax = 0, hmax = 0;
+    for (cusolverEigMode_t jobz : {CUSOLVER_EIG_MODE_VECTOR, CUSOLVER_EIG_MODE_NOVECTOR}) {
+      size_t dv = 0, hv = 0;
+      if (cs.syev_batched_buf(handle, sp, jobz, CUBLAS_FILL_MODE_LOWER, nmax, CUDA_R_64F, nullptr, nmax, CUDA_R_64F,
+                              nullptr, CUDA_R_64F, &dv, &hv, G) != CUSOLVER_STATUS_SUCCESS)
+        return 0;
+      dmax = std::max(dmax, dv);
+      hmax = std::max(hmax, hv);
+    }
+    *host = hmax;
+    return std::max<size_t>(dmax, 1);
+  };
+  auto syevd_ws = [&](int nmax) -> size_t {
+    int lwork = 0;
+    if (cs.syevd_buf(handle, CUSOLVER_EIG_MODE_VECTOR, CUBLAS_FILL_MODE_LOWER, nmax, nullptr, nmax, nullptr, &lwork) !=
+        CUSOLVER_STATUS_SUCCESS)
+      return 0;
+    return (size_t)lwork * sizeof(double);
+  };
+  const size_t loop_ws_all = syevd_ws(nmax_all);
+  if (!loop_ws_all) {
+    *err = "cusolverDnDsyevd_bufferSize failed";
+    return TZR_ERR_CUDA;
+  }
+  size_t host_ws = 0;
+  const size_t ws1 = batched ? batched_ws(nmax_all, 1, &host_ws) : 0;
+  if (batched && !ws1) batched = false;  // the batched call refuses nmax: loop route
+  // trajectory columns kept on the device: what the caller can receive, at most the iteration cap
+  const double maxit = prm.max_iterations;
+  int T = 0;
+  for (int b = 0; traj && traj_cap && b < B; ++b)
+    if (traj[b]) T = std::max(T, (int)traj_cap[b]);
+  T = (int)std::min<double>(T, std::max(0.0, std::ceil(maxit)));
+  size_t fr = 0, tot = 0;
+  cudaMemGetInfo(&fr, &tot);
+  const size_t budget = (size_t)(0.9 * (double)(fr + *scratch_cap));
+  const double nbs = prm.cbar2 * prm.noise_bound * prm.noise_bound;
+
+  // groups of consecutive problems that fit the device, each run to completion in one launch sequence
+  for (int b0 = 0; b0 < B;) {
+    int b1 = b0, nmax = 0;
+    long long K = 0, P = 0;
+    size_t need = 0;
+    while (b1 < B && b1 - b0 < 65535) {
+      const int nm2 = std::max(nmax, 4 * N[b1] + 4), G2 = b1 - b0 + 1;
+      const long long K2 = K + N[b1], P2 = P + (long long)N[b1] * (N[b1] + 1) / 2;
+      const size_t ws = std::max(loop_ws_all, batched ? ws1 * (size_t)G2 : 0);
+      const size_t need2 = cbt_carve(nullptr, G2, K2, P2, nm2, T, ws, nullptr);
+      if (need2 > budget && b1 > b0) break;
+      if (need2 > budget) {
+        *err = "the certifier batch workspace of " + std::to_string(need2) + " bytes (one problem, 4N+4 = " +
+               std::to_string(nm2) + ") does not fit the device";
+        return TZR_ERR_ALLOC;
+      }
+      nmax = nm2; K = K2; P = P2; need = need2;
+      ++b1;
+    }
+    // The estimate above scales the one-problem workspace; the group's own query decides.  Halve the group until the
+    // workspace it really needs fits.
+    bool bat = false;
+    size_t hws = 0, dws = 0, lwork_bytes = 0;
+    for (;;) {
+      bat = batched && b1 - b0 >= kCertBatchedMinActive;
+      hws = dws = 0;
+      if (bat) {
+        dws = batched_ws(nmax, b1 - b0, &hws);
+        if (!dws) bat = false;
+      }
+      lwork_bytes = syevd_ws(nmax);
+      need = cbt_carve(nullptr, b1 - b0, K, P, nmax, T, std::max(dws, lwork_bytes), nullptr);
+      if (need <= budget || b1 - b0 == 1) break;
+      b1 = b0 + (b1 - b0) / 2;
+      nmax = 0; K = 0; P = 0;
+      for (int b = b0; b < b1; ++b) {
+        nmax = std::max(nmax, 4 * N[b] + 4);
+        K += N[b];
+        P += (long long)N[b] * (N[b] + 1) / 2;
+      }
+    }
+    const int G = b1 - b0;
+    if (need > *scratch_cap) {
+      if (*scratch) cudaFree(*scratch);
+      *scratch = nullptr;
+      *scratch_cap = 0;
+      if (cudaMalloc(scratch, need) != cudaSuccess) {
+        cudaGetLastError();
+        *err = "cudaMalloc of " + std::to_string(need) + " bytes for the certifier batch failed";
+        return TZR_ERR_ALLOC;
+      }
+      *scratch_cap = need;
+    }
+    CertBatchWork w;
+    cbt_carve(*scratch, G, K, P, nmax, T, std::max(dws, lwork_bytes), &w);
+    std::vector<char> host_work(std::max<size_t>(hws, 1));
+    // host tables
+    std::vector<CertBatchProb> tab(G);
+    std::vector<double> h_src(3 * K), h_dst(3 * K), h_th(K), h_thp(K + G), h_R(9 * (size_t)G), h_q(4 * (size_t)G);
+    int maxN = 0;
+    for (int g = 0, k = 0; g < G; ++g) {
+      const int b = b0 + g, Nb = N[b];
+      CertBatchProb& t = tab[g];
+      t.N = Nb; t.n = 4 * Nb + 4; t.k_off = k; t.v_off = k + g;
+      t.p_off = g ? tab[g - 1].p_off + (long long)tab[g - 1].N * (tab[g - 1].N + 1) / 2 : 0;
+      t.active = 1; t.iters = 0; t.first_pos = 0; t.pad = 0; t.mu = 0; t.best = INFINITY;
+      std::copy(src[b], src[b] + 3 * (size_t)Nb, h_src.begin() + 3 * (size_t)k);
+      std::copy(dst[b], dst[b] + 3 * (size_t)Nb, h_dst.begin() + 3 * (size_t)k);
+      std::copy(theta[b], theta[b] + Nb, h_th.begin() + k);
+      h_thp[k + g] = 1.0;
+      std::copy(theta[b], theta[b] + Nb, h_thp.begin() + k + g + 1);
+      std::copy(R_cm + 9 * (size_t)b, R_cm + 9 * (size_t)b + 9, h_R.begin() + 9 * (size_t)g);
+      quaternion_xyzw(R_cm + 9 * (size_t)b, &h_q[4 * (size_t)g]);
+      maxN = std::max(maxN, Nb);
+      k += Nb;
+    }
+    cudaMemcpyAsync(w.src, h_src.data(), h_src.size() * sizeof(double), cudaMemcpyHostToDevice, st);
+    cudaMemcpyAsync(w.dst, h_dst.data(), h_dst.size() * sizeof(double), cudaMemcpyHostToDevice, st);
+    cudaMemcpyAsync(w.theta, h_th.data(), h_th.size() * sizeof(double), cudaMemcpyHostToDevice, st);
+    cudaMemcpyAsync(w.thp, h_thp.data(), h_thp.size() * sizeof(double), cudaMemcpyHostToDevice, st);
+    cudaMemcpyAsync(w.R, h_R.data(), h_R.size() * sizeof(double), cudaMemcpyHostToDevice, st);
+    cudaMemcpyAsync(w.q, h_q.data(), h_q.size() * sizeof(double), cudaMemcpyHostToDevice, st);
+    cudaMemcpyAsync(w.pr, tab.data(), G * sizeof(CertBatchProb), cudaMemcpyHostToDevice, st);
+    const long long nn = (long long)nmax * nmax;
+    const dim3 ge(grid1(nn, 256), G), gp(grid1(maxN + 1, 128), maxN, G), gt((nmax + kPT - 1) / kPT, (nmax + kPT - 1) / kPT, G);
+    cbt_blocks_kernel<<<dim3(grid1(maxN, 128), G), 128, 0, st>>>(w.pr, w.src, w.dst, w.theta, w.R, w.q, nbs, w.offA,
+                                                                  w.diagB, w.lam, w.mu_terms);
+    cbt_reduce_kernel<<<G, 256, 0, st>>>(w.pr, w.lam, w.mu_terms, w.top);
+    cbt_fill_kernel<<<ge, 256, 0, st>>>(w.pr, nmax, w.offA, w.diagB, w.lam, w.top, w.M_init);
+    *launches += 3;
+    cudaMemcpyAsync(w.M, w.M_init, (size_t)G * nn * sizeof(double), cudaMemcpyDeviceToDevice, st);
+    std::vector<int> act(G, 1), idx;  // active flags of the last read-back; their indices (compact batch)
+    int n_act = G, idx_for = -1;         // idx_for: the n_act whose idx is on the device
+    bool full_step = bat;                // the step's eigen columns cover nmax (batched call) or n (Dsyevd)
+    // one eigendecomposition of every active problem's Bm, and nothing for the finished ones: the batched call over the
+    // padded matrices (in place while every problem is active, else over the active ones gathered into W, which is dead
+    // at both eigen steps) while at least kCertBatchedMinActive are active, else cusolverDnDsyevd on each active real
+    // block.  If the batched call
+    // refuses, the Dsyevd loop serves the rest of the call.  Every eigensolver call counts as one launch.
+    auto eig = [&](cusolverEigMode_t jobz) -> int {
+      full_step = bat && n_act >= kCertBatchedMinActive;
+      if (full_step) {
+        size_t dws_a = dws, hws_a = hws;
+        if (n_act < G) {
+          dws_a = batched_ws(nmax, n_act, &hws_a);
+          if (idx_for != n_act) {
+            idx.clear();
+            for (int g = 0; g < G; ++g)
+              if (act[g]) idx.push_back(g);
+            cudaMemcpyAsync(w.idx, idx.data(), n_act * sizeof(int), cudaMemcpyHostToDevice, st);
+            idx_for = n_act;
+          }
+        }
+        if (dws_a && dws_a <= dws && hws_a <= hws) {
+          const bool all = n_act == G;
+          const dim3 gc(grid1(nn, 256), n_act);
+          if (!all) cbt_gather_kernel<<<gc, 256, 0, st>>>(w.idx, nmax, w.Bm, w.W);
+          if (cs.syev_batched(handle, sp, jobz, CUBLAS_FILL_MODE_LOWER, nmax, CUDA_R_64F, all ? w.Bm : w.W, nmax,
+                              CUDA_R_64F, all ? w.w : w.wc, CUDA_R_64F, w.work, dws_a, host_work.data(), hws_a,
+                              all ? w.info : w.infoc, n_act) == CUSOLVER_STATUS_SUCCESS) {
+            if (!all)
+              cbt_scatter_kernel<<<gc, 256, 0, st>>>(w.idx, nmax, jobz == CUSOLVER_EIG_MODE_VECTOR ? 1 : 0, w.W, w.wc,
+                                                     w.infoc, w.Bm, w.w, w.info);
+            *launches += all ? 1 : 3;
+            return TZR_OK;
+          }
+          if (!all) *launches += 1;
+        }
+        bat = full_step = false;
+      }
+      for (int g = 0; g < G; ++g) {
+        if (!act[g]) continue;
+        if (cs.syevd(handle, jobz, CUBLAS_FILL_MODE_LOWER, tab[g].n, w.Bm + (size_t)g * nn, nmax,
+                     w.w + (size_t)g * nmax, (double*)w.work, (int)(lwork_bytes / sizeof(double)),
+                     w.info + g) != CUSOLVER_STATUS_SUCCESS) {
+          *err = "cusolverDnDsyevd failed";
+          return TZR_ERR_CUDA;
+        }
+        *launches += 1;
+      }
+      return TZR_OK;
+    };
+    for (int iter = 0; (double)iter < maxit; ++iter) {
+      cbt_sym_kernel<<<ge, 256, 0, st>>>(w.pr, nmax, w.M, w.Bm);
+      if (int rc = eig(CUSOLVER_EIG_MODE_VECTOR)) return rc;
+      cbt_first_pos_kernel<<<grid1(G, 128), 128, 0, st>>>(w.pr, G, nmax, full_step ? 1 : 0, w.w);
+      cbt_psd_kernel<<<gt, 256, 0, st>>>(w.pr, nmax, full_step ? 1 : 0, w.Bm, w.w, w.M_psd);
+      cbt_affine_kernel<<<ge, 256, 0, st>>>(w.pr, nmax, 0, w.M_psd, w.M, w.W, w.M_init, 0.0);
+      cbt_dual_bw_kernel<<<gp, 128, 0, st>>>(w.pr, nmax, w.W, w.thp, w.bW);
+      cbt_dual_sums_kernel<<<dim3(grid1(3 * (maxN + 1), 128), G), 128, 0, st>>>(w.pr, w.bW, w.thp, w.D);
+      cbt_dual_off_kernel<<<gp, 128, 0, st>>>(w.pr, nmax, w.W, w.thp, w.bW, w.D, w.Wd);
+      cbt_dual_diag_kernel<<<dim3(grid1(maxN + 1, 4), G), 128, 0, st>>>(w.pr, nmax, w.W, w.thp, w.Wd, w.diag3);
+      cbt_dual_mean_kernel<<<G, 256, 0, st>>>(w.pr, nmax, w.diag3, w.Wd);
+      cbt_affine_kernel<<<ge, 256, 0, st>>>(w.pr, nmax, 1, w.Wd, nullptr, w.M_aff, w.M_init, 0.0);
+      cbt_sym_kernel<<<ge, 256, 0, st>>>(w.pr, nmax, w.M_aff, w.Bm);
+      if (int rc = eig(CUSOLVER_EIG_MODE_NOVECTOR)) return rc;
+      cbt_gap_kernel<<<grid1(G, 128), 128, 0, st>>>(w.pr, G, nmax, w.w, w.info, iter, prm.sub_optimality, maxit,
+                                                     w.traj, T, w.active);
+      *launches += 13;
+      cudaMemcpyAsync(act.data(), w.active, G * sizeof(int), cudaMemcpyDeviceToHost, st);
+      if (cudaStreamSynchronize(st) != cudaSuccess) {
+        *err = cudaGetErrorString(cudaGetLastError());
+        return TZR_ERR_CUDA;
+      }
+      n_act = (int)std::count(act.begin(), act.end(), 1);
+      if (n_act == 0) break;
+      cbt_affine_kernel<<<ge, 256, 0, st>>>(w.pr, nmax, 2, w.M_aff, w.M_psd, w.M, nullptr, prm.gamma_tau);
+      *launches += 1;
+    }
+    std::vector<double> h_traj((size_t)G * T);
+    cudaMemcpyAsync(tab.data(), w.pr, G * sizeof(CertBatchProb), cudaMemcpyDeviceToHost, st);
+    if (T) cudaMemcpyAsync(h_traj.data(), w.traj, h_traj.size() * sizeof(double), cudaMemcpyDeviceToHost, st);
+    if (cudaStreamSynchronize(st) != cudaSuccess) {
+      *err = cudaGetErrorString(cudaGetLastError());
+      return TZR_ERR_CUDA;
+    }
+    for (int g = 0; g < G; ++g) {
+      const int b = b0 + g;
+      results[b].is_optimal = tab[g].best < prm.sub_optimality ? 1 : 0;
+      results[b].n_iterations = tab[g].iters;
+      results[b].best_suboptimality = tab[g].best;
+      if (traj && traj_cap && traj[b]) {
+        const int m = std::min(std::min(tab[g].iters, (int)traj_cap[b]), T);
+        std::copy(h_traj.begin() + (size_t)g * T, h_traj.begin() + (size_t)g * T + m, traj[b]);
+      }
+    }
+    b0 = b1;
+  }
   return TZR_OK;
 }
 

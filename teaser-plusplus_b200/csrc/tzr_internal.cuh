@@ -249,6 +249,13 @@ int certify_device(int mode, double noise_bound, double cbar2, double sub_optima
                    int N, int* is_optimal, double* best_subopt, int* n_iters, double* traj, int traj_cap,
                    double* M_init_out, double* mu_out, const double* W_in, double* Wd_out, void** scratch,
                    size_t* scratch_cap, void** solver_handle, int64_t* launches, cudaStream_t st, std::string* err);
+// B problems (host pointers, validated by the caller) in device-sized groups of one launch sequence each; loop_eig: one
+// cusolverDnDsyevd per active problem instead of cusolverDnXsyevBatched (debug flag 2097152)
+int certify_batch_device(const tzr_certifier_params& prm, int B, const int32_t* N, const double* R_cm,
+                         const double* const* src, const double* const* dst, const double* const* theta,
+                         tzr_certification_result* results, double* const* traj, const int32_t* traj_cap,
+                         bool loop_eig, void** scratch, size_t* scratch_cap, void** solver_handle, int64_t* launches,
+                         cudaStream_t st, std::string* err);
 void certify_release(void* solver_handle);
 
 // matcher.cu (Matcher::calculateCorrespondences, matcher.cc:21-337), over B cloud pairs stored back to back

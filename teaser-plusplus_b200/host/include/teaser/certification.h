@@ -58,6 +58,18 @@ class DRSCertifier : public AbstractRotationCertifier {
                               const Eigen::Matrix<double, 3, Eigen::Dynamic>& dst,
                               const Eigen::Matrix<double, 1, Eigen::Dynamic>& theta);
 
+  /// certify on every problem of the vectors in one device call (tzr_certify_batch); result b is what certify gives
+  /// for problem b alone.  All four vectors have the same, non-zero length.
+  std::vector<CertificationResult> certifyBatch(const std::vector<Eigen::Matrix3d>& R_solutions,
+                                                const std::vector<Eigen::Matrix<double, 3, Eigen::Dynamic>>& src,
+                                                const std::vector<Eigen::Matrix<double, 3, Eigen::Dynamic>>& dst,
+                                                const std::vector<Eigen::Matrix<bool, 1, Eigen::Dynamic>>& theta);
+
+  std::vector<CertificationResult> certifyBatch(const std::vector<Eigen::Matrix3d>& R_solutions,
+                                                const std::vector<Eigen::Matrix<double, 3, Eigen::Dynamic>>& src,
+                                                const std::vector<Eigen::Matrix<double, 3, Eigen::Dynamic>>& dst,
+                                                const std::vector<Eigen::Matrix<double, 1, Eigen::Dynamic>>& theta);
+
   /// certification.cc:293-303; q given as (x, y, z, w)
   Eigen::Matrix4d getOmega1(double qx, double qy, double qz, double qw);
 

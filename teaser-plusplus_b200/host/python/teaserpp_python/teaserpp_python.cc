@@ -250,6 +250,40 @@ PYBIND11_MODULE(_teaserpp, m) {
         Eigen::Matrix<double, 1, Eigen::Dynamic> th(1, td.size());
         std::memcpy(th.data(), td.data(), sizeof(double) * static_cast<size_t>(td.size()));
         return c.certify(to_r3(R), to_mat3x(src), to_mat3x(dst), th);
+      })
+      // lists of rotations, (3,N) arrays and thetas; all-bool thetas take the bool overload, otherwise every theta is
+      // taken as +-1 doubles (a bool one mapped true -> 1, false -> -1)
+      .def("certify_batch", [to_r3](Cert& c, const std::vector<ArrD>& Rs, const std::vector<ArrD>& srcs,
+                                    const std::vector<ArrD>& dsts, const std::vector<py::array>& thetas) {
+        std::vector<Eigen::Matrix3d> R;
+        std::vector<teaser::Mat3X> s, d;
+        for (const auto& x : Rs) R.push_back(to_r3(x));
+        for (const auto& x : srcs) s.push_back(to_mat3x(x));
+        for (const auto& x : dsts) d.push_back(to_mat3x(x));
+        bool all_bool = !thetas.empty();
+        for (const auto& t : thetas) all_bool = all_bool && t.dtype().kind() == 'b';
+        if (all_bool) {
+          std::vector<Eigen::Matrix<bool, 1, Eigen::Dynamic>> th;
+          for (const auto& t : thetas) {
+            auto tb = py::array_t<bool, py::array::c_style | py::array::forcecast>::ensure(t);
+            Eigen::Matrix<bool, 1, Eigen::Dynamic> m(1, tb.size());
+            for (py::ssize_t i = 0; i < tb.size(); ++i) m(i) = tb.data()[i];
+            th.push_back(m);
+          }
+          py::gil_scoped_release release;
+          return c.certifyBatch(R, s, d, th);
+        }
+        std::vector<Eigen::Matrix<double, 1, Eigen::Dynamic>> th;
+        for (const auto& t : thetas) {
+          auto td = py::array_t<double, py::array::c_style | py::array::forcecast>::ensure(t);
+          if (!td) throw std::invalid_argument("theta must be a bool or float array");
+          Eigen::Matrix<double, 1, Eigen::Dynamic> m(1, td.size());
+          for (py::ssize_t i = 0; i < td.size(); ++i)
+            m(i) = t.dtype().kind() == 'b' ? (td.data()[i] != 0 ? 1.0 : -1.0) : td.data()[i];
+          th.push_back(m);
+        }
+        py::gil_scoped_release release;
+        return c.certifyBatch(R, s, d, th);
       });
 
   py::class_<Cert::Params>(certifier, "Params")

@@ -1,6 +1,7 @@
 // teaser::DRSCertifier façade: forwards to the C-ABI (no CPU implementation behind it).
 #include "teaser/certification.h"
 
+#include <algorithm>
 #include <cmath>
 #include <stdexcept>
 #include <string>
@@ -57,6 +58,60 @@ CertificationResult DRSCertifier::certify(const Eigen::Matrix3d& R_solution,
   out.suboptimality_traj.resize(r.n_iterations);
   out.is_optimal = r.is_optimal != 0;
   out.best_suboptimality = r.best_suboptimality;
+  return out;
+}
+
+std::vector<CertificationResult> DRSCertifier::certifyBatch(
+    const std::vector<Eigen::Matrix3d>& R_solutions, const std::vector<Eigen::Matrix<double, 3, Eigen::Dynamic>>& src,
+    const std::vector<Eigen::Matrix<double, 3, Eigen::Dynamic>>& dst,
+    const std::vector<Eigen::Matrix<bool, 1, Eigen::Dynamic>>& theta) {
+  std::vector<Eigen::Matrix<double, 1, Eigen::Dynamic>> theta_double;
+  theta_double.reserve(theta.size());
+  for (const auto& t : theta) {
+    Eigen::Matrix<double, 1, Eigen::Dynamic> td(1, t.cols());
+    for (Eigen::Index i = 0; i < t.cols(); ++i) td(i) = t(i) ? 1 : -1;
+    theta_double.push_back(td);
+  }
+  return certifyBatch(R_solutions, src, dst, theta_double);
+}
+
+std::vector<CertificationResult> DRSCertifier::certifyBatch(
+    const std::vector<Eigen::Matrix3d>& R_solutions, const std::vector<Eigen::Matrix<double, 3, Eigen::Dynamic>>& src,
+    const std::vector<Eigen::Matrix<double, 3, Eigen::Dynamic>>& dst,
+    const std::vector<Eigen::Matrix<double, 1, Eigen::Dynamic>>& theta) {
+  const size_t B = R_solutions.size();
+  if (B == 0 || src.size() != B || dst.size() != B || theta.size() != B)
+    throw std::invalid_argument("teaser::DRSCertifier::certifyBatch: the four vectors must have the same, non-zero size");
+  std::vector<int32_t> n(B), caps(B);
+  std::vector<double> R(9 * B);
+  std::vector<const double*> s(B), d(B), t(B);
+  std::vector<double*> traj(B);
+  std::vector<CertificationResult> out(B);
+  const int cap = static_cast<int>(std::max(1.0, std::ceil(params_.max_iterations)));
+  for (size_t b = 0; b < B; ++b) {
+    n[b] = static_cast<int32_t>(src[b].cols());
+    if (dst[b].cols() != src[b].cols() || theta[b].cols() != src[b].cols() || n[b] == 0)
+      throw std::invalid_argument("teaser::DRSCertifier::certifyBatch: problem " + std::to_string(b) +
+                                  ": src, dst and theta must have the same, non-zero width");
+    std::copy(R_solutions[b].data(), R_solutions[b].data() + 9, R.begin() + 9 * b);
+    s[b] = src[b].data();
+    d[b] = dst[b].data();
+    t[b] = theta[b].data();
+    out[b].suboptimality_traj.resize(cap);
+    traj[b] = out[b].suboptimality_traj.data();
+    caps[b] = cap;
+  }
+  tzr_ctx* ctx = b200_context();
+  const tzr_certifier_params p = to_c(params_);
+  std::vector<tzr_certification_result> r(B);
+  const int rc = tzr_certify_batch(ctx, &p, static_cast<int>(B), n.data(), R.data(), s.data(), d.data(), t.data(),
+                                   r.data(), traj.data(), caps.data());
+  if (rc != TZR_OK) fail("teaser::DRSCertifier::certifyBatch (GPU)", rc, ctx);
+  for (size_t b = 0; b < B; ++b) {
+    out[b].suboptimality_traj.resize(r[b].n_iterations);
+    out[b].is_optimal = r[b].is_optimal != 0;
+    out[b].best_suboptimality = r[b].best_suboptimality;
+  }
   return out;
 }
 
