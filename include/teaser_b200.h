@@ -166,7 +166,10 @@ int tzr_gnc_tls_rotation(tzr_ctx* ctx, const double* src_3xM, const double* dst_
 
 /* Same stage for any of the reference's rotation back-ends on caller-supplied TIMs: algorithm 0 GNC_TLS
  * (registration.cc:764-866), 1 FGR (FastGlobalRegistrationSolver::solveForRotation, registration.cc:206-278),
- * 2 QUATRO (QuatroSolver::solveForRotation, registration.cc:280-408; yaw only). */
+ * 2 QUATRO (QuatroSolver::solveForRotation, registration.cc:280-408; yaw only).
+ * With max_iterations = 0 no iteration runs: R is the identity, the cost +inf, iterations 0 and every mask entry 1
+ * (the reference leaves its rotation untouched there).  A GNC-TLS or Quatro run whose first residuals all lie below
+ * noise_bound^2 / 2 stops at mu <= 0 after one iteration with the cost still +inf. */
 int tzr_rotation_solve(tzr_ctx* ctx, int algorithm, const double* src_3xM, const double* dst_3xM, int m,
                        double noise_bound, double gnc_factor, uint64_t max_iterations, double cost_threshold,
                        double* R_colmajor9, uint8_t* inlier_mask, double* cost_at_termination, int32_t* iterations);

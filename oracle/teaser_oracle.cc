@@ -194,6 +194,19 @@ void svd3(const M3& H, M3& U, double S[3], M3& V) {
   }
 }
 
+// R maximising tr(R H) is invariant under positive scaling of H.  Like Eigen's JacobiSVD, which divides the matrix by
+// its largest |entry| first, bring an H whose largest |entry| lies outside [2^-400, 2^400] into [1/2, 1) by an exact
+// power of two; entries inside that range keep their bits (rot_trans.cu does the same).
+void normalise_scale(double* a, int n) {
+  double mx = 0.0;
+  for (int i = 0; i < n; ++i) mx = std::max(mx, std::fabs(a[i]));
+  if (mx > 0.0 && mx <= std::numeric_limits<double>::max() && (mx < 0x1p-400 || mx > 0x1p400)) {
+    int e;
+    std::frexp(mx, &e);
+    for (int i = 0; i < n; ++i) a[i] = std::ldexp(a[i], -e);
+  }
+}
+
 // utils::svdRot  (teaser/include/teaser/utils.h:121-136)
 //   H = X * diag(W) * Y^T ; SVD ; if det(U)*det(V) < 0 negate V.col(2) ; R = V * U^T
 M3 svd_rot(const double* X, const double* Y, const double* W, i64 m) {
@@ -209,6 +222,7 @@ M3 svd_rot(const double* X, const double* Y, const double* W, i64 m) {
   }
   M3 U, V;
   double S[3];
+  normalise_scale(H.a, 9);
   svd3(H, U, S, V);
   if (m3_det(U) * m3_det(V) < 0) {
     for (int r = 0; r < 3; ++r) V(r, 2) = -V(r, 2);
@@ -517,6 +531,11 @@ void svd_rot2d(const double* X, const double* Y, const double* W, i64 m, double 
     const double y0 = Y[3 * j], y1 = Y[3 * j + 1];
     h00 += x0 * y0; h01 += x0 * y1;
     h10 += x1 * y0; h11 += x1 * y1;
+  }
+  {
+    double h[4] = {h00, h01, h10, h11};
+    normalise_scale(h, 4);
+    h00 = h[0], h01 = h[1], h10 = h[2], h11 = h[3];
   }
   // step 1: G1 = [c1 s1; -s1 c1] such that G1*H is symmetric
   double c1 = 1, s1 = 0;

@@ -142,10 +142,25 @@ __device__ void svd3(const M3& H, M3& U, double S[3], M3& V) {
   }
 }
 
+// R maximising tr(R H) does not change when H is scaled by a positive number.  If H's largest |entry| lies outside
+// [2^-400, 2^400], scale the n entries by the power of two that brings it into [1/2, 1): exact, and it keeps the Jacobi
+// threshold (tiny / eps*max_diag) and the squares of the planar closed form clear of underflow and overflow.  Entries
+// already in that range keep their bits, so ordinary inputs are untouched.
+__device__ inline void normalise_scale(double* a, int n) {
+  double mx = 0.0;
+  for (int i = 0; i < n; ++i) mx = fmax(mx, fabs(a[i]));
+  if (mx > 0.0 && mx <= 1.7976931348623157e308 && (mx < 0x1p-400 || mx > 0x1p400)) {
+    int e;
+    frexp(mx, &e);
+    for (int i = 0; i < n; ++i) a[i] = ldexp(a[i], -e);
+  }
+}
+
 // R = V * U^T with the reflection fix (utils.h:130-135)
-__device__ void rotation_from_H(const M3& H, M3& R) {
-  M3 U, V;
+__device__ void rotation_from_H(const M3& H0, M3& R) {
+  M3 H = H0, U, V;
   double S[3];
+  normalise_scale(H.a, 9);
   svd3(H, U, S, V);
   if (m3_det(U) * m3_det(V) < 0.0) {
     for (int r = 0; r < 3; ++r) V(r, 2) = -V(r, 2);
@@ -250,7 +265,9 @@ __device__ void rotation_step(const TimSrc& ts, const double* __restrict__ wgt, 
     } else {
       // utils::svdRot2d (utils.h:145-160): the proper rotation maximising tr(R H2) for the 2x2 block
       // H2 = [h00 h01; h10 h11] is R = [c -s; s c] with (c, s) ~ (h00 + h11, h01 - h10)  (closed form of V U^T)
-      const double ca = h[0] + h[4], sb = h[3] - h[1];
+      double h2[4] = {h[0], h[1], h[3], h[4]};
+      normalise_scale(h2, 4);
+      const double ca = h2[0] + h2[3], sb = h2[2] - h2[1];
       const double nrm = sqrt(ca * ca + sb * sb);
       m3_identity(R);
       if (nrm > 0.0) {
