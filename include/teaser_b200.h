@@ -278,7 +278,8 @@ int tzr_certify(tzr_ctx* ctx, const tzr_certifier_params* params, const double* 
  * The problems run together: one launch sequence per iteration for the whole batch, one read-back of the active flags
  * per iteration, the trajectories copied back once at the end.  Finished problems are skipped by every kernel and by the
  * eigensolver.  The eigendecompositions of an iteration are one cusolverDnXsyevBatched call over the active problems'
- * matrices padded to 4 max N + 4 with an identity block (DESIGN.md 3.9; once some problems have finished, the active
+ * matrices padded to 4 max N + 4 with a multiple of the identity that follows each problem's scale (DESIGN.md 3.9;
+ * once some problems have finished, the active
  * ones are gathered into a compact batch first) while at least 8 problems are active, else one cusolverDnDsyevd per
  * active problem; the loop is also taken
  * when the batched symbol is missing, the batched call refuses the size, or debug flag 2097152 is set.
@@ -301,6 +302,18 @@ int tzr_certifier_initial_matrix(tzr_ctx* ctx, const tzr_certifier_params* param
                                  const double* src_3xN, const double* dst_3xN, const double* theta, int n,
                                  double* M_init, double* mu);
 int tzr_certifier_dual_projection(tzr_ctx* ctx, const double* W, const double* theta, int n, double* W_dual);
+/* tzr_certifier_psd_projection: the nearest-PSD step of one DRS iteration (linalg.h:84-99) on the path tzr_certify
+ *   takes: M is any (4n+4)^2 column-major matrix, M_psd receives V+ diag(w+) V+^T of sym(M) = (M + M^T)/2 over its
+ *   positive eigenpairs, w the (4n+4) ascending eigenvalues of sym(M).
+ * tzr_certifier_batch_psd_projection / tzr_certifier_batch_dual_projection: the same step, and the dual projection, on
+ *   B problems of N[b] measurements on tzr_certify_batch's path: its padded layout and, for the PSD step, the
+ *   eigensolver route that call would take for B problems (debug flag 2097152 included).  M[b], M_psd[b], W[b],
+ *   W_dual[b]: (4N[b]+4)^2 column-major; theta[b]: N[b] doubles. */
+int tzr_certifier_psd_projection(tzr_ctx* ctx, const double* M, int n, double* M_psd, double* w);
+int tzr_certifier_batch_psd_projection(tzr_ctx* ctx, int B, const int32_t* N, const double* const* M,
+                                       double* const* M_psd);
+int tzr_certifier_batch_dual_projection(tzr_ctx* ctx, int B, const int32_t* N, const double* const* W,
+                                        const double* const* theta, double* const* W_dual);
 
 /* ---- whole path -----------------------------------------------------------------------------
  * Replaces RobustRegistrationSolver::solve(src, dst) (registration.cc:568-737) for one problem

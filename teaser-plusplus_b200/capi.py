@@ -97,6 +97,7 @@ _SYMBOLS = [
     "tzr_certifier_initial_matrix", "tzr_certifier_dual_projection", "tzr_last_graph_info", "tzr_ctx_stage_log",
     "tzr_ctx_stage_log_read", "tzr_solve_batch_multi", "tzr_ctx_clique_info", "tzr_compute_fpfh_batch",
     "tzr_match_correspondences_batch", "tzr_ctx_set_max_n", "tzr_ctx_clique_route", "tzr_certify_batch",
+    "tzr_certifier_psd_projection", "tzr_certifier_batch_psd_projection", "tzr_certifier_batch_dual_projection",
 ]
 
 
@@ -178,6 +179,9 @@ def lib():
                                     C.POINTER(dp), C.POINTER(CertificationResult), C.POINTER(dp), i32p]
     L.tzr_certifier_initial_matrix.argtypes = [vp, C.POINTER(CertifierParams), dp, dp, dp, dp, C.c_int, dp, dp]
     L.tzr_certifier_dual_projection.argtypes = [vp, dp, dp, C.c_int, dp]
+    L.tzr_certifier_psd_projection.argtypes = [vp, dp, C.c_int, dp, dp]
+    L.tzr_certifier_batch_psd_projection.argtypes = [vp, C.c_int, i32p, C.POINTER(dp), C.POINTER(dp)]
+    L.tzr_certifier_batch_dual_projection.argtypes = [vp, C.c_int, i32p, C.POINTER(dp), C.POINTER(dp), C.POINTER(dp)]
     for s in _SYMBOLS:
         getattr(L, s)  # raises AttributeError if the header and the library disagree
     _lib = L
@@ -473,6 +477,51 @@ class Context:
         self._ck(lib().tzr_certifier_dual_projection(self._h, _p(Wc, C.c_double), _p(th, C.c_double), th.size,
                                                      _p(out, C.c_double)))
         return out.T.copy()
+
+    @staticmethod
+    def _cert_square(M, what):
+        """Column-major copy of a (4N+4, 4N+4) matrix and its N."""
+        Mc = np.ascontiguousarray(np.asarray(M, dtype=np.float64).T)
+        n = Mc.shape[0]
+        if Mc.ndim != 2 or Mc.shape != (n, n) or n < 8 or n % 4:
+            raise TzrError(f"{what}: M must be (4N+4, 4N+4) with N >= 1")
+        return Mc, (n - 4) // 4
+
+    def certifier_psd_projection(self, M):
+        """The nearest-PSD step of tzr_certify on any (4N+4)^2 M: (V+ diag(w+) V+^T of (M + M^T)/2, ascending w)."""
+        Mc, N = self._cert_square(M, "certifier_psd_projection")
+        out, w = np.zeros_like(Mc), np.zeros(Mc.shape[0])
+        self._ck(lib().tzr_certifier_psd_projection(self._h, _p(Mc, C.c_double), N, _p(out, C.c_double),
+                                                    _p(w, C.c_double)))
+        return out.T.copy(), w
+
+    def certifier_batch_psd_projection(self, Ms):
+        """The nearest-PSD step of tzr_certify_batch on every matrix of the list, one call (padded layout, the batch's
+        eigensolver route)."""
+        ins = [self._cert_square(M, "certifier_batch_psd_projection") for M in Ms]
+        if not ins:
+            raise TzrError("certifier_batch_psd_projection: no matrices")
+        outs = [np.zeros_like(m) for m, _ in ins]
+        N = np.array([k for _, k in ins], dtype=np.int32)
+        dp = C.POINTER(C.c_double)
+        arr = lambda xs: (dp * len(xs))(*[_p(x, C.c_double) for x in xs])
+        self._ck(lib().tzr_certifier_batch_psd_projection(self._h, len(ins), _p(N, C.c_int32), arr([m for m, _ in ins]),
+                                                          arr(outs)))
+        return [o.T.copy() for o in outs]
+
+    def certifier_batch_dual_projection(self, Ws, thetas):
+        """The dual projection of tzr_certify_batch on every (W, theta) pair of the lists, one call."""
+        ins = [self._cert_square(W, "certifier_batch_dual_projection") for W in Ws]
+        ths = [np.ascontiguousarray(np.asarray(t, dtype=np.float64).ravel()) for t in thetas]
+        if not ins or len(ths) != len(ins) or any(t.size != k for t, (_, k) in zip(ths, ins)):
+            raise TzrError("certifier_batch_dual_projection: one theta of N values per (4N+4)^2 W is required")
+        outs = [np.zeros_like(m) for m, _ in ins]
+        N = np.array([k for _, k in ins], dtype=np.int32)
+        dp = C.POINTER(C.c_double)
+        arr = lambda xs: (dp * len(xs))(*[_p(x, C.c_double) for x in xs])
+        self._ck(lib().tzr_certifier_batch_dual_projection(self._h, len(ins), _p(N, C.c_int32),
+                                                           arr([m for m, _ in ins]), arr(ths), arr(outs)))
+        return [o.T.copy() for o in outs]
 
     # -- upstream of solve(): Matcher::calculateCorrespondences (matcher.cc:21-337)
     def match_correspondences(self, src_pts, dst_pts, src_feat, dst_feat, use_absolute_scale=True,

@@ -1501,7 +1501,7 @@ int tzr_certify(tzr_ctx* ctx, const tzr_certifier_params* params, const double* 
   double best = 0;
   const int rc = certify_device(0, params->noise_bound, params->cbar2, params->sub_optimality, params->max_iterations,
                                 params->gamma_tau, R_colmajor9, src_3xN, dst_3xN, theta, n, &opt, &best, &iters, traj,
-                                traj_capacity, nullptr, nullptr, nullptr, nullptr, &ctx->cert.p, &ctx->cert.cap,
+                                traj_capacity, nullptr, nullptr, nullptr, nullptr, nullptr, &ctx->cert.p, &ctx->cert.cap,
                                 &ctx->solver_handle, &ctx->launches, ctx->stream, &ctx->last_error);
   if (rc != TZR_OK) return rc;
   result->is_optimal = opt;
@@ -1521,8 +1521,8 @@ int tzr_certify_batch(tzr_ctx* ctx, const tzr_certifier_params* params, int B, c
     if (N[b] <= 0 || !src_3xN[b] || !dst_3xN[b] || !theta[b] || (traj_capacity && traj_capacity[b] < 0))
       return TZR_ERR_INVALID_ARG;
   cudaSetDevice(ctx->device);
-  return certify_batch_device(*params, B, N, R_colmajor9xB, src_3xN, dst_3xN, theta, results, traj, traj_capacity,
-                              (ctx->flags & 2097152u) != 0, &ctx->certb.p, &ctx->certb.cap, &ctx->solver_handle,
+  return certify_batch_device(0, *params, B, N, R_colmajor9xB, src_3xN, dst_3xN, theta, results, traj, traj_capacity,
+                              nullptr, nullptr, (ctx->flags & 2097152u) != 0, &ctx->certb.p, &ctx->certb.cap, &ctx->solver_handle,
                               &ctx->launches, ctx->stream, &ctx->last_error);
 }
 
@@ -1533,7 +1533,7 @@ int tzr_certifier_initial_matrix(tzr_ctx* ctx, const tzr_certifier_params* param
     return TZR_ERR_INVALID_ARG;
   cudaSetDevice(ctx->device);
   return certify_device(1, params->noise_bound, params->cbar2, 0, 0, 0, R_colmajor9, src_3xN, dst_3xN, theta, n,
-                        nullptr, nullptr, nullptr, nullptr, 0, M_init, mu, nullptr, nullptr, &ctx->cert.p,
+                        nullptr, nullptr, nullptr, nullptr, 0, M_init, mu, nullptr, nullptr, nullptr, &ctx->cert.p,
                         &ctx->cert.cap, &ctx->solver_handle, &ctx->launches, ctx->stream, &ctx->last_error);
 }
 
@@ -1541,8 +1541,40 @@ int tzr_certifier_dual_projection(tzr_ctx* ctx, const double* W, const double* t
   if (!ctx || !W || !theta || !W_dual || n <= 0) return TZR_ERR_INVALID_ARG;
   cudaSetDevice(ctx->device);
   return certify_device(2, 0, 0, 0, 0, 0, nullptr, nullptr, nullptr, theta, n, nullptr, nullptr, nullptr, nullptr, 0,
-                        nullptr, nullptr, W, W_dual, &ctx->cert.p, &ctx->cert.cap, &ctx->solver_handle, &ctx->launches, ctx->stream,
+                        nullptr, nullptr, W, W_dual, nullptr, &ctx->cert.p, &ctx->cert.cap, &ctx->solver_handle, &ctx->launches, ctx->stream,
                         &ctx->last_error);
+}
+
+int tzr_certifier_psd_projection(tzr_ctx* ctx, const double* M, int n, double* M_psd, double* w) {
+  if (!ctx || !M || !M_psd || !w || n <= 0) return TZR_ERR_INVALID_ARG;
+  cudaSetDevice(ctx->device);
+  return certify_device(3, 0, 0, 0, 0, 0, nullptr, nullptr, nullptr, nullptr, n, nullptr, nullptr, nullptr, nullptr, 0,
+                        nullptr, nullptr, M, M_psd, w, &ctx->cert.p, &ctx->cert.cap, &ctx->solver_handle,
+                        &ctx->launches, ctx->stream, &ctx->last_error);
+}
+
+// the batch building blocks (certify_batch_device modes 1 and 2): B problems of N[b] >= 1 measurements
+static int certifier_batch_block(tzr_ctx* ctx, int mode, int B, const int32_t* N, const double* const* X,
+                                 const double* const* theta, double* const* Y) {
+  if (!ctx || B <= 0 || !N || !X || !Y || (mode == 2 && !theta)) return TZR_ERR_INVALID_ARG;
+  for (int b = 0; b < B; ++b)
+    if (N[b] <= 0 || !X[b] || !Y[b] || (mode == 2 && !theta[b])) return TZR_ERR_INVALID_ARG;
+  cudaSetDevice(ctx->device);
+  tzr_certifier_params prm;
+  tzr_certifier_params_default(&prm);
+  return certify_batch_device(mode, prm, B, N, nullptr, nullptr, nullptr, theta, nullptr, nullptr, nullptr, X, Y,
+                              (ctx->flags & 2097152u) != 0, &ctx->certb.p, &ctx->certb.cap, &ctx->solver_handle,
+                              &ctx->launches, ctx->stream, &ctx->last_error);
+}
+
+int tzr_certifier_batch_psd_projection(tzr_ctx* ctx, int B, const int32_t* N, const double* const* M,
+                                       double* const* M_psd) {
+  return certifier_batch_block(ctx, 1, B, N, M, nullptr, M_psd);
+}
+
+int tzr_certifier_batch_dual_projection(tzr_ctx* ctx, int B, const int32_t* N, const double* const* W,
+                                        const double* const* theta, double* const* W_dual) {
+  return certifier_batch_block(ctx, 2, B, N, W, theta, W_dual);
 }
 
 int tzr_compute_fpfh(tzr_ctx* ctx, const float* pts, int n, double normal_search_radius, double fpfh_search_radius,

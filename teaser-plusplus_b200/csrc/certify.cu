@@ -20,6 +20,7 @@
 
 #include <algorithm>
 #include <cmath>
+#include <cstring>
 #include <string>
 #include <vector>
 
@@ -498,13 +499,18 @@ struct CertBatchProb {
   int active;          // 1 while the iteration runs
   int iters;           // iterations done (length of the trajectory)
   int first_pos;       // first eigen column with a positive eigenvalue
-  int pad;
+  unsigned long long pad_bits;  // largest |entry| of the starting matrix (M_init), as its bit pattern
   double mu, best;
 };
 
 // Eigenvalue of the pad block (the identity times it) of a padded problem: block diagonal, so the padded matrix has the
-// real block's eigenpairs plus (kCertPad, e_k) with e_k zero on the real rows; see DESIGN.md 3.9.
-constexpr double kCertPad = 1.0;
+// real block's eigenpairs plus (c, e_k) with e_k zero on the real rows; see DESIGN.md 3.9.  c is the largest power of
+// two not above the largest |entry| of the problem's starting matrix (1 if that is 0): it follows the problem's scale,
+// so the padded matrix has the real block's norm at any scale, and scaling a problem by 2^k scales c exactly.
+__device__ __forceinline__ double cert_pad(unsigned long long bits) {
+  const double m = __longlong_as_double(bits);
+  return m > 0 ? ldexp(1.0, ilogb(m)) : 1.0;
+}
 
 __global__ void cbt_blocks_kernel(const CertBatchProb* __restrict__ pr, const double* __restrict__ src,
                                   const double* __restrict__ dst, const double* __restrict__ theta,
@@ -527,21 +533,27 @@ __global__ void __launch_bounds__(256) cbt_reduce_kernel(CertBatchProb* pr, cons
   if (threadIdx.x == 0) pr[b].mu = mu;
 }
 
-// M_init of every problem; the pad region is zero
-__global__ void cbt_fill_kernel(const CertBatchProb* __restrict__ pr, int nmax, const double* offA,
-                                const double* diagB, const double* lam, const double* top, double* M_init) {
+// M_init of every problem, the pad region zero; the largest |entry| into pad_bits (non-negative doubles order like
+// their bit patterns; one atomic per warp)
+__global__ void cbt_fill_kernel(CertBatchProb* __restrict__ pr, int nmax, const double* offA, const double* diagB,
+                                const double* lam, const double* top, double* M_init) {
   const int b = blockIdx.y;
   const long long e = blockIdx.x * (long long)blockDim.x + threadIdx.x;
-  if (e >= (long long)nmax * nmax) return;
-  const CertBatchProb& p = pr[b];
-  const int r = (int)(e % nmax), c = (int)(e / nmax);
-  const size_t o = p.k_off;
-  M_init[(size_t)b * nmax * nmax + e] =
-      (r < p.n && c < p.n) ? cert_fill_value(r, c, offA + 16 * o, diagB + 16 * o, lam + 16 * o, top + 16 * b, &p.mu)
-                           : 0.0;
+  CertBatchProb& p = pr[b];
+  double v = 0;
+  if (e < (long long)nmax * nmax) {
+    const int r = (int)(e % nmax), c = (int)(e / nmax);
+    const size_t o = p.k_off;
+    if (r < p.n && c < p.n)
+      v = cert_fill_value(r, c, offA + 16 * o, diagB + 16 * o, lam + 16 * o, top + 16 * b, &p.mu);
+    M_init[(size_t)b * nmax * nmax + e] = v;
+  }
+  unsigned long long m = (unsigned long long)__double_as_longlong(fabs(v));
+  for (int off = 16; off > 0; off >>= 1) m = max(m, __shfl_xor_sync(0xffffffffu, m, off));
+  if ((threadIdx.x & 31) == 0 && m) atomicMax(&p.pad_bits, m);
 }
 
-// B = (M + M^T) / 2 on the real block, kCertPad * I on the pad block
+// B = (M + M^T) / 2 on the real block, cert_pad * I on the pad block
 __global__ void cbt_sym_kernel(const CertBatchProb* __restrict__ pr, int nmax, const double* __restrict__ M,
                                double* __restrict__ Bm) {
   const int b = blockIdx.y;
@@ -550,7 +562,8 @@ __global__ void cbt_sym_kernel(const CertBatchProb* __restrict__ pr, int nmax, c
   const int n = pr[b].n;
   const int r = (int)(e % nmax), c = (int)(e / nmax);
   const size_t base = (size_t)b * nmax * nmax;
-  Bm[base + e] = (r < n && c < n) ? (M[base + e] + M[base + (size_t)r * nmax + c]) / 2 : (r == c ? kCertPad : 0.0);
+  Bm[base + e] =
+      (r < n && c < n) ? (M[base + e] + M[base + (size_t)r * nmax + c]) / 2 : (r == c ? cert_pad(pr[b].pad_bits) : 0.0);
 }
 
 // first eigen column with w > 0 (w ascending); ne_full: the eigensolver ran on the padded nmax (else on n)
@@ -789,6 +802,21 @@ static int launch_dual_projection(const CertWork& w, int N, cudaStream_t st) {
   return 5;
 }
 
+// nearest PSD matrix of w.M (linalg.h:84-99): B = sym(M) -> eigenvectors in w.B, ascending eigenvalues in w.w, M_PSD
+// in w.M_psd; 4 kernels and one Dsyevd.  false when the eigensolver call is refused.
+static bool launch_psd_step(Cusolver& cs, cusolverDnHandle_t handle, const CertWork& w, size_t n, cudaStream_t st) {
+  const int ge = grid1((long long)(n * n), 256);
+  sym_kernel<<<ge, 256, 0, st>>>(w.M, (int)n, w.B);
+  if (cs.syevd(handle, CUSOLVER_EIG_MODE_VECTOR, CUBLAS_FILL_MODE_LOWER, (int)n, w.B, (int)n, w.w, w.work, w.lwork,
+               w.info) != CUSOLVER_STATUS_SUCCESS)
+    return false;
+  first_pos_kernel<<<1, 32, 0, st>>>(w.w, (int)n, w.first_pos);
+  scale_pos_kernel<<<ge, 256, 0, st>>>(w.B, w.w, (int)n, w.Vs);
+  dim3 gg((unsigned)((n + kGT - 1) / kGT), (unsigned)((n + kGT - 1) / kGT));
+  psd_gemm_kernel<<<gg, 256, 0, st>>>(w.Vs, w.B, (int)n, w.first_pos, w.M_psd);
+  return true;
+}
+
 // quaternion of R (Eigen::Quaterniond(R).normalize(), :66-69) on the host: 20 flops
 static void quaternion_xyzw(const double* R_cm, double q[4]) {
   const double* R = R_cm;  // column-major: R(r,c) = R[r + 3c]
@@ -821,18 +849,20 @@ static void quaternion_xyzw(const double* R_cm, double q[4]) {
 }
 
 // Returns TZR_OK or a negative status; err receives a message.  All pointers host.  mode: 0 full certify,
-// 1 initial matrix only (M_init_out n*n, mu_out), 2 dual projection only (W_in n*n -> Wd_out n*n; theta = N values).
+// 1 initial matrix only (M_init_out n*n, mu_out), 2 dual projection only (W_in n*n -> Wd_out n*n; theta = N values),
+// 3 nearest-PSD step only (W_in n*n -> Wd_out n*n and the ascending eigenvalues of sym(W_in) in w_out).
 int certify_device(int mode, double noise_bound, double cbar2, double sub_optimality, double max_iterations,
                    double gamma_tau, const double* R_cm, const double* src, const double* dst, const double* theta,
                    int N, int* is_optimal, double* best_subopt, int* n_iters, double* traj, int traj_cap,
-                   double* M_init_out, double* mu_out, const double* W_in, double* Wd_out, void** scratch,
-                   size_t* scratch_cap, void** solver_handle, int64_t* launches, cudaStream_t st, std::string* err) {
+                   double* M_init_out, double* mu_out, const double* W_in, double* Wd_out, double* w_out,
+                   void** scratch, size_t* scratch_cap, void** solver_handle, int64_t* launches, cudaStream_t st,
+                   std::string* err) {
   const size_t n = 4 * (size_t)N + 4, nn = n * n;
   if (n > 32768) return TZR_ERR_TOO_LARGE;
   int lwork = 0;
   Cusolver& cs = cusolver();
   cusolverDnHandle_t& handle = *reinterpret_cast<cusolverDnHandle_t*>(solver_handle);  // owned by the context
-  if (mode == 0) {
+  if (mode == 0 || mode == 3) {
     if (!cs.ok) {
       *err = cs.err;
       return TZR_ERR_UNSUPPORTED;
@@ -861,6 +891,24 @@ int certify_device(int mode, double noise_bound, double cbar2, double sub_optima
     *scratch_cap = need;
   }
   CertWork w = carve(*scratch, N, lwork);
+  if (mode == 3) {
+    int info = 0;
+    cudaMemcpyAsync(w.M, W_in, nn * sizeof(double), cudaMemcpyHostToDevice, st);
+    if (!launch_psd_step(cs, handle, w, n, st)) {
+      *err = "cusolverDnDsyevd failed";
+      return TZR_ERR_CUDA;
+    }
+    *launches += 5;
+    cudaMemcpyAsync(Wd_out, w.M_psd, nn * sizeof(double), cudaMemcpyDeviceToHost, st);
+    cudaMemcpyAsync(w_out, w.w, n * sizeof(double), cudaMemcpyDeviceToHost, st);
+    cudaMemcpyAsync(&info, w.info, sizeof(int), cudaMemcpyDeviceToHost, st);
+    if (cudaStreamSynchronize(st) != cudaSuccess) return TZR_ERR_CUDA;
+    if (info != 0) {
+      *err = "cusolverDnDsyevd reported info " + std::to_string(info);
+      return TZR_ERR_CUDA;
+    }
+    return TZR_OK;
+  }
   std::vector<double> thp((size_t)N + 1);
   thp[0] = 1.0;
   for (int i = 0; i < N; ++i) thp[i + 1] = theta[i];
@@ -900,17 +948,10 @@ int certify_device(int mode, double noise_bound, double cbar2, double sub_optima
   int iters = 0;
   std::vector<double> wh(n);
   for (size_t iter = 0; (double)iter < max_iterations; ++iter) {
-    // nearest PSD matrix (linalg.h:84-99)
-    sym_kernel<<<ge, 256, 0, st>>>(w.M, (int)n, w.B);
-    if (cs.syevd(handle, CUSOLVER_EIG_MODE_VECTOR, CUBLAS_FILL_MODE_LOWER, (int)n, w.B, (int)n, w.w, w.work,
-                 lwork, w.info) != CUSOLVER_STATUS_SUCCESS) {
+    if (!launch_psd_step(cs, handle, w, n, st)) {
       *err = "cusolverDnDsyevd failed";
       return TZR_ERR_CUDA;
     }
-    first_pos_kernel<<<1, 32, 0, st>>>(w.w, (int)n, w.first_pos);
-    scale_pos_kernel<<<ge, 256, 0, st>>>(w.B, w.w, (int)n, w.Vs);
-    dim3 gg((unsigned)((n + kGT - 1) / kGT), (unsigned)((n + kGT - 1) / kGT));
-    psd_gemm_kernel<<<gg, 256, 0, st>>>(w.Vs, w.B, (int)n, w.first_pos, w.M_psd);
     affine_in_kernel<<<ge, 256, 0, st>>>(w.M_psd, w.M, w.M_init, (long long)nn, w.W);
     *launches += 5 + launch_dual_projection(w, N, st);
     affine_out_kernel<<<ge, 256, 0, st>>>(w.M_init, w.Wd, (long long)nn, w.M_aff);
@@ -994,11 +1035,12 @@ size_t cbt_carve(void* base, int G, long long K, long long P, int nmax, int T, s
 }
 }  // namespace
 
-int certify_batch_device(const tzr_certifier_params& prm, int B, const int32_t* N, const double* R_cm,
+int certify_batch_device(int mode, const tzr_certifier_params& prm, int B, const int32_t* N, const double* R_cm,
                          const double* const* src, const double* const* dst, const double* const* theta,
                          tzr_certification_result* results, double* const* traj, const int32_t* traj_cap,
-                         bool loop_eig, void** scratch, size_t* scratch_cap, void** solver_handle, int64_t* launches,
-                         cudaStream_t st, std::string* err) {
+                         const double* const* X_in, double* const* X_out, bool loop_eig, void** scratch,
+                         size_t* scratch_cap, void** solver_handle, int64_t* launches, cudaStream_t st,
+                         std::string* err) {
   int nmax_all = 0;
   for (int b = 0; b < B; ++b) {
     if (4 * (size_t)N[b] + 4 > 32768) {
@@ -1131,14 +1173,21 @@ int certify_batch_device(const tzr_certifier_params& prm, int B, const int32_t* 
       CertBatchProb& t = tab[g];
       t.N = Nb; t.n = 4 * Nb + 4; t.k_off = k; t.v_off = k + g;
       t.p_off = g ? tab[g - 1].p_off + (long long)tab[g - 1].N * (tab[g - 1].N + 1) / 2 : 0;
-      t.active = 1; t.iters = 0; t.first_pos = 0; t.pad = 0; t.mu = 0; t.best = INFINITY;
-      std::copy(src[b], src[b] + 3 * (size_t)Nb, h_src.begin() + 3 * (size_t)k);
-      std::copy(dst[b], dst[b] + 3 * (size_t)Nb, h_dst.begin() + 3 * (size_t)k);
-      std::copy(theta[b], theta[b] + Nb, h_th.begin() + k);
+      t.active = 1; t.iters = 0; t.first_pos = 0; t.pad_bits = 0; t.mu = 0; t.best = INFINITY;
+      if (mode == 1) {  // the PSD building block starts from X_in[b]: its pad follows that matrix
+        double m = 0;
+        for (size_t e = 0; e < (size_t)t.n * t.n; ++e) m = std::max(m, std::fabs(X_in[b][e]));
+        std::memcpy(&t.pad_bits, &m, sizeof m);
+      }
+      if (mode == 0) {
+        std::copy(src[b], src[b] + 3 * (size_t)Nb, h_src.begin() + 3 * (size_t)k);
+        std::copy(dst[b], dst[b] + 3 * (size_t)Nb, h_dst.begin() + 3 * (size_t)k);
+        std::copy(theta[b], theta[b] + Nb, h_th.begin() + k);
+        std::copy(R_cm + 9 * (size_t)b, R_cm + 9 * (size_t)b + 9, h_R.begin() + 9 * (size_t)g);
+        quaternion_xyzw(R_cm + 9 * (size_t)b, &h_q[4 * (size_t)g]);
+      }
       h_thp[k + g] = 1.0;
-      std::copy(theta[b], theta[b] + Nb, h_thp.begin() + k + g + 1);
-      std::copy(R_cm + 9 * (size_t)b, R_cm + 9 * (size_t)b + 9, h_R.begin() + 9 * (size_t)g);
-      quaternion_xyzw(R_cm + 9 * (size_t)b, &h_q[4 * (size_t)g]);
+      if (mode != 1) std::copy(theta[b], theta[b] + Nb, h_thp.begin() + k + g + 1);
       maxN = std::max(maxN, Nb);
       k += Nb;
     }
@@ -1151,12 +1200,14 @@ int certify_batch_device(const tzr_certifier_params& prm, int B, const int32_t* 
     cudaMemcpyAsync(w.pr, tab.data(), G * sizeof(CertBatchProb), cudaMemcpyHostToDevice, st);
     const long long nn = (long long)nmax * nmax;
     const dim3 ge(grid1(nn, 256), G), gp(grid1(maxN + 1, 128), maxN, G), gt((nmax + kPT - 1) / kPT, (nmax + kPT - 1) / kPT, G);
-    cbt_blocks_kernel<<<dim3(grid1(maxN, 128), G), 128, 0, st>>>(w.pr, w.src, w.dst, w.theta, w.R, w.q, nbs, w.offA,
-                                                                  w.diagB, w.lam, w.mu_terms);
-    cbt_reduce_kernel<<<G, 256, 0, st>>>(w.pr, w.lam, w.mu_terms, w.top);
-    cbt_fill_kernel<<<ge, 256, 0, st>>>(w.pr, nmax, w.offA, w.diagB, w.lam, w.top, w.M_init);
-    *launches += 3;
-    cudaMemcpyAsync(w.M, w.M_init, (size_t)G * nn * sizeof(double), cudaMemcpyDeviceToDevice, st);
+    if (mode == 0) {
+      cbt_blocks_kernel<<<dim3(grid1(maxN, 128), G), 128, 0, st>>>(w.pr, w.src, w.dst, w.theta, w.R, w.q, nbs,
+                                                                    w.offA, w.diagB, w.lam, w.mu_terms);
+      cbt_reduce_kernel<<<G, 256, 0, st>>>(w.pr, w.lam, w.mu_terms, w.top);
+      cbt_fill_kernel<<<ge, 256, 0, st>>>(w.pr, nmax, w.offA, w.diagB, w.lam, w.top, w.M_init);
+      *launches += 3;
+      cudaMemcpyAsync(w.M, w.M_init, (size_t)G * nn * sizeof(double), cudaMemcpyDeviceToDevice, st);
+    }
     std::vector<int> act(G, 1), idx;  // active flags of the last read-back; their indices (compact batch)
     int n_act = G, idx_for = -1;         // idx_for: the n_act whose idx is on the device
     bool full_step = bat;                // the step's eigen columns cover nmax (batched call) or n (Dsyevd)
@@ -1208,6 +1259,48 @@ int certify_batch_device(const tzr_certifier_params& prm, int B, const int32_t* 
       }
       return TZR_OK;
     };
+    if (mode != 0) {
+      // one building block on the group, in the layout and on the eigen route of the iteration below: each problem's
+      // n x n input into the real block of M (mode 1) or W (mode 2), the real block of M_psd or Wd back
+      double* in = mode == 1 ? w.M : w.W;
+      const double* out = mode == 1 ? w.M_psd : w.Wd;
+      const size_t ld = (size_t)nmax * sizeof(double);
+      for (int g = 0; g < G; ++g) {
+        const size_t nb = (size_t)tab[g].n * sizeof(double);
+        cudaMemcpy2DAsync(in + (size_t)g * nn, ld, X_in[b0 + g], nb, nb, tab[g].n, cudaMemcpyHostToDevice, st);
+      }
+      if (mode == 1) {
+        cbt_sym_kernel<<<ge, 256, 0, st>>>(w.pr, nmax, w.M, w.Bm);
+        if (int rc = eig(CUSOLVER_EIG_MODE_VECTOR)) return rc;
+        cbt_first_pos_kernel<<<grid1(G, 128), 128, 0, st>>>(w.pr, G, nmax, full_step ? 1 : 0, w.w);
+        cbt_psd_kernel<<<gt, 256, 0, st>>>(w.pr, nmax, full_step ? 1 : 0, w.Bm, w.w, w.M_psd);
+        *launches += 3;
+      } else {
+        cbt_dual_bw_kernel<<<gp, 128, 0, st>>>(w.pr, nmax, w.W, w.thp, w.bW);
+        cbt_dual_sums_kernel<<<dim3(grid1(3 * (maxN + 1), 128), G), 128, 0, st>>>(w.pr, w.bW, w.thp, w.D);
+        cbt_dual_off_kernel<<<gp, 128, 0, st>>>(w.pr, nmax, w.W, w.thp, w.bW, w.D, w.Wd);
+        cbt_dual_diag_kernel<<<dim3(grid1(maxN + 1, 4), G), 128, 0, st>>>(w.pr, nmax, w.W, w.thp, w.Wd, w.diag3);
+        cbt_dual_mean_kernel<<<G, 256, 0, st>>>(w.pr, nmax, w.diag3, w.Wd);
+        *launches += 5;
+      }
+      for (int g = 0; g < G; ++g) {
+        const size_t nb = (size_t)tab[g].n * sizeof(double);
+        cudaMemcpy2DAsync(X_out[b0 + g], nb, out + (size_t)g * nn, ld, nb, tab[g].n, cudaMemcpyDeviceToHost, st);
+      }
+      std::vector<int> info(G, 0);
+      if (mode == 1) cudaMemcpyAsync(info.data(), w.info, G * sizeof(int), cudaMemcpyDeviceToHost, st);
+      if (cudaStreamSynchronize(st) != cudaSuccess) {
+        *err = cudaGetErrorString(cudaGetLastError());
+        return TZR_ERR_CUDA;
+      }
+      for (int g = 0; g < G; ++g)
+        if (info[g] != 0) {
+          *err = "problem " + std::to_string(b0 + g) + ": the eigensolver reported info " + std::to_string(info[g]);
+          return TZR_ERR_CUDA;
+        }
+      b0 = b1;
+      continue;
+    }
     for (int iter = 0; (double)iter < maxit; ++iter) {
       cbt_sym_kernel<<<ge, 256, 0, st>>>(w.pr, nmax, w.M, w.Bm);
       if (int rc = eig(CUSOLVER_EIG_MODE_VECTOR)) return rc;

@@ -243,19 +243,24 @@ int fpfh_plan(int B, const int32_t* n, double normal_radius, double fpfh_radius,
 int launch_fpfh(const FpfhPlan& plan, const float* pts, FpfhCloud* clouds, double normal_radius, double fpfh_radius,
                 float4* normals, float* spfh, float* out, int* overflow, void* grid_scratch, cudaStream_t st);
 
-// certify.cu (DRSCertifier::certify, certification.cc:40-190); mode 0 certify, 1 initial matrix, 2 dual projection
+// certify.cu (DRSCertifier::certify, certification.cc:40-190); mode 0 certify, 1 initial matrix, 2 dual projection,
+// 3 nearest-PSD step (W_in -> Wd_out, eigenvalues in w_out)
 int certify_device(int mode, double noise_bound, double cbar2, double sub_optimality, double max_iterations,
                    double gamma_tau, const double* R_cm, const double* src, const double* dst, const double* theta,
                    int N, int* is_optimal, double* best_subopt, int* n_iters, double* traj, int traj_cap,
-                   double* M_init_out, double* mu_out, const double* W_in, double* Wd_out, void** scratch,
-                   size_t* scratch_cap, void** solver_handle, int64_t* launches, cudaStream_t st, std::string* err);
+                   double* M_init_out, double* mu_out, const double* W_in, double* Wd_out, double* w_out,
+                   void** scratch, size_t* scratch_cap, void** solver_handle, int64_t* launches, cudaStream_t st,
+                   std::string* err);
 // B problems (host pointers, validated by the caller) in device-sized groups of one launch sequence each; loop_eig: one
-// cusolverDnDsyevd per active problem instead of cusolverDnXsyevBatched (debug flag 2097152)
-int certify_batch_device(const tzr_certifier_params& prm, int B, const int32_t* N, const double* R_cm,
+// cusolverDnDsyevd per active problem instead of cusolverDnXsyevBatched (debug flag 2097152).  mode 0 certify; the
+// building blocks run one step of the batch's iteration on X_in[b] (n x n) into X_out[b]: 1 nearest-PSD step, 2 dual
+// projection (theta as for mode 0; src, dst, R_cm, results and traj unused)
+int certify_batch_device(int mode, const tzr_certifier_params& prm, int B, const int32_t* N, const double* R_cm,
                          const double* const* src, const double* const* dst, const double* const* theta,
                          tzr_certification_result* results, double* const* traj, const int32_t* traj_cap,
-                         bool loop_eig, void** scratch, size_t* scratch_cap, void** solver_handle, int64_t* launches,
-                         cudaStream_t st, std::string* err);
+                         const double* const* X_in, double* const* X_out, bool loop_eig, void** scratch,
+                         size_t* scratch_cap, void** solver_handle, int64_t* launches, cudaStream_t st,
+                         std::string* err);
 void certify_release(void* solver_handle);
 
 // matcher.cu (Matcher::calculateCorrespondences, matcher.cc:21-337), over B cloud pairs stored back to back

@@ -1,6 +1,7 @@
 """CPU checks of the certifier batch (tzr_certify_batch, DESIGN.md 3.9).
 
-The batch pads every problem's symmetric matrix to the batch's largest size with c * I (c > 0) in the pad block and
+The batch pads every problem's symmetric matrix to the batch's largest size with c * I (c > 0) in the pad block, c the
+largest power of two not above the largest |entry| of the problem's starting matrix (pad_value below), and
 decomposes the padded matrices together.  These tests check, with numpy and oracle/certifier_oracle.py, that the two
 quantities the certifier takes from a decomposition do not change under that padding: the positive-part projection
 V+ L+ V+^T restricted to the real block, and the sub-optimality gap of certification.cc:192-231.  They also check the
@@ -20,10 +21,14 @@ import certifier_fixtures as cf  # noqa: E402
 
 capi = importlib.import_module("teaser-plusplus_b200.capi")
 HEADER = os.path.join(ROOT, "include", "teaser_b200.h")
-PAD = 1.0  # kCertPad in csrc/certify.cu
+def pad_value(A):
+    """cert_pad in csrc/certify.cu: the largest power of two not above max |A|, 1 for a zero matrix."""
+    m = np.abs(A).max()
+    return float(np.ldexp(1.0, np.frexp(m)[1] - 1)) if m > 0 else 1.0
 
 
-def _pad(A, nmax, c=PAD):
+def _pad(A, nmax, c=None):
+    c = pad_value(A) if c is None else c
     n = A.shape[0]
     P = np.zeros((nmax, nmax))
     P[:n, :n] = A
@@ -113,7 +118,7 @@ def test_pad_value_positive_keeps_nonpositive_minimum():
     """The smallest eigenvalue is unchanged whenever it is <= 0, for any c > 0; when it is > 0 the gap is 0 either
     way."""
     rng = np.random.default_rng(7)
-    for c in (1e-6, 0.5, PAD, 30.0):
+    for c in (1e-6, 0.5, 1.0, 30.0, None):
         A = _random_sym(rng, 24, rng.uniform(-1, 2, 24))
         A = (A + A.T) / 2
         w0 = np.linalg.eigvalsh(A)[0]
@@ -172,3 +177,14 @@ def test_entry_point_exported_declared_bound_and_flag_documented():
     assert "tzr_certify_batch" in capi._SYMBOLS
     assert len(capi.lib().tzr_certify_batch.argtypes) == len(args)
     assert "bit 21 (2097152)" in raw
+
+
+@pytest.mark.parametrize("k", [-1074, -1060, -40, -1, 0, 1, 40, 1000])
+def test_pad_value_follows_the_scale_exactly(k):
+    """The pad is a power of two in (max|A| / 2, max|A|], so scaling A by 2^k scales it by 2^k: the padded matrix
+    scales exactly and its norm is the real block's."""
+    A = np.array([[0.75, -3.0], [-3.0, 1.5]])
+    c = pad_value(np.ldexp(A, k))
+    assert c == np.ldexp(pad_value(A), k) == np.ldexp(2.0, k)
+    assert c <= np.abs(np.ldexp(A, k)).max() < 2 * c
+    assert pad_value(np.zeros((4, 4))) == 1.0
