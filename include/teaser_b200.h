@@ -222,6 +222,17 @@ int tzr_compute_fpfh_batch(tzr_ctx* ctx, int B, const int32_t* n, const float* c
                            double normal_search_radius, double fpfh_search_radius, float* const* fpfh_out,
                            float* const* normals_out, int32_t* status);
 
+/* Building blocks of tzr_compute_fpfh, exposed so that each can be checked on any input, not only on the ones a cloud
+ * produces.  Host pointers, synchronous; each runs the production device function, one item per thread.
+ * tzr_fpfh_pair_features: pcl::computePairFeatures (features/src/pfh_tools.cpp) on n point pairs: p1, n1, p2, n2 are
+ *   n x 3 floats (points and normals); f_out (n x 3) receives (f1, f2, f3), ok_out (n int32) 1 where the features are
+ *   defined and 0 where they are not (coincident points, or a zero cross product); f_out is zero there.
+ * tzr_fpfh_smallest_eigenpair: pcl::eigen33's smallest eigenpair (common/impl/eigen.hpp) of n symmetric 3 x 3 float
+ *   matrices: cov is n x 9 (row-major); ev_out (n) and vec_out (n x 3, unit length). */
+int tzr_fpfh_pair_features(tzr_ctx* ctx, int n, const float* p1, const float* n1, const float* p2, const float* n2,
+                           float* f_out, int32_t* ok_out);
+int tzr_fpfh_smallest_eigenpair(tzr_ctx* ctx, int n, const float* cov, float* ev_out, float* vec_out);
+
 /* Correspondences of B cloud pairs: pair b has ns[b] source points (src_pts[b], src_feat[b]) and nd[b] target points
  * (dst_pts[b], dst_feat[b]); dim and the flags apply to every pair; tuple_seeds: B seeds.  pairs[b]: capacity[b] x 2
  * int32 rows.  n_pairs[b] (B entries) is always set.  If some pair needs more than capacity[b] rows the call returns
@@ -385,8 +396,11 @@ int tzr_solve_batch_multi(const int32_t* devices, int n_devices, const tzr_param
  * large clique route at every n (tzr_ctx_clique_route), so that the two routes can be compared on the same graphs,
  * bit 20 (1048576) = cap the large route's compacted core at 64 vertices instead of 32768, so that its "core too large"
  * outcome is reachable at test sizes, bit 21 (2097152) = tzr_certify_batch loops cusolverDnDsyevd over the active
- * problems instead of one cusolverDnXsyevBatched call, so that the two eigen routes can be compared on the same batch.
- * Bits 15 to 21 change host code only. */
+ * problems instead of one cusolverDnXsyevBatched call, so that the two eigen routes can be compared on the same batch,
+ * bit 22 (4194304) = tzr_compute_fpfh(_batch) searches every cloud's radius neighbours by brute force, bit 23
+ * (8388608) = through the hashed grid at any cloud size (DESIGN.md 3.7; a cloud the grid cannot index still falls back
+ * to brute force), so that the two routes can be compared on one input; bit 22 wins when both are set.
+ * Bits 15 to 23 change host code only. */
 int tzr_ctx_set_flags(tzr_ctx* ctx, uint32_t flags);
 int64_t tzr_ctx_filter_mismatches(tzr_ctx* ctx);
 /* Number of pairs of the most recent graph build that needed the exact FP64 re-check. */

@@ -64,13 +64,22 @@ inline float det_atan_pos(float x) {  // x >= 0
   return y + p;
 }
 
+// std::atan2's special values: atan2(+-0, x) is +-0 for x >= +0 and +-pi for x <= -0; both infinite: +-pi/4, +-3pi/4
 inline float det_atan2(float y, float x) {
   if (x != x || y != y) return std::numeric_limits<float>::quiet_NaN();
-  if (y == 0.0f) return (x < 0.0f) ? kPiF : 0.0f;
+  if (y == 0.0f) return std::signbit(x) ? std::copysign(kPiF, y) : y;
   if (x == 0.0f) return y > 0.0f ? kPio2F : -kPio2F;
+  if (std::isinf(x) && std::isinf(y)) return std::copysign(x > 0.0f ? kPio4F : 3.0f * kPio4F, y);
   float a = det_atan_pos(std::fabs(y) / std::fabs(x));
   if (x < 0.0f) a = kPiF - a;
   return y < 0.0f ? -a : a;
+}
+
+// computeRoots' angle: y = sqrt(-q) is +0 or -0 (sqrt(-0) = -0) when q = 0, and both zeros give pi for x < 0 and 0
+// otherwise, so that theta stays in det_sincos_0_pi2's domain [0, pi/3]
+inline float det_atan2_roots(float y, float x) {
+  if (y == 0.0f && x == x) return (x < 0.0f) ? kPiF : 0.0f;
+  return det_atan2(y, x);
 }
 
 inline float det_asin_small(float x) {  // |x| <= 0.5
@@ -132,7 +141,7 @@ void compute_roots(const float m[3][3], float* roots) {
   float q = half_b * half_b + a_over_3 * a_over_3 * a_over_3;
   if (q > 0.0f) q = 0.0f;
   const float rho = std::sqrt(-a_over_3);
-  const float theta = det_atan2(std::sqrt(-q), half_b) * s_inv3;  // in [0, pi/3]
+  const float theta = det_atan2_roots(std::sqrt(-q), half_b) * s_inv3;  // in [0, pi/3]
   float cos_theta, sin_theta;
   det_sincos_0_pi2(theta, &sin_theta, &cos_theta);
   roots[0] = c2_over_3 + 2.0f * rho * cos_theta;
@@ -348,6 +357,39 @@ void orc_fpfh_from_normals(const float* pts, const float* normals, int n, double
       float sc = sum[s];
       if (sc != 0) sc = static_cast<float>(100.0 / sc);
       for (int k = 0; k < 11; ++k) o[11 * s + k] *= sc;
+    }
+  }
+}
+
+// The building blocks, with tzr_fpfh_pair_features / tzr_fpfh_smallest_eigenpair's layouts (include/teaser_b200.h).
+void orc_fpfh_pair_features(int n, const float* p1, const float* n1, const float* p2, const float* n2, float* f_out,
+                            int32_t* ok_out) {
+  for (int i = 0; i < n; ++i) {
+    const size_t o = 3 * (size_t)i;
+    float f4;
+    ok_out[i] = pair_features(p1 + o, n1 + o, p2 + o, n2 + o, f_out + o, f_out + o + 1, f_out + o + 2, &f4);
+  }
+}
+
+void orc_fpfh_smallest_eigenpair(int n, const float* cov, float* ev_out, float* vec_out) {
+  for (int i = 0; i < n; ++i) {
+    float m[3][3];
+    for (int k = 0; k < 9; ++k) m[k / 3][k % 3] = cov[9 * (size_t)i + k];
+    eigen33_smallest(m, ev_out + i, vec_out + 3 * (size_t)i);
+  }
+}
+
+// The elementary functions on their own: fn 0 det_atan2(a, b), 1 det_acos01(a), 2 / 3 the sine / cosine of
+// det_sincos_0_pi2(a).
+void orc_fpfh_elementary(int fn, int n, const float* a, const float* b, float* out) {
+  for (int i = 0; i < n; ++i) {
+    float s, c;
+    switch (fn) {
+      case 0: out[i] = det_atan2(a[i], b[i]); break;
+      case 1: out[i] = det_acos01(a[i]); break;
+      default:
+        det_sincos_0_pi2(a[i], &s, &c);
+        out[i] = fn == 2 ? s : c;
     }
   }
 }

@@ -98,7 +98,12 @@ _SYMBOLS = [
     "tzr_ctx_stage_log_read", "tzr_solve_batch_multi", "tzr_ctx_clique_info", "tzr_compute_fpfh_batch",
     "tzr_match_correspondences_batch", "tzr_ctx_set_max_n", "tzr_ctx_clique_route", "tzr_certify_batch",
     "tzr_certifier_psd_projection", "tzr_certifier_batch_psd_projection", "tzr_certifier_batch_dual_projection",
+    "tzr_fpfh_pair_features", "tzr_fpfh_smallest_eigenpair",
 ]
+
+# debug flags of tzr_ctx_set_flags that choose tzr_compute_fpfh(_batch)'s radius search for every cloud
+FLAG_FPFH_BRUTE_FORCE = 4194304
+FLAG_FPFH_GRID = 8388608
 
 
 def build(verbose: bool = False):
@@ -169,6 +174,8 @@ def lib():
     L.tzr_compute_fpfh.argtypes = [vp, fp, C.c_int, C.c_double, C.c_double, fp, fp]
     fpp = C.POINTER(fp)
     L.tzr_compute_fpfh_batch.argtypes = [vp, C.c_int, i32p, fpp, C.c_double, C.c_double, fpp, fpp, i32p]
+    L.tzr_fpfh_pair_features.argtypes = [vp, C.c_int, fp, fp, fp, fp, fp, i32p]
+    L.tzr_fpfh_smallest_eigenpair.argtypes = [vp, C.c_int, fp, fp, fp]
     L.tzr_match_correspondences_batch.argtypes = [vp, C.c_int, i32p, fpp, i32p, fpp, fpp, fpp, C.c_int, C.c_int,
                                                   C.c_int, C.c_int, C.c_float, u64p, C.POINTER(i32p), i64p, i64p, fp]
     L.tzr_certifier_params_default.argtypes = [C.POINTER(CertifierParams)]
@@ -584,6 +591,37 @@ class Context:
             e.status, e.result = status, result
             raise
         return result
+
+    @staticmethod
+    def _rows3(a, n, what):
+        a = np.ascontiguousarray(a, dtype=np.float32)
+        if a.shape != (n, 3):
+            raise TzrError(f"{what}: every input must be (n,3)")
+        return a
+
+    def fpfh_pair_features(self, p1, n1, p2, n2):
+        """pcl::computePairFeatures on n pairs of (point, normal), each (n,3): ((n,3) float32 f1, f2, f3, (n,) bool ok),
+        the device function the SPFH kernel runs; rows where ok is False are zero."""
+        n = np.asarray(p1).shape[0]
+        ins = [self._rows3(a, n, "fpfh_pair_features") for a in (p1, n1, p2, n2)]
+        f = np.zeros((n, 3), dtype=np.float32)
+        ok = np.zeros(n, dtype=np.int32)
+        self._ck(lib().tzr_fpfh_pair_features(self._h, n, *[_p(a, C.c_float) for a in ins], _p(f, C.c_float),
+                                              _p(ok, C.c_int32)))
+        return f, ok.astype(bool)
+
+    def fpfh_smallest_eigenpair(self, cov):
+        """pcl::eigen33's smallest eigenpair of every symmetric (3,3) float32 matrix of an (n,3,3) array, the device
+        function the normals kernel runs: ((n,) eigenvalues, (n,3) unit eigenvectors)."""
+        c = np.ascontiguousarray(cov, dtype=np.float32)
+        if c.ndim != 3 or c.shape[1:] != (3, 3) or c.shape[0] == 0:
+            raise TzrError("fpfh_smallest_eigenpair: cov must be (n,3,3) with n >= 1")
+        n = c.shape[0]
+        ev = np.zeros(n, dtype=np.float32)
+        vec = np.zeros((n, 3), dtype=np.float32)
+        self._ck(lib().tzr_fpfh_smallest_eigenpair(self._h, n, _p(c, C.c_float), _p(ev, C.c_float),
+                                                   _p(vec, C.c_float)))
+        return ev, vec
 
     def match_correspondences_batch(self, src_pts, dst_pts, src_feat, dst_feat, use_absolute_scale=True,
                                     use_crosscheck=True, use_tuple_test=True, tuple_scale=0.0, tuple_seeds=None,

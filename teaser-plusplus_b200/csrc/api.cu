@@ -711,7 +711,8 @@ int fpfh_run(tzr_ctx* ctx, int B, const int32_t* n, const float* const* pts, dou
   }
   std::vector<FpfhCloud> clouds((size_t)B);
   FpfhPlan plan;
-  if (fpfh_plan(B, n, normal_radius, fpfh_radius, clouds.data(), &plan) != TZR_OK) {
+  const int route = (ctx->flags & 4194304u) ? kFpfhRouteBrute : (ctx->flags & 8388608u) ? kFpfhRouteGrid : kFpfhRouteAuto;
+  if (fpfh_plan(B, n, normal_radius, fpfh_radius, route, clouds.data(), &plan) != TZR_OK) {
     ctx->last_error = "the batch's points do not fit 32-bit indices";
     return TZR_ERR_TOO_LARGE;
   }
@@ -1587,6 +1588,51 @@ int tzr_compute_fpfh_batch(tzr_ctx* ctx, int B, const int32_t* n, const float* c
                            double normal_search_radius, double fpfh_search_radius, float* const* fpfh_out,
                            float* const* normals_out, int32_t* status) {
   return fpfh_run(ctx, B, n, pts, normal_search_radius, fpfh_search_radius, fpfh_out, normals_out, status);
+}
+
+int tzr_fpfh_pair_features(tzr_ctx* ctx, int n, const float* p1, const float* n1, const float* p2, const float* n2,
+                           float* f_out, int32_t* ok_out) {
+  if (!ctx || n <= 0 || !p1 || !n1 || !p2 || !n2 || !f_out || !ok_out) return TZR_ERR_INVALID_ARG;
+  cudaSetDevice(ctx->device);
+  cudaStream_t st = ctx->stream;
+  const size_t vb = (size_t)n * 12;
+  int rc;
+  if ((rc = ensure(ctx, ctx->m_in, 4 * al256(vb))) != TZR_OK) return rc;
+  if ((rc = ensure(ctx, ctx->m_out, al256(vb) + (size_t)n * 4)) != TZR_OK) return rc;
+  char* d_in = (char*)ctx->m_in.p;
+  const float* h_in[4] = {p1, n1, p2, n2};
+  for (int k = 0; k < 4; ++k) CK(cudaMemcpyAsync(d_in + k * al256(vb), h_in[k], vb, cudaMemcpyHostToDevice, st));
+  float* d_f = (float*)ctx->m_out.p;
+  int32_t* d_ok = (int32_t*)((char*)ctx->m_out.p + al256(vb));
+  launch_fpfh_pair_features(n, (const float*)d_in, (const float*)(d_in + al256(vb)),
+                            (const float*)(d_in + 2 * al256(vb)), (const float*)(d_in + 3 * al256(vb)), d_f, d_ok, st);
+  ctx->launches += 1;
+  if ((rc = check_launch(ctx, "pair features launch")) != TZR_OK) return rc;
+  CK(cudaMemcpyAsync(f_out, d_f, vb, cudaMemcpyDeviceToHost, st));
+  CK(cudaMemcpyAsync(ok_out, d_ok, (size_t)n * 4, cudaMemcpyDeviceToHost, st));
+  CK(cudaStreamSynchronize(st));
+  return TZR_OK;
+}
+
+int tzr_fpfh_smallest_eigenpair(tzr_ctx* ctx, int n, const float* cov, float* ev_out, float* vec_out) {
+  if (!ctx || n <= 0 || !cov || !ev_out || !vec_out) return TZR_ERR_INVALID_ARG;
+  cudaSetDevice(ctx->device);
+  cudaStream_t st = ctx->stream;
+  const size_t cb = (size_t)n * 36, eb = (size_t)n * 4, vb = (size_t)n * 12;
+  int rc;
+  if ((rc = ensure(ctx, ctx->m_in, cb)) != TZR_OK) return rc;
+  if ((rc = ensure(ctx, ctx->m_out, al256(eb) + vb)) != TZR_OK) return rc;
+  float* d_cov = (float*)ctx->m_in.p;
+  float* d_ev = (float*)ctx->m_out.p;
+  float* d_vec = (float*)((char*)ctx->m_out.p + al256(eb));
+  CK(cudaMemcpyAsync(d_cov, cov, cb, cudaMemcpyHostToDevice, st));
+  launch_fpfh_smallest_eigenpair(n, d_cov, d_ev, d_vec, st);
+  ctx->launches += 1;
+  if ((rc = check_launch(ctx, "smallest eigenpair launch")) != TZR_OK) return rc;
+  CK(cudaMemcpyAsync(ev_out, d_ev, eb, cudaMemcpyDeviceToHost, st));
+  CK(cudaMemcpyAsync(vec_out, d_vec, vb, cudaMemcpyDeviceToHost, st));
+  CK(cudaStreamSynchronize(st));
+  return TZR_OK;
 }
 
 int tzr_feature_nn(tzr_ctx* ctx, const float* query, int nq, const float* db, int ndb, int dim, int32_t* nn_index,

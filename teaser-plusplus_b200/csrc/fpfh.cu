@@ -20,7 +20,9 @@
 // by bucket (CUB radix sort — library call, like the matcher's), every query visits the <= 27 distinct buckets of its
 // 3x3x3 cell neighbourhood and applies the SAME float distance test, so the neighbour sets — and everything downstream —
 // are identical to the brute-force ones (a point two cells away is farther than the radius by more than the float
-// error of the test; hash collisions only add candidates that fail it).
+// error of the test; hash collisions only add candidates that fail it).  A cloud with a finite point too far from its
+// bounding-box minimum for an accurate double cell index (kCellIndexMax) is searched by brute force.  Debug flags
+// 4194304 / 8388608 force brute force / the grid for every cloud.
 //
 // Batches: every kernel runs over B clouds stored back to back (one CTA per point of the whole batch); a CTA finds its
 // cloud from the per-cloud FpfhCloud table and searches only inside it.  Each grid cloud owns the bucket range
@@ -62,13 +64,22 @@ __device__ __forceinline__ float det_atan_pos(float x) {  // x >= 0
   return y + p;
 }
 
+// std::atan2's special values: atan2(+-0, x) is +-0 for x >= +0 and +-pi for x <= -0; both infinite: +-pi/4, +-3pi/4
 __device__ __forceinline__ float det_atan2(float y, float x) {
   if (x != x || y != y) return CUDART_NAN_F;
-  if (y == 0.0f) return (x < 0.0f) ? kPiF : 0.0f;
+  if (y == 0.0f) return signbit(x) ? copysignf(kPiF, y) : y;
   if (x == 0.0f) return y > 0.0f ? kPio2F : -kPio2F;
+  if (isinf(x) && isinf(y)) return copysignf(x > 0.0f ? kPio4F : 3.0f * kPio4F, y);
   float a = det_atan_pos(fabsf(y) / fabsf(x));
   if (x < 0.0f) a = kPiF - a;
   return y < 0.0f ? -a : a;
+}
+
+// computeRoots' angle: y = sqrtf(-q) is +0 or -0 (sqrtf(-0) = -0) when q = 0, and both zeros give pi for x < 0 and 0
+// otherwise, so that theta stays in det_sincos_0_pi2's domain [0, pi/3]
+__device__ __forceinline__ float det_atan2_roots(float y, float x) {
+  if (y == 0.0f && x == x) return (x < 0.0f) ? kPiF : 0.0f;
+  return det_atan2(y, x);
 }
 
 __device__ __forceinline__ float det_asin_small(float x) {  // |x| <= 0.5
@@ -130,7 +141,7 @@ __device__ void compute_roots(const float m[3][3], float* roots) {
   float q = half_b * half_b + a_over_3 * a_over_3 * a_over_3;
   if (q > 0.0f) q = 0.0f;
   const float rho = sqrtf(-a_over_3);
-  const float theta = det_atan2(sqrtf(-q), half_b) * s_inv3;
+  const float theta = det_atan2_roots(sqrtf(-q), half_b) * s_inv3;
   float cos_theta, sin_theta;
   det_sincos_0_pi2(theta, &sin_theta, &cos_theta);
   roots[0] = c2_over_3 + 2.0f * rho * cos_theta;
@@ -247,12 +258,25 @@ __device__ __forceinline__ unsigned int cell_hash(long long ix, long long iy, lo
   return ((unsigned int)(ix * 73856093ll) ^ (unsigned int)(iy * 19349663ll) ^ (unsigned int)(iz * 83492791ll)) & mask;
 }
 
+// Largest cell index the grid uses.  The index is u = fl(fl(x - o) * fl(1/h)) with x and the origin o floats (exact in
+// double): the subtraction and the product each round by at most 2^-53 relative, and fl(1/h) and h = r (1 + 1e-5)
+// carry two more such roundings, so |u - (x - o)/h| <= |u| 2^-51 (to first order).  Two points that pass the float
+// test d^2 < r^2 are at most r (1 + 2^-20) apart per axis (the test's own rounding is a few 2^-24 relative), so their
+// exact indices differ by at most (1 + 2^-20) / (1 + 1e-5) < 1 - 9e-6.  Their floors then differ by at most 1, which
+// is what the 3x3x3 search needs, while the two index errors sum to less than 9e-6.  With |u| < 2^32 each error is at
+// most 2^-19 < 1.91e-6, well inside that margin.  The bound grows with the extent and passes half the margin (4.5e-6)
+// near 1e10 cells, about 2^33 (one far point at 1e11 with r = 0.01 is 2^43 cells: true neighbours land two cells
+// apart), so a cloud
+// with a finite point outside the range is searched by brute force.
+constexpr double kCellIndexMax = 4294967296.0;  // 2^32
+
 __device__ __forceinline__ bool cell_of(const Grid& g, float x, float y, float z, long long* ix, long long* iy,
                                         long long* iz) {
   if (!(x == x) || !(y == y) || !(z == z)) return false;
   const double fx = floor(((double)x - g.ox) * g.inv_h), fy = floor(((double)y - g.oy) * g.inv_h),
                fz = floor(((double)z - g.oz) * g.inv_h);
-  if (!(fabs(fx) < 4e18) || !(fabs(fy) < 4e18) || !(fabs(fz) < 4e18)) return false;  // +-inf coordinates
+  // +-inf coordinates, and finite ones too far from the origin for an accurate index
+  if (!(fabs(fx) < kCellIndexMax) || !(fabs(fy) < kCellIndexMax) || !(fabs(fz) < kCellIndexMax)) return false;
   *ix = (long long)fx;
   *iy = (long long)fy;
   *iz = (long long)fz;
@@ -295,7 +319,7 @@ __global__ void bbox_min_kernel(const float* __restrict__ pts, int N, FpfhCloud*
     if (clouds[c].grid)
       for (int k = 0; k < 3; ++k) {
         const float v = pts[3 * (size_t)i + k];
-        if (v == v && fabsf(v) < 3.0e38f) m[k] = f2ord(v);
+        if (isfinite(v)) m[k] = f2ord(v);
       }
   }
   const bool uniform = __all_sync(0xffffffffu, c == __shfl_sync(0xffffffffu, c, 0));
@@ -328,9 +352,9 @@ __global__ void bucket_kernel(const float* __restrict__ pts, int N, FpfhCloud* c
   const float x = pts[3 * (size_t)i], y = pts[3 * (size_t)i + 1], z = pts[3 * (size_t)i + 2];
   const bool ok = cell_of(g, x, y, z, &ix, &iy, &iz);
   keys[i] = ok ? cl.base + cell_hash(ix, iy, iz, cl.mask) : buckets;
-  // a finite point the grid cannot index (extent / radius beyond 2^62 cells): this cloud falls back to brute force
-  if (!ok && x == x && y == y && z == z && fabsf(x) < 3.0e38f && fabsf(y) < 3.0e38f && fabsf(z) < 3.0e38f)
-    cl.mins[3] = 1;
+  // a finite point the grid cannot index accurately (kCellIndexMax cells or more from the origin): this cloud falls
+  // back to brute force
+  if (!ok && isfinite(x) && isfinite(y) && isfinite(z)) cl.mins[3] = 1;
 }
 
 __global__ void bucket_bounds_kernel(const unsigned int* __restrict__ keys, int n, unsigned int buckets,
@@ -587,6 +611,31 @@ __global__ void __launch_bounds__(kFpfhThreads) fpfh_kernel(Clouds cs, const flo
   for (int k = 0; k < 11; ++k) out[(size_t)p * 33 + 11 * s + k] = acc[k] * sc;
 }
 
+// tzr_fpfh_pair_features / tzr_fpfh_smallest_eigenpair: the production device functions, one item per thread
+__global__ void pair_features_kernel(int n, const float* __restrict__ p1, const float* __restrict__ n1,
+                                     const float* __restrict__ p2, const float* __restrict__ n2, float* __restrict__ f,
+                                     int32_t* __restrict__ ok) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  float f1, f2, f3;
+  const size_t o = 3 * (size_t)i;
+  const bool good = pair_features(p1 + o, n1 + o, p2 + o, n2 + o, &f1, &f2, &f3);
+  f[o] = good ? f1 : 0.f;
+  f[o + 1] = good ? f2 : 0.f;
+  f[o + 2] = good ? f3 : 0.f;
+  ok[i] = good;
+}
+
+__global__ void smallest_eigenpair_kernel(int n, const float* __restrict__ cov, float* __restrict__ ev,
+                                          float* __restrict__ vec) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  float m[3][3], v[3];
+  for (int k = 0; k < 9; ++k) m[k / 3][k % 3] = cov[9 * (size_t)i + k];
+  eigen33_smallest(m, &ev[i], v);
+  for (int k = 0; k < 3; ++k) vec[3 * (size_t)i + k] = v[k];
+}
+
 size_t radix_bytes(int n, int bits) {
   size_t cub_bytes = 0;
   cub::DeviceRadixSort::SortPairs(nullptr, cub_bytes, (const unsigned int*)nullptr, (unsigned int*)nullptr,
@@ -602,7 +651,8 @@ int key_bits(unsigned int buckets) {  // keys go up to `buckets` (the sentinel)
 
 }  // namespace
 
-int fpfh_plan(int B, const int32_t* n, double normal_radius, double fpfh_radius, FpfhCloud* clouds, FpfhPlan* plan) {
+int fpfh_plan(int B, const int32_t* n, double normal_radius, double fpfh_radius, int route, FpfhCloud* clouds,
+              FpfhPlan* plan) {
   const double h = std::max(normal_radius, fpfh_radius) * (1.0 + 1e-5);
   long long lo = 0, buckets = 0;
   bool any_grid = false;
@@ -611,7 +661,7 @@ int fpfh_plan(int B, const int32_t* n, double normal_radius, double fpfh_radius,
     cl = FpfhCloud{};
     cl.lo = (int)lo;
     cl.n = n[c];
-    cl.grid = n[c] >= kGridMinN;
+    cl.grid = route == kFpfhRouteBrute ? 0 : route == kFpfhRouteGrid ? 1 : n[c] >= kGridMinN;
     cl.mins[0] = cl.mins[1] = cl.mins[2] = 0x7fffffff;
     cl.mins[3] = 0;
     cl.inv_h = 1.0 / h;
@@ -669,6 +719,15 @@ int launch_fpfh(const FpfhPlan& plan, const float* pts, FpfhCloud* clouds, doubl
   spfh_kernel<<<N, kFpfhThreads, 0, st>>>(cs, normals, r2f, spfh, overflow);
   fpfh_kernel<<<N, kFpfhThreads, 0, st>>>(cs, spfh, r2f, out, overflow);
   return nl + 3;
+}
+
+void launch_fpfh_pair_features(int n, const float* p1, const float* n1, const float* p2, const float* n2, float* f,
+                               int32_t* ok, cudaStream_t st) {
+  pair_features_kernel<<<(n + 255) / 256, 256, 0, st>>>(n, p1, n1, p2, n2, f, ok);
+}
+
+void launch_fpfh_smallest_eigenpair(int n, const float* cov, float* ev, float* vec, cudaStream_t st) {
+  smallest_eigenpair_kernel<<<(n + 255) / 256, 256, 0, st>>>(n, cov, ev, vec);
 }
 
 }  // namespace tzr

@@ -223,10 +223,11 @@ void launch_translation_only(const double* src, const double* dst, int m, double
 // fpfh.cu (FPFHEstimation::computeFPFHFeatures, fpfh.cc:15-43), over B clouds stored back to back
 struct FpfhCloud {     // one per cloud, filled by fpfh_plan, read by the kernels from device memory
   int lo, n;           // first point of the cloud in the flat array, point count
-  int grid;            // 1: radius search through the hashed grid (n >= kGridMinN), 0: brute force
+  int grid;            // 1: radius search through the hashed grid (n >= kGridMinN, or forced), 0: brute force
   unsigned int mask;   // T_b - 1 (T_b buckets, a power of two)
   unsigned int base;   // first bucket of the cloud in the batch's bucket range
-  int mins[4];         // bounding-box minimum (ordered-int floats; the grid origin); [3] = 1: the grid cannot index
+  int mins[4];         // bounding-box minimum of the finite coordinates (ordered-int floats; the grid origin); [3] = 1:
+                       // a finite point lies outside the grid's accurate index range, the cloud uses brute force
   double inv_h;        // 1 / cell edge
 };
 struct FpfhPlan {
@@ -235,13 +236,23 @@ struct FpfhPlan {
   unsigned int buckets = 0;    // sum of T_b over the grid clouds (also the sentinel key of unsorted points)
   size_t grid_bytes = 0;       // device scratch of the grid path (0 without grid clouds)
 };
+// Radius-search route of every cloud: by size (the grid from kGridMinN points on), or forced by the debug flags
+// 4194304 (brute force) and 8388608 (the grid at any size).
+constexpr int kFpfhRouteAuto = 0, kFpfhRouteBrute = 1, kFpfhRouteGrid = 2;
 // Fills clouds[0..B) (host copy, to be staged to the device before launch_fpfh) and the plan.  TZR_ERR_TOO_LARGE when
 // the points or buckets of the batch do not fit 32-bit indices.
-int fpfh_plan(int B, const int32_t* n, double normal_radius, double fpfh_radius, FpfhCloud* clouds, FpfhPlan* plan);
+int fpfh_plan(int B, const int32_t* n, double normal_radius, double fpfh_radius, int route, FpfhCloud* clouds,
+              FpfhPlan* plan);
 // pts (plan.N x 3), clouds (device copy of fpfh_plan's table), normals (N float4), spfh (N x 33), out (N x 33),
 // overflow (B ints, zeroed here), grid_scratch (plan.grid_bytes): device pointers.  Returns the launches.
 int launch_fpfh(const FpfhPlan& plan, const float* pts, FpfhCloud* clouds, double normal_radius, double fpfh_radius,
                 float4* normals, float* spfh, float* out, int* overflow, void* grid_scratch, cudaStream_t st);
+// The descriptor kernels' device functions on their own, one item per thread (device pointers; one launch each).
+// pair_features: p1, n1, p2, n2 are n x 3, f (n x 3) receives f1, f2, f3 and ok (n) 1 where pcl::computePairFeatures
+// succeeds; f is zero where it does not.  smallest_eigenpair: cov is n x 9 (row-major 3 x 3), ev (n), vec (n x 3).
+void launch_fpfh_pair_features(int n, const float* p1, const float* n1, const float* p2, const float* n2, float* f,
+                               int32_t* ok, cudaStream_t st);
+void launch_fpfh_smallest_eigenpair(int n, const float* cov, float* ev, float* vec, cudaStream_t st);
 
 // certify.cu (DRSCertifier::certify, certification.cc:40-190); mode 0 certify, 1 initial matrix, 2 dual projection,
 // 3 nearest-PSD step (W_in -> Wd_out, eigenvalues in w_out)

@@ -134,6 +134,12 @@ def lib():
     L.orc_nn1.restype = None
     L.orc_compute_fpfh.argtypes = [fp, C.c_int, C.c_double, C.c_double, C.c_int, fp, fp]
     L.orc_compute_fpfh.restype = None
+    L.orc_fpfh_pair_features.argtypes = [C.c_int, fp, fp, fp, fp, fp, i32p]
+    L.orc_fpfh_pair_features.restype = None
+    L.orc_fpfh_smallest_eigenpair.argtypes = [C.c_int, fp, fp, fp]
+    L.orc_fpfh_smallest_eigenpair.restype = None
+    L.orc_fpfh_elementary.argtypes = [C.c_int, C.c_int, fp, fp, fp]
+    L.orc_fpfh_elementary.restype = None
     _lib = L
     return L
 
@@ -329,6 +335,37 @@ def nn1(query, db):
     d = np.ascontiguousarray(db, dtype=np.float32)
     out = np.zeros(q.shape[0], dtype=np.int32)
     lib().orc_nn1(_p(q, C.c_float), q.shape[0], _p(d, C.c_float), d.shape[0], q.shape[1], _p(out, C.c_int32))
+    return out
+
+
+def fpfh_pair_features(p1, n1, p2, n2):
+    """pcl::computePairFeatures restatement on n pairs ((n,3) each): ((n,3) f1 f2 f3, (n,) bool ok)."""
+    ins = [np.ascontiguousarray(a, dtype=np.float32).reshape(-1, 3) for a in (p1, n1, p2, n2)]
+    n = ins[0].shape[0]
+    f = np.zeros((n, 3), dtype=np.float32)
+    ok = np.zeros(n, dtype=np.int32)
+    lib().orc_fpfh_pair_features(n, *[_p(a, C.c_float) for a in ins], _p(f, C.c_float), _p(ok, C.c_int32))
+    return f, ok.astype(bool)
+
+
+def fpfh_smallest_eigenpair(cov):
+    """pcl::eigen33 restatement on (n,3,3) float32 matrices: ((n,) eigenvalues, (n,3) vectors)."""
+    c = np.ascontiguousarray(cov, dtype=np.float32).reshape(-1, 3, 3)
+    n = c.shape[0]
+    ev = np.zeros(n, dtype=np.float32)
+    vec = np.zeros((n, 3), dtype=np.float32)
+    lib().orc_fpfh_smallest_eigenpair(n, _p(c, C.c_float), _p(ev, C.c_float), _p(vec, C.c_float))
+    return ev, vec
+
+
+def fpfh_elementary(fn, a, b=None):
+    """The FPFH restatement's elementary functions: fn 'atan2' (a = y, b = x), 'acos01', 'sin', 'cos' (of
+    det_sincos_0_pi2)."""
+    a = np.ascontiguousarray(a, dtype=np.float32).ravel()
+    b = np.ascontiguousarray(a if b is None else b, dtype=np.float32).ravel()
+    out = np.zeros(a.size, dtype=np.float32)
+    code = {"atan2": 0, "acos01": 1, "sin": 2, "cos": 3}[fn]
+    lib().orc_fpfh_elementary(code, a.size, _p(a, C.c_float), _p(b, C.c_float), _p(out, C.c_float))
     return out
 
 
