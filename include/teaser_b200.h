@@ -336,7 +336,13 @@ int tzr_solve(tzr_ctx* ctx, const tzr_params* params, const double* src_3xN, con
               tzr_solution* solution, int32_t* clique, uint8_t* rot_inliers, uint8_t* trans_inliers);
 
 /* B problems, problem b has n[b] correspondences at src[b] / dst[b] (host pointers).
- * cliques: B*max_n int32, problem b's clique at cliques + b*max_n (may be NULL). */
+ * cliques: B*max_n int32, problem b's clique at cliques + b*max_n (may be NULL).
+ * Sizes may differ.  A ragged batch runs as a few padded device batches (size classes, DESIGN.md 4.2): the problems,
+ * ordered by n, are cut wherever n falls below the class's largest n divided by sqrt(2); a problem above 32768 is a class
+ * of its own, and with estimate_scaling no class mixes problems on both sides of 256 (the two scale paths).  Padding rows
+ * are isolated vertices, and every stage uses each problem's own n where the result depends on it, so each solution
+ * (every field but stage_ms) and clique are the ones tzr_solve gives for that problem alone.  The classes share one
+ * workspace and one host synchronisation. */
 int tzr_solve_batch(tzr_ctx* ctx, const tzr_params* params, int B, const int32_t* n, const double* const* src,
                     const double* const* dst, tzr_solution* solutions, int32_t* cliques, int max_n);
 
@@ -346,10 +352,22 @@ int tzr_solve_batch(tzr_ctx* ctx, const tzr_params* params, int B, const int32_t
 int tzr_solve_batch_dev(tzr_ctx* ctx, const tzr_params* params, int B, int n, const double* src_dev,
                         const double* dst_dev, tzr_solution* solutions_dev, int32_t* cliques_dev);
 
+/* Device-resident ragged batch: problem b has n[b] >= 1 correspondences (n is a host array).  src_dev/dst_dev hold the
+ * problems back to back, sum(n) rows of 3 doubles each, problem b from row sum_{c<b} n[c] (the layout
+ * tzr_match_correspondences_batch's outputs give).  solutions_dev: B tzr_solution in the caller's order.  cliques_dev
+ * (sum(n) int32, may be NULL): problem b's sorted clique from the same row offset, -1 past its clique_size.  The size
+ * classes of tzr_solve_batch; the results are those of tzr_solve on each problem alone.  Asynchronous on the context's
+ * stream like tzr_solve_batch_dev, except that a class above 32768 correspondences reads back its core sizes. */
+int tzr_solve_batch_ragged_dev(tzr_ctx* ctx, const tzr_params* params, int B, const int32_t* n, const double* src_dev,
+                               const double* dst_dev, tzr_solution* solutions_dev, int32_t* cliques_dev);
+
 /* Retrieve the adjacency bitset / degrees of problem b of the most recent solve on this context
- * (lazy materialisation of getInlierGraph(), registration.h:772; SURVEY a16). Host pointers. */
+ * (lazy materialisation of getInlierGraph(), registration.h:772; SURVEY a16). Host pointers.  After a ragged batch,
+ * problem b (caller's order) has its own n[b] rows of tzr_words_per_row(n[b]) words and n[b] degrees, equal to its
+ * single-solve graph. */
 int tzr_last_graph(tzr_ctx* ctx, int b, uint64_t* adj_bits, int32_t* degree);
-/* What tzr_last_graph would return: batch size and n of the retained solve (0, 0 if none), whether a graph was
+/* What tzr_last_graph would return: batch size and n of the retained solve (0, 0 if none; the largest n after a ragged
+ * batch), whether a graph was
  * built (0 after inlier selection NONE: the reference never populates the graph, registration.cc:607-650, and
  * tzr_last_graph then yields an empty adjacency), and a generation counter that changes with every call that
  * rebuilds or invalidates the retained graph — callers that share a context (the C++ facade's per-thread context)
@@ -379,9 +397,9 @@ int tzr_solve_batch_multi(const int32_t* devices, int n_devices, const tzr_param
  * bit 1 (2) = verify the FP32 / tensor-core filter against FP64 for every pair and count mismatches,
  * bit 2 (4) = count exact re-checks and clique search nodes, bit 8 (256) = degrees by a separate pass,
  * bit 10 (1024) = build the graph with the tensor-core kernel (wgmma Gram norms; bit-identical to the default CUDA-core
- * kernel: DESIGN.md 3.1), bit 9 (512) = the square-root interval test for every problem (no Gram test, no tensor-core
+ * kernel: DESIGN.md 3.1; uniform batches only: the size classes of a ragged batch run the default kernel), bit 9 (512) = the square-root interval test for every problem (no Gram test, no tensor-core
  * kernel; bit-identical), bit 11 (2048) = the one-MUFU
- * CUDA-core variant (graph_strip3_kernel; bit-identical), bit 13 (8192) = exact clique
+ * CUDA-core variant (graph_strip3_kernel; bit-identical; uniform batches only, like bit 10), bit 13 (8192) = exact clique
  * search without the singleton-class path of the colouring (A/B), bit 12 (4096) = without the block colour bound (only
  * present in builds with -DTZR_BLOCK_BOUND), bit 14 (16384) = cap the graph kernels' re-check queue at 64 entries (the
  * buffer keeps its full size), so that the queue-full path (pairs evaluated in place by the graph kernel) runs at test
@@ -399,8 +417,10 @@ int tzr_solve_batch_multi(const int32_t* devices, int n_devices, const tzr_param
  * problems instead of one cusolverDnXsyevBatched call, so that the two eigen routes can be compared on the same batch,
  * bit 22 (4194304) = tzr_compute_fpfh(_batch) searches every cloud's radius neighbours by brute force, bit 23
  * (8388608) = through the hashed grid at any cloud size (DESIGN.md 3.7; a cloud the grid cannot index still falls back
- * to brute force), so that the two routes can be compared on one input; bit 22 wins when both are set.
- * Bits 15 to 23 change host code only. */
+ * to brute force), so that the two routes can be compared on one input; bit 22 wins when both are set, bit 24
+ * (16777216) = a ragged batch forms one size class wherever the large-route and scale-path rules allow, however far
+ * apart its sizes are, so that tests can pad n = 2 to n = 4000 in one device batch.
+ * Bits 15 to 24 change host code only. */
 int tzr_ctx_set_flags(tzr_ctx* ctx, uint32_t flags);
 int64_t tzr_ctx_filter_mismatches(tzr_ctx* ctx);
 /* Number of pairs of the most recent graph build that needed the exact FP64 re-check. */

@@ -86,6 +86,14 @@ for flags in (1024, 1024 | 2, 2048, 2048 | 2, 2048 | 1):
     sols, cl = ctx.solve_batch_array(src[:9], dst[:9], capi.default_params(**dict(kw, noise_bound=prs[0]["noise_bound"])))
     print("batch flags", flags, int(sols["valid"].sum()), "/ 9")
 ctx.set_flags(0)
+# ragged batch padded into one size class (debug flag 16777216): n = 1 ... 700 share one padded device batch
+rg = [synth.make_problem(n, 0.5, 40 + n, "ball") for n in (700, 1, 2, 129, 33, 300)]
+for rflags, est in ((16777216, 0), (16777216 | 2, 0), (16777216, 1)):
+    ctx.set_flags(rflags)
+    sols, cl = ctx.solve_batch([q["src"] for q in rg], [q["dst"] for q in rg],
+                               capi.default_params(noise_bound=rg[0]["noise_bound"], estimate_scaling=est))
+    print("ragged flags", rflags, "scale", est, [int(c) for c in sols["clique_size"]])
+ctx.set_flags(0)
 sols, cl = capi.solve_batch_multi([p["src"] for p in prs[:5]], [p["dst"] for p in prs[:5]],
                                   capi.default_params(**dict(kw, noise_bound=prs[0]["noise_bound"])))
 print("multi", int(sols["valid"].sum()), "/ 5")

@@ -91,7 +91,7 @@ _SYMBOLS = [
     "tzr_abi_version", "tzr_status_string", "tzr_last_error", "tzr_params_default", "tzr_ctx_create",
     "tzr_ctx_destroy", "tzr_ctx_set_stream", "tzr_ctx_synchronize", "tzr_ctx_kernel_launches", "tzr_words_per_row",
     "tzr_graph_build", "tzr_max_clique", "tzr_max_clique_batch", "tzr_gnc_tls_rotation", "tzr_rotation_solve", "tzr_tls_translation", "tzr_scalar_tls",
-    "tzr_solve", "tzr_solve_batch", "tzr_solve_batch_dev", "tzr_last_graph", "tzr_last_stage_ms",
+    "tzr_solve", "tzr_solve_batch", "tzr_solve_batch_dev", "tzr_solve_batch_ragged_dev", "tzr_last_graph", "tzr_last_stage_ms",
     "tzr_ctx_set_flags", "tzr_ctx_filter_mismatches", "tzr_ctx_filter_rechecks", "tzr_ctx_debug_counters",
     "tzr_match_correspondences", "tzr_feature_nn", "tzr_compute_fpfh", "tzr_certifier_params_default", "tzr_certify",
     "tzr_certifier_initial_matrix", "tzr_certifier_dual_projection", "tzr_last_graph_info", "tzr_ctx_stage_log",
@@ -151,6 +151,7 @@ def lib():
     L.tzr_solve_batch.argtypes = [vp, C.POINTER(Params), C.c_int, i32p, C.POINTER(dp), C.POINTER(dp),
                                   C.POINTER(Solution), i32p, C.c_int]
     L.tzr_solve_batch_dev.argtypes = [vp, C.POINTER(Params), C.c_int, C.c_int, vp, vp, vp, vp]
+    L.tzr_solve_batch_ragged_dev.argtypes = [vp, C.POINTER(Params), C.c_int, i32p, vp, vp, vp, vp]
     L.tzr_last_graph.argtypes = [vp, C.c_int, u64p, i32p]
     L.tzr_last_stage_ms.argtypes = [vp, dp, dp, dp, dp]
     L.tzr_last_graph_info.argtypes = [vp, i32p, i32p, i32p, u64p]
@@ -743,6 +744,15 @@ class Context:
         """Device pointers (e.g. torch tensors' data_ptr()); asynchronous on the context's stream."""
         self._ck(lib().tzr_solve_batch_dev(self._h, C.byref(params), B, n, C.c_void_p(src_ptr), C.c_void_p(dst_ptr),
                                            C.c_void_p(sol_ptr), C.c_void_p(clique_ptr) if clique_ptr else None))
+
+    def solve_batch_ragged_dev(self, params: Params, ns, src_ptr: int, dst_ptr: int, sol_ptr: int, clq_ptr: int = 0):
+        """tzr_solve_batch_ragged_dev: ns[b] correspondences per problem, the problems back to back in flat (sum ns, 3)
+        float64 device arrays; solutions (B records) and cliques (sum ns int32, -1 past each clique) at device pointers.
+        Asynchronous on the context's stream."""
+        ns = np.ascontiguousarray(ns, dtype=np.int32)
+        self._ck(lib().tzr_solve_batch_ragged_dev(self._h, C.byref(params), int(ns.size), _p(ns, C.c_int32),
+                                                  C.c_void_p(src_ptr), C.c_void_p(dst_ptr), C.c_void_p(sol_ptr),
+                                                  C.c_void_p(clq_ptr) if clq_ptr else None))
 
     def last_graph(self, b: int, n: int):
         W = lib().tzr_words_per_row(n)

@@ -34,6 +34,8 @@ struct tzr_ctx {
       certb;
   // large clique route (n > kMaxN or debug flag 524288): scratch on the full graph, and the compacted batch's buffers
   DevBuf lg, cq;
+  // ragged batches (DESIGN.md §4.2): the size-class tables, and the flat inputs / outputs of host-pointer calls
+  DevBuf rg;
   int max_n = kMaxN;  // per-problem size limit of this context (tzr_ctx_set_max_n: kMaxN ... kMaxNLarge)
   // pinned host staging
   void* h_pin = nullptr;
@@ -65,6 +67,13 @@ struct tzr_ctx {
   // clique route of every problem of the most recent clique stage (tzr_ctx_clique_route); route_B = 0 once reused
   std::vector<int32_t> route;
   int route_B = 0;
+  // retained graph of a ragged solve, per problem in the caller's order (empty after a uniform one): its padded slot
+  struct RaggedGraph {
+    const uint64_t* adj;  // n_pad rows of pitch64(n_pad) words; the problem's graph is the first n rows
+    const int32_t* deg;
+    int n, n_pad;
+  };
+  std::vector<RaggedGraph> ragged_last;
 };
 
 namespace {
@@ -194,6 +203,8 @@ void parallel_stage(char* dst_base, const double* const* bufs, int first, int co
   parallel_copy(spans);
 }
 
+size_t al256(size_t x) { return (x + 255) & ~(size_t)255; }
+
 // effective inlier selection mode (registration.cc:574-583)
 int effective_mode(const tzr_params& p) {
   int mode = p.inlier_selection_mode;
@@ -229,141 +240,173 @@ void search_geometry(const tzr_ctx* ctx, int B, int n, int* ctas, int* depth_out
   }
 }
 
-// Size the workspace for a (B, n) batch and fill the Batch descriptor (src/dst left to the caller).
-int setup_batch(tzr_ctx* ctx, int B, int n, bool own_points, Batch* out, bool complete_graph = false) {
-  if (B <= 0 || n <= 0) return TZR_ERR_INVALID_ARG;
-  if (n > ctx->max_n) {
-    ctx->last_error = "n = " + std::to_string(n) + " exceeds this context's limit of " + std::to_string(ctx->max_n) +
-                      " correspondences (tzr_ctx_set_max_n raises it to " + std::to_string(kMaxNLarge) + ")";
-    return TZR_ERR_TOO_LARGE;
+// Size the workspace for C size classes (class c: B[c] problems of n[c] correspondences) and fill one Batch descriptor
+// per class (src/dst left to the caller unless own_points).  Per-problem buffers hold the classes back to back in class
+// order; the re-check queue, the exact-phase scratch and the debug counters are shared (the classes' pipelines run in
+// stream order on each lane).  A uniform batch is one class.
+int setup_classes(tzr_ctx* ctx, int C, const int* Bs, const int* ns, bool own_points, Batch* out,
+                  bool complete_graph = false) {
+  for (int c = 0; c < C; ++c) {
+    if (Bs[c] <= 0 || ns[c] <= 0) return TZR_ERR_INVALID_ARG;
+    if (ns[c] > ctx->max_n) {
+      ctx->last_error = "n = " + std::to_string(ns[c]) + " exceeds this context's limit of " + std::to_string(ctx->max_n) +
+                        " correspondences (tzr_ctx_set_max_n raises it to " + std::to_string(kMaxNLarge) + ")";
+      return TZR_ERR_TOO_LARGE;
+    }
   }
   // the workspace is about to be re-used (and possibly re-allocated): the retained graph of the previous call is gone
   ctx->have_last = false;
   ctx->last_has_graph = false;
+  ctx->ragged_last.clear();
   ++ctx->generation;
   ctx->clique_B = 0;
   ctx->route_B = 0;
-  Batch bt{};
-  bt.B = B;
-  bt.n = n;
-  const size_t Bn = (size_t)B * n;
-  const int W32 = pitch32(n);
+  // per class: geometry, then the bytes of every buffer (summed over classes, or the largest for the shared ones)
+  enum { kSrc, kDst, kSf, kDf, kPk, kOpnd, kTcl, kGc, kAdj, kDeg, kNe, kHclq, kHsize, kClq, kL, kAlive, kBest, kAcnt,
+         kRctr, kLock, kFlg, kKfin, kTst, kStack, kCv, kCentry, kPs, kPd, kWgt, kRes, kSkey, kSidx, kSorted, kRmask,
+         kTmask, kSol, kDbg, kBufs };
+  DevBuf* bufs[kBufs] = {&ctx->src, &ctx->dst, &ctx->sf, &ctx->df, &ctx->pk, &ctx->opnd, &ctx->tclist, &ctx->gc,
+                         &ctx->adj, &ctx->deg, &ctx->nedges, &ctx->hclq, &ctx->hsize, &ctx->clq, &ctx->L, &ctx->alive,
+                         &ctx->best_bits, &ctx->alive_cnt, &ctx->root_ctr, &ctx->lock, &ctx->flg, &ctx->kfinal,
+                         &ctx->tstart, &ctx->stack, &ctx->cv, &ctx->centry, &ctx->ps, &ctx->pd, &ctx->wgt, &ctx->res,
+                         &ctx->skey, &ctx->sidx, &ctx->sorted, &ctx->rmask, &ctx->tmask, &ctx->sol, &ctx->dbg};
+  bool shared[kBufs] = {};
+  for (int k : {(int)kTcl, (int)kStack, (int)kCv, (int)kCentry, (int)kDbg}) shared[k] = true;
+  std::vector<size_t> off((size_t)C * kBufs, 0);  // byte offset of class c in buffer k
+  size_t total[kBufs] = {};
+  for (int c = 0; c < C; ++c) {
+    const int B = Bs[c], n = ns[c];
+    Batch& bt = out[c];
+    bt = Batch{};
+    bt.B = B;
+    bt.n = n;
+    const size_t Bn = (size_t)B * n;
+    const int W32 = pitch32(n);
+    size_t bytes[kBufs] = {};
+    if (own_points) {
+      bytes[kSrc] = Bn * 3 * sizeof(double);
+      bytes[kDst] = Bn * 3 * sizeof(double);
+    }
+    bytes[kSf] = Bn * sizeof(float4);
+    bytes[kDf] = Bn * sizeof(float4);
+    bytes[kPk] = (size_t)B * 6 * npad128(n) * sizeof(float);
+    bytes[kOpnd] = tc_operand_bytes(B, n);
+    bt.tc_list_cap = (unsigned int)tc_list_entries(B, n);
+    bytes[kTcl] = (size_t)bt.tc_list_cap * sizeof(uint2) + 256;
+    // debug flag 16384: a re-check queue of 64 entries (the buffer keeps its full size), so that the queue-full path of
+    // the graph kernels (void entries, in-place exact evaluation, the patch kernel's clamp) runs at test sizes
+    if (ctx->flags & 16384u) bt.tc_list_cap = std::min(bt.tc_list_cap, 64u);
+    bytes[kGc] = (size_t)B * sizeof(GraphConsts);
+    bytes[kAdj] = Bn * pitch64(n) * sizeof(uint64_t);
+    bytes[kDeg] = Bn * sizeof(int32_t);
+    bytes[kNe] = (size_t)B * sizeof(unsigned long long);
+    bytes[kHclq] = Bn * kHeurRoots * sizeof(int32_t);
+    bytes[kHsize] = (size_t)B * kHeurRoots * sizeof(int32_t);
+    bytes[kClq] = Bn * sizeof(int32_t);
+    bytes[kL] = bytes[kAcnt] = bytes[kRctr] = bytes[kLock] = bytes[kFlg] = bytes[kKfin] = (size_t)B * sizeof(int32_t);
+    bytes[kAlive] = bytes[kBest] = (size_t)B * W32 * sizeof(uint32_t);
+    bytes[kTst] = (size_t)B * sizeof(unsigned long long);
+    // exact phase: above kMaxN the search runs on the large route's compacted batch, which has its own scratch
+    if (n <= kMaxN) {
+      search_geometry(ctx, B, n, &bt.exact_ctas, &bt.max_depth, &bt.exact_conc);
+      const size_t warps = (size_t)bt.exact_ctas * 8;
+      const size_t level_bytes = (size_t)2 * W32 * sizeof(uint32_t);
+      bytes[kStack] = warps * bt.max_depth * level_bytes;
+      bytes[kCv] = std::max(warps, (size_t)4 * B) * (size_t)n * sizeof(int32_t);
+      bytes[kCentry] = warps * bt.max_depth * sizeof(int32_t);
+    }
+    bt.sort_cap = next_pow2(2 * n);
+    bytes[kPs] = bytes[kPd] = Bn * 3 * sizeof(double);
+    // rotation TIM capacity: n for CHAIN; for COMPLETE min(n(n-1)/2, what a 4 GiB budget allows)
+    bt.rot_cap = n;
+    if (complete_graph) {
+      const long long full = (long long)n * (n - 1) / 2;
+      const long long budget = ((long long)4 << 30) / (9LL * B);
+      bt.rot_cap = std::max<long long>(n, std::min(full, budget));
+    }
+    bytes[kWgt] = (size_t)B * bt.rot_cap * sizeof(double);
+    bytes[kRes] = Bn * sizeof(double);
+    bytes[kSkey] = (size_t)B * 3 * bt.sort_cap * sizeof(double);
+    bytes[kSidx] = (size_t)B * 3 * bt.sort_cap * sizeof(int32_t);
+    bytes[kSorted] = Bn * sizeof(int32_t);
+    bytes[kRmask] = (size_t)B * bt.rot_cap;
+    bytes[kTmask] = Bn;
+    bytes[kSol] = (size_t)B * sizeof(tzr_solution);
+    bytes[kDbg] = 16 * sizeof(unsigned long long);
+    for (int k = 0; k < kBufs; ++k) {
+      if (shared[k]) {
+        total[k] = std::max(total[k], bytes[k]);
+      } else {
+        off[(size_t)c * kBufs + k] = total[k];
+        total[k] += al256(bytes[k]);
+      }
+    }
+  }
   int rc;
-#define ENS(buf, bytes)                                  \
-  if ((rc = ensure(ctx, ctx->buf, (bytes))) != TZR_OK) return rc;
-  if (own_points) {
-    ENS(src, Bn * 3 * sizeof(double));
-    ENS(dst, Bn * 3 * sizeof(double));
-  }
-  ENS(sf, Bn * sizeof(float4));
-  ENS(df, Bn * sizeof(float4));
-  ENS(pk, (size_t)B * 6 * npad128(n) * sizeof(float));
-  ENS(opnd, tc_operand_bytes(B, n));
-  bt.tc_list_cap = (unsigned int)tc_list_entries(B, n);
-  ENS(tclist, (size_t)bt.tc_list_cap * sizeof(uint2) + 256);
-  // debug flag 16384: a re-check queue of 64 entries (the buffer keeps its full size), so that the queue-full path of the
-  // graph kernels (void entries, in-place exact evaluation, the patch kernel's clamp) runs at test sizes
-  if (ctx->flags & 16384u) bt.tc_list_cap = std::min(bt.tc_list_cap, 64u);
-  ENS(gc, (size_t)B * sizeof(GraphConsts));
-  ENS(adj, Bn * pitch64(n) * sizeof(uint64_t));
-  ENS(deg, Bn * sizeof(int32_t));
-  ENS(nedges, (size_t)B * sizeof(unsigned long long));
-  ENS(hclq, Bn * kHeurRoots * sizeof(int32_t));
-  ENS(hsize, (size_t)B * kHeurRoots * sizeof(int32_t));
-  ENS(clq, Bn * sizeof(int32_t));
-  ENS(L, (size_t)B * sizeof(int32_t));
-  ENS(alive, (size_t)B * W32 * sizeof(uint32_t));
-  ENS(best_bits, (size_t)B * W32 * sizeof(uint32_t));
-  ENS(alive_cnt, (size_t)B * sizeof(int32_t));
-  ENS(root_ctr, (size_t)B * sizeof(int32_t));
-  ENS(lock, (size_t)B * sizeof(int32_t));
-  ENS(flg, (size_t)B * sizeof(int32_t));
-  ENS(kfinal, (size_t)B * sizeof(int32_t));
-  ENS(tstart, (size_t)B * sizeof(unsigned long long));
-  // exact phase: above kMaxN the search runs on the large route's compacted batch, which has its own scratch
-  if (n <= kMaxN) {
-    search_geometry(ctx, B, n, &bt.exact_ctas, &bt.max_depth, &bt.exact_conc);
-    const size_t warps = (size_t)bt.exact_ctas * 8;
-    const size_t level_bytes = (size_t)2 * W32 * sizeof(uint32_t);
-    ENS(stack, warps * bt.max_depth * level_bytes);
-    ENS(cv, std::max(warps, (size_t)4 * B) * (size_t)n * sizeof(int32_t));
-    ENS(centry, warps * bt.max_depth * sizeof(int32_t));
-  }
-  bt.sort_cap = next_pow2(2 * n);
-  ENS(ps, Bn * 3 * sizeof(double));
-  ENS(pd, Bn * 3 * sizeof(double));
-  // rotation TIM capacity: n for CHAIN; for COMPLETE min(n(n-1)/2, what a 4 GiB budget allows)
-  bt.rot_cap = n;
-  if (complete_graph) {
-    const long long full = (long long)n * (n - 1) / 2;
-    const long long budget = ((long long)4 << 30) / (9LL * B);
-    bt.rot_cap = std::max<long long>(n, std::min(full, budget));
-  }
-  ENS(wgt, (size_t)B * bt.rot_cap * sizeof(double));
-  ENS(res, Bn * sizeof(double));
-  ENS(skey, (size_t)B * 3 * bt.sort_cap * sizeof(double));
-  ENS(sidx, (size_t)B * 3 * bt.sort_cap * sizeof(int32_t));
-  ENS(sorted, Bn * sizeof(int32_t));
-  ENS(rmask, (size_t)B * bt.rot_cap);
-  ENS(tmask, Bn);
-  ENS(sol, (size_t)B * sizeof(tzr_solution));
-  ENS(dbg, 16 * sizeof(unsigned long long));
-#undef ENS
-  bt.src = (const double*)ctx->src.p;
-  bt.dst = (const double*)ctx->dst.p;
-  bt.sf = (float4*)ctx->sf.p;
-  bt.df = (float4*)ctx->df.p;
-  bt.pk = (float*)ctx->pk.p;
-  bt.opnd = (float*)ctx->opnd.p;
-  bt.tc_list_count = (unsigned int*)ctx->tclist.p;
-  bt.tc_list = (uint2*)((char*)ctx->tclist.p + 256);
-  bt.gc = (GraphConsts*)ctx->gc.p;
-  bt.adj = (uint64_t*)ctx->adj.p;
-  bt.deg = (int32_t*)ctx->deg.p;
-  bt.n_edges2 = (unsigned long long*)ctx->nedges.p;
-  bt.hclq = (int32_t*)ctx->hclq.p;
-  bt.hsize = (int32_t*)ctx->hsize.p;
-  bt.clq = (int32_t*)ctx->clq.p;
-  bt.L = (int32_t*)ctx->L.p;
-  bt.alive = (uint32_t*)ctx->alive.p;
-  bt.best_bits = (uint32_t*)ctx->best_bits.p;
-  bt.alive_cnt = (int32_t*)ctx->alive_cnt.p;
-  bt.root_ctr = (int32_t*)ctx->root_ctr.p;
-  bt.lock = (int32_t*)ctx->lock.p;
-  bt.flags = (int32_t*)ctx->flg.p;
-  bt.kcore_final = (int32_t*)ctx->kfinal.p;
-  bt.t_start = (unsigned long long*)ctx->tstart.p;
-  bt.stack = (uint32_t*)ctx->stack.p;
-  bt.cv = (int32_t*)ctx->cv.p;
-  bt.centry = (int32_t*)ctx->centry.p;
-  bt.ps = (double*)ctx->ps.p;
-  bt.pd = (double*)ctx->pd.p;
-  bt.wgt = (double*)ctx->wgt.p;
-  bt.res = (double*)ctx->res.p;
-  bt.skey = (double*)ctx->skey.p;
-  bt.sidx = (int32_t*)ctx->sidx.p;
-  bt.sorted_clq = (int32_t*)ctx->sorted.p;
-  bt.rot_mask = (uint8_t*)ctx->rmask.p;
-  bt.trans_mask = (uint8_t*)ctx->tmask.p;
-  bt.sol = (tzr_solution*)ctx->sol.p;
-  bt.mismatches = (unsigned long long*)ctx->dbg.p;
-  bt.rechecks = (ctx->flags & 4u) ? (unsigned long long*)ctx->dbg.p + 1 : nullptr;
-  bt.flags_dbg = ctx->flags;
-  {
-    static const double kappa_env = [] {
-      const char* e = std::getenv("TZR_TC_KAPPA");
-      return e ? std::atof(e) : 0.0;
-    }();
-    static const int swap_env = [] {
-      const char* e = std::getenv("TZR_TC_SWAP");
-      return e ? std::atoi(e) : 0;
-    }();
+  for (int k = 0; k < kBufs; ++k)
+    if ((k != kSrc && k != kDst) || own_points)
+      if ((rc = ensure(ctx, *bufs[k], total[k])) != TZR_OK) return rc;
+  static const double kappa_env = [] {
+    const char* e = std::getenv("TZR_TC_KAPPA");
+    return e ? std::atof(e) : 0.0;
+  }();
+  static const int swap_env = [] {
+    const char* e = std::getenv("TZR_TC_SWAP");
+    return e ? std::atoi(e) : 0;
+  }();
+  for (int c = 0; c < C; ++c) {
+    Batch& bt = out[c];
+    auto at = [&](int k) { return (void*)((char*)bufs[k]->p + off[(size_t)c * kBufs + k]); };
+    bt.src = (const double*)at(kSrc);
+    bt.dst = (const double*)at(kDst);
+    bt.sf = (float4*)at(kSf);
+    bt.df = (float4*)at(kDf);
+    bt.pk = (float*)at(kPk);
+    bt.opnd = (float*)at(kOpnd);
+    bt.tc_list_count = (unsigned int*)ctx->tclist.p;
+    bt.tc_list = (uint2*)((char*)ctx->tclist.p + 256);
+    bt.gc = (GraphConsts*)at(kGc);
+    bt.adj = (uint64_t*)at(kAdj);
+    bt.deg = (int32_t*)at(kDeg);
+    bt.n_edges2 = (unsigned long long*)at(kNe);
+    bt.hclq = (int32_t*)at(kHclq);
+    bt.hsize = (int32_t*)at(kHsize);
+    bt.clq = (int32_t*)at(kClq);
+    bt.L = (int32_t*)at(kL);
+    bt.alive = (uint32_t*)at(kAlive);
+    bt.best_bits = (uint32_t*)at(kBest);
+    bt.alive_cnt = (int32_t*)at(kAcnt);
+    bt.root_ctr = (int32_t*)at(kRctr);
+    bt.lock = (int32_t*)at(kLock);
+    bt.flags = (int32_t*)at(kFlg);
+    bt.kcore_final = (int32_t*)at(kKfin);
+    bt.t_start = (unsigned long long*)at(kTst);
+    bt.stack = (uint32_t*)ctx->stack.p;
+    bt.cv = (int32_t*)ctx->cv.p;
+    bt.centry = (int32_t*)ctx->centry.p;
+    bt.ps = (double*)at(kPs);
+    bt.pd = (double*)at(kPd);
+    bt.wgt = (double*)at(kWgt);
+    bt.res = (double*)at(kRes);
+    bt.skey = (double*)at(kSkey);
+    bt.sidx = (int32_t*)at(kSidx);
+    bt.sorted_clq = (int32_t*)at(kSorted);
+    bt.rot_mask = (uint8_t*)at(kRmask);
+    bt.trans_mask = (uint8_t*)at(kTmask);
+    bt.sol = (tzr_solution*)at(kSol);
+    bt.mismatches = (unsigned long long*)ctx->dbg.p;
+    bt.rechecks = (ctx->flags & 4u) ? (unsigned long long*)ctx->dbg.p + 1 : nullptr;
+    bt.flags_dbg = ctx->flags;
     bt.tc_kappa = kappa_env;
     bt.tc_desc_swap = swap_env;
+    bt.budget_ns = 0ull;
   }
-  bt.budget_ns = 0ull;
-  *out = bt;
   return TZR_OK;
+}
+
+// Size the workspace for a (B, n) batch and fill the Batch descriptor (src/dst left to the caller).
+int setup_batch(tzr_ctx* ctx, int B, int n, bool own_points, Batch* out, bool complete_graph = false) {
+  return setup_classes(ctx, 1, &B, &n, own_points, out, complete_graph);
 }
 
 int check_launch(tzr_ctx* ctx, const char* what) {
@@ -434,6 +477,8 @@ Batch sub_batch(const Batch& bt, int b0, int Bc) {
   s.rot_mask = bt.rot_mask + o * (size_t)bt.rot_cap;
   s.trans_mask = bt.trans_mask + o * n;
   s.sol = bt.sol + o;
+  if (bt.nb) s.nb = bt.nb + o;
+  if (bt.nb_host) s.nb_host = bt.nb_host + o;
   return s;
 }
 
@@ -455,8 +500,6 @@ int l2_chunk(const tzr_ctx* ctx, int B, int n, const tzr_params& p) {
   if (c >= B) return B;
   return (int)c;
 }
-
-size_t al256(size_t x) { return (x + 255) & ~(size_t)255; }
 
 // Large clique route (DESIGN.md §3.2), taken when n > kMaxN or under debug flag 524288: the heuristic on the full graph,
 // its (L-1)-core on many CTAs, the cores compacted (order-preserving) into a batch of at most kMaxN vertices per problem
@@ -635,11 +678,12 @@ int run_pipeline(tzr_ctx* ctx, Batch& bt, const tzr_params& p, cudaEvent_t* ev, 
   return check_launch(ctx, "pipeline launch");
 }
 
-// Run the pipeline chunk by chunk on the compute stream.  ready[c] (optional) is an event the chunk's inputs wait for.
-// bounds = n_chunks+1 ascending problem offsets (bounds[0] = 0, bounds[n_chunks] = B).
-int run_chunked(tzr_ctx* ctx, Batch& bt, const tzr_params& p, const std::vector<int>& bounds,
-                const cudaEvent_t* ready, const std::function<int(int)>& before_chunk = nullptr) {
-  const int n_chunks = (int)bounds.size() - 1;
+// Run the pipeline chunk by chunk on the compute stream.  chunks: views of consecutive problems, chunk c starting at
+// problem bounds[c] of the call's B = bounds.back() (route entries).  ready[c] (optional) is an event the chunk's inputs
+// wait for.  lanes_ok: several chunks may alternate between the two compute lanes.
+int run_chunks(tzr_ctx* ctx, std::vector<Batch>& chunks, const std::vector<int>& bounds, const tzr_params& p,
+               const cudaEvent_t* ready, const std::function<int(int)>& before_chunk, bool lanes_ok) {
+  const int n_chunks = (int)chunks.size();
   if (!ctx->stage_log) {
     ctx->graph_ev_used = 0;
     ctx->stage_chunks = 0;
@@ -651,8 +695,8 @@ int run_chunked(tzr_ctx* ctx, Batch& bt, const tzr_params& p, const std::vector<
     if (cudaEventCreate(&e) != cudaSuccess) return TZR_ERR_CUDA;
     ctx->stage_ev.push_back(e);
   }
-  const bool lanes = n_chunks > 1 && ctx->gstream && ctx->hstream && l2_chunk(ctx, bt.B, bt.n, p) >= bt.B;
-  ctx->route.assign((size_t)bt.B, 0);
+  const bool lanes = n_chunks > 1 && ctx->gstream && ctx->hstream && lanes_ok;
+  ctx->route.assign((size_t)bounds.back(), 0);
   // debug counters cover the whole call: zeroed once, ahead of every chunk on either lane (not per chunk, which would
   // keep only the last chunk's counts)
   if (ctx->flags & 6u) CK(cudaMemsetAsync((void*)ctx->dbg.p, 0, 16 * sizeof(unsigned long long), ctx->stream));
@@ -667,7 +711,7 @@ int run_chunked(tzr_ctx* ctx, Batch& bt, const tzr_params& p, const std::vector<
     if (cudaStreamWaitEvent(ctx->hstream, ctx->join_ev, 0) != cudaSuccess) return TZR_ERR_CUDA;
   }
   for (int c = 0; c < n_chunks; ++c) {
-    const int b0 = bounds[c], Bc = bounds[c + 1] - b0;
+    const int b0 = bounds[c];
     cudaStream_t st = lanes ? ctx->hstream : ctx->stream;
     cudaStream_t sg = lanes ? ctx->gstream : ctx->stream;
     if (before_chunk) {  // host-side work that produces this chunk's inputs (staging + H2D enqueue)
@@ -677,11 +721,9 @@ int run_chunked(tzr_ctx* ctx, Batch& bt, const tzr_params& p, const std::vector<
     if (ready) {
       if (cudaStreamWaitEvent(sg, ready[c], 0) != cudaSuccess) return TZR_ERR_CUDA;
     }
-    Batch sb = (n_chunks > 1) ? sub_batch(bt, b0, Bc) : bt;
-    int rc = run_pipeline(ctx, sb, p, ctx->stage_ev.data() + 5 * (ctx->stage_first + c), st, ctx->route.data() + b0, sg,
-                          lanes ? ctx->gdone_ev[c] : nullptr);
+    int rc = run_pipeline(ctx, chunks[c], p, ctx->stage_ev.data() + 5 * (ctx->stage_first + c), st,
+                          ctx->route.data() + b0, sg, lanes ? ctx->gdone_ev[c] : nullptr);
     if (rc) return rc;
-    if (n_chunks == 1) bt = sb;  // keep fields filled in by run_pipeline (beta, scale_mode, ...)
   }
   if (lanes) {  // everything later on ctx->stream (D2H, the caller's work) is ordered after both lanes
     if (cudaEventRecord(ctx->join_ev, ctx->hstream) != cudaSuccess) return TZR_ERR_CUDA;
@@ -691,10 +733,214 @@ int run_chunked(tzr_ctx* ctx, Batch& bt, const tzr_params& p, const std::vector<
   }
   ctx->stage_chunks = ctx->stage_first + n_chunks;
   if (ctx->stage_log) ++ctx->stage_log_calls;
+  return TZR_OK;
+}
+
+// run_chunks over the chunks [bounds[c], bounds[c+1]) of one uniform batch; the batch becomes the retained graph.
+int run_chunked(tzr_ctx* ctx, Batch& bt, const tzr_params& p, const std::vector<int>& bounds,
+                const cudaEvent_t* ready, const std::function<int(int)>& before_chunk = nullptr) {
+  const int n_chunks = (int)bounds.size() - 1;
+  std::vector<Batch> chunks;
+  for (int c = 0; c < n_chunks; ++c)
+    chunks.push_back(n_chunks > 1 ? sub_batch(bt, bounds[c], bounds[c + 1] - bounds[c]) : bt);
+  const int rc = run_chunks(ctx, chunks, bounds, p, ready, before_chunk, l2_chunk(ctx, bt.B, bt.n, p) >= bt.B);
+  if (rc) return rc;
+  if (n_chunks == 1) bt = chunks[0];  // keep fields filled in by run_pipeline (beta, scale_mode, ...)
   ctx->last = bt;
   ctx->have_last = true;
   ctx->last_has_graph = effective_mode(p) != 3;  // NONE: populateVertices is never called (registration.cc:607-650)
   ctx->route_B = ctx->last_has_graph ? bt.B : 0;
+  return TZR_OK;
+}
+
+// Pipeline chunks of a (B, n) batch as n_chunks+1 ascending problem offsets.  The H2D copy of chunk k+1 overlaps the
+// kernels of chunk k and the clique / rotation kernels of one chunk run under the graph kernel of the next: PCIe moves a
+// problem ~3x faster than the kernels consume it, so only the first chunk's copy is exposed: it is kept small (B/32) and
+// the later chunks grow (3B/32, B/8, then B/4 each) to keep launch tails few.
+std::vector<int> chunk_bounds(int B, int n, const tzr_params& p) {
+  std::vector<int> bounds{0};
+  if (n > kMaxN) {  // one such problem fills the GPU (a 512 MiB bitset at n = 65536): one per chunk
+    for (int b = 1; b <= B; ++b) bounds.push_back(b);
+  } else if (B >= 64 && !p.estimate_scaling) {
+    const int unit = std::max(8, B / 32);
+    const int sizes[3] = {unit, 3 * unit, 4 * unit};
+    for (int k = 0; bounds.back() < B; ++k) {
+      const int sz = k < 3 ? sizes[k] : 8 * unit;
+      bounds.push_back(std::min(B, bounds.back() + sz));
+    }
+  } else {
+    bounds.push_back(B);
+  }
+  return bounds;
+}
+
+// ---- ragged batches (DESIGN.md §4.2) -----------------------------------------------------------------------------
+// Problems ordered by n (largest first) are cut into size classes; a class runs as one padded device batch of its
+// largest n, each problem's own n in Batch::nb.  One entry per problem in class order:
+struct RaggedSlot {
+  double* src;             // the problem's padded slot (n_pad rows; rows past n are zero)
+  double* dst;
+  const tzr_solution* sol; // its record in the class
+  const int32_t* clq;      // its sorted clique row
+  long long flat;          // first row of the problem in the caller's flat arrays
+  int n, n_pad, q, pad_;   // own size, class size, index in the caller's order
+};
+
+__global__ void __launch_bounds__(256) ragged_gather_kernel(const RaggedSlot* slots, const double* src,
+                                                            const double* dst) {
+  const RaggedSlot sl = slots[blockIdx.x];
+  const long long own = 3LL * sl.n, all = 3LL * sl.n_pad;
+  const double* s = src + 3 * sl.flat;
+  const double* d = dst + 3 * sl.flat;
+  for (long long i = threadIdx.x; i < all; i += blockDim.x) {
+    sl.src[i] = i < own ? s[i] : 0.0;
+    sl.dst[i] = i < own ? d[i] : 0.0;
+  }
+}
+
+// solutions[q] and the clique row at cliques + flat (n entries, -1 past the clique)
+__global__ void __launch_bounds__(256) ragged_scatter_kernel(const RaggedSlot* slots, tzr_solution* solutions,
+                                                             int32_t* cliques) {
+  const RaggedSlot sl = slots[blockIdx.x];
+  static_assert(sizeof(tzr_solution) % 4 == 0, "tzr_solution is copied in 4-byte words");
+  const uint32_t* from = reinterpret_cast<const uint32_t*>(sl.sol);
+  uint32_t* to = reinterpret_cast<uint32_t*>(solutions + sl.q);
+  for (int i = threadIdx.x; i < (int)(sizeof(tzr_solution) / 4); i += blockDim.x) to[i] = from[i];
+  if (!cliques) return;
+  const int m = max(0, min(sl.n, sl.sol->clique_size));
+  for (int i = threadIdx.x; i < sl.n; i += blockDim.x) cliques[sl.flat + i] = i < m ? sl.clq[i] : -1;
+}
+
+// Size classes over `order` (problem indices by n, largest first): [lo[c], lo[c+1]).  A class starts at its largest n and
+// takes the next problems while n >= n_class / r, so that its padded bitset is at most r^2 times theirs.  Two rules keep
+// every problem on the path it takes alone: a problem above kMaxN (the large clique route) is a class of its own, and
+// with estimate_scaling a class never mixes the two scale paths.  Debug flag 16777216 drops the ratio rule (one class
+// wherever the two path rules allow).
+std::vector<int> ragged_classes(const int32_t* n, const std::vector<int>& order, const tzr_params& p, uint32_t flags,
+                                double r) {
+  std::vector<int> lo;
+  const int B = (int)order.size();
+  for (int s = 0; s < B;) {
+    lo.push_back(s);
+    const int nc = n[order[s]];
+    int e = s + 1;
+    while (e < B && nc <= kMaxN) {
+      const int m = n[order[e]];
+      if (!(flags & 16777216u) && (double)m * r < (double)nc) break;
+      if (p.estimate_scaling && scale_large(nc, flags) != scale_large(m, flags)) break;
+      ++e;
+    }
+    s = e;
+  }
+  lo.push_back(B);
+  return lo;
+}
+
+// Padding ratio r of the size classes (DESIGN.md §4.2).  TZR_RAGGED_RATIO overrides it for measurements.
+double ragged_ratio() {
+  const char* e = std::getenv("TZR_RAGGED_RATIO");
+  const double r = e ? std::atof(e) : 0.0;
+  return r >= 1.0 ? r : std::sqrt(2.0);
+}
+
+// A ragged batch on the device.  src/dst: the caller's flat arrays (problem b's n[b] rows of 3 doubles at row
+// sum_{c<b} n[c]); solutions: B records in the caller's order; cliques (may be NULL): sum n int32 at the same row
+// offsets.  All device pointers; asynchronous on ctx->stream except where a large-route class reads back its core sizes.
+int solve_ragged_dev(tzr_ctx* ctx, const tzr_params& p, int B, const int32_t* n, const double* src, const double* dst,
+                     tzr_solution* solutions, int32_t* cliques) {
+  for (int b = 0; b < B; ++b)
+    if (n[b] <= 0) return TZR_ERR_INVALID_ARG;
+  std::vector<int> order(B);
+  for (int b = 0; b < B; ++b) order[b] = b;
+  std::stable_sort(order.begin(), order.end(), [&](int a, int c) { return n[a] > n[c]; });
+  const std::vector<int> lo = ragged_classes(n, order, p, ctx->flags, ragged_ratio());
+  const int C = (int)lo.size() - 1;
+  std::vector<int> Bs(C), ns(C);
+  for (int c = 0; c < C; ++c) {
+    Bs[c] = lo[c + 1] - lo[c];
+    ns[c] = n[order[lo[c]]];
+  }
+  std::vector<Batch> cls(C);
+  int rc = setup_classes(ctx, C, Bs.data(), ns.data(), true, cls.data(), p.rotation_tim_graph == 1);
+  if (rc) return rc;
+  std::vector<long long> flat(B + 1, 0);
+  for (int b = 0; b < B; ++b) flat[b + 1] = flat[b] + n[b];
+  std::vector<int32_t> nb(B);
+  std::vector<RaggedSlot> slots(B);
+  for (int c = 0; c < C; ++c)
+    for (int s = lo[c]; s < lo[c + 1]; ++s) {
+      const int q = order[s], k = s - lo[c];
+      nb[s] = n[q];
+      RaggedSlot& sl = slots[s];
+      sl.src = const_cast<double*>(cls[c].src) + (size_t)k * ns[c] * 3;
+      sl.dst = const_cast<double*>(cls[c].dst) + (size_t)k * ns[c] * 3;
+      sl.sol = cls[c].sol + k;
+      sl.clq = cls[c].sorted_clq + (size_t)k * ns[c];
+      sl.flat = flat[q];
+      sl.n = n[q];
+      sl.n_pad = ns[c];
+      sl.q = q;
+      sl.pad_ = 0;
+    }
+  const size_t o_nb = al256((size_t)B * sizeof(RaggedSlot));
+  if ((rc = ensure(ctx, ctx->rg, o_nb + (size_t)B * sizeof(int32_t))) != TZR_OK) return rc;
+  RaggedSlot* d_slots = (RaggedSlot*)ctx->rg.p;
+  int32_t* d_nb = (int32_t*)((char*)ctx->rg.p + o_nb);
+  cudaStream_t st = ctx->stream;
+  CK(cudaMemcpyAsync(d_slots, slots.data(), (size_t)B * sizeof(RaggedSlot), cudaMemcpyHostToDevice, st));
+  CK(cudaMemcpyAsync(d_nb, nb.data(), (size_t)B * sizeof(int32_t), cudaMemcpyHostToDevice, st));
+  ragged_gather_kernel<<<B, 256, 0, st>>>(d_slots, src, dst);
+  ctx->launches += 1;
+  // chunks: every class as a uniform batch of its size would be cut, its own n per problem unless all are equal
+  std::vector<Batch> chunks;
+  std::vector<int> bounds{0};
+  bool lanes_ok = true;
+  size_t sc_bytes = 0;
+  for (int c = 0; c < C; ++c) {
+    if (nb[lo[c + 1] - 1] != ns[c]) {
+      cls[c].nb = d_nb + lo[c];
+      cls[c].nb_host = nb.data() + lo[c];
+    }
+    const std::vector<int> cb = chunk_bounds(Bs[c], ns[c], p);
+    lanes_ok &= l2_chunk(ctx, Bs[c], ns[c], p) >= Bs[c];
+    for (size_t k = 0; k + 1 < cb.size(); ++k) {
+      const int Bc = cb[k + 1] - cb[k];
+      chunks.push_back(cb.size() > 2 ? sub_batch(cls[c], cb[k], Bc) : cls[c]);
+      bounds.push_back(lo[c] + cb[k + 1]);
+      if (p.estimate_scaling) {
+        // sized here for every chunk at once: run_pipeline must not re-allocate it under an earlier chunk's kernels
+        const size_t bytes = scale_scratch_bytes(Bc, ns[c], ctx->flags);
+        if (!bytes) {
+          ctx->last_error = "estimate_scaling: 2K end points exceed 2^31";
+          return TZR_ERR_TOO_LARGE;
+        }
+        sc_bytes = std::max(sc_bytes, bytes);
+      }
+    }
+  }
+  if (sc_bytes && (rc = ensure(ctx, ctx->sc, sc_bytes)) != TZR_OK) return rc;
+  rc = run_chunks(ctx, chunks, bounds, p, nullptr, nullptr, lanes_ok);
+  if (rc) return rc;
+  ragged_scatter_kernel<<<B, 256, 0, st>>>(d_slots, solutions, cliques);
+  ctx->launches += 1;
+  if ((rc = check_launch(ctx, "ragged gather / scatter")) != TZR_OK) return rc;
+  // the retained graph and the clique routes, in the caller's order
+  const bool has_graph = effective_mode(p) != 3;
+  std::vector<int32_t> route(B, 0);
+  ctx->ragged_last.resize(B);
+  for (int c = 0; c < C; ++c)
+    for (int s = lo[c]; s < lo[c + 1]; ++s) {
+      const size_t k = (size_t)(s - lo[c]);
+      ctx->ragged_last[order[s]] = {cls[c].adj + k * ns[c] * pitch64(ns[c]), cls[c].deg + k * ns[c], nb[s], ns[c]};
+      route[order[s]] = ctx->route[s];
+    }
+  ctx->route = route;
+  ctx->last = cls[0];
+  ctx->last.B = B;
+  ctx->last.n = ns[0];
+  ctx->have_last = true;
+  ctx->last_has_graph = has_graph;
+  ctx->route_B = has_graph ? B : 0;
   return TZR_OK;
 }
 
@@ -942,7 +1188,7 @@ int tzr_ctx_destroy(tzr_ctx* ctx) {
                     &ctx->hclq, &ctx->hsize, &ctx->clq, &ctx->L, &ctx->alive, &ctx->best_bits, &ctx->alive_cnt, &ctx->root_ctr,
                     &ctx->lock, &ctx->flg, &ctx->kfinal, &ctx->tstart, &ctx->stack, &ctx->cv, &ctx->centry, &ctx->ps, &ctx->pd, &ctx->wgt,
                     &ctx->res, &ctx->skey, &ctx->sidx, &ctx->sorted, &ctx->rmask, &ctx->tmask, &ctx->sol, &ctx->dbg,
-                    &ctx->misc, &ctx->sc, &ctx->m_in, &ctx->m_scratch, &ctx->m_out, &ctx->cert, &ctx->certb, &ctx->lg, &ctx->cq};
+                    &ctx->misc, &ctx->sc, &ctx->m_in, &ctx->m_scratch, &ctx->m_out, &ctx->cert, &ctx->certb, &ctx->lg, &ctx->cq, &ctx->rg};
   for (DevBuf* b : bufs)
     if (b->p) cudaFree(b->p);
   if (ctx->h_pin) cudaFreeHost(ctx->h_pin);
@@ -1298,21 +1544,7 @@ static int solve_uniform_host(tzr_ctx* ctx, const tzr_params* params, int B, int
     hd = h_dst;
   }
   // Chunked pipeline: the H2D copy of chunk k+1 (copy stream) overlaps the kernels of chunk k (compute streams).
-  // PCIe moves a problem ~3x faster than the kernels consume it, so only the first chunk's copy is exposed: it is
-  // kept small (B/32) and the later chunks grow (3B/32, B/8, then B/4 each) to keep launch tails few.
-  std::vector<int> bounds{0};
-  if (n > kMaxN) {  // one such problem fills the GPU (a 512 MiB bitset at n = 65536): one per chunk
-    for (int b = 1; b <= B; ++b) bounds.push_back(b);
-  } else if (B >= 64 && !params->estimate_scaling) {
-    const int unit = std::max(8, B / 32);
-    const int sizes[3] = {unit, 3 * unit, 4 * unit};
-    for (int k = 0; bounds.back() < B; ++k) {
-      const int sz = k < 3 ? sizes[k] : 8 * unit;
-      bounds.push_back(std::min(B, bounds.back() + sz));
-    }
-  } else {
-    bounds.push_back(B);
-  }
+  const std::vector<int> bounds = chunk_bounds(B, n, *params);
   const int n_chunks = (int)bounds.size() - 1;
   while ((int)ctx->chunk_ev.size() < n_chunks + 1) {
     cudaEvent_t e;
@@ -1397,48 +1629,76 @@ int tzr_solve_batch(tzr_ctx* ctx, const tzr_params* params, int B, const int32_t
   for (int b = 1; b < B; ++b) uniform &= (n[b] == n[0]);
   if (cliques && max_n < *std::max_element(n, n + B)) return TZR_ERR_INVALID_ARG;
   if (uniform) return solve_uniform_host(ctx, params, B, n[0], src, dst, solutions, cliques, max_n, nullptr, nullptr);
-  // ragged batch: problems of equal size are solved together (one device batch per distinct n, largest first)
-  std::vector<int> order(B);
-  for (int b = 0; b < B; ++b) order[b] = b;
-  std::stable_sort(order.begin(), order.end(), [&](int a, int c) { return n[a] > n[c]; });
-  std::vector<const double*> gs, gd;
-  std::vector<tzr_solution> gsol;
-  std::vector<int32_t> gclq;
-  for (int lo = 0; lo < B;) {
-    int hi = lo;
-    while (hi < B && n[order[hi]] == n[order[lo]]) ++hi;
-    const int G = hi - lo, ng = n[order[lo]];
-    if (ng <= 0) return TZR_ERR_INVALID_ARG;
-    gs.resize(G);
-    gd.resize(G);
-    gsol.resize(G);
-    for (int g = 0; g < G; ++g) {
-      gs[g] = src[order[lo + g]];
-      gd[g] = dst[order[lo + g]];
-      if (!gs[g] || !gd[g]) return TZR_ERR_INVALID_ARG;
-    }
-    if (cliques) gclq.resize((size_t)G * ng);
-    int rc = solve_uniform_host(ctx, params, G, ng, gs.data(), gd.data(), gsol.data(), cliques ? gclq.data() : nullptr,
-                                ng, nullptr, nullptr);
-    if (rc) return rc;
-    for (int g = 0; g < G; ++g) {
-      const int b = order[lo + g];
-      solutions[b] = gsol[g];
-      if (cliques) {
-        const int m = std::max(0, std::min(ng, gsol[g].clique_size));
-        memcpy(cliques + (size_t)b * max_n, gclq.data() + (size_t)g * ng, (size_t)m * sizeof(int32_t));
-      }
-    }
-    lo = hi;
+  // ragged batch: size classes (solve_ragged_dev) over the problems staged back to back, one read-back at the end
+  long long N = 0;
+  for (int b = 0; b < B; ++b) {
+    if (n[b] <= 0 || !src[b] || !dst[b]) return TZR_ERR_INVALID_ARG;
+    N += n[b];
   }
+  cudaSetDevice(ctx->device);
+  cudaStream_t st = ctx->stream;
+  const size_t pts = (size_t)N * 3 * sizeof(double), o_clq = al256((size_t)B * sizeof(tzr_solution));
+  const size_t out_bytes = o_clq + (size_t)N * sizeof(int32_t);
+  int rc;
+  if ((rc = ensure(ctx, ctx->m_in, 2 * al256(pts))) != TZR_OK) return rc;
+  if ((rc = ensure(ctx, ctx->m_out, out_bytes)) != TZR_OK) return rc;
+  if ((rc = ensure_pinned(ctx, std::max(2 * al256(pts), out_bytes))) != TZR_OK) return rc;
+  char* h = (char*)ctx->h_pin;
+  std::vector<CopySpan> spans;
+  size_t at = 0;
+  for (int b = 0; b < B; ++b) {
+    const size_t bytes = (size_t)n[b] * 3 * sizeof(double);
+    spans.push_back(CopySpan{h + at, src[b], bytes});
+    spans.push_back(CopySpan{h + al256(pts) + at, dst[b], bytes});
+    at += bytes;
+  }
+  parallel_copy(spans);
+  char* d_in = (char*)ctx->m_in.p;
+  char* d_out = (char*)ctx->m_out.p;
+  CK(cudaMemcpyAsync(d_in, h, 2 * al256(pts), cudaMemcpyHostToDevice, st));
+  rc = solve_ragged_dev(ctx, *params, B, n, (const double*)d_in, (const double*)(d_in + al256(pts)),
+                        (tzr_solution*)d_out, cliques ? (int32_t*)(d_out + o_clq) : nullptr);
+  if (rc) return rc;
+  CK(cudaMemcpyAsync(h, d_out, cliques ? out_bytes : (size_t)B * sizeof(tzr_solution), cudaMemcpyDeviceToHost, st));
+  CK(cudaStreamSynchronize(st));
+  const tzr_solution* h_sol = (const tzr_solution*)h;
+  memcpy(solutions, h_sol, (size_t)B * sizeof(tzr_solution));
+  if (cliques) {
+    spans.clear();
+    const int32_t* h_clq = (const int32_t*)(h + o_clq);
+    size_t row = 0;
+    for (int b = 0; b < B; ++b) {
+      const int m = std::max(0, std::min(n[b], h_sol[b].clique_size));
+      spans.push_back(CopySpan{cliques + (size_t)b * max_n, h_clq + row, (size_t)m * sizeof(int32_t)});
+      row += (size_t)n[b];
+    }
+    parallel_copy(spans);
+  }
+  for (int b = 0; b < B; ++b)
+    if (h_sol[b].clique_proven_optimal == -2) {
+      ctx->last_error = "COMPLETE TIM graph of this clique does not fit the rotation workspace";
+      return TZR_ERR_TOO_LARGE;
+    }
   return TZR_OK;
+}
+
+int tzr_solve_batch_ragged_dev(tzr_ctx* ctx, const tzr_params* params, int B, const int32_t* n, const double* src_dev,
+                               const double* dst_dev, tzr_solution* solutions_dev, int32_t* cliques_dev) {
+  if (!ctx || !params || !n || !src_dev || !dst_dev || !solutions_dev || B <= 0) return TZR_ERR_INVALID_ARG;
+  cudaSetDevice(ctx->device);
+  return solve_ragged_dev(ctx, *params, B, n, src_dev, dst_dev, solutions_dev, cliques_dev);
 }
 
 int tzr_last_graph(tzr_ctx* ctx, int b, uint64_t* adj_bits, int32_t* degree) {
   if (!ctx || !ctx->have_last || b < 0 || b >= ctx->last.B) return TZR_ERR_INVALID_ARG;
   cudaSetDevice(ctx->device);
   const Batch& bt = ctx->last;
-  const int n = bt.n;
+  // a ragged solve: problem b's own n rows of its padded slot
+  const bool ragged = !ctx->ragged_last.empty();
+  const int n = ragged ? ctx->ragged_last[b].n : bt.n;
+  const int np = ragged ? ctx->ragged_last[b].n_pad : n;
+  const uint64_t* adj = ragged ? ctx->ragged_last[b].adj : bt.adj + (size_t)b * n * pitch64(n);
+  const int32_t* deg = ragged ? ctx->ragged_last[b].deg : bt.deg + (size_t)b * n;
   if (!ctx->last_has_graph) {  // inlier selection NONE: the reference never populates the graph -> no edges
     if (adj_bits) memset(adj_bits, 0, (size_t)n * words64(n) * 8);
     if (degree) memset(degree, 0, (size_t)n * 4);
@@ -1446,9 +1706,9 @@ int tzr_last_graph(tzr_ctx* ctx, int b, uint64_t* adj_bits, int32_t* degree) {
   }
   cudaStream_t st = ctx->stream;
   if (adj_bits)
-    CK(cudaMemcpy2DAsync(adj_bits, (size_t)words64(n) * 8, bt.adj + (size_t)b * n * pitch64(n), (size_t)pitch64(n) * 8,
-                         (size_t)words64(n) * 8, n, cudaMemcpyDeviceToHost, st));
-  if (degree) CK(cudaMemcpyAsync(degree, bt.deg + (size_t)b * n, (size_t)n * 4, cudaMemcpyDeviceToHost, st));
+    CK(cudaMemcpy2DAsync(adj_bits, (size_t)words64(n) * 8, adj, (size_t)pitch64(np) * 8, (size_t)words64(n) * 8, n,
+                         cudaMemcpyDeviceToHost, st));
+  if (degree) CK(cudaMemcpyAsync(degree, deg, (size_t)n * 4, cudaMemcpyDeviceToHost, st));
   CK(cudaStreamSynchronize(st));
   return TZR_OK;
 }

@@ -44,6 +44,7 @@ __host__ __device__ __forceinline__ bool tc_path_active(uint32_t flags) {
 __global__ void __launch_bounds__(256) prep_kernel(Batch bt) {
   const int b = blockIdx.x;
   const int n = bt.n;
+  const int nv = bt.nb ? bt.nb[b] : n;  // the problem's own points (ragged class: the rest of the slot is padding)
   const double* src = bt.src + (size_t)b * n * 3;
   const double* dst = bt.dst + (size_t)b * n * 3;
   __shared__ double s_red[8][12];
@@ -55,7 +56,7 @@ __global__ void __launch_bounds__(256) prep_kernel(Batch bt) {
     mx[k] = -1.0 / 0.0;
   }
   int bad = 0;
-  for (int i = threadIdx.x; i < n; i += blockDim.x) {
+  for (int i = threadIdx.x; i < nv; i += blockDim.x) {
     for (int k = 0; k < 3; ++k) {
       const double a = src[3 * i + k], c = dst[3 * i + k];
       bad |= !isfinite(a) | !isfinite(c);
@@ -234,7 +235,7 @@ __global__ void __launch_bounds__(256) prep_kernel(Batch bt) {
   for (int j = threadIdx.x; j < npad; j += blockDim.x) {
     const int o = j & 127, pos = (j & ~127) + (o >> 6) * 64 + (o & 31) * 2 + ((o >> 5) & 1);
     float v[6] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
-    if (j < n) {
+    if (j < nv) {
       v[0] = (float)((src[3 * j + 0] - s_c[0]) * s_c[6]);
       v[1] = (float)((src[3 * j + 1] - s_c[1]) * s_c[6]);
       v[2] = (float)((src[3 * j + 2] - s_c[2]) * s_c[6]);
@@ -661,9 +662,11 @@ struct __align__(16) IPointNeg2 {
 // problem under debug flags 1 and 512).  kFuseDeg: vertex degrees are accumulated here (row part: one atomic per row and
 // strip; column part: one 32-lane RED per transposed word) instead of a second pass over the B*n^2/8-byte bitset; deg[] is
 // zeroed by prep_kernel.
-template <bool kVerify, bool kFuseDeg>
+// kRagged: n is the problem's own size nb[b] (validity masks); nl = bt.n the padded size of every offset and pitch.
+template <bool kVerify, bool kFuseDeg, bool kRagged>
 __device__ __forceinline__ void strip_interval(const Batch& bt, const int b, const int I, const int J0, const int J1) {
-  const int n = bt.n;
+  const int nl = bt.n;
+  const int n = kRagged ? bt.nb[b] : nl;
   __shared__ IPointNeg2 s_ip[kTile];
   __shared__ __align__(16) uint32_t s_rw[kTile][4];
 
@@ -673,10 +676,10 @@ __device__ __forceinline__ void strip_interval(const Batch& bt, const int b, con
   const bool scale_mode = bt.scale_mode != 0;
   const double s_hat = scale_mode ? bt.sol[b].scale : 1.0;
 
-  const float4* sf = bt.sf + (size_t)b * n;
-  const float4* df = bt.df + (size_t)b * n;
-  const double* src = bt.src + (size_t)b * n * 3;
-  const double* dst = bt.dst + (size_t)b * n * 3;
+  const float4* sf = bt.sf + (size_t)b * nl;
+  const float4* df = bt.df + (size_t)b * nl;
+  const double* src = bt.src + (size_t)b * nl * 3;
+  const double* dst = bt.dst + (size_t)b * nl * 3;
 
   const int tid = threadIdx.x, w = tid >> 5, lane = tid & 31;
   const int ibase = I * kTile + 32 * w;
@@ -693,13 +696,13 @@ __device__ __forceinline__ void strip_interval(const Batch& bt, const int b, con
     s_ip[tid] = ip;
   }
   __syncwarp();
-  uint32_t* adj32 = reinterpret_cast<uint32_t*>(bt.adj) + (size_t)b * n * pitch32(n);
-  const int P32 = pitch32(n);
+  uint32_t* adj32 = reinterpret_cast<uint32_t*>(bt.adj) + (size_t)b * nl * pitch32(nl);
+  const int P32 = pitch32(nl);
   const uint32_t rmask = nrows >= 32 ? 0xffffffffu : ((1u << nrows) - 1u);
 
-  const int npadh = npad128(n) / 2;  // 64-bit elements per packed array
-  const f32x2* pkp = reinterpret_cast<const f32x2*>(bt.pk + (size_t)b * 6 * npad128(n));
-  int* degp = bt.deg + (size_t)b * n;
+  const int npadh = npad128(nl) / 2;  // 64-bit elements per packed array
+  const f32x2* pkp = reinterpret_cast<const f32x2*>(bt.pk + (size_t)b * 6 * npad128(nl));
+  int* degp = bt.deg + (size_t)b * nl;
   int rdeg = 0;
   for (int J = J0; J < J1; ++J) {
     const int jb = J * kTile + lane;
@@ -871,9 +874,10 @@ __device__ __forceinline__ void gram_sweep(const float4* rows, const int nr, con
 // and leaves as one 16-byte store per column row, with one degree atomic per column row carrying the sum of the four
 // warps' popcounts.  Every warp of the CTA runs every block of the strip and reaches every barrier: a warp without rows
 // (only in the last row block) sweeps nothing and contributes zero words.
-template <bool kVerify, bool kFuseDeg>
+template <bool kVerify, bool kFuseDeg, bool kRagged>
 __device__ __forceinline__ void strip_gram(const Batch& bt, const int b, const int I, const int J0, const int J1) {
-  const int n = bt.n;
+  const int nl = bt.n;
+  const int n = kRagged ? bt.nb[b] : nl;
   __shared__ float4 s_gr[2 + 2 * kTile];
   __shared__ __align__(16) uint32_t s_mir[2][kTile][4];  // [block parity][column row][warp]
 
@@ -883,10 +887,10 @@ __device__ __forceinline__ void strip_gram(const Batch& bt, const int b, const i
   const bool scale_mode = bt.scale_mode != 0;
   const double s_hat = scale_mode ? bt.sol[b].scale : 1.0;
 
-  const float4* sf = bt.sf + (size_t)b * n;
-  const float4* df = bt.df + (size_t)b * n;
-  const double* src = bt.src + (size_t)b * n * 3;
-  const double* dst = bt.dst + (size_t)b * n * 3;
+  const float4* sf = bt.sf + (size_t)b * nl;
+  const float4* df = bt.df + (size_t)b * nl;
+  const double* src = bt.src + (size_t)b * nl * 3;
+  const double* dst = bt.dst + (size_t)b * nl * 3;
 
   const int tid = threadIdx.x, w = tid >> 5, lane = tid & 31;
   const int ibase = I * kTile + 32 * w;
@@ -899,13 +903,13 @@ __device__ __forceinline__ void strip_gram(const Batch& bt, const int b, const i
     s_gr[2 + 2 * tid + 1] = make_float4(-2.f * d.x, -2.f * d.y, -2.f * d.z, d.w);
   }
   __syncwarp();
-  uint32_t* adj32 = reinterpret_cast<uint32_t*>(bt.adj) + (size_t)b * n * pitch32(n);
-  const int P32 = pitch32(n);
+  uint32_t* adj32 = reinterpret_cast<uint32_t*>(bt.adj) + (size_t)b * nl * pitch32(nl);
+  const int P32 = pitch32(nl);
   const uint32_t rmask = nrows >= 32 ? 0xffffffffu : ((1u << nrows) - 1u);
   const int nr = (nrows + 3) & ~3;  // rows swept: the rows below n, rounded up to the sweep's unroll
   const float4* rows = s_gr + 2 + 2 * 32 * w;
 
-  int* degp = bt.deg + (size_t)b * n;
+  int* degp = bt.deg + (size_t)b * nl;
   int rdeg = 0;
   for (int J = J0; J < J1; ++J) {
     const int jb = J * kTile + lane;
@@ -1033,8 +1037,13 @@ __device__ __forceinline__ void strip_gram(const Batch& bt, const int b, const i
 // graph strip kernel (default): one launch for the whole batch; each problem runs the Gram test or the interval test, as
 // prep_kernel chose (CTA-uniform: a strip belongs to one problem).  Undecided pairs of the Gram test are settled by
 // tc_patch_kernel afterwards (launch_graph).
-template <bool kVerify, int kMinBlocks, bool kFuseDeg>
-__global__ void __launch_bounds__(kGraphThreads, kMinBlocks) graph_strip2_kernel(Batch bt) {
+//
+// kRagged (graph_strip2_ragged_kernel): a ragged size class (Batch::nb).  The grid covers the class's padded size; a strip
+// of problem b keeps the (I, J0) it has in b's own grid, its blocks stop at b's last tile, and a strip wholly past that
+// tile returns before it touches shared memory.  Words the kernel does not write (padding rows, and the columns of tiles
+// past b's last one) keep the zeros launch_graph cleared them to, so problem b's rows equal its single-problem graph.
+template <bool kVerify, int kMinBlocks, bool kFuseDeg, bool kRagged>
+__device__ __forceinline__ void strip2_body(const Batch& bt) {
   const int b = blockIdx.y;
   const int nt = (bt.n + kTile - 1) / kTile;
   int I = 0, p = blockIdx.x;
@@ -1045,13 +1054,28 @@ __global__ void __launch_bounds__(kGraphThreads, kMinBlocks) graph_strip2_kernel
     ++I;
   }
   const int J0 = I + p * kStripBlocks;
-  const int J1 = min(nt, J0 + kStripBlocks);
+  int J1 = min(nt, J0 + kStripBlocks);
+  if (kRagged) {
+    const int ntb = (bt.nb[b] + kTile - 1) / kTile;
+    if (J0 >= ntb) return;  // I <= J0: the whole strip lies past the problem's last tile
+    J1 = min(ntb, J1);
+  }
   const GraphConsts* gcp = bt.gc + b;
   if (bt.tc_active && gcp->use_tc) return;  // built by graph_tc_kernel
   if (gcp->use_gram)
-    strip_gram<kVerify, kFuseDeg>(bt, b, I, J0, J1);
+    strip_gram<kVerify, kFuseDeg, kRagged>(bt, b, I, J0, J1);
   else
-    strip_interval<kVerify, kFuseDeg>(bt, b, I, J0, J1);
+    strip_interval<kVerify, kFuseDeg, kRagged>(bt, b, I, J0, J1);
+}
+
+template <bool kVerify, int kMinBlocks, bool kFuseDeg>
+__global__ void __launch_bounds__(kGraphThreads, kMinBlocks) graph_strip2_kernel(Batch bt) {
+  strip2_body<kVerify, kMinBlocks, kFuseDeg, false>(bt);
+}
+
+template <bool kVerify, int kMinBlocks, bool kFuseDeg>
+__global__ void __launch_bounds__(kGraphThreads, kMinBlocks) graph_strip2_ragged_kernel(Batch bt) {
+  strip2_body<kVerify, kMinBlocks, kFuseDeg, true>(bt);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -1302,8 +1326,8 @@ void launch_prep(const Batch& bt, cudaStream_t st) { prep_kernel<<<bt.B, 256, 0,
 int launch_graph(const Batch& bt0, cudaStream_t st, int num_sms) {
   Batch bt = bt0;
   // default: CUDA-core strip kernel.  Debug flag 1024 routes every problem prep_kernel marked use_tc through the
-  // tensor-core kernel instead (bit-identical output: DESIGN.md §3.1)
-  bt.tc_active = tc_path_active(bt.flags_dbg) ? 1 : 0;
+  // tensor-core kernel instead (bit-identical output: DESIGN.md §3.1); not in ragged size classes
+  bt.tc_active = (tc_path_active(bt.flags_dbg) && !bt.nb) ? 1 : 0;
   int launches = 1;  // the CUDA-core strip kernel below (grid covers every problem; TC problems return at once)
   if (bt.tc_active) launches += launch_graph_tc(bt, st, num_sms);
   const int nt = (bt.n + kTile - 1) / kTile;
@@ -1320,7 +1344,13 @@ int launch_graph(const Batch& bt0, cudaStream_t st, int num_sms) {
   dim3 sgrid((unsigned)strip_grid(bt.n), (unsigned)bt.B);
   if (!bt.tc_active) cudaMemsetAsync(bt.tc_list_count, 0, sizeof(unsigned int), st);  // (launch_graph_tc zeroes it otherwise)
   bool v7 = false;
-  if (bt.flags_dbg & 2048u) {  // v7 (one MUFU, sign-bit words, re-check queue): fewer instructions, but FMA-pipe bound
+  if (bt.nb) {  // ragged size class: the default kernel (or its verify variant) whatever the opt-in flags 1024 and 2048 say
+    cudaMemsetAsync(bt.adj, 0, (size_t)bt.B * bt.n * pitch64(bt.n) * sizeof(uint64_t), st);
+    if (bt.flags_dbg & 2u)
+      graph_strip2_ragged_kernel<true, 5, false><<<sgrid, kGraphThreads, 0, st>>>(bt);
+    else
+      graph_strip2_ragged_kernel<false, TZR_STRIP_MIN_BLOCKS, true><<<sgrid, kGraphThreads, 0, st>>>(bt);
+  } else if (bt.flags_dbg & 2048u) {  // v7 (one MUFU, sign-bit words, re-check queue): fewer instructions, but FMA-pipe bound
     v7 = true;
     if (bt.flags_dbg & 2u)
       graph_strip3_kernel<true, 5><<<sgrid, kGraphThreads, 0, st>>>(bt);
@@ -1353,6 +1383,7 @@ int launch_graph(const Batch& bt0, cudaStream_t st, int num_sms) {
 
 // fused degrees: the default kernel (not its verify variant), and v7 always
 bool graph_fuses_degrees(const Batch& bt) {
+  if (bt.nb) return (bt.flags_dbg & 2u) == 0;  // launch_graph's ragged choice
   if (bt.flags_dbg & (8u | 16u | 32u | 64u | 128u | 256u)) return false;
   if (bt.flags_dbg & 2048u) return true;
   return (bt.flags_dbg & 2u) == 0;

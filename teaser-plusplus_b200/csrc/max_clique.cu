@@ -617,6 +617,7 @@ size_t clique_kcore_smem(int n) { return (size_t)pitch32(n) * 4 * 3 + 16; }
 __global__ void __launch_bounds__(kPeelThreads) clique_kcore_kernel(Batch bt, double kcore_thr) {
   const int b = blockIdx.x;
   const int n = bt.n, W = pitch32(n);
+  const int nv = bt.nb ? bt.nb[b] : n;  // |V| of the problem itself (a ragged class pads it with isolated vertices)
   extern __shared__ __align__(16) unsigned char smem_raw[];
   uint32_t* A = reinterpret_cast<uint32_t*>(smem_raw);
   uint32_t* T = A + W;
@@ -631,8 +632,8 @@ __global__ void __launch_bounds__(kPeelThreads) clique_kcore_kernel(Batch bt, do
   for (int x = tid; x < W; x += blockDim.x) {
     uint32_t m = 0xffffffffu;
     const int base = x * 32;
-    if (base >= n) m = 0u;
-    else if (base + 32 > n) m = (1u << (n - base)) - 1u;
+    if (base >= nv) m = 0u;
+    else if (base + 32 > nv) m = (1u << (nv - base)) - 1u;
     A[x] = m;
   }
   __syncthreads();
@@ -693,7 +694,7 @@ __global__ void __launch_bounds__(kPeelThreads) clique_kcore_kernel(Batch bt, do
   }
   const int max_core = lo;
   // graph.cc:66-69: threshold != 1 short-circuits; compare against int(thr * |V|)
-  const bool shortcut = (kcore_thr != 1.0) && (max_core > (int)(kcore_thr * (double)n));
+  const bool shortcut = (kcore_thr != 1.0) && (max_core > (int)(kcore_thr * (double)nv));
   if (!shortcut) {
     if (tid == 0) bt.kcore_final[b] = 0;
     return;

@@ -511,8 +511,8 @@ __global__ void __launch_bounds__(kRTThreads) rot_trans_kernel(Batch bt, tzr_par
       __syncthreads();
     }
   } else {
-    m = n;  // inlier selection NONE: every measurement is "in the clique" (registration.cc:650-653)
-    for (int i = tid; i < n; i += kRTThreads) sc[i] = i;
+    m = bt.nb ? bt.nb[b] : n;  // inlier selection NONE: every measurement is "in the clique" (registration.cc:650-653)
+    for (int i = tid; i < m; i += kRTThreads) sc[i] = i;
   }
   __syncthreads();
   const double scale = sol->scale;

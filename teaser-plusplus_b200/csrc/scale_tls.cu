@@ -25,13 +25,14 @@ namespace tzr {
 __global__ void __launch_bounds__(256) scale_pairs_kernel(Batch bt, double* X, double* Rg) {
   const int i = blockIdx.x, b = blockIdx.y;
   const int n = bt.n;
+  const int nv = bt.nb ? bt.nb[b] : n;  // ragged size class: the problem's own TIMs, packed in its own order
   const long long K = (long long)n * (n - 1) / 2;
   const double* src = bt.src + (size_t)b * n * 3;
   const double* dst = bt.dst + (size_t)b * n * 3;
   double* x = X + (size_t)b * K;
   double* r = Rg + (size_t)b * K;
-  const long long seg = (long long)i * n - (long long)i * (i + 1) / 2;  // registration.cc:531
-  for (int j = i + 1 + threadIdx.x; j < n; j += blockDim.x) {
+  const long long seg = (long long)i * nv - (long long)i * (i + 1) / 2;  // registration.cc:531
+  for (int j = i + 1 + threadIdx.x; j < nv; j += blockDim.x) {
     const double d1 = tim_norm_exact(src, i, j);
     const double d2 = tim_norm_exact(dst, i, j);
     const long long k = seg + (j - i - 1);
@@ -46,8 +47,11 @@ __global__ void __launch_bounds__(1024) scale_tls_kernel(Batch bt, const double*
   const int b = blockIdx.x;
   const int K = bt.n * (bt.n - 1) / 2;
   const int npad = next_pow2(2 * K);
+  const int nv = bt.nb ? bt.nb[b] : bt.n;
+  if (nv < 2) return;  // no TIM: the scale stays 1, as launch_scale_estimation leaves it for n < 2
+  const int Kb = nv * (nv - 1) / 2;
   __shared__ double s_est;
-  tls_block(X + (size_t)b * K, Rg + (size_t)b * K, 0.0, K, 1, key + (size_t)b * npad, idx + (size_t)b * npad, &s_est);
+  tls_block(X + (size_t)b * K, Rg + (size_t)b * K, 0.0, Kb, 1, key + (size_t)b * npad, idx + (size_t)b * npad, &s_est);
   if (threadIdx.x == 0) bt.sol[b].scale = s_est;
 }
 
@@ -272,14 +276,14 @@ int launch_tls_large(const double* X, const double* Rg, long long K, void* scrat
   return 5 + 8;
 }
 
+size_t align256(size_t v) { return (v + 255) & ~(size_t)255; }
+
+}  // namespace
+
 constexpr int kScaleSmallN = 256;  // single-CTA bitonic sort + sequential one-thread sweep up to here (bit-exact vs the
                                    // reference's order; ~1 ms at 256), radix-sort + parallel-scan pipeline above
 // debug flag 262144: the large path at every size (same results within the rounding of its summation tree)
 bool scale_large(int n, uint32_t flags) { return n > kScaleSmallN || (flags & 262144u); }
-
-size_t align256(size_t v) { return (v + 255) & ~(size_t)255; }
-
-}  // namespace
 
 size_t tls_scratch_bytes(long long m, int count, bool large) {
   if (2 * m >= (1LL << 31)) return 0;  // end-point payloads are ints
@@ -328,12 +332,15 @@ int launch_scale_estimation(const Batch& bt, uint32_t flags, void* scratch, cuda
   }
   int launches = 0;
   for (int b = 0; b < bt.B; ++b) {
-    Batch one = bt;  // view of problem b for the pairs kernel
+    Batch one = bt;  // view of problem b (its own size in a ragged class) for the pairs kernel
     one.B = 1;
+    one.n = bt.nb_host ? bt.nb_host[b] : n;
+    one.nb = nullptr;
     one.src = bt.src + (size_t)b * n * 3;
     one.dst = bt.dst + (size_t)b * n * 3;
-    scale_pairs_kernel<<<(unsigned)(n - 1), 256, 0, st>>>(one, X, Rg);
-    launches += 1 + launch_tls_large(X, Rg, K, sort, &bt.sol[b].scale, st);
+    if (one.n < 2) continue;
+    scale_pairs_kernel<<<(unsigned)(one.n - 1), 256, 0, st>>>(one, X, Rg);
+    launches += 1 + launch_tls_large(X, Rg, (long long)one.n * (one.n - 1) / 2, sort, &bt.sol[b].scale, st);
   }
   return launches;
 }

@@ -136,6 +136,11 @@ struct Batch {
   uint32_t flags_dbg;
   unsigned long long budget_ns;    // time budget of the exact clique search per problem (0 = none), Params::max_clique_time_limit
   unsigned long long* t_start;     // B: %globaltimer when the first search warp of the problem started (0 = not yet)
+  // Ragged size class (DESIGN.md §4.2): problem b has nb[b] <= n correspondences in the first nb[b] rows of its padded
+  // slot; n stays the size of every pitch and offset.  nullptr for uniform batches.  Kept last so that the fields above
+  // keep their parameter offsets in every kernel.
+  const int32_t* nb;        // device, B entries
+  const int32_t* nb_host;   // host copy of nb (the unknown-scale large path's per-problem host loop)
 };
 
 // ||v_j - v_i|| exactly as the reference computes a TIM norm: IEEE double, no FMA contraction,
@@ -192,6 +197,9 @@ int launch_scalar_tls(const double* x, const double* ranges, long long m, bool l
                       uint8_t* inliers, cudaStream_t st);
 // Unknown-scale stage: TIM ratios, ranges and sort scratch of a batch (0: too large), and its launches.
 size_t scale_scratch_bytes(int B, int n, uint32_t flags);
+// Which of the two scale paths a problem of n correspondences takes (the large one above 256, or under debug flag 262144).
+// The paths differ in the last bits of the estimate, so a ragged size class never mixes them.
+bool scale_large(int n, uint32_t flags);
 int launch_scale_estimation(const Batch& bt, uint32_t flags, void* scratch, cudaStream_t st);
 void launch_rot_trans(const Batch& bt, const tzr_params& p, int use_clique, cudaStream_t st);
 // Large route (n > kMaxN or debug flag 524288; DESIGN.md §3.2).  lists: B * kHeurRoots * 2n u16 of heuristic scratch;
