@@ -374,6 +374,40 @@ int tzr_last_graph(tzr_ctx* ctx, int b, uint64_t* adj_bits, int32_t* degree);
  * compare it with the value they saw after their own solve before trusting tzr_last_graph. */
 int tzr_last_graph_info(const tzr_ctx* ctx, int32_t* B, int32_t* n, int32_t* has_graph, uint64_t* generation);
 
+/* ---- certifying the most recent solve ---------------------------------------------------------
+ * Every solve entry (tzr_solve, tzr_solve_batch uniform or ragged, tzr_solve_batch_dev, tzr_solve_batch_ragged_dev)
+ * leaves each problem's record, clique, inlier masks and inputs in the context's workspace until the next call that
+ * reuses it (another solve, tzr_graph_build, tzr_max_clique(_batch)).  tzr_solve_batch_dev reads the caller's src_dev /
+ * dst_dev in place and keeps no copy: those buffers must still hold the solve's inputs when tzr_certify_last_solve runs.
+ *
+ * tzr_last_inliers: masks of problem b (caller's order) of the most recent solve on this context: rot_inliers receives
+ * n_rot bytes (clique_size for CHAIN, clique_size*(clique_size-1)/2 for COMPLETE), trans_inliers clique_size bytes;
+ * each may be NULL.  n_rot / n_trans (may be NULL) receive the counts; 0 and 0 for a problem whose solution is not
+ * valid.  TZR_ERR_INVALID_ARG when no solve is retained (none yet, or a later call reused the workspace) or b is out
+ * of range.  Equal, byte for byte, to what tzr_solve returns for that problem alone.  Host-synchronous, like
+ * tzr_last_graph; ordered after every kernel of the solve, including those of the asynchronous _dev entries. */
+int tzr_last_inliers(tzr_ctx* ctx, int b, uint8_t* rot_inliers, uint8_t* trans_inliers, int64_t* n_rot,
+                     int32_t* n_trans);
+
+/* DRSCertifier::certify(R, getMaxCliqueSrcTIMs(), getMaxCliqueDstTIMs(), getRotationInliersMask()) on problems of the
+ * most recent solve, on tzr_certify_batch's path.  problems: count indices into the retained solve (duplicates and any
+ * order allowed); NULL only when count equals the solve's B, then all problems in order.  Entry j of results, status
+ * (may be NULL), traj and traj_capacity belongs to problems[j]; traj and traj_capacity follow tzr_certify_batch.
+ * Problem b's inputs are built on the device from the workspace, bitwise the TIMs its rotation was solved on: R =
+ * solution.rotation; CHAIN TIM i = src[leaf] - src[root] and (dst[leaf] - dst[root]) * (1.0 / scale) over the sorted
+ * clique; COMPLETE TIMs in computeTIMs order with the same de-scaling; theta = +1 where the rotation mask is set, -1
+ * elsewhere; N = n_rot.  Noise bound of problem b: noise_bound / scale_b (nbs = cbar2 * nb * nb).  The rotation solver
+ * ran with 2 * the solve's noise_bound / scale (registration.cc:702-704): set params->noise_bound to 2 * the solve's
+ * noise_bound to certify the problem it solved.  Only the B solution records cross PCIe; no TIM or mask does.
+ * status[j]: TZR_OK certified; TZR_ERR_INVALID_ARG the solution is not valid, or a gathered measurement is not finite (inlier selection NONE with a non-finite input row), never certified, result
+ * {0, 0, +inf} and no trajectory; TZR_ERR_TOO_LARGE 4N + 4 > 32768 (COMPLETE above 128 clique points), result
+ * {0, 0, +inf}.  Every other entry is certified.  Returns TZR_ERR_TOO_LARGE when some entry was too large, TZR_OK
+ * otherwise; TZR_ERR_INVALID_ARG (nothing written) when no solve is retained or an argument is out of range.
+ * tzr_ctx_kernel_launches counts tzr_certify_batch's launches plus one gather launch per group. */
+int tzr_certify_last_solve(tzr_ctx* ctx, const tzr_certifier_params* params, int count, const int32_t* problems,
+                           tzr_certification_result* results, int32_t* status, double* const* traj,
+                           const int32_t* traj_capacity);
+
 /* Graph-stage timing of the most recent tzr_solve_batch_dev, in milliseconds, measured with CUDA
  * events on the context's stream (for the roofline line in bench.py). Requires a prior synchronize. */
 int tzr_last_stage_ms(tzr_ctx* ctx, double* prep_ms, double* graph_ms, double* clique_ms, double* rot_trans_ms);

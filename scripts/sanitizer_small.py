@@ -94,6 +94,13 @@ for rflags, est in ((16777216, 0), (16777216 | 2, 0), (16777216, 1)):
                                capi.default_params(noise_bound=rg[0]["noise_bound"], estimate_scaling=est))
     print("ragged flags", rflags, "scale", est, [int(c) for c in sols["clique_size"]])
 ctx.set_flags(0)
+if "--no-cert" not in sys.argv:  # solve then certify its retained results: the gather kernel on CHAIN and COMPLETE TIMs
+    for tim in (0, 1):
+        sc = [synth.make_problem(n, 0.5, 60 + n, "ball") for n in (40, 30, 36)]
+        ctx.solve_batch([q["src"] for q in sc], [q["dst"] for q in sc],
+                        capi.default_params(noise_bound=sc[0]["noise_bound"], estimate_scaling=1, rotation_tim_graph=tim))
+        rc = ctx.certify_last(noise_bound=2 * sc[0]["noise_bound"], max_iterations=3)
+        print("certify_last tim", tim, [(r["status"], len(r["suboptimality_traj"])) for r in rc])
 sols, cl = capi.solve_batch_multi([p["src"] for p in prs[:5]], [p["dst"] for p in prs[:5]],
                                   capi.default_params(**dict(kw, noise_bound=prs[0]["noise_bound"])))
 print("multi", int(sols["valid"].sum()), "/ 5")

@@ -98,8 +98,13 @@ _SYMBOLS = [
     "tzr_ctx_stage_log_read", "tzr_solve_batch_multi", "tzr_ctx_clique_info", "tzr_compute_fpfh_batch",
     "tzr_match_correspondences_batch", "tzr_ctx_set_max_n", "tzr_ctx_clique_route", "tzr_certify_batch",
     "tzr_certifier_psd_projection", "tzr_certifier_batch_psd_projection", "tzr_certifier_batch_dual_projection",
-    "tzr_fpfh_pair_features", "tzr_fpfh_smallest_eigenpair",
+    "tzr_fpfh_pair_features", "tzr_fpfh_smallest_eigenpair", "tzr_last_inliers", "tzr_certify_last_solve",
 ]
+
+# status codes (tzr_status)
+TZR_OK = 0
+TZR_ERR_INVALID_ARG = -1
+TZR_ERR_TOO_LARGE = -6
 
 # debug flags of tzr_ctx_set_flags that choose tzr_compute_fpfh(_batch)'s radius search for every cloud
 FLAG_FPFH_BRUTE_FORCE = 4194304
@@ -190,6 +195,9 @@ def lib():
     L.tzr_certifier_psd_projection.argtypes = [vp, dp, C.c_int, dp, dp]
     L.tzr_certifier_batch_psd_projection.argtypes = [vp, C.c_int, i32p, C.POINTER(dp), C.POINTER(dp)]
     L.tzr_certifier_batch_dual_projection.argtypes = [vp, C.c_int, i32p, C.POINTER(dp), C.POINTER(dp), C.POINTER(dp)]
+    L.tzr_last_inliers.argtypes = [vp, C.c_int, u8p, u8p, i64p, i32p]
+    L.tzr_certify_last_solve.argtypes = [vp, C.POINTER(CertifierParams), C.c_int, i32p, C.POINTER(CertificationResult),
+                                         i32p, C.POINTER(dp), i32p]
     for s in _SYMBOLS:
         getattr(L, s)  # raises AttributeError if the header and the library disagree
     _lib = L
@@ -753,6 +761,54 @@ class Context:
         self._ck(lib().tzr_solve_batch_ragged_dev(self._h, C.byref(params), int(ns.size), _p(ns, C.c_int32),
                                                   C.c_void_p(src_ptr), C.c_void_p(dst_ptr), C.c_void_p(sol_ptr),
                                                   C.c_void_p(clq_ptr) if clq_ptr else None))
+
+    def last_inliers(self, b: int):
+        """tzr_last_inliers: (rotation mask, translation mask) of problem b of the most recent solve on this context,
+        as bool arrays (empty for a problem whose solution is not valid)."""
+        n_rot, n_trans = C.c_int64(0), C.c_int32(0)
+        self._ck(lib().tzr_last_inliers(self._h, int(b), None, None, C.byref(n_rot), C.byref(n_trans)))
+        rot = np.zeros(max(1, n_rot.value), dtype=np.uint8)
+        trans = np.zeros(max(1, n_trans.value), dtype=np.uint8)
+        self._ck(lib().tzr_last_inliers(self._h, int(b), _p(rot, C.c_uint8), _p(trans, C.c_uint8), None, None))
+        return rot[:n_rot.value].astype(bool), trans[:n_trans.value].astype(bool)
+
+    @staticmethod
+    def _certify_last_problems(problems):
+        """certify_last's problem list as contiguous int32 (None: every problem of the retained solve)."""
+        if problems is None:
+            return None
+        pr = np.asarray(problems)
+        if pr.ndim != 1 or pr.size == 0 or not np.issubdtype(pr.dtype, np.integer):
+            raise TzrError("certify_last: problems must be a non-empty 1-D sequence of integers")
+        return np.ascontiguousarray(pr, dtype=np.int32)
+
+    def certify_last(self, problems=None, **params):
+        """tzr_certify_last_solve: certify problems of the most recent solve on this context (all of them, in order, by
+        default), with their inputs built on the device.  noise_bound is divided by each problem's scale; pass 2x the
+        solve's noise_bound to certify what the rotation solver solved.  Returns a list of dicts shaped like
+        certify_batch's, plus status (0 certified, else the entry's TZR status)."""
+        pr = self._certify_last_problems(problems)
+        if pr is None:
+            B = C.c_int32(0)
+            self._ck(lib().tzr_last_graph_info(self._h, C.byref(B), None, None, None))
+            count = max(1, B.value)  # 0: nothing retained, the call below reports it
+        else:
+            count = int(pr.size)
+        p = self.certifier_params(**params)
+        cap = int(max(1, np.ceil(p.max_iterations)))
+        trajs = [np.zeros(cap) for _ in range(count)]
+        caps = np.full(count, cap, dtype=np.int32)
+        res = (CertificationResult * count)()
+        status = np.zeros(count, dtype=np.int32)
+        dp = C.POINTER(C.c_double)
+        rc = lib().tzr_certify_last_solve(self._h, C.byref(p), count, None if pr is None else _p(pr, C.c_int32), res,
+                                          _p(status, C.c_int32), (dp * count)(*[_p(t, C.c_double) for t in trajs]),
+                                          _p(caps, C.c_int32))
+        if rc not in (0, TZR_ERR_TOO_LARGE):
+            self._ck(rc)
+        return [dict(is_optimal=bool(r.is_optimal), best_suboptimality=r.best_suboptimality,
+                     suboptimality_traj=t[:r.n_iterations].copy(), status=int(s))
+                for r, t, s in zip(res, trajs, status)]
 
     def last_graph(self, b: int, n: int):
         W = lib().tzr_words_per_row(n)

@@ -43,6 +43,10 @@ struct tzr_ctx {
   // last batch geometry
   Batch last{};
   bool have_last = false;
+  // the retained call was a solve: every problem's record, clique, masks and inputs are still in the workspace
+  // (tzr_last_inliers, tzr_certify_last_solve); last_complete: its rotation ran on COMPLETE TIMs
+  bool last_is_solve = false;
+  bool last_complete = false;
   cudaEvent_t ev[5] = {nullptr, nullptr, nullptr, nullptr, nullptr};  // start | prep | graph tiles | clique (incl. degrees) | rot+trans
   std::vector<cudaEvent_t> graph_ev;  // pairs around every graph-kernel launch of the last call (roofline timing)
   int graph_ev_used = 0;
@@ -67,11 +71,17 @@ struct tzr_ctx {
   // clique route of every problem of the most recent clique stage (tzr_ctx_clique_route); route_B = 0 once reused
   std::vector<int32_t> route;
   int route_B = 0;
-  // retained graph of a ragged solve, per problem in the caller's order (empty after a uniform one): its padded slot
+  // retained results of a ragged solve, per problem in the caller's order (empty after a uniform one): its padded slot
   struct RaggedGraph {
     const uint64_t* adj;  // n_pad rows of pitch64(n_pad) words; the problem's graph is the first n rows
     const int32_t* deg;
     int n, n_pad;
+    const double* src;    // its points (n_pad rows, the first n its own)
+    const double* dst;
+    const tzr_solution* sol;
+    const int32_t* clq;   // sorted clique row
+    const uint8_t* rmask; // rotation inlier mask (rot_cap of its class)
+    const uint8_t* tmask; // translation inlier mask
   };
   std::vector<RaggedGraph> ragged_last;
 };
@@ -256,6 +266,7 @@ int setup_classes(tzr_ctx* ctx, int C, const int* Bs, const int* ns, bool own_po
   }
   // the workspace is about to be re-used (and possibly re-allocated): the retained graph of the previous call is gone
   ctx->have_last = false;
+  ctx->last_is_solve = false;
   ctx->last_has_graph = false;
   ctx->ragged_last.clear();
   ++ctx->generation;
@@ -748,6 +759,8 @@ int run_chunked(tzr_ctx* ctx, Batch& bt, const tzr_params& p, const std::vector<
   if (n_chunks == 1) bt = chunks[0];  // keep fields filled in by run_pipeline (beta, scale_mode, ...)
   ctx->last = bt;
   ctx->have_last = true;
+  ctx->last_is_solve = true;  // every uniform solve entry (tzr_solve, tzr_solve_batch, tzr_solve_batch_dev) ends here
+  ctx->last_complete = p.rotation_tim_graph == 1;
   ctx->last_has_graph = effective_mode(p) != 3;  // NONE: populateVertices is never called (registration.cc:607-650)
   ctx->route_B = ctx->last_has_graph ? bt.B : 0;
   return TZR_OK;
@@ -931,7 +944,9 @@ int solve_ragged_dev(tzr_ctx* ctx, const tzr_params& p, int B, const int32_t* n,
   for (int c = 0; c < C; ++c)
     for (int s = lo[c]; s < lo[c + 1]; ++s) {
       const size_t k = (size_t)(s - lo[c]);
-      ctx->ragged_last[order[s]] = {cls[c].adj + k * ns[c] * pitch64(ns[c]), cls[c].deg + k * ns[c], nb[s], ns[c]};
+      ctx->ragged_last[order[s]] = {cls[c].adj + k * ns[c] * pitch64(ns[c]), cls[c].deg + k * ns[c], nb[s], ns[c],
+                                    slots[s].src, slots[s].dst, slots[s].sol, slots[s].clq,
+                                    cls[c].rot_mask + k * (size_t)cls[c].rot_cap, cls[c].trans_mask + k * ns[c]};
       route[order[s]] = ctx->route[s];
     }
   ctx->route = route;
@@ -939,6 +954,8 @@ int solve_ragged_dev(tzr_ctx* ctx, const tzr_params& p, int B, const int32_t* n,
   ctx->last.B = B;
   ctx->last.n = ns[0];
   ctx->have_last = true;
+  ctx->last_is_solve = true;
+  ctx->last_complete = p.rotation_tim_graph == 1;
   ctx->last_has_graph = has_graph;
   ctx->route_B = has_graph ? B : 0;
   return TZR_OK;
@@ -1285,6 +1302,7 @@ int tzr_graph_build(tzr_ctx* ctx, const double* src, const double* dst, int n, d
   if (n_edges) *n_edges = (int64_t)(e2 / 2);
   ctx->last = bt;
   ctx->have_last = true;
+  ctx->last_is_solve = false;  // a graph without solution records
   ctx->last_has_graph = true;
   return TZR_OK;
 }
@@ -1301,6 +1319,7 @@ int tzr_max_clique_batch(tzr_ctx* ctx, int B, int n, const uint64_t* adj_bits, i
   Batch bt;
   int rc = setup_batch(ctx, B, n, false, &bt);
   if (rc) return rc;
+  ctx->last_is_solve = false;  // the clique stage reuses the solve's workspace
   cudaStream_t st = ctx->stream;
   const size_t rows = (size_t)B * n;
   CK(cudaMemsetAsync(bt.adj, 0, rows * pitch64(n) * 8, st));
@@ -1722,6 +1741,152 @@ int tzr_last_graph_info(const tzr_ctx* ctx, int32_t* B, int32_t* n, int32_t* has
   return TZR_OK;
 }
 
+// Where problem b (caller's order) of the retained solve lies in the workspace.
+struct SolveSlot {
+  const double* src;
+  const double* dst;
+  const tzr_solution* sol;
+  const int32_t* clq;
+  const uint8_t* rmask;
+  const uint8_t* tmask;
+};
+
+static SolveSlot last_solve_slot(const tzr_ctx* ctx, int b) {
+  if (!ctx->ragged_last.empty()) {
+    const tzr_ctx::RaggedGraph& r = ctx->ragged_last[b];
+    return SolveSlot{r.src, r.dst, r.sol, r.clq, r.rmask, r.tmask};
+  }
+  const Batch& bt = ctx->last;
+  const size_t n = (size_t)bt.n, o = (size_t)b;
+  return SolveSlot{bt.src + o * n * 3, bt.dst + o * n * 3, bt.sol + o, bt.sorted_clq + o * n,
+                   bt.rot_mask + o * (size_t)bt.rot_cap, bt.trans_mask + o * n};
+}
+
+// rotation TIMs (and rotation mask bytes) of a retained solution record: 0 when it is not valid
+static long long last_rot_count(const tzr_ctx* ctx, const tzr_solution& s) {
+  if (!s.valid) return 0;
+  const long long m = std::max(0, s.clique_size);
+  return ctx->last_complete ? m * (m - 1) / 2 : m;
+}
+
+int tzr_last_inliers(tzr_ctx* ctx, int b, uint8_t* rot_inliers, uint8_t* trans_inliers, int64_t* n_rot,
+                     int32_t* n_trans) {
+  if (!ctx || !ctx->last_is_solve || b < 0 || b >= ctx->last.B) return TZR_ERR_INVALID_ARG;
+  cudaSetDevice(ctx->device);
+  // every stream of the solve joins ctx->stream before its call returns: work queued here runs after all of it
+  cudaStream_t st = ctx->stream;
+  const SolveSlot s = last_solve_slot(ctx, b);
+  tzr_solution rec;
+  CK(cudaMemcpyAsync(&rec, s.sol, sizeof(rec), cudaMemcpyDeviceToHost, st));
+  CK(cudaStreamSynchronize(st));
+  const long long nr = last_rot_count(ctx, rec);
+  const int nt = rec.valid ? std::max(0, rec.clique_size) : 0;
+  if (rot_inliers && nr > 0) CK(cudaMemcpyAsync(rot_inliers, s.rmask, (size_t)nr, cudaMemcpyDeviceToHost, st));
+  if (trans_inliers && nt > 0) CK(cudaMemcpyAsync(trans_inliers, s.tmask, (size_t)nt, cudaMemcpyDeviceToHost, st));
+  CK(cudaStreamSynchronize(st));
+  if (n_rot) *n_rot = nr;
+  if (n_trans) *n_trans = nt;
+  return TZR_OK;
+}
+
+int tzr_certify_last_solve(tzr_ctx* ctx, const tzr_certifier_params* params, int count, const int32_t* problems,
+                           tzr_certification_result* results, int32_t* status, double* const* traj,
+                           const int32_t* traj_capacity) {
+  if (!ctx || !params || !results || count <= 0 || (traj && !traj_capacity)) return TZR_ERR_INVALID_ARG;
+  if (!ctx->last_is_solve) {
+    ctx->last_error = "no solve is retained on this context";
+    return TZR_ERR_INVALID_ARG;
+  }
+  const int B = ctx->last.B;
+  if (!problems && count != B) return TZR_ERR_INVALID_ARG;
+  for (int j = 0; j < count; ++j) {
+    const int b = problems ? problems[j] : j;
+    if (b < 0 || b >= B || (traj_capacity && traj_capacity[j] < 0)) return TZR_ERR_INVALID_ARG;
+  }
+  cudaSetDevice(ctx->device);
+  cudaStream_t st = ctx->stream;
+  // the B solution records: one read-back of the span of the workspace that holds them (the size classes of a ragged
+  // solve lie back to back in one buffer)
+  std::vector<const tzr_solution*> at((size_t)B);
+  const char *lo = nullptr, *hi = nullptr;
+  for (int b = 0; b < B; ++b) {
+    at[b] = last_solve_slot(ctx, b).sol;
+    const char* p = (const char*)at[b];
+    if (!lo || p < lo) lo = p;
+    if (!hi || p + sizeof(tzr_solution) > hi) hi = p + sizeof(tzr_solution);
+  }
+  std::vector<char> span((size_t)(hi - lo));
+  CK(cudaMemcpyAsync(span.data(), lo, span.size(), cudaMemcpyDeviceToHost, st));
+  CK(cudaStreamSynchronize(st));
+  // the certifiable entries: a valid record and 4N + 4 <= 32768 (non-finite measurements: flagged by the gather)
+  std::vector<int32_t> N;
+  std::vector<double> R;
+  std::vector<CertGatherProb> gin;
+  std::vector<int> which;
+  std::vector<double*> tr;
+  std::vector<int32_t> tc;
+  bool too_large = false;
+  for (int j = 0; j < count; ++j) {
+    const int b = problems ? problems[j] : j;
+    tzr_solution s;
+    memcpy(&s, span.data() + ((const char*)at[b] - lo), sizeof(s));
+    results[j].is_optimal = 0;
+    results[j].n_iterations = 0;
+    results[j].best_suboptimality = INFINITY;
+    int stj = TZR_OK;
+    const long long nr = last_rot_count(ctx, s);
+    if (nr <= 0) {
+      stj = TZR_ERR_INVALID_ARG;
+    } else if (4 * nr + 4 > 32768) {
+      stj = TZR_ERR_TOO_LARGE;
+      too_large = true;
+    } else {
+      const SolveSlot sl = last_solve_slot(ctx, b);
+      const double nb = params->noise_bound / s.scale;
+      CertGatherProb g;
+      g.src = sl.src;
+      g.dst = sl.dst;
+      g.clq = sl.clq;
+      g.rmask = sl.rmask;
+      g.scale = s.scale;
+      g.nbs = params->cbar2 * nb * nb;
+      g.m = s.clique_size;
+      g.complete = ctx->last_complete ? 1 : 0;
+      g.k_off = g.v_off = 0;
+      gin.push_back(g);
+      N.push_back((int32_t)nr);
+      R.insert(R.end(), s.rotation, s.rotation + 9);
+      which.push_back(j);
+      tr.push_back(traj ? traj[j] : nullptr);
+      tc.push_back(traj ? traj_capacity[j] : 0);
+    }
+    if (status) status[j] = stj;
+  }
+  if (!gin.empty()) {
+    const int K = (int)gin.size();
+    std::vector<tzr_certification_result> res((size_t)K);
+    std::vector<int32_t> ok((size_t)K, 0);
+    const int rc = certify_batch_device(0, *params, K, N.data(), R.data(), nullptr, nullptr, nullptr, gin.data(),
+                                        ok.data(), res.data(), traj ? tr.data() : nullptr, traj ? tc.data() : nullptr,
+                                        nullptr, nullptr, (ctx->flags & 2097152u) != 0, &ctx->certb.p,
+                                        &ctx->certb.cap, &ctx->solver_handle, &ctx->launches, st, &ctx->last_error);
+    if (rc != TZR_OK) return rc;
+    for (int i = 0; i < K; ++i) {
+      const int j = which[i];
+      if (!ok[i]) {  // a non-finite gathered measurement: never certified
+        if (status) status[j] = TZR_ERR_INVALID_ARG;
+        continue;
+      }
+      results[j] = res[i];
+    }
+  }
+  if (too_large) {
+    ctx->last_error = "a problem's certifier matrix exceeds 32768 rows (4N + 4)";
+    return TZR_ERR_TOO_LARGE;
+  }
+  return TZR_OK;
+}
+
 int tzr_match_correspondences(tzr_ctx* ctx, const float* src_pts, int ns, const float* dst_pts, int nd,
                               const float* src_feat, const float* dst_feat, int dim, int use_absolute_scale,
                               int use_crosscheck, int use_tuple_test, float tuple_scale, uint64_t tuple_seed,
@@ -1782,8 +1947,8 @@ int tzr_certify_batch(tzr_ctx* ctx, const tzr_certifier_params* params, int B, c
     if (N[b] <= 0 || !src_3xN[b] || !dst_3xN[b] || !theta[b] || (traj_capacity && traj_capacity[b] < 0))
       return TZR_ERR_INVALID_ARG;
   cudaSetDevice(ctx->device);
-  return certify_batch_device(0, *params, B, N, R_colmajor9xB, src_3xN, dst_3xN, theta, results, traj, traj_capacity,
-                              nullptr, nullptr, (ctx->flags & 2097152u) != 0, &ctx->certb.p, &ctx->certb.cap, &ctx->solver_handle,
+  return certify_batch_device(0, *params, B, N, R_colmajor9xB, src_3xN, dst_3xN, theta, nullptr, nullptr, results,
+                              traj, traj_capacity, nullptr, nullptr, (ctx->flags & 2097152u) != 0, &ctx->certb.p, &ctx->certb.cap, &ctx->solver_handle,
                               &ctx->launches, ctx->stream, &ctx->last_error);
 }
 
@@ -1823,7 +1988,8 @@ static int certifier_batch_block(tzr_ctx* ctx, int mode, int B, const int32_t* N
   cudaSetDevice(ctx->device);
   tzr_certifier_params prm;
   tzr_certifier_params_default(&prm);
-  return certify_batch_device(mode, prm, B, N, nullptr, nullptr, nullptr, theta, nullptr, nullptr, nullptr, X, Y,
+  return certify_batch_device(mode, prm, B, N, nullptr, nullptr, nullptr, theta, nullptr, nullptr, nullptr, nullptr,
+                              nullptr, X, Y,
                               (ctx->flags & 2097152u) != 0, &ctx->certb.p, &ctx->certb.cap, &ctx->solver_handle,
                               &ctx->launches, ctx->stream, &ctx->last_error);
 }

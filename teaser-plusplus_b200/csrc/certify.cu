@@ -501,6 +501,7 @@ struct CertBatchProb {
   int first_pos;       // first eigen column with a positive eigenvalue
   unsigned long long pad_bits;  // largest |entry| of the starting matrix (M_init), as its bit pattern
   double mu, best;
+  double nbs;          // cbar2 * noise_bound^2 of this problem
 };
 
 // Eigenvalue of the pad block (the identity times it) of a padded problem: block diagonal, so the padded matrix has the
@@ -514,14 +515,74 @@ __device__ __forceinline__ double cert_pad(unsigned long long bits) {
 
 __global__ void cbt_blocks_kernel(const CertBatchProb* __restrict__ pr, const double* __restrict__ src,
                                   const double* __restrict__ dst, const double* __restrict__ theta,
-                                  const double* __restrict__ R, const double* __restrict__ q, double nbs, double* offA,
+                                  const double* __restrict__ R, const double* __restrict__ q, double* offA,
                                   double* diagB, double* lam, double* mu_terms) {
   const CertBatchProb p = pr[blockIdx.y];
   const int k = blockIdx.x * blockDim.x + threadIdx.x;
   if (k >= p.N) return;
   const size_t o = p.k_off;
-  cert_block(k, src + 3 * o, dst + 3 * o, theta + o, R + 9 * blockIdx.y, q + 4 * blockIdx.y, nbs, offA + 16 * o,
+  cert_block(k, src + 3 * o, dst + 3 * o, theta + o, R + 9 * blockIdx.y, q + 4 * blockIdx.y, p.nbs, offA + 16 * o,
              diagB + 16 * o, lam + 16 * o, mu_terms + o);
+}
+
+// The measurements of a retained solve's problem (one CTA of kRTThreads per problem of the group), written where the
+// host path would have copied them: src/dst/theta at k_off, thp (1, theta) at v_off.  The TIMs are the rotation stage's,
+// bit for bit (rot_trans.cu): CHAIN TIM i runs from clique point i to point i+1 (the last one back to point 0), its dst
+// side times 1/scale; COMPLETE walks the clique points with for_each_tim.  A problem with a non-finite measurement is
+// marked inactive, so no later kernel or eigensolver call touches it; active[g] receives the flag.
+__global__ void __launch_bounds__(kRTThreads) cbt_solve_gather_kernel(const CertGatherProb* __restrict__ gt,
+                                                                      CertBatchProb* pr, double* src, double* dst,
+                                                                      double* theta, double* thp, int* active) {
+  __shared__ double s_a[3 * 128], s_b[3 * 128];  // COMPLETE clique points (4N + 4 <= 32768 keeps m <= 128)
+  const CertGatherProb g = gt[blockIdx.x];
+  const int m = g.m, tid = threadIdx.x;
+  const double inv_scale = 1.0 / g.scale;
+  double* s = src + 3 * (size_t)g.k_off;
+  double* d = dst + 3 * (size_t)g.k_off;
+  double* th = theta + g.k_off;
+  double* tp = thp + g.v_off + 1;
+  bool bad = false;
+  auto put = [&](long long k, double x0, double x1, double x2, double y0, double y1, double y2) {
+    s[3 * k] = x0; s[3 * k + 1] = x1; s[3 * k + 2] = x2;
+    d[3 * k] = y0; d[3 * k + 1] = y1; d[3 * k + 2] = y2;
+    const double t = g.rmask[k] ? 1.0 : -1.0;
+    th[k] = t;
+    tp[k] = t;
+    bad |= !(isfinite(x0) && isfinite(x1) && isfinite(x2) && isfinite(y0) && isfinite(y1) && isfinite(y2));
+  };
+  if (!g.complete) {
+    for (int i = tid; i < m; i += kRTThreads) {
+      const int root = g.clq[i];
+      const int leaf = (i != m - 1) ? g.clq[i + 1] : g.clq[0];
+      const double* sr = g.src + 3 * (size_t)root;
+      const double* sl = g.src + 3 * (size_t)leaf;
+      const double* dr = g.dst + 3 * (size_t)root;
+      const double* dl = g.dst + 3 * (size_t)leaf;
+      put(i, sl[0] - sr[0], sl[1] - sr[1], sl[2] - sr[2], (dl[0] - dr[0]) * inv_scale, (dl[1] - dr[1]) * inv_scale,
+          (dl[2] - dr[2]) * inv_scale);
+    }
+  } else {
+    for (int i = tid; i < m; i += kRTThreads)
+      for (int r = 0; r < 3; ++r) {
+        s_a[3 * i + r] = g.src[3 * (size_t)g.clq[i] + r];
+        s_b[3 * i + r] = g.dst[3 * (size_t)g.clq[i] + r];
+      }
+    __syncthreads();
+    TimSrc ts;
+    ts.complete = 1;
+    ts.m = m;
+    ts.count = (long long)m * (m - 1) / 2;
+    ts.a = s_a;
+    ts.b = s_b;
+    ts.inv_scale = inv_scale;
+    for_each_tim(ts, put);
+  }
+  bad = __syncthreads_or(bad) != 0;
+  if (tid == 0) {
+    thp[g.v_off] = 1.0;
+    pr[blockIdx.x].active = bad ? 0 : 1;
+    active[blockIdx.x] = bad ? 0 : 1;
+  }
 }
 
 __global__ void __launch_bounds__(256) cbt_reduce_kernel(CertBatchProb* pr, const double* lam,
@@ -1004,11 +1065,13 @@ struct CertBatchWork {
   CertBatchProb* pr;
   int *info, *active, *infoc, *idx;
   void* work;
+  CertGatherProb* gt;  // device inputs of the group (gather: certify_batch_device's device input mode), else null
 };
 
 // Device bytes of a group of G problems with K measurements, P block pairs, padded size nmax and T trajectory columns,
-// plus `work` bytes of eigensolver workspace; carve() of the same arguments lays them out.
-size_t cbt_carve(void* base, int G, long long K, long long P, int nmax, int T, size_t work, CertBatchWork* out) {
+// plus `work` bytes of eigensolver workspace (and the group's gather table); carve() of the same arguments lays them out.
+size_t cbt_carve(void* base, int G, long long K, long long P, int nmax, int T, size_t work, CertBatchWork* out,
+                 bool gather = false) {
   char* p = (char*)base;
   auto take = [&](size_t bytes) {
     void* r = p;
@@ -1030,6 +1093,7 @@ size_t cbt_carve(void* base, int G, long long K, long long P, int nmax, int T, s
   w.info = (int*)take(G * sizeof(int)); w.active = (int*)take(G * sizeof(int));
   w.wc = (double*)take((size_t)G * nmax * d); w.infoc = (int*)take(G * sizeof(int)); w.idx = (int*)take(G * sizeof(int));
   w.work = take(work);
+  w.gt = gather ? (CertGatherProb*)take(G * sizeof(CertGatherProb)) : nullptr;
   if (out) *out = w;
   return (size_t)(p - (char*)base);
 }
@@ -1037,10 +1101,12 @@ size_t cbt_carve(void* base, int G, long long K, long long P, int nmax, int T, s
 
 int certify_batch_device(int mode, const tzr_certifier_params& prm, int B, const int32_t* N, const double* R_cm,
                          const double* const* src, const double* const* dst, const double* const* theta,
+                         const CertGatherProb* gather, int32_t* gathered,
                          tzr_certification_result* results, double* const* traj, const int32_t* traj_cap,
                          const double* const* X_in, double* const* X_out, bool loop_eig, void** scratch,
                          size_t* scratch_cap, void** solver_handle, int64_t* launches, cudaStream_t st,
                          std::string* err) {
+  const bool dev_in = mode == 0 && gather;  // measurements gathered on the device from a retained solve
   int nmax_all = 0;
   for (int b = 0; b < B; ++b) {
     if (4 * (size_t)N[b] + 4 > 32768) {
@@ -1117,7 +1183,7 @@ int certify_batch_device(int mode, const tzr_certifier_params& prm, int B, const
       const int nm2 = std::max(nmax, 4 * N[b1] + 4), G2 = b1 - b0 + 1;
       const long long K2 = K + N[b1], P2 = P + (long long)N[b1] * (N[b1] + 1) / 2;
       const size_t ws = std::max(loop_ws_all, batched ? ws1 * (size_t)G2 : 0);
-      const size_t need2 = cbt_carve(nullptr, G2, K2, P2, nm2, T, ws, nullptr);
+      const size_t need2 = cbt_carve(nullptr, G2, K2, P2, nm2, T, ws, nullptr, dev_in);
       if (need2 > budget && b1 > b0) break;
       if (need2 > budget) {
         *err = "the certifier batch workspace of " + std::to_string(need2) + " bytes (one problem, 4N+4 = " +
@@ -1139,7 +1205,7 @@ int certify_batch_device(int mode, const tzr_certifier_params& prm, int B, const
         if (!dws) bat = false;
       }
       lwork_bytes = syevd_ws(nmax);
-      need = cbt_carve(nullptr, b1 - b0, K, P, nmax, T, std::max(dws, lwork_bytes), nullptr);
+      need = cbt_carve(nullptr, b1 - b0, K, P, nmax, T, std::max(dws, lwork_bytes), nullptr, dev_in);
       if (need <= budget || b1 - b0 == 1) break;
       b1 = b0 + (b1 - b0) / 2;
       nmax = 0; K = 0; P = 0;
@@ -1162,11 +1228,14 @@ int certify_batch_device(int mode, const tzr_certifier_params& prm, int B, const
       *scratch_cap = need;
     }
     CertBatchWork w;
-    cbt_carve(*scratch, G, K, P, nmax, T, std::max(dws, lwork_bytes), &w);
+    cbt_carve(*scratch, G, K, P, nmax, T, std::max(dws, lwork_bytes), &w, dev_in);
     std::vector<char> host_work(std::max<size_t>(hws, 1));
-    // host tables
+    // host tables (device input mode: only the rotations and the gather table; the kernel below writes the rest)
     std::vector<CertBatchProb> tab(G);
-    std::vector<double> h_src(3 * K), h_dst(3 * K), h_th(K), h_thp(K + G), h_R(9 * (size_t)G), h_q(4 * (size_t)G);
+    const long long Kh = dev_in ? 0 : K;
+    std::vector<double> h_src(3 * Kh), h_dst(3 * Kh), h_th(Kh), h_thp(dev_in ? 0 : K + G), h_R(9 * (size_t)G),
+        h_q(4 * (size_t)G);
+    std::vector<CertGatherProb> h_gt(dev_in ? G : 0);
     int maxN = 0;
     for (int g = 0, k = 0; g < G; ++g) {
       const int b = b0 + g, Nb = N[b];
@@ -1174,42 +1243,66 @@ int certify_batch_device(int mode, const tzr_certifier_params& prm, int B, const
       t.N = Nb; t.n = 4 * Nb + 4; t.k_off = k; t.v_off = k + g;
       t.p_off = g ? tab[g - 1].p_off + (long long)tab[g - 1].N * (tab[g - 1].N + 1) / 2 : 0;
       t.active = 1; t.iters = 0; t.first_pos = 0; t.pad_bits = 0; t.mu = 0; t.best = INFINITY;
+      t.nbs = dev_in ? gather[b].nbs : nbs;
       if (mode == 1) {  // the PSD building block starts from X_in[b]: its pad follows that matrix
         double m = 0;
         for (size_t e = 0; e < (size_t)t.n * t.n; ++e) m = std::max(m, std::fabs(X_in[b][e]));
         std::memcpy(&t.pad_bits, &m, sizeof m);
       }
       if (mode == 0) {
-        std::copy(src[b], src[b] + 3 * (size_t)Nb, h_src.begin() + 3 * (size_t)k);
-        std::copy(dst[b], dst[b] + 3 * (size_t)Nb, h_dst.begin() + 3 * (size_t)k);
-        std::copy(theta[b], theta[b] + Nb, h_th.begin() + k);
+        if (dev_in) {
+          h_gt[g] = gather[b];
+          h_gt[g].k_off = t.k_off;
+          h_gt[g].v_off = t.v_off;
+        } else {
+          std::copy(src[b], src[b] + 3 * (size_t)Nb, h_src.begin() + 3 * (size_t)k);
+          std::copy(dst[b], dst[b] + 3 * (size_t)Nb, h_dst.begin() + 3 * (size_t)k);
+          std::copy(theta[b], theta[b] + Nb, h_th.begin() + k);
+        }
         std::copy(R_cm + 9 * (size_t)b, R_cm + 9 * (size_t)b + 9, h_R.begin() + 9 * (size_t)g);
         quaternion_xyzw(R_cm + 9 * (size_t)b, &h_q[4 * (size_t)g]);
       }
-      h_thp[k + g] = 1.0;
-      if (mode != 1) std::copy(theta[b], theta[b] + Nb, h_thp.begin() + k + g + 1);
+      if (!dev_in) {
+        h_thp[k + g] = 1.0;
+        if (mode != 1) std::copy(theta[b], theta[b] + Nb, h_thp.begin() + k + g + 1);
+      }
       maxN = std::max(maxN, Nb);
       k += Nb;
     }
-    cudaMemcpyAsync(w.src, h_src.data(), h_src.size() * sizeof(double), cudaMemcpyHostToDevice, st);
-    cudaMemcpyAsync(w.dst, h_dst.data(), h_dst.size() * sizeof(double), cudaMemcpyHostToDevice, st);
-    cudaMemcpyAsync(w.theta, h_th.data(), h_th.size() * sizeof(double), cudaMemcpyHostToDevice, st);
-    cudaMemcpyAsync(w.thp, h_thp.data(), h_thp.size() * sizeof(double), cudaMemcpyHostToDevice, st);
+    if (!dev_in) {
+      cudaMemcpyAsync(w.src, h_src.data(), h_src.size() * sizeof(double), cudaMemcpyHostToDevice, st);
+      cudaMemcpyAsync(w.dst, h_dst.data(), h_dst.size() * sizeof(double), cudaMemcpyHostToDevice, st);
+      cudaMemcpyAsync(w.theta, h_th.data(), h_th.size() * sizeof(double), cudaMemcpyHostToDevice, st);
+      cudaMemcpyAsync(w.thp, h_thp.data(), h_thp.size() * sizeof(double), cudaMemcpyHostToDevice, st);
+    }
     cudaMemcpyAsync(w.R, h_R.data(), h_R.size() * sizeof(double), cudaMemcpyHostToDevice, st);
     cudaMemcpyAsync(w.q, h_q.data(), h_q.size() * sizeof(double), cudaMemcpyHostToDevice, st);
     cudaMemcpyAsync(w.pr, tab.data(), G * sizeof(CertBatchProb), cudaMemcpyHostToDevice, st);
+    if (dev_in) {
+      cudaMemcpyAsync(w.gt, h_gt.data(), G * sizeof(CertGatherProb), cudaMemcpyHostToDevice, st);
+      cbt_solve_gather_kernel<<<G, kRTThreads, 0, st>>>(w.gt, w.pr, w.src, w.dst, w.theta, w.thp, w.active);
+      *launches += 1;
+    }
     const long long nn = (long long)nmax * nmax;
     const dim3 ge(grid1(nn, 256), G), gp(grid1(maxN + 1, 128), maxN, G), gt((nmax + kPT - 1) / kPT, (nmax + kPT - 1) / kPT, G);
     if (mode == 0) {
-      cbt_blocks_kernel<<<dim3(grid1(maxN, 128), G), 128, 0, st>>>(w.pr, w.src, w.dst, w.theta, w.R, w.q, nbs,
-                                                                    w.offA, w.diagB, w.lam, w.mu_terms);
+      cbt_blocks_kernel<<<dim3(grid1(maxN, 128), G), 128, 0, st>>>(w.pr, w.src, w.dst, w.theta, w.R, w.q, w.offA,
+                                                                    w.diagB, w.lam, w.mu_terms);
       cbt_reduce_kernel<<<G, 256, 0, st>>>(w.pr, w.lam, w.mu_terms, w.top);
       cbt_fill_kernel<<<ge, 256, 0, st>>>(w.pr, nmax, w.offA, w.diagB, w.lam, w.top, w.M_init);
       *launches += 3;
       cudaMemcpyAsync(w.M, w.M_init, (size_t)G * nn * sizeof(double), cudaMemcpyDeviceToDevice, st);
     }
     std::vector<int> act(G, 1), idx;  // active flags of the last read-back; their indices (compact batch)
-    int n_act = G, idx_for = -1;         // idx_for: the n_act whose idx is on the device
+    if (dev_in) {  // the gather's flags: a problem with a non-finite measurement starts (and stays) inactive
+      cudaMemcpyAsync(act.data(), w.active, G * sizeof(int), cudaMemcpyDeviceToHost, st);
+      if (cudaStreamSynchronize(st) != cudaSuccess) {
+        *err = cudaGetErrorString(cudaGetLastError());
+        return TZR_ERR_CUDA;
+      }
+      for (int g = 0; g < G; ++g) gathered[b0 + g] = act[g];
+    }
+    int n_act = (int)std::count(act.begin(), act.end(), 1), idx_for = -1;  // idx_for: the n_act whose idx is on the device
     bool full_step = bat;                // the step's eigen columns cover nmax (batched call) or n (Dsyevd)
     // one eigendecomposition of every active problem's Bm, and nothing for the finished ones: the batched call over the
     // padded matrices (in place while every problem is active, else over the active ones gathered into W, which is dead
@@ -1301,7 +1394,7 @@ int certify_batch_device(int mode, const tzr_certifier_params& prm, int B, const
       b0 = b1;
       continue;
     }
-    for (int iter = 0; (double)iter < maxit; ++iter) {
+    for (int iter = 0; n_act > 0 && (double)iter < maxit; ++iter) {
       cbt_sym_kernel<<<ge, 256, 0, st>>>(w.pr, nmax, w.M, w.Bm);
       if (int rc = eig(CUSOLVER_EIG_MODE_VECTOR)) return rc;
       cbt_first_pos_kernel<<<grid1(G, 128), 128, 0, st>>>(w.pr, G, nmax, full_step ? 1 : 0, w.w);

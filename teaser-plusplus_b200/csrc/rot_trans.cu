@@ -19,8 +19,7 @@ namespace tzr {
 
 namespace {
 
-constexpr int kRTThreads = 128;  // 128 regs x 128 threads: 4 CTAs/SM (256 threads: 2)
-constexpr int kRTWarps = kRTThreads / 32;
+constexpr int kRTWarps = kRTThreads / 32;  // kRTThreads (tzr_internal.cuh): 128 regs x 128 threads, 4 CTAs/SM
 
 // ---- 3x3 helpers (column-major like Eigen::Matrix3d) -------------------------------------------
 struct M3 {
@@ -205,36 +204,7 @@ __device__ double block_max(double v, double* s_buf) {
   return s_buf[kRTWarps];
 }
 
-// ---- rotation TIM sets --------------------------------------------------------------------------------
-// CHAIN (registration.cc:657-680): m TIMs materialised in ps/pd (pd already de-scaled, :697).
-// COMPLETE (registration.cc:681-694): all m(m-1)/2 differences of the clique points, in computeTIMs order
-// k = i*m - i(i+1)/2 + (j-i-1); they are recomputed from the m clique points on every pass instead of being
-// materialised (only the per-TIM weight has to persist between GNC iterations).
-struct TimSrc {
-  int complete;
-  int m;                // chain: number of TIMs; complete: number of clique points
-  long long count;      // number of TIMs
-  const double* a;      // chain: src TIMs (3*m)        complete: clique src points (3*m)
-  const double* b;      // chain: dst TIMs, de-scaled   complete: clique dst points (3*m)
-  double inv_scale;     // complete only: 1/scale applied to dst differences
-};
-
-template <class F>
-__device__ __forceinline__ void for_each_tim(const TimSrc& t, F&& f) {
-  if (!t.complete) {
-    for (int k = threadIdx.x; k < t.m; k += kRTThreads)
-      f((long long)k, t.a[3 * k], t.a[3 * k + 1], t.a[3 * k + 2], t.b[3 * k], t.b[3 * k + 1], t.b[3 * k + 2]);
-  } else {
-    for (int i = 0; i + 1 < t.m; ++i) {
-      const long long base = (long long)i * t.m - (long long)i * (i + 1) / 2 - i - 1;
-      const double sx = t.a[3 * i], sy = t.a[3 * i + 1], sz = t.a[3 * i + 2];
-      const double dx = t.b[3 * i], dy = t.b[3 * i + 1], dz = t.b[3 * i + 2];
-      for (int j = i + 1 + threadIdx.x; j < t.m; j += kRTThreads)
-        f(base + j, t.a[3 * j] - sx, t.a[3 * j + 1] - sy, t.a[3 * j + 2] - sz, (t.b[3 * j] - dx) * t.inv_scale,
-          (t.b[3 * j + 1] - dy) * t.inv_scale, (t.b[3 * j + 2] - dz) * t.inv_scale);
-    }
-  }
-}
+// ---- rotation TIM sets: TimSrc and for_each_tim (tzr_internal.cuh) ----------------------------------------------
 
 struct GncOut {
   M3 R;

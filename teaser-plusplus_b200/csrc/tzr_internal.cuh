@@ -143,6 +143,40 @@ struct Batch {
   const int32_t* nb_host;   // host copy of nb (the unknown-scale large path's per-problem host loop)
 };
 
+// ---- rotation TIM sets (shared by rot_trans_kernel and the certifier's gather of a retained solve) ----------------------
+constexpr int kRTThreads = 128;  // threads of the CTAs that walk a TIM set (rot_trans.cu: 128 regs x 128 threads, 4 CTAs/SM)
+
+// CHAIN (registration.cc:657-680): m TIMs materialised in ps/pd (pd already de-scaled, :697).
+// COMPLETE (registration.cc:681-694): all m(m-1)/2 differences of the clique points, in computeTIMs order
+// k = i*m - i(i+1)/2 + (j-i-1); they are recomputed from the m clique points on every pass instead of being
+// materialised (only the per-TIM weight has to persist between GNC iterations).
+struct TimSrc {
+  int complete;
+  int m;                // chain: number of TIMs; complete: number of clique points
+  long long count;      // number of TIMs
+  const double* a;      // chain: src TIMs (3*m)        complete: clique src points (3*m)
+  const double* b;      // chain: dst TIMs, de-scaled   complete: clique dst points (3*m)
+  double inv_scale;     // complete only: 1/scale applied to dst differences
+};
+
+// f(k, src TIM xyz, dst TIM xyz) for every TIM of the set, strided over a CTA of kRTThreads threads
+template <class F>
+__device__ __forceinline__ void for_each_tim(const TimSrc& t, F&& f) {
+  if (!t.complete) {
+    for (int k = threadIdx.x; k < t.m; k += kRTThreads)
+      f((long long)k, t.a[3 * k], t.a[3 * k + 1], t.a[3 * k + 2], t.b[3 * k], t.b[3 * k + 1], t.b[3 * k + 2]);
+  } else {
+    for (int i = 0; i + 1 < t.m; ++i) {
+      const long long base = (long long)i * t.m - (long long)i * (i + 1) / 2 - i - 1;
+      const double sx = t.a[3 * i], sy = t.a[3 * i + 1], sz = t.a[3 * i + 2];
+      const double dx = t.b[3 * i], dy = t.b[3 * i + 1], dz = t.b[3 * i + 2];
+      for (int j = i + 1 + threadIdx.x; j < t.m; j += kRTThreads)
+        f(base + j, t.a[3 * j] - sx, t.a[3 * j + 1] - sy, t.a[3 * j + 2] - sz, (t.b[3 * j] - dx) * t.inv_scale,
+          (t.b[3 * j + 1] - dy) * t.inv_scale, (t.b[3 * j + 2] - dz) * t.inv_scale);
+    }
+  }
+}
+
 // ||v_j - v_i|| exactly as the reference computes a TIM norm: IEEE double, no FMA contraction,
 // src.array().square().colwise().sum() summed as (x^2 + y^2) + z^2   (registration.cc:415-418, :434-437)
 __device__ __forceinline__ double tim_norm_exact(const double* __restrict__ p, int i, int j) {
@@ -270,12 +304,29 @@ int certify_device(int mode, double noise_bound, double cbar2, double sub_optima
                    double* M_init_out, double* mu_out, const double* W_in, double* Wd_out, double* w_out,
                    void** scratch, size_t* scratch_cap, void** solver_handle, int64_t* launches, cudaStream_t st,
                    std::string* err);
+// Device input of one certify_batch_device problem (tzr_certify_last_solve): its measurements are built on the device
+// from a retained solve, exactly as the rotation stage built the TIMs it solved on (rot_trans.cu).
+struct CertGatherProb {
+  const double* src;     // the problem's points (rows of 3 doubles, device)
+  const double* dst;
+  const int32_t* clq;    // its sorted clique, m entries
+  const uint8_t* rmask;  // its rotation inlier mask, N entries: theta = +1 where set, -1 elsewhere
+  double scale;          // solution scale: dst TIMs are multiplied by 1 / scale
+  double nbs;            // cbar2 * nb * nb with nb = noise_bound / scale (host arithmetic, in that order)
+  int m;                 // clique size
+  int complete;          // 1: COMPLETE TIM graph (N = m(m-1)/2), 0: CHAIN (N = m)
+  int k_off, v_off;      // set by certify_batch_device: first measurement and first block row inside the group
+};
+
 // B problems (host pointers, validated by the caller) in device-sized groups of one launch sequence each; loop_eig: one
 // cusolverDnDsyevd per active problem instead of cusolverDnXsyevBatched (debug flag 2097152).  mode 0 certify; the
 // building blocks run one step of the batch's iteration on X_in[b] (n x n) into X_out[b]: 1 nearest-PSD step, 2 dual
-// projection (theta as for mode 0; src, dst, R_cm, results and traj unused)
+// projection (theta as for mode 0; src, dst, R_cm, results and traj unused).  gather (mode 0, may be NULL): B device
+// inputs that replace src, dst, theta and the scalar noise bound; gathered[b] then receives 1, or 0 where the gathered
+// measurements hold a non-finite value (the problem never reaches the eigensolver; result {0, 0, +inf}).
 int certify_batch_device(int mode, const tzr_certifier_params& prm, int B, const int32_t* N, const double* R_cm,
                          const double* const* src, const double* const* dst, const double* const* theta,
+                         const CertGatherProb* gather, int32_t* gathered,
                          tzr_certification_result* results, double* const* traj, const int32_t* traj_cap,
                          const double* const* X_in, double* const* X_out, bool loop_eig, void** scratch,
                          size_t* scratch_cap, void** solver_handle, int64_t* launches, cudaStream_t st,

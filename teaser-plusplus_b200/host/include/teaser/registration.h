@@ -29,6 +29,7 @@
 #include "teaser/eigen_lite.h"
 #endif
 
+#include "teaser/certification.h"
 #include "teaser/geometry.h"
 #include "teaser/graph.h"
 
@@ -257,6 +258,22 @@ class RobustRegistrationSolver {
   std::vector<RegistrationSolution> solveBatch(
       const std::vector<Mat3X>& src, const std::vector<Mat3X>& dst, std::vector<std::vector<int>>* cliques = nullptr,
       const std::vector<int>& devices = {});
+  // One problem of solveAndCertifyBatch: what solve() and the getters give for it alone, and its certification.
+  struct SolveCertifyResult {
+    RegistrationSolution solution;
+    std::vector<int> max_clique;
+    BoolRow rotation_inliers_mask;     // getRotationInliersMask()
+    BoolRow translation_inliers_mask;  // getTranslationInliersMask()
+    bool certified = false;            // false: invalid solution, a non-finite input, or 4N + 4 > 32768
+    CertificationResult certification;
+  };
+  // solve() then DRSCertifier(cert_params).certify(R, getMaxCliqueSrcTIMs(), getMaxCliqueDstTIMs(),
+  // getRotationInliersMask()) on many problems: one batched solve (tzr_solve_batch) and one batched certification of
+  // its retained results (tzr_certify_last_solve) on this thread's context, one device.  Problem b is certified with
+  // noise bound cert_params.noise_bound / scale_b; 2 * this solver's noise_bound certifies what the rotation solver
+  // solved.  The per-problem getters of this object are not touched.
+  std::vector<SolveCertifyResult> solveAndCertifyBatch(const std::vector<Mat3X>& src, const std::vector<Mat3X>& dst,
+                                                       const DRSCertifier::Params& cert_params);
   bool isMaxCliqueProvenOptimal() const { return clique_proven_; }
   long long getNumInlierGraphEdges() const { return n_edges_; }
   int getGNCRotationIterations() const { return gnc_iterations_; }

@@ -127,6 +127,27 @@ PYBIND11_MODULE(_teaserpp, m) {
              return py::make_tuple(sols, cliques);
            },
            py::arg("src"), py::arg("dst"), py::arg("devices") = std::vector<int>{})
+      .def("solve_and_certify_batch",
+           [](Solver& s, const std::vector<ArrD>& src, const std::vector<ArrD>& dst,
+              const teaser::DRSCertifier::Params& cert_params) {
+             // GPU extra: one batched solve and one batched certification of its retained results, one device
+             std::vector<teaser::Mat3X> a, b;
+             for (const auto& x : src) a.push_back(to_mat3x(x));
+             for (const auto& x : dst) b.push_back(to_mat3x(x));
+             std::vector<Solver::SolveCertifyResult> res;
+             {
+               py::gil_scoped_release release;
+               res = s.solveAndCertifyBatch(a, b, cert_params);
+             }
+             py::list out;
+             for (const auto& r : res)
+               out.append(py::dict(py::arg("solution") = r.solution, py::arg("max_clique") = r.max_clique,
+                                   py::arg("rotation_inliers_mask") = row_to_numpy(r.rotation_inliers_mask),
+                                   py::arg("translation_inliers_mask") = row_to_numpy(r.translation_inliers_mask),
+                                   py::arg("certified") = r.certified, py::arg("certification") = r.certification));
+             return out;
+           },
+           py::arg("src"), py::arg("dst"), py::arg("cert_params"))
       .def_property_readonly("solution", &Solver::getSolution)
       .def("getSolution", &Solver::getSolution)
       .def_property_readonly("gnc_rotation_cost_at_termination", &Solver::getGNCRotationCostAtTermination)

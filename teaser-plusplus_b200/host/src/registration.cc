@@ -560,6 +560,73 @@ std::vector<RegistrationSolution> RobustRegistrationSolver::solveBatch(
   return out;
 }
 
+std::vector<RobustRegistrationSolver::SolveCertifyResult> RobustRegistrationSolver::solveAndCertifyBatch(
+    const std::vector<Mat3X>& src, const std::vector<Mat3X>& dst, const DRSCertifier::Params& cert_params) {
+  if (src.size() != dst.size())
+    throw std::invalid_argument("teaser: solveAndCertifyBatch needs as many src as dst clouds");
+  const int B = static_cast<int>(src.size());
+  std::vector<SolveCertifyResult> out(B);
+  if (B == 0) return out;
+  std::vector<int32_t> n(B);
+  std::vector<const double*> sp(B), dp(B);
+  int max_n = 0;
+  for (int b = 0; b < B; ++b) {
+    if (src[b].cols() != dst[b].cols()) throw std::invalid_argument("teaser: src and dst must have the same number of columns");
+    n[b] = static_cast<int32_t>(src[b].cols());
+    sp[b] = src[b].data();
+    dp[b] = dst[b].data();
+    max_n = std::max(max_n, static_cast<int>(n[b]));
+  }
+  tzr_ctx* ctx = b200_context();
+  std::vector<tzr_solution> sols(B);
+  std::vector<int32_t> clq(static_cast<size_t>(B) * max_n);
+  const tzr_params p = to_c(params_);
+  int rc = tzr_solve_batch(ctx, &p, B, n.data(), sp.data(), dp.data(), sols.data(), clq.data(), max_n);
+  if (rc != TZR_OK) fail("RobustRegistrationSolver::solveAndCertifyBatch (solve)", rc, ctx);
+  const bool complete = params_.rotation_tim_graph == INLIER_GRAPH_FORMULATION::COMPLETE;
+  for (int b = 0; b < B; ++b) {
+    SolveCertifyResult& r = out[b];
+    r.solution.valid = sols[b].valid != 0;
+    r.solution.scale = sols[b].scale;
+    for (int k = 0; k < 3; ++k) r.solution.translation(k) = sols[b].translation[k];
+    std::memcpy(r.solution.rotation.data(), sols[b].rotation, sizeof(sols[b].rotation));
+    const size_t m = static_cast<size_t>(std::max(0, sols[b].clique_size));
+    r.max_clique.assign(clq.begin() + static_cast<size_t>(b) * max_n, clq.begin() + static_cast<size_t>(b) * max_n + m);
+    const size_t rot_cap = complete ? (m > 0 ? m * (m - 1) / 2 : 0) : m;
+    std::vector<uint8_t> rm(std::max<size_t>(1, rot_cap)), tm(std::max<size_t>(1, m));
+    int64_t n_rot = 0;
+    int32_t n_trans = 0;
+    rc = tzr_last_inliers(ctx, b, rm.data(), tm.data(), &n_rot, &n_trans);
+    if (rc != TZR_OK) fail("RobustRegistrationSolver::solveAndCertifyBatch (inlier masks)", rc, ctx);
+    mask_from_bytes(rm, static_cast<size_t>(n_rot), &r.rotation_inliers_mask);
+    mask_from_bytes(tm, static_cast<size_t>(n_trans), &r.translation_inliers_mask);
+  }
+  tzr_certifier_params c;
+  tzr_certifier_params_default(&c);
+  c.noise_bound = cert_params.noise_bound;
+  c.cbar2 = cert_params.cbar2;
+  c.sub_optimality = cert_params.sub_optimality;
+  c.max_iterations = cert_params.max_iterations;
+  c.gamma_tau = cert_params.gamma_tau;
+  c.eig_decomposition_solver = static_cast<int>(cert_params.eig_decomposition_solver);
+  const int cap = static_cast<int>(std::max(1.0, std::ceil(cert_params.max_iterations)));
+  std::vector<std::vector<double>> traj(B, std::vector<double>(cap));
+  std::vector<double*> tp(B);
+  for (int b = 0; b < B; ++b) tp[b] = traj[b].data();
+  std::vector<int32_t> caps(B, cap), status(B);
+  std::vector<tzr_certification_result> res(B);
+  rc = tzr_certify_last_solve(ctx, &c, B, nullptr, res.data(), status.data(), tp.data(), caps.data());
+  if (rc != TZR_OK && rc != TZR_ERR_TOO_LARGE) fail("RobustRegistrationSolver::solveAndCertifyBatch (certify)", rc, ctx);
+  for (int b = 0; b < B; ++b) {
+    SolveCertifyResult& r = out[b];
+    r.certified = status[b] == TZR_OK;
+    r.certification.is_optimal = res[b].is_optimal != 0;
+    r.certification.best_suboptimality = res[b].best_suboptimality;
+    r.certification.suboptimality_traj.assign(traj[b].begin(), traj[b].begin() + std::min(res[b].n_iterations, cap));
+  }
+  return out;
+}
+
 void RobustRegistrationSolver::materialise_tims() {
   if (have_tims_ || !solved_) return;
   src_tims_ = computeTIMs(last_src_, &src_tims_map_);
