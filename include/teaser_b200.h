@@ -354,7 +354,7 @@ int tzr_solve_batch_dev(tzr_ctx* ctx, const tzr_params* params, int B, int n, co
 
 /* Device-resident ragged batch: problem b has n[b] >= 1 correspondences (n is a host array).  src_dev/dst_dev hold the
  * problems back to back, sum(n) rows of 3 doubles each, problem b from row sum_{c<b} n[c] (the layout
- * tzr_match_correspondences_batch's outputs give).  solutions_dev: B tzr_solution in the caller's order.  cliques_dev
+ * tzr_register_cloud_pairs builds on the device from the matcher's index pairs).  solutions_dev: B tzr_solution in the caller's order.  cliques_dev
  * (sum(n) int32, may be NULL): problem b's sorted clique from the same row offset, -1 past its clique_size.  The size
  * classes of tzr_solve_batch; the results are those of tzr_solve on each problem alone.  Asynchronous on the context's
  * stream like tzr_solve_batch_dev, except that a class above 32768 correspondences reads back its core sizes. */
@@ -407,6 +407,46 @@ int tzr_last_inliers(tzr_ctx* ctx, int b, uint8_t* rot_inliers, uint8_t* trans_i
 int tzr_certify_last_solve(tzr_ctx* ctx, const tzr_certifier_params* params, int count, const int32_t* problems,
                            tzr_certification_result* results, int32_t* status, double* const* traj,
                            const int32_t* traj_capacity);
+
+/* ---- registering cloud pairs: descriptors, matching and the robust solve in one call --------------------------
+ * What the reference example teaser_cpp_fpfh does per pair (FPFHEstimation::computeFPFHFeatures on both clouds,
+ * Matcher::calculateCorrespondences, solve(src_cloud, dst_cloud, correspondences), registration.cc:553-566), for many
+ * pairs over a shared table of clouds, with every stage on the device and each cloud's descriptors computed once. */
+typedef struct tzr_frontend_params {
+  double normal_search_radius;  /* FPFHEstimation::computeFPFHFeatures, default 0.03 */
+  double fpfh_search_radius;    /* default 0.05 */
+  int32_t use_absolute_scale;   /* Matcher::calculateCorrespondences defaults: 1, 1, 1, 0 */
+  int32_t use_crosscheck;
+  int32_t use_tuple_test;
+  float tuple_scale;
+} tzr_frontend_params;
+
+void tzr_frontend_params_default(tzr_frontend_params* p);
+
+/* n_clouds clouds (host pointers): cloud c has n[c] >= 1 points at pts[c] (n[c] x 3 float).  P pairs: pair_clouds is
+ * P x 2 int32 (source cloud, target cloud); a cloud may appear in any number of pairs, on either side, and a pair may
+ * match a cloud with itself.  tuple_seeds: P seeds of the tuple test (NULL: 0 for every pair).  Synchronous.
+ * Per pair p: solutions[p], status[p] and n_corr[p] are always written.  corr[p] (may be NULL, or hold NULL entries;
+ * capacity n[src] + n[dst] rows x 2 int32) receives the sorted unique correspondences; cliques[p] (same rules and
+ * capacity) the sorted max clique, as rows of corr[p]; global_scale (P floats, may be NULL) Matcher::global_scale_;
+ * problem_index (P int32, may be NULL) p's index in the retained solve, -1 when p was not solved.
+ * status[p]: TZR_OK solved; TZR_ERR_TOO_LARGE when a point of one of its clouds has more than 4096 neighbours inside a
+ * radius (nothing matched, n_corr = 0), or its correspondences exceed the context's max_n, or with estimate_scaling
+ * reach 46341 (correspondences written, not solved); TZR_ERR_INVALID_ARG no correspondence.  An unsolved pair gets a
+ * zeroed record (valid = 0).  Returns TZR_ERR_TOO_LARGE when some pair was too large (every other pair is complete),
+ * TZR_ERR_ALLOC when the batch's buffers do not fit the device (tzr_last_error names the size).
+ * For every solved pair the outputs are bit-identical (the record except stage_ms, the clique, the correspondences and
+ * the global scale) to tzr_compute_fpfh_batch over the clouds, tzr_match_correspondences_batch over the pairs with the
+ * same seeds, the float points at the correspondences converted to float64, then tzr_solve_batch over the solved pairs.
+ * The call is a solve entry: tzr_last_inliers, tzr_last_graph and tzr_certify_last_solve then see the solved pairs in
+ * ascending pair order (problem_index).  Two host synchronisations (plus the core-size read-back of a class above 32768
+ * correspondences): the per-cloud overflow flags, per-pair counts and global scales after matching, from which the
+ * solve's size classes are planned, and the records, correspondences and cliques at the end.  DESIGN.md §3.10. */
+int tzr_register_cloud_pairs(tzr_ctx* ctx, const tzr_frontend_params* fparams, const tzr_params* params,
+                             int n_clouds, const int32_t* n, const float* const* pts,
+                             int P, const int32_t* pair_clouds, const uint64_t* tuple_seeds,
+                             tzr_solution* solutions, int32_t* status, int32_t* problem_index,
+                             int64_t* n_corr, int32_t* const* corr, int32_t* const* cliques, float* global_scale);
 
 /* Graph-stage timing of the most recent tzr_solve_batch_dev, in milliseconds, measured with CUDA
  * events on the context's stream (for the roofline line in bench.py). Requires a prior synchronize. */

@@ -87,6 +87,13 @@ class CertificationResult(C.Structure):
     _fields_ = [("is_optimal", C.c_int32), ("n_iterations", C.c_int32), ("best_suboptimality", C.c_double)]
 
 
+class FrontendParams(C.Structure):
+    """tzr_frontend_params: FPFHEstimation::computeFPFHFeatures' radii and Matcher::calculateCorrespondences' flags."""
+    _fields_ = [("normal_search_radius", C.c_double), ("fpfh_search_radius", C.c_double),
+                ("use_absolute_scale", C.c_int32), ("use_crosscheck", C.c_int32), ("use_tuple_test", C.c_int32),
+                ("tuple_scale", C.c_float)]
+
+
 _SYMBOLS = [
     "tzr_abi_version", "tzr_status_string", "tzr_last_error", "tzr_params_default", "tzr_ctx_create",
     "tzr_ctx_destroy", "tzr_ctx_set_stream", "tzr_ctx_synchronize", "tzr_ctx_kernel_launches", "tzr_words_per_row",
@@ -99,6 +106,7 @@ _SYMBOLS = [
     "tzr_match_correspondences_batch", "tzr_ctx_set_max_n", "tzr_ctx_clique_route", "tzr_certify_batch",
     "tzr_certifier_psd_projection", "tzr_certifier_batch_psd_projection", "tzr_certifier_batch_dual_projection",
     "tzr_fpfh_pair_features", "tzr_fpfh_smallest_eigenpair", "tzr_last_inliers", "tzr_certify_last_solve",
+    "tzr_frontend_params_default", "tzr_register_cloud_pairs",
 ]
 
 # status codes (tzr_status)
@@ -198,6 +206,11 @@ def lib():
     L.tzr_last_inliers.argtypes = [vp, C.c_int, u8p, u8p, i64p, i32p]
     L.tzr_certify_last_solve.argtypes = [vp, C.POINTER(CertifierParams), C.c_int, i32p, C.POINTER(CertificationResult),
                                          i32p, C.POINTER(dp), i32p]
+    L.tzr_frontend_params_default.argtypes = [C.POINTER(FrontendParams)]
+    L.tzr_frontend_params_default.restype = None
+    L.tzr_register_cloud_pairs.argtypes = [vp, C.POINTER(FrontendParams), C.POINTER(Params), C.c_int, i32p, fpp,
+                                           C.c_int, i32p, u64p, C.POINTER(Solution), i32p, i32p, i64p,
+                                           C.POINTER(i32p), C.POINTER(i32p), fp]
     for s in _SYMBOLS:
         getattr(L, s)  # raises AttributeError if the header and the library disagree
     _lib = L
@@ -809,6 +822,53 @@ class Context:
         return [dict(is_optimal=bool(r.is_optimal), best_suboptimality=r.best_suboptimality,
                      suboptimality_traj=t[:r.n_iterations].copy(), status=int(s))
                 for r, t, s in zip(res, trajs, status)]
+
+    def register_cloud_pairs(self, clouds, pairs, params: Params, normal_search_radius=0.03, fpfh_search_radius=0.05,
+                             use_absolute_scale=True, use_crosscheck=True, use_tuple_test=True, tuple_scale=0.0,
+                             tuple_seeds=None):
+        """tzr_register_cloud_pairs: FPFH descriptors of every (n,3) float32 cloud, the correspondences of every
+        (source cloud, target cloud) index pair, and the robust solve of every pair, chained on the device.
+        tuple_seeds: one seed per pair (default 0 each).  Returns (solutions structured array (P,), status (P,) int32,
+        problem_index (P,) int32 (-1: not solved), correspondences (list of (m_p,2) int32), cliques (list of sorted
+        row indices into the correspondences, empty when not solved), global scales (list of floats)).  The call
+        raises only for errors of the whole call; TZR_ERR_TOO_LARGE of some pairs is reported in status."""
+        cl = [np.ascontiguousarray(c, dtype=np.float32) for c in clouds]
+        if not cl or any(c.ndim != 2 or c.shape[1] != 3 or c.shape[0] == 0 for c in cl):
+            raise TzrError("register_cloud_pairs: a non-empty list of non-empty (n,3) clouds is required")
+        pc = np.ascontiguousarray(pairs, dtype=np.int32).reshape(-1, 2)
+        P = pc.shape[0]
+        if P == 0:
+            raise TzrError("register_cloud_pairs: at least one pair is required")
+        seeds = np.zeros(P, dtype=np.uint64) if tuple_seeds is None else \
+            np.ascontiguousarray([int(s) for s in tuple_seeds], dtype=np.uint64)
+        if seeds.shape != (P,):
+            raise TzrError("register_cloud_pairs: tuple_seeds needs one entry per pair")
+        n = np.array([c.shape[0] for c in cl], dtype=np.int32)
+        if pc.min() < 0 or pc.max() >= len(cl):
+            raise TzrError("register_cloud_pairs: a pair names a cloud that is not in the list")
+        fpar = FrontendParams(float(normal_search_radius), float(fpfh_search_radius), int(bool(use_absolute_scale)),
+                              int(bool(use_crosscheck)), int(bool(use_tuple_test)), float(tuple_scale))
+        cap = [int(n[a]) + int(n[b]) for a, b in pc]
+        corr = [np.zeros((c, 2), dtype=np.int32) for c in cap]
+        clq = [np.zeros(c, dtype=np.int32) for c in cap]
+        sols = np.zeros(P, dtype=SOLUTION_DTYPE)
+        status = np.zeros(P, dtype=np.int32)
+        index = np.zeros(P, dtype=np.int32)
+        cnt = np.zeros(P, dtype=np.int64)
+        g = np.zeros(P, dtype=np.float32)
+        fp, i32p = C.POINTER(C.c_float), C.POINTER(C.c_int32)
+        rc = lib().tzr_register_cloud_pairs(
+            self._h, C.byref(fpar), C.byref(params), len(cl), _p(n, C.c_int32),
+            (fp * len(cl))(*[_p(c, C.c_float) for c in cl]), P, _p(pc, C.c_int32), _p(seeds, C.c_uint64),
+            sols.ctypes.data_as(C.POINTER(Solution)), _p(status, C.c_int32), _p(index, C.c_int32),
+            _p(cnt, C.c_int64), (i32p * P)(*[_p(c, C.c_int32) for c in corr]),
+            (i32p * P)(*[_p(c, C.c_int32) for c in clq]), _p(g, C.c_float))
+        if rc not in (0, TZR_ERR_TOO_LARGE):
+            self._ck(rc)
+        corr = [c[:k].copy() for c, k in zip(corr, cnt)]
+        clq = [c[:max(0, int(s["clique_size"]))].copy() if i >= 0 else np.zeros(0, dtype=np.int32)
+               for c, s, i in zip(clq, sols, index)]
+        return sols, status, index, corr, clq, [float(x) for x in g]
 
     def last_graph(self, b: int, n: int):
         W = lib().tzr_words_per_row(n)

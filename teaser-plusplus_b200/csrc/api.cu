@@ -2016,6 +2016,213 @@ int tzr_compute_fpfh_batch(tzr_ctx* ctx, int B, const int32_t* n, const float* c
   return fpfh_run(ctx, B, n, pts, normal_search_radius, fpfh_search_radius, fpfh_out, normals_out, status);
 }
 
+void tzr_frontend_params_default(tzr_frontend_params* p) {
+  if (!p) return;
+  p->normal_search_radius = 0.03;  // fpfh.h:39-41
+  p->fpfh_search_radius = 0.05;
+  p->use_absolute_scale = 1;       // matcher.h:39-43
+  p->use_crosscheck = 1;
+  p->use_tuple_test = 1;
+  p->tuple_scale = 0.f;
+}
+
+// FPFH over the clouds, matching over the pairs, the ragged solve over the pairs that can be solved (DESIGN.md §3.10).
+// Workspace: m_in holds the clouds and every table, m_scratch the FPFH scratch and then the matcher's, m_out the stages'
+// outputs (descriptors alive while matching runs) and the solve's inputs and outputs.  All of it is sized before any work.
+int tzr_register_cloud_pairs(tzr_ctx* ctx, const tzr_frontend_params* fp, const tzr_params* params, int n_clouds,
+                             const int32_t* n, const float* const* pts, int P, const int32_t* pair_clouds,
+                             const uint64_t* tuple_seeds, tzr_solution* solutions, int32_t* status,
+                             int32_t* problem_index, int64_t* n_corr, int32_t* const* corr, int32_t* const* cliques,
+                             float* global_scale) {
+  if (!ctx || !fp || !params || n_clouds < 1 || !n || !pts || P < 1 || !pair_clouds || !solutions || !status ||
+      !n_corr || !(fp->normal_search_radius > 0) || !(fp->fpfh_search_radius > 0))
+    return TZR_ERR_INVALID_ARG;
+  for (int c = 0; c < n_clouds; ++c)
+    if (n[c] <= 0 || !pts[c]) return TZR_ERR_INVALID_ARG;
+  std::vector<int32_t> ns(P), nd(P);
+  std::vector<uint64_t> seeds(P, 0);
+  std::vector<int2> cloud_lo(P);
+  for (int p = 0; p < P; ++p) {
+    const int a = pair_clouds[2 * p], b = pair_clouds[2 * p + 1];
+    if (a < 0 || a >= n_clouds || b < 0 || b >= n_clouds) return TZR_ERR_INVALID_ARG;
+    ns[p] = n[a];
+    nd[p] = n[b];
+    if (tuple_seeds) seeds[p] = tuple_seeds[p];
+  }
+  std::vector<FpfhCloud> clouds((size_t)n_clouds);
+  FpfhPlan fplan;
+  std::vector<MatchPair> MP;
+  std::vector<NnWork> W;
+  MatchPlan mplan;
+  const int route = (ctx->flags & 4194304u) ? kFpfhRouteBrute : (ctx->flags & 8388608u) ? kFpfhRouteGrid : kFpfhRouteAuto;
+  if (fpfh_plan(n_clouds, n, fp->normal_search_radius, fp->fpfh_search_radius, route, clouds.data(), &fplan) != TZR_OK ||
+      match_plan(P, ns.data(), nd.data(), seeds.data(), ctx->num_sms, &MP, &W, &mplan) != TZR_OK) {
+    ctx->last_error = "the batch's points do not fit 32-bit indices";
+    return TZR_ERR_TOO_LARGE;
+  }
+  for (int p = 0; p < P; ++p) cloud_lo[p] = make_int2(clouds[pair_clouds[2 * p]].lo, clouds[pair_clouds[2 * p + 1]].lo);
+  cudaSetDevice(ctx->device);
+  cudaStream_t st = ctx->stream;
+  const size_t N = (size_t)fplan.N, NS = (size_t)mplan.NS, ND = (size_t)mplan.ND, C = NS + ND;
+  // m_in: cloud points | FPFH cloud table | pair table | NN work list | cloud offsets per pair | gather table
+  const size_t o_ct = al256(N * 12), o_mp = o_ct + al256((size_t)n_clouds * sizeof(FpfhCloud)),
+               o_w = o_mp + al256((size_t)P * sizeof(MatchPair)), o_lo = o_w + al256(W.size() * sizeof(NnWork)),
+               o_g = o_lo + al256((size_t)P * sizeof(int2)), in_bytes = o_g + (size_t)P * sizeof(PairGather);
+  // m_out: [overflow | counts | global scales] | descriptors | normals | matcher points and descriptors | matcher rows |
+  // solve src | solve dst | records | compacted index pairs | cliques
+  const size_t o_cnt = al256((size_t)n_clouds * 4), o_gs = o_cnt + (size_t)P * 4, head = o_gs + (size_t)P * 4;
+  const size_t o_desc = al256(head), o_nrm = o_desc + al256(N * 33 * 4), o_msp = o_nrm + al256(N * 16),
+               o_mdp = o_msp + al256(NS * 12), o_msf = o_mdp + al256(ND * 12), o_mdf = o_msf + al256(NS * 33 * 4),
+               o_pairs = o_mdf + al256(ND * 33 * 4), o_src = o_pairs + al256(C * 8), o_dst = o_src + al256(C * 24),
+               o_sol = o_dst + al256(C * 24), o_corr = o_sol + al256((size_t)P * sizeof(tzr_solution)),
+               o_clq = o_corr + al256(C * 8), out_bytes = o_clq + C * 4;
+  const size_t scratch_bytes = std::max(al256(N * 33 * 4) + fplan.grid_bytes, match_scratch_bytes(mplan));
+  // pinned: staged inputs | read-back head | gather table | records | index pairs | cliques
+  const size_t h_head = al256(o_g), h_g = h_head + al256(head), h_sol = h_g + al256((size_t)P * sizeof(PairGather)),
+               h_corr = h_sol + al256((size_t)P * sizeof(tzr_solution)), h_clq = h_corr + al256(C * 8),
+               pin_bytes = h_clq + C * 4;
+  int rc;
+  if ((rc = ensure(ctx, ctx->m_in, in_bytes)) != TZR_OK) return rc;
+  if ((rc = ensure(ctx, ctx->m_scratch, scratch_bytes)) != TZR_OK) return rc;
+  if ((rc = ensure(ctx, ctx->m_out, out_bytes)) != TZR_OK) return rc;
+  if ((rc = ensure_pinned(ctx, pin_bytes)) != TZR_OK) return rc;
+  char* h = (char*)ctx->h_pin;
+  char* d_in = (char*)ctx->m_in.p;
+  char* d_out = (char*)ctx->m_out.p;
+  std::vector<CopySpan> spans;
+  for (int c = 0; c < n_clouds; ++c) spans.push_back(CopySpan{h + (size_t)clouds[c].lo * 12, pts[c], (size_t)n[c] * 12});
+  spans.push_back(CopySpan{h + o_ct, clouds.data(), (size_t)n_clouds * sizeof(FpfhCloud)});
+  spans.push_back(CopySpan{h + o_mp, MP.data(), (size_t)P * sizeof(MatchPair)});
+  spans.push_back(CopySpan{h + o_w, W.data(), W.size() * sizeof(NnWork)});
+  spans.push_back(CopySpan{h + o_lo, cloud_lo.data(), (size_t)P * sizeof(int2)});
+  CK(stage_in(spans, h, d_in, o_ct, o_g, false, st));
+  const float* d_pts = (const float*)d_in;
+  const MatchPair* d_mp = (const MatchPair*)(d_in + o_mp);
+  float* d_desc = (float*)(d_out + o_desc);
+  ctx->launches += launch_fpfh(fplan, d_pts, (FpfhCloud*)(d_in + o_ct), fp->normal_search_radius,
+                               fp->fpfh_search_radius, (float4*)(d_out + o_nrm), (float*)ctx->m_scratch.p, d_desc,
+                               (int*)d_out, fplan.grid_bytes ? (char*)ctx->m_scratch.p + al256(N * 33 * 4) : nullptr, st);
+  float* d_msp = (float*)(d_out + o_msp);
+  float* d_mdp = (float*)(d_out + o_mdp);
+  float* d_msf = (float*)(d_out + o_msf);
+  float* d_mdf = (float*)(d_out + o_mdf);
+  ctx->launches += launch_pair_rows(mplan, d_mp, (const int2*)(d_in + o_lo), d_pts, d_desc, d_msp, d_mdp, d_msf, d_mdf,
+                                    ctx->num_sms, st);
+  const int32_t* d_pairs = (const int32_t*)(d_out + o_pairs);
+  ctx->launches += launch_match(mplan, d_mp, (const NnWork*)(d_in + o_w), (int)W.size(), d_msp, d_mdp, d_msf, d_mdf,
+                                33, fp->use_absolute_scale, fp->use_crosscheck, fp->use_tuple_test, fp->tuple_scale,
+                                ctx->m_scratch.p, (int32_t*)d_pairs, (int*)(d_out + o_cnt), (float*)(d_out + o_gs),
+                                ctx->num_sms, st);
+  if ((rc = check_launch(ctx, "front-end launch")) != TZR_OK) return rc;
+  // synchronisation 1: which pairs go on, and their sizes (the solve's size classes are planned on the host)
+  CK(cudaMemcpyAsync(h + h_head, d_out, head, cudaMemcpyDeviceToHost, st));
+  CK(cudaStreamSynchronize(st));
+  const int* overflow = (const int*)(h + h_head);
+  const int* counts = (const int*)(h + h_head + o_cnt);
+  const float* gs = (const float*)(h + h_head + o_gs);
+  PairGather* table = (PairGather*)(h + h_g);
+  std::vector<int32_t> solved_n;
+  std::vector<int> solved;  // pair of every retained problem
+  std::vector<long long> corr_row(P, -1);
+  int n_table = 0, max_count = 0;
+  long long corr_rows = 0, solve_rows = 0;
+  bool too_large = false;
+  for (int p = 0; p < P; ++p) {
+    if (global_scale) global_scale[p] = gs[p];
+    if (problem_index) problem_index[p] = -1;
+    memset(&solutions[p], 0, sizeof(tzr_solution));
+    if (overflow[pair_clouds[2 * p]] || overflow[pair_clouds[2 * p + 1]]) {
+      status[p] = TZR_ERR_TOO_LARGE;
+      n_corr[p] = 0;
+      too_large = true;
+      continue;
+    }
+    const int cnt = counts[p];
+    n_corr[p] = cnt;
+    if (cnt == 0) {
+      status[p] = TZR_ERR_INVALID_ARG;
+      continue;
+    }
+    const bool solve = cnt <= ctx->max_n && !(params->estimate_scaling && !scale_scratch_bytes(1, cnt, ctx->flags));
+    status[p] = solve ? TZR_OK : TZR_ERR_TOO_LARGE;
+    too_large |= !solve;
+    const bool want_corr = corr && corr[p];
+    if (!solve && !want_corr) continue;
+    PairGather& g = table[n_table++];
+    g.src_lo = cloud_lo[p].x;
+    g.dst_lo = cloud_lo[p].y;
+    g.slot = MP[p].s_off + MP[p].d_off;
+    g.count = cnt;
+    g.corr_row = want_corr ? corr_rows : -1;
+    g.solve_row = solve ? solve_rows : -1;
+    max_count = std::max(max_count, cnt);
+    if (want_corr) {
+      corr_row[p] = corr_rows;
+      corr_rows += cnt;
+    }
+    if (solve) {
+      if (problem_index) problem_index[p] = (int32_t)solved.size();
+      solved.push_back(p);
+      solved_n.push_back(cnt);
+      solve_rows += cnt;
+    }
+  }
+  double* d_src = (double*)(d_out + o_src);
+  double* d_dst = (double*)(d_out + o_dst);
+  int2* d_corr = (int2*)(d_out + o_corr);
+  if (n_table > 0) {
+    CK(cudaMemcpyAsync(d_in + o_g, table, (size_t)n_table * sizeof(PairGather), cudaMemcpyHostToDevice, st));
+    ctx->launches += launch_corr_gather((const PairGather*)(d_in + o_g), n_table, max_count, d_pairs, d_pts, d_corr,
+                                        d_src, d_dst, st);
+    if ((rc = check_launch(ctx, "correspondence gather")) != TZR_OK) return rc;
+  }
+  const int S = (int)solved.size();
+  bool want_clq = false;
+  for (int k = 0; k < S && cliques; ++k) want_clq |= cliques[solved[k]] != nullptr;
+  tzr_solution* d_sol = (tzr_solution*)(d_out + o_sol);
+  int32_t* d_clq = (int32_t*)(d_out + o_clq);
+  if (S > 0) {
+    rc = solve_ragged_dev(ctx, *params, S, solved_n.data(), d_src, d_dst, d_sol, want_clq ? d_clq : nullptr);
+    if (rc) return rc;
+  } else {  // nothing solved: no solve is retained
+    ctx->have_last = false;
+    ctx->last_is_solve = false;
+    ctx->last_has_graph = false;
+    ctx->ragged_last.clear();
+    ++ctx->generation;
+  }
+  // synchronisation 2: the records, and the index pairs and cliques that were asked for
+  if (S > 0) CK(cudaMemcpyAsync(h + h_sol, d_sol, (size_t)S * sizeof(tzr_solution), cudaMemcpyDeviceToHost, st));
+  if (corr_rows > 0) CK(cudaMemcpyAsync(h + h_corr, d_corr, (size_t)corr_rows * 8, cudaMemcpyDeviceToHost, st));
+  if (want_clq) CK(cudaMemcpyAsync(h + h_clq, d_clq, (size_t)solve_rows * 4, cudaMemcpyDeviceToHost, st));
+  CK(cudaStreamSynchronize(st));
+  const tzr_solution* sol = (const tzr_solution*)(h + h_sol);
+  spans.clear();
+  for (int p = 0; p < P; ++p)
+    if (corr_row[p] >= 0) spans.push_back(CopySpan{corr[p], h + h_corr + (size_t)corr_row[p] * 8, (size_t)n_corr[p] * 8});
+  bool no_room = false;
+  long long row = 0;
+  for (int k = 0; k < S; ++k) {
+    const int p = solved[k];
+    solutions[p] = sol[k];
+    no_room |= sol[k].clique_proven_optimal == -2;
+    const int m = std::max(0, std::min(solved_n[k], sol[k].clique_size));
+    if (want_clq && cliques[p]) spans.push_back(CopySpan{cliques[p], h + h_clq + (size_t)row * 4, (size_t)m * 4});
+    row += solved_n[k];
+  }
+  parallel_copy(spans);
+  if (no_room) {
+    ctx->last_error = "COMPLETE TIM graph of this clique does not fit the rotation workspace";
+    return TZR_ERR_TOO_LARGE;
+  }
+  if (too_large) {
+    ctx->last_error = "a pair's cloud has a point with more than 4096 neighbours inside a radius, or its correspondences "
+                      "exceed the solve's size limit";
+    return TZR_ERR_TOO_LARGE;
+  }
+  return TZR_OK;
+}
+
 int tzr_fpfh_pair_features(tzr_ctx* ctx, int n, const float* p1, const float* n1, const float* p2, const float* n2,
                            float* f_out, int32_t* ok_out) {
   if (!ctx || n <= 0 || !p1 || !n1 || !p2 || !n2 || !f_out || !ok_out) return TZR_ERR_INVALID_ARG;

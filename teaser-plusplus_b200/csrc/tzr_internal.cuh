@@ -370,5 +370,22 @@ int launch_match(const MatchPlan& plan, const MatchPair* pairs, const NnWork* wo
                  int use_crosscheck, int use_tuple_test, float tuple_scale, void* scratch, int32_t* out_pairs,
                  int* counts, float* gscale, int num_sms, cudaStream_t st);
 
+// register_pairs.cu (tzr_register_cloud_pairs, DESIGN.md §3.10): the handoffs FPFH -> matcher -> ragged solve
+struct PairGather {     // one per pair whose matcher rows go on, built on the host from the read-back counts
+  int src_lo, dst_lo;   // first point of the pair's source / target cloud in the flat cloud array
+  int slot, count;      // first row of the pair in the matcher's output (s_off + d_off), its correspondences
+  long long corr_row;   // first row of its compacted index pairs, -1: not written
+  long long solve_row;  // first row of its problem in the solve's flat float64 arrays, -1: not solved
+};
+// Copies every pair's rows of the clouds (pts: flat n x 3, feat: flat n x 33; cloud_lo[b] = first point of pair b's
+// source, target cloud) into the matcher's flat source / target arrays of `plan`.  Returns the launches.
+int launch_pair_rows(const MatchPlan& plan, const MatchPair* pairs, const int2* cloud_lo, const float* pts,
+                     const float* feat, float* src_pts, float* dst_pts, float* src_feat, float* dst_feat, int num_sms,
+                     cudaStream_t st);
+// For the n_entries pairs of `table` (max_count: their largest count): the matcher's rows `pairs` -> corr (int2) and
+// src / dst (float64 rows of pts).  Returns the launches.
+int launch_corr_gather(const PairGather* table, int n_entries, int max_count, const int32_t* pairs, const float* pts,
+                       int2* corr, double* src, double* dst, cudaStream_t st);
+
 
 }  // namespace tzr

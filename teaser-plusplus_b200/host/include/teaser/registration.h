@@ -13,6 +13,7 @@
 //       access, never inside solve().
 #pragma once
 
+#include <cstdint>
 #include <memory>
 #include <stdexcept>
 #include <tuple>
@@ -274,6 +275,37 @@ class RobustRegistrationSolver {
   // solved.  The per-problem getters of this object are not touched.
   std::vector<SolveCertifyResult> solveAndCertifyBatch(const std::vector<Mat3X>& src, const std::vector<Mat3X>& dst,
                                                        const DRSCertifier::Params& cert_params);
+  // The front end of solveCloudPairs: FPFHEstimation::computeFPFHFeatures' radii and Matcher::calculateCorrespondences'
+  // flags (same defaults).  Pair p uses tuple seed tuple_seed + p * 0x9E3779B97F4A7C15, the seed
+  // Matcher::calculateCorrespondencesBatch gives its p-th pair (tuple_seed: a fresh Matcher's).
+  struct CloudPairParams {
+    double normal_search_radius = 0.03;
+    double fpfh_search_radius = 0.05;
+    bool use_absolute_scale = true;
+    bool use_crosscheck = true;
+    bool use_tuple_test = true;
+    float tuple_scale = 0;
+    uint64_t tuple_seed = 0x7ea5e2ull;
+  };
+  // One pair of solveCloudPairs.  status: 0 (TZR_OK) solved; TZR_ERR_TOO_LARGE (-6) a cloud with a point of more than
+  // 4096 neighbours (no correspondences), or more correspondences than one solve takes (65536, or 46340 with
+  // estimate_scaling; correspondences given, not solved); TZR_ERR_INVALID_ARG (-1) no correspondence.  An unsolved
+  // pair has an invalid solution and an empty clique.
+  struct CloudPairResult {
+    int status = 0;
+    std::vector<std::pair<int, int>> correspondences;  // sorted, unique (source index, target index)
+    RegistrationSolution solution;
+    std::vector<int> max_clique;  // sorted rows of correspondences
+    float global_scale = 1;       // Matcher::getGlobalScale()
+  };
+  // FPFHEstimation::computeFPFHFeaturesBatch(clouds), Matcher::calculateCorrespondencesBatch over the pairs (source
+  // cloud, target cloud) and solve(clouds[src], clouds[dst], correspondences) per pair with this solver's Params, in
+  // one device call (tzr_register_cloud_pairs) on this thread's context: each cloud's descriptors are computed once,
+  // however many pairs name it.  Every cloud must be non-empty.  The per-problem getters of this object are not
+  // touched.
+  std::vector<CloudPairResult> solveCloudPairs(const std::vector<PointCloud>& clouds,
+                                               const std::vector<std::pair<int, int>>& pairs,
+                                               const CloudPairParams& params);
   bool isMaxCliqueProvenOptimal() const { return clique_proven_; }
   long long getNumInlierGraphEdges() const { return n_edges_; }
   int getGNCRotationIterations() const { return gnc_iterations_; }

@@ -148,6 +148,43 @@ PYBIND11_MODULE(_teaserpp, m) {
              return out;
            },
            py::arg("src"), py::arg("dst"), py::arg("cert_params"))
+      .def("solve_cloud_pairs",
+           [](Solver& s, const std::vector<py::array_t<float, py::array::c_style | py::array::forcecast>>& clouds,
+              const std::vector<std::pair<int, int>>& pairs, double normal_search_radius, double fpfh_search_radius,
+              bool use_absolute_scale, bool use_crosscheck, bool use_tuple_test, float tuple_scale,
+              uint64_t tuple_seed) {
+             // GPU extra: FPFH, matching and the solve of many cloud pairs in one device call (solveCloudPairs)
+             std::vector<teaser::PointCloud> pcs(clouds.size());
+             for (size_t c = 0; c < clouds.size(); ++c) {
+               const auto& a = clouds[c];
+               if (a.ndim() != 2 || a.shape(1) != 3) throw std::invalid_argument("clouds must be (n,3) arrays");
+               const float* d = a.data();
+               pcs[c].reserve(static_cast<size_t>(a.shape(0)));
+               for (py::ssize_t i = 0; i < a.shape(0); ++i) pcs[c].push_back({d[3 * i], d[3 * i + 1], d[3 * i + 2]});
+             }
+             Solver::CloudPairParams cp;
+             cp.normal_search_radius = normal_search_radius;
+             cp.fpfh_search_radius = fpfh_search_radius;
+             cp.use_absolute_scale = use_absolute_scale;
+             cp.use_crosscheck = use_crosscheck;
+             cp.use_tuple_test = use_tuple_test;
+             cp.tuple_scale = tuple_scale;
+             cp.tuple_seed = tuple_seed;
+             std::vector<Solver::CloudPairResult> res;
+             {
+               py::gil_scoped_release release;
+               res = s.solveCloudPairs(pcs, pairs, cp);
+             }
+             py::list out;
+             for (const auto& r : res)
+               out.append(py::dict(py::arg("status") = r.status, py::arg("correspondences") = r.correspondences,
+                                   py::arg("solution") = r.solution, py::arg("max_clique") = r.max_clique,
+                                   py::arg("global_scale") = r.global_scale));
+             return out;
+           },
+           py::arg("clouds"), py::arg("pairs"), py::arg("normal_search_radius") = 0.03,
+           py::arg("fpfh_search_radius") = 0.05, py::arg("use_absolute_scale") = true, py::arg("use_crosscheck") = true,
+           py::arg("use_tuple_test") = true, py::arg("tuple_scale") = 0.0f, py::arg("tuple_seed") = 0x7ea5e2ull)
       .def_property_readonly("solution", &Solver::getSolution)
       .def("getSolution", &Solver::getSolution)
       .def_property_readonly("gnc_rotation_cost_at_termination", &Solver::getGNCRotationCostAtTermination)

@@ -627,6 +627,66 @@ std::vector<RobustRegistrationSolver::SolveCertifyResult> RobustRegistrationSolv
   return out;
 }
 
+std::vector<RobustRegistrationSolver::CloudPairResult> RobustRegistrationSolver::solveCloudPairs(
+    const std::vector<PointCloud>& clouds, const std::vector<std::pair<int, int>>& pairs, const CloudPairParams& cp) {
+  const int K = static_cast<int>(clouds.size()), P = static_cast<int>(pairs.size());
+  std::vector<CloudPairResult> out(P);
+  if (P == 0) return out;
+  static_assert(sizeof(PointXYZ) == 3 * sizeof(float), "PointXYZ must be three packed floats");
+  std::vector<int32_t> n(K), pc(2 * static_cast<size_t>(P)), status(P), index(P);
+  std::vector<const float*> pts(K);
+  for (int c = 0; c < K; ++c) {
+    if (clouds[c].empty()) throw std::invalid_argument("teaser: solveCloudPairs needs non-empty clouds");
+    n[c] = static_cast<int32_t>(clouds[c].size());
+    pts[c] = &clouds[c][0].x;
+  }
+  std::vector<uint64_t> seeds(P);
+  std::vector<std::vector<int32_t>> corr(P), clq(P);
+  std::vector<int32_t*> corr_p(P), clq_p(P);
+  for (int p = 0; p < P; ++p) {
+    const int a = pairs[p].first, b = pairs[p].second;
+    if (a < 0 || a >= K || b < 0 || b >= K) throw std::invalid_argument("teaser: solveCloudPairs: no such cloud");
+    pc[2 * p] = a;
+    pc[2 * p + 1] = b;
+    seeds[p] = cp.tuple_seed + 0x9E3779B97F4A7C15ull * static_cast<uint64_t>(p);
+    const size_t cap = static_cast<size_t>(n[a]) + n[b];
+    corr[p].resize(2 * cap);
+    clq[p].resize(cap);
+    corr_p[p] = corr[p].data();
+    clq_p[p] = clq[p].data();
+  }
+  tzr_frontend_params f;
+  tzr_frontend_params_default(&f);
+  f.normal_search_radius = cp.normal_search_radius;
+  f.fpfh_search_radius = cp.fpfh_search_radius;
+  f.use_absolute_scale = cp.use_absolute_scale ? 1 : 0;
+  f.use_crosscheck = cp.use_crosscheck ? 1 : 0;
+  f.use_tuple_test = cp.use_tuple_test ? 1 : 0;
+  f.tuple_scale = cp.tuple_scale;
+  const tzr_params p = to_c(params_);
+  std::vector<tzr_solution> sols(P);
+  std::vector<int64_t> n_corr(P);
+  std::vector<float> scales(P);
+  tzr_ctx* ctx = b200_context();
+  const int rc = tzr_register_cloud_pairs(ctx, &f, &p, K, n.data(), pts.data(), P, pc.data(), seeds.data(), sols.data(),
+                                          status.data(), index.data(), n_corr.data(), corr_p.data(), clq_p.data(),
+                                          scales.data());
+  if (rc != TZR_OK && rc != TZR_ERR_TOO_LARGE) fail("RobustRegistrationSolver::solveCloudPairs", rc, ctx);
+  for (int q = 0; q < P; ++q) {
+    CloudPairResult& r = out[q];
+    r.status = status[q];
+    r.global_scale = scales[q];
+    r.correspondences.reserve(static_cast<size_t>(n_corr[q]));
+    for (int64_t c = 0; c < n_corr[q]; ++c) r.correspondences.emplace_back(corr[q][2 * c], corr[q][2 * c + 1]);
+    r.solution.valid = sols[q].valid != 0;
+    r.solution.scale = sols[q].scale;
+    for (int k = 0; k < 3; ++k) r.solution.translation(k) = sols[q].translation[k];
+    std::memcpy(r.solution.rotation.data(), sols[q].rotation, sizeof(sols[q].rotation));
+    if (index[q] >= 0) r.max_clique.assign(clq[q].begin(), clq[q].begin() + std::max(0, sols[q].clique_size));
+  }
+  return out;
+}
+
 void RobustRegistrationSolver::materialise_tims() {
   if (have_tims_ || !solved_) return;
   src_tims_ = computeTIMs(last_src_, &src_tims_map_);
