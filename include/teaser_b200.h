@@ -448,6 +448,91 @@ int tzr_register_cloud_pairs(tzr_ctx* ctx, const tzr_frontend_params* fparams, c
                              tzr_solution* solutions, int32_t* status, int32_t* problem_index,
                              int64_t* n_corr, int32_t* const* corr, int32_t* const* cliques, float* global_scale);
 
+/* ---- refining registrations: point-to-point ICP -------------------------------------------------------------
+ * The refinement step of the reference's FPFH + TEASER++ + ICP tutorial (examples/teaser_python_fpfh_icp: Open3D's
+ * registration_icp with TransformationEstimationPointToPoint, seeded with TEASER's solution), for many problems at once.
+ * The loop is Open3D's RegistrationICP with ICPConvergenceCriteria, defined here as follows (DESIGN.md §3.11):
+ *   - Inputs: source x (ns float xyz), target y (nd float xyz), both read exactly as float64, and an initial similarity
+ *     (s, R0, t0).  s is held fixed (1 for rigid ICP, a solve's scale when seeded from an estimate_scaling solve).
+ *   - Transform: p_i = s * (R x_i) + t, row r computed as s * ((R(r,0) x + R(r,1) y) + R(r,2) z) + t(r) from the
+ *     original point and the current (R, t), never incrementally (IEEE double, no FMA contraction).
+ *   - Correspondence of p_i: the target with the smallest d^2 = (dx dx + dy dy) + dz dz in float64, strictly d^2 < r^2
+ *     with r = max_correspondence_distance and r^2 rounded once; the lowest target index among equal d^2; none for a
+ *     non-finite p_i, and a non-finite target point is never matched.
+ *   - eval(T): count of correspondences, fitness = count / ns (ns includes non-finite points), inlier_rmse =
+ *     sqrt(sum d^2 / count); both 0 when count = 0.
+ *   - Update (R_u, t_u) from the current correspondences: count >= 3: Kabsch on centred coordinates, H = sum (p - mu_p)
+ *     (q - mu_q)^T, R_u the rotation stage's SVD with the reflection fix, t_u = mu_q - R_u mu_p; count 1 or 2: R_u = I,
+ *     t_u = mu_q - mu_p; count 0: the identity.
+ *   - Loop: r_0 = eval(T_0); for i < max_iteration: R <- R_u R, t <- R_u t + t_u, r_{i+1} = eval(T_{i+1}), iterations =
+ *     i + 1, stop with converged = 1 when |delta fitness| < relative_fitness and |delta rmse| < relative_rmse.
+ * Host pointers, synchronous.  The iterations are enqueued without a host synchronisation: 2 + 4 * max_iteration kernel
+ * launches per call (+ 4 for the grid build when some target has at least 1024 points), whatever B; a finished problem
+ * costs nothing in later launches.  The nearest-neighbour search is brute force below 1024 target points and a hashed
+ * uniform grid (cell edge r (1 + 1e-5)) from there on; both give the same correspondences (debug flags 33554432 and
+ * 67108864).  These calls are not solve entries: they use a workspace of their own, so a retained solve
+ * (tzr_last_inliers, tzr_last_graph, tzr_certify_last_solve) stays retained across them. */
+typedef struct tzr_icp_params {
+  double max_correspondence_distance;  /* no default, as in Open3D: <= 0 or non-finite is TZR_ERR_INVALID_ARG */
+  double relative_fitness;             /* 1e-6 (ICPConvergenceCriteria) */
+  double relative_rmse;                /* 1e-6 */
+  int32_t max_iteration;               /* 30; >= 0 */
+  int32_t reserved;
+} tzr_icp_params;
+
+typedef struct tzr_similarity {
+  double scale;
+  double rotation[9];    /* column-major */
+  double translation[3];
+} tzr_similarity;
+
+typedef struct tzr_icp_result {
+  tzr_similarity transform;  /* the last T (scale unchanged) */
+  double fitness;
+  double inlier_rmse;
+  int32_t iterations;
+  int32_t n_correspondences;
+  int32_t converged;
+  int32_t reserved;
+} tzr_icp_result;
+
+/* max_correspondence_distance 0 (the caller must set it), relative_fitness 1e-6, relative_rmse 1e-6, max_iteration 30. */
+void tzr_icp_params_default(tzr_icp_params* p);
+
+/* One problem.  init may be NULL (identity, scale 1); a non-finite init or a scale <= 0 is TZR_ERR_INVALID_ARG.
+ * corr (may be NULL; capacity ns x 2 int32): the final correspondences (source index, target index), ascending by
+ * source, result->n_correspondences rows.  With max_iteration = 0 the result is init, its evaluation, 0 iterations and
+ * converged = 0.  This is tzr_icp_batch with B = 1. */
+int tzr_icp(tzr_ctx* ctx, const tzr_icp_params* params, const float* src, int ns, const float* dst, int nd,
+            const tzr_similarity* init, tzr_icp_result* result, int32_t* corr);
+
+/* B ragged problems: problem b has ns[b] >= 1 source points at src[b] and nd[b] >= 1 target points at dst[b], its
+ * initial similarity at init[b]; params apply to every problem.  results: B entries.  corr (may be NULL, or hold NULL
+ * entries): as tzr_icp's, per problem.  Per problem, every output is bit-identical to tzr_icp on that problem alone:
+ * every reduction runs in an order fixed by the problem's own points.  TZR_ERR_TOO_LARGE when the sources or the targets
+ * of the batch exceed 2^31 - 1 points; TZR_ERR_ALLOC when the workspace does not fit the device (tzr_last_error names
+ * the size). */
+int tzr_icp_batch(tzr_ctx* ctx, const tzr_icp_params* params, int B, const int32_t* ns, const float* const* src,
+                  const int32_t* nd, const float* const* dst, const tzr_similarity* init, tzr_icp_result* results,
+                  int32_t* const* corr);
+
+/* tzr_register_cloud_pairs (same arguments, same outputs bit for bit), then ICP of every solved pair whose solution is
+ * valid, on the pair's two clouds (source cloud, target cloud), seeded with (scale, rotation, translation) of its
+ * solution.  icp (required) applies to every pair.  icp_results: P entries; a pair that was not refined (not solved,
+ * or its solution not valid or not finite) gets a zeroed record, which the caller can tell from status[p] and
+ * solutions[p].valid.  Each refined record is bit-identical to tzr_icp_batch over the valid solved pairs seeded with
+ * their records.  The clouds and records are already on the device: the refinement adds no host synchronisation and no
+ * upload of points, and it runs before the call's second synchronisation.  Launches: tzr_register_cloud_pairs' own plus,
+ * when some pair was solved, 1 seed launch and tzr_icp_batch's (2 + 4 * max_iteration, + 4 when some cloud has 1024
+ * points or more).  Like tzr_register_cloud_pairs this is a solve entry: tzr_last_inliers, tzr_last_graph and
+ * tzr_certify_last_solve see its solve, which the refinement does not touch. */
+int tzr_register_cloud_pairs_icp(tzr_ctx* ctx, const tzr_frontend_params* fparams, const tzr_params* params,
+                                 int n_clouds, const int32_t* n, const float* const* pts,
+                                 int P, const int32_t* pair_clouds, const uint64_t* tuple_seeds,
+                                 tzr_solution* solutions, int32_t* status, int32_t* problem_index,
+                                 int64_t* n_corr, int32_t* const* corr, int32_t* const* cliques, float* global_scale,
+                                 const tzr_icp_params* icp, tzr_icp_result* icp_results);
+
 /* Graph-stage timing of the most recent tzr_solve_batch_dev, in milliseconds, measured with CUDA
  * events on the context's stream (for the roofline line in bench.py). Requires a prior synchronize. */
 int tzr_last_stage_ms(tzr_ctx* ctx, double* prep_ms, double* graph_ms, double* clique_ms, double* rot_trans_ms);
@@ -493,8 +578,11 @@ int tzr_solve_batch_multi(const int32_t* devices, int n_devices, const tzr_param
  * (8388608) = through the hashed grid at any cloud size (DESIGN.md 3.7; a cloud the grid cannot index still falls back
  * to brute force), so that the two routes can be compared on one input; bit 22 wins when both are set, bit 24
  * (16777216) = a ragged batch forms one size class wherever the large-route and scale-path rules allow, however far
- * apart its sizes are, so that tests can pad n = 2 to n = 4000 in one device batch.
- * Bits 15 to 24 change host code only. */
+ * apart its sizes are, so that tests can pad n = 2 to n = 4000 in one device batch, bit 25 (33554432) = tzr_icp(_batch)
+ * searches every target by brute force, bit 26 (67108864) = through the hashed grid at any target size (a target the
+ * grid cannot index still falls back to brute force), so that the two routes can be compared on one input; bit 25 wins
+ * when both are set.
+ * Bits 15 to 26 change host code only. */
 int tzr_ctx_set_flags(tzr_ctx* ctx, uint32_t flags);
 int64_t tzr_ctx_filter_mismatches(tzr_ctx* ctx);
 /* Number of pairs of the most recent graph build that needed the exact FP64 re-check. */

@@ -101,6 +101,16 @@ if "--no-cert" not in sys.argv:  # solve then certify its retained results: the 
                         capi.default_params(noise_bound=sc[0]["noise_bound"], estimate_scaling=1, rotation_tim_graph=tim))
         rc = ctx.certify_last(noise_bound=2 * sc[0]["noise_bound"], max_iterations=3)
         print("certify_last tim", tim, [(r["status"], len(r["suboptimality_traj"])) for r in rc])
+# point-to-point ICP: both nearest-neighbour routes (brute force, and the grid with a far point forcing a fallback)
+ic_src = rng.uniform(0, 0.3, size=(300, 3)).astype(np.float32)
+ic_dst = (ic_src + rng.normal(scale=0.005, size=ic_src.shape)).astype(np.float32)
+ic_dst[0] = np.nan
+for iflags in (33554432, 67108864):
+    ctx.set_flags(iflags)
+    res, corr = ctx.icp_batch([ic_src, ic_src[:3]], [ic_dst, np.concatenate([ic_dst, [[1e9, 0, 0]]]).astype(np.float32)],
+                              0.05, max_iteration=3)
+    print("icp flags", iflags, [int(r) for r in res["n_correspondences"]], [int(r) for r in res["iterations"]])
+ctx.set_flags(0)
 sols, cl = capi.solve_batch_multi([p["src"] for p in prs[:5]], [p["dst"] for p in prs[:5]],
                                   capi.default_params(**dict(kw, noise_bound=prs[0]["noise_bound"])))
 print("multi", int(sols["valid"].sum()), "/ 5")

@@ -94,6 +94,34 @@ class FrontendParams(C.Structure):
                 ("tuple_scale", C.c_float)]
 
 
+class IcpParams(C.Structure):
+    """tzr_icp_params: Open3D's registration_icp distance and ICPConvergenceCriteria."""
+    _fields_ = [("max_correspondence_distance", C.c_double), ("relative_fitness", C.c_double),
+                ("relative_rmse", C.c_double), ("max_iteration", C.c_int32), ("reserved", C.c_int32)]
+
+
+class Similarity(C.Structure):
+    """tzr_similarity: scale, column-major rotation, translation."""
+    _fields_ = [("scale", C.c_double), ("rotation", C.c_double * 9), ("translation", C.c_double * 3)]
+
+
+class IcpResult(C.Structure):
+    """tzr_icp_result."""
+    _fields_ = [("transform", Similarity), ("fitness", C.c_double), ("inlier_rmse", C.c_double),
+                ("iterations", C.c_int32), ("n_correspondences", C.c_int32), ("converged", C.c_int32),
+                ("reserved", C.c_int32)]
+
+
+SIMILARITY_DTYPE = np.dtype([("scale", np.float64), ("rotation", np.float64, (9,)), ("translation", np.float64, (3,))],
+                            align=True)
+ICP_RESULT_DTYPE = np.dtype([
+    ("transform", SIMILARITY_DTYPE), ("fitness", np.float64), ("inlier_rmse", np.float64), ("iterations", np.int32),
+    ("n_correspondences", np.int32), ("converged", np.int32), ("reserved", np.int32)], align=True)
+assert C.sizeof(IcpParams) == 32, C.sizeof(IcpParams)
+assert SIMILARITY_DTYPE.itemsize == C.sizeof(Similarity) == 104, C.sizeof(Similarity)
+assert ICP_RESULT_DTYPE.itemsize == C.sizeof(IcpResult) == 136, (ICP_RESULT_DTYPE.itemsize, C.sizeof(IcpResult))
+
+
 _SYMBOLS = [
     "tzr_abi_version", "tzr_status_string", "tzr_last_error", "tzr_params_default", "tzr_ctx_create",
     "tzr_ctx_destroy", "tzr_ctx_set_stream", "tzr_ctx_synchronize", "tzr_ctx_kernel_launches", "tzr_words_per_row",
@@ -106,7 +134,8 @@ _SYMBOLS = [
     "tzr_match_correspondences_batch", "tzr_ctx_set_max_n", "tzr_ctx_clique_route", "tzr_certify_batch",
     "tzr_certifier_psd_projection", "tzr_certifier_batch_psd_projection", "tzr_certifier_batch_dual_projection",
     "tzr_fpfh_pair_features", "tzr_fpfh_smallest_eigenpair", "tzr_last_inliers", "tzr_certify_last_solve",
-    "tzr_frontend_params_default", "tzr_register_cloud_pairs",
+    "tzr_frontend_params_default", "tzr_register_cloud_pairs", "tzr_icp_params_default", "tzr_icp", "tzr_icp_batch",
+    "tzr_register_cloud_pairs_icp",
 ]
 
 # status codes (tzr_status)
@@ -117,6 +146,9 @@ TZR_ERR_TOO_LARGE = -6
 # debug flags of tzr_ctx_set_flags that choose tzr_compute_fpfh(_batch)'s radius search for every cloud
 FLAG_FPFH_BRUTE_FORCE = 4194304
 FLAG_FPFH_GRID = 8388608
+# ... and tzr_icp(_batch)'s nearest-neighbour search for every target
+FLAG_ICP_BRUTE_FORCE = 33554432
+FLAG_ICP_GRID = 67108864
 
 
 def build(verbose: bool = False):
@@ -211,6 +243,14 @@ def lib():
     L.tzr_register_cloud_pairs.argtypes = [vp, C.POINTER(FrontendParams), C.POINTER(Params), C.c_int, i32p, fpp,
                                            C.c_int, i32p, u64p, C.POINTER(Solution), i32p, i32p, i64p,
                                            C.POINTER(i32p), C.POINTER(i32p), fp]
+    L.tzr_icp_params_default.argtypes = [C.POINTER(IcpParams)]
+    L.tzr_icp_params_default.restype = None
+    L.tzr_icp.argtypes = [vp, C.POINTER(IcpParams), fp, C.c_int, fp, C.c_int, C.POINTER(Similarity),
+                          C.POINTER(IcpResult), i32p]
+    L.tzr_icp_batch.argtypes = [vp, C.POINTER(IcpParams), C.c_int, i32p, fpp, i32p, fpp, C.POINTER(Similarity),
+                                C.POINTER(IcpResult), C.POINTER(i32p)]
+    L.tzr_register_cloud_pairs_icp.argtypes = L.tzr_register_cloud_pairs.argtypes + [C.POINTER(IcpParams),
+                                                                                    C.POINTER(IcpResult)]
     for s in _SYMBOLS:
         getattr(L, s)  # raises AttributeError if the header and the library disagree
     _lib = L
@@ -225,6 +265,56 @@ def default_params(**kw) -> Params:
             raise AttributeError(k)
         setattr(p, k, v)
     return p
+
+
+def icp_params(max_correspondence_distance: float, **kw) -> IcpParams:
+    """tzr_icp_params_default with max_correspondence_distance and any field in kw set."""
+    p = IcpParams()
+    lib().tzr_icp_params_default(C.byref(p))
+    p.max_correspondence_distance = float(max_correspondence_distance)
+    for k, v in kw.items():
+        if not hasattr(p, k):
+            raise AttributeError(k)
+        setattr(p, k, v)
+    return p
+
+
+def similarity(init=None) -> Similarity:
+    """A tzr_similarity from None (identity), a (4,4) rigid matrix, a dict / record with scale, rotation (3x3 or
+    column-major 9) and translation, or a Similarity."""
+    if isinstance(init, Similarity):
+        return init
+    s = Similarity()
+    if init is None:
+        s.scale, R, t = 1.0, np.eye(3), np.zeros(3)
+    elif isinstance(init, np.ndarray) and init.shape == (4, 4):
+        s.scale, R, t = 1.0, init[:3, :3], init[:3, 3]
+    else:
+        R = np.asarray(init["rotation"], dtype=np.float64)
+        R = R.reshape(3, 3).T if R.shape == (9,) else R
+        s.scale, t = float(init["scale"]), np.asarray(init["translation"], dtype=np.float64)
+    s.rotation[:] = [float(x) for x in np.asarray(R, dtype=np.float64).T.reshape(-1)]
+    s.translation[:] = [float(x) for x in np.asarray(t, dtype=np.float64).reshape(3)]
+    return s
+
+
+def icp_result_dict(r) -> dict:
+    """An IcpResult (or an ICP_RESULT_DTYPE record) as a dict: scale, R (3x3), t, fitness, inlier_rmse, iterations,
+    n_correspondences, converged."""
+    if isinstance(r, IcpResult):
+        r = np.frombuffer(bytes(r), dtype=ICP_RESULT_DTYPE)[0]
+    tr = r["transform"]
+    return dict(scale=float(tr["scale"]), R=np.asarray(tr["rotation"]).reshape(3, 3).T.copy(),
+                t=np.asarray(tr["translation"]).copy(), fitness=float(r["fitness"]),
+                inlier_rmse=float(r["inlier_rmse"]), iterations=int(r["iterations"]),
+                n_correspondences=int(r["n_correspondences"]), converged=bool(r["converged"]))
+
+
+def _cloud32(a, what):
+    a = np.ascontiguousarray(a, dtype=np.float32)
+    if a.ndim != 2 or a.shape[1] != 3 or a.shape[0] == 0:
+        raise TzrError(f"{what}: clouds must be non-empty (n,3) arrays")
+    return a
 
 
 def _pts(a):
@@ -832,6 +922,23 @@ class Context:
         problem_index (P,) int32 (-1: not solved), correspondences (list of (m_p,2) int32), cliques (list of sorted
         row indices into the correspondences, empty when not solved), global scales (list of floats)).  The call
         raises only for errors of the whole call; TZR_ERR_TOO_LARGE of some pairs is reported in status."""
+        return self._register_pairs(clouds, pairs, params, normal_search_radius, fpfh_search_radius, use_absolute_scale,
+                                    use_crosscheck, use_tuple_test, tuple_scale, tuple_seeds, None)
+
+    def register_cloud_pairs_icp(self, clouds, pairs, params: Params, max_correspondence_distance, normal_search_radius=0.03,
+                                 fpfh_search_radius=0.05, use_absolute_scale=True, use_crosscheck=True,
+                                 use_tuple_test=True, tuple_scale=0.0, tuple_seeds=None, max_iteration=30,
+                                 relative_fitness=1e-6, relative_rmse=1e-6):
+        """tzr_register_cloud_pairs_icp: register_cloud_pairs, then ICP of every pair with a valid solution on its two
+        clouds, seeded with that solution, in the same call.  Returns register_cloud_pairs' six results plus the ICP
+        records (structured array (P,) of ICP_RESULT_DTYPE, zeroed for a pair that was not refined)."""
+        icp = icp_params(max_correspondence_distance, max_iteration=int(max_iteration),
+                         relative_fitness=float(relative_fitness), relative_rmse=float(relative_rmse))
+        return self._register_pairs(clouds, pairs, params, normal_search_radius, fpfh_search_radius, use_absolute_scale,
+                                    use_crosscheck, use_tuple_test, tuple_scale, tuple_seeds, icp)
+
+    def _register_pairs(self, clouds, pairs, params, normal_search_radius, fpfh_search_radius, use_absolute_scale,
+                        use_crosscheck, use_tuple_test, tuple_scale, tuple_seeds, icp):
         cl = [np.ascontiguousarray(c, dtype=np.float32) for c in clouds]
         if not cl or any(c.ndim != 2 or c.shape[1] != 3 or c.shape[0] == 0 for c in cl):
             raise TzrError("register_cloud_pairs: a non-empty list of non-empty (n,3) clouds is required")
@@ -857,18 +964,63 @@ class Context:
         cnt = np.zeros(P, dtype=np.int64)
         g = np.zeros(P, dtype=np.float32)
         fp, i32p = C.POINTER(C.c_float), C.POINTER(C.c_int32)
-        rc = lib().tzr_register_cloud_pairs(
-            self._h, C.byref(fpar), C.byref(params), len(cl), _p(n, C.c_int32),
-            (fp * len(cl))(*[_p(c, C.c_float) for c in cl]), P, _p(pc, C.c_int32), _p(seeds, C.c_uint64),
-            sols.ctypes.data_as(C.POINTER(Solution)), _p(status, C.c_int32), _p(index, C.c_int32),
-            _p(cnt, C.c_int64), (i32p * P)(*[_p(c, C.c_int32) for c in corr]),
-            (i32p * P)(*[_p(c, C.c_int32) for c in clq]), _p(g, C.c_float))
+        args = (self._h, C.byref(fpar), C.byref(params), len(cl), _p(n, C.c_int32),
+                (fp * len(cl))(*[_p(c, C.c_float) for c in cl]), P, _p(pc, C.c_int32), _p(seeds, C.c_uint64),
+                sols.ctypes.data_as(C.POINTER(Solution)), _p(status, C.c_int32), _p(index, C.c_int32),
+                _p(cnt, C.c_int64), (i32p * P)(*[_p(c, C.c_int32) for c in corr]),
+                (i32p * P)(*[_p(c, C.c_int32) for c in clq]), _p(g, C.c_float))
+        if icp is None:
+            rc = lib().tzr_register_cloud_pairs(*args)
+        else:
+            icp_res = np.zeros(P, dtype=ICP_RESULT_DTYPE)
+            rc = lib().tzr_register_cloud_pairs_icp(*args, C.byref(icp), icp_res.ctypes.data_as(C.POINTER(IcpResult)))
         if rc not in (0, TZR_ERR_TOO_LARGE):
             self._ck(rc)
         corr = [c[:k].copy() for c, k in zip(corr, cnt)]
         clq = [c[:max(0, int(s["clique_size"]))].copy() if i >= 0 else np.zeros(0, dtype=np.int32)
                for c, s, i in zip(clq, sols, index)]
-        return sols, status, index, corr, clq, [float(x) for x in g]
+        out = (sols, status, index, corr, clq, [float(x) for x in g])
+        return out if icp is None else out + (icp_res,)
+
+    def icp(self, src, dst, max_correspondence_distance, init=None, max_iteration=30, relative_fitness=1e-6,
+            relative_rmse=1e-6):
+        """tzr_icp: point-to-point ICP of the (ns,3) source onto the (nd,3) target (float32), seeded with init (see
+        similarity(); None = identity; its scale stays fixed).  Returns (result dict as icp_result_dict, final
+        correspondences (m,2) int32 rows (source index, target index) ascending by source)."""
+        res, corr = self.icp_batch([src], [dst], max_correspondence_distance, None if init is None else [init],
+                                   max_iteration=max_iteration, relative_fitness=relative_fitness,
+                                   relative_rmse=relative_rmse, single=True)
+        return icp_result_dict(res[0]), corr[0]
+
+    def icp_batch(self, srcs, dsts, max_correspondence_distance, inits=None, max_iteration=30, relative_fitness=1e-6,
+                  relative_rmse=1e-6, single=False):
+        """tzr_icp_batch over B (source, target) cloud pairs; inits: B seeds (None = identity for all).  Returns
+        (results structured array (B,) of ICP_RESULT_DTYPE, list of B correspondence arrays).  single=True goes through
+        tzr_icp (B must be 1)."""
+        S = [_cloud32(a, "icp") for a in srcs]
+        D = [_cloud32(a, "icp") for a in dsts]
+        B = len(S)
+        if B == 0 or len(D) != B or (inits is not None and len(inits) != B):
+            raise TzrError("icp_batch: one target and one seed per source cloud are required")
+        p = icp_params(max_correspondence_distance, max_iteration=int(max_iteration),
+                       relative_fitness=float(relative_fitness), relative_rmse=float(relative_rmse))
+        init = (Similarity * B)(*[similarity(None if inits is None else x) for x in inits or [None] * B])
+        res = (IcpResult * B)()
+        corr = [np.zeros((a.shape[0], 2), dtype=np.int32) for a in S]
+        fp, i32p = C.POINTER(C.c_float), C.POINTER(C.c_int32)
+        if single:
+            assert B == 1
+            rc = lib().tzr_icp(self._h, C.byref(p), _p(S[0], C.c_float), S[0].shape[0], _p(D[0], C.c_float),
+                               D[0].shape[0], init, res, _p(corr[0], C.c_int32))
+        else:
+            ns = np.array([a.shape[0] for a in S], dtype=np.int32)
+            nd = np.array([a.shape[0] for a in D], dtype=np.int32)
+            rc = lib().tzr_icp_batch(self._h, C.byref(p), B, _p(ns, C.c_int32), (fp * B)(*[_p(a, C.c_float) for a in S]),
+                                     _p(nd, C.c_int32), (fp * B)(*[_p(a, C.c_float) for a in D]), init, res,
+                                     (i32p * B)(*[_p(c, C.c_int32) for c in corr]))
+        self._ck(rc)
+        out = np.frombuffer(bytes(res), dtype=ICP_RESULT_DTYPE).copy()
+        return out, [c[:int(r["n_correspondences"])].copy() for c, r in zip(corr, out)]
 
     def last_graph(self, b: int, n: int):
         W = lib().tzr_words_per_row(n)

@@ -36,6 +36,8 @@ struct tzr_ctx {
   DevBuf lg, cq;
   // ragged batches (DESIGN.md §4.2): the size-class tables, and the flat inputs / outputs of host-pointer calls
   DevBuf rg;
+  // tzr_icp(_batch): its own workspace, so that refinement leaves a retained solve intact
+  DevBuf icp;
   int max_n = kMaxN;  // per-problem size limit of this context (tzr_ctx_set_max_n: kMaxN ... kMaxNLarge)
   // pinned host staging
   void* h_pin = nullptr;
@@ -1205,7 +1207,7 @@ int tzr_ctx_destroy(tzr_ctx* ctx) {
                     &ctx->hclq, &ctx->hsize, &ctx->clq, &ctx->L, &ctx->alive, &ctx->best_bits, &ctx->alive_cnt, &ctx->root_ctr,
                     &ctx->lock, &ctx->flg, &ctx->kfinal, &ctx->tstart, &ctx->stack, &ctx->cv, &ctx->centry, &ctx->ps, &ctx->pd, &ctx->wgt,
                     &ctx->res, &ctx->skey, &ctx->sidx, &ctx->sorted, &ctx->rmask, &ctx->tmask, &ctx->sol, &ctx->dbg,
-                    &ctx->misc, &ctx->sc, &ctx->m_in, &ctx->m_scratch, &ctx->m_out, &ctx->cert, &ctx->certb, &ctx->lg, &ctx->cq, &ctx->rg};
+                    &ctx->misc, &ctx->sc, &ctx->m_in, &ctx->m_scratch, &ctx->m_out, &ctx->cert, &ctx->certb, &ctx->lg, &ctx->cq, &ctx->rg, &ctx->icp};
   for (DevBuf* b : bufs)
     if (b->p) cudaFree(b->p);
   if (ctx->h_pin) cudaFreeHost(ctx->h_pin);
@@ -2026,17 +2028,39 @@ void tzr_frontend_params_default(tzr_frontend_params* p) {
   p->tuple_scale = 0.f;
 }
 
+static bool icp_params_ok(const tzr_icp_params* p) {
+  return p && p->max_correspondence_distance > 0 && std::isfinite(p->max_correspondence_distance) &&
+         p->max_iteration >= 0 && !std::isnan(p->relative_fitness) && !std::isnan(p->relative_rmse);
+}
+
+static void icp_result_of(const IcpProb& pr, tzr_icp_result* out) {
+  memset(out, 0, sizeof(*out));
+  if (!pr.seeded) return;
+  out->transform.scale = pr.s;
+  for (int k = 0; k < 9; ++k) out->transform.rotation[k] = pr.R[k];
+  for (int k = 0; k < 3; ++k) out->transform.translation[k] = pr.t[k];
+  out->fitness = pr.fitness;
+  out->inlier_rmse = pr.rmse;
+  out->iterations = pr.iterations;
+  out->n_correspondences = pr.count;
+  out->converged = pr.converged;
+}
+
 // FPFH over the clouds, matching over the pairs, the ragged solve over the pairs that can be solved (DESIGN.md §3.10).
 // Workspace: m_in holds the clouds and every table, m_scratch the FPFH scratch and then the matcher's, m_out the stages'
 // outputs (descriptors alive while matching runs) and the solve's inputs and outputs.  All of it is sized before any work.
-int tzr_register_cloud_pairs(tzr_ctx* ctx, const tzr_frontend_params* fp, const tzr_params* params, int n_clouds,
-                             const int32_t* n, const float* const* pts, int P, const int32_t* pair_clouds,
-                             const uint64_t* tuple_seeds, tzr_solution* solutions, int32_t* status,
-                             int32_t* problem_index, int64_t* n_corr, int32_t* const* corr, int32_t* const* cliques,
-                             float* global_scale) {
+// icp (may be NULL): after the solve, ICP of every solved pair on its two clouds (already in m_in), seeded on the device
+// from its record (ctx->icp holds the ICP workspace); icp_results (P entries) then receives the refinements, zeroed for a
+// pair that was not refined.  Without icp the launches, synchronisations and outputs are tzr_register_cloud_pairs'.
+static int register_pairs_run(tzr_ctx* ctx, const tzr_frontend_params* fp, const tzr_params* params, int n_clouds,
+                              const int32_t* n, const float* const* pts, int P, const int32_t* pair_clouds,
+                              const uint64_t* tuple_seeds, tzr_solution* solutions, int32_t* status,
+                              int32_t* problem_index, int64_t* n_corr, int32_t* const* corr, int32_t* const* cliques,
+                              float* global_scale, const tzr_icp_params* icp, tzr_icp_result* icp_results) {
   if (!ctx || !fp || !params || n_clouds < 1 || !n || !pts || P < 1 || !pair_clouds || !solutions || !status ||
       !n_corr || !(fp->normal_search_radius > 0) || !(fp->fpfh_search_radius > 0))
     return TZR_ERR_INVALID_ARG;
+  if (icp && (!icp_params_ok(icp) || !icp_results)) return TZR_ERR_INVALID_ARG;
   for (int c = 0; c < n_clouds; ++c)
     if (n[c] <= 0 || !pts[c]) return TZR_ERR_INVALID_ARG;
   std::vector<int32_t> ns(P), nd(P);
@@ -2080,7 +2104,32 @@ int tzr_register_cloud_pairs(tzr_ctx* ctx, const tzr_frontend_params* fp, const 
   // pinned: staged inputs | read-back head | gather table | records | index pairs | cliques
   const size_t h_head = al256(o_g), h_g = h_head + al256(head), h_sol = h_g + al256((size_t)P * sizeof(PairGather)),
                h_corr = h_sol + al256((size_t)P * sizeof(tzr_solution)), h_clq = h_corr + al256(C * 8),
-               pin_bytes = h_clq + C * 4;
+               pin_base = h_clq + C * 4;
+  // with ICP: [ICP problem table | target cloud table | chunk table] staged in and the problem table read back
+  std::vector<FpfhCloud> iclouds;
+  IcpPlan iplan;
+  long long i_ns = 0, i_chunks = 0;
+  if (icp) {
+    for (int p = 0; p < P; ++p) {
+      i_ns += n[pair_clouds[2 * p]];
+      i_chunks += (n[pair_clouds[2 * p]] + kIcpChunk - 1) / kIcpChunk;
+    }
+    iclouds.resize((size_t)n_clouds);
+    const int iroute = (ctx->flags & 33554432u) ? kFpfhRouteBrute : (ctx->flags & 67108864u) ? kFpfhRouteGrid : kFpfhRouteAuto;
+    const double r = icp->max_correspondence_distance;
+    if (i_ns > 0x7fffffffll ||
+        fpfh_plan(n_clouds, n, r, r, iroute, iclouds.data(), &iplan.grid, kIcpGridMinN) != TZR_OK) {
+      ctx->last_error = "the refinement's points or target grid do not fit 32-bit indices";
+      return TZR_ERR_TOO_LARGE;
+    }
+    iplan.max_iteration = icp->max_iteration;
+    iplan.r2 = r * r;
+    iplan.relative_fitness = icp->relative_fitness;
+    iplan.relative_rmse = icp->relative_rmse;
+  }
+  const size_t hi_prob = al256(pin_base), hi_cl = hi_prob + al256((size_t)P * sizeof(IcpProb)),
+               hi_ck = hi_cl + al256((size_t)n_clouds * sizeof(FpfhCloud)), hi_end = hi_ck + (size_t)i_chunks * 4,
+               pin_bytes = icp ? hi_end : pin_base;
   int rc;
   if ((rc = ensure(ctx, ctx->m_in, in_bytes)) != TZR_OK) return rc;
   if ((rc = ensure(ctx, ctx->m_scratch, scratch_bytes)) != TZR_OK) return rc;
@@ -2191,6 +2240,47 @@ int tzr_register_cloud_pairs(tzr_ctx* ctx, const tzr_frontend_params* fp, const 
     ctx->ragged_last.clear();
     ++ctx->generation;
   }
+  // the refinement of the solved pairs, seeded on the device from their records (no synchronisation, no upload of points)
+  IcpProb* hi_probs = (IcpProb*)(h + hi_prob);
+  if (icp && S > 0) {
+    int c_lo = 0, m_lo = 0;
+    for (int k = 0; k < S; ++k) {
+      const int a = pair_clouds[2 * solved[k]], b = pair_clouds[2 * solved[k] + 1];
+      IcpProb& pr = hi_probs[k];
+      pr = IcpProb{};
+      pr.s_lo = clouds[a].lo;
+      pr.ns = n[a];
+      pr.d_lo = clouds[b].lo;
+      pr.nd = n[b];
+      pr.c_lo = c_lo;
+      pr.m_lo = m_lo;
+      pr.tc = b;
+      const int nc = (n[a] + kIcpChunk - 1) / kIcpChunk;
+      for (int c = 0; c < nc; ++c) ((int*)(h + hi_ck))[c_lo + c] = k;
+      c_lo += nc;
+      m_lo += n[a];
+    }
+    iplan.B = S;
+    iplan.NS = m_lo;
+    iplan.ND = (int)N;
+    iplan.chunks = c_lo;
+    memcpy(h + hi_cl, iclouds.data(), (size_t)n_clouds * sizeof(FpfhCloud));
+    const size_t pb = (size_t)S * sizeof(IcpProb), cb = (size_t)n_clouds * sizeof(FpfhCloud), kb = (size_t)c_lo * 4;
+    const size_t o_prob = 0, o_cl = al256(pb), o_ck = o_cl + al256(cb), o_match = o_ck + al256(kb),
+                 o_part = o_match + al256((size_t)m_lo * 4), o_grid = o_part + al256((size_t)c_lo * 9 * 8),
+                 total = o_grid + iplan.grid.grid_bytes;
+    if ((rc = ensure(ctx, ctx->icp, total)) != TZR_OK) return rc;
+    char* di = (char*)ctx->icp.p;
+    CK(cudaMemcpyAsync(di + o_prob, hi_probs, pb, cudaMemcpyHostToDevice, st));
+    CK(cudaMemcpyAsync(di + o_cl, h + hi_cl, cb, cudaMemcpyHostToDevice, st));
+    CK(cudaMemcpyAsync(di + o_ck, h + hi_ck, kb, cudaMemcpyHostToDevice, st));
+    ctx->launches += launch_icp_seed((IcpProb*)(di + o_prob), S, d_sol, st);
+    ctx->launches += launch_icp(iplan, d_pts, d_pts, (IcpProb*)(di + o_prob), (FpfhCloud*)(di + o_cl),
+                                (const int*)(di + o_ck), (int*)(di + o_match), (double*)(di + o_part),
+                                iplan.grid.grid_bytes ? di + o_grid : nullptr, st);
+    if ((rc = check_launch(ctx, "icp launch")) != TZR_OK) return rc;
+    CK(cudaMemcpyAsync(hi_probs, di + o_prob, pb, cudaMemcpyDeviceToHost, st));
+  }
   // synchronisation 2: the records, and the index pairs and cliques that were asked for
   if (S > 0) CK(cudaMemcpyAsync(h + h_sol, d_sol, (size_t)S * sizeof(tzr_solution), cudaMemcpyDeviceToHost, st));
   if (corr_rows > 0) CK(cudaMemcpyAsync(h + h_corr, d_corr, (size_t)corr_rows * 8, cudaMemcpyDeviceToHost, st));
@@ -2211,6 +2301,10 @@ int tzr_register_cloud_pairs(tzr_ctx* ctx, const tzr_frontend_params* fp, const 
     row += solved_n[k];
   }
   parallel_copy(spans);
+  if (icp) {
+    for (int p = 0; p < P; ++p) memset(&icp_results[p], 0, sizeof(tzr_icp_result));
+    for (int k = 0; k < S; ++k) icp_result_of(hi_probs[k], &icp_results[solved[k]]);
+  }
   if (no_room) {
     ctx->last_error = "COMPLETE TIM graph of this clique does not fit the rotation workspace";
     return TZR_ERR_TOO_LARGE;
@@ -2221,6 +2315,159 @@ int tzr_register_cloud_pairs(tzr_ctx* ctx, const tzr_frontend_params* fp, const 
     return TZR_ERR_TOO_LARGE;
   }
   return TZR_OK;
+}
+
+int tzr_register_cloud_pairs(tzr_ctx* ctx, const tzr_frontend_params* fp, const tzr_params* params, int n_clouds,
+                             const int32_t* n, const float* const* pts, int P, const int32_t* pair_clouds,
+                             const uint64_t* tuple_seeds, tzr_solution* solutions, int32_t* status,
+                             int32_t* problem_index, int64_t* n_corr, int32_t* const* corr, int32_t* const* cliques,
+                             float* global_scale) {
+  return register_pairs_run(ctx, fp, params, n_clouds, n, pts, P, pair_clouds, tuple_seeds, solutions, status,
+                            problem_index, n_corr, corr, cliques, global_scale, nullptr, nullptr);
+}
+
+int tzr_register_cloud_pairs_icp(tzr_ctx* ctx, const tzr_frontend_params* fp, const tzr_params* params, int n_clouds,
+                                 const int32_t* n, const float* const* pts, int P, const int32_t* pair_clouds,
+                                 const uint64_t* tuple_seeds, tzr_solution* solutions, int32_t* status,
+                                 int32_t* problem_index, int64_t* n_corr, int32_t* const* corr,
+                                 int32_t* const* cliques, float* global_scale, const tzr_icp_params* icp,
+                                 tzr_icp_result* icp_results) {
+  if (!icp) return TZR_ERR_INVALID_ARG;
+  return register_pairs_run(ctx, fp, params, n_clouds, n, pts, P, pair_clouds, tuple_seeds, solutions, status,
+                            problem_index, n_corr, corr, cliques, global_scale, icp, icp_results);
+}
+
+void tzr_icp_params_default(tzr_icp_params* p) {
+  if (!p) return;
+  memset(p, 0, sizeof(*p));
+  p->max_correspondence_distance = 0;  // no default (Open3D takes it as an argument)
+  p->relative_fitness = 1e-6;
+  p->relative_rmse = 1e-6;
+  p->max_iteration = 30;
+}
+
+// tzr_icp(_batch): sources and targets staged back to back, one H2D copy, every iteration enqueued (launch_icp), one
+// D2H copy of the problem table (and of the per-point matches when correspondences are asked for).
+int tzr_icp_batch(tzr_ctx* ctx, const tzr_icp_params* params, int B, const int32_t* ns, const float* const* src,
+                  const int32_t* nd, const float* const* dst, const tzr_similarity* init, tzr_icp_result* results,
+                  int32_t* const* corr) {
+  if (!ctx || !icp_params_ok(params) || B < 1 || !ns || !src || !nd || !dst || !init || !results)
+    return TZR_ERR_INVALID_ARG;
+  const double r = params->max_correspondence_distance;
+  long long NS = 0, ND = 0, chunks = 0;
+  bool want_corr = false;
+  for (int b = 0; b < B; ++b) {
+    if (ns[b] < 1 || nd[b] < 1 || !src[b] || !dst[b]) return TZR_ERR_INVALID_ARG;
+    const tzr_similarity& s = init[b];
+    bool finite = std::isfinite(s.scale) && s.scale > 0;
+    for (int k = 0; k < 9; ++k) finite &= std::isfinite(s.rotation[k]) != 0;
+    for (int k = 0; k < 3; ++k) finite &= std::isfinite(s.translation[k]) != 0;
+    if (!finite) return TZR_ERR_INVALID_ARG;
+    NS += ns[b];
+    ND += nd[b];
+    chunks += (ns[b] + kIcpChunk - 1) / kIcpChunk;
+    want_corr |= corr && corr[b];
+  }
+  if (NS > 0x7fffffffll || ND > 0x7fffffffll) {
+    ctx->last_error = "the batch's points do not fit 32-bit indices";
+    return TZR_ERR_TOO_LARGE;
+  }
+  IcpPlan plan;
+  plan.B = B;
+  plan.NS = (int)NS;
+  plan.ND = (int)ND;
+  plan.chunks = (int)chunks;
+  plan.max_iteration = params->max_iteration;
+  plan.r2 = r * r;
+  plan.relative_fitness = params->relative_fitness;
+  plan.relative_rmse = params->relative_rmse;
+  std::vector<FpfhCloud> clouds((size_t)B);
+  const int route = (ctx->flags & 33554432u) ? kFpfhRouteBrute : (ctx->flags & 67108864u) ? kFpfhRouteGrid : kFpfhRouteAuto;
+  if (fpfh_plan(B, nd, r, r, route, clouds.data(), &plan.grid, kIcpGridMinN) != TZR_OK) {
+    ctx->last_error = "the batch's target grid does not fit 32-bit indices";
+    return TZR_ERR_TOO_LARGE;
+  }
+  std::vector<IcpProb> probs((size_t)B);
+  std::vector<int> chunk_prob((size_t)chunks);
+  {
+    int s_lo = 0, c_lo = 0;
+    for (int b = 0; b < B; ++b) {
+      IcpProb& pr = probs[b];
+      pr = IcpProb{};
+      pr.s_lo = s_lo;
+      pr.ns = ns[b];
+      pr.d_lo = clouds[b].lo;
+      pr.nd = nd[b];
+      pr.c_lo = c_lo;
+      pr.m_lo = s_lo;
+      pr.tc = b;
+      pr.active = pr.seeded = 1;
+      pr.s = init[b].scale;
+      for (int k = 0; k < 9; ++k) pr.R[k] = init[b].rotation[k];
+      for (int k = 0; k < 3; ++k) pr.t[k] = init[b].translation[k];
+      const int nc = (ns[b] + kIcpChunk - 1) / kIcpChunk;
+      for (int c = 0; c < nc; ++c) chunk_prob[c_lo + c] = b;
+      s_lo += ns[b];
+      c_lo += nc;
+    }
+  }
+  cudaSetDevice(ctx->device);
+  cudaStream_t st = ctx->stream;
+  const size_t sb = (size_t)NS * 12, db = (size_t)ND * 12, pb = (size_t)B * sizeof(IcpProb),
+               cb = (size_t)B * sizeof(FpfhCloud), kb = (size_t)chunks * 4, mb = (size_t)NS * 4,
+               hb = (size_t)chunks * 9 * 8;
+  const size_t o_dst = al256(sb), o_prob = o_dst + al256(db), o_cl = o_prob + al256(pb), o_ck = o_cl + al256(cb),
+               in_bytes = o_ck + kb, o_match = al256(in_bytes), o_part = o_match + al256(mb),
+               o_grid = o_part + al256(hb), total = o_grid + plan.grid.grid_bytes;
+  int rc;
+  if ((rc = ensure(ctx, ctx->icp, total)) != TZR_OK) return rc;
+  std::vector<char> h(in_bytes);
+  for (int b = 0; b < B; ++b) {
+    memcpy(h.data() + (size_t)probs[b].s_lo * 12, src[b], (size_t)ns[b] * 12);
+    memcpy(h.data() + o_dst + (size_t)probs[b].d_lo * 12, dst[b], (size_t)nd[b] * 12);
+  }
+  memcpy(h.data() + o_prob, probs.data(), pb);
+  memcpy(h.data() + o_cl, clouds.data(), cb);
+  memcpy(h.data() + o_ck, chunk_prob.data(), kb);
+  char* d = (char*)ctx->icp.p;
+  CK(cudaMemcpyAsync(d, h.data(), in_bytes, cudaMemcpyHostToDevice, st));
+  ctx->launches += launch_icp(plan, (const float*)d, (const float*)(d + o_dst), (IcpProb*)(d + o_prob),
+                              (FpfhCloud*)(d + o_cl), (const int*)(d + o_ck), (int*)(d + o_match),
+                              (double*)(d + o_part), plan.grid.grid_bytes ? d + o_grid : nullptr, st);
+  if ((rc = check_launch(ctx, "icp launch")) != TZR_OK) return rc;
+  CK(cudaMemcpyAsync(probs.data(), d + o_prob, pb, cudaMemcpyDeviceToHost, st));
+  std::vector<int32_t> match(want_corr ? (size_t)NS : 0);
+  if (want_corr) CK(cudaMemcpyAsync(match.data(), d + o_match, mb, cudaMemcpyDeviceToHost, st));
+  CK(cudaStreamSynchronize(st));
+  for (int b = 0; b < B; ++b) {
+    const IcpProb& pr = probs[b];
+    icp_result_of(pr, &results[b]);
+    if (corr && corr[b]) {
+      int32_t* rows = corr[b];
+      long long k = 0;
+      for (int i = 0; i < pr.ns; ++i) {
+        const int j = match[(size_t)pr.m_lo + i];
+        if (j < 0) continue;
+        rows[2 * k] = i;
+        rows[2 * k + 1] = j;
+        ++k;
+      }
+    }
+  }
+  return TZR_OK;
+}
+
+int tzr_icp(tzr_ctx* ctx, const tzr_icp_params* params, const float* src, int ns, const float* dst, int nd,
+            const tzr_similarity* init, tzr_icp_result* result, int32_t* corr) {
+  tzr_similarity id;
+  if (!init) {
+    memset(&id, 0, sizeof(id));
+    id.scale = 1.0;
+    id.rotation[0] = id.rotation[4] = id.rotation[8] = 1.0;
+    init = &id;
+  }
+  int32_t* const corrs[1] = {corr};
+  return tzr_icp_batch(ctx, params, 1, &ns, &src, &nd, &dst, init, result, corr ? corrs : nullptr);
 }
 
 int tzr_fpfh_pair_features(tzr_ctx* ctx, int n, const float* p1, const float* n1, const float* p2, const float* n2,

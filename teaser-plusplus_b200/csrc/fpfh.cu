@@ -254,22 +254,6 @@ struct Grid {           // the radius search of one cloud; n_sorted == 0 means b
   double inv_h;         // 1 / cell edge
 };
 
-__device__ __forceinline__ unsigned int cell_hash(long long ix, long long iy, long long iz, unsigned int mask) {
-  return ((unsigned int)(ix * 73856093ll) ^ (unsigned int)(iy * 19349663ll) ^ (unsigned int)(iz * 83492791ll)) & mask;
-}
-
-// Largest cell index the grid uses.  The index is u = fl(fl(x - o) * fl(1/h)) with x and the origin o floats (exact in
-// double): the subtraction and the product each round by at most 2^-53 relative, and fl(1/h) and h = r (1 + 1e-5)
-// carry two more such roundings, so |u - (x - o)/h| <= |u| 2^-51 (to first order).  Two points that pass the float
-// test d^2 < r^2 are at most r (1 + 2^-20) apart per axis (the test's own rounding is a few 2^-24 relative), so their
-// exact indices differ by at most (1 + 2^-20) / (1 + 1e-5) < 1 - 9e-6.  Their floors then differ by at most 1, which
-// is what the 3x3x3 search needs, while the two index errors sum to less than 9e-6.  With |u| < 2^32 each error is at
-// most 2^-19 < 1.91e-6, well inside that margin.  The bound grows with the extent and passes half the margin (4.5e-6)
-// near 1e10 cells, about 2^33 (one far point at 1e11 with r = 0.01 is 2^43 cells: true neighbours land two cells
-// apart), so a cloud
-// with a finite point outside the range is searched by brute force.
-constexpr double kCellIndexMax = 4294967296.0;  // 2^32
-
 __device__ __forceinline__ bool cell_of(const Grid& g, float x, float y, float z, long long* ix, long long* iy,
                                         long long* iz) {
   if (!(x == x) || !(y == y) || !(z == z)) return false;
@@ -282,13 +266,6 @@ __device__ __forceinline__ bool cell_of(const Grid& g, float x, float y, float z
   *iz = (long long)fz;
   return true;
 }
-
-// bounding-box minimum over finite coordinates (ordered-int encoding of floats)
-__device__ __forceinline__ int f2ord(float f) {
-  const int i = __float_as_int(f);
-  return i >= 0 ? i : i ^ 0x7fffffff;
-}
-__device__ __forceinline__ float ord2f(int i) { return __int_as_float(i >= 0 ? i : i ^ 0x7fffffff); }
 
 // The search of cloud c: the grid when the cloud has one and every finite point of it found a cell, else brute force.
 __device__ __forceinline__ Grid grid_of(const FpfhCloud& cl, const int* sorted, const int* bstart, const int* bend) {
@@ -652,7 +629,8 @@ int key_bits(unsigned int buckets) {  // keys go up to `buckets` (the sentinel)
 }  // namespace
 
 int fpfh_plan(int B, const int32_t* n, double normal_radius, double fpfh_radius, int route, FpfhCloud* clouds,
-              FpfhPlan* plan) {
+              FpfhPlan* plan, int grid_min_n) {
+  if (grid_min_n < 0) grid_min_n = kGridMinN;
   const double h = std::max(normal_radius, fpfh_radius) * (1.0 + 1e-5);
   long long lo = 0, buckets = 0;
   bool any_grid = false;
@@ -661,7 +639,7 @@ int fpfh_plan(int B, const int32_t* n, double normal_radius, double fpfh_radius,
     cl = FpfhCloud{};
     cl.lo = (int)lo;
     cl.n = n[c];
-    cl.grid = route == kFpfhRouteBrute ? 0 : route == kFpfhRouteGrid ? 1 : n[c] >= kGridMinN;
+    cl.grid = route == kFpfhRouteBrute ? 0 : route == kFpfhRouteGrid ? 1 : n[c] >= grid_min_n;
     cl.mins[0] = cl.mins[1] = cl.mins[2] = 0x7fffffff;
     cl.mins[3] = 0;
     cl.inv_h = 1.0 / h;
@@ -686,6 +664,30 @@ int fpfh_plan(int B, const int32_t* n, double normal_radius, double fpfh_radius,
   return TZR_OK;
 }
 
+int launch_fpfh_grid(const FpfhPlan& plan, const float* pts, FpfhCloud* clouds, void* grid_scratch, cudaStream_t st,
+                     const int** sorted, const int** bstart_out, const int** bend_out) {
+  const int N = plan.N, B = plan.B;
+  const unsigned int T = plan.buckets;
+  char* w = (char*)grid_scratch;
+  unsigned int* keys = (unsigned int*)w;  w += (size_t)N * 4;
+  unsigned int* keys2 = (unsigned int*)w; w += (size_t)N * 4;
+  int* idx = (int*)w;                     w += (size_t)N * 4;
+  int* idx2 = (int*)w;                    w += (size_t)N * 4;
+  int* bstart = (int*)w;                  w += (size_t)T * 4;
+  int* bend = (int*)w;                    w += (size_t)T * 4;
+  const int bits = key_bits(T);
+  size_t cub_bytes = radix_bytes(N, bits);
+  cudaMemsetAsync(bstart, 0, 2 * (size_t)T * 4, st);
+  bbox_min_kernel<<<(N + 255) / 256, 256, 0, st>>>(pts, N, clouds, B);
+  bucket_kernel<<<(N + 255) / 256, 256, 0, st>>>(pts, N, clouds, B, T, keys, idx);
+  cub::DeviceRadixSort::SortPairs((void*)w, cub_bytes, keys, keys2, idx, idx2, N, 0, bits, st);
+  bucket_bounds_kernel<<<(N + 255) / 256, 256, 0, st>>>(keys2, N, T, bstart, bend);
+  *sorted = idx2;
+  *bstart_out = bstart;
+  *bend_out = bend;
+  return 4;
+}
+
 int launch_fpfh(const FpfhPlan& plan, const float* pts, FpfhCloud* clouds, double normal_radius, double fpfh_radius,
                 float4* normals, float* spfh, float* out, int* overflow, void* grid_scratch, cudaStream_t st) {
   const float r2n = (float)(normal_radius * normal_radius);
@@ -694,27 +696,7 @@ int launch_fpfh(const FpfhPlan& plan, const float* pts, FpfhCloud* clouds, doubl
   int nl = 0;
   cudaMemsetAsync(overflow, 0, (size_t)B * sizeof(int), st);
   Clouds cs{pts, clouds, B, nullptr, nullptr, nullptr};
-  if (plan.any_grid) {
-    const unsigned int T = plan.buckets;
-    char* w = (char*)grid_scratch;
-    unsigned int* keys = (unsigned int*)w;  w += (size_t)N * 4;
-    unsigned int* keys2 = (unsigned int*)w; w += (size_t)N * 4;
-    int* idx = (int*)w;                     w += (size_t)N * 4;
-    int* idx2 = (int*)w;                    w += (size_t)N * 4;
-    int* bstart = (int*)w;                  w += (size_t)T * 4;
-    int* bend = (int*)w;                    w += (size_t)T * 4;
-    const int bits = key_bits(T);
-    size_t cub_bytes = radix_bytes(N, bits);
-    cudaMemsetAsync(bstart, 0, 2 * (size_t)T * 4, st);
-    bbox_min_kernel<<<(N + 255) / 256, 256, 0, st>>>(pts, N, clouds, B);
-    bucket_kernel<<<(N + 255) / 256, 256, 0, st>>>(pts, N, clouds, B, T, keys, idx);
-    cub::DeviceRadixSort::SortPairs((void*)w, cub_bytes, keys, keys2, idx, idx2, N, 0, bits, st);
-    bucket_bounds_kernel<<<(N + 255) / 256, 256, 0, st>>>(keys2, N, T, bstart, bend);
-    nl += 4;
-    cs.sorted = idx2;
-    cs.bstart = bstart;
-    cs.bend = bend;
-  }
+  if (plan.any_grid) nl += launch_fpfh_grid(plan, pts, clouds, grid_scratch, st, &cs.sorted, &cs.bstart, &cs.bend);
   normals_kernel<<<N, kFpfhThreads, 0, st>>>(cs, r2n, normals, overflow);
   spfh_kernel<<<N, kFpfhThreads, 0, st>>>(cs, normals, r2f, spfh, overflow);
   fpfh_kernel<<<N, kFpfhThreads, 0, st>>>(cs, spfh, r2f, out, overflow);

@@ -1,0 +1,304 @@
+// Point-to-point ICP (the refinement step of the reference's FPFH + TEASER++ + ICP tutorial, DESIGN.md §3.11): Open3D's
+// RegistrationICP with TransformationEstimationPointToPoint and ICPConvergenceCriteria, written out as this project's
+// own definition in include/teaser_b200.h, for B problems at once.
+//
+//   icp_nn_kernel      one CTA per chunk of kIcpChunk source points: p = s (R x) + t in float64 (icp_transform), the
+//                      nearest target with d^2 < r^2 (lowest index among equal d^2), by brute force through shared
+//                      memory or through the target's hashed grid; writes the match per point and the chunk's sums
+//                      (count, sum p, sum q, sum d^2).
+//   icp_eval_kernel    one warp per problem: combines the chunk sums in a fixed order, evaluates fitness and rmse,
+//                      applies the convergence test and clears the active flag.
+//   icp_cov_kernel     one CTA per chunk: the centred cross-covariance sum (p - mu_p)(q - mu_q)^T of its matches.
+//   icp_update_kernel  one warp per problem: combines it, runs rotation_from_H (the rotation stage's SVD and reflection
+//                      fix), and composes the update into (R, t).
+//
+// Every reduction runs in an order fixed by the problem's own points (chunk k of a problem always holds its points
+// [256 k, 256 k + 256), and the chunks of a problem are combined by lane k mod 32 then a butterfly), so a problem's
+// bits do not depend on the batch it runs in.  Finished problems return at once from every kernel.  The iterations are
+// enqueued back to back without a host synchronisation; the launch count depends on max_iteration only.
+#include "rot3.cuh"
+#include "tzr_internal.cuh"
+
+namespace tzr {
+
+namespace {
+
+constexpr int kIcpThreads = kIcpChunk;
+
+// p = s * (R x) + t, each row (R(r,0) x + R(r,1) y) + R(r,2) z, with -fmad=false: tests/icp_reference.py reproduces it
+// bit for bit
+__device__ __forceinline__ void icp_transform(const IcpProb& pr, const float* __restrict__ src, int i, double p[3]) {
+  const double x = src[3 * (size_t)i], y = src[3 * (size_t)i + 1], z = src[3 * (size_t)i + 2];
+#pragma unroll
+  for (int r = 0; r < 3; ++r) {
+    const double rx = (pr.R[r] * x + pr.R[3 + r] * y) + pr.R[6 + r] * z;
+    p[r] = pr.s * rx + pr.t[r];
+  }
+}
+
+__device__ __forceinline__ double icp_d2(const double p[3], double qx, double qy, double qz) {
+  const double dx = p[0] - qx, dy = p[1] - qy, dz = p[2] - qz;
+  return (dx * dx + dy * dy) + dz * dz;
+}
+
+// keep the lexicographically smallest (d2, j); *best starts at r^2 with *bj = INT_MAX (no match), and d2 = r^2 is no
+// match (the bound is strict)
+__device__ __forceinline__ void icp_keep(double d2, int j, double* best, int* bj) {
+  if (d2 < *best || (d2 == *best && j < *bj && *bj != 0x7fffffff)) {
+    *best = d2;
+    *bj = j;
+  }
+}
+
+// Fixed-order sum over a CTA of kIcpThreads threads: butterfly inside each warp (every lane ends with the same bits),
+// then the warp sums in warp order by one thread.  Result in s_out[0..K).
+template <int K>
+__device__ void icp_block_sum(double (&v)[K], double* s_buf /* (kIcpThreads/32) * K */, double* s_out) {
+  const int w = threadIdx.x >> 5, lane = threadIdx.x & 31;
+#pragma unroll
+  for (int k = 0; k < K; ++k)
+    for (int o = 16; o; o >>= 1) v[k] += __shfl_xor_sync(0xffffffffu, v[k], o);
+  if (lane == 0)
+#pragma unroll
+    for (int k = 0; k < K; ++k) s_buf[w * K + k] = v[k];
+  __syncthreads();
+  if (threadIdx.x < K) {
+    double s = 0.0;
+    for (int q = 0; q < kIcpThreads / 32; ++q) s += s_buf[q * K + threadIdx.x];
+    s_out[threadIdx.x] = s;
+  }
+}
+
+// Fixed-order sum of the problem's nc chunk partials (K of the 9 doubles each) over one warp: lane l takes chunks l,
+// l + 32, ..., then a butterfly; every lane returns the same bits.
+template <int K>
+__device__ void icp_warp_combine(const double* __restrict__ partial, int c_lo, int nc, double (&v)[K]) {
+  const int lane = threadIdx.x & 31;
+#pragma unroll
+  for (int k = 0; k < K; ++k) v[k] = 0.0;
+  for (int c = lane; c < nc; c += 32)
+#pragma unroll
+    for (int k = 0; k < K; ++k) v[k] += partial[9 * (size_t)(c_lo + c) + k];
+#pragma unroll
+  for (int k = 0; k < K; ++k)
+    for (int o = 16; o; o >>= 1) v[k] += __shfl_xor_sync(0xffffffffu, v[k], o);
+}
+
+struct IcpArgs {
+  const float* src;
+  const float* dst;
+  IcpProb* probs;
+  const FpfhCloud* clouds;
+  const int* chunk_prob;
+  int* match;
+  double* partial;
+  const int* sorted;    // the target grid (nullptr without grid targets)
+  const int* bstart;
+  const int* bend;
+  double r2;
+};
+
+// Nearest target of p over all targets of the problem, read from global memory (a grid problem's query that the grid
+// cannot index)
+__device__ void icp_nn_scan(const float* __restrict__ dst, int d_lo, int nd, const double p[3], double* best,
+                            int* bj) {
+  for (int j = 0; j < nd; ++j) {
+    const size_t o = 3 * (size_t)(d_lo + j);
+    icp_keep(icp_d2(p, dst[o], dst[o + 1], dst[o + 2]), j, best, bj);
+  }
+}
+
+__global__ void __launch_bounds__(kIcpThreads) icp_nn_kernel(IcpArgs a) {
+  __shared__ double s_t[3][kIcpThreads];
+  __shared__ double s_buf[(kIcpThreads / 32) * 8];
+  const int c = blockIdx.x;
+  const int b = a.chunk_prob[c];
+  const IcpProb& pr = a.probs[b];
+  if (!pr.active) return;
+  const int i = (c - pr.c_lo) * kIcpChunk + threadIdx.x;  // source point inside the problem
+  const bool have = i < pr.ns;
+  double p[3] = {0.0, 0.0, 0.0};
+  bool query = false;
+  if (have) {
+    icp_transform(pr, a.src, pr.s_lo + i, p);
+    query = isfinite(p[0]) && isfinite(p[1]) && isfinite(p[2]);
+  }
+  double best = a.r2;  // strict d^2 < r^2: a candidate must be smaller than r^2 itself
+  int bj = 0x7fffffff;
+  const FpfhCloud& cl = a.clouds[pr.tc];
+  if (!cl.grid || cl.mins[3]) {
+    // brute force, the problem's targets tiled through shared memory
+    for (int t0 = 0; t0 < pr.nd; t0 += kIcpThreads) {
+      const int m = min(kIcpThreads, pr.nd - t0);
+      __syncthreads();
+      if (threadIdx.x < m) {
+        const size_t o = 3 * (size_t)(pr.d_lo + t0 + threadIdx.x);
+        s_t[0][threadIdx.x] = a.dst[o];
+        s_t[1][threadIdx.x] = a.dst[o + 1];
+        s_t[2][threadIdx.x] = a.dst[o + 2];
+      }
+      __syncthreads();
+      if (query)
+        for (int k = 0; k < m; ++k) {
+          const double d2 = icp_d2(p, s_t[0][k], s_t[1][k], s_t[2][k]);
+          if (d2 < best) {  // ascending j: the first of equal d^2 stays
+            best = d2;
+            bj = t0 + k;
+          }
+        }
+    }
+  } else if (query) {
+    // the cell of the float64 query in the target's grid (DESIGN.md §3.11); out of the accurate range: brute force
+    const double fx = floor((p[0] - (double)ord2f(cl.mins[0])) * cl.inv_h);
+    const double fy = floor((p[1] - (double)ord2f(cl.mins[1])) * cl.inv_h);
+    const double fz = floor((p[2] - (double)ord2f(cl.mins[2])) * cl.inv_h);
+    if (fabs(fx) < kCellIndexMax && fabs(fy) < kCellIndexMax && fabs(fz) < kCellIndexMax) {
+      const long long ix = (long long)fx, iy = (long long)fy, iz = (long long)fz;
+      for (int t = 0; t < 27; ++t) {
+        const unsigned int h = cl.base + cell_hash(ix + (t % 3) - 1, iy + ((t / 3) % 3) - 1, iz + (t / 9) - 1, cl.mask);
+        const int e = a.bend[h];
+        for (int k = a.bstart[h]; k < e; ++k) {
+          const int j = a.sorted[k];
+          const size_t o = 3 * (size_t)j;
+          icp_keep(icp_d2(p, a.dst[o], a.dst[o + 1], a.dst[o + 2]), j - pr.d_lo, &best, &bj);
+        }
+      }
+    } else {
+      icp_nn_scan(a.dst, pr.d_lo, pr.nd, p, &best, &bj);
+    }
+  }
+  const bool hit = query && bj != 0x7fffffff;
+  if (have) a.match[pr.m_lo + i] = hit ? bj : -1;
+  double v[8] = {0, 0, 0, 0, 0, 0, 0, 0};
+  if (hit) {
+    const size_t o = 3 * (size_t)(pr.d_lo + bj);
+    v[0] = 1.0;
+    v[1] = p[0];
+    v[2] = p[1];
+    v[3] = p[2];
+    v[4] = a.dst[o];
+    v[5] = a.dst[o + 1];
+    v[6] = a.dst[o + 2];
+    v[7] = best;
+  }
+  icp_block_sum<8>(v, s_buf, a.partial + 9 * (size_t)c);
+}
+
+__global__ void icp_eval_kernel(IcpArgs a, int max_iteration, double relative_fitness, double relative_rmse) {
+  IcpProb& pr = a.probs[blockIdx.x];
+  if (!pr.active) return;
+  const int nc = (pr.ns + kIcpChunk - 1) / kIcpChunk;
+  double v[8];
+  icp_warp_combine<8>(a.partial, pr.c_lo, nc, v);
+  if (threadIdx.x != 0) return;
+  const int count = (int)v[0];
+  const double fitness = count ? (double)count / (double)pr.ns : 0.0;
+  const double rmse = count ? sqrt(v[7] / (double)count) : 0.0;
+  if (pr.iterations > 0 && fabs(pr.fitness - fitness) < relative_fitness && fabs(pr.rmse - rmse) < relative_rmse)
+    pr.converged = 1;
+  if (pr.converged || pr.iterations >= max_iteration) pr.active = 0;
+  pr.count = count;
+  pr.fitness = fitness;
+  pr.rmse = rmse;
+  const double inv = count ? 1.0 / (double)count : 0.0;
+  for (int k = 0; k < 3; ++k) {
+    pr.mup[k] = v[1 + k] * inv;
+    pr.muq[k] = v[4 + k] * inv;
+  }
+}
+
+__global__ void __launch_bounds__(kIcpThreads) icp_cov_kernel(IcpArgs a) {
+  __shared__ double s_buf[(kIcpThreads / 32) * 9];
+  const int c = blockIdx.x;
+  const int b = a.chunk_prob[c];
+  const IcpProb& pr = a.probs[b];
+  if (!pr.active || pr.count < 3) return;  // the update of fewer than 3 correspondences reads no covariance
+  const int i = (c - pr.c_lo) * kIcpChunk + threadIdx.x;
+  double h[9] = {0, 0, 0, 0, 0, 0, 0, 0, 0};
+  const int j = i < pr.ns ? a.match[pr.m_lo + i] : -1;
+  if (j >= 0) {
+    double p[3];
+    icp_transform(pr, a.src, pr.s_lo + i, p);
+    const size_t o = 3 * (size_t)(pr.d_lo + j);
+    const double u[3] = {p[0] - pr.mup[0], p[1] - pr.mup[1], p[2] - pr.mup[2]};
+    const double w[3] = {(double)a.dst[o] - pr.muq[0], (double)a.dst[o + 1] - pr.muq[1],
+                         (double)a.dst[o + 2] - pr.muq[2]};
+#pragma unroll
+    for (int cc = 0; cc < 3; ++cc)
+#pragma unroll
+      for (int r = 0; r < 3; ++r) h[3 * cc + r] = u[r] * w[cc];  // H(r, c) column-major
+  }
+  icp_block_sum<9>(h, s_buf, a.partial + 9 * (size_t)c);
+}
+
+__global__ void icp_update_kernel(IcpArgs a) {
+  IcpProb& pr = a.probs[blockIdx.x];
+  if (!pr.active) return;
+  const int nc = (pr.ns + kIcpChunk - 1) / kIcpChunk;
+  double h[9];
+  if (pr.count >= 3) icp_warp_combine<9>(a.partial, pr.c_lo, nc, h);
+  if (threadIdx.x != 0) return;
+  M3 Ru;
+  m3_identity(Ru);
+  double tu[3] = {0.0, 0.0, 0.0};
+  if (pr.count >= 3) {
+    M3 H;
+    for (int k = 0; k < 9; ++k) H.a[k] = h[k];
+    rotation_from_H(H, Ru);
+    for (int r = 0; r < 3; ++r) tu[r] = pr.muq[r] - ((Ru(r, 0) * pr.mup[0] + Ru(r, 1) * pr.mup[1]) + Ru(r, 2) * pr.mup[2]);
+  } else if (pr.count > 0) {
+    for (int r = 0; r < 3; ++r) tu[r] = pr.muq[r] - pr.mup[r];
+  }
+  // R <- Ru R, t <- Ru t + tu
+  double R[9], t[3];
+  for (int r = 0; r < 3; ++r) {
+    for (int cc = 0; cc < 3; ++cc)
+      R[3 * cc + r] = (Ru(r, 0) * pr.R[3 * cc] + Ru(r, 1) * pr.R[3 * cc + 1]) + Ru(r, 2) * pr.R[3 * cc + 2];
+    t[r] = ((Ru(r, 0) * pr.t[0] + Ru(r, 1) * pr.t[1]) + Ru(r, 2) * pr.t[2]) + tu[r];
+  }
+  for (int k = 0; k < 9; ++k) pr.R[k] = R[k];
+  for (int k = 0; k < 3; ++k) pr.t[k] = t[k];
+  pr.iterations += 1;
+}
+
+__global__ void icp_seed_kernel(IcpProb* probs, int B, const tzr_solution* __restrict__ sol) {
+  const int b = blockIdx.x * blockDim.x + threadIdx.x;
+  if (b >= B) return;
+  const tzr_solution& s = sol[b];
+  IcpProb& pr = probs[b];
+  bool ok = s.valid && isfinite(s.scale) && s.scale > 0.0;
+  for (int k = 0; k < 9; ++k) ok &= isfinite(s.rotation[k]) != 0;
+  for (int k = 0; k < 3; ++k) ok &= isfinite(s.translation[k]) != 0;
+  pr.active = pr.seeded = ok ? 1 : 0;
+  if (!ok) return;
+  pr.s = s.scale;
+  for (int k = 0; k < 9; ++k) pr.R[k] = s.rotation[k];
+  for (int k = 0; k < 3; ++k) pr.t[k] = s.translation[k];
+}
+
+}  // namespace
+
+int launch_icp_seed(IcpProb* probs, int B, const tzr_solution* sol, cudaStream_t st) {
+  icp_seed_kernel<<<(B + 127) / 128, 128, 0, st>>>(probs, B, sol);
+  return 1;
+}
+
+int launch_icp(const IcpPlan& plan, const float* src, const float* dst, IcpProb* probs, FpfhCloud* clouds,
+               const int* chunk_prob, int* match, double* partial, void* grid_scratch, cudaStream_t st) {
+  int nl = 0;
+  IcpArgs a{src, dst, probs, clouds, chunk_prob, match, partial, nullptr, nullptr, nullptr, plan.r2};
+  if (plan.grid.any_grid) nl += launch_fpfh_grid(plan.grid, dst, clouds, grid_scratch, st, &a.sorted, &a.bstart, &a.bend);
+  icp_nn_kernel<<<plan.chunks, kIcpThreads, 0, st>>>(a);
+  icp_eval_kernel<<<plan.B, 32, 0, st>>>(a, plan.max_iteration, plan.relative_fitness, plan.relative_rmse);
+  nl += 2;
+  for (int it = 0; it < plan.max_iteration; ++it) {
+    icp_cov_kernel<<<plan.chunks, kIcpThreads, 0, st>>>(a);
+    icp_update_kernel<<<plan.B, 32, 0, st>>>(a);
+    icp_nn_kernel<<<plan.chunks, kIcpThreads, 0, st>>>(a);
+    icp_eval_kernel<<<plan.B, 32, 0, st>>>(a, plan.max_iteration, plan.relative_fitness, plan.relative_rmse);
+    nl += 4;
+  }
+  return nl;
+}
+
+}  // namespace tzr

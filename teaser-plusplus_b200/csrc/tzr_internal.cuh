@@ -272,6 +272,31 @@ struct FpfhCloud {     // one per cloud, filled by fpfh_plan, read by the kernel
                        // a finite point lies outside the grid's accurate index range, the cloud uses brute force
   double inv_h;        // 1 / cell edge
 };
+
+// The hashed uniform grid of the radius searches (fpfh.cu) and of ICP's nearest-neighbour search (icp.cu)
+__device__ __forceinline__ unsigned int cell_hash(long long ix, long long iy, long long iz, unsigned int mask) {
+  return ((unsigned int)(ix * 73856093ll) ^ (unsigned int)(iy * 19349663ll) ^ (unsigned int)(iz * 83492791ll)) & mask;
+}
+
+// Largest cell index the grid uses.  The index is u = fl(fl(x - o) * fl(1/h)) with x and the origin o floats (exact in
+// double): the subtraction and the product each round by at most 2^-53 relative, and fl(1/h) and h = r (1 + 1e-5)
+// carry two more such roundings, so |u - (x - o)/h| <= |u| 2^-51 (to first order).  Two points that pass the float
+// test d^2 < r^2 are at most r (1 + 2^-20) apart per axis (the test's own rounding is a few 2^-24 relative), so their
+// exact indices differ by at most (1 + 2^-20) / (1 + 1e-5) < 1 - 9e-6.  Their floors then differ by at most 1, which
+// is what the 3x3x3 search needs, while the two index errors sum to less than 9e-6.  With |u| < 2^32 each error is at
+// most 2^-19 < 1.91e-6, well inside that margin.  The bound grows with the extent and passes half the margin (4.5e-6)
+// near 1e10 cells, about 2^33 (one far point at 1e11 with r = 0.01 is 2^43 cells: true neighbours land two cells
+// apart), so a cloud
+// with a finite point outside the range is searched by brute force.
+constexpr double kCellIndexMax = 4294967296.0;  // 2^32
+
+// bounding-box minimum over finite coordinates (ordered-int encoding of floats)
+__device__ __forceinline__ int f2ord(float f) {
+  const int i = __float_as_int(f);
+  return i >= 0 ? i : i ^ 0x7fffffff;
+}
+__device__ __forceinline__ float ord2f(int i) { return __int_as_float(i >= 0 ? i : i ^ 0x7fffffff); }
+
 struct FpfhPlan {
   int B = 0, N = 0;            // clouds, points in all of them
   bool any_grid = false;
@@ -282,9 +307,15 @@ struct FpfhPlan {
 // 4194304 (brute force) and 8388608 (the grid at any size).
 constexpr int kFpfhRouteAuto = 0, kFpfhRouteBrute = 1, kFpfhRouteGrid = 2;
 // Fills clouds[0..B) (host copy, to be staged to the device before launch_fpfh) and the plan.  TZR_ERR_TOO_LARGE when
-// the points or buckets of the batch do not fit 32-bit indices.
+// the points or buckets of the batch do not fit 32-bit indices.  grid_min_n: the size from which kFpfhRouteAuto uses
+// the grid (-1: the descriptor stage's own, 4096).
 int fpfh_plan(int B, const int32_t* n, double normal_radius, double fpfh_radius, int route, FpfhCloud* clouds,
-              FpfhPlan* plan);
+              FpfhPlan* plan, int grid_min_n = -1);
+// The grid build alone (bounding boxes, bucket keys, CUB radix sort, bucket bounds) over plan.any_grid clouds: *sorted
+// receives the flat point indices ordered by bucket, *bstart / *bend the bucket ranges (inside grid_scratch).  Returns
+// the launches.  launch_fpfh runs it first; icp.cu reuses it on the target clouds.
+int launch_fpfh_grid(const FpfhPlan& plan, const float* pts, FpfhCloud* clouds, void* grid_scratch, cudaStream_t st,
+                     const int** sorted, const int** bstart, const int** bend);
 // pts (plan.N x 3), clouds (device copy of fpfh_plan's table), normals (N float4), spfh (N x 33), out (N x 33),
 // overflow (B ints, zeroed here), grid_scratch (plan.grid_bytes): device pointers.  Returns the launches.
 int launch_fpfh(const FpfhPlan& plan, const float* pts, FpfhCloud* clouds, double normal_radius, double fpfh_radius,
@@ -386,6 +417,41 @@ int launch_pair_rows(const MatchPlan& plan, const MatchPair* pairs, const int2* 
 // src / dst (float64 rows of pts).  Returns the launches.
 int launch_corr_gather(const PairGather* table, int n_entries, int max_count, const int32_t* pairs, const float* pts,
                        int2* corr, double* src, double* dst, cudaStream_t st);
+
+// icp.cu (point-to-point ICP, DESIGN.md §3.11): B problems, sources back to back and targets back to back
+constexpr int kIcpChunk = 256;    // source points per chunk: the unit of the fixed-order reductions (one CTA each)
+constexpr int kIcpGridMinN = 1024;  // targets from which the nearest-neighbour search goes through the hashed grid
+struct IcpProb {        // one per problem, device-resident; the host fills the inputs, the kernels the rest
+  int s_lo, ns;         // sources: flat points [s_lo, s_lo + ns)
+  int d_lo, nd;         // targets: flat points [d_lo, d_lo + nd) (also FpfhCloud b of the target table)
+  int c_lo;             // first chunk of the problem (chunks are consecutive)
+  int active;           // 0: finished (converged or max_iteration reached); every kernel skips the problem
+  int iterations, converged;
+  int count;            // correspondences of the current transform
+  int m_lo;             // first entry of the problem in the per-point match array
+  int tc;               // its target's entry in the FpfhCloud table of the targets (lo = d_lo)
+  int seeded;           // 1: the problem runs (tzr_register_cloud_pairs_icp: 0 for a pair without a valid solution)
+  int pad;
+  double s;             // fixed scale
+  double R[9], t[3];    // current transform (column-major R)
+  double fitness, rmse; // evaluation of the current transform
+  double mup[3], muq[3];  // means of the current correspondences (source side transformed)
+};
+struct IcpPlan {
+  int B = 0, NS = 0, ND = 0, chunks = 0;
+  int max_iteration = 0;
+  double r2 = 0, relative_fitness = 0, relative_rmse = 0;
+  FpfhPlan grid;        // the target grid (fpfh_plan with both radii = r)
+};
+// src (NS x 3 floats), dst (ND x 3 floats), probs (B), clouds (B, fpfh_plan's table of the targets), chunk_prob
+// (chunks: the problem of every chunk), match (target index or -1 per source point from m_lo, final correspondences),
+// partial (chunks x 9 doubles), grid_scratch (plan.grid.grid_bytes): device pointers.  Enqueues every iteration without
+// synchronising; returns the launches: 4 for the grid build (when some target uses it) + 2 + 4 * max_iteration.
+int launch_icp(const IcpPlan& plan, const float* src, const float* dst, IcpProb* probs, FpfhCloud* clouds,
+               const int* chunk_prob, int* match, double* partial, void* grid_scratch, cudaStream_t st);
+// The seeds of B problems from B solution records (tzr_register_cloud_pairs_icp): a valid record with a finite transform
+// and a positive scale sets (s, R, t) and active = seeded = 1, any other leaves the problem inactive.  One launch.
+int launch_icp_seed(IcpProb* probs, int B, const tzr_solution* sol, cudaStream_t st);
 
 
 }  // namespace tzr

@@ -47,6 +47,24 @@ struct RegistrationSolution {
   EIGEN_MAKE_ALIGNED_OPERATOR_NEW
 };
 
+// Point-to-point ICP (teaser/icp.h, tzr_icp): the parameters and the result of PointToPointICP, declared here so that
+// solveCloudPairs can refine its pairs.  Open3D's registration_icp distance and ICPConvergenceCriteria.
+struct PointToPointICPParams {
+  double max_correspondence_distance = 0;  // no default, as in Open3D: must be set (> 0)
+  int max_iteration = 30;
+  double relative_fitness = 1e-6;
+  double relative_rmse = 1e-6;
+};
+struct PointToPointICPResult {
+  RegistrationSolution solution;  // the refined transform; scale is the seed's, held fixed
+  double fitness = 0;
+  double inlier_rmse = 0;
+  int iterations = 0;
+  bool converged = false;
+  std::vector<std::pair<int, int>> correspondences;  // final (source index, target index), ascending by source
+  EIGEN_MAKE_ALIGNED_OPERATOR_NEW
+};
+
 using Mat3X = Eigen::Matrix<double, 3, Eigen::Dynamic>;
 using BoolRow = Eigen::Matrix<bool, 1, Eigen::Dynamic>;
 using Map2X = Eigen::Matrix<int, 2, Eigen::Dynamic>;
@@ -306,6 +324,16 @@ class RobustRegistrationSolver {
   std::vector<CloudPairResult> solveCloudPairs(const std::vector<PointCloud>& clouds,
                                                const std::vector<std::pair<int, int>>& pairs,
                                                const CloudPairParams& params);
+  // solveCloudPairs, then point-to-point ICP of every pair whose solution is valid, on its two clouds, seeded with that
+  // solution, in the same device call (tzr_register_cloud_pairs_icp).  refined = false (and icp zeroed) for a pair
+  // that was not refined.  The pair results are those of the overload above.
+  struct CloudPairICPResult : CloudPairResult {
+    bool refined = false;
+    PointToPointICPResult icp;
+  };
+  std::vector<CloudPairICPResult> solveCloudPairs(const std::vector<PointCloud>& clouds,
+                                                  const std::vector<std::pair<int, int>>& pairs,
+                                                  const CloudPairParams& params, const PointToPointICPParams& icp);
   bool isMaxCliqueProvenOptimal() const { return clique_proven_; }
   long long getNumInlierGraphEdges() const { return n_edges_; }
   int getGNCRotationIterations() const { return gnc_iterations_; }

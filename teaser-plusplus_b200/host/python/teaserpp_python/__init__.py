@@ -12,7 +12,8 @@ from . import _teaserpp as _ext
 
 # ---- re-exports -----------------------------------------------------------------------------------------------------
 _PUBLIC = ("OMP_MAX_THREADS", "CertificationResult", "DRSCertifier", "EigSolverType", "InlierGraphFormulation",
-           "InlierSelectionMode", "RegistrationSolution", "RobustRegistrationSolver", "RotationEstimationAlgorithm")
+           "InlierSelectionMode", "PointToPointICP", "RegistrationSolution", "RobustRegistrationSolver",
+           "RotationEstimationAlgorithm")
 globals().update({name: getattr(_ext, name) for name in _PUBLIC})
 
 # ---- v1.0 spellings of the enums, kept as class attributes ----------------------------------------------------------

@@ -11,6 +11,7 @@
 #include <sstream>
 
 #include "teaser/certification.h"
+#include "teaser/icp.h"
 #include "teaser/registration.h"
 
 namespace py = pybind11;
@@ -50,12 +51,35 @@ py::array_t<int> irow_to_numpy(const Eigen::Matrix<int, 1, Eigen::Dynamic>& m) {
   return out;
 }
 
+using CloudArray = py::array_t<float, py::array::c_style | py::array::forcecast>;
+
+teaser::PointCloud cloud_of(const CloudArray& a) {
+  if (a.ndim() != 2 || a.shape(1) != 3) throw std::invalid_argument("clouds must be (n,3) arrays");
+  teaser::PointCloud pc;
+  const float* d = a.data();
+  pc.reserve(static_cast<size_t>(a.shape(0)));
+  for (py::ssize_t i = 0; i < a.shape(0); ++i) pc.push_back({d[3 * i], d[3 * i + 1], d[3 * i + 2]});
+  return pc;
+}
+
+py::dict icp_dict(const teaser::PointToPointICPResult& r) {
+  return py::dict(py::arg("solution") = r.solution, py::arg("fitness") = r.fitness,
+                  py::arg("inlier_rmse") = r.inlier_rmse, py::arg("iterations") = r.iterations,
+                  py::arg("converged") = r.converged, py::arg("correspondences") = r.correspondences);
+}
+
 }  // namespace
 
 PYBIND11_MODULE(_teaserpp, m) {
   m.doc() = "Python binding for TEASER++ (GPU-native solve() path)";
 
   py::class_<teaser::RegistrationSolution>(m, "RegistrationSolution")
+      .def(py::init([]() {  // identity (seeds for PointToPointICP.refine)
+        teaser::RegistrationSolution s;
+        s.rotation.setIdentity();
+        s.translation.setZero();
+        return s;
+      }))
       .def_readwrite("valid", &teaser::RegistrationSolution::valid)
       .def_readwrite("scale", &teaser::RegistrationSolution::scale)
       .def_property(
@@ -75,6 +99,48 @@ PYBIND11_MODULE(_teaserpp, m) {
         os << ">";
         return os.str();
       });
+
+  // GPU extra: the refinement step of the reference's FPFH + TEASER++ + ICP tutorial (teaser::PointToPointICP)
+  py::class_<teaser::PointToPointICP>(m, "PointToPointICP")
+      .def(py::init([](double max_correspondence_distance, int max_iteration, double relative_fitness,
+                       double relative_rmse) {
+             teaser::PointToPointICP::Params p;
+             p.max_correspondence_distance = max_correspondence_distance;
+             p.max_iteration = max_iteration;
+             p.relative_fitness = relative_fitness;
+             p.relative_rmse = relative_rmse;
+             return teaser::PointToPointICP(p);
+           }),
+           py::arg("max_correspondence_distance"), py::arg("max_iteration") = 30, py::arg("relative_fitness") = 1e-6,
+           py::arg("relative_rmse") = 1e-6)
+      .def("refine",
+           [](const teaser::PointToPointICP& icp, const CloudArray& src, const CloudArray& dst,
+              const teaser::RegistrationSolution& init) {
+             const teaser::PointCloud s = cloud_of(src), d = cloud_of(dst);
+             teaser::PointToPointICP::Result r;
+             {
+               py::gil_scoped_release release;
+               r = icp.refine(s, d, init);
+             }
+             return icp_dict(r);
+           },
+           py::arg("src"), py::arg("dst"), py::arg("init"))
+      .def("refine_batch",
+           [](const teaser::PointToPointICP& icp, const std::vector<CloudArray>& src, const std::vector<CloudArray>& dst,
+              const std::vector<teaser::RegistrationSolution>& init) {
+             std::vector<teaser::PointCloud> s, d;
+             for (const auto& a : src) s.push_back(cloud_of(a));
+             for (const auto& a : dst) d.push_back(cloud_of(a));
+             std::vector<teaser::PointToPointICP::Result> res;
+             {
+               py::gil_scoped_release release;
+               res = icp.refineBatch(s, d, init);
+             }
+             py::list out;
+             for (const auto& r : res) out.append(icp_dict(r));
+             return out;
+           },
+           py::arg("src"), py::arg("dst"), py::arg("init"));
 
   m.attr("OMP_MAX_THREADS") = 0;  // the GPU path ignores max_clique_num_threads
 
@@ -183,6 +249,44 @@ PYBIND11_MODULE(_teaserpp, m) {
              return out;
            },
            py::arg("clouds"), py::arg("pairs"), py::arg("normal_search_radius") = 0.03,
+           py::arg("fpfh_search_radius") = 0.05, py::arg("use_absolute_scale") = true, py::arg("use_crosscheck") = true,
+           py::arg("use_tuple_test") = true, py::arg("tuple_scale") = 0.0f, py::arg("tuple_seed") = 0x7ea5e2ull)
+      .def("solve_cloud_pairs_icp",
+           [](Solver& s, const std::vector<CloudArray>& clouds, const std::vector<std::pair<int, int>>& pairs,
+              double max_correspondence_distance, int max_iteration, double relative_fitness, double relative_rmse,
+              double normal_search_radius, double fpfh_search_radius, bool use_absolute_scale, bool use_crosscheck,
+              bool use_tuple_test, float tuple_scale, uint64_t tuple_seed) {
+             // GPU extra: solve_cloud_pairs, then point-to-point ICP of every pair with a valid solution, in one call
+             std::vector<teaser::PointCloud> pcs;
+             for (const auto& a : clouds) pcs.push_back(cloud_of(a));
+             Solver::CloudPairParams cp;
+             cp.normal_search_radius = normal_search_radius;
+             cp.fpfh_search_radius = fpfh_search_radius;
+             cp.use_absolute_scale = use_absolute_scale;
+             cp.use_crosscheck = use_crosscheck;
+             cp.use_tuple_test = use_tuple_test;
+             cp.tuple_scale = tuple_scale;
+             cp.tuple_seed = tuple_seed;
+             teaser::PointToPointICP::Params ip;
+             ip.max_correspondence_distance = max_correspondence_distance;
+             ip.max_iteration = max_iteration;
+             ip.relative_fitness = relative_fitness;
+             ip.relative_rmse = relative_rmse;
+             std::vector<Solver::CloudPairICPResult> res;
+             {
+               py::gil_scoped_release release;
+               res = s.solveCloudPairs(pcs, pairs, cp, ip);
+             }
+             py::list out;
+             for (const auto& r : res)
+               out.append(py::dict(py::arg("status") = r.status, py::arg("correspondences") = r.correspondences,
+                                   py::arg("solution") = r.solution, py::arg("max_clique") = r.max_clique,
+                                   py::arg("global_scale") = r.global_scale, py::arg("refined") = r.refined,
+                                   py::arg("icp") = r.refined ? py::object(icp_dict(r.icp)) : py::object(py::none())));
+             return out;
+           },
+           py::arg("clouds"), py::arg("pairs"), py::arg("max_correspondence_distance"), py::arg("max_iteration") = 30,
+           py::arg("relative_fitness") = 1e-6, py::arg("relative_rmse") = 1e-6, py::arg("normal_search_radius") = 0.03,
            py::arg("fpfh_search_radius") = 0.05, py::arg("use_absolute_scale") = true, py::arg("use_crosscheck") = true,
            py::arg("use_tuple_test") = true, py::arg("tuple_scale") = 0.0f, py::arg("tuple_seed") = 0x7ea5e2ull)
       .def_property_readonly("solution", &Solver::getSolution)

@@ -1,0 +1,91 @@
+// teaser::PointToPointICP (teaser/icp.h) on top of the C-ABI: marshalling only, the loop runs in libteaser_b200.so.
+#include "teaser/icp.h"
+
+#include <cstring>
+#include <stdexcept>
+#include <string>
+
+#include "teaser_b200.h"
+
+namespace teaser {
+
+tzr_ctx* b200_context();  // registration.cc: one context per host thread
+
+namespace {
+
+tzr_icp_params to_c(const PointToPointICPParams& p) {
+  tzr_icp_params c;
+  tzr_icp_params_default(&c);
+  c.max_correspondence_distance = p.max_correspondence_distance;
+  c.max_iteration = p.max_iteration;
+  c.relative_fitness = p.relative_fitness;
+  c.relative_rmse = p.relative_rmse;
+  return c;
+}
+
+tzr_similarity to_c(const RegistrationSolution& s) {
+  tzr_similarity c;
+  c.scale = s.scale;
+  std::memcpy(c.rotation, s.rotation.data(), sizeof(c.rotation));
+  for (int k = 0; k < 3; ++k) c.translation[k] = s.translation(k);
+  return c;
+}
+
+}  // namespace
+
+// shared with registration.cc's solveCloudPairs overload
+void icp_result_from_c(const tzr_icp_result& r, const int32_t* corr, PointToPointICPResult* out) {
+  out->solution.valid = true;
+  out->solution.scale = r.transform.scale;
+  std::memcpy(out->solution.rotation.data(), r.transform.rotation, sizeof(r.transform.rotation));
+  for (int k = 0; k < 3; ++k) out->solution.translation(k) = r.transform.translation[k];
+  out->fitness = r.fitness;
+  out->inlier_rmse = r.inlier_rmse;
+  out->iterations = r.iterations;
+  out->converged = r.converged != 0;
+  out->correspondences.clear();
+  if (corr)
+    for (int c = 0; c < r.n_correspondences; ++c) out->correspondences.emplace_back(corr[2 * c], corr[2 * c + 1]);
+}
+
+PointToPointICP::Result PointToPointICP::refine(const PointCloud& src, const PointCloud& dst,
+                                                const RegistrationSolution& init) const {
+  return refineBatch({src}, {dst}, {init})[0];
+}
+
+std::vector<PointToPointICP::Result> PointToPointICP::refineBatch(const std::vector<PointCloud>& src,
+                                                                  const std::vector<PointCloud>& dst,
+                                                                  const std::vector<RegistrationSolution>& init) const {
+  const size_t B = src.size();
+  if (dst.size() != B || init.size() != B) throw std::invalid_argument("PointToPointICP: one target and seed per source");
+  std::vector<Result> out(B);
+  if (B == 0) return out;
+  static_assert(sizeof(PointXYZ) == 3 * sizeof(float), "PointXYZ must be three packed floats");
+  std::vector<int32_t> ns(B), nd(B);
+  std::vector<const float*> sp(B), dp(B);
+  std::vector<tzr_similarity> seeds(B);
+  std::vector<std::vector<int32_t>> corr(B);
+  std::vector<int32_t*> corr_p(B);
+  for (size_t b = 0; b < B; ++b) {
+    if (src[b].empty() || dst[b].empty()) throw std::invalid_argument("PointToPointICP: clouds must be non-empty");
+    ns[b] = static_cast<int32_t>(src[b].size());
+    nd[b] = static_cast<int32_t>(dst[b].size());
+    sp[b] = &src[b][0].x;
+    dp[b] = &dst[b][0].x;
+    seeds[b] = to_c(init[b]);
+    corr[b].resize(2 * src[b].size());
+    corr_p[b] = corr[b].data();
+  }
+  const tzr_icp_params p = to_c(params_);
+  std::vector<tzr_icp_result> res(B);
+  tzr_ctx* ctx = b200_context();
+  const int rc = B == 1 ? tzr_icp(ctx, &p, sp[0], ns[0], dp[0], nd[0], seeds.data(), res.data(), corr_p[0])
+                        : tzr_icp_batch(ctx, &p, static_cast<int>(B), ns.data(), sp.data(), nd.data(), dp.data(),
+                                        seeds.data(), res.data(), corr_p.data());
+  if (rc != TZR_OK)
+    throw std::runtime_error(std::string("PointToPointICP: ") + tzr_status_string(rc) + " (" + tzr_last_error(ctx) + ")");
+  for (size_t b = 0; b < B; ++b) icp_result_from_c(res[b], corr[b].data(), &out[b]);
+  return out;
+}
+
+}  // namespace teaser

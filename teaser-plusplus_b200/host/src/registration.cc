@@ -627,8 +627,17 @@ std::vector<RobustRegistrationSolver::SolveCertifyResult> RobustRegistrationSolv
   return out;
 }
 
-std::vector<RobustRegistrationSolver::CloudPairResult> RobustRegistrationSolver::solveCloudPairs(
-    const std::vector<PointCloud>& clouds, const std::vector<std::pair<int, int>>& pairs, const CloudPairParams& cp) {
+void icp_result_from_c(const tzr_icp_result& r, const int32_t* corr, PointToPointICPResult* out);  // icp.cc
+
+namespace {
+
+// solveCloudPairs' body: tzr_register_cloud_pairs, or tzr_register_cloud_pairs_icp when icp is given (icp_res then
+// receives P records)
+std::vector<RobustRegistrationSolver::CloudPairResult> run_cloud_pairs(
+    const tzr_params& p, const std::vector<PointCloud>& clouds, const std::vector<std::pair<int, int>>& pairs,
+    const RobustRegistrationSolver::CloudPairParams& cp, const tzr_icp_params* icp,
+    std::vector<tzr_icp_result>* icp_res) {
+  using CloudPairResult = RobustRegistrationSolver::CloudPairResult;
   const int K = static_cast<int>(clouds.size()), P = static_cast<int>(pairs.size());
   std::vector<CloudPairResult> out(P);
   if (P == 0) return out;
@@ -663,14 +672,21 @@ std::vector<RobustRegistrationSolver::CloudPairResult> RobustRegistrationSolver:
   f.use_crosscheck = cp.use_crosscheck ? 1 : 0;
   f.use_tuple_test = cp.use_tuple_test ? 1 : 0;
   f.tuple_scale = cp.tuple_scale;
-  const tzr_params p = to_c(params_);
   std::vector<tzr_solution> sols(P);
   std::vector<int64_t> n_corr(P);
   std::vector<float> scales(P);
   tzr_ctx* ctx = b200_context();
-  const int rc = tzr_register_cloud_pairs(ctx, &f, &p, K, n.data(), pts.data(), P, pc.data(), seeds.data(), sols.data(),
-                                          status.data(), index.data(), n_corr.data(), corr_p.data(), clq_p.data(),
-                                          scales.data());
+  int rc;
+  if (!icp) {
+    rc = tzr_register_cloud_pairs(ctx, &f, &p, K, n.data(), pts.data(), P, pc.data(), seeds.data(), sols.data(),
+                                  status.data(), index.data(), n_corr.data(), corr_p.data(), clq_p.data(),
+                                  scales.data());
+  } else {
+    icp_res->assign(P, tzr_icp_result{});
+    rc = tzr_register_cloud_pairs_icp(ctx, &f, &p, K, n.data(), pts.data(), P, pc.data(), seeds.data(), sols.data(),
+                                      status.data(), index.data(), n_corr.data(), corr_p.data(), clq_p.data(),
+                                      scales.data(), icp, icp_res->data());
+  }
   if (rc != TZR_OK && rc != TZR_ERR_TOO_LARGE) fail("RobustRegistrationSolver::solveCloudPairs", rc, ctx);
   for (int q = 0; q < P; ++q) {
     CloudPairResult& r = out[q];
@@ -683,6 +699,34 @@ std::vector<RobustRegistrationSolver::CloudPairResult> RobustRegistrationSolver:
     for (int k = 0; k < 3; ++k) r.solution.translation(k) = sols[q].translation[k];
     std::memcpy(r.solution.rotation.data(), sols[q].rotation, sizeof(sols[q].rotation));
     if (index[q] >= 0) r.max_clique.assign(clq[q].begin(), clq[q].begin() + std::max(0, sols[q].clique_size));
+  }
+  return out;
+}
+
+}  // namespace
+
+std::vector<RobustRegistrationSolver::CloudPairResult> RobustRegistrationSolver::solveCloudPairs(
+    const std::vector<PointCloud>& clouds, const std::vector<std::pair<int, int>>& pairs, const CloudPairParams& cp) {
+  return run_cloud_pairs(to_c(params_), clouds, pairs, cp, nullptr, nullptr);
+}
+
+std::vector<RobustRegistrationSolver::CloudPairICPResult> RobustRegistrationSolver::solveCloudPairs(
+    const std::vector<PointCloud>& clouds, const std::vector<std::pair<int, int>>& pairs, const CloudPairParams& cp,
+    const PointToPointICPParams& icp) {
+  tzr_icp_params ip;
+  tzr_icp_params_default(&ip);
+  ip.max_correspondence_distance = icp.max_correspondence_distance;
+  ip.max_iteration = icp.max_iteration;
+  ip.relative_fitness = icp.relative_fitness;
+  ip.relative_rmse = icp.relative_rmse;
+  std::vector<tzr_icp_result> res;
+  std::vector<CloudPairResult> base = run_cloud_pairs(to_c(params_), clouds, pairs, cp, &ip, &res);
+  std::vector<CloudPairICPResult> out(base.size());
+  for (size_t q = 0; q < base.size(); ++q) {
+    static_cast<CloudPairResult&>(out[q]) = std::move(base[q]);
+    // a refined pair: solved with a valid solution (the library zeroes every other pair's record)
+    out[q].refined = out[q].status == TZR_OK && out[q].solution.valid && res[q].transform.scale > 0;
+    if (out[q].refined) icp_result_from_c(res[q], nullptr, &out[q].icp);
   }
   return out;
 }
