@@ -533,6 +533,47 @@ int tzr_register_cloud_pairs_icp(tzr_ctx* ctx, const tzr_frontend_params* fparam
                                  int64_t* n_corr, int32_t* const* corr, int32_t* const* cliques, float* global_scale,
                                  const tzr_icp_params* icp, tzr_icp_result* icp_results);
 
+/* ---- downsampling point clouds: voxel-grid averaging ----------------------------------------------------------
+ * The first step of the reference's FPFH + TEASER++ + ICP tutorial (voxel_down_sample on both raw scans), for many
+ * clouds at once.  Open3D's PointCloud::VoxelDownSample, points only, with a defined order.  Per cloud, all arithmetic
+ * is IEEE float64 with no FMA contraction (DESIGN.md §3.12):
+ *   - Inputs: n float xyz points, read exactly as float64, and one voxel_size v for the whole call; v must be finite
+ *     and > 0 (anything else is TZR_ERR_INVALID_ARG, as Open3D's voxel_size <= 0 check).
+ *   - Finite points only: a point with any non-finite coordinate belongs to no voxel (voxel_of -1) and does not affect
+ *     the bounds.  (Open3D's result is undefined there.)
+ *   - Bounds: min and max are the component-wise bounds over the finite points; vmin = min - (v * 0.5) and
+ *     vmax = max + (v * 0.5).
+ *   - Too small a voxel: a cloud with v * INT_MAX < max_k (vmax_k - vmin_k) (Open3D's check) gets TZR_ERR_TOO_LARGE.
+ *   - Voxel index: i_k = (int) floor((p_k - vmin_k) / v), a division as Open3D writes it (not a product with 1/v,
+ *     which gives a different voxel on some voxel edges).
+ *   - Grid-size limit: points are grouped by the exact triple (i_x, i_y, i_z), packed into one 64-bit key; a cloud
+ *     whose per-axis voxel counts (i_k of its largest finite coordinate, + 1) multiply to more than 2^62 gets
+ *     TZR_ERR_TOO_LARGE.
+ *   - Output point: each voxel's point is the sum of its member points, added one at a time in ascending input index
+ *     starting from 0.0 (Open3D's AccumulatedPoint), divided by (double) count, the mean rounded once to float.
+ *   - Output order: voxels ordered by their first (lowest-index) member.  (Open3D's order is its unordered_map's.)  A
+ *     cloud already sparser than the grid comes back unchanged, in the same order.
+ *   - Colours and normals are not carried.
+ * Cost: a voxel of k points costs one thread k dependent additions (the bit-exact sequential sum), so one voxel holding
+ * a whole cloud is correct but slow.  Host pointers, synchronous; 10 kernel launches per call (CUB calls counted as
+ * one), whatever B.  These calls are not solve entries: they use a workspace of their own, so a retained solve
+ * (tzr_last_inliers, tzr_last_graph, tzr_certify_last_solve) stays retained across them. */
+
+/* One cloud of n >= 1 points: tzr_voxel_downsample_batch with B = 1 (its status is the return value). */
+int tzr_voxel_downsample(tzr_ctx* ctx, const float* pts, int n, double voxel_size,
+                         float* pts_out, int32_t* n_out, int32_t* voxel_of);
+
+/* B clouds: cloud b has n[b] >= 1 points at pts[b].  pts_out[b]: room for n[b] x 3 floats (always enough), receives
+ * n_out[b] rows (n_out: B entries).  voxel_of (may be NULL or hold NULL entries): voxel_of[b][i] is the output row of
+ * input point i, or -1 (Open3D's VoxelDownSampleAndTrace, in a form that carries labels or colours).  status (may be
+ * NULL; B entries): TZR_OK, or TZR_ERR_TOO_LARGE for a cloud whose grid is too large; such a cloud gets n_out = 0 and
+ * voxel_of -1, every other cloud's outputs are still written, and the call returns TZR_ERR_TOO_LARGE.  A cloud with no
+ * finite point gets n_out = 0 and status TZR_OK.  Per cloud, every output is bit-identical to the call on that cloud
+ * alone.  TZR_ERR_TOO_LARGE when the batch holds more than 2^31 - 1 points; TZR_ERR_ALLOC when the workspace does not
+ * fit the device (tzr_last_error names the size). */
+int tzr_voxel_downsample_batch(tzr_ctx* ctx, int B, const int32_t* n, const float* const* pts, double voxel_size,
+                               float* const* pts_out, int32_t* n_out, int32_t* const* voxel_of, int32_t* status);
+
 /* Graph-stage timing of the most recent tzr_solve_batch_dev, in milliseconds, measured with CUDA
  * events on the context's stream (for the roofline line in bench.py). Requires a prior synchronize. */
 int tzr_last_stage_ms(tzr_ctx* ctx, double* prep_ms, double* graph_ms, double* clique_ms, double* rot_trans_ms);

@@ -111,6 +111,14 @@ for iflags in (33554432, 67108864):
                               0.05, max_iteration=3)
     print("icp flags", iflags, [int(r) for r in res["n_correspondences"]], [int(r) for r in res["iterations"]])
 ctx.set_flags(0)
+# voxel downsampling: a ragged batch with a NaN row, an all-NaN cloud and a cloud too wide for the voxel (INT_MAX check)
+vx = [rng.uniform(0, 1, size=(500, 3)).astype(np.float32), np.full((3, 3), np.nan, dtype=np.float32),
+      np.array([[0, 0, 0], [1e9, 0, 0]], dtype=np.float32), rng.uniform(0, 1, size=(1, 3)).astype(np.float32)]
+vx[0][7] = np.nan
+try:
+    ctx.voxel_downsample_batch(vx, 0.1, return_trace=True)
+except capi.TzrError as e:
+    print("voxel status", e.status.tolist(), [len(o) for o in e.result[0]])
 sols, cl = capi.solve_batch_multi([p["src"] for p in prs[:5]], [p["dst"] for p in prs[:5]],
                                   capi.default_params(**dict(kw, noise_bound=prs[0]["noise_bound"])))
 print("multi", int(sols["valid"].sum()), "/ 5")

@@ -135,7 +135,7 @@ _SYMBOLS = [
     "tzr_certifier_psd_projection", "tzr_certifier_batch_psd_projection", "tzr_certifier_batch_dual_projection",
     "tzr_fpfh_pair_features", "tzr_fpfh_smallest_eigenpair", "tzr_last_inliers", "tzr_certify_last_solve",
     "tzr_frontend_params_default", "tzr_register_cloud_pairs", "tzr_icp_params_default", "tzr_icp", "tzr_icp_batch",
-    "tzr_register_cloud_pairs_icp",
+    "tzr_register_cloud_pairs_icp", "tzr_voxel_downsample", "tzr_voxel_downsample_batch",
 ]
 
 # status codes (tzr_status)
@@ -251,6 +251,8 @@ def lib():
                                 C.POINTER(IcpResult), C.POINTER(i32p)]
     L.tzr_register_cloud_pairs_icp.argtypes = L.tzr_register_cloud_pairs.argtypes + [C.POINTER(IcpParams),
                                                                                     C.POINTER(IcpResult)]
+    L.tzr_voxel_downsample.argtypes = [vp, fp, C.c_int, C.c_double, fp, i32p, i32p]
+    L.tzr_voxel_downsample_batch.argtypes = [vp, C.c_int, i32p, fpp, C.c_double, fpp, i32p, C.POINTER(i32p), i32p]
     for s in _SYMBOLS:
         getattr(L, s)  # raises AttributeError if the header and the library disagree
     _lib = L
@@ -1021,6 +1023,49 @@ class Context:
         self._ck(rc)
         out = np.frombuffer(bytes(res), dtype=ICP_RESULT_DTYPE).copy()
         return out, [c[:int(r["n_correspondences"])].copy() for c, r in zip(corr, out)]
+
+    def voxel_downsample(self, pts, voxel_size, return_trace=False):
+        """tzr_voxel_downsample: Open3D's voxel_down_sample of one (n,3) float32 cloud, points only (the definition is
+        include/teaser_b200.h's): the (m,3) float32 voxel means ordered by each voxel's first member, and with
+        return_trace the (n,) int32 output row of every input point (-1: a non-finite point)."""
+        p = _cloud32(pts, "voxel_downsample")
+        out = np.zeros_like(p)
+        trace = np.zeros(p.shape[0], dtype=np.int32)
+        m = np.zeros(1, dtype=np.int32)
+        self._ck(lib().tzr_voxel_downsample(self._h, _p(p, C.c_float), p.shape[0], float(voxel_size),
+                                            _p(out, C.c_float), _p(m, C.c_int32),
+                                            _p(trace, C.c_int32) if return_trace else None))
+        out = out[:int(m[0])].copy()
+        return (out, trace) if return_trace else out
+
+    def voxel_downsample_batch(self, pts_list, voxel_size, return_trace=False):
+        """voxel_downsample of every (n_b,3) cloud of the list in one call (tzr_voxel_downsample_batch): a list of
+        (m_b,3) voxel means (and a list of traces), each bit-identical to voxel_downsample on that cloud alone.  When a
+        cloud's grid is too large the TzrError carries `status` (per cloud 0 or the error code) and `result` (the
+        outputs of every cloud, written for the others; empty for the too-large ones)."""
+        pts = [_cloud32(p, "voxel_downsample_batch") for p in pts_list]
+        if not pts:
+            raise TzrError("voxel_downsample_batch: a non-empty list of (n,3) clouds is required")
+        B = len(pts)
+        n = np.array([p.shape[0] for p in pts], dtype=np.int32)
+        outs = [np.zeros_like(p) for p in pts]
+        traces = [np.zeros(p.shape[0], dtype=np.int32) for p in pts] if return_trace else None
+        m = np.zeros(B, dtype=np.int32)
+        status = np.zeros(B, dtype=np.int32)
+        fp, i32p = C.POINTER(C.c_float), C.POINTER(C.c_int32)
+        rc = lib().tzr_voxel_downsample_batch(self._h, B, _p(n, C.c_int32), (fp * B)(*[_p(p, C.c_float) for p in pts]),
+                                              float(voxel_size), (fp * B)(*[_p(o, C.c_float) for o in outs]),
+                                              _p(m, C.c_int32),
+                                              (i32p * B)(*[_p(t, C.c_int32) for t in traces]) if traces else None,
+                                              _p(status, C.c_int32))
+        outs = [o[:int(k)].copy() for o, k in zip(outs, m)]
+        result = (outs, traces) if return_trace else outs
+        try:
+            self._ck(rc)
+        except TzrError as e:
+            e.status, e.result = status, result
+            raise
+        return result
 
     def last_graph(self, b: int, n: int):
         W = lib().tzr_words_per_row(n)

@@ -38,6 +38,8 @@ struct tzr_ctx {
   DevBuf rg;
   // tzr_icp(_batch): its own workspace, so that refinement leaves a retained solve intact
   DevBuf icp;
+  // tzr_voxel_downsample(_batch): its own workspace, for the same reason
+  DevBuf vox;
   int max_n = kMaxN;  // per-problem size limit of this context (tzr_ctx_set_max_n: kMaxN ... kMaxNLarge)
   // pinned host staging
   void* h_pin = nullptr;
@@ -1207,7 +1209,8 @@ int tzr_ctx_destroy(tzr_ctx* ctx) {
                     &ctx->hclq, &ctx->hsize, &ctx->clq, &ctx->L, &ctx->alive, &ctx->best_bits, &ctx->alive_cnt, &ctx->root_ctr,
                     &ctx->lock, &ctx->flg, &ctx->kfinal, &ctx->tstart, &ctx->stack, &ctx->cv, &ctx->centry, &ctx->ps, &ctx->pd, &ctx->wgt,
                     &ctx->res, &ctx->skey, &ctx->sidx, &ctx->sorted, &ctx->rmask, &ctx->tmask, &ctx->sol, &ctx->dbg,
-                    &ctx->misc, &ctx->sc, &ctx->m_in, &ctx->m_scratch, &ctx->m_out, &ctx->cert, &ctx->certb, &ctx->lg, &ctx->cq, &ctx->rg, &ctx->icp};
+                    &ctx->misc, &ctx->sc, &ctx->m_in, &ctx->m_scratch, &ctx->m_out, &ctx->cert, &ctx->certb, &ctx->lg, &ctx->cq, &ctx->rg, &ctx->icp,
+                    &ctx->vox};
   for (DevBuf* b : bufs)
     if (b->p) cudaFree(b->p);
   if (ctx->h_pin) cudaFreeHost(ctx->h_pin);
@@ -2468,6 +2471,80 @@ int tzr_icp(tzr_ctx* ctx, const tzr_icp_params* params, const float* src, int ns
   }
   int32_t* const corrs[1] = {corr};
   return tzr_icp_batch(ctx, params, 1, &ns, &src, &nd, &dst, init, result, corr ? corrs : nullptr);
+}
+
+// tzr_voxel_downsample(_batch): the clouds staged back to back (one H2D copy), the batch's launches (launch_voxel), a
+// read-back of the cloud table, then one D2H copy of the batch's voxels (and of voxel_of when some cloud asks for it).
+// Workspace ctx->vox: [points | cloud table | voxels | voxel_of | scratch]; the pinned area mirrors its first four.
+int tzr_voxel_downsample_batch(tzr_ctx* ctx, int B, const int32_t* n, const float* const* pts, double voxel_size,
+                               float* const* pts_out, int32_t* n_out, int32_t* const* voxel_of, int32_t* status) {
+  if (!ctx || B < 1 || !n || !pts || !pts_out || !n_out || !(voxel_size > 0) || !std::isfinite(voxel_size))
+    return TZR_ERR_INVALID_ARG;
+  bool want_trace = false;
+  for (int b = 0; b < B; ++b) {
+    if (n[b] < 1 || !pts[b] || !pts_out[b]) return TZR_ERR_INVALID_ARG;
+    want_trace |= voxel_of && voxel_of[b];
+  }
+  std::vector<VoxCloud> clouds((size_t)B);
+  VoxPlan plan;
+  if (voxel_plan(B, n, clouds.data(), &plan) != TZR_OK) {
+    ctx->last_error = "the batch's points do not fit 32-bit indices";
+    return TZR_ERR_TOO_LARGE;
+  }
+  cudaSetDevice(ctx->device);
+  cudaStream_t st = ctx->stream;
+  const size_t N = (size_t)plan.N, pb = N * 12, tb = (size_t)B * sizeof(VoxCloud);
+  const size_t o_tab = al256(pb), in_bytes = o_tab + tb, o_out = al256(in_bytes), o_vo = o_out + al256(pb),
+               o_scr = o_vo + al256(N * 4), total = o_scr + plan.scratch_bytes;
+  int rc;
+  if ((rc = ensure(ctx, ctx->vox, total)) != TZR_OK) return rc;
+  if ((rc = ensure_pinned(ctx, o_scr)) != TZR_OK) return rc;
+  char* h = (char*)ctx->h_pin;
+  char* d = (char*)ctx->vox.p;
+  std::vector<CopySpan> spans;
+  for (int b = 0; b < B; ++b) spans.push_back(CopySpan{h + (size_t)clouds[b].lo * 12, pts[b], (size_t)n[b] * 12});
+  spans.push_back(CopySpan{h + o_tab, clouds.data(), tb});
+  CK(stage_in(spans, h, d, o_tab, in_bytes, B == 1, st));
+  ctx->launches += launch_voxel(plan, voxel_size, (const float*)d, (VoxCloud*)(d + o_tab), d + o_scr,
+                                (float*)(d + o_out), (int*)(d + o_vo), st);
+  if ((rc = check_launch(ctx, "voxel launch")) != TZR_OK) return rc;
+  CK(cudaMemcpyAsync(clouds.data(), d + o_tab, tb, cudaMemcpyDeviceToHost, st));
+  CK(cudaStreamSynchronize(st));
+  const size_t rows = (size_t)clouds[B - 1].out_lo + (size_t)clouds[B - 1].n_out;
+  spans.clear();
+  for (int b = 0; b < B; ++b) {
+    const VoxCloud& c = clouds[b];
+    spans.push_back(CopySpan{pts_out[b], h + o_out + (size_t)c.out_lo * 12, (size_t)c.n_out * 12});
+    if (voxel_of && voxel_of[b]) spans.push_back(CopySpan{voxel_of[b], h + o_vo + (size_t)c.lo * 4, (size_t)c.n * 4});
+  }
+  if (B == 1) {  // straight into the caller's buffers
+    for (const CopySpan& s : spans)
+      if (s.bytes) CK(cudaMemcpyAsync(s.dst, d + ((const char*)s.src - h), s.bytes, cudaMemcpyDeviceToHost, st));
+    CK(cudaStreamSynchronize(st));
+  } else {
+    if (rows) CK(cudaMemcpyAsync(h + o_out, d + o_out, rows * 12, cudaMemcpyDeviceToHost, st));
+    if (want_trace) CK(cudaMemcpyAsync(h + o_vo, d + o_vo, N * 4, cudaMemcpyDeviceToHost, st));
+    CK(cudaStreamSynchronize(st));
+    parallel_copy(spans);
+  }
+  bool too_large = false;
+  for (int b = 0; b < B; ++b) {
+    n_out[b] = clouds[b].n_out;
+    if (status) status[b] = clouds[b].status;
+    too_large |= clouds[b].status != TZR_OK;
+  }
+  if (too_large) {
+    ctx->last_error = "a cloud's voxel grid is too large for the voxel size (Open3D's INT_MAX check or 2^62 cells)";
+    return TZR_ERR_TOO_LARGE;
+  }
+  return TZR_OK;
+}
+
+int tzr_voxel_downsample(tzr_ctx* ctx, const float* pts, int n, double voxel_size, float* pts_out, int32_t* n_out,
+                         int32_t* voxel_of) {
+  const int32_t n1 = n;
+  int32_t* const vo[1] = {voxel_of};
+  return tzr_voxel_downsample_batch(ctx, 1, &n1, &pts, voxel_size, &pts_out, n_out, vo, nullptr);
 }
 
 int tzr_fpfh_pair_features(tzr_ctx* ctx, int n, const float* p1, const float* n1, const float* p2, const float* n2,

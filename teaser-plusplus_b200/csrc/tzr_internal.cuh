@@ -453,5 +453,30 @@ int launch_icp(const IcpPlan& plan, const float* src, const float* dst, IcpProb*
 // and a positive scale sets (s, R, t) and active = seeded = 1, any other leaves the problem inactive.  One launch.
 int launch_icp_seed(IcpProb* probs, int B, const tzr_solution* sol, cudaStream_t st);
 
+// voxel.cu (voxel-grid downsampling, DESIGN.md §3.12): B clouds stored back to back
+constexpr unsigned long long kVoxNone = 1ull << 62;  // sort key of a point in no voxel: above every voxel key (< 2^62)
+constexpr int kVoxKeyBits = 63;                      // key bits the sort looks at
+struct VoxCloud {       // one per cloud; the host fills lo, n and the bound sentinels, the kernels the rest
+  int lo, n;            // first point of the cloud in the flat array, point count
+  int mn[3], mx[3];     // bounds of the finite points (ordered-int floats; INT_MAX / INT_MIN: none yet)
+  double vmin[3];       // min - v * 0.5
+  long long cy, cz;     // voxels along y and z (the key's strides)
+  int status;           // TZR_OK, or TZR_ERR_TOO_LARGE (Open3D's INT_MAX check or the 2^62-cell limit)
+  int valid;            // 1: the cloud has a finite point and its grid fits; its finite points get voxel keys
+  int out_lo, n_out;    // its first output row in the batch, its voxels
+};
+struct VoxPlan {
+  int B = 0, N = 0;
+  size_t scratch_bytes = 0;
+};
+// Fills clouds[0..B) (host copy, staged to the device before launch_voxel) and the plan; TZR_ERR_TOO_LARGE when the
+// batch's points do not fit 32-bit indices.
+int voxel_plan(int B, const int32_t* n, VoxCloud* clouds, VoxPlan* plan);
+// pts (N x 3 floats), clouds (device copy of voxel_plan's table), scratch (plan.scratch_bytes), out (N x 3 floats: the
+// voxels of the batch in cloud order, cloud b's from row out_lo), voxel_of (N ints: the cloud-local output row of every
+// point, -1 for a point in no voxel): device pointers.  Returns the launches (10).
+int launch_voxel(const VoxPlan& plan, double voxel_size, const float* pts, VoxCloud* clouds, void* scratch, float* out,
+                 int* voxel_of, cudaStream_t st);
+
 
 }  // namespace tzr

@@ -13,6 +13,7 @@
 #include "teaser/certification.h"
 #include "teaser/icp.h"
 #include "teaser/registration.h"
+#include "teaser/voxel.h"
 
 namespace py = pybind11;
 using Solver = teaser::RobustRegistrationSolver;
@@ -60,6 +61,17 @@ teaser::PointCloud cloud_of(const CloudArray& a) {
   pc.reserve(static_cast<size_t>(a.shape(0)));
   for (py::ssize_t i = 0; i < a.shape(0); ++i) pc.push_back({d[3 * i], d[3 * i + 1], d[3 * i + 2]});
   return pc;
+}
+
+py::array_t<float> cloud_to_numpy(const teaser::PointCloud& pc) {
+  py::array_t<float> out({static_cast<py::ssize_t>(pc.size()), static_cast<py::ssize_t>(3)});
+  float* d = out.mutable_data();
+  for (size_t i = 0; i < pc.size(); ++i) {
+    d[3 * i] = pc[i].x;
+    d[3 * i + 1] = pc[i].y;
+    d[3 * i + 2] = pc[i].z;
+  }
+  return out;
 }
 
 py::dict icp_dict(const teaser::PointToPointICPResult& r) {
@@ -141,6 +153,33 @@ PYBIND11_MODULE(_teaserpp, m) {
              return out;
            },
            py::arg("src"), py::arg("dst"), py::arg("init"));
+
+  // GPU extra: the first step of the same tutorial, Open3D's voxel_down_sample (teaser::voxelDownSample)
+  m.def("voxel_down_sample",
+        [](const CloudArray& points, double voxel_size) {
+          const teaser::PointCloud pc = cloud_of(points);
+          teaser::PointCloud out;
+          {
+            py::gil_scoped_release release;
+            out = teaser::voxelDownSample(pc, voxel_size);
+          }
+          return cloud_to_numpy(out);
+        },
+        py::arg("points"), py::arg("voxel_size"));
+  m.def("voxel_down_sample_batch",
+        [](const std::vector<CloudArray>& points, double voxel_size) {
+          std::vector<teaser::PointCloud> pcs;
+          for (const auto& a : points) pcs.push_back(cloud_of(a));
+          std::vector<teaser::PointCloud> res;
+          {
+            py::gil_scoped_release release;
+            res = teaser::voxelDownSampleBatch(pcs, voxel_size);
+          }
+          py::list out;
+          for (const auto& pc : res) out.append(cloud_to_numpy(pc));
+          return out;
+        },
+        py::arg("points"), py::arg("voxel_size"));
 
   m.attr("OMP_MAX_THREADS") = 0;  // the GPU path ignores max_clique_num_threads
 
