@@ -222,6 +222,21 @@ int tzr_compute_fpfh_batch(tzr_ctx* ctx, int B, const int32_t* n, const float* c
                            double normal_search_radius, double fpfh_search_radius, float* const* fpfh_out,
                            float* const* normals_out, int32_t* status);
 
+/* Normals alone: the first pass of tzr_compute_fpfh (PCL's NormalEstimationOMP, radius normal_search_radius, viewpoint
+ * at the origin) without the descriptor passes, e.g. the target normals of point-to-plane ICP.  normals_out: n x 4
+ * floats (normal_x, normal_y, normal_z, curvature), bit-identical to tzr_compute_fpfh's normals_out at the same normal
+ * radius, whatever its fpfh_search_radius: a point's neighbours are the points with float d^2 < r^2, sorted by
+ * (d^2, index) before the covariance is summed, so neither the grid's cell edge nor the search route changes them.
+ * NaN where a point has fewer than 3 neighbours.  The search route is tzr_compute_fpfh's (brute force below 4096
+ * points, the hashed grid from there; debug flags 4194304 and 8388608).  Arguments, status, TZR_ERR_TOO_LARGE (a point
+ * with more than 4096 neighbours; the other clouds are still written) and workspace as tzr_compute_fpfh(_batch): the
+ * calls share the front end's buffers, so a retained tzr_solve / tzr_solve_batch stays retained across them.
+ * Batch: normals_out[b] (every entry required): n[b] x 4 floats; status (may be NULL): B entries.  Per cloud, the
+ * output is bit-identical to tzr_estimate_normals on that cloud alone. */
+int tzr_estimate_normals(tzr_ctx* ctx, const float* pts, int n, double normal_search_radius, float* normals_out);
+int tzr_estimate_normals_batch(tzr_ctx* ctx, int B, const int32_t* n, const float* const* pts,
+                               double normal_search_radius, float* const* normals_out, int32_t* status);
+
 /* Building blocks of tzr_compute_fpfh, exposed so that each can be checked on any input, not only on the ones a cloud
  * produces.  Host pointers, synchronous; each runs the production device function, one item per thread.
  * tzr_fpfh_pair_features: pcl::computePairFeatures (features/src/pfh_tools.cpp) on n point pairs: p1, n1, p2, n2 are
@@ -533,6 +548,71 @@ int tzr_register_cloud_pairs_icp(tzr_ctx* ctx, const tzr_frontend_params* fparam
                                  int64_t* n_corr, int32_t* const* corr, int32_t* const* cliques, float* global_scale,
                                  const tzr_icp_params* icp, tzr_icp_result* icp_results);
 
+/* ---- refining registrations: point-to-plane ICP -------------------------------------------------------------
+ * Open3D's registration_icp with TransformationEstimationPointToPlane, for many problems at once, defined here as
+ * follows (DESIGN.md §3.13):
+ *   - Unchanged from tzr_icp: the inputs x, y and (s, R0, t0), the fixed scale, the transform p_i = s (R x_i) + t from the
+ *     original point on every iteration, the correspondence search and its routes, eval(T) (fitness and inlier_rmse from
+ *     the point distances d^2, as Open3D evaluates point-to-plane runs), the loop, the convergence test and the
+ *     composition R <- R_u R, t <- R_u t + t_u.  The target normals play no part in the search or in the evaluation.
+ *   - Target normals: nd x 4 floats per target in the library's normals layout (normal_x, normal_y, normal_z,
+ *     curvature: tzr_compute_fpfh's and tzr_estimate_normals' normals_out); the fourth float is ignored.  Read exactly as
+ *     float64 and used as given: not renormalised, and their sign does not matter (below).
+ *   - Update (R_u, t_u) from the current correspondences, in IEEE float64 with no FMA contraction.  count = 0: the
+ *     identity.  Otherwise c = mu_p, the mean of the matched transformed sources, and each correspondence (i, j) whose
+ *     normal n = n_j has three finite components contributes, with u = p_i - c and q = y_j:
+ *       a = u x n:  a0 = u1 n2 - u2 n1,  a1 = u2 n0 - u0 n2,  a2 = u0 n1 - u1 n0
+ *       J = (a0, a1, a2, n0, n1, n2),  r = ((p0 - q0) n0 + (p1 - q1) n1) + (p2 - q2) n2
+ *     A correspondence with a non-finite normal counts for fitness and rmse but adds nothing here.  A = sum J J^T (its
+ *     21 distinct entries) and g = sum J r, summed in the fixed chunk order of tzr_icp's sums; x solves A x = -g by the
+ *     6 x 6 solve below.  With ca = cos x0, sa = sin x0, cb = cos x1, sb = sin x1, cg = cos x2, sg = sin x2,
+ *     R_u = Rz(x2) Ry(x1) Rx(x0) (Open3D's TransformVector6dToMatrix4d) =
+ *       [ cg cb   (cg sb) sa - sg ca   (cg sb) ca + sg sa ]
+ *       [ sg cb   (sg sb) sa + cg ca   (sg sb) ca - cg sa ]
+ *       [ -sb     cb sa                cb ca              ]
+ *     and t_u = (c + tau) - R_u c with tau = (x3, x4, x5), row r: (c(r) + tau(r)) - ((R_u(r,0) c0 + R_u(r,1) c1) +
+ *     R_u(r,2) c2).  If any component of x is non-finite the update is the identity.  Flipping n negates J and r
+ *     exactly, so A, g and every output are bit-identical under any choice of normal signs.
+ *   - The 6 x 6 solve: a truncated LDL^T with diagonal pivoting.  tol = 1e-10 * max_k A_kk (the original diagonal).
+ *     Step k picks the remaining index with the largest current diagonal (the lowest index on ties; a NaN diagonal is
+ *     never the largest); if that diagonal is not > tol (NaN included), elimination stops and every remaining component
+ *     of the permuted solution is 0.  Otherwise it eliminates as usual; then forward substitution, scaling by the
+ *     pivots and back substitution over the leading block.  So a flat target (all normals parallel) gets no motion
+ *     along its unobservable directions.
+ *   - Centred linearisation: Open3D linearises about the origin; this one about c.  The two are the same Gauss-Newton
+ *     step up to second order in the rotation angle and have the same fixed points, and the centred one keeps its
+ *     digits far from the origin (DESIGN.md §3.13).
+ * Launches: 2 + 4 * max_iteration (+ 4 for the grid build when some target has at least 1024 points), whatever B, as
+ * tzr_icp_batch.  Workspace: tzr_icp's own, so a retained solve stays retained. */
+
+/* One problem: tzr_icp's arguments plus dst_normals (nd x 4 floats, required).  This is tzr_icp_point_to_plane_batch
+ * with B = 1. */
+int tzr_icp_point_to_plane(tzr_ctx* ctx, const tzr_icp_params* params, const float* src, int ns, const float* dst,
+                           int nd, const float* dst_normals, const tzr_similarity* init, tzr_icp_result* result,
+                           int32_t* corr);
+
+/* B ragged problems: tzr_icp_batch's arguments plus dst_normals (B entries, entry b nd[b] x 4 floats; NULL or a NULL
+ * entry is TZR_ERR_INVALID_ARG).  Per problem, every output is bit-identical to tzr_icp_point_to_plane on that problem
+ * alone. */
+int tzr_icp_point_to_plane_batch(tzr_ctx* ctx, const tzr_icp_params* params, int B, const int32_t* ns,
+                                 const float* const* src, const int32_t* nd, const float* const* dst,
+                                 const float* const* dst_normals, const tzr_similarity* init,
+                                 tzr_icp_result* results, int32_t* const* corr);
+
+/* tzr_register_cloud_pairs_icp with point-to-plane ICP: the same arguments and the same outputs, except that each
+ * refined record is point-to-plane ICP on the pair's two clouds, using the target cloud's normals from the call's own
+ * FPFH stage (normal_search_radius, viewpoint at the origin).  No normal pass, upload or host synchronisation is added.
+ * Each refined record is bit-identical to tzr_register_cloud_pairs, then tzr_estimate_normals_batch over the clouds at
+ * fparams->normal_search_radius, then tzr_icp_point_to_plane_batch over the valid solved pairs seeded with their
+ * records.  Launches: as tzr_register_cloud_pairs_icp. */
+int tzr_register_cloud_pairs_icp_point_to_plane(tzr_ctx* ctx, const tzr_frontend_params* fparams,
+                                                const tzr_params* params, int n_clouds, const int32_t* n,
+                                                const float* const* pts, int P, const int32_t* pair_clouds,
+                                                const uint64_t* tuple_seeds, tzr_solution* solutions,
+                                                int32_t* status, int32_t* problem_index, int64_t* n_corr,
+                                                int32_t* const* corr, int32_t* const* cliques, float* global_scale,
+                                                const tzr_icp_params* icp, tzr_icp_result* icp_results);
+
 /* ---- downsampling point clouds: voxel-grid averaging ----------------------------------------------------------
  * The first step of the reference's FPFH + TEASER++ + ICP tutorial (voxel_down_sample on both raw scans), for many
  * clouds at once.  Open3D's PointCloud::VoxelDownSample, points only, with a defined order.  Per cloud, all arithmetic
@@ -620,6 +700,7 @@ int tzr_solve_batch_multi(const int32_t* devices, int n_devices, const tzr_param
  * to brute force), so that the two routes can be compared on one input; bit 22 wins when both are set, bit 24
  * (16777216) = a ragged batch forms one size class wherever the large-route and scale-path rules allow, however far
  * apart its sizes are, so that tests can pad n = 2 to n = 4000 in one device batch, bit 25 (33554432) = tzr_icp(_batch)
+ * and tzr_icp_point_to_plane(_batch)
  * searches every target by brute force, bit 26 (67108864) = through the hashed grid at any target size (a target the
  * grid cannot index still falls back to brute force), so that the two routes can be compared on one input; bit 25 wins
  * when both are set.

@@ -111,6 +111,20 @@ for iflags in (33554432, 67108864):
                               0.05, max_iteration=3)
     print("icp flags", iflags, [int(r) for r in res["n_correspondences"]], [int(r) for r in res["iterations"]])
 ctx.set_flags(0)
+# normals alone and point-to-plane ICP: a ragged batch with NaN normals, a non-finite point and an overflowing cloud
+nm = [ic_src, ic_dst, np.zeros((4100, 3), dtype=np.float32), ic_src[:2]]
+try:
+    ctx.estimate_normals_batch(nm, 0.05)
+except capi.TzrError as e:
+    print("normals status", e.status.tolist())
+    nrm = e.result
+nrm[0][::4] = np.nan
+for iflags in (33554432, 67108864):
+    ctx.set_flags(iflags)
+    res, corr = ctx.icp_point_to_plane_batch([ic_dst, ic_src[:3], ic_src], [ic_src, ic_dst, ic_src[:2]],
+                                             [nrm[0], nrm[1], nrm[3]], 0.05, max_iteration=3)
+    print("icp plane flags", iflags, [int(r) for r in res["n_correspondences"]], [int(r) for r in res["iterations"]])
+ctx.set_flags(0)
 # voxel downsampling: a ragged batch with a NaN row, an all-NaN cloud and a cloud too wide for the voxel (INT_MAX check)
 vx = [rng.uniform(0, 1, size=(500, 3)).astype(np.float32), np.full((3, 3), np.nan, dtype=np.float32),
       np.array([[0, 0, 0], [1e9, 0, 0]], dtype=np.float32), rng.uniform(0, 1, size=(1, 3)).astype(np.float32)]

@@ -135,7 +135,9 @@ _SYMBOLS = [
     "tzr_certifier_psd_projection", "tzr_certifier_batch_psd_projection", "tzr_certifier_batch_dual_projection",
     "tzr_fpfh_pair_features", "tzr_fpfh_smallest_eigenpair", "tzr_last_inliers", "tzr_certify_last_solve",
     "tzr_frontend_params_default", "tzr_register_cloud_pairs", "tzr_icp_params_default", "tzr_icp", "tzr_icp_batch",
-    "tzr_register_cloud_pairs_icp", "tzr_voxel_downsample", "tzr_voxel_downsample_batch",
+    "tzr_register_cloud_pairs_icp", "tzr_voxel_downsample", "tzr_voxel_downsample_batch", "tzr_estimate_normals",
+    "tzr_estimate_normals_batch", "tzr_icp_point_to_plane", "tzr_icp_point_to_plane_batch",
+    "tzr_register_cloud_pairs_icp_point_to_plane",
 ]
 
 # status codes (tzr_status)
@@ -251,6 +253,13 @@ def lib():
                                 C.POINTER(IcpResult), C.POINTER(i32p)]
     L.tzr_register_cloud_pairs_icp.argtypes = L.tzr_register_cloud_pairs.argtypes + [C.POINTER(IcpParams),
                                                                                     C.POINTER(IcpResult)]
+    L.tzr_estimate_normals.argtypes = [vp, fp, C.c_int, C.c_double, fp]
+    L.tzr_estimate_normals_batch.argtypes = [vp, C.c_int, i32p, fpp, C.c_double, fpp, i32p]
+    L.tzr_icp_point_to_plane.argtypes = [vp, C.POINTER(IcpParams), fp, C.c_int, fp, C.c_int, fp, C.POINTER(Similarity),
+                                         C.POINTER(IcpResult), i32p]
+    L.tzr_icp_point_to_plane_batch.argtypes = [vp, C.POINTER(IcpParams), C.c_int, i32p, fpp, i32p, fpp, fpp,
+                                               C.POINTER(Similarity), C.POINTER(IcpResult), C.POINTER(i32p)]
+    L.tzr_register_cloud_pairs_icp_point_to_plane.argtypes = L.tzr_register_cloud_pairs_icp.argtypes
     L.tzr_voxel_downsample.argtypes = [vp, fp, C.c_int, C.c_double, fp, i32p, i32p]
     L.tzr_voxel_downsample_batch.argtypes = [vp, C.c_int, i32p, fpp, C.c_double, fpp, i32p, C.POINTER(i32p), i32p]
     for s in _SYMBOLS:
@@ -317,6 +326,17 @@ def _cloud32(a, what):
     if a.ndim != 2 or a.shape[1] != 3 or a.shape[0] == 0:
         raise TzrError(f"{what}: clouds must be non-empty (n,3) arrays")
     return a
+
+
+def _normals32(a, n, what):
+    """Target normals as (n,4) float32 rows (nx, ny, nz, curvature): an (n,4) array as given, an (n,3) one with a zero
+    fourth column (the library ignores it)."""
+    a = np.asarray(a, dtype=np.float32)
+    if a.ndim != 2 or a.shape[0] != n or a.shape[1] not in (3, 4):
+        raise TzrError(f"{what}: normals must be (nd,3) or (nd,4) with one row per target point")
+    if a.shape[1] == 3:
+        a = np.concatenate([a, np.zeros((n, 1), dtype=np.float32)], axis=1)
+    return np.ascontiguousarray(a)
 
 
 def _pts(a):
@@ -706,6 +726,38 @@ class Context:
             raise
         return result
 
+    def estimate_normals(self, pts, normal_search_radius=0.03):
+        """tzr_estimate_normals: compute_fpfh's normals alone, (n,3) float32 -> (n,4) float32 (nx, ny, nz, curvature),
+        bit-identical to compute_fpfh(..., return_normals=True)'s normals at the same normal radius."""
+        p = _cloud32(pts, "estimate_normals")
+        nor = np.zeros((p.shape[0], 4), dtype=np.float32)
+        self._ck(lib().tzr_estimate_normals(self._h, _p(p, C.c_float), p.shape[0], float(normal_search_radius),
+                                            _p(nor, C.c_float)))
+        return nor
+
+    def estimate_normals_batch(self, pts_list, normal_search_radius=0.03):
+        """estimate_normals on every (n_b,3) cloud of the list in one call: a list of (n_b,4) normals, each
+        bit-identical to estimate_normals on that cloud alone.  When a cloud has a point with more than 4096
+        neighbours the TzrError carries `status` (per cloud 0 or the error code) and `result` (every cloud's normals,
+        written for the others)."""
+        pts = [_cloud32(p, "estimate_normals_batch") for p in pts_list]
+        if not pts:
+            raise TzrError("estimate_normals_batch: a non-empty list of (n,3) clouds is required")
+        B = len(pts)
+        n = np.array([p.shape[0] for p in pts], dtype=np.int32)
+        nors = [np.zeros((p.shape[0], 4), dtype=np.float32) for p in pts]
+        status = np.zeros(B, dtype=np.int32)
+        fp = C.POINTER(C.c_float)
+        rc = lib().tzr_estimate_normals_batch(self._h, B, _p(n, C.c_int32), (fp * B)(*[_p(p, C.c_float) for p in pts]),
+                                              float(normal_search_radius), (fp * B)(*[_p(x, C.c_float) for x in nors]),
+                                              _p(status, C.c_int32))
+        try:
+            self._ck(rc)
+        except TzrError as e:
+            e.status, e.result = status, nors
+            raise
+        return nors
+
     @staticmethod
     def _rows3(a, n, what):
         a = np.ascontiguousarray(a, dtype=np.float32)
@@ -930,17 +982,22 @@ class Context:
     def register_cloud_pairs_icp(self, clouds, pairs, params: Params, max_correspondence_distance, normal_search_radius=0.03,
                                  fpfh_search_radius=0.05, use_absolute_scale=True, use_crosscheck=True,
                                  use_tuple_test=True, tuple_scale=0.0, tuple_seeds=None, max_iteration=30,
-                                 relative_fitness=1e-6, relative_rmse=1e-6):
+                                 relative_fitness=1e-6, relative_rmse=1e-6, method="point_to_point"):
         """tzr_register_cloud_pairs_icp: register_cloud_pairs, then ICP of every pair with a valid solution on its two
         clouds, seeded with that solution, in the same call.  Returns register_cloud_pairs' six results plus the ICP
-        records (structured array (P,) of ICP_RESULT_DTYPE, zeroed for a pair that was not refined)."""
+        records (structured array (P,) of ICP_RESULT_DTYPE, zeroed for a pair that was not refined).
+        method="point_to_plane" runs point-to-plane ICP (tzr_register_cloud_pairs_icp_point_to_plane) with the target
+        normals of the call's own FPFH stage."""
+        if method not in ("point_to_point", "point_to_plane"):
+            raise TzrError(f"register_cloud_pairs_icp: unknown method {method!r}")
         icp = icp_params(max_correspondence_distance, max_iteration=int(max_iteration),
                          relative_fitness=float(relative_fitness), relative_rmse=float(relative_rmse))
         return self._register_pairs(clouds, pairs, params, normal_search_radius, fpfh_search_radius, use_absolute_scale,
-                                    use_crosscheck, use_tuple_test, tuple_scale, tuple_seeds, icp)
+                                    use_crosscheck, use_tuple_test, tuple_scale, tuple_seeds, icp,
+                                    plane=method == "point_to_plane")
 
     def _register_pairs(self, clouds, pairs, params, normal_search_radius, fpfh_search_radius, use_absolute_scale,
-                        use_crosscheck, use_tuple_test, tuple_scale, tuple_seeds, icp):
+                        use_crosscheck, use_tuple_test, tuple_scale, tuple_seeds, icp, plane=False):
         cl = [np.ascontiguousarray(c, dtype=np.float32) for c in clouds]
         if not cl or any(c.ndim != 2 or c.shape[1] != 3 or c.shape[0] == 0 for c in cl):
             raise TzrError("register_cloud_pairs: a non-empty list of non-empty (n,3) clouds is required")
@@ -975,7 +1032,8 @@ class Context:
             rc = lib().tzr_register_cloud_pairs(*args)
         else:
             icp_res = np.zeros(P, dtype=ICP_RESULT_DTYPE)
-            rc = lib().tzr_register_cloud_pairs_icp(*args, C.byref(icp), icp_res.ctypes.data_as(C.POINTER(IcpResult)))
+            entry = lib().tzr_register_cloud_pairs_icp_point_to_plane if plane else lib().tzr_register_cloud_pairs_icp
+            rc = entry(*args, C.byref(icp), icp_res.ctypes.data_as(C.POINTER(IcpResult)))
         if rc not in (0, TZR_ERR_TOO_LARGE):
             self._ck(rc)
         corr = [c[:k].copy() for c, k in zip(corr, cnt)]
@@ -994,16 +1052,40 @@ class Context:
                                    relative_rmse=relative_rmse, single=True)
         return icp_result_dict(res[0]), corr[0]
 
+    def icp_point_to_plane(self, src, dst, dst_normals, max_correspondence_distance, init=None, max_iteration=30,
+                           relative_fitness=1e-6, relative_rmse=1e-6):
+        """tzr_icp_point_to_plane: icp() with point-to-plane updates; dst_normals: (nd,3) or (nd,4) float32 target
+        normals (e.g. estimate_normals(dst)), used as given.  Returns what icp() returns."""
+        res, corr = self.icp_point_to_plane_batch([src], [dst], [dst_normals], max_correspondence_distance,
+                                                  None if init is None else [init], max_iteration=max_iteration,
+                                                  relative_fitness=relative_fitness, relative_rmse=relative_rmse,
+                                                  single=True)
+        return icp_result_dict(res[0]), corr[0]
+
+    def icp_point_to_plane_batch(self, srcs, dsts, dst_normals, max_correspondence_distance, inits=None,
+                                 max_iteration=30, relative_fitness=1e-6, relative_rmse=1e-6, single=False):
+        """tzr_icp_point_to_plane_batch: icp_batch() with point-to-plane updates and one (nd_b,3) or (nd_b,4) normals
+        array per target.  single=True goes through tzr_icp_point_to_plane (B must be 1)."""
+        return self._icp(srcs, dsts, dst_normals, max_correspondence_distance, inits, max_iteration, relative_fitness,
+                         relative_rmse, single)
+
     def icp_batch(self, srcs, dsts, max_correspondence_distance, inits=None, max_iteration=30, relative_fitness=1e-6,
                   relative_rmse=1e-6, single=False):
         """tzr_icp_batch over B (source, target) cloud pairs; inits: B seeds (None = identity for all).  Returns
         (results structured array (B,) of ICP_RESULT_DTYPE, list of B correspondence arrays).  single=True goes through
         tzr_icp (B must be 1)."""
+        return self._icp(srcs, dsts, None, max_correspondence_distance, inits, max_iteration, relative_fitness,
+                         relative_rmse, single)
+
+    def _icp(self, srcs, dsts, normals, max_correspondence_distance, inits, max_iteration, relative_fitness,
+             relative_rmse, single):
+        """icp_batch (normals None) and icp_point_to_plane_batch."""
         S = [_cloud32(a, "icp") for a in srcs]
         D = [_cloud32(a, "icp") for a in dsts]
         B = len(S)
-        if B == 0 or len(D) != B or (inits is not None and len(inits) != B):
-            raise TzrError("icp_batch: one target and one seed per source cloud are required")
+        if B == 0 or len(D) != B or (inits is not None and len(inits) != B) or (normals is not None and len(normals) != B):
+            raise TzrError("icp_batch: one target, one seed (and one normals array) per source cloud are required")
+        N = None if normals is None else [_normals32(a, d.shape[0], "icp_point_to_plane") for a, d in zip(normals, D)]
         p = icp_params(max_correspondence_distance, max_iteration=int(max_iteration),
                        relative_fitness=float(relative_fitness), relative_rmse=float(relative_rmse))
         init = (Similarity * B)(*[similarity(None if inits is None else x) for x in inits or [None] * B])
@@ -1012,14 +1094,18 @@ class Context:
         fp, i32p = C.POINTER(C.c_float), C.POINTER(C.c_int32)
         if single:
             assert B == 1
-            rc = lib().tzr_icp(self._h, C.byref(p), _p(S[0], C.c_float), S[0].shape[0], _p(D[0], C.c_float),
-                               D[0].shape[0], init, res, _p(corr[0], C.c_int32))
+            head = (self._h, C.byref(p), _p(S[0], C.c_float), S[0].shape[0], _p(D[0], C.c_float), D[0].shape[0])
+            tail = (init, res, _p(corr[0], C.c_int32))
+            rc = lib().tzr_icp(*head, *tail) if N is None else \
+                lib().tzr_icp_point_to_plane(*head, _p(N[0], C.c_float), *tail)
         else:
             ns = np.array([a.shape[0] for a in S], dtype=np.int32)
             nd = np.array([a.shape[0] for a in D], dtype=np.int32)
-            rc = lib().tzr_icp_batch(self._h, C.byref(p), B, _p(ns, C.c_int32), (fp * B)(*[_p(a, C.c_float) for a in S]),
-                                     _p(nd, C.c_int32), (fp * B)(*[_p(a, C.c_float) for a in D]), init, res,
-                                     (i32p * B)(*[_p(c, C.c_int32) for c in corr]))
+            head = (self._h, C.byref(p), B, _p(ns, C.c_int32), (fp * B)(*[_p(a, C.c_float) for a in S]),
+                    _p(nd, C.c_int32), (fp * B)(*[_p(a, C.c_float) for a in D]))
+            tail = (init, res, (i32p * B)(*[_p(c, C.c_int32) for c in corr]))
+            rc = lib().tzr_icp_batch(*head, *tail) if N is None else \
+                lib().tzr_icp_point_to_plane_batch(*head, (fp * B)(*[_p(a, C.c_float) for a in N]), *tail)
         self._ck(rc)
         out = np.frombuffer(bytes(res), dtype=ICP_RESULT_DTYPE).copy()
         return out, [c[:int(r["n_correspondences"])].copy() for c, r in zip(corr, out)]

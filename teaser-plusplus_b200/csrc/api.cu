@@ -967,13 +967,21 @@ int solve_ragged_dev(tzr_ctx* ctx, const tzr_params& p, int B, const int32_t* n,
 
 // tzr_compute_fpfh(_batch): B clouds staged back to back in one pinned area, one H2D copy, the batched launches, one
 // D2H copy of [overflow flags | descriptors | normals], then the caller's buffers are filled from the pinned copy.
+// normals_only (tzr_estimate_normals(_batch)): fpfh_out and fpfh_radius are not used, every normals_out[b] is required,
+// the grid is planned with both radii equal to the normal radius, and no descriptor pass runs.
 int fpfh_run(tzr_ctx* ctx, int B, const int32_t* n, const float* const* pts, double normal_radius,
-             double fpfh_radius, float* const* fpfh_out, float* const* normals_out, int32_t* status) {
-  if (!ctx || B < 1 || !n || !pts || !fpfh_out || !(normal_radius > 0) || !(fpfh_radius > 0))
+             double fpfh_radius, float* const* fpfh_out, float* const* normals_out, int32_t* status,
+             bool normals_only = false) {
+  if (normals_only) {
+    fpfh_out = nullptr;
+    fpfh_radius = normal_radius;
+  }
+  if (!ctx || B < 1 || !n || !pts || !(normals_only ? normals_out != nullptr : fpfh_out != nullptr) ||
+      !(normal_radius > 0) || !(fpfh_radius > 0))
     return TZR_ERR_INVALID_ARG;
   bool want_normals = false;
   for (int b = 0; b < B; ++b) {
-    if (n[b] <= 0 || !pts[b] || !fpfh_out[b]) return TZR_ERR_INVALID_ARG;
+    if (n[b] <= 0 || !pts[b] || (normals_only ? !normals_out[b] : !fpfh_out[b])) return TZR_ERR_INVALID_ARG;
     want_normals |= normals_out && normals_out[b];
   }
   std::vector<FpfhCloud> clouds((size_t)B);
@@ -986,7 +994,8 @@ int fpfh_run(tzr_ctx* ctx, int B, const int32_t* n, const float* const* pts, dou
   cudaSetDevice(ctx->device);
   cudaStream_t st = ctx->stream;
   const size_t N = (size_t)plan.N;
-  const size_t pb = N * 12, cb = (size_t)B * sizeof(FpfhCloud), ob = (size_t)B * 4, hb = N * 33 * 4, nb = N * 16;
+  const size_t pb = N * 12, cb = (size_t)B * sizeof(FpfhCloud), ob = (size_t)B * 4, hb = normals_only ? 0 : N * 33 * 4,
+               nb = N * 16;
   const size_t in_bytes = al256(pb) + cb, out_bytes = al256(ob) + al256(hb) + (want_normals ? nb : 0);
   int rc;
   if ((rc = ensure(ctx, ctx->m_in, in_bytes)) != TZR_OK) return rc;
@@ -1007,13 +1016,15 @@ int fpfh_run(tzr_ctx* ctx, int B, const int32_t* n, const float* const* pts, dou
   float* d_fpfh = (float*)(d_out + al256(ob));
   float4* d_normals = (float4*)(d_out + al256(ob) + al256(hb));
   ctx->launches += launch_fpfh(plan, (const float*)d_in, (FpfhCloud*)(d_in + al256(pb)), normal_radius, fpfh_radius,
-                               d_normals, d_spfh, d_fpfh, d_overflow, d_grid, st);
+                               d_normals, normals_only ? nullptr : d_spfh, normals_only ? nullptr : d_fpfh, d_overflow,
+                               d_grid, st);
   if ((rc = check_launch(ctx, "fpfh launch")) != TZR_OK) return rc;
   spans.clear();
   spans.push_back(CopySpan{h_out, h_out, ob});  // the overflow flags stay in the pinned area
   for (int b = 0; b < B; ++b) {
     const size_t lo = (size_t)clouds[b].lo;
-    spans.push_back(CopySpan{fpfh_out[b], h_out + al256(ob) + lo * 33 * 4, (size_t)n[b] * 33 * 4});
+    if (!normals_only)
+      spans.push_back(CopySpan{fpfh_out[b], h_out + al256(ob) + lo * 33 * 4, (size_t)n[b] * 33 * 4});
     if (normals_out && normals_out[b])
       spans.push_back(CopySpan{normals_out[b], h_out + al256(ob) + al256(hb) + lo * 16, (size_t)n[b] * 16});
   }
@@ -2021,6 +2032,16 @@ int tzr_compute_fpfh_batch(tzr_ctx* ctx, int B, const int32_t* n, const float* c
   return fpfh_run(ctx, B, n, pts, normal_search_radius, fpfh_search_radius, fpfh_out, normals_out, status);
 }
 
+int tzr_estimate_normals(tzr_ctx* ctx, const float* pts, int n, double normal_search_radius, float* normals_out) {
+  const int32_t n1 = n;
+  return fpfh_run(ctx, 1, &n1, &pts, normal_search_radius, 0.0, nullptr, &normals_out, nullptr, true);
+}
+
+int tzr_estimate_normals_batch(tzr_ctx* ctx, int B, const int32_t* n, const float* const* pts,
+                               double normal_search_radius, float* const* normals_out, int32_t* status) {
+  return fpfh_run(ctx, B, n, pts, normal_search_radius, 0.0, nullptr, normals_out, status, true);
+}
+
 void tzr_frontend_params_default(tzr_frontend_params* p) {
   if (!p) return;
   p->normal_search_radius = 0.03;  // fpfh.h:39-41
@@ -2059,7 +2080,8 @@ static int register_pairs_run(tzr_ctx* ctx, const tzr_frontend_params* fp, const
                               const int32_t* n, const float* const* pts, int P, const int32_t* pair_clouds,
                               const uint64_t* tuple_seeds, tzr_solution* solutions, int32_t* status,
                               int32_t* problem_index, int64_t* n_corr, int32_t* const* corr, int32_t* const* cliques,
-                              float* global_scale, const tzr_icp_params* icp, tzr_icp_result* icp_results) {
+                              float* global_scale, const tzr_icp_params* icp, tzr_icp_result* icp_results,
+                              int icp_mode = kIcpPointToPoint) {
   if (!ctx || !fp || !params || n_clouds < 1 || !n || !pts || P < 1 || !pair_clouds || !solutions || !status ||
       !n_corr || !(fp->normal_search_radius > 0) || !(fp->fpfh_search_radius > 0))
     return TZR_ERR_INVALID_ARG;
@@ -2126,6 +2148,7 @@ static int register_pairs_run(tzr_ctx* ctx, const tzr_frontend_params* fp, const
       return TZR_ERR_TOO_LARGE;
     }
     iplan.max_iteration = icp->max_iteration;
+    iplan.mode = icp_mode;
     iplan.r2 = r * r;
     iplan.relative_fitness = icp->relative_fitness;
     iplan.relative_rmse = icp->relative_rmse;
@@ -2258,6 +2281,7 @@ static int register_pairs_run(tzr_ctx* ctx, const tzr_frontend_params* fp, const
       pr.c_lo = c_lo;
       pr.m_lo = m_lo;
       pr.tc = b;
+      pr.n_lo = clouds[b].lo;
       const int nc = (n[a] + kIcpChunk - 1) / kIcpChunk;
       for (int c = 0; c < nc; ++c) ((int*)(h + hi_ck))[c_lo + c] = k;
       c_lo += nc;
@@ -2270,7 +2294,8 @@ static int register_pairs_run(tzr_ctx* ctx, const tzr_frontend_params* fp, const
     memcpy(h + hi_cl, iclouds.data(), (size_t)n_clouds * sizeof(FpfhCloud));
     const size_t pb = (size_t)S * sizeof(IcpProb), cb = (size_t)n_clouds * sizeof(FpfhCloud), kb = (size_t)c_lo * 4;
     const size_t o_prob = 0, o_cl = al256(pb), o_ck = o_cl + al256(cb), o_match = o_ck + al256(kb),
-                 o_part = o_match + al256((size_t)m_lo * 4), o_grid = o_part + al256((size_t)c_lo * 9 * 8),
+                 o_part = o_match + al256((size_t)m_lo * 4),
+                 o_grid = o_part + al256((size_t)c_lo * icp_partial_stride(icp_mode) * 8),
                  total = o_grid + iplan.grid.grid_bytes;
     if ((rc = ensure(ctx, ctx->icp, total)) != TZR_OK) return rc;
     char* di = (char*)ctx->icp.p;
@@ -2278,7 +2303,10 @@ static int register_pairs_run(tzr_ctx* ctx, const tzr_frontend_params* fp, const
     CK(cudaMemcpyAsync(di + o_cl, h + hi_cl, cb, cudaMemcpyHostToDevice, st));
     CK(cudaMemcpyAsync(di + o_ck, h + hi_ck, kb, cudaMemcpyHostToDevice, st));
     ctx->launches += launch_icp_seed((IcpProb*)(di + o_prob), S, d_sol, st);
-    ctx->launches += launch_icp(iplan, d_pts, d_pts, (IcpProb*)(di + o_prob), (FpfhCloud*)(di + o_cl),
+    // point-to-plane: the target normals are the FPFH stage's (normal_search_radius, viewpoint at the origin), still
+    // in m_out: nothing after the FPFH stage writes that region, and they share the cloud table's indexing
+    ctx->launches += launch_icp(iplan, d_pts, d_pts, (const float4*)(d_out + o_nrm), (IcpProb*)(di + o_prob),
+                                (FpfhCloud*)(di + o_cl),
                                 (const int*)(di + o_ck), (int*)(di + o_match), (double*)(di + o_part),
                                 iplan.grid.grid_bytes ? di + o_grid : nullptr, st);
     if ((rc = check_launch(ctx, "icp launch")) != TZR_OK) return rc;
@@ -2340,6 +2368,18 @@ int tzr_register_cloud_pairs_icp(tzr_ctx* ctx, const tzr_frontend_params* fp, co
                             problem_index, n_corr, corr, cliques, global_scale, icp, icp_results);
 }
 
+int tzr_register_cloud_pairs_icp_point_to_plane(tzr_ctx* ctx, const tzr_frontend_params* fp, const tzr_params* params,
+                                                int n_clouds, const int32_t* n, const float* const* pts, int P,
+                                                const int32_t* pair_clouds, const uint64_t* tuple_seeds,
+                                                tzr_solution* solutions, int32_t* status, int32_t* problem_index,
+                                                int64_t* n_corr, int32_t* const* corr, int32_t* const* cliques,
+                                                float* global_scale, const tzr_icp_params* icp,
+                                                tzr_icp_result* icp_results) {
+  if (!icp) return TZR_ERR_INVALID_ARG;
+  return register_pairs_run(ctx, fp, params, n_clouds, n, pts, P, pair_clouds, tuple_seeds, solutions, status,
+                            problem_index, n_corr, corr, cliques, global_scale, icp, icp_results, kIcpPointToPlane);
+}
+
 void tzr_icp_params_default(tzr_icp_params* p) {
   if (!p) return;
   memset(p, 0, sizeof(*p));
@@ -2349,18 +2389,22 @@ void tzr_icp_params_default(tzr_icp_params* p) {
   p->max_iteration = 30;
 }
 
-// tzr_icp(_batch): sources and targets staged back to back, one H2D copy, every iteration enqueued (launch_icp), one
-// D2H copy of the problem table (and of the per-point matches when correspondences are asked for).
-int tzr_icp_batch(tzr_ctx* ctx, const tzr_icp_params* params, int B, const int32_t* ns, const float* const* src,
-                  const int32_t* nd, const float* const* dst, const tzr_similarity* init, tzr_icp_result* results,
-                  int32_t* const* corr) {
-  if (!ctx || !icp_params_ok(params) || B < 1 || !ns || !src || !nd || !dst || !init || !results)
+// tzr_icp(_batch) and tzr_icp_point_to_plane(_batch): sources, targets (and target normals) staged back to back, one
+// H2D copy, every iteration enqueued (launch_icp), one D2H copy of the problem table (and of the per-point matches when
+// correspondences are asked for).  dst_normals: required for kIcpPointToPlane, unused otherwise.
+static int icp_batch_run(tzr_ctx* ctx, const tzr_icp_params* params, int mode, int B, const int32_t* ns,
+                         const float* const* src, const int32_t* nd, const float* const* dst,
+                         const float* const* dst_normals, const tzr_similarity* init, tzr_icp_result* results,
+                         int32_t* const* corr) {
+  const bool plane = mode == kIcpPointToPlane;
+  if (!ctx || !icp_params_ok(params) || B < 1 || !ns || !src || !nd || !dst || (plane && !dst_normals) || !init ||
+      !results)
     return TZR_ERR_INVALID_ARG;
   const double r = params->max_correspondence_distance;
   long long NS = 0, ND = 0, chunks = 0;
   bool want_corr = false;
   for (int b = 0; b < B; ++b) {
-    if (ns[b] < 1 || nd[b] < 1 || !src[b] || !dst[b]) return TZR_ERR_INVALID_ARG;
+    if (ns[b] < 1 || nd[b] < 1 || !src[b] || !dst[b] || (plane && !dst_normals[b])) return TZR_ERR_INVALID_ARG;
     const tzr_similarity& s = init[b];
     bool finite = std::isfinite(s.scale) && s.scale > 0;
     for (int k = 0; k < 9; ++k) finite &= std::isfinite(s.rotation[k]) != 0;
@@ -2381,6 +2425,7 @@ int tzr_icp_batch(tzr_ctx* ctx, const tzr_icp_params* params, int B, const int32
   plan.ND = (int)ND;
   plan.chunks = (int)chunks;
   plan.max_iteration = params->max_iteration;
+  plan.mode = mode;
   plan.r2 = r * r;
   plan.relative_fitness = params->relative_fitness;
   plan.relative_rmse = params->relative_rmse;
@@ -2404,6 +2449,7 @@ int tzr_icp_batch(tzr_ctx* ctx, const tzr_icp_params* params, int B, const int32
       pr.c_lo = c_lo;
       pr.m_lo = s_lo;
       pr.tc = b;
+      pr.n_lo = clouds[b].lo;
       pr.active = pr.seeded = 1;
       pr.s = init[b].scale;
       for (int k = 0; k < 9; ++k) pr.R[k] = init[b].rotation[k];
@@ -2416,25 +2462,29 @@ int tzr_icp_batch(tzr_ctx* ctx, const tzr_icp_params* params, int B, const int32
   }
   cudaSetDevice(ctx->device);
   cudaStream_t st = ctx->stream;
+  // [sources | targets | problems | target clouds | chunk table | (target normals)] staged, then the matches, the
+  // partials and the grid scratch
   const size_t sb = (size_t)NS * 12, db = (size_t)ND * 12, pb = (size_t)B * sizeof(IcpProb),
                cb = (size_t)B * sizeof(FpfhCloud), kb = (size_t)chunks * 4, mb = (size_t)NS * 4,
-               hb = (size_t)chunks * 9 * 8;
+               hb = (size_t)chunks * icp_partial_stride(mode) * 8, nb = plane ? (size_t)ND * 16 : 0;
   const size_t o_dst = al256(sb), o_prob = o_dst + al256(db), o_cl = o_prob + al256(pb), o_ck = o_cl + al256(cb),
-               in_bytes = o_ck + kb, o_match = al256(in_bytes), o_part = o_match + al256(mb),
-               o_grid = o_part + al256(hb), total = o_grid + plan.grid.grid_bytes;
+               o_nrm = o_ck + al256(kb), in_bytes = plane ? o_nrm + nb : o_ck + kb, o_match = al256(in_bytes),
+               o_part = o_match + al256(mb), o_grid = o_part + al256(hb), total = o_grid + plan.grid.grid_bytes;
   int rc;
   if ((rc = ensure(ctx, ctx->icp, total)) != TZR_OK) return rc;
   std::vector<char> h(in_bytes);
   for (int b = 0; b < B; ++b) {
     memcpy(h.data() + (size_t)probs[b].s_lo * 12, src[b], (size_t)ns[b] * 12);
     memcpy(h.data() + o_dst + (size_t)probs[b].d_lo * 12, dst[b], (size_t)nd[b] * 12);
+    if (plane) memcpy(h.data() + o_nrm + (size_t)probs[b].n_lo * 16, dst_normals[b], (size_t)nd[b] * 16);
   }
   memcpy(h.data() + o_prob, probs.data(), pb);
   memcpy(h.data() + o_cl, clouds.data(), cb);
   memcpy(h.data() + o_ck, chunk_prob.data(), kb);
   char* d = (char*)ctx->icp.p;
   CK(cudaMemcpyAsync(d, h.data(), in_bytes, cudaMemcpyHostToDevice, st));
-  ctx->launches += launch_icp(plan, (const float*)d, (const float*)(d + o_dst), (IcpProb*)(d + o_prob),
+  ctx->launches += launch_icp(plan, (const float*)d, (const float*)(d + o_dst),
+                              plane ? (const float4*)(d + o_nrm) : nullptr, (IcpProb*)(d + o_prob),
                               (FpfhCloud*)(d + o_cl), (const int*)(d + o_ck), (int*)(d + o_match),
                               (double*)(d + o_part), plan.grid.grid_bytes ? d + o_grid : nullptr, st);
   if ((rc = check_launch(ctx, "icp launch")) != TZR_OK) return rc;
@@ -2460,8 +2510,23 @@ int tzr_icp_batch(tzr_ctx* ctx, const tzr_icp_params* params, int B, const int32
   return TZR_OK;
 }
 
-int tzr_icp(tzr_ctx* ctx, const tzr_icp_params* params, const float* src, int ns, const float* dst, int nd,
-            const tzr_similarity* init, tzr_icp_result* result, int32_t* corr) {
+int tzr_icp_batch(tzr_ctx* ctx, const tzr_icp_params* params, int B, const int32_t* ns, const float* const* src,
+                  const int32_t* nd, const float* const* dst, const tzr_similarity* init, tzr_icp_result* results,
+                  int32_t* const* corr) {
+  return icp_batch_run(ctx, params, kIcpPointToPoint, B, ns, src, nd, dst, nullptr, init, results, corr);
+}
+
+int tzr_icp_point_to_plane_batch(tzr_ctx* ctx, const tzr_icp_params* params, int B, const int32_t* ns,
+                                 const float* const* src, const int32_t* nd, const float* const* dst,
+                                 const float* const* dst_normals, const tzr_similarity* init,
+                                 tzr_icp_result* results, int32_t* const* corr) {
+  return icp_batch_run(ctx, params, kIcpPointToPlane, B, ns, src, nd, dst, dst_normals, init, results, corr);
+}
+
+// the single-problem entries: icp_batch_run with B = 1 and init NULL meaning the identity
+static int icp_single(tzr_ctx* ctx, const tzr_icp_params* params, int mode, const float* src, int ns, const float* dst,
+                      int nd, const float* dst_normals, const tzr_similarity* init, tzr_icp_result* result,
+                      int32_t* corr) {
   tzr_similarity id;
   if (!init) {
     memset(&id, 0, sizeof(id));
@@ -2470,7 +2535,19 @@ int tzr_icp(tzr_ctx* ctx, const tzr_icp_params* params, const float* src, int ns
     init = &id;
   }
   int32_t* const corrs[1] = {corr};
-  return tzr_icp_batch(ctx, params, 1, &ns, &src, &nd, &dst, init, result, corr ? corrs : nullptr);
+  return icp_batch_run(ctx, params, mode, 1, &ns, &src, &nd, &dst, dst_normals ? &dst_normals : nullptr, init, result,
+                       corr ? corrs : nullptr);
+}
+
+int tzr_icp(tzr_ctx* ctx, const tzr_icp_params* params, const float* src, int ns, const float* dst, int nd,
+            const tzr_similarity* init, tzr_icp_result* result, int32_t* corr) {
+  return icp_single(ctx, params, kIcpPointToPoint, src, ns, dst, nd, nullptr, init, result, corr);
+}
+
+int tzr_icp_point_to_plane(tzr_ctx* ctx, const tzr_icp_params* params, const float* src, int ns, const float* dst,
+                           int nd, const float* dst_normals, const tzr_similarity* init, tzr_icp_result* result,
+                           int32_t* corr) {
+  return icp_single(ctx, params, kIcpPointToPlane, src, ns, dst, nd, dst_normals, init, result, corr);
 }
 
 // tzr_voxel_downsample(_batch): the clouds staged back to back (one H2D copy), the batch's launches (launch_voxel), a

@@ -698,6 +698,7 @@ int launch_fpfh(const FpfhPlan& plan, const float* pts, FpfhCloud* clouds, doubl
   Clouds cs{pts, clouds, B, nullptr, nullptr, nullptr};
   if (plan.any_grid) nl += launch_fpfh_grid(plan, pts, clouds, grid_scratch, st, &cs.sorted, &cs.bstart, &cs.bend);
   normals_kernel<<<N, kFpfhThreads, 0, st>>>(cs, r2n, normals, overflow);
+  if (!out) return nl + 1;  // normals only
   spfh_kernel<<<N, kFpfhThreads, 0, st>>>(cs, normals, r2f, spfh, overflow);
   fpfh_kernel<<<N, kFpfhThreads, 0, st>>>(cs, spfh, r2f, out, overflow);
   return nl + 3;

@@ -1,6 +1,8 @@
 // Point-to-point ICP (the refinement step of the reference's FPFH + TEASER++ + ICP tutorial, DESIGN.md §3.11): Open3D's
 // RegistrationICP with TransformationEstimationPointToPoint and ICPConvergenceCriteria, written out as this project's
-// own definition in include/teaser_b200.h, for B problems at once.
+// own definition in include/teaser_b200.h, for B problems at once.  Point-to-plane ICP (DESIGN.md §3.13) shares the
+// search, the evaluation and the loop, and replaces the covariance and update pair with icp_plane_system_kernel (the
+// centred 6 x 6 Gauss-Newton system) and icp_plane_update_kernel (its pivoted solve and the Euler rotation).
 //
 //   icp_nn_kernel      one CTA per chunk of kIcpChunk source points: p = s (R x) + t in float64 (icp_transform), the
 //                      nearest target with d^2 < r^2 (lowest index among equal d^2), by brute force through shared
@@ -69,16 +71,17 @@ __device__ void icp_block_sum(double (&v)[K], double* s_buf /* (kIcpThreads/32) 
   }
 }
 
-// Fixed-order sum of the problem's nc chunk partials (K of the 9 doubles each) over one warp: lane l takes chunks l,
-// l + 32, ..., then a butterfly; every lane returns the same bits.
-template <int K>
+// Fixed-order sum of the problem's nc chunk partials (K of the S doubles each: S = 9 for the nearest-neighbour sums and
+// the covariance, 27 for the point-to-plane system) over one warp: lane l takes chunks l, l + 32, ..., then a
+// butterfly; every lane returns the same bits.
+template <int K, int S = 9>
 __device__ void icp_warp_combine(const double* __restrict__ partial, int c_lo, int nc, double (&v)[K]) {
   const int lane = threadIdx.x & 31;
 #pragma unroll
   for (int k = 0; k < K; ++k) v[k] = 0.0;
   for (int c = lane; c < nc; c += 32)
 #pragma unroll
-    for (int k = 0; k < K; ++k) v[k] += partial[9 * (size_t)(c_lo + c) + k];
+    for (int k = 0; k < K; ++k) v[k] += partial[S * (size_t)(c_lo + c) + k];
 #pragma unroll
   for (int k = 0; k < K; ++k)
     for (int o = 16; o; o >>= 1) v[k] += __shfl_xor_sync(0xffffffffu, v[k], o);
@@ -231,6 +234,19 @@ __global__ void __launch_bounds__(kIcpThreads) icp_cov_kernel(IcpArgs a) {
   icp_block_sum<9>(h, s_buf, a.partial + 9 * (size_t)c);
 }
 
+// R <- Ru R, t <- Ru t + tu, and one more iteration (both update kernels)
+__device__ __forceinline__ void icp_compose(IcpProb& pr, const M3& Ru, const double tu[3]) {
+  double R[9], t[3];
+  for (int r = 0; r < 3; ++r) {
+    for (int cc = 0; cc < 3; ++cc)
+      R[3 * cc + r] = (Ru(r, 0) * pr.R[3 * cc] + Ru(r, 1) * pr.R[3 * cc + 1]) + Ru(r, 2) * pr.R[3 * cc + 2];
+    t[r] = ((Ru(r, 0) * pr.t[0] + Ru(r, 1) * pr.t[1]) + Ru(r, 2) * pr.t[2]) + tu[r];
+  }
+  for (int k = 0; k < 9; ++k) pr.R[k] = R[k];
+  for (int k = 0; k < 3; ++k) pr.t[k] = t[k];
+  pr.iterations += 1;
+}
+
 __global__ void icp_update_kernel(IcpArgs a) {
   IcpProb& pr = a.probs[blockIdx.x];
   if (!pr.active) return;
@@ -249,16 +265,134 @@ __global__ void icp_update_kernel(IcpArgs a) {
   } else if (pr.count > 0) {
     for (int r = 0; r < 3; ++r) tu[r] = pr.muq[r] - pr.mup[r];
   }
-  // R <- Ru R, t <- Ru t + tu
-  double R[9], t[3];
-  for (int r = 0; r < 3; ++r) {
-    for (int cc = 0; cc < 3; ++cc)
-      R[3 * cc + r] = (Ru(r, 0) * pr.R[3 * cc] + Ru(r, 1) * pr.R[3 * cc + 1]) + Ru(r, 2) * pr.R[3 * cc + 2];
-    t[r] = ((Ru(r, 0) * pr.t[0] + Ru(r, 1) * pr.t[1]) + Ru(r, 2) * pr.t[2]) + tu[r];
+  icp_compose(pr, Ru, tu);
+}
+
+// ---- point-to-plane (DESIGN.md §3.13) ----------------------------------------------------------------------------------
+// One CTA per chunk: each correspondence (i, j) whose target normal n has three finite components adds J J^T (the 21
+// entries of the upper triangle, row by row) and J r (6), with u = p - c (c = mu_p of the current correspondences),
+// J = (u x n, n) and r = ((p0 - q0) n0 + (p1 - q1) n1) + (p2 - q2) n2.  Flipping n negates J and r exactly, so the sums do
+// not depend on the normal's sign.  The partials of this pass use 27 doubles per chunk; the nearest-neighbour pass that
+// follows writes its 8 sums over them with stride 9 only after the update has read them.
+__global__ void __launch_bounds__(kIcpThreads) icp_plane_system_kernel(IcpArgs a, const float4* __restrict__ normals) {
+  __shared__ double s_buf[(kIcpThreads / 32) * kIcpPlaneSums];
+  const int c = blockIdx.x;
+  const int b = a.chunk_prob[c];
+  const IcpProb& pr = a.probs[b];
+  if (!pr.active || pr.count == 0) return;  // the update of no correspondence reads no system
+  const int i = (c - pr.c_lo) * kIcpChunk + threadIdx.x;
+  double v[kIcpPlaneSums];
+#pragma unroll
+  for (int k = 0; k < kIcpPlaneSums; ++k) v[k] = 0.0;
+  const int j = i < pr.ns ? a.match[pr.m_lo + i] : -1;
+  if (j >= 0) {
+    const float4 nf = normals[pr.n_lo + j];
+    const double n[3] = {nf.x, nf.y, nf.z};
+    if (isfinite(n[0]) && isfinite(n[1]) && isfinite(n[2])) {
+      double p[3];
+      icp_transform(pr, a.src, pr.s_lo + i, p);
+      const size_t o = 3 * (size_t)(pr.d_lo + j);
+      const double u[3] = {p[0] - pr.mup[0], p[1] - pr.mup[1], p[2] - pr.mup[2]};
+      const double J[6] = {u[1] * n[2] - u[2] * n[1], u[2] * n[0] - u[0] * n[2], u[0] * n[1] - u[1] * n[0],
+                           n[0], n[1], n[2]};
+      const double r = ((p[0] - (double)a.dst[o]) * n[0] + (p[1] - (double)a.dst[o + 1]) * n[1]) +
+                       (p[2] - (double)a.dst[o + 2]) * n[2];
+      int k = 0;
+#pragma unroll
+      for (int row = 0; row < 6; ++row)
+#pragma unroll
+        for (int col = row; col < 6; ++col) v[k++] = J[row] * J[col];
+#pragma unroll
+      for (int row = 0; row < 6; ++row) v[21 + row] = J[row] * r;
+    }
   }
-  for (int k = 0; k < 9; ++k) pr.R[k] = R[k];
-  for (int k = 0; k < 3; ++k) pr.t[k] = t[k];
-  pr.iterations += 1;
+  icp_block_sum<kIcpPlaneSums>(v, s_buf, a.partial + kIcpPlaneSums * (size_t)c);
+}
+
+// x with A x = -g by the truncated, diagonally pivoted LDL^T of include/teaser_b200.h (one thread).  A: the 21 entries of
+// the upper triangle row by row.  tol = 1e-10 max_k A_kk; step k takes the remaining index with the largest current
+// diagonal (a NaN diagonal is never the largest; the lowest index on ties) and stops unless that diagonal is > tol;
+// every component not reached is 0.
+__device__ void icp_solve6(const double* __restrict__ Aup, const double* __restrict__ g, double x[6]) {
+  double S[6][6];
+  int k = 0;
+  for (int r = 0; r < 6; ++r)
+    for (int c = r; c < 6; ++c) S[r][c] = S[c][r] = Aup[k++];
+  double amax = S[0][0];
+  for (int r = 1; r < 6; ++r) amax = fmax(amax, S[r][r]);
+  const double tol = 1e-10 * amax;
+  int piv[6];
+  bool used[6] = {false, false, false, false, false, false};
+  double d[6], L[6][6];  // L[i][s]: multiplier of original index i at step s
+  int rank = 0;
+  for (int s = 0; s < 6; ++s) {
+    int best = -1;
+    for (int i = 0; i < 6; ++i)
+      if (!used[i] && (best < 0 || S[i][i] > S[best][best] || (S[best][best] != S[best][best] && S[i][i] == S[i][i])))
+        best = i;
+    if (!(S[best][best] > tol)) break;
+    used[best] = true;
+    piv[s] = best;
+    d[s] = S[best][best];
+    rank = s + 1;
+    for (int i = 0; i < 6; ++i)
+      if (!used[i]) L[i][s] = S[i][best] / d[s];
+    for (int i = 0; i < 6; ++i)
+      if (!used[i])
+        for (int c = 0; c < 6; ++c)
+          if (!used[c]) S[i][c] = S[i][c] - L[i][s] * S[best][c];
+  }
+  double y[6];
+  for (int s = 0; s < rank; ++s) {  // L z = -P g, z / d
+    double z = -g[piv[s]];
+    for (int q = 0; q < s; ++q) z = z - L[piv[s]][q] * y[q];
+    y[s] = z;
+  }
+  for (int s = 0; s < rank; ++s) y[s] = y[s] / d[s];
+  for (int s = rank - 1; s >= 0; --s) {  // L^T y = w
+    double z = y[s];
+    for (int q = s + 1; q < rank; ++q) z = z - L[piv[q]][s] * y[q];
+    y[s] = z;
+  }
+  for (int i = 0; i < 6; ++i) x[i] = 0.0;
+  for (int s = 0; s < rank; ++s) x[piv[s]] = y[s];
+}
+
+__global__ void icp_plane_update_kernel(IcpArgs a) {
+  IcpProb& pr = a.probs[blockIdx.x];
+  if (!pr.active) return;
+  const int nc = (pr.ns + kIcpChunk - 1) / kIcpChunk;
+  double v[kIcpPlaneSums];
+  if (pr.count > 0) icp_warp_combine<kIcpPlaneSums, kIcpPlaneSums>(a.partial, pr.c_lo, nc, v);
+  if (threadIdx.x != 0) return;
+  M3 Ru;
+  m3_identity(Ru);
+  double tu[3] = {0.0, 0.0, 0.0};
+  if (pr.count > 0) {
+    double x[6];
+    icp_solve6(v, v + 21, x);
+    bool finite = true;
+    for (int k = 0; k < 6; ++k) finite &= isfinite(x[k]) != 0;
+    if (finite) {
+      // Ru = Rz(x2) Ry(x1) Rx(x0)
+      double sa, ca, sb, cb, sg, cg;
+      sincos(x[0], &sa, &ca);
+      sincos(x[1], &sb, &cb);
+      sincos(x[2], &sg, &cg);
+      Ru(0, 0) = cg * cb;
+      Ru(0, 1) = (cg * sb) * sa - sg * ca;
+      Ru(0, 2) = (cg * sb) * ca + sg * sa;
+      Ru(1, 0) = sg * cb;
+      Ru(1, 1) = (sg * sb) * sa + cg * ca;
+      Ru(1, 2) = (sg * sb) * ca - cg * sa;
+      Ru(2, 0) = -sb;
+      Ru(2, 1) = cb * sa;
+      Ru(2, 2) = cb * ca;
+      for (int r = 0; r < 3; ++r)
+        tu[r] = (pr.mup[r] + x[3 + r]) - ((Ru(r, 0) * pr.mup[0] + Ru(r, 1) * pr.mup[1]) + Ru(r, 2) * pr.mup[2]);
+    }
+  }
+  icp_compose(pr, Ru, tu);
 }
 
 __global__ void icp_seed_kernel(IcpProb* probs, int B, const tzr_solution* __restrict__ sol) {
@@ -283,8 +417,9 @@ int launch_icp_seed(IcpProb* probs, int B, const tzr_solution* sol, cudaStream_t
   return 1;
 }
 
-int launch_icp(const IcpPlan& plan, const float* src, const float* dst, IcpProb* probs, FpfhCloud* clouds,
-               const int* chunk_prob, int* match, double* partial, void* grid_scratch, cudaStream_t st) {
+int launch_icp(const IcpPlan& plan, const float* src, const float* dst, const float4* dst_normals, IcpProb* probs,
+               FpfhCloud* clouds, const int* chunk_prob, int* match, double* partial, void* grid_scratch,
+               cudaStream_t st) {
   int nl = 0;
   IcpArgs a{src, dst, probs, clouds, chunk_prob, match, partial, nullptr, nullptr, nullptr, plan.r2};
   if (plan.grid.any_grid) nl += launch_fpfh_grid(plan.grid, dst, clouds, grid_scratch, st, &a.sorted, &a.bstart, &a.bend);
@@ -292,8 +427,13 @@ int launch_icp(const IcpPlan& plan, const float* src, const float* dst, IcpProb*
   icp_eval_kernel<<<plan.B, 32, 0, st>>>(a, plan.max_iteration, plan.relative_fitness, plan.relative_rmse);
   nl += 2;
   for (int it = 0; it < plan.max_iteration; ++it) {
-    icp_cov_kernel<<<plan.chunks, kIcpThreads, 0, st>>>(a);
-    icp_update_kernel<<<plan.B, 32, 0, st>>>(a);
+    if (plan.mode == kIcpPointToPlane) {
+      icp_plane_system_kernel<<<plan.chunks, kIcpThreads, 0, st>>>(a, dst_normals);
+      icp_plane_update_kernel<<<plan.B, 32, 0, st>>>(a);
+    } else {
+      icp_cov_kernel<<<plan.chunks, kIcpThreads, 0, st>>>(a);
+      icp_update_kernel<<<plan.B, 32, 0, st>>>(a);
+    }
     icp_nn_kernel<<<plan.chunks, kIcpThreads, 0, st>>>(a);
     icp_eval_kernel<<<plan.B, 32, 0, st>>>(a, plan.max_iteration, plan.relative_fitness, plan.relative_rmse);
     nl += 4;

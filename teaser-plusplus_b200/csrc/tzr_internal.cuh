@@ -317,7 +317,10 @@ int fpfh_plan(int B, const int32_t* n, double normal_radius, double fpfh_radius,
 int launch_fpfh_grid(const FpfhPlan& plan, const float* pts, FpfhCloud* clouds, void* grid_scratch, cudaStream_t st,
                      const int** sorted, const int** bstart, const int** bend);
 // pts (plan.N x 3), clouds (device copy of fpfh_plan's table), normals (N float4), spfh (N x 33), out (N x 33),
-// overflow (B ints, zeroed here), grid_scratch (plan.grid_bytes): device pointers.  Returns the launches.
+// overflow (B ints, zeroed here), grid_scratch (plan.grid_bytes): device pointers.  Returns the launches.  Normals only
+// (tzr_estimate_normals): spfh and out nullptr, fpfh_radius unused; the grid build (when some cloud uses it) and the
+// normals pass alone.  The normals do not depend on the plan's cell edge: the neighbour sets are the same at any cell
+// edge of at least the normal radius, and they are sorted by (distance, index) before the covariance is summed.
 int launch_fpfh(const FpfhPlan& plan, const float* pts, FpfhCloud* clouds, double normal_radius, double fpfh_radius,
                 float4* normals, float* spfh, float* out, int* overflow, void* grid_scratch, cudaStream_t st);
 // The descriptor kernels' device functions on their own, one item per thread (device pointers; one launch each).
@@ -418,9 +421,14 @@ int launch_pair_rows(const MatchPlan& plan, const MatchPair* pairs, const int2* 
 int launch_corr_gather(const PairGather* table, int n_entries, int max_count, const int32_t* pairs, const float* pts,
                        int2* corr, double* src, double* dst, cudaStream_t st);
 
-// icp.cu (point-to-point ICP, DESIGN.md §3.11): B problems, sources back to back and targets back to back
+// icp.cu (point-to-point ICP, DESIGN.md §3.11, and point-to-plane ICP, §3.13): B problems, sources back to back and
+// targets back to back
 constexpr int kIcpChunk = 256;    // source points per chunk: the unit of the fixed-order reductions (one CTA each)
 constexpr int kIcpGridMinN = 1024;  // targets from which the nearest-neighbour search goes through the hashed grid
+constexpr int kIcpPointToPoint = 0, kIcpPointToPlane = 1;  // IcpPlan::mode
+constexpr int kIcpPlaneSums = 27;  // doubles per chunk of the point-to-plane system: 21 of J J^T, 6 of J r
+// doubles per chunk of launch_icp's partial buffer (the point-to-point pass sums 9)
+inline int icp_partial_stride(int mode) { return mode == kIcpPointToPlane ? kIcpPlaneSums : 9; }
 struct IcpProb {        // one per problem, device-resident; the host fills the inputs, the kernels the rest
   int s_lo, ns;         // sources: flat points [s_lo, s_lo + ns)
   int d_lo, nd;         // targets: flat points [d_lo, d_lo + nd) (also FpfhCloud b of the target table)
@@ -431,7 +439,7 @@ struct IcpProb {        // one per problem, device-resident; the host fills the 
   int m_lo;             // first entry of the problem in the per-point match array
   int tc;               // its target's entry in the FpfhCloud table of the targets (lo = d_lo)
   int seeded;           // 1: the problem runs (tzr_register_cloud_pairs_icp: 0 for a pair without a valid solution)
-  int pad;
+  int n_lo;             // point-to-plane: the normal of target j is normals[n_lo + j]
   double s;             // fixed scale
   double R[9], t[3];    // current transform (column-major R)
   double fitness, rmse; // evaluation of the current transform
@@ -440,15 +448,19 @@ struct IcpProb {        // one per problem, device-resident; the host fills the 
 struct IcpPlan {
   int B = 0, NS = 0, ND = 0, chunks = 0;
   int max_iteration = 0;
+  int mode = kIcpPointToPoint;
   double r2 = 0, relative_fitness = 0, relative_rmse = 0;
   FpfhPlan grid;        // the target grid (fpfh_plan with both radii = r)
 };
-// src (NS x 3 floats), dst (ND x 3 floats), probs (B), clouds (B, fpfh_plan's table of the targets), chunk_prob
-// (chunks: the problem of every chunk), match (target index or -1 per source point from m_lo, final correspondences),
-// partial (chunks x 9 doubles), grid_scratch (plan.grid.grid_bytes): device pointers.  Enqueues every iteration without
-// synchronising; returns the launches: 4 for the grid build (when some target uses it) + 2 + 4 * max_iteration.
-int launch_icp(const IcpPlan& plan, const float* src, const float* dst, IcpProb* probs, FpfhCloud* clouds,
-               const int* chunk_prob, int* match, double* partial, void* grid_scratch, cudaStream_t st);
+// src (NS x 3 floats), dst (ND x 3 floats), dst_normals (point-to-plane: the target normals, (nx, ny, nz, curvature) per
+// point; unused and may be nullptr for point-to-point), probs (B), clouds (B, fpfh_plan's table of the targets),
+// chunk_prob (chunks: the problem of every chunk), match (target index or -1 per source point from m_lo, final
+// correspondences), partial (chunks x icp_partial_stride(plan.mode) doubles), grid_scratch (plan.grid.grid_bytes): device
+// pointers.  Enqueues every iteration without synchronising; returns the launches: 4 for the grid build (when some target
+// uses it) + 2 + 4 * max_iteration, in either mode.
+int launch_icp(const IcpPlan& plan, const float* src, const float* dst, const float4* dst_normals, IcpProb* probs,
+               FpfhCloud* clouds, const int* chunk_prob, int* match, double* partial, void* grid_scratch,
+               cudaStream_t st);
 // The seeds of B problems from B solution records (tzr_register_cloud_pairs_icp): a valid record with a finite transform
 // and a positive scale sets (s, R, t) and active = seeded = 1, any other leaves the problem inactive.  One launch.
 int launch_icp_seed(IcpProb* probs, int B, const tzr_solution* sol, cudaStream_t st);

@@ -1,11 +1,14 @@
 // teaser::PointToPointICP — the refinement step of the reference's FPFH + TEASER++ + ICP tutorial
 // (examples/teaser_python_fpfh_icp: Open3D's registration_icp with TransformationEstimationPointToPoint), on the GPU
-// through the C-ABI (tzr_icp, tzr_icp_batch; include/teaser_b200.h defines the loop).  No CPU implementation: without a
-// CUDA device the first call throws std::runtime_error.
+// through the C-ABI (tzr_icp, tzr_icp_batch; include/teaser_b200.h defines the loop).  teaser::PointToPlaneICP is the
+// same with TransformationEstimationPointToPlane (tzr_icp_point_to_plane, tzr_icp_point_to_plane_batch), given the
+// target normals (teaser::estimateNormals, teaser/normals.h).  No CPU implementation: without a CUDA device the first
+// call throws std::runtime_error.
 #pragma once
 
 #include <vector>
 
+#include "teaser/fpfh.h"
 #include "teaser/geometry.h"
 #include "teaser/registration.h"
 
@@ -23,6 +26,31 @@ class PointToPointICP {
   Result refine(const PointCloud& src, const PointCloud& dst, const RegistrationSolution& init) const;
   // Many problems in one device call (tzr_icp_batch); result b is refine(src[b], dst[b], init[b]) bit for bit.
   std::vector<Result> refineBatch(const std::vector<PointCloud>& src, const std::vector<PointCloud>& dst,
+                                  const std::vector<RegistrationSolution>& init) const;
+
+  const Params& getParams() const { return params_; }
+  void setParams(const Params& params) { params_ = params; }
+
+ private:
+  Params params_;
+};
+
+class PointToPlaneICP {
+ public:
+  using Params = PointToPointICPParams;
+  using Result = PointToPointICPResult;
+
+  PointToPlaneICP() = default;
+  explicit PointToPlaneICP(const Params& params) : params_(params) {}
+
+  // Point-to-plane ICP of src onto dst seeded with init (its scale held fixed), on this thread's context.  dst_normals:
+  // one normal per target point (curvature ignored; used as given, their signs do not matter).  Both clouds non-empty.
+  Result refine(const PointCloud& src, const PointCloud& dst, const NormalCloud& dst_normals,
+                const RegistrationSolution& init) const;
+  // Many problems in one device call (tzr_icp_point_to_plane_batch); result b is refine(src[b], dst[b],
+  // dst_normals[b], init[b]) bit for bit.
+  std::vector<Result> refineBatch(const std::vector<PointCloud>& src, const std::vector<PointCloud>& dst,
+                                  const std::vector<NormalCloud>& dst_normals,
                                   const std::vector<RegistrationSolution>& init) const;
 
   const Params& getParams() const { return params_; }

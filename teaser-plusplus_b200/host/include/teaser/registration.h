@@ -334,6 +334,13 @@ class RobustRegistrationSolver {
   std::vector<CloudPairICPResult> solveCloudPairs(const std::vector<PointCloud>& clouds,
                                                   const std::vector<std::pair<int, int>>& pairs,
                                                   const CloudPairParams& params, const PointToPointICPParams& icp);
+  // The overload above with point-to-plane ICP (tzr_register_cloud_pairs_icp_point_to_plane): each target cloud's
+  // normals are the ones the call's FPFH stage computed at params.normal_search_radius (PointToPlaneICP's parameters
+  // are PointToPointICP's).
+  std::vector<CloudPairICPResult> solveCloudPairsPointToPlane(const std::vector<PointCloud>& clouds,
+                                                              const std::vector<std::pair<int, int>>& pairs,
+                                                              const CloudPairParams& params,
+                                                              const PointToPointICPParams& icp);
   bool isMaxCliqueProvenOptimal() const { return clique_proven_; }
   long long getNumInlierGraphEdges() const { return n_edges_; }
   int getGNCRotationIterations() const { return gnc_iterations_; }

@@ -12,6 +12,7 @@
 
 #include "teaser/certification.h"
 #include "teaser/icp.h"
+#include "teaser/normals.h"
 #include "teaser/registration.h"
 #include "teaser/voxel.h"
 
@@ -71,6 +72,24 @@ py::array_t<float> cloud_to_numpy(const teaser::PointCloud& pc) {
     d[3 * i + 1] = pc[i].y;
     d[3 * i + 2] = pc[i].z;
   }
+  return out;
+}
+
+// (n,3) or (n,4) float normals (a fourth column is the curvature, which ICP ignores)
+teaser::NormalCloud normals_of(const CloudArray& a) {
+  if (a.ndim() != 2 || (a.shape(1) != 3 && a.shape(1) != 4))
+    throw std::invalid_argument("normals must be (n,3) or (n,4) arrays");
+  const py::ssize_t w = a.shape(1);
+  teaser::NormalCloud nc(static_cast<size_t>(a.shape(0)));
+  const float* d = a.data();
+  for (py::ssize_t i = 0; i < a.shape(0); ++i)
+    nc[i] = {d[w * i], d[w * i + 1], d[w * i + 2], w == 4 ? d[w * i + 3] : 0.f};
+  return nc;
+}
+
+py::array_t<float> normals_to_numpy(const teaser::NormalCloud& nc) {
+  py::array_t<float> out({static_cast<py::ssize_t>(nc.size()), static_cast<py::ssize_t>(4)});
+  if (!nc.empty()) std::memcpy(out.mutable_data(), &nc[0].normal_x, sizeof(float) * 4 * nc.size());
   return out;
 }
 
@@ -153,6 +172,78 @@ PYBIND11_MODULE(_teaserpp, m) {
              return out;
            },
            py::arg("src"), py::arg("dst"), py::arg("init"));
+
+  // GPU extra: point-to-plane ICP (teaser::PointToPlaneICP), given the target normals
+  py::class_<teaser::PointToPlaneICP>(m, "PointToPlaneICP")
+      .def(py::init([](double max_correspondence_distance, int max_iteration, double relative_fitness,
+                       double relative_rmse) {
+             teaser::PointToPlaneICP::Params p;
+             p.max_correspondence_distance = max_correspondence_distance;
+             p.max_iteration = max_iteration;
+             p.relative_fitness = relative_fitness;
+             p.relative_rmse = relative_rmse;
+             return teaser::PointToPlaneICP(p);
+           }),
+           py::arg("max_correspondence_distance"), py::arg("max_iteration") = 30, py::arg("relative_fitness") = 1e-6,
+           py::arg("relative_rmse") = 1e-6)
+      .def("refine",
+           [](const teaser::PointToPlaneICP& icp, const CloudArray& src, const CloudArray& dst,
+              const CloudArray& dst_normals, const teaser::RegistrationSolution& init) {
+             const teaser::PointCloud s = cloud_of(src), d = cloud_of(dst);
+             const teaser::NormalCloud n = normals_of(dst_normals);
+             teaser::PointToPlaneICP::Result r;
+             {
+               py::gil_scoped_release release;
+               r = icp.refine(s, d, n, init);
+             }
+             return icp_dict(r);
+           },
+           py::arg("src"), py::arg("dst"), py::arg("dst_normals"), py::arg("init"))
+      .def("refine_batch",
+           [](const teaser::PointToPlaneICP& icp, const std::vector<CloudArray>& src, const std::vector<CloudArray>& dst,
+              const std::vector<CloudArray>& dst_normals, const std::vector<teaser::RegistrationSolution>& init) {
+             std::vector<teaser::PointCloud> s, d;
+             std::vector<teaser::NormalCloud> n;
+             for (const auto& a : src) s.push_back(cloud_of(a));
+             for (const auto& a : dst) d.push_back(cloud_of(a));
+             for (const auto& a : dst_normals) n.push_back(normals_of(a));
+             std::vector<teaser::PointToPlaneICP::Result> res;
+             {
+               py::gil_scoped_release release;
+               res = icp.refineBatch(s, d, n, init);
+             }
+             py::list out;
+             for (const auto& r : res) out.append(icp_dict(r));
+             return out;
+           },
+           py::arg("src"), py::arg("dst"), py::arg("dst_normals"), py::arg("init"));
+
+  // GPU extra: FPFHEstimation's normals alone (teaser::estimateNormals), as (n,4) float32 (nx, ny, nz, curvature)
+  m.def("estimate_normals",
+        [](const CloudArray& points, double normal_search_radius) {
+          const teaser::PointCloud pc = cloud_of(points);
+          teaser::NormalCloud out;
+          {
+            py::gil_scoped_release release;
+            out = teaser::estimateNormals(pc, normal_search_radius);
+          }
+          return normals_to_numpy(out);
+        },
+        py::arg("points"), py::arg("normal_search_radius") = 0.03);
+  m.def("estimate_normals_batch",
+        [](const std::vector<CloudArray>& points, double normal_search_radius) {
+          std::vector<teaser::PointCloud> pcs;
+          for (const auto& a : points) pcs.push_back(cloud_of(a));
+          std::vector<teaser::NormalCloud> res;
+          {
+            py::gil_scoped_release release;
+            res = teaser::estimateNormalsBatch(pcs, normal_search_radius);
+          }
+          py::list out;
+          for (const auto& nc : res) out.append(normals_to_numpy(nc));
+          return out;
+        },
+        py::arg("points"), py::arg("normal_search_radius") = 0.03);
 
   // GPU extra: the first step of the same tutorial, Open3D's voxel_down_sample (teaser::voxelDownSample)
   m.def("voxel_down_sample",
@@ -294,8 +385,11 @@ PYBIND11_MODULE(_teaserpp, m) {
            [](Solver& s, const std::vector<CloudArray>& clouds, const std::vector<std::pair<int, int>>& pairs,
               double max_correspondence_distance, int max_iteration, double relative_fitness, double relative_rmse,
               double normal_search_radius, double fpfh_search_radius, bool use_absolute_scale, bool use_crosscheck,
-              bool use_tuple_test, float tuple_scale, uint64_t tuple_seed) {
-             // GPU extra: solve_cloud_pairs, then point-to-point ICP of every pair with a valid solution, in one call
+              bool use_tuple_test, float tuple_scale, uint64_t tuple_seed, const std::string& method) {
+             // GPU extra: solve_cloud_pairs, then point-to-point (or point-to-plane) ICP of every pair with a valid
+             // solution, in one call
+             if (method != "point_to_point" && method != "point_to_plane")
+               throw std::invalid_argument("method must be \"point_to_point\" or \"point_to_plane\"");
              std::vector<teaser::PointCloud> pcs;
              for (const auto& a : clouds) pcs.push_back(cloud_of(a));
              Solver::CloudPairParams cp;
@@ -314,7 +408,8 @@ PYBIND11_MODULE(_teaserpp, m) {
              std::vector<Solver::CloudPairICPResult> res;
              {
                py::gil_scoped_release release;
-               res = s.solveCloudPairs(pcs, pairs, cp, ip);
+               res = method == "point_to_plane" ? s.solveCloudPairsPointToPlane(pcs, pairs, cp, ip)
+                                                : s.solveCloudPairs(pcs, pairs, cp, ip);
              }
              py::list out;
              for (const auto& r : res)
@@ -327,7 +422,8 @@ PYBIND11_MODULE(_teaserpp, m) {
            py::arg("clouds"), py::arg("pairs"), py::arg("max_correspondence_distance"), py::arg("max_iteration") = 30,
            py::arg("relative_fitness") = 1e-6, py::arg("relative_rmse") = 1e-6, py::arg("normal_search_radius") = 0.03,
            py::arg("fpfh_search_radius") = 0.05, py::arg("use_absolute_scale") = true, py::arg("use_crosscheck") = true,
-           py::arg("use_tuple_test") = true, py::arg("tuple_scale") = 0.0f, py::arg("tuple_seed") = 0x7ea5e2ull)
+           py::arg("use_tuple_test") = true, py::arg("tuple_scale") = 0.0f, py::arg("tuple_seed") = 0x7ea5e2ull,
+           py::arg("method") = "point_to_point")
       .def_property_readonly("solution", &Solver::getSolution)
       .def("getSolution", &Solver::getSolution)
       .def_property_readonly("gnc_rotation_cost_at_termination", &Solver::getGNCRotationCostAtTermination)

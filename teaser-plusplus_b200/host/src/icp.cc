@@ -1,4 +1,5 @@
-// teaser::PointToPointICP (teaser/icp.h) on top of the C-ABI: marshalling only, the loop runs in libteaser_b200.so.
+// teaser::PointToPointICP and teaser::PointToPlaneICP (teaser/icp.h) on top of the C-ABI: marshalling only, the loop
+// runs in libteaser_b200.so.
 #include "teaser/icp.h"
 
 #include <cstring>
@@ -48,6 +49,62 @@ void icp_result_from_c(const tzr_icp_result& r, const int32_t* corr, PointToPoin
     for (int c = 0; c < r.n_correspondences; ++c) out->correspondences.emplace_back(corr[2 * c], corr[2 * c + 1]);
 }
 
+namespace {
+
+// both classes' refineBatch: point-to-point when dst_normals is null
+std::vector<PointToPointICPResult> refine_batch(const char* who, const PointToPointICPParams& params,
+                                                const std::vector<PointCloud>& src, const std::vector<PointCloud>& dst,
+                                                const std::vector<NormalCloud>* dst_normals,
+                                                const std::vector<RegistrationSolution>& init) {
+  const size_t B = src.size();
+  if (dst.size() != B || init.size() != B || (dst_normals && dst_normals->size() != B))
+    throw std::invalid_argument(std::string(who) + ": one target and seed (and normal cloud) per source");
+  std::vector<PointToPointICPResult> out(B);
+  if (B == 0) return out;
+  static_assert(sizeof(PointXYZ) == 3 * sizeof(float), "PointXYZ must be three packed floats");
+  static_assert(sizeof(Normal) == 4 * sizeof(float), "Normal must be 4 packed floats");
+  std::vector<int32_t> ns(B), nd(B);
+  std::vector<const float*> sp(B), dp(B), np(B, nullptr);
+  std::vector<tzr_similarity> seeds(B);
+  std::vector<std::vector<int32_t>> corr(B);
+  std::vector<int32_t*> corr_p(B);
+  for (size_t b = 0; b < B; ++b) {
+    if (src[b].empty() || dst[b].empty()) throw std::invalid_argument(std::string(who) + ": clouds must be non-empty");
+    ns[b] = static_cast<int32_t>(src[b].size());
+    nd[b] = static_cast<int32_t>(dst[b].size());
+    sp[b] = &src[b][0].x;
+    dp[b] = &dst[b][0].x;
+    if (dst_normals) {
+      if ((*dst_normals)[b].size() != dst[b].size())
+        throw std::invalid_argument(std::string(who) + ": one normal per target point");
+      np[b] = &(*dst_normals)[b][0].normal_x;
+    }
+    seeds[b] = to_c(init[b]);
+    corr[b].resize(2 * src[b].size());
+    corr_p[b] = corr[b].data();
+  }
+  const tzr_icp_params p = to_c(params);
+  std::vector<tzr_icp_result> res(B);
+  tzr_ctx* ctx = b200_context();
+  const int Bi = static_cast<int>(B);
+  int rc;
+  if (!dst_normals)
+    rc = B == 1 ? tzr_icp(ctx, &p, sp[0], ns[0], dp[0], nd[0], seeds.data(), res.data(), corr_p[0])
+                : tzr_icp_batch(ctx, &p, Bi, ns.data(), sp.data(), nd.data(), dp.data(), seeds.data(), res.data(),
+                                corr_p.data());
+  else
+    rc = B == 1 ? tzr_icp_point_to_plane(ctx, &p, sp[0], ns[0], dp[0], nd[0], np[0], seeds.data(), res.data(),
+                                         corr_p[0])
+                : tzr_icp_point_to_plane_batch(ctx, &p, Bi, ns.data(), sp.data(), nd.data(), dp.data(), np.data(),
+                                               seeds.data(), res.data(), corr_p.data());
+  if (rc != TZR_OK)
+    throw std::runtime_error(std::string(who) + ": " + tzr_status_string(rc) + " (" + tzr_last_error(ctx) + ")");
+  for (size_t b = 0; b < B; ++b) icp_result_from_c(res[b], corr[b].data(), &out[b]);
+  return out;
+}
+
+}  // namespace
+
 PointToPointICP::Result PointToPointICP::refine(const PointCloud& src, const PointCloud& dst,
                                                 const RegistrationSolution& init) const {
   return refineBatch({src}, {dst}, {init})[0];
@@ -56,36 +113,20 @@ PointToPointICP::Result PointToPointICP::refine(const PointCloud& src, const Poi
 std::vector<PointToPointICP::Result> PointToPointICP::refineBatch(const std::vector<PointCloud>& src,
                                                                   const std::vector<PointCloud>& dst,
                                                                   const std::vector<RegistrationSolution>& init) const {
-  const size_t B = src.size();
-  if (dst.size() != B || init.size() != B) throw std::invalid_argument("PointToPointICP: one target and seed per source");
-  std::vector<Result> out(B);
-  if (B == 0) return out;
-  static_assert(sizeof(PointXYZ) == 3 * sizeof(float), "PointXYZ must be three packed floats");
-  std::vector<int32_t> ns(B), nd(B);
-  std::vector<const float*> sp(B), dp(B);
-  std::vector<tzr_similarity> seeds(B);
-  std::vector<std::vector<int32_t>> corr(B);
-  std::vector<int32_t*> corr_p(B);
-  for (size_t b = 0; b < B; ++b) {
-    if (src[b].empty() || dst[b].empty()) throw std::invalid_argument("PointToPointICP: clouds must be non-empty");
-    ns[b] = static_cast<int32_t>(src[b].size());
-    nd[b] = static_cast<int32_t>(dst[b].size());
-    sp[b] = &src[b][0].x;
-    dp[b] = &dst[b][0].x;
-    seeds[b] = to_c(init[b]);
-    corr[b].resize(2 * src[b].size());
-    corr_p[b] = corr[b].data();
-  }
-  const tzr_icp_params p = to_c(params_);
-  std::vector<tzr_icp_result> res(B);
-  tzr_ctx* ctx = b200_context();
-  const int rc = B == 1 ? tzr_icp(ctx, &p, sp[0], ns[0], dp[0], nd[0], seeds.data(), res.data(), corr_p[0])
-                        : tzr_icp_batch(ctx, &p, static_cast<int>(B), ns.data(), sp.data(), nd.data(), dp.data(),
-                                        seeds.data(), res.data(), corr_p.data());
-  if (rc != TZR_OK)
-    throw std::runtime_error(std::string("PointToPointICP: ") + tzr_status_string(rc) + " (" + tzr_last_error(ctx) + ")");
-  for (size_t b = 0; b < B; ++b) icp_result_from_c(res[b], corr[b].data(), &out[b]);
-  return out;
+  return refine_batch("PointToPointICP", params_, src, dst, nullptr, init);
+}
+
+PointToPlaneICP::Result PointToPlaneICP::refine(const PointCloud& src, const PointCloud& dst,
+                                                const NormalCloud& dst_normals,
+                                                const RegistrationSolution& init) const {
+  return refineBatch({src}, {dst}, {dst_normals}, {init})[0];
+}
+
+std::vector<PointToPlaneICP::Result> PointToPlaneICP::refineBatch(const std::vector<PointCloud>& src,
+                                                                  const std::vector<PointCloud>& dst,
+                                                                  const std::vector<NormalCloud>& dst_normals,
+                                                                  const std::vector<RegistrationSolution>& init) const {
+  return refine_batch("PointToPlaneICP", params_, src, dst, &dst_normals, init);
 }
 
 }  // namespace teaser

@@ -631,12 +631,12 @@ void icp_result_from_c(const tzr_icp_result& r, const int32_t* corr, PointToPoin
 
 namespace {
 
-// solveCloudPairs' body: tzr_register_cloud_pairs, or tzr_register_cloud_pairs_icp when icp is given (icp_res then
-// receives P records)
+// solveCloudPairs' body: tzr_register_cloud_pairs, or tzr_register_cloud_pairs_icp(_point_to_plane) when icp is given
+// (icp_res then receives P records)
 std::vector<RobustRegistrationSolver::CloudPairResult> run_cloud_pairs(
     const tzr_params& p, const std::vector<PointCloud>& clouds, const std::vector<std::pair<int, int>>& pairs,
     const RobustRegistrationSolver::CloudPairParams& cp, const tzr_icp_params* icp,
-    std::vector<tzr_icp_result>* icp_res) {
+    std::vector<tzr_icp_result>* icp_res, bool point_to_plane = false) {
   using CloudPairResult = RobustRegistrationSolver::CloudPairResult;
   const int K = static_cast<int>(clouds.size()), P = static_cast<int>(pairs.size());
   std::vector<CloudPairResult> out(P);
@@ -683,9 +683,9 @@ std::vector<RobustRegistrationSolver::CloudPairResult> run_cloud_pairs(
                                   scales.data());
   } else {
     icp_res->assign(P, tzr_icp_result{});
-    rc = tzr_register_cloud_pairs_icp(ctx, &f, &p, K, n.data(), pts.data(), P, pc.data(), seeds.data(), sols.data(),
-                                      status.data(), index.data(), n_corr.data(), corr_p.data(), clq_p.data(),
-                                      scales.data(), icp, icp_res->data());
+    rc = (point_to_plane ? tzr_register_cloud_pairs_icp_point_to_plane : tzr_register_cloud_pairs_icp)(
+        ctx, &f, &p, K, n.data(), pts.data(), P, pc.data(), seeds.data(), sols.data(), status.data(), index.data(),
+        n_corr.data(), corr_p.data(), clq_p.data(), scales.data(), icp, icp_res->data());
   }
   if (rc != TZR_OK && rc != TZR_ERR_TOO_LARGE) fail("RobustRegistrationSolver::solveCloudPairs", rc, ctx);
   for (int q = 0; q < P; ++q) {
@@ -710,9 +710,12 @@ std::vector<RobustRegistrationSolver::CloudPairResult> RobustRegistrationSolver:
   return run_cloud_pairs(to_c(params_), clouds, pairs, cp, nullptr, nullptr);
 }
 
-std::vector<RobustRegistrationSolver::CloudPairICPResult> RobustRegistrationSolver::solveCloudPairs(
-    const std::vector<PointCloud>& clouds, const std::vector<std::pair<int, int>>& pairs, const CloudPairParams& cp,
-    const PointToPointICPParams& icp) {
+// both ICP overloads of solveCloudPairs
+static std::vector<RobustRegistrationSolver::CloudPairICPResult> run_cloud_pairs_icp(
+    const tzr_params& p, const std::vector<PointCloud>& clouds, const std::vector<std::pair<int, int>>& pairs,
+    const RobustRegistrationSolver::CloudPairParams& cp, const PointToPointICPParams& icp, bool point_to_plane) {
+  using CloudPairResult = RobustRegistrationSolver::CloudPairResult;
+  using CloudPairICPResult = RobustRegistrationSolver::CloudPairICPResult;
   tzr_icp_params ip;
   tzr_icp_params_default(&ip);
   ip.max_correspondence_distance = icp.max_correspondence_distance;
@@ -720,7 +723,7 @@ std::vector<RobustRegistrationSolver::CloudPairICPResult> RobustRegistrationSolv
   ip.relative_fitness = icp.relative_fitness;
   ip.relative_rmse = icp.relative_rmse;
   std::vector<tzr_icp_result> res;
-  std::vector<CloudPairResult> base = run_cloud_pairs(to_c(params_), clouds, pairs, cp, &ip, &res);
+  std::vector<CloudPairResult> base = run_cloud_pairs(p, clouds, pairs, cp, &ip, &res, point_to_plane);
   std::vector<CloudPairICPResult> out(base.size());
   for (size_t q = 0; q < base.size(); ++q) {
     static_cast<CloudPairResult&>(out[q]) = std::move(base[q]);
@@ -729,6 +732,18 @@ std::vector<RobustRegistrationSolver::CloudPairICPResult> RobustRegistrationSolv
     if (out[q].refined) icp_result_from_c(res[q], nullptr, &out[q].icp);
   }
   return out;
+}
+
+std::vector<RobustRegistrationSolver::CloudPairICPResult> RobustRegistrationSolver::solveCloudPairs(
+    const std::vector<PointCloud>& clouds, const std::vector<std::pair<int, int>>& pairs, const CloudPairParams& cp,
+    const PointToPointICPParams& icp) {
+  return run_cloud_pairs_icp(to_c(params_), clouds, pairs, cp, icp, false);
+}
+
+std::vector<RobustRegistrationSolver::CloudPairICPResult> RobustRegistrationSolver::solveCloudPairsPointToPlane(
+    const std::vector<PointCloud>& clouds, const std::vector<std::pair<int, int>>& pairs, const CloudPairParams& cp,
+    const PointToPointICPParams& icp) {
+  return run_cloud_pairs_icp(to_c(params_), clouds, pairs, cp, icp, true);
 }
 
 void RobustRegistrationSolver::materialise_tims() {
