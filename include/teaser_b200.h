@@ -703,8 +703,9 @@ int tzr_solve_batch_multi(const int32_t* devices, int n_devices, const tzr_param
  * and tzr_icp_point_to_plane(_batch)
  * searches every target by brute force, bit 26 (67108864) = through the hashed grid at any target size (a target the
  * grid cannot index still falls back to brute force), so that the two routes can be compared on one input; bit 25 wins
- * when both are set.
- * Bits 15 to 26 change host code only. */
+ * when both are set, bit 27 (134217728) = the default graph kernel's Gram test in its two-slope form on the unscaled float
+ * copies instead of the single-slope form in units of 2 beta (DESIGN.md 3.1; bit-identical; a same-build A/B switch).
+ * Bits 15 to 26 change host code only; bit 27 changes device code. */
 int tzr_ctx_set_flags(tzr_ctx* ctx, uint32_t flags);
 int64_t tzr_ctx_filter_mismatches(tzr_ctx* ctx);
 /* Number of pairs of the most recent graph build that needed the exact FP64 re-check. */

@@ -29,7 +29,7 @@ struct tzr_ctx {
   uint32_t flags = 0;
   int num_sms = 132;
   // device buffers (grow-only)
-  DevBuf src, dst, sf, df, pk, opnd, tclist, gc, adj, deg, nedges, hclq, hsize, clq, L, alive, best_bits, alive_cnt, root_ctr, lock, flg, kfinal, tstart, stack, cv,
+  DevBuf src, dst, sf, df, gq, pk, opnd, tclist, gc, adj, deg, nedges, hclq, hsize, clq, L, alive, best_bits, alive_cnt, root_ctr, lock, flg, kfinal, tstart, stack, cv,
       centry, ps, pd, wgt, res, skey, sidx, sorted, rmask, tmask, sol, dbg, misc, sc, m_in, m_scratch, m_out, cert,
       certb;
   // large clique route (n > kMaxN or debug flag 524288): scratch on the full graph, and the compacted batch's buffers
@@ -277,10 +277,10 @@ int setup_classes(tzr_ctx* ctx, int C, const int* Bs, const int* ns, bool own_po
   ctx->clique_B = 0;
   ctx->route_B = 0;
   // per class: geometry, then the bytes of every buffer (summed over classes, or the largest for the shared ones)
-  enum { kSrc, kDst, kSf, kDf, kPk, kOpnd, kTcl, kGc, kAdj, kDeg, kNe, kHclq, kHsize, kClq, kL, kAlive, kBest, kAcnt,
+  enum { kSrc, kDst, kSf, kDf, kGq, kPk, kOpnd, kTcl, kGc, kAdj, kDeg, kNe, kHclq, kHsize, kClq, kL, kAlive, kBest, kAcnt,
          kRctr, kLock, kFlg, kKfin, kTst, kStack, kCv, kCentry, kPs, kPd, kWgt, kRes, kSkey, kSidx, kSorted, kRmask,
          kTmask, kSol, kDbg, kBufs };
-  DevBuf* bufs[kBufs] = {&ctx->src, &ctx->dst, &ctx->sf, &ctx->df, &ctx->pk, &ctx->opnd, &ctx->tclist, &ctx->gc,
+  DevBuf* bufs[kBufs] = {&ctx->src, &ctx->dst, &ctx->sf, &ctx->df, &ctx->gq, &ctx->pk, &ctx->opnd, &ctx->tclist, &ctx->gc,
                          &ctx->adj, &ctx->deg, &ctx->nedges, &ctx->hclq, &ctx->hsize, &ctx->clq, &ctx->L, &ctx->alive,
                          &ctx->best_bits, &ctx->alive_cnt, &ctx->root_ctr, &ctx->lock, &ctx->flg, &ctx->kfinal,
                          &ctx->tstart, &ctx->stack, &ctx->cv, &ctx->centry, &ctx->ps, &ctx->pd, &ctx->wgt, &ctx->res,
@@ -304,6 +304,7 @@ int setup_classes(tzr_ctx* ctx, int C, const int* Bs, const int* ns, bool own_po
     }
     bytes[kSf] = Bn * sizeof(float4);
     bytes[kDf] = Bn * sizeof(float4);
+    bytes[kGq] = 2 * Bn * sizeof(float4);
     bytes[kPk] = (size_t)B * 6 * npad128(n) * sizeof(float);
     bytes[kOpnd] = tc_operand_bytes(B, n);
     bt.tc_list_cap = (unsigned int)tc_list_entries(B, n);
@@ -376,6 +377,7 @@ int setup_classes(tzr_ctx* ctx, int C, const int* Bs, const int* ns, bool own_po
     bt.dst = (const double*)at(kDst);
     bt.sf = (float4*)at(kSf);
     bt.df = (float4*)at(kDf);
+    bt.gq = (float4*)at(kGq);
     bt.pk = (float*)at(kPk);
     bt.opnd = (float*)at(kOpnd);
     bt.tc_list_count = (unsigned int*)ctx->tclist.p;
@@ -464,6 +466,7 @@ Batch sub_batch(const Batch& bt, int b0, int Bc) {
   s.dst = bt.dst + o * n * 3;
   s.sf = bt.sf + o * n;
   s.df = bt.df + o * n;
+  s.gq = bt.gq + 2 * o * n;
   s.pk = bt.pk + o * 6 * (size_t)npad128(bt.n);
   s.opnd = bt.opnd + tc_operand_bytes(b0, bt.n) / sizeof(float);
   s.gc = bt.gc + o;
@@ -1216,7 +1219,7 @@ int tzr_ctx_destroy(tzr_ctx* ctx) {
   if (!ctx) return TZR_OK;
   cudaSetDevice(ctx->device);
   cudaStreamSynchronize(ctx->stream);
-  DevBuf* bufs[] = {&ctx->src, &ctx->dst, &ctx->sf, &ctx->df, &ctx->pk, &ctx->opnd, &ctx->tclist, &ctx->gc, &ctx->adj, &ctx->deg, &ctx->nedges,
+  DevBuf* bufs[] = {&ctx->src, &ctx->dst, &ctx->sf, &ctx->df, &ctx->gq, &ctx->pk, &ctx->opnd, &ctx->tclist, &ctx->gc, &ctx->adj, &ctx->deg, &ctx->nedges,
                     &ctx->hclq, &ctx->hsize, &ctx->clq, &ctx->L, &ctx->alive, &ctx->best_bits, &ctx->alive_cnt, &ctx->root_ctr,
                     &ctx->lock, &ctx->flg, &ctx->kfinal, &ctx->tstart, &ctx->stack, &ctx->cv, &ctx->centry, &ctx->ps, &ctx->pd, &ctx->wgt,
                     &ctx->res, &ctx->skey, &ctx->sidx, &ctx->sorted, &ctx->rmask, &ctx->tmask, &ctx->sol, &ctx->dbg,

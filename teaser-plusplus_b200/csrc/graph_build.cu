@@ -35,6 +35,9 @@ __device__ __forceinline__ double warp_max(double v) {
   return v;
 }
 
+// debug bit 27: the Gram test's two-slope form on the unscaled copies (sf, df) instead of the single-slope form (gq)
+constexpr uint32_t kFlagTwoSlope = 134217728u;
+
 // launch_graph sends the problems prep_kernel marked use_tc to graph_tc_kernel only under debug flag 1024 without an A/B
 // flag (8-256) or the interval-test flag 512
 __host__ __device__ __forceinline__ bool tc_path_active(uint32_t flags) {
@@ -49,7 +52,7 @@ __global__ void __launch_bounds__(256) prep_kernel(Batch bt) {
   const double* dst = bt.dst + (size_t)b * n * 3;
   __shared__ double s_red[8][12];
   __shared__ int s_bad[8];
-  __shared__ double s_c[7];
+  __shared__ double s_c[8];
   double mn[6], mx[6];
   for (int k = 0; k < 6; ++k) {
     mn[k] = 1.0 / 0.0;
@@ -204,6 +207,38 @@ __global__ void __launch_bounds__(256) prep_kernel(Batch bt) {
       // the band narrow against beta (and k <= 1/64).  C1 (outliers moved 5-10 extents away, beta/D ~ 1e-4) fails it.
       gc.use_gram = (!use64 && (bt.flags_dbg & 512u) == 0 && Ds2 > 0 && Dd2 > 0 && Ds2 < 1e8 && Dd2 < 1e8 && b4 > 1e-30 &&
                      isfinite(gE) && 8.0 * beta <= Dmin && 64.0 * gE <= 0.75 * Dmin * beta) ? 1 : 0;
+      // ---- single-slope form of the Gram test (default; derivation in DESIGN.md §3.1).  Lengths in units of 2 beta
+      // (sig = 1 / (2 beta), so beta^2 -> 1/4):  f = (A - B + 1/4)^2 - A,  edge <= f <= 0,  non-edge <= f > 1/16.  The kernel
+      // computes u = c_u - A', v = c_v - B' (A', B' within Eu, Ev of A, B; c_v = c_u + 1/4 exactly), T = fl(v - u),
+      // dh = fma(T, T, u) and dl = fl(dh + dl_c):
+      //   dh < 0   =>  T^2 < A - c_u + Eu  =>  f <= -c_u + Eu + 5u As + 2 E1 |T| (1 + 2u) + E1^2 <= 0         (edge)
+      //   dl >= 0  =>  T^2 >= A + K, K = |dl_c| (1 - u) - c_u - Eu  =>  f >= K (1 - 2u) - 2u As - 2 E1 sqrt(As + K) > 1/16
+      // with E1 = Eu + Ev, |T| <= sqrt(As + Eu) and A <= As (the scaled source diagonal squared).  Eu = 25 u R^2 + 5 u c_u
+      // to first order (conversion 8, norms 2, the row constant 1, the FADD 2, three FMAs 12; R^2 = As / 4); 28 and 6 are
+      // used.  c_u appears on both sides with a slope far below 1, so the fixed point is reached from below by iteration.
+      if (gc.use_gram && !(bt.flags_dbg & kFlagTwoSlope)) {
+        const double sig = 0.5 / beta, As = sig * sig * Ds2, Ad = sig * sig * Dd2;
+        auto eu = [&](double c) { return u32 * (7.0 * As + 6.0 * c); };
+        auto ev = [&](double c) { return u32 * (7.0 * Ad + 6.0 * (c + 0.25)); };
+        double cu = 0.0;
+        for (int it = 0; it < 8; ++it) {
+          const double Eu = eu(cu), E1 = Eu + ev(cu);
+          cu = Eu + 5.0 * u32 * (As + Eu) + 2.0 * (1.0 + 2.0 * u32) * E1 * sqrt(As + Eu) + E1 * E1;
+        }
+        const float cv_f = __double2float_ru((double)__double2float_ru(cu * (1.0 + 1.52587890625e-05)) + 0.25);
+        const double cu_f = (double)cv_f - 0.25;  // exact: c_v - c_u = 1/4 in the kernel's floats
+        const double Eu = eu(cu_f), E1 = Eu + ev(cu_f);
+        double K = 0.0;
+        for (int it = 0; it < 8; ++it) K = (0.0625 + 2.0 * u32 * As + 2.0 * E1 * sqrt(As + K)) / (1.0 - 2.0 * u32);
+        K *= 1.0 + 1.52587890625e-05;  // 1 + 2^-16 over the iterate (the iteration converges from below)
+        gc.g_cu = (float)cu_f;
+        gc.g_cv = cv_f;
+        gc.g_dl = -__double2float_ru((K + cu_f + Eu) / (1.0 - u32));
+        s_c[7] = sig;
+      } else {
+        gc.g_cu = gc.g_cv = gc.g_dl = 0.f;
+        s_c[7] = 0.0;
+      }
       // debug counter 15: problems graph_strip2_kernel builds with the Gram test (not those graph_tc_kernel or
       // graph_strip3_kernel builds; launch_graph makes the same choice)
       if (gc.use_gram && bt.rechecks && !(ok && tc_path_active(bt.flags_dbg)) && !(bt.flags_dbg & 2048u))
@@ -215,19 +250,33 @@ __global__ void __launch_bounds__(256) prep_kernel(Batch bt) {
   __syncthreads();
   float4* sf = bt.sf + (size_t)b * n;
   float4* df = bt.df + (size_t)b * n;
+  // the single-slope Gram test's operands (problems that run it): the same centred points in units of 2 beta, rounded
+  // once from FP64
+  float4* gq = s_c[7] > 0.0 ? bt.gq + (size_t)b * n * 2 : nullptr;
+  const double ss = s_c[6] * s_c[7], sd = s_c[7];
   for (int i = threadIdx.x; i < n; i += blockDim.x) {
+    const double vs[3] = {src[3 * i + 0] - s_c[0], src[3 * i + 1] - s_c[1], src[3 * i + 2] - s_c[2]};
+    const double vd[3] = {dst[3 * i + 0] - s_c[3], dst[3 * i + 1] - s_c[4], dst[3 * i + 2] - s_c[5]};
     float4 a, c;
-    a.x = (float)((src[3 * i + 0] - s_c[0]) * s_c[6]);
-    a.y = (float)((src[3 * i + 1] - s_c[1]) * s_c[6]);
-    a.z = (float)((src[3 * i + 2] - s_c[2]) * s_c[6]);
+    a.x = (float)(vs[0] * s_c[6]);
+    a.y = (float)(vs[1] * s_c[6]);
+    a.z = (float)(vs[2] * s_c[6]);
     a.w = (float)((double)a.x * a.x + (double)a.y * a.y + (double)a.z * a.z);  // squares exact in FP64: one rounding
-    c.x = (float)(dst[3 * i + 0] - s_c[3]);
-    c.y = (float)(dst[3 * i + 1] - s_c[4]);
-    c.z = (float)(dst[3 * i + 2] - s_c[5]);
+    c.x = (float)vd[0];
+    c.y = (float)vd[1];
+    c.z = (float)vd[2];
     c.w = (float)((double)c.x * c.x + (double)c.y * c.y + (double)c.z * c.z);
     sf[i] = a;
     df[i] = c;
     bt.deg[(size_t)b * n + i] = 0;  // accumulated by the graph kernel (fused-degree path)
+    if (gq) {
+      a = make_float4((float)(vs[0] * ss), (float)(vs[1] * ss), (float)(vs[2] * ss), 0.f);
+      a.w = (float)((double)a.x * a.x + (double)a.y * a.y + (double)a.z * a.z);
+      c = make_float4((float)(vd[0] * sd), (float)(vd[1] * sd), (float)(vd[2] * sd), 0.f);
+      c.w = (float)((double)c.x * c.x + (double)c.y * c.y + (double)c.z * c.z);
+      gq[2 * i] = a;
+      gq[2 * i + 1] = c;
+    }
   }
   // pair-interleaved copy for the packed kernel: (point o, point o+32) of every 64-column half block adjacent
   const int npad = npad128(n);
@@ -870,11 +919,55 @@ __device__ __forceinline__ void gram_sweep(const float4* rows, const int nr, con
   }
 }
 
+// Single-slope sweep (the default form; gram_sweep is the debug-flag-134217728 form).  Same rows, order and prefetch as
+// gram_sweep, on the points in units of 2 beta: rows (2x, 2y, 2z, fl(c_u - N)), (2u, 2v, 2w, fl(c_v - M)), columns
+// (x, y, z, N), (u, v, w, M).  Per pair u = c_u - a', v = c_v - b' (a FADD and three FMAs each), T = v - u, dh = fma(T, T, u),
+// dl = dh + dlc: 13 FP32 operations and the two funnel shifts; sign(dh) = 1 proves an edge, sign(dl) = 0 a non-edge.
+template <int NC>
+__device__ __forceinline__ void slope_sweep(const float4* rows, const int nr, const float4 (&cs)[4], const float4 (&cd)[4],
+                                            const float dlc, uint32_t (&hi)[4], uint32_t (&lo)[4]) {
+  float4 ns = rows[2 * nr - 2], nd = rows[2 * nr - 1];
+  for (int g = nr / 4 - 1; g >= 0; --g) {
+#pragma unroll
+    for (int k = 3; k >= 0; --k) {
+      const int ii = 4 * g + k;
+      const float4 rs = ns, rd = nd;
+      ns = rows[2 * ii - 2];
+      nd = rows[2 * ii - 1];
+#pragma unroll
+      for (int c = 0; c < NC; ++c) {
+        float u = __fsub_rn(rs.w, cs[c].w);
+        u = __fmaf_rn(cs[c].x, rs.x, u);
+        u = __fmaf_rn(cs[c].y, rs.y, u);
+        u = __fmaf_rn(cs[c].z, rs.z, u);
+        float v = __fsub_rn(rd.w, cd[c].w);
+        v = __fmaf_rn(cd[c].x, rd.x, v);
+        v = __fmaf_rn(cd[c].y, rd.y, v);
+        v = __fmaf_rn(cd[c].z, rd.z, v);
+        const float T = __fsub_rn(v, u);
+        const float dh = __fmaf_rn(T, T, u);
+        const float dl = __fadd_rn(dh, dlc);
+        hi[c] = __funnelshift_l(__float_as_uint(dh), hi[c], 1);
+        lo[c] = __funnelshift_l(__float_as_uint(dl), lo[c], 1);
+      }
+    }
+  }
+}
+
+template <int NC>
+__device__ __forceinline__ void gram_sweep_any(const bool slope, const float4* rows, const int nr, const float4 (&cs)[4],
+                                               const float4 (&cd)[4], const float4 k, uint32_t (&hi)[4], uint32_t (&lo)[4]) {
+  if (slope)
+    slope_sweep<NC>(rows, nr, cs, cd, k.x, hi, lo);
+  else
+    gram_sweep<NC>(rows, nr, cs, cd, k.x, k.y, k.z, k.w, hi, lo);
+}
+
 // The mirror half of an off-diagonal block (column words, 4 B per column row and warp) is gathered in a CTA-shared slice
 // and leaves as one 16-byte store per column row, with one degree atomic per column row carrying the sum of the four
 // warps' popcounts.  Every warp of the CTA runs every block of the strip and reaches every barrier: a warp without rows
 // (only in the last row block) sweeps nothing and contributes zero words.
-template <bool kVerify, bool kFuseDeg, bool kRagged>
+template <bool kVerify, bool kFuseDeg, bool kRagged, bool kSlope>
 __device__ __forceinline__ void strip_gram(const Batch& bt, const int b, const int I, const int J0, const int J1) {
   const int nl = bt.n;
   const int n = kRagged ? bt.nb[b] : nl;
@@ -882,13 +975,15 @@ __device__ __forceinline__ void strip_gram(const Batch& bt, const int b, const i
   __shared__ __align__(16) uint32_t s_mir[2][kTile][4];  // [block parity][column row][warp]
 
   const GraphConsts* gcp = bt.gc + b;
-  const float mhi = gcp->g_mhi, chi = gcp->g_chi, mlo = gcp->g_mlo, clo = gcp->g_clo;
+  constexpr bool slope = kSlope;  // the two-slope form is a kernel instance of its own (debug flag 134217728)
+  const float4 kc = slope ? make_float4(gcp->g_dl, 0.f, 0.f, 0.f) : make_float4(gcp->g_mhi, gcp->g_chi, gcp->g_mlo, gcp->g_clo);
   const double beta = gcp->beta;
   const bool scale_mode = bt.scale_mode != 0;
   const double s_hat = scale_mode ? bt.sol[b].scale : 1.0;
 
   const float4* sf = bt.sf + (size_t)b * nl;
   const float4* df = bt.df + (size_t)b * nl;
+  const float4* gq = bt.gq + (size_t)b * nl * 2;
   const double* src = bt.src + (size_t)b * nl * 3;
   const double* dst = bt.dst + (size_t)b * nl * 3;
 
@@ -898,9 +993,15 @@ __device__ __forceinline__ void strip_gram(const Batch& bt, const int b, const i
   const float4 z4 = make_float4(0.f, 0.f, 0.f, 0.f);
   {
     const int i = ibase + lane;
-    const float4 s = (i < n) ? sf[i] : z4, d = (i < n) ? df[i] : z4;
-    s_gr[2 + 2 * tid] = make_float4(-2.f * s.x, -2.f * s.y, -2.f * s.z, s.w);
-    s_gr[2 + 2 * tid + 1] = make_float4(-2.f * d.x, -2.f * d.y, -2.f * d.z, d.w);
+    if (slope) {
+      const float4 s = (i < n) ? gq[2 * i] : z4, d = (i < n) ? gq[2 * i + 1] : z4;
+      s_gr[2 + 2 * tid] = make_float4(2.f * s.x, 2.f * s.y, 2.f * s.z, __fsub_rn(gcp->g_cu, s.w));
+      s_gr[2 + 2 * tid + 1] = make_float4(2.f * d.x, 2.f * d.y, 2.f * d.z, __fsub_rn(gcp->g_cv, d.w));
+    } else {
+      const float4 s = (i < n) ? sf[i] : z4, d = (i < n) ? df[i] : z4;
+      s_gr[2 + 2 * tid] = make_float4(-2.f * s.x, -2.f * s.y, -2.f * s.z, s.w);
+      s_gr[2 + 2 * tid + 1] = make_float4(-2.f * d.x, -2.f * d.y, -2.f * d.z, d.w);
+    }
   }
   __syncwarp();
   uint32_t* adj32 = reinterpret_cast<uint32_t*>(bt.adj) + (size_t)b * nl * pitch32(nl);
@@ -921,21 +1022,21 @@ __device__ __forceinline__ void strip_gram(const Batch& bt, const int b, const i
       for (int c = 0; c < 4; ++c) {
         const int j = jb + 32 * c;
         vj[c] = j < n;
-        cs[c] = vj[c] ? sf[j] : z4;
-        cd[c] = vj[c] ? df[j] : z4;
+        cs[c] = vj[c] ? (slope ? gq[2 * j] : sf[j]) : z4;
+        cd[c] = vj[c] ? (slope ? gq[2 * j + 1] : df[j]) : z4;
       }
       // column words of this lane: bit ii = pair (row ibase+ii, column jb + 32c); hi = surely an edge, lo = edge or
       // undecided
       uint32_t hi[4] = {0u, 0u, 0u, 0u}, lo[4] = {0u, 0u, 0u, 0u};
       const int ncg = min(4, (n - J * kTile + 31) / 32);  // column groups with at least one point below n
       if (ncg == 4)
-        gram_sweep<4>(rows, nr, cs, cd, mhi, chi, mlo, clo, hi, lo);
+        gram_sweep_any<4>(slope, rows, nr, cs, cd, kc, hi, lo);
       else if (ncg == 3)
-        gram_sweep<3>(rows, nr, cs, cd, mhi, chi, mlo, clo, hi, lo);
+        gram_sweep_any<3>(slope, rows, nr, cs, cd, kc, hi, lo);
       else if (ncg == 2)
-        gram_sweep<2>(rows, nr, cs, cd, mhi, chi, mlo, clo, hi, lo);
+        gram_sweep_any<2>(slope, rows, nr, cs, cd, kc, hi, lo);
       else
-        gram_sweep<1>(rows, nr, cs, cd, mhi, chi, mlo, clo, hi, lo);
+        gram_sweep_any<1>(slope, rows, nr, cs, cd, kc, hi, lo);
       // ---- validity (rows < n, columns < n, i != j), undecided pairs, tentative column words
       int nflag = 0;
 #pragma unroll
@@ -1042,7 +1143,7 @@ __device__ __forceinline__ void strip_gram(const Batch& bt, const int b, const i
 // of problem b keeps the (I, J0) it has in b's own grid, its blocks stop at b's last tile, and a strip wholly past that
 // tile returns before it touches shared memory.  Words the kernel does not write (padding rows, and the columns of tiles
 // past b's last one) keep the zeros launch_graph cleared them to, so problem b's rows equal its single-problem graph.
-template <bool kVerify, int kMinBlocks, bool kFuseDeg, bool kRagged>
+template <bool kVerify, int kMinBlocks, bool kFuseDeg, bool kRagged, bool kSlope>
 __device__ __forceinline__ void strip2_body(const Batch& bt) {
   const int b = blockIdx.y;
   const int nt = (bt.n + kTile - 1) / kTile;
@@ -1063,19 +1164,38 @@ __device__ __forceinline__ void strip2_body(const Batch& bt) {
   const GraphConsts* gcp = bt.gc + b;
   if (bt.tc_active && gcp->use_tc) return;  // built by graph_tc_kernel
   if (gcp->use_gram)
-    strip_gram<kVerify, kFuseDeg, kRagged>(bt, b, I, J0, J1);
+    strip_gram<kVerify, kFuseDeg, kRagged, kSlope>(bt, b, I, J0, J1);
   else
     strip_interval<kVerify, kFuseDeg, kRagged>(bt, b, I, J0, J1);
 }
 
-template <bool kVerify, int kMinBlocks, bool kFuseDeg>
+// kSlope: the Gram test's single-slope form (default) or its two-slope form (debug flag 134217728)
+template <bool kVerify, int kMinBlocks, bool kFuseDeg, bool kSlope = true>
 __global__ void __launch_bounds__(kGraphThreads, kMinBlocks) graph_strip2_kernel(Batch bt) {
-  strip2_body<kVerify, kMinBlocks, kFuseDeg, false>(bt);
+  strip2_body<kVerify, kMinBlocks, kFuseDeg, false, kSlope>(bt);
 }
 
-template <bool kVerify, int kMinBlocks, bool kFuseDeg>
+template <bool kVerify, int kMinBlocks, bool kFuseDeg, bool kSlope = true>
 __global__ void __launch_bounds__(kGraphThreads, kMinBlocks) graph_strip2_ragged_kernel(Batch bt) {
-  strip2_body<kVerify, kMinBlocks, kFuseDeg, true>(bt);
+  strip2_body<kVerify, kMinBlocks, kFuseDeg, true, kSlope>(bt);
+}
+
+// the default strip kernel's instances: ragged size class or uniform batch, verifying (flag 2), separate degree pass
+// (flag 256) or the production template
+template <bool kSlope>
+void launch_strip2(const Batch& bt, const dim3 sgrid, cudaStream_t st) {
+  if (bt.nb) {
+    if (bt.flags_dbg & 2u)
+      graph_strip2_ragged_kernel<true, 5, false, kSlope><<<sgrid, kGraphThreads, 0, st>>>(bt);
+    else
+      graph_strip2_ragged_kernel<false, TZR_STRIP_MIN_BLOCKS, true, kSlope><<<sgrid, kGraphThreads, 0, st>>>(bt);
+  } else if (bt.flags_dbg & 2u) {
+    graph_strip2_kernel<true, 5, false, kSlope><<<sgrid, kGraphThreads, 0, st>>>(bt);
+  } else if (bt.flags_dbg & 256u) {  // degrees by the separate degree kernel (A/B against the fused default)
+    graph_strip2_kernel<false, TZR_STRIP_MIN_BLOCKS, false, kSlope><<<sgrid, kGraphThreads, 0, st>>>(bt);
+  } else {  // default: Gram test (interval test where prep_kernel's guard fails), degrees fused
+    graph_strip2_kernel<false, TZR_STRIP_MIN_BLOCKS, true, kSlope><<<sgrid, kGraphThreads, 0, st>>>(bt);
+  }
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -1346,10 +1466,10 @@ int launch_graph(const Batch& bt0, cudaStream_t st, int num_sms) {
   bool v7 = false;
   if (bt.nb) {  // ragged size class: the default kernel (or its verify variant) whatever the opt-in flags 1024 and 2048 say
     cudaMemsetAsync(bt.adj, 0, (size_t)bt.B * bt.n * pitch64(bt.n) * sizeof(uint64_t), st);
-    if (bt.flags_dbg & 2u)
-      graph_strip2_ragged_kernel<true, 5, false><<<sgrid, kGraphThreads, 0, st>>>(bt);
+    if (bt.flags_dbg & kFlagTwoSlope)
+      launch_strip2<false>(bt, sgrid, st);
     else
-      graph_strip2_ragged_kernel<false, TZR_STRIP_MIN_BLOCKS, true><<<sgrid, kGraphThreads, 0, st>>>(bt);
+      launch_strip2<true>(bt, sgrid, st);
   } else if (bt.flags_dbg & 2048u) {  // v7 (one MUFU, sign-bit words, re-check queue): fewer instructions, but FMA-pipe bound
     v7 = true;
     if (bt.flags_dbg & 2u)
@@ -1364,15 +1484,17 @@ int launch_graph(const Batch& bt0, cudaStream_t st, int num_sms) {
     graph_strip_kernel<false, 5><<<sgrid, kGraphThreads, 0, st>>>(bt);
   else if (bt.flags_dbg & 64u)  // scalar-FP32 strip kernel (A/B against the paired default)
     graph_strip_kernel<false, 8><<<sgrid, kGraphThreads, 0, st>>>(bt);
-  else if (bt.flags_dbg & 128u)  // paired kernel at 6 CTAs/SM
-    graph_strip2_kernel<false, 6, false><<<sgrid, kGraphThreads, 0, st>>>(bt);
+  else if (bt.flags_dbg & 128u) {  // paired kernel at 6 CTAs/SM (either form of the Gram test, as bit 27 says)
+    if (bt.flags_dbg & kFlagTwoSlope)
+      graph_strip2_kernel<false, 6, false, false><<<sgrid, kGraphThreads, 0, st>>>(bt);
+    else
+      graph_strip2_kernel<false, 6, false, true><<<sgrid, kGraphThreads, 0, st>>>(bt);
+  }
 #endif
-  else if (bt.flags_dbg & 2u)
-    graph_strip2_kernel<true, 5, false><<<sgrid, kGraphThreads, 0, st>>>(bt);
-  else if (bt.flags_dbg & 256u)  // degrees by the separate degree kernel (A/B against the fused default)
-    graph_strip2_kernel<false, TZR_STRIP_MIN_BLOCKS, false><<<sgrid, kGraphThreads, 0, st>>>(bt);
-  else  // default: Gram test (interval test where prep_kernel's guard fails), degrees fused
-    graph_strip2_kernel<false, TZR_STRIP_MIN_BLOCKS, true><<<sgrid, kGraphThreads, 0, st>>>(bt);
+  else if (bt.flags_dbg & kFlagTwoSlope)
+    launch_strip2<false>(bt, sgrid, st);
+  else
+    launch_strip2<true>(bt, sgrid, st);
   // exact re-check of the pairs the strip kernel queued (v7, or the Gram test: every problem unless debug flag 512)
   if (v7 || !(bt.flags_dbg & 512u)) {
     launch_graph_patch(bt, st, num_sms);

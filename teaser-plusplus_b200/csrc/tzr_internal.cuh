@@ -71,7 +71,10 @@ struct GraphConsts {
   // Gram-form test of graph_strip2_kernel (DESIGN.md §3.1): with a', b' the FP32 Gram-form squared norms, t = a' - b',
   // s = a' + b':  t^2 + g_mhi s + g_chi <= 0 proves an edge, t^2 + g_mlo s + g_clo >= 0 proves a non-edge
   int use_gram;   // 1: the conditioning guard holds, the strip kernel runs the Gram test; 0: the sqrt interval test (b1, b2)
-  float g_mhi, g_chi, g_mlo, g_clo;
+  float g_mhi, g_chi, g_mlo, g_clo;  // two-slope form (debug flag 134217728)
+  // single-slope form (default), lengths in units of 2 beta (Batch::gq): with u = c_u - a', v = c_v - b' (c_v = c_u + 1/4
+  // exactly) and T = v - u, sign(fma(T, T, u)) = 1 proves an edge and sign(fma(T, T, u) + g_dl) = 0 a non-edge
+  float g_cu, g_cv, g_dl;
 };
 
 // Everything the device kernels need to know about one batch (passed by value).
@@ -87,7 +90,9 @@ struct Batch {
   const double* dst;  // B*n*3
   float4* sf;     // B*n centred float copies; w = their squared norm, rounded to float (Gram-form test)
   float4* df;
-  float* opnd;    // B * ceil(n/128) * 2 roles * 2 clouds * 6 planes * 128 rows * 4: tf32-split MMA operand tiles of the
+  float4* gq;     // B*n*2: the same points in units of 2 beta (x, y, z, squared norm), source at 2i and destination at
+                  // 2i+1; written by prep_kernel for the problems that run the single-slope Gram test
+  float* opnd;   // B * ceil(n/128) * 2 roles * 2 clouds * 6 planes * 128 rows * 4: tf32-split MMA operand tiles of the
                   // tensor-core graph kernel (graph_tc.cu), written by tc_prep_kernel
   uint2* tc_list;         // re-check queue of the tensor-core graph kernel: (problem, i << 16 | j)
   unsigned int* tc_list_count;  // 1 (may exceed the capacity: writers past it evaluate in place)
