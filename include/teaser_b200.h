@@ -613,6 +613,68 @@ int tzr_register_cloud_pairs_icp_point_to_plane(tzr_ctx* ctx, const tzr_frontend
                                                 int32_t* const* corr, int32_t* const* cliques, float* global_scale,
                                                 const tzr_icp_params* icp, tzr_icp_result* icp_results);
 
+/* ---- refining registrations: generalized ICP -----------------------------------------------------------------
+ * Open3D's registration_generalized_icp (TransformationEstimationForGeneralizedICP, its default L2 loss), for many
+ * problems at once, defined here as follows (DESIGN.md §3.14):
+ *   - Unchanged from tzr_icp_point_to_plane: the inputs and the fixed scale s, the transform p_i = s (R x_i) + t, the
+ *     search and both of its routes, eval(T), the loop, the convergence test, the composition, the 6 x 6 solve of
+ *     A x = -g, R_u = Rz(x2) Ry(x1) Rx(x0) and t_u = (c + tau) - R_u c with c = mu_p.  Only the system changes.
+ *   - Normals: the source normals (ns x 4 floats) and the target normals (nd x 4 floats), both in the library's normals
+ *     layout (curvature ignored), read exactly as float64 and used up to length and sign.
+ *   - System, in IEEE float64 with no FMA contraction.  For each correspondence (i, j), with u = p_i - c, d = p_i - y_j,
+ *     m = m_i (source normal) and n = n_j (target normal):
+ *       m' = R m, row r: (R(r,0) m0 + R(r,1) m1) + R(r,2) m2 with the current R, without the scale.
+ *       C(v) = I - (k v_a) v_b, k = (1 - epsilon) / ((v0 v0 + v1 v1) + v2 v2): each of the six upper entries
+ *         (00, 01, 02, 11, 12, 22) is delta_ab - (k v_a) v_b, mirrored below.  For a unit v this is Open3D's
+ *         Rx diag(epsilon, 1, 1) Rx^T with Rx = GetRotationFromE1ToX(v); dividing by v^T v uses normals up to length,
+ *         and a negated v gives the same bits.
+ *       M = s2 C(m') + C(n) entry by entry, s2 = s * s rounded once (Open3D's (sR) C (sR)^T plus the target's).
+ *       cofactors c00 = M11 M22 - M12 M12, c01 = M02 M12 - M01 M22, c02 = M01 M12 - M02 M11,
+ *                 c11 = M00 M22 - M02 M02, c12 = M01 M02 - M00 M12, c22 = M00 M11 - M01 M01;
+ *       det = (M00 c00 + M01 c01) + M02 c02, A = M^-1 with A_ab = c_ab / det.
+ *       J = [e_k x u (k = 0..2), I] (3 x 6).  The correspondence adds J^T A J (21 entries, the upper triangle row by
+ *       row as point-to-plane's) and J^T A d (6) to the fixed-order chunk sums, evaluated as
+ *         omega-omega (k <= l): (u x A (e_l x u))_k,  omega-tau: (u x a_l)_k with a_l = column l of A,
+ *         tau-tau (k <= l): A_kl,  g = (u x w, w) with w = A d,
+ *       where a x b = (a1 b2 - a2 b1, a2 b0 - a0 b2, a0 b1 - a1 b0) and A v row r is (A(r,0) v0 + A(r,1) v1) + A(r,2) v2.
+ *     A correspondence adds nothing, but still counts for fitness and rmse, when either normal has a non-finite
+ *     component or zero length, or when det is not > 0 or not finite.
+ *   - epsilon (Open3D's epsilon, 1e-3 there) must be finite and > 0; anything else is TZR_ERR_INVALID_ARG.
+ *   - Relation to Open3D: Open3D forms W = M^-1/2 and sums three weighted rows per correspondence; with the L2 loss
+ *     sum rows^T rows = J^T M^-1 J, so no matrix square root is needed.  Open3D's GetRotationFromE1ToX returns the
+ *     identity when e1 . n < -0.99, which makes its covariance depend on the normal's sign there; this definition uses
+ *     the closed form and does not.  The step is linearised about c, as point-to-plane's (DESIGN.md §3.13).
+ * Launches: 2 + 4 * max_iteration (+ 4 for the grid build when some target has at least 1024 points), whatever B, as
+ * tzr_icp_batch.  Workspace: tzr_icp's own, so a retained solve stays retained. */
+
+/* One problem: tzr_icp_point_to_plane's arguments plus epsilon and src_normals (ns x 4 floats, required).  This is
+ * tzr_icp_generalized_batch with B = 1. */
+int tzr_icp_generalized(tzr_ctx* ctx, const tzr_icp_params* params, double epsilon, const float* src, int ns,
+                        const float* src_normals, const float* dst, int nd, const float* dst_normals,
+                        const tzr_similarity* init, tzr_icp_result* result, int32_t* corr);
+
+/* B ragged problems: tzr_icp_point_to_plane_batch's arguments plus epsilon and src_normals (B entries, entry b ns[b] x 4
+ * floats).  Either normals array NULL, or holding a NULL entry, is TZR_ERR_INVALID_ARG.  Per problem, every output is
+ * bit-identical to tzr_icp_generalized on that problem alone. */
+int tzr_icp_generalized_batch(tzr_ctx* ctx, const tzr_icp_params* params, double epsilon, int B, const int32_t* ns,
+                              const float* const* src, const float* const* src_normals, const int32_t* nd,
+                              const float* const* dst, const float* const* dst_normals, const tzr_similarity* init,
+                              tzr_icp_result* results, int32_t* const* corr);
+
+/* tzr_register_cloud_pairs_icp with generalized ICP: the same arguments plus epsilon, and the same outputs, except that
+ * each refined record is generalized ICP on the pair's two clouds, using both clouds' normals from the call's own FPFH
+ * stage (normal_search_radius, viewpoint at the origin).  No normal pass, upload or host synchronisation is added.
+ * Each refined record is bit-identical to tzr_register_cloud_pairs, then tzr_estimate_normals_batch over the clouds at
+ * fparams->normal_search_radius, then tzr_icp_generalized_batch over the valid solved pairs seeded with their records.
+ * Launches: as tzr_register_cloud_pairs_icp. */
+int tzr_register_cloud_pairs_icp_generalized(tzr_ctx* ctx, const tzr_frontend_params* fparams,
+                                             const tzr_params* params, int n_clouds, const int32_t* n,
+                                             const float* const* pts, int P, const int32_t* pair_clouds,
+                                             const uint64_t* tuple_seeds, tzr_solution* solutions, int32_t* status,
+                                             int32_t* problem_index, int64_t* n_corr, int32_t* const* corr,
+                                             int32_t* const* cliques, float* global_scale, const tzr_icp_params* icp,
+                                             double epsilon, tzr_icp_result* icp_results);
+
 /* ---- downsampling point clouds: voxel-grid averaging ----------------------------------------------------------
  * The first step of the reference's FPFH + TEASER++ + ICP tutorial (voxel_down_sample on both raw scans), for many
  * clouds at once.  Open3D's PointCloud::VoxelDownSample, points only, with a defined order.  Per cloud, all arithmetic
@@ -700,7 +762,7 @@ int tzr_solve_batch_multi(const int32_t* devices, int n_devices, const tzr_param
  * to brute force), so that the two routes can be compared on one input; bit 22 wins when both are set, bit 24
  * (16777216) = a ragged batch forms one size class wherever the large-route and scale-path rules allow, however far
  * apart its sizes are, so that tests can pad n = 2 to n = 4000 in one device batch, bit 25 (33554432) = tzr_icp(_batch)
- * and tzr_icp_point_to_plane(_batch)
+ * and tzr_icp_point_to_plane(_batch) and tzr_icp_generalized(_batch)
  * searches every target by brute force, bit 26 (67108864) = through the hashed grid at any target size (a target the
  * grid cannot index still falls back to brute force), so that the two routes can be compared on one input; bit 25 wins
  * when both are set, bit 27 (134217728) = the default graph kernel's Gram test in its two-slope form on the unscaled float

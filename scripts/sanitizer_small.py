@@ -124,7 +124,19 @@ for iflags in (33554432, 67108864):
     res, corr = ctx.icp_point_to_plane_batch([ic_dst, ic_src[:3], ic_src], [ic_src, ic_dst, ic_src[:2]],
                                              [nrm[0], nrm[1], nrm[3]], 0.05, max_iteration=3)
     print("icp plane flags", iflags, [int(r) for r in res["n_correspondences"]], [int(r) for r in res["iterations"]])
+    # generalized ICP: the same batch with source normals too (NaN rows on both sides)
+    res, corr = ctx.icp_generalized_batch([ic_dst, ic_src[:3], ic_src], [ic_src, ic_dst, ic_src[:2]],
+                                          [nrm[1], nrm[0][:3], nrm[0]], [nrm[0], nrm[1], nrm[3]], 0.05,
+                                          max_iteration=3)
+    print("icp generalized flags", iflags, [int(r) for r in res["n_correspondences"]],
+          [int(r) for r in res["iterations"]])
 ctx.set_flags(0)
+# the chained entry with generalized ICP: both clouds' normals from its own FPFH stage
+gp = ctx.register_cloud_pairs_icp([ic_src[1:], ic_dst[1:]], [(0, 1), (1, 0)],
+                                  capi.default_params(noise_bound=0.01, estimate_scaling=0), 0.05,
+                                  normal_search_radius=0.05, fpfh_search_radius=0.1, method="generalized",
+                                  max_iteration=3)
+print("register_cloud_pairs_icp generalized", gp[1].tolist(), [int(r) for r in gp[6]["iterations"]])
 # voxel downsampling: a ragged batch with a NaN row, an all-NaN cloud and a cloud too wide for the voxel (INT_MAX check)
 vx = [rng.uniform(0, 1, size=(500, 3)).astype(np.float32), np.full((3, 3), np.nan, dtype=np.float32),
       np.array([[0, 0, 0], [1e9, 0, 0]], dtype=np.float32), rng.uniform(0, 1, size=(1, 3)).astype(np.float32)]

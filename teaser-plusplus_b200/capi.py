@@ -137,7 +137,8 @@ _SYMBOLS = [
     "tzr_frontend_params_default", "tzr_register_cloud_pairs", "tzr_icp_params_default", "tzr_icp", "tzr_icp_batch",
     "tzr_register_cloud_pairs_icp", "tzr_voxel_downsample", "tzr_voxel_downsample_batch", "tzr_estimate_normals",
     "tzr_estimate_normals_batch", "tzr_icp_point_to_plane", "tzr_icp_point_to_plane_batch",
-    "tzr_register_cloud_pairs_icp_point_to_plane",
+    "tzr_register_cloud_pairs_icp_point_to_plane", "tzr_icp_generalized", "tzr_icp_generalized_batch",
+    "tzr_register_cloud_pairs_icp_generalized",
 ]
 
 # status codes (tzr_status)
@@ -260,6 +261,12 @@ def lib():
     L.tzr_icp_point_to_plane_batch.argtypes = [vp, C.POINTER(IcpParams), C.c_int, i32p, fpp, i32p, fpp, fpp,
                                                C.POINTER(Similarity), C.POINTER(IcpResult), C.POINTER(i32p)]
     L.tzr_register_cloud_pairs_icp_point_to_plane.argtypes = L.tzr_register_cloud_pairs_icp.argtypes
+    L.tzr_icp_generalized.argtypes = [vp, C.POINTER(IcpParams), C.c_double, fp, C.c_int, fp, fp, C.c_int, fp,
+                                      C.POINTER(Similarity), C.POINTER(IcpResult), i32p]
+    L.tzr_icp_generalized_batch.argtypes = [vp, C.POINTER(IcpParams), C.c_double, C.c_int, i32p, fpp, fpp, i32p, fpp,
+                                            fpp, C.POINTER(Similarity), C.POINTER(IcpResult), C.POINTER(i32p)]
+    L.tzr_register_cloud_pairs_icp_generalized.argtypes = L.tzr_register_cloud_pairs.argtypes + [
+        C.POINTER(IcpParams), C.c_double, C.POINTER(IcpResult)]
     L.tzr_voxel_downsample.argtypes = [vp, fp, C.c_int, C.c_double, fp, i32p, i32p]
     L.tzr_voxel_downsample_batch.argtypes = [vp, C.c_int, i32p, fpp, C.c_double, fpp, i32p, C.POINTER(i32p), i32p]
     for s in _SYMBOLS:
@@ -982,22 +989,24 @@ class Context:
     def register_cloud_pairs_icp(self, clouds, pairs, params: Params, max_correspondence_distance, normal_search_radius=0.03,
                                  fpfh_search_radius=0.05, use_absolute_scale=True, use_crosscheck=True,
                                  use_tuple_test=True, tuple_scale=0.0, tuple_seeds=None, max_iteration=30,
-                                 relative_fitness=1e-6, relative_rmse=1e-6, method="point_to_point"):
+                                 relative_fitness=1e-6, relative_rmse=1e-6, method="point_to_point", epsilon=1e-3):
         """tzr_register_cloud_pairs_icp: register_cloud_pairs, then ICP of every pair with a valid solution on its two
         clouds, seeded with that solution, in the same call.  Returns register_cloud_pairs' six results plus the ICP
         records (structured array (P,) of ICP_RESULT_DTYPE, zeroed for a pair that was not refined).
         method="point_to_plane" runs point-to-plane ICP (tzr_register_cloud_pairs_icp_point_to_plane) with the target
-        normals of the call's own FPFH stage."""
-        if method not in ("point_to_point", "point_to_plane"):
+        normals of the call's own FPFH stage; method="generalized" runs generalized ICP
+        (tzr_register_cloud_pairs_icp_generalized) with both clouds' normals from that stage and the given epsilon."""
+        if method not in ("point_to_point", "point_to_plane", "generalized"):
             raise TzrError(f"register_cloud_pairs_icp: unknown method {method!r}")
         icp = icp_params(max_correspondence_distance, max_iteration=int(max_iteration),
                          relative_fitness=float(relative_fitness), relative_rmse=float(relative_rmse))
         return self._register_pairs(clouds, pairs, params, normal_search_radius, fpfh_search_radius, use_absolute_scale,
                                     use_crosscheck, use_tuple_test, tuple_scale, tuple_seeds, icp,
-                                    plane=method == "point_to_plane")
+                                    plane=method == "point_to_plane",
+                                    epsilon=float(epsilon) if method == "generalized" else None)
 
     def _register_pairs(self, clouds, pairs, params, normal_search_radius, fpfh_search_radius, use_absolute_scale,
-                        use_crosscheck, use_tuple_test, tuple_scale, tuple_seeds, icp, plane=False):
+                        use_crosscheck, use_tuple_test, tuple_scale, tuple_seeds, icp, plane=False, epsilon=None):
         cl = [np.ascontiguousarray(c, dtype=np.float32) for c in clouds]
         if not cl or any(c.ndim != 2 or c.shape[1] != 3 or c.shape[0] == 0 for c in cl):
             raise TzrError("register_cloud_pairs: a non-empty list of non-empty (n,3) clouds is required")
@@ -1032,8 +1041,12 @@ class Context:
             rc = lib().tzr_register_cloud_pairs(*args)
         else:
             icp_res = np.zeros(P, dtype=ICP_RESULT_DTYPE)
-            entry = lib().tzr_register_cloud_pairs_icp_point_to_plane if plane else lib().tzr_register_cloud_pairs_icp
-            rc = entry(*args, C.byref(icp), icp_res.ctypes.data_as(C.POINTER(IcpResult)))
+            out_res = icp_res.ctypes.data_as(C.POINTER(IcpResult))
+            if epsilon is not None:
+                rc = lib().tzr_register_cloud_pairs_icp_generalized(*args, C.byref(icp), epsilon, out_res)
+            else:
+                entry = lib().tzr_register_cloud_pairs_icp_point_to_plane if plane else lib().tzr_register_cloud_pairs_icp
+                rc = entry(*args, C.byref(icp), out_res)
         if rc not in (0, TZR_ERR_TOO_LARGE):
             self._ck(rc)
         corr = [c[:k].copy() for c, k in zip(corr, cnt)]
@@ -1069,6 +1082,28 @@ class Context:
         return self._icp(srcs, dsts, dst_normals, max_correspondence_distance, inits, max_iteration, relative_fitness,
                          relative_rmse, single)
 
+    def icp_generalized(self, src, dst, src_normals, dst_normals, max_correspondence_distance, init=None, epsilon=1e-3,
+                        max_iteration=30, relative_fitness=1e-6, relative_rmse=1e-6):
+        """tzr_icp_generalized: icp() with generalized-ICP updates; src_normals / dst_normals: (n,3) or (n,4) float32
+        normals of each cloud (e.g. estimate_normals()), used as given; epsilon: the covariances' epsilon (finite,
+        > 0).  Returns what icp() returns."""
+        res, corr = self.icp_generalized_batch([src], [dst], [src_normals], [dst_normals], max_correspondence_distance,
+                                               None if init is None else [init], epsilon=epsilon,
+                                               max_iteration=max_iteration, relative_fitness=relative_fitness,
+                                               relative_rmse=relative_rmse, single=True)
+        return icp_result_dict(res[0]), corr[0]
+
+    def icp_generalized_batch(self, srcs, dsts, src_normals, dst_normals, max_correspondence_distance, inits=None,
+                              epsilon=1e-3, max_iteration=30, relative_fitness=1e-6, relative_rmse=1e-6,
+                              single=False):
+        """tzr_icp_generalized_batch: icp_batch() with generalized-ICP updates and one (n,3) or (n,4) normals array per
+        source and per target.  single=True goes through tzr_icp_generalized (B must be 1)."""
+        if len(src_normals) != len(srcs):
+            raise TzrError("icp_generalized_batch: one normals array per source cloud is required")
+        SN = [_normals32(a, _cloud32(s, "icp").shape[0], "icp_generalized") for a, s in zip(src_normals, srcs)]
+        return self._icp(srcs, dsts, dst_normals, max_correspondence_distance, inits, max_iteration, relative_fitness,
+                         relative_rmse, single, src_normals=SN, epsilon=float(epsilon))
+
     def icp_batch(self, srcs, dsts, max_correspondence_distance, inits=None, max_iteration=30, relative_fitness=1e-6,
                   relative_rmse=1e-6, single=False):
         """tzr_icp_batch over B (source, target) cloud pairs; inits: B seeds (None = identity for all).  Returns
@@ -1078,8 +1113,9 @@ class Context:
                          relative_rmse, single)
 
     def _icp(self, srcs, dsts, normals, max_correspondence_distance, inits, max_iteration, relative_fitness,
-             relative_rmse, single):
-        """icp_batch (normals None) and icp_point_to_plane_batch."""
+             relative_rmse, single, src_normals=None, epsilon=None):
+        """icp_batch (normals None), icp_point_to_plane_batch and icp_generalized_batch (src_normals: (n,4) float32
+        arrays, epsilon given)."""
         S = [_cloud32(a, "icp") for a in srcs]
         D = [_cloud32(a, "icp") for a in dsts]
         B = len(S)
@@ -1096,16 +1132,25 @@ class Context:
             assert B == 1
             head = (self._h, C.byref(p), _p(S[0], C.c_float), S[0].shape[0], _p(D[0], C.c_float), D[0].shape[0])
             tail = (init, res, _p(corr[0], C.c_int32))
-            rc = lib().tzr_icp(*head, *tail) if N is None else \
-                lib().tzr_icp_point_to_plane(*head, _p(N[0], C.c_float), *tail)
+            if src_normals is not None:
+                rc = lib().tzr_icp_generalized(self._h, C.byref(p), epsilon, head[2], head[3],
+                                               _p(src_normals[0], C.c_float), *head[4:], _p(N[0], C.c_float), *tail)
+            else:
+                rc = lib().tzr_icp(*head, *tail) if N is None else \
+                    lib().tzr_icp_point_to_plane(*head, _p(N[0], C.c_float), *tail)
         else:
             ns = np.array([a.shape[0] for a in S], dtype=np.int32)
             nd = np.array([a.shape[0] for a in D], dtype=np.int32)
             head = (self._h, C.byref(p), B, _p(ns, C.c_int32), (fp * B)(*[_p(a, C.c_float) for a in S]),
                     _p(nd, C.c_int32), (fp * B)(*[_p(a, C.c_float) for a in D]))
             tail = (init, res, (i32p * B)(*[_p(c, C.c_int32) for c in corr]))
-            rc = lib().tzr_icp_batch(*head, *tail) if N is None else \
-                lib().tzr_icp_point_to_plane_batch(*head, (fp * B)(*[_p(a, C.c_float) for a in N]), *tail)
+            if src_normals is not None:
+                rc = lib().tzr_icp_generalized_batch(self._h, C.byref(p), epsilon, B, head[3], head[4],
+                                                     (fp * B)(*[_p(a, C.c_float) for a in src_normals]), *head[5:],
+                                                     (fp * B)(*[_p(a, C.c_float) for a in N]), *tail)
+            else:
+                rc = lib().tzr_icp_batch(*head, *tail) if N is None else \
+                    lib().tzr_icp_point_to_plane_batch(*head, (fp * B)(*[_p(a, C.c_float) for a in N]), *tail)
         self._ck(rc)
         out = np.frombuffer(bytes(res), dtype=ICP_RESULT_DTYPE).copy()
         return out, [c[:int(r["n_correspondences"])].copy() for c, r in zip(corr, out)]

@@ -2060,6 +2060,9 @@ static bool icp_params_ok(const tzr_icp_params* p) {
          p->max_iteration >= 0 && !std::isnan(p->relative_fitness) && !std::isnan(p->relative_rmse);
 }
 
+// generalized ICP's epsilon: finite and > 0
+static bool icp_epsilon_ok(double epsilon) { return std::isfinite(epsilon) && epsilon > 0; }
+
 static void icp_result_of(const IcpProb& pr, tzr_icp_result* out) {
   memset(out, 0, sizeof(*out));
   if (!pr.seeded) return;
@@ -2084,11 +2087,12 @@ static int register_pairs_run(tzr_ctx* ctx, const tzr_frontend_params* fp, const
                               const uint64_t* tuple_seeds, tzr_solution* solutions, int32_t* status,
                               int32_t* problem_index, int64_t* n_corr, int32_t* const* corr, int32_t* const* cliques,
                               float* global_scale, const tzr_icp_params* icp, tzr_icp_result* icp_results,
-                              int icp_mode = kIcpPointToPoint) {
+                              int icp_mode = kIcpPointToPoint, double icp_epsilon = 0) {
   if (!ctx || !fp || !params || n_clouds < 1 || !n || !pts || P < 1 || !pair_clouds || !solutions || !status ||
       !n_corr || !(fp->normal_search_radius > 0) || !(fp->fpfh_search_radius > 0))
     return TZR_ERR_INVALID_ARG;
   if (icp && (!icp_params_ok(icp) || !icp_results)) return TZR_ERR_INVALID_ARG;
+  if (icp && icp_mode == kIcpGeneralized && !icp_epsilon_ok(icp_epsilon)) return TZR_ERR_INVALID_ARG;
   for (int c = 0; c < n_clouds; ++c)
     if (n[c] <= 0 || !pts[c]) return TZR_ERR_INVALID_ARG;
   std::vector<int32_t> ns(P), nd(P);
@@ -2152,6 +2156,7 @@ static int register_pairs_run(tzr_ctx* ctx, const tzr_frontend_params* fp, const
     }
     iplan.max_iteration = icp->max_iteration;
     iplan.mode = icp_mode;
+    iplan.epsilon = icp_epsilon;
     iplan.r2 = r * r;
     iplan.relative_fitness = icp->relative_fitness;
     iplan.relative_rmse = icp->relative_rmse;
@@ -2285,6 +2290,7 @@ static int register_pairs_run(tzr_ctx* ctx, const tzr_frontend_params* fp, const
       pr.m_lo = m_lo;
       pr.tc = b;
       pr.n_lo = clouds[b].lo;
+      pr.sn_lo = clouds[a].lo;
       const int nc = (n[a] + kIcpChunk - 1) / kIcpChunk;
       for (int c = 0; c < nc; ++c) ((int*)(h + hi_ck))[c_lo + c] = k;
       c_lo += nc;
@@ -2306,10 +2312,11 @@ static int register_pairs_run(tzr_ctx* ctx, const tzr_frontend_params* fp, const
     CK(cudaMemcpyAsync(di + o_cl, h + hi_cl, cb, cudaMemcpyHostToDevice, st));
     CK(cudaMemcpyAsync(di + o_ck, h + hi_ck, kb, cudaMemcpyHostToDevice, st));
     ctx->launches += launch_icp_seed((IcpProb*)(di + o_prob), S, d_sol, st);
-    // point-to-plane: the target normals are the FPFH stage's (normal_search_radius, viewpoint at the origin), still
-    // in m_out: nothing after the FPFH stage writes that region, and they share the cloud table's indexing
-    ctx->launches += launch_icp(iplan, d_pts, d_pts, (const float4*)(d_out + o_nrm), (IcpProb*)(di + o_prob),
-                                (FpfhCloud*)(di + o_cl),
+    // point-to-plane and generalized: the target (and source) normals are the FPFH stage's (normal_search_radius,
+    // viewpoint at the origin), still in m_out: nothing after the FPFH stage writes that region, and they share the
+    // cloud table's indexing
+    const float4* d_nrm = (const float4*)(d_out + o_nrm);
+    ctx->launches += launch_icp(iplan, d_pts, d_pts, d_nrm, d_nrm, (IcpProb*)(di + o_prob), (FpfhCloud*)(di + o_cl),
                                 (const int*)(di + o_ck), (int*)(di + o_match), (double*)(di + o_part),
                                 iplan.grid.grid_bytes ? di + o_grid : nullptr, st);
     if ((rc = check_launch(ctx, "icp launch")) != TZR_OK) return rc;
@@ -2383,6 +2390,19 @@ int tzr_register_cloud_pairs_icp_point_to_plane(tzr_ctx* ctx, const tzr_frontend
                             problem_index, n_corr, corr, cliques, global_scale, icp, icp_results, kIcpPointToPlane);
 }
 
+int tzr_register_cloud_pairs_icp_generalized(tzr_ctx* ctx, const tzr_frontend_params* fp, const tzr_params* params,
+                                             int n_clouds, const int32_t* n, const float* const* pts, int P,
+                                             const int32_t* pair_clouds, const uint64_t* tuple_seeds,
+                                             tzr_solution* solutions, int32_t* status, int32_t* problem_index,
+                                             int64_t* n_corr, int32_t* const* corr, int32_t* const* cliques,
+                                             float* global_scale, const tzr_icp_params* icp, double epsilon,
+                                             tzr_icp_result* icp_results) {
+  if (!icp) return TZR_ERR_INVALID_ARG;
+  return register_pairs_run(ctx, fp, params, n_clouds, n, pts, P, pair_clouds, tuple_seeds, solutions, status,
+                            problem_index, n_corr, corr, cliques, global_scale, icp, icp_results, kIcpGeneralized,
+                            epsilon);
+}
+
 void tzr_icp_params_default(tzr_icp_params* p) {
   if (!p) return;
   memset(p, 0, sizeof(*p));
@@ -2392,22 +2412,24 @@ void tzr_icp_params_default(tzr_icp_params* p) {
   p->max_iteration = 30;
 }
 
-// tzr_icp(_batch) and tzr_icp_point_to_plane(_batch): sources, targets (and target normals) staged back to back, one
-// H2D copy, every iteration enqueued (launch_icp), one D2H copy of the problem table (and of the per-point matches when
-// correspondences are asked for).  dst_normals: required for kIcpPointToPlane, unused otherwise.
+// tzr_icp(_batch), tzr_icp_point_to_plane(_batch) and tzr_icp_generalized(_batch): sources, targets (and target and
+// source normals) staged back to back, one H2D copy, every iteration enqueued (launch_icp), one D2H copy of the problem
+// table (and of the per-point matches when correspondences are asked for).  dst_normals: required for kIcpPointToPlane
+// and kIcpGeneralized, src_normals and epsilon for kIcpGeneralized; unused otherwise.
 static int icp_batch_run(tzr_ctx* ctx, const tzr_icp_params* params, int mode, int B, const int32_t* ns,
-                         const float* const* src, const int32_t* nd, const float* const* dst,
-                         const float* const* dst_normals, const tzr_similarity* init, tzr_icp_result* results,
-                         int32_t* const* corr) {
-  const bool plane = mode == kIcpPointToPlane;
-  if (!ctx || !icp_params_ok(params) || B < 1 || !ns || !src || !nd || !dst || (plane && !dst_normals) || !init ||
-      !results)
+                         const float* const* src, const float* const* src_normals, const int32_t* nd,
+                         const float* const* dst, const float* const* dst_normals, double epsilon,
+                         const tzr_similarity* init, tzr_icp_result* results, int32_t* const* corr) {
+  const bool plane = mode != kIcpPointToPoint, gicp = mode == kIcpGeneralized;
+  if (!ctx || !icp_params_ok(params) || B < 1 || !ns || !src || !nd || !dst || (plane && !dst_normals) ||
+      (gicp && (!src_normals || !icp_epsilon_ok(epsilon))) || !init || !results)
     return TZR_ERR_INVALID_ARG;
   const double r = params->max_correspondence_distance;
   long long NS = 0, ND = 0, chunks = 0;
   bool want_corr = false;
   for (int b = 0; b < B; ++b) {
-    if (ns[b] < 1 || nd[b] < 1 || !src[b] || !dst[b] || (plane && !dst_normals[b])) return TZR_ERR_INVALID_ARG;
+    if (ns[b] < 1 || nd[b] < 1 || !src[b] || !dst[b] || (plane && !dst_normals[b]) || (gicp && !src_normals[b]))
+      return TZR_ERR_INVALID_ARG;
     const tzr_similarity& s = init[b];
     bool finite = std::isfinite(s.scale) && s.scale > 0;
     for (int k = 0; k < 9; ++k) finite &= std::isfinite(s.rotation[k]) != 0;
@@ -2429,6 +2451,7 @@ static int icp_batch_run(tzr_ctx* ctx, const tzr_icp_params* params, int mode, i
   plan.chunks = (int)chunks;
   plan.max_iteration = params->max_iteration;
   plan.mode = mode;
+  plan.epsilon = epsilon;
   plan.r2 = r * r;
   plan.relative_fitness = params->relative_fitness;
   plan.relative_rmse = params->relative_rmse;
@@ -2453,6 +2476,7 @@ static int icp_batch_run(tzr_ctx* ctx, const tzr_icp_params* params, int mode, i
       pr.m_lo = s_lo;
       pr.tc = b;
       pr.n_lo = clouds[b].lo;
+      pr.sn_lo = s_lo;
       pr.active = pr.seeded = 1;
       pr.s = init[b].scale;
       for (int k = 0; k < 9; ++k) pr.R[k] = init[b].rotation[k];
@@ -2465,13 +2489,15 @@ static int icp_batch_run(tzr_ctx* ctx, const tzr_icp_params* params, int mode, i
   }
   cudaSetDevice(ctx->device);
   cudaStream_t st = ctx->stream;
-  // [sources | targets | problems | target clouds | chunk table | (target normals)] staged, then the matches, the
-  // partials and the grid scratch
+  // [sources | targets | problems | target clouds | chunk table | (target normals | (source normals))] staged, then the
+  // matches, the partials and the grid scratch
   const size_t sb = (size_t)NS * 12, db = (size_t)ND * 12, pb = (size_t)B * sizeof(IcpProb),
                cb = (size_t)B * sizeof(FpfhCloud), kb = (size_t)chunks * 4, mb = (size_t)NS * 4,
-               hb = (size_t)chunks * icp_partial_stride(mode) * 8, nb = plane ? (size_t)ND * 16 : 0;
+               hb = (size_t)chunks * icp_partial_stride(mode) * 8, nb = plane ? (size_t)ND * 16 : 0,
+               snb = gicp ? (size_t)NS * 16 : 0;
   const size_t o_dst = al256(sb), o_prob = o_dst + al256(db), o_cl = o_prob + al256(pb), o_ck = o_cl + al256(cb),
-               o_nrm = o_ck + al256(kb), in_bytes = plane ? o_nrm + nb : o_ck + kb, o_match = al256(in_bytes),
+               o_nrm = o_ck + al256(kb), o_snrm = o_nrm + al256(nb),
+               in_bytes = gicp ? o_snrm + snb : plane ? o_nrm + nb : o_ck + kb, o_match = al256(in_bytes),
                o_part = o_match + al256(mb), o_grid = o_part + al256(hb), total = o_grid + plan.grid.grid_bytes;
   int rc;
   if ((rc = ensure(ctx, ctx->icp, total)) != TZR_OK) return rc;
@@ -2480,6 +2506,7 @@ static int icp_batch_run(tzr_ctx* ctx, const tzr_icp_params* params, int mode, i
     memcpy(h.data() + (size_t)probs[b].s_lo * 12, src[b], (size_t)ns[b] * 12);
     memcpy(h.data() + o_dst + (size_t)probs[b].d_lo * 12, dst[b], (size_t)nd[b] * 12);
     if (plane) memcpy(h.data() + o_nrm + (size_t)probs[b].n_lo * 16, dst_normals[b], (size_t)nd[b] * 16);
+    if (gicp) memcpy(h.data() + o_snrm + (size_t)probs[b].sn_lo * 16, src_normals[b], (size_t)ns[b] * 16);
   }
   memcpy(h.data() + o_prob, probs.data(), pb);
   memcpy(h.data() + o_cl, clouds.data(), cb);
@@ -2487,6 +2514,7 @@ static int icp_batch_run(tzr_ctx* ctx, const tzr_icp_params* params, int mode, i
   char* d = (char*)ctx->icp.p;
   CK(cudaMemcpyAsync(d, h.data(), in_bytes, cudaMemcpyHostToDevice, st));
   ctx->launches += launch_icp(plan, (const float*)d, (const float*)(d + o_dst),
+                              gicp ? (const float4*)(d + o_snrm) : nullptr,
                               plane ? (const float4*)(d + o_nrm) : nullptr, (IcpProb*)(d + o_prob),
                               (FpfhCloud*)(d + o_cl), (const int*)(d + o_ck), (int*)(d + o_match),
                               (double*)(d + o_part), plan.grid.grid_bytes ? d + o_grid : nullptr, st);
@@ -2516,20 +2544,29 @@ static int icp_batch_run(tzr_ctx* ctx, const tzr_icp_params* params, int mode, i
 int tzr_icp_batch(tzr_ctx* ctx, const tzr_icp_params* params, int B, const int32_t* ns, const float* const* src,
                   const int32_t* nd, const float* const* dst, const tzr_similarity* init, tzr_icp_result* results,
                   int32_t* const* corr) {
-  return icp_batch_run(ctx, params, kIcpPointToPoint, B, ns, src, nd, dst, nullptr, init, results, corr);
+  return icp_batch_run(ctx, params, kIcpPointToPoint, B, ns, src, nullptr, nd, dst, nullptr, 0.0, init, results, corr);
 }
 
 int tzr_icp_point_to_plane_batch(tzr_ctx* ctx, const tzr_icp_params* params, int B, const int32_t* ns,
                                  const float* const* src, const int32_t* nd, const float* const* dst,
                                  const float* const* dst_normals, const tzr_similarity* init,
                                  tzr_icp_result* results, int32_t* const* corr) {
-  return icp_batch_run(ctx, params, kIcpPointToPlane, B, ns, src, nd, dst, dst_normals, init, results, corr);
+  return icp_batch_run(ctx, params, kIcpPointToPlane, B, ns, src, nullptr, nd, dst, dst_normals, 0.0, init, results,
+                       corr);
+}
+
+int tzr_icp_generalized_batch(tzr_ctx* ctx, const tzr_icp_params* params, double epsilon, int B, const int32_t* ns,
+                              const float* const* src, const float* const* src_normals, const int32_t* nd,
+                              const float* const* dst, const float* const* dst_normals, const tzr_similarity* init,
+                              tzr_icp_result* results, int32_t* const* corr) {
+  return icp_batch_run(ctx, params, kIcpGeneralized, B, ns, src, src_normals, nd, dst, dst_normals, epsilon, init,
+                       results, corr);
 }
 
 // the single-problem entries: icp_batch_run with B = 1 and init NULL meaning the identity
-static int icp_single(tzr_ctx* ctx, const tzr_icp_params* params, int mode, const float* src, int ns, const float* dst,
-                      int nd, const float* dst_normals, const tzr_similarity* init, tzr_icp_result* result,
-                      int32_t* corr) {
+static int icp_single(tzr_ctx* ctx, const tzr_icp_params* params, int mode, const float* src, int ns,
+                      const float* src_normals, const float* dst, int nd, const float* dst_normals, double epsilon,
+                      const tzr_similarity* init, tzr_icp_result* result, int32_t* corr) {
   tzr_similarity id;
   if (!init) {
     memset(&id, 0, sizeof(id));
@@ -2538,19 +2575,26 @@ static int icp_single(tzr_ctx* ctx, const tzr_icp_params* params, int mode, cons
     init = &id;
   }
   int32_t* const corrs[1] = {corr};
-  return icp_batch_run(ctx, params, mode, 1, &ns, &src, &nd, &dst, dst_normals ? &dst_normals : nullptr, init, result,
-                       corr ? corrs : nullptr);
+  return icp_batch_run(ctx, params, mode, 1, &ns, &src, src_normals ? &src_normals : nullptr, &nd, &dst,
+                       dst_normals ? &dst_normals : nullptr, epsilon, init, result, corr ? corrs : nullptr);
 }
 
 int tzr_icp(tzr_ctx* ctx, const tzr_icp_params* params, const float* src, int ns, const float* dst, int nd,
             const tzr_similarity* init, tzr_icp_result* result, int32_t* corr) {
-  return icp_single(ctx, params, kIcpPointToPoint, src, ns, dst, nd, nullptr, init, result, corr);
+  return icp_single(ctx, params, kIcpPointToPoint, src, ns, nullptr, dst, nd, nullptr, 0.0, init, result, corr);
 }
 
 int tzr_icp_point_to_plane(tzr_ctx* ctx, const tzr_icp_params* params, const float* src, int ns, const float* dst,
                            int nd, const float* dst_normals, const tzr_similarity* init, tzr_icp_result* result,
                            int32_t* corr) {
-  return icp_single(ctx, params, kIcpPointToPlane, src, ns, dst, nd, dst_normals, init, result, corr);
+  return icp_single(ctx, params, kIcpPointToPlane, src, ns, nullptr, dst, nd, dst_normals, 0.0, init, result, corr);
+}
+
+int tzr_icp_generalized(tzr_ctx* ctx, const tzr_icp_params* params, double epsilon, const float* src, int ns,
+                        const float* src_normals, const float* dst, int nd, const float* dst_normals,
+                        const tzr_similarity* init, tzr_icp_result* result, int32_t* corr) {
+  return icp_single(ctx, params, kIcpGeneralized, src, ns, src_normals, dst, nd, dst_normals, epsilon, init, result,
+                    corr);
 }
 
 // tzr_voxel_downsample(_batch): the clouds staged back to back (one H2D copy), the batch's launches (launch_voxel), a

@@ -3,6 +3,8 @@
 // own definition in include/teaser_b200.h, for B problems at once.  Point-to-plane ICP (DESIGN.md §3.13) shares the
 // search, the evaluation and the loop, and replaces the covariance and update pair with icp_plane_system_kernel (the
 // centred 6 x 6 Gauss-Newton system) and icp_plane_update_kernel (its pivoted solve and the Euler rotation).
+// Generalized ICP (DESIGN.md §3.14) replaces only the system, with icp_gicp_system_kernel (plane-to-plane covariances
+// from both clouds' normals, the same 27 sums), and shares icp_plane_update_kernel.
 //
 //   icp_nn_kernel      one CTA per chunk of kIcpChunk source points: p = s (R x) + t in float64 (icp_transform), the
 //                      nearest target with d^2 < r^2 (lowest index among equal d^2), by brute force through shared
@@ -358,6 +360,124 @@ __device__ void icp_solve6(const double* __restrict__ Aup, const double* __restr
   for (int s = 0; s < rank; ++s) x[piv[s]] = y[s];
 }
 
+// ---- generalized ICP (DESIGN.md §3.14) --------------------------------------------------------------------------------
+// C(v) = I - (k v_a) v_b with k = (1 - eps) / ((v0 v0 + v1 v1) + v2 v2): the upper triangle (00, 01, 02, 11, 12, 22).
+// Negating v negates k v_a and v_b, so the entries keep their bits.
+__device__ __forceinline__ void gicp_cov(const double v[3], double k, double c[6]) {
+  c[0] = 1.0 - (k * v[0]) * v[0];
+  c[1] = 0.0 - (k * v[0]) * v[1];
+  c[2] = 0.0 - (k * v[0]) * v[2];
+  c[3] = 1.0 - (k * v[1]) * v[1];
+  c[4] = 0.0 - (k * v[1]) * v[2];
+  c[5] = 1.0 - (k * v[2]) * v[2];
+}
+
+// (v0 v0 + v1 v1) + v2 v2 of a normal with three finite components, or 0 (the correspondence adds nothing) otherwise
+__device__ __forceinline__ double gicp_len2(const double v[3]) {
+  if (!(isfinite(v[0]) && isfinite(v[1]) && isfinite(v[2]))) return 0.0;
+  return (v[0] * v[0] + v[1] * v[1]) + v[2] * v[2];
+}
+
+// a x b
+__device__ __forceinline__ void gicp_cross(const double a[3], const double b[3], double o[3]) {
+  o[0] = a[1] * b[2] - a[2] * b[1];
+  o[1] = a[2] * b[0] - a[0] * b[2];
+  o[2] = a[0] * b[1] - a[1] * b[0];
+}
+
+// S v for a symmetric S held as its upper triangle (00, 01, 02, 11, 12, 22), row r: (S(r,0) v0 + S(r,1) v1) + S(r,2) v2
+__device__ __forceinline__ void gicp_symv(const double S[6], const double v[3], double o[3]) {
+  o[0] = (S[0] * v[0] + S[1] * v[1]) + S[2] * v[2];
+  o[1] = (S[1] * v[0] + S[3] * v[1]) + S[4] * v[2];
+  o[2] = (S[2] * v[0] + S[4] * v[1]) + S[5] * v[2];
+}
+
+// One CTA per chunk: each correspondence (i, j) whose source normal m and target normal n are finite and of non-zero
+// length adds J^T A J (21 entries, the plane system's order) and J^T A d (6), with u = p - c, d = p - q,
+// J = [e_k x u (k = 0..2), I] and A = (s^2 C(R m) + C(n))^-1 by the symmetric adjugate (include/teaser_b200.h writes
+// out every formula and its order).  The 27 sums and their layout are the plane system's, so icp_plane_update_kernel
+// solves them unchanged.
+__global__ void __launch_bounds__(kIcpThreads) icp_gicp_system_kernel(IcpArgs a, const float4* __restrict__ src_normals,
+                                                                      const float4* __restrict__ dst_normals,
+                                                                      double epsilon) {
+  __shared__ double s_buf[(kIcpThreads / 32) * kIcpPlaneSums];
+  const int c = blockIdx.x;
+  const int b = a.chunk_prob[c];
+  const IcpProb& pr = a.probs[b];
+  if (!pr.active || pr.count == 0) return;  // the update of no correspondence reads no system
+  const int i = (c - pr.c_lo) * kIcpChunk + threadIdx.x;
+  double v[kIcpPlaneSums];
+#pragma unroll
+  for (int k = 0; k < kIcpPlaneSums; ++k) v[k] = 0.0;
+  const int j = i < pr.ns ? a.match[pr.m_lo + i] : -1;
+  if (j >= 0) {
+    const float4 mf = src_normals[pr.sn_lo + i], nf = dst_normals[pr.n_lo + j];
+    const double m0[3] = {mf.x, mf.y, mf.z}, n[3] = {nf.x, nf.y, nf.z};
+    const double lm = gicp_len2(m0), ln = gicp_len2(n);
+    if (lm > 0.0 && ln > 0.0) {
+      double m[3];  // R m, without the scale
+#pragma unroll
+      for (int r = 0; r < 3; ++r) m[r] = (pr.R[r] * m0[0] + pr.R[3 + r] * m0[1]) + pr.R[6 + r] * m0[2];
+      double Cm[6], Cn[6], M[6];
+      gicp_cov(m, (1.0 - epsilon) / ((m[0] * m[0] + m[1] * m[1]) + m[2] * m[2]), Cm);
+      gicp_cov(n, (1.0 - epsilon) / ln, Cn);
+      const double s2 = pr.s * pr.s;
+#pragma unroll
+      for (int k = 0; k < 6; ++k) M[k] = s2 * Cm[k] + Cn[k];
+      // cofactors of M = [M0 M1 M2; M1 M3 M4; M2 M4 M5]
+      const double c00 = M[3] * M[5] - M[4] * M[4], c01 = M[2] * M[4] - M[1] * M[5], c02 = M[1] * M[4] - M[2] * M[3];
+      const double c11 = M[0] * M[5] - M[2] * M[2], c12 = M[1] * M[2] - M[0] * M[4], c22 = M[0] * M[3] - M[1] * M[1];
+      const double det = (M[0] * c00 + M[1] * c01) + M[2] * c02;
+      if (det > 0.0 && isfinite(det)) {
+        const double A[6] = {c00 / det, c01 / det, c02 / det, c11 / det, c12 / det, c22 / det};
+        double p[3];
+        icp_transform(pr, a.src, pr.s_lo + i, p);
+        const size_t o = 3 * (size_t)(pr.d_lo + j);
+        const double u[3] = {p[0] - pr.mup[0], p[1] - pr.mup[1], p[2] - pr.mup[2]};
+        const double d[3] = {p[0] - (double)a.dst[o], p[1] - (double)a.dst[o + 1], p[2] - (double)a.dst[o + 2]};
+        // ww[l] = u x A (e_l x u), wt[l] = u x A e_l: column l of the omega-omega and omega-tau blocks
+        double ww[3][3], wt[3][3];
+#pragma unroll
+        for (int l = 0; l < 3; ++l) {
+          const double e[3] = {l == 0 ? 1.0 : 0.0, l == 1 ? 1.0 : 0.0, l == 2 ? 1.0 : 0.0};
+          double eu[3], Aeu[3], Ae[3];
+          gicp_cross(e, u, eu);
+          gicp_symv(A, eu, Aeu);
+          gicp_cross(u, Aeu, ww[l]);
+          Ae[0] = A[l == 0 ? 0 : l == 1 ? 1 : 2];
+          Ae[1] = A[l == 0 ? 1 : l == 1 ? 3 : 4];
+          Ae[2] = A[l == 0 ? 2 : l == 1 ? 4 : 5];
+          gicp_cross(u, Ae, wt[l]);
+        }
+        int k = 0;
+#pragma unroll
+        for (int row = 0; row < 3; ++row) {
+#pragma unroll
+          for (int col = row; col < 3; ++col) v[k++] = ww[col][row];
+#pragma unroll
+          for (int col = 0; col < 3; ++col) v[k++] = wt[col][row];
+        }
+        v[k++] = A[0];
+        v[k++] = A[1];
+        v[k++] = A[2];
+        v[k++] = A[3];
+        v[k++] = A[4];
+        v[k++] = A[5];
+        double w[3], uw[3];
+        gicp_symv(A, d, w);
+        gicp_cross(u, w, uw);
+        v[21] = uw[0];
+        v[22] = uw[1];
+        v[23] = uw[2];
+        v[24] = w[0];
+        v[25] = w[1];
+        v[26] = w[2];
+      }
+    }
+  }
+  icp_block_sum<kIcpPlaneSums>(v, s_buf, a.partial + kIcpPlaneSums * (size_t)c);
+}
+
 __global__ void icp_plane_update_kernel(IcpArgs a) {
   IcpProb& pr = a.probs[blockIdx.x];
   if (!pr.active) return;
@@ -417,9 +537,9 @@ int launch_icp_seed(IcpProb* probs, int B, const tzr_solution* sol, cudaStream_t
   return 1;
 }
 
-int launch_icp(const IcpPlan& plan, const float* src, const float* dst, const float4* dst_normals, IcpProb* probs,
-               FpfhCloud* clouds, const int* chunk_prob, int* match, double* partial, void* grid_scratch,
-               cudaStream_t st) {
+int launch_icp(const IcpPlan& plan, const float* src, const float* dst, const float4* src_normals,
+               const float4* dst_normals, IcpProb* probs, FpfhCloud* clouds, const int* chunk_prob, int* match,
+               double* partial, void* grid_scratch, cudaStream_t st) {
   int nl = 0;
   IcpArgs a{src, dst, probs, clouds, chunk_prob, match, partial, nullptr, nullptr, nullptr, plan.r2};
   if (plan.grid.any_grid) nl += launch_fpfh_grid(plan.grid, dst, clouds, grid_scratch, st, &a.sorted, &a.bstart, &a.bend);
@@ -429,6 +549,9 @@ int launch_icp(const IcpPlan& plan, const float* src, const float* dst, const fl
   for (int it = 0; it < plan.max_iteration; ++it) {
     if (plan.mode == kIcpPointToPlane) {
       icp_plane_system_kernel<<<plan.chunks, kIcpThreads, 0, st>>>(a, dst_normals);
+      icp_plane_update_kernel<<<plan.B, 32, 0, st>>>(a);
+    } else if (plan.mode == kIcpGeneralized) {
+      icp_gicp_system_kernel<<<plan.chunks, kIcpThreads, 0, st>>>(a, src_normals, dst_normals, plan.epsilon);
       icp_plane_update_kernel<<<plan.B, 32, 0, st>>>(a);
     } else {
       icp_cov_kernel<<<plan.chunks, kIcpThreads, 0, st>>>(a);

@@ -426,14 +426,15 @@ int launch_pair_rows(const MatchPlan& plan, const MatchPair* pairs, const int2* 
 int launch_corr_gather(const PairGather* table, int n_entries, int max_count, const int32_t* pairs, const float* pts,
                        int2* corr, double* src, double* dst, cudaStream_t st);
 
-// icp.cu (point-to-point ICP, DESIGN.md §3.11, and point-to-plane ICP, §3.13): B problems, sources back to back and
-// targets back to back
+// icp.cu (point-to-point ICP, DESIGN.md §3.11, point-to-plane ICP, §3.13, and generalized ICP, §3.14): B problems,
+// sources back to back and targets back to back
 constexpr int kIcpChunk = 256;    // source points per chunk: the unit of the fixed-order reductions (one CTA each)
 constexpr int kIcpGridMinN = 1024;  // targets from which the nearest-neighbour search goes through the hashed grid
-constexpr int kIcpPointToPoint = 0, kIcpPointToPlane = 1;  // IcpPlan::mode
-constexpr int kIcpPlaneSums = 27;  // doubles per chunk of the point-to-plane system: 21 of J J^T, 6 of J r
+constexpr int kIcpPointToPoint = 0, kIcpPointToPlane = 1, kIcpGeneralized = 2;  // IcpPlan::mode
+// doubles per chunk of the point-to-plane and generalized systems: 21 of the upper triangle of A, 6 of g
+constexpr int kIcpPlaneSums = 27;
 // doubles per chunk of launch_icp's partial buffer (the point-to-point pass sums 9)
-inline int icp_partial_stride(int mode) { return mode == kIcpPointToPlane ? kIcpPlaneSums : 9; }
+inline int icp_partial_stride(int mode) { return mode == kIcpPointToPoint ? 9 : kIcpPlaneSums; }
 struct IcpProb {        // one per problem, device-resident; the host fills the inputs, the kernels the rest
   int s_lo, ns;         // sources: flat points [s_lo, s_lo + ns)
   int d_lo, nd;         // targets: flat points [d_lo, d_lo + nd) (also FpfhCloud b of the target table)
@@ -444,7 +445,8 @@ struct IcpProb {        // one per problem, device-resident; the host fills the 
   int m_lo;             // first entry of the problem in the per-point match array
   int tc;               // its target's entry in the FpfhCloud table of the targets (lo = d_lo)
   int seeded;           // 1: the problem runs (tzr_register_cloud_pairs_icp: 0 for a pair without a valid solution)
-  int n_lo;             // point-to-plane: the normal of target j is normals[n_lo + j]
+  int n_lo;             // point-to-plane and generalized: the normal of target j is dst_normals[n_lo + j]
+  int sn_lo;            // generalized: the normal of source i is src_normals[sn_lo + i]
   double s;             // fixed scale
   double R[9], t[3];    // current transform (column-major R)
   double fitness, rmse; // evaluation of the current transform
@@ -455,17 +457,19 @@ struct IcpPlan {
   int max_iteration = 0;
   int mode = kIcpPointToPoint;
   double r2 = 0, relative_fitness = 0, relative_rmse = 0;
+  double epsilon = 0;   // generalized: the covariances' epsilon (finite, > 0)
   FpfhPlan grid;        // the target grid (fpfh_plan with both radii = r)
 };
-// src (NS x 3 floats), dst (ND x 3 floats), dst_normals (point-to-plane: the target normals, (nx, ny, nz, curvature) per
-// point; unused and may be nullptr for point-to-point), probs (B), clouds (B, fpfh_plan's table of the targets),
+// src (NS x 3 floats), dst (ND x 3 floats), src_normals (generalized: the source normals, (nx, ny, nz, curvature) per
+// point; unused and may be nullptr otherwise), dst_normals (point-to-plane and generalized: the target normals, same
+// layout; unused and may be nullptr for point-to-point), probs (B), clouds (B, fpfh_plan's table of the targets),
 // chunk_prob (chunks: the problem of every chunk), match (target index or -1 per source point from m_lo, final
 // correspondences), partial (chunks x icp_partial_stride(plan.mode) doubles), grid_scratch (plan.grid.grid_bytes): device
 // pointers.  Enqueues every iteration without synchronising; returns the launches: 4 for the grid build (when some target
-// uses it) + 2 + 4 * max_iteration, in either mode.
-int launch_icp(const IcpPlan& plan, const float* src, const float* dst, const float4* dst_normals, IcpProb* probs,
-               FpfhCloud* clouds, const int* chunk_prob, int* match, double* partial, void* grid_scratch,
-               cudaStream_t st);
+// uses it) + 2 + 4 * max_iteration, in every mode.
+int launch_icp(const IcpPlan& plan, const float* src, const float* dst, const float4* src_normals,
+               const float4* dst_normals, IcpProb* probs, FpfhCloud* clouds, const int* chunk_prob, int* match,
+               double* partial, void* grid_scratch, cudaStream_t st);
 // The seeds of B problems from B solution records (tzr_register_cloud_pairs_icp): a valid record with a finite transform
 // and a positive scale sets (s, R, t) and active = seeded = 1, any other leaves the problem inactive.  One launch.
 int launch_icp_seed(IcpProb* probs, int B, const tzr_solution* sol, cudaStream_t st);

@@ -2,8 +2,9 @@
 // (examples/teaser_python_fpfh_icp: Open3D's registration_icp with TransformationEstimationPointToPoint), on the GPU
 // through the C-ABI (tzr_icp, tzr_icp_batch; include/teaser_b200.h defines the loop).  teaser::PointToPlaneICP is the
 // same with TransformationEstimationPointToPlane (tzr_icp_point_to_plane, tzr_icp_point_to_plane_batch), given the
-// target normals (teaser::estimateNormals, teaser/normals.h).  No CPU implementation: without a CUDA device the first
-// call throws std::runtime_error.
+// target normals (teaser::estimateNormals, teaser/normals.h).  teaser::GeneralizedICP is the same with Open3D's
+// registration_generalized_icp (tzr_icp_generalized, tzr_icp_generalized_batch), given both clouds' normals.  No CPU
+// implementation: without a CUDA device the first call throws std::runtime_error.
 #pragma once
 
 #include <vector>
@@ -50,6 +51,33 @@ class PointToPlaneICP {
   // Many problems in one device call (tzr_icp_point_to_plane_batch); result b is refine(src[b], dst[b],
   // dst_normals[b], init[b]) bit for bit.
   std::vector<Result> refineBatch(const std::vector<PointCloud>& src, const std::vector<PointCloud>& dst,
+                                  const std::vector<NormalCloud>& dst_normals,
+                                  const std::vector<RegistrationSolution>& init) const;
+
+  const Params& getParams() const { return params_; }
+  void setParams(const Params& params) { params_ = params; }
+
+ private:
+  Params params_;
+};
+
+class GeneralizedICP {
+ public:
+  using Params = GeneralizedICPParams;
+  using Result = PointToPointICPResult;
+
+  GeneralizedICP() = default;
+  explicit GeneralizedICP(const Params& params) : params_(params) {}
+
+  // Generalized ICP of src onto dst seeded with init (its scale held fixed), on this thread's context.  src_normals /
+  // dst_normals: one normal per source / target point (curvature ignored; used up to length and sign).  Both clouds
+  // non-empty.
+  Result refine(const PointCloud& src, const PointCloud& dst, const NormalCloud& src_normals,
+                const NormalCloud& dst_normals, const RegistrationSolution& init) const;
+  // Many problems in one device call (tzr_icp_generalized_batch); result b is refine(src[b], dst[b], src_normals[b],
+  // dst_normals[b], init[b]) bit for bit.
+  std::vector<Result> refineBatch(const std::vector<PointCloud>& src, const std::vector<PointCloud>& dst,
+                                  const std::vector<NormalCloud>& src_normals,
                                   const std::vector<NormalCloud>& dst_normals,
                                   const std::vector<RegistrationSolution>& init) const;
 

@@ -55,6 +55,11 @@ struct PointToPointICPParams {
   double relative_fitness = 1e-6;
   double relative_rmse = 1e-6;
 };
+// Generalized ICP (teaser/icp.h, tzr_icp_generalized): PointToPointICP's parameters plus Open3D's epsilon of the
+// plane-to-plane covariances (finite, > 0).
+struct GeneralizedICPParams : PointToPointICPParams {
+  double epsilon = 1e-3;
+};
 struct PointToPointICPResult {
   RegistrationSolution solution;  // the refined transform; scale is the seed's, held fixed
   double fitness = 0;
@@ -341,6 +346,12 @@ class RobustRegistrationSolver {
                                                               const std::vector<std::pair<int, int>>& pairs,
                                                               const CloudPairParams& params,
                                                               const PointToPointICPParams& icp);
+  // The overload above with generalized ICP (tzr_register_cloud_pairs_icp_generalized): both clouds' normals are the
+  // ones the call's FPFH stage computed at params.normal_search_radius.
+  std::vector<CloudPairICPResult> solveCloudPairsGeneralizedICP(const std::vector<PointCloud>& clouds,
+                                                                const std::vector<std::pair<int, int>>& pairs,
+                                                                const CloudPairParams& params,
+                                                                const GeneralizedICPParams& icp);
   bool isMaxCliqueProvenOptimal() const { return clique_proven_; }
   long long getNumInlierGraphEdges() const { return n_edges_; }
   int getGNCRotationIterations() const { return gnc_iterations_; }

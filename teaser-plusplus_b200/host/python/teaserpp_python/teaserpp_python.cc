@@ -218,6 +218,54 @@ PYBIND11_MODULE(_teaserpp, m) {
            },
            py::arg("src"), py::arg("dst"), py::arg("dst_normals"), py::arg("init"));
 
+  // GPU extra: generalized ICP (teaser::GeneralizedICP), given both clouds' normals
+  py::class_<teaser::GeneralizedICP>(m, "GeneralizedICP")
+      .def(py::init([](double max_correspondence_distance, int max_iteration, double relative_fitness,
+                       double relative_rmse, double epsilon) {
+             teaser::GeneralizedICP::Params p;
+             p.max_correspondence_distance = max_correspondence_distance;
+             p.max_iteration = max_iteration;
+             p.relative_fitness = relative_fitness;
+             p.relative_rmse = relative_rmse;
+             p.epsilon = epsilon;
+             return teaser::GeneralizedICP(p);
+           }),
+           py::arg("max_correspondence_distance"), py::arg("max_iteration") = 30, py::arg("relative_fitness") = 1e-6,
+           py::arg("relative_rmse") = 1e-6, py::arg("epsilon") = 1e-3)
+      .def("refine",
+           [](const teaser::GeneralizedICP& icp, const CloudArray& src, const CloudArray& dst,
+              const CloudArray& src_normals, const CloudArray& dst_normals, const teaser::RegistrationSolution& init) {
+             const teaser::PointCloud s = cloud_of(src), d = cloud_of(dst);
+             const teaser::NormalCloud sn = normals_of(src_normals), dn = normals_of(dst_normals);
+             teaser::GeneralizedICP::Result r;
+             {
+               py::gil_scoped_release release;
+               r = icp.refine(s, d, sn, dn, init);
+             }
+             return icp_dict(r);
+           },
+           py::arg("src"), py::arg("dst"), py::arg("src_normals"), py::arg("dst_normals"), py::arg("init"))
+      .def("refine_batch",
+           [](const teaser::GeneralizedICP& icp, const std::vector<CloudArray>& src, const std::vector<CloudArray>& dst,
+              const std::vector<CloudArray>& src_normals, const std::vector<CloudArray>& dst_normals,
+              const std::vector<teaser::RegistrationSolution>& init) {
+             std::vector<teaser::PointCloud> s, d;
+             std::vector<teaser::NormalCloud> sn, dn;
+             for (const auto& a : src) s.push_back(cloud_of(a));
+             for (const auto& a : dst) d.push_back(cloud_of(a));
+             for (const auto& a : src_normals) sn.push_back(normals_of(a));
+             for (const auto& a : dst_normals) dn.push_back(normals_of(a));
+             std::vector<teaser::GeneralizedICP::Result> res;
+             {
+               py::gil_scoped_release release;
+               res = icp.refineBatch(s, d, sn, dn, init);
+             }
+             py::list out;
+             for (const auto& r : res) out.append(icp_dict(r));
+             return out;
+           },
+           py::arg("src"), py::arg("dst"), py::arg("src_normals"), py::arg("dst_normals"), py::arg("init"));
+
   // GPU extra: FPFHEstimation's normals alone (teaser::estimateNormals), as (n,4) float32 (nx, ny, nz, curvature)
   m.def("estimate_normals",
         [](const CloudArray& points, double normal_search_radius) {
@@ -385,11 +433,11 @@ PYBIND11_MODULE(_teaserpp, m) {
            [](Solver& s, const std::vector<CloudArray>& clouds, const std::vector<std::pair<int, int>>& pairs,
               double max_correspondence_distance, int max_iteration, double relative_fitness, double relative_rmse,
               double normal_search_radius, double fpfh_search_radius, bool use_absolute_scale, bool use_crosscheck,
-              bool use_tuple_test, float tuple_scale, uint64_t tuple_seed, const std::string& method) {
-             // GPU extra: solve_cloud_pairs, then point-to-point (or point-to-plane) ICP of every pair with a valid
-             // solution, in one call
-             if (method != "point_to_point" && method != "point_to_plane")
-               throw std::invalid_argument("method must be \"point_to_point\" or \"point_to_plane\"");
+              bool use_tuple_test, float tuple_scale, uint64_t tuple_seed, const std::string& method, double epsilon) {
+             // GPU extra: solve_cloud_pairs, then point-to-point (point-to-plane, generalized) ICP of every pair with a
+             // valid solution, in one call
+             if (method != "point_to_point" && method != "point_to_plane" && method != "generalized")
+               throw std::invalid_argument("method must be \"point_to_point\", \"point_to_plane\" or \"generalized\"");
              std::vector<teaser::PointCloud> pcs;
              for (const auto& a : clouds) pcs.push_back(cloud_of(a));
              Solver::CloudPairParams cp;
@@ -400,16 +448,18 @@ PYBIND11_MODULE(_teaserpp, m) {
              cp.use_tuple_test = use_tuple_test;
              cp.tuple_scale = tuple_scale;
              cp.tuple_seed = tuple_seed;
-             teaser::PointToPointICP::Params ip;
+             teaser::GeneralizedICP::Params ip;
              ip.max_correspondence_distance = max_correspondence_distance;
              ip.max_iteration = max_iteration;
              ip.relative_fitness = relative_fitness;
              ip.relative_rmse = relative_rmse;
+             ip.epsilon = epsilon;
              std::vector<Solver::CloudPairICPResult> res;
              {
                py::gil_scoped_release release;
-               res = method == "point_to_plane" ? s.solveCloudPairsPointToPlane(pcs, pairs, cp, ip)
-                                                : s.solveCloudPairs(pcs, pairs, cp, ip);
+               res = method == "generalized"      ? s.solveCloudPairsGeneralizedICP(pcs, pairs, cp, ip)
+                     : method == "point_to_plane" ? s.solveCloudPairsPointToPlane(pcs, pairs, cp, ip)
+                                                  : s.solveCloudPairs(pcs, pairs, cp, ip);
              }
              py::list out;
              for (const auto& r : res)
@@ -423,7 +473,7 @@ PYBIND11_MODULE(_teaserpp, m) {
            py::arg("relative_fitness") = 1e-6, py::arg("relative_rmse") = 1e-6, py::arg("normal_search_radius") = 0.03,
            py::arg("fpfh_search_radius") = 0.05, py::arg("use_absolute_scale") = true, py::arg("use_crosscheck") = true,
            py::arg("use_tuple_test") = true, py::arg("tuple_scale") = 0.0f, py::arg("tuple_seed") = 0x7ea5e2ull,
-           py::arg("method") = "point_to_point")
+           py::arg("method") = "point_to_point", py::arg("epsilon") = 1e-3)
       .def_property_readonly("solution", &Solver::getSolution)
       .def("getSolution", &Solver::getSolution)
       .def_property_readonly("gnc_rotation_cost_at_termination", &Solver::getGNCRotationCostAtTermination)

@@ -1,5 +1,5 @@
-// teaser::PointToPointICP and teaser::PointToPlaneICP (teaser/icp.h) on top of the C-ABI: marshalling only, the loop
-// runs in libteaser_b200.so.
+// teaser::PointToPointICP, teaser::PointToPlaneICP and teaser::GeneralizedICP (teaser/icp.h) on top of the C-ABI:
+// marshalling only, the loop runs in libteaser_b200.so.
 #include "teaser/icp.h"
 
 #include <cstring>
@@ -51,20 +51,24 @@ void icp_result_from_c(const tzr_icp_result& r, const int32_t* corr, PointToPoin
 
 namespace {
 
-// both classes' refineBatch: point-to-point when dst_normals is null
+// every class's refineBatch: point-to-point when dst_normals is null, generalized when src_normals is given (with
+// epsilon), point-to-plane otherwise
 std::vector<PointToPointICPResult> refine_batch(const char* who, const PointToPointICPParams& params,
                                                 const std::vector<PointCloud>& src, const std::vector<PointCloud>& dst,
                                                 const std::vector<NormalCloud>* dst_normals,
-                                                const std::vector<RegistrationSolution>& init) {
+                                                const std::vector<RegistrationSolution>& init,
+                                                const std::vector<NormalCloud>* src_normals = nullptr,
+                                                double epsilon = 0) {
   const size_t B = src.size();
-  if (dst.size() != B || init.size() != B || (dst_normals && dst_normals->size() != B))
+  if (dst.size() != B || init.size() != B || (dst_normals && dst_normals->size() != B) ||
+      (src_normals && src_normals->size() != B))
     throw std::invalid_argument(std::string(who) + ": one target and seed (and normal cloud) per source");
   std::vector<PointToPointICPResult> out(B);
   if (B == 0) return out;
   static_assert(sizeof(PointXYZ) == 3 * sizeof(float), "PointXYZ must be three packed floats");
   static_assert(sizeof(Normal) == 4 * sizeof(float), "Normal must be 4 packed floats");
   std::vector<int32_t> ns(B), nd(B);
-  std::vector<const float*> sp(B), dp(B), np(B, nullptr);
+  std::vector<const float*> sp(B), dp(B), np(B, nullptr), snp(B, nullptr);
   std::vector<tzr_similarity> seeds(B);
   std::vector<std::vector<int32_t>> corr(B);
   std::vector<int32_t*> corr_p(B);
@@ -79,6 +83,11 @@ std::vector<PointToPointICPResult> refine_batch(const char* who, const PointToPo
         throw std::invalid_argument(std::string(who) + ": one normal per target point");
       np[b] = &(*dst_normals)[b][0].normal_x;
     }
+    if (src_normals) {
+      if ((*src_normals)[b].size() != src[b].size())
+        throw std::invalid_argument(std::string(who) + ": one normal per source point");
+      snp[b] = &(*src_normals)[b][0].normal_x;
+    }
     seeds[b] = to_c(init[b]);
     corr[b].resize(2 * src[b].size());
     corr_p[b] = corr[b].data();
@@ -88,7 +97,12 @@ std::vector<PointToPointICPResult> refine_batch(const char* who, const PointToPo
   tzr_ctx* ctx = b200_context();
   const int Bi = static_cast<int>(B);
   int rc;
-  if (!dst_normals)
+  if (src_normals)
+    rc = B == 1 ? tzr_icp_generalized(ctx, &p, epsilon, sp[0], ns[0], snp[0], dp[0], nd[0], np[0], seeds.data(),
+                                      res.data(), corr_p[0])
+                : tzr_icp_generalized_batch(ctx, &p, epsilon, Bi, ns.data(), sp.data(), snp.data(), nd.data(),
+                                            dp.data(), np.data(), seeds.data(), res.data(), corr_p.data());
+  else if (!dst_normals)
     rc = B == 1 ? tzr_icp(ctx, &p, sp[0], ns[0], dp[0], nd[0], seeds.data(), res.data(), corr_p[0])
                 : tzr_icp_batch(ctx, &p, Bi, ns.data(), sp.data(), nd.data(), dp.data(), seeds.data(), res.data(),
                                 corr_p.data());
@@ -127,6 +141,20 @@ std::vector<PointToPlaneICP::Result> PointToPlaneICP::refineBatch(const std::vec
                                                                   const std::vector<NormalCloud>& dst_normals,
                                                                   const std::vector<RegistrationSolution>& init) const {
   return refine_batch("PointToPlaneICP", params_, src, dst, &dst_normals, init);
+}
+
+GeneralizedICP::Result GeneralizedICP::refine(const PointCloud& src, const PointCloud& dst,
+                                              const NormalCloud& src_normals, const NormalCloud& dst_normals,
+                                              const RegistrationSolution& init) const {
+  return refineBatch({src}, {dst}, {src_normals}, {dst_normals}, {init})[0];
+}
+
+std::vector<GeneralizedICP::Result> GeneralizedICP::refineBatch(const std::vector<PointCloud>& src,
+                                                                const std::vector<PointCloud>& dst,
+                                                                const std::vector<NormalCloud>& src_normals,
+                                                                const std::vector<NormalCloud>& dst_normals,
+                                                                const std::vector<RegistrationSolution>& init) const {
+  return refine_batch("GeneralizedICP", params_, src, dst, &dst_normals, init, &src_normals, params_.epsilon);
 }
 
 }  // namespace teaser

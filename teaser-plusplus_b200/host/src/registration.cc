@@ -631,12 +631,13 @@ void icp_result_from_c(const tzr_icp_result& r, const int32_t* corr, PointToPoin
 
 namespace {
 
-// solveCloudPairs' body: tzr_register_cloud_pairs, or tzr_register_cloud_pairs_icp(_point_to_plane) when icp is given
-// (icp_res then receives P records)
+// solveCloudPairs' body: tzr_register_cloud_pairs, or tzr_register_cloud_pairs_icp(_point_to_plane, _generalized) when
+// icp is given (icp_res then receives P records)
+enum class IcpMethod { kPointToPoint, kPointToPlane, kGeneralized };
 std::vector<RobustRegistrationSolver::CloudPairResult> run_cloud_pairs(
     const tzr_params& p, const std::vector<PointCloud>& clouds, const std::vector<std::pair<int, int>>& pairs,
     const RobustRegistrationSolver::CloudPairParams& cp, const tzr_icp_params* icp,
-    std::vector<tzr_icp_result>* icp_res, bool point_to_plane = false) {
+    std::vector<tzr_icp_result>* icp_res, IcpMethod method = IcpMethod::kPointToPoint, double epsilon = 0) {
   using CloudPairResult = RobustRegistrationSolver::CloudPairResult;
   const int K = static_cast<int>(clouds.size()), P = static_cast<int>(pairs.size());
   std::vector<CloudPairResult> out(P);
@@ -683,9 +684,16 @@ std::vector<RobustRegistrationSolver::CloudPairResult> run_cloud_pairs(
                                   scales.data());
   } else {
     icp_res->assign(P, tzr_icp_result{});
-    rc = (point_to_plane ? tzr_register_cloud_pairs_icp_point_to_plane : tzr_register_cloud_pairs_icp)(
-        ctx, &f, &p, K, n.data(), pts.data(), P, pc.data(), seeds.data(), sols.data(), status.data(), index.data(),
-        n_corr.data(), corr_p.data(), clq_p.data(), scales.data(), icp, icp_res->data());
+    if (method == IcpMethod::kGeneralized)
+      rc = tzr_register_cloud_pairs_icp_generalized(ctx, &f, &p, K, n.data(), pts.data(), P, pc.data(), seeds.data(),
+                                                    sols.data(), status.data(), index.data(), n_corr.data(),
+                                                    corr_p.data(), clq_p.data(), scales.data(), icp, epsilon,
+                                                    icp_res->data());
+    else
+      rc = (method == IcpMethod::kPointToPlane ? tzr_register_cloud_pairs_icp_point_to_plane
+                                               : tzr_register_cloud_pairs_icp)(
+          ctx, &f, &p, K, n.data(), pts.data(), P, pc.data(), seeds.data(), sols.data(), status.data(), index.data(),
+          n_corr.data(), corr_p.data(), clq_p.data(), scales.data(), icp, icp_res->data());
   }
   if (rc != TZR_OK && rc != TZR_ERR_TOO_LARGE) fail("RobustRegistrationSolver::solveCloudPairs", rc, ctx);
   for (int q = 0; q < P; ++q) {
@@ -710,10 +718,11 @@ std::vector<RobustRegistrationSolver::CloudPairResult> RobustRegistrationSolver:
   return run_cloud_pairs(to_c(params_), clouds, pairs, cp, nullptr, nullptr);
 }
 
-// both ICP overloads of solveCloudPairs
+// every ICP overload of solveCloudPairs
 static std::vector<RobustRegistrationSolver::CloudPairICPResult> run_cloud_pairs_icp(
     const tzr_params& p, const std::vector<PointCloud>& clouds, const std::vector<std::pair<int, int>>& pairs,
-    const RobustRegistrationSolver::CloudPairParams& cp, const PointToPointICPParams& icp, bool point_to_plane) {
+    const RobustRegistrationSolver::CloudPairParams& cp, const PointToPointICPParams& icp, IcpMethod method,
+    double epsilon = 0) {
   using CloudPairResult = RobustRegistrationSolver::CloudPairResult;
   using CloudPairICPResult = RobustRegistrationSolver::CloudPairICPResult;
   tzr_icp_params ip;
@@ -723,7 +732,7 @@ static std::vector<RobustRegistrationSolver::CloudPairICPResult> run_cloud_pairs
   ip.relative_fitness = icp.relative_fitness;
   ip.relative_rmse = icp.relative_rmse;
   std::vector<tzr_icp_result> res;
-  std::vector<CloudPairResult> base = run_cloud_pairs(p, clouds, pairs, cp, &ip, &res, point_to_plane);
+  std::vector<CloudPairResult> base = run_cloud_pairs(p, clouds, pairs, cp, &ip, &res, method, epsilon);
   std::vector<CloudPairICPResult> out(base.size());
   for (size_t q = 0; q < base.size(); ++q) {
     static_cast<CloudPairResult&>(out[q]) = std::move(base[q]);
@@ -737,13 +746,19 @@ static std::vector<RobustRegistrationSolver::CloudPairICPResult> run_cloud_pairs
 std::vector<RobustRegistrationSolver::CloudPairICPResult> RobustRegistrationSolver::solveCloudPairs(
     const std::vector<PointCloud>& clouds, const std::vector<std::pair<int, int>>& pairs, const CloudPairParams& cp,
     const PointToPointICPParams& icp) {
-  return run_cloud_pairs_icp(to_c(params_), clouds, pairs, cp, icp, false);
+  return run_cloud_pairs_icp(to_c(params_), clouds, pairs, cp, icp, IcpMethod::kPointToPoint);
 }
 
 std::vector<RobustRegistrationSolver::CloudPairICPResult> RobustRegistrationSolver::solveCloudPairsPointToPlane(
     const std::vector<PointCloud>& clouds, const std::vector<std::pair<int, int>>& pairs, const CloudPairParams& cp,
     const PointToPointICPParams& icp) {
-  return run_cloud_pairs_icp(to_c(params_), clouds, pairs, cp, icp, true);
+  return run_cloud_pairs_icp(to_c(params_), clouds, pairs, cp, icp, IcpMethod::kPointToPlane);
+}
+
+std::vector<RobustRegistrationSolver::CloudPairICPResult> RobustRegistrationSolver::solveCloudPairsGeneralizedICP(
+    const std::vector<PointCloud>& clouds, const std::vector<std::pair<int, int>>& pairs, const CloudPairParams& cp,
+    const GeneralizedICPParams& icp) {
+  return run_cloud_pairs_icp(to_c(params_), clouds, pairs, cp, icp, IcpMethod::kGeneralized, icp.epsilon);
 }
 
 void RobustRegistrationSolver::materialise_tims() {
