@@ -675,6 +675,85 @@ int tzr_register_cloud_pairs_icp_generalized(tzr_ctx* ctx, const tzr_frontend_pa
                                              int32_t* const* cliques, float* global_scale, const tzr_icp_params* icp,
                                              double epsilon, tzr_icp_result* icp_results);
 
+/* ---- refining registrations: robust kernels ------------------------------------------------------------------
+ * Open3D's robust kernels (L1Loss, HuberLoss, CauchyLoss, GMLoss, TukeyLoss) for point-to-plane ICP
+ * (TransformationEstimationPointToPlane(kernel)) and generalized ICP (TransformationEstimationForGeneralizedICP(epsilon,
+ * kernel)), for many problems at once, defined here as follows (DESIGN.md §3.15):
+ *   - Unchanged from tzr_icp_point_to_plane and tzr_icp_generalized: the inputs, the search and both of its routes,
+ *     eval(T) (fitness and inlier_rmse stay unweighted, as in Open3D), the loop, the convergence test, the 6 x 6 solve,
+ *     R_u, t_u and the composition.  Only each correspondence's contribution to the system is weighted.
+ *   - Weights, in IEEE float64 with no FMA contraction, from e = |r| (a residual's sign never matters), k = kernel->k:
+ *       TZR_LOSS_L2      1
+ *       TZR_LOSS_L1      1 / e
+ *       TZR_LOSS_HUBER   k / max(e, k)
+ *       TZR_LOSS_CAUCHY  q = e / k, then 1 / (1 + q q)
+ *       TZR_LOSS_GM      t = k + e e, then k / (t t)  (k in squared residual units, as Open3D's GMLoss)
+ *       TZR_LOSS_TUKEY   0 when e > k; otherwise q = e / k, t = 1 - q q, then t t
+ *     Each is rho'(r) / r of Open3D's published rho.  A weight that is not finite (L1 at e = 0) removes that residual's
+ *     correspondence from the system; it still counts for fitness and rmse.  (Open3D would multiply an infinite weight by
+ *     a zero residual and put NaN into its normal equations.)
+ *   - Point-to-plane: w = weight(r) with tzr_icp_point_to_plane's r and J; the correspondence adds (w J_a) J_b to the 21
+ *     upper entries and (w J_a) r to g.  With w = 1 these are J_a J_b and J_a r bit for bit.
+ *   - Generalized: M = s2 C(m') + C(n) as tzr_icp_generalized's.  W = M^-1/2 from the two-sided Jacobi SVD of the
+ *     rotation stage (M = V diag(sigma) V^T for the symmetric positive definite M, sigma descending), with
+ *     q_k = 1 / sqrt(sigma_k) and W_ab = ((V_a0 q_0) V_b0 + (V_a1 q_1) V_b1) + (V_a2 q_2) V_b2.  The three whitened
+ *     residuals r_k = (W_k0 d0 + W_k1 d1) + W_k2 d2 (d = p_i - y_j) give w_k = weight(r_k), and
+ *     A~_ab = ((w_0 W_0a) W_0b + (w_1 W_1a) W_1b) + (w_2 W_2a) W_2b, i.e. W diag(w) W, the sum over Open3D's three
+ *     weighted rows.  A~ replaces A in tzr_icp_generalized's J^T A J and J^T A d, evaluated as written there.
+ *     M and so every output does not depend on either normal's sign.  A correspondence adds nothing, but still counts
+ *     for fitness and rmse, when either normal has a non-finite component or zero length, when some sigma_k is not > 0
+ *     or not finite, or when some w_k is not finite.
+ *   - TZR_LOSS_L2 runs tzr_icp_point_to_plane's or tzr_icp_generalized's own system (the adjugate inverse), so its
+ *     results are bit-identical to those entries'.  (W W equals M^-1 only up to rounding.)
+ *   - kernel NULL, an unknown type, or a k that is not finite and > 0 for HUBER, CAUCHY, GM and TUKEY (k is ignored for
+ *     L2 and L1) is TZR_ERR_INVALID_ARG, checked before any device work.
+ * Launches: 2 + 4 * max_iteration (+ 4 for the grid build when some target has at least 1024 points), whatever B, as
+ * tzr_icp_batch.  Workspace: tzr_icp's own, so a retained solve stays retained. */
+#define TZR_LOSS_L2 0
+#define TZR_LOSS_L1 1
+#define TZR_LOSS_HUBER 2
+#define TZR_LOSS_CAUCHY 3
+#define TZR_LOSS_GM 4
+#define TZR_LOSS_TUKEY 5
+
+typedef struct tzr_robust_kernel {
+  int32_t type;     /* TZR_LOSS_* */
+  int32_t reserved; /* 0 */
+  double k;         /* finite and > 0 for HUBER, CAUCHY, GM and TUKEY; ignored for L2 and L1 */
+} tzr_robust_kernel;
+
+/* B ragged problems: tzr_icp_point_to_plane_batch's arguments plus the kernel.  Per problem, every output is
+ * bit-identical to the same call on that problem alone. */
+int tzr_icp_point_to_plane_robust_batch(tzr_ctx* ctx, const tzr_icp_params* params, int B, const int32_t* ns,
+                                        const float* const* src, const int32_t* nd, const float* const* dst,
+                                        const float* const* dst_normals, const tzr_similarity* init,
+                                        tzr_icp_result* results, int32_t* const* corr,
+                                        const tzr_robust_kernel* kernel);
+
+/* B ragged problems: tzr_icp_generalized_batch's arguments plus the kernel.  Per problem, every output is bit-identical
+ * to the same call on that problem alone. */
+int tzr_icp_generalized_robust_batch(tzr_ctx* ctx, const tzr_icp_params* params, double epsilon, int B,
+                                     const int32_t* ns, const float* const* src, const float* const* src_normals,
+                                     const int32_t* nd, const float* const* dst, const float* const* dst_normals,
+                                     const tzr_similarity* init, tzr_icp_result* results, int32_t* const* corr,
+                                     const tzr_robust_kernel* kernel);
+
+/* tzr_register_cloud_pairs_icp with a robust kernel: the same arguments plus method (1 = point-to-plane, 2 =
+ * generalized; anything else is TZR_ERR_INVALID_ARG), epsilon (read for method 2 only) and the kernel, and the same
+ * outputs.  The normals are the call's own FPFH stage's, as in tzr_register_cloud_pairs_icp_point_to_plane and
+ * tzr_register_cloud_pairs_icp_generalized.  Each refined record is bit-identical to tzr_register_cloud_pairs, then
+ * tzr_estimate_normals_batch over the clouds at fparams->normal_search_radius, then
+ * tzr_icp_point_to_plane_robust_batch or tzr_icp_generalized_robust_batch over the valid solved pairs seeded with
+ * their records.  Launches: as tzr_register_cloud_pairs_icp. */
+int tzr_register_cloud_pairs_icp_robust(tzr_ctx* ctx, const tzr_frontend_params* fparams, const tzr_params* params,
+                                        int n_clouds, const int32_t* n, const float* const* pts, int P,
+                                        const int32_t* pair_clouds, const uint64_t* tuple_seeds,
+                                        tzr_solution* solutions, int32_t* status, int32_t* problem_index,
+                                        int64_t* n_corr, int32_t* const* corr, int32_t* const* cliques,
+                                        float* global_scale, const tzr_icp_params* icp, int32_t method,
+                                        double epsilon, const tzr_robust_kernel* kernel,
+                                        tzr_icp_result* icp_results);
+
 /* ---- downsampling point clouds: voxel-grid averaging ----------------------------------------------------------
  * The first step of the reference's FPFH + TEASER++ + ICP tutorial (voxel_down_sample on both raw scans), for many
  * clouds at once.  Open3D's PointCloud::VoxelDownSample, points only, with a defined order.  Per cloud, all arithmetic
@@ -762,7 +841,7 @@ int tzr_solve_batch_multi(const int32_t* devices, int n_devices, const tzr_param
  * to brute force), so that the two routes can be compared on one input; bit 22 wins when both are set, bit 24
  * (16777216) = a ragged batch forms one size class wherever the large-route and scale-path rules allow, however far
  * apart its sizes are, so that tests can pad n = 2 to n = 4000 in one device batch, bit 25 (33554432) = tzr_icp(_batch)
- * and tzr_icp_point_to_plane(_batch) and tzr_icp_generalized(_batch)
+ * and tzr_icp_point_to_plane(_batch) and tzr_icp_generalized(_batch) (and their robust batch entries)
  * searches every target by brute force, bit 26 (67108864) = through the hashed grid at any target size (a target the
  * grid cannot index still falls back to brute force), so that the two routes can be compared on one input; bit 25 wins
  * when both are set, bit 27 (134217728) = the default graph kernel's Gram test in its two-slope form on the unscaled float

@@ -137,6 +137,23 @@ gp = ctx.register_cloud_pairs_icp([ic_src[1:], ic_dst[1:]], [(0, 1), (1, 0)],
                                   normal_search_radius=0.05, fpfh_search_radius=0.1, method="generalized",
                                   max_iteration=3)
 print("register_cloud_pairs_icp generalized", gp[1].tolist(), [int(r) for r in gp[6]["iterations"]])
+# robust kernels: both batch entries with a NaN normal, L1 at a zero residual (a problem onto itself) and Tukey with
+# every residual beyond k, then the chained entry with each method
+for kern in (("l1", 0.0), ("tukey", 1e-12), ("cauchy", 0.02)):
+    res, _ = ctx.icp_point_to_plane_batch([ic_dst, ic_src, ic_src], [ic_src, ic_src, ic_dst[:2]],
+                                          [nrm[0], nrm[0], nrm[1][:2]], 0.05, max_iteration=3, kernel=kern)
+    print("icp plane robust", kern, [int(r) for r in res["n_correspondences"]], [int(r) for r in res["iterations"]])
+    res, _ = ctx.icp_generalized_batch([ic_dst, ic_src, ic_src], [ic_src, ic_src, ic_dst[:2]],
+                                       [nrm[1], nrm[0], nrm[0]], [nrm[0], nrm[0], nrm[1][:2]], 0.05, max_iteration=3,
+                                       kernel=kern)
+    print("icp generalized robust", kern, [int(r) for r in res["n_correspondences"]],
+          [int(r) for r in res["iterations"]])
+for method in ("point_to_plane", "generalized"):
+    gp = ctx.register_cloud_pairs_icp([ic_src[1:], ic_dst[1:]], [(0, 1), (1, 0)],
+                                      capi.default_params(noise_bound=0.01, estimate_scaling=0), 0.05,
+                                      normal_search_radius=0.05, fpfh_search_radius=0.1, method=method,
+                                      max_iteration=3, kernel=("tukey", 0.05))
+    print("register_cloud_pairs_icp robust", method, gp[1].tolist(), [int(r) for r in gp[6]["iterations"]])
 # voxel downsampling: a ragged batch with a NaN row, an all-NaN cloud and a cloud too wide for the voxel (INT_MAX check)
 vx = [rng.uniform(0, 1, size=(500, 3)).astype(np.float32), np.full((3, 3), np.nan, dtype=np.float32),
       np.array([[0, 0, 0], [1e9, 0, 0]], dtype=np.float32), rng.uniform(0, 1, size=(1, 3)).astype(np.float32)]

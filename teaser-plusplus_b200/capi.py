@@ -117,7 +117,17 @@ SIMILARITY_DTYPE = np.dtype([("scale", np.float64), ("rotation", np.float64, (9,
 ICP_RESULT_DTYPE = np.dtype([
     ("transform", SIMILARITY_DTYPE), ("fitness", np.float64), ("inlier_rmse", np.float64), ("iterations", np.int32),
     ("n_correspondences", np.int32), ("converged", np.int32), ("reserved", np.int32)], align=True)
+
+
+class RobustKernel(C.Structure):
+    """tzr_robust_kernel: type (LOSS_*) and k (finite and > 0 for HUBER, CAUCHY, GM and TUKEY)."""
+    _fields_ = [("type", C.c_int32), ("reserved", C.c_int32), ("k", C.c_double)]
+
+
+# robust kernel types (TZR_LOSS_*), by the names robust_kernel() accepts
+LOSS_TYPES = {"l2": 0, "l1": 1, "huber": 2, "cauchy": 3, "gm": 4, "tukey": 5}
 assert C.sizeof(IcpParams) == 32, C.sizeof(IcpParams)
+assert C.sizeof(RobustKernel) == 16 and RobustKernel.k.offset == 8, C.sizeof(RobustKernel)
 assert SIMILARITY_DTYPE.itemsize == C.sizeof(Similarity) == 104, C.sizeof(Similarity)
 assert ICP_RESULT_DTYPE.itemsize == C.sizeof(IcpResult) == 136, (ICP_RESULT_DTYPE.itemsize, C.sizeof(IcpResult))
 
@@ -138,7 +148,8 @@ _SYMBOLS = [
     "tzr_register_cloud_pairs_icp", "tzr_voxel_downsample", "tzr_voxel_downsample_batch", "tzr_estimate_normals",
     "tzr_estimate_normals_batch", "tzr_icp_point_to_plane", "tzr_icp_point_to_plane_batch",
     "tzr_register_cloud_pairs_icp_point_to_plane", "tzr_icp_generalized", "tzr_icp_generalized_batch",
-    "tzr_register_cloud_pairs_icp_generalized",
+    "tzr_register_cloud_pairs_icp_generalized", "tzr_icp_point_to_plane_robust_batch", "tzr_icp_generalized_robust_batch",
+    "tzr_register_cloud_pairs_icp_robust",
 ]
 
 # status codes (tzr_status)
@@ -267,6 +278,10 @@ def lib():
                                             fpp, C.POINTER(Similarity), C.POINTER(IcpResult), C.POINTER(i32p)]
     L.tzr_register_cloud_pairs_icp_generalized.argtypes = L.tzr_register_cloud_pairs.argtypes + [
         C.POINTER(IcpParams), C.c_double, C.POINTER(IcpResult)]
+    L.tzr_icp_point_to_plane_robust_batch.argtypes = L.tzr_icp_point_to_plane_batch.argtypes + [C.POINTER(RobustKernel)]
+    L.tzr_icp_generalized_robust_batch.argtypes = L.tzr_icp_generalized_batch.argtypes + [C.POINTER(RobustKernel)]
+    L.tzr_register_cloud_pairs_icp_robust.argtypes = L.tzr_register_cloud_pairs.argtypes + [
+        C.POINTER(IcpParams), C.c_int32, C.c_double, C.POINTER(RobustKernel), C.POINTER(IcpResult)]
     L.tzr_voxel_downsample.argtypes = [vp, fp, C.c_int, C.c_double, fp, i32p, i32p]
     L.tzr_voxel_downsample_batch.argtypes = [vp, C.c_int, i32p, fpp, C.c_double, fpp, i32p, C.POINTER(i32p), i32p]
     for s in _SYMBOLS:
@@ -295,6 +310,17 @@ def icp_params(max_correspondence_distance: float, **kw) -> IcpParams:
             raise AttributeError(k)
         setattr(p, k, v)
     return p
+
+
+def robust_kernel(kernel) -> RobustKernel | None:
+    """A tzr_robust_kernel from None (None: no kernel), a RobustKernel (as given), a name ("l2", "l1", "huber",
+    "cauchy", "gm", "tukey") or a (name, k) pair, e.g. ("tukey", 0.05).  The library checks the type and k."""
+    if kernel is None or isinstance(kernel, RobustKernel):
+        return kernel
+    name, k = (kernel, 0.0) if isinstance(kernel, str) else (kernel[0], kernel[1] if len(kernel) > 1 else 0.0)
+    if str(name).lower() not in LOSS_TYPES:
+        raise TzrError(f"robust_kernel: unknown kernel {name!r} (one of {sorted(LOSS_TYPES)})")
+    return RobustKernel(LOSS_TYPES[str(name).lower()], 0, float(k))
 
 
 def similarity(init=None) -> Similarity:
@@ -989,24 +1015,31 @@ class Context:
     def register_cloud_pairs_icp(self, clouds, pairs, params: Params, max_correspondence_distance, normal_search_radius=0.03,
                                  fpfh_search_radius=0.05, use_absolute_scale=True, use_crosscheck=True,
                                  use_tuple_test=True, tuple_scale=0.0, tuple_seeds=None, max_iteration=30,
-                                 relative_fitness=1e-6, relative_rmse=1e-6, method="point_to_point", epsilon=1e-3):
+                                 relative_fitness=1e-6, relative_rmse=1e-6, method="point_to_point", epsilon=1e-3,
+                                 kernel=None):
         """tzr_register_cloud_pairs_icp: register_cloud_pairs, then ICP of every pair with a valid solution on its two
         clouds, seeded with that solution, in the same call.  Returns register_cloud_pairs' six results plus the ICP
         records (structured array (P,) of ICP_RESULT_DTYPE, zeroed for a pair that was not refined).
         method="point_to_plane" runs point-to-plane ICP (tzr_register_cloud_pairs_icp_point_to_plane) with the target
         normals of the call's own FPFH stage; method="generalized" runs generalized ICP
-        (tzr_register_cloud_pairs_icp_generalized) with both clouds' normals from that stage and the given epsilon."""
+        (tzr_register_cloud_pairs_icp_generalized) with both clouds' normals from that stage and the given epsilon.
+        kernel (see robust_kernel(); point-to-plane and generalized only) runs the method with that robust kernel
+        (tzr_register_cloud_pairs_icp_robust); None keeps the entries above."""
         if method not in ("point_to_point", "point_to_plane", "generalized"):
             raise TzrError(f"register_cloud_pairs_icp: unknown method {method!r}")
+        kernel = robust_kernel(kernel)
+        if kernel is not None and method == "point_to_point":
+            raise TzrError("register_cloud_pairs_icp: point-to-point ICP takes no robust kernel")
         icp = icp_params(max_correspondence_distance, max_iteration=int(max_iteration),
                          relative_fitness=float(relative_fitness), relative_rmse=float(relative_rmse))
         return self._register_pairs(clouds, pairs, params, normal_search_radius, fpfh_search_radius, use_absolute_scale,
                                     use_crosscheck, use_tuple_test, tuple_scale, tuple_seeds, icp,
                                     plane=method == "point_to_plane",
-                                    epsilon=float(epsilon) if method == "generalized" else None)
+                                    epsilon=float(epsilon) if method == "generalized" else None, kernel=kernel)
 
     def _register_pairs(self, clouds, pairs, params, normal_search_radius, fpfh_search_radius, use_absolute_scale,
-                        use_crosscheck, use_tuple_test, tuple_scale, tuple_seeds, icp, plane=False, epsilon=None):
+                        use_crosscheck, use_tuple_test, tuple_scale, tuple_seeds, icp, plane=False, epsilon=None,
+                        kernel=None):
         cl = [np.ascontiguousarray(c, dtype=np.float32) for c in clouds]
         if not cl or any(c.ndim != 2 or c.shape[1] != 3 or c.shape[0] == 0 for c in cl):
             raise TzrError("register_cloud_pairs: a non-empty list of non-empty (n,3) clouds is required")
@@ -1042,7 +1075,11 @@ class Context:
         else:
             icp_res = np.zeros(P, dtype=ICP_RESULT_DTYPE)
             out_res = icp_res.ctypes.data_as(C.POINTER(IcpResult))
-            if epsilon is not None:
+            if kernel is not None:
+                rc = lib().tzr_register_cloud_pairs_icp_robust(*args, C.byref(icp), 1 if plane else 2,
+                                                               0.0 if epsilon is None else epsilon, C.byref(kernel),
+                                                               out_res)
+            elif epsilon is not None:
                 rc = lib().tzr_register_cloud_pairs_icp_generalized(*args, C.byref(icp), epsilon, out_res)
             else:
                 entry = lib().tzr_register_cloud_pairs_icp_point_to_plane if plane else lib().tzr_register_cloud_pairs_icp
@@ -1066,43 +1103,48 @@ class Context:
         return icp_result_dict(res[0]), corr[0]
 
     def icp_point_to_plane(self, src, dst, dst_normals, max_correspondence_distance, init=None, max_iteration=30,
-                           relative_fitness=1e-6, relative_rmse=1e-6):
+                           relative_fitness=1e-6, relative_rmse=1e-6, kernel=None):
         """tzr_icp_point_to_plane: icp() with point-to-plane updates; dst_normals: (nd,3) or (nd,4) float32 target
-        normals (e.g. estimate_normals(dst)), used as given.  Returns what icp() returns."""
+        normals (e.g. estimate_normals(dst)), used as given.  kernel (see robust_kernel()): the robust kernel, through
+        tzr_icp_point_to_plane_robust_batch with B = 1.  Returns what icp() returns."""
         res, corr = self.icp_point_to_plane_batch([src], [dst], [dst_normals], max_correspondence_distance,
                                                   None if init is None else [init], max_iteration=max_iteration,
                                                   relative_fitness=relative_fitness, relative_rmse=relative_rmse,
-                                                  single=True)
+                                                  single=True, kernel=kernel)
         return icp_result_dict(res[0]), corr[0]
 
     def icp_point_to_plane_batch(self, srcs, dsts, dst_normals, max_correspondence_distance, inits=None,
-                                 max_iteration=30, relative_fitness=1e-6, relative_rmse=1e-6, single=False):
+                                 max_iteration=30, relative_fitness=1e-6, relative_rmse=1e-6, single=False,
+                                 kernel=None):
         """tzr_icp_point_to_plane_batch: icp_batch() with point-to-plane updates and one (nd_b,3) or (nd_b,4) normals
-        array per target.  single=True goes through tzr_icp_point_to_plane (B must be 1)."""
+        array per target.  single=True goes through tzr_icp_point_to_plane (B must be 1).  kernel (see
+        robust_kernel()): the robust kernel, through tzr_icp_point_to_plane_robust_batch."""
         return self._icp(srcs, dsts, dst_normals, max_correspondence_distance, inits, max_iteration, relative_fitness,
-                         relative_rmse, single)
+                         relative_rmse, single, kernel=robust_kernel(kernel))
 
     def icp_generalized(self, src, dst, src_normals, dst_normals, max_correspondence_distance, init=None, epsilon=1e-3,
-                        max_iteration=30, relative_fitness=1e-6, relative_rmse=1e-6):
+                        max_iteration=30, relative_fitness=1e-6, relative_rmse=1e-6, kernel=None):
         """tzr_icp_generalized: icp() with generalized-ICP updates; src_normals / dst_normals: (n,3) or (n,4) float32
         normals of each cloud (e.g. estimate_normals()), used as given; epsilon: the covariances' epsilon (finite,
-        > 0).  Returns what icp() returns."""
+        > 0).  kernel (see robust_kernel()): the robust kernel, through tzr_icp_generalized_robust_batch with B = 1.
+        Returns what icp() returns."""
         res, corr = self.icp_generalized_batch([src], [dst], [src_normals], [dst_normals], max_correspondence_distance,
                                                None if init is None else [init], epsilon=epsilon,
                                                max_iteration=max_iteration, relative_fitness=relative_fitness,
-                                               relative_rmse=relative_rmse, single=True)
+                                               relative_rmse=relative_rmse, single=True, kernel=kernel)
         return icp_result_dict(res[0]), corr[0]
 
     def icp_generalized_batch(self, srcs, dsts, src_normals, dst_normals, max_correspondence_distance, inits=None,
                               epsilon=1e-3, max_iteration=30, relative_fitness=1e-6, relative_rmse=1e-6,
-                              single=False):
+                              single=False, kernel=None):
         """tzr_icp_generalized_batch: icp_batch() with generalized-ICP updates and one (n,3) or (n,4) normals array per
-        source and per target.  single=True goes through tzr_icp_generalized (B must be 1)."""
+        source and per target.  single=True goes through tzr_icp_generalized (B must be 1).  kernel (see
+        robust_kernel()): the robust kernel, through tzr_icp_generalized_robust_batch."""
         if len(src_normals) != len(srcs):
             raise TzrError("icp_generalized_batch: one normals array per source cloud is required")
         SN = [_normals32(a, _cloud32(s, "icp").shape[0], "icp_generalized") for a, s in zip(src_normals, srcs)]
         return self._icp(srcs, dsts, dst_normals, max_correspondence_distance, inits, max_iteration, relative_fitness,
-                         relative_rmse, single, src_normals=SN, epsilon=float(epsilon))
+                         relative_rmse, single, src_normals=SN, epsilon=float(epsilon), kernel=robust_kernel(kernel))
 
     def icp_batch(self, srcs, dsts, max_correspondence_distance, inits=None, max_iteration=30, relative_fitness=1e-6,
                   relative_rmse=1e-6, single=False):
@@ -1113,9 +1155,9 @@ class Context:
                          relative_rmse, single)
 
     def _icp(self, srcs, dsts, normals, max_correspondence_distance, inits, max_iteration, relative_fitness,
-             relative_rmse, single, src_normals=None, epsilon=None):
+             relative_rmse, single, src_normals=None, epsilon=None, kernel=None):
         """icp_batch (normals None), icp_point_to_plane_batch and icp_generalized_batch (src_normals: (n,4) float32
-        arrays, epsilon given)."""
+        arrays, epsilon given); a RobustKernel goes through the robust batch entries, also for single=True."""
         S = [_cloud32(a, "icp") for a in srcs]
         D = [_cloud32(a, "icp") for a in dsts]
         B = len(S)
@@ -1128,7 +1170,7 @@ class Context:
         res = (IcpResult * B)()
         corr = [np.zeros((a.shape[0], 2), dtype=np.int32) for a in S]
         fp, i32p = C.POINTER(C.c_float), C.POINTER(C.c_int32)
-        if single:
+        if single and kernel is None:
             assert B == 1
             head = (self._h, C.byref(p), _p(S[0], C.c_float), S[0].shape[0], _p(D[0], C.c_float), D[0].shape[0])
             tail = (init, res, _p(corr[0], C.c_int32))
@@ -1144,7 +1186,15 @@ class Context:
             head = (self._h, C.byref(p), B, _p(ns, C.c_int32), (fp * B)(*[_p(a, C.c_float) for a in S]),
                     _p(nd, C.c_int32), (fp * B)(*[_p(a, C.c_float) for a in D]))
             tail = (init, res, (i32p * B)(*[_p(c, C.c_int32) for c in corr]))
-            if src_normals is not None:
+            if kernel is not None:
+                tail = tail + (C.byref(kernel),)
+            if kernel is not None and src_normals is not None:
+                rc = lib().tzr_icp_generalized_robust_batch(self._h, C.byref(p), epsilon, B, head[3], head[4],
+                                                            (fp * B)(*[_p(a, C.c_float) for a in src_normals]),
+                                                            *head[5:], (fp * B)(*[_p(a, C.c_float) for a in N]), *tail)
+            elif kernel is not None:
+                rc = lib().tzr_icp_point_to_plane_robust_batch(*head, (fp * B)(*[_p(a, C.c_float) for a in N]), *tail)
+            elif src_normals is not None:
                 rc = lib().tzr_icp_generalized_batch(self._h, C.byref(p), epsilon, B, head[3], head[4],
                                                      (fp * B)(*[_p(a, C.c_float) for a in src_normals]), *head[5:],
                                                      (fp * B)(*[_p(a, C.c_float) for a in N]), *tail)

@@ -2063,6 +2063,23 @@ static bool icp_params_ok(const tzr_icp_params* p) {
 // generalized ICP's epsilon: finite and > 0
 static bool icp_epsilon_ok(double epsilon) { return std::isfinite(epsilon) && epsilon > 0; }
 
+// a robust kernel (DESIGN.md §3.15): a known type, and k finite and > 0 where the weight reads it
+static bool robust_kernel_ok(const tzr_robust_kernel* k) {
+  if (!k) return false;
+  switch (k->type) {
+    case TZR_LOSS_L2:
+    case TZR_LOSS_L1:
+      return true;
+    case TZR_LOSS_HUBER:
+    case TZR_LOSS_CAUCHY:
+    case TZR_LOSS_GM:
+    case TZR_LOSS_TUKEY:
+      return std::isfinite(k->k) && k->k > 0;
+    default:
+      return false;
+  }
+}
+
 static void icp_result_of(const IcpProb& pr, tzr_icp_result* out) {
   memset(out, 0, sizeof(*out));
   if (!pr.seeded) return;
@@ -2082,12 +2099,14 @@ static void icp_result_of(const IcpProb& pr, tzr_icp_result* out) {
 // icp (may be NULL): after the solve, ICP of every solved pair on its two clouds (already in m_in), seeded on the device
 // from its record (ctx->icp holds the ICP workspace); icp_results (P entries) then receives the refinements, zeroed for a
 // pair that was not refined.  Without icp the launches, synchronisations and outputs are tzr_register_cloud_pairs'.
+// icp_kernel: the robust kernel of the point-to-plane and generalized modes (checked by the caller; NULL = L2).
 static int register_pairs_run(tzr_ctx* ctx, const tzr_frontend_params* fp, const tzr_params* params, int n_clouds,
                               const int32_t* n, const float* const* pts, int P, const int32_t* pair_clouds,
                               const uint64_t* tuple_seeds, tzr_solution* solutions, int32_t* status,
                               int32_t* problem_index, int64_t* n_corr, int32_t* const* corr, int32_t* const* cliques,
                               float* global_scale, const tzr_icp_params* icp, tzr_icp_result* icp_results,
-                              int icp_mode = kIcpPointToPoint, double icp_epsilon = 0) {
+                              int icp_mode = kIcpPointToPoint, double icp_epsilon = 0,
+                              const tzr_robust_kernel* icp_kernel = nullptr) {
   if (!ctx || !fp || !params || n_clouds < 1 || !n || !pts || P < 1 || !pair_clouds || !solutions || !status ||
       !n_corr || !(fp->normal_search_radius > 0) || !(fp->fpfh_search_radius > 0))
     return TZR_ERR_INVALID_ARG;
@@ -2157,6 +2176,10 @@ static int register_pairs_run(tzr_ctx* ctx, const tzr_frontend_params* fp, const
     iplan.max_iteration = icp->max_iteration;
     iplan.mode = icp_mode;
     iplan.epsilon = icp_epsilon;
+    if (icp_kernel) {
+      iplan.loss = icp_kernel->type;
+      iplan.loss_k = icp_kernel->k;
+    }
     iplan.r2 = r * r;
     iplan.relative_fitness = icp->relative_fitness;
     iplan.relative_rmse = icp->relative_rmse;
@@ -2403,6 +2426,20 @@ int tzr_register_cloud_pairs_icp_generalized(tzr_ctx* ctx, const tzr_frontend_pa
                             epsilon);
 }
 
+int tzr_register_cloud_pairs_icp_robust(tzr_ctx* ctx, const tzr_frontend_params* fp, const tzr_params* params,
+                                        int n_clouds, const int32_t* n, const float* const* pts, int P,
+                                        const int32_t* pair_clouds, const uint64_t* tuple_seeds,
+                                        tzr_solution* solutions, int32_t* status, int32_t* problem_index,
+                                        int64_t* n_corr, int32_t* const* corr, int32_t* const* cliques,
+                                        float* global_scale, const tzr_icp_params* icp, int32_t method,
+                                        double epsilon, const tzr_robust_kernel* kernel,
+                                        tzr_icp_result* icp_results) {
+  if (!icp || (method != 1 && method != 2) || !robust_kernel_ok(kernel)) return TZR_ERR_INVALID_ARG;
+  return register_pairs_run(ctx, fp, params, n_clouds, n, pts, P, pair_clouds, tuple_seeds, solutions, status,
+                            problem_index, n_corr, corr, cliques, global_scale, icp, icp_results,
+                            method == 1 ? kIcpPointToPlane : kIcpGeneralized, epsilon, kernel);
+}
+
 void tzr_icp_params_default(tzr_icp_params* p) {
   if (!p) return;
   memset(p, 0, sizeof(*p));
@@ -2415,11 +2452,13 @@ void tzr_icp_params_default(tzr_icp_params* p) {
 // tzr_icp(_batch), tzr_icp_point_to_plane(_batch) and tzr_icp_generalized(_batch): sources, targets (and target and
 // source normals) staged back to back, one H2D copy, every iteration enqueued (launch_icp), one D2H copy of the problem
 // table (and of the per-point matches when correspondences are asked for).  dst_normals: required for kIcpPointToPlane
-// and kIcpGeneralized, src_normals and epsilon for kIcpGeneralized; unused otherwise.
+// and kIcpGeneralized, src_normals and epsilon for kIcpGeneralized; unused otherwise.  kernel: the robust kernel of the
+// point-to-plane and generalized modes (checked by the caller; NULL = L2).
 static int icp_batch_run(tzr_ctx* ctx, const tzr_icp_params* params, int mode, int B, const int32_t* ns,
                          const float* const* src, const float* const* src_normals, const int32_t* nd,
                          const float* const* dst, const float* const* dst_normals, double epsilon,
-                         const tzr_similarity* init, tzr_icp_result* results, int32_t* const* corr) {
+                         const tzr_similarity* init, tzr_icp_result* results, int32_t* const* corr,
+                         const tzr_robust_kernel* kernel = nullptr) {
   const bool plane = mode != kIcpPointToPoint, gicp = mode == kIcpGeneralized;
   if (!ctx || !icp_params_ok(params) || B < 1 || !ns || !src || !nd || !dst || (plane && !dst_normals) ||
       (gicp && (!src_normals || !icp_epsilon_ok(epsilon))) || !init || !results)
@@ -2452,6 +2491,10 @@ static int icp_batch_run(tzr_ctx* ctx, const tzr_icp_params* params, int mode, i
   plan.max_iteration = params->max_iteration;
   plan.mode = mode;
   plan.epsilon = epsilon;
+  if (kernel) {
+    plan.loss = kernel->type;
+    plan.loss_k = kernel->k;
+  }
   plan.r2 = r * r;
   plan.relative_fitness = params->relative_fitness;
   plan.relative_rmse = params->relative_rmse;
@@ -2561,6 +2604,26 @@ int tzr_icp_generalized_batch(tzr_ctx* ctx, const tzr_icp_params* params, double
                               tzr_icp_result* results, int32_t* const* corr) {
   return icp_batch_run(ctx, params, kIcpGeneralized, B, ns, src, src_normals, nd, dst, dst_normals, epsilon, init,
                        results, corr);
+}
+
+int tzr_icp_point_to_plane_robust_batch(tzr_ctx* ctx, const tzr_icp_params* params, int B, const int32_t* ns,
+                                        const float* const* src, const int32_t* nd, const float* const* dst,
+                                        const float* const* dst_normals, const tzr_similarity* init,
+                                        tzr_icp_result* results, int32_t* const* corr,
+                                        const tzr_robust_kernel* kernel) {
+  if (!robust_kernel_ok(kernel)) return TZR_ERR_INVALID_ARG;
+  return icp_batch_run(ctx, params, kIcpPointToPlane, B, ns, src, nullptr, nd, dst, dst_normals, 0.0, init, results,
+                       corr, kernel);
+}
+
+int tzr_icp_generalized_robust_batch(tzr_ctx* ctx, const tzr_icp_params* params, double epsilon, int B,
+                                     const int32_t* ns, const float* const* src, const float* const* src_normals,
+                                     const int32_t* nd, const float* const* dst, const float* const* dst_normals,
+                                     const tzr_similarity* init, tzr_icp_result* results, int32_t* const* corr,
+                                     const tzr_robust_kernel* kernel) {
+  if (!robust_kernel_ok(kernel)) return TZR_ERR_INVALID_ARG;
+  return icp_batch_run(ctx, params, kIcpGeneralized, B, ns, src, src_normals, nd, dst, dst_normals, epsilon, init,
+                       results, corr, kernel);
 }
 
 // the single-problem entries: icp_batch_run with B = 1 and init NULL meaning the identity

@@ -4,7 +4,9 @@
 // search, the evaluation and the loop, and replaces the covariance and update pair with icp_plane_system_kernel (the
 // centred 6 x 6 Gauss-Newton system) and icp_plane_update_kernel (its pivoted solve and the Euler rotation).
 // Generalized ICP (DESIGN.md §3.14) replaces only the system, with icp_gicp_system_kernel (plane-to-plane covariances
-// from both clouds' normals, the same 27 sums), and shares icp_plane_update_kernel.
+// from both clouds' normals, the same 27 sums), and shares icp_plane_update_kernel.  Robust kernels (DESIGN.md §3.15)
+// are the <true> instances of both system kernels: weighted sums, the same layout; the <false> instances are the
+// unweighted systems and run for TZR_LOSS_L2.
 //
 //   icp_nn_kernel      one CTA per chunk of kIcpChunk source points: p = s (R x) + t in float64 (icp_transform), the
 //                      nearest target with d^2 < r^2 (lowest index among equal d^2), by brute force through shared
@@ -270,13 +272,40 @@ __global__ void icp_update_kernel(IcpArgs a) {
   icp_compose(pr, Ru, tu);
 }
 
+// ---- robust kernels (DESIGN.md §3.15) ----------------------------------------------------------------------------------
+// The weight rho'(r) / r of the kernel TZR_LOSS_* with parameter k, from e = |r| (include/teaser_b200.h writes out each
+// one).  L1 at e = 0 gives +inf: the callers drop a correspondence whose weight is not finite.
+__device__ __forceinline__ double icp_robust_weight(int loss, double k, double r) {
+  const double e = fabs(r);
+  if (loss == TZR_LOSS_L1) return 1.0 / e;
+  if (loss == TZR_LOSS_HUBER) return k / fmax(e, k);
+  if (loss == TZR_LOSS_CAUCHY) {
+    const double q = e / k;
+    return 1.0 / (1.0 + q * q);
+  }
+  if (loss == TZR_LOSS_GM) {
+    const double t = k + e * e;
+    return k / (t * t);
+  }
+  if (loss == TZR_LOSS_TUKEY) {
+    if (e > k) return 0.0;
+    const double q = e / k, t = 1.0 - q * q;
+    return t * t;
+  }
+  return 1.0;
+}
+
 // ---- point-to-plane (DESIGN.md §3.13) ----------------------------------------------------------------------------------
 // One CTA per chunk: each correspondence (i, j) whose target normal n has three finite components adds J J^T (the 21
 // entries of the upper triangle, row by row) and J r (6), with u = p - c (c = mu_p of the current correspondences),
 // J = (u x n, n) and r = ((p0 - q0) n0 + (p1 - q1) n1) + (p2 - q2) n2.  Flipping n negates J and r exactly, so the sums do
 // not depend on the normal's sign.  The partials of this pass use 27 doubles per chunk; the nearest-neighbour pass that
 // follows writes its 8 sums over them with stride 9 only after the update has read them.
-__global__ void __launch_bounds__(kIcpThreads) icp_plane_system_kernel(IcpArgs a, const float4* __restrict__ normals) {
+// kRobust (DESIGN.md §3.15): the correspondence adds (w J_a) J_b and (w J_a) r with w = icp_robust_weight(loss, loss_k,
+// r), and nothing when w is not finite.  The instance without it ignores loss and loss_k.
+template <bool kRobust>
+__global__ void __launch_bounds__(kIcpThreads) icp_plane_system_kernel(IcpArgs a, const float4* __restrict__ normals,
+                                                                       int loss, double loss_k) {
   __shared__ double s_buf[(kIcpThreads / 32) * kIcpPlaneSums];
   const int c = blockIdx.x;
   const int b = a.chunk_prob[c];
@@ -299,13 +328,29 @@ __global__ void __launch_bounds__(kIcpThreads) icp_plane_system_kernel(IcpArgs a
                            n[0], n[1], n[2]};
       const double r = ((p[0] - (double)a.dst[o]) * n[0] + (p[1] - (double)a.dst[o + 1]) * n[1]) +
                        (p[2] - (double)a.dst[o + 2]) * n[2];
-      int k = 0;
+      if constexpr (kRobust) {
+        const double w = icp_robust_weight(loss, loss_k, r);
+        if (isfinite(w)) {
+          double wJ[6];
 #pragma unroll
-      for (int row = 0; row < 6; ++row)
+          for (int row = 0; row < 6; ++row) wJ[row] = w * J[row];
+          int k = 0;
 #pragma unroll
-        for (int col = row; col < 6; ++col) v[k++] = J[row] * J[col];
+          for (int row = 0; row < 6; ++row)
 #pragma unroll
-      for (int row = 0; row < 6; ++row) v[21 + row] = J[row] * r;
+            for (int col = row; col < 6; ++col) v[k++] = wJ[row] * J[col];
+#pragma unroll
+          for (int row = 0; row < 6; ++row) v[21 + row] = wJ[row] * r;
+        }
+      } else {
+        int k = 0;
+#pragma unroll
+        for (int row = 0; row < 6; ++row)
+#pragma unroll
+          for (int col = row; col < 6; ++col) v[k++] = J[row] * J[col];
+#pragma unroll
+        for (int row = 0; row < 6; ++row) v[21 + row] = J[row] * r;
+      }
     }
   }
   icp_block_sum<kIcpPlaneSums>(v, s_buf, a.partial + kIcpPlaneSums * (size_t)c);
@@ -392,14 +437,103 @@ __device__ __forceinline__ void gicp_symv(const double S[6], const double v[3], 
   o[2] = (S[2] * v[0] + S[4] * v[1]) + S[5] * v[2];
 }
 
+// The 27 sums of one correspondence: J^T A J (21 entries, the plane system's order) and J^T A d (6), with
+// J = [e_k x u (k = 0..2), I], evaluated as include/teaser_b200.h writes them
+__device__ __forceinline__ void gicp_add(const double A[6], const double u[3], const double d[3],
+                                         double (&v)[kIcpPlaneSums]) {
+  // ww[l] = u x A (e_l x u), wt[l] = u x A e_l: column l of the omega-omega and omega-tau blocks
+  double ww[3][3], wt[3][3];
+#pragma unroll
+  for (int l = 0; l < 3; ++l) {
+    const double e[3] = {l == 0 ? 1.0 : 0.0, l == 1 ? 1.0 : 0.0, l == 2 ? 1.0 : 0.0};
+    double eu[3], Aeu[3], Ae[3];
+    gicp_cross(e, u, eu);
+    gicp_symv(A, eu, Aeu);
+    gicp_cross(u, Aeu, ww[l]);
+    Ae[0] = A[l == 0 ? 0 : l == 1 ? 1 : 2];
+    Ae[1] = A[l == 0 ? 1 : l == 1 ? 3 : 4];
+    Ae[2] = A[l == 0 ? 2 : l == 1 ? 4 : 5];
+    gicp_cross(u, Ae, wt[l]);
+  }
+  int k = 0;
+#pragma unroll
+  for (int row = 0; row < 3; ++row) {
+#pragma unroll
+    for (int col = row; col < 3; ++col) v[k++] = ww[col][row];
+#pragma unroll
+    for (int col = 0; col < 3; ++col) v[k++] = wt[col][row];
+  }
+  v[k++] = A[0];
+  v[k++] = A[1];
+  v[k++] = A[2];
+  v[k++] = A[3];
+  v[k++] = A[4];
+  v[k++] = A[5];
+  double w[3], uw[3];
+  gicp_symv(A, d, w);
+  gicp_cross(u, w, uw);
+  v[21] = uw[0];
+  v[22] = uw[1];
+  v[23] = uw[2];
+  v[24] = w[0];
+  v[25] = w[1];
+  v[26] = w[2];
+}
+
+// The robust information matrix A~ = W diag(w) W (upper triangle) with W = M^-1/2 = V diag(1 / sqrt(sigma)) V^T from
+// svd3 of the symmetric M (upper triangle) and w_k the weight of the whitened residual r_k = W_k . d (DESIGN.md §3.15,
+// include/teaser_b200.h writes out every sum and its order).  False, and A~ unset, when some sigma is not > 0 or not
+// finite, or some weight is not finite.
+__device__ __forceinline__ bool gicp_robust_info(const double M[6], const double d[3], int loss, double loss_k,
+                                                 double At[6]) {
+  M3 H, U, V;
+  H.a[0] = M[0];
+  H.a[1] = M[1];
+  H.a[2] = M[2];
+  H.a[3] = M[1];
+  H.a[4] = M[3];
+  H.a[5] = M[4];
+  H.a[6] = M[2];
+  H.a[7] = M[4];
+  H.a[8] = M[5];
+  double S[3], q[3];
+  svd3(H, U, S, V);
+#pragma unroll
+  for (int k = 0; k < 3; ++k) {
+    if (!(S[k] > 0.0 && isfinite(S[k]))) return false;
+    q[k] = 1.0 / sqrt(S[k]);
+  }
+  double W[3][3], w[3];
+#pragma unroll
+  for (int r = 0; r < 3; ++r)
+#pragma unroll
+    for (int c = 0; c < 3; ++c)
+      W[r][c] = ((V(r, 0) * q[0]) * V(c, 0) + (V(r, 1) * q[1]) * V(c, 1)) + (V(r, 2) * q[2]) * V(c, 2);
+#pragma unroll
+  for (int k = 0; k < 3; ++k) {
+    w[k] = icp_robust_weight(loss, loss_k, (W[k][0] * d[0] + W[k][1] * d[1]) + W[k][2] * d[2]);
+    if (!isfinite(w[k])) return false;
+  }
+  int e = 0;
+#pragma unroll
+  for (int r = 0; r < 3; ++r)
+#pragma unroll
+    for (int c = r; c < 3; ++c)
+      At[e++] = ((w[0] * W[0][r]) * W[0][c] + (w[1] * W[1][r]) * W[1][c]) + (w[2] * W[2][r]) * W[2][c];
+  return true;
+}
+
 // One CTA per chunk: each correspondence (i, j) whose source normal m and target normal n are finite and of non-zero
 // length adds J^T A J (21 entries, the plane system's order) and J^T A d (6), with u = p - c, d = p - q,
 // J = [e_k x u (k = 0..2), I] and A = (s^2 C(R m) + C(n))^-1 by the symmetric adjugate (include/teaser_b200.h writes
 // out every formula and its order).  The 27 sums and their layout are the plane system's, so icp_plane_update_kernel
 // solves them unchanged.
+// kRobust (DESIGN.md §3.15): A~ of gicp_robust_info (loss, loss_k) in place of A, from the same M; the instance without
+// it ignores loss and loss_k.
+template <bool kRobust>
 __global__ void __launch_bounds__(kIcpThreads) icp_gicp_system_kernel(IcpArgs a, const float4* __restrict__ src_normals,
                                                                       const float4* __restrict__ dst_normals,
-                                                                      double epsilon) {
+                                                                      double epsilon, int loss, double loss_k) {
   __shared__ double s_buf[(kIcpThreads / 32) * kIcpPlaneSums];
   const int c = blockIdx.x;
   const int b = a.chunk_prob[c];
@@ -424,54 +558,68 @@ __global__ void __launch_bounds__(kIcpThreads) icp_gicp_system_kernel(IcpArgs a,
       const double s2 = pr.s * pr.s;
 #pragma unroll
       for (int k = 0; k < 6; ++k) M[k] = s2 * Cm[k] + Cn[k];
-      // cofactors of M = [M0 M1 M2; M1 M3 M4; M2 M4 M5]
-      const double c00 = M[3] * M[5] - M[4] * M[4], c01 = M[2] * M[4] - M[1] * M[5], c02 = M[1] * M[4] - M[2] * M[3];
-      const double c11 = M[0] * M[5] - M[2] * M[2], c12 = M[1] * M[2] - M[0] * M[4], c22 = M[0] * M[3] - M[1] * M[1];
-      const double det = (M[0] * c00 + M[1] * c01) + M[2] * c02;
-      if (det > 0.0 && isfinite(det)) {
-        const double A[6] = {c00 / det, c01 / det, c02 / det, c11 / det, c12 / det, c22 / det};
+      if constexpr (kRobust) {
         double p[3];
         icp_transform(pr, a.src, pr.s_lo + i, p);
         const size_t o = 3 * (size_t)(pr.d_lo + j);
-        const double u[3] = {p[0] - pr.mup[0], p[1] - pr.mup[1], p[2] - pr.mup[2]};
         const double d[3] = {p[0] - (double)a.dst[o], p[1] - (double)a.dst[o + 1], p[2] - (double)a.dst[o + 2]};
-        // ww[l] = u x A (e_l x u), wt[l] = u x A e_l: column l of the omega-omega and omega-tau blocks
-        double ww[3][3], wt[3][3];
-#pragma unroll
-        for (int l = 0; l < 3; ++l) {
-          const double e[3] = {l == 0 ? 1.0 : 0.0, l == 1 ? 1.0 : 0.0, l == 2 ? 1.0 : 0.0};
-          double eu[3], Aeu[3], Ae[3];
-          gicp_cross(e, u, eu);
-          gicp_symv(A, eu, Aeu);
-          gicp_cross(u, Aeu, ww[l]);
-          Ae[0] = A[l == 0 ? 0 : l == 1 ? 1 : 2];
-          Ae[1] = A[l == 0 ? 1 : l == 1 ? 3 : 4];
-          Ae[2] = A[l == 0 ? 2 : l == 1 ? 4 : 5];
-          gicp_cross(u, Ae, wt[l]);
+        double At[6];
+        if (gicp_robust_info(M, d, loss, loss_k, At)) {
+          const double u[3] = {p[0] - pr.mup[0], p[1] - pr.mup[1], p[2] - pr.mup[2]};
+          gicp_add(At, u, d, v);
         }
-        int k = 0;
+      } else {
+        // cofactors of M = [M0 M1 M2; M1 M3 M4; M2 M4 M5]
+        const double c00 = M[3] * M[5] - M[4] * M[4], c01 = M[2] * M[4] - M[1] * M[5],
+                     c02 = M[1] * M[4] - M[2] * M[3];
+        const double c11 = M[0] * M[5] - M[2] * M[2], c12 = M[1] * M[2] - M[0] * M[4],
+                     c22 = M[0] * M[3] - M[1] * M[1];
+        const double det = (M[0] * c00 + M[1] * c01) + M[2] * c02;
+        if (det > 0.0 && isfinite(det)) {
+          const double A[6] = {c00 / det, c01 / det, c02 / det, c11 / det, c12 / det, c22 / det};
+          double p[3];
+          icp_transform(pr, a.src, pr.s_lo + i, p);
+          const size_t o = 3 * (size_t)(pr.d_lo + j);
+          const double u[3] = {p[0] - pr.mup[0], p[1] - pr.mup[1], p[2] - pr.mup[2]};
+          const double d[3] = {p[0] - (double)a.dst[o], p[1] - (double)a.dst[o + 1], p[2] - (double)a.dst[o + 2]};
+          // gicp_add written out: the form this instance has always had, so its code does not move
+          double ww[3][3], wt[3][3];
 #pragma unroll
-        for (int row = 0; row < 3; ++row) {
+          for (int l = 0; l < 3; ++l) {
+            const double e[3] = {l == 0 ? 1.0 : 0.0, l == 1 ? 1.0 : 0.0, l == 2 ? 1.0 : 0.0};
+            double eu[3], Aeu[3], Ae[3];
+            gicp_cross(e, u, eu);
+            gicp_symv(A, eu, Aeu);
+            gicp_cross(u, Aeu, ww[l]);
+            Ae[0] = A[l == 0 ? 0 : l == 1 ? 1 : 2];
+            Ae[1] = A[l == 0 ? 1 : l == 1 ? 3 : 4];
+            Ae[2] = A[l == 0 ? 2 : l == 1 ? 4 : 5];
+            gicp_cross(u, Ae, wt[l]);
+          }
+          int k = 0;
 #pragma unroll
-          for (int col = row; col < 3; ++col) v[k++] = ww[col][row];
+          for (int row = 0; row < 3; ++row) {
 #pragma unroll
-          for (int col = 0; col < 3; ++col) v[k++] = wt[col][row];
+            for (int col = row; col < 3; ++col) v[k++] = ww[col][row];
+#pragma unroll
+            for (int col = 0; col < 3; ++col) v[k++] = wt[col][row];
+          }
+          v[k++] = A[0];
+          v[k++] = A[1];
+          v[k++] = A[2];
+          v[k++] = A[3];
+          v[k++] = A[4];
+          v[k++] = A[5];
+          double w[3], uw[3];
+          gicp_symv(A, d, w);
+          gicp_cross(u, w, uw);
+          v[21] = uw[0];
+          v[22] = uw[1];
+          v[23] = uw[2];
+          v[24] = w[0];
+          v[25] = w[1];
+          v[26] = w[2];
         }
-        v[k++] = A[0];
-        v[k++] = A[1];
-        v[k++] = A[2];
-        v[k++] = A[3];
-        v[k++] = A[4];
-        v[k++] = A[5];
-        double w[3], uw[3];
-        gicp_symv(A, d, w);
-        gicp_cross(u, w, uw);
-        v[21] = uw[0];
-        v[22] = uw[1];
-        v[23] = uw[2];
-        v[24] = w[0];
-        v[25] = w[1];
-        v[26] = w[2];
       }
     }
   }
@@ -548,10 +696,18 @@ int launch_icp(const IcpPlan& plan, const float* src, const float* dst, const fl
   nl += 2;
   for (int it = 0; it < plan.max_iteration; ++it) {
     if (plan.mode == kIcpPointToPlane) {
-      icp_plane_system_kernel<<<plan.chunks, kIcpThreads, 0, st>>>(a, dst_normals);
+      if (plan.loss == TZR_LOSS_L2)
+        icp_plane_system_kernel<false><<<plan.chunks, kIcpThreads, 0, st>>>(a, dst_normals, 0, 0.0);
+      else
+        icp_plane_system_kernel<true><<<plan.chunks, kIcpThreads, 0, st>>>(a, dst_normals, plan.loss, plan.loss_k);
       icp_plane_update_kernel<<<plan.B, 32, 0, st>>>(a);
     } else if (plan.mode == kIcpGeneralized) {
-      icp_gicp_system_kernel<<<plan.chunks, kIcpThreads, 0, st>>>(a, src_normals, dst_normals, plan.epsilon);
+      if (plan.loss == TZR_LOSS_L2)
+        icp_gicp_system_kernel<false><<<plan.chunks, kIcpThreads, 0, st>>>(a, src_normals, dst_normals, plan.epsilon, 0,
+                                                                           0.0);
+      else
+        icp_gicp_system_kernel<true><<<plan.chunks, kIcpThreads, 0, st>>>(a, src_normals, dst_normals, plan.epsilon,
+                                                                          plan.loss, plan.loss_k);
       icp_plane_update_kernel<<<plan.B, 32, 0, st>>>(a);
     } else {
       icp_cov_kernel<<<plan.chunks, kIcpThreads, 0, st>>>(a);

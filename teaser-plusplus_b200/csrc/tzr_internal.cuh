@@ -458,6 +458,10 @@ struct IcpPlan {
   int mode = kIcpPointToPoint;
   double r2 = 0, relative_fitness = 0, relative_rmse = 0;
   double epsilon = 0;   // generalized: the covariances' epsilon (finite, > 0)
+  // point-to-plane and generalized: the robust kernel (TZR_LOSS_*, DESIGN.md §3.15) and its k; TZR_LOSS_L2 runs the
+  // unweighted system kernels
+  int loss = 0;
+  double loss_k = 0;
   FpfhPlan grid;        // the target grid (fpfh_plan with both radii = r)
 };
 // src (NS x 3 floats), dst (ND x 3 floats), src_normals (generalized: the source normals, (nx, ny, nz, curvature) per

@@ -3,8 +3,10 @@
 // through the C-ABI (tzr_icp, tzr_icp_batch; include/teaser_b200.h defines the loop).  teaser::PointToPlaneICP is the
 // same with TransformationEstimationPointToPlane (tzr_icp_point_to_plane, tzr_icp_point_to_plane_batch), given the
 // target normals (teaser::estimateNormals, teaser/normals.h).  teaser::GeneralizedICP is the same with Open3D's
-// registration_generalized_icp (tzr_icp_generalized, tzr_icp_generalized_batch), given both clouds' normals.  No CPU
-// implementation: without a CUDA device the first call throws std::runtime_error.
+// registration_generalized_icp (tzr_icp_generalized, tzr_icp_generalized_batch), given both clouds' normals.  Both of
+// the last two take a teaser::RobustKernel (teaser/registration.h; L2 by default), Open3D's robust losses
+// (tzr_icp_point_to_plane_robust_batch, tzr_icp_generalized_robust_batch).  No CPU implementation: without a CUDA
+// device the first call throws std::runtime_error.
 #pragma once
 
 #include <vector>
@@ -43,6 +45,7 @@ class PointToPlaneICP {
 
   PointToPlaneICP() = default;
   explicit PointToPlaneICP(const Params& params) : params_(params) {}
+  PointToPlaneICP(const Params& params, const RobustKernel& kernel) : params_(params), kernel_(kernel) {}
 
   // Point-to-plane ICP of src onto dst seeded with init (its scale held fixed), on this thread's context.  dst_normals:
   // one normal per target point (curvature ignored; used as given, their signs do not matter).  Both clouds non-empty.
@@ -56,9 +59,13 @@ class PointToPlaneICP {
 
   const Params& getParams() const { return params_; }
   void setParams(const Params& params) { params_ = params; }
+  // The robust kernel: L2 (the default) runs tzr_icp_point_to_plane(_batch), any other tzr_icp_point_to_plane_robust_batch
+  const RobustKernel& getKernel() const { return kernel_; }
+  void setKernel(const RobustKernel& kernel) { kernel_ = kernel; }
 
  private:
   Params params_;
+  RobustKernel kernel_;
 };
 
 class GeneralizedICP {
@@ -68,6 +75,7 @@ class GeneralizedICP {
 
   GeneralizedICP() = default;
   explicit GeneralizedICP(const Params& params) : params_(params) {}
+  GeneralizedICP(const Params& params, const RobustKernel& kernel) : params_(params), kernel_(kernel) {}
 
   // Generalized ICP of src onto dst seeded with init (its scale held fixed), on this thread's context.  src_normals /
   // dst_normals: one normal per source / target point (curvature ignored; used up to length and sign).  Both clouds
@@ -83,9 +91,13 @@ class GeneralizedICP {
 
   const Params& getParams() const { return params_; }
   void setParams(const Params& params) { params_ = params; }
+  // The robust kernel: L2 (the default) runs tzr_icp_generalized(_batch), any other tzr_icp_generalized_robust_batch
+  const RobustKernel& getKernel() const { return kernel_; }
+  void setKernel(const RobustKernel& kernel) { kernel_ = kernel; }
 
  private:
   Params params_;
+  RobustKernel kernel_;
 };
 
 }  // namespace teaser

@@ -60,6 +60,16 @@ struct PointToPointICPParams {
 struct GeneralizedICPParams : PointToPointICPParams {
   double epsilon = 1e-3;
 };
+// A robust kernel for point-to-plane and generalized ICP (tzr_robust_kernel, DESIGN.md §3.15): Open3D's L2Loss (the
+// default, no weighting), L1Loss, HuberLoss(k), CauchyLoss(k), GMLoss(k) and TukeyLoss(k).  k must be finite and > 0 for
+// Huber, Cauchy, GM and Tukey; it is ignored for L2 and L1.
+struct RobustKernel {
+  enum Type { kL2 = 0, kL1 = 1, kHuber = 2, kCauchy = 3, kGM = 4, kTukey = 5 };
+  Type type = kL2;
+  double k = 1.0;
+  RobustKernel() = default;
+  RobustKernel(Type type_, double k_ = 1.0) : type(type_), k(k_) {}
+};
 struct PointToPointICPResult {
   RegistrationSolution solution;  // the refined transform; scale is the seed's, held fixed
   double fitness = 0;
@@ -352,6 +362,18 @@ class RobustRegistrationSolver {
                                                                 const std::vector<std::pair<int, int>>& pairs,
                                                                 const CloudPairParams& params,
                                                                 const GeneralizedICPParams& icp);
+  // The two overloads above with a robust kernel (tzr_register_cloud_pairs_icp_robust); each refined record equals
+  // PointToPlaneICP / GeneralizedICP with that kernel on the pair, seeded with its solution.
+  std::vector<CloudPairICPResult> solveCloudPairsPointToPlane(const std::vector<PointCloud>& clouds,
+                                                              const std::vector<std::pair<int, int>>& pairs,
+                                                              const CloudPairParams& params,
+                                                              const PointToPointICPParams& icp,
+                                                              const RobustKernel& kernel);
+  std::vector<CloudPairICPResult> solveCloudPairsGeneralizedICP(const std::vector<PointCloud>& clouds,
+                                                                const std::vector<std::pair<int, int>>& pairs,
+                                                                const CloudPairParams& params,
+                                                                const GeneralizedICPParams& icp,
+                                                                const RobustKernel& kernel);
   bool isMaxCliqueProvenOptimal() const { return clique_proven_; }
   long long getNumInlierGraphEdges() const { return n_edges_; }
   int getGNCRotationIterations() const { return gnc_iterations_; }

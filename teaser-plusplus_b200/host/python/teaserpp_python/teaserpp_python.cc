@@ -173,19 +173,42 @@ PYBIND11_MODULE(_teaserpp, m) {
            },
            py::arg("src"), py::arg("dst"), py::arg("init"));
 
+  // GPU extra: robust kernels for point-to-plane and generalized ICP (teaser::RobustKernel): RobustKernel("tukey", k)
+  // or RobustKernel(RobustKernel.Type.TUKEY, k); L2 by default
+  py::class_<teaser::RobustKernel> rk(m, "RobustKernel");
+  py::enum_<teaser::RobustKernel::Type>(rk, "Type")
+      .value("L2", teaser::RobustKernel::kL2)
+      .value("L1", teaser::RobustKernel::kL1)
+      .value("HUBER", teaser::RobustKernel::kHuber)
+      .value("CAUCHY", teaser::RobustKernel::kCauchy)
+      .value("GM", teaser::RobustKernel::kGM)
+      .value("TUKEY", teaser::RobustKernel::kTukey);
+  rk.def(py::init<>())
+      .def(py::init<teaser::RobustKernel::Type, double>(), py::arg("type"), py::arg("k") = 1.0)
+      .def(py::init([](const std::string& name, double k) {
+             static const char* names[] = {"l2", "l1", "huber", "cauchy", "gm", "tukey"};
+             for (int t = 0; t < 6; ++t)
+               if (name == names[t]) return teaser::RobustKernel(static_cast<teaser::RobustKernel::Type>(t), k);
+             throw std::invalid_argument("RobustKernel: unknown kernel \"" + name + "\"");
+           }),
+           py::arg("type"), py::arg("k") = 1.0)
+      .def_readwrite("type", &teaser::RobustKernel::type)
+      .def_readwrite("k", &teaser::RobustKernel::k);
+
   // GPU extra: point-to-plane ICP (teaser::PointToPlaneICP), given the target normals
   py::class_<teaser::PointToPlaneICP>(m, "PointToPlaneICP")
       .def(py::init([](double max_correspondence_distance, int max_iteration, double relative_fitness,
-                       double relative_rmse) {
+                       double relative_rmse, const teaser::RobustKernel& kernel) {
              teaser::PointToPlaneICP::Params p;
              p.max_correspondence_distance = max_correspondence_distance;
              p.max_iteration = max_iteration;
              p.relative_fitness = relative_fitness;
              p.relative_rmse = relative_rmse;
-             return teaser::PointToPlaneICP(p);
+             return teaser::PointToPlaneICP(p, kernel);
            }),
            py::arg("max_correspondence_distance"), py::arg("max_iteration") = 30, py::arg("relative_fitness") = 1e-6,
-           py::arg("relative_rmse") = 1e-6)
+           py::arg("relative_rmse") = 1e-6, py::arg("kernel") = teaser::RobustKernel())
+      .def_property("kernel", &teaser::PointToPlaneICP::getKernel, &teaser::PointToPlaneICP::setKernel)
       .def("refine",
            [](const teaser::PointToPlaneICP& icp, const CloudArray& src, const CloudArray& dst,
               const CloudArray& dst_normals, const teaser::RegistrationSolution& init) {
@@ -221,17 +244,18 @@ PYBIND11_MODULE(_teaserpp, m) {
   // GPU extra: generalized ICP (teaser::GeneralizedICP), given both clouds' normals
   py::class_<teaser::GeneralizedICP>(m, "GeneralizedICP")
       .def(py::init([](double max_correspondence_distance, int max_iteration, double relative_fitness,
-                       double relative_rmse, double epsilon) {
+                       double relative_rmse, double epsilon, const teaser::RobustKernel& kernel) {
              teaser::GeneralizedICP::Params p;
              p.max_correspondence_distance = max_correspondence_distance;
              p.max_iteration = max_iteration;
              p.relative_fitness = relative_fitness;
              p.relative_rmse = relative_rmse;
              p.epsilon = epsilon;
-             return teaser::GeneralizedICP(p);
+             return teaser::GeneralizedICP(p, kernel);
            }),
            py::arg("max_correspondence_distance"), py::arg("max_iteration") = 30, py::arg("relative_fitness") = 1e-6,
-           py::arg("relative_rmse") = 1e-6, py::arg("epsilon") = 1e-3)
+           py::arg("relative_rmse") = 1e-6, py::arg("epsilon") = 1e-3, py::arg("kernel") = teaser::RobustKernel())
+      .def_property("kernel", &teaser::GeneralizedICP::getKernel, &teaser::GeneralizedICP::setKernel)
       .def("refine",
            [](const teaser::GeneralizedICP& icp, const CloudArray& src, const CloudArray& dst,
               const CloudArray& src_normals, const CloudArray& dst_normals, const teaser::RegistrationSolution& init) {
@@ -433,11 +457,17 @@ PYBIND11_MODULE(_teaserpp, m) {
            [](Solver& s, const std::vector<CloudArray>& clouds, const std::vector<std::pair<int, int>>& pairs,
               double max_correspondence_distance, int max_iteration, double relative_fitness, double relative_rmse,
               double normal_search_radius, double fpfh_search_radius, bool use_absolute_scale, bool use_crosscheck,
-              bool use_tuple_test, float tuple_scale, uint64_t tuple_seed, const std::string& method, double epsilon) {
+              bool use_tuple_test, float tuple_scale, uint64_t tuple_seed, const std::string& method, double epsilon,
+              const py::object& kernel) {
              // GPU extra: solve_cloud_pairs, then point-to-point (point-to-plane, generalized) ICP of every pair with a
              // valid solution, in one call
              if (method != "point_to_point" && method != "point_to_plane" && method != "generalized")
                throw std::invalid_argument("method must be \"point_to_point\", \"point_to_plane\" or \"generalized\"");
+             // a robust kernel (point-to-plane and generalized only; None keeps the unweighted entries)
+             if (!kernel.is_none() && method == "point_to_point")
+               throw std::invalid_argument("point-to-point ICP takes no robust kernel");
+             const bool robust = !kernel.is_none();
+             const teaser::RobustKernel rk = robust ? kernel.cast<teaser::RobustKernel>() : teaser::RobustKernel();
              std::vector<teaser::PointCloud> pcs;
              for (const auto& a : clouds) pcs.push_back(cloud_of(a));
              Solver::CloudPairParams cp;
@@ -457,9 +487,13 @@ PYBIND11_MODULE(_teaserpp, m) {
              std::vector<Solver::CloudPairICPResult> res;
              {
                py::gil_scoped_release release;
-               res = method == "generalized"      ? s.solveCloudPairsGeneralizedICP(pcs, pairs, cp, ip)
-                     : method == "point_to_plane" ? s.solveCloudPairsPointToPlane(pcs, pairs, cp, ip)
-                                                  : s.solveCloudPairs(pcs, pairs, cp, ip);
+               if (robust)
+                 res = method == "generalized" ? s.solveCloudPairsGeneralizedICP(pcs, pairs, cp, ip, rk)
+                                               : s.solveCloudPairsPointToPlane(pcs, pairs, cp, ip, rk);
+               else
+                 res = method == "generalized"      ? s.solveCloudPairsGeneralizedICP(pcs, pairs, cp, ip)
+                       : method == "point_to_plane" ? s.solveCloudPairsPointToPlane(pcs, pairs, cp, ip)
+                                                    : s.solveCloudPairs(pcs, pairs, cp, ip);
              }
              py::list out;
              for (const auto& r : res)
@@ -473,7 +507,7 @@ PYBIND11_MODULE(_teaserpp, m) {
            py::arg("relative_fitness") = 1e-6, py::arg("relative_rmse") = 1e-6, py::arg("normal_search_radius") = 0.03,
            py::arg("fpfh_search_radius") = 0.05, py::arg("use_absolute_scale") = true, py::arg("use_crosscheck") = true,
            py::arg("use_tuple_test") = true, py::arg("tuple_scale") = 0.0f, py::arg("tuple_seed") = 0x7ea5e2ull,
-           py::arg("method") = "point_to_point", py::arg("epsilon") = 1e-3)
+           py::arg("method") = "point_to_point", py::arg("epsilon") = 1e-3, py::arg("kernel") = py::none())
       .def_property_readonly("solution", &Solver::getSolution)
       .def("getSolution", &Solver::getSolution)
       .def_property_readonly("gnc_rotation_cost_at_termination", &Solver::getGNCRotationCostAtTermination)

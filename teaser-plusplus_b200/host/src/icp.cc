@@ -52,13 +52,13 @@ void icp_result_from_c(const tzr_icp_result& r, const int32_t* corr, PointToPoin
 namespace {
 
 // every class's refineBatch: point-to-point when dst_normals is null, generalized when src_normals is given (with
-// epsilon), point-to-plane otherwise
+// epsilon), point-to-plane otherwise; a kernel other than L2 goes through the robust batch entries
 std::vector<PointToPointICPResult> refine_batch(const char* who, const PointToPointICPParams& params,
                                                 const std::vector<PointCloud>& src, const std::vector<PointCloud>& dst,
                                                 const std::vector<NormalCloud>* dst_normals,
                                                 const std::vector<RegistrationSolution>& init,
                                                 const std::vector<NormalCloud>* src_normals = nullptr,
-                                                double epsilon = 0) {
+                                                double epsilon = 0, const RobustKernel* kernel = nullptr) {
   const size_t B = src.size();
   if (dst.size() != B || init.size() != B || (dst_normals && dst_normals->size() != B) ||
       (src_normals && src_normals->size() != B))
@@ -97,7 +97,17 @@ std::vector<PointToPointICPResult> refine_batch(const char* who, const PointToPo
   tzr_ctx* ctx = b200_context();
   const int Bi = static_cast<int>(B);
   int rc;
-  if (src_normals)
+  if (kernel && kernel->type != RobustKernel::kL2) {
+    tzr_robust_kernel k;
+    std::memset(&k, 0, sizeof(k));
+    k.type = static_cast<int32_t>(kernel->type);
+    k.k = kernel->k;
+    rc = src_normals ? tzr_icp_generalized_robust_batch(ctx, &p, epsilon, Bi, ns.data(), sp.data(), snp.data(),
+                                                        nd.data(), dp.data(), np.data(), seeds.data(), res.data(),
+                                                        corr_p.data(), &k)
+                     : tzr_icp_point_to_plane_robust_batch(ctx, &p, Bi, ns.data(), sp.data(), nd.data(), dp.data(),
+                                                           np.data(), seeds.data(), res.data(), corr_p.data(), &k);
+  } else if (src_normals)
     rc = B == 1 ? tzr_icp_generalized(ctx, &p, epsilon, sp[0], ns[0], snp[0], dp[0], nd[0], np[0], seeds.data(),
                                       res.data(), corr_p[0])
                 : tzr_icp_generalized_batch(ctx, &p, epsilon, Bi, ns.data(), sp.data(), snp.data(), nd.data(),
@@ -140,7 +150,7 @@ std::vector<PointToPlaneICP::Result> PointToPlaneICP::refineBatch(const std::vec
                                                                   const std::vector<PointCloud>& dst,
                                                                   const std::vector<NormalCloud>& dst_normals,
                                                                   const std::vector<RegistrationSolution>& init) const {
-  return refine_batch("PointToPlaneICP", params_, src, dst, &dst_normals, init);
+  return refine_batch("PointToPlaneICP", params_, src, dst, &dst_normals, init, nullptr, 0, &kernel_);
 }
 
 GeneralizedICP::Result GeneralizedICP::refine(const PointCloud& src, const PointCloud& dst,
@@ -154,7 +164,8 @@ std::vector<GeneralizedICP::Result> GeneralizedICP::refineBatch(const std::vecto
                                                                 const std::vector<NormalCloud>& src_normals,
                                                                 const std::vector<NormalCloud>& dst_normals,
                                                                 const std::vector<RegistrationSolution>& init) const {
-  return refine_batch("GeneralizedICP", params_, src, dst, &dst_normals, init, &src_normals, params_.epsilon);
+  return refine_batch("GeneralizedICP", params_, src, dst, &dst_normals, init, &src_normals, params_.epsilon,
+                      &kernel_);
 }
 
 }  // namespace teaser

@@ -637,7 +637,8 @@ enum class IcpMethod { kPointToPoint, kPointToPlane, kGeneralized };
 std::vector<RobustRegistrationSolver::CloudPairResult> run_cloud_pairs(
     const tzr_params& p, const std::vector<PointCloud>& clouds, const std::vector<std::pair<int, int>>& pairs,
     const RobustRegistrationSolver::CloudPairParams& cp, const tzr_icp_params* icp,
-    std::vector<tzr_icp_result>* icp_res, IcpMethod method = IcpMethod::kPointToPoint, double epsilon = 0) {
+    std::vector<tzr_icp_result>* icp_res, IcpMethod method = IcpMethod::kPointToPoint, double epsilon = 0,
+    const RobustKernel* kernel = nullptr) {
   using CloudPairResult = RobustRegistrationSolver::CloudPairResult;
   const int K = static_cast<int>(clouds.size()), P = static_cast<int>(pairs.size());
   std::vector<CloudPairResult> out(P);
@@ -684,7 +685,17 @@ std::vector<RobustRegistrationSolver::CloudPairResult> run_cloud_pairs(
                                   scales.data());
   } else {
     icp_res->assign(P, tzr_icp_result{});
-    if (method == IcpMethod::kGeneralized)
+    if (kernel) {
+      tzr_robust_kernel k;
+      std::memset(&k, 0, sizeof(k));
+      k.type = static_cast<int32_t>(kernel->type);
+      k.k = kernel->k;
+      rc = tzr_register_cloud_pairs_icp_robust(ctx, &f, &p, K, n.data(), pts.data(), P, pc.data(), seeds.data(),
+                                               sols.data(), status.data(), index.data(), n_corr.data(), corr_p.data(),
+                                               clq_p.data(), scales.data(), icp,
+                                               method == IcpMethod::kGeneralized ? 2 : 1, epsilon, &k,
+                                               icp_res->data());
+    } else if (method == IcpMethod::kGeneralized)
       rc = tzr_register_cloud_pairs_icp_generalized(ctx, &f, &p, K, n.data(), pts.data(), P, pc.data(), seeds.data(),
                                                     sols.data(), status.data(), index.data(), n_corr.data(),
                                                     corr_p.data(), clq_p.data(), scales.data(), icp, epsilon,
@@ -722,7 +733,7 @@ std::vector<RobustRegistrationSolver::CloudPairResult> RobustRegistrationSolver:
 static std::vector<RobustRegistrationSolver::CloudPairICPResult> run_cloud_pairs_icp(
     const tzr_params& p, const std::vector<PointCloud>& clouds, const std::vector<std::pair<int, int>>& pairs,
     const RobustRegistrationSolver::CloudPairParams& cp, const PointToPointICPParams& icp, IcpMethod method,
-    double epsilon = 0) {
+    double epsilon = 0, const RobustKernel* kernel = nullptr) {
   using CloudPairResult = RobustRegistrationSolver::CloudPairResult;
   using CloudPairICPResult = RobustRegistrationSolver::CloudPairICPResult;
   tzr_icp_params ip;
@@ -732,7 +743,7 @@ static std::vector<RobustRegistrationSolver::CloudPairICPResult> run_cloud_pairs
   ip.relative_fitness = icp.relative_fitness;
   ip.relative_rmse = icp.relative_rmse;
   std::vector<tzr_icp_result> res;
-  std::vector<CloudPairResult> base = run_cloud_pairs(p, clouds, pairs, cp, &ip, &res, method, epsilon);
+  std::vector<CloudPairResult> base = run_cloud_pairs(p, clouds, pairs, cp, &ip, &res, method, epsilon, kernel);
   std::vector<CloudPairICPResult> out(base.size());
   for (size_t q = 0; q < base.size(); ++q) {
     static_cast<CloudPairResult&>(out[q]) = std::move(base[q]);
@@ -759,6 +770,18 @@ std::vector<RobustRegistrationSolver::CloudPairICPResult> RobustRegistrationSolv
     const std::vector<PointCloud>& clouds, const std::vector<std::pair<int, int>>& pairs, const CloudPairParams& cp,
     const GeneralizedICPParams& icp) {
   return run_cloud_pairs_icp(to_c(params_), clouds, pairs, cp, icp, IcpMethod::kGeneralized, icp.epsilon);
+}
+
+std::vector<RobustRegistrationSolver::CloudPairICPResult> RobustRegistrationSolver::solveCloudPairsPointToPlane(
+    const std::vector<PointCloud>& clouds, const std::vector<std::pair<int, int>>& pairs, const CloudPairParams& cp,
+    const PointToPointICPParams& icp, const RobustKernel& kernel) {
+  return run_cloud_pairs_icp(to_c(params_), clouds, pairs, cp, icp, IcpMethod::kPointToPlane, 0, &kernel);
+}
+
+std::vector<RobustRegistrationSolver::CloudPairICPResult> RobustRegistrationSolver::solveCloudPairsGeneralizedICP(
+    const std::vector<PointCloud>& clouds, const std::vector<std::pair<int, int>>& pairs, const CloudPairParams& cp,
+    const GeneralizedICPParams& icp, const RobustKernel& kernel) {
+  return run_cloud_pairs_icp(to_c(params_), clouds, pairs, cp, icp, IcpMethod::kGeneralized, icp.epsilon, &kernel);
 }
 
 void RobustRegistrationSolver::materialise_tims() {
