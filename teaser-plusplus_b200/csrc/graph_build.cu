@@ -19,6 +19,7 @@
 // Only pairs inside the 2*delta band (typically < 1e-4 of all pairs) are re-evaluated with the
 // exact double sequence, so the bitset is identical to a pure-FP64 evaluation (verified on device
 // by the TZR_FLAG_VERIFY mode and against the oracle in tests/).
+#include "tc_ptx.cuh"
 #include "tzr_internal.cuh"
 
 namespace tzr {
@@ -499,6 +500,26 @@ __host__ __device__ inline int strip_grid(int n) {
   return total;
 }
 
+// Strips of at most L blocks (graph_strip2_kernel, whose strip length is a launch parameter).  A row block of m blocks
+// has ceil(m / L) strips, so the rows of 1 ... m blocks hold strips_below(m, L) = L a (a + 1) / 2 + r (a + 1) of them,
+// m = a L + r, 0 <= r < L.  Strips are numbered from the longest row block (I = 0) down, row block by row block.
+__host__ __device__ inline int strips_below(int m, int L) {
+  const int a = m / L, r = m - a * L;
+  return L * (a * (a + 1) / 2) + r * (a + 1);
+}
+// strip p of strips_below(nt, L): its row block I and first column block J0
+__host__ __device__ inline void strip_decode(int p, int nt, int L, int* I, int* J0) {
+  const int q = strips_below(nt, L) - 1 - p;  // counted from the shortest row block up
+  // q lies in the row of m = a L + r + 1 blocks: a from L a (a + 1) / 2 <= q, by a float estimate and an exact fix-up
+  int a = (int)((sqrtf(1.f + 8.f * (float)q / (float)L) - 1.f) * 0.5f);
+  while (L * (a * (a + 1) / 2) > q) --a;
+  while (L * ((a + 1) * (a + 2) / 2) <= q) ++a;
+  const int rem = q - L * (a * (a + 1) / 2), r = rem / (a + 1);
+  const int m = a * L + r + 1;
+  *I = nt - m;
+  *J0 = *I + (a - (rem - r * (a + 1))) * L;  // the row's strips run left to right as p grows
+}
+
 // 32x32 bit transpose across the lanes of a warp: lane l passes row l, receives column l (bit i of the result =
 // bit l of lane i's input).  5 butterfly stages (shuffle + 4 logic ops each).
 __device__ __forceinline__ uint32_t warp_transpose32(uint32_t x, int lane) {
@@ -965,14 +986,31 @@ __device__ __forceinline__ void gram_sweep_any(const bool slope, const float4* r
 
 // The mirror half of an off-diagonal block (column words, 4 B per column row and warp) is gathered in a CTA-shared slice
 // and leaves as one 16-byte store per column row, with one degree atomic per column row carrying the sum of the four
-// warps' popcounts.  Every warp of the CTA runs every block of the strip and reaches every barrier: a warp without rows
-// (only in the last row block) sweeps nothing and contributes zero words.
+// warps' popcounts.
+//
+// The four warps of a CTA are coupled by mbarriers only, never by a CTA-wide barrier inside the strip:
+//   * column operands: the 128 column points of a block are one contiguous 4 KB run of gq (two 2 KB runs of sf and df in
+//     the two-slope form).  Thread 0 copies them with the bulk-copy engine into a ring of kColSlots CTA-shared slots, two
+//     blocks ahead of the sweep; the copy completes the slot's `full` mbarrier in hardware, and a warp that waits on it
+//     depends on no sibling.  One global read per CTA and block instead of one per warp.
+//   * `done` (4 arrivals, one per warp): a warp arrives at the end of block k of the strip, after it has written its
+//     words of block k into s_mir[k & 1] and has read the slice of block k-1.  Phase k therefore orders (1) every warp's
+//     s_mir writes of block k before any warp's read of that slice, which happens after the sweep of block k+1 (or after
+//     the strip's last block); (2) every warp's read of slice k-1 before the writes of block k+1 into the same slice;
+//     (3) every warp's read of the column slot of block k before thread 0 refills it with block k+3.  A warp waits for
+//     phase k-1 after its sweep of block k, so it stalls only if a sibling is a whole block behind.
+// Every warp of the CTA runs every block of the strip and arrives at every phase: a warp without rows (only in the last
+// row block) sweeps nothing, waits on no column slot and contributes zero words.
+constexpr int kColSlots = 3;
+
 template <bool kVerify, bool kFuseDeg, bool kRagged, bool kSlope>
 __device__ __forceinline__ void strip_gram(const Batch& bt, const int b, const int I, const int J0, const int J1) {
   const int nl = bt.n;
   const int n = kRagged ? bt.nb[b] : nl;
   __shared__ float4 s_gr[2 + 2 * kTile];
   __shared__ __align__(16) uint32_t s_mir[2][kTile][4];  // [block parity][column row][warp]
+  __shared__ __align__(128) float4 s_col[kColSlots][2 * kTile];
+  __shared__ __align__(8) uint64_t s_bar[kColSlots + 1];  // full[kColSlots], done
 
   const GraphConsts* gcp = bt.gc + b;
   constexpr bool slope = kSlope;  // the two-slope form is a kernel instance of its own (debug flag 134217728)
@@ -991,6 +1029,28 @@ __device__ __forceinline__ void strip_gram(const Batch& bt, const int b, const i
   const int ibase = I * kTile + 32 * w;
   const int nrows = max(0, min(32, n - ibase));  // 0 only in the last row block, whose one block is diagonal
   const float4 z4 = make_float4(0.f, 0.f, 0.f, 0.f);
+  const uint32_t bar_full = tc::smem_u32(s_bar), bar_done = bar_full + 8u * kColSlots;
+  // thread 0: the column points of block J that lie below n, into the ring slot of block J
+  auto fetch_columns = [&](const int J) {
+    const uint32_t slot = (uint32_t)(J - J0) % kColSlots;
+    const uint32_t cnt = (uint32_t)min(kTile, n - J * kTile);
+    const uint32_t dst = tc::smem_u32(&s_col[slot][0]), bar = bar_full + 8u * slot;
+    tc::mbar_arrive_expect_tx(bar, cnt * 32u);
+    if (slope) {
+      tc::bulk_g2s(dst, gq + 2 * (size_t)J * kTile, cnt * 32u, bar);
+    } else {
+      tc::bulk_g2s(dst, sf + (size_t)J * kTile, cnt * 16u, bar);
+      tc::bulk_g2s(dst + kTile * 16u, df + (size_t)J * kTile, cnt * 16u, bar);
+    }
+  };
+  if (tid == 0) {
+    for (int s = 0; s < kColSlots; ++s) tc::mbar_init(bar_full + 8u * s, 1);
+    tc::mbar_init(bar_done, kGraphThreads / 32);
+    tc::mbar_fence_init();
+  }
+  __syncthreads();  // the only CTA-wide barrier: publishes the initialised mbarriers
+  if (tid == 0)
+    for (int J = J0; J < min(J1, J0 + kColSlots); ++J) fetch_columns(J);
   {
     const int i = ibase + lane;
     if (slope) {
@@ -1012,18 +1072,31 @@ __device__ __forceinline__ void strip_gram(const Batch& bt, const int b, const i
 
   int* degp = bt.deg + (size_t)b * nl;
   int rdeg = 0;
+  // mirror half of block J: one 16-byte store and one degree atomic per column row, from the CTA-shared slice
+  auto store_mirror = [&](const int J) {
+    const int j = J * kTile + tid;
+    if (j < n) {
+      const uint4 v = *reinterpret_cast<const uint4*>(&s_mir[J & 1][tid][0]);
+      *reinterpret_cast<uint4*>(adj32 + (size_t)j * P32 + 4 * I) = v;
+      const int d = __popc(v.x) + __popc(v.y) + __popc(v.z) + __popc(v.w);
+      if (kFuseDeg && d) atomicAdd(degp + j, d);
+    }
+  };
+  uint32_t slot = 0u, full_parity = 0u;  // ring slot of block J and the phase of its `full` mbarrier
   for (int J = J0; J < J1; ++J) {
     const int jb = J * kTile + lane;
     uint32_t colw[4] = {0u, 0u, 0u, 0u};
     if (nrows > 0) {  // warp-uniform
       float4 cs[4], cd[4];
       bool vj[4];
+      tc::mbar_wait(bar_full + 8u * slot, full_parity);
+      const float4* col = s_col[slot];
 #pragma unroll
       for (int c = 0; c < 4; ++c) {
-        const int j = jb + 32 * c;
-        vj[c] = j < n;
-        cs[c] = vj[c] ? (slope ? gq[2 * j] : sf[j]) : z4;
-        cd[c] = vj[c] ? (slope ? gq[2 * j + 1] : df[j]) : z4;
+        const int jl = lane + 32 * c;
+        vj[c] = jb + 32 * c < n;  // the copy stopped at n: the slot's points past it are stale and not read
+        cs[c] = vj[c] ? col[slope ? 2 * jl : jl] : z4;
+        cd[c] = vj[c] ? col[slope ? 2 * jl + 1 : kTile + jl] : z4;
       }
       // column words of this lane: bit ii = pair (row ibase+ii, column jb + 32c); hi = surely an edge, lo = edge or
       // undecided
@@ -1110,20 +1183,27 @@ __device__ __forceinline__ void strip_gram(const Batch& bt, const int b, const i
             make_uint4(roww[0], roww[1], roww[2], roww[3]);
       if (kFuseDeg) rdeg += __popc(roww[0]) + __popc(roww[1]) + __popc(roww[2]) + __popc(roww[3]);
     }
-    // ---- mirror half (CTA-uniform: the diagonal block holds both orientations in its row words)
-    if (I != J) {
-      uint32_t(*mir)[4] = s_mir[J & 1];  // two slices: the barrier of block J+1 orders the reads of J before J+2's writes
-#pragma unroll
-      for (int c = 0; c < 4; ++c) mir[32 * c + lane][w] = colw[c];
-      __syncthreads();
-      const int j = J * kTile + tid;
-      if (j < n) {
-        const uint4 v = *reinterpret_cast<const uint4*>(&mir[tid][0]);
-        *reinterpret_cast<uint4*>(adj32 + (size_t)j * P32 + 4 * I) = v;
-        const int d = __popc(v.x) + __popc(v.y) + __popc(v.z) + __popc(v.w);
-        if (kFuseDeg && d) atomicAdd(degp + j, d);
-      }
+    if (++slot == kColSlots) {
+      slot = 0u;
+      full_parity ^= 1u;
     }
+    // ---- mirror half (CTA-uniform: the diagonal block, only ever a strip's first, holds both orientations in its row
+    // words and has no mirror).  Every warp has finished block J-1 once phase J-1-J0 of `done` completes.
+    if (J > J0) {
+      tc::mbar_wait(bar_done, (uint32_t)(J - 1 - J0) & 1u);
+      if (tid == 0 && J + 2 < J1) fetch_columns(J + 2);  // into the slot of block J-1
+    }
+    if (I != J) {
+#pragma unroll
+      for (int c = 0; c < 4; ++c) s_mir[J & 1][32 * c + lane][w] = colw[c];
+    }
+    if (J > J0 && I != J - 1) store_mirror(J - 1);
+    __syncwarp();
+    if (lane == 0) tc::mbar_arrive(bar_done);
+  }
+  if (I != J1 - 1) {
+    tc::mbar_wait(bar_done, (uint32_t)(J1 - 1 - J0) & 1u);
+    store_mirror(J1 - 1);
   }
   if (kFuseDeg && lane < nrows && rdeg) atomicAdd(degp + ibase + lane, rdeg);
 }
@@ -1147,15 +1227,9 @@ template <bool kVerify, int kMinBlocks, bool kFuseDeg, bool kRagged, bool kSlope
 __device__ __forceinline__ void strip2_body(const Batch& bt) {
   const int b = blockIdx.y;
   const int nt = (bt.n + kTile - 1) / kTile;
-  int I = 0, p = blockIdx.x;
-  while (true) {
-    const int ng = (nt - I + kStripBlocks - 1) / kStripBlocks;
-    if (p < ng) break;
-    p -= ng;
-    ++I;
-  }
-  const int J0 = I + p * kStripBlocks;
-  int J1 = min(nt, J0 + kStripBlocks);
+  int I, J0;
+  strip_decode((int)blockIdx.x, nt, bt.strip_blocks, &I, &J0);
+  int J1 = min(nt, J0 + bt.strip_blocks);
   if (kRagged) {
     const int ntb = (bt.nb[b] + kTile - 1) / kTile;
     if (J0 >= ntb) return;  // I <= J0: the whole strip lies past the problem's last tile
@@ -1180,10 +1254,27 @@ __global__ void __launch_bounds__(kGraphThreads, kMinBlocks) graph_strip2_ragged
   strip2_body<kVerify, kMinBlocks, kFuseDeg, true, kSlope>(bt);
 }
 
+// Strip length of graph_strip2_kernel, from the batch alone.  A strip pays its decode, the staging of its 128 row points,
+// one row-degree atomic per row and the start and drain of its CTA once, so longer strips amortise more; but the CTAs in
+// flight then spread over more problems, and past about 18 MB of bitsets in flight the stores stop merging in the L2 and
+// the kernel slows down sharply (DESIGN.md §3.1: 7 blocks already lose on C2 and C5).  kStripBlocksLong is used when
+// every CTA slot (num_sms x TZR_STRIP_MIN_BLOCKS of them) has at least kStripLongMinBlocks blocks to sweep in the launch
+// (C2, C4, C5); smaller batches (C2cube, C3, single problems) end on a tail of strips, which is shorter with kStripBlocks.
+constexpr int kStripBlocksLong = 6;
+constexpr long long kStripLongMinBlocks = 512;
+static int strip_blocks_for(int B, int n, int num_sms) {
+  const long long nt = (n + kTile - 1) / kTile;
+  const long long per_slot = (long long)B * nt * (nt + 1) / 2 / ((long long)num_sms * TZR_STRIP_MIN_BLOCKS);
+  return per_slot >= kStripLongMinBlocks ? kStripBlocksLong : kStripBlocks;
+}
+
 // the default strip kernel's instances: ragged size class or uniform batch, verifying (flag 2), separate degree pass
 // (flag 256) or the production template
 template <bool kSlope>
-void launch_strip2(const Batch& bt, const dim3 sgrid, cudaStream_t st) {
+void launch_strip2(Batch bt, const int num_sms, cudaStream_t st) {
+  const int nt = (bt.n + kTile - 1) / kTile;
+  bt.strip_blocks = strip_blocks_for(bt.B, bt.n, num_sms);
+  const dim3 sgrid((unsigned)strips_below(nt, bt.strip_blocks), (unsigned)bt.B);
   if (bt.nb) {
     if (bt.flags_dbg & 2u)
       graph_strip2_ragged_kernel<true, 5, false, kSlope><<<sgrid, kGraphThreads, 0, st>>>(bt);
@@ -1445,6 +1536,7 @@ void launch_prep(const Batch& bt, cudaStream_t st) { prep_kernel<<<bt.B, 256, 0,
 
 int launch_graph(const Batch& bt0, cudaStream_t st, int num_sms) {
   Batch bt = bt0;
+  bt.strip_blocks = kStripBlocks;  // (launch_strip2 chooses the default kernel's strip length)
   // default: CUDA-core strip kernel.  Debug flag 1024 routes every problem prep_kernel marked use_tc through the
   // tensor-core kernel instead (bit-identical output: DESIGN.md §3.1); not in ragged size classes
   bt.tc_active = (tc_path_active(bt.flags_dbg) && !bt.nb) ? 1 : 0;
@@ -1467,9 +1559,9 @@ int launch_graph(const Batch& bt0, cudaStream_t st, int num_sms) {
   if (bt.nb) {  // ragged size class: the default kernel (or its verify variant) whatever the opt-in flags 1024 and 2048 say
     cudaMemsetAsync(bt.adj, 0, (size_t)bt.B * bt.n * pitch64(bt.n) * sizeof(uint64_t), st);
     if (bt.flags_dbg & kFlagTwoSlope)
-      launch_strip2<false>(bt, sgrid, st);
+      launch_strip2<false>(bt, num_sms, st);
     else
-      launch_strip2<true>(bt, sgrid, st);
+      launch_strip2<true>(bt, num_sms, st);
   } else if (bt.flags_dbg & 2048u) {  // v7 (one MUFU, sign-bit words, re-check queue): fewer instructions, but FMA-pipe bound
     v7 = true;
     if (bt.flags_dbg & 2u)
@@ -1492,9 +1584,9 @@ int launch_graph(const Batch& bt0, cudaStream_t st, int num_sms) {
   }
 #endif
   else if (bt.flags_dbg & kFlagTwoSlope)
-    launch_strip2<false>(bt, sgrid, st);
+    launch_strip2<false>(bt, num_sms, st);
   else
-    launch_strip2<true>(bt, sgrid, st);
+    launch_strip2<true>(bt, num_sms, st);
   // exact re-check of the pairs the strip kernel queued (v7, or the Gram test: every problem unless debug flag 512)
   if (v7 || !(bt.flags_dbg & 512u)) {
     launch_graph_patch(bt, st, num_sms);

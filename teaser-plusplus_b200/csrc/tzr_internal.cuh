@@ -146,6 +146,7 @@ struct Batch {
   // keep their parameter offsets in every kernel.
   const int32_t* nb;        // device, B entries
   const int32_t* nb_host;   // host copy of nb (the unknown-scale large path's per-problem host loop)
+  int strip_blocks;         // 128-column blocks per strip of graph_strip2_kernel; set by launch_graph from B and n
 };
 
 // ---- rotation TIM sets (shared by rot_trans_kernel and the certifier's gather of a retained solve) ----------------------
