@@ -291,6 +291,13 @@ typedef struct tzr_certification_result {
 
 void tzr_certifier_params_default(tzr_certifier_params* p);
 
+/* tzr_certify and the single building blocks below (tzr_certifier_initial_matrix, tzr_certifier_dual_projection,
+ * tzr_certifier_psd_projection) are tzr_certify_batch's path with B = 1: the same kernels, and one cusolverDnDsyevd on
+ * the problem's (4n+4)^2 matrix per eigen step, so each result equals the batch entry's on that one problem bit for bit.
+ * traj may be NULL (no trajectory).  The trajectory is kept on the device (at most ceil(max_iterations) gaps) and the
+ * workspace is checked against free device memory.  Status: TZR_ERR_INVALID_ARG for a NULL pointer, n <= 0 or
+ * traj_capacity < 0; TZR_ERR_TOO_LARGE when 4n+4 exceeds 32768; TZR_ERR_ALLOC when the workspace does not fit the
+ * device; TZR_ERR_UNSUPPORTED when cuSOLVER cannot be loaded (tzr_certify and the PSD step only). */
 int tzr_certify(tzr_ctx* ctx, const tzr_certifier_params* params, const double* R_colmajor9, const double* src_3xN,
                 const double* dst_3xN, const double* theta, int n, tzr_certification_result* result, double* traj,
                 int traj_capacity);
@@ -334,7 +341,9 @@ int tzr_certifier_dual_projection(tzr_ctx* ctx, const double* W, const double* t
  * tzr_certifier_batch_psd_projection / tzr_certifier_batch_dual_projection: the same step, and the dual projection, on
  *   B problems of N[b] measurements on tzr_certify_batch's path: its padded layout and, for the PSD step, the
  *   eigensolver route that call would take for B problems (debug flag 2097152 included).  M[b], M_psd[b], W[b],
- *   W_dual[b]: (4N[b]+4)^2 column-major; theta[b]: N[b] doubles. */
+ *   W_dual[b]: (4N[b]+4)^2 column-major; theta[b]: N[b] doubles.
+ * The initial matrix and the dual projections (single and batch) run no eigensolver and do not load cuSOLVER: they
+ * work where it cannot be loaded. */
 int tzr_certifier_psd_projection(tzr_ctx* ctx, const double* M, int n, double* M_psd, double* w);
 int tzr_certifier_batch_psd_projection(tzr_ctx* ctx, int B, const int32_t* N, const double* const* M,
                                        double* const* M_psd);

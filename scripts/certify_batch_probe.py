@@ -1,4 +1,4 @@
-"""Times tzr_certify_batch against a loop of tzr_certify on the same inputs, and the two PSD-product kernels.
+"""Times tzr_certify_batch against a loop of tzr_certify (its B = 1 case) on the same inputs.
 
 Inputs: m chain TIMs of a noisy registration problem (unit-cube points, uniform noise inside the noise bound, 10 %
 outliers, the true rotation as the estimate; the TIM noise bound is twice the point noise bound), m in {50, 100, 250},
@@ -11,9 +11,7 @@ problem).  Cases whose loop takes longer than --budget seconds per call are time
 Uneven convergence, the normal case, gets two more lines timed the same way at the default sub_optimality: the five
 reference fixtures in one batch (9, 11, 15, 20 and 1000 iterations; large/case_2 scaled to the common noise bound, which
 leaves its gap trajectory unchanged), and m = 250 with one problem held at a wrong rotation (it runs to the cap of 50
-iterations) beside 15 that converge on iteration 1.  Then
-one torch.profiler run (separate from the timed runs) gives the mean device time of psd_gemm_kernel (tzr_certify,
-CUDA cores) and cbt_psd_kernel (the batch, DMMA) at each m.  The card name and power limit are read in the same run.
+iterations) beside 15 that converge on iteration 1.  The card name and power limit are read in the same run.
 
     python scripts/certify_batch_probe.py [--iters 10] [--reps 3] [--budget 20]
 """
@@ -149,23 +147,6 @@ def main():
             row["speedup"] = row["loop_ms"] / row["batch_ms"]
             row["speedup_loop_eig"] = row["loop_ms"] / row["batch_loop_eig_ms"]
             print(json.dumps(row), flush=True)
-    # kernel times of the two PSD products (profiler run of its own)
-    import torch
-    from torch.profiler import ProfilerActivity, profile
-    torch.cuda.init()
-    for m in [int(x) for x in a.ms.split(",")]:
-        p = chain_tims(m, 7)
-        with profile(activities=[ProfilerActivity.CUDA]) as prof:
-            ctx.certify(*p, **kw)
-            ctx.certify_batch(*[[x] for x in p], **kw)
-        acc = {}
-        for e in prof.events():
-            for k in ("psd_gemm_kernel", "cbt_psd_kernel"):
-                if k in e.name and e.device_type.name == "CUDA":
-                    acc.setdefault(k, []).append(e.device_time_total if hasattr(e, "device_time_total")
-                                                 else e.cuda_time_total)
-        print(json.dumps(dict(gpu=gpu, m=m, n=4 * m + 4, kernel_us={k: statistics.mean(v) for k, v in acc.items()},
-                              launches={k: len(v) for k, v in acc.items()})), flush=True)
     ctx.close()
 
 

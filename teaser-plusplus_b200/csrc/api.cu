@@ -30,7 +30,7 @@ struct tzr_ctx {
   int num_sms = 132;
   // device buffers (grow-only)
   DevBuf src, dst, sf, df, gq, pk, opnd, tclist, gc, adj, deg, nedges, hclq, hsize, clq, L, alive, best_bits, alive_cnt, root_ctr, lock, flg, kfinal, tstart, stack, cv,
-      centry, ps, pd, wgt, res, skey, sidx, sorted, rmask, tmask, sol, dbg, misc, sc, m_in, m_scratch, m_out, cert,
+      centry, ps, pd, wgt, res, skey, sidx, sorted, rmask, tmask, sol, dbg, misc, sc, m_in, m_scratch, m_out,
       certb;
   // large clique route (n > kMaxN or debug flag 524288): scratch on the full graph, and the compacted batch's buffers
   DevBuf lg, cq;
@@ -1223,7 +1223,7 @@ int tzr_ctx_destroy(tzr_ctx* ctx) {
                     &ctx->hclq, &ctx->hsize, &ctx->clq, &ctx->L, &ctx->alive, &ctx->best_bits, &ctx->alive_cnt, &ctx->root_ctr,
                     &ctx->lock, &ctx->flg, &ctx->kfinal, &ctx->tstart, &ctx->stack, &ctx->cv, &ctx->centry, &ctx->ps, &ctx->pd, &ctx->wgt,
                     &ctx->res, &ctx->skey, &ctx->sidx, &ctx->sorted, &ctx->rmask, &ctx->tmask, &ctx->sol, &ctx->dbg,
-                    &ctx->misc, &ctx->sc, &ctx->m_in, &ctx->m_scratch, &ctx->m_out, &ctx->cert, &ctx->certb, &ctx->lg, &ctx->cq, &ctx->rg, &ctx->icp,
+                    &ctx->misc, &ctx->sc, &ctx->m_in, &ctx->m_scratch, &ctx->m_out, &ctx->certb, &ctx->lg, &ctx->cq, &ctx->rg, &ctx->icp,
                     &ctx->vox};
   for (DevBuf* b : bufs)
     if (b->p) cudaFree(b->p);
@@ -1885,10 +1885,11 @@ int tzr_certify_last_solve(tzr_ctx* ctx, const tzr_certifier_params* params, int
     const int K = (int)gin.size();
     std::vector<tzr_certification_result> res((size_t)K);
     std::vector<int32_t> ok((size_t)K, 0);
-    const int rc = certify_batch_device(0, *params, K, N.data(), R.data(), nullptr, nullptr, nullptr, gin.data(),
-                                        ok.data(), res.data(), traj ? tr.data() : nullptr, traj ? tc.data() : nullptr,
-                                        nullptr, nullptr, (ctx->flags & 2097152u) != 0, &ctx->certb.p,
-                                        &ctx->certb.cap, &ctx->solver_handle, &ctx->launches, st, &ctx->last_error);
+    const int rc = certify_batch_device(CertMode::kCertify, *params, K, N.data(), R.data(), nullptr, nullptr, nullptr,
+                                        gin.data(), ok.data(), res.data(), traj ? tr.data() : nullptr,
+                                        traj ? tc.data() : nullptr, nullptr, nullptr, nullptr, nullptr,
+                                        (ctx->flags & 2097152u) != 0, &ctx->certb.p, &ctx->certb.cap,
+                                        &ctx->solver_handle, &ctx->launches, st, &ctx->last_error);
     if (rc != TZR_OK) return rc;
     for (int i = 0; i < K; ++i) {
       const int j = which[i];
@@ -1942,17 +1943,11 @@ int tzr_certify(tzr_ctx* ctx, const tzr_certifier_params* params, const double* 
   if (!ctx || !params || !R_colmajor9 || !src_3xN || !dst_3xN || !theta || !result || n <= 0 || traj_capacity < 0)
     return TZR_ERR_INVALID_ARG;
   cudaSetDevice(ctx->device);
-  int opt = 0, iters = 0;
-  double best = 0;
-  const int rc = certify_device(0, params->noise_bound, params->cbar2, params->sub_optimality, params->max_iterations,
-                                params->gamma_tau, R_colmajor9, src_3xN, dst_3xN, theta, n, &opt, &best, &iters, traj,
-                                traj_capacity, nullptr, nullptr, nullptr, nullptr, nullptr, &ctx->cert.p, &ctx->cert.cap,
-                                &ctx->solver_handle, &ctx->launches, ctx->stream, &ctx->last_error);
-  if (rc != TZR_OK) return rc;
-  result->is_optimal = opt;
-  result->n_iterations = iters;
-  result->best_suboptimality = best;
-  return TZR_OK;
+  const int32_t N = n, cap = traj_capacity;
+  return certify_batch_device(CertMode::kCertify, *params, 1, &N, R_colmajor9, &src_3xN, &dst_3xN, &theta, nullptr,
+                              nullptr, result, traj ? &traj : nullptr, &cap, nullptr, nullptr, nullptr, nullptr, false,
+                              &ctx->certb.p, &ctx->certb.cap, &ctx->solver_handle, &ctx->launches, ctx->stream,
+                              &ctx->last_error);
 }
 
 int tzr_certify_batch(tzr_ctx* ctx, const tzr_certifier_params* params, int B, const int32_t* N,
@@ -1966,8 +1961,9 @@ int tzr_certify_batch(tzr_ctx* ctx, const tzr_certifier_params* params, int B, c
     if (N[b] <= 0 || !src_3xN[b] || !dst_3xN[b] || !theta[b] || (traj_capacity && traj_capacity[b] < 0))
       return TZR_ERR_INVALID_ARG;
   cudaSetDevice(ctx->device);
-  return certify_batch_device(0, *params, B, N, R_colmajor9xB, src_3xN, dst_3xN, theta, nullptr, nullptr, results,
-                              traj, traj_capacity, nullptr, nullptr, (ctx->flags & 2097152u) != 0, &ctx->certb.p, &ctx->certb.cap, &ctx->solver_handle,
+  return certify_batch_device(CertMode::kCertify, *params, B, N, R_colmajor9xB, src_3xN, dst_3xN, theta, nullptr,
+                              nullptr, results, traj, traj_capacity, nullptr, nullptr, nullptr, nullptr,
+                              (ctx->flags & 2097152u) != 0, &ctx->certb.p, &ctx->certb.cap, &ctx->solver_handle,
                               &ctx->launches, ctx->stream, &ctx->last_error);
 }
 
@@ -1977,50 +1973,47 @@ int tzr_certifier_initial_matrix(tzr_ctx* ctx, const tzr_certifier_params* param
   if (!ctx || !params || !R_colmajor9 || !src_3xN || !dst_3xN || !theta || !M_init || !mu || n <= 0)
     return TZR_ERR_INVALID_ARG;
   cudaSetDevice(ctx->device);
-  return certify_device(1, params->noise_bound, params->cbar2, 0, 0, 0, R_colmajor9, src_3xN, dst_3xN, theta, n,
-                        nullptr, nullptr, nullptr, nullptr, 0, M_init, mu, nullptr, nullptr, nullptr, &ctx->cert.p,
-                        &ctx->cert.cap, &ctx->solver_handle, &ctx->launches, ctx->stream, &ctx->last_error);
+  const int32_t N = n;
+  return certify_batch_device(CertMode::kSetup, *params, 1, &N, R_colmajor9, &src_3xN, &dst_3xN, &theta, nullptr,
+                              nullptr, nullptr, nullptr, nullptr, nullptr, &M_init, nullptr, mu, false, &ctx->certb.p,
+                              &ctx->certb.cap, &ctx->solver_handle, &ctx->launches, ctx->stream, &ctx->last_error);
 }
 
-int tzr_certifier_dual_projection(tzr_ctx* ctx, const double* W, const double* theta, int n, double* W_dual) {
-  if (!ctx || !W || !theta || !W_dual || n <= 0) return TZR_ERR_INVALID_ARG;
-  cudaSetDevice(ctx->device);
-  return certify_device(2, 0, 0, 0, 0, 0, nullptr, nullptr, nullptr, theta, n, nullptr, nullptr, nullptr, nullptr, 0,
-                        nullptr, nullptr, W, W_dual, nullptr, &ctx->cert.p, &ctx->cert.cap, &ctx->solver_handle, &ctx->launches, ctx->stream,
-                        &ctx->last_error);
-}
-
-int tzr_certifier_psd_projection(tzr_ctx* ctx, const double* M, int n, double* M_psd, double* w) {
-  if (!ctx || !M || !M_psd || !w || n <= 0) return TZR_ERR_INVALID_ARG;
-  cudaSetDevice(ctx->device);
-  return certify_device(3, 0, 0, 0, 0, 0, nullptr, nullptr, nullptr, nullptr, n, nullptr, nullptr, nullptr, nullptr, 0,
-                        nullptr, nullptr, M, M_psd, w, &ctx->cert.p, &ctx->cert.cap, &ctx->solver_handle,
-                        &ctx->launches, ctx->stream, &ctx->last_error);
-}
-
-// the batch building blocks (certify_batch_device modes 1 and 2): B problems of N[b] >= 1 measurements
-static int certifier_batch_block(tzr_ctx* ctx, int mode, int B, const int32_t* N, const double* const* X,
-                                 const double* const* theta, double* const* Y) {
-  if (!ctx || B <= 0 || !N || !X || !Y || (mode == 2 && !theta)) return TZR_ERR_INVALID_ARG;
+// the building blocks (certify_batch_device's kPsd and kDual): B problems of N[b] >= 1 measurements; w (kPsd, may be
+// NULL) as certify_batch_device's w_out
+static int certifier_block(tzr_ctx* ctx, CertMode mode, int B, const int32_t* N, const double* const* X,
+                           const double* const* theta, double* const* Y, double* const* w) {
+  const bool dual = mode == CertMode::kDual;
+  if (!ctx || B <= 0 || !N || !X || !Y || (dual && !theta)) return TZR_ERR_INVALID_ARG;
   for (int b = 0; b < B; ++b)
-    if (N[b] <= 0 || !X[b] || !Y[b] || (mode == 2 && !theta[b])) return TZR_ERR_INVALID_ARG;
+    if (N[b] <= 0 || !X[b] || !Y[b] || (dual && !theta[b])) return TZR_ERR_INVALID_ARG;
   cudaSetDevice(ctx->device);
   tzr_certifier_params prm;
   tzr_certifier_params_default(&prm);
   return certify_batch_device(mode, prm, B, N, nullptr, nullptr, nullptr, theta, nullptr, nullptr, nullptr, nullptr,
-                              nullptr, X, Y,
-                              (ctx->flags & 2097152u) != 0, &ctx->certb.p, &ctx->certb.cap, &ctx->solver_handle,
-                              &ctx->launches, ctx->stream, &ctx->last_error);
+                              nullptr, X, Y, w, nullptr, (ctx->flags & 2097152u) != 0, &ctx->certb.p, &ctx->certb.cap,
+                              &ctx->solver_handle, &ctx->launches, ctx->stream, &ctx->last_error);
+}
+
+int tzr_certifier_dual_projection(tzr_ctx* ctx, const double* W, const double* theta, int n, double* W_dual) {
+  const int32_t N = n;
+  return certifier_block(ctx, CertMode::kDual, 1, &N, &W, &theta, &W_dual, nullptr);
+}
+
+int tzr_certifier_psd_projection(tzr_ctx* ctx, const double* M, int n, double* M_psd, double* w) {
+  if (!w) return TZR_ERR_INVALID_ARG;
+  const int32_t N = n;
+  return certifier_block(ctx, CertMode::kPsd, 1, &N, &M, nullptr, &M_psd, &w);
 }
 
 int tzr_certifier_batch_psd_projection(tzr_ctx* ctx, int B, const int32_t* N, const double* const* M,
                                        double* const* M_psd) {
-  return certifier_batch_block(ctx, 1, B, N, M, nullptr, M_psd);
+  return certifier_block(ctx, CertMode::kPsd, B, N, M, nullptr, M_psd, nullptr);
 }
 
 int tzr_certifier_batch_dual_projection(tzr_ctx* ctx, int B, const int32_t* N, const double* const* W,
                                         const double* const* theta, double* const* W_dual) {
-  return certifier_batch_block(ctx, 2, B, N, W, theta, W_dual);
+  return certifier_block(ctx, CertMode::kDual, B, N, W, theta, W_dual, nullptr);
 }
 
 int tzr_compute_fpfh(tzr_ctx* ctx, const float* pts, int n, double normal_search_radius, double fpfh_search_radius,

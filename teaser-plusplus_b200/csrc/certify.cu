@@ -1,20 +1,23 @@
 // Certification downstream of solve(): teaser::DRSCertifier::certify (reference teaser/src/certification.cc:40-190)
-// on the device, FP64 throughout.  n = 4N + 4; all matrices are dense n x n, column-major.
+// on the device, FP64 throughout, for B problems in one launch sequence; tzr_certify and the single building blocks
+// are the case B = 1.  Problem b has n = 4N + 4; its matrices are dense, column-major, padded to the group's nmax.
 //
-//   cert_blocks_kernel   per measurement k: the 4x4 blocks of Q_cost (getQCost, :233-291) already rotated by the
+//   cbt_blocks_kernel    per measurement k: the 4x4 blocks of Q_cost (getQCost, :233-291) already rotated by the
 //                        block-diagonal Omega (:293-314: Q_bar = D^T Q D acts block-wise), the 4x4 block of the initial
 //                        multiplier guess (getLambdaGuess, :448-529) and the terms of mu = x^T Q x (:92).
-//   cert_reduce_kernel   sums those per-k terms (top-left lambda block, mu).
-//   cert_fill_kernel     assembles M_init = Q_bar - mu J_bar - lambda_bar_init (:100).
-//   sym_kernel           B = (M + M^T) / 2 (getNearestPSD linalg.h:90; computeSubOptimalityGap :193).
-//   [eigendecomposition of B: cusolverDnDsyevd, loaded lazily with dlopen — the one library call of this stage, in
-//    the role cuBLAS has for plain GEMMs; see DESIGN.md 3.10]
-//   psd_gemm_kernel      M_PSD = V diag(max(w, 0)) V^T over the positive eigenpairs only (linalg.h:93-98).
-//   affine_in_kernel     W = 2 M_PSD - M - M_init (:139).
-//   dual_bw_kernel .. dual_diag_kernel   getOptimalDualProjection (:316-446) with the sparse inverse map A_inv
+//   cbt_reduce_kernel    sums those per-k terms (top-left lambda block, mu).
+//   cbt_fill_kernel      assembles M_init = Q_bar - mu J_bar - lambda_bar_init (:100).
+//   cbt_sym_kernel       B = (M + M^T) / 2 (getNearestPSD linalg.h:90; computeSubOptimalityGap :193).
+//   [eigendecomposition of B: cusolverDnDsyevd per problem, or cusolverDnXsyevBatched over 8 or more, loaded lazily
+//    with dlopen — the one library call of this stage, in the role cuBLAS has for plain GEMMs; see DESIGN.md 3.10]
+//   cbt_psd_kernel       M_PSD = V diag(max(w, 0)) V^T over the positive eigenpairs only (linalg.h:93-98), from the first
+//                        positive eigenvalue that cbt_first_pos_kernel finds; FP64 tensor cores.
+//   cbt_affine_kernel    W = 2 M_PSD - M - M_init (:139); M_affine = M_init + W_dual (:153);
+//                        M += gamma_tau (M_affine - M_PSD) (:181).
+//   cbt_dual_bw_kernel .. cbt_dual_mean_kernel   getOptimalDualProjection (:316-446) with the sparse inverse map A_inv
 //                        (getLinearProjection, :531-655: (N(N+1)/2)^2 entries in the reference) applied in closed form:
 //                        out[a,b] = (x+2y) B[a,b] + y (th_a (Rs[b]-Cs[b]) - th_b (Rs[a]-Cs[a])) with two O(N^2) sums.
-//   update_kernel        M_affine = M_init + W_dual (:153); M += gamma_tau (M_affine - M_PSD) (:181).
+//   cbt_gap_kernel       the sub-optimality gap (:192-231), the trajectory and the stop rule.
 #include <cusolverDn.h>
 #include <dlfcn.h>
 
@@ -197,15 +200,6 @@ __device__ __forceinline__ void cert_block(int k, const double* __restrict__ src
   for (int e = 0; e < 16; ++e) lam[16 * (size_t)k + e] = blk[e];
 }
 
-__global__ void cert_blocks_kernel(const double* __restrict__ src, const double* __restrict__ dst,
-                                   const double* __restrict__ theta, int N, const double* __restrict__ Rcm,
-                                   const double* __restrict__ q_xyzw, double nbs, double* offA, double* diagB,
-                                   double* lam, double* mu_terms) {
-  const int k = blockIdx.x * blockDim.x + threadIdx.x;
-  if (k >= N) return;
-  cert_block(k, src, dst, theta, Rcm, q_xyzw, nbs, offA, diagB, lam, mu_terms);
-}
-
 // one CTA: top[16] = sum_k lam_k, *mu = sum_k mu_terms[k] (k ascending per thread, then a fixed tree: deterministic)
 __device__ __forceinline__ void cert_reduce_cta(const double* lam, const double* mu_terms, int N, double* top,
                                                 double* mu) {
@@ -227,11 +221,6 @@ __device__ __forceinline__ void cert_reduce_cta(const double* lam, const double*
   }
 }
 
-__global__ void __launch_bounds__(256) cert_reduce_kernel(const double* lam, const double* mu_terms, int N,
-                                                         double* top, double* mu) {
-  cert_reduce_cta(lam, mu_terms, N, top, mu);
-}
-
 // M_init = Q_bar - mu J_bar - lambda_bar_init, one thread per entry
 __device__ __forceinline__ double cert_fill_value(int r, int c, const double* offA, const double* diagB,
                                                   const double* lam, const double* top, const double* mu) {
@@ -249,91 +238,6 @@ __device__ __forceinline__ double cert_fill_value(int r, int c, const double* of
   return v;
 }
 
-__global__ void cert_fill_kernel(int N, const double* offA, const double* diagB, const double* lam, const double* top,
-                                 const double* mu, double* M_init) {
-  const int n = 4 * N + 4;
-  const long long e = blockIdx.x * (long long)blockDim.x + threadIdx.x;
-  if (e >= (long long)n * n) return;
-  M_init[e] = cert_fill_value((int)(e % n), (int)(e / n), offA, diagB, lam, top, mu);
-}
-
-__global__ void sym_kernel(const double* __restrict__ M, int n, double* __restrict__ B) {
-  const long long e = blockIdx.x * (long long)blockDim.x + threadIdx.x;
-  if (e >= (long long)n * n) return;
-  const int r = (int)(e % n), c = (int)(e / n);
-  B[e] = (M[e] + M[(size_t)r * n + c]) / 2;
-}
-
-// first index with w > 0 (w ascending) and Vs = V * diag(max(w, 0)) for those columns
-__global__ void scale_pos_kernel(const double* __restrict__ V, const double* __restrict__ w, int n,
-                                 double* __restrict__ Vs) {
-  const long long e = blockIdx.x * (long long)blockDim.x + threadIdx.x;
-  if (e >= (long long)n * n) return;
-  const int c = (int)(e / n);
-  const double wc = w[c];
-  Vs[e] = wc > 0 ? V[e] * wc : 0.0;
-}
-
-__global__ void first_pos_kernel(const double* w, int n, int* first_pos) {
-  if (threadIdx.x == 0 && blockIdx.x == 0) {
-    int lo = 0, hi = n;  // w ascending
-    while (lo < hi) {
-      const int mid = (lo + hi) >> 1;
-      if (w[mid] > 0) hi = mid;
-      else lo = mid + 1;
-    }
-    *first_pos = lo;
-  }
-}
-
-// C (n x n) = Vs[:, k0:] * V[:, k0:]^T, 64 x 64 tile per CTA, 16 x 16 threads x (4 x 4), k in slabs of 16
-constexpr int kGT = 64, kGK = 16;
-__global__ void __launch_bounds__(256) psd_gemm_kernel(const double* __restrict__ Vs, const double* __restrict__ V,
-                                                      int n, const int* __restrict__ first_pos,
-                                                      double* __restrict__ C) {
-  __shared__ double As[kGK][kGT + 1], Bs[kGK][kGT + 1];
-  const int k0 = *first_pos;
-  const int tx = threadIdx.x & 15, ty = threadIdx.x >> 4;
-  const int r0 = blockIdx.x * kGT, c0 = blockIdx.y * kGT;
-  double acc[4][4];
-  for (int i = 0; i < 4; ++i)
-    for (int j = 0; j < 4; ++j) acc[i][j] = 0;
-  for (int kb = k0; kb < n; kb += kGK) {
-    for (int e = threadIdx.x; e < kGK * kGT; e += 256) {
-      const int kk = e / kGT, i = e % kGT;
-      const int k = kb + kk;
-      As[kk][i] = (k < n && r0 + i < n) ? Vs[(size_t)k * n + r0 + i] : 0.0;
-      Bs[kk][i] = (k < n && c0 + i < n) ? V[(size_t)k * n + c0 + i] : 0.0;
-    }
-    __syncthreads();
-#pragma unroll
-    for (int kk = 0; kk < kGK; ++kk) {
-      double a[4], b[4];
-#pragma unroll
-      for (int i = 0; i < 4; ++i) {
-        a[i] = As[kk][ty * 4 + i];
-        b[i] = Bs[kk][tx * 4 + i];
-      }
-#pragma unroll
-      for (int i = 0; i < 4; ++i)
-#pragma unroll
-        for (int j = 0; j < 4; ++j) acc[i][j] = fma(a[i], b[j], acc[i][j]);
-    }
-    __syncthreads();
-  }
-  for (int i = 0; i < 4; ++i)
-    for (int j = 0; j < 4; ++j) {
-      const int r = r0 + ty * 4 + i, c = c0 + tx * 4 + j;
-      if (r < n && c < n) C[(size_t)c * n + r] = acc[i][j];
-    }
-}
-
-__global__ void affine_in_kernel(const double* __restrict__ Mpsd, const double* __restrict__ M,
-                                 const double* __restrict__ Minit, long long nn, double* __restrict__ W) {
-  const long long e = blockIdx.x * (long long)blockDim.x + threadIdx.x;
-  if (e < nn) W[e] = 2 * Mpsd[e] - M[e] - Minit[e];
-}
-
 // ---- getOptimalDualProjection -----------------------------------------------------------------------------------
 // pair (i, j), 0 <= i < j <= N, running index as in the reference's double loop (:342-343)
 __device__ __forceinline__ long long pair_id(int i, int j, int N1) {  // N1 = N + 1 blocks
@@ -342,8 +246,7 @@ __device__ __forceinline__ long long pair_id(int i, int j, int N1) {  // N1 = N 
 
 #define WAT(r, c) W[(size_t)(c) * n + (r)]
 
-// The bodies below take the leading dimension n of W / Wd as an argument: 4N+4 for tzr_certify, the padded size of a
-// certify batch (cbt_* kernels further down).
+// The bodies below take the leading dimension n of W / Wd as an argument: the padded size of a certify batch.
 // bW[p][0..2] = -th_ij C + D - E + th_ij F (:349-368)
 __device__ __forceinline__ void dual_bw_at(const double* __restrict__ W, int n, const double* __restrict__ thp, int N,
                                            int i, int j, double* __restrict__ bW) {
@@ -358,11 +261,6 @@ __device__ __forceinline__ void dual_bw_at(const double* __restrict__ W, int n, 
   }
 }
 
-__global__ void dual_bw_kernel(const double* __restrict__ W, const double* __restrict__ thp, int N,
-                               double* __restrict__ bW) {
-  dual_bw_at(W, 4 * N + 4, thp, N, blockIdx.y, blockIdx.x * blockDim.x + threadIdx.x, bW);
-}
-
 // D[v][c] = Rs[v][c] - Cs[v][c]: Rs[v] = sum_{j>v} th_j B[v,j], Cs[v] = sum_{i<v} th_i B[i,v]   (one thread per (v,c))
 __device__ __forceinline__ void dual_sums_at(const double* __restrict__ bW, const double* __restrict__ thp, int N,
                                              int t, double* __restrict__ D) {
@@ -373,11 +271,6 @@ __device__ __forceinline__ void dual_sums_at(const double* __restrict__ bW, cons
   for (int j = v + 1; j < N1; ++j) rs += thp[j] * bW[3 * pair_id(v, j, N1) + c];
   for (int i = 0; i < v; ++i) cs += thp[i] * bW[3 * pair_id(i, v, N1) + c];
   D[t] = rs - cs;
-}
-
-__global__ void dual_sums_kernel(const double* __restrict__ bW, const double* __restrict__ thp, int N,
-                                 double* __restrict__ D) {
-  dual_sums_at(bW, thp, N, blockIdx.x * blockDim.x + threadIdx.x, D);
 }
 
 // off-diagonal blocks of W_dual (both triangles) (:381-415), A_inv applied in closed form
@@ -403,12 +296,6 @@ __device__ __forceinline__ void dual_off_at(const double* __restrict__ W, int n,
       Wd[(size_t)(4 * j + c) * n + 4 * i + r] = blk[r + 4 * c];
       Wd[(size_t)(4 * i + r) * n + 4 * j + c] = blk[r + 4 * c];  // transpose (:416-417)
     }
-}
-
-__global__ void dual_off_kernel(const double* __restrict__ W, const double* __restrict__ thp,
-                                const double* __restrict__ bW, const double* __restrict__ D, int N,
-                                double* __restrict__ Wd) {
-  dual_off_at(W, 4 * N + 4, thp, bW, D, N, blockIdx.y, blockIdx.x * blockDim.x + threadIdx.x, Wd);
 }
 
 // diagonal blocks (:419-434): one warp per block row; then diag3[i][9] holds the 3x3 corner for the mean
@@ -439,12 +326,6 @@ __device__ __forceinline__ void dual_diag_at(const double* __restrict__ W, int n
   }
 }
 
-__global__ void dual_diag_kernel(const double* __restrict__ W, const double* __restrict__ thp, int N,
-                                 double* __restrict__ Wd, double* __restrict__ diag3) {
-  dual_diag_at(W, 4 * N + 4, thp, N, blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5), threadIdx.x & 31, Wd,
-               diag3);
-}
-
 // one CTA: mean of the 3x3 corners, subtracted from every diagonal block (:435-445)
 __device__ __forceinline__ void dual_mean_cta(const double* __restrict__ diag3, int n, int N,
                                               double* __restrict__ Wd) {
@@ -467,23 +348,6 @@ __device__ __forceinline__ void dual_mean_cta(const double* __restrict__ diag3, 
     const int i = t / 9, e = t % 9, r = e % 3, c = e / 3;
     Wd[(size_t)(4 * i + c) * n + 4 * i + r] -= mean[e];
   }
-}
-
-__global__ void __launch_bounds__(256) dual_mean_kernel(const double* __restrict__ diag3, int N,
-                                                       double* __restrict__ Wd) {
-  dual_mean_cta(diag3, 4 * N + 4, N, Wd);
-}
-
-__global__ void affine_out_kernel(const double* __restrict__ Minit, const double* __restrict__ Wd, long long nn,
-                                  double* __restrict__ Maff) {
-  const long long e = blockIdx.x * (long long)blockDim.x + threadIdx.x;
-  if (e < nn) Maff[e] = Minit[e] + Wd[e];
-}
-
-__global__ void update_kernel(double* __restrict__ M, const double* __restrict__ Maff,
-                              const double* __restrict__ Mpsd, long long nn, double gamma_tau) {
-  const long long e = blockIdx.x * (long long)blockDim.x + threadIdx.x;
-  if (e < nn) M[e] += gamma_tau * (Maff[e] - Mpsd[e]);
 }
 
 inline int grid1(long long items, int threads) { return (int)((items + threads - 1) / threads); }
@@ -781,7 +645,7 @@ __global__ void cbt_scatter_kernel(const int* __restrict__ idx, int nmax, int ve
   if (e == 0) info[b] = infoc[s];
 }
 
-// certify_device's gap rule per active problem (info != 0 -> inf, min_eig > 0 -> 0, else -min_eig (N+1) / mu), the
+// The gap rule per active problem (info != 0 -> inf, min_eig > 0 -> 0, else -min_eig (N+1) / mu), the
 // trajectory entry, the best gap, and the stop rule (gap < sub_optimality or the iteration cap); active_out: the flags
 __global__ void cbt_gap_kernel(CertBatchProb* pr, int B, int nmax, const double* __restrict__ w,
                                const int* __restrict__ info, int iter, double sub_optimality, double max_iterations,
@@ -805,78 +669,6 @@ __global__ void cbt_gap_kernel(CertBatchProb* pr, int B, int nmax, const double*
 
 
 }  // namespace
-
-// ---- host-side driver objects ------------------------------------------------------------------------------------
-struct CertWork {
-  // device pointers carved from one scratch allocation
-  double *src, *dst, *theta, *thp, *R, *q, *offA, *diagB, *lam, *mu_terms, *top, *mu;
-  double *M_init, *M, *B, *w, *Vs, *M_psd, *W, *Wd, *M_aff, *bW, *D, *diag3, *work;
-  int *first_pos, *info;
-  int lwork;
-};
-
-size_t cert_scratch_bytes(int N, int lwork) {
-  const size_t n = 4 * (size_t)N + 4, nn = n * n, N1 = (size_t)N + 1;
-  size_t d = 0;
-  d += 3 * N + 3 * N + N + N1 + 9 + 4;              // src dst theta thp R q
-  d += 16 * (size_t)N * 3 + N + 16 + 1;             // offA diagB lam mu_terms top mu
-  d += nn * 8;                                      // M_init M B Vs M_psd W Wd M_aff
-  d += n;                                           // w
-  d += 3 * N1 * (N1 - 1) / 2 + 3 * N1 + 9 * N1;     // bW D diag3
-  d += (size_t)lwork;
-  return d * sizeof(double) + 64 * 34 + 256;
-}
-
-static CertWork carve(void* scratch, int N, int lwork) {
-  const size_t n = 4 * (size_t)N + 4, nn = n * n, N1 = (size_t)N + 1;
-  char* p = (char*)scratch;
-  auto take = [&](size_t doubles) {
-    double* r = (double*)p;
-    p += ((doubles * sizeof(double) + 63) / 64) * 64;
-    return r;
-  };
-  CertWork w;
-  w.src = take(3 * N); w.dst = take(3 * N); w.theta = take(N); w.thp = take(N1); w.R = take(9); w.q = take(4);
-  w.offA = take(16 * (size_t)N); w.diagB = take(16 * (size_t)N); w.lam = take(16 * (size_t)N);
-  w.mu_terms = take(N); w.top = take(16); w.mu = take(1);
-  w.M_init = take(nn); w.M = take(nn); w.B = take(nn); w.Vs = take(nn); w.M_psd = take(nn); w.W = take(nn);
-  w.Wd = take(nn); w.M_aff = take(nn); w.w = take(n);
-  w.bW = take(3 * N1 * (N1 - 1) / 2); w.D = take(3 * N1); w.diag3 = take(9 * N1);
-  w.work = take((size_t)lwork);
-  w.first_pos = (int*)p;
-  w.info = w.first_pos + 1;
-  w.lwork = lwork;
-  return w;
-}
-
-// getOptimalDualProjection on device buffers (W -> Wd); 5 launches
-static int launch_dual_projection(const CertWork& w, int N, cudaStream_t st) {
-  const int N1 = N + 1;
-  const size_t n = 4 * (size_t)N + 4;
-  cudaMemsetAsync(w.Wd, 0, n * n * sizeof(double), st);
-  dim3 gp(grid1(N1, 128), N);
-  dual_bw_kernel<<<gp, 128, 0, st>>>(w.W, w.thp, N, w.bW);
-  dual_sums_kernel<<<grid1(3 * N1, 128), 128, 0, st>>>(w.bW, w.thp, N, w.D);
-  dual_off_kernel<<<gp, 128, 0, st>>>(w.W, w.thp, w.bW, w.D, N, w.Wd);
-  dual_diag_kernel<<<grid1(N1, 4), 128, 0, st>>>(w.W, w.thp, N, w.Wd, w.diag3);
-  dual_mean_kernel<<<1, 256, 0, st>>>(w.diag3, N, w.Wd);
-  return 5;
-}
-
-// nearest PSD matrix of w.M (linalg.h:84-99): B = sym(M) -> eigenvectors in w.B, ascending eigenvalues in w.w, M_PSD
-// in w.M_psd; 4 kernels and one Dsyevd.  false when the eigensolver call is refused.
-static bool launch_psd_step(Cusolver& cs, cusolverDnHandle_t handle, const CertWork& w, size_t n, cudaStream_t st) {
-  const int ge = grid1((long long)(n * n), 256);
-  sym_kernel<<<ge, 256, 0, st>>>(w.M, (int)n, w.B);
-  if (cs.syevd(handle, CUSOLVER_EIG_MODE_VECTOR, CUBLAS_FILL_MODE_LOWER, (int)n, w.B, (int)n, w.w, w.work, w.lwork,
-               w.info) != CUSOLVER_STATUS_SUCCESS)
-    return false;
-  first_pos_kernel<<<1, 32, 0, st>>>(w.w, (int)n, w.first_pos);
-  scale_pos_kernel<<<ge, 256, 0, st>>>(w.B, w.w, (int)n, w.Vs);
-  dim3 gg((unsigned)((n + kGT - 1) / kGT), (unsigned)((n + kGT - 1) / kGT));
-  psd_gemm_kernel<<<gg, 256, 0, st>>>(w.Vs, w.B, (int)n, w.first_pos, w.M_psd);
-  return true;
-}
 
 // quaternion of R (Eigen::Quaterniond(R).normalize(), :66-69) on the host: 20 flops
 static void quaternion_xyzw(const double* R_cm, double q[4]) {
@@ -907,147 +699,6 @@ static void quaternion_xyzw(const double* R_cm, double q[4]) {
   }
   const double nrm = std::sqrt(x * x + y * y + z * z + ww * ww);
   q[0] = x / nrm; q[1] = y / nrm; q[2] = z / nrm; q[3] = ww / nrm;
-}
-
-// Returns TZR_OK or a negative status; err receives a message.  All pointers host.  mode: 0 full certify,
-// 1 initial matrix only (M_init_out n*n, mu_out), 2 dual projection only (W_in n*n -> Wd_out n*n; theta = N values),
-// 3 nearest-PSD step only (W_in n*n -> Wd_out n*n and the ascending eigenvalues of sym(W_in) in w_out).
-int certify_device(int mode, double noise_bound, double cbar2, double sub_optimality, double max_iterations,
-                   double gamma_tau, const double* R_cm, const double* src, const double* dst, const double* theta,
-                   int N, int* is_optimal, double* best_subopt, int* n_iters, double* traj, int traj_cap,
-                   double* M_init_out, double* mu_out, const double* W_in, double* Wd_out, double* w_out,
-                   void** scratch, size_t* scratch_cap, void** solver_handle, int64_t* launches, cudaStream_t st,
-                   std::string* err) {
-  const size_t n = 4 * (size_t)N + 4, nn = n * n;
-  if (n > 32768) return TZR_ERR_TOO_LARGE;
-  int lwork = 0;
-  Cusolver& cs = cusolver();
-  cusolverDnHandle_t& handle = *reinterpret_cast<cusolverDnHandle_t*>(solver_handle);  // owned by the context
-  if (mode == 0 || mode == 3) {
-    if (!cs.ok) {
-      *err = cs.err;
-      return TZR_ERR_UNSUPPORTED;
-    }
-    if (!handle && cs.create(&handle) != CUSOLVER_STATUS_SUCCESS) {
-      *err = "cusolverDnCreate failed";
-      return TZR_ERR_CUDA;
-    }
-    cs.set_stream(handle, st);
-    if (cs.syevd_buf(handle, CUSOLVER_EIG_MODE_VECTOR, CUBLAS_FILL_MODE_LOWER, (int)n, nullptr, (int)n, nullptr,
-                     &lwork) != CUSOLVER_STATUS_SUCCESS) {
-      *err = "cusolverDnDsyevd_bufferSize failed";
-      return TZR_ERR_CUDA;
-    }
-  }
-  const size_t need = cert_scratch_bytes(N, lwork);
-  if (need > *scratch_cap) {
-    if (*scratch) cudaFree(*scratch);
-    *scratch = nullptr;
-    *scratch_cap = 0;
-    if (cudaMalloc(scratch, need) != cudaSuccess) {
-      *err = "cudaMalloc of the certifier workspace failed";
-      cudaGetLastError();
-      return TZR_ERR_ALLOC;
-    }
-    *scratch_cap = need;
-  }
-  CertWork w = carve(*scratch, N, lwork);
-  if (mode == 3) {
-    int info = 0;
-    cudaMemcpyAsync(w.M, W_in, nn * sizeof(double), cudaMemcpyHostToDevice, st);
-    if (!launch_psd_step(cs, handle, w, n, st)) {
-      *err = "cusolverDnDsyevd failed";
-      return TZR_ERR_CUDA;
-    }
-    *launches += 5;
-    cudaMemcpyAsync(Wd_out, w.M_psd, nn * sizeof(double), cudaMemcpyDeviceToHost, st);
-    cudaMemcpyAsync(w_out, w.w, n * sizeof(double), cudaMemcpyDeviceToHost, st);
-    cudaMemcpyAsync(&info, w.info, sizeof(int), cudaMemcpyDeviceToHost, st);
-    if (cudaStreamSynchronize(st) != cudaSuccess) return TZR_ERR_CUDA;
-    if (info != 0) {
-      *err = "cusolverDnDsyevd reported info " + std::to_string(info);
-      return TZR_ERR_CUDA;
-    }
-    return TZR_OK;
-  }
-  std::vector<double> thp((size_t)N + 1);
-  thp[0] = 1.0;
-  for (int i = 0; i < N; ++i) thp[i + 1] = theta[i];
-  cudaMemcpyAsync(w.thp, thp.data(), (N + 1) * sizeof(double), cudaMemcpyHostToDevice, st);
-  if (mode == 2) {
-    cudaMemcpyAsync(w.W, W_in, nn * sizeof(double), cudaMemcpyHostToDevice, st);
-    *launches += launch_dual_projection(w, N, st);
-    cudaMemcpyAsync(Wd_out, w.Wd, nn * sizeof(double), cudaMemcpyDeviceToHost, st);
-    if (cudaStreamSynchronize(st) != cudaSuccess) return TZR_ERR_CUDA;
-    return TZR_OK;
-  }
-  double q[4];
-  quaternion_xyzw(R_cm, q);
-  cudaMemcpyAsync(w.src, src, 3 * (size_t)N * sizeof(double), cudaMemcpyHostToDevice, st);
-  cudaMemcpyAsync(w.dst, dst, 3 * (size_t)N * sizeof(double), cudaMemcpyHostToDevice, st);
-  cudaMemcpyAsync(w.theta, theta, (size_t)N * sizeof(double), cudaMemcpyHostToDevice, st);
-  cudaMemcpyAsync(w.R, R_cm, 9 * sizeof(double), cudaMemcpyHostToDevice, st);
-  cudaMemcpyAsync(w.q, q, 4 * sizeof(double), cudaMemcpyHostToDevice, st);
-  const double nbs = cbar2 * noise_bound * noise_bound;
-  cert_blocks_kernel<<<grid1(N, 128), 128, 0, st>>>(w.src, w.dst, w.theta, N, w.R, w.q, nbs, w.offA, w.diagB, w.lam,
-                                                    w.mu_terms);
-  cert_reduce_kernel<<<1, 256, 0, st>>>(w.lam, w.mu_terms, N, w.top, w.mu);
-  cert_fill_kernel<<<grid1((long long)nn, 256), 256, 0, st>>>(N, w.offA, w.diagB, w.lam, w.top, w.mu, w.M_init);
-  *launches += 3;
-  double mu = 0;
-  cudaMemcpyAsync(&mu, w.mu, sizeof(double), cudaMemcpyDeviceToHost, st);
-  if (mode == 1) {
-    cudaMemcpyAsync(M_init_out, w.M_init, nn * sizeof(double), cudaMemcpyDeviceToHost, st);
-    if (cudaStreamSynchronize(st) != cudaSuccess) return TZR_ERR_CUDA;
-    *mu_out = mu;
-    return TZR_OK;
-  }
-  cudaMemcpyAsync(w.M, w.M_init, nn * sizeof(double), cudaMemcpyDeviceToDevice, st);
-  if (cudaStreamSynchronize(st) != cudaSuccess) return TZR_ERR_CUDA;
-  const int ge = grid1((long long)nn, 256);
-  double best = INFINITY;
-  int iters = 0;
-  std::vector<double> wh(n);
-  for (size_t iter = 0; (double)iter < max_iterations; ++iter) {
-    if (!launch_psd_step(cs, handle, w, n, st)) {
-      *err = "cusolverDnDsyevd failed";
-      return TZR_ERR_CUDA;
-    }
-    affine_in_kernel<<<ge, 256, 0, st>>>(w.M_psd, w.M, w.M_init, (long long)nn, w.W);
-    *launches += 5 + launch_dual_projection(w, N, st);
-    affine_out_kernel<<<ge, 256, 0, st>>>(w.M_init, w.Wd, (long long)nn, w.M_aff);
-    // sub-optimality gap (:192-231): smallest eigenvalue of sym(M_affine)
-    sym_kernel<<<ge, 256, 0, st>>>(w.M_aff, (int)n, w.B);
-    if (cs.syevd(handle, CUSOLVER_EIG_MODE_NOVECTOR, CUBLAS_FILL_MODE_LOWER, (int)n, w.B, (int)n, w.w, w.work,
-                 lwork, w.info) != CUSOLVER_STATUS_SUCCESS) {
-      *err = "cusolverDnDsyevd (values) failed";
-      return TZR_ERR_CUDA;
-    }
-    *launches += 2;
-    double min_eig = 0;
-    int info = 0;
-    cudaMemcpyAsync(&min_eig, w.w, sizeof(double), cudaMemcpyDeviceToHost, st);  // ascending: w[0] is the minimum
-    cudaMemcpyAsync(&info, w.info, sizeof(int), cudaMemcpyDeviceToHost, st);
-    if (cudaStreamSynchronize(st) != cudaSuccess) {
-      *err = cudaGetErrorString(cudaGetLastError());
-      return TZR_ERR_CUDA;
-    }
-    double gap;
-    if (info != 0) gap = INFINITY;  // "Failed to find the minimal eigenvalue" (:221-225)
-    else if (min_eig > 0) gap = 0;
-    else gap = (-min_eig * (N + 1)) / mu;
-    if ((int)iter < traj_cap && traj) traj[iter] = gap;
-    iters = (int)iter + 1;
-    if (gap < best) best = gap;
-    if (gap < sub_optimality) break;
-    update_kernel<<<ge, 256, 0, st>>>(w.M, w.M_aff, w.M_psd, (long long)nn, gamma_tau);
-    *launches += 1;
-  }
-  *is_optimal = best < sub_optimality ? 1 : 0;
-  *best_subopt = best;
-  *n_iters = iters;
-  if (cudaStreamSynchronize(st) != cudaSuccess) return TZR_ERR_CUDA;
-  return TZR_OK;
 }
 
 // ---- tzr_certify_batch ---------------------------------------------------------------------------------------------
@@ -1099,14 +750,17 @@ size_t cbt_carve(void* base, int G, long long K, long long P, int nmax, int T, s
 }
 }  // namespace
 
-int certify_batch_device(int mode, const tzr_certifier_params& prm, int B, const int32_t* N, const double* R_cm,
+int certify_batch_device(CertMode mode, const tzr_certifier_params& prm, int B, const int32_t* N, const double* R_cm,
                          const double* const* src, const double* const* dst, const double* const* theta,
                          const CertGatherProb* gather, int32_t* gathered,
                          tzr_certification_result* results, double* const* traj, const int32_t* traj_cap,
-                         const double* const* X_in, double* const* X_out, bool loop_eig, void** scratch,
-                         size_t* scratch_cap, void** solver_handle, int64_t* launches, cudaStream_t st,
-                         std::string* err) {
-  const bool dev_in = mode == 0 && gather;  // measurements gathered on the device from a retained solve
+                         const double* const* X_in, double* const* X_out, double* const* w_out, double* mu_out,
+                         bool loop_eig, void** scratch, size_t* scratch_cap, void** solver_handle, int64_t* launches,
+                         cudaStream_t st, std::string* err) {
+  const bool certify = mode == CertMode::kCertify;
+  const bool dev_in = certify && gather;  // measurements gathered on the device from a retained solve
+  const bool eigen = certify || mode == CertMode::kPsd;  // the modes that run the eigensolver
+  const bool setup = certify || mode == CertMode::kSetup;  // the modes that build M_init
   int nmax_all = 0;
   for (int b = 0; b < B; ++b) {
     if (4 * (size_t)N[b] + 4 > 32768) {
@@ -1115,23 +769,28 @@ int certify_batch_device(int mode, const tzr_certifier_params& prm, int B, const
     }
     nmax_all = std::max(nmax_all, 4 * N[b] + 4);
   }
-  Cusolver& cs = cusolver();
-  if (!cs.ok) {
-    *err = cs.err;
-    return TZR_ERR_UNSUPPORTED;
-  }
+  // cuSOLVER is loaded, and the handle created, only where the eigensolver runs: the setup and dual-projection modes
+  // work without the library
+  Cusolver* cs = nullptr;
   cusolverDnHandle_t& handle = *reinterpret_cast<cusolverDnHandle_t*>(solver_handle);  // owned by the context
-  if (!handle && cs.create(&handle) != CUSOLVER_STATUS_SUCCESS) {
-    *err = "cusolverDnCreate failed";
-    return TZR_ERR_CUDA;
+  if (eigen) {
+    cs = &cusolver();
+    if (!cs->ok) {
+      *err = cs->err;
+      return TZR_ERR_UNSUPPORTED;
+    }
+    if (!handle && cs->create(&handle) != CUSOLVER_STATUS_SUCCESS) {
+      *err = "cusolverDnCreate failed";
+      return TZR_ERR_CUDA;
+    }
+    cs->set_stream(handle, st);
   }
-  cs.set_stream(handle, st);
   cusolverDnParams_t sp = nullptr;
-  bool batched = !loop_eig && cs.batched && B > 1 && cs.create_params(&sp) == CUSOLVER_STATUS_SUCCESS;
+  bool batched = eigen && !loop_eig && cs->batched && B > 1 && cs->create_params(&sp) == CUSOLVER_STATUS_SUCCESS;
   struct ParamsGuard {
-    Cusolver& cs;
+    Cusolver* cs;
     cusolverDnParams_t& p;
-    ~ParamsGuard() { if (p) cs.destroy_params(p); }
+    ~ParamsGuard() { if (p) cs->destroy_params(p); }
   } guard{cs, sp};
   // eigensolver workspace of `G` problems padded to `nmax`: (device bytes, host bytes); {0, 0} when the batched call
   // refuses the size
@@ -1139,8 +798,8 @@ int certify_batch_device(int mode, const tzr_certifier_params& prm, int B, const
     size_t dmax = 0, hmax = 0;
     for (cusolverEigMode_t jobz : {CUSOLVER_EIG_MODE_VECTOR, CUSOLVER_EIG_MODE_NOVECTOR}) {
       size_t dv = 0, hv = 0;
-      if (cs.syev_batched_buf(handle, sp, jobz, CUBLAS_FILL_MODE_LOWER, nmax, CUDA_R_64F, nullptr, nmax, CUDA_R_64F,
-                              nullptr, CUDA_R_64F, &dv, &hv, G) != CUSOLVER_STATUS_SUCCESS)
+      if (cs->syev_batched_buf(handle, sp, jobz, CUBLAS_FILL_MODE_LOWER, nmax, CUDA_R_64F, nullptr, nmax, CUDA_R_64F,
+                               nullptr, CUDA_R_64F, &dv, &hv, G) != CUSOLVER_STATUS_SUCCESS)
         return 0;
       dmax = std::max(dmax, dv);
       hmax = std::max(hmax, hv);
@@ -1148,15 +807,16 @@ int certify_batch_device(int mode, const tzr_certifier_params& prm, int B, const
     *host = hmax;
     return std::max<size_t>(dmax, 1);
   };
+  // Dsyevd workspace bytes at `nmax`: 0 when the query fails, and in the modes without an eigensolver
   auto syevd_ws = [&](int nmax) -> size_t {
     int lwork = 0;
-    if (cs.syevd_buf(handle, CUSOLVER_EIG_MODE_VECTOR, CUBLAS_FILL_MODE_LOWER, nmax, nullptr, nmax, nullptr, &lwork) !=
-        CUSOLVER_STATUS_SUCCESS)
+    if (!eigen || cs->syevd_buf(handle, CUSOLVER_EIG_MODE_VECTOR, CUBLAS_FILL_MODE_LOWER, nmax, nullptr, nmax, nullptr,
+                                &lwork) != CUSOLVER_STATUS_SUCCESS)
       return 0;
     return (size_t)lwork * sizeof(double);
   };
   const size_t loop_ws_all = syevd_ws(nmax_all);
-  if (!loop_ws_all) {
+  if (eigen && !loop_ws_all) {
     *err = "cusolverDnDsyevd_bufferSize failed";
     return TZR_ERR_CUDA;
   }
@@ -1244,12 +904,12 @@ int certify_batch_device(int mode, const tzr_certifier_params& prm, int B, const
       t.p_off = g ? tab[g - 1].p_off + (long long)tab[g - 1].N * (tab[g - 1].N + 1) / 2 : 0;
       t.active = 1; t.iters = 0; t.first_pos = 0; t.pad_bits = 0; t.mu = 0; t.best = INFINITY;
       t.nbs = dev_in ? gather[b].nbs : nbs;
-      if (mode == 1) {  // the PSD building block starts from X_in[b]: its pad follows that matrix
+      if (mode == CertMode::kPsd) {  // the PSD building block starts from X_in[b]: its pad follows that matrix
         double m = 0;
         for (size_t e = 0; e < (size_t)t.n * t.n; ++e) m = std::max(m, std::fabs(X_in[b][e]));
         std::memcpy(&t.pad_bits, &m, sizeof m);
       }
-      if (mode == 0) {
+      if (setup) {
         if (dev_in) {
           h_gt[g] = gather[b];
           h_gt[g].k_off = t.k_off;
@@ -1264,7 +924,7 @@ int certify_batch_device(int mode, const tzr_certifier_params& prm, int B, const
       }
       if (!dev_in) {
         h_thp[k + g] = 1.0;
-        if (mode != 1) std::copy(theta[b], theta[b] + Nb, h_thp.begin() + k + g + 1);
+        if (mode != CertMode::kPsd) std::copy(theta[b], theta[b] + Nb, h_thp.begin() + k + g + 1);
       }
       maxN = std::max(maxN, Nb);
       k += Nb;
@@ -1285,13 +945,13 @@ int certify_batch_device(int mode, const tzr_certifier_params& prm, int B, const
     }
     const long long nn = (long long)nmax * nmax;
     const dim3 ge(grid1(nn, 256), G), gp(grid1(maxN + 1, 128), maxN, G), gt((nmax + kPT - 1) / kPT, (nmax + kPT - 1) / kPT, G);
-    if (mode == 0) {
+    if (setup) {
       cbt_blocks_kernel<<<dim3(grid1(maxN, 128), G), 128, 0, st>>>(w.pr, w.src, w.dst, w.theta, w.R, w.q, w.offA,
                                                                     w.diagB, w.lam, w.mu_terms);
       cbt_reduce_kernel<<<G, 256, 0, st>>>(w.pr, w.lam, w.mu_terms, w.top);
       cbt_fill_kernel<<<ge, 256, 0, st>>>(w.pr, nmax, w.offA, w.diagB, w.lam, w.top, w.M_init);
       *launches += 3;
-      cudaMemcpyAsync(w.M, w.M_init, (size_t)G * nn * sizeof(double), cudaMemcpyDeviceToDevice, st);
+      if (certify) cudaMemcpyAsync(w.M, w.M_init, (size_t)G * nn * sizeof(double), cudaMemcpyDeviceToDevice, st);
     }
     std::vector<int> act(G, 1), idx;  // active flags of the last read-back; their indices (compact batch)
     if (dev_in) {  // the gather's flags: a problem with a non-finite measurement starts (and stays) inactive
@@ -1327,9 +987,9 @@ int certify_batch_device(int mode, const tzr_certifier_params& prm, int B, const
           const bool all = n_act == G;
           const dim3 gc(grid1(nn, 256), n_act);
           if (!all) cbt_gather_kernel<<<gc, 256, 0, st>>>(w.idx, nmax, w.Bm, w.W);
-          if (cs.syev_batched(handle, sp, jobz, CUBLAS_FILL_MODE_LOWER, nmax, CUDA_R_64F, all ? w.Bm : w.W, nmax,
-                              CUDA_R_64F, all ? w.w : w.wc, CUDA_R_64F, w.work, dws_a, host_work.data(), hws_a,
-                              all ? w.info : w.infoc, n_act) == CUSOLVER_STATUS_SUCCESS) {
+          if (cs->syev_batched(handle, sp, jobz, CUBLAS_FILL_MODE_LOWER, nmax, CUDA_R_64F, all ? w.Bm : w.W, nmax,
+                               CUDA_R_64F, all ? w.w : w.wc, CUDA_R_64F, w.work, dws_a, host_work.data(), hws_a,
+                               all ? w.info : w.infoc, n_act) == CUSOLVER_STATUS_SUCCESS) {
             if (!all)
               cbt_scatter_kernel<<<gc, 256, 0, st>>>(w.idx, nmax, jobz == CUSOLVER_EIG_MODE_VECTOR ? 1 : 0, w.W, w.wc,
                                                      w.infoc, w.Bm, w.w, w.info);
@@ -1342,9 +1002,9 @@ int certify_batch_device(int mode, const tzr_certifier_params& prm, int B, const
       }
       for (int g = 0; g < G; ++g) {
         if (!act[g]) continue;
-        if (cs.syevd(handle, jobz, CUBLAS_FILL_MODE_LOWER, tab[g].n, w.Bm + (size_t)g * nn, nmax,
-                     w.w + (size_t)g * nmax, (double*)w.work, (int)(lwork_bytes / sizeof(double)),
-                     w.info + g) != CUSOLVER_STATUS_SUCCESS) {
+        if (cs->syevd(handle, jobz, CUBLAS_FILL_MODE_LOWER, tab[g].n, w.Bm + (size_t)g * nn, nmax,
+                      w.w + (size_t)g * nmax, (double*)w.work, (int)(lwork_bytes / sizeof(double)),
+                      w.info + g) != CUSOLVER_STATUS_SUCCESS) {
           *err = "cusolverDnDsyevd failed";
           return TZR_ERR_CUDA;
         }
@@ -1352,23 +1012,24 @@ int certify_batch_device(int mode, const tzr_certifier_params& prm, int B, const
       }
       return TZR_OK;
     };
-    if (mode != 0) {
+    if (!certify) {
       // one building block on the group, in the layout and on the eigen route of the iteration below: each problem's
-      // n x n input into the real block of M (mode 1) or W (mode 2), the real block of M_psd or Wd back
-      double* in = mode == 1 ? w.M : w.W;
-      const double* out = mode == 1 ? w.M_psd : w.Wd;
+      // n x n input into the real block of M (PSD) or W (dual); the real block of M_init (setup), M_psd or Wd back
       const size_t ld = (size_t)nmax * sizeof(double);
-      for (int g = 0; g < G; ++g) {
-        const size_t nb = (size_t)tab[g].n * sizeof(double);
-        cudaMemcpy2DAsync(in + (size_t)g * nn, ld, X_in[b0 + g], nb, nb, tab[g].n, cudaMemcpyHostToDevice, st);
+      if (mode != CertMode::kSetup) {
+        double* in = mode == CertMode::kPsd ? w.M : w.W;
+        for (int g = 0; g < G; ++g) {
+          const size_t nb = (size_t)tab[g].n * sizeof(double);
+          cudaMemcpy2DAsync(in + (size_t)g * nn, ld, X_in[b0 + g], nb, nb, tab[g].n, cudaMemcpyHostToDevice, st);
+        }
       }
-      if (mode == 1) {
+      if (mode == CertMode::kPsd) {
         cbt_sym_kernel<<<ge, 256, 0, st>>>(w.pr, nmax, w.M, w.Bm);
         if (int rc = eig(CUSOLVER_EIG_MODE_VECTOR)) return rc;
         cbt_first_pos_kernel<<<grid1(G, 128), 128, 0, st>>>(w.pr, G, nmax, full_step ? 1 : 0, w.w);
         cbt_psd_kernel<<<gt, 256, 0, st>>>(w.pr, nmax, full_step ? 1 : 0, w.Bm, w.w, w.M_psd);
         *launches += 3;
-      } else {
+      } else if (mode == CertMode::kDual) {
         cbt_dual_bw_kernel<<<gp, 128, 0, st>>>(w.pr, nmax, w.W, w.thp, w.bW);
         cbt_dual_sums_kernel<<<dim3(grid1(3 * (maxN + 1), 128), G), 128, 0, st>>>(w.pr, w.bW, w.thp, w.D);
         cbt_dual_off_kernel<<<gp, 128, 0, st>>>(w.pr, nmax, w.W, w.thp, w.bW, w.D, w.Wd);
@@ -1376,21 +1037,28 @@ int certify_batch_device(int mode, const tzr_certifier_params& prm, int B, const
         cbt_dual_mean_kernel<<<G, 256, 0, st>>>(w.pr, nmax, w.diag3, w.Wd);
         *launches += 5;
       }
+      const double* out = mode == CertMode::kSetup ? w.M_init : mode == CertMode::kPsd ? w.M_psd : w.Wd;
       for (int g = 0; g < G; ++g) {
         const size_t nb = (size_t)tab[g].n * sizeof(double);
         cudaMemcpy2DAsync(X_out[b0 + g], nb, out + (size_t)g * nn, ld, nb, tab[g].n, cudaMemcpyDeviceToHost, st);
+        if (w_out && w_out[b0 + g])
+          cudaMemcpyAsync(w_out[b0 + g], w.w + (size_t)g * nmax, nb, cudaMemcpyDeviceToHost, st);
       }
       std::vector<int> info(G, 0);
-      if (mode == 1) cudaMemcpyAsync(info.data(), w.info, G * sizeof(int), cudaMemcpyDeviceToHost, st);
+      if (mode == CertMode::kPsd) cudaMemcpyAsync(info.data(), w.info, G * sizeof(int), cudaMemcpyDeviceToHost, st);
+      if (mode == CertMode::kSetup)
+        cudaMemcpyAsync(tab.data(), w.pr, G * sizeof(CertBatchProb), cudaMemcpyDeviceToHost, st);
       if (cudaStreamSynchronize(st) != cudaSuccess) {
         *err = cudaGetErrorString(cudaGetLastError());
         return TZR_ERR_CUDA;
       }
-      for (int g = 0; g < G; ++g)
+      for (int g = 0; g < G; ++g) {
         if (info[g] != 0) {
           *err = "problem " + std::to_string(b0 + g) + ": the eigensolver reported info " + std::to_string(info[g]);
           return TZR_ERR_CUDA;
         }
+        if (mode == CertMode::kSetup) mu_out[b0 + g] = tab[g].mu;
+      }
       b0 = b1;
       continue;
     }

@@ -336,14 +336,7 @@ void launch_fpfh_pair_features(int n, const float* p1, const float* n1, const fl
                                int32_t* ok, cudaStream_t st);
 void launch_fpfh_smallest_eigenpair(int n, const float* cov, float* ev, float* vec, cudaStream_t st);
 
-// certify.cu (DRSCertifier::certify, certification.cc:40-190); mode 0 certify, 1 initial matrix, 2 dual projection,
-// 3 nearest-PSD step (W_in -> Wd_out, eigenvalues in w_out)
-int certify_device(int mode, double noise_bound, double cbar2, double sub_optimality, double max_iterations,
-                   double gamma_tau, const double* R_cm, const double* src, const double* dst, const double* theta,
-                   int N, int* is_optimal, double* best_subopt, int* n_iters, double* traj, int traj_cap,
-                   double* M_init_out, double* mu_out, const double* W_in, double* Wd_out, double* w_out,
-                   void** scratch, size_t* scratch_cap, void** solver_handle, int64_t* launches, cudaStream_t st,
-                   std::string* err);
+// certify.cu (DRSCertifier::certify, certification.cc:40-190)
 // Device input of one certify_batch_device problem (tzr_certify_last_solve): its measurements are built on the device
 // from a retained solve, exactly as the rotation stage built the TIMs it solved on (rot_trans.cu).
 struct CertGatherProb {
@@ -358,19 +351,24 @@ struct CertGatherProb {
   int k_off, v_off;      // set by certify_batch_device: first measurement and first block row inside the group
 };
 
+// What certify_batch_device runs: the whole certifier, or one of its building blocks on X_in[b] / into X_out[b]
+// (n x n each): the initial matrix (M_init into X_out, mu into mu_out), one nearest-PSD step or one dual projection.
+enum class CertMode { kCertify, kSetup, kPsd, kDual };
 // B problems (host pointers, validated by the caller) in device-sized groups of one launch sequence each; loop_eig: one
-// cusolverDnDsyevd per active problem instead of cusolverDnXsyevBatched (debug flag 2097152).  mode 0 certify; the
-// building blocks run one step of the batch's iteration on X_in[b] (n x n) into X_out[b]: 1 nearest-PSD step, 2 dual
-// projection (theta as for mode 0; src, dst, R_cm, results and traj unused).  gather (mode 0, may be NULL): B device
-// inputs that replace src, dst, theta and the scalar noise bound; gathered[b] then receives 1, or 0 where the gathered
-// measurements hold a non-finite value (the problem never reaches the eigensolver; result {0, 0, +inf}).
-int certify_batch_device(int mode, const tzr_certifier_params& prm, int B, const int32_t* N, const double* R_cm,
+// cusolverDnDsyevd per active problem instead of cusolverDnXsyevBatched (debug flag 2097152).  src, dst, R_cm and
+// results / traj (trajectories may be NULL) serve kCertify and kSetup; theta serves those and kDual.  gather (kCertify,
+// may be NULL): B device inputs that replace src, dst, theta and the scalar noise bound; gathered[b] then receives 1, or
+// 0 where the gathered measurements hold a non-finite value (the problem never reaches the eigensolver; result {0, 0,
+// +inf}).  w_out (kPsd, may be NULL, as may its entries): the n ascending eigenvalues of each problem's symmetrised real
+// block; they are defined only where the step takes cusolverDnDsyevd on that block, which a call with B = 1 always
+// does.  cuSOLVER is loaded only in kCertify and kPsd; without it those return TZR_ERR_UNSUPPORTED.
+int certify_batch_device(CertMode mode, const tzr_certifier_params& prm, int B, const int32_t* N, const double* R_cm,
                          const double* const* src, const double* const* dst, const double* const* theta,
                          const CertGatherProb* gather, int32_t* gathered,
                          tzr_certification_result* results, double* const* traj, const int32_t* traj_cap,
-                         const double* const* X_in, double* const* X_out, bool loop_eig, void** scratch,
-                         size_t* scratch_cap, void** solver_handle, int64_t* launches, cudaStream_t st,
-                         std::string* err);
+                         const double* const* X_in, double* const* X_out, double* const* w_out, double* mu_out,
+                         bool loop_eig, void** scratch, size_t* scratch_cap, void** solver_handle, int64_t* launches,
+                         cudaStream_t st, std::string* err);
 void certify_release(void* solver_handle);
 
 // matcher.cu (Matcher::calculateCorrespondences, matcher.cc:21-337), over B cloud pairs stored back to back

@@ -92,6 +92,26 @@ def test_bool_theta_and_iteration_cap(ctx):
     assert np.abs(r3["suboptimality_traj"] - c["suboptimality_traj"][:3]).max() < TOL
 
 
+def test_single_entry_launch_counts(ctx):
+    """tzr_certify with k iterations (sub_optimality < 0: it never stops early) launches 16k + 2: the setup's 3
+    kernels, per iteration 13 kernels and 2 cusolverDnDsyevd calls, and an update after every iteration but the last.
+    The building blocks: initial matrix 3, nearest-PSD step 4 (one of them Dsyevd), dual projection 5."""
+    c = SMALL[0]
+    args = (c["R_est"], c["v1"], c["v2"], c["theta_est"])
+    kw = dict(noise_bound=c["params"]["noise_bound"], cbar2=c["params"]["cbar2"])
+
+    def launches(fn):
+        before = ctx.kernel_launches()
+        fn()
+        return ctx.kernel_launches() - before
+
+    for k in (1, 2, 5):
+        assert launches(lambda: ctx.certify(*args, max_iterations=k, sub_optimality=-1.0, **kw)) == 16 * k + 2
+    assert launches(lambda: ctx.certifier_initial_matrix(*args, **kw)) == 3
+    assert launches(lambda: ctx.certifier_psd_projection(c["W_1st_iter"])) == 4
+    assert launches(lambda: ctx.certifier_dual_projection(c["W_1st_iter"], c["theta_est"])) == 5
+
+
 def test_solve_then_certify_end_to_end(ctx):
     """solve() -> DRSCertifier on the clique's chain TIMs with the rotation inlier mask, the way the reference's
     certification example chains them."""

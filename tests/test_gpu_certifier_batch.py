@@ -102,14 +102,16 @@ def test_mixed_random_batch_matches_oracle_and_single_call(ctx, flags):
 
 
 def test_single_problem_batch_equals_certify(ctx):
-    for c in FIXTURES[:4]:
-        kw = dict(noise_bound=c["params"]["noise_bound"], cbar2=1.0)
-        args = (c["R_est"], c["v1"], c["v2"], c["theta_est"])
+    """tzr_certify is tzr_certify_batch with B = 1: the same results, bit for bit."""
+    cases = [((c["R_est"], c["v1"], c["v2"], c["theta_est"]), dict(noise_bound=c["params"]["noise_bound"], cbar2=1.0))
+             for c in FIXTURES[:4]]
+    cases += [(p, dict(noise_bound=0.01, cbar2=1.0, max_iterations=25)) for p in _mixed_problems()]
+    for args, kw in cases:
         (r,) = ctx.certify_batch(*[[a] for a in args], **kw)
         one = ctx.certify(*args, **kw)
         assert r["is_optimal"] == one["is_optimal"]
-        assert _close(r["suboptimality_traj"], one["suboptimality_traj"], TOL)
-        assert abs(r["best_suboptimality"] - one["best_suboptimality"]) < TOL
+        assert np.array_equal(r["suboptimality_traj"], one["suboptimality_traj"])
+        assert r["best_suboptimality"] == one["best_suboptimality"]
 
 
 def test_eigen_routes_agree(ctx):

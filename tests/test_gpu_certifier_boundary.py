@@ -1,11 +1,12 @@
 """GPU tests of the certifier's building blocks where they can be wrong (`pytest -m gpu`, DESIGN.md 3.9).
 
-* The nearest-PSD step, single call (psd_gemm_kernel over Dsyevd) and batch (cbt_psd_kernel, DMMA, over the batch's
-  padded layout and eigen route), against matrices whose spectrum and positive part are exact in FP64
+* The nearest-PSD step, single call (the batch with B = 1: cbt_psd_kernel over cusolverDnDsyevd on the real block,
+  bit for bit the batch entry with one matrix) and batch (cbt_psd_kernel, DMMA, over the batch's padded layout and
+  eigen route), against matrices whose spectrum and positive part are exact in FP64
   (tests/certifier_reference.py): the first positive eigenvalue at 0, at n - 1 and either side of the 16-deep k slabs,
   n at and just past the 64-wide tiles, exact zeros, repeated and widely spread eigenvalues, and the batch at scales
   2^-40 .. 2^40, where an identity pad of fixed size would be far from the real block's scale.
-* The dual projection, single and batch, at the N where its reductions change shape (a warp over N + 1 block rows,
+* The dual projection, single (bit for bit the batch entry with one problem) and batch, at the N where its reductions change shape (a warp over N + 1 block rows,
   256-thread CTAs, 128-wide pair blocks), against oracle/certifier_oracle.py.
 * The whole certifier, single and batch, on inputs scaled by 2^k: the problem is homogeneous, so the trajectory must not
   change.
@@ -62,6 +63,7 @@ CASES = cr.psd_cases()
 def test_psd_single_against_exact(ctx, n, kind):
     M, P, lam, _ = _exact(n, kind)
     got, w = ctx.certifier_psd_projection(M)
+    assert np.array_equal(got, ctx.certifier_batch_psd_projection([M])[0])
     _check_psd(got, M, P, kind, single=True)
     if kind == "all_positive":
         assert np.linalg.norm(got - M) <= cr.psd_bound(M)
@@ -76,6 +78,7 @@ def test_psd_single_asymmetric_input(ctx, n):
     A = M + (K - K.T)
     assert np.array_equal((A + A.T) / 2, M)
     got, w = ctx.certifier_psd_projection(A)
+    assert np.array_equal(got, ctx.certifier_batch_psd_projection([A])[0])
     _check_psd(got, M, P, "", single=True)
     assert np.abs(w - lam).max() <= cr.eig_bound(lam)
 
@@ -171,6 +174,7 @@ def test_dual_projection_single(ctx, N, tk):
     W = _W(N, N)
     th = _theta(N, tk, N + 1)
     got = ctx.certifier_dual_projection(W, th)
+    assert np.array_equal(got, ctx.certifier_batch_dual_projection([W], [th])[0])
     want = _oracle_dual(W, th)
     assert np.abs(got - want).max() <= cr.dual_bound(W, N)
     if N <= 40:
