@@ -854,9 +854,22 @@ int tzr_solve_batch_multi(const int32_t* devices, int n_devices, const tzr_param
  * searches every target by brute force, bit 26 (67108864) = through the hashed grid at any target size (a target the
  * grid cannot index still falls back to brute force), so that the two routes can be compared on one input; bit 25 wins
  * when both are set, bit 27 (134217728) = the default graph kernel's Gram test in its two-slope form on the unscaled float
- * copies instead of the single-slope form in units of 2 beta (DESIGN.md 3.1; bit-identical; a same-build A/B switch).
- * Bits 15 to 26 change host code only; bit 27 changes device code. */
+ * copies instead of the single-slope form in units of 2 beta (DESIGN.md 3.1; bit-identical; a same-build A/B switch),
+ * bits 28 to 31 = a 4-bit field L: 0 lets the default graph kernel choose its strip length from the batch and the SM
+ * count (4 or 6 blocks of 128 columns), L = 1 ... 15 forces strips of L blocks in every instance of that kernel
+ * (production, verifying, separate degree pass, ragged size class, two-slope form; bit-identical), so that tests reach
+ * every strip length whatever the batch and the device; the opt-in kernels of bits 3 to 7, 10 and 11 ignore it.
+ * Bits 15 to 26 and 28 to 31 change host code only; bit 27 changes device code. */
 int tzr_ctx_set_flags(tzr_ctx* ctx, uint32_t flags);
+/* Strip length (blocks of 128 columns) of the default graph kernel's most recent launch on this context (the last size
+ * class or sub-chunk of a batch); 0 before any graph build, or when that build ran another kernel (debug bits 3 to 7
+ * and 11). */
+int tzr_ctx_last_strip_blocks(const tzr_ctx* ctx);
+/* The default graph kernel's strip order over nt row blocks of 128 points, as the device decodes it, for strips of L
+ * blocks: I[p] (row block) and J0[p] (first column block) of strip p = 0 ... count - 1, strips numbered from row block 0
+ * down, each row block's strips left to right.  Host-only, needs no device; I and J0 may be NULL.  Returns the count,
+ * or TZR_ERR_INVALID_ARG unless 1 <= nt <= 512 and 1 <= L <= 15. */
+int tzr_graph_strip_schedule(int nt, int L, int32_t* I, int32_t* J0);
 int64_t tzr_ctx_filter_mismatches(tzr_ctx* ctx);
 /* Number of pairs of the most recent graph build that needed the exact FP64 re-check. */
 int64_t tzr_ctx_filter_rechecks(tzr_ctx* ctx);

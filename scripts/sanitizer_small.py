@@ -94,6 +94,23 @@ for rflags, est in ((16777216, 0), (16777216 | 2, 0), (16777216, 1)):
                                capi.default_params(noise_bound=rg[0]["noise_bound"], estimate_scaling=est))
     print("ragged flags", rflags, "scale", est, [int(c) for c in sols["clique_size"]])
 ctx.set_flags(0)
+# the default graph kernel's long strips (forced through debug flag bits 28-31; the automatic choice needs batches of
+# thousands): 5, 6 and 8 blocks refill every slot of the column ring, 8 fills one a third time.  A uniform batch at
+# n = 1100 (9 row blocks), under the production, verifying, two-slope and 64-entry-queue instances, then the ragged class
+# above, whose problems end inside and before whole strips
+lg = [synth.config_problem("C2", 70 + b, n=1100) for b in range(3)]
+ls, ld = np.ascontiguousarray(np.stack([q["src"] for q in lg])), np.ascontiguousarray(np.stack([q["dst"] for q in lg]))
+for L in (5, 6, 8):
+    for sflags in (0, 2 | 4, 134217728, 16384 | 4):
+        ctx.set_flags(sflags | capi.strip_flags(L))
+        sols, cl = ctx.solve_batch_array(ls, ld, capi.default_params(**dict(kw, noise_bound=lg[0]["noise_bound"])))
+        print("strips", L, "flags", sflags, ctx.last_strip_blocks(), [int(s) for s in sols["n_edges"]])
+    for rflags in (16777216, 16777216 | 134217728 | 16384):
+        ctx.set_flags(rflags | capi.strip_flags(L))
+        sols, cl = ctx.solve_batch([q["src"] for q in rg], [q["dst"] for q in rg],
+                                   capi.default_params(noise_bound=rg[0]["noise_bound"], estimate_scaling=0))
+        print("ragged strips", L, "flags", rflags, ctx.last_strip_blocks(), [int(c) for c in sols["clique_size"]])
+ctx.set_flags(0)
 if "--no-cert" not in sys.argv:  # solve then certify its retained results: the gather kernel on CHAIN and COMPLETE TIMs
     for tim in (0, 1):
         sc = [synth.make_problem(n, 0.5, 60 + n, "ball") for n in (40, 30, 36)]

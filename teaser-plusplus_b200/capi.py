@@ -149,13 +149,35 @@ _SYMBOLS = [
     "tzr_estimate_normals_batch", "tzr_icp_point_to_plane", "tzr_icp_point_to_plane_batch",
     "tzr_register_cloud_pairs_icp_point_to_plane", "tzr_icp_generalized", "tzr_icp_generalized_batch",
     "tzr_register_cloud_pairs_icp_generalized", "tzr_icp_point_to_plane_robust_batch", "tzr_icp_generalized_robust_batch",
-    "tzr_register_cloud_pairs_icp_robust",
+    "tzr_register_cloud_pairs_icp_robust", "tzr_ctx_last_strip_blocks", "tzr_graph_strip_schedule",
 ]
 
 # status codes (tzr_status)
 TZR_OK = 0
 TZR_ERR_INVALID_ARG = -1
 TZR_ERR_TOO_LARGE = -6
+
+# debug flag bits 28-31 of tzr_ctx_set_flags: the default graph kernel's strip length (0: chosen from the batch)
+FLAG_STRIP_SHIFT = 28
+
+
+def strip_flags(L: int) -> int:
+    """The debug flag bits that force strips of L = 1 ... 15 blocks in the default graph kernel (0: its own choice)."""
+    if not 0 <= L <= 15:
+        raise ValueError(f"strip length {L} outside 0 ... 15")
+    return L << FLAG_STRIP_SHIFT
+
+
+def strip_schedule(nt: int, L: int):
+    """tzr_graph_strip_schedule: (I, J0) int32 arrays of the default graph kernel's strips over nt row blocks, strips of
+    L blocks, in the device's order (host only)."""
+    count = lib().tzr_graph_strip_schedule(nt, L, None, None)
+    if count < 0:
+        raise TzrError(f"tzr_graph_strip_schedule({nt}, {L}): {lib().tzr_status_string(count).decode()}")
+    I, J0 = np.zeros(count, dtype=np.int32), np.zeros(count, dtype=np.int32)
+    lib().tzr_graph_strip_schedule(nt, L, _p(I, C.c_int32), _p(J0, C.c_int32))
+    return I, J0
+
 
 # debug flags of tzr_ctx_set_flags that choose tzr_compute_fpfh(_batch)'s radius search for every cloud
 FLAG_FPFH_BRUTE_FORCE = 4194304
@@ -224,6 +246,8 @@ def lib():
     L.tzr_ctx_filter_rechecks.argtypes = [vp]
     L.tzr_ctx_filter_rechecks.restype = C.c_int64
     L.tzr_ctx_debug_counters.argtypes = [vp, i64p]
+    L.tzr_ctx_last_strip_blocks.argtypes = [vp]
+    L.tzr_graph_strip_schedule.argtypes = [C.c_int, C.c_int, i32p, i32p]
     L.tzr_ctx_clique_info.argtypes = [vp, i32p, i32p]
     L.tzr_ctx_set_max_n.argtypes = [vp, C.c_int]
     L.tzr_ctx_clique_route.argtypes = [vp, i32p]
@@ -437,6 +461,10 @@ class Context:
                     root_ns_total=int(out[12]), roots_over_1ms=int(out[13]), block_bound_prunes=int(out[14]),
                     # problems graph_strip2_kernel built with the Gram-form test (the rest: interval test or another kernel)
                     gram_problems=int(out[15]))
+
+    def last_strip_blocks(self) -> int:
+        """Strip length of the default graph kernel's most recent launch (0: none, or another kernel built the graph)."""
+        return int(lib().tzr_ctx_last_strip_blocks(self._h))
 
     def clique_info(self, B: int):
         """Geometry of the most recent max_clique(_batch) call and each problem's root-heuristic clique size."""

@@ -40,6 +40,7 @@ struct tzr_ctx {
   DevBuf icp;
   // tzr_voxel_downsample(_batch): its own workspace, for the same reason
   DevBuf vox;
+  int last_strip_blocks = 0;  // strip length of the most recent graph kernel launch (tzr_ctx_last_strip_blocks)
   int max_n = kMaxN;  // per-problem size limit of this context (tzr_ctx_set_max_n: kMaxN ... kMaxNLarge)
   // pinned host staging
   void* h_pin = nullptr;
@@ -669,7 +670,7 @@ int run_pipeline(tzr_ctx* ctx, Batch& bt, const tzr_params& p, cudaEvent_t* ev, 
         ctx->graph_ev.push_back(e);
       }
       cudaEventRecord(ctx->graph_ev[ctx->graph_ev_used], sg);
-      nl += launch_graph(sb, sg, ctx->num_sms) - 1;
+      nl += launch_graph(sb, sg, ctx->num_sms, &ctx->last_strip_blocks) - 1;
       cudaEventRecord(ctx->graph_ev[ctx->graph_ev_used + 1], sg);
       ctx->graph_ev_used += 2;
       if (sg != st) {  // two lanes (never combined with L2 sub-chunking: gch == B there)
@@ -1284,6 +1285,13 @@ int tzr_ctx_debug_counters(tzr_ctx* ctx, int64_t* out16) {
   return TZR_OK;
 }
 
+int tzr_ctx_last_strip_blocks(const tzr_ctx* ctx) { return ctx ? ctx->last_strip_blocks : 0; }
+
+int tzr_graph_strip_schedule(int nt, int L, int32_t* I, int32_t* J0) {
+  if (nt < 1 || nt > kMaxNLarge / kTile || L < 1 || L > 15) return TZR_ERR_INVALID_ARG;
+  return strip_schedule(nt, L, I, J0);
+}
+
 int64_t tzr_ctx_filter_rechecks(tzr_ctx* ctx) {
   if (!ctx || !ctx->dbg.p) return -1;
   unsigned long long v = 0;
@@ -1308,7 +1316,7 @@ int tzr_graph_build(tzr_ctx* ctx, const double* src, const double* dst, int n, d
   CK(cudaMemcpyAsync((void*)bt.dst, dst, (size_t)n * 3 * sizeof(double), cudaMemcpyHostToDevice, st));
   if (ctx->flags & 6u) cudaMemsetAsync((void*)ctx->dbg.p, 0, 16 * sizeof(unsigned long long), st);
   launch_prep(bt, st);
-  ctx->launches += 2 + launch_graph(bt, st, ctx->num_sms);
+  ctx->launches += 2 + launch_graph(bt, st, ctx->num_sms, &ctx->last_strip_blocks);
   launch_degree(bt, st);
   rc = check_launch(ctx, "graph build");
   if (rc) return rc;

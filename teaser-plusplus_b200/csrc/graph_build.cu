@@ -38,6 +38,8 @@ __device__ __forceinline__ double warp_max(double v) {
 
 // debug bit 27: the Gram test's two-slope form on the unscaled copies (sf, df) instead of the single-slope form (gq)
 constexpr uint32_t kFlagTwoSlope = 134217728u;
+// debug bits 28-31: graph_strip2_kernel's strip length, 1 ... 15 blocks (0: chosen from the batch; launch_strip2)
+constexpr int kFlagStripShift = 28;
 
 // launch_graph sends the problems prep_kernel marked use_tc to graph_tc_kernel only under debug flag 1024 without an A/B
 // flag (8-256) or the interval-test flag 512
@@ -1269,11 +1271,13 @@ static int strip_blocks_for(int B, int n, int num_sms) {
 }
 
 // the default strip kernel's instances: ragged size class or uniform batch, verifying (flag 2), separate degree pass
-// (flag 256) or the production template
+// (flag 256) or the production template.  Debug flag bits 28-31 force the strip length (1 ... 15; 0: strip_blocks_for's
+// choice), so that tests reach every length whatever the batch and the SM count.  Returns the strip length launched.
 template <bool kSlope>
-void launch_strip2(Batch bt, const int num_sms, cudaStream_t st) {
+int launch_strip2(Batch bt, const int num_sms, cudaStream_t st) {
   const int nt = (bt.n + kTile - 1) / kTile;
-  bt.strip_blocks = strip_blocks_for(bt.B, bt.n, num_sms);
+  const int forced = (int)(bt.flags_dbg >> kFlagStripShift);
+  bt.strip_blocks = forced ? forced : strip_blocks_for(bt.B, bt.n, num_sms);
   const dim3 sgrid((unsigned)strips_below(nt, bt.strip_blocks), (unsigned)bt.B);
   if (bt.nb) {
     if (bt.flags_dbg & 2u)
@@ -1287,6 +1291,19 @@ void launch_strip2(Batch bt, const int num_sms, cudaStream_t st) {
   } else {  // default: Gram test (interval test where prep_kernel's guard fails), degrees fused
     graph_strip2_kernel<false, TZR_STRIP_MIN_BLOCKS, true, kSlope><<<sgrid, kGraphThreads, 0, st>>>(bt);
   }
+  return bt.strip_blocks;
+}
+
+int strip_schedule(int nt, int L, int32_t* I, int32_t* J0) {
+  if (nt <= 0 || L <= 0) return 0;
+  const int count = strips_below(nt, L);
+  for (int p = 0; p < count; ++p) {
+    int i, j;
+    strip_decode(p, nt, L, &i, &j);
+    if (I) I[p] = i;
+    if (J0) J0[p] = j;
+  }
+  return count;
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -1534,8 +1551,9 @@ __global__ void __launch_bounds__(256) degree_kernel(Batch bt) {
 
 void launch_prep(const Batch& bt, cudaStream_t st) { prep_kernel<<<bt.B, 256, 0, st>>>(bt); }
 
-int launch_graph(const Batch& bt0, cudaStream_t st, int num_sms) {
+int launch_graph(const Batch& bt0, cudaStream_t st, int num_sms, int* strip_blocks) {
   Batch bt = bt0;
+  int L = 0;  // strip length of graph_strip2_kernel, 0 while another kernel builds the graph
   bt.strip_blocks = kStripBlocks;  // (launch_strip2 chooses the default kernel's strip length)
   // default: CUDA-core strip kernel.  Debug flag 1024 routes every problem prep_kernel marked use_tc through the
   // tensor-core kernel instead (bit-identical output: DESIGN.md §3.1); not in ragged size classes
@@ -1550,6 +1568,7 @@ int launch_graph(const Batch& bt0, cudaStream_t st, int num_sms) {
       graph_tile_kernel<true><<<grid, kGraphThreads, 0, st>>>(bt);
     else
       graph_tile_kernel<false><<<grid, kGraphThreads, 0, st>>>(bt);
+    if (strip_blocks) *strip_blocks = 0;
     return launches;
   }
 #endif
@@ -1559,9 +1578,9 @@ int launch_graph(const Batch& bt0, cudaStream_t st, int num_sms) {
   if (bt.nb) {  // ragged size class: the default kernel (or its verify variant) whatever the opt-in flags 1024 and 2048 say
     cudaMemsetAsync(bt.adj, 0, (size_t)bt.B * bt.n * pitch64(bt.n) * sizeof(uint64_t), st);
     if (bt.flags_dbg & kFlagTwoSlope)
-      launch_strip2<false>(bt, num_sms, st);
+      L = launch_strip2<false>(bt, num_sms, st);
     else
-      launch_strip2<true>(bt, num_sms, st);
+      L = launch_strip2<true>(bt, num_sms, st);
   } else if (bt.flags_dbg & 2048u) {  // v7 (one MUFU, sign-bit words, re-check queue): fewer instructions, but FMA-pipe bound
     v7 = true;
     if (bt.flags_dbg & 2u)
@@ -1584,14 +1603,15 @@ int launch_graph(const Batch& bt0, cudaStream_t st, int num_sms) {
   }
 #endif
   else if (bt.flags_dbg & kFlagTwoSlope)
-    launch_strip2<false>(bt, num_sms, st);
+    L = launch_strip2<false>(bt, num_sms, st);
   else
-    launch_strip2<true>(bt, num_sms, st);
+    L = launch_strip2<true>(bt, num_sms, st);
   // exact re-check of the pairs the strip kernel queued (v7, or the Gram test: every problem unless debug flag 512)
   if (v7 || !(bt.flags_dbg & 512u)) {
     launch_graph_patch(bt, st, num_sms);
     ++launches;
   }
+  if (strip_blocks) *strip_blocks = L;
   return launches;
 }
 

@@ -219,7 +219,11 @@ static __device__ __noinline__ bool edge_exact_scale(const double* __restrict__ 
 
 // kernels (defined in the .cu files) -------------------------------------------------------------
 void launch_prep(const Batch& bt, cudaStream_t st);
-int launch_graph(const Batch& bt, cudaStream_t st, int num_sms);  // returns the number of kernels launched
+// returns the number of kernels launched; strip_blocks (may be NULL): graph_strip2_kernel's strip length, 0 if it did not run
+int launch_graph(const Batch& bt, cudaStream_t st, int num_sms, int* strip_blocks = nullptr);
+// graph_strip2_kernel's strip order on the host: the (I, J0) of strips 0 ... strips_below(nt, L) - 1 (either may be
+// NULL); returns their count, 0 when nt or L is not positive
+int strip_schedule(int nt, int L, int32_t* I, int32_t* J0);
 // graph_tc.cu: tensor-core path (operand tiles + wgmma kernel) for the problems prep_kernel marked use_tc
 int launch_graph_tc(const Batch& bt, cudaStream_t st, int num_sms);
 size_t tc_operand_bytes(int B, int n);
