@@ -763,6 +763,124 @@ int tzr_register_cloud_pairs_icp_robust(tzr_ctx* ctx, const tzr_frontend_params*
                                         double epsilon, const tzr_robust_kernel* kernel,
                                         tzr_icp_result* icp_results);
 
+/* ---- multiway registration: information matrices ------------------------------------------------------------
+ * Open3D's GetInformationMatrixFromPointClouds(source, target, max_correspondence_distance, T) for many pairs at once,
+ * defined here as follows (DESIGN.md §3.16):
+ *   - Inputs: source x (ns float xyz), target y (nd float xyz), a similarity T = (s, R, t) with s held as tzr_icp holds it
+ *     (finite, > 0; R and t finite), and one distance r for the call (finite and > 0, else TZR_ERR_INVALID_ARG).
+ *   - Correspondences: exactly tzr_icp's at T: p_i = s (R x_i) + t, the nearest target with d^2 < r^2, the lowest target
+ *     index on ties, brute force below 1024 target points and the hashed grid from there (debug flags 33554432 and
+ *     67108864 force either route; both give the same correspondences).
+ *   - Sum: each correspondence (i, j), with q = y_j = (x, y, z) the target point, adds G^T G with G = [-[q]x | I] (3 x 6,
+ *     ordering (omega, tau)), rows (0, z, -y, 1, 0, 0), (-z, 0, x, 0, 1, 0), (y, -x, 0, 0, 0, 1).  Each of the 21 upper
+ *     entries (a, b) is ((G(0,a) G(0,b) + G(1,a) G(1,b)) + G(2,a) G(2,b)) in IEEE float64 with no FMA contraction, summed
+ *     in tzr_icp's chunk order (chunk k holds source points [256 k, 256 k + 256), a butterfly inside each warp, the
+ *     warps in order; the chunks by lane k mod 32, then a butterfly).  Lambda(5,5) is therefore the correspondence count.
+ *   - Outputs: Lambda as 36 doubles (row-major, mirrored, so symmetric bit for bit) and the count.
+ * Host pointers, synchronous.  Launches: 3 (+ 4 for the grid build when some target has at least 1024 points), whatever
+ * B.  Workspace: tzr_icp's own, so a retained solve stays retained. */
+int tzr_information_matrix(tzr_ctx* ctx, const float* src, int ns, const float* dst, int nd,
+                           const tzr_similarity* transform, double max_correspondence_distance, double* information,
+                           int32_t* count);
+
+/* B ragged pairs: pair b has ns[b] >= 1 source points at src[b], nd[b] >= 1 target points at dst[b] and its transform
+ * at transforms[b].  information: B x 36 doubles; counts (may be NULL): B.  Per pair, both outputs are bit-identical to
+ * tzr_information_matrix on that pair alone.  TZR_ERR_TOO_LARGE when the sources or targets exceed 2^31 - 1 points. */
+int tzr_information_matrix_batch(tzr_ctx* ctx, int B, const int32_t* ns, const float* const* src, const int32_t* nd,
+                                 const float* const* dst, const tzr_similarity* transforms,
+                                 double max_correspondence_distance, double* information, int32_t* counts);
+
+/* ---- multiway registration: robust pose graph ------------------------------------------------------------------
+ * The global step of Open3D's multiway registration (global_optimization over a PoseGraph), with GNC-TLS pruning the
+ * uncertain edges instead of Open3D's line process.  One graph per call, defined here as follows (DESIGN.md §3.16):
+ *   - Nodes: K poses T_k = (R_k, t_k), 2 <= K <= 1024 (K > 1024 is TZR_ERR_TOO_LARGE); T_k maps cloud k into the world
+ *     frame.  The node reference_node is held fixed.
+ *   - Edges: E >= 1 edges e = (s, d, T_sd, Lambda_e, uncertain_e) in the cloud-pair orientation p_d ~ T_sd p_s, so a
+ *     consistent graph has T_s = T_d T_sd.  T_sd is rigid: its scale is ignored, and a rotation that is not orthonormal
+ *     to 1e-6 (max |R^T R - I|), has a determinant below 0, or any non-finite entry is TZR_ERR_INVALID_ARG.  Lambda_e: 36
+ *     doubles, row-major, finite, Lambda(5,5) >= 0 (tzr_information_matrix's).  s = d is allowed (the edge adds a
+ *     constant to the cost).  An edge with Lambda(5,5) = 0 carries no information: it adds nothing and connects nothing.
+ *   - Connectivity: if the edges with s != d and Lambda(5,5) > 0 do not connect every node to the reference node, the
+ *     call returns TZR_ERR_INVALID_ARG and writes nothing.
+ *   - Residual: E = T_d^-1 T_s T_sd^-1 and e = (omega, tau) with omega = log R_E, tau = t_E.  The log: v = vee(R - R^T)
+ *     / 2, c = (tr R - 1) / 2, theta = atan2(|v|, c); theta < 1e-5: omega = (1 + theta^2 / 6) v (small-angle branch);
+ *     c < -0.9: omega = theta a with a the column of the symmetric part (R + R^T) / 2 - c I of largest diagonal,
+ *     normalised, with the sign of v (near pi); otherwise omega = (theta / |v|) v.
+ *   - Linearisation: left perturbations T_k <- Exp(delta_k) T_k, delta = (omega, tau), Exp the SE(3) exponential (R =
+ *     Rodrigues(omega), t = V(omega) tau); Jacobians J_s = Ad(T_d^-1), J_d = -Ad(T_d^-1), Ad(T) = [[R, 0], [[t]x R, R]].
+ *   - Normalised residual: r-bar_e = e^T Lambda_e e / (c^2 Lambda_e(5,5)) with c = max_correspondence_distance (0 where
+ *     Lambda_e(5,5) = 0): an edge is an outlier when it moves its overlap by more than c RMS.
+ *   - GNC-TLS on the uncertain edges (the rotation stage's schedule): weights start at 1; for i < max_iterations: the
+ *     inner solve with the current weights; if no edge is uncertain, stop; at i = 0, mu = 1 / (2 max r-bar - 1) over
+ *     the uncertain edges, and stop if mu <= 0; then, per uncertain edge, w = 0 where r-bar >= (mu + 1) / mu, 1 where
+ *     r-bar <= mu / (mu + 1), sqrt(mu (mu + 1) / r-bar) - mu between; cost = sum over the uncertain edges of the
+ *     previous w times r-bar; mu <- mu * gnc_factor; stop when |cost - previous cost| < cost_threshold (previous cost
+ *     +inf at i = 0).  Certain edges keep weight 1.  inlier = w >= 0.5.
+ *   - Inner solve: Levenberg-Marquardt on F = sum_e w_e e^T Lambda_e e over the K - 1 free nodes, n = 6 (K - 1) unknowns.
+ *     H = sum w J^T Lambda J and g = sum w J^T Lambda e, assembled per 6 x 6 block in ascending edge index; damping
+ *     H_ii <- H_ii + lambda (H_ii + 1), lambda = 1e-4 at the start of every inner solve (the additive part keeps a
+ *     node whose every edge has weight 0 solvable: its step is then 0 and the other nodes still move); delta solves H delta = -g by Cholesky
+ *     (cuSOLVER potrf / potrs).  Per iteration, with F' the cost at the candidate poses: if the factorisation failed
+ *     (a non-positive pivot) or F' is not finite, reject: lambda <- 10 lambda, and stop once lambda > 1e8; else if
+ *     |F - F'| <= 1e-10 F + 1e-24 c^2 sum_e Lambda_e(5,5), take the candidate when F' < F and stop; else if F' < F,
+ *     accept and lambda <- lambda / 10; else reject as above.  At most max_inner_iterations iterations, all enqueued.
+ *   - Initial poses: initial_poses (K, may be NULL; rigid and finite as the edges).  NULL: breadth-first from the
+ *     reference node (identity), first over the certain edges, then over all edges (those with s != d and
+ *     Lambda(5,5) > 0), each node's edges in ascending index, T_s = T_d T_sd or T_d = T_s T_sd^-1.
+ * Outputs: poses (K, scale 1); per edge (each may be NULL): the final weight, the inlier mask and r-bar at the returned
+ * poses; summary (may be NULL).  The returned poses come from the last inner solve, the weights from the GNC update
+ * after it (as the rotation stage returns them).  Host pointers, synchronous; one host read-back per GNC iteration.
+ * Launches: (3 + 4 max_inner_iterations) per GNC iteration, plus 2 cuSOLVER calls per inner iteration.  Workspace of
+ * its own (n^2 doubles for H: about 301 MB at K = 1024), so a retained solve stays retained.  TZR_ERR_UNSUPPORTED when
+ * cuSOLVER cannot be loaded. */
+typedef struct tzr_pose_graph_params {
+  double max_correspondence_distance;  /* c: no default; finite and > 0 */
+  double gnc_factor;                   /* 1.4; > 1 */
+  double cost_threshold;               /* 1e-6 */
+  int32_t max_iterations;              /* 100 GNC iterations; >= 1 */
+  int32_t max_inner_iterations;        /* 10 Levenberg-Marquardt iterations per GNC iteration; >= 1 */
+  int32_t reference_node;              /* 0 */
+  int32_t reserved;
+} tzr_pose_graph_params;
+
+typedef struct tzr_pose_graph_summary {
+  int32_t iterations;        /* GNC iterations (inner solves) run */
+  int32_t inner_iterations;  /* Levenberg-Marquardt iterations, summed over them */
+  double cost;               /* F of the last inner solve at the returned poses */
+} tzr_pose_graph_summary;
+
+/* max_correspondence_distance 0 (the caller must set it), gnc_factor 1.4, cost_threshold 1e-6, max_iterations 100,
+ * max_inner_iterations 10, reference_node 0. */
+void tzr_pose_graph_params_default(tzr_pose_graph_params* p);
+
+/* edges: E x 2 (s, d); edge_transforms, information (E x 36): per edge; uncertain (E, may be NULL: every edge certain). */
+int tzr_pose_graph_optimize(tzr_ctx* ctx, const tzr_pose_graph_params* params, int K, int E, const int32_t* edges,
+                            const tzr_similarity* edge_transforms, const double* information, const int32_t* uncertain,
+                            const tzr_similarity* initial_poses, tzr_similarity* poses, double* weights,
+                            uint8_t* inlier_mask, double* residuals, tzr_pose_graph_summary* summary);
+
+/* tzr_register_cloud_pairs_icp_point_to_plane (same arguments, same outputs bit for bit), then the information matrix
+ * of every refined pair (solved, valid and finite record) at its ICP transform and the ICP's
+ * max_correspondence_distance, from the clouds and transforms already on the device (no upload), then
+ * tzr_pose_graph_optimize over the n_clouds clouds with one edge per refined pair (s, d) = pair_clouds[p], T_sd its ICP
+ * transform, Lambda its information matrix and uncertain[p] (P entries, required).  params->estimate_scaling = 1 is
+ * TZR_ERR_INVALID_ARG (the pose graph is rigid).  Outputs: information (P x 36) and info_counts (P), zeroed for a pair
+ * that was not refined; edge_weights (P doubles) and edge_mask (P bytes), 0 for a pair that is not an edge; poses
+ * (n_clouds); pg_summary (may be NULL); *pg_status receives the pose graph's status (TZR_OK, or its error, e.g.
+ * TZR_ERR_INVALID_ARG for a disconnected graph; poses, weights and masks are then zero).  Every output equals
+ * tzr_register_cloud_pairs_icp_point_to_plane, then tzr_information_matrix_batch over the refined pairs in pair order,
+ * then tzr_pose_graph_optimize over them, bit for bit.  Returns what the registration returns.  A solve entry:
+ * tzr_last_inliers and tzr_certify_last_solve see its solve. */
+int tzr_register_cloud_pairs_multiway(tzr_ctx* ctx, const tzr_frontend_params* fparams, const tzr_params* params,
+                                      int n_clouds, const int32_t* n, const float* const* pts, int P,
+                                      const int32_t* pair_clouds, const uint64_t* tuple_seeds,
+                                      tzr_solution* solutions, int32_t* status, int32_t* problem_index,
+                                      int64_t* n_corr, int32_t* const* corr, int32_t* const* cliques,
+                                      float* global_scale, const tzr_icp_params* icp, tzr_icp_result* icp_results,
+                                      const int32_t* uncertain, const tzr_pose_graph_params* pg, double* information,
+                                      int32_t* info_counts, double* edge_weights, uint8_t* edge_mask,
+                                      tzr_similarity* poses, tzr_pose_graph_summary* pg_summary, int32_t* pg_status);
+
 /* ---- downsampling point clouds: voxel-grid averaging ----------------------------------------------------------
  * The first step of the reference's FPFH + TEASER++ + ICP tutorial (voxel_down_sample on both raw scans), for many
  * clouds at once.  Open3D's PointCloud::VoxelDownSample, points only, with a defined order.  Per cloud, all arithmetic

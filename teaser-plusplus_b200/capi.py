@@ -124,9 +124,23 @@ class RobustKernel(C.Structure):
     _fields_ = [("type", C.c_int32), ("reserved", C.c_int32), ("k", C.c_double)]
 
 
+class PoseGraphParams(C.Structure):
+    """tzr_pose_graph_params: the GNC-TLS pose graph's distance c, schedule and reference node."""
+    _fields_ = [("max_correspondence_distance", C.c_double), ("gnc_factor", C.c_double),
+                ("cost_threshold", C.c_double), ("max_iterations", C.c_int32), ("max_inner_iterations", C.c_int32),
+                ("reference_node", C.c_int32), ("reserved", C.c_int32)]
+
+
+class PoseGraphSummary(C.Structure):
+    """tzr_pose_graph_summary."""
+    _fields_ = [("iterations", C.c_int32), ("inner_iterations", C.c_int32), ("cost", C.c_double)]
+
+
 # robust kernel types (TZR_LOSS_*), by the names robust_kernel() accepts
 LOSS_TYPES = {"l2": 0, "l1": 1, "huber": 2, "cauchy": 3, "gm": 4, "tukey": 5}
 assert C.sizeof(IcpParams) == 32, C.sizeof(IcpParams)
+assert C.sizeof(PoseGraphParams) == 40 and PoseGraphParams.reference_node.offset == 32, C.sizeof(PoseGraphParams)
+assert C.sizeof(PoseGraphSummary) == 16 and PoseGraphSummary.cost.offset == 8, C.sizeof(PoseGraphSummary)
 assert C.sizeof(RobustKernel) == 16 and RobustKernel.k.offset == 8, C.sizeof(RobustKernel)
 assert SIMILARITY_DTYPE.itemsize == C.sizeof(Similarity) == 104, C.sizeof(Similarity)
 assert ICP_RESULT_DTYPE.itemsize == C.sizeof(IcpResult) == 136, (ICP_RESULT_DTYPE.itemsize, C.sizeof(IcpResult))
@@ -150,6 +164,8 @@ _SYMBOLS = [
     "tzr_register_cloud_pairs_icp_point_to_plane", "tzr_icp_generalized", "tzr_icp_generalized_batch",
     "tzr_register_cloud_pairs_icp_generalized", "tzr_icp_point_to_plane_robust_batch", "tzr_icp_generalized_robust_batch",
     "tzr_register_cloud_pairs_icp_robust", "tzr_ctx_last_strip_blocks", "tzr_graph_strip_schedule",
+    "tzr_information_matrix", "tzr_information_matrix_batch", "tzr_pose_graph_params_default", "tzr_pose_graph_optimize",
+    "tzr_register_cloud_pairs_multiway",
 ]
 
 # status codes (tzr_status)
@@ -306,6 +322,16 @@ def lib():
     L.tzr_icp_generalized_robust_batch.argtypes = L.tzr_icp_generalized_batch.argtypes + [C.POINTER(RobustKernel)]
     L.tzr_register_cloud_pairs_icp_robust.argtypes = L.tzr_register_cloud_pairs.argtypes + [
         C.POINTER(IcpParams), C.c_int32, C.c_double, C.POINTER(RobustKernel), C.POINTER(IcpResult)]
+    L.tzr_information_matrix.argtypes = [vp, fp, C.c_int, fp, C.c_int, C.POINTER(Similarity), C.c_double, dp, i32p]
+    L.tzr_information_matrix_batch.argtypes = [vp, C.c_int, i32p, fpp, i32p, fpp, C.POINTER(Similarity), C.c_double,
+                                               dp, i32p]
+    L.tzr_pose_graph_params_default.argtypes = [C.POINTER(PoseGraphParams)]
+    L.tzr_pose_graph_params_default.restype = None
+    L.tzr_pose_graph_optimize.argtypes = [vp, C.POINTER(PoseGraphParams), C.c_int, C.c_int, i32p,
+                                          C.POINTER(Similarity), dp, i32p, C.POINTER(Similarity),
+                                          C.POINTER(Similarity), dp, u8p, dp, C.POINTER(PoseGraphSummary)]
+    L.tzr_register_cloud_pairs_multiway.argtypes = L.tzr_register_cloud_pairs_icp.argtypes + [
+        i32p, C.POINTER(PoseGraphParams), dp, i32p, dp, u8p, C.POINTER(Similarity), C.POINTER(PoseGraphSummary), i32p]
     L.tzr_voxel_downsample.argtypes = [vp, fp, C.c_int, C.c_double, fp, i32p, i32p]
     L.tzr_voxel_downsample_batch.argtypes = [vp, C.c_int, i32p, fpp, C.c_double, fpp, i32p, C.POINTER(i32p), i32p]
     for s in _SYMBOLS:
@@ -334,6 +360,28 @@ def icp_params(max_correspondence_distance: float, **kw) -> IcpParams:
             raise AttributeError(k)
         setattr(p, k, v)
     return p
+
+
+def pose_graph_params(max_correspondence_distance: float, **kw) -> PoseGraphParams:
+    """tzr_pose_graph_params_default with max_correspondence_distance and any field in kw set."""
+    p = PoseGraphParams()
+    lib().tzr_pose_graph_params_default(C.byref(p))
+    p.max_correspondence_distance = float(max_correspondence_distance)
+    for k, v in kw.items():
+        if not hasattr(p, k):
+            raise AttributeError(k)
+        setattr(p, k, v)
+    return p
+
+
+def _poses(sims):
+    """(K,4,4) float64 rigid matrices from K Similarity records."""
+    out = np.zeros((len(sims), 4, 4))
+    for k, x in enumerate(sims):
+        out[k, :3, :3] = np.asarray(x.rotation[:]).reshape(3, 3).T
+        out[k, :3, 3] = x.translation[:]
+        out[k, 3, 3] = 1.0
+    return out
 
 
 def robust_kernel(kernel) -> RobustKernel | None:
@@ -1067,7 +1115,7 @@ class Context:
 
     def _register_pairs(self, clouds, pairs, params, normal_search_radius, fpfh_search_radius, use_absolute_scale,
                         use_crosscheck, use_tuple_test, tuple_scale, tuple_seeds, icp, plane=False, epsilon=None,
-                        kernel=None):
+                        kernel=None, multiway=None):
         cl = [np.ascontiguousarray(c, dtype=np.float32) for c in clouds]
         if not cl or any(c.ndim != 2 or c.shape[1] != 3 or c.shape[0] == 0 for c in cl):
             raise TzrError("register_cloud_pairs: a non-empty list of non-empty (n,3) clouds is required")
@@ -1103,7 +1151,26 @@ class Context:
         else:
             icp_res = np.zeros(P, dtype=ICP_RESULT_DTYPE)
             out_res = icp_res.ctypes.data_as(C.POINTER(IcpResult))
-            if kernel is not None:
+            if multiway is not None:
+                unc, pg = multiway
+                unc = np.ascontiguousarray(unc, dtype=np.int32)
+                if unc.shape != (P,):
+                    raise TzrError("register_multiway: uncertain needs one entry per pair")
+                info = np.zeros((P, 6, 6))
+                icnt = np.zeros(P, dtype=np.int32)
+                ew = np.zeros(P)
+                em = np.zeros(P, dtype=np.uint8)
+                poses = (Similarity * len(cl))()
+                summ = PoseGraphSummary()
+                pg_status = C.c_int32(0)
+                rc = lib().tzr_register_cloud_pairs_multiway(*args, C.byref(icp), out_res, _p(unc, C.c_int32),
+                                                             C.byref(pg), _p(info, C.c_double), _p(icnt, C.c_int32),
+                                                             _p(ew, C.c_double), _p(em, C.c_uint8), poses,
+                                                             C.byref(summ), C.byref(pg_status))
+                mw = dict(information=info, counts=icnt, weights=ew, mask=em.astype(bool), poses=_poses(poses),
+                          status=int(pg_status.value), iterations=int(summ.iterations),
+                          inner_iterations=int(summ.inner_iterations), cost=float(summ.cost))
+            elif kernel is not None:
                 rc = lib().tzr_register_cloud_pairs_icp_robust(*args, C.byref(icp), 1 if plane else 2,
                                                                0.0 if epsilon is None else epsilon, C.byref(kernel),
                                                                out_res)
@@ -1118,7 +1185,87 @@ class Context:
         clq = [c[:max(0, int(s["clique_size"]))].copy() if i >= 0 else np.zeros(0, dtype=np.int32)
                for c, s, i in zip(clq, sols, index)]
         out = (sols, status, index, corr, clq, [float(x) for x in g])
+        if multiway is not None:
+            return out + (icp_res, mw)
         return out if icp is None else out + (icp_res,)
+
+    def register_multiway(self, clouds, pairs, params: Params, max_correspondence_distance, uncertain=None,
+                          normal_search_radius=0.03, fpfh_search_radius=0.05, use_absolute_scale=True,
+                          use_crosscheck=True, use_tuple_test=True, tuple_scale=0.0, tuple_seeds=None, max_iteration=30,
+                          relative_fitness=1e-6, relative_rmse=1e-6, pose_graph=None):
+        """tzr_register_cloud_pairs_multiway: register_cloud_pairs_icp(method="point_to_plane"), the information
+        matrix of every refined pair and the GNC-TLS pose graph over the clouds, in one call.  uncertain: one flag per
+        pair (None: Open3D's tutorial rule, pair (k, k + 1) certain and every other pair uncertain).  pose_graph: a
+        PoseGraphParams (None: the defaults with c = max_correspondence_distance).  Returns register_cloud_pairs_icp's
+        seven results plus a dict: information (P,6,6), counts (P,), weights (P,), mask (P,) bool, poses (n_clouds,4,4),
+        status (the pose graph's TZR status), iterations, inner_iterations, cost."""
+        pc = np.ascontiguousarray(pairs, dtype=np.int32).reshape(-1, 2)
+        if uncertain is None:
+            uncertain = [0 if b == a + 1 else 1 for a, b in pc]
+        pg = pose_graph if pose_graph is not None else pose_graph_params(max_correspondence_distance)
+        icp = icp_params(max_correspondence_distance, max_iteration=int(max_iteration),
+                         relative_fitness=float(relative_fitness), relative_rmse=float(relative_rmse))
+        return self._register_pairs(clouds, pc, params, normal_search_radius, fpfh_search_radius, use_absolute_scale,
+                                    use_crosscheck, use_tuple_test, tuple_scale, tuple_seeds, icp, plane=True,
+                                    multiway=(uncertain, pg))
+
+    def information_matrix(self, src, dst, transform, max_correspondence_distance):
+        """tzr_information_matrix: (Lambda (6,6) float64, count) of the (ns,3) source at transform (see similarity())
+        against the (nd,3) target."""
+        S, D = _cloud32(src, "information_matrix"), _cloud32(dst, "information_matrix")
+        info = np.zeros((6, 6))
+        cnt = C.c_int32(0)
+        tr = similarity(transform)
+        self._ck(lib().tzr_information_matrix(self._h, _p(S, C.c_float), S.shape[0], _p(D, C.c_float), D.shape[0],
+                                              C.byref(tr), float(max_correspondence_distance), _p(info, C.c_double),
+                                              C.byref(cnt)))
+        return info, int(cnt.value)
+
+    def information_matrix_batch(self, srcs, dsts, transforms, max_correspondence_distance):
+        """tzr_information_matrix_batch over B pairs: (Lambda (B,6,6), counts (B,) int32)."""
+        S = [_cloud32(a, "information_matrix_batch") for a in srcs]
+        D = [_cloud32(a, "information_matrix_batch") for a in dsts]
+        B = len(S)
+        if B == 0 or len(D) != B or len(transforms) != B:
+            raise TzrError("information_matrix_batch: one target and one transform per source are required")
+        ns = np.array([a.shape[0] for a in S], dtype=np.int32)
+        nd = np.array([a.shape[0] for a in D], dtype=np.int32)
+        fp = C.POINTER(C.c_float)
+        tr = (Similarity * B)(*[similarity(x) for x in transforms])
+        info = np.zeros((B, 6, 6))
+        cnt = np.zeros(B, dtype=np.int32)
+        self._ck(lib().tzr_information_matrix_batch(self._h, B, _p(ns, C.c_int32), (fp * B)(*[_p(a, C.c_float) for a in S]),
+                                                    _p(nd, C.c_int32), (fp * B)(*[_p(a, C.c_float) for a in D]), tr,
+                                                    float(max_correspondence_distance), _p(info, C.c_double),
+                                                    _p(cnt, C.c_int32)))
+        return info, cnt
+
+    def optimize_pose_graph(self, K, edges, transforms, information, max_correspondence_distance, uncertain=None,
+                            initial_poses=None, **params):
+        """tzr_pose_graph_optimize: K nodes, edges (E,2) (s, d), transforms (E rigid T_sd: (4,4) matrices or anything
+        similarity() takes), information (E,6,6), uncertain (E flags, None: every edge certain), initial_poses (K, None:
+        breadth-first from the reference node); params: any PoseGraphParams field.  Returns a dict: poses (K,4,4),
+        weights (E,), mask (E,) bool, residuals (E,) r-bar, iterations, inner_iterations, cost."""
+        ed = np.ascontiguousarray(edges, dtype=np.int32).reshape(-1, 2)
+        E = ed.shape[0]
+        info = np.ascontiguousarray(information, dtype=np.float64).reshape(E, 36)
+        if len(transforms) != E:
+            raise TzrError("optimize_pose_graph: one transform per edge is required")
+        tr = (Similarity * E)(*[similarity(x) for x in transforms])
+        unc = None if uncertain is None else np.ascontiguousarray(uncertain, dtype=np.int32)
+        if unc is not None and unc.shape != (E,):
+            raise TzrError("optimize_pose_graph: uncertain needs one entry per edge")
+        init = None if initial_poses is None else (Similarity * int(K))(*[similarity(x) for x in initial_poses])
+        pg = pose_graph_params(max_correspondence_distance, **params)
+        poses = (Similarity * max(1, int(K)))()
+        w, m, r = np.zeros(max(1, E)), np.zeros(max(1, E), dtype=np.uint8), np.zeros(max(1, E))
+        summ = PoseGraphSummary()
+        self._ck(lib().tzr_pose_graph_optimize(self._h, C.byref(pg), int(K), E, _p(ed, C.c_int32), tr,
+                                               _p(info, C.c_double), None if unc is None else _p(unc, C.c_int32), init,
+                                               poses, _p(w, C.c_double), _p(m, C.c_uint8), _p(r, C.c_double),
+                                               C.byref(summ)))
+        return dict(poses=_poses(poses), weights=w[:E], mask=m[:E].astype(bool), residuals=r[:E],
+                    iterations=int(summ.iterations), inner_iterations=int(summ.inner_iterations), cost=float(summ.cost))
 
     def icp(self, src, dst, max_correspondence_distance, init=None, max_iteration=30, relative_fitness=1e-6,
             relative_rmse=1e-6):

@@ -40,6 +40,8 @@ struct tzr_ctx {
   DevBuf icp;
   // tzr_voxel_downsample(_batch): its own workspace, for the same reason
   DevBuf vox;
+  // tzr_pose_graph_optimize: its own workspace, for the same reason
+  DevBuf pg;
   int last_strip_blocks = 0;  // strip length of the most recent graph kernel launch (tzr_ctx_last_strip_blocks)
   int max_n = kMaxN;  // per-problem size limit of this context (tzr_ctx_set_max_n: kMaxN ... kMaxNLarge)
   // pinned host staging
@@ -1225,7 +1227,7 @@ int tzr_ctx_destroy(tzr_ctx* ctx) {
                     &ctx->lock, &ctx->flg, &ctx->kfinal, &ctx->tstart, &ctx->stack, &ctx->cv, &ctx->centry, &ctx->ps, &ctx->pd, &ctx->wgt,
                     &ctx->res, &ctx->skey, &ctx->sidx, &ctx->sorted, &ctx->rmask, &ctx->tmask, &ctx->sol, &ctx->dbg,
                     &ctx->misc, &ctx->sc, &ctx->m_in, &ctx->m_scratch, &ctx->m_out, &ctx->certb, &ctx->lg, &ctx->cq, &ctx->rg, &ctx->icp,
-                    &ctx->vox};
+                    &ctx->vox, &ctx->pg};
   for (DevBuf* b : bufs)
     if (b->p) cudaFree(b->p);
   if (ctx->h_pin) cudaFreeHost(ctx->h_pin);
@@ -2081,6 +2083,281 @@ static bool robust_kernel_ok(const tzr_robust_kernel* k) {
   }
 }
 
+// ---- multiway registration: the robust pose graph (DESIGN.md §3.16) ----------------------------------------------------
+static bool pg_params_ok(const tzr_pose_graph_params* p) {
+  return p && std::isfinite(p->max_correspondence_distance) && p->max_correspondence_distance > 0 &&
+         std::isfinite(p->gnc_factor) && p->gnc_factor > 1 && !std::isnan(p->cost_threshold) &&
+         p->max_iterations >= 1 && p->max_inner_iterations >= 1;
+}
+
+// a rigid transform: finite, R^T R = I to 1e-6 in every entry, det R > 0 (the scale is not read)
+static bool rigid_ok(const tzr_similarity& T) {
+  const double* R = T.rotation;
+  for (int k = 0; k < 9; ++k)
+    if (!std::isfinite(R[k])) return false;
+  for (int k = 0; k < 3; ++k)
+    if (!std::isfinite(T.translation[k])) return false;
+  for (int a = 0; a < 3; ++a)
+    for (int b = 0; b < 3; ++b) {
+      const double d = (R[3 * a] * R[3 * b] + R[3 * a + 1] * R[3 * b + 1]) + R[3 * a + 2] * R[3 * b + 2];
+      if (std::fabs(d - (a == b ? 1.0 : 0.0)) > 1e-6) return false;
+    }
+  const double det = R[0] * (R[4] * R[8] - R[7] * R[5]) - R[3] * (R[1] * R[8] - R[7] * R[2]) +
+                     R[6] * (R[1] * R[5] - R[4] * R[2]);
+  return det > 0;
+}
+
+// c = a b (column-major 3 x 3), entry (r, k) = (a(r,0) b(0,k) + a(r,1) b(1,k)) + a(r,2) b(2,k); y = a x likewise
+static void h_m33(const double* a, const double* b, double* c) {
+  for (int k = 0; k < 3; ++k)
+    for (int r = 0; r < 3; ++r) c[3 * k + r] = (a[r] * b[3 * k] + a[3 + r] * b[3 * k + 1]) + a[6 + r] * b[3 * k + 2];
+}
+static void h_mv3(const double* a, const double* x, double* y) {
+  for (int r = 0; r < 3; ++r) y[r] = (a[r] * x[0] + a[3 + r] * x[1]) + a[6 + r] * x[2];
+}
+
+// The breadth-first initial poses and the connectivity check (include/teaser_b200.h): false when some node is not
+// reached from the reference node.  pose: K x 12 (R column-major, t); with `given` the poses are kept, only reached.
+static bool pg_bfs(int K, int E, const int32_t* ends, const tzr_similarity* T, const std::vector<char>& live,
+                   const int32_t* uncertain, int ref, bool given, std::vector<double>* pose) {
+  std::vector<std::vector<int>> adj((size_t)K);
+  for (int e = 0; e < E; ++e)
+    if (live[e]) {
+      adj[ends[2 * e]].push_back(e);
+      adj[ends[2 * e + 1]].push_back(e);
+    }
+  std::vector<char> seen((size_t)K, 0);
+  std::vector<int> order{ref};
+  seen[ref] = 1;
+  if (!given) {
+    double* P = pose->data() + 12 * (size_t)ref;
+    for (int k = 0; k < 12; ++k) P[k] = (k == 0 || k == 4 || k == 8) ? 1.0 : 0.0;
+  }
+  for (int phase = 0; phase < 2; ++phase) {
+    std::vector<int> queue = order;
+    for (size_t head = 0; head < queue.size(); ++head) {
+      const int u = queue[head];
+      for (int e : adj[u]) {
+        if (phase == 0 && uncertain && uncertain[e]) continue;
+        const int s = ends[2 * e], d = ends[2 * e + 1], v = u == s ? d : s;
+        if (seen[v]) continue;
+        seen[v] = 1;
+        queue.push_back(v);
+        order.push_back(v);
+        if (given) continue;
+        const double* Ru = pose->data() + 12 * (size_t)u;
+        double* Pv = pose->data() + 12 * (size_t)v;
+        const double* Rsd = T[e].rotation;
+        const double* tsd = T[e].translation;
+        if (u == d) {  // T_s = T_d T_sd
+          double x[3];
+          h_m33(Ru, Rsd, Pv);
+          h_mv3(Ru, tsd, x);
+          for (int r = 0; r < 3; ++r) Pv[9 + r] = x[r] + Ru[9 + r];
+        } else {  // T_d = T_s T_sd^-1: R_d = R_s R_sd^T, t_d = t_s - R_d t_sd
+          double Rt[9], x[3];
+          for (int k = 0; k < 3; ++k)
+            for (int r = 0; r < 3; ++r) Rt[3 * k + r] = Rsd[3 * r + k];
+          h_m33(Ru, Rt, Pv);
+          h_mv3(Pv, tsd, x);
+          for (int r = 0; r < 3; ++r) Pv[9 + r] = Ru[9 + r] - x[r];
+        }
+      }
+    }
+  }
+  return (int)order.size() == K;
+}
+
+static int pose_graph_run(tzr_ctx* ctx, const tzr_pose_graph_params* prm, int K, int E, const int32_t* ends,
+                          const tzr_similarity* T, const double* info, const int32_t* uncertain,
+                          const tzr_similarity* init, tzr_similarity* poses, double* weights, uint8_t* inlier_mask,
+                          double* residuals, tzr_pose_graph_summary* summary) {
+  if (!ctx || !pg_params_ok(prm) || K < 2 || E < 1 || !ends || !T || !info || !poses) {
+    if (ctx) ctx->last_error = "pose graph: invalid arguments (K >= 2, E >= 1 and the parameters' ranges)";
+    return TZR_ERR_INVALID_ARG;
+  }
+  if (K > 1024) {
+    ctx->last_error = "pose graph: more than 1024 nodes";
+    return TZR_ERR_TOO_LARGE;
+  }
+  const int ref = prm->reference_node;
+  if (ref < 0 || ref >= K) {
+    ctx->last_error = "pose graph: reference_node " + std::to_string(ref) + " is not a node";
+    return TZR_ERR_INVALID_ARG;
+  }
+  std::vector<char> live((size_t)E);
+  double info_sum = 0.0;
+  for (int e = 0; e < E; ++e) {
+    const int s = ends[2 * e], d = ends[2 * e + 1];
+    if (s < 0 || s >= K || d < 0 || d >= K || !rigid_ok(T[e])) {
+      ctx->last_error = "pose graph: edge " + std::to_string(e) + " has a node out of range or is not rigid";
+      return TZR_ERR_INVALID_ARG;
+    }
+    for (int k = 0; k < 36; ++k)
+      if (!std::isfinite(info[36 * (size_t)e + k])) {
+        ctx->last_error = "pose graph: edge " + std::to_string(e) + " has a non-finite information entry";
+        return TZR_ERR_INVALID_ARG;
+      }
+    const double l55 = info[36 * (size_t)e + 35];
+    if (l55 < 0) {
+      ctx->last_error = "pose graph: edge " + std::to_string(e) + " has Lambda(5,5) < 0";
+      return TZR_ERR_INVALID_ARG;
+    }
+    live[e] = s != d && l55 > 0;
+    info_sum += l55;
+  }
+  if (init)
+    for (int k = 0; k < K; ++k)
+      if (!rigid_ok(init[k])) {
+        ctx->last_error = "pose graph: initial pose " + std::to_string(k) + " is not rigid and finite";
+        return TZR_ERR_INVALID_ARG;
+      }
+  std::vector<double> pose((size_t)K * 12);
+  if (init)
+    for (int k = 0; k < K; ++k) {
+      memcpy(&pose[12 * (size_t)k], init[k].rotation, 72);
+      memcpy(&pose[12 * (size_t)k + 9], init[k].translation, 24);
+    }
+  if (!pg_bfs(K, E, ends, T, live, uncertain, ref, init != nullptr, &pose)) {
+    ctx->last_error = "pose graph: the edges do not connect every node to the reference node";
+    return TZR_ERR_INVALID_ARG;
+  }
+  const double c = prm->max_correspondence_distance;
+  // edge table; the plan of H's lower blocks and of the right-hand side, each block's terms in ascending edge index
+  std::vector<PgEdge> ed((size_t)E);
+  std::map<std::pair<int, int>, std::vector<PgTerm>> plan_map;
+  for (int e = 0; e < E; ++e) {
+    PgEdge& x = ed[e];
+    x = PgEdge{};
+    x.s = ends[2 * e];
+    x.d = ends[2 * e + 1];
+    x.fs = x.s == ref ? -1 : x.s < ref ? x.s : x.s - 1;
+    x.fd = x.d == ref ? -1 : x.d < ref ? x.d : x.d - 1;
+    x.uncertain = uncertain && uncertain[e] ? 1 : 0;
+    memcpy(x.R, T[e].rotation, 72);
+    memcpy(x.t, T[e].translation, 24);
+    const double l55 = info[36 * (size_t)e + 35];
+    if (l55 > 0) {
+      memcpy(x.L, info + 36 * (size_t)e, 36 * 8);
+      x.inv_norm = 1.0 / ((c * c) * l55);
+    }
+    if (!live[e]) continue;
+    if (x.fs >= 0) {
+      plan_map[{x.fs, x.fs}].push_back(PgTerm{e, 1});
+      plan_map[{x.fs, -1}].push_back(PgTerm{e, 1});
+    }
+    if (x.fd >= 0) {
+      plan_map[{x.fd, x.fd}].push_back(PgTerm{e, 1});
+      plan_map[{x.fd, -1}].push_back(PgTerm{e, -1});
+    }
+    if (x.fs >= 0 && x.fd >= 0) plan_map[{std::max(x.fs, x.fd), std::min(x.fs, x.fd)}].push_back(PgTerm{e, -1});
+  }
+  std::vector<PgBlock> blocks;
+  std::vector<PgTerm> terms;
+  for (const auto& kv : plan_map) {
+    blocks.push_back(PgBlock{kv.first.first, kv.first.second, (int)terms.size(), 0});
+    terms.insert(terms.end(), kv.second.begin(), kv.second.end());
+    blocks.back().hi = (int)terms.size();
+  }
+  PgPlan plan;
+  plan.K = K;
+  plan.E = E;
+  plan.n = 6 * (K - 1);
+  plan.blocks = (int)blocks.size();
+  plan.max_inner = prm->max_inner_iterations;
+  plan.gnc_factor = prm->gnc_factor;
+  plan.cost_threshold = prm->cost_threshold;
+  const double cost_floor = 1e-24 * (c * c) * info_sum;
+  const size_t n = (size_t)plan.n;
+  // workspace: [edges | blocks | terms | poses (2 buffers) | weights | state] staged in one copy, then the edge terms,
+  // H, g and the factorisation's workspace
+  const size_t o_blk = al256((size_t)E * sizeof(PgEdge)), o_trm = o_blk + al256(blocks.size() * sizeof(PgBlock)),
+               o_pose = o_trm + al256(terms.size() * sizeof(PgTerm)), o_w = o_pose + al256((size_t)K * 24 * 8),
+               o_st = o_w + al256((size_t)E * 8), in_bytes = o_st + sizeof(PgState),
+               o_term = al256(in_bytes), o_H = o_term + al256((size_t)E * 2 * kPgTermStride * 8),
+               o_g = o_H + al256(n * n * 8), o_work = o_g + al256(n * 8);
+  cudaSetDevice(ctx->device);
+  cudaStream_t st = ctx->stream;
+  int rc;
+  if ((rc = ensure(ctx, ctx->pg, o_work + 256)) != TZR_OK) return rc;
+  int lwork = 0;
+  if ((rc = dense_cholesky_setup(&ctx->solver_handle, (int)n, (double*)((char*)ctx->pg.p + o_H), &lwork, st,
+                                 &ctx->last_error)) != TZR_OK)
+    return rc;
+  if ((rc = ensure(ctx, ctx->pg, o_work + (size_t)std::max(lwork, 1) * 8)) != TZR_OK) return rc;
+  char* d = (char*)ctx->pg.p;
+  std::vector<char> h(in_bytes, 0);
+  memcpy(h.data(), ed.data(), (size_t)E * sizeof(PgEdge));
+  memcpy(h.data() + o_blk, blocks.data(), blocks.size() * sizeof(PgBlock));
+  memcpy(h.data() + o_trm, terms.data(), terms.size() * sizeof(PgTerm));
+  memcpy(h.data() + o_pose, pose.data(), (size_t)K * 12 * 8);
+  for (int e = 0; e < E; ++e) ((double*)(h.data() + o_w))[e] = 1.0;
+  PgState s0{};
+  s0.gnc_cost = INFINITY;
+  memcpy(h.data() + o_st, &s0, sizeof(s0));
+  CK(cudaMemcpyAsync(d, h.data(), in_bytes, cudaMemcpyHostToDevice, st));
+  PgDev dv{(const PgEdge*)d, (const PgBlock*)(d + o_blk), (const PgTerm*)(d + o_trm), (double*)(d + o_pose),
+           (double*)(d + o_term), (double*)(d + o_w), (double*)(d + o_H), (double*)(d + o_g), (PgState*)(d + o_st)};
+  PgState hs{};
+  int outer = 0;
+  long long inner_total = 0;
+  for (int it = 0; it < prm->max_iterations; ++it) {
+    ctx->launches += launch_pose_graph_begin(plan, dv, cost_floor, st);
+    for (int j = 0; j < plan.max_inner; ++j) {
+      CK(cudaMemsetAsync(dv.H, 0, n * n * 8, st));
+      ctx->launches += launch_pose_graph_assemble(plan, dv, st);
+      if ((rc = dense_cholesky_solve(ctx->solver_handle, (int)n, dv.H, dv.g, (double*)(d + o_work), lwork,
+                                     dv.state->info, &ctx->last_error)) != TZR_OK)
+        return rc;
+      ctx->launches += launch_pose_graph_step(plan, dv, ref, cost_floor, st);
+    }
+    ctx->launches += launch_pose_graph_gnc(plan, dv, it, st);
+    if ((rc = check_launch(ctx, "pose graph launch")) != TZR_OK) return rc;
+    // the one read-back of a GNC iteration
+    CK(cudaMemcpyAsync(&hs, dv.state, sizeof(hs), cudaMemcpyDeviceToHost, st));
+    CK(cudaStreamSynchronize(st));
+    outer = it + 1;
+    inner_total += hs.inner;
+    if (hs.stop) break;
+  }
+  std::vector<double> w((size_t)E), terms_out((size_t)E * kPgTermStride);
+  CK(cudaMemcpyAsync(pose.data(), dv.poses + (size_t)hs.cur * K * 12, (size_t)K * 12 * 8, cudaMemcpyDeviceToHost, st));
+  CK(cudaMemcpyAsync(w.data(), dv.weight, (size_t)E * 8, cudaMemcpyDeviceToHost, st));
+  CK(cudaMemcpyAsync(terms_out.data(), dv.eterm + (size_t)hs.cur * E * kPgTermStride, (size_t)E * kPgTermStride * 8,
+                     cudaMemcpyDeviceToHost, st));
+  CK(cudaStreamSynchronize(st));
+  for (int k = 0; k < K; ++k) {
+    memset(&poses[k], 0, sizeof(tzr_similarity));
+    poses[k].scale = 1.0;
+    memcpy(poses[k].rotation, &pose[12 * (size_t)k], 72);
+    memcpy(poses[k].translation, &pose[12 * (size_t)k + 9], 24);
+  }
+  for (int e = 0; e < E; ++e) {
+    if (weights) weights[e] = w[e];
+    if (inlier_mask) inlier_mask[e] = w[e] >= 0.5 ? 1 : 0;
+    if (residuals) residuals[e] = terms_out[(size_t)e * kPgTermStride + 43];
+  }
+  if (summary) {
+    summary->iterations = outer;
+    summary->inner_iterations = (int32_t)inner_total;
+    summary->cost = hs.cost;
+  }
+  return TZR_OK;
+}
+
+// what tzr_register_cloud_pairs_multiway adds to register_pairs_run (include/teaser_b200.h)
+struct MultiwayOut {
+  const int32_t* uncertain;
+  const tzr_pose_graph_params* pg;
+  double* information;
+  int32_t* info_counts;
+  double* edge_weights;
+  uint8_t* edge_mask;
+  tzr_similarity* poses;
+  tzr_pose_graph_summary* summary;
+  int32_t* pg_status;
+};
+
 static void icp_result_of(const IcpProb& pr, tzr_icp_result* out) {
   memset(out, 0, sizeof(*out));
   if (!pr.seeded) return;
@@ -2107,11 +2384,14 @@ static int register_pairs_run(tzr_ctx* ctx, const tzr_frontend_params* fp, const
                               int32_t* problem_index, int64_t* n_corr, int32_t* const* corr, int32_t* const* cliques,
                               float* global_scale, const tzr_icp_params* icp, tzr_icp_result* icp_results,
                               int icp_mode = kIcpPointToPoint, double icp_epsilon = 0,
-                              const tzr_robust_kernel* icp_kernel = nullptr) {
+                              const tzr_robust_kernel* icp_kernel = nullptr, const MultiwayOut* mw = nullptr) {
   if (!ctx || !fp || !params || n_clouds < 1 || !n || !pts || P < 1 || !pair_clouds || !solutions || !status ||
       !n_corr || !(fp->normal_search_radius > 0) || !(fp->fpfh_search_radius > 0))
     return TZR_ERR_INVALID_ARG;
   if (icp && (!icp_params_ok(icp) || !icp_results)) return TZR_ERR_INVALID_ARG;
+  if (mw && (!icp || params->estimate_scaling || !mw->uncertain || !pg_params_ok(mw->pg) || !mw->information ||
+             !mw->info_counts || !mw->edge_weights || !mw->edge_mask || !mw->poses || !mw->pg_status))
+    return TZR_ERR_INVALID_ARG;
   if (icp && icp_mode == kIcpGeneralized && !icp_epsilon_ok(icp_epsilon)) return TZR_ERR_INVALID_ARG;
   for (int c = 0; c < n_clouds; ++c)
     if (n[c] <= 0 || !pts[c]) return TZR_ERR_INVALID_ARG;
@@ -2185,9 +2465,11 @@ static int register_pairs_run(tzr_ctx* ctx, const tzr_frontend_params* fp, const
     iplan.relative_fitness = icp->relative_fitness;
     iplan.relative_rmse = icp->relative_rmse;
   }
+  // with the multiway step: [information | counts] of the refined pairs read back
   const size_t hi_prob = al256(pin_base), hi_cl = hi_prob + al256((size_t)P * sizeof(IcpProb)),
                hi_ck = hi_cl + al256((size_t)n_clouds * sizeof(FpfhCloud)), hi_end = hi_ck + (size_t)i_chunks * 4,
-               pin_bytes = icp ? hi_end : pin_base;
+               hi_info = al256(hi_end), hi_icnt = hi_info + al256((size_t)P * 36 * 8),
+               pin_bytes = mw ? hi_icnt + (size_t)P * 4 : icp ? hi_end : pin_base;
   int rc;
   if ((rc = ensure(ctx, ctx->m_in, in_bytes)) != TZR_OK) return rc;
   if ((rc = ensure(ctx, ctx->m_scratch, scratch_bytes)) != TZR_OK) return rc;
@@ -2329,7 +2611,8 @@ static int register_pairs_run(tzr_ctx* ctx, const tzr_frontend_params* fp, const
     const size_t o_prob = 0, o_cl = al256(pb), o_ck = o_cl + al256(cb), o_match = o_ck + al256(kb),
                  o_part = o_match + al256((size_t)m_lo * 4),
                  o_grid = o_part + al256((size_t)c_lo * icp_partial_stride(icp_mode) * 8),
-                 total = o_grid + iplan.grid.grid_bytes;
+                 o_info = al256(o_grid + iplan.grid.grid_bytes), o_icnt = o_info + al256((size_t)S * 36 * 8),
+                 total = mw ? o_icnt + (size_t)S * 4 : o_grid + iplan.grid.grid_bytes;
     if ((rc = ensure(ctx, ctx->icp, total)) != TZR_OK) return rc;
     char* di = (char*)ctx->icp.p;
     CK(cudaMemcpyAsync(di + o_prob, hi_probs, pb, cudaMemcpyHostToDevice, st));
@@ -2340,11 +2623,21 @@ static int register_pairs_run(tzr_ctx* ctx, const tzr_frontend_params* fp, const
     // viewpoint at the origin), still in m_out: nothing after the FPFH stage writes that region, and they share the
     // cloud table's indexing
     const float4* d_nrm = (const float4*)(d_out + o_nrm);
+    IcpGrid grid{nullptr, nullptr, nullptr};
     ctx->launches += launch_icp(iplan, d_pts, d_pts, d_nrm, d_nrm, (IcpProb*)(di + o_prob), (FpfhCloud*)(di + o_cl),
                                 (const int*)(di + o_ck), (int*)(di + o_match), (double*)(di + o_part),
-                                iplan.grid.grid_bytes ? di + o_grid : nullptr, st);
+                                iplan.grid.grid_bytes ? di + o_grid : nullptr, st, &grid);
     if ((rc = check_launch(ctx, "icp launch")) != TZR_OK) return rc;
     CK(cudaMemcpyAsync(hi_probs, di + o_prob, pb, cudaMemcpyDeviceToHost, st));
+    if (mw) {  // the information matrices at the refined transforms, from the clouds and the problem table in place
+      ctx->launches += launch_icp_information(iplan, d_pts, d_pts, (IcpProb*)(di + o_prob), (FpfhCloud*)(di + o_cl),
+                                              (const int*)(di + o_ck), (int*)(di + o_match), (double*)(di + o_part),
+                                              iplan.grid.grid_bytes ? di + o_grid : nullptr, true,
+                                              (double*)(di + o_info), (int*)(di + o_icnt), st, &grid);
+      if ((rc = check_launch(ctx, "information launch")) != TZR_OK) return rc;
+      CK(cudaMemcpyAsync(h + hi_info, di + o_info, (size_t)S * 36 * 8, cudaMemcpyDeviceToHost, st));
+      CK(cudaMemcpyAsync(h + hi_icnt, di + o_icnt, (size_t)S * 4, cudaMemcpyDeviceToHost, st));
+    }
   }
   // synchronisation 2: the records, and the index pairs and cliques that were asked for
   if (S > 0) CK(cudaMemcpyAsync(h + h_sol, d_sol, (size_t)S * sizeof(tzr_solution), cudaMemcpyDeviceToHost, st));
@@ -2369,6 +2662,45 @@ static int register_pairs_run(tzr_ctx* ctx, const tzr_frontend_params* fp, const
   if (icp) {
     for (int p = 0; p < P; ++p) memset(&icp_results[p], 0, sizeof(tzr_icp_result));
     for (int k = 0; k < S; ++k) icp_result_of(hi_probs[k], &icp_results[solved[k]]);
+  }
+  if (mw) {  // the pose graph over the refined pairs, in pair order
+    memset(mw->information, 0, (size_t)P * 36 * 8);
+    memset(mw->info_counts, 0, (size_t)P * 4);
+    memset(mw->edge_weights, 0, (size_t)P * 8);
+    memset(mw->edge_mask, 0, (size_t)P);
+    memset(mw->poses, 0, (size_t)n_clouds * sizeof(tzr_similarity));
+    std::vector<int> edge_pair;
+    std::vector<int32_t> ends, unc;
+    std::vector<tzr_similarity> Tsd;
+    for (int k = 0; k < S; ++k) {
+      if (!hi_probs[k].seeded) continue;
+      const int p = solved[k];
+      memcpy(mw->information + (size_t)p * 36, h + hi_info + (size_t)k * 36 * 8, 36 * 8);
+      mw->info_counts[p] = ((const int*)(h + hi_icnt))[k];
+      edge_pair.push_back(p);
+      ends.push_back(pair_clouds[2 * p]);
+      ends.push_back(pair_clouds[2 * p + 1]);
+      unc.push_back(mw->uncertain[p]);
+      Tsd.push_back(icp_results[p].transform);
+    }
+    const int E = (int)edge_pair.size();
+    std::vector<double> L((size_t)std::max(E, 1) * 36), w(std::max(E, 1));
+    std::vector<uint8_t> m(std::max(E, 1));
+    for (int e = 0; e < E; ++e) memcpy(&L[(size_t)e * 36], mw->information + (size_t)edge_pair[e] * 36, 36 * 8);
+    const std::string reg_error = ctx->last_error;
+    *mw->pg_status = pose_graph_run(ctx, mw->pg, n_clouds, E, ends.data(), Tsd.data(), L.data(), unc.data(), nullptr,
+                                    mw->poses, w.data(), m.data(), nullptr, mw->summary);
+    if (*mw->pg_status == TZR_OK) {
+      for (int e = 0; e < E; ++e) {
+        mw->edge_weights[edge_pair[e]] = w[e];
+        mw->edge_mask[edge_pair[e]] = m[e];
+      }
+    } else {
+      memset(mw->poses, 0, (size_t)n_clouds * sizeof(tzr_similarity));
+      if (mw->summary) memset(mw->summary, 0, sizeof(*mw->summary));
+      if (*mw->pg_status == TZR_ERR_CUDA) return TZR_ERR_CUDA;
+    }
+    if (no_room || too_large) ctx->last_error = reg_error;
   }
   if (no_room) {
     ctx->last_error = "COMPLETE TIM graph of this clique does not fit the rotation workspace";
@@ -2659,6 +2991,143 @@ int tzr_icp_generalized(tzr_ctx* ctx, const tzr_icp_params* params, double epsil
                         const tzr_similarity* init, tzr_icp_result* result, int32_t* corr) {
   return icp_single(ctx, params, kIcpGeneralized, src, ns, src_normals, dst, nd, dst_normals, epsilon, init, result,
                     corr);
+}
+
+// tzr_information_matrix(_batch): the sources, targets and tables staged in one copy (tzr_icp_batch's layout), the
+// search and the sums (launch_icp_information), one read-back
+int tzr_information_matrix_batch(tzr_ctx* ctx, int B, const int32_t* ns, const float* const* src, const int32_t* nd,
+                                 const float* const* dst, const tzr_similarity* transforms,
+                                 double max_correspondence_distance, double* information, int32_t* counts) {
+  const double r = max_correspondence_distance;
+  if (!ctx || B < 1 || !ns || !src || !nd || !dst || !transforms || !information || !(r > 0) || !std::isfinite(r))
+    return TZR_ERR_INVALID_ARG;
+  long long NS = 0, ND = 0, chunks = 0;
+  for (int b = 0; b < B; ++b) {
+    if (ns[b] < 1 || nd[b] < 1 || !src[b] || !dst[b]) return TZR_ERR_INVALID_ARG;
+    const tzr_similarity& s = transforms[b];
+    bool finite = std::isfinite(s.scale) && s.scale > 0;
+    for (int k = 0; k < 9; ++k) finite &= std::isfinite(s.rotation[k]) != 0;
+    for (int k = 0; k < 3; ++k) finite &= std::isfinite(s.translation[k]) != 0;
+    if (!finite) return TZR_ERR_INVALID_ARG;
+    NS += ns[b];
+    ND += nd[b];
+    chunks += (ns[b] + kIcpChunk - 1) / kIcpChunk;
+  }
+  if (NS > 0x7fffffffll || ND > 0x7fffffffll) {
+    ctx->last_error = "the batch's points do not fit 32-bit indices";
+    return TZR_ERR_TOO_LARGE;
+  }
+  IcpPlan plan;
+  plan.B = B;
+  plan.NS = (int)NS;
+  plan.ND = (int)ND;
+  plan.chunks = (int)chunks;
+  plan.r2 = r * r;
+  std::vector<FpfhCloud> clouds((size_t)B);
+  const int route = (ctx->flags & 33554432u) ? kFpfhRouteBrute : (ctx->flags & 67108864u) ? kFpfhRouteGrid : kFpfhRouteAuto;
+  if (fpfh_plan(B, nd, r, r, route, clouds.data(), &plan.grid, kIcpGridMinN) != TZR_OK) {
+    ctx->last_error = "the batch's target grid does not fit 32-bit indices";
+    return TZR_ERR_TOO_LARGE;
+  }
+  std::vector<IcpProb> probs((size_t)B);
+  std::vector<int> chunk_prob((size_t)chunks);
+  {
+    int s_lo = 0, c_lo = 0;
+    for (int b = 0; b < B; ++b) {
+      IcpProb& pr = probs[b];
+      pr = IcpProb{};
+      pr.s_lo = s_lo;
+      pr.ns = ns[b];
+      pr.d_lo = clouds[b].lo;
+      pr.nd = nd[b];
+      pr.c_lo = c_lo;
+      pr.m_lo = s_lo;
+      pr.tc = b;
+      pr.active = pr.seeded = 1;
+      pr.s = transforms[b].scale;
+      for (int k = 0; k < 9; ++k) pr.R[k] = transforms[b].rotation[k];
+      for (int k = 0; k < 3; ++k) pr.t[k] = transforms[b].translation[k];
+      const int nc = (ns[b] + kIcpChunk - 1) / kIcpChunk;
+      for (int c = 0; c < nc; ++c) chunk_prob[c_lo + c] = b;
+      s_lo += ns[b];
+      c_lo += nc;
+    }
+  }
+  cudaSetDevice(ctx->device);
+  cudaStream_t st = ctx->stream;
+  // [sources | targets | problems | target clouds | chunk table] staged, then the matches, the partials, the grid
+  // scratch, the information matrices and the counts
+  const size_t sb = (size_t)NS * 12, db = (size_t)ND * 12, pb = (size_t)B * sizeof(IcpProb),
+               cb = (size_t)B * sizeof(FpfhCloud), kb = (size_t)chunks * 4;
+  const size_t o_dst = al256(sb), o_prob = o_dst + al256(db), o_cl = o_prob + al256(pb), o_ck = o_cl + al256(cb),
+               in_bytes = o_ck + kb, o_match = al256(in_bytes), o_part = o_match + al256((size_t)NS * 4),
+               o_grid = o_part + al256((size_t)chunks * kIcpInfoSums * 8), o_info = al256(o_grid + plan.grid.grid_bytes),
+               o_cnt = o_info + al256((size_t)B * 36 * 8), total = o_cnt + (size_t)B * 4;
+  int rc;
+  if ((rc = ensure(ctx, ctx->icp, total)) != TZR_OK) return rc;
+  std::vector<char> h(in_bytes);
+  for (int b = 0; b < B; ++b) {
+    memcpy(h.data() + (size_t)probs[b].s_lo * 12, src[b], (size_t)ns[b] * 12);
+    memcpy(h.data() + o_dst + (size_t)probs[b].d_lo * 12, dst[b], (size_t)nd[b] * 12);
+  }
+  memcpy(h.data() + o_prob, probs.data(), pb);
+  memcpy(h.data() + o_cl, clouds.data(), cb);
+  memcpy(h.data() + o_ck, chunk_prob.data(), kb);
+  char* d = (char*)ctx->icp.p;
+  CK(cudaMemcpyAsync(d, h.data(), in_bytes, cudaMemcpyHostToDevice, st));
+  ctx->launches += launch_icp_information(plan, (const float*)d, (const float*)(d + o_dst), (IcpProb*)(d + o_prob),
+                                          (FpfhCloud*)(d + o_cl), (const int*)(d + o_ck), (int*)(d + o_match),
+                                          (double*)(d + o_part), plan.grid.grid_bytes ? d + o_grid : nullptr, false,
+                                          (double*)(d + o_info), (int*)(d + o_cnt), st);
+  if ((rc = check_launch(ctx, "information launch")) != TZR_OK) return rc;
+  std::vector<int32_t> cnt((size_t)B);
+  CK(cudaMemcpyAsync(information, d + o_info, (size_t)B * 36 * 8, cudaMemcpyDeviceToHost, st));
+  CK(cudaMemcpyAsync(cnt.data(), d + o_cnt, (size_t)B * 4, cudaMemcpyDeviceToHost, st));
+  CK(cudaStreamSynchronize(st));
+  if (counts) memcpy(counts, cnt.data(), (size_t)B * 4);
+  return TZR_OK;
+}
+
+int tzr_information_matrix(tzr_ctx* ctx, const float* src, int ns, const float* dst, int nd,
+                           const tzr_similarity* transform, double max_correspondence_distance, double* information,
+                           int32_t* count) {
+  return tzr_information_matrix_batch(ctx, 1, &ns, &src, &nd, &dst, transform, max_correspondence_distance,
+                                      information, count);
+}
+
+void tzr_pose_graph_params_default(tzr_pose_graph_params* p) {
+  if (!p) return;
+  memset(p, 0, sizeof(*p));
+  p->max_correspondence_distance = 0;  // no default (the caller's ICP distance)
+  p->gnc_factor = 1.4;
+  p->cost_threshold = 1e-6;
+  p->max_iterations = 100;
+  p->max_inner_iterations = 10;
+  p->reference_node = 0;
+}
+
+int tzr_pose_graph_optimize(tzr_ctx* ctx, const tzr_pose_graph_params* params, int K, int E, const int32_t* edges,
+                            const tzr_similarity* edge_transforms, const double* information, const int32_t* uncertain,
+                            const tzr_similarity* initial_poses, tzr_similarity* poses, double* weights,
+                            uint8_t* inlier_mask, double* residuals, tzr_pose_graph_summary* summary) {
+  return pose_graph_run(ctx, params, K, E, edges, edge_transforms, information, uncertain, initial_poses, poses,
+                        weights, inlier_mask, residuals, summary);
+}
+
+int tzr_register_cloud_pairs_multiway(tzr_ctx* ctx, const tzr_frontend_params* fp, const tzr_params* params,
+                                      int n_clouds, const int32_t* n, const float* const* pts, int P,
+                                      const int32_t* pair_clouds, const uint64_t* tuple_seeds,
+                                      tzr_solution* solutions, int32_t* status, int32_t* problem_index,
+                                      int64_t* n_corr, int32_t* const* corr, int32_t* const* cliques,
+                                      float* global_scale, const tzr_icp_params* icp, tzr_icp_result* icp_results,
+                                      const int32_t* uncertain, const tzr_pose_graph_params* pg, double* information,
+                                      int32_t* info_counts, double* edge_weights, uint8_t* edge_mask,
+                                      tzr_similarity* poses, tzr_pose_graph_summary* pg_summary, int32_t* pg_status) {
+  if (!icp) return TZR_ERR_INVALID_ARG;
+  const MultiwayOut mw{uncertain, pg, information, info_counts, edge_weights, edge_mask, poses, pg_summary, pg_status};
+  return register_pairs_run(ctx, fp, params, n_clouds, n, pts, P, pair_clouds, tuple_seeds, solutions, status,
+                            problem_index, n_corr, corr, cliques, global_scale, icp, icp_results, kIcpPointToPlane, 0,
+                            nullptr, &mw);
 }
 
 // tzr_voxel_downsample(_batch): the clouds staged back to back (one H2D copy), the batch's launches (launch_voxel), a

@@ -52,6 +52,12 @@ struct Cusolver {
   cusolverStatus_t (*syev_batched)(cusolverDnHandle_t, cusolverDnParams_t, cusolverEigMode_t, cublasFillMode_t,
                                    int64_t, cudaDataType, void*, int64_t, cudaDataType, void*, cudaDataType, void*,
                                    size_t, void*, size_t, int*, int64_t) = nullptr;
+  // dense Cholesky of the pose graph's normal equations (pose_graph.cu, DESIGN.md §3.16)
+  cusolverStatus_t (*potrf_buf)(cusolverDnHandle_t, cublasFillMode_t, int, double*, int, int*) = nullptr;
+  cusolverStatus_t (*potrf)(cusolverDnHandle_t, cublasFillMode_t, int, double*, int, double*, int, int*) = nullptr;
+  cusolverStatus_t (*potrs)(cusolverDnHandle_t, cublasFillMode_t, int, int, const double*, int, double*, int,
+                            int*) = nullptr;
+  bool cholesky = false;
   bool batched = false;
   bool ok = false;
   std::string err;
@@ -79,6 +85,10 @@ Cusolver& cusolver() {
     s.syev_batched_buf = (decltype(s.syev_batched_buf))dlsym(s.lib, "cusolverDnXsyevBatched_bufferSize");
     s.syev_batched = (decltype(s.syev_batched))dlsym(s.lib, "cusolverDnXsyevBatched");
     s.batched = s.create_params && s.destroy_params && s.syev_batched_buf && s.syev_batched;
+    s.potrf_buf = (decltype(s.potrf_buf))dlsym(s.lib, "cusolverDnDpotrf_bufferSize");
+    s.potrf = (decltype(s.potrf))dlsym(s.lib, "cusolverDnDpotrf");
+    s.potrs = (decltype(s.potrs))dlsym(s.lib, "cusolverDnDpotrs");
+    s.cholesky = s.potrf_buf && s.potrf && s.potrs;
     s.ok = s.create && s.destroy && s.set_stream && s.syevd_buf && s.syevd;
     if (!s.ok) s.err = "libcusolver lacks the Dsyevd entry points";
     return s;
@@ -1107,6 +1117,37 @@ int certify_batch_device(CertMode mode, const tzr_certifier_params& prm, int B, 
       }
     }
     b0 = b1;
+  }
+  return TZR_OK;
+}
+
+int dense_cholesky_setup(void** solver_handle, int n, double* A, int* lwork, cudaStream_t st, std::string* err) {
+  Cusolver& cs = cusolver();
+  if (!cs.ok || !cs.cholesky) {
+    *err = cs.ok ? "libcusolver lacks the Dpotrf / Dpotrs entry points" : cs.err;
+    return TZR_ERR_UNSUPPORTED;
+  }
+  cusolverDnHandle_t& handle = *reinterpret_cast<cusolverDnHandle_t*>(solver_handle);  // owned by the context
+  if (!handle && cs.create(&handle) != CUSOLVER_STATUS_SUCCESS) {
+    *err = "cusolverDnCreate failed";
+    return TZR_ERR_CUDA;
+  }
+  cs.set_stream(handle, st);
+  if (cs.potrf_buf(handle, CUBLAS_FILL_MODE_LOWER, n, A, n, lwork) != CUSOLVER_STATUS_SUCCESS) {
+    *err = "cusolverDnDpotrf_bufferSize failed";
+    return TZR_ERR_CUDA;
+  }
+  return TZR_OK;
+}
+
+int dense_cholesky_solve(void* solver_handle, int n, double* A, double* b, double* work, int lwork, int* info,
+                         std::string* err) {
+  Cusolver& cs = cusolver();
+  cusolverDnHandle_t handle = (cusolverDnHandle_t)solver_handle;
+  if (cs.potrf(handle, CUBLAS_FILL_MODE_LOWER, n, A, n, work, lwork, info) != CUSOLVER_STATUS_SUCCESS ||
+      cs.potrs(handle, CUBLAS_FILL_MODE_LOWER, n, 1, A, n, b, n, info + 1) != CUSOLVER_STATUS_SUCCESS) {
+    *err = "cusolverDnDpotrf / cusolverDnDpotrs failed";
+    return TZR_ERR_CUDA;
   }
   return TZR_OK;
 }

@@ -18,6 +18,9 @@
 //   icp_update_kernel  one warp per problem: combines it, runs rotation_from_H (the rotation stage's SVD and reflection
 //                      fix), and composes the update into (R, t).
 //
+// Information matrices (DESIGN.md §3.16) reuse the grid build and icp_nn_kernel as they are, then sum the 21 entries of
+// G^T G per correspondence in icp_info_kernel and combine them per problem in icp_info_combine_kernel.
+//
 // Every reduction runs in an order fixed by the problem's own points (chunk k of a problem always holds its points
 // [256 k, 256 k + 256), and the chunks of a problem are combined by lane k mod 32 then a butterfly), so a problem's
 // bits do not depend on the batch it runs in.  Finished problems return at once from every kernel.  The iterations are
@@ -678,7 +681,87 @@ __global__ void icp_seed_kernel(IcpProb* probs, int B, const tzr_solution* __res
   for (int k = 0; k < 3; ++k) pr.t[k] = s.translation[k];
 }
 
+// ---- information matrices (DESIGN.md §3.16) -----------------------------------------------------------------------
+// Open3D's GetInformationMatrixFromPointClouds: one CTA per chunk; each correspondence (i, j) of the stored matches adds
+// G^T G with q = y_j (the target point) and G = [-[q]x | I] (3 x 6, ordering (omega, tau)), its 21 upper entries row by
+// row, each ((G(0,a) G(0,b) + G(1,a) G(1,b)) + G(2,a) G(2,b)).  Entry 20 (Lambda(5,5)) is the correspondence count.
+// A problem that was not seeded (a chained pair without a valid record) adds nothing.
+__global__ void __launch_bounds__(kIcpThreads) icp_info_kernel(IcpArgs a) {
+  __shared__ double s_buf[(kIcpThreads / 32) * kIcpInfoSums];
+  const int c = blockIdx.x;
+  const IcpProb& pr = a.probs[a.chunk_prob[c]];
+  if (!pr.seeded) return;
+  const int i = (c - pr.c_lo) * kIcpChunk + threadIdx.x;
+  double v[kIcpInfoSums];
+#pragma unroll
+  for (int k = 0; k < kIcpInfoSums; ++k) v[k] = 0.0;
+  const int j = i < pr.ns ? a.match[pr.m_lo + i] : -1;
+  if (j >= 0) {
+    const size_t o = 3 * (size_t)(pr.d_lo + j);
+    const double x = a.dst[o], y = a.dst[o + 1], z = a.dst[o + 2];
+    const double G[3][6] = {{0.0, z, -y, 1.0, 0.0, 0.0}, {-z, 0.0, x, 0.0, 1.0, 0.0}, {y, -x, 0.0, 0.0, 0.0, 1.0}};
+    int k = 0;
+#pragma unroll
+    for (int row = 0; row < 6; ++row)
+#pragma unroll
+      for (int col = row; col < 6; ++col)
+        v[k++] = (G[0][row] * G[0][col] + G[1][row] * G[1][col]) + G[2][row] * G[2][col];
+  }
+  icp_block_sum<kIcpInfoSums>(v, s_buf, a.partial + kIcpInfoSums * (size_t)c);
+}
+
+// One warp per problem: the chunk sums in ICP's fixed order, mirrored into 36 doubles (row-major, symmetric), and the
+// count; zeros for a problem that was not seeded
+__global__ void icp_info_combine_kernel(IcpArgs a, double* __restrict__ info, int* __restrict__ counts) {
+  const IcpProb& pr = a.probs[blockIdx.x];
+  double v[kIcpInfoSums];
+  if (pr.seeded) {
+    icp_warp_combine<kIcpInfoSums, kIcpInfoSums>(a.partial, pr.c_lo, (pr.ns + kIcpChunk - 1) / kIcpChunk, v);
+  } else {
+#pragma unroll
+    for (int k = 0; k < kIcpInfoSums; ++k) v[k] = 0.0;
+  }
+  if (threadIdx.x != 0) return;
+  double* L = info + 36 * (size_t)blockIdx.x;
+  int k = 0;
+  for (int row = 0; row < 6; ++row)
+    for (int col = row; col < 6; ++col) {
+      L[6 * row + col] = v[k];
+      L[6 * col + row] = v[k];
+      ++k;
+    }
+  counts[blockIdx.x] = (int)v[kIcpInfoSums - 1];
+}
+
+// a chained call's problems run their search once more after ICP finished them: active again where seeded
+__global__ void icp_info_seed_kernel(IcpProb* probs, int B) {
+  const int b = blockIdx.x * blockDim.x + threadIdx.x;
+  if (b < B) probs[b].active = probs[b].seeded;
+}
+
 }  // namespace
+
+int launch_icp_information(const IcpPlan& plan, const float* src, const float* dst, IcpProb* probs, FpfhCloud* clouds,
+                           const int* chunk_prob, int* match, double* partial, void* grid_scratch, bool reseed,
+                           double* info, int* counts, cudaStream_t st, const IcpGrid* grid) {
+  int nl = 0;
+  IcpArgs a{src, dst, probs, clouds, chunk_prob, match, partial, nullptr, nullptr, nullptr, plan.r2};
+  if (reseed) {
+    icp_info_seed_kernel<<<(plan.B + 127) / 128, 128, 0, st>>>(probs, plan.B);
+    ++nl;
+  }
+  if (grid) {  // launch_icp's grid over the same targets, still in grid_scratch
+    a.sorted = grid->sorted;
+    a.bstart = grid->bstart;
+    a.bend = grid->bend;
+  } else if (plan.grid.any_grid) {
+    nl += launch_fpfh_grid(plan.grid, dst, clouds, grid_scratch, st, &a.sorted, &a.bstart, &a.bend);
+  }
+  icp_nn_kernel<<<plan.chunks, kIcpThreads, 0, st>>>(a);
+  icp_info_kernel<<<plan.chunks, kIcpThreads, 0, st>>>(a);
+  icp_info_combine_kernel<<<plan.B, 32, 0, st>>>(a, info, counts);
+  return nl + 3;
+}
 
 int launch_icp_seed(IcpProb* probs, int B, const tzr_solution* sol, cudaStream_t st) {
   icp_seed_kernel<<<(B + 127) / 128, 128, 0, st>>>(probs, B, sol);
@@ -687,10 +770,11 @@ int launch_icp_seed(IcpProb* probs, int B, const tzr_solution* sol, cudaStream_t
 
 int launch_icp(const IcpPlan& plan, const float* src, const float* dst, const float4* src_normals,
                const float4* dst_normals, IcpProb* probs, FpfhCloud* clouds, const int* chunk_prob, int* match,
-               double* partial, void* grid_scratch, cudaStream_t st) {
+               double* partial, void* grid_scratch, cudaStream_t st, IcpGrid* grid_out) {
   int nl = 0;
   IcpArgs a{src, dst, probs, clouds, chunk_prob, match, partial, nullptr, nullptr, nullptr, plan.r2};
   if (plan.grid.any_grid) nl += launch_fpfh_grid(plan.grid, dst, clouds, grid_scratch, st, &a.sorted, &a.bstart, &a.bend);
+  if (grid_out) *grid_out = IcpGrid{a.sorted, a.bstart, a.bend};
   icp_nn_kernel<<<plan.chunks, kIcpThreads, 0, st>>>(a);
   icp_eval_kernel<<<plan.B, 32, 0, st>>>(a, plan.max_iteration, plan.relative_fitness, plan.relative_rmse);
   nl += 2;

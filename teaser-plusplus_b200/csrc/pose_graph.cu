@@ -1,0 +1,410 @@
+// Robust pose-graph optimisation (tzr_pose_graph_optimize, DESIGN.md §3.16): Open3D's multiway-registration step with
+// GNC-TLS in place of its line process, written out as this project's own definition in include/teaser_b200.h.  One
+// graph per call; the host runs the GNC-TLS iterations and reads back PgState once per iteration, and every inner
+// Levenberg-Marquardt iteration is enqueued without a synchronisation:
+//
+//   pg_edge_kernel      one thread per edge: the residual e = (log R_E, t_E) of E = T_d^-1 T_s T_sd^-1 at the current or
+//                       the candidate poses, e^T Lambda e, r-bar, and the Jacobian terms A^T Lambda A and A^T Lambda e
+//                       with A = Ad(T_d^-1).
+//   pg_cost_kernel      one warp: the weighted cost sum w_e e^T Lambda e in a fixed order; starts the inner solve (mode
+//                       0) or decides on a candidate step (mode 1: accept or reject, the damping, the stop test).
+//   pg_assemble_kernel  one warp per listed 6 x 6 block of H (lower triangle) or 6-row block of the right-hand side:
+//                       its contributions in ascending edge index, in the order the host planned, so no atomics and no
+//                       dependence on scheduling; the diagonal carries the damping.
+//   (cuSOLVER)          cusolverDnDpotrf + cusolverDnDpotrs on the dense (K - 1) 6-row system.
+//   pg_update_kernel    one thread per node: the candidate pose Exp(delta_k) T_k.
+//   pg_gnc_kernel       one warp: the GNC-TLS weight update of the uncertain edges from r-bar, the rotation stage's
+//                       schedule.
+//
+// Everything is IEEE float64 with no FMA contraction (the library's -fmad=false).
+#include "tzr_internal.cuh"
+
+namespace tzr {
+
+namespace {
+
+constexpr double kPgLambda0 = 1e-4;      // initial damping of every inner solve
+constexpr double kPgLambdaMax = 1e8;     // a rejection that raises the damping past this ends the inner solve
+constexpr double kPgRelTol = 1e-10;      // |cost - candidate cost| <= kPgRelTol cost + floor ends the inner solve
+
+// c = a b for 3 x 3 column-major matrices; entry (r, k): (a(r,0) b(0,k) + a(r,1) b(1,k)) + a(r,2) b(2,k)
+__device__ __forceinline__ void m33(const double* a, const double* b, double* c) {
+#pragma unroll
+  for (int k = 0; k < 3; ++k)
+#pragma unroll
+    for (int r = 0; r < 3; ++r) c[3 * k + r] = (a[r] * b[3 * k] + a[3 + r] * b[3 * k + 1]) + a[6 + r] * b[3 * k + 2];
+}
+// c = a^T b
+__device__ __forceinline__ void m33_tn(const double* a, const double* b, double* c) {
+#pragma unroll
+  for (int k = 0; k < 3; ++k)
+#pragma unroll
+    for (int r = 0; r < 3; ++r)
+      c[3 * k + r] = (a[3 * r] * b[3 * k] + a[3 * r + 1] * b[3 * k + 1]) + a[3 * r + 2] * b[3 * k + 2];
+}
+// c = a b^T
+__device__ __forceinline__ void m33_nt(const double* a, const double* b, double* c) {
+#pragma unroll
+  for (int k = 0; k < 3; ++k)
+#pragma unroll
+    for (int r = 0; r < 3; ++r) c[3 * k + r] = (a[r] * b[k] + a[3 + r] * b[3 + k]) + a[6 + r] * b[6 + k];
+}
+// y = a x, y = a^T x
+__device__ __forceinline__ void mv3(const double* a, const double* x, double* y) {
+#pragma unroll
+  for (int r = 0; r < 3; ++r) y[r] = (a[r] * x[0] + a[3 + r] * x[1]) + a[6 + r] * x[2];
+}
+__device__ __forceinline__ void mtv3(const double* a, const double* x, double* y) {
+#pragma unroll
+  for (int r = 0; r < 3; ++r) y[r] = (a[3 * r] * x[0] + a[3 * r + 1] * x[1]) + a[3 * r + 2] * x[2];
+}
+
+// omega = log(R) (column-major R), include/teaser_b200.h: v = vee(R - R^T) / 2, c = (tr R - 1) / 2,
+// theta = atan2(|v|, c); theta < 1e-5: omega = (1 + theta^2 / 6) v; c < -0.9: the axis from the symmetric part
+// (its largest diagonal's column) with the sign of v; otherwise omega = (theta / |v|) v
+__device__ void so3_log(const double* R, double w[3]) {
+  const double v[3] = {0.5 * (R[5] - R[7]), 0.5 * (R[6] - R[2]), 0.5 * (R[1] - R[3])};
+  const double s = sqrt((v[0] * v[0] + v[1] * v[1]) + v[2] * v[2]);
+  const double c = 0.5 * (((R[0] + R[4]) + R[8]) - 1.0);
+  const double th = atan2(s, c);
+  if (th < 1e-5) {
+    const double f = 1.0 + th * th / 6.0;
+#pragma unroll
+    for (int k = 0; k < 3; ++k) w[k] = f * v[k];
+  } else if (c < -0.9) {
+    double B[9];
+#pragma unroll
+    for (int k = 0; k < 3; ++k)
+#pragma unroll
+      for (int r = 0; r < 3; ++r) B[3 * k + r] = 0.5 * (R[3 * k + r] + R[3 * r + k]) - (r == k ? c : 0.0);
+    int k = 0;
+    if (B[4] > B[0]) k = 1;
+    if (B[8] > B[4 * k]) k = 2;
+    const double nrm = sqrt(B[4 * k] * (1.0 - c));
+    double a[3] = {B[3 * k] / nrm, B[3 * k + 1] / nrm, B[3 * k + 2] / nrm};
+    if ((a[0] * v[0] + a[1] * v[1]) + a[2] * v[2] < 0.0)
+#pragma unroll
+      for (int r = 0; r < 3; ++r) a[r] = -a[r];
+#pragma unroll
+    for (int r = 0; r < 3; ++r) w[r] = th * a[r];
+  } else {
+    const double f = th / s;
+#pragma unroll
+    for (int k = 0; k < 3; ++k) w[k] = f * v[k];
+  }
+}
+
+// (R, t) = Exp(w, tau) in SE(3): R = I + b [w]x + a' [w]x^2 (Rodrigues), t = V tau with V = I + b' [w]x + c' [w]x^2;
+// theta = |w| < 1e-5 takes the series a' = 1/2 - theta^2/24, b = 1 - theta^2/6, b' = 1/2 - theta^2/24,
+// c' = 1/6 - theta^2/120
+__device__ void se3_exp(const double w[3], const double tau[3], double R[9], double t[3]) {
+  const double th2 = (w[0] * w[0] + w[1] * w[1]) + w[2] * w[2];
+  const double th = sqrt(th2);
+  double A, Bq, Vb, Vc;
+  if (th < 1e-5) {
+    A = 1.0 - th2 / 6.0;
+    Bq = 0.5 - th2 / 24.0;
+    Vb = 0.5 - th2 / 24.0;
+    Vc = 1.0 / 6.0 - th2 / 120.0;
+  } else {
+    const double sn = sin(th), cs = cos(th);
+    A = sn / th;
+    Bq = (1.0 - cs) / th2;
+    Vb = Bq;
+    Vc = (th - sn) / (th2 * th);
+  }
+  // W = [w]x, W2 = W W (column-major)
+  const double W[9] = {0.0, w[2], -w[1], -w[2], 0.0, w[0], w[1], -w[0], 0.0};
+  double W2[9];
+  m33(W, W, W2);
+#pragma unroll
+  for (int k = 0; k < 9; ++k) {
+    const double I = (k == 0 || k == 4 || k == 8) ? 1.0 : 0.0;
+    R[k] = (I + A * W[k]) + Bq * W2[k];
+  }
+  double V[9];
+#pragma unroll
+  for (int k = 0; k < 9; ++k) {
+    const double I = (k == 0 || k == 4 || k == 8) ? 1.0 : 0.0;
+    V[k] = (I + Vb * W[k]) + Vc * W2[k];
+  }
+  mv3(V, tau, t);
+}
+
+__device__ __forceinline__ double* pose_at(const PgDev& dv, int K, int buf, int k) {
+  return dv.poses + 12 * ((size_t)buf * K + k);
+}
+__device__ __forceinline__ double* term_at(const PgDev& dv, int E, int buf, int e) {
+  return dv.eterm + kPgTermStride * ((size_t)buf * E + e);
+}
+
+// which = 0: the current poses into the current terms; 1: the candidate poses (the other buffer), skipped once the
+// inner solve has stopped
+__global__ void pg_edge_kernel(PgDev dv, int K, int E, int which) {
+  const int e = blockIdx.x * blockDim.x + threadIdx.x;
+  if (e >= E) return;
+  const PgState& st = *dv.state;
+  if (which == 1 && st.done) return;
+  const int buf = which == 0 ? st.cur : 1 - st.cur;
+  const PgEdge& ed = dv.edges[e];
+  const double* Ts = pose_at(dv, K, buf, ed.s);
+  const double* Td = pose_at(dv, K, buf, ed.d);
+  // R_E = R_d^T (R_s R_sd^T), t_E = R_d^T ((t_s - t_d) - (R_s R_sd^T) t_sd)
+  double Q[9], RE[9], u[3], w[3], tE[3];
+  m33_nt(Ts, ed.R, Q);
+  m33_tn(Td, Q, RE);
+  mv3(Q, ed.t, u);
+#pragma unroll
+  for (int r = 0; r < 3; ++r) w[r] = (Ts[9 + r] - Td[9 + r]) - u[r];
+  mtv3(Td, w, tE);
+  double err[6];
+  so3_log(RE, err);
+  err[3] = tE[0];
+  err[4] = tE[1];
+  err[5] = tE[2];
+  // Le = Lambda e, c = e^T Lambda e
+  double Le[6];
+#pragma unroll
+  for (int r = 0; r < 6; ++r) {
+    double a = 0.0;
+#pragma unroll
+    for (int k = 0; k < 6; ++k) a = a + ed.L[6 * r + k] * err[k];
+    Le[r] = a;
+  }
+  double c = 0.0;
+#pragma unroll
+  for (int k = 0; k < 6; ++k) c = c + err[k] * Le[k];
+  // A = Ad(T_d^-1) = [[Rt, 0], [[p]x Rt, Rt]] with Rt = R_d^T, p = -R_d^T t_d
+  double p[3], Rt[9];
+  mtv3(Td, Td + 9, p);
+#pragma unroll
+  for (int r = 0; r < 3; ++r) p[r] = -p[r];
+#pragma unroll
+  for (int k = 0; k < 3; ++k)
+#pragma unroll
+    for (int r = 0; r < 3; ++r) Rt[3 * k + r] = Td[3 * r + k];
+  const double P[9] = {0.0, p[2], -p[1], -p[2], 0.0, p[0], p[1], -p[0], 0.0};
+  double PR[9];
+  m33(P, Rt, PR);
+  double A[6][6];  // A[row][col]
+#pragma unroll
+  for (int r = 0; r < 3; ++r)
+#pragma unroll
+    for (int k = 0; k < 3; ++k) {
+      A[r][k] = Rt[3 * k + r];
+      A[r][3 + k] = 0.0;
+      A[3 + r][k] = PR[3 * k + r];
+      A[3 + r][3 + k] = Rt[3 * k + r];
+    }
+  double* out = term_at(dv, E, buf, e);
+  // LA = Lambda A; M = A^T (Lambda A), v = A^T Le
+  double LA[6][6];
+#pragma unroll
+  for (int r = 0; r < 6; ++r)
+#pragma unroll
+    for (int k = 0; k < 6; ++k) {
+      double a = 0.0;
+#pragma unroll
+      for (int q = 0; q < 6; ++q) a = a + ed.L[6 * r + q] * A[q][k];
+      LA[r][k] = a;
+    }
+#pragma unroll
+  for (int r = 0; r < 6; ++r) {
+#pragma unroll
+    for (int k = 0; k < 6; ++k) {
+      double a = 0.0;
+#pragma unroll
+      for (int q = 0; q < 6; ++q) a = a + A[q][r] * LA[q][k];
+      out[6 * r + k] = a;
+    }
+    double a = 0.0;
+#pragma unroll
+    for (int q = 0; q < 6; ++q) a = a + A[q][r] * Le[q];
+    out[36 + r] = a;
+  }
+  out[42] = c;
+  out[43] = c * ed.inv_norm;
+}
+
+// The fixed-order weighted sum over one warp: lane l adds w_e x_e for e = l, l + 32, ... in turn, then a butterfly
+__device__ double pg_warp_sum(const PgDev& dv, int E, int buf) {
+  double a = 0.0;
+  for (int e = threadIdx.x; e < E; e += 32) a = a + dv.weight[e] * term_at(dv, E, buf, e)[42];
+  for (int o = 16; o; o >>= 1) a += __shfl_xor_sync(0xffffffffu, a, o);
+  return a;
+}
+
+// mode 0: start the inner solve at the current poses; mode 1: decide on the candidate (include/teaser_b200.h states
+// the rule)
+__global__ void pg_cost_kernel(PgDev dv, int E, int mode, double cost_floor) {
+  PgState& st = *dv.state;
+  if (mode == 0) {
+    const double cost = pg_warp_sum(dv, E, st.cur);
+    if (threadIdx.x != 0) return;
+    st.cost = cost;
+    st.lambda = kPgLambda0;
+    st.done = 0;
+    st.inner = 0;
+    return;
+  }
+  if (st.done) return;
+  const double cand = pg_warp_sum(dv, E, 1 - st.cur);
+  if (threadIdx.x != 0) return;
+  st.cand_cost = cand;
+  st.inner += 1;
+  const bool ok = st.info[0] == 0 && st.info[1] == 0 && isfinite(cand);
+  if (ok && fabs(st.cost - cand) <= kPgRelTol * st.cost + cost_floor) {
+    if (cand < st.cost) {
+      st.cur = 1 - st.cur;
+      st.cost = cand;
+    }
+    st.done = 1;
+  } else if (ok && cand < st.cost) {
+    st.cur = 1 - st.cur;
+    st.cost = cand;
+    st.lambda = st.lambda * 0.1;
+  } else {
+    st.lambda = st.lambda * 10.0;
+    if (st.lambda > kPgLambdaMax) st.done = 1;
+  }
+}
+
+// One warp per listed block.  H block (bi, bj), bi >= bj: entry (r, k) = sum over its terms of sign * (w_e M_e(r, k))
+// in the listed order, then on a diagonal block's diagonal a + lambda (a + 1): the additive part keeps the damped system
+// positive definite when a node's every edge has weight 0 (its block of H is then 0); H is column-major n x n and
+// only its lower triangle is read.  Right-hand-side block bi (bj = -1): -(sum of sign * (w_e v_e(r))).
+__global__ void pg_assemble_kernel(PgDev dv, int E, int n, int nblocks) {
+  const int b = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
+  const int lane = threadIdx.x & 31;
+  if (b >= nblocks) return;
+  const PgState& st = *dv.state;
+  if (st.done) return;
+  const PgBlock bl = dv.blocks[b];
+  const int cur = st.cur;
+  if (bl.bj < 0) {
+    if (lane >= 6) return;
+    double a = 0.0;
+    for (int q = bl.lo; q < bl.hi; ++q) {
+      const PgTerm tm = dv.terms[q];
+      a = a + (double)tm.sign * (dv.weight[tm.e] * term_at(dv, E, cur, tm.e)[36 + lane]);
+    }
+    dv.g[6 * bl.bi + lane] = -a;
+    return;
+  }
+  for (int l = lane; l < 36; l += 32) {
+    const int r = l / 6, k = l % 6;
+    double a = 0.0;
+    for (int q = bl.lo; q < bl.hi; ++q) {
+      const PgTerm tm = dv.terms[q];
+      a = a + (double)tm.sign * (dv.weight[tm.e] * term_at(dv, E, cur, tm.e)[6 * r + k]);
+    }
+    if (bl.bi == bl.bj && r == k) a = a + st.lambda * (a + 1.0);
+    dv.H[(size_t)(6 * bl.bi + r) + (size_t)(6 * bl.bj + k) * (size_t)n] = a;
+  }
+}
+
+// One thread per node: the candidate T_k' = Exp(delta_k) T_k (R' = R_x R, t' = R_x t + t_x); the reference node keeps
+// its pose
+__global__ void pg_update_kernel(PgDev dv, int K, int ref) {
+  const int k = blockIdx.x * blockDim.x + threadIdx.x;
+  if (k >= K) return;
+  const PgState& st = *dv.state;
+  if (st.done) return;
+  const double* T = pose_at(dv, K, st.cur, k);
+  double* Tn = pose_at(dv, K, 1 - st.cur, k);
+  if (k == ref) {
+    for (int q = 0; q < 12; ++q) Tn[q] = T[q];
+    return;
+  }
+  const double* x = dv.g + 6 * (k < ref ? k : k - 1);
+  double Rx[9], tx[3], u[3];
+  se3_exp(x, x + 3, Rx, tx);
+  m33(Rx, T, Tn);
+  mv3(Rx, T + 9, u);
+#pragma unroll
+  for (int r = 0; r < 3; ++r) Tn[9 + r] = u[r] + tx[r];
+}
+
+// GNC-TLS after GNC iteration `iter` (the rotation stage's schedule on r-bar, include/teaser_b200.h).  The weight
+// formula is a copy of gnc_tls_block's (rot_trans.cu), not a shared function: sharing it would move the rotation
+// kernels' code, which must stay as it is, and this one reads a normalised residual (noise bound 1) from one warp.
+__global__ void pg_gnc_kernel(PgDev dv, int E, int iter, double gnc_factor, double cost_threshold) {
+  PgState& st = *dv.state;
+  const int lane = threadIdx.x;
+  const int cur = st.cur;
+  int n_unc = 0;
+  double rmax = 0.0;
+  for (int e = lane; e < E; e += 32)
+    if (dv.edges[e].uncertain) {
+      ++n_unc;
+      rmax = fmax(rmax, term_at(dv, E, cur, e)[43]);
+    }
+  for (int o = 16; o; o >>= 1) {
+    n_unc += __shfl_xor_sync(0xffffffffu, n_unc, o);
+    rmax = fmax(rmax, __shfl_xor_sync(0xffffffffu, rmax, o));
+  }
+  if (n_unc == 0) {  // every edge certain: no GNC step
+    if (lane == 0) st.stop = 1;
+    return;
+  }
+  double mu = st.mu;
+  if (iter == 0) {
+    mu = 1.0 / (2.0 * rmax - 1.0);
+    if (mu <= 0.0) {
+      if (lane == 0) {
+        st.mu = mu;
+        st.stop = 1;
+      }
+      return;
+    }
+  }
+  const double th1 = (mu + 1.0) / mu;
+  const double th2 = mu / (mu + 1.0);
+  double c = 0.0;
+  for (int e = lane; e < E; e += 32) {
+    if (!dv.edges[e].uncertain) continue;
+    const double r = term_at(dv, E, cur, e)[43];
+    c = c + dv.weight[e] * r;
+    double wn;
+    if (r >= th1)
+      wn = 0.0;
+    else if (r <= th2)
+      wn = 1.0;
+    else
+      wn = sqrt(mu * (mu + 1.0) / r) - mu;
+    dv.weight[e] = wn;
+  }
+  for (int o = 16; o; o >>= 1) c += __shfl_xor_sync(0xffffffffu, c, o);
+  if (lane != 0) return;
+  const double diff = fabs(c - st.gnc_cost);
+  st.mu = mu * gnc_factor;
+  st.gnc_cost = c;
+  if (diff < cost_threshold) st.stop = 1;
+}
+
+}  // namespace
+
+int launch_pose_graph_begin(const PgPlan& plan, const PgDev& dv, double cost_floor, cudaStream_t st) {
+  pg_edge_kernel<<<(plan.E + 127) / 128, 128, 0, st>>>(dv, plan.K, plan.E, 0);
+  pg_cost_kernel<<<1, 32, 0, st>>>(dv, plan.E, 0, cost_floor);
+  return 2;
+}
+
+int launch_pose_graph_assemble(const PgPlan& plan, const PgDev& dv, cudaStream_t st) {
+  pg_assemble_kernel<<<(plan.blocks + 3) / 4, 128, 0, st>>>(dv, plan.E, plan.n, plan.blocks);
+  return 1;
+}
+
+int launch_pose_graph_step(const PgPlan& plan, const PgDev& dv, int ref, double cost_floor, cudaStream_t st) {
+  pg_update_kernel<<<(plan.K + 127) / 128, 128, 0, st>>>(dv, plan.K, ref);
+  pg_edge_kernel<<<(plan.E + 127) / 128, 128, 0, st>>>(dv, plan.K, plan.E, 1);
+  pg_cost_kernel<<<1, 32, 0, st>>>(dv, plan.E, 1, cost_floor);
+  return 3;
+}
+
+int launch_pose_graph_gnc(const PgPlan& plan, const PgDev& dv, int iter, cudaStream_t st) {
+  pg_gnc_kernel<<<1, 32, 0, st>>>(dv, plan.E, iter, plan.gnc_factor, plan.cost_threshold);
+  return 1;
+}
+
+}  // namespace tzr

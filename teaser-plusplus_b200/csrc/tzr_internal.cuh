@@ -474,12 +474,95 @@ struct IcpPlan {
 // correspondences), partial (chunks x icp_partial_stride(plan.mode) doubles), grid_scratch (plan.grid.grid_bytes): device
 // pointers.  Enqueues every iteration without synchronising; returns the launches: 4 for the grid build (when some target
 // uses it) + 2 + 4 * max_iteration, in every mode.
+// grid_out (may be nullptr): the target grid's sorted indices and bucket ranges inside grid_scratch (all nullptr without
+// grid targets), for launch_icp_information to reuse.
+struct IcpGrid {
+  const int* sorted;
+  const int* bstart;
+  const int* bend;
+};
 int launch_icp(const IcpPlan& plan, const float* src, const float* dst, const float4* src_normals,
                const float4* dst_normals, IcpProb* probs, FpfhCloud* clouds, const int* chunk_prob, int* match,
-               double* partial, void* grid_scratch, cudaStream_t st);
+               double* partial, void* grid_scratch, cudaStream_t st, IcpGrid* grid_out = nullptr);
 // The seeds of B problems from B solution records (tzr_register_cloud_pairs_icp): a valid record with a finite transform
 // and a positive scale sets (s, R, t) and active = seeded = 1, any other leaves the problem inactive.  One launch.
 int launch_icp_seed(IcpProb* probs, int B, const tzr_solution* sol, cudaStream_t st);
+// Information matrices (tzr_information_matrix_batch, DESIGN.md §3.16) of B problems at their current transforms: the
+// grid build (when some target uses it), icp_nn_kernel as launch_icp runs it, then the 21 sums of G^T G per chunk into
+// partial (chunks x kIcpInfoSums doubles) and their fixed-order combination into info (B x 36 doubles, device) and
+// counts (B ints, device).  reseed: set active = seeded first (a chained call, after launch_icp finished its problems);
+// otherwise the problems must be active.  A problem that is not seeded gets zeros.  grid (may be nullptr): launch_icp's
+// grid of the same targets, reused instead of built again.  Returns the launches: 3, + 1 with reseed, + 4 for the grid
+// build when some target uses the grid and grid is nullptr.
+constexpr int kIcpInfoSums = 21;
+int launch_icp_information(const IcpPlan& plan, const float* src, const float* dst, IcpProb* probs, FpfhCloud* clouds,
+                           const int* chunk_prob, int* match, double* partial, void* grid_scratch, bool reseed,
+                           double* info, int* counts, cudaStream_t st, const IcpGrid* grid = nullptr);
+
+// pose_graph.cu (tzr_pose_graph_optimize, DESIGN.md §3.16): one graph of K nodes and E edges, device-resident
+struct PgEdge {         // one per edge; the host fills it, the kernels read it
+  int s, d;             // source and target node
+  int fs, fd;           // their free-node index (-1: the reference node)
+  int uncertain;        // 1: the edge takes part in GNC-TLS
+  int pad;
+  double R[9], t[3];    // T_sd (column-major R)
+  double L[36];         // Lambda_e (row-major)
+  double inv_norm;      // 1 / (c^2 Lambda_e(5,5)), 0 when Lambda_e(5,5) = 0
+};
+struct PgState {        // the solve's device-side state, read back once per GNC iteration
+  double lambda;        // Levenberg-Marquardt damping
+  double cost;          // sum w_e e^T Lambda_e e at the current poses
+  double cand_cost;     // the same at the candidate poses
+  double mu, gnc_cost;  // GNC-TLS: the control parameter and the previous weighted residual sum
+  int cur;              // which of the two pose / edge-term buffers holds the current poses
+  int done;             // 1: the inner solve has stopped
+  int inner;            // inner iterations of this GNC iteration
+  int stop;             // 1: GNC-TLS has stopped
+  int info[2];          // potrf / potrs status of the latest step
+};
+struct PgPlan {
+  int K = 0, E = 0, n = 0;        // nodes, edges, rows of the normal equations (6 (K - 1))
+  int blocks = 0;                 // 6 x 6 blocks of H's lower triangle with some contribution
+  int max_inner = 0;              // inner iterations enqueued per GNC iteration
+  double gnc_factor = 1.4, cost_threshold = 1e-6;
+};
+struct PgBlock {        // one 6 x 6 block (bi >= bj) of H's lower triangle, or the gradient block bi (bj = -1)
+  int bi, bj;
+  int lo, hi;           // its contributions [lo, hi) in the plan's term list, ascending edge index
+};
+struct PgTerm {         // one contribution: edge e with sign +1 / -1
+  int e, sign;
+};
+// The buffers of launch_pose_graph_*: device pointers.  poses: 2 buffers of K x 12 doubles (R column-major, t); eterm:
+// 2 buffers of E x kPgTermStride doubles; weight: E; H: n x n column-major; g: n; state: one PgState.
+struct PgDev {
+  const PgEdge* edges;
+  const PgBlock* blocks;
+  const PgTerm* terms;
+  double* poses;
+  double* eterm;
+  double* weight;
+  double* H;
+  double* g;
+  PgState* state;
+};
+constexpr int kPgTermStride = 44;  // doubles per edge in eterm: A^T Lambda A (36), A^T Lambda e (6), e^T Lambda e, r-bar
+// Evaluates every edge at the current poses and starts the inner solve (its cost, damping and flags).  Returns the
+// launches (2).
+int launch_pose_graph_begin(const PgPlan& plan, const PgDev& dv, double cost_floor, cudaStream_t st);
+// The damped H (lower triangle, every listed block; the caller clears H first) and the right-hand side -g of one inner
+// iteration.  Returns the launches (1).
+int launch_pose_graph_assemble(const PgPlan& plan, const PgDev& dv, cudaStream_t st);
+// The candidate poses from the solved step, their edge terms and the accept / reject decision.  Returns the launches (3).
+int launch_pose_graph_step(const PgPlan& plan, const PgDev& dv, int ref, double cost_floor, cudaStream_t st);
+// GNC-TLS weight update after GNC iteration `iter`.  Returns the launches (1).
+int launch_pose_graph_gnc(const PgPlan& plan, const PgDev& dv, int iter, cudaStream_t st);
+// dense Cholesky through the lazily loaded cuSOLVER (certify.cu): handle and workspace size of an n x n lower factor;
+// TZR_ERR_UNSUPPORTED when cuSOLVER cannot be loaded
+int dense_cholesky_setup(void** solver_handle, int n, double* A, int* lwork, cudaStream_t st, std::string* err);
+// potrf of A (lower, in place) and potrs of b (in place); info[0] / info[1] (device) their status
+int dense_cholesky_solve(void* solver_handle, int n, double* A, double* b, double* work, int lwork, int* info,
+                         std::string* err);
 
 // voxel.cu (voxel-grid downsampling, DESIGN.md §3.12): B clouds stored back to back
 constexpr unsigned long long kVoxNone = 1ull << 62;  // sort key of a point in no voxel: above every voxel key (< 2^62)

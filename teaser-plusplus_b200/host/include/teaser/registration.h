@@ -70,6 +70,16 @@ struct RobustKernel {
   RobustKernel() = default;
   RobustKernel(Type type_, double k_ = 1.0) : type(type_), k(k_) {}
 };
+// The GNC-TLS pose graph of multiway registration (teaser/pose_graph.h, tzr_pose_graph_optimize): the distance c of
+// the normalised residual, the GNC-TLS schedule, the inner Levenberg-Marquardt iterations and the fixed node.
+struct PoseGraphParams {
+  double max_correspondence_distance = 0;  // no default: must be set (> 0), normally the ICP distance
+  double gnc_factor = 1.4;
+  double cost_threshold = 1e-6;
+  int max_iterations = 100;
+  int max_inner_iterations = 10;
+  int reference_node = 0;
+};
 struct PointToPointICPResult {
   RegistrationSolution solution;  // the refined transform; scale is the seed's, held fixed
   double fitness = 0;
@@ -374,6 +384,31 @@ class RobustRegistrationSolver {
                                                                 const CloudPairParams& params,
                                                                 const GeneralizedICPParams& icp,
                                                                 const RobustKernel& kernel);
+  // Multiway registration (tzr_register_cloud_pairs_multiway): solveCloudPairsPointToPlane, then the information
+  // matrix of every refined pair at its ICP transform and distance, then the GNC-TLS pose graph over the clouds with one
+  // edge per refined pair, in one device call.  uncertain: one flag per pair; the overload without it takes Open3D's
+  // tutorial rule, pair (k, k + 1) certain and every other pair uncertain.  estimate_scaling must be off (the pose
+  // graph is rigid).  information and weights are zero, inliers false, for a pair that is not an edge; poses (one per
+  // cloud, cloud into the world frame) are zero when pose_graph_status is not 0 (e.g. TZR_ERR_INVALID_ARG for a
+  // disconnected graph).
+  struct MultiwayResult {
+    std::vector<CloudPairICPResult> pairs;
+    std::vector<Eigen::Matrix<double, 6, 6>> information;
+    std::vector<int> information_counts;
+    std::vector<double> edge_weights;
+    std::vector<bool> edge_inliers;
+    std::vector<Eigen::Matrix4d> poses;
+    int pose_graph_status = 0;
+    int iterations = 0;
+    int inner_iterations = 0;
+    double cost = 0;
+  };
+  MultiwayResult solveMultiway(const std::vector<PointCloud>& clouds, const std::vector<std::pair<int, int>>& pairs,
+                               const CloudPairParams& params, const PointToPointICPParams& icp,
+                               const PoseGraphParams& pose_graph);
+  MultiwayResult solveMultiway(const std::vector<PointCloud>& clouds, const std::vector<std::pair<int, int>>& pairs,
+                               const CloudPairParams& params, const PointToPointICPParams& icp,
+                               const PoseGraphParams& pose_graph, const std::vector<bool>& uncertain);
   bool isMaxCliqueProvenOptimal() const { return clique_proven_; }
   long long getNumInlierGraphEdges() const { return n_edges_; }
   int getGNCRotationIterations() const { return gnc_iterations_; }

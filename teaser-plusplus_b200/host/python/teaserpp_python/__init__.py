@@ -12,9 +12,11 @@ from . import _teaserpp as _ext
 
 # ---- re-exports -----------------------------------------------------------------------------------------------------
 _PUBLIC = ("OMP_MAX_THREADS", "CertificationResult", "DRSCertifier", "EigSolverType", "GeneralizedICP",
-           "InlierGraphFormulation", "InlierSelectionMode", "PointToPlaneICP", "PointToPointICP", "RegistrationSolution",
-           "RobustKernel", "RobustRegistrationSolver", "RotationEstimationAlgorithm", "estimate_normals",
-           "estimate_normals_batch", "voxel_down_sample", "voxel_down_sample_batch")
+           "InlierGraphFormulation", "InlierSelectionMode", "PointToPlaneICP", "PointToPointICP", "PoseGraph",
+           "RegistrationSolution", "RobustKernel", "RobustRegistrationSolver", "RotationEstimationAlgorithm",
+           "estimate_normals",
+           "estimate_normals_batch", "information_matrix", "information_matrix_batch", "voxel_down_sample",
+           "voxel_down_sample_batch")
 globals().update({name: getattr(_ext, name) for name in _PUBLIC})
 
 # ---- v1.0 spellings of the enums, kept as class attributes ----------------------------------------------------------

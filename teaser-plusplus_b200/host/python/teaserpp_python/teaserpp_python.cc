@@ -12,6 +12,7 @@
 
 #include "teaser/certification.h"
 #include "teaser/icp.h"
+#include "teaser/pose_graph.h"
 #include "teaser/normals.h"
 #include "teaser/registration.h"
 #include "teaser/voxel.h"
@@ -98,6 +99,24 @@ py::dict icp_dict(const teaser::PointToPointICPResult& r) {
                   py::arg("inlier_rmse") = r.inlier_rmse, py::arg("iterations") = r.iterations,
                   py::arg("converged") = r.converged, py::arg("correspondences") = r.correspondences);
 }
+
+// (4,4) float64 matrices <-> Eigen::Matrix4d, (6,6) <-> teaser::Matrix6d
+template <int N>
+Eigen::Matrix<double, N, N> square_of(const py::array_t<double, py::array::c_style | py::array::forcecast>& a) {
+  if (a.ndim() != 2 || a.shape(0) != N || a.shape(1) != N) throw std::invalid_argument("expected a square matrix");
+  Eigen::Matrix<double, N, N> M;
+  for (int r = 0; r < N; ++r)
+    for (int c = 0; c < N; ++c) M(r, c) = a.at(r, c);
+  return M;
+}
+template <int N>
+py::array_t<double> square_to_numpy(const Eigen::Matrix<double, N, N>& M) {
+  py::array_t<double> out({static_cast<py::ssize_t>(N), static_cast<py::ssize_t>(N)});
+  for (int r = 0; r < N; ++r)
+    for (int c = 0; c < N; ++c) out.mutable_at(r, c) = M(r, c);
+  return out;
+}
+using SqArr = py::array_t<double, py::array::c_style | py::array::forcecast>;
 
 }  // namespace
 
@@ -194,6 +213,86 @@ PYBIND11_MODULE(_teaserpp, m) {
            py::arg("type"), py::arg("k") = 1.0)
       .def_readwrite("type", &teaser::RobustKernel::type)
       .def_readwrite("k", &teaser::RobustKernel::k);
+
+  // GPU extra: multiway registration (teaser/pose_graph.h): information matrices and the GNC-TLS pose graph
+  m.def(
+      "information_matrix",
+      [](const CloudArray& src, const CloudArray& dst, const teaser::RegistrationSolution& T,
+         double max_correspondence_distance) {
+        teaser::PointCloud s = cloud_of(src), d = cloud_of(dst);
+        int count = 0;
+        teaser::Matrix6d L;
+        {
+          py::gil_scoped_release release;
+          L = teaser::informationMatrix(s, d, T, max_correspondence_distance, &count);
+        }
+        return py::make_tuple(square_to_numpy<6>(L), count);
+      },
+      py::arg("src"), py::arg("dst"), py::arg("transform"), py::arg("max_correspondence_distance"));
+  m.def(
+      "information_matrix_batch",
+      [](const std::vector<CloudArray>& src, const std::vector<CloudArray>& dst,
+         const std::vector<teaser::RegistrationSolution>& T, double max_correspondence_distance) {
+        std::vector<teaser::PointCloud> s, d;
+        for (const auto& a : src) s.push_back(cloud_of(a));
+        for (const auto& a : dst) d.push_back(cloud_of(a));
+        std::vector<int> counts;
+        std::vector<teaser::Matrix6d> L;
+        {
+          py::gil_scoped_release release;
+          L = teaser::informationMatrixBatch(s, d, T, max_correspondence_distance, &counts);
+        }
+        py::list out;
+        for (const auto& M : L) out.append(square_to_numpy<6>(M));
+        return py::make_tuple(out, counts);
+      },
+      py::arg("src"), py::arg("dst"), py::arg("transforms"), py::arg("max_correspondence_distance"));
+  py::class_<teaser::PoseGraph>(m, "PoseGraph")
+      .def(py::init([](double max_correspondence_distance, double gnc_factor, double cost_threshold,
+                       int max_iterations, int max_inner_iterations, int reference_node) {
+             teaser::PoseGraph::Params p;
+             p.max_correspondence_distance = max_correspondence_distance;
+             p.gnc_factor = gnc_factor;
+             p.cost_threshold = cost_threshold;
+             p.max_iterations = max_iterations;
+             p.max_inner_iterations = max_inner_iterations;
+             p.reference_node = reference_node;
+             return teaser::PoseGraph(p);
+           }),
+           py::arg("max_correspondence_distance"), py::arg("gnc_factor") = 1.4, py::arg("cost_threshold") = 1e-6,
+           py::arg("max_iterations") = 100, py::arg("max_inner_iterations") = 10, py::arg("reference_node") = 0)
+      .def(
+          "optimize",
+          [](const teaser::PoseGraph& g, int num_nodes, const std::vector<std::pair<int, int>>& edges,
+             const std::vector<SqArr>& transforms, const std::vector<SqArr>& information,
+             const std::vector<bool>& uncertain, const py::object& initial_poses) {
+            if (transforms.size() != edges.size() || information.size() != edges.size() ||
+                (!uncertain.empty() && uncertain.size() != edges.size()))
+              throw std::invalid_argument("one transform, information matrix (and uncertain flag) per edge");
+            std::vector<teaser::PoseGraph::Edge> E(edges.size());
+            for (size_t e = 0; e < edges.size(); ++e) {
+              E[e].source = edges[e].first;
+              E[e].target = edges[e].second;
+              E[e].transform = square_of<4>(transforms[e]);
+              E[e].information = square_of<6>(information[e]);
+              E[e].uncertain = !uncertain.empty() && uncertain[e];
+            }
+            std::vector<Eigen::Matrix4d> init;
+            if (!initial_poses.is_none())
+              for (const auto& a : initial_poses.cast<std::vector<SqArr>>()) init.push_back(square_of<4>(a));
+            teaser::PoseGraph::Result r;
+            {
+              py::gil_scoped_release release;
+              r = g.optimize(num_nodes, E, initial_poses.is_none() ? nullptr : &init);
+            }
+            py::list poses;
+            for (const auto& T : r.poses) poses.append(square_to_numpy<4>(T));
+            return py::dict(py::arg("poses") = poses, py::arg("weights") = r.weights, py::arg("inliers") = r.inliers,
+                            py::arg("residuals") = r.residuals, py::arg("iterations") = r.iterations,
+                            py::arg("inner_iterations") = r.inner_iterations, py::arg("cost") = r.cost);
+          },
+          py::arg("num_nodes"), py::arg("edges"), py::arg("transforms"), py::arg("information"),
+          py::arg("uncertain") = std::vector<bool>(), py::arg("initial_poses") = py::none());
 
   // GPU extra: point-to-plane ICP (teaser::PointToPlaneICP), given the target normals
   py::class_<teaser::PointToPlaneICP>(m, "PointToPlaneICP")
@@ -508,6 +607,66 @@ PYBIND11_MODULE(_teaserpp, m) {
            py::arg("fpfh_search_radius") = 0.05, py::arg("use_absolute_scale") = true, py::arg("use_crosscheck") = true,
            py::arg("use_tuple_test") = true, py::arg("tuple_scale") = 0.0f, py::arg("tuple_seed") = 0x7ea5e2ull,
            py::arg("method") = "point_to_point", py::arg("epsilon") = 1e-3, py::arg("kernel") = py::none())
+      .def(
+          "solve_multiway",
+          [](Solver& s, const std::vector<CloudArray>& clouds, const std::vector<std::pair<int, int>>& pairs,
+             double max_correspondence_distance, const py::object& uncertain, int max_iteration,
+             double relative_fitness, double relative_rmse, double normal_search_radius, double fpfh_search_radius,
+             bool use_absolute_scale, bool use_crosscheck, bool use_tuple_test, float tuple_scale,
+             uint64_t tuple_seed, double gnc_factor, double cost_threshold, int max_iterations,
+             int max_inner_iterations, int reference_node) {
+            // GPU extra: solve_cloud_pairs_icp(method="point_to_plane"), information matrices and the GNC-TLS pose
+            // graph in one call (solveMultiway); uncertain None: pair (k, k + 1) certain, every other pair uncertain
+            std::vector<teaser::PointCloud> pcs;
+            for (const auto& a : clouds) pcs.push_back(cloud_of(a));
+            Solver::CloudPairParams cp;
+            cp.normal_search_radius = normal_search_radius;
+            cp.fpfh_search_radius = fpfh_search_radius;
+            cp.use_absolute_scale = use_absolute_scale;
+            cp.use_crosscheck = use_crosscheck;
+            cp.use_tuple_test = use_tuple_test;
+            cp.tuple_scale = tuple_scale;
+            cp.tuple_seed = tuple_seed;
+            teaser::PointToPointICPParams ip;
+            ip.max_correspondence_distance = max_correspondence_distance;
+            ip.max_iteration = max_iteration;
+            ip.relative_fitness = relative_fitness;
+            ip.relative_rmse = relative_rmse;
+            teaser::PoseGraphParams pg;
+            pg.max_correspondence_distance = max_correspondence_distance;
+            pg.gnc_factor = gnc_factor;
+            pg.cost_threshold = cost_threshold;
+            pg.max_iterations = max_iterations;
+            pg.max_inner_iterations = max_inner_iterations;
+            pg.reference_node = reference_node;
+            const bool given = !uncertain.is_none();
+            const std::vector<bool> unc = given ? uncertain.cast<std::vector<bool>>() : std::vector<bool>();
+            Solver::MultiwayResult r;
+            {
+              py::gil_scoped_release release;
+              r = given ? s.solveMultiway(pcs, pairs, cp, ip, pg, unc) : s.solveMultiway(pcs, pairs, cp, ip, pg);
+            }
+            py::list pair_out, info, poses;
+            for (const auto& q : r.pairs)
+              pair_out.append(py::dict(py::arg("status") = q.status, py::arg("solution") = q.solution,
+                                       py::arg("refined") = q.refined,
+                                       py::arg("icp") = q.refined ? py::object(icp_dict(q.icp)) : py::object(py::none())));
+            for (const auto& M : r.information) info.append(square_to_numpy<6>(M));
+            for (const auto& T : r.poses) poses.append(square_to_numpy<4>(T));
+            return py::dict(py::arg("pairs") = pair_out, py::arg("information") = info,
+                            py::arg("information_counts") = r.information_counts,
+                            py::arg("edge_weights") = r.edge_weights, py::arg("edge_inliers") = r.edge_inliers,
+                            py::arg("poses") = poses, py::arg("pose_graph_status") = r.pose_graph_status,
+                            py::arg("iterations") = r.iterations, py::arg("inner_iterations") = r.inner_iterations,
+                            py::arg("cost") = r.cost);
+          },
+          py::arg("clouds"), py::arg("pairs"), py::arg("max_correspondence_distance"), py::arg("uncertain") = py::none(),
+          py::arg("max_iteration") = 30, py::arg("relative_fitness") = 1e-6, py::arg("relative_rmse") = 1e-6,
+          py::arg("normal_search_radius") = 0.03, py::arg("fpfh_search_radius") = 0.05,
+          py::arg("use_absolute_scale") = true, py::arg("use_crosscheck") = true, py::arg("use_tuple_test") = true,
+          py::arg("tuple_scale") = 0.0f, py::arg("tuple_seed") = 0x7ea5e2ull, py::arg("gnc_factor") = 1.4,
+          py::arg("cost_threshold") = 1e-6, py::arg("max_iterations") = 100, py::arg("max_inner_iterations") = 10,
+          py::arg("reference_node") = 0)
       .def_property_readonly("solution", &Solver::getSolution)
       .def("getSolution", &Solver::getSolution)
       .def_property_readonly("gnc_rotation_cost_at_termination", &Solver::getGNCRotationCostAtTermination)

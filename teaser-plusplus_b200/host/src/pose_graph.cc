@@ -1,0 +1,153 @@
+// teaser::informationMatrix(Batch) and teaser::PoseGraph (teaser/pose_graph.h) on top of the C-ABI: marshalling only,
+// the sums and the solve run in libteaser_b200.so.
+#include "teaser/pose_graph.h"
+
+#include <cstring>
+#include <stdexcept>
+#include <string>
+
+#include "teaser_b200.h"
+
+namespace teaser {
+
+tzr_ctx* b200_context();  // registration.cc: one context per host thread
+
+namespace {
+
+[[noreturn]] void fail(const char* who, int rc, tzr_ctx* ctx) {
+  throw std::runtime_error(std::string(who) + ": " + tzr_status_string(rc) + ": " + tzr_last_error(ctx));
+}
+
+tzr_similarity sim_of(const RegistrationSolution& s) {
+  tzr_similarity c;
+  c.scale = s.scale;
+  std::memcpy(c.rotation, s.rotation.data(), sizeof(c.rotation));
+  for (int k = 0; k < 3; ++k) c.translation[k] = s.translation(k);
+  return c;
+}
+
+tzr_similarity sim_of(const Eigen::Matrix4d& T) {
+  tzr_similarity c;
+  c.scale = 1.0;
+  for (int r = 0; r < 3; ++r) {
+    for (int col = 0; col < 3; ++col) c.rotation[3 * col + r] = T(r, col);
+    c.translation[r] = T(r, 3);
+  }
+  return c;
+}
+
+Eigen::Matrix4d matrix_of(const tzr_similarity& s) {
+  Eigen::Matrix4d T = Eigen::Matrix4d::Zero();
+  for (int r = 0; r < 3; ++r) {
+    for (int c = 0; c < 3; ++c) T(r, c) = s.rotation[3 * c + r];
+    T(r, 3) = s.translation[r];
+  }
+  T(3, 3) = 1.0;
+  return T;
+}
+
+Matrix6d matrix6_of(const double* L) {
+  Matrix6d M;
+  for (int r = 0; r < 6; ++r)
+    for (int c = 0; c < 6; ++c) M(r, c) = L[6 * r + c];
+  return M;
+}
+
+}  // namespace
+
+std::vector<Matrix6d> informationMatrixBatch(const std::vector<PointCloud>& src, const std::vector<PointCloud>& dst,
+                                             const std::vector<RegistrationSolution>& T,
+                                             double max_correspondence_distance, std::vector<int>* counts) {
+  const size_t B = src.size();
+  if (dst.size() != B || T.size() != B)
+    throw std::invalid_argument("teaser::informationMatrixBatch: one target and one transform per source");
+  std::vector<Matrix6d> out(B);
+  if (counts) counts->assign(B, 0);
+  if (B == 0) return out;
+  static_assert(sizeof(PointXYZ) == 3 * sizeof(float), "PointXYZ must be three packed floats");
+  std::vector<int32_t> ns(B), nd(B), cnt(B);
+  std::vector<const float*> sp(B), dp(B);
+  std::vector<tzr_similarity> tr(B);
+  for (size_t b = 0; b < B; ++b) {
+    if (src[b].empty() || dst[b].empty())
+      throw std::invalid_argument("teaser::informationMatrixBatch: clouds must be non-empty");
+    ns[b] = static_cast<int32_t>(src[b].size());
+    nd[b] = static_cast<int32_t>(dst[b].size());
+    sp[b] = &src[b][0].x;
+    dp[b] = &dst[b][0].x;
+    tr[b] = sim_of(T[b]);
+  }
+  std::vector<double> L(36 * B);
+  tzr_ctx* ctx = b200_context();
+  const int rc = tzr_information_matrix_batch(ctx, static_cast<int>(B), ns.data(), sp.data(), nd.data(), dp.data(),
+                                              tr.data(), max_correspondence_distance, L.data(), cnt.data());
+  if (rc != TZR_OK) fail("teaser::informationMatrixBatch", rc, ctx);
+  for (size_t b = 0; b < B; ++b) {
+    out[b] = matrix6_of(&L[36 * b]);
+    if (counts) (*counts)[b] = cnt[b];
+  }
+  return out;
+}
+
+Matrix6d informationMatrix(const PointCloud& src, const PointCloud& dst, const RegistrationSolution& T,
+                           double max_correspondence_distance, int* count) {
+  if (src.empty() || dst.empty()) throw std::invalid_argument("teaser::informationMatrix: clouds must be non-empty");
+  const tzr_similarity tr = sim_of(T);
+  double L[36];
+  int32_t cnt = 0;
+  tzr_ctx* ctx = b200_context();
+  const int rc = tzr_information_matrix(ctx, &src[0].x, static_cast<int>(src.size()), &dst[0].x,
+                                        static_cast<int>(dst.size()), &tr, max_correspondence_distance, L, &cnt);
+  if (rc != TZR_OK) fail("teaser::informationMatrix", rc, ctx);
+  if (count) *count = cnt;
+  return matrix6_of(L);
+}
+
+PoseGraph::Result PoseGraph::optimize(int num_nodes, const std::vector<Edge>& edges,
+                                      const std::vector<Eigen::Matrix4d>* initial_poses) const {
+  const size_t E = edges.size();
+  if (initial_poses && initial_poses->size() != static_cast<size_t>(num_nodes))
+    throw std::invalid_argument("teaser::PoseGraph::optimize: one initial pose per node");
+  tzr_pose_graph_params p;
+  tzr_pose_graph_params_default(&p);
+  p.max_correspondence_distance = params_.max_correspondence_distance;
+  p.gnc_factor = params_.gnc_factor;
+  p.cost_threshold = params_.cost_threshold;
+  p.max_iterations = params_.max_iterations;
+  p.max_inner_iterations = params_.max_inner_iterations;
+  p.reference_node = params_.reference_node;
+  std::vector<int32_t> ends(2 * E), unc(E);
+  std::vector<tzr_similarity> tr(E);
+  std::vector<double> L(36 * E);
+  for (size_t e = 0; e < E; ++e) {
+    ends[2 * e] = edges[e].source;
+    ends[2 * e + 1] = edges[e].target;
+    unc[e] = edges[e].uncertain ? 1 : 0;
+    tr[e] = sim_of(edges[e].transform);
+    for (int r = 0; r < 6; ++r)
+      for (int c = 0; c < 6; ++c) L[36 * e + 6 * r + c] = edges[e].information(r, c);
+  }
+  std::vector<tzr_similarity> init;
+  if (initial_poses)
+    for (const Eigen::Matrix4d& T : *initial_poses) init.push_back(sim_of(T));
+  std::vector<tzr_similarity> poses(num_nodes > 0 ? num_nodes : 1);
+  std::vector<double> w(E ? E : 1), res(E ? E : 1);
+  std::vector<uint8_t> mask(E ? E : 1);
+  tzr_pose_graph_summary summary{};
+  tzr_ctx* ctx = b200_context();
+  const int rc = tzr_pose_graph_optimize(ctx, &p, num_nodes, static_cast<int>(E), ends.data(), tr.data(), L.data(),
+                                         unc.data(), initial_poses ? init.data() : nullptr, poses.data(), w.data(),
+                                         mask.data(), res.data(), &summary);
+  if (rc != TZR_OK) fail("teaser::PoseGraph::optimize", rc, ctx);
+  Result out;
+  for (int k = 0; k < num_nodes; ++k) out.poses.push_back(matrix_of(poses[k]));
+  out.weights.assign(w.begin(), w.begin() + E);
+  for (size_t e = 0; e < E; ++e) out.inliers.push_back(mask[e] != 0);
+  out.residuals.assign(res.begin(), res.begin() + E);
+  out.iterations = summary.iterations;
+  out.inner_iterations = summary.inner_iterations;
+  out.cost = summary.cost;
+  return out;
+}
+
+}  // namespace teaser

@@ -634,11 +634,23 @@ namespace {
 // solveCloudPairs' body: tzr_register_cloud_pairs, or tzr_register_cloud_pairs_icp(_point_to_plane, _generalized) when
 // icp is given (icp_res then receives P records)
 enum class IcpMethod { kPointToPoint, kPointToPlane, kGeneralized };
+// the multiway step's inputs and outputs (solveMultiway: tzr_register_cloud_pairs_multiway, point-to-plane)
+struct MultiwayCall {
+  const int32_t* uncertain;
+  const tzr_pose_graph_params* pg;
+  double* information;
+  int32_t* info_counts;
+  double* edge_weights;
+  uint8_t* edge_mask;
+  tzr_similarity* poses;
+  tzr_pose_graph_summary* summary;
+  int32_t* pg_status;
+};
 std::vector<RobustRegistrationSolver::CloudPairResult> run_cloud_pairs(
     const tzr_params& p, const std::vector<PointCloud>& clouds, const std::vector<std::pair<int, int>>& pairs,
     const RobustRegistrationSolver::CloudPairParams& cp, const tzr_icp_params* icp,
     std::vector<tzr_icp_result>* icp_res, IcpMethod method = IcpMethod::kPointToPoint, double epsilon = 0,
-    const RobustKernel* kernel = nullptr) {
+    const RobustKernel* kernel = nullptr, const MultiwayCall* mw = nullptr) {
   using CloudPairResult = RobustRegistrationSolver::CloudPairResult;
   const int K = static_cast<int>(clouds.size()), P = static_cast<int>(pairs.size());
   std::vector<CloudPairResult> out(P);
@@ -685,7 +697,13 @@ std::vector<RobustRegistrationSolver::CloudPairResult> run_cloud_pairs(
                                   scales.data());
   } else {
     icp_res->assign(P, tzr_icp_result{});
-    if (kernel) {
+    if (mw) {
+      rc = tzr_register_cloud_pairs_multiway(ctx, &f, &p, K, n.data(), pts.data(), P, pc.data(), seeds.data(),
+                                             sols.data(), status.data(), index.data(), n_corr.data(), corr_p.data(),
+                                             clq_p.data(), scales.data(), icp, icp_res->data(), mw->uncertain, mw->pg,
+                                             mw->information, mw->info_counts, mw->edge_weights, mw->edge_mask,
+                                             mw->poses, mw->summary, mw->pg_status);
+    } else if (kernel) {
       tzr_robust_kernel k;
       std::memset(&k, 0, sizeof(k));
       k.type = static_cast<int32_t>(kernel->type);
@@ -751,6 +769,76 @@ static std::vector<RobustRegistrationSolver::CloudPairICPResult> run_cloud_pairs
     out[q].refined = out[q].status == TZR_OK && out[q].solution.valid && res[q].transform.scale > 0;
     if (out[q].refined) icp_result_from_c(res[q], nullptr, &out[q].icp);
   }
+  return out;
+}
+
+RobustRegistrationSolver::MultiwayResult RobustRegistrationSolver::solveMultiway(
+    const std::vector<PointCloud>& clouds, const std::vector<std::pair<int, int>>& pairs, const CloudPairParams& cp,
+    const PointToPointICPParams& icp, const PoseGraphParams& pose_graph) {
+  std::vector<bool> uncertain(pairs.size());
+  for (size_t q = 0; q < pairs.size(); ++q) uncertain[q] = pairs[q].second != pairs[q].first + 1;  // Open3D's tutorial
+  return solveMultiway(clouds, pairs, cp, icp, pose_graph, uncertain);
+}
+
+RobustRegistrationSolver::MultiwayResult RobustRegistrationSolver::solveMultiway(
+    const std::vector<PointCloud>& clouds, const std::vector<std::pair<int, int>>& pairs, const CloudPairParams& cp,
+    const PointToPointICPParams& icp, const PoseGraphParams& pose_graph, const std::vector<bool>& uncertain) {
+  const size_t P = pairs.size(), K = clouds.size();
+  if (uncertain.size() != P) throw std::invalid_argument("teaser: solveMultiway: one uncertain flag per pair");
+  tzr_icp_params ip;
+  tzr_icp_params_default(&ip);
+  ip.max_correspondence_distance = icp.max_correspondence_distance;
+  ip.max_iteration = icp.max_iteration;
+  ip.relative_fitness = icp.relative_fitness;
+  ip.relative_rmse = icp.relative_rmse;
+  tzr_pose_graph_params pg;
+  tzr_pose_graph_params_default(&pg);
+  pg.max_correspondence_distance = pose_graph.max_correspondence_distance;
+  pg.gnc_factor = pose_graph.gnc_factor;
+  pg.cost_threshold = pose_graph.cost_threshold;
+  pg.max_iterations = pose_graph.max_iterations;
+  pg.max_inner_iterations = pose_graph.max_inner_iterations;
+  pg.reference_node = pose_graph.reference_node;
+  std::vector<int32_t> unc(P), counts(P);
+  for (size_t q = 0; q < P; ++q) unc[q] = uncertain[q] ? 1 : 0;
+  std::vector<double> info(P * 36), w(P);
+  std::vector<uint8_t> mask(P);
+  std::vector<tzr_similarity> poses(K);
+  tzr_pose_graph_summary summary{};
+  int32_t pg_status = 0;
+  const MultiwayCall mw{unc.data(), &pg, info.data(), counts.data(), w.data(), mask.data(), poses.data(), &summary,
+                        &pg_status};
+  std::vector<tzr_icp_result> res;
+  std::vector<CloudPairResult> base =
+      run_cloud_pairs(to_c(params_), clouds, pairs, cp, &ip, &res, IcpMethod::kPointToPlane, 0, nullptr, &mw);
+  MultiwayResult out;
+  out.pairs.resize(P);
+  out.information.resize(P);
+  out.information_counts.assign(counts.begin(), counts.end());
+  out.edge_weights = w;
+  out.edge_inliers.resize(P);
+  for (size_t q = 0; q < P; ++q) {
+    static_cast<CloudPairResult&>(out.pairs[q]) = std::move(base[q]);
+    out.pairs[q].refined = out.pairs[q].status == TZR_OK && out.pairs[q].solution.valid && res[q].transform.scale > 0;
+    if (out.pairs[q].refined) icp_result_from_c(res[q], nullptr, &out.pairs[q].icp);
+    for (int r = 0; r < 6; ++r)
+      for (int c = 0; c < 6; ++c) out.information[q](r, c) = info[36 * q + 6 * r + c];
+    out.edge_inliers[q] = mask[q] != 0;
+  }
+  out.poses.resize(K);
+  for (size_t k = 0; k < K; ++k) {
+    Eigen::Matrix4d T = Eigen::Matrix4d::Zero();
+    for (int r = 0; r < 3; ++r) {
+      for (int c = 0; c < 3; ++c) T(r, c) = poses[k].rotation[3 * c + r];
+      T(r, 3) = poses[k].translation[r];
+    }
+    T(3, 3) = 1.0;
+    out.poses[k] = T;
+  }
+  out.pose_graph_status = pg_status;
+  out.iterations = summary.iterations;
+  out.inner_iterations = summary.inner_iterations;
+  out.cost = summary.cost;
   return out;
 }
 
