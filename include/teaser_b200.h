@@ -812,7 +812,8 @@ int tzr_information_matrix_batch(tzr_ctx* ctx, int B, const int32_t* ns, const f
  *     Lambda_e(5,5) = 0): an edge is an outlier when it moves its overlap by more than c RMS.
  *   - GNC-TLS on the uncertain edges (the rotation stage's schedule): weights start at 1; for i < max_iterations: the
  *     inner solve with the current weights; if no edge is uncertain, stop; at i = 0, mu = 1 / (2 max r-bar - 1) over
- *     the uncertain edges, and stop if mu <= 0; then, per uncertain edge, w = 0 where r-bar >= (mu + 1) / mu, 1 where
+ *     the uncertain edges, and stop unless mu is finite and positive (2 max r-bar - 1 <= 0, every uncertain edge an
+ *     inlier, stops with weights 1; so does max r-bar = +inf); then, per uncertain edge, w = 0 where r-bar >= (mu + 1) / mu, 1 where
  *     r-bar <= mu / (mu + 1), sqrt(mu (mu + 1) / r-bar) - mu between; cost = sum over the uncertain edges of the
  *     previous w times r-bar; mu <- mu * gnc_factor; stop when |cost - previous cost| < cost_threshold (previous cost
  *     +inf at i = 0).  Certain edges keep weight 1.  inlier = w >= 0.5.

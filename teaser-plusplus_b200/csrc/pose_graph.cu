@@ -349,8 +349,10 @@ __global__ void pg_gnc_kernel(PgDev dv, int E, int iter, double gnc_factor, doub
   }
   double mu = st.mu;
   if (iter == 0) {
+    // stop unless mu is finite and positive: 2 max r-bar - 1 <= 0 means every uncertain edge is an inlier, and at
+    // max r-bar = 1/2 exactly mu would be +inf and every weight NaN
     mu = 1.0 / (2.0 * rmax - 1.0);
-    if (mu <= 0.0) {
+    if (!(mu > 0.0) || isinf(mu)) {
       if (lane == 0) {
         st.mu = mu;
         st.stop = 1;

@@ -10,6 +10,7 @@ for bit.  Poses are (4,4) float64 rigid matrices.
 from __future__ import annotations
 
 import numpy as np
+import scipy.linalg
 
 import icp_reference as icp
 
@@ -229,9 +230,15 @@ def bfs(K, edges, T, live, uncertain, ref):
 
 
 def optimize(K, edges, T, L, c, uncertain=None, init=None, ref=0, gnc_factor=1.4, cost_threshold=1e-6,
-             max_iterations=100, max_inner_iterations=10):
+             max_iterations=100, max_inner_iterations=10, trace=None):
     """tzr_pose_graph_optimize.  edges (E,2), T (E,4,4), L (E,6,6).  Returns None for a disconnected graph, else a dict:
-    poses (K,4,4), weights, mask, residuals (r-bar), iterations, inner_iterations, cost."""
+    poses (K,4,4), weights, mask, residuals (r-bar), iterations, inner_iterations, cost.
+
+    trace (a list, or None): every decision is appended to it, so a test can check that none of them lies within
+    rounding of flipping.  Per inner iteration: dict(kind="inner", it, lam, F, Fc (nan when the step was not formed),
+    tol (1e-10 F + the floor), eig (the smallest and largest |eigenvalue| of the damped H), factored, outcome: "stop",
+    "accept", "reject" or "reject-stop" (lambda past 1e8)).  Per GNC weight update: dict(kind="gnc", it, mu, cost,
+    diff)."""
     edges = np.asarray(edges).reshape(-1, 2)
     E = edges.shape[0]
     T = [np.asarray(x, dtype=np.float64) for x in T]
@@ -293,11 +300,20 @@ def optimize(K, edges, T, L, c, uncertain=None, init=None, ref=0, gnc_factor=1.4
             H = np.tril(H) + np.tril(H, -1).T
             H[np.diag_indices(n)] += lam * (np.diag(H) + 1.0)
             inner += 1
+            rec = None
+            if trace is not None:
+                ev = np.linalg.eigvalsh(H) if np.isfinite(H).all() else np.array([np.nan])
+                rec = dict(kind="inner", it=it, lam=lam, F=cost, tol=REL_TOL * cost + floor,
+                           eig=(float(ev[0]), float(np.abs(ev).max())))
+                trace.append(rec)
             try:
-                delta = np.linalg.solve(np.linalg.cholesky(H).T, np.linalg.solve(np.linalg.cholesky(H), -g))
+                C = np.linalg.cholesky(H)
+                factored = True
+                delta = scipy.linalg.solve_triangular(C.T, scipy.linalg.solve_triangular(C, -g, lower=True),
+                                                      lower=False)
                 ok = bool(np.isfinite(delta).all())
             except np.linalg.LinAlgError:
-                ok = False
+                factored = ok = False
             cand_cost = np.nan
             if ok:
                 cand = [poses[k] if k == ref else se3_exp(delta[6 * fidx[k]:6 * fidx[k] + 6]) @ poses[k]
@@ -305,15 +321,23 @@ def optimize(K, edges, T, L, c, uncertain=None, init=None, ref=0, gnc_factor=1.4
                 cand_terms = terms(cand)
                 cand_cost = _warp_sum([w[e] * cand_terms[e][2] for e in range(E)])
                 ok = bool(np.isfinite(cand_cost))
+            if rec is not None:
+                rec.update(Fc=cand_cost, factored=factored)
             if ok and abs(cost - cand_cost) <= REL_TOL * cost + floor:
+                if rec is not None:
+                    rec["outcome"] = "stop"
                 if cand_cost < cost:
                     poses, cur, cost = cand, cand_terms, cand_cost
                 break
             if ok and cand_cost < cost:
                 poses, cur, cost = cand, cand_terms, cand_cost
                 lam = lam * 0.1
+                if rec is not None:
+                    rec["outcome"] = "accept"
             else:
                 lam = lam * 10.0
+                if rec is not None:
+                    rec["outcome"] = "reject-stop" if lam > LAMBDA_MAX else "reject"
                 if lam > LAMBDA_MAX:
                     break
         outer, inner_total = it + 1, inner_total + inner
@@ -321,8 +345,14 @@ def optimize(K, edges, T, L, c, uncertain=None, init=None, ref=0, gnc_factor=1.4
             break
         rbar = np.array([cur[e][3] for e in range(E)])
         if it == 0:
-            mu = 1.0 / (2.0 * rbar[unc].max() - 1.0)
-            if mu <= 0.0:
+            # fmax from 0 as the device does (a NaN r-bar is skipped); stop unless mu is finite and positive, which
+            # includes max r-bar = 1/2 exactly (mu = +inf would make every weight NaN)
+            rmax = np.float64(0.0)
+            for r in rbar[unc]:
+                rmax = np.fmax(rmax, r)
+            with np.errstate(divide="ignore"):
+                mu = np.float64(1.0) / (2.0 * rmax - 1.0)
+            if not (mu > 0.0 and np.isfinite(mu)):
                 break
         th1, th2 = (mu + 1.0) / mu, mu / (mu + 1.0)
         lanes = np.zeros(32)
@@ -334,6 +364,8 @@ def optimize(K, edges, T, L, c, uncertain=None, init=None, ref=0, gnc_factor=1.4
             w[e] = 0.0 if r >= th1 else 1.0 if r <= th2 else np.sqrt(mu * (mu + 1.0) / r) - mu
         gc = _butterfly(lanes)
         diff = abs(gc - prev)
+        if trace is not None:
+            trace.append(dict(kind="gnc", it=it, mu=mu, cost=gc, diff=diff))
         mu, prev = mu * gnc_factor, gc
         if diff < cost_threshold:
             break
