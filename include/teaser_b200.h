@@ -648,7 +648,10 @@ int tzr_register_cloud_pairs_icp_point_to_plane(tzr_ctx* ctx, const tzr_frontend
  *       where a x b = (a1 b2 - a2 b1, a2 b0 - a0 b2, a0 b1 - a1 b0) and A v row r is (A(r,0) v0 + A(r,1) v1) + A(r,2) v2.
  *     A correspondence adds nothing, but still counts for fitness and rmse, when either normal has a non-finite
  *     component or zero length, or when det is not > 0 or not finite.
- *   - epsilon (Open3D's epsilon, 1e-3 there) must be finite and > 0; anything else is TZR_ERR_INVALID_ARG.
+ *   - epsilon (Open3D's epsilon, 1e-3 there) must be finite and > 0; anything else is TZR_ERR_INVALID_ARG.  Where R m
+ *     is parallel to n, M has the eigenvalue (s2 + 1) epsilon and A loses accuracy like 2^-53 / epsilon, so below
+ *     about 1e-9 a step is less accurate than its float inputs, and near 1e-20 the det > 0 rule drops an arbitrary
+ *     subset of such correspondences (DESIGN.md §3.14 has the measured errors).
  *   - Relation to Open3D: Open3D forms W = M^-1/2 and sums three weighted rows per correspondence; with the L2 loss
  *     sum rows^T rows = J^T M^-1 J, so no matrix square root is needed.  Open3D's GetRotationFromE1ToX returns the
  *     identity when e1 . n < -0.99, which makes its covariance depend on the normal's sign there; this definition uses
