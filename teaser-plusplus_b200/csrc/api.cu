@@ -220,8 +220,6 @@ void parallel_stage(char* dst_base, const double* const* bufs, int first, int co
   parallel_copy(spans);
 }
 
-size_t al256(size_t x) { return (x + 255) & ~(size_t)255; }
-
 // effective inlier selection mode (registration.cc:574-583)
 int effective_mode(const tzr_params& p) {
   int mode = p.inlier_selection_mode;
@@ -992,7 +990,7 @@ int fpfh_run(tzr_ctx* ctx, int B, const int32_t* n, const float* const* pts, dou
   }
   std::vector<FpfhCloud> clouds((size_t)B);
   FpfhPlan plan;
-  const int route = (ctx->flags & 4194304u) ? kFpfhRouteBrute : (ctx->flags & 8388608u) ? kFpfhRouteGrid : kFpfhRouteAuto;
+  const int route = search_route(ctx->flags, kFlagFpfhBrute, kFlagFpfhGrid);
   if (fpfh_plan(B, n, normal_radius, fpfh_radius, route, clouds.data(), &plan) != TZR_OK) {
     ctx->last_error = "the batch's points do not fit 32-bit indices";
     return TZR_ERR_TOO_LARGE;
@@ -2066,6 +2064,28 @@ static bool icp_params_ok(const tzr_icp_params* p) {
 // generalized ICP's epsilon: finite and > 0
 static bool icp_epsilon_ok(double epsilon) { return std::isfinite(epsilon) && epsilon > 0; }
 
+// a transform that ICP or the information matrices start from: scale finite and > 0, R and t finite
+static bool similarity_ok(const tzr_similarity& s) {
+  bool ok = std::isfinite(s.scale) && s.scale > 0;
+  for (int k = 0; k < 9; ++k) ok &= std::isfinite(s.rotation[k]) != 0;
+  for (int k = 0; k < 3; ++k) ok &= std::isfinite(s.translation[k]) != 0;
+  return ok;
+}
+
+// launch_icp's iteration settings (kernel: the robust kernel of the point-to-plane and generalized modes, NULL = L2)
+static void icp_iteration_settings(IcpPlan* plan, const tzr_icp_params& p, int mode, double epsilon,
+                                   const tzr_robust_kernel* kernel) {
+  plan->max_iteration = p.max_iteration;
+  plan->mode = mode;
+  plan->epsilon = epsilon;
+  if (kernel) {
+    plan->loss = kernel->type;
+    plan->loss_k = kernel->k;
+  }
+  plan->relative_fitness = p.relative_fitness;
+  plan->relative_rmse = p.relative_rmse;
+}
+
 // a robust kernel (DESIGN.md §3.15): a known type, and k finite and > 0 where the weight reads it
 static bool robust_kernel_ok(const tzr_robust_kernel* k) {
   if (!k) return false;
@@ -2410,7 +2430,7 @@ static int register_pairs_run(tzr_ctx* ctx, const tzr_frontend_params* fp, const
   std::vector<MatchPair> MP;
   std::vector<NnWork> W;
   MatchPlan mplan;
-  const int route = (ctx->flags & 4194304u) ? kFpfhRouteBrute : (ctx->flags & 8388608u) ? kFpfhRouteGrid : kFpfhRouteAuto;
+  const int route = search_route(ctx->flags, kFlagFpfhBrute, kFlagFpfhGrid);
   if (fpfh_plan(n_clouds, n, fp->normal_search_radius, fp->fpfh_search_radius, route, clouds.data(), &fplan) != TZR_OK ||
       match_plan(P, ns.data(), nd.data(), seeds.data(), ctx->num_sms, &MP, &W, &mplan) != TZR_OK) {
     ctx->last_error = "the batch's points do not fit 32-bit indices";
@@ -2437,39 +2457,40 @@ static int register_pairs_run(tzr_ctx* ctx, const tzr_frontend_params* fp, const
   const size_t h_head = al256(o_g), h_g = h_head + al256(head), h_sol = h_g + al256((size_t)P * sizeof(PairGather)),
                h_corr = h_sol + al256((size_t)P * sizeof(tzr_solution)), h_clq = h_corr + al256(C * 8),
                pin_base = h_clq + C * 4;
-  // with ICP: [ICP problem table | target cloud table | chunk table] staged in and the problem table read back
-  std::vector<FpfhCloud> iclouds;
+  // with ICP: the refinement of every pair planned here, which sizes its tables and checks them before any work, and
+  // planned again over the solved pairs once they are known (plan_icp: sources from a pair's first cloud, targets its
+  // second).  Its workspace ctx->icp is laid out from 0 (icp_layout); the pinned area mirrors the layout's tables
+  // ([problems | target clouds | chunks], staged in and the problem table read back) and, with the multiway step, holds
+  // the [information | counts] of the refined pairs read back.
   IcpPlan iplan;
-  long long i_ns = 0, i_chunks = 0;
-  if (icp) {
-    for (int p = 0; p < P; ++p) {
-      i_ns += n[pair_clouds[2 * p]];
-      i_chunks += (n[pair_clouds[2 * p]] + kIcpChunk - 1) / kIcpChunk;
+  std::vector<FpfhCloud> iclouds;
+  std::vector<IcpProb> iprobs;
+  std::vector<int> ichunks;
+  auto plan_icp = [&](const std::vector<int>& pairs) {
+    std::vector<int32_t> i_ns, i_slo, i_tc;
+    for (int p : pairs) {
+      i_ns.push_back(n[pair_clouds[2 * p]]);
+      i_slo.push_back(clouds[pair_clouds[2 * p]].lo);
+      i_tc.push_back(pair_clouds[2 * p + 1]);
     }
-    iclouds.resize((size_t)n_clouds);
-    const int iroute = (ctx->flags & 33554432u) ? kFpfhRouteBrute : (ctx->flags & 67108864u) ? kFpfhRouteGrid : kFpfhRouteAuto;
-    const double r = icp->max_correspondence_distance;
-    if (i_ns > 0x7fffffffll ||
-        fpfh_plan(n_clouds, n, r, r, iroute, iclouds.data(), &iplan.grid, kIcpGridMinN) != TZR_OK) {
+    return icp_plan((int)pairs.size(), i_ns.data(), i_slo.data(), i_tc.data(), n_clouds, n,
+                    icp->max_correspondence_distance, search_route(ctx->flags, kFlagIcpBrute, kFlagIcpGrid), nullptr,
+                    &iplan, &iclouds, &iprobs, &ichunks);
+  };
+  IcpLayout il{};
+  if (icp) {
+    std::vector<int> every(P);
+    for (int p = 0; p < P; ++p) every[p] = p;
+    icp_iteration_settings(&iplan, *icp, icp_mode, icp_epsilon, icp_kernel);
+    if (plan_icp(every) != TZR_OK) {
       ctx->last_error = "the refinement's points or target grid do not fit 32-bit indices";
       return TZR_ERR_TOO_LARGE;
     }
-    iplan.max_iteration = icp->max_iteration;
-    iplan.mode = icp_mode;
-    iplan.epsilon = icp_epsilon;
-    if (icp_kernel) {
-      iplan.loss = icp_kernel->type;
-      iplan.loss_k = icp_kernel->k;
-    }
-    iplan.r2 = r * r;
-    iplan.relative_fitness = icp->relative_fitness;
-    iplan.relative_rmse = icp->relative_rmse;
+    il = icp_layout(iplan, 0, mw != nullptr);
   }
-  // with the multiway step: [information | counts] of the refined pairs read back
-  const size_t hi_prob = al256(pin_base), hi_cl = hi_prob + al256((size_t)P * sizeof(IcpProb)),
-               hi_ck = hi_cl + al256((size_t)n_clouds * sizeof(FpfhCloud)), hi_end = hi_ck + (size_t)i_chunks * 4,
-               hi_info = al256(hi_end), hi_icnt = hi_info + al256((size_t)P * 36 * 8),
-               pin_bytes = mw ? hi_icnt + (size_t)P * 4 : icp ? hi_end : pin_base;
+  const size_t hi_tab = al256(pin_base), hi_info = al256(hi_tab + il.match),
+               hi_icnt = hi_info + al256((size_t)P * 36 * 8),
+               pin_bytes = mw ? hi_icnt + (size_t)P * 4 : icp ? hi_tab + il.match : pin_base;
   int rc;
   if ((rc = ensure(ctx, ctx->m_in, in_bytes)) != TZR_OK) return rc;
   if ((rc = ensure(ctx, ctx->m_scratch, scratch_bytes)) != TZR_OK) return rc;
@@ -2581,62 +2602,33 @@ static int register_pairs_run(tzr_ctx* ctx, const tzr_frontend_params* fp, const
     ++ctx->generation;
   }
   // the refinement of the solved pairs, seeded on the device from their records (no synchronisation, no upload of points)
-  IcpProb* hi_probs = (IcpProb*)(h + hi_prob);
+  char* hi = h + hi_tab;
+  const IcpProb* hi_probs = (const IcpProb*)(hi + il.probs);
   if (icp && S > 0) {
-    int c_lo = 0, m_lo = 0;
-    for (int k = 0; k < S; ++k) {
-      const int a = pair_clouds[2 * solved[k]], b = pair_clouds[2 * solved[k] + 1];
-      IcpProb& pr = hi_probs[k];
-      pr = IcpProb{};
-      pr.s_lo = clouds[a].lo;
-      pr.ns = n[a];
-      pr.d_lo = clouds[b].lo;
-      pr.nd = n[b];
-      pr.c_lo = c_lo;
-      pr.m_lo = m_lo;
-      pr.tc = b;
-      pr.n_lo = clouds[b].lo;
-      pr.sn_lo = clouds[a].lo;
-      const int nc = (n[a] + kIcpChunk - 1) / kIcpChunk;
-      for (int c = 0; c < nc; ++c) ((int*)(h + hi_ck))[c_lo + c] = k;
-      c_lo += nc;
-      m_lo += n[a];
-    }
-    iplan.B = S;
-    iplan.NS = m_lo;
-    iplan.ND = (int)N;
-    iplan.chunks = c_lo;
-    memcpy(h + hi_cl, iclouds.data(), (size_t)n_clouds * sizeof(FpfhCloud));
-    const size_t pb = (size_t)S * sizeof(IcpProb), cb = (size_t)n_clouds * sizeof(FpfhCloud), kb = (size_t)c_lo * 4;
-    const size_t o_prob = 0, o_cl = al256(pb), o_ck = o_cl + al256(cb), o_match = o_ck + al256(kb),
-                 o_part = o_match + al256((size_t)m_lo * 4),
-                 o_grid = o_part + al256((size_t)c_lo * icp_partial_stride(icp_mode) * 8),
-                 o_info = al256(o_grid + iplan.grid.grid_bytes), o_icnt = o_info + al256((size_t)S * 36 * 8),
-                 total = mw ? o_icnt + (size_t)S * 4 : o_grid + iplan.grid.grid_bytes;
-    if ((rc = ensure(ctx, ctx->icp, total)) != TZR_OK) return rc;
+    plan_icp(solved);  // a subset of the pairs planned above: it fits
+    il = icp_layout(iplan, 0, mw != nullptr);
+    if ((rc = ensure(ctx, ctx->icp, il.end)) != TZR_OK) return rc;
+    memcpy(hi + il.probs, iprobs.data(), (size_t)S * sizeof(IcpProb));
+    memcpy(hi + il.clouds, iclouds.data(), (size_t)n_clouds * sizeof(FpfhCloud));
+    memcpy(hi + il.chunks, ichunks.data(), ichunks.size() * 4);
     char* di = (char*)ctx->icp.p;
-    CK(cudaMemcpyAsync(di + o_prob, hi_probs, pb, cudaMemcpyHostToDevice, st));
-    CK(cudaMemcpyAsync(di + o_cl, h + hi_cl, cb, cudaMemcpyHostToDevice, st));
-    CK(cudaMemcpyAsync(di + o_ck, h + hi_ck, kb, cudaMemcpyHostToDevice, st));
-    ctx->launches += launch_icp_seed((IcpProb*)(di + o_prob), S, d_sol, st);
+    CK(cudaMemcpyAsync(di, hi, il.match, cudaMemcpyHostToDevice, st));
+    IcpBuffers buf = icp_buffers(di, il);
+    ctx->launches += launch_icp_seed(buf.probs, S, d_sol, st);
     // point-to-plane and generalized: the target (and source) normals are the FPFH stage's (normal_search_radius,
     // viewpoint at the origin), still in m_out: nothing after the FPFH stage writes that region, and they share the
     // cloud table's indexing
-    const float4* d_nrm = (const float4*)(d_out + o_nrm);
+    buf.src = buf.dst = d_pts;
+    buf.src_normals = buf.dst_normals = (const float4*)(d_out + o_nrm);
     IcpGrid grid{nullptr, nullptr, nullptr};
-    ctx->launches += launch_icp(iplan, d_pts, d_pts, d_nrm, d_nrm, (IcpProb*)(di + o_prob), (FpfhCloud*)(di + o_cl),
-                                (const int*)(di + o_ck), (int*)(di + o_match), (double*)(di + o_part),
-                                iplan.grid.grid_bytes ? di + o_grid : nullptr, st, &grid);
+    ctx->launches += launch_icp(iplan, buf, st, &grid);
     if ((rc = check_launch(ctx, "icp launch")) != TZR_OK) return rc;
-    CK(cudaMemcpyAsync(hi_probs, di + o_prob, pb, cudaMemcpyDeviceToHost, st));
+    CK(cudaMemcpyAsync(hi + il.probs, buf.probs, (size_t)S * sizeof(IcpProb), cudaMemcpyDeviceToHost, st));
     if (mw) {  // the information matrices at the refined transforms, from the clouds and the problem table in place
-      ctx->launches += launch_icp_information(iplan, d_pts, d_pts, (IcpProb*)(di + o_prob), (FpfhCloud*)(di + o_cl),
-                                              (const int*)(di + o_ck), (int*)(di + o_match), (double*)(di + o_part),
-                                              iplan.grid.grid_bytes ? di + o_grid : nullptr, true,
-                                              (double*)(di + o_info), (int*)(di + o_icnt), st, &grid);
+      ctx->launches += launch_icp_information(iplan, buf, true, st, &grid);
       if ((rc = check_launch(ctx, "information launch")) != TZR_OK) return rc;
-      CK(cudaMemcpyAsync(h + hi_info, di + o_info, (size_t)S * 36 * 8, cudaMemcpyDeviceToHost, st));
-      CK(cudaMemcpyAsync(h + hi_icnt, di + o_icnt, (size_t)S * 4, cudaMemcpyDeviceToHost, st));
+      CK(cudaMemcpyAsync(h + hi_info, buf.info, (size_t)S * 36 * 8, cudaMemcpyDeviceToHost, st));
+      CK(cudaMemcpyAsync(h + hi_icnt, buf.counts, (size_t)S * 4, cudaMemcpyDeviceToHost, st));
     }
   }
   // synchronisation 2: the records, and the index pairs and cliques that were asked for
@@ -2782,122 +2774,83 @@ void tzr_icp_params_default(tzr_icp_params* p) {
   p->max_iteration = 30;
 }
 
-// tzr_icp(_batch), tzr_icp_point_to_plane(_batch) and tzr_icp_generalized(_batch): sources, targets (and target and
-// source normals) staged back to back, one H2D copy, every iteration enqueued (launch_icp), one D2H copy of the problem
-// table (and of the per-point matches when correspondences are asked for).  dst_normals: required for kIcpPointToPlane
-// and kIcpGeneralized, src_normals and epsilon for kIcpGeneralized; unused otherwise.  kernel: the robust kernel of the
-// point-to-plane and generalized modes (checked by the caller; NULL = L2).
+// Validation, planning and staging of tzr_icp*(_batch) and tzr_information_matrix(_batch): the problems planned by
+// icp_plan and seeded from init, then [sources | targets | (target normals | (source normals))] and the layout's
+// tables after them ([problems | target clouds | chunks], icp_layout) staged in one H2D copy into ctx->icp.  plan->mode
+// (set by the caller) decides which normals are required and staged; information: room for the information matrices.
+// On success *probs holds the staged problem table and *buf the workspace's device buffers.
+static int icp_batch_stage(tzr_ctx* ctx, IcpPlan* plan, int B, const int32_t* ns, const float* const* src,
+                           const float* const* src_normals, const int32_t* nd, const float* const* dst,
+                           const float* const* dst_normals, const tzr_similarity* init, double r, bool information,
+                           std::vector<IcpProb>* probs, IcpBuffers* buf) {
+  const bool plane = plan->mode != kIcpPointToPoint, gicp = plan->mode == kIcpGeneralized;
+  if (!ctx || B < 1 || !ns || !src || !nd || !dst || (plane && !dst_normals) || (gicp && !src_normals) || !init)
+    return TZR_ERR_INVALID_ARG;
+  for (int b = 0; b < B; ++b)
+    if (ns[b] < 1 || nd[b] < 1 || !src[b] || !dst[b] || (plane && !dst_normals[b]) || (gicp && !src_normals[b]) ||
+        !similarity_ok(init[b]))
+      return TZR_ERR_INVALID_ARG;
+  std::vector<FpfhCloud> clouds;
+  std::vector<int> chunk_prob;
+  if (icp_plan(B, ns, nullptr, nullptr, B, nd, r, search_route(ctx->flags, kFlagIcpBrute, kFlagIcpGrid), init, plan,
+               &clouds, probs, &chunk_prob) != TZR_OK) {
+    ctx->last_error = "the batch's points or target grid do not fit 32-bit indices";
+    return TZR_ERR_TOO_LARGE;
+  }
+  cudaSetDevice(ctx->device);
+  const size_t NS = (size_t)plan->NS, ND = (size_t)plan->ND;
+  const size_t o_dst = al256(NS * 12), o_nrm = o_dst + al256(ND * 12), o_snrm = o_nrm + al256(plane ? ND * 16 : 0);
+  const IcpLayout L = icp_layout(*plan, al256(o_snrm + (gicp ? NS * 16 : 0)), information);
+  int rc;
+  if ((rc = ensure(ctx, ctx->icp, L.end)) != TZR_OK) return rc;
+  std::vector<char> h(L.match);
+  for (int b = 0; b < B; ++b) {
+    const IcpProb& pr = (*probs)[b];
+    memcpy(h.data() + (size_t)pr.s_lo * 12, src[b], (size_t)ns[b] * 12);
+    memcpy(h.data() + o_dst + (size_t)pr.d_lo * 12, dst[b], (size_t)nd[b] * 12);
+    if (plane) memcpy(h.data() + o_nrm + (size_t)pr.n_lo * 16, dst_normals[b], (size_t)nd[b] * 16);
+    if (gicp) memcpy(h.data() + o_snrm + (size_t)pr.sn_lo * 16, src_normals[b], (size_t)ns[b] * 16);
+  }
+  memcpy(h.data() + L.probs, probs->data(), (size_t)B * sizeof(IcpProb));
+  memcpy(h.data() + L.clouds, clouds.data(), (size_t)B * sizeof(FpfhCloud));
+  memcpy(h.data() + L.chunks, chunk_prob.data(), chunk_prob.size() * 4);
+  char* d = (char*)ctx->icp.p;
+  CK(cudaMemcpyAsync(d, h.data(), L.match, cudaMemcpyHostToDevice, ctx->stream));
+  *buf = icp_buffers(d, L);
+  buf->src = (const float*)d;
+  buf->dst = (const float*)(d + o_dst);
+  buf->dst_normals = plane ? (const float4*)(d + o_nrm) : nullptr;
+  buf->src_normals = gicp ? (const float4*)(d + o_snrm) : nullptr;
+  return TZR_OK;
+}
+
+// tzr_icp(_batch), tzr_icp_point_to_plane(_batch) and tzr_icp_generalized(_batch): icp_batch_stage, every iteration
+// enqueued (launch_icp), one D2H copy of the problem table (and of the per-point matches when correspondences are asked
+// for).  dst_normals: required for kIcpPointToPlane and kIcpGeneralized, src_normals and epsilon for kIcpGeneralized;
+// unused otherwise.  kernel: the robust kernel of the point-to-plane and generalized modes (checked by the caller;
+// NULL = L2).
 static int icp_batch_run(tzr_ctx* ctx, const tzr_icp_params* params, int mode, int B, const int32_t* ns,
                          const float* const* src, const float* const* src_normals, const int32_t* nd,
                          const float* const* dst, const float* const* dst_normals, double epsilon,
                          const tzr_similarity* init, tzr_icp_result* results, int32_t* const* corr,
                          const tzr_robust_kernel* kernel = nullptr) {
-  const bool plane = mode != kIcpPointToPoint, gicp = mode == kIcpGeneralized;
-  if (!ctx || !icp_params_ok(params) || B < 1 || !ns || !src || !nd || !dst || (plane && !dst_normals) ||
-      (gicp && (!src_normals || !icp_epsilon_ok(epsilon))) || !init || !results)
+  if (!icp_params_ok(params) || (mode == kIcpGeneralized && !icp_epsilon_ok(epsilon)) || !results)
     return TZR_ERR_INVALID_ARG;
-  const double r = params->max_correspondence_distance;
-  long long NS = 0, ND = 0, chunks = 0;
-  bool want_corr = false;
-  for (int b = 0; b < B; ++b) {
-    if (ns[b] < 1 || nd[b] < 1 || !src[b] || !dst[b] || (plane && !dst_normals[b]) || (gicp && !src_normals[b]))
-      return TZR_ERR_INVALID_ARG;
-    const tzr_similarity& s = init[b];
-    bool finite = std::isfinite(s.scale) && s.scale > 0;
-    for (int k = 0; k < 9; ++k) finite &= std::isfinite(s.rotation[k]) != 0;
-    for (int k = 0; k < 3; ++k) finite &= std::isfinite(s.translation[k]) != 0;
-    if (!finite) return TZR_ERR_INVALID_ARG;
-    NS += ns[b];
-    ND += nd[b];
-    chunks += (ns[b] + kIcpChunk - 1) / kIcpChunk;
-    want_corr |= corr && corr[b];
-  }
-  if (NS > 0x7fffffffll || ND > 0x7fffffffll) {
-    ctx->last_error = "the batch's points do not fit 32-bit indices";
-    return TZR_ERR_TOO_LARGE;
-  }
   IcpPlan plan;
-  plan.B = B;
-  plan.NS = (int)NS;
-  plan.ND = (int)ND;
-  plan.chunks = (int)chunks;
-  plan.max_iteration = params->max_iteration;
-  plan.mode = mode;
-  plan.epsilon = epsilon;
-  if (kernel) {
-    plan.loss = kernel->type;
-    plan.loss_k = kernel->k;
-  }
-  plan.r2 = r * r;
-  plan.relative_fitness = params->relative_fitness;
-  plan.relative_rmse = params->relative_rmse;
-  std::vector<FpfhCloud> clouds((size_t)B);
-  const int route = (ctx->flags & 33554432u) ? kFpfhRouteBrute : (ctx->flags & 67108864u) ? kFpfhRouteGrid : kFpfhRouteAuto;
-  if (fpfh_plan(B, nd, r, r, route, clouds.data(), &plan.grid, kIcpGridMinN) != TZR_OK) {
-    ctx->last_error = "the batch's target grid does not fit 32-bit indices";
-    return TZR_ERR_TOO_LARGE;
-  }
-  std::vector<IcpProb> probs((size_t)B);
-  std::vector<int> chunk_prob((size_t)chunks);
-  {
-    int s_lo = 0, c_lo = 0;
-    for (int b = 0; b < B; ++b) {
-      IcpProb& pr = probs[b];
-      pr = IcpProb{};
-      pr.s_lo = s_lo;
-      pr.ns = ns[b];
-      pr.d_lo = clouds[b].lo;
-      pr.nd = nd[b];
-      pr.c_lo = c_lo;
-      pr.m_lo = s_lo;
-      pr.tc = b;
-      pr.n_lo = clouds[b].lo;
-      pr.sn_lo = s_lo;
-      pr.active = pr.seeded = 1;
-      pr.s = init[b].scale;
-      for (int k = 0; k < 9; ++k) pr.R[k] = init[b].rotation[k];
-      for (int k = 0; k < 3; ++k) pr.t[k] = init[b].translation[k];
-      const int nc = (ns[b] + kIcpChunk - 1) / kIcpChunk;
-      for (int c = 0; c < nc; ++c) chunk_prob[c_lo + c] = b;
-      s_lo += ns[b];
-      c_lo += nc;
-    }
-  }
-  cudaSetDevice(ctx->device);
+  icp_iteration_settings(&plan, *params, mode, epsilon, kernel);
+  std::vector<IcpProb> probs;
+  IcpBuffers buf;
+  int rc = icp_batch_stage(ctx, &plan, B, ns, src, src_normals, nd, dst, dst_normals, init,
+                           params->max_correspondence_distance, false, &probs, &buf);
+  if (rc != TZR_OK) return rc;
   cudaStream_t st = ctx->stream;
-  // [sources | targets | problems | target clouds | chunk table | (target normals | (source normals))] staged, then the
-  // matches, the partials and the grid scratch
-  const size_t sb = (size_t)NS * 12, db = (size_t)ND * 12, pb = (size_t)B * sizeof(IcpProb),
-               cb = (size_t)B * sizeof(FpfhCloud), kb = (size_t)chunks * 4, mb = (size_t)NS * 4,
-               hb = (size_t)chunks * icp_partial_stride(mode) * 8, nb = plane ? (size_t)ND * 16 : 0,
-               snb = gicp ? (size_t)NS * 16 : 0;
-  const size_t o_dst = al256(sb), o_prob = o_dst + al256(db), o_cl = o_prob + al256(pb), o_ck = o_cl + al256(cb),
-               o_nrm = o_ck + al256(kb), o_snrm = o_nrm + al256(nb),
-               in_bytes = gicp ? o_snrm + snb : plane ? o_nrm + nb : o_ck + kb, o_match = al256(in_bytes),
-               o_part = o_match + al256(mb), o_grid = o_part + al256(hb), total = o_grid + plan.grid.grid_bytes;
-  int rc;
-  if ((rc = ensure(ctx, ctx->icp, total)) != TZR_OK) return rc;
-  std::vector<char> h(in_bytes);
-  for (int b = 0; b < B; ++b) {
-    memcpy(h.data() + (size_t)probs[b].s_lo * 12, src[b], (size_t)ns[b] * 12);
-    memcpy(h.data() + o_dst + (size_t)probs[b].d_lo * 12, dst[b], (size_t)nd[b] * 12);
-    if (plane) memcpy(h.data() + o_nrm + (size_t)probs[b].n_lo * 16, dst_normals[b], (size_t)nd[b] * 16);
-    if (gicp) memcpy(h.data() + o_snrm + (size_t)probs[b].sn_lo * 16, src_normals[b], (size_t)ns[b] * 16);
-  }
-  memcpy(h.data() + o_prob, probs.data(), pb);
-  memcpy(h.data() + o_cl, clouds.data(), cb);
-  memcpy(h.data() + o_ck, chunk_prob.data(), kb);
-  char* d = (char*)ctx->icp.p;
-  CK(cudaMemcpyAsync(d, h.data(), in_bytes, cudaMemcpyHostToDevice, st));
-  ctx->launches += launch_icp(plan, (const float*)d, (const float*)(d + o_dst),
-                              gicp ? (const float4*)(d + o_snrm) : nullptr,
-                              plane ? (const float4*)(d + o_nrm) : nullptr, (IcpProb*)(d + o_prob),
-                              (FpfhCloud*)(d + o_cl), (const int*)(d + o_ck), (int*)(d + o_match),
-                              (double*)(d + o_part), plan.grid.grid_bytes ? d + o_grid : nullptr, st);
+  ctx->launches += launch_icp(plan, buf, st);
   if ((rc = check_launch(ctx, "icp launch")) != TZR_OK) return rc;
-  CK(cudaMemcpyAsync(probs.data(), d + o_prob, pb, cudaMemcpyDeviceToHost, st));
-  std::vector<int32_t> match(want_corr ? (size_t)NS : 0);
-  if (want_corr) CK(cudaMemcpyAsync(match.data(), d + o_match, mb, cudaMemcpyDeviceToHost, st));
+  CK(cudaMemcpyAsync(probs.data(), buf.probs, (size_t)B * sizeof(IcpProb), cudaMemcpyDeviceToHost, st));
+  bool want_corr = false;
+  for (int b = 0; b < B && corr; ++b) want_corr |= corr[b] != nullptr;
+  std::vector<int32_t> match(want_corr ? (size_t)plan.NS : 0);
+  if (want_corr) CK(cudaMemcpyAsync(match.data(), buf.match, (size_t)plan.NS * 4, cudaMemcpyDeviceToHost, st));
   CK(cudaStreamSynchronize(st));
   for (int b = 0; b < B; ++b) {
     const IcpProb& pr = probs[b];
@@ -2993,96 +2946,24 @@ int tzr_icp_generalized(tzr_ctx* ctx, const tzr_icp_params* params, double epsil
                     corr);
 }
 
-// tzr_information_matrix(_batch): the sources, targets and tables staged in one copy (tzr_icp_batch's layout), the
-// search and the sums (launch_icp_information), one read-back
+// tzr_information_matrix(_batch): icp_batch_stage (point-to-point, no normals), the search and the sums
+// (launch_icp_information), one read-back
 int tzr_information_matrix_batch(tzr_ctx* ctx, int B, const int32_t* ns, const float* const* src, const int32_t* nd,
                                  const float* const* dst, const tzr_similarity* transforms,
                                  double max_correspondence_distance, double* information, int32_t* counts) {
   const double r = max_correspondence_distance;
-  if (!ctx || B < 1 || !ns || !src || !nd || !dst || !transforms || !information || !(r > 0) || !std::isfinite(r))
-    return TZR_ERR_INVALID_ARG;
-  long long NS = 0, ND = 0, chunks = 0;
-  for (int b = 0; b < B; ++b) {
-    if (ns[b] < 1 || nd[b] < 1 || !src[b] || !dst[b]) return TZR_ERR_INVALID_ARG;
-    const tzr_similarity& s = transforms[b];
-    bool finite = std::isfinite(s.scale) && s.scale > 0;
-    for (int k = 0; k < 9; ++k) finite &= std::isfinite(s.rotation[k]) != 0;
-    for (int k = 0; k < 3; ++k) finite &= std::isfinite(s.translation[k]) != 0;
-    if (!finite) return TZR_ERR_INVALID_ARG;
-    NS += ns[b];
-    ND += nd[b];
-    chunks += (ns[b] + kIcpChunk - 1) / kIcpChunk;
-  }
-  if (NS > 0x7fffffffll || ND > 0x7fffffffll) {
-    ctx->last_error = "the batch's points do not fit 32-bit indices";
-    return TZR_ERR_TOO_LARGE;
-  }
+  if (!information || !(r > 0) || !std::isfinite(r)) return TZR_ERR_INVALID_ARG;
   IcpPlan plan;
-  plan.B = B;
-  plan.NS = (int)NS;
-  plan.ND = (int)ND;
-  plan.chunks = (int)chunks;
-  plan.r2 = r * r;
-  std::vector<FpfhCloud> clouds((size_t)B);
-  const int route = (ctx->flags & 33554432u) ? kFpfhRouteBrute : (ctx->flags & 67108864u) ? kFpfhRouteGrid : kFpfhRouteAuto;
-  if (fpfh_plan(B, nd, r, r, route, clouds.data(), &plan.grid, kIcpGridMinN) != TZR_OK) {
-    ctx->last_error = "the batch's target grid does not fit 32-bit indices";
-    return TZR_ERR_TOO_LARGE;
-  }
-  std::vector<IcpProb> probs((size_t)B);
-  std::vector<int> chunk_prob((size_t)chunks);
-  {
-    int s_lo = 0, c_lo = 0;
-    for (int b = 0; b < B; ++b) {
-      IcpProb& pr = probs[b];
-      pr = IcpProb{};
-      pr.s_lo = s_lo;
-      pr.ns = ns[b];
-      pr.d_lo = clouds[b].lo;
-      pr.nd = nd[b];
-      pr.c_lo = c_lo;
-      pr.m_lo = s_lo;
-      pr.tc = b;
-      pr.active = pr.seeded = 1;
-      pr.s = transforms[b].scale;
-      for (int k = 0; k < 9; ++k) pr.R[k] = transforms[b].rotation[k];
-      for (int k = 0; k < 3; ++k) pr.t[k] = transforms[b].translation[k];
-      const int nc = (ns[b] + kIcpChunk - 1) / kIcpChunk;
-      for (int c = 0; c < nc; ++c) chunk_prob[c_lo + c] = b;
-      s_lo += ns[b];
-      c_lo += nc;
-    }
-  }
-  cudaSetDevice(ctx->device);
+  std::vector<IcpProb> probs;
+  IcpBuffers buf;
+  int rc = icp_batch_stage(ctx, &plan, B, ns, src, nullptr, nd, dst, nullptr, transforms, r, true, &probs, &buf);
+  if (rc != TZR_OK) return rc;
   cudaStream_t st = ctx->stream;
-  // [sources | targets | problems | target clouds | chunk table] staged, then the matches, the partials, the grid
-  // scratch, the information matrices and the counts
-  const size_t sb = (size_t)NS * 12, db = (size_t)ND * 12, pb = (size_t)B * sizeof(IcpProb),
-               cb = (size_t)B * sizeof(FpfhCloud), kb = (size_t)chunks * 4;
-  const size_t o_dst = al256(sb), o_prob = o_dst + al256(db), o_cl = o_prob + al256(pb), o_ck = o_cl + al256(cb),
-               in_bytes = o_ck + kb, o_match = al256(in_bytes), o_part = o_match + al256((size_t)NS * 4),
-               o_grid = o_part + al256((size_t)chunks * kIcpInfoSums * 8), o_info = al256(o_grid + plan.grid.grid_bytes),
-               o_cnt = o_info + al256((size_t)B * 36 * 8), total = o_cnt + (size_t)B * 4;
-  int rc;
-  if ((rc = ensure(ctx, ctx->icp, total)) != TZR_OK) return rc;
-  std::vector<char> h(in_bytes);
-  for (int b = 0; b < B; ++b) {
-    memcpy(h.data() + (size_t)probs[b].s_lo * 12, src[b], (size_t)ns[b] * 12);
-    memcpy(h.data() + o_dst + (size_t)probs[b].d_lo * 12, dst[b], (size_t)nd[b] * 12);
-  }
-  memcpy(h.data() + o_prob, probs.data(), pb);
-  memcpy(h.data() + o_cl, clouds.data(), cb);
-  memcpy(h.data() + o_ck, chunk_prob.data(), kb);
-  char* d = (char*)ctx->icp.p;
-  CK(cudaMemcpyAsync(d, h.data(), in_bytes, cudaMemcpyHostToDevice, st));
-  ctx->launches += launch_icp_information(plan, (const float*)d, (const float*)(d + o_dst), (IcpProb*)(d + o_prob),
-                                          (FpfhCloud*)(d + o_cl), (const int*)(d + o_ck), (int*)(d + o_match),
-                                          (double*)(d + o_part), plan.grid.grid_bytes ? d + o_grid : nullptr, false,
-                                          (double*)(d + o_info), (int*)(d + o_cnt), st);
+  ctx->launches += launch_icp_information(plan, buf, false, st);
   if ((rc = check_launch(ctx, "information launch")) != TZR_OK) return rc;
   std::vector<int32_t> cnt((size_t)B);
-  CK(cudaMemcpyAsync(information, d + o_info, (size_t)B * 36 * 8, cudaMemcpyDeviceToHost, st));
-  CK(cudaMemcpyAsync(cnt.data(), d + o_cnt, (size_t)B * 4, cudaMemcpyDeviceToHost, st));
+  CK(cudaMemcpyAsync(information, buf.info, (size_t)B * 36 * 8, cudaMemcpyDeviceToHost, st));
+  CK(cudaMemcpyAsync(cnt.data(), buf.counts, (size_t)B * 4, cudaMemcpyDeviceToHost, st));
   CK(cudaStreamSynchronize(st));
   if (counts) memcpy(counts, cnt.data(), (size_t)B * 4);
   return TZR_OK;

@@ -25,6 +25,8 @@
 // [256 k, 256 k + 256), and the chunks of a problem are combined by lane k mod 32 then a butterfly), so a problem's
 // bits do not depend on the batch it runs in.  Finished problems return at once from every kernel.  The iterations are
 // enqueued back to back without a host synchronisation; the launch count depends on max_iteration only.
+#include <algorithm>
+
 #include "rot3.cuh"
 #include "tzr_internal.cuh"
 
@@ -741,13 +743,82 @@ __global__ void icp_info_seed_kernel(IcpProb* probs, int B) {
 
 }  // namespace
 
-int launch_icp_information(const IcpPlan& plan, const float* src, const float* dst, IcpProb* probs, FpfhCloud* clouds,
-                           const int* chunk_prob, int* match, double* partial, void* grid_scratch, bool reseed,
-                           double* info, int* counts, cudaStream_t st, const IcpGrid* grid) {
+int icp_plan(int B, const int32_t* ns, const int32_t* s_lo, const int32_t* tc, int T, const int32_t* nt, double r,
+             int route, const tzr_similarity* init, IcpPlan* plan, std::vector<FpfhCloud>* clouds,
+             std::vector<IcpProb>* probs, std::vector<int>* chunk_prob) {
+  long long NS = 0, chunks = 0;
+  for (int b = 0; b < B; ++b) {
+    NS += ns[b];
+    chunks += (ns[b] + kIcpChunk - 1) / kIcpChunk;
+  }
+  clouds->resize((size_t)T);
+  if (NS > 0x7fffffffll || fpfh_plan(T, nt, r, r, route, clouds->data(), &plan->grid, kIcpGridMinN) != TZR_OK)
+    return TZR_ERR_TOO_LARGE;
+  plan->B = B;
+  plan->NS = (int)NS;
+  plan->ND = plan->grid.N;
+  plan->chunks = (int)chunks;
+  plan->r2 = r * r;
+  probs->assign((size_t)B, IcpProb{});
+  chunk_prob->resize((size_t)chunks);
+  int m_lo = 0, c_lo = 0;
+  for (int b = 0; b < B; ++b) {
+    IcpProb& pr = (*probs)[b];
+    const FpfhCloud& t = (*clouds)[tc ? tc[b] : b];
+    pr.s_lo = s_lo ? s_lo[b] : m_lo;
+    pr.ns = ns[b];
+    pr.d_lo = t.lo;
+    pr.nd = t.n;
+    pr.c_lo = c_lo;
+    pr.m_lo = m_lo;
+    pr.tc = tc ? tc[b] : b;
+    pr.n_lo = t.lo;
+    pr.sn_lo = pr.s_lo;
+    if (init) {
+      pr.active = pr.seeded = 1;
+      pr.s = init[b].scale;
+      for (int k = 0; k < 9; ++k) pr.R[k] = init[b].rotation[k];
+      for (int k = 0; k < 3; ++k) pr.t[k] = init[b].translation[k];
+    }
+    const int nc = (ns[b] + kIcpChunk - 1) / kIcpChunk;
+    for (int c = 0; c < nc; ++c) (*chunk_prob)[c_lo + c] = b;
+    m_lo += ns[b];
+    c_lo += nc;
+  }
+  return TZR_OK;
+}
+
+IcpLayout icp_layout(const IcpPlan& plan, size_t base, bool information) {
+  const int stride = std::max(icp_partial_stride(plan.mode), information ? kIcpInfoSums : 0);
+  IcpLayout L;
+  L.probs = base;
+  L.clouds = L.probs + al256((size_t)plan.B * sizeof(IcpProb));
+  L.chunks = L.clouds + al256((size_t)plan.grid.B * sizeof(FpfhCloud));
+  L.match = L.chunks + al256((size_t)plan.chunks * 4);
+  L.partial = L.match + al256((size_t)plan.NS * 4);
+  L.grid = L.partial + al256((size_t)plan.chunks * stride * 8);
+  L.info = L.counts = L.end = L.grid + plan.grid.grid_bytes;
+  if (information) {
+    L.info = al256(L.end);
+    L.counts = L.info + al256((size_t)plan.B * 36 * 8);
+    L.end = L.counts + (size_t)plan.B * 4;
+  }
+  return L;
+}
+
+IcpBuffers icp_buffers(char* d, const IcpLayout& L) {
+  return IcpBuffers{nullptr, nullptr, nullptr, nullptr, (IcpProb*)(d + L.probs), (FpfhCloud*)(d + L.clouds),
+                    (const int*)(d + L.chunks), (int*)(d + L.match), (double*)(d + L.partial), d + L.grid,
+                    (double*)(d + L.info), (int*)(d + L.counts)};
+}
+
+int launch_icp_information(const IcpPlan& plan, const IcpBuffers& buf, bool reseed, cudaStream_t st,
+                           const IcpGrid* grid) {
   int nl = 0;
-  IcpArgs a{src, dst, probs, clouds, chunk_prob, match, partial, nullptr, nullptr, nullptr, plan.r2};
+  IcpArgs a{buf.src, buf.dst, buf.probs, buf.clouds, buf.chunk_prob, buf.match, buf.partial, nullptr, nullptr, nullptr,
+            plan.r2};
   if (reseed) {
-    icp_info_seed_kernel<<<(plan.B + 127) / 128, 128, 0, st>>>(probs, plan.B);
+    icp_info_seed_kernel<<<(plan.B + 127) / 128, 128, 0, st>>>(buf.probs, plan.B);
     ++nl;
   }
   if (grid) {  // launch_icp's grid over the same targets, still in grid_scratch
@@ -755,11 +826,11 @@ int launch_icp_information(const IcpPlan& plan, const float* src, const float* d
     a.bstart = grid->bstart;
     a.bend = grid->bend;
   } else if (plan.grid.any_grid) {
-    nl += launch_fpfh_grid(plan.grid, dst, clouds, grid_scratch, st, &a.sorted, &a.bstart, &a.bend);
+    nl += launch_fpfh_grid(plan.grid, buf.dst, buf.clouds, buf.grid_scratch, st, &a.sorted, &a.bstart, &a.bend);
   }
   icp_nn_kernel<<<plan.chunks, kIcpThreads, 0, st>>>(a);
   icp_info_kernel<<<plan.chunks, kIcpThreads, 0, st>>>(a);
-  icp_info_combine_kernel<<<plan.B, 32, 0, st>>>(a, info, counts);
+  icp_info_combine_kernel<<<plan.B, 32, 0, st>>>(a, buf.info, buf.counts);
   return nl + 3;
 }
 
@@ -768,12 +839,12 @@ int launch_icp_seed(IcpProb* probs, int B, const tzr_solution* sol, cudaStream_t
   return 1;
 }
 
-int launch_icp(const IcpPlan& plan, const float* src, const float* dst, const float4* src_normals,
-               const float4* dst_normals, IcpProb* probs, FpfhCloud* clouds, const int* chunk_prob, int* match,
-               double* partial, void* grid_scratch, cudaStream_t st, IcpGrid* grid_out) {
+int launch_icp(const IcpPlan& plan, const IcpBuffers& buf, cudaStream_t st, IcpGrid* grid_out) {
   int nl = 0;
-  IcpArgs a{src, dst, probs, clouds, chunk_prob, match, partial, nullptr, nullptr, nullptr, plan.r2};
-  if (plan.grid.any_grid) nl += launch_fpfh_grid(plan.grid, dst, clouds, grid_scratch, st, &a.sorted, &a.bstart, &a.bend);
+  IcpArgs a{buf.src, buf.dst, buf.probs, buf.clouds, buf.chunk_prob, buf.match, buf.partial, nullptr, nullptr, nullptr,
+            plan.r2};
+  if (plan.grid.any_grid)
+    nl += launch_fpfh_grid(plan.grid, buf.dst, buf.clouds, buf.grid_scratch, st, &a.sorted, &a.bstart, &a.bend);
   if (grid_out) *grid_out = IcpGrid{a.sorted, a.bstart, a.bend};
   icp_nn_kernel<<<plan.chunks, kIcpThreads, 0, st>>>(a);
   icp_eval_kernel<<<plan.B, 32, 0, st>>>(a, plan.max_iteration, plan.relative_fitness, plan.relative_rmse);
@@ -781,17 +852,18 @@ int launch_icp(const IcpPlan& plan, const float* src, const float* dst, const fl
   for (int it = 0; it < plan.max_iteration; ++it) {
     if (plan.mode == kIcpPointToPlane) {
       if (plan.loss == TZR_LOSS_L2)
-        icp_plane_system_kernel<false><<<plan.chunks, kIcpThreads, 0, st>>>(a, dst_normals, 0, 0.0);
+        icp_plane_system_kernel<false><<<plan.chunks, kIcpThreads, 0, st>>>(a, buf.dst_normals, 0, 0.0);
       else
-        icp_plane_system_kernel<true><<<plan.chunks, kIcpThreads, 0, st>>>(a, dst_normals, plan.loss, plan.loss_k);
+        icp_plane_system_kernel<true><<<plan.chunks, kIcpThreads, 0, st>>>(a, buf.dst_normals, plan.loss,
+                                                                           plan.loss_k);
       icp_plane_update_kernel<<<plan.B, 32, 0, st>>>(a);
     } else if (plan.mode == kIcpGeneralized) {
       if (plan.loss == TZR_LOSS_L2)
-        icp_gicp_system_kernel<false><<<plan.chunks, kIcpThreads, 0, st>>>(a, src_normals, dst_normals, plan.epsilon, 0,
-                                                                           0.0);
+        icp_gicp_system_kernel<false><<<plan.chunks, kIcpThreads, 0, st>>>(a, buf.src_normals, buf.dst_normals,
+                                                                           plan.epsilon, 0, 0.0);
       else
-        icp_gicp_system_kernel<true><<<plan.chunks, kIcpThreads, 0, st>>>(a, src_normals, dst_normals, plan.epsilon,
-                                                                          plan.loss, plan.loss_k);
+        icp_gicp_system_kernel<true><<<plan.chunks, kIcpThreads, 0, st>>>(a, buf.src_normals, buf.dst_normals,
+                                                                          plan.epsilon, plan.loss, plan.loss_k);
       icp_plane_update_kernel<<<plan.B, 32, 0, st>>>(a);
     } else {
       icp_cov_kernel<<<plan.chunks, kIcpThreads, 0, st>>>(a);

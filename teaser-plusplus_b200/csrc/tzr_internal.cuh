@@ -27,6 +27,8 @@ __host__ __device__ inline int next_pow2(int v) {
   while (p < v) p <<= 1;
   return p;
 }
+// byte offsets of workspace regions: every region starts on a 256-byte boundary
+inline size_t al256(size_t x) { return (x + 255) & ~(size_t)255; }
 
 constexpr int kTile = 128;          // graph tile edge (pairs per tile = 128*128)
 constexpr int kGraphThreads = 128;  // 4 warps, each owns a 32x128 sub-tile (4 pairs per lane per step)
@@ -313,9 +315,14 @@ struct FpfhPlan {
   unsigned int buckets = 0;    // sum of T_b over the grid clouds (also the sentinel key of unsorted points)
   size_t grid_bytes = 0;       // device scratch of the grid path (0 without grid clouds)
 };
-// Radius-search route of every cloud: by size (the grid from kGridMinN points on), or forced by the debug flags
-// 4194304 (brute force) and 8388608 (the grid at any size).
+// Radius-search route of every cloud: by size (the grid from kGridMinN points on), or forced by a debug flag pair:
+// brute force or the grid at any size, bits 22 / 23 for the descriptor stage and bits 25 / 26 for ICP's target search.
 constexpr int kFpfhRouteAuto = 0, kFpfhRouteBrute = 1, kFpfhRouteGrid = 2;
+constexpr uint32_t kFlagFpfhBrute = 1u << 22, kFlagFpfhGrid = 1u << 23;
+constexpr uint32_t kFlagIcpBrute = 1u << 25, kFlagIcpGrid = 1u << 26;
+inline int search_route(uint32_t flags, uint32_t brute, uint32_t grid) {
+  return (flags & brute) ? kFpfhRouteBrute : (flags & grid) ? kFpfhRouteGrid : kFpfhRouteAuto;
+}
 // Fills clouds[0..B) (host copy, to be staged to the device before launch_fpfh) and the plan.  TZR_ERR_TOO_LARGE when
 // the points or buckets of the batch do not fit 32-bit indices.  grid_min_n: the size from which kFpfhRouteAuto uses
 // the grid (-1: the descriptor stage's own, 4096).
@@ -429,8 +436,8 @@ int launch_pair_rows(const MatchPlan& plan, const MatchPair* pairs, const int2* 
 int launch_corr_gather(const PairGather* table, int n_entries, int max_count, const int32_t* pairs, const float* pts,
                        int2* corr, double* src, double* dst, cudaStream_t st);
 
-// icp.cu (point-to-point ICP, DESIGN.md §3.11, point-to-plane ICP, §3.13, and generalized ICP, §3.14): B problems,
-// sources back to back and targets back to back
+// icp.cu (point-to-point ICP, DESIGN.md §3.11, point-to-plane ICP, §3.13, and generalized ICP, §3.14): B problems
+// over flat source and target point arrays
 constexpr int kIcpChunk = 256;    // source points per chunk: the unit of the fixed-order reductions (one CTA each)
 constexpr int kIcpGridMinN = 1024;  // targets from which the nearest-neighbour search goes through the hashed grid
 constexpr int kIcpPointToPoint = 0, kIcpPointToPlane = 1, kIcpGeneralized = 2;  // IcpPlan::mode
@@ -440,7 +447,7 @@ constexpr int kIcpPlaneSums = 27;
 inline int icp_partial_stride(int mode) { return mode == kIcpPointToPoint ? 9 : kIcpPlaneSums; }
 struct IcpProb {        // one per problem, device-resident; the host fills the inputs, the kernels the rest
   int s_lo, ns;         // sources: flat points [s_lo, s_lo + ns)
-  int d_lo, nd;         // targets: flat points [d_lo, d_lo + nd) (also FpfhCloud b of the target table)
+  int d_lo, nd;         // targets: flat points [d_lo, d_lo + nd) (also FpfhCloud tc of the target table)
   int c_lo;             // first chunk of the problem (chunks are consecutive)
   int active;           // 0: finished (converged or max_iteration reached); every kernel skips the problem
   int iterations, converged;
@@ -467,13 +474,48 @@ struct IcpPlan {
   double loss_k = 0;
   FpfhPlan grid;        // the target grid (fpfh_plan with both radii = r)
 };
-// src (NS x 3 floats), dst (ND x 3 floats), src_normals (generalized: the source normals, (nx, ny, nz, curvature) per
-// point; unused and may be nullptr otherwise), dst_normals (point-to-plane and generalized: the target normals, same
-// layout; unused and may be nullptr for point-to-point), probs (B), clouds (B, fpfh_plan's table of the targets),
-// chunk_prob (chunks: the problem of every chunk), match (target index or -1 per source point from m_lo, final
-// correspondences), partial (chunks x icp_partial_stride(plan.mode) doubles), grid_scratch (plan.grid.grid_bytes): device
-// pointers.  Enqueues every iteration without synchronising; returns the launches: 4 for the grid build (when some target
-// uses it) + 2 + 4 * max_iteration, in every mode.
+constexpr int kIcpInfoSums = 21;  // doubles per chunk of launch_icp_information's partial buffer
+// The tables of B problems against T target clouds of nt[0..T) points, back to back in the flat target array: problem
+// b refines ns[b] sources from flat point s_lo[b] (s_lo nullptr: the sources back to back) onto target cloud tc[b]
+// (tc nullptr: cloud b).  Fills plan's B, NS, ND, chunks, r2 and grid (route: the targets' search route), clouds (T,
+// the targets' fpfh_plan table), probs (B; m_lo and c_lo running sums, the normals indexed like the points) and
+// chunk_prob (chunks: the problem of every chunk).  init (may be nullptr): the problems' transforms, which makes them
+// active and seeded; without it every problem waits for launch_icp_seed.  The other fields of plan are left as they
+// are.  TZR_ERR_TOO_LARGE when the sources, the targets or the grid do not fit 32-bit indices.
+int icp_plan(int B, const int32_t* ns, const int32_t* s_lo, const int32_t* tc, int T, const int32_t* nt, double r,
+             int route, const tzr_similarity* init, IcpPlan* plan, std::vector<FpfhCloud>* clouds,
+             std::vector<IcpProb>* probs, std::vector<int>* chunk_prob);
+// Byte offsets of an ICP workspace from `base` on: [problems | target clouds | chunks | matches | partials | grid
+// scratch | information | counts]; the last two are empty without `information`, whose partials have room for both
+// launch_icp's sums and kIcpInfoSums.  end: the workspace's size.
+struct IcpLayout {
+  size_t probs, clouds, chunks, match, partial, grid, info, counts, end;
+};
+IcpLayout icp_layout(const IcpPlan& plan, size_t base, bool information);
+// The device buffers of launch_icp and launch_icp_information.  src (NS x 3 floats), dst (ND x 3 floats), src_normals
+// (generalized: the source normals, (nx, ny, nz, curvature) per point; may be nullptr otherwise), dst_normals
+// (point-to-plane and generalized: the target normals, same layout; may be nullptr for point-to-point), probs (B),
+// clouds (icp_plan's table of the targets), chunk_prob (chunks), match (target index or -1 per source point from m_lo,
+// final correspondences), partial (chunks x icp_partial_stride(plan.mode) doubles, kIcpInfoSums for the information
+// matrices), grid_scratch (plan.grid.grid_bytes), info (B x 36 doubles) and counts (B ints).
+struct IcpBuffers {
+  const float* src;
+  const float* dst;
+  const float4* src_normals;
+  const float4* dst_normals;
+  IcpProb* probs;
+  FpfhCloud* clouds;
+  const int* chunk_prob;
+  int* match;
+  double* partial;
+  void* grid_scratch;
+  double* info;
+  int* counts;
+};
+// the table and scratch buffers of a workspace at d laid out by L; the points and normals are left nullptr
+IcpBuffers icp_buffers(char* d, const IcpLayout& L);
+// Enqueues every iteration without synchronising; returns the launches: 4 for the grid build (when some target uses
+// it) + 2 + 4 * max_iteration, in every mode.  info and counts are not used.
 // grid_out (may be nullptr): the target grid's sorted indices and bucket ranges inside grid_scratch (all nullptr without
 // grid targets), for launch_icp_information to reuse.
 struct IcpGrid {
@@ -481,23 +523,19 @@ struct IcpGrid {
   const int* bstart;
   const int* bend;
 };
-int launch_icp(const IcpPlan& plan, const float* src, const float* dst, const float4* src_normals,
-               const float4* dst_normals, IcpProb* probs, FpfhCloud* clouds, const int* chunk_prob, int* match,
-               double* partial, void* grid_scratch, cudaStream_t st, IcpGrid* grid_out = nullptr);
+int launch_icp(const IcpPlan& plan, const IcpBuffers& buf, cudaStream_t st, IcpGrid* grid_out = nullptr);
 // The seeds of B problems from B solution records (tzr_register_cloud_pairs_icp): a valid record with a finite transform
 // and a positive scale sets (s, R, t) and active = seeded = 1, any other leaves the problem inactive.  One launch.
 int launch_icp_seed(IcpProb* probs, int B, const tzr_solution* sol, cudaStream_t st);
 // Information matrices (tzr_information_matrix_batch, DESIGN.md §3.16) of B problems at their current transforms: the
 // grid build (when some target uses it), icp_nn_kernel as launch_icp runs it, then the 21 sums of G^T G per chunk into
-// partial (chunks x kIcpInfoSums doubles) and their fixed-order combination into info (B x 36 doubles, device) and
-// counts (B ints, device).  reseed: set active = seeded first (a chained call, after launch_icp finished its problems);
-// otherwise the problems must be active.  A problem that is not seeded gets zeros.  grid (may be nullptr): launch_icp's
-// grid of the same targets, reused instead of built again.  Returns the launches: 3, + 1 with reseed, + 4 for the grid
-// build when some target uses the grid and grid is nullptr.
-constexpr int kIcpInfoSums = 21;
-int launch_icp_information(const IcpPlan& plan, const float* src, const float* dst, IcpProb* probs, FpfhCloud* clouds,
-                           const int* chunk_prob, int* match, double* partial, void* grid_scratch, bool reseed,
-                           double* info, int* counts, cudaStream_t st, const IcpGrid* grid = nullptr);
+// partial and their fixed-order combination into info and counts.  The normals are not used.  reseed: set active =
+// seeded first (a chained call, after launch_icp finished its problems); otherwise the problems must be active.  A
+// problem that is not seeded gets zeros.  grid (may be nullptr): launch_icp's grid of the same targets, reused instead
+// of built again.  Returns the launches: 3, + 1 with reseed, + 4 for the grid build when some target uses the grid and
+// grid is nullptr.
+int launch_icp_information(const IcpPlan& plan, const IcpBuffers& buf, bool reseed, cudaStream_t st,
+                           const IcpGrid* grid = nullptr);
 
 // pose_graph.cu (tzr_pose_graph_optimize, DESIGN.md §3.16): one graph of K nodes and E edges, device-resident
 struct PgEdge {         // one per edge; the host fills it, the kernels read it
