@@ -154,7 +154,9 @@ int tzr_ctx_set_max_n(tzr_ctx* ctx, int max_n);
  * entries; TZR_ERR_INVALID_ARG once another call has reused the workspace): 0 = small route; k > 0 = large route with
  * the core compacted to k vertices, where k equal to the clique size means the core was the clique itself (or a
  * heuristic mode, or a clique of size <= 1) and no search ran; -1 = large route whose core kept more vertices than the
- * cap, the heuristic clique is returned with clique_proven_optimal = 0 (search flags 1 | 16). */
+ * cap, the heuristic clique is returned with clique_proven_optimal = 0 (search flags 1 | 16).  k and the cap test
+ * always refer to the (L-1)-core itself, never to a superset of it: a graph that peels slowly (long pendant paths)
+ * is peeled on until its core is reached. */
 int tzr_ctx_clique_route(tzr_ctx* ctx, int32_t* per_problem);
 
 /* ---- stage 3: GNC-TLS rotation --------------------------------------------------------------

@@ -528,7 +528,7 @@ class Context:
     def clique_route(self, B: int):
         """(B,) int32 clique route of each problem of the most recent clique stage: 0 small route, k > 0 large route
         with the core compacted to k vertices (k = clique size: no search ran), -1 core above the cap (heuristic
-        clique, not proven)."""
+        clique, not proven).  k and the cap test refer to the (L-1)-core itself, never to a superset of it."""
         out = np.zeros(B, dtype=np.int32)
         self._ck(lib().tzr_ctx_clique_route(self._h, _p(out, C.c_int32)))
         return out

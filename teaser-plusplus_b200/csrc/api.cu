@@ -523,7 +523,11 @@ int l2_chunk(const tzr_ctx* ctx, int B, int n, const tzr_params& p) {
 // Large clique route (DESIGN.md §3.2), taken when n > kMaxN or under debug flag 524288: the heuristic on the full graph,
 // its (L-1)-core on many CTAs, the cores compacted (order-preserving) into a batch of at most kMaxN vertices per problem
 // (64 under debug flag 1048576), the small route's peel and exact passes on that batch, the cliques mapped back.  One
-// host read-back: the core sizes, which size the compacted batch.  route: B entries as tzr_ctx_clique_route reports them.
+// host read-back: the core sizes, which size the compacted batch, with each problem's last change counter.  A problem
+// whose last round still removed vertices holds a superset of its core (a pendant path loses one or two vertices per
+// round); while such a problem would be searched or capped, further blocks of kCoreRounds rounds run on it, each with
+// its own read-back, so that every decision below is made on the core.  Graphs that converge inside the first block
+// take no extra launch.  route: B entries as tzr_ctx_clique_route reports them.
 int run_clique_large(tzr_ctx* ctx, const Batch& bt, const tzr_params& p, int mode, cudaStream_t st, int* nl,
                      int32_t* route) {
   const int B = bt.B, n = bt.n;
@@ -534,7 +538,7 @@ int run_clique_large(tzr_ctx* ctx, const Batch& bt, const tzr_params& p, int mod
     off = al256(off + bytes);
     return o;
   };
-  const size_t o_lists = carve(Bn * kHeurRoots * 2 * sizeof(uint16_t)), o_chg = carve((size_t)B * kCoreRounds * 4),
+  const size_t o_lists = carve(Bn * kHeurRoots * 2 * sizeof(uint16_t)), o_chg = carve((size_t)B * kCoreSlots * 4),
                o_n2o = carve(Bn * 4), o_o2n = carve(Bn * 4), o_cnt = carve((size_t)B * 4), o_route = carve((size_t)B * 4);
   int rc = ensure(ctx, ctx->lg, off);
   if (rc) return rc;
@@ -543,12 +547,39 @@ int run_clique_large(tzr_ctx* ctx, const Batch& bt, const tzr_params& p, int mod
   int32_t* o2n = (int32_t*)(lg + o_o2n);
   int32_t* cnt_d = (int32_t*)(lg + o_cnt);
   int32_t* route_d = (int32_t*)(lg + o_route);
+  int32_t* chg_d = (int32_t*)(lg + o_chg);
   launch_clique_large_front(bt, p, mode, (uint16_t*)(lg + o_lists), st, nl);
-  std::vector<int32_t> L(B), cnt(B, 0);
-  if (mode == 0) launch_core(bt, (int32_t*)(lg + o_chg), n2o, o2n, cnt_d, ctx->num_sms, st, nl);
+  std::vector<int32_t> L(B), cnt(B, 0), last(B, 0);
+  // the core sizes and each problem's last change counter (slot kCoreRounds: removals in the block's last round)
+  auto read_core = [&]() -> int {
+    CK(cudaMemcpyAsync(cnt.data(), cnt_d, (size_t)B * 4, cudaMemcpyDeviceToHost, st));
+    CK(cudaMemcpy2DAsync(last.data(), 4, chg_d + kCoreRounds, (size_t)kCoreSlots * 4, 4, (size_t)B,
+                         cudaMemcpyDeviceToHost, st));
+    return TZR_OK;
+  };
+  if (mode == 0) launch_core(bt, chg_d, n2o, o2n, cnt_d, ctx->num_sms, st, nl);
   CK(cudaMemcpyAsync(L.data(), bt.L, (size_t)B * 4, cudaMemcpyDeviceToHost, st));
-  if (mode == 0) CK(cudaMemcpyAsync(cnt.data(), cnt_d, (size_t)B * 4, cudaMemcpyDeviceToHost, st));
+  if (mode == 0 && (rc = read_core())) return rc;
   CK(cudaStreamSynchronize(st));
+  if (mode == 0) {
+    // peel on while a problem that would be searched or capped still shrinks (L <= 1 and the shortcut are final: a
+    // set of exactly L survivors is the incumbent itself)
+    std::vector<int32_t> go((size_t)B * kCoreSlots);
+    for (;;) {
+      std::fill(go.begin(), go.end(), 0);
+      bool more = false;
+      for (int b = 0; b < B; ++b)
+        if (L[b] > 1 && cnt[b] != L[b] && last[b] != 0) {
+          go[(size_t)b * kCoreSlots] = 1;
+          more = true;
+        }
+      if (!more) break;
+      CK(cudaMemcpyAsync(chg_d, go.data(), go.size() * 4, cudaMemcpyHostToDevice, st));
+      launch_core_rounds(bt, chg_d, n2o, o2n, cnt_d, ctx->num_sms, st, nl);
+      if ((rc = read_core())) return rc;
+      CK(cudaStreamSynchronize(st));
+    }
+  }
   // heuristic modes, L <= 1 and the uniqueness shortcut (only the incumbent survives its own core bound): the result is
   // final, reported as the clique size (at least 1)
   const int cap = (ctx->flags & 1048576u) ? 64 : kMaxN;

@@ -365,11 +365,13 @@ __device__ int block_popcount(const uint32_t* S, int W, int* s_cnt) {
   return *s_cnt;
 }
 
-// Peel S in place to its k-core (vertices with >= k neighbours inside the set).  Sn: scratch of W words.
+// Peel S in place to its k-core (vertices with >= k neighbours inside the set).  Sn: scratch of W words.  Runs to
+// convergence (a round removes at least one vertex, so at most n + 1 rounds): a pendant path loses one vertex per
+// layered round, and a set stopped early would be a superset whose size the shortcut and the second chance misread.
 __device__ void peel_to_core(const Batch& bt, int b, uint32_t* S, uint32_t* Sn, int W, int k, int* s_changed) {
   for (int x = threadIdx.x; x < W; x += blockDim.x) Sn[x] = S[x];
   __syncthreads();
-  for (int round = 0; round < 256; ++round) {
+  for (int round = 0; round <= bt.n; ++round) {
     peel_round(bt, b, S, Sn, W, k, nullptr, s_changed);
     const int ch = *s_changed;
     for (int x = threadIdx.x; x < W; x += blockDim.x) S[x] = Sn[x];
@@ -1690,12 +1692,12 @@ __global__ void clique_resume_kernel(Batch bt) {
 // from the heuristic cliques; every clique of size >= L lies inside the (L-1)-core.
 // =================================================================================================
 
-// alive0 = {v : deg[v] >= L - 1} (the first peel round, from the degrees the graph stage already has); zeroes the
-// per-round change counters.  Grid (ceil(W / 256), B).
+// alive0 = {v : deg[v] >= L - 1} (the first peel round, from the degrees the graph stage already has); sets the
+// problem's change counters to "peel on" (slot 0) and no removals yet (slots 1 ... kCoreRounds).  Grid (ceil(W / 256), B).
 __global__ void __launch_bounds__(256) core_init_kernel(Batch bt, int32_t* chg) {
   const int b = blockIdx.y, n = bt.n, W = pitch32(n);
   const int x = blockIdx.x * 256 + threadIdx.x;
-  if (blockIdx.x == 0 && threadIdx.x < kCoreRounds) chg[b * kCoreRounds + threadIdx.x] = 0;
+  if (blockIdx.x == 0 && threadIdx.x <= kCoreRounds) chg[b * kCoreSlots + threadIdx.x] = threadIdx.x == 0 ? 1 : 0;
   if (x >= W) return;
   const int thr = bt.L[b] - 1;
   const int32_t* deg = bt.deg + (size_t)b * n;
@@ -1710,12 +1712,14 @@ __global__ void __launch_bounds__(256) core_init_kernel(Batch bt, int32_t* chg) 
 // One peel round over every problem, one warp per alive word (grid-stride), four vertices at a time.  Degrees count
 // only the alive words of the set, and each row word is loaded only where the set has vertices.  The set is peeled in
 // place: a vertex whose degree inside some superset of the core is below L - 1 is not in the core, so concurrent
-// removals only speed convergence.  A round that removes nothing proves the set is the core; later rounds return at
-// once (chg[r - 1] == 0).  Grid (ctas, B).
+// removals only speed convergence.  Round r of a block runs while slot r of the problem's counters is non-zero (slot 0:
+// the block is to peel this problem, slot r > 0: round r - 1 removed something) and counts its removals in slot r + 1,
+// so a round that removes nothing proves the set is the core and the block's later rounds return at once.
+// Grid (ctas, B).
 __global__ void __launch_bounds__(256) core_round_kernel(Batch bt, int32_t* chg, int r) {
   const int b = blockIdx.y, n = bt.n, W = pitch32(n);
-  int32_t* cb = chg + b * kCoreRounds;
-  if (r > 0 && *(volatile int32_t*)(cb + r - 1) == 0) return;
+  int32_t* cb = chg + b * kCoreSlots;
+  if (*(volatile int32_t*)(cb + r) == 0) return;
   const int thr = bt.L[b] - 1;
   if (thr <= 0) return;  // L <= 1: nothing to peel
   uint32_t* S = bt.alive + (size_t)b * W;
@@ -1759,7 +1763,7 @@ __global__ void __launch_bounds__(256) core_round_kernel(Batch bt, int32_t* chg,
       }
     }
   }
-  if (removed) atomicAdd(cb + r, 1);
+  if (removed) atomicAdd(cb + r + 1, 1);
 }
 
 // Survivors in ascending order: new2old[0..cnt) and old2new[v] for every survivor; core_cnt[b] = cnt.  One CTA per
@@ -1957,14 +1961,21 @@ void launch_clique_large_front(const Batch& bt, const tzr_params& p, int mode, u
   if (n_launches) *n_launches += launches;
 }
 
+void launch_core_rounds(const Batch& bt, int32_t* chg, int32_t* new2old, int32_t* old2new, int32_t* core_cnt,
+                        int num_sms, cudaStream_t st, int* n_launches) {
+  const int W = pitch32(bt.n);
+  const int per = std::max(1, std::min((W + 7) / 8, (2 * num_sms + bt.B - 1) / bt.B));
+  for (int r = 0; r < kCoreRounds; ++r) core_round_kernel<<<dim3((unsigned)per, (unsigned)bt.B), 256, 0, st>>>(bt, chg, r);
+  core_list_kernel<<<bt.B, kPeelThreads, 0, st>>>(bt, new2old, old2new, core_cnt);
+  if (n_launches) *n_launches += kCoreRounds + 1;
+}
+
 void launch_core(const Batch& bt, int32_t* chg, int32_t* new2old, int32_t* old2new, int32_t* core_cnt, int num_sms,
                  cudaStream_t st, int* n_launches) {
   const int W = pitch32(bt.n);
   core_init_kernel<<<dim3((unsigned)((W + 255) / 256), (unsigned)bt.B), 256, 0, st>>>(bt, chg);
-  const int per = std::max(1, std::min((W + 7) / 8, (2 * num_sms + bt.B - 1) / bt.B));
-  for (int r = 0; r < kCoreRounds; ++r) core_round_kernel<<<dim3((unsigned)per, (unsigned)bt.B), 256, 0, st>>>(bt, chg, r);
-  core_list_kernel<<<bt.B, kPeelThreads, 0, st>>>(bt, new2old, old2new, core_cnt);
-  if (n_launches) *n_launches += kCoreRounds + 2;
+  if (n_launches) *n_launches += 1;
+  launch_core_rounds(bt, chg, new2old, old2new, core_cnt, num_sms, st, n_launches);
 }
 
 size_t core_compact_smem(int n2) { return (size_t)8 * pitch32(n2) * 4; }

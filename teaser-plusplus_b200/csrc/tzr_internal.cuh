@@ -49,8 +49,9 @@ constexpr int kMaxN = 32768;        // per-problem size limit of the shared-memo
 constexpr int kMaxNLarge = 65536;   // per-problem size limit of the whole pipeline (tzr_ctx_set_max_n): the graph kernels'
                                     // re-check queue packs a pair as (i << 16) | j and the heuristic keeps u16 candidate
                                     // lists and in-set degrees, so every vertex index must fit 16 bits
-constexpr int kCoreRounds = 48;     // peel rounds (one launch each) of the large route's core; a set still shrinking
-                                    // after them is a superset of the core, which the compacted search peels again
+constexpr int kCoreRounds = 48;     // peel rounds (one launch each) per block of the large route's core peel; the host
+                                    // runs further blocks while a problem it would search or cap is still shrinking
+constexpr int kCoreSlots = kCoreRounds + 1;  // change counters per problem: "peel on" + one per round of a block
 
 // Per-problem constants of the FP32 filter (see graph_build.cu).
 struct GraphConsts {
@@ -249,13 +250,18 @@ bool scale_large(int n, uint32_t flags);
 int launch_scale_estimation(const Batch& bt, uint32_t flags, void* scratch, cudaStream_t st);
 void launch_rot_trans(const Batch& bt, const tzr_params& p, int use_clique, cudaStream_t st);
 // Large route (n > kMaxN or debug flag 524288; DESIGN.md §3.2).  lists: B * kHeurRoots * 2n u16 of heuristic scratch;
-// chg: B * kCoreRounds per-round change counters; new2old / old2new: B * n; core_cnt / route: B.  route[b] (device copy,
-// set by the host after reading core_cnt): > 0 search the compacted core, 0 not searched (result already final),
-// -1 core above the cap (heuristic clique, not proven).
+// chg: B * kCoreSlots change counters (slot 0: peel this problem in the next block of rounds; slot r + 1: removals in
+// round r of the block); new2old / old2new: B * n; core_cnt / route: B.  launch_core starts the peel (alive0 and one
+// block), launch_core_rounds runs one more block of kCoreRounds rounds on the problems whose slot 0 the host set, then
+// re-lists the survivors.  route[b] (device copy, set by the host once every problem it decides on holds its core):
+// > 0 search the compacted core, 0 not searched (result already final), -1 core above the cap (heuristic clique, not
+// proven).
 void launch_clique_large_front(const Batch& bt, const tzr_params& p, int mode, uint16_t* lists, cudaStream_t st,
                                int* n_launches);
 void launch_core(const Batch& bt, int32_t* chg, int32_t* new2old, int32_t* old2new, int32_t* core_cnt, int num_sms,
                  cudaStream_t st, int* n_launches);
+void launch_core_rounds(const Batch& bt, int32_t* chg, int32_t* new2old, int32_t* old2new, int32_t* core_cnt,
+                        int num_sms, cudaStream_t st, int* n_launches);
 void launch_core_compact(const Batch& bt, const Batch& cb, const int32_t* new2old, const int32_t* old2new,
                          const int32_t* core_cnt, const int32_t* route, cudaStream_t st, int* n_launches);
 void launch_clique_search(const Batch& cb, cudaStream_t st, int* n_launches);  // peel (mode 0) + the exact passes
