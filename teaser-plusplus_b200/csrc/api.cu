@@ -15,10 +15,102 @@
 
 using namespace tzr;
 
+// A grow-only device buffer (ensure), freed with its context.
 struct DevBuf {
   void* p = nullptr;
   size_t cap = 0;
+  DevBuf() = default;
+  DevBuf(const DevBuf&) = delete;
+  DevBuf& operator=(const DevBuf&) = delete;
+  ~DevBuf() {
+    if (p) cudaFree(p);
+  }
 };
+
+namespace {
+
+// What a per-problem buffer of a Batch holds: the input points (in the workspace only when the call owns them, not for
+// tzr_solve_batch_dev or a caller's bitsets), the clique state (carved again for the large route's compacted batch), or
+// the rest of the pipeline's per-problem state.
+enum BufKind { kPoints, kClique, kOther };
+
+// Every per-problem buffer of bt, in a fixed order: f(field, elements per problem, kind).  A batch's buffer holds its B
+// problems back to back, so problem b starts b * elements in.
+template <class F>
+void batch_buffers(Batch& bt, F&& f) {
+  const size_t n = (size_t)bt.n, W32 = (size_t)pitch32(bt.n), rot = (size_t)bt.rot_cap, sort = (size_t)bt.sort_cap;
+  f(bt.src, 3 * n, kPoints);
+  f(bt.dst, 3 * n, kPoints);
+  f(bt.sf, n, kOther);
+  f(bt.df, n, kOther);
+  f(bt.gq, 2 * n, kOther);
+  f(bt.pk, 6 * (size_t)npad128(bt.n), kOther);
+  f(bt.opnd, tc_operand_bytes(1, bt.n) / sizeof(float), kOther);
+  f(bt.gc, 1, kOther);
+  f(bt.adj, n * pitch64(bt.n), kClique);
+  f(bt.deg, n, kClique);
+  f(bt.n_edges2, 1, kClique);
+  f(bt.hclq, kHeurRoots * n, kClique);
+  f(bt.hsize, kHeurRoots, kClique);
+  f(bt.clq, n, kClique);
+  f(bt.L, 1, kClique);
+  f(bt.alive, W32, kClique);
+  f(bt.best_bits, W32, kClique);
+  f(bt.alive_cnt, 1, kClique);
+  f(bt.root_ctr, 1, kClique);
+  f(bt.lock, 1, kClique);
+  f(bt.flags, 1, kClique);
+  f(bt.kcore_final, 1, kClique);
+  f(bt.t_start, 1, kClique);
+  f(bt.ps, 3 * n, kOther);
+  f(bt.pd, 3 * n, kOther);
+  f(bt.wgt, rot, kOther);
+  f(bt.res, n, kOther);
+  f(bt.skey, 3 * sort, kOther);
+  f(bt.sidx, 3 * sort, kOther);
+  f(bt.sorted_clq, n, kOther);
+  f(bt.rot_mask, rot, kOther);
+  f(bt.trans_mask, n, kOther);
+  f(bt.sol, 1, kOther);
+}
+constexpr int kBatchBuffers = 33;  // the fields batch_buffers visits
+
+// Point a buffer field at byte `at` of a workspace allocation.
+template <class T>
+void point_at(T*& field, void* base, size_t at) {
+  field = (T*)((char*)base + at);
+}
+
+// Bytes of the exact phase's scratch (Batch::stack, cv, centry) for bt's persistent grid (exact_ctas, max_depth).
+struct ExactScratch {
+  size_t stack, cv, centry;
+};
+ExactScratch exact_scratch(const Batch& bt) {
+  const size_t warps = (size_t)bt.exact_ctas * 8;
+  return ExactScratch{warps * bt.max_depth * 2 * pitch32(bt.n) * sizeof(uint32_t),
+                      std::max(warps, (size_t)4 * bt.B) * bt.n * sizeof(int32_t),
+                      warps * bt.max_depth * sizeof(int32_t)};
+}
+
+// The retained result of the most recent solve or graph build: its size classes (one for a uniform solve or a graph
+// build) and where each problem lies in them; problem b is sub_batch(cls[at[b].c], at[b].k, 1).  Cleared whenever the
+// workspace is reused (forget_retained).
+struct Retained {
+  struct Problem {
+    int c, k, n;  // class, index in the class, own correspondences (<= the class's n)
+  };
+  std::vector<Batch> cls;
+  std::vector<Problem> at;  // per problem in the caller's order; empty: nothing retained
+  bool is_solve = false;    // every problem's record, clique, masks and inputs are in the workspace (tzr_last_inliers,
+                            // tzr_certify_last_solve); false after tzr_graph_build
+  bool complete = false;    // its rotation ran on COMPLETE TIMs
+  bool has_graph = false;   // false: the solve ran with inlier selection NONE (no graph was built)
+  // clique route of every problem of the most recent clique stage, a solve's or tzr_max_clique(_batch)'s, in the
+  // caller's order (tzr_ctx_clique_route); empty after NONE or a graph build
+  std::vector<int32_t> route;
+};
+
+}  // namespace
 
 struct tzr_ctx {
   int device = 0;
@@ -28,10 +120,12 @@ struct tzr_ctx {
   int64_t launches = 0;
   uint32_t flags = 0;
   int num_sms = 132;
-  // device buffers (grow-only)
-  DevBuf src, dst, sf, df, gq, pk, opnd, tclist, gc, adj, deg, nedges, hclq, hsize, clq, L, alive, best_bits, alive_cnt, root_ctr, lock, flg, kfinal, tstart, stack, cv,
-      centry, ps, pd, wgt, res, skey, sidx, sorted, rmask, tmask, sol, dbg, misc, sc, m_in, m_scratch, m_out,
-      certb;
+  // the solve's workspace: one buffer per field of batch_buffers, in its order, then the buffers every size class
+  // shares: the re-check queue, the exact-phase scratch and the debug counters
+  DevBuf ws[kBatchBuffers];
+  DevBuf tclist, stack, cv, centry, dbg;
+  // the single-stage entry points, the unknown-scale stage, the front end and the certifier
+  DevBuf misc, sc, m_in, m_scratch, m_out, certb;
   // large clique route (n > kMaxN or debug flag 524288): scratch on the full graph, and the compacted batch's buffers
   DevBuf lg, cq;
   // ragged batches (DESIGN.md §4.2): the size-class tables, and the flat inputs / outputs of host-pointer calls
@@ -47,13 +141,7 @@ struct tzr_ctx {
   // pinned host staging
   void* h_pin = nullptr;
   size_t h_pin_cap = 0;
-  // last batch geometry
-  Batch last{};
-  bool have_last = false;
-  // the retained call was a solve: every problem's record, clique, masks and inputs are still in the workspace
-  // (tzr_last_inliers, tzr_certify_last_solve); last_complete: its rotation ran on COMPLETE TIMs
-  bool last_is_solve = false;
-  bool last_complete = false;
+  Retained last;
   cudaEvent_t ev[5] = {nullptr, nullptr, nullptr, nullptr, nullptr};  // start | prep | graph tiles | clique (incl. degrees) | rot+trans
   std::vector<cudaEvent_t> graph_ev;  // pairs around every graph-kernel launch of the last call (roofline timing)
   int graph_ev_used = 0;
@@ -62,7 +150,6 @@ struct tzr_ctx {
   bool stage_log = false;  // keep the events of every call since the last tzr_ctx_stage_log_read (bench.py: no sync per step)
   int stage_log_calls = 0;
   uint64_t generation = 0;   // bumped by every call that rebuilds or invalidates the retained graph (ctx->last)
-  bool last_has_graph = false;  // false: the last solve ran with inlier selection NONE (no graph was built)
   // chunked batches run on two lanes: the issue-bound graph kernels queue back to back on the low-priority gstream,
   // the latency-/HBM-bound degree, clique and rotation kernels of the previous chunk run on the high-priority hstream
   // and slot into the SMs as graph CTAs retire
@@ -72,25 +159,8 @@ struct tzr_ctx {
   void* solver_handle = nullptr;  // cusolverDnHandle_t of the certifier, created on first use (certify.cu)
   cudaStream_t copy_stream = nullptr;  // H2D of chunk k+1 overlaps the kernels of chunk k (host-pointer batches)
   std::vector<cudaEvent_t> chunk_ev;
-  // geometry of the most recent tzr_max_clique(_batch) call (tzr_ctx_clique_info); clique_B = 0 once the workspace is reused
-  int clique_B = 0;
-  int clique_geom[3] = {0, 0, 0};  // exact_ctas, exact_conc, max_depth
-  // clique route of every problem of the most recent clique stage (tzr_ctx_clique_route); route_B = 0 once reused
-  std::vector<int32_t> route;
-  int route_B = 0;
-  // retained results of a ragged solve, per problem in the caller's order (empty after a uniform one): its padded slot
-  struct RaggedGraph {
-    const uint64_t* adj;  // n_pad rows of pitch64(n_pad) words; the problem's graph is the first n rows
-    const int32_t* deg;
-    int n, n_pad;
-    const double* src;    // its points (n_pad rows, the first n its own)
-    const double* dst;
-    const tzr_solution* sol;
-    const int32_t* clq;   // sorted clique row
-    const uint8_t* rmask; // rotation inlier mask (rot_cap of its class)
-    const uint8_t* tmask; // translation inlier mask
-  };
-  std::vector<RaggedGraph> ragged_last;
+  // the batch of the most recent tzr_max_clique(_batch) call (tzr_ctx_clique_info); B = 0 once the workspace is reused
+  Batch clique{};
 };
 
 namespace {
@@ -255,6 +325,38 @@ void search_geometry(const tzr_ctx* ctx, int B, int n, int* ctas, int* depth_out
   }
 }
 
+// Nothing is retained any more: the workspace is about to be reused, or a call solved nothing.
+void forget_retained(tzr_ctx* ctx) {
+  ctx->last = Retained{};
+  ++ctx->generation;
+}
+
+// Retain the size classes of the call that just ran.  Problem s in class order (the classes' problems back to back) is
+// problem order[s] of the caller, with n[order[s]] correspondences of its own; order and n are nullptr for one class in
+// the caller's order.  route: the clique routes in class order.  p: the solve's parameters, nullptr for a graph without
+// solution records (tzr_graph_build).
+void retain(tzr_ctx* ctx, std::vector<Batch> cls, const int* order, const int32_t* n, const std::vector<int32_t>& route,
+            const tzr_params* p) {
+  Retained& r = ctx->last;
+  r.cls = std::move(cls);
+  r.is_solve = p != nullptr;
+  r.complete = p && p->rotation_tim_graph == 1;
+  r.has_graph = !p || effective_mode(*p) != 3;  // NONE: populateVertices is never called (registration.cc:607-650)
+  int B = 0;
+  for (const Batch& bt : r.cls) B += bt.B;
+  r.at.assign((size_t)B, Retained::Problem{});
+  r.route.assign(r.has_graph ? route.size() : 0, 0);
+  for (int c = 0, s = 0; c < (int)r.cls.size(); ++c) {
+    Batch& bt = r.cls[c];
+    for (int k = 0; k < bt.B; ++k, ++s) {
+      const int q = order ? order[s] : s;
+      r.at[q] = Retained::Problem{c, k, n ? n[q] : bt.n};
+      if (!r.route.empty()) r.route[q] = route[s];
+    }
+    bt.nb_host = nullptr;  // the call's own host copy, gone once it returns
+  }
+}
+
 // Size the workspace for C size classes (class c: B[c] problems of n[c] correspondences) and fill one Batch descriptor
 // per class (src/dst left to the caller unless own_points).  Per-problem buffers hold the classes back to back in class
 // order; the re-check queue, the exact-phase scratch and the debug counters are shared (the classes' pipelines run in
@@ -270,70 +372,29 @@ int setup_classes(tzr_ctx* ctx, int C, const int* Bs, const int* ns, bool own_po
     }
   }
   // the workspace is about to be re-used (and possibly re-allocated): the retained graph of the previous call is gone
-  ctx->have_last = false;
-  ctx->last_is_solve = false;
-  ctx->last_has_graph = false;
-  ctx->ragged_last.clear();
-  ++ctx->generation;
-  ctx->clique_B = 0;
-  ctx->route_B = 0;
-  // per class: geometry, then the bytes of every buffer (summed over classes, or the largest for the shared ones)
-  enum { kSrc, kDst, kSf, kDf, kGq, kPk, kOpnd, kTcl, kGc, kAdj, kDeg, kNe, kHclq, kHsize, kClq, kL, kAlive, kBest, kAcnt,
-         kRctr, kLock, kFlg, kKfin, kTst, kStack, kCv, kCentry, kPs, kPd, kWgt, kRes, kSkey, kSidx, kSorted, kRmask,
-         kTmask, kSol, kDbg, kBufs };
-  DevBuf* bufs[kBufs] = {&ctx->src, &ctx->dst, &ctx->sf, &ctx->df, &ctx->gq, &ctx->pk, &ctx->opnd, &ctx->tclist, &ctx->gc,
-                         &ctx->adj, &ctx->deg, &ctx->nedges, &ctx->hclq, &ctx->hsize, &ctx->clq, &ctx->L, &ctx->alive,
-                         &ctx->best_bits, &ctx->alive_cnt, &ctx->root_ctr, &ctx->lock, &ctx->flg, &ctx->kfinal,
-                         &ctx->tstart, &ctx->stack, &ctx->cv, &ctx->centry, &ctx->ps, &ctx->pd, &ctx->wgt, &ctx->res,
-                         &ctx->skey, &ctx->sidx, &ctx->sorted, &ctx->rmask, &ctx->tmask, &ctx->sol, &ctx->dbg};
-  bool shared[kBufs] = {};
-  for (int k : {(int)kTcl, (int)kStack, (int)kCv, (int)kCentry, (int)kDbg}) shared[k] = true;
-  std::vector<size_t> off((size_t)C * kBufs, 0);  // byte offset of class c in buffer k
-  size_t total[kBufs] = {};
+  forget_retained(ctx);
+  ctx->clique.B = 0;
+  // per class: geometry, and the largest size of each shared buffer
+  size_t tcl = 0;
+  ExactScratch ex{0, 0, 0};
   for (int c = 0; c < C; ++c) {
     const int B = Bs[c], n = ns[c];
     Batch& bt = out[c];
     bt = Batch{};
     bt.B = B;
     bt.n = n;
-    const size_t Bn = (size_t)B * n;
-    const int W32 = pitch32(n);
-    size_t bytes[kBufs] = {};
-    if (own_points) {
-      bytes[kSrc] = Bn * 3 * sizeof(double);
-      bytes[kDst] = Bn * 3 * sizeof(double);
-    }
-    bytes[kSf] = Bn * sizeof(float4);
-    bytes[kDf] = Bn * sizeof(float4);
-    bytes[kGq] = 2 * Bn * sizeof(float4);
-    bytes[kPk] = (size_t)B * 6 * npad128(n) * sizeof(float);
-    bytes[kOpnd] = tc_operand_bytes(B, n);
     bt.tc_list_cap = (unsigned int)tc_list_entries(B, n);
-    bytes[kTcl] = (size_t)bt.tc_list_cap * sizeof(uint2) + 256;
+    tcl = std::max(tcl, (size_t)bt.tc_list_cap * sizeof(uint2) + 256);
     // debug flag 16384: a re-check queue of 64 entries (the buffer keeps its full size), so that the queue-full path of
     // the graph kernels (void entries, in-place exact evaluation, the patch kernel's clamp) runs at test sizes
     if (ctx->flags & 16384u) bt.tc_list_cap = std::min(bt.tc_list_cap, 64u);
-    bytes[kGc] = (size_t)B * sizeof(GraphConsts);
-    bytes[kAdj] = Bn * pitch64(n) * sizeof(uint64_t);
-    bytes[kDeg] = Bn * sizeof(int32_t);
-    bytes[kNe] = (size_t)B * sizeof(unsigned long long);
-    bytes[kHclq] = Bn * kHeurRoots * sizeof(int32_t);
-    bytes[kHsize] = (size_t)B * kHeurRoots * sizeof(int32_t);
-    bytes[kClq] = Bn * sizeof(int32_t);
-    bytes[kL] = bytes[kAcnt] = bytes[kRctr] = bytes[kLock] = bytes[kFlg] = bytes[kKfin] = (size_t)B * sizeof(int32_t);
-    bytes[kAlive] = bytes[kBest] = (size_t)B * W32 * sizeof(uint32_t);
-    bytes[kTst] = (size_t)B * sizeof(unsigned long long);
     // exact phase: above kMaxN the search runs on the large route's compacted batch, which has its own scratch
     if (n <= kMaxN) {
       search_geometry(ctx, B, n, &bt.exact_ctas, &bt.max_depth, &bt.exact_conc);
-      const size_t warps = (size_t)bt.exact_ctas * 8;
-      const size_t level_bytes = (size_t)2 * W32 * sizeof(uint32_t);
-      bytes[kStack] = warps * bt.max_depth * level_bytes;
-      bytes[kCv] = std::max(warps, (size_t)4 * B) * (size_t)n * sizeof(int32_t);
-      bytes[kCentry] = warps * bt.max_depth * sizeof(int32_t);
+      const ExactScratch e = exact_scratch(bt);
+      ex = ExactScratch{std::max(ex.stack, e.stack), std::max(ex.cv, e.cv), std::max(ex.centry, e.centry)};
     }
     bt.sort_cap = next_pow2(2 * n);
-    bytes[kPs] = bytes[kPd] = Bn * 3 * sizeof(double);
     // rotation TIM capacity: n for CHAIN; for COMPLETE min(n(n-1)/2, what a 4 GiB budget allows)
     bt.rot_cap = n;
     if (complete_graph) {
@@ -341,28 +402,30 @@ int setup_classes(tzr_ctx* ctx, int C, const int* Bs, const int* ns, bool own_po
       const long long budget = ((long long)4 << 30) / (9LL * B);
       bt.rot_cap = std::max<long long>(n, std::min(full, budget));
     }
-    bytes[kWgt] = (size_t)B * bt.rot_cap * sizeof(double);
-    bytes[kRes] = Bn * sizeof(double);
-    bytes[kSkey] = (size_t)B * 3 * bt.sort_cap * sizeof(double);
-    bytes[kSidx] = (size_t)B * 3 * bt.sort_cap * sizeof(int32_t);
-    bytes[kSorted] = Bn * sizeof(int32_t);
-    bytes[kRmask] = (size_t)B * bt.rot_cap;
-    bytes[kTmask] = Bn;
-    bytes[kSol] = (size_t)B * sizeof(tzr_solution);
-    bytes[kDbg] = 16 * sizeof(unsigned long long);
-    for (int k = 0; k < kBufs; ++k) {
-      if (shared[k]) {
-        total[k] = std::max(total[k], bytes[k]);
-      } else {
-        off[(size_t)c * kBufs + k] = total[k];
-        total[k] += al256(bytes[k]);
-      }
-    }
   }
+  // per-problem buffers: the classes back to back, each class's share 256-byte aligned.  The first pass sizes the
+  // buffers, the second (after they are allocated) points every class at its share.
+  size_t total[kBatchBuffers];
+  auto lay_out = [&](bool point) {
+    std::fill(total, total + kBatchBuffers, (size_t)0);
+    for (int c = 0; c < C; ++c) {
+      int k = 0;
+      batch_buffers(out[c], [&](auto& field, size_t per, BufKind kind) {
+        if (point) point_at(field, ctx->ws[k].p, total[k]);
+        if (kind != kPoints || own_points) total[k] += al256((size_t)out[c].B * per * sizeof(*field));
+        ++k;
+      });
+    }
+  };
+  lay_out(false);
   int rc;
-  for (int k = 0; k < kBufs; ++k)
-    if ((k != kSrc && k != kDst) || own_points)
-      if ((rc = ensure(ctx, *bufs[k], total[k])) != TZR_OK) return rc;
+  for (int k = 0; k < kBatchBuffers; ++k)
+    if (total[k] && (rc = ensure(ctx, ctx->ws[k], total[k])) != TZR_OK) return rc;
+  if ((rc = ensure(ctx, ctx->tclist, tcl)) != TZR_OK || (rc = ensure(ctx, ctx->stack, ex.stack)) != TZR_OK ||
+      (rc = ensure(ctx, ctx->cv, ex.cv)) != TZR_OK || (rc = ensure(ctx, ctx->centry, ex.centry)) != TZR_OK ||
+      (rc = ensure(ctx, ctx->dbg, 16 * sizeof(unsigned long long))) != TZR_OK)
+    return rc;
+  lay_out(true);
   static const double kappa_env = [] {
     const char* e = std::getenv("TZR_TC_KAPPA");
     return e ? std::atof(e) : 0.0;
@@ -373,51 +436,16 @@ int setup_classes(tzr_ctx* ctx, int C, const int* Bs, const int* ns, bool own_po
   }();
   for (int c = 0; c < C; ++c) {
     Batch& bt = out[c];
-    auto at = [&](int k) { return (void*)((char*)bufs[k]->p + off[(size_t)c * kBufs + k]); };
-    bt.src = (const double*)at(kSrc);
-    bt.dst = (const double*)at(kDst);
-    bt.sf = (float4*)at(kSf);
-    bt.df = (float4*)at(kDf);
-    bt.gq = (float4*)at(kGq);
-    bt.pk = (float*)at(kPk);
-    bt.opnd = (float*)at(kOpnd);
     bt.tc_list_count = (unsigned int*)ctx->tclist.p;
     bt.tc_list = (uint2*)((char*)ctx->tclist.p + 256);
-    bt.gc = (GraphConsts*)at(kGc);
-    bt.adj = (uint64_t*)at(kAdj);
-    bt.deg = (int32_t*)at(kDeg);
-    bt.n_edges2 = (unsigned long long*)at(kNe);
-    bt.hclq = (int32_t*)at(kHclq);
-    bt.hsize = (int32_t*)at(kHsize);
-    bt.clq = (int32_t*)at(kClq);
-    bt.L = (int32_t*)at(kL);
-    bt.alive = (uint32_t*)at(kAlive);
-    bt.best_bits = (uint32_t*)at(kBest);
-    bt.alive_cnt = (int32_t*)at(kAcnt);
-    bt.root_ctr = (int32_t*)at(kRctr);
-    bt.lock = (int32_t*)at(kLock);
-    bt.flags = (int32_t*)at(kFlg);
-    bt.kcore_final = (int32_t*)at(kKfin);
-    bt.t_start = (unsigned long long*)at(kTst);
     bt.stack = (uint32_t*)ctx->stack.p;
     bt.cv = (int32_t*)ctx->cv.p;
     bt.centry = (int32_t*)ctx->centry.p;
-    bt.ps = (double*)at(kPs);
-    bt.pd = (double*)at(kPd);
-    bt.wgt = (double*)at(kWgt);
-    bt.res = (double*)at(kRes);
-    bt.skey = (double*)at(kSkey);
-    bt.sidx = (int32_t*)at(kSidx);
-    bt.sorted_clq = (int32_t*)at(kSorted);
-    bt.rot_mask = (uint8_t*)at(kRmask);
-    bt.trans_mask = (uint8_t*)at(kTmask);
-    bt.sol = (tzr_solution*)at(kSol);
     bt.mismatches = (unsigned long long*)ctx->dbg.p;
     bt.rechecks = (ctx->flags & 4u) ? (unsigned long long*)ctx->dbg.p + 1 : nullptr;
     bt.flags_dbg = ctx->flags;
     bt.tc_kappa = kappa_env;
     bt.tc_desc_swap = swap_env;
-    bt.budget_ns = 0ull;
   }
   return TZR_OK;
 }
@@ -460,45 +488,18 @@ __global__ void init_solutions_kernel(tzr_solution* sol, int B) {
 // View of problems [b0, b0+Bc) of a batch: every per-problem buffer is offset, geometry is unchanged.
 Batch sub_batch(const Batch& bt, int b0, int Bc) {
   Batch s = bt;
-  const size_t n = (size_t)bt.n, o = (size_t)b0;
-  const size_t W32 = (size_t)pitch32(bt.n);
+  const size_t o = (size_t)b0;
   s.B = Bc;
-  s.src = bt.src + o * n * 3;
-  s.dst = bt.dst + o * n * 3;
-  s.sf = bt.sf + o * n;
-  s.df = bt.df + o * n;
-  s.gq = bt.gq + 2 * o * n;
-  s.pk = bt.pk + o * 6 * (size_t)npad128(bt.n);
-  s.opnd = bt.opnd + tc_operand_bytes(b0, bt.n) / sizeof(float);
-  s.gc = bt.gc + o;
-  s.adj = bt.adj + o * n * pitch64(bt.n);
-  s.deg = bt.deg + o * n;
-  s.n_edges2 = bt.n_edges2 + o;
-  s.hclq = bt.hclq + o * kHeurRoots * n;
-  s.hsize = bt.hsize + o * kHeurRoots;
-  s.clq = bt.clq + o * n;
-  s.L = bt.L + o;
-  s.alive = bt.alive + o * W32;
-  s.best_bits = bt.best_bits + o * W32;
-  s.alive_cnt = bt.alive_cnt + o;
-  s.root_ctr = bt.root_ctr + o;
-  s.lock = bt.lock + o;
-  s.flags = bt.flags + o;
-  s.kcore_final = bt.kcore_final + o;
-  s.t_start = bt.t_start + o;
-  s.ps = bt.ps + o * n * 3;
-  s.pd = bt.pd + o * n * 3;
-  s.wgt = bt.wgt + o * (size_t)bt.rot_cap;
-  s.res = bt.res + o * n;
-  s.skey = bt.skey + o * 3 * (size_t)bt.sort_cap;
-  s.sidx = bt.sidx + o * 3 * (size_t)bt.sort_cap;
-  s.sorted_clq = bt.sorted_clq + o * n;
-  s.rot_mask = bt.rot_mask + o * (size_t)bt.rot_cap;
-  s.trans_mask = bt.trans_mask + o * n;
-  s.sol = bt.sol + o;
+  batch_buffers(s, [o](auto& field, size_t per, BufKind) { field += o * per; });
   if (bt.nb) s.nb = bt.nb + o;
   if (bt.nb_host) s.nb_host = bt.nb_host + o;
   return s;
+}
+
+// Problem b (caller's order) of the retained record: a view of its slot in its class.
+Batch retained_problem(const tzr_ctx* ctx, int b) {
+  const Retained::Problem& q = ctx->last.at[b];
+  return sub_batch(ctx->last.cls[q.c], q.k, 1);
 }
 
 // Problems per pipeline chunk: small enough that a chunk's adjacency bitsets (written by the graph kernel, then
@@ -601,40 +602,28 @@ int run_clique_large(tzr_ctx* ctx, const Batch& bt, const tzr_params& p, int mod
   CK(cudaMemcpyAsync(route_d, search.data(), (size_t)B * 4, cudaMemcpyHostToDevice, st));
   Batch cb = bt;
   if (n2 > 0) {
-    // the compacted batch: B problems of n2 vertices, its own clique state and exact-phase scratch
-    const size_t Bn2 = (size_t)B * n2;
-    const int W2 = pitch32(n2);
-    search_geometry(ctx, B, n2, &cb.exact_ctas, &cb.max_depth, &cb.exact_conc);
-    const size_t warps = (size_t)cb.exact_ctas * 8;
-    off = 0;
-    const size_t c_adj = carve(Bn2 * pitch64(n2) * 8), c_deg = carve(Bn2 * 4), c_ne = carve((size_t)B * 8),
-                 c_hclq = carve(Bn2 * kHeurRoots * 4), c_hsize = carve((size_t)B * kHeurRoots * 4), c_clq = carve(Bn2 * 4),
-                 c_L = carve((size_t)B * 4), c_alive = carve((size_t)B * W2 * 4), c_bb = carve((size_t)B * W2 * 4),
-                 c_acnt = carve((size_t)B * 4), c_rctr = carve((size_t)B * 4), c_lock = carve((size_t)B * 4),
-                 c_flg = carve((size_t)B * 4), c_ts = carve((size_t)B * 8),
-                 c_stack = carve(warps * cb.max_depth * 2 * W2 * 4),
-                 c_cv = carve(std::max(warps, (size_t)4 * B) * n2 * 4), c_centry = carve(warps * cb.max_depth * 4);
-    rc = ensure(ctx, ctx->cq, off);
-    if (rc) return rc;
-    char* q = (char*)ctx->cq.p;
+    // the compacted batch: B problems of n2 vertices, its own clique state and exact-phase scratch carved from one
+    // buffer.  The first pass sizes it, the second (after it is allocated) points the fields at their shares.
     cb.n = n2;
-    cb.adj = (uint64_t*)(q + c_adj);
-    cb.deg = (int32_t*)(q + c_deg);
-    cb.n_edges2 = (unsigned long long*)(q + c_ne);
-    cb.hclq = (int32_t*)(q + c_hclq);
-    cb.hsize = (int32_t*)(q + c_hsize);
-    cb.clq = (int32_t*)(q + c_clq);
-    cb.L = (int32_t*)(q + c_L);
-    cb.alive = (uint32_t*)(q + c_alive);
-    cb.best_bits = (uint32_t*)(q + c_bb);
-    cb.alive_cnt = (int32_t*)(q + c_acnt);
-    cb.root_ctr = (int32_t*)(q + c_rctr);
-    cb.lock = (int32_t*)(q + c_lock);
-    cb.flags = (int32_t*)(q + c_flg);
-    cb.t_start = (unsigned long long*)(q + c_ts);
-    cb.stack = (uint32_t*)(q + c_stack);
-    cb.cv = (int32_t*)(q + c_cv);
-    cb.centry = (int32_t*)(q + c_centry);
+    search_geometry(ctx, B, n2, &cb.exact_ctas, &cb.max_depth, &cb.exact_conc);
+    const ExactScratch ex = exact_scratch(cb);
+    auto lay_out = [&](char* q) {
+      off = 0;
+      batch_buffers(cb, [&](auto& field, size_t per, BufKind kind) {
+        if (kind != kClique) return;
+        const size_t at = carve((size_t)B * per * sizeof(*field));
+        if (q) point_at(field, q, at);
+      });
+      const size_t at[3] = {carve(ex.stack), carve(ex.cv), carve(ex.centry)};
+      if (q) {
+        point_at(cb.stack, q, at[0]);
+        point_at(cb.cv, q, at[1]);
+        point_at(cb.centry, q, at[2]);
+      }
+    };
+    lay_out(nullptr);
+    if ((rc = ensure(ctx, ctx->cq, off))) return rc;
+    lay_out((char*)ctx->cq.p);
     cb.kcore_final = nullptr;
     launch_core_compact(bt, cb, n2o, o2n, cnt_d, route_d, st, nl);
     CK(cudaMemsetAsync(cb.n_edges2, 0, (size_t)B * 8, st));
@@ -657,7 +646,7 @@ int run_clique(tzr_ctx* ctx, const Batch& bt, const tzr_params& p, int mode, cud
 // The fused device pipeline for one uniform batch.  src/dst must already be set in bt.
 // st: stream of the clique / rotation stages; sg: stream of prep + graph (== st for the single-lane form, otherwise
 // gdone is recorded on sg after the graph kernel and st waits for it).
-// route: the batch's entries of ctx->route.
+// route: the batch's clique routes.
 int run_pipeline(tzr_ctx* ctx, Batch& bt, const tzr_params& p, cudaEvent_t* ev, cudaStream_t st, int32_t* route,
                  cudaStream_t sg = nullptr, cudaEvent_t gdone = nullptr) {
   if (!sg) sg = st;
@@ -729,10 +718,11 @@ int run_pipeline(tzr_ctx* ctx, Batch& bt, const tzr_params& p, cudaEvent_t* ev, 
 }
 
 // Run the pipeline chunk by chunk on the compute stream.  chunks: views of consecutive problems, chunk c starting at
-// problem bounds[c] of the call's B = bounds.back() (route entries).  ready[c] (optional) is an event the chunk's inputs
-// wait for.  lanes_ok: several chunks may alternate between the two compute lanes.
+// problem bounds[c] of the call's B = bounds.back() (route: B entries).  ready[c] (optional) is an event the chunk's
+// inputs wait for.  lanes_ok: several chunks may alternate between the two compute lanes.
 int run_chunks(tzr_ctx* ctx, std::vector<Batch>& chunks, const std::vector<int>& bounds, const tzr_params& p,
-               const cudaEvent_t* ready, const std::function<int(int)>& before_chunk, bool lanes_ok) {
+               const cudaEvent_t* ready, const std::function<int(int)>& before_chunk, bool lanes_ok,
+               std::vector<int32_t>& route) {
   const int n_chunks = (int)chunks.size();
   if (!ctx->stage_log) {
     ctx->graph_ev_used = 0;
@@ -746,7 +736,7 @@ int run_chunks(tzr_ctx* ctx, std::vector<Batch>& chunks, const std::vector<int>&
     ctx->stage_ev.push_back(e);
   }
   const bool lanes = n_chunks > 1 && ctx->gstream && ctx->hstream && lanes_ok;
-  ctx->route.assign((size_t)bounds.back(), 0);
+  route.assign((size_t)bounds.back(), 0);
   // debug counters cover the whole call: zeroed once, ahead of every chunk on either lane (not per chunk, which would
   // keep only the last chunk's counts)
   if (ctx->flags & 6u) CK(cudaMemsetAsync((void*)ctx->dbg.p, 0, 16 * sizeof(unsigned long long), ctx->stream));
@@ -772,7 +762,7 @@ int run_chunks(tzr_ctx* ctx, std::vector<Batch>& chunks, const std::vector<int>&
       if (cudaStreamWaitEvent(sg, ready[c], 0) != cudaSuccess) return TZR_ERR_CUDA;
     }
     int rc = run_pipeline(ctx, chunks[c], p, ctx->stage_ev.data() + 5 * (ctx->stage_first + c), st,
-                          ctx->route.data() + b0, sg, lanes ? ctx->gdone_ev[c] : nullptr);
+                          route.data() + b0, sg, lanes ? ctx->gdone_ev[c] : nullptr);
     if (rc) return rc;
   }
   if (lanes) {  // everything later on ctx->stream (D2H, the caller's work) is ordered after both lanes
@@ -793,15 +783,12 @@ int run_chunked(tzr_ctx* ctx, Batch& bt, const tzr_params& p, const std::vector<
   std::vector<Batch> chunks;
   for (int c = 0; c < n_chunks; ++c)
     chunks.push_back(n_chunks > 1 ? sub_batch(bt, bounds[c], bounds[c + 1] - bounds[c]) : bt);
-  const int rc = run_chunks(ctx, chunks, bounds, p, ready, before_chunk, l2_chunk(ctx, bt.B, bt.n, p) >= bt.B);
+  std::vector<int32_t> route;
+  const int rc =
+      run_chunks(ctx, chunks, bounds, p, ready, before_chunk, l2_chunk(ctx, bt.B, bt.n, p) >= bt.B, route);
   if (rc) return rc;
   if (n_chunks == 1) bt = chunks[0];  // keep fields filled in by run_pipeline (beta, scale_mode, ...)
-  ctx->last = bt;
-  ctx->have_last = true;
-  ctx->last_is_solve = true;  // every uniform solve entry (tzr_solve, tzr_solve_batch, tzr_solve_batch_dev) ends here
-  ctx->last_complete = p.rotation_tim_graph == 1;
-  ctx->last_has_graph = effective_mode(p) != 3;  // NONE: populateVertices is never called (registration.cc:607-650)
-  ctx->route_B = ctx->last_has_graph ? bt.B : 0;
+  retain(ctx, {bt}, nullptr, nullptr, route, &p);  // every uniform solve entry (tzr_solve, tzr_solve_batch(_dev)) ends here
   return TZR_OK;
 }
 
@@ -921,13 +908,14 @@ int solve_ragged_dev(tzr_ctx* ctx, const tzr_params& p, int B, const int32_t* n,
   std::vector<RaggedSlot> slots(B);
   for (int c = 0; c < C; ++c)
     for (int s = lo[c]; s < lo[c + 1]; ++s) {
-      const int q = order[s], k = s - lo[c];
+      const int q = order[s];
       nb[s] = n[q];
+      const Batch v = sub_batch(cls[c], s - lo[c], 1);
       RaggedSlot& sl = slots[s];
-      sl.src = const_cast<double*>(cls[c].src) + (size_t)k * ns[c] * 3;
-      sl.dst = const_cast<double*>(cls[c].dst) + (size_t)k * ns[c] * 3;
-      sl.sol = cls[c].sol + k;
-      sl.clq = cls[c].sorted_clq + (size_t)k * ns[c];
+      sl.src = const_cast<double*>(v.src);
+      sl.dst = const_cast<double*>(v.dst);
+      sl.sol = v.sol;
+      sl.clq = v.sorted_clq;
       sl.flat = flat[q];
       sl.n = n[q];
       sl.n_pad = ns[c];
@@ -971,32 +959,13 @@ int solve_ragged_dev(tzr_ctx* ctx, const tzr_params& p, int B, const int32_t* n,
     }
   }
   if (sc_bytes && (rc = ensure(ctx, ctx->sc, sc_bytes)) != TZR_OK) return rc;
-  rc = run_chunks(ctx, chunks, bounds, p, nullptr, nullptr, lanes_ok);
+  std::vector<int32_t> route;
+  rc = run_chunks(ctx, chunks, bounds, p, nullptr, nullptr, lanes_ok, route);
   if (rc) return rc;
   ragged_scatter_kernel<<<B, 256, 0, st>>>(d_slots, solutions, cliques);
   ctx->launches += 1;
   if ((rc = check_launch(ctx, "ragged gather / scatter")) != TZR_OK) return rc;
-  // the retained graph and the clique routes, in the caller's order
-  const bool has_graph = effective_mode(p) != 3;
-  std::vector<int32_t> route(B, 0);
-  ctx->ragged_last.resize(B);
-  for (int c = 0; c < C; ++c)
-    for (int s = lo[c]; s < lo[c + 1]; ++s) {
-      const size_t k = (size_t)(s - lo[c]);
-      ctx->ragged_last[order[s]] = {cls[c].adj + k * ns[c] * pitch64(ns[c]), cls[c].deg + k * ns[c], nb[s], ns[c],
-                                    slots[s].src, slots[s].dst, slots[s].sol, slots[s].clq,
-                                    cls[c].rot_mask + k * (size_t)cls[c].rot_cap, cls[c].trans_mask + k * ns[c]};
-      route[order[s]] = ctx->route[s];
-    }
-  ctx->route = route;
-  ctx->last = cls[0];
-  ctx->last.B = B;
-  ctx->last.n = ns[0];
-  ctx->have_last = true;
-  ctx->last_is_solve = true;
-  ctx->last_complete = p.rotation_tim_graph == 1;
-  ctx->last_has_graph = has_graph;
-  ctx->route_B = has_graph ? B : 0;
+  retain(ctx, std::move(cls), order.data(), n, route, &p);
   return TZR_OK;
 }
 
@@ -1251,14 +1220,6 @@ int tzr_ctx_destroy(tzr_ctx* ctx) {
   if (!ctx) return TZR_OK;
   cudaSetDevice(ctx->device);
   cudaStreamSynchronize(ctx->stream);
-  DevBuf* bufs[] = {&ctx->src, &ctx->dst, &ctx->sf, &ctx->df, &ctx->gq, &ctx->pk, &ctx->opnd, &ctx->tclist, &ctx->gc, &ctx->adj, &ctx->deg, &ctx->nedges,
-                    &ctx->hclq, &ctx->hsize, &ctx->clq, &ctx->L, &ctx->alive, &ctx->best_bits, &ctx->alive_cnt, &ctx->root_ctr,
-                    &ctx->lock, &ctx->flg, &ctx->kfinal, &ctx->tstart, &ctx->stack, &ctx->cv, &ctx->centry, &ctx->ps, &ctx->pd, &ctx->wgt,
-                    &ctx->res, &ctx->skey, &ctx->sidx, &ctx->sorted, &ctx->rmask, &ctx->tmask, &ctx->sol, &ctx->dbg,
-                    &ctx->misc, &ctx->sc, &ctx->m_in, &ctx->m_scratch, &ctx->m_out, &ctx->certb, &ctx->lg, &ctx->cq, &ctx->rg, &ctx->icp,
-                    &ctx->vox, &ctx->pg};
-  for (DevBuf* b : bufs)
-    if (b->p) cudaFree(b->p);
   if (ctx->h_pin) cudaFreeHost(ctx->h_pin);
   for (int i = 0; i < 5; ++i)
     if (ctx->ev[i]) cudaEventDestroy(ctx->ev[i]);
@@ -1358,10 +1319,7 @@ int tzr_graph_build(tzr_ctx* ctx, const double* src, const double* dst, int n, d
   CK(cudaMemcpyAsync(&e2, bt.n_edges2, sizeof(e2), cudaMemcpyDeviceToHost, st));
   CK(cudaStreamSynchronize(st));
   if (n_edges) *n_edges = (int64_t)(e2 / 2);
-  ctx->last = bt;
-  ctx->have_last = true;
-  ctx->last_is_solve = false;  // a graph without solution records
-  ctx->last_has_graph = true;
+  retain(ctx, {bt}, nullptr, nullptr, {}, nullptr);
   return TZR_OK;
 }
 
@@ -1377,7 +1335,6 @@ int tzr_max_clique_batch(tzr_ctx* ctx, int B, int n, const uint64_t* adj_bits, i
   Batch bt;
   int rc = setup_batch(ctx, B, n, false, &bt);
   if (rc) return rc;
-  ctx->last_is_solve = false;  // the clique stage reuses the solve's workspace
   cudaStream_t st = ctx->stream;
   const size_t rows = (size_t)B * n;
   CK(cudaMemsetAsync(bt.adj, 0, rows * pitch64(n) * 8, st));
@@ -1391,17 +1348,14 @@ int tzr_max_clique_batch(tzr_ctx* ctx, int B, int n, const uint64_t* adj_bits, i
   p.kcore_heuristic_threshold = kcore_thr;
   if (mode == 0 && time_limit_s > 0 && time_limit_s < 1e7) bt.budget_ns = (unsigned long long)(time_limit_s * 1e9);
   int nl = 2;
-  ctx->route.assign((size_t)B, 0);
-  rc = run_clique(ctx, bt, p, mode, st, &nl, ctx->route.data());
+  std::vector<int32_t> route((size_t)B, 0);
+  rc = run_clique(ctx, bt, p, mode, st, &nl, route.data());
   ctx->launches += nl;
   if (rc) return rc;
   rc = check_launch(ctx, "max clique");
   if (rc) return rc;
-  ctx->clique_B = B;
-  ctx->route_B = B;
-  ctx->clique_geom[0] = bt.exact_ctas;
-  ctx->clique_geom[1] = bt.exact_conc;
-  ctx->clique_geom[2] = bt.max_depth;
+  ctx->clique = bt;
+  ctx->last.route = std::move(route);  // no solve is retained, but the routes are readable
   std::vector<int32_t> L(B), fl(B);
   CK(cudaMemcpyAsync(L.data(), bt.L, (size_t)B * sizeof(int32_t), cudaMemcpyDeviceToHost, st));
   CK(cudaMemcpyAsync(fl.data(), bt.flags, (size_t)B * sizeof(int32_t), cudaMemcpyDeviceToHost, st));
@@ -1426,14 +1380,17 @@ int tzr_max_clique(tzr_ctx* ctx, const uint64_t* adj_bits, int n, int mode, doub
 }
 
 int tzr_ctx_clique_info(tzr_ctx* ctx, int32_t* geometry3, int32_t* heuristic_best) {
-  if (!ctx || !geometry3 || ctx->clique_B <= 0) return TZR_ERR_INVALID_ARG;
-  for (int i = 0; i < 3; ++i) geometry3[i] = ctx->clique_geom[i];
+  if (!ctx || !geometry3 || ctx->clique.B <= 0) return TZR_ERR_INVALID_ARG;
+  const Batch& bt = ctx->clique;
+  geometry3[0] = bt.exact_ctas;
+  geometry3[1] = bt.exact_conc;
+  geometry3[2] = bt.max_depth;
   if (heuristic_best) {
     cudaSetDevice(ctx->device);
-    std::vector<int32_t> hs((size_t)ctx->clique_B * kHeurRoots);
-    CK(cudaMemcpyAsync(hs.data(), ctx->hsize.p, hs.size() * sizeof(int32_t), cudaMemcpyDeviceToHost, ctx->stream));
+    std::vector<int32_t> hs((size_t)bt.B * kHeurRoots);
+    CK(cudaMemcpyAsync(hs.data(), bt.hsize, hs.size() * sizeof(int32_t), cudaMemcpyDeviceToHost, ctx->stream));
     CK(cudaStreamSynchronize(ctx->stream));
-    for (int b = 0; b < ctx->clique_B; ++b)
+    for (int b = 0; b < bt.B; ++b)
       heuristic_best[b] = *std::max_element(hs.begin() + (size_t)b * kHeurRoots, hs.begin() + (size_t)(b + 1) * kHeurRoots);
   }
   return TZR_OK;
@@ -1446,8 +1403,8 @@ int tzr_ctx_set_max_n(tzr_ctx* ctx, int max_n) {
 }
 
 int tzr_ctx_clique_route(tzr_ctx* ctx, int32_t* per_problem) {
-  if (!ctx || !per_problem || ctx->route_B <= 0) return TZR_ERR_INVALID_ARG;
-  std::copy(ctx->route.begin(), ctx->route.begin() + ctx->route_B, per_problem);
+  if (!ctx || !per_problem || ctx->last.route.empty()) return TZR_ERR_INVALID_ARG;
+  std::copy(ctx->last.route.begin(), ctx->last.route.end(), per_problem);
   return TZR_OK;
 }
 
@@ -1767,80 +1724,56 @@ int tzr_solve_batch_ragged_dev(tzr_ctx* ctx, const tzr_params* params, int B, co
 }
 
 int tzr_last_graph(tzr_ctx* ctx, int b, uint64_t* adj_bits, int32_t* degree) {
-  if (!ctx || !ctx->have_last || b < 0 || b >= ctx->last.B) return TZR_ERR_INVALID_ARG;
+  if (!ctx || b < 0 || b >= (int)ctx->last.at.size()) return TZR_ERR_INVALID_ARG;
   cudaSetDevice(ctx->device);
-  const Batch& bt = ctx->last;
-  // a ragged solve: problem b's own n rows of its padded slot
-  const bool ragged = !ctx->ragged_last.empty();
-  const int n = ragged ? ctx->ragged_last[b].n : bt.n;
-  const int np = ragged ? ctx->ragged_last[b].n_pad : n;
-  const uint64_t* adj = ragged ? ctx->ragged_last[b].adj : bt.adj + (size_t)b * n * pitch64(n);
-  const int32_t* deg = ragged ? ctx->ragged_last[b].deg : bt.deg + (size_t)b * n;
-  if (!ctx->last_has_graph) {  // inlier selection NONE: the reference never populates the graph -> no edges
+  // problem b's own n rows of its slot (padded to its class's n after a ragged solve)
+  const int n = ctx->last.at[b].n;
+  const Batch v = retained_problem(ctx, b);
+  if (!ctx->last.has_graph) {  // inlier selection NONE: the reference never populates the graph -> no edges
     if (adj_bits) memset(adj_bits, 0, (size_t)n * words64(n) * 8);
     if (degree) memset(degree, 0, (size_t)n * 4);
     return TZR_OK;
   }
   cudaStream_t st = ctx->stream;
   if (adj_bits)
-    CK(cudaMemcpy2DAsync(adj_bits, (size_t)words64(n) * 8, adj, (size_t)pitch64(np) * 8, (size_t)words64(n) * 8, n,
+    CK(cudaMemcpy2DAsync(adj_bits, (size_t)words64(n) * 8, v.adj, (size_t)pitch64(v.n) * 8, (size_t)words64(n) * 8, n,
                          cudaMemcpyDeviceToHost, st));
-  if (degree) CK(cudaMemcpyAsync(degree, deg, (size_t)n * 4, cudaMemcpyDeviceToHost, st));
+  if (degree) CK(cudaMemcpyAsync(degree, v.deg, (size_t)n * 4, cudaMemcpyDeviceToHost, st));
   CK(cudaStreamSynchronize(st));
   return TZR_OK;
 }
 
 int tzr_last_graph_info(const tzr_ctx* ctx, int32_t* B, int32_t* n, int32_t* has_graph, uint64_t* generation) {
   if (!ctx) return TZR_ERR_INVALID_ARG;
-  if (B) *B = ctx->have_last ? ctx->last.B : 0;
-  if (n) *n = ctx->have_last ? ctx->last.n : 0;
-  if (has_graph) *has_graph = (ctx->have_last && ctx->last_has_graph) ? 1 : 0;
+  const Retained& r = ctx->last;
+  if (B) *B = (int32_t)r.at.size();
+  if (n) *n = r.cls.empty() ? 0 : r.cls[0].n;  // the largest n: the classes run largest first
+  if (has_graph) *has_graph = (!r.at.empty() && r.has_graph) ? 1 : 0;
   if (generation) *generation = ctx->generation;
   return TZR_OK;
-}
-
-// Where problem b (caller's order) of the retained solve lies in the workspace.
-struct SolveSlot {
-  const double* src;
-  const double* dst;
-  const tzr_solution* sol;
-  const int32_t* clq;
-  const uint8_t* rmask;
-  const uint8_t* tmask;
-};
-
-static SolveSlot last_solve_slot(const tzr_ctx* ctx, int b) {
-  if (!ctx->ragged_last.empty()) {
-    const tzr_ctx::RaggedGraph& r = ctx->ragged_last[b];
-    return SolveSlot{r.src, r.dst, r.sol, r.clq, r.rmask, r.tmask};
-  }
-  const Batch& bt = ctx->last;
-  const size_t n = (size_t)bt.n, o = (size_t)b;
-  return SolveSlot{bt.src + o * n * 3, bt.dst + o * n * 3, bt.sol + o, bt.sorted_clq + o * n,
-                   bt.rot_mask + o * (size_t)bt.rot_cap, bt.trans_mask + o * n};
 }
 
 // rotation TIMs (and rotation mask bytes) of a retained solution record: 0 when it is not valid
 static long long last_rot_count(const tzr_ctx* ctx, const tzr_solution& s) {
   if (!s.valid) return 0;
   const long long m = std::max(0, s.clique_size);
-  return ctx->last_complete ? m * (m - 1) / 2 : m;
+  return ctx->last.complete ? m * (m - 1) / 2 : m;
 }
 
 int tzr_last_inliers(tzr_ctx* ctx, int b, uint8_t* rot_inliers, uint8_t* trans_inliers, int64_t* n_rot,
                      int32_t* n_trans) {
-  if (!ctx || !ctx->last_is_solve || b < 0 || b >= ctx->last.B) return TZR_ERR_INVALID_ARG;
+  if (!ctx || !ctx->last.is_solve || b < 0 || b >= (int)ctx->last.at.size()) return TZR_ERR_INVALID_ARG;
   cudaSetDevice(ctx->device);
   // every stream of the solve joins ctx->stream before its call returns: work queued here runs after all of it
   cudaStream_t st = ctx->stream;
-  const SolveSlot s = last_solve_slot(ctx, b);
+  const Batch v = retained_problem(ctx, b);
   tzr_solution rec;
-  CK(cudaMemcpyAsync(&rec, s.sol, sizeof(rec), cudaMemcpyDeviceToHost, st));
+  CK(cudaMemcpyAsync(&rec, v.sol, sizeof(rec), cudaMemcpyDeviceToHost, st));
   CK(cudaStreamSynchronize(st));
   const long long nr = last_rot_count(ctx, rec);
   const int nt = rec.valid ? std::max(0, rec.clique_size) : 0;
-  if (rot_inliers && nr > 0) CK(cudaMemcpyAsync(rot_inliers, s.rmask, (size_t)nr, cudaMemcpyDeviceToHost, st));
-  if (trans_inliers && nt > 0) CK(cudaMemcpyAsync(trans_inliers, s.tmask, (size_t)nt, cudaMemcpyDeviceToHost, st));
+  if (rot_inliers && nr > 0) CK(cudaMemcpyAsync(rot_inliers, v.rot_mask, (size_t)nr, cudaMemcpyDeviceToHost, st));
+  if (trans_inliers && nt > 0) CK(cudaMemcpyAsync(trans_inliers, v.trans_mask, (size_t)nt, cudaMemcpyDeviceToHost, st));
   CK(cudaStreamSynchronize(st));
   if (n_rot) *n_rot = nr;
   if (n_trans) *n_trans = nt;
@@ -1851,11 +1784,11 @@ int tzr_certify_last_solve(tzr_ctx* ctx, const tzr_certifier_params* params, int
                            tzr_certification_result* results, int32_t* status, double* const* traj,
                            const int32_t* traj_capacity) {
   if (!ctx || !params || !results || count <= 0 || (traj && !traj_capacity)) return TZR_ERR_INVALID_ARG;
-  if (!ctx->last_is_solve) {
+  if (!ctx->last.is_solve) {
     ctx->last_error = "no solve is retained on this context";
     return TZR_ERR_INVALID_ARG;
   }
-  const int B = ctx->last.B;
+  const int B = (int)ctx->last.at.size();
   if (!problems && count != B) return TZR_ERR_INVALID_ARG;
   for (int j = 0; j < count; ++j) {
     const int b = problems ? problems[j] : j;
@@ -1868,7 +1801,7 @@ int tzr_certify_last_solve(tzr_ctx* ctx, const tzr_certifier_params* params, int
   std::vector<const tzr_solution*> at((size_t)B);
   const char *lo = nullptr, *hi = nullptr;
   for (int b = 0; b < B; ++b) {
-    at[b] = last_solve_slot(ctx, b).sol;
+    at[b] = retained_problem(ctx, b).sol;
     const char* p = (const char*)at[b];
     if (!lo || p < lo) lo = p;
     if (!hi || p + sizeof(tzr_solution) > hi) hi = p + sizeof(tzr_solution);
@@ -1899,17 +1832,17 @@ int tzr_certify_last_solve(tzr_ctx* ctx, const tzr_certifier_params* params, int
       stj = TZR_ERR_TOO_LARGE;
       too_large = true;
     } else {
-      const SolveSlot sl = last_solve_slot(ctx, b);
+      const Batch v = retained_problem(ctx, b);
       const double nb = params->noise_bound / s.scale;
       CertGatherProb g;
-      g.src = sl.src;
-      g.dst = sl.dst;
-      g.clq = sl.clq;
-      g.rmask = sl.rmask;
+      g.src = v.src;
+      g.dst = v.dst;
+      g.clq = v.sorted_clq;
+      g.rmask = v.rot_mask;
       g.scale = s.scale;
       g.nbs = params->cbar2 * nb * nb;
       g.m = s.clique_size;
-      g.complete = ctx->last_complete ? 1 : 0;
+      g.complete = ctx->last.complete ? 1 : 0;
       g.k_off = g.v_off = 0;
       gin.push_back(g);
       N.push_back((int32_t)nr);
@@ -2626,11 +2559,7 @@ static int register_pairs_run(tzr_ctx* ctx, const tzr_frontend_params* fp, const
     rc = solve_ragged_dev(ctx, *params, S, solved_n.data(), d_src, d_dst, d_sol, want_clq ? d_clq : nullptr);
     if (rc) return rc;
   } else {  // nothing solved: no solve is retained
-    ctx->have_last = false;
-    ctx->last_is_solve = false;
-    ctx->last_has_graph = false;
-    ctx->ragged_last.clear();
-    ++ctx->generation;
+    forget_retained(ctx);
   }
   // the refinement of the solved pairs, seeded on the device from their records (no synchronisation, no upload of points)
   char* hi = h + hi_tab;
@@ -3223,7 +3152,7 @@ static int sum_stage_events(tzr_ctx* ctx, int c0, int c1, int g0, int g1, double
 }
 
 int tzr_last_stage_ms(tzr_ctx* ctx, double* prep_ms, double* graph_ms, double* clique_ms, double* rot_trans_ms) {
-  if (!ctx || !ctx->have_last) return TZR_ERR_INVALID_ARG;
+  if (!ctx || ctx->last.at.empty()) return TZR_ERR_INVALID_ARG;
   double acc[4];
   const int rc = sum_stage_events(ctx, ctx->stage_first, ctx->stage_chunks, ctx->graph_first, ctx->graph_ev_used, acc);
   if (rc) return rc;
