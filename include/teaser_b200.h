@@ -768,6 +768,88 @@ int tzr_register_cloud_pairs_icp_robust(tzr_ctx* ctx, const tzr_frontend_params*
                                         double epsilon, const tzr_robust_kernel* kernel,
                                         tzr_icp_result* icp_results);
 
+/* ---- refining registrations: coloured ICP -------------------------------------------------------------------
+ * Open3D's registration_colored_icp (TransformationEstimationForColoredICP with InitializePointCloudForColoredICP's
+ * colour gradients), for many problems at once, defined here as follows (DESIGN.md §3.17):
+ *   - Colours: n x 3 floats (r, g, b) per point, any range (Open3D uses [0, 1]), read exactly as float64.  A point's
+ *     intensity is ((r + g) + b) / 3.0.
+ *   - Colour gradients of a target cloud (tzr_estimate_color_gradients), in IEEE float64 with no FMA contraction, for
+ *     every point k with position v_k, normal n_k (the library's normals layout, curvature ignored) and intensity i_k:
+ *       neighbours: the radius search of tzr_estimate_normals (float d^2 < R^2 with R^2 = (float)(R * R), the list
+ *         ordered by (d^2, index)), cut to its first nn = min(count, 30) entries (Open3D's KDTreeSearchParamHybrid(R,
+ *         30)).  The 30 are chosen by a bounded selection, so no neighbourhood is too large.  nn < 4: the gradient is
+ *         (0, 0, 0).
+ *       rows: entry 0 is skipped, whatever it is (Open3D's loop starts at 1).  Entry e = 1 ... nn - 1 at point v with
+ *         intensity i gives s = ((v0 - vk0) n0 + (v1 - vk1) n1) + (v2 - vk2) n2, a_e(c) = (v(c) - s n(c)) - vk(c)
+ *         (v projected onto the tangent plane, minus v_k) and b_e = i - i_k.  One more row c = (nn - 1) n with
+ *         right-hand side 0 pins the normal component.
+ *       system: M_ab = sum_e a_e(a) a_e(b) + c_a c_b and h_a = sum_e a_e(a) b_e, each summed from 0.0 in list order with
+ *         the constraint row last.  If an entry of M or h is not finite, the gradient is (NaN, NaN, NaN).  Otherwise
+ *         the gradient x solves M x = h by the truncated, diagonally pivoted LDL^T of the 6 x 6 step below (the same
+ *         device code at size 3; tol = 1e-10 max_k M_kk, the lowest index on ties), so a direction the neighbours do
+ *         not observe (collinear neighbours) gets 0.  Open3D solves with Eigen's LDLT: the two agree up to rounding,
+ *         and only on neighbourhoods that are not degenerate.
+ *     The gradient is float64 and does not depend on the normal's sign (n enters as s n, n n^T and c c^T only).
+ *   - Step: tzr_icp_point_to_plane's inputs, search, eval(T), loop, convergence test, centring (c = mu_p, u = p - c),
+ *     6 x 6 solve, R_u, t_u and composition, unchanged.  Each correspondence (i, j) with p the transformed source
+ *     point, q = y_j, n its target normal, g its target's gradient, i_s the source's and i_t the target's intensity,
+ *     sg = sqrt(lambda) and si = sqrt(1 - lambda) (lambda = lambda_geometric) gives two rows:
+ *       geometric:    J_G = (sg a0, sg a1, sg a2, sg n0, sg n1, sg n2) with a = u x n as in point-to-plane, and
+ *                     r_G = sg r, r = ((p0 - q0) n0 + (p1 - q1) n1) + (p2 - q2) n2.
+ *       photometric:  d(c) = (p(c) - r n(c)) - q(c) (the projection of p, minus q), i_hat = ((g0 d0 + g1 d1) + g2 d2) +
+ *                     i_t, m_k = -((g0 M_0k + g1 M_1k) + g2 M_2k) with M_ab = delta_ab - n_a n_b,
+ *                     J_I = (si e0, si e1, si e2, si m0, si m1, si m2) with e = u x m written as point-to-plane's
+ *                     a = u x n, and r_I = si (i_s - i_hat).
+ *     Each row has its own weight w = weight(r_row) of the TZR_LOSS_* kernel (w = 1 without a kernel) and adds its own
+ *     terms, the geometric row first: (w J_a) J_b to the 21 upper entries and (w J_a) r_row to g, as the robust
+ *     point-to-plane step (without a kernel, J_a J_b and J_a r_row).  A row adds nothing when its factor (sg or si) is
+ *     0 or its weight is not finite; the photometric row adds nothing when the source colour, the target colour or g
+ *     has a non-finite component; a correspondence whose normal has a non-finite component adds nothing.  Every such
+ *     correspondence still counts for fitness and rmse.
+ *     Consequences: with lambda = 1 every output is bit-identical to tzr_icp_point_to_plane_robust_batch with the same
+ *     kernel, and with no kernel or TZR_LOSS_L2 to tzr_icp_point_to_plane_batch; flipping any normal changes no bit.
+ *   - lambda_geometric: Open3D's default is 0.968.  A value outside [0, 1] is replaced by 0.968, as Open3D's
+ *     constructor does; a non-finite value is TZR_ERR_INVALID_ARG.
+ *   - Gradients inside the call: from the targets and their normals and colours already uploaded, at radius
+ *     2 max_correspondence_distance (RegistrationColoredICP's), bit-identical to tzr_estimate_color_gradients_batch
+ *     over the targets at that radius.
+ * Launches: tzr_icp_point_to_plane_batch's (2 + 4 * max_iteration, + 4 when some target has 1024 points or more) plus
+ * the gradient pass (1, + 4 when some target has 4096 points or more, or under debug flag 8388608), whatever B.
+ * Workspace: tzr_icp's own, so a retained solve stays retained. */
+
+/* Colour gradients of one cloud: pts (n x 3 floats), normals (n x 4 floats, nx, ny, nz, curvature), colors (n x 3
+ * floats), radius (finite and > 0, else TZR_ERR_INVALID_ARG), grad_out (n x 3 doubles).  The search route is
+ * tzr_estimate_normals' (brute force below 4096 points, the hashed grid from there; debug flags 4194304 and 8388608);
+ * both routes give the same bits.  Workspace as tzr_estimate_normals: the front end's buffers, so a retained solve
+ * stays retained. */
+int tzr_estimate_color_gradients(tzr_ctx* ctx, const float* pts, int n, const float* normals, const float* colors,
+                                 double radius, double* grad_out);
+
+/* B clouds: entry b of pts, normals, colors and grad_out as the single call's with n[b] points (every entry required).
+ * status (may be NULL): B entries, TZR_OK each (no neighbourhood is too large).  TZR_ERR_TOO_LARGE when the batch holds
+ * more than 2^31 - 1 points.  Per cloud, the output is bit-identical to tzr_estimate_color_gradients on that cloud
+ * alone. */
+int tzr_estimate_color_gradients_batch(tzr_ctx* ctx, int B, const int32_t* n, const float* const* pts,
+                                       const float* const* normals, const float* const* colors, double radius,
+                                       double* const* grad_out, int32_t* status);
+
+/* B ragged problems: tzr_icp_point_to_plane_batch's arguments plus src_colors (B entries, entry b ns[b] x 3 floats),
+ * dst_colors (B entries, entry b nd[b] x 3 floats), lambda_geometric and kernel (NULL: no kernel; otherwise checked as
+ * tzr_icp_point_to_plane_robust_batch checks it).  A NULL array or entry is TZR_ERR_INVALID_ARG.  Per problem, every
+ * output is bit-identical to tzr_icp_colored on that problem alone. */
+int tzr_icp_colored_batch(tzr_ctx* ctx, const tzr_icp_params* params, int B, const int32_t* ns,
+                          const float* const* src, const int32_t* nd, const float* const* dst,
+                          const float* const* dst_normals, const tzr_similarity* init, tzr_icp_result* results,
+                          int32_t* const* corr, const float* const* src_colors, const float* const* dst_colors,
+                          double lambda_geometric, const tzr_robust_kernel* kernel);
+
+/* One problem: tzr_icp_point_to_plane's arguments plus src_colors (ns x 3 floats), dst_colors (nd x 3 floats),
+ * lambda_geometric and kernel (may be NULL).  This is tzr_icp_colored_batch with B = 1. */
+int tzr_icp_colored(tzr_ctx* ctx, const tzr_icp_params* params, const float* src, int ns, const float* dst, int nd,
+                    const float* dst_normals, const tzr_similarity* init, tzr_icp_result* result, int32_t* corr,
+                    const float* src_colors, const float* dst_colors, double lambda_geometric,
+                    const tzr_robust_kernel* kernel);
+
 /* ---- multiway registration: information matrices ------------------------------------------------------------
  * Open3D's GetInformationMatrixFromPointClouds(source, target, max_correspondence_distance, T) for many pairs at once,
  * defined here as follows (DESIGN.md §3.16):
@@ -907,7 +989,7 @@ int tzr_register_cloud_pairs_multiway(tzr_ctx* ctx, const tzr_frontend_params* f
  *     starting from 0.0 (Open3D's AccumulatedPoint), divided by (double) count, the mean rounded once to float.
  *   - Output order: voxels ordered by their first (lowest-index) member.  (Open3D's order is its unordered_map's.)  A
  *     cloud already sparser than the grid comes back unchanged, in the same order.
- *   - Colours and normals are not carried.
+ *   - Normals are not carried; colours are, by tzr_voxel_downsample_colors(_batch) below.
  * Cost: a voxel of k points costs one thread k dependent additions (the bit-exact sequential sum), so one voxel holding
  * a whole cloud is correct but slow.  Host pointers, synchronous; 10 kernel launches per call (CUB calls counted as
  * one), whatever B.  These calls are not solve entries: they use a workspace of their own, so a retained solve
@@ -927,6 +1009,19 @@ int tzr_voxel_downsample(tzr_ctx* ctx, const float* pts, int n, double voxel_siz
  * fit the device (tzr_last_error names the size). */
 int tzr_voxel_downsample_batch(tzr_ctx* ctx, int B, const int32_t* n, const float* const* pts, double voxel_size,
                                float* const* pts_out, int32_t* n_out, int32_t* const* voxel_of, int32_t* status);
+
+/* Voxel downsampling with colours (coloured ICP's input, DESIGN.md §3.17): tzr_voxel_downsample(_batch)'s arguments
+ * plus colors (n x 3 floats per cloud, read as float64) and colors_out (room for n x 3 floats per cloud; receives
+ * n_out rows).  Each voxel's colour is the sum of its members' colours, added one at a time in ascending input index
+ * starting from 0.0, divided by (double) count and rounded once to float, exactly like its point.  Points, n_out,
+ * voxel_of and status are bit-identical to tzr_voxel_downsample(_batch)'s; a NULL colors or colors_out (or entry) is
+ * TZR_ERR_INVALID_ARG.  Launches and workspace as tzr_voxel_downsample(_batch). */
+int tzr_voxel_downsample_colors(tzr_ctx* ctx, const float* pts, int n, double voxel_size, float* pts_out,
+                                int32_t* n_out, int32_t* voxel_of, const float* colors, float* colors_out);
+int tzr_voxel_downsample_colors_batch(tzr_ctx* ctx, int B, const int32_t* n, const float* const* pts,
+                                      double voxel_size, float* const* pts_out, int32_t* n_out,
+                                      int32_t* const* voxel_of, int32_t* status, const float* const* colors,
+                                      float* const* colors_out);
 
 /* Graph-stage timing of the most recent tzr_solve_batch_dev, in milliseconds, measured with CUDA
  * events on the context's stream (for the roofline line in bench.py). Requires a prior synchronize. */

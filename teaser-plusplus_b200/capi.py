@@ -165,7 +165,8 @@ _SYMBOLS = [
     "tzr_register_cloud_pairs_icp_generalized", "tzr_icp_point_to_plane_robust_batch", "tzr_icp_generalized_robust_batch",
     "tzr_register_cloud_pairs_icp_robust", "tzr_ctx_last_strip_blocks", "tzr_graph_strip_schedule",
     "tzr_information_matrix", "tzr_information_matrix_batch", "tzr_pose_graph_params_default", "tzr_pose_graph_optimize",
-    "tzr_register_cloud_pairs_multiway",
+    "tzr_register_cloud_pairs_multiway", "tzr_estimate_color_gradients", "tzr_estimate_color_gradients_batch",
+    "tzr_icp_colored", "tzr_icp_colored_batch", "tzr_voxel_downsample_colors", "tzr_voxel_downsample_colors_batch",
 ]
 
 # status codes (tzr_status)
@@ -332,8 +333,15 @@ def lib():
                                           C.POINTER(Similarity), dp, u8p, dp, C.POINTER(PoseGraphSummary)]
     L.tzr_register_cloud_pairs_multiway.argtypes = L.tzr_register_cloud_pairs_icp.argtypes + [
         i32p, C.POINTER(PoseGraphParams), dp, i32p, dp, u8p, C.POINTER(Similarity), C.POINTER(PoseGraphSummary), i32p]
+    L.tzr_estimate_color_gradients.argtypes = [vp, fp, C.c_int, fp, fp, C.c_double, dp]
+    L.tzr_estimate_color_gradients_batch.argtypes = [vp, C.c_int, i32p, fpp, fpp, fpp, C.c_double, C.POINTER(dp), i32p]
+    L.tzr_icp_colored.argtypes = L.tzr_icp_point_to_plane.argtypes + [fp, fp, C.c_double, C.POINTER(RobustKernel)]
+    L.tzr_icp_colored_batch.argtypes = L.tzr_icp_point_to_plane_batch.argtypes + [fpp, fpp, C.c_double,
+                                                                                   C.POINTER(RobustKernel)]
     L.tzr_voxel_downsample.argtypes = [vp, fp, C.c_int, C.c_double, fp, i32p, i32p]
     L.tzr_voxel_downsample_batch.argtypes = [vp, C.c_int, i32p, fpp, C.c_double, fpp, i32p, C.POINTER(i32p), i32p]
+    L.tzr_voxel_downsample_colors.argtypes = L.tzr_voxel_downsample.argtypes + [fp, fp]
+    L.tzr_voxel_downsample_colors_batch.argtypes = L.tzr_voxel_downsample_batch.argtypes + [fpp, fpp]
     for s in _SYMBOLS:
         getattr(L, s)  # raises AttributeError if the header and the library disagree
     _lib = L
@@ -442,6 +450,14 @@ def _normals32(a, n, what):
     if a.shape[1] == 3:
         a = np.concatenate([a, np.zeros((n, 1), dtype=np.float32)], axis=1)
     return np.ascontiguousarray(a)
+
+
+def _colors32(a, n, what):
+    """Colours as (n,3) float32 rows (r, g, b), one per point."""
+    a = np.ascontiguousarray(a, dtype=np.float32)
+    if a.shape != (n, 3):
+        raise TzrError(f"{what}: colours must be (n,3) with one row per point")
+    return a
 
 
 def _pts(a):
@@ -866,6 +882,86 @@ class Context:
             e.status, e.result = status, nors
             raise
         return nors
+
+    def estimate_color_gradients(self, pts, normals, colors, radius):
+        """tzr_estimate_color_gradients: Open3D's colour gradients of one (n,3) float32 cloud with its (n,3) or (n,4)
+        normals and (n,3) colours, at `radius`: (n,3) float64."""
+        return self.estimate_color_gradients_batch([pts], [normals], [colors], radius, single=True)[0]
+
+    def estimate_color_gradients_batch(self, pts_list, normals, colors, radius, single=False):
+        """estimate_color_gradients of every cloud of the list in one call (tzr_estimate_color_gradients_batch): a list
+        of (n_b,3) float64 gradients, each bit-identical to estimate_color_gradients on that cloud alone.  single=True
+        goes through tzr_estimate_color_gradients (one cloud)."""
+        pts = [_cloud32(p, "estimate_color_gradients") for p in pts_list]
+        if not pts or len(normals) != len(pts) or len(colors) != len(pts):
+            raise TzrError("estimate_color_gradients_batch: one normals and one colours array per cloud are required")
+        N = [_normals32(a, p.shape[0], "estimate_color_gradients") for a, p in zip(normals, pts)]
+        K = [_colors32(a, p.shape[0], "estimate_color_gradients") for a, p in zip(colors, pts)]
+        B = len(pts)
+        grads = [np.zeros((p.shape[0], 3), dtype=np.float64) for p in pts]
+        fp, dp = C.POINTER(C.c_float), C.POINTER(C.c_double)
+        if single:
+            assert B == 1
+            rc = lib().tzr_estimate_color_gradients(self._h, _p(pts[0], C.c_float), pts[0].shape[0], _p(N[0], C.c_float),
+                                                    _p(K[0], C.c_float), float(radius), _p(grads[0], C.c_double))
+        else:
+            n = np.array([p.shape[0] for p in pts], dtype=np.int32)
+            rc = lib().tzr_estimate_color_gradients_batch(
+                self._h, B, _p(n, C.c_int32), (fp * B)(*[_p(p, C.c_float) for p in pts]),
+                (fp * B)(*[_p(a, C.c_float) for a in N]), (fp * B)(*[_p(a, C.c_float) for a in K]), float(radius),
+                (dp * B)(*[_p(g, C.c_double) for g in grads]), None)
+        self._ck(rc)
+        return grads
+
+    def icp_colored(self, src, dst, dst_normals, src_colors, dst_colors, max_correspondence_distance, init=None,
+                    lambda_geometric=0.968, max_iteration=30, relative_fitness=1e-6, relative_rmse=1e-6, kernel=None):
+        """tzr_icp_colored: Open3D's coloured ICP of the (ns,3) source onto the (nd,3) target with the target's normals
+        and both clouds' (n,3) colours; kernel (see robust_kernel()) may be None.  Returns what icp() returns."""
+        res, corr = self.icp_colored_batch([src], [dst], [dst_normals], [src_colors], [dst_colors],
+                                           max_correspondence_distance, None if init is None else [init],
+                                           lambda_geometric=lambda_geometric, max_iteration=max_iteration,
+                                           relative_fitness=relative_fitness, relative_rmse=relative_rmse,
+                                           single=True, kernel=kernel)
+        return icp_result_dict(res[0]), corr[0]
+
+    def icp_colored_batch(self, srcs, dsts, dst_normals, src_colors, dst_colors, max_correspondence_distance,
+                          inits=None, lambda_geometric=0.968, max_iteration=30, relative_fitness=1e-6,
+                          relative_rmse=1e-6, single=False, kernel=None):
+        """tzr_icp_colored_batch: icp_point_to_plane_batch() with coloured updates and one (n,3) colours array per
+        source and per target.  single=True goes through tzr_icp_colored (B must be 1).  Returns what icp_batch()
+        returns."""
+        S = [_cloud32(a, "icp_colored") for a in srcs]
+        D = [_cloud32(a, "icp_colored") for a in dsts]
+        B = len(S)
+        if B == 0 or len(D) != B or len(dst_normals) != B or len(src_colors) != B or len(dst_colors) != B or \
+                (inits is not None and len(inits) != B):
+            raise TzrError("icp_colored_batch: one target, normals, colours and seed per source cloud are required")
+        N = [_normals32(a, d.shape[0], "icp_colored") for a, d in zip(dst_normals, D)]
+        SC = [_colors32(a, x.shape[0], "icp_colored") for a, x in zip(src_colors, S)]
+        DC = [_colors32(a, x.shape[0], "icp_colored") for a, x in zip(dst_colors, D)]
+        p = icp_params(max_correspondence_distance, max_iteration=int(max_iteration),
+                       relative_fitness=float(relative_fitness), relative_rmse=float(relative_rmse))
+        init = (Similarity * B)(*[similarity(None if inits is None else x) for x in inits or [None] * B])
+        res = (IcpResult * B)()
+        corr = [np.zeros((a.shape[0], 2), dtype=np.int32) for a in S]
+        kern = robust_kernel(kernel)
+        kp = C.byref(kern) if kern is not None else None
+        fp, i32p = C.POINTER(C.c_float), C.POINTER(C.c_int32)
+        if single:
+            assert B == 1
+            rc = lib().tzr_icp_colored(self._h, C.byref(p), _p(S[0], C.c_float), S[0].shape[0], _p(D[0], C.c_float),
+                                       D[0].shape[0], _p(N[0], C.c_float), init, res, _p(corr[0], C.c_int32),
+                                       _p(SC[0], C.c_float), _p(DC[0], C.c_float), float(lambda_geometric), kp)
+        else:
+            ns = np.array([a.shape[0] for a in S], dtype=np.int32)
+            nd = np.array([a.shape[0] for a in D], dtype=np.int32)
+            arr = lambda xs: (fp * B)(*[_p(a, C.c_float) for a in xs])  # noqa: E731
+            rc = lib().tzr_icp_colored_batch(self._h, C.byref(p), B, _p(ns, C.c_int32), arr(S), _p(nd, C.c_int32),
+                                             arr(D), arr(N), init, res, (i32p * B)(*[_p(c, C.c_int32) for c in corr]),
+                                             arr(SC), arr(DC), float(lambda_geometric), kp)
+        self._ck(rc)
+        out = np.frombuffer(bytes(res), dtype=ICP_RESULT_DTYPE).copy()
+        return out, [c[:int(r["n_correspondences"])].copy() for c, r in zip(corr, out)]
 
     @staticmethod
     def _rows3(a, n, what):
@@ -1380,42 +1476,65 @@ class Context:
         out = np.frombuffer(bytes(res), dtype=ICP_RESULT_DTYPE).copy()
         return out, [c[:int(r["n_correspondences"])].copy() for c, r in zip(corr, out)]
 
-    def voxel_downsample(self, pts, voxel_size, return_trace=False):
-        """tzr_voxel_downsample: Open3D's voxel_down_sample of one (n,3) float32 cloud, points only (the definition is
+    def voxel_downsample(self, pts, voxel_size, return_trace=False, colors=None):
+        """tzr_voxel_downsample: Open3D's voxel_down_sample of one (n,3) float32 cloud (the definition is
         include/teaser_b200.h's): the (m,3) float32 voxel means ordered by each voxel's first member, and with
-        return_trace the (n,) int32 output row of every input point (-1: a non-finite point)."""
+        return_trace the (n,) int32 output row of every input point (-1: a non-finite point).  colors ((n,3), through
+        tzr_voxel_downsample_colors): the (m,3) float32 colour means are returned after the points."""
         p = _cloud32(pts, "voxel_downsample")
+        K = None if colors is None else _colors32(colors, p.shape[0], "voxel_downsample")
         out = np.zeros_like(p)
+        cout = None if K is None else np.zeros_like(p)
         trace = np.zeros(p.shape[0], dtype=np.int32)
         m = np.zeros(1, dtype=np.int32)
-        self._ck(lib().tzr_voxel_downsample(self._h, _p(p, C.c_float), p.shape[0], float(voxel_size),
-                                            _p(out, C.c_float), _p(m, C.c_int32),
-                                            _p(trace, C.c_int32) if return_trace else None))
-        out = out[:int(m[0])].copy()
-        return (out, trace) if return_trace else out
+        args = (self._h, _p(p, C.c_float), p.shape[0], float(voxel_size), _p(out, C.c_float), _p(m, C.c_int32),
+                _p(trace, C.c_int32) if return_trace else None)
+        if K is None:
+            self._ck(lib().tzr_voxel_downsample(*args))
+        else:
+            self._ck(lib().tzr_voxel_downsample_colors(*args, _p(K, C.c_float), _p(cout, C.c_float)))
+        res = [out[:int(m[0])].copy()]
+        if K is not None:
+            res.append(cout[:int(m[0])].copy())
+        if return_trace:
+            res.append(trace)
+        return res[0] if len(res) == 1 else tuple(res)
 
-    def voxel_downsample_batch(self, pts_list, voxel_size, return_trace=False):
+    def voxel_downsample_batch(self, pts_list, voxel_size, return_trace=False, colors=None):
         """voxel_downsample of every (n_b,3) cloud of the list in one call (tzr_voxel_downsample_batch): a list of
-        (m_b,3) voxel means (and a list of traces), each bit-identical to voxel_downsample on that cloud alone.  When a
-        cloud's grid is too large the TzrError carries `status` (per cloud 0 or the error code) and `result` (the
-        outputs of every cloud, written for the others; empty for the too-large ones)."""
+        (m_b,3) voxel means (and a list of traces), each bit-identical to voxel_downsample on that cloud alone.  colors
+        (one (n_b,3) array per cloud, through tzr_voxel_downsample_colors_batch): a list of colour means follows the
+        points.  When a cloud's grid is too large the TzrError carries `status` (per cloud 0 or the error code) and
+        `result` (the outputs of every cloud, written for the others; empty for the too-large ones)."""
         pts = [_cloud32(p, "voxel_downsample_batch") for p in pts_list]
         if not pts:
             raise TzrError("voxel_downsample_batch: a non-empty list of (n,3) clouds is required")
         B = len(pts)
+        if colors is not None and len(colors) != B:
+            raise TzrError("voxel_downsample_batch: one colours array per cloud is required")
+        K = None if colors is None else [_colors32(c, p.shape[0], "voxel_downsample_batch") for c, p in zip(colors, pts)]
         n = np.array([p.shape[0] for p in pts], dtype=np.int32)
         outs = [np.zeros_like(p) for p in pts]
+        couts = None if K is None else [np.zeros_like(p) for p in pts]
         traces = [np.zeros(p.shape[0], dtype=np.int32) for p in pts] if return_trace else None
         m = np.zeros(B, dtype=np.int32)
         status = np.zeros(B, dtype=np.int32)
         fp, i32p = C.POINTER(C.c_float), C.POINTER(C.c_int32)
-        rc = lib().tzr_voxel_downsample_batch(self._h, B, _p(n, C.c_int32), (fp * B)(*[_p(p, C.c_float) for p in pts]),
-                                              float(voxel_size), (fp * B)(*[_p(o, C.c_float) for o in outs]),
-                                              _p(m, C.c_int32),
-                                              (i32p * B)(*[_p(t, C.c_int32) for t in traces]) if traces else None,
-                                              _p(status, C.c_int32))
+        args = (self._h, B, _p(n, C.c_int32), (fp * B)(*[_p(p, C.c_float) for p in pts]), float(voxel_size),
+                (fp * B)(*[_p(o, C.c_float) for o in outs]), _p(m, C.c_int32),
+                (i32p * B)(*[_p(t, C.c_int32) for t in traces]) if traces else None, _p(status, C.c_int32))
+        if K is None:
+            rc = lib().tzr_voxel_downsample_batch(*args)
+        else:
+            rc = lib().tzr_voxel_downsample_colors_batch(*args, (fp * B)(*[_p(c, C.c_float) for c in K]),
+                                                         (fp * B)(*[_p(c, C.c_float) for c in couts]))
         outs = [o[:int(k)].copy() for o, k in zip(outs, m)]
-        result = (outs, traces) if return_trace else outs
+        res = [outs]
+        if K is not None:
+            res.append([o[:int(k)].copy() for o, k in zip(couts, m)])
+        if return_trace:
+            res.append(traces)
+        result = res[0] if len(res) == 1 else tuple(res)
         try:
             self._ck(rc)
         except TzrError as e:

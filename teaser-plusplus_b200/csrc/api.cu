@@ -1046,6 +1046,57 @@ int fpfh_run(tzr_ctx* ctx, int B, const int32_t* n, const float* const* pts, dou
   return TZR_OK;
 }
 
+// tzr_estimate_color_gradients(_batch): the front end's buffers as fpfh_run's.  m_in: [points | cloud table | normals
+// | colours], one H2D copy; m_scratch: the grid; m_out: the gradients, one D2H copy.
+int gradients_run(tzr_ctx* ctx, int B, const int32_t* n, const float* const* pts, const float* const* normals,
+                  const float* const* colors, double radius, double* const* grad_out, int32_t* status) {
+  if (!ctx || B < 1 || !n || !pts || !normals || !colors || !grad_out || !(radius > 0) || !std::isfinite(radius))
+    return TZR_ERR_INVALID_ARG;
+  for (int b = 0; b < B; ++b)
+    if (n[b] <= 0 || !pts[b] || !normals[b] || !colors[b] || !grad_out[b]) return TZR_ERR_INVALID_ARG;
+  std::vector<FpfhCloud> clouds((size_t)B);
+  FpfhPlan plan;
+  const int route = search_route(ctx->flags, kFlagFpfhBrute, kFlagFpfhGrid);
+  if (fpfh_plan(B, n, radius, radius, route, clouds.data(), &plan) != TZR_OK) {
+    ctx->last_error = "the batch's points do not fit 32-bit indices";
+    return TZR_ERR_TOO_LARGE;
+  }
+  cudaSetDevice(ctx->device);
+  cudaStream_t st = ctx->stream;
+  const size_t N = (size_t)plan.N;
+  const size_t o_cl = al256(N * 12), o_nrm = o_cl + al256((size_t)B * sizeof(FpfhCloud)), o_col = o_nrm + al256(N * 16);
+  const size_t in_bytes = o_col + N * 12, out_bytes = N * 24;
+  int rc;
+  if ((rc = ensure(ctx, ctx->m_in, in_bytes)) != TZR_OK) return rc;
+  if ((rc = ensure(ctx, ctx->m_scratch, plan.grid_bytes + 256)) != TZR_OK) return rc;
+  if ((rc = ensure(ctx, ctx->m_out, out_bytes)) != TZR_OK) return rc;
+  if ((rc = ensure_pinned(ctx, al256(in_bytes) + out_bytes)) != TZR_OK) return rc;
+  char* h_in = (char*)ctx->h_pin;
+  char* h_out = h_in + al256(in_bytes);
+  std::vector<CopySpan> spans;
+  for (int b = 0; b < B; ++b) {
+    const size_t lo = (size_t)clouds[b].lo;
+    spans.push_back(CopySpan{h_in + lo * 12, pts[b], (size_t)n[b] * 12});
+    spans.push_back(CopySpan{h_in + o_nrm + lo * 16, normals[b], (size_t)n[b] * 16});
+    spans.push_back(CopySpan{h_in + o_col + lo * 12, colors[b], (size_t)n[b] * 12});
+  }
+  memcpy(h_in + o_cl, clouds.data(), (size_t)B * sizeof(FpfhCloud));
+  parallel_copy(spans);
+  char* d_in = (char*)ctx->m_in.p;
+  CK(cudaMemcpyAsync(d_in, h_in, in_bytes, cudaMemcpyHostToDevice, st));
+  double* d_grad = (double*)ctx->m_out.p;
+  ctx->launches += launch_color_gradients(plan, (const float*)d_in, (FpfhCloud*)(d_in + o_cl), radius,
+                                          (const float4*)(d_in + o_nrm), (const float*)(d_in + o_col), d_grad,
+                                          plan.grid_bytes ? ctx->m_scratch.p : nullptr, st);
+  if ((rc = check_launch(ctx, "color gradient launch")) != TZR_OK) return rc;
+  spans.clear();
+  for (int b = 0; b < B; ++b)
+    spans.push_back(CopySpan{grad_out[b], h_out + (size_t)clouds[b].lo * 24, (size_t)n[b] * 24});
+  CK(stage_out(spans, h_out, (const char*)d_grad, out_bytes, false, st));
+  for (int b = 0; b < B && status; ++b) status[b] = TZR_OK;
+  return TZR_OK;
+}
+
 // tzr_match_correspondences(_batch): B pairs staged back to back in one pinned area with the pair table and the NN
 // work list, one H2D copy, the batched launches, one D2H copy of [counts | global scales | pairs].
 int match_run(tzr_ctx* ctx, int B, const int32_t* ns, const float* const* src_pts, const int32_t* nd,
@@ -2010,6 +2061,18 @@ int tzr_estimate_normals_batch(tzr_ctx* ctx, int B, const int32_t* n, const floa
   return fpfh_run(ctx, B, n, pts, normal_search_radius, 0.0, nullptr, normals_out, status, true);
 }
 
+int tzr_estimate_color_gradients(tzr_ctx* ctx, const float* pts, int n, const float* normals, const float* colors,
+                                 double radius, double* grad_out) {
+  const int32_t n1 = n;
+  return gradients_run(ctx, 1, &n1, &pts, &normals, &colors, radius, &grad_out, nullptr);
+}
+
+int tzr_estimate_color_gradients_batch(tzr_ctx* ctx, int B, const int32_t* n, const float* const* pts,
+                                       const float* const* normals, const float* const* colors, double radius,
+                                       double* const* grad_out, int32_t* status) {
+  return gradients_run(ctx, B, n, pts, normals, colors, radius, grad_out, status);
+}
+
 void tzr_frontend_params_default(tzr_frontend_params* p) {
   if (!p) return;
   p->normal_search_radius = 0.03;  // fpfh.h:39-41
@@ -2742,25 +2805,38 @@ void tzr_icp_params_default(tzr_icp_params* p) {
 static int icp_batch_stage(tzr_ctx* ctx, IcpPlan* plan, int B, const int32_t* ns, const float* const* src,
                            const float* const* src_normals, const int32_t* nd, const float* const* dst,
                            const float* const* dst_normals, const tzr_similarity* init, double r, bool information,
-                           std::vector<IcpProb>* probs, IcpBuffers* buf) {
+                           std::vector<IcpProb>* probs, IcpBuffers* buf, const float* const* src_colors = nullptr,
+                           const float* const* dst_colors = nullptr) {
   const bool plane = plan->mode != kIcpPointToPoint, gicp = plan->mode == kIcpGeneralized;
-  if (!ctx || B < 1 || !ns || !src || !nd || !dst || (plane && !dst_normals) || (gicp && !src_normals) || !init)
+  const bool colored = plan->mode == kIcpColored;
+  if (!ctx || B < 1 || !ns || !src || !nd || !dst || (plane && !dst_normals) || (gicp && !src_normals) || !init ||
+      (colored && (!src_colors || !dst_colors)))
     return TZR_ERR_INVALID_ARG;
   for (int b = 0; b < B; ++b)
     if (ns[b] < 1 || nd[b] < 1 || !src[b] || !dst[b] || (plane && !dst_normals[b]) || (gicp && !src_normals[b]) ||
-        !similarity_ok(init[b]))
+        (colored && (!src_colors[b] || !dst_colors[b])) || !similarity_ok(init[b]))
       return TZR_ERR_INVALID_ARG;
-  std::vector<FpfhCloud> clouds;
+  std::vector<FpfhCloud> clouds, gclouds;
   std::vector<int> chunk_prob;
   if (icp_plan(B, ns, nullptr, nullptr, B, nd, r, search_route(ctx->flags, kFlagIcpBrute, kFlagIcpGrid), init, plan,
                &clouds, probs, &chunk_prob) != TZR_OK) {
     ctx->last_error = "the batch's points or target grid do not fit 32-bit indices";
     return TZR_ERR_TOO_LARGE;
   }
+  if (colored) {  // the gradient pass: tzr_estimate_color_gradients_batch's plan over the same targets at 2 r
+    plan->grad_r = 2.0 * r;
+    gclouds.resize((size_t)B);
+    if (fpfh_plan(B, nd, plan->grad_r, plan->grad_r, search_route(ctx->flags, kFlagFpfhBrute, kFlagFpfhGrid),
+                  gclouds.data(), &plan->ggrid) != TZR_OK) {
+      ctx->last_error = "the batch's targets do not fit 32-bit indices";
+      return TZR_ERR_TOO_LARGE;
+    }
+  }
   cudaSetDevice(ctx->device);
   const size_t NS = (size_t)plan->NS, ND = (size_t)plan->ND;
   const size_t o_dst = al256(NS * 12), o_nrm = o_dst + al256(ND * 12), o_snrm = o_nrm + al256(plane ? ND * 16 : 0);
-  const IcpLayout L = icp_layout(*plan, al256(o_snrm + (gicp ? NS * 16 : 0)), information);
+  const size_t o_scol = o_snrm + al256(gicp ? NS * 16 : 0), o_dcol = o_scol + al256(colored ? NS * 12 : 0);
+  const IcpLayout L = icp_layout(*plan, al256(o_dcol + (colored ? ND * 12 : 0)), information);
   int rc;
   if ((rc = ensure(ctx, ctx->icp, L.end)) != TZR_OK) return rc;
   std::vector<char> h(L.match);
@@ -2770,17 +2846,28 @@ static int icp_batch_stage(tzr_ctx* ctx, IcpPlan* plan, int B, const int32_t* ns
     memcpy(h.data() + o_dst + (size_t)pr.d_lo * 12, dst[b], (size_t)nd[b] * 12);
     if (plane) memcpy(h.data() + o_nrm + (size_t)pr.n_lo * 16, dst_normals[b], (size_t)nd[b] * 16);
     if (gicp) memcpy(h.data() + o_snrm + (size_t)pr.sn_lo * 16, src_normals[b], (size_t)ns[b] * 16);
+    if (colored) {
+      memcpy(h.data() + o_scol + (size_t)pr.s_lo * 12, src_colors[b], (size_t)ns[b] * 12);
+      memcpy(h.data() + o_dcol + (size_t)pr.d_lo * 12, dst_colors[b], (size_t)nd[b] * 12);
+    }
   }
   memcpy(h.data() + L.probs, probs->data(), (size_t)B * sizeof(IcpProb));
   memcpy(h.data() + L.clouds, clouds.data(), (size_t)B * sizeof(FpfhCloud));
   memcpy(h.data() + L.chunks, chunk_prob.data(), chunk_prob.size() * 4);
   char* d = (char*)ctx->icp.p;
   CK(cudaMemcpyAsync(d, h.data(), L.match, cudaMemcpyHostToDevice, ctx->stream));
+  if (colored)
+    CK(cudaMemcpyAsync(d + L.gclouds, gclouds.data(), (size_t)B * sizeof(FpfhCloud), cudaMemcpyHostToDevice,
+                       ctx->stream));
   *buf = icp_buffers(d, L);
   buf->src = (const float*)d;
   buf->dst = (const float*)(d + o_dst);
   buf->dst_normals = plane ? (const float4*)(d + o_nrm) : nullptr;
   buf->src_normals = gicp ? (const float4*)(d + o_snrm) : nullptr;
+  if (colored) {
+    buf->src_colors = (const float*)(d + o_scol);
+    buf->dst_colors = (const float*)(d + o_dcol);
+  }
   return TZR_OK;
 }
 
@@ -2793,15 +2880,17 @@ static int icp_batch_run(tzr_ctx* ctx, const tzr_icp_params* params, int mode, i
                          const float* const* src, const float* const* src_normals, const int32_t* nd,
                          const float* const* dst, const float* const* dst_normals, double epsilon,
                          const tzr_similarity* init, tzr_icp_result* results, int32_t* const* corr,
-                         const tzr_robust_kernel* kernel = nullptr) {
+                         const tzr_robust_kernel* kernel = nullptr, double lambda_geometric = 0.0,
+                         const float* const* src_colors = nullptr, const float* const* dst_colors = nullptr) {
   if (!icp_params_ok(params) || (mode == kIcpGeneralized && !icp_epsilon_ok(epsilon)) || !results)
     return TZR_ERR_INVALID_ARG;
   IcpPlan plan;
   icp_iteration_settings(&plan, *params, mode, epsilon, kernel);
+  plan.lambda_geometric = lambda_geometric;
   std::vector<IcpProb> probs;
   IcpBuffers buf;
   int rc = icp_batch_stage(ctx, &plan, B, ns, src, src_normals, nd, dst, dst_normals, init,
-                           params->max_correspondence_distance, false, &probs, &buf);
+                           params->max_correspondence_distance, false, &probs, &buf, src_colors, dst_colors);
   if (rc != TZR_OK) return rc;
   cudaStream_t st = ctx->stream;
   ctx->launches += launch_icp(plan, buf, st);
@@ -2870,6 +2959,35 @@ int tzr_icp_generalized_robust_batch(tzr_ctx* ctx, const tzr_icp_params* params,
   if (!robust_kernel_ok(kernel)) return TZR_ERR_INVALID_ARG;
   return icp_batch_run(ctx, params, kIcpGeneralized, B, ns, src, src_normals, nd, dst, dst_normals, epsilon, init,
                        results, corr, kernel);
+}
+
+// tzr_icp_colored(_batch): lambda outside [0, 1] becomes 0.968 (Open3D's TransformationEstimationForColoredICP), a
+// non-finite one and a bad kernel are refused before any device work; NULL kernel = L2.
+int tzr_icp_colored_batch(tzr_ctx* ctx, const tzr_icp_params* params, int B, const int32_t* ns,
+                          const float* const* src, const int32_t* nd, const float* const* dst,
+                          const float* const* dst_normals, const tzr_similarity* init, tzr_icp_result* results,
+                          int32_t* const* corr, const float* const* src_colors, const float* const* dst_colors,
+                          double lambda_geometric, const tzr_robust_kernel* kernel) {
+  if (!std::isfinite(lambda_geometric) || (kernel && !robust_kernel_ok(kernel))) return TZR_ERR_INVALID_ARG;
+  if (lambda_geometric < 0.0 || lambda_geometric > 1.0) lambda_geometric = 0.968;
+  return icp_batch_run(ctx, params, kIcpColored, B, ns, src, nullptr, nd, dst, dst_normals, 0.0, init, results, corr,
+                       kernel, lambda_geometric, src_colors, dst_colors);
+}
+
+int tzr_icp_colored(tzr_ctx* ctx, const tzr_icp_params* params, const float* src, int ns, const float* dst, int nd,
+                    const float* dst_normals, const tzr_similarity* init, tzr_icp_result* result, int32_t* corr,
+                    const float* src_colors, const float* dst_colors, double lambda_geometric,
+                    const tzr_robust_kernel* kernel) {
+  tzr_similarity id;
+  if (!init) {
+    memset(&id, 0, sizeof(id));
+    id.scale = 1.0;
+    id.rotation[0] = id.rotation[4] = id.rotation[8] = 1.0;
+    init = &id;
+  }
+  int32_t* const corrs[1] = {corr};
+  return tzr_icp_colored_batch(ctx, params, 1, &ns, &src, &nd, &dst, &dst_normals, init, result,
+                               corr ? corrs : nullptr, &src_colors, &dst_colors, lambda_geometric, kernel);
 }
 
 // the single-problem entries: icp_batch_run with B = 1 and init NULL meaning the identity
@@ -2974,13 +3092,18 @@ int tzr_register_cloud_pairs_multiway(tzr_ctx* ctx, const tzr_frontend_params* f
 // tzr_voxel_downsample(_batch): the clouds staged back to back (one H2D copy), the batch's launches (launch_voxel), a
 // read-back of the cloud table, then one D2H copy of the batch's voxels (and of voxel_of when some cloud asks for it).
 // Workspace ctx->vox: [points | cloud table | voxels | voxel_of | scratch]; the pinned area mirrors its first four.
-int tzr_voxel_downsample_batch(tzr_ctx* ctx, int B, const int32_t* n, const float* const* pts, double voxel_size,
-                               float* const* pts_out, int32_t* n_out, int32_t* const* voxel_of, int32_t* status) {
-  if (!ctx || B < 1 || !n || !pts || !pts_out || !n_out || !(voxel_size > 0) || !std::isfinite(voxel_size))
+// With colours (tzr_voxel_downsample_colors(_batch)): [points | colours | cloud table | voxels | colour means | voxel_of
+// | scratch]; without them the colour regions are empty and the layout is the one above.
+static int voxel_run(tzr_ctx* ctx, int B, const int32_t* n, const float* const* pts, double voxel_size,
+                     float* const* pts_out, int32_t* n_out, int32_t* const* voxel_of, int32_t* status,
+                     const float* const* colors, float* const* colors_out, bool with_colors) {
+  if (!ctx || B < 1 || !n || !pts || !pts_out || !n_out || !(voxel_size > 0) || !std::isfinite(voxel_size) ||
+      (with_colors && (!colors || !colors_out)))
     return TZR_ERR_INVALID_ARG;
   bool want_trace = false;
   for (int b = 0; b < B; ++b) {
-    if (n[b] < 1 || !pts[b] || !pts_out[b]) return TZR_ERR_INVALID_ARG;
+    if (n[b] < 1 || !pts[b] || !pts_out[b] || (with_colors && (!colors[b] || !colors_out[b])))
+      return TZR_ERR_INVALID_ARG;
     want_trace |= voxel_of && voxel_of[b];
   }
   std::vector<VoxCloud> clouds((size_t)B);
@@ -2991,9 +3114,10 @@ int tzr_voxel_downsample_batch(tzr_ctx* ctx, int B, const int32_t* n, const floa
   }
   cudaSetDevice(ctx->device);
   cudaStream_t st = ctx->stream;
-  const size_t N = (size_t)plan.N, pb = N * 12, tb = (size_t)B * sizeof(VoxCloud);
-  const size_t o_tab = al256(pb), in_bytes = o_tab + tb, o_out = al256(in_bytes), o_vo = o_out + al256(pb),
-               o_scr = o_vo + al256(N * 4), total = o_scr + plan.scratch_bytes;
+  const size_t N = (size_t)plan.N, pb = N * 12, tb = (size_t)B * sizeof(VoxCloud), cb = with_colors ? pb : 0;
+  const size_t o_col = al256(pb), o_tab = o_col + al256(cb), in_bytes = o_tab + tb, o_out = al256(in_bytes),
+               o_cout = o_out + al256(pb), o_vo = o_cout + al256(cb), o_scr = o_vo + al256(N * 4),
+               total = o_scr + plan.scratch_bytes;
   int rc;
   if ((rc = ensure(ctx, ctx->vox, total)) != TZR_OK) return rc;
   if ((rc = ensure_pinned(ctx, o_scr)) != TZR_OK) return rc;
@@ -3001,10 +3125,15 @@ int tzr_voxel_downsample_batch(tzr_ctx* ctx, int B, const int32_t* n, const floa
   char* d = (char*)ctx->vox.p;
   std::vector<CopySpan> spans;
   for (int b = 0; b < B; ++b) spans.push_back(CopySpan{h + (size_t)clouds[b].lo * 12, pts[b], (size_t)n[b] * 12});
+  if (with_colors)
+    for (int b = 0; b < B; ++b)
+      spans.push_back(CopySpan{h + o_col + (size_t)clouds[b].lo * 12, colors[b], (size_t)n[b] * 12});
   spans.push_back(CopySpan{h + o_tab, clouds.data(), tb});
   CK(stage_in(spans, h, d, o_tab, in_bytes, B == 1, st));
   ctx->launches += launch_voxel(plan, voxel_size, (const float*)d, (VoxCloud*)(d + o_tab), d + o_scr,
-                                (float*)(d + o_out), (int*)(d + o_vo), st);
+                                (float*)(d + o_out), (int*)(d + o_vo), st,
+                                with_colors ? (const float*)(d + o_col) : nullptr,
+                                with_colors ? (float*)(d + o_cout) : nullptr);
   if ((rc = check_launch(ctx, "voxel launch")) != TZR_OK) return rc;
   CK(cudaMemcpyAsync(clouds.data(), d + o_tab, tb, cudaMemcpyDeviceToHost, st));
   CK(cudaStreamSynchronize(st));
@@ -3013,6 +3142,8 @@ int tzr_voxel_downsample_batch(tzr_ctx* ctx, int B, const int32_t* n, const floa
   for (int b = 0; b < B; ++b) {
     const VoxCloud& c = clouds[b];
     spans.push_back(CopySpan{pts_out[b], h + o_out + (size_t)c.out_lo * 12, (size_t)c.n_out * 12});
+    if (with_colors)
+      spans.push_back(CopySpan{colors_out[b], h + o_cout + (size_t)c.out_lo * 12, (size_t)c.n_out * 12});
     if (voxel_of && voxel_of[b]) spans.push_back(CopySpan{voxel_of[b], h + o_vo + (size_t)c.lo * 4, (size_t)c.n * 4});
   }
   if (B == 1) {  // straight into the caller's buffers
@@ -3021,6 +3152,7 @@ int tzr_voxel_downsample_batch(tzr_ctx* ctx, int B, const int32_t* n, const floa
     CK(cudaStreamSynchronize(st));
   } else {
     if (rows) CK(cudaMemcpyAsync(h + o_out, d + o_out, rows * 12, cudaMemcpyDeviceToHost, st));
+    if (rows && with_colors) CK(cudaMemcpyAsync(h + o_cout, d + o_cout, rows * 12, cudaMemcpyDeviceToHost, st));
     if (want_trace) CK(cudaMemcpyAsync(h + o_vo, d + o_vo, N * 4, cudaMemcpyDeviceToHost, st));
     CK(cudaStreamSynchronize(st));
     parallel_copy(spans);
@@ -3036,6 +3168,26 @@ int tzr_voxel_downsample_batch(tzr_ctx* ctx, int B, const int32_t* n, const floa
     return TZR_ERR_TOO_LARGE;
   }
   return TZR_OK;
+}
+
+int tzr_voxel_downsample_batch(tzr_ctx* ctx, int B, const int32_t* n, const float* const* pts, double voxel_size,
+                               float* const* pts_out, int32_t* n_out, int32_t* const* voxel_of, int32_t* status) {
+  return voxel_run(ctx, B, n, pts, voxel_size, pts_out, n_out, voxel_of, status, nullptr, nullptr, false);
+}
+
+int tzr_voxel_downsample_colors_batch(tzr_ctx* ctx, int B, const int32_t* n, const float* const* pts,
+                                      double voxel_size, float* const* pts_out, int32_t* n_out,
+                                      int32_t* const* voxel_of, int32_t* status, const float* const* colors,
+                                      float* const* colors_out) {
+  return voxel_run(ctx, B, n, pts, voxel_size, pts_out, n_out, voxel_of, status, colors, colors_out, true);
+}
+
+int tzr_voxel_downsample_colors(tzr_ctx* ctx, const float* pts, int n, double voxel_size, float* pts_out,
+                                int32_t* n_out, int32_t* voxel_of, const float* colors, float* colors_out) {
+  const int32_t n1 = n;
+  int32_t* const vo[1] = {voxel_of};
+  return tzr_voxel_downsample_colors_batch(ctx, 1, &n1, &pts, voxel_size, &pts_out, n_out, vo, nullptr, &colors,
+                                           &colors_out);
 }
 
 int tzr_voxel_downsample(tzr_ctx* ctx, const float* pts, int n, double voxel_size, float* pts_out, int32_t* n_out,

@@ -9,6 +9,9 @@
 //                    pcl::computePairFeatures and bins f1/f2/f3 (11 bins each); the `+= hist_incr` float additions are
 //                    replayed per bin from the integer counts (adding the same constant c times does not depend on
 //                    which neighbour came first).
+//   color_gradients_kernel  (coloured ICP, DESIGN.md §3.17) one CTA per point: the same radius search with a bounded
+//                    selection of the 30 nearest by (distance, index), then Open3D's 3 x 3 least-squares colour
+//                    gradient, solved by ldlt_solve<3>.
 //   fpfh_kernel      one CTA per point: radius search + sort, then pcl's weightPointSPFHSignature as written: three
 //                    threads (one per sub-histogram) run the sequential 1/d^2-weighted float sums in neighbour order
 //                    and normalise to 100.
@@ -588,6 +591,146 @@ __global__ void __launch_bounds__(kFpfhThreads) fpfh_kernel(Clouds cs, const flo
   for (int k = 0; k < 11; ++k) out[(size_t)p * 33 + 11 * s + k] = acc[k] * sc;
 }
 
+// ---- colour gradients (DESIGN.md §3.17) -------------------------------------------------------------------------------
+constexpr int kGradNn = 30;     // neighbours of a gradient (KDTreeSearchParamHybrid(R, 30))
+constexpr int kGradBuf = 512;   // shared candidate keys: kGradNn kept + at most 256 per round, compacted above 256
+
+// One CTA per point: the kGradNn smallest (d^2 bits << 32 | index) keys with float d^2 < r^2 (collect_neighbors' test,
+// over the same brute-force range or grid buckets), by a bounded selection: the candidates go through in rounds of
+// blockDim.x; a key enters the shared buffer only below the current threshold (the kGradNn-th key after the last
+// compaction), and once the buffer holds more than kGradBuf - kFpfhThreads keys it is sorted and cut to kGradNn.  No
+// key among the kGradNn smallest is ever dropped, so the result is the first kGradNn of the full (d^2, index) order,
+// whatever the neighbourhood's size.  Then one thread builds Open3D's 3 x 3 system (entry 0 skipped, the rows of
+// entries 1 ... nn - 1 in list order, the constraint row (nn - 1) n last) and solves it with ldlt_solve<3>.
+__global__ void __launch_bounds__(kFpfhThreads) color_gradients_kernel(Clouds cs, float r2,
+                                                                      const float4* __restrict__ normals,
+                                                                      const float* __restrict__ colors,
+                                                                      double* __restrict__ grad) {
+  __shared__ unsigned long long keys[kGradBuf];
+  __shared__ unsigned long long s_thresh;
+  __shared__ int s_count;
+  __shared__ int s_rs[28], s_re[28], s_pref[28];
+  const float* __restrict__ pts = cs.pts;
+  const int p = blockIdx.x;
+  const Grid g = cs.grid(cs.cloud(p));
+  const float qx = pts[3 * (size_t)p], qy = pts[3 * (size_t)p + 1], qz = pts[3 * (size_t)p + 2];
+  if (threadIdx.x == 0) {
+    s_count = 0;
+    s_thresh = ~0ull;
+  }
+  int total = g.n;  // brute force: candidate c is point g.lo + c
+  if (g.n_sorted) {  // the <= 27 distinct buckets of the 3x3x3 cell neighbourhood, as collect_neighbors walks them
+    if (threadIdx.x < 27) {
+      long long ix, iy, iz;
+      int rs = 0, re = 0;
+      if (cell_of(g, qx, qy, qz, &ix, &iy, &iz)) {
+        const int t = threadIdx.x;
+        const unsigned int b = cell_hash(ix + (t % 3) - 1, iy + ((t / 3) % 3) - 1, iz + (t / 9) - 1, g.mask);
+        bool dup = false;
+        for (int u = 0; u < t; ++u)
+          dup |= cell_hash(ix + (u % 3) - 1, iy + ((u / 3) % 3) - 1, iz + (u / 9) - 1, g.mask) == b;
+        if (!dup) {
+          rs = g.bstart[g.base + b];
+          re = g.bend[g.base + b];
+        }
+      }
+      s_rs[threadIdx.x] = rs;
+      s_re[threadIdx.x] = re;
+    }
+    __syncthreads();
+    if (threadIdx.x == 0) {
+      int acc = 0;
+      for (int t = 0; t < 27; ++t) {
+        s_pref[t] = acc;
+        acc += s_re[t] - s_rs[t];
+      }
+      s_pref[27] = acc;
+    }
+    __syncthreads();
+    total = s_pref[27];
+  }
+  __syncthreads();
+  for (int c0 = 0; c0 < total; c0 += blockDim.x) {
+    const int c = c0 + threadIdx.x;
+    if (c < total) {
+      int i;
+      if (g.n_sorted) {
+        int t = 0;
+        while (c >= s_pref[t + 1]) ++t;
+        i = g.sorted[s_rs[t] + (c - s_pref[t])];
+      } else {
+        i = g.lo + c;
+      }
+      const float dx = qx - pts[3 * (size_t)i], dy = qy - pts[3 * (size_t)i + 1], dz = qz - pts[3 * (size_t)i + 2];
+      float d = dx * dx;
+      d += dy * dy;
+      d += dz * dz;
+      if (d < r2) {
+        const unsigned long long key = ((unsigned long long)__float_as_uint(d) << 32) | (unsigned int)i;
+        if (key < s_thresh) keys[atomicAdd(&s_count, 1)] = key;
+      }
+    }
+    __syncthreads();
+    if (s_count > kGradBuf - kFpfhThreads) {  // uniform: every thread read s_count after the barrier
+      sort_keys(keys, s_count);
+      if (threadIdx.x == 0) {
+        s_count = kGradNn;
+        s_thresh = keys[kGradNn - 1];
+      }
+    }
+    __syncthreads();
+  }
+  const int cnt = s_count;
+  sort_keys(keys, cnt);
+  if (threadIdx.x != 0) return;
+  const int nn = min(cnt, kGradNn);
+  double x[3] = {0.0, 0.0, 0.0};
+  if (nn >= 4) {
+    const float4 nf = normals[p];
+    const double n[3] = {nf.x, nf.y, nf.z};
+    const double vk[3] = {qx, qy, qz};
+    const double ik = (((double)colors[3 * (size_t)p] + (double)colors[3 * (size_t)p + 1]) +
+                       (double)colors[3 * (size_t)p + 2]) / 3.0;
+    double M[6] = {0.0, 0.0, 0.0, 0.0, 0.0, 0.0}, h[3] = {0.0, 0.0, 0.0};
+    for (int e = 1; e < nn; ++e) {
+      const int i = (int)(unsigned int)keys[e];
+      const double v[3] = {pts[3 * (size_t)i], pts[3 * (size_t)i + 1], pts[3 * (size_t)i + 2]};
+      const double s = ((v[0] - vk[0]) * n[0] + (v[1] - vk[1]) * n[1]) + (v[2] - vk[2]) * n[2];
+      const double a[3] = {(v[0] - s * n[0]) - vk[0], (v[1] - s * n[1]) - vk[1], (v[2] - s * n[2]) - vk[2]};
+      const double bi = (((double)colors[3 * (size_t)i] + (double)colors[3 * (size_t)i + 1]) +
+                         (double)colors[3 * (size_t)i + 2]) / 3.0 - ik;
+      int k = 0;
+      for (int r = 0; r < 3; ++r) {
+        for (int c = r; c < 3; ++c) {
+          M[k] = M[k] + a[r] * a[c];
+          ++k;
+        }
+        h[r] = h[r] + a[r] * bi;
+      }
+    }
+    const double w = (double)(nn - 1), cr[3] = {w * n[0], w * n[1], w * n[2]};
+    bool fin = true;
+    int k = 0;
+    for (int r = 0; r < 3; ++r) {
+      for (int c = r; c < 3; ++c) {
+        M[k] = M[k] + cr[r] * cr[c];
+        fin &= isfinite(M[k]) != 0;
+        ++k;
+      }
+      fin &= isfinite(h[r]) != 0;
+    }
+    if (fin) {
+      const double mh[3] = {-h[0], -h[1], -h[2]};  // ldlt_solve solves M x = -g
+      ldlt_solve<3>(M, mh, x);
+    } else {
+      x[0] = x[1] = x[2] = CUDART_NAN;
+    }
+  }
+  grad[3 * (size_t)p] = x[0];
+  grad[3 * (size_t)p + 1] = x[1];
+  grad[3 * (size_t)p + 2] = x[2];
+}
+
 // tzr_fpfh_pair_features / tzr_fpfh_smallest_eigenpair: the production device functions, one item per thread
 __global__ void pair_features_kernel(int n, const float* __restrict__ p1, const float* __restrict__ n1,
                                      const float* __restrict__ p2, const float* __restrict__ n2, float* __restrict__ f,
@@ -702,6 +845,16 @@ int launch_fpfh(const FpfhPlan& plan, const float* pts, FpfhCloud* clouds, doubl
   spfh_kernel<<<N, kFpfhThreads, 0, st>>>(cs, normals, r2f, spfh, overflow);
   fpfh_kernel<<<N, kFpfhThreads, 0, st>>>(cs, spfh, r2f, out, overflow);
   return nl + 3;
+}
+
+int launch_color_gradients(const FpfhPlan& plan, const float* pts, FpfhCloud* clouds, double radius,
+                           const float4* normals, const float* colors, double* grad, void* grid_scratch,
+                           cudaStream_t st) {
+  int nl = 0;
+  Clouds cs{pts, clouds, plan.B, nullptr, nullptr, nullptr};
+  if (plan.any_grid) nl += launch_fpfh_grid(plan, pts, clouds, grid_scratch, st, &cs.sorted, &cs.bstart, &cs.bend);
+  color_gradients_kernel<<<plan.N, kFpfhThreads, 0, st>>>(cs, (float)(radius * radius), normals, colors, grad);
+  return nl + 1;
 }
 
 void launch_fpfh_pair_features(int n, const float* p1, const float* n1, const float* p2, const float* n2, float* f,

@@ -6,7 +6,9 @@
 // Generalized ICP (DESIGN.md §3.14) replaces only the system, with icp_gicp_system_kernel (plane-to-plane covariances
 // from both clouds' normals, the same 27 sums), and shares icp_plane_update_kernel.  Robust kernels (DESIGN.md §3.15)
 // are the <true> instances of both system kernels: weighted sums, the same layout; the <false> instances are the
-// unweighted systems and run for TZR_LOSS_L2.
+// unweighted systems and run for TZR_LOSS_L2.  Coloured ICP (DESIGN.md §3.17) replaces only the system, with
+// icp_colored_system_kernel (a geometric and a photometric row per correspondence, the same 27 sums), after the
+// targets' colour-gradient pass (fpfh.cu's launch_color_gradients).
 //
 //   icp_nn_kernel      one CTA per chunk of kIcpChunk source points: p = s (R x) + t in float64 (icp_transform), the
 //                      nearest target with d^2 < r^2 (lowest index among equal d^2), by brute force through shared
@@ -361,55 +363,6 @@ __global__ void __launch_bounds__(kIcpThreads) icp_plane_system_kernel(IcpArgs a
   icp_block_sum<kIcpPlaneSums>(v, s_buf, a.partial + kIcpPlaneSums * (size_t)c);
 }
 
-// x with A x = -g by the truncated, diagonally pivoted LDL^T of include/teaser_b200.h (one thread).  A: the 21 entries of
-// the upper triangle row by row.  tol = 1e-10 max_k A_kk; step k takes the remaining index with the largest current
-// diagonal (a NaN diagonal is never the largest; the lowest index on ties) and stops unless that diagonal is > tol;
-// every component not reached is 0.
-__device__ void icp_solve6(const double* __restrict__ Aup, const double* __restrict__ g, double x[6]) {
-  double S[6][6];
-  int k = 0;
-  for (int r = 0; r < 6; ++r)
-    for (int c = r; c < 6; ++c) S[r][c] = S[c][r] = Aup[k++];
-  double amax = S[0][0];
-  for (int r = 1; r < 6; ++r) amax = fmax(amax, S[r][r]);
-  const double tol = 1e-10 * amax;
-  int piv[6];
-  bool used[6] = {false, false, false, false, false, false};
-  double d[6], L[6][6];  // L[i][s]: multiplier of original index i at step s
-  int rank = 0;
-  for (int s = 0; s < 6; ++s) {
-    int best = -1;
-    for (int i = 0; i < 6; ++i)
-      if (!used[i] && (best < 0 || S[i][i] > S[best][best] || (S[best][best] != S[best][best] && S[i][i] == S[i][i])))
-        best = i;
-    if (!(S[best][best] > tol)) break;
-    used[best] = true;
-    piv[s] = best;
-    d[s] = S[best][best];
-    rank = s + 1;
-    for (int i = 0; i < 6; ++i)
-      if (!used[i]) L[i][s] = S[i][best] / d[s];
-    for (int i = 0; i < 6; ++i)
-      if (!used[i])
-        for (int c = 0; c < 6; ++c)
-          if (!used[c]) S[i][c] = S[i][c] - L[i][s] * S[best][c];
-  }
-  double y[6];
-  for (int s = 0; s < rank; ++s) {  // L z = -P g, z / d
-    double z = -g[piv[s]];
-    for (int q = 0; q < s; ++q) z = z - L[piv[s]][q] * y[q];
-    y[s] = z;
-  }
-  for (int s = 0; s < rank; ++s) y[s] = y[s] / d[s];
-  for (int s = rank - 1; s >= 0; --s) {  // L^T y = w
-    double z = y[s];
-    for (int q = s + 1; q < rank; ++q) z = z - L[piv[q]][s] * y[q];
-    y[s] = z;
-  }
-  for (int i = 0; i < 6; ++i) x[i] = 0.0;
-  for (int s = 0; s < rank; ++s) x[piv[s]] = y[s];
-}
-
 // ---- generalized ICP (DESIGN.md §3.14) --------------------------------------------------------------------------------
 // C(v) = I - (k v_a) v_b with k = (1 - eps) / ((v0 v0 + v1 v1) + v2 v2): the upper triangle (00, 01, 02, 11, 12, 22).
 // Negating v negates k v_a and v_b, so the entries keep their bits.
@@ -631,6 +584,103 @@ __global__ void __launch_bounds__(kIcpThreads) icp_gicp_system_kernel(IcpArgs a,
   icp_block_sum<kIcpPlaneSums>(v, s_buf, a.partial + kIcpPlaneSums * (size_t)c);
 }
 
+// ---- coloured ICP (DESIGN.md §3.17) ---------------------------------------------------------------------------------
+// The terms of one row (J, r) with weight w (kRobust) into v: (w J_a) J_b (21) and (w J_a) r (6); without kRobust J_a J_b
+// and J_a r, point-to-plane's unweighted products.  add: v += the terms, else v = the terms.
+template <bool kRobust>
+__device__ __forceinline__ void icp_row_terms(const double J[6], double r, double w, bool add,
+                                              double (&v)[kIcpPlaneSums]) {
+  double wJ[6];
+#pragma unroll
+  for (int row = 0; row < 6; ++row) wJ[row] = kRobust ? w * J[row] : J[row];
+  int k = 0;
+#pragma unroll
+  for (int row = 0; row < 6; ++row)
+#pragma unroll
+    for (int col = row; col < 6; ++col) {
+      const double t = wJ[row] * J[col];
+      v[k] = add ? v[k] + t : t;
+      ++k;
+    }
+#pragma unroll
+  for (int row = 0; row < 6; ++row) v[21 + row] = add ? v[21 + row] + wJ[row] * r : wJ[row] * r;
+}
+
+// One CTA per chunk: each correspondence (i, j) whose target normal n has three finite components adds a geometric row
+// J_G = sqrt(lambda) (u x n, n), r_G = sqrt(lambda) r (r: point-to-plane's residual) and then a photometric row
+// J_I = sqrt(1 - lambda) (u x m, m), r_I = sqrt(1 - lambda) (i_s - i_hat) with m = -(I - n n^T) g, g the target's
+// colour gradient and i_hat = g . (p - s n - q) + i_t (include/teaser_b200.h writes out every expression and its
+// order).  A row adds nothing when its factor is 0 or its weight is not finite; the photometric row adds nothing when
+// a colour or g has a non-finite component.  The 27 sums and their layout are the plane system's, so
+// icp_plane_update_kernel solves them unchanged; with lambda = 1 they are icp_plane_system_kernel's bit for bit.
+// kRobust (DESIGN.md §3.15): each row has its own weight, icp_robust_weight(loss, loss_k, r_row).
+template <bool kRobust>
+__global__ void __launch_bounds__(kIcpThreads) icp_colored_system_kernel(IcpArgs a, const float4* __restrict__ normals,
+                                                                         const float* __restrict__ src_colors,
+                                                                         const float* __restrict__ dst_colors,
+                                                                         const double* __restrict__ grad,
+                                                                         double lambda, int loss, double loss_k) {
+  __shared__ double s_buf[(kIcpThreads / 32) * kIcpPlaneSums];
+  const int c = blockIdx.x;
+  const int b = a.chunk_prob[c];
+  const IcpProb& pr = a.probs[b];
+  if (!pr.active || pr.count == 0) return;  // the update of no correspondence reads no system
+  const int i = (c - pr.c_lo) * kIcpChunk + threadIdx.x;
+  double v[kIcpPlaneSums];
+#pragma unroll
+  for (int k = 0; k < kIcpPlaneSums; ++k) v[k] = 0.0;
+  const int j = i < pr.ns ? a.match[pr.m_lo + i] : -1;
+  if (j >= 0) {
+    const float4 nf = normals[pr.n_lo + j];
+    const double n[3] = {nf.x, nf.y, nf.z};
+    if (isfinite(n[0]) && isfinite(n[1]) && isfinite(n[2])) {
+      const double sg = sqrt(lambda), si = sqrt(1.0 - lambda);
+      double p[3];
+      icp_transform(pr, a.src, pr.s_lo + i, p);
+      const size_t o = 3 * (size_t)(pr.d_lo + j);
+      const double q[3] = {a.dst[o], a.dst[o + 1], a.dst[o + 2]};
+      const double u[3] = {p[0] - pr.mup[0], p[1] - pr.mup[1], p[2] - pr.mup[2]};
+      const double r = ((p[0] - q[0]) * n[0] + (p[1] - q[1]) * n[1]) + (p[2] - q[2]) * n[2];
+      bool any = false;
+      if (sg != 0.0) {
+        const double J[6] = {sg * (u[1] * n[2] - u[2] * n[1]), sg * (u[2] * n[0] - u[0] * n[2]),
+                             sg * (u[0] * n[1] - u[1] * n[0]), sg * n[0], sg * n[1], sg * n[2]};
+        const double rg = sg * r;
+        const double w = kRobust ? icp_robust_weight(loss, loss_k, rg) : 1.0;
+        if (isfinite(w)) {
+          icp_row_terms<kRobust>(J, rg, w, false, v);
+          any = true;
+        }
+      }
+      const size_t ks = (size_t)(pr.s_lo + i), kt = (size_t)(pr.d_lo + j), kg = 3 * (size_t)(pr.n_lo + j);
+      const double g[3] = {grad[kg], grad[kg + 1], grad[kg + 2]};
+      const double cs[3] = {src_colors[3 * ks], src_colors[3 * ks + 1], src_colors[3 * ks + 2]};
+      const double ct[3] = {dst_colors[3 * kt], dst_colors[3 * kt + 1], dst_colors[3 * kt + 2]};
+      bool fin = true;
+#pragma unroll
+      for (int k = 0; k < 3; ++k) fin &= isfinite(g[k]) && isfinite(cs[k]) && isfinite(ct[k]);
+      if (si != 0.0 && fin) {
+        const double is = ((cs[0] + cs[1]) + cs[2]) / 3.0, it = ((ct[0] + ct[1]) + ct[2]) / 3.0;
+        const double d[3] = {(p[0] - r * n[0]) - q[0], (p[1] - r * n[1]) - q[1], (p[2] - r * n[2]) - q[2]};
+        const double ihat = ((g[0] * d[0] + g[1] * d[1]) + g[2] * d[2]) + it;
+        double m[3];
+#pragma unroll
+        for (int k = 0; k < 3; ++k) {
+          const double M0 = (k == 0 ? 1.0 : 0.0) - n[0] * n[k], M1 = (k == 1 ? 1.0 : 0.0) - n[1] * n[k],
+                       M2 = (k == 2 ? 1.0 : 0.0) - n[2] * n[k];
+          m[k] = -((g[0] * M0 + g[1] * M1) + g[2] * M2);
+        }
+        const double J[6] = {si * (u[1] * m[2] - u[2] * m[1]), si * (u[2] * m[0] - u[0] * m[2]),
+                             si * (u[0] * m[1] - u[1] * m[0]), si * m[0], si * m[1], si * m[2]};
+        const double ri = si * (is - ihat);
+        const double w = kRobust ? icp_robust_weight(loss, loss_k, ri) : 1.0;
+        if (isfinite(w)) icp_row_terms<kRobust>(J, ri, w, any, v);
+      }
+    }
+  }
+  icp_block_sum<kIcpPlaneSums>(v, s_buf, a.partial + kIcpPlaneSums * (size_t)c);
+}
+
 __global__ void icp_plane_update_kernel(IcpArgs a) {
   IcpProb& pr = a.probs[blockIdx.x];
   if (!pr.active) return;
@@ -643,7 +693,7 @@ __global__ void icp_plane_update_kernel(IcpArgs a) {
   double tu[3] = {0.0, 0.0, 0.0};
   if (pr.count > 0) {
     double x[6];
-    icp_solve6(v, v + 21, x);
+    ldlt_solve<6>(v, v + 21, x);
     bool finite = true;
     for (int k = 0; k < 6; ++k) finite &= isfinite(x[k]) != 0;
     if (finite) {
@@ -797,19 +847,32 @@ IcpLayout icp_layout(const IcpPlan& plan, size_t base, bool information) {
   L.match = L.chunks + al256((size_t)plan.chunks * 4);
   L.partial = L.match + al256((size_t)plan.NS * 4);
   L.grid = L.partial + al256((size_t)plan.chunks * stride * 8);
-  L.info = L.counts = L.end = L.grid + plan.grid.grid_bytes;
+  const bool colored = plan.mode == kIcpColored;
+  const size_t grid_bytes = colored ? std::max(plan.grid.grid_bytes, plan.ggrid.grid_bytes) : plan.grid.grid_bytes;
+  L.info = L.counts = L.end = L.grid + grid_bytes;
   if (information) {
     L.info = al256(L.end);
     L.counts = L.info + al256((size_t)plan.B * 36 * 8);
     L.end = L.counts + (size_t)plan.B * 4;
   }
+  L.gclouds = L.grad = L.end;
+  if (colored) {
+    L.gclouds = al256(L.end);
+    L.grad = L.gclouds + al256((size_t)plan.ggrid.B * sizeof(FpfhCloud));
+    L.end = L.grad + (size_t)plan.ND * 3 * 8;
+  }
   return L;
 }
 
 IcpBuffers icp_buffers(char* d, const IcpLayout& L) {
-  return IcpBuffers{nullptr, nullptr, nullptr, nullptr, (IcpProb*)(d + L.probs), (FpfhCloud*)(d + L.clouds),
-                    (const int*)(d + L.chunks), (int*)(d + L.match), (double*)(d + L.partial), d + L.grid,
-                    (double*)(d + L.info), (int*)(d + L.counts)};
+  IcpBuffers b{nullptr, nullptr, nullptr, nullptr, (IcpProb*)(d + L.probs), (FpfhCloud*)(d + L.clouds),
+               (const int*)(d + L.chunks), (int*)(d + L.match), (double*)(d + L.partial), d + L.grid,
+               (double*)(d + L.info), (int*)(d + L.counts), nullptr, nullptr, nullptr, nullptr};
+  if (L.grad != L.end) {
+    b.gclouds = (FpfhCloud*)(d + L.gclouds);
+    b.grad = (double*)(d + L.grad);
+  }
+  return b;
 }
 
 int launch_icp_information(const IcpPlan& plan, const IcpBuffers& buf, bool reseed, cudaStream_t st,
@@ -843,6 +906,9 @@ int launch_icp(const IcpPlan& plan, const IcpBuffers& buf, cudaStream_t st, IcpG
   int nl = 0;
   IcpArgs a{buf.src, buf.dst, buf.probs, buf.clouds, buf.chunk_prob, buf.match, buf.partial, nullptr, nullptr, nullptr,
             plan.r2};
+  if (plan.mode == kIcpColored)  // the targets' gradients, before ICP's own grid reuses the scratch
+    nl += launch_color_gradients(plan.ggrid, buf.dst, buf.gclouds, plan.grad_r, buf.dst_normals, buf.dst_colors,
+                                 buf.grad, buf.grid_scratch, st);
   if (plan.grid.any_grid)
     nl += launch_fpfh_grid(plan.grid, buf.dst, buf.clouds, buf.grid_scratch, st, &a.sorted, &a.bstart, &a.bend);
   if (grid_out) *grid_out = IcpGrid{a.sorted, a.bstart, a.bend};
@@ -864,6 +930,15 @@ int launch_icp(const IcpPlan& plan, const IcpBuffers& buf, cudaStream_t st, IcpG
       else
         icp_gicp_system_kernel<true><<<plan.chunks, kIcpThreads, 0, st>>>(a, buf.src_normals, buf.dst_normals,
                                                                           plan.epsilon, plan.loss, plan.loss_k);
+      icp_plane_update_kernel<<<plan.B, 32, 0, st>>>(a);
+    } else if (plan.mode == kIcpColored) {
+      if (plan.loss == TZR_LOSS_L2)
+        icp_colored_system_kernel<false><<<plan.chunks, kIcpThreads, 0, st>>>(
+            a, buf.dst_normals, buf.src_colors, buf.dst_colors, buf.grad, plan.lambda_geometric, 0, 0.0);
+      else
+        icp_colored_system_kernel<true><<<plan.chunks, kIcpThreads, 0, st>>>(
+            a, buf.dst_normals, buf.src_colors, buf.dst_colors, buf.grad, plan.lambda_geometric, plan.loss,
+            plan.loss_k);
       icp_plane_update_kernel<<<plan.B, 32, 0, st>>>(a);
     } else {
       icp_cov_kernel<<<plan.chunks, kIcpThreads, 0, st>>>(a);

@@ -220,6 +220,58 @@ static __device__ __noinline__ bool edge_exact_scale(const double* __restrict__ 
   return fabs(__dsub_rn(ratio, s_hat)) <= alpha;
 }
 
+// x with A x = -g by the truncated, diagonally pivoted LDL^T of include/teaser_b200.h (one thread): ICP's 6 x 6 step
+// (icp.cu) and the 3 x 3 colour gradients (fpfh.cu, which pass g = -h to solve A x = h; the negation is exact).  A: the
+// N (N + 1) / 2 entries of the upper triangle row by row.  tol = 1e-10 max_k A_kk; step k takes the remaining index
+// with the largest current diagonal (a NaN diagonal is never the largest; the lowest index on ties) and stops unless
+// that diagonal is > tol; every component not reached is 0.
+template <int N>
+__device__ void ldlt_solve(const double* __restrict__ Aup, const double* __restrict__ g, double x[N]) {
+  double S[N][N];
+  int k = 0;
+  for (int r = 0; r < N; ++r)
+    for (int c = r; c < N; ++c) S[r][c] = S[c][r] = Aup[k++];
+  double amax = S[0][0];
+  for (int r = 1; r < N; ++r) amax = fmax(amax, S[r][r]);
+  const double tol = 1e-10 * amax;
+  int piv[N];
+  bool used[N];
+  for (int i = 0; i < N; ++i) used[i] = false;
+  double d[N], L[N][N];  // L[i][s]: multiplier of original index i at step s
+  int rank = 0;
+  for (int s = 0; s < N; ++s) {
+    int best = -1;
+    for (int i = 0; i < N; ++i)
+      if (!used[i] && (best < 0 || S[i][i] > S[best][best] || (S[best][best] != S[best][best] && S[i][i] == S[i][i])))
+        best = i;
+    if (!(S[best][best] > tol)) break;
+    used[best] = true;
+    piv[s] = best;
+    d[s] = S[best][best];
+    rank = s + 1;
+    for (int i = 0; i < N; ++i)
+      if (!used[i]) L[i][s] = S[i][best] / d[s];
+    for (int i = 0; i < N; ++i)
+      if (!used[i])
+        for (int c = 0; c < N; ++c)
+          if (!used[c]) S[i][c] = S[i][c] - L[i][s] * S[best][c];
+  }
+  double y[N];
+  for (int s = 0; s < rank; ++s) {  // L z = -P g, z / d
+    double z = -g[piv[s]];
+    for (int q = 0; q < s; ++q) z = z - L[piv[s]][q] * y[q];
+    y[s] = z;
+  }
+  for (int s = 0; s < rank; ++s) y[s] = y[s] / d[s];
+  for (int s = rank - 1; s >= 0; --s) {  // L^T y = w
+    double z = y[s];
+    for (int q = s + 1; q < rank; ++q) z = z - L[piv[q]][s] * y[q];
+    y[s] = z;
+  }
+  for (int i = 0; i < N; ++i) x[i] = 0.0;
+  for (int s = 0; s < rank; ++s) x[piv[s]] = y[s];
+}
+
 // kernels (defined in the .cu files) -------------------------------------------------------------
 void launch_prep(const Batch& bt, cudaStream_t st);
 // returns the number of kernels launched; strip_blocks (may be NULL): graph_strip2_kernel's strip length, 0 if it did not run
@@ -352,6 +404,13 @@ int launch_fpfh(const FpfhPlan& plan, const float* pts, FpfhCloud* clouds, doubl
 void launch_fpfh_pair_features(int n, const float* p1, const float* n1, const float* p2, const float* n2, float* f,
                                int32_t* ok, cudaStream_t st);
 void launch_fpfh_smallest_eigenpair(int n, const float* cov, float* ev, float* vec, cudaStream_t st);
+// Colour gradients (tzr_estimate_color_gradients, DESIGN.md §3.17) of every point of plan's clouds: pts (N x 3 floats),
+// clouds (device copy of fpfh_plan's table for this radius), normals (N float4), colors (N x 3 floats), grad (N x 3
+// doubles), grid_scratch (plan.grid_bytes): device pointers.  The 30 nearest neighbours by (d^2, index) of a bounded
+// selection, so no neighbourhood is too large.  Returns the launches: 1, + 4 for the grid build when some cloud uses it.
+int launch_color_gradients(const FpfhPlan& plan, const float* pts, FpfhCloud* clouds, double radius,
+                           const float4* normals, const float* colors, double* grad, void* grid_scratch,
+                           cudaStream_t st);
 
 // certify.cu (DRSCertifier::certify, certification.cc:40-190)
 // Device input of one certify_batch_device problem (tzr_certify_last_solve): its measurements are built on the device
@@ -442,11 +501,12 @@ int launch_pair_rows(const MatchPlan& plan, const MatchPair* pairs, const int2* 
 int launch_corr_gather(const PairGather* table, int n_entries, int max_count, const int32_t* pairs, const float* pts,
                        int2* corr, double* src, double* dst, cudaStream_t st);
 
-// icp.cu (point-to-point ICP, DESIGN.md §3.11, point-to-plane ICP, §3.13, and generalized ICP, §3.14): B problems
+// icp.cu (point-to-point ICP, DESIGN.md §3.11, point-to-plane ICP, §3.13, generalized ICP, §3.14, and coloured ICP,
+// §3.17): B problems
 // over flat source and target point arrays
 constexpr int kIcpChunk = 256;    // source points per chunk: the unit of the fixed-order reductions (one CTA each)
 constexpr int kIcpGridMinN = 1024;  // targets from which the nearest-neighbour search goes through the hashed grid
-constexpr int kIcpPointToPoint = 0, kIcpPointToPlane = 1, kIcpGeneralized = 2;  // IcpPlan::mode
+constexpr int kIcpPointToPoint = 0, kIcpPointToPlane = 1, kIcpGeneralized = 2, kIcpColored = 3;  // IcpPlan::mode
 // doubles per chunk of the point-to-plane and generalized systems: 21 of the upper triangle of A, 6 of g
 constexpr int kIcpPlaneSums = 27;
 // doubles per chunk of launch_icp's partial buffer (the point-to-point pass sums 9)
@@ -479,6 +539,11 @@ struct IcpPlan {
   int loss = 0;
   double loss_k = 0;
   FpfhPlan grid;        // the target grid (fpfh_plan with both radii = r)
+  // coloured (DESIGN.md §3.17): lambda_geometric in [0, 1], and the targets' colour-gradient pass at radius grad_r =
+  // 2 r with its own plan (fpfh_plan over the same targets, the descriptor stage's route); unused in the other modes
+  double lambda_geometric = 0;
+  double grad_r = 0;
+  FpfhPlan ggrid;
 };
 constexpr int kIcpInfoSums = 21;  // doubles per chunk of launch_icp_information's partial buffer
 // The tables of B problems against T target clouds of nt[0..T) points, back to back in the flat target array: problem
@@ -493,9 +558,12 @@ int icp_plan(int B, const int32_t* ns, const int32_t* s_lo, const int32_t* tc, i
              std::vector<IcpProb>* probs, std::vector<int>* chunk_prob);
 // Byte offsets of an ICP workspace from `base` on: [problems | target clouds | chunks | matches | partials | grid
 // scratch | information | counts]; the last two are empty without `information`, whose partials have room for both
-// launch_icp's sums and kIcpInfoSums.  end: the workspace's size.
+// launch_icp's sums and kIcpInfoSums.  In kIcpColored mode two more regions follow: the gradient pass's cloud table
+// (plan.ggrid.B entries) and the targets' gradients (ND x 3 doubles), and the grid scratch has room for either grid
+// (the gradient pass finishes before ICP builds its own).  end: the workspace's size.
 struct IcpLayout {
   size_t probs, clouds, chunks, match, partial, grid, info, counts, end;
+  size_t gclouds, grad;  // kIcpColored only (equal to end otherwise)
 };
 IcpLayout icp_layout(const IcpPlan& plan, size_t base, bool information);
 // The device buffers of launch_icp and launch_icp_information.  src (NS x 3 floats), dst (ND x 3 floats), src_normals
@@ -517,11 +585,18 @@ struct IcpBuffers {
   void* grid_scratch;
   double* info;
   int* counts;
+  // kIcpColored: the source and target colours (NS x 3 and ND x 3 floats, set by the caller), the gradient pass's cloud
+  // table and the targets' gradients (ND x 3 doubles, written by launch_icp); nullptr in the other modes
+  const float* src_colors;
+  const float* dst_colors;
+  FpfhCloud* gclouds;
+  double* grad;
 };
-// the table and scratch buffers of a workspace at d laid out by L; the points and normals are left nullptr
+// the table and scratch buffers of a workspace at d laid out by L; the points, normals and colours are left nullptr
 IcpBuffers icp_buffers(char* d, const IcpLayout& L);
 // Enqueues every iteration without synchronising; returns the launches: 4 for the grid build (when some target uses
-// it) + 2 + 4 * max_iteration, in every mode.  info and counts are not used.
+// it) + 2 + 4 * max_iteration, in every mode; kIcpColored adds the gradient pass first (launch_color_gradients: 1, + 4
+// when some target uses its grid).  info and counts are not used.
 // grid_out (may be nullptr): the target grid's sorted indices and bucket ranges inside grid_scratch (all nullptr without
 // grid targets), for launch_icp_information to reuse.
 struct IcpGrid {
@@ -629,9 +704,10 @@ struct VoxPlan {
 int voxel_plan(int B, const int32_t* n, VoxCloud* clouds, VoxPlan* plan);
 // pts (N x 3 floats), clouds (device copy of voxel_plan's table), scratch (plan.scratch_bytes), out (N x 3 floats: the
 // voxels of the batch in cloud order, cloud b's from row out_lo), voxel_of (N ints: the cloud-local output row of every
-// point, -1 for a point in no voxel): device pointers.  Returns the launches (10).
+// point, -1 for a point in no voxel): device pointers.  colors (may be nullptr; N x 3 floats) and colors_out (as out):
+// each voxel's colour mean, summed like its point.  Returns the launches (10).
 int launch_voxel(const VoxPlan& plan, double voxel_size, const float* pts, VoxCloud* clouds, void* scratch, float* out,
-                 int* voxel_of, cudaStream_t st);
+                 int* voxel_of, cudaStream_t st, const float* colors = nullptr, float* colors_out = nullptr);
 
 
 }  // namespace tzr

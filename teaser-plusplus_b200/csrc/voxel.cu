@@ -1,5 +1,5 @@
 // Voxel-grid downsampling (the first step of the reference's FPFH + TEASER++ + ICP tutorial, DESIGN.md §3.12):
-// Open3D's PointCloud::VoxelDownSample, points only, with the output order and the non-finite rule that
+// Open3D's PointCloud::VoxelDownSample, points and optionally colours, with the output order and the non-finite rule that
 // include/teaser_b200.h defines, for B clouds stored back to back.
 //
 //   vox_bounds_kernel  per point: component-wise min / max of each cloud's finite points (ordered-int float atomics)
@@ -11,6 +11,7 @@
 //   vox_head_kernel    per sorted point: marks the first member of every voxel (by input index) and the group bounds
 //   CUB exclusive sum  of those marks in input order: each voxel's output row, ordered by its first member
 //   vox_mean_kernel    per voxel: the sequential float64 sum of its members in ascending index, the mean, voxel_of
+//                      (<true>: also the members' colours, tzr_voxel_downsample_colors)
 //   vox_count_kernel   per cloud: its first output row and its number of voxels
 //
 // Ten launches whatever B.  Every per-cloud quantity depends on the cloud's own points only, so a cloud's outputs do not
@@ -143,12 +144,17 @@ __global__ void vox_head_kernel(const int* __restrict__ idx, const unsigned int*
 
 // One thread per voxel: its members are the sorted positions [r, e) up to the next mark, ascending by input index; the
 // sum starts at 0.0 and adds them one at a time (Open3D's AccumulatedPoint), the mean is rounded once to float.
+// kColors (tzr_voxel_downsample_colors, DESIGN.md §3.17): the members' colours are averaged the same way into
+// colors_out; the instance without it ignores both pointers.
+template <bool kColors>
 __global__ void __launch_bounds__(kVoxThreads) vox_mean_kernel(const float* __restrict__ pts, const int* __restrict__ idx,
                                                                const unsigned int* __restrict__ cloud,
                                                                const unsigned char* __restrict__ mark,
                                                                const int* __restrict__ row, int N,
                                                                const VoxCloud* __restrict__ cl,
-                                                               float* __restrict__ out, int* __restrict__ voxel_of) {
+                                                               float* __restrict__ out, int* __restrict__ voxel_of,
+                                                               const float* __restrict__ colors,
+                                                               float* __restrict__ colors_out) {
   const int r = blockIdx.x * blockDim.x + threadIdx.x;
   if (r >= N) return;
   const int f = mark[r];
@@ -175,6 +181,18 @@ __global__ void __launch_bounds__(kVoxThreads) vox_mean_kernel(const float* __re
   out[3 * (size_t)g] = __double2float_rn(__ddiv_rn(s0, cnt));
   out[3 * (size_t)g + 1] = __double2float_rn(__ddiv_rn(s1, cnt));
   out[3 * (size_t)g + 2] = __double2float_rn(__ddiv_rn(s2, cnt));
+  if constexpr (kColors) {
+    double c0 = 0.0, c1 = 0.0, c2 = 0.0;
+    for (int q = r; q < e; ++q) {
+      const size_t j = (size_t)idx[q];
+      c0 = __dadd_rn(c0, (double)colors[3 * j]);
+      c1 = __dadd_rn(c1, (double)colors[3 * j + 1]);
+      c2 = __dadd_rn(c2, (double)colors[3 * j + 2]);
+    }
+    colors_out[3 * (size_t)g] = __double2float_rn(__ddiv_rn(c0, cnt));
+    colors_out[3 * (size_t)g + 1] = __double2float_rn(__ddiv_rn(c1, cnt));
+    colors_out[3 * (size_t)g + 2] = __double2float_rn(__ddiv_rn(c2, cnt));
+  }
 }
 
 __global__ void vox_count_kernel(const int* __restrict__ head, const int* __restrict__ row, VoxCloud* cl, int B) {
@@ -258,7 +276,7 @@ int voxel_plan(int B, const int32_t* n, VoxCloud* clouds, VoxPlan* plan) {
 }
 
 int launch_voxel(const VoxPlan& plan, double voxel_size, const float* pts, VoxCloud* clouds, void* scratch, float* out,
-                 int* voxel_of, cudaStream_t st) {
+                 int* voxel_of, cudaStream_t st, const float* colors, float* colors_out) {
   const int N = plan.N, B = plan.B;
   VoxScratch s;
   vox_carve(N, B, (char*)scratch, &s);
@@ -275,7 +293,12 @@ int launch_voxel(const VoxPlan& plan, double voxel_size, const float* pts, VoxCl
   vox_head_kernel<<<gp, kVoxThreads, 0, st>>>(s.idx2, s.cloud2, s.key, N, s.mark, s.head);
   t = s.cub_bytes;
   cub::DeviceScan::ExclusiveSum(s.cub, t, s.head, s.row, N, st);
-  vox_mean_kernel<<<gp, kVoxThreads, 0, st>>>(pts, s.idx2, s.cloud2, s.mark, s.row, N, clouds, out, voxel_of);
+  if (colors)
+    vox_mean_kernel<true><<<gp, kVoxThreads, 0, st>>>(pts, s.idx2, s.cloud2, s.mark, s.row, N, clouds, out, voxel_of,
+                                                        colors, colors_out);
+  else
+    vox_mean_kernel<false><<<gp, kVoxThreads, 0, st>>>(pts, s.idx2, s.cloud2, s.mark, s.row, N, clouds, out, voxel_of,
+                                                         nullptr, nullptr);
   vox_count_kernel<<<gc, 128, 0, st>>>(s.head, s.row, clouds, B);
   return 10;
 }

@@ -12,6 +12,13 @@ struct PointXYZ {
   friend bool operator!=(const PointXYZ& a, const PointXYZ& b) { return !(a == b); }
 };
 
+// One point's colour (r, g, b as floats, any range; Open3D uses [0, 1]): coloured ICP and voxel downsampling with
+// colours (teaser/icp.h, teaser/voxel.h).
+struct ColorRGB {
+  float r, g, b;
+};
+using ColorCloud = std::vector<ColorRGB>;
+
 class PointCloud {
  public:
   using value_type = PointXYZ;

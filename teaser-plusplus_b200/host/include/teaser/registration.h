@@ -60,6 +60,11 @@ struct PointToPointICPParams {
 struct GeneralizedICPParams : PointToPointICPParams {
   double epsilon = 1e-3;
 };
+// Coloured ICP (teaser/icp.h, tzr_icp_colored): PointToPointICP's parameters plus Open3D's lambda_geometric (outside
+// [0, 1] it becomes 0.968; a non-finite value is refused).
+struct ColoredICPParams : PointToPointICPParams {
+  double lambda_geometric = 0.968;
+};
 // A robust kernel for point-to-plane and generalized ICP (tzr_robust_kernel, DESIGN.md §3.15): Open3D's L2Loss (the
 // default, no weighting), L1Loss, HuberLoss(k), CauchyLoss(k), GMLoss(k) and TukeyLoss(k).  k must be finite and > 0 for
 // Huber, Cauchy, GM and Tukey; it is ignored for L2 and L1.

@@ -20,4 +20,13 @@ PointCloud voxelDownSample(const PointCloud& cloud, double voxel_size, std::vect
 std::vector<PointCloud> voxelDownSampleBatch(const std::vector<PointCloud>& clouds, double voxel_size,
                                              std::vector<std::vector<int>>* voxel_of = nullptr);
 
+// With colours (tzr_voxel_downsample_colors(_batch)): the same points, and in colors_out each voxel's colour mean, summed
+// in ascending input index like its point.  colors: one per point.
+PointCloud voxelDownSample(const PointCloud& cloud, const ColorCloud& colors, double voxel_size, ColorCloud* colors_out,
+                           std::vector<int>* voxel_of = nullptr);
+std::vector<PointCloud> voxelDownSampleBatch(const std::vector<PointCloud>& clouds,
+                                             const std::vector<ColorCloud>& colors, double voxel_size,
+                                             std::vector<ColorCloud>* colors_out,
+                                             std::vector<std::vector<int>>* voxel_of = nullptr);
+
 }  // namespace teaser

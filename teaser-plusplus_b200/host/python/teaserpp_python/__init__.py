@@ -11,10 +11,10 @@ import functools
 from . import _teaserpp as _ext
 
 # ---- re-exports -----------------------------------------------------------------------------------------------------
-_PUBLIC = ("OMP_MAX_THREADS", "CertificationResult", "DRSCertifier", "EigSolverType", "GeneralizedICP",
+_PUBLIC = ("OMP_MAX_THREADS", "CertificationResult", "ColoredICP", "DRSCertifier", "EigSolverType", "GeneralizedICP",
            "InlierGraphFormulation", "InlierSelectionMode", "PointToPlaneICP", "PointToPointICP", "PoseGraph",
            "RegistrationSolution", "RobustKernel", "RobustRegistrationSolver", "RotationEstimationAlgorithm",
-           "estimate_normals",
+           "estimate_color_gradients", "estimate_color_gradients_batch", "estimate_normals",
            "estimate_normals_batch", "information_matrix", "information_matrix_batch", "voxel_down_sample",
            "voxel_down_sample_batch")
 globals().update({name: getattr(_ext, name) for name in _PUBLIC})

@@ -8,6 +8,8 @@
 #include <pybind11/pybind11.h>
 #include <pybind11/stl.h>
 
+#include <array>
+#include <cstring>
 #include <sstream>
 
 #include "teaser/certification.h"
@@ -91,6 +93,25 @@ teaser::NormalCloud normals_of(const CloudArray& a) {
 py::array_t<float> normals_to_numpy(const teaser::NormalCloud& nc) {
   py::array_t<float> out({static_cast<py::ssize_t>(nc.size()), static_cast<py::ssize_t>(4)});
   if (!nc.empty()) std::memcpy(out.mutable_data(), &nc[0].normal_x, sizeof(float) * 4 * nc.size());
+  return out;
+}
+
+teaser::ColorCloud colors_of(const CloudArray& a) {
+  if (a.ndim() != 2 || a.shape(1) != 3) throw std::invalid_argument("colours must be (n,3) arrays");
+  teaser::ColorCloud cc(static_cast<size_t>(a.shape(0)));
+  if (!cc.empty()) std::memcpy(&cc[0].r, a.data(), sizeof(float) * 3 * cc.size());
+  return cc;
+}
+
+py::array_t<float> colors_to_numpy(const teaser::ColorCloud& cc) {
+  py::array_t<float> out({static_cast<py::ssize_t>(cc.size()), static_cast<py::ssize_t>(3)});
+  if (!cc.empty()) std::memcpy(out.mutable_data(), &cc[0].r, sizeof(float) * 3 * cc.size());
+  return out;
+}
+
+py::array_t<double> gradients_to_numpy(const std::vector<std::array<double, 3>>& g) {
+  py::array_t<double> out({static_cast<py::ssize_t>(g.size()), static_cast<py::ssize_t>(3)});
+  if (!g.empty()) std::memcpy(out.mutable_data(), g[0].data(), sizeof(double) * 3 * g.size());
   return out;
 }
 
@@ -389,6 +410,95 @@ PYBIND11_MODULE(_teaserpp, m) {
            },
            py::arg("src"), py::arg("dst"), py::arg("src_normals"), py::arg("dst_normals"), py::arg("init"));
 
+  // GPU extra: coloured ICP (teaser::ColoredICP), given the target normals and both clouds' (n,3) colours
+  py::class_<teaser::ColoredICP>(m, "ColoredICP")
+      .def(py::init([](double max_correspondence_distance, int max_iteration, double relative_fitness,
+                       double relative_rmse, double lambda_geometric, const teaser::RobustKernel& kernel) {
+             teaser::ColoredICP::Params p;
+             p.max_correspondence_distance = max_correspondence_distance;
+             p.max_iteration = max_iteration;
+             p.relative_fitness = relative_fitness;
+             p.relative_rmse = relative_rmse;
+             p.lambda_geometric = lambda_geometric;
+             return teaser::ColoredICP(p, kernel);
+           }),
+           py::arg("max_correspondence_distance"), py::arg("max_iteration") = 30, py::arg("relative_fitness") = 1e-6,
+           py::arg("relative_rmse") = 1e-6, py::arg("lambda_geometric") = 0.968,
+           py::arg("kernel") = teaser::RobustKernel())
+      .def_property("kernel", &teaser::ColoredICP::getKernel, &teaser::ColoredICP::setKernel)
+      .def("refine",
+           [](const teaser::ColoredICP& icp, const CloudArray& src, const CloudArray& dst, const CloudArray& dst_normals,
+              const CloudArray& src_colors, const CloudArray& dst_colors, const teaser::RegistrationSolution& init) {
+             const teaser::PointCloud s = cloud_of(src), d = cloud_of(dst);
+             const teaser::NormalCloud n = normals_of(dst_normals);
+             const teaser::ColorCloud sc = colors_of(src_colors), dc = colors_of(dst_colors);
+             teaser::ColoredICP::Result r;
+             {
+               py::gil_scoped_release release;
+               r = icp.refine(s, d, n, sc, dc, init);
+             }
+             return icp_dict(r);
+           },
+           py::arg("src"), py::arg("dst"), py::arg("dst_normals"), py::arg("src_colors"), py::arg("dst_colors"),
+           py::arg("init"))
+      .def("refine_batch",
+           [](const teaser::ColoredICP& icp, const std::vector<CloudArray>& src, const std::vector<CloudArray>& dst,
+              const std::vector<CloudArray>& dst_normals, const std::vector<CloudArray>& src_colors,
+              const std::vector<CloudArray>& dst_colors, const std::vector<teaser::RegistrationSolution>& init) {
+             std::vector<teaser::PointCloud> s, d;
+             std::vector<teaser::NormalCloud> n;
+             std::vector<teaser::ColorCloud> sc, dc;
+             for (const auto& a : src) s.push_back(cloud_of(a));
+             for (const auto& a : dst) d.push_back(cloud_of(a));
+             for (const auto& a : dst_normals) n.push_back(normals_of(a));
+             for (const auto& a : src_colors) sc.push_back(colors_of(a));
+             for (const auto& a : dst_colors) dc.push_back(colors_of(a));
+             std::vector<teaser::ColoredICP::Result> res;
+             {
+               py::gil_scoped_release release;
+               res = icp.refineBatch(s, d, n, sc, dc, init);
+             }
+             py::list out;
+             for (const auto& r : res) out.append(icp_dict(r));
+             return out;
+           },
+           py::arg("src"), py::arg("dst"), py::arg("dst_normals"), py::arg("src_colors"), py::arg("dst_colors"),
+           py::arg("init"));
+
+  // GPU extra: coloured ICP's colour gradients (teaser::estimateColorGradients), as (n,3) float64
+  m.def("estimate_color_gradients",
+        [](const CloudArray& points, const CloudArray& normals, const CloudArray& colors, double radius) {
+          const teaser::PointCloud pc = cloud_of(points);
+          const teaser::NormalCloud nc = normals_of(normals);
+          const teaser::ColorCloud cc = colors_of(colors);
+          std::vector<std::array<double, 3>> g;
+          {
+            py::gil_scoped_release release;
+            g = teaser::estimateColorGradients(pc, nc, cc, radius);
+          }
+          return gradients_to_numpy(g);
+        },
+        py::arg("points"), py::arg("normals"), py::arg("colors"), py::arg("radius"));
+  m.def("estimate_color_gradients_batch",
+        [](const std::vector<CloudArray>& points, const std::vector<CloudArray>& normals,
+           const std::vector<CloudArray>& colors, double radius) {
+          std::vector<teaser::PointCloud> pcs;
+          std::vector<teaser::NormalCloud> ncs;
+          std::vector<teaser::ColorCloud> ccs;
+          for (const auto& a : points) pcs.push_back(cloud_of(a));
+          for (const auto& a : normals) ncs.push_back(normals_of(a));
+          for (const auto& a : colors) ccs.push_back(colors_of(a));
+          std::vector<std::vector<std::array<double, 3>>> res;
+          {
+            py::gil_scoped_release release;
+            res = teaser::estimateColorGradientsBatch(pcs, ncs, ccs, radius);
+          }
+          py::list out;
+          for (const auto& g : res) out.append(gradients_to_numpy(g));
+          return out;
+        },
+        py::arg("points"), py::arg("normals"), py::arg("colors"), py::arg("radius"));
+
   // GPU extra: FPFHEstimation's normals alone (teaser::estimateNormals), as (n,4) float32 (nx, ny, nz, curvature)
   m.def("estimate_normals",
         [](const CloudArray& points, double normal_search_radius) {
@@ -416,32 +526,52 @@ PYBIND11_MODULE(_teaserpp, m) {
         },
         py::arg("points"), py::arg("normal_search_radius") = 0.03);
 
-  // GPU extra: the first step of the same tutorial, Open3D's voxel_down_sample (teaser::voxelDownSample)
+  // GPU extra: the first step of the same tutorial, Open3D's voxel_down_sample (teaser::voxelDownSample); with colors
+  // ((n,3)) it returns (points, colour means)
   m.def("voxel_down_sample",
-        [](const CloudArray& points, double voxel_size) {
+        [](const CloudArray& points, double voxel_size, const py::object& colors) -> py::object {
           const teaser::PointCloud pc = cloud_of(points);
+          if (colors.is_none()) {
+            teaser::PointCloud out;
+            {
+              py::gil_scoped_release release;
+              out = teaser::voxelDownSample(pc, voxel_size);
+            }
+            return cloud_to_numpy(out);
+          }
+          const teaser::ColorCloud cc = colors_of(colors.cast<CloudArray>());
           teaser::PointCloud out;
+          teaser::ColorCloud cout;
           {
             py::gil_scoped_release release;
-            out = teaser::voxelDownSample(pc, voxel_size);
+            out = teaser::voxelDownSample(pc, cc, voxel_size, &cout);
           }
-          return cloud_to_numpy(out);
+          return py::make_tuple(cloud_to_numpy(out), colors_to_numpy(cout));
         },
-        py::arg("points"), py::arg("voxel_size"));
+        py::arg("points"), py::arg("voxel_size"), py::arg("colors") = py::none());
   m.def("voxel_down_sample_batch",
-        [](const std::vector<CloudArray>& points, double voxel_size) {
+        [](const std::vector<CloudArray>& points, double voxel_size, const py::object& colors) -> py::object {
           std::vector<teaser::PointCloud> pcs;
           for (const auto& a : points) pcs.push_back(cloud_of(a));
           std::vector<teaser::PointCloud> res;
-          {
+          std::vector<teaser::ColorCloud> cres;
+          if (colors.is_none()) {
             py::gil_scoped_release release;
             res = teaser::voxelDownSampleBatch(pcs, voxel_size);
+          } else {
+            std::vector<teaser::ColorCloud> ccs;
+            for (const auto& a : colors.cast<std::vector<CloudArray>>()) ccs.push_back(colors_of(a));
+            py::gil_scoped_release release;
+            res = teaser::voxelDownSampleBatch(pcs, ccs, voxel_size, &cres);
           }
           py::list out;
           for (const auto& pc : res) out.append(cloud_to_numpy(pc));
-          return out;
+          if (colors.is_none()) return out;
+          py::list cout;
+          for (const auto& cc : cres) cout.append(colors_to_numpy(cc));
+          return py::make_tuple(out, cout);
         },
-        py::arg("points"), py::arg("voxel_size"));
+        py::arg("points"), py::arg("voxel_size"), py::arg("colors") = py::none());
 
   m.attr("OMP_MAX_THREADS") = 0;  // the GPU path ignores max_clique_num_threads
 

@@ -168,4 +168,63 @@ std::vector<GeneralizedICP::Result> GeneralizedICP::refineBatch(const std::vecto
                       &kernel_);
 }
 
+ColoredICP::Result ColoredICP::refine(const PointCloud& src, const PointCloud& dst, const NormalCloud& dst_normals,
+                                      const ColorCloud& src_colors, const ColorCloud& dst_colors,
+                                      const RegistrationSolution& init) const {
+  return refineBatch({src}, {dst}, {dst_normals}, {src_colors}, {dst_colors}, {init})[0];
+}
+
+std::vector<ColoredICP::Result> ColoredICP::refineBatch(const std::vector<PointCloud>& src,
+                                                        const std::vector<PointCloud>& dst,
+                                                        const std::vector<NormalCloud>& dst_normals,
+                                                        const std::vector<ColorCloud>& src_colors,
+                                                        const std::vector<ColorCloud>& dst_colors,
+                                                        const std::vector<RegistrationSolution>& init) const {
+  const size_t B = src.size();
+  if (dst.size() != B || init.size() != B || dst_normals.size() != B || src_colors.size() != B ||
+      dst_colors.size() != B)
+    throw std::invalid_argument("ColoredICP: one target, normal cloud, colour clouds and seed per source");
+  std::vector<Result> out(B);
+  if (B == 0) return out;
+  static_assert(sizeof(ColorRGB) == 3 * sizeof(float), "ColorRGB must be three packed floats");
+  std::vector<int32_t> ns(B), nd(B);
+  std::vector<const float*> sp(B), dp(B), np(B), scp(B), dcp(B);
+  std::vector<tzr_similarity> seeds(B);
+  std::vector<std::vector<int32_t>> corr(B);
+  std::vector<int32_t*> corr_p(B);
+  for (size_t b = 0; b < B; ++b) {
+    if (src[b].empty() || dst[b].empty()) throw std::invalid_argument("ColoredICP: clouds must be non-empty");
+    if (dst_normals[b].size() != dst[b].size() || dst_colors[b].size() != dst[b].size() ||
+        src_colors[b].size() != src[b].size())
+      throw std::invalid_argument("ColoredICP: one normal per target point and one colour per point");
+    ns[b] = static_cast<int32_t>(src[b].size());
+    nd[b] = static_cast<int32_t>(dst[b].size());
+    sp[b] = &src[b][0].x;
+    dp[b] = &dst[b][0].x;
+    np[b] = &dst_normals[b][0].normal_x;
+    scp[b] = &src_colors[b][0].r;
+    dcp[b] = &dst_colors[b][0].r;
+    seeds[b] = to_c(init[b]);
+    corr[b].resize(2 * src[b].size());
+    corr_p[b] = corr[b].data();
+  }
+  const tzr_icp_params p = to_c(params_);
+  tzr_robust_kernel k;
+  std::memset(&k, 0, sizeof(k));
+  k.type = static_cast<int32_t>(kernel_.type);
+  k.k = kernel_.k;
+  const tzr_robust_kernel* kp = kernel_.type == RobustKernel::kL2 ? nullptr : &k;
+  std::vector<tzr_icp_result> res(B);
+  tzr_ctx* ctx = b200_context();
+  const int rc = B == 1 ? tzr_icp_colored(ctx, &p, sp[0], ns[0], dp[0], nd[0], np[0], seeds.data(), res.data(),
+                                          corr_p[0], scp[0], dcp[0], params_.lambda_geometric, kp)
+                        : tzr_icp_colored_batch(ctx, &p, static_cast<int>(B), ns.data(), sp.data(), nd.data(),
+                                                dp.data(), np.data(), seeds.data(), res.data(), corr_p.data(),
+                                                scp.data(), dcp.data(), params_.lambda_geometric, kp);
+  if (rc != TZR_OK)
+    throw std::runtime_error(std::string("ColoredICP: ") + tzr_status_string(rc) + " (" + tzr_last_error(ctx) + ")");
+  for (size_t b = 0; b < B; ++b) icp_result_from_c(res[b], corr[b].data(), &out[b]);
+  return out;
+}
+
 }  // namespace teaser
