@@ -850,6 +850,37 @@ int tzr_icp_colored(tzr_ctx* ctx, const tzr_icp_params* params, const float* src
                     const float* src_colors, const float* dst_colors, double lambda_geometric,
                     const tzr_robust_kernel* kernel);
 
+/* tzr_register_cloud_pairs_icp with coloured ICP: the same arguments plus colors, lambda_geometric and kernel, and the
+ * same outputs, except that each refined record is coloured ICP (DESIGN.md §3.18).
+ *   - Arguments, all checked before any device work: colors (n_clouds entries, entry c n[c] x 3 floats aligned with
+ *     pts[c]; a NULL array or entry is TZR_ERR_INVALID_ARG); lambda_geometric (non-finite: TZR_ERR_INVALID_ARG; outside
+ *     [0, 1]: 0.968, as tzr_icp_colored_batch); kernel (NULL: L2; otherwise checked as tzr_icp_colored_batch checks it).
+ *   - Solve outputs: solutions, status, problem_index, correspondences, cliques, global scales and the retained solve are
+ *     tzr_register_cloud_pairs' bit for bit.
+ *   - Refinement: each pair p whose solve succeeded with a valid, finite record gets coloured ICP of cloud
+ *     pair_clouds[2p] onto cloud pair_clouds[2p + 1], seeded on the device from its record, its scale held fixed.  The
+ *     target normals are the call's own FPFH stage's (normal_search_radius, viewpoint at the origin); the target
+ *     gradients are taken at 2 max_correspondence_distance, as RegistrationColoredICP takes them.  Each refined record
+ *     is bit-identical to tzr_icp_colored_batch on that pair, with the two clouds and their colours,
+ *     tzr_estimate_normals_batch(fparams->normal_search_radius) of the target, the pair's solution as init, the same
+ *     lambda_geometric and the same kernel.  A pair that is not refined gets a zeroed record.
+ *   - Gradients: one batched pass over every cloud of the call (tzr_estimate_color_gradients_batch at that radius, the
+ *     descriptor stage's route), so each cloud's gradients are computed once however many pairs name it as target.
+ *   - With lambda_geometric = 1 every output equals tzr_register_cloud_pairs_icp_point_to_plane (no kernel) and
+ *     tzr_register_cloud_pairs_icp_robust with method 1 and the same kernel, bit for bit.
+ * Launches: tzr_register_cloud_pairs_icp_point_to_plane's, plus, when some pair was solved, the gradient pass (1, + 4
+ * when some cloud of the call has 4096 points or more, or under debug flag 8388608), whatever P.  Like
+ * tzr_register_cloud_pairs this is a solve entry: tzr_last_inliers, tzr_last_graph and tzr_certify_last_solve see its
+ * solve, which the refinement does not touch. */
+int tzr_register_cloud_pairs_icp_colored(tzr_ctx* ctx, const tzr_frontend_params* fparams, const tzr_params* params,
+                                         int n_clouds, const int32_t* n, const float* const* pts, int P,
+                                         const int32_t* pair_clouds, const uint64_t* tuple_seeds,
+                                         tzr_solution* solutions, int32_t* status, int32_t* problem_index,
+                                         int64_t* n_corr, int32_t* const* corr, int32_t* const* cliques,
+                                         float* global_scale, const tzr_icp_params* icp, const float* const* colors,
+                                         double lambda_geometric, const tzr_robust_kernel* kernel,
+                                         tzr_icp_result* icp_results);
+
 /* ---- multiway registration: information matrices ------------------------------------------------------------
  * Open3D's GetInformationMatrixFromPointClouds(source, target, max_correspondence_distance, T) for many pairs at once,
  * defined here as follows (DESIGN.md §3.16):
@@ -968,6 +999,23 @@ int tzr_register_cloud_pairs_multiway(tzr_ctx* ctx, const tzr_frontend_params* f
                                       const int32_t* uncertain, const tzr_pose_graph_params* pg, double* information,
                                       int32_t* info_counts, double* edge_weights, uint8_t* edge_mask,
                                       tzr_similarity* poses, tzr_pose_graph_summary* pg_summary, int32_t* pg_status);
+
+/* tzr_register_cloud_pairs_multiway with coloured ICP: its arguments plus colors, lambda_geometric and kernel (checked as
+ * tzr_register_cloud_pairs_icp_colored checks them, before any device work).  It runs
+ * tzr_register_cloud_pairs_icp_colored, then the information matrix of every refined pair at its coloured ICP
+ * transform and max_correspondence_distance (geometric only, as Open3D's GetInformationMatrixFromPointClouds: the
+ * colours play no part), then the GNC-TLS pose graph, all in one call as tzr_register_cloud_pairs_multiway.  Every
+ * output equals tzr_register_cloud_pairs_icp_colored, then tzr_information_matrix_batch over the refined pairs in pair
+ * order, then tzr_pose_graph_optimize over them, bit for bit; with lambda_geometric = 1 and no kernel it equals
+ * tzr_register_cloud_pairs_multiway bit for bit.  params->estimate_scaling = 1 is TZR_ERR_INVALID_ARG. */
+int tzr_register_cloud_pairs_multiway_colored(
+    tzr_ctx* ctx, const tzr_frontend_params* fparams, const tzr_params* params, int n_clouds, const int32_t* n,
+    const float* const* pts, int P, const int32_t* pair_clouds, const uint64_t* tuple_seeds, tzr_solution* solutions,
+    int32_t* status, int32_t* problem_index, int64_t* n_corr, int32_t* const* corr, int32_t* const* cliques,
+    float* global_scale, const tzr_icp_params* icp, const float* const* colors, double lambda_geometric,
+    const tzr_robust_kernel* kernel, tzr_icp_result* icp_results, const int32_t* uncertain,
+    const tzr_pose_graph_params* pg, double* information, int32_t* info_counts, double* edge_weights,
+    uint8_t* edge_mask, tzr_similarity* poses, tzr_pose_graph_summary* pg_summary, int32_t* pg_status);
 
 /* ---- downsampling point clouds: voxel-grid averaging ----------------------------------------------------------
  * The first step of the reference's FPFH + TEASER++ + ICP tutorial (voxel_down_sample on both raw scans), for many

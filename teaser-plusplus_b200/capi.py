@@ -167,6 +167,7 @@ _SYMBOLS = [
     "tzr_information_matrix", "tzr_information_matrix_batch", "tzr_pose_graph_params_default", "tzr_pose_graph_optimize",
     "tzr_register_cloud_pairs_multiway", "tzr_estimate_color_gradients", "tzr_estimate_color_gradients_batch",
     "tzr_icp_colored", "tzr_icp_colored_batch", "tzr_voxel_downsample_colors", "tzr_voxel_downsample_colors_batch",
+    "tzr_register_cloud_pairs_icp_colored", "tzr_register_cloud_pairs_multiway_colored",
 ]
 
 # status codes (tzr_status)
@@ -338,6 +339,10 @@ def lib():
     L.tzr_icp_colored.argtypes = L.tzr_icp_point_to_plane.argtypes + [fp, fp, C.c_double, C.POINTER(RobustKernel)]
     L.tzr_icp_colored_batch.argtypes = L.tzr_icp_point_to_plane_batch.argtypes + [fpp, fpp, C.c_double,
                                                                                    C.POINTER(RobustKernel)]
+    L.tzr_register_cloud_pairs_icp_colored.argtypes = L.tzr_register_cloud_pairs.argtypes + [
+        C.POINTER(IcpParams), fpp, C.c_double, C.POINTER(RobustKernel), C.POINTER(IcpResult)]
+    L.tzr_register_cloud_pairs_multiway_colored.argtypes = L.tzr_register_cloud_pairs_icp_colored.argtypes + \
+        L.tzr_register_cloud_pairs_multiway.argtypes[len(L.tzr_register_cloud_pairs_icp.argtypes):]
     L.tzr_voxel_downsample.argtypes = [vp, fp, C.c_int, C.c_double, fp, i32p, i32p]
     L.tzr_voxel_downsample_batch.argtypes = [vp, C.c_int, i32p, fpp, C.c_double, fpp, i32p, C.POINTER(i32p), i32p]
     L.tzr_voxel_downsample_colors.argtypes = L.tzr_voxel_downsample.argtypes + [fp, fp]
@@ -1188,7 +1193,7 @@ class Context:
                                  fpfh_search_radius=0.05, use_absolute_scale=True, use_crosscheck=True,
                                  use_tuple_test=True, tuple_scale=0.0, tuple_seeds=None, max_iteration=30,
                                  relative_fitness=1e-6, relative_rmse=1e-6, method="point_to_point", epsilon=1e-3,
-                                 kernel=None):
+                                 kernel=None, colors=None, lambda_geometric=0.968):
         """tzr_register_cloud_pairs_icp: register_cloud_pairs, then ICP of every pair with a valid solution on its two
         clouds, seeded with that solution, in the same call.  Returns register_cloud_pairs' six results plus the ICP
         records (structured array (P,) of ICP_RESULT_DTYPE, zeroed for a pair that was not refined).
@@ -1196,9 +1201,13 @@ class Context:
         normals of the call's own FPFH stage; method="generalized" runs generalized ICP
         (tzr_register_cloud_pairs_icp_generalized) with both clouds' normals from that stage and the given epsilon.
         kernel (see robust_kernel(); point-to-plane and generalized only) runs the method with that robust kernel
-        (tzr_register_cloud_pairs_icp_robust); None keeps the entries above."""
-        if method not in ("point_to_point", "point_to_plane", "generalized"):
+        (tzr_register_cloud_pairs_icp_robust); None keeps the entries above.  method="colored" runs coloured ICP
+        (tzr_register_cloud_pairs_icp_colored) with colors (one (n,3) array per cloud, required for this method and
+        refused for the others), lambda_geometric and kernel (None: L2)."""
+        if method not in ("point_to_point", "point_to_plane", "generalized", "colored"):
             raise TzrError(f"register_cloud_pairs_icp: unknown method {method!r}")
+        if (colors is None) != (method != "colored"):
+            raise TzrError("register_cloud_pairs_icp: colors are required by method='colored' and by no other method")
         kernel = robust_kernel(kernel)
         if kernel is not None and method == "point_to_point":
             raise TzrError("register_cloud_pairs_icp: point-to-point ICP takes no robust kernel")
@@ -1207,11 +1216,12 @@ class Context:
         return self._register_pairs(clouds, pairs, params, normal_search_radius, fpfh_search_radius, use_absolute_scale,
                                     use_crosscheck, use_tuple_test, tuple_scale, tuple_seeds, icp,
                                     plane=method == "point_to_plane",
-                                    epsilon=float(epsilon) if method == "generalized" else None, kernel=kernel)
+                                    epsilon=float(epsilon) if method == "generalized" else None, kernel=kernel,
+                                    colored=None if colors is None else (colors, float(lambda_geometric)))
 
     def _register_pairs(self, clouds, pairs, params, normal_search_radius, fpfh_search_radius, use_absolute_scale,
                         use_crosscheck, use_tuple_test, tuple_scale, tuple_seeds, icp, plane=False, epsilon=None,
-                        kernel=None, multiway=None):
+                        kernel=None, multiway=None, colored=None):
         cl = [np.ascontiguousarray(c, dtype=np.float32) for c in clouds]
         if not cl or any(c.ndim != 2 or c.shape[1] != 3 or c.shape[0] == 0 for c in cl):
             raise TzrError("register_cloud_pairs: a non-empty list of non-empty (n,3) clouds is required")
@@ -1226,6 +1236,13 @@ class Context:
         n = np.array([c.shape[0] for c in cl], dtype=np.int32)
         if pc.min() < 0 or pc.max() >= len(cl):
             raise TzrError("register_cloud_pairs: a pair names a cloud that is not in the list")
+        if colored is not None:  # (colours per cloud, lambda_geometric): the coloured entries' extra arguments
+            cols, lam = colored
+            if len(cols) != len(cl):
+                raise TzrError("register_cloud_pairs: colors needs one (n,3) array per cloud")
+            K = [_colors32(k, c.shape[0], "register_cloud_pairs") for k, c in zip(cols, cl)]
+            col_args = ((C.POINTER(C.c_float) * len(cl))(*[_p(k, C.c_float) for k in K]), lam,
+                        None if kernel is None else C.byref(kernel))
         fpar = FrontendParams(float(normal_search_radius), float(fpfh_search_radius), int(bool(use_absolute_scale)),
                               int(bool(use_crosscheck)), int(bool(use_tuple_test)), float(tuple_scale))
         cap = [int(n[a]) + int(n[b]) for a, b in pc]
@@ -1259,13 +1276,18 @@ class Context:
                 poses = (Similarity * len(cl))()
                 summ = PoseGraphSummary()
                 pg_status = C.c_int32(0)
-                rc = lib().tzr_register_cloud_pairs_multiway(*args, C.byref(icp), out_res, _p(unc, C.c_int32),
-                                                             C.byref(pg), _p(info, C.c_double), _p(icnt, C.c_int32),
-                                                             _p(ew, C.c_double), _p(em, C.c_uint8), poses,
-                                                             C.byref(summ), C.byref(pg_status))
+                mw_out = (_p(unc, C.c_int32), C.byref(pg), _p(info, C.c_double), _p(icnt, C.c_int32),
+                          _p(ew, C.c_double), _p(em, C.c_uint8), poses, C.byref(summ), C.byref(pg_status))
+                if colored is not None:
+                    rc = lib().tzr_register_cloud_pairs_multiway_colored(*args, C.byref(icp), *col_args, out_res,
+                                                                         *mw_out)
+                else:
+                    rc = lib().tzr_register_cloud_pairs_multiway(*args, C.byref(icp), out_res, *mw_out)
                 mw = dict(information=info, counts=icnt, weights=ew, mask=em.astype(bool), poses=_poses(poses),
                           status=int(pg_status.value), iterations=int(summ.iterations),
                           inner_iterations=int(summ.inner_iterations), cost=float(summ.cost))
+            elif colored is not None:
+                rc = lib().tzr_register_cloud_pairs_icp_colored(*args, C.byref(icp), *col_args, out_res)
             elif kernel is not None:
                 rc = lib().tzr_register_cloud_pairs_icp_robust(*args, C.byref(icp), 1 if plane else 2,
                                                                0.0 if epsilon is None else epsilon, C.byref(kernel),
@@ -1288,13 +1310,19 @@ class Context:
     def register_multiway(self, clouds, pairs, params: Params, max_correspondence_distance, uncertain=None,
                           normal_search_radius=0.03, fpfh_search_radius=0.05, use_absolute_scale=True,
                           use_crosscheck=True, use_tuple_test=True, tuple_scale=0.0, tuple_seeds=None, max_iteration=30,
-                          relative_fitness=1e-6, relative_rmse=1e-6, pose_graph=None):
+                          relative_fitness=1e-6, relative_rmse=1e-6, pose_graph=None, colors=None,
+                          lambda_geometric=0.968, kernel=None):
         """tzr_register_cloud_pairs_multiway: register_cloud_pairs_icp(method="point_to_plane"), the information
         matrix of every refined pair and the GNC-TLS pose graph over the clouds, in one call.  uncertain: one flag per
         pair (None: Open3D's tutorial rule, pair (k, k + 1) certain and every other pair uncertain).  pose_graph: a
         PoseGraphParams (None: the defaults with c = max_correspondence_distance).  Returns register_cloud_pairs_icp's
         seven results plus a dict: information (P,6,6), counts (P,), weights (P,), mask (P,) bool, poses (n_clouds,4,4),
-        status (the pose graph's TZR status), iterations, inner_iterations, cost."""
+        status (the pose graph's TZR status), iterations, inner_iterations, cost.  colors (one (n,3) array per cloud)
+        refines by coloured ICP instead (tzr_register_cloud_pairs_multiway_colored) with lambda_geometric and kernel
+        (None: L2); a kernel without colours is refused."""
+        kernel = robust_kernel(kernel)
+        if kernel is not None and colors is None:
+            raise TzrError("register_multiway: a robust kernel needs colors (coloured ICP)")
         pc = np.ascontiguousarray(pairs, dtype=np.int32).reshape(-1, 2)
         if uncertain is None:
             uncertain = [0 if b == a + 1 else 1 for a, b in pc]
@@ -1303,7 +1331,8 @@ class Context:
                          relative_fitness=float(relative_fitness), relative_rmse=float(relative_rmse))
         return self._register_pairs(clouds, pc, params, normal_search_radius, fpfh_search_radius, use_absolute_scale,
                                     use_crosscheck, use_tuple_test, tuple_scale, tuple_seeds, icp, plane=True,
-                                    multiway=(uncertain, pg))
+                                    kernel=kernel, multiway=(uncertain, pg),
+                                    colored=None if colors is None else (colors, float(lambda_geometric)))
 
     def information_matrix(self, src, dst, transform, max_correspondence_distance):
         """tzr_information_matrix: (Lambda (6,6) float64, count) of the (ns,3) source at transform (see similarity())

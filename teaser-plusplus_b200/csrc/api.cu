@@ -2424,14 +2424,18 @@ static void icp_result_of(const IcpProb& pr, tzr_icp_result* out) {
 // icp (may be NULL): after the solve, ICP of every solved pair on its two clouds (already in m_in), seeded on the device
 // from its record (ctx->icp holds the ICP workspace); icp_results (P entries) then receives the refinements, zeroed for a
 // pair that was not refined.  Without icp the launches, synchronisations and outputs are tzr_register_cloud_pairs'.
-// icp_kernel: the robust kernel of the point-to-plane and generalized modes (checked by the caller; NULL = L2).
+// icp_kernel: the robust kernel of the point-to-plane, generalized and coloured modes (checked by the caller; NULL = L2).
+// colors, lambda_geometric: the coloured mode's (n_clouds entries aligned with pts; lambda already checked and mapped
+// into [0, 1] by the caller).
 static int register_pairs_run(tzr_ctx* ctx, const tzr_frontend_params* fp, const tzr_params* params, int n_clouds,
                               const int32_t* n, const float* const* pts, int P, const int32_t* pair_clouds,
                               const uint64_t* tuple_seeds, tzr_solution* solutions, int32_t* status,
                               int32_t* problem_index, int64_t* n_corr, int32_t* const* corr, int32_t* const* cliques,
                               float* global_scale, const tzr_icp_params* icp, tzr_icp_result* icp_results,
                               int icp_mode = kIcpPointToPoint, double icp_epsilon = 0,
-                              const tzr_robust_kernel* icp_kernel = nullptr, const MultiwayOut* mw = nullptr) {
+                              const tzr_robust_kernel* icp_kernel = nullptr, const MultiwayOut* mw = nullptr,
+                              const float* const* colors = nullptr, double lambda_geometric = 0) {
+  const bool colored = icp && icp_mode == kIcpColored;
   if (!ctx || !fp || !params || n_clouds < 1 || !n || !pts || P < 1 || !pair_clouds || !solutions || !status ||
       !n_corr || !(fp->normal_search_radius > 0) || !(fp->fpfh_search_radius > 0))
     return TZR_ERR_INVALID_ARG;
@@ -2440,8 +2444,9 @@ static int register_pairs_run(tzr_ctx* ctx, const tzr_frontend_params* fp, const
              !mw->info_counts || !mw->edge_weights || !mw->edge_mask || !mw->poses || !mw->pg_status))
     return TZR_ERR_INVALID_ARG;
   if (icp && icp_mode == kIcpGeneralized && !icp_epsilon_ok(icp_epsilon)) return TZR_ERR_INVALID_ARG;
+  if (colored && !colors) return TZR_ERR_INVALID_ARG;
   for (int c = 0; c < n_clouds; ++c)
-    if (n[c] <= 0 || !pts[c]) return TZR_ERR_INVALID_ARG;
+    if (n[c] <= 0 || !pts[c] || (colored && !colors[c])) return TZR_ERR_INVALID_ARG;
   std::vector<int32_t> ns(P), nd(P);
   std::vector<uint64_t> seeds(P, 0);
   std::vector<int2> cloud_lo(P);
@@ -2467,10 +2472,13 @@ static int register_pairs_run(tzr_ctx* ctx, const tzr_frontend_params* fp, const
   cudaSetDevice(ctx->device);
   cudaStream_t st = ctx->stream;
   const size_t N = (size_t)fplan.N, NS = (size_t)mplan.NS, ND = (size_t)mplan.ND, C = NS + ND;
-  // m_in: cloud points | FPFH cloud table | pair table | NN work list | cloud offsets per pair | gather table
+  // m_in: cloud points | FPFH cloud table | pair table | NN work list | cloud offsets per pair | (coloured mode: cloud
+  // colours | gradient cloud table) | gather table; without colours the two regions are empty
   const size_t o_ct = al256(N * 12), o_mp = o_ct + al256((size_t)n_clouds * sizeof(FpfhCloud)),
                o_w = o_mp + al256((size_t)P * sizeof(MatchPair)), o_lo = o_w + al256(W.size() * sizeof(NnWork)),
-               o_g = o_lo + al256((size_t)P * sizeof(int2)), in_bytes = o_g + (size_t)P * sizeof(PairGather);
+               o_col = o_lo + al256((size_t)P * sizeof(int2)), o_gct = o_col + al256(colored ? N * 12 : 0),
+               o_g = o_gct + al256(colored ? (size_t)n_clouds * sizeof(FpfhCloud) : 0),
+               in_bytes = o_g + (size_t)P * sizeof(PairGather);
   // m_out: [overflow | counts | global scales] | descriptors | normals | matcher points and descriptors | matcher rows |
   // solve src | solve dst | records | compacted index pairs | cliques
   const size_t o_cnt = al256((size_t)n_clouds * 4), o_gs = o_cnt + (size_t)P * 4, head = o_gs + (size_t)P * 4;
@@ -2489,8 +2497,13 @@ static int register_pairs_run(tzr_ctx* ctx, const tzr_frontend_params* fp, const
   // second).  Its workspace ctx->icp is laid out from 0 (icp_layout); the pinned area mirrors the layout's tables
   // ([problems | target clouds | chunks], staged in and the problem table read back) and, with the multiway step, holds
   // the [information | counts] of the refined pairs read back.
+  // Coloured mode: the gradient pass (tzr_estimate_color_gradients_batch at 2 max_correspondence_distance, the FPFH
+  // stage's route) spans every cloud, so it writes each cloud's gradients at its cloud-table rows, where the coloured
+  // system reads them through buf.dst, and computes them once however many pairs target the cloud.  Its table does not
+  // depend on which pairs are solved, so it is planned once, here, and staged with the clouds and their colours; the
+  // layout's own slot for it in ctx->icp stays unused.
   IcpPlan iplan;
-  std::vector<FpfhCloud> iclouds;
+  std::vector<FpfhCloud> iclouds, gclouds;
   std::vector<IcpProb> iprobs;
   std::vector<int> ichunks;
   auto plan_icp = [&](const std::vector<int>& pairs) {
@@ -2509,6 +2522,15 @@ static int register_pairs_run(tzr_ctx* ctx, const tzr_frontend_params* fp, const
     std::vector<int> every(P);
     for (int p = 0; p < P; ++p) every[p] = p;
     icp_iteration_settings(&iplan, *icp, icp_mode, icp_epsilon, icp_kernel);
+    iplan.lambda_geometric = lambda_geometric;
+    if (colored) {
+      iplan.grad_r = 2.0 * icp->max_correspondence_distance;
+      gclouds.resize((size_t)n_clouds);
+      if (fpfh_plan(n_clouds, n, iplan.grad_r, iplan.grad_r, route, gclouds.data(), &iplan.ggrid) != TZR_OK) {
+        ctx->last_error = "the clouds' gradient grid does not fit 32-bit indices";
+        return TZR_ERR_TOO_LARGE;
+      }
+    }
     if (plan_icp(every) != TZR_OK) {
       ctx->last_error = "the refinement's points or target grid do not fit 32-bit indices";
       return TZR_ERR_TOO_LARGE;
@@ -2532,6 +2554,11 @@ static int register_pairs_run(tzr_ctx* ctx, const tzr_frontend_params* fp, const
   spans.push_back(CopySpan{h + o_mp, MP.data(), (size_t)P * sizeof(MatchPair)});
   spans.push_back(CopySpan{h + o_w, W.data(), W.size() * sizeof(NnWork)});
   spans.push_back(CopySpan{h + o_lo, cloud_lo.data(), (size_t)P * sizeof(int2)});
+  if (colored) {
+    for (int c = 0; c < n_clouds; ++c)
+      spans.push_back(CopySpan{h + o_col + (size_t)clouds[c].lo * 12, colors[c], (size_t)n[c] * 12});
+    spans.push_back(CopySpan{h + o_gct, gclouds.data(), (size_t)n_clouds * sizeof(FpfhCloud)});
+  }
   CK(stage_in(spans, h, d_in, o_ct, o_g, false, st));
   const float* d_pts = (const float*)d_in;
   const MatchPair* d_mp = (const MatchPair*)(d_in + o_mp);
@@ -2643,6 +2670,10 @@ static int register_pairs_run(tzr_ctx* ctx, const tzr_frontend_params* fp, const
     // cloud table's indexing
     buf.src = buf.dst = d_pts;
     buf.src_normals = buf.dst_normals = (const float4*)(d_out + o_nrm);
+    if (colored) {  // the colours and the gradient table share the cloud table's indexing; launch_icp runs the pass
+      buf.src_colors = buf.dst_colors = (const float*)(d_in + o_col);
+      buf.gclouds = (FpfhCloud*)(d_in + o_gct);
+    }
     IcpGrid grid{nullptr, nullptr, nullptr};
     ctx->launches += launch_icp(iplan, buf, st, &grid);
     if ((rc = check_launch(ctx, "icp launch")) != TZR_OK) return rc;
@@ -2786,6 +2817,28 @@ int tzr_register_cloud_pairs_icp_robust(tzr_ctx* ctx, const tzr_frontend_params*
   return register_pairs_run(ctx, fp, params, n_clouds, n, pts, P, pair_clouds, tuple_seeds, solutions, status,
                             problem_index, n_corr, corr, cliques, global_scale, icp, icp_results,
                             method == 1 ? kIcpPointToPlane : kIcpGeneralized, epsilon, kernel);
+}
+
+// every coloured entry's lambda and kernel, checked before any device work: TZR_OK when they pass, lambda then mapped
+// into [0, 1] (outside it: 0.968, Open3D's TransformationEstimationForColoredICP)
+static int colored_args(double* lambda_geometric, const tzr_robust_kernel* kernel) {
+  if (!std::isfinite(*lambda_geometric) || (kernel && !robust_kernel_ok(kernel))) return TZR_ERR_INVALID_ARG;
+  if (*lambda_geometric < 0.0 || *lambda_geometric > 1.0) *lambda_geometric = 0.968;
+  return TZR_OK;
+}
+
+int tzr_register_cloud_pairs_icp_colored(tzr_ctx* ctx, const tzr_frontend_params* fp, const tzr_params* params,
+                                         int n_clouds, const int32_t* n, const float* const* pts, int P,
+                                         const int32_t* pair_clouds, const uint64_t* tuple_seeds,
+                                         tzr_solution* solutions, int32_t* status, int32_t* problem_index,
+                                         int64_t* n_corr, int32_t* const* corr, int32_t* const* cliques,
+                                         float* global_scale, const tzr_icp_params* icp, const float* const* colors,
+                                         double lambda_geometric, const tzr_robust_kernel* kernel,
+                                         tzr_icp_result* icp_results) {
+  if (!icp || !colors || colored_args(&lambda_geometric, kernel) != TZR_OK) return TZR_ERR_INVALID_ARG;
+  return register_pairs_run(ctx, fp, params, n_clouds, n, pts, P, pair_clouds, tuple_seeds, solutions, status,
+                            problem_index, n_corr, corr, cliques, global_scale, icp, icp_results, kIcpColored, 0,
+                            kernel, nullptr, colors, lambda_geometric);
 }
 
 void tzr_icp_params_default(tzr_icp_params* p) {
@@ -2968,8 +3021,7 @@ int tzr_icp_colored_batch(tzr_ctx* ctx, const tzr_icp_params* params, int B, con
                           const float* const* dst_normals, const tzr_similarity* init, tzr_icp_result* results,
                           int32_t* const* corr, const float* const* src_colors, const float* const* dst_colors,
                           double lambda_geometric, const tzr_robust_kernel* kernel) {
-  if (!std::isfinite(lambda_geometric) || (kernel && !robust_kernel_ok(kernel))) return TZR_ERR_INVALID_ARG;
-  if (lambda_geometric < 0.0 || lambda_geometric > 1.0) lambda_geometric = 0.968;
+  if (colored_args(&lambda_geometric, kernel) != TZR_OK) return TZR_ERR_INVALID_ARG;
   return icp_batch_run(ctx, params, kIcpColored, B, ns, src, nullptr, nd, dst, dst_normals, 0.0, init, results, corr,
                        kernel, lambda_geometric, src_colors, dst_colors);
 }
@@ -3087,6 +3139,21 @@ int tzr_register_cloud_pairs_multiway(tzr_ctx* ctx, const tzr_frontend_params* f
   return register_pairs_run(ctx, fp, params, n_clouds, n, pts, P, pair_clouds, tuple_seeds, solutions, status,
                             problem_index, n_corr, corr, cliques, global_scale, icp, icp_results, kIcpPointToPlane, 0,
                             nullptr, &mw);
+}
+
+int tzr_register_cloud_pairs_multiway_colored(
+    tzr_ctx* ctx, const tzr_frontend_params* fp, const tzr_params* params, int n_clouds, const int32_t* n,
+    const float* const* pts, int P, const int32_t* pair_clouds, const uint64_t* tuple_seeds, tzr_solution* solutions,
+    int32_t* status, int32_t* problem_index, int64_t* n_corr, int32_t* const* corr, int32_t* const* cliques,
+    float* global_scale, const tzr_icp_params* icp, const float* const* colors, double lambda_geometric,
+    const tzr_robust_kernel* kernel, tzr_icp_result* icp_results, const int32_t* uncertain,
+    const tzr_pose_graph_params* pg, double* information, int32_t* info_counts, double* edge_weights,
+    uint8_t* edge_mask, tzr_similarity* poses, tzr_pose_graph_summary* pg_summary, int32_t* pg_status) {
+  if (!icp || !colors || colored_args(&lambda_geometric, kernel) != TZR_OK) return TZR_ERR_INVALID_ARG;
+  const MultiwayOut mw{uncertain, pg, information, info_counts, edge_weights, edge_mask, poses, pg_summary, pg_status};
+  return register_pairs_run(ctx, fp, params, n_clouds, n, pts, P, pair_clouds, tuple_seeds, solutions, status,
+                            problem_index, n_corr, corr, cliques, global_scale, icp, icp_results, kIcpColored, 0,
+                            kernel, &mw, colors, lambda_geometric);
 }
 
 // tzr_voxel_downsample(_batch): the clouds staged back to back (one H2D copy), the batch's launches (launch_voxel), a

@@ -13,6 +13,10 @@ class PLYReader {
   PLYReader() {}
   /// Reads the vertices of a PLY file into `cloud` (appending).  Returns 0 on success, -1 on failure (ply_io.cc:22-81).
   int read(const std::string& file_name, PointCloud& cloud);
+  /// The same, plus the vertices' red, green and blue (any scalar type, each divided by 255 as Open3D reads them, so
+  /// uchar colours land in [0, 1]) appended to `colors`, one per point.  A vertex element without all three channels
+  /// returns -1 and appends nothing.
+  int read(const std::string& file_name, PointCloud& cloud, ColorCloud& colors);
 };
 
 class PLYWriter {

@@ -389,6 +389,16 @@ class RobustRegistrationSolver {
                                                                 const CloudPairParams& params,
                                                                 const GeneralizedICPParams& icp,
                                                                 const RobustKernel& kernel);
+  // The overloads above with coloured ICP (tzr_register_cloud_pairs_icp_colored): colors holds one ColorCloud per
+  // cloud, aligned with it.  Each target's normals are the ones the call's FPFH stage computed at
+  // params.normal_search_radius, and each cloud's colour gradients are computed once per call, at 2
+  // max_correspondence_distance.  Each refined record equals ColoredICP with the same parameters and kernel (L2 by
+  // default) on the pair, seeded with its solution, with those normals.
+  std::vector<CloudPairICPResult> solveCloudPairsColoredICP(const std::vector<PointCloud>& clouds,
+                                                            const std::vector<ColorCloud>& colors,
+                                                            const std::vector<std::pair<int, int>>& pairs,
+                                                            const CloudPairParams& params, const ColoredICPParams& icp,
+                                                            const RobustKernel& kernel = RobustKernel());
   // Multiway registration (tzr_register_cloud_pairs_multiway): solveCloudPairsPointToPlane, then the information
   // matrix of every refined pair at its ICP transform and distance, then the GNC-TLS pose graph over the clouds with one
   // edge per refined pair, in one device call.  uncertain: one flag per pair; the overload without it takes Open3D's
@@ -414,6 +424,16 @@ class RobustRegistrationSolver {
   MultiwayResult solveMultiway(const std::vector<PointCloud>& clouds, const std::vector<std::pair<int, int>>& pairs,
                                const CloudPairParams& params, const PointToPointICPParams& icp,
                                const PoseGraphParams& pose_graph, const std::vector<bool>& uncertain);
+  // The two overloads above with coloured ICP (tzr_register_cloud_pairs_multiway_colored): solveCloudPairsColoredICP
+  // in place of solveCloudPairsPointToPlane.  The information matrices are geometric, as without colours.
+  MultiwayResult solveMultiway(const std::vector<PointCloud>& clouds, const std::vector<ColorCloud>& colors,
+                               const std::vector<std::pair<int, int>>& pairs, const CloudPairParams& params,
+                               const ColoredICPParams& icp, const PoseGraphParams& pose_graph,
+                               const RobustKernel& kernel = RobustKernel());
+  MultiwayResult solveMultiway(const std::vector<PointCloud>& clouds, const std::vector<ColorCloud>& colors,
+                               const std::vector<std::pair<int, int>>& pairs, const CloudPairParams& params,
+                               const ColoredICPParams& icp, const PoseGraphParams& pose_graph,
+                               const std::vector<bool>& uncertain, const RobustKernel& kernel = RobustKernel());
   bool isMaxCliqueProvenOptimal() const { return clique_proven_; }
   long long getNumInlierGraphEdges() const { return n_edges_; }
   int getGNCRotationIterations() const { return gnc_iterations_; }

@@ -687,11 +687,16 @@ PYBIND11_MODULE(_teaserpp, m) {
               double max_correspondence_distance, int max_iteration, double relative_fitness, double relative_rmse,
               double normal_search_radius, double fpfh_search_radius, bool use_absolute_scale, bool use_crosscheck,
               bool use_tuple_test, float tuple_scale, uint64_t tuple_seed, const std::string& method, double epsilon,
-              const py::object& kernel) {
-             // GPU extra: solve_cloud_pairs, then point-to-point (point-to-plane, generalized) ICP of every pair with a
-             // valid solution, in one call
-             if (method != "point_to_point" && method != "point_to_plane" && method != "generalized")
-               throw std::invalid_argument("method must be \"point_to_point\", \"point_to_plane\" or \"generalized\"");
+              const py::object& kernel, const py::object& colors, double lambda_geometric) {
+             // GPU extra: solve_cloud_pairs, then point-to-point (point-to-plane, generalized, coloured) ICP of every
+             // pair with a valid solution, in one call
+             if (method != "point_to_point" && method != "point_to_plane" && method != "generalized" &&
+                 method != "colored")
+               throw std::invalid_argument(
+                   "method must be \"point_to_point\", \"point_to_plane\", \"generalized\" or \"colored\"");
+             // colours: one (n,3) array per cloud, for method="colored" and no other
+             if (colors.is_none() != (method != "colored"))
+               throw std::invalid_argument("colors are required by method=\"colored\" and by no other method");
              // a robust kernel (point-to-plane and generalized only; None keeps the unweighted entries)
              if (!kernel.is_none() && method == "point_to_point")
                throw std::invalid_argument("point-to-point ICP takes no robust kernel");
@@ -699,6 +704,9 @@ PYBIND11_MODULE(_teaserpp, m) {
              const teaser::RobustKernel rk = robust ? kernel.cast<teaser::RobustKernel>() : teaser::RobustKernel();
              std::vector<teaser::PointCloud> pcs;
              for (const auto& a : clouds) pcs.push_back(cloud_of(a));
+             std::vector<teaser::ColorCloud> ccs;
+             if (!colors.is_none())
+               for (const auto& a : colors.cast<std::vector<CloudArray>>()) ccs.push_back(colors_of(a));
              Solver::CloudPairParams cp;
              cp.normal_search_radius = normal_search_radius;
              cp.fpfh_search_radius = fpfh_search_radius;
@@ -716,7 +724,12 @@ PYBIND11_MODULE(_teaserpp, m) {
              std::vector<Solver::CloudPairICPResult> res;
              {
                py::gil_scoped_release release;
-               if (robust)
+               if (method == "colored") {
+                 teaser::ColoredICPParams cip;
+                 static_cast<teaser::PointToPointICPParams&>(cip) = ip;
+                 cip.lambda_geometric = lambda_geometric;
+                 res = s.solveCloudPairsColoredICP(pcs, ccs, pairs, cp, cip, rk);
+               } else if (robust)
                  res = method == "generalized" ? s.solveCloudPairsGeneralizedICP(pcs, pairs, cp, ip, rk)
                                                : s.solveCloudPairsPointToPlane(pcs, pairs, cp, ip, rk);
                else
@@ -736,7 +749,8 @@ PYBIND11_MODULE(_teaserpp, m) {
            py::arg("relative_fitness") = 1e-6, py::arg("relative_rmse") = 1e-6, py::arg("normal_search_radius") = 0.03,
            py::arg("fpfh_search_radius") = 0.05, py::arg("use_absolute_scale") = true, py::arg("use_crosscheck") = true,
            py::arg("use_tuple_test") = true, py::arg("tuple_scale") = 0.0f, py::arg("tuple_seed") = 0x7ea5e2ull,
-           py::arg("method") = "point_to_point", py::arg("epsilon") = 1e-3, py::arg("kernel") = py::none())
+           py::arg("method") = "point_to_point", py::arg("epsilon") = 1e-3, py::arg("kernel") = py::none(),
+           py::arg("colors") = py::none(), py::arg("lambda_geometric") = 0.968)
       .def(
           "solve_multiway",
           [](Solver& s, const std::vector<CloudArray>& clouds, const std::vector<std::pair<int, int>>& pairs,
@@ -744,11 +758,19 @@ PYBIND11_MODULE(_teaserpp, m) {
              double relative_fitness, double relative_rmse, double normal_search_radius, double fpfh_search_radius,
              bool use_absolute_scale, bool use_crosscheck, bool use_tuple_test, float tuple_scale,
              uint64_t tuple_seed, double gnc_factor, double cost_threshold, int max_iterations,
-             int max_inner_iterations, int reference_node) {
+             int max_inner_iterations, int reference_node, const py::object& colors, double lambda_geometric,
+             const py::object& kernel) {
             // GPU extra: solve_cloud_pairs_icp(method="point_to_plane"), information matrices and the GNC-TLS pose
-            // graph in one call (solveMultiway); uncertain None: pair (k, k + 1) certain, every other pair uncertain
+            // graph in one call (solveMultiway); uncertain None: pair (k, k + 1) certain, every other pair uncertain.
+            // colors (one (n,3) array per cloud): method="colored" instead, with lambda_geometric and kernel (None: L2)
+            if (!kernel.is_none() && colors.is_none())
+              throw std::invalid_argument("a robust kernel needs colors (coloured ICP)");
+            const teaser::RobustKernel rk = kernel.is_none() ? teaser::RobustKernel() : kernel.cast<teaser::RobustKernel>();
             std::vector<teaser::PointCloud> pcs;
             for (const auto& a : clouds) pcs.push_back(cloud_of(a));
+            std::vector<teaser::ColorCloud> ccs;
+            if (!colors.is_none())
+              for (const auto& a : colors.cast<std::vector<CloudArray>>()) ccs.push_back(colors_of(a));
             Solver::CloudPairParams cp;
             cp.normal_search_radius = normal_search_radius;
             cp.fpfh_search_radius = fpfh_search_radius;
@@ -774,7 +796,15 @@ PYBIND11_MODULE(_teaserpp, m) {
             Solver::MultiwayResult r;
             {
               py::gil_scoped_release release;
-              r = given ? s.solveMultiway(pcs, pairs, cp, ip, pg, unc) : s.solveMultiway(pcs, pairs, cp, ip, pg);
+              if (!colors.is_none()) {
+                teaser::ColoredICPParams cip;
+                static_cast<teaser::PointToPointICPParams&>(cip) = ip;
+                cip.lambda_geometric = lambda_geometric;
+                r = given ? s.solveMultiway(pcs, ccs, pairs, cp, cip, pg, unc, rk)
+                          : s.solveMultiway(pcs, ccs, pairs, cp, cip, pg, rk);
+              } else {
+                r = given ? s.solveMultiway(pcs, pairs, cp, ip, pg, unc) : s.solveMultiway(pcs, pairs, cp, ip, pg);
+              }
             }
             py::list pair_out, info, poses;
             for (const auto& q : r.pairs)
@@ -796,7 +826,8 @@ PYBIND11_MODULE(_teaserpp, m) {
           py::arg("use_absolute_scale") = true, py::arg("use_crosscheck") = true, py::arg("use_tuple_test") = true,
           py::arg("tuple_scale") = 0.0f, py::arg("tuple_seed") = 0x7ea5e2ull, py::arg("gnc_factor") = 1.4,
           py::arg("cost_threshold") = 1e-6, py::arg("max_iterations") = 100, py::arg("max_inner_iterations") = 10,
-          py::arg("reference_node") = 0)
+          py::arg("reference_node") = 0, py::arg("colors") = py::none(), py::arg("lambda_geometric") = 0.968,
+          py::arg("kernel") = py::none())
       .def_property_readonly("solution", &Solver::getSolution)
       .def("getSolution", &Solver::getSolution)
       .def_property_readonly("gnc_rotation_cost_at_termination", &Solver::getGNCRotationCostAtTermination)

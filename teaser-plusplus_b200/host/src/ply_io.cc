@@ -81,9 +81,9 @@ double decode(const unsigned char* p, int bytes, char kind, bool swap) {
   }
 }
 
-}  // namespace
-
-int PLYReader::read(const std::string& file_name, PointCloud& cloud) {
+// Both PLYReader::read overloads: the vertex element's x, y, z into cloud and, with colors, its red, green and blue
+// divided by 255 (Open3D's ReadColorCallback) into colors.  A file without the channels asked for appends nothing.
+int read_vertices(const std::string& file_name, PointCloud& cloud, ColorCloud* colors) {
   std::ifstream f(file_name, std::ios::binary);
   if (!f) {
     std::cerr << "Failed to open " << file_name << std::endl;
@@ -139,16 +139,20 @@ int PLYReader::read(const std::string& file_name, PointCloud& cloud) {
   const bool swap = (fmt == LE) != host_is_little_endian();
   bool found_vertices = false;
   for (const Element& e : elements) {
-    int ix = -1, iy = -1, iz = -1;
-    for (size_t k = 0; k < e.props.size(); ++k) {
-      if (e.props[k].name == "x") ix = static_cast<int>(k);
-      if (e.props[k].name == "y") iy = static_cast<int>(k);
-      if (e.props[k].name == "z") iz = static_cast<int>(k);
-    }
+    // slot of every property: 0 ... 2 x, y, z, 3 ... 5 red, green, blue, -1 skipped
+    static const char* const names[6] = {"x", "y", "z", "red", "green", "blue"};
+    std::vector<int> slot(e.props.size(), -1);
+    bool seen[6] = {false, false, false, false, false, false};
+    for (size_t k = 0; k < e.props.size(); ++k)
+      for (int c = 0; c < (colors ? 6 : 3); ++c)
+        if (e.props[k].name == names[c]) {
+          slot[k] = c;
+          seen[c] = true;
+        }
     const bool is_vertex = e.name == "vertex";
-    if (is_vertex && (ix < 0 || iy < 0 || iz < 0)) return -1;
+    if (is_vertex && !(seen[0] && seen[1] && seen[2] && (!colors || (seen[3] && seen[4] && seen[5])))) return -1;
     for (long r = 0; r < e.count; ++r) {
-      double xyz[3] = {0, 0, 0};
+      double xyz[6] = {0, 0, 0, 0, 0, 0};
       if (fmt == ASCII) {
         if (!std::getline(f, line)) return -1;
         std::istringstream is(line);
@@ -162,9 +166,7 @@ int PLYReader::read(const std::string& file_name, PointCloud& cloud) {
           } else {
             double v = 0;
             is >> v;
-            if (static_cast<int>(k) == ix) xyz[0] = v;
-            if (static_cast<int>(k) == iy) xyz[1] = v;
-            if (static_cast<int>(k) == iz) xyz[2] = v;
+            if (slot[k] >= 0) xyz[slot[k]] = v;
           }
         }
         if (is_vertex && !is) return -1;
@@ -179,14 +181,16 @@ int PLYReader::read(const std::string& file_name, PointCloud& cloud) {
           } else {
             if (!f.read(reinterpret_cast<char*>(buf), p.bytes)) return -1;
             const double v = decode(buf, p.bytes, p.kind, swap);
-            if (static_cast<int>(k) == ix) xyz[0] = v;
-            if (static_cast<int>(k) == iy) xyz[1] = v;
-            if (static_cast<int>(k) == iz) xyz[2] = v;
+            if (slot[k] >= 0) xyz[slot[k]] = v;
           }
         }
       }
-      if (is_vertex)
+      if (is_vertex) {
         cloud.push_back({static_cast<float>(xyz[0]), static_cast<float>(xyz[1]), static_cast<float>(xyz[2])});
+        if (colors)
+          colors->push_back({static_cast<float>(xyz[3] / 255.0), static_cast<float>(xyz[4] / 255.0),
+                             static_cast<float>(xyz[5] / 255.0)});
+      }
     }
     if (is_vertex) {
       found_vertices = true;
@@ -194,6 +198,14 @@ int PLYReader::read(const std::string& file_name, PointCloud& cloud) {
     }
   }
   return found_vertices ? 0 : -1;
+}
+
+}  // namespace
+
+int PLYReader::read(const std::string& file_name, PointCloud& cloud) { return read_vertices(file_name, cloud, nullptr); }
+
+int PLYReader::read(const std::string& file_name, PointCloud& cloud, ColorCloud& colors) {
+  return read_vertices(file_name, cloud, &colors);
 }
 
 int PLYWriter::write(const std::string& file_name, const PointCloud& cloud, bool binary_mode) {

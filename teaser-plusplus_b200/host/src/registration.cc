@@ -631,10 +631,10 @@ void icp_result_from_c(const tzr_icp_result& r, const int32_t* corr, PointToPoin
 
 namespace {
 
-// solveCloudPairs' body: tzr_register_cloud_pairs, or tzr_register_cloud_pairs_icp(_point_to_plane, _generalized) when
-// icp is given (icp_res then receives P records)
-enum class IcpMethod { kPointToPoint, kPointToPlane, kGeneralized };
-// the multiway step's inputs and outputs (solveMultiway: tzr_register_cloud_pairs_multiway, point-to-plane)
+// solveCloudPairs' body: tzr_register_cloud_pairs, or tzr_register_cloud_pairs_icp(_point_to_plane, _generalized,
+// _robust, _colored) when icp is given (icp_res then receives P records)
+enum class IcpMethod { kPointToPoint, kPointToPlane, kGeneralized, kColored };
+// the multiway step's inputs and outputs (solveMultiway: tzr_register_cloud_pairs_multiway(_colored))
 struct MultiwayCall {
   const int32_t* uncertain;
   const tzr_pose_graph_params* pg;
@@ -650,11 +650,22 @@ std::vector<RobustRegistrationSolver::CloudPairResult> run_cloud_pairs(
     const tzr_params& p, const std::vector<PointCloud>& clouds, const std::vector<std::pair<int, int>>& pairs,
     const RobustRegistrationSolver::CloudPairParams& cp, const tzr_icp_params* icp,
     std::vector<tzr_icp_result>* icp_res, IcpMethod method = IcpMethod::kPointToPoint, double epsilon = 0,
-    const RobustKernel* kernel = nullptr, const MultiwayCall* mw = nullptr) {
+    const RobustKernel* kernel = nullptr, const MultiwayCall* mw = nullptr,
+    const std::vector<ColorCloud>* colors = nullptr, double lambda_geometric = 0) {
   using CloudPairResult = RobustRegistrationSolver::CloudPairResult;
   const int K = static_cast<int>(clouds.size()), P = static_cast<int>(pairs.size());
   std::vector<CloudPairResult> out(P);
   if (P == 0) return out;
+  static_assert(sizeof(ColorRGB) == 3 * sizeof(float), "ColorRGB must be three packed floats");
+  std::vector<const float*> col;
+  if (method == IcpMethod::kColored) {
+    if (colors->size() != clouds.size()) throw std::invalid_argument("teaser: solveCloudPairs: one ColorCloud per cloud");
+    for (int c = 0; c < K; ++c) {
+      if ((*colors)[c].size() != clouds[c].size())
+        throw std::invalid_argument("teaser: solveCloudPairs: a ColorCloud's size differs from its cloud's");
+      col.push_back(clouds[c].empty() ? nullptr : &(*colors)[c][0].r);
+    }
+  }
   static_assert(sizeof(PointXYZ) == 3 * sizeof(float), "PointXYZ must be three packed floats");
   std::vector<int32_t> n(K), pc(2 * static_cast<size_t>(P)), status(P), index(P);
   std::vector<const float*> pts(K);
@@ -697,17 +708,30 @@ std::vector<RobustRegistrationSolver::CloudPairResult> run_cloud_pairs(
                                   scales.data());
   } else {
     icp_res->assign(P, tzr_icp_result{});
-    if (mw) {
+    tzr_robust_kernel k;
+    std::memset(&k, 0, sizeof(k));
+    if (kernel) {
+      k.type = static_cast<int32_t>(kernel->type);
+      k.k = kernel->k;
+    }
+    if (mw && method == IcpMethod::kColored) {
+      rc = tzr_register_cloud_pairs_multiway_colored(
+          ctx, &f, &p, K, n.data(), pts.data(), P, pc.data(), seeds.data(), sols.data(), status.data(), index.data(),
+          n_corr.data(), corr_p.data(), clq_p.data(), scales.data(), icp, col.data(), lambda_geometric,
+          kernel ? &k : nullptr, icp_res->data(), mw->uncertain, mw->pg, mw->information, mw->info_counts,
+          mw->edge_weights, mw->edge_mask, mw->poses, mw->summary, mw->pg_status);
+    } else if (mw) {
       rc = tzr_register_cloud_pairs_multiway(ctx, &f, &p, K, n.data(), pts.data(), P, pc.data(), seeds.data(),
                                              sols.data(), status.data(), index.data(), n_corr.data(), corr_p.data(),
                                              clq_p.data(), scales.data(), icp, icp_res->data(), mw->uncertain, mw->pg,
                                              mw->information, mw->info_counts, mw->edge_weights, mw->edge_mask,
                                              mw->poses, mw->summary, mw->pg_status);
+    } else if (method == IcpMethod::kColored) {
+      rc = tzr_register_cloud_pairs_icp_colored(ctx, &f, &p, K, n.data(), pts.data(), P, pc.data(), seeds.data(),
+                                                sols.data(), status.data(), index.data(), n_corr.data(), corr_p.data(),
+                                                clq_p.data(), scales.data(), icp, col.data(), lambda_geometric,
+                                                kernel ? &k : nullptr, icp_res->data());
     } else if (kernel) {
-      tzr_robust_kernel k;
-      std::memset(&k, 0, sizeof(k));
-      k.type = static_cast<int32_t>(kernel->type);
-      k.k = kernel->k;
       rc = tzr_register_cloud_pairs_icp_robust(ctx, &f, &p, K, n.data(), pts.data(), P, pc.data(), seeds.data(),
                                                sols.data(), status.data(), index.data(), n_corr.data(), corr_p.data(),
                                                clq_p.data(), scales.data(), icp,
@@ -751,7 +775,8 @@ std::vector<RobustRegistrationSolver::CloudPairResult> RobustRegistrationSolver:
 static std::vector<RobustRegistrationSolver::CloudPairICPResult> run_cloud_pairs_icp(
     const tzr_params& p, const std::vector<PointCloud>& clouds, const std::vector<std::pair<int, int>>& pairs,
     const RobustRegistrationSolver::CloudPairParams& cp, const PointToPointICPParams& icp, IcpMethod method,
-    double epsilon = 0, const RobustKernel* kernel = nullptr) {
+    double epsilon = 0, const RobustKernel* kernel = nullptr, const std::vector<ColorCloud>* colors = nullptr,
+    double lambda_geometric = 0) {
   using CloudPairResult = RobustRegistrationSolver::CloudPairResult;
   using CloudPairICPResult = RobustRegistrationSolver::CloudPairICPResult;
   tzr_icp_params ip;
@@ -761,7 +786,8 @@ static std::vector<RobustRegistrationSolver::CloudPairICPResult> run_cloud_pairs
   ip.relative_fitness = icp.relative_fitness;
   ip.relative_rmse = icp.relative_rmse;
   std::vector<tzr_icp_result> res;
-  std::vector<CloudPairResult> base = run_cloud_pairs(p, clouds, pairs, cp, &ip, &res, method, epsilon, kernel);
+  std::vector<CloudPairResult> base =
+      run_cloud_pairs(p, clouds, pairs, cp, &ip, &res, method, epsilon, kernel, nullptr, colors, lambda_geometric);
   std::vector<CloudPairICPResult> out(base.size());
   for (size_t q = 0; q < base.size(); ++q) {
     static_cast<CloudPairResult&>(out[q]) = std::move(base[q]);
@@ -772,17 +798,21 @@ static std::vector<RobustRegistrationSolver::CloudPairICPResult> run_cloud_pairs
   return out;
 }
 
-RobustRegistrationSolver::MultiwayResult RobustRegistrationSolver::solveMultiway(
-    const std::vector<PointCloud>& clouds, const std::vector<std::pair<int, int>>& pairs, const CloudPairParams& cp,
-    const PointToPointICPParams& icp, const PoseGraphParams& pose_graph) {
+// Open3D's tutorial rule: pair (k, k + 1) certain, every other pair uncertain
+static std::vector<bool> tutorial_uncertain(const std::vector<std::pair<int, int>>& pairs) {
   std::vector<bool> uncertain(pairs.size());
-  for (size_t q = 0; q < pairs.size(); ++q) uncertain[q] = pairs[q].second != pairs[q].first + 1;  // Open3D's tutorial
-  return solveMultiway(clouds, pairs, cp, icp, pose_graph, uncertain);
+  for (size_t q = 0; q < pairs.size(); ++q) uncertain[q] = pairs[q].second != pairs[q].first + 1;
+  return uncertain;
 }
 
-RobustRegistrationSolver::MultiwayResult RobustRegistrationSolver::solveMultiway(
-    const std::vector<PointCloud>& clouds, const std::vector<std::pair<int, int>>& pairs, const CloudPairParams& cp,
-    const PointToPointICPParams& icp, const PoseGraphParams& pose_graph, const std::vector<bool>& uncertain) {
+// every solveMultiway overload: point-to-plane without colours, coloured ICP with them
+static RobustRegistrationSolver::MultiwayResult run_multiway(
+    const tzr_params& p, const std::vector<PointCloud>& clouds, const std::vector<std::pair<int, int>>& pairs,
+    const RobustRegistrationSolver::CloudPairParams& cp, const PointToPointICPParams& icp,
+    const PoseGraphParams& pose_graph, const std::vector<bool>& uncertain,
+    const std::vector<ColorCloud>* colors = nullptr, double lambda_geometric = 0,
+    const RobustKernel* kernel = nullptr) {
+  using CloudPairResult = RobustRegistrationSolver::CloudPairResult;
   const size_t P = pairs.size(), K = clouds.size();
   if (uncertain.size() != P) throw std::invalid_argument("teaser: solveMultiway: one uncertain flag per pair");
   tzr_icp_params ip;
@@ -810,8 +840,9 @@ RobustRegistrationSolver::MultiwayResult RobustRegistrationSolver::solveMultiway
                         &pg_status};
   std::vector<tzr_icp_result> res;
   std::vector<CloudPairResult> base =
-      run_cloud_pairs(to_c(params_), clouds, pairs, cp, &ip, &res, IcpMethod::kPointToPlane, 0, nullptr, &mw);
-  MultiwayResult out;
+      run_cloud_pairs(p, clouds, pairs, cp, &ip, &res, colors ? IcpMethod::kColored : IcpMethod::kPointToPlane, 0,
+                      kernel, &mw, colors, lambda_geometric);
+  RobustRegistrationSolver::MultiwayResult out;
   out.pairs.resize(P);
   out.information.resize(P);
   out.information_counts.assign(counts.begin(), counts.end());
@@ -842,6 +873,33 @@ RobustRegistrationSolver::MultiwayResult RobustRegistrationSolver::solveMultiway
   return out;
 }
 
+RobustRegistrationSolver::MultiwayResult RobustRegistrationSolver::solveMultiway(
+    const std::vector<PointCloud>& clouds, const std::vector<std::pair<int, int>>& pairs, const CloudPairParams& cp,
+    const PointToPointICPParams& icp, const PoseGraphParams& pose_graph) {
+  return run_multiway(to_c(params_), clouds, pairs, cp, icp, pose_graph, tutorial_uncertain(pairs));
+}
+
+RobustRegistrationSolver::MultiwayResult RobustRegistrationSolver::solveMultiway(
+    const std::vector<PointCloud>& clouds, const std::vector<std::pair<int, int>>& pairs, const CloudPairParams& cp,
+    const PointToPointICPParams& icp, const PoseGraphParams& pose_graph, const std::vector<bool>& uncertain) {
+  return run_multiway(to_c(params_), clouds, pairs, cp, icp, pose_graph, uncertain);
+}
+
+RobustRegistrationSolver::MultiwayResult RobustRegistrationSolver::solveMultiway(
+    const std::vector<PointCloud>& clouds, const std::vector<ColorCloud>& colors,
+    const std::vector<std::pair<int, int>>& pairs, const CloudPairParams& cp, const ColoredICPParams& icp,
+    const PoseGraphParams& pose_graph, const RobustKernel& kernel) {
+  return solveMultiway(clouds, colors, pairs, cp, icp, pose_graph, tutorial_uncertain(pairs), kernel);
+}
+
+RobustRegistrationSolver::MultiwayResult RobustRegistrationSolver::solveMultiway(
+    const std::vector<PointCloud>& clouds, const std::vector<ColorCloud>& colors,
+    const std::vector<std::pair<int, int>>& pairs, const CloudPairParams& cp, const ColoredICPParams& icp,
+    const PoseGraphParams& pose_graph, const std::vector<bool>& uncertain, const RobustKernel& kernel) {
+  return run_multiway(to_c(params_), clouds, pairs, cp, icp, pose_graph, uncertain, &colors, icp.lambda_geometric,
+                      &kernel);
+}
+
 std::vector<RobustRegistrationSolver::CloudPairICPResult> RobustRegistrationSolver::solveCloudPairs(
     const std::vector<PointCloud>& clouds, const std::vector<std::pair<int, int>>& pairs, const CloudPairParams& cp,
     const PointToPointICPParams& icp) {
@@ -870,6 +928,14 @@ std::vector<RobustRegistrationSolver::CloudPairICPResult> RobustRegistrationSolv
     const std::vector<PointCloud>& clouds, const std::vector<std::pair<int, int>>& pairs, const CloudPairParams& cp,
     const GeneralizedICPParams& icp, const RobustKernel& kernel) {
   return run_cloud_pairs_icp(to_c(params_), clouds, pairs, cp, icp, IcpMethod::kGeneralized, icp.epsilon, &kernel);
+}
+
+std::vector<RobustRegistrationSolver::CloudPairICPResult> RobustRegistrationSolver::solveCloudPairsColoredICP(
+    const std::vector<PointCloud>& clouds, const std::vector<ColorCloud>& colors,
+    const std::vector<std::pair<int, int>>& pairs, const CloudPairParams& cp, const ColoredICPParams& icp,
+    const RobustKernel& kernel) {
+  return run_cloud_pairs_icp(to_c(params_), clouds, pairs, cp, icp, IcpMethod::kColored, 0, &kernel, &colors,
+                             icp.lambda_geometric);
 }
 
 void RobustRegistrationSolver::materialise_tims() {
