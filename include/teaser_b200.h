@@ -908,6 +908,77 @@ int tzr_information_matrix_batch(tzr_ctx* ctx, int B, const int32_t* ns, const f
                                  const float* const* dst, const tzr_similarity* transforms,
                                  double max_correspondence_distance, double* information, int32_t* counts);
 
+/* ---- refining registrations coarse to fine: multi-scale ICP -------------------------------------------------------
+ * Open3D's multi-scale refinement (the coloured-ICP tutorial's schedule, the reconstruction system's multiscale_icp) for
+ * many cloud pairs in one call, defined here as follows (DESIGN.md §3.19):
+ *   - Methods: TZR_ICP_* below, the `method` values of the chained robust entries plus 3 for coloured ICP.
+ *   - Clouds and pairs: n_clouds clouds (n[c] >= 1 float xyz points at pts[c]; colors[c], n[c] x 3 floats, for
+ *     TZR_ICP_COLORED only, where colors and every entry are required) and P pairs in tzr_register_cloud_pairs'
+ *     convention: pair p refines cloud pair_clouds[2p] (source) onto cloud pair_clouds[2p + 1] (target), starting from
+ *     init[p], its scale held fixed throughout.  A cloud named by several pairs is downsampled, and gets its normals and
+ *     gradients, once per scale.
+ *   - The chain it equals: scale s's record of pair p is bit-identical to this chain of public calls:
+ *       1. tzr_voxel_downsample_batch (tzr_voxel_downsample_colors_batch for TZR_ICP_COLORED) of the cloud table at
+ *          scales[s].voxel_size; skipped when the size is 0 (the clouds as given).
+ *       2. tzr_estimate_normals_batch of those clouds at scales[s].normal_search_radius (point-to-plane, generalized and
+ *          coloured only).
+ *       3. The method's tzr_icp_*_batch (tzr_icp_batch, tzr_icp_point_to_plane(_robust)_batch,
+ *          tzr_icp_generalized(_robust)_batch with epsilon, tzr_icp_colored_batch with lambda_geometric) on the pair's
+ *          two clouds from steps 1 and 2, with scales[s]'s distance and criteria and the same kernel.  The seed is init[p]
+ *          at s = 0 and the transform of pair p's record at s - 1 otherwise.
+ *   - information (P x 36 doubles, may be NULL) and info_counts (P, may be NULL), each on its own:
+ *     tzr_information_matrix_batch on the last scale's pair at its final transform and that scale's
+ *     max_correspondence_distance (what the reconstruction system's multiscale_icp returns); zero for a pair not refined
+ *     at the last scale.  Either one given runs the information pass.
+ *   - colors is read for TZR_ICP_COLORED only (NULL or anything for the other methods).
+ *   - Arguments, all checked before any device work (TZR_ERR_INVALID_ARG): method outside 0 ... 3; S < 1; a scale whose
+ *     voxel_size is not finite and >= 0, whose max_correspondence_distance is not finite and > 0, whose
+ *     normal_search_radius is not finite and > 0 for a method with normals, whose max_iteration is < 0 or whose criteria
+ *     are NaN; a pair index outside the cloud table; a seed that tzr_icp refuses; a kernel with TZR_ICP_POINT_TO_POINT,
+ *     or one tzr_icp_point_to_plane_robust_batch refuses; epsilon as tzr_icp_generalized_batch checks it (method 2 only);
+ *     lambda_geometric as tzr_icp_colored_batch handles it (method 3 only: non-finite refused, outside [0, 1] 0.968).
+ *   - Empty cloud at a scale: a cloud with no finite point has no voxel; a pair that uses a cloud with n_down 0 is not
+ *     refined at that scale, and its record carries its pose in (transform as it entered the scale; fitness, rmse,
+ *     iterations, correspondences and converged 0).
+ *   - n_down (n_clouds x S, cloud-major, may be NULL): each cloud's points at each scale (n[c] where voxel_size is 0).
+ *   - status (n_clouds x S, cloud-major, may be NULL): TZR_OK, or TZR_ERR_TOO_LARGE where
+ *       - the cloud's voxel grid fails Open3D's INT_MAX check or the 2^62-cell limit.  This is found before any normals
+ *         or ICP run; then nothing else runs, every record and information matrix is zero, and the call returns
+ *         TZR_ERR_TOO_LARGE;
+ *       - a point of the cloud has more than 4096 neighbours at that scale's normal radius.  This is found at the end of
+ *         the call: the records (and information) of every pair that uses the cloud at that scale or later are zeroed,
+ *         every other record is still the chain's, and the call returns TZR_ERR_TOO_LARGE.
+ * Device flow: one upload of the clouds, every voxel scale back to back, one read-back of the voxel tables (the call's
+ * planning synchronisation, only when some voxel_size > 0), one upload of every scale's tables, then everything else
+ * enqueued and one read-back at the end: at most two host synchronisations whatever S and P.
+ * Launches, per scale: 10 when voxel_size > 0; for the methods with normals the normals pass, 1 (+ 4 when some cloud of
+ * the scale has 4096 points or more); 1 pose store; and when some pair is refined at the scale, 1 pose load and the
+ * method's tzr_icp_*_batch launches (2 + 4 max_iteration, + 4 when some cloud of the scale has 1024 points or more;
+ * coloured: + 1 for the gradient pass, + 4 more when some cloud of the scale has 4096 points or more).  With
+ * information or info_counts, 4 more after the last scale when some pair is refined there.  The debug flags of
+ * tzr_estimate_normals (4194304, 8388608) and tzr_icp (33554432, 67108864) force the routes here too.  Not a solve
+ * entry: the workspace is tzr_icp's, so a retained solve stays retained. */
+#define TZR_ICP_POINT_TO_POINT 0
+#define TZR_ICP_POINT_TO_PLANE 1
+#define TZR_ICP_GENERALIZED 2
+#define TZR_ICP_COLORED 3
+
+typedef struct tzr_icp_scale {
+  double voxel_size;                   /* > 0: voxel-downsample every cloud at this size; 0: the clouds as given */
+  double max_correspondence_distance;  /* finite, > 0 */
+  double normal_search_radius;         /* finite, > 0 for the methods that use normals (Open3D: 2 voxel_size) */
+  double relative_fitness, relative_rmse;
+  int32_t max_iteration;               /* >= 0 */
+  int32_t reserved;
+} tzr_icp_scale;
+
+/* results: P x S records, pair-major (pair p's record of scale s at p * S + s). */
+int tzr_icp_multiscale_batch(tzr_ctx* ctx, int method, int S, const tzr_icp_scale* scales, int n_clouds,
+                             const int32_t* n, const float* const* pts, const float* const* colors, int P,
+                             const int32_t* pair_clouds, const tzr_similarity* init, double epsilon,
+                             double lambda_geometric, const tzr_robust_kernel* kernel, tzr_icp_result* results,
+                             int32_t* n_down, int32_t* status, double* information, int32_t* info_counts);
+
 /* ---- multiway registration: robust pose graph ------------------------------------------------------------------
  * The global step of Open3D's multiway registration (global_optimization over a PoseGraph), with GNC-TLS pruning the
  * uncertain edges instead of Open3D's line process.  One graph per call, defined here as follows (DESIGN.md §3.16):

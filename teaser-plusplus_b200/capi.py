@@ -119,6 +119,45 @@ ICP_RESULT_DTYPE = np.dtype([
     ("n_correspondences", np.int32), ("converged", np.int32), ("reserved", np.int32)], align=True)
 
 
+class IcpScale(C.Structure):
+    """tzr_icp_scale: one scale of tzr_icp_multiscale_batch's schedule."""
+    _fields_ = [("voxel_size", C.c_double), ("max_correspondence_distance", C.c_double),
+                ("normal_search_radius", C.c_double), ("relative_fitness", C.c_double), ("relative_rmse", C.c_double),
+                ("max_iteration", C.c_int32), ("reserved", C.c_int32)]
+
+
+# tzr_icp_multiscale_batch's methods (TZR_ICP_*), by the names Context.icp_multiscale accepts
+ICP_METHODS = {"point_to_point": 0, "point_to_plane": 1, "generalized": 2, "colored": 3}
+# the fields of a scale in the order a tuple gives them, and the defaults of the optional ones
+ICP_SCALE_FIELDS = ("voxel_size", "max_correspondence_distance", "max_iteration", "normal_search_radius",
+                    "relative_fitness", "relative_rmse")
+
+
+def icp_scale(scale) -> IcpScale:
+    """A tzr_icp_scale from an IcpScale (as given), a dict or a tuple in ICP_SCALE_FIELDS order.  voxel_size,
+    max_correspondence_distance and max_iteration are required; normal_search_radius defaults to 2 voxel_size (Open3D's
+    tutorials) and the criteria to 1e-6.  The library checks the values."""
+    if isinstance(scale, IcpScale):
+        return scale
+    if isinstance(scale, dict):
+        unknown = set(scale) - set(ICP_SCALE_FIELDS)
+        if unknown:
+            raise TzrError(f"icp_scale: unknown field(s) {sorted(unknown)} (fields: {ICP_SCALE_FIELDS})")
+        d = dict(scale)
+    else:
+        t = tuple(scale)
+        if len(t) > len(ICP_SCALE_FIELDS):
+            raise TzrError(f"icp_scale: a tuple has at most {len(ICP_SCALE_FIELDS)} entries {ICP_SCALE_FIELDS}")
+        d = dict(zip(ICP_SCALE_FIELDS, t))
+    missing = [k for k in ICP_SCALE_FIELDS[:3] if k not in d]
+    if missing:
+        raise TzrError(f"icp_scale: {missing} required")
+    v = float(d["voxel_size"])
+    return IcpScale(v, float(d["max_correspondence_distance"]), float(d.get("normal_search_radius", 2.0 * v)),
+                    float(d.get("relative_fitness", 1e-6)), float(d.get("relative_rmse", 1e-6)),
+                    int(d["max_iteration"]), 0)
+
+
 class RobustKernel(C.Structure):
     """tzr_robust_kernel: type (LOSS_*) and k (finite and > 0 for HUBER, CAUCHY, GM and TUKEY)."""
     _fields_ = [("type", C.c_int32), ("reserved", C.c_int32), ("k", C.c_double)]
@@ -141,6 +180,7 @@ LOSS_TYPES = {"l2": 0, "l1": 1, "huber": 2, "cauchy": 3, "gm": 4, "tukey": 5}
 assert C.sizeof(IcpParams) == 32, C.sizeof(IcpParams)
 assert C.sizeof(PoseGraphParams) == 40 and PoseGraphParams.reference_node.offset == 32, C.sizeof(PoseGraphParams)
 assert C.sizeof(PoseGraphSummary) == 16 and PoseGraphSummary.cost.offset == 8, C.sizeof(PoseGraphSummary)
+assert C.sizeof(IcpScale) == 48 and IcpScale.max_iteration.offset == 40, C.sizeof(IcpScale)
 assert C.sizeof(RobustKernel) == 16 and RobustKernel.k.offset == 8, C.sizeof(RobustKernel)
 assert SIMILARITY_DTYPE.itemsize == C.sizeof(Similarity) == 104, C.sizeof(Similarity)
 assert ICP_RESULT_DTYPE.itemsize == C.sizeof(IcpResult) == 136, (ICP_RESULT_DTYPE.itemsize, C.sizeof(IcpResult))
@@ -167,7 +207,7 @@ _SYMBOLS = [
     "tzr_information_matrix", "tzr_information_matrix_batch", "tzr_pose_graph_params_default", "tzr_pose_graph_optimize",
     "tzr_register_cloud_pairs_multiway", "tzr_estimate_color_gradients", "tzr_estimate_color_gradients_batch",
     "tzr_icp_colored", "tzr_icp_colored_batch", "tzr_voxel_downsample_colors", "tzr_voxel_downsample_colors_batch",
-    "tzr_register_cloud_pairs_icp_colored", "tzr_register_cloud_pairs_multiway_colored",
+    "tzr_register_cloud_pairs_icp_colored", "tzr_register_cloud_pairs_multiway_colored", "tzr_icp_multiscale_batch",
 ]
 
 # status codes (tzr_status)
@@ -347,6 +387,9 @@ def lib():
     L.tzr_voxel_downsample_batch.argtypes = [vp, C.c_int, i32p, fpp, C.c_double, fpp, i32p, C.POINTER(i32p), i32p]
     L.tzr_voxel_downsample_colors.argtypes = L.tzr_voxel_downsample.argtypes + [fp, fp]
     L.tzr_voxel_downsample_colors_batch.argtypes = L.tzr_voxel_downsample_batch.argtypes + [fpp, fpp]
+    L.tzr_icp_multiscale_batch.argtypes = [vp, C.c_int, C.c_int, C.POINTER(IcpScale), C.c_int, i32p, fpp, fpp,
+                                           C.c_int, i32p, C.POINTER(Similarity), C.c_double, C.c_double,
+                                           C.POINTER(RobustKernel), C.POINTER(IcpResult), i32p, i32p, dp, i32p]
     for s in _SYMBOLS:
         getattr(L, s)  # raises AttributeError if the header and the library disagree
     _lib = L
@@ -1504,6 +1547,66 @@ class Context:
         self._ck(rc)
         out = np.frombuffer(bytes(res), dtype=ICP_RESULT_DTYPE).copy()
         return out, [c[:int(r["n_correspondences"])].copy() for c, r in zip(corr, out)]
+
+    def icp_multiscale(self, clouds, pairs, scales, inits=None, method="point_to_plane", colors=None,
+                       lambda_geometric=0.968, epsilon=1e-3, kernel=None, information=False):
+        """tzr_icp_multiscale_batch: coarse-to-fine ICP of P cloud pairs over S scales in one call.  clouds: (n_c,3)
+        float32 arrays; pairs: (P,2) (source cloud, target cloud); scales: S entries for icp_scale() (dicts or tuples);
+        inits: P seeds for similarity() (None: identity), e.g. register_cloud_pairs' solutions; method: a name of
+        ICP_METHODS or its number; colors: one (n_c,3) array per cloud (read by coloured ICP only, ignored otherwise
+        as the library ignores them); inits may be a list, a SOLUTION_DTYPE array or a (P,4,4) array; kernel: see
+        robust_kernel().  Returns (results (P,S) ICP_RESULT_DTYPE, n_down (n_clouds,S) int32), and with information
+        (Lambda (P,6,6), counts (P,)) after them.  A TzrError for TZR_ERR_TOO_LARGE carries `status` (n_clouds,S) and
+        `result` (what the call returns, zeroed where the contract says)."""
+        pts = [_cloud32(p, "icp_multiscale") for p in clouds]
+        K = len(pts)
+        pc = np.ascontiguousarray(pairs, dtype=np.int32)
+        if K == 0 or pc.ndim != 2 or pc.shape[1] != 2 or pc.shape[0] == 0:
+            raise TzrError("icp_multiscale: a non-empty list of clouds and a (P,2) array of pairs are required")
+        P = pc.shape[0]
+        if pc.min() < 0 or pc.max() >= K:
+            raise TzrError("icp_multiscale: a pair names a cloud outside the list")
+        sc = [icp_scale(x) for x in scales]
+        S = len(sc)
+        if S == 0:
+            raise TzrError("icp_multiscale: at least one scale is required")
+        m = ICP_METHODS.get(method) if isinstance(method, str) else method
+        if m not in ICP_METHODS.values():
+            raise TzrError(f"icp_multiscale: unknown method {method!r} (one of {sorted(ICP_METHODS)})")
+        if m != ICP_METHODS["colored"]:
+            colors = None  # read by coloured ICP only, as the library reads them
+        elif colors is None:
+            raise TzrError("icp_multiscale: colours are required for coloured ICP")
+        if colors is not None and len(colors) != K:
+            raise TzrError("icp_multiscale: one colours array per cloud is required")
+        if inits is not None and len(inits) != P:
+            raise TzrError("icp_multiscale: one seed per pair is required")
+        kern = robust_kernel(kernel)
+        if kern is not None and m == ICP_METHODS["point_to_point"]:
+            raise TzrError("icp_multiscale: point-to-point ICP takes no robust kernel")
+        KC = None if colors is None else [_colors32(c, p.shape[0], "icp_multiscale") for c, p in zip(colors, pts)]
+        n = np.array([p.shape[0] for p in pts], dtype=np.int32)
+        init = (Similarity * P)(*[similarity(x) for x in (inits if inits is not None else [None] * P)])
+        res = (IcpResult * (P * S))()
+        n_down = np.zeros((K, S), dtype=np.int32)
+        status = np.zeros((K, S), dtype=np.int32)
+        info = np.zeros((P, 6, 6)) if information else None
+        cnt = np.zeros(P, dtype=np.int32) if information else None
+        fp = C.POINTER(C.c_float)
+        rc = lib().tzr_icp_multiscale_batch(
+            self._h, int(m), S, (IcpScale * S)(*sc), K, _p(n, C.c_int32), (fp * K)(*[_p(p, C.c_float) for p in pts]),
+            None if KC is None else (fp * K)(*[_p(c, C.c_float) for c in KC]), P, _p(pc, C.c_int32), init,
+            float(epsilon), float(lambda_geometric), C.byref(kern) if kern is not None else None, res,
+            _p(n_down, C.c_int32), _p(status, C.c_int32), None if info is None else _p(info, C.c_double),
+            None if cnt is None else _p(cnt, C.c_int32))
+        out = np.frombuffer(bytes(res), dtype=ICP_RESULT_DTYPE).copy().reshape(P, S)
+        result = (out, n_down) + ((info, cnt) if information else ())
+        try:
+            self._ck(rc)
+        except TzrError as e:
+            e.status, e.result = status, result
+            raise
+        return result
 
     def voxel_downsample(self, pts, voxel_size, return_trace=False, colors=None):
         """tzr_voxel_downsample: Open3D's voxel_down_sample of one (n,3) float32 cloud (the definition is

@@ -3106,6 +3106,290 @@ int tzr_information_matrix(tzr_ctx* ctx, const float* src, int ns, const float* 
                                       information, count);
 }
 
+// ---- multi-scale ICP (DESIGN.md §3.19) ------------------------------------------------------------------------------
+static bool icp_scale_ok(const tzr_icp_scale& sc, bool normals) {
+  return std::isfinite(sc.voxel_size) && sc.voxel_size >= 0 && std::isfinite(sc.max_correspondence_distance) &&
+         sc.max_correspondence_distance > 0 && sc.max_iteration >= 0 && !std::isnan(sc.relative_fitness) &&
+         !std::isnan(sc.relative_rmse) &&
+         (!normals || (std::isfinite(sc.normal_search_radius) && sc.normal_search_radius > 0));
+}
+
+// One scale of the schedule, planned on the host from its cloud sizes exactly as the public calls plan them
+struct IcpScalePlan {
+  std::vector<int32_t> nd;     // points of every cloud at this scale
+  FpfhPlan nplan;              // the normals pass over every cloud (tzr_estimate_normals_batch's plan)
+  std::vector<FpfhCloud> ncl;
+  IcpPlan ip;                  // ICP of the refined pairs onto the cloud table (and the gradient pass, coloured)
+  std::vector<FpfhCloud> icl, gcl;
+  std::vector<IcpProb> probs;
+  std::vector<int> chunks, pair_of, prob_of;
+};
+
+// Plans scale s over clouds of nd points (prob_of / pair_of: the pairs whose two clouds have points).  TZR_OK, or
+// TZR_ERR_TOO_LARGE when a table does not fit 32-bit indices.
+static int icp_scale_plan(const tzr_ctx* ctx, const tzr_icp_scale& sc, int method, double epsilon,
+                          double lambda_geometric, const tzr_robust_kernel* kernel, int n_clouds,
+                          const int32_t* nd, int P, const int32_t* pair_clouds, IcpScalePlan* out) {
+  const int froute = search_route(ctx->flags, kFlagFpfhBrute, kFlagFpfhGrid);
+  out->nd.assign(nd, nd + n_clouds);
+  out->ncl.resize((size_t)n_clouds);
+  if (method != kIcpPointToPoint &&
+      fpfh_plan(n_clouds, nd, sc.normal_search_radius, sc.normal_search_radius, froute, out->ncl.data(),
+                &out->nplan) != TZR_OK)
+    return TZR_ERR_TOO_LARGE;
+  std::vector<int32_t> lo((size_t)n_clouds), ns, slo, tc;
+  for (int c = 0, l = 0; c < n_clouds; l += nd[c], ++c) lo[c] = l;
+  out->prob_of.assign((size_t)P, -1);
+  out->pair_of.clear();
+  for (int p = 0; p < P; ++p) {
+    const int a = pair_clouds[2 * p], b = pair_clouds[2 * p + 1];
+    if (nd[a] < 1 || nd[b] < 1) continue;
+    out->prob_of[p] = (int)out->pair_of.size();
+    out->pair_of.push_back(p);
+    ns.push_back(nd[a]);
+    slo.push_back(lo[a]);
+    tc.push_back(b);
+  }
+  const tzr_icp_params prm{sc.max_correspondence_distance, sc.relative_fitness, sc.relative_rmse, sc.max_iteration, 0};
+  out->ip = IcpPlan{};
+  icp_iteration_settings(&out->ip, prm, method, epsilon, kernel);
+  out->ip.lambda_geometric = lambda_geometric;
+  if (out->pair_of.empty()) return TZR_OK;
+  if (method == kIcpColored) {  // every cloud's gradients at 2 r, as the chained coloured entries take them
+    out->ip.grad_r = 2.0 * sc.max_correspondence_distance;
+    out->gcl.resize((size_t)n_clouds);
+    if (fpfh_plan(n_clouds, nd, out->ip.grad_r, out->ip.grad_r, froute, out->gcl.data(), &out->ip.ggrid) != TZR_OK)
+      return TZR_ERR_TOO_LARGE;
+  }
+  return icp_plan((int)ns.size(), ns.data(), slo.data(), tc.data(), n_clouds, nd, sc.max_correspondence_distance,
+                  search_route(ctx->flags, kFlagIcpBrute, kFlagIcpGrid), nullptr, &out->ip, &out->icl, &out->probs,
+                  &out->chunks);
+}
+
+// Bytes of scale work in the shared region: [normals | max(normals grid, ICP workspace from its layout)]
+static size_t icp_scale_work(const IcpScalePlan& sp, int method, size_t n_points, bool information) {
+  const size_t nrm = method != kIcpPointToPoint ? al256(n_points * 16) : 0;
+  const size_t icp = sp.pair_of.empty() ? 0 : icp_layout(sp.ip, 0, information).end;
+  return nrm + std::max(method != kIcpPointToPoint ? sp.nplan.grid_bytes : 0, icp);
+}
+
+// Workspace ctx->icp: [clouds | colours | voxel tables | poses] (one upload) | per voxel scale: voxels | their colours |
+// per scale: tables (one upload) | records | normals overflow flags (one read-back) | shared scale work.  Every region
+// is sized from the dense clouds before any device work: a scale never has more points than the clouds as given, and
+// every table and grid grows with the points.
+int tzr_icp_multiscale_batch(tzr_ctx* ctx, int method, int S, const tzr_icp_scale* scales, int n_clouds,
+                             const int32_t* n, const float* const* pts, const float* const* colors, int P,
+                             const int32_t* pair_clouds, const tzr_similarity* init, double epsilon,
+                             double lambda_geometric, const tzr_robust_kernel* kernel, tzr_icp_result* results,
+                             int32_t* n_down, int32_t* status, double* information, int32_t* info_counts) {
+  const bool normals = method != kIcpPointToPoint, colored = method == kIcpColored;
+  if (!ctx || method < kIcpPointToPoint || method > kIcpColored || S < 1 || !scales || n_clouds < 1 || !n || !pts ||
+      P < 1 || !pair_clouds || !init || !results || (colored && !colors))
+    return TZR_ERR_INVALID_ARG;
+  if ((method == kIcpPointToPoint && kernel) || (method == kIcpGeneralized && !icp_epsilon_ok(epsilon)))
+    return TZR_ERR_INVALID_ARG;
+  if (colored ? colored_args(&lambda_geometric, kernel) != TZR_OK : kernel && !robust_kernel_ok(kernel))
+    return TZR_ERR_INVALID_ARG;
+  if (!colored) lambda_geometric = 0.0;
+  for (int s = 0; s < S; ++s)
+    if (!icp_scale_ok(scales[s], normals)) return TZR_ERR_INVALID_ARG;
+  for (int c = 0; c < n_clouds; ++c)
+    if (n[c] < 1 || !pts[c] || (colored && !colors[c])) return TZR_ERR_INVALID_ARG;
+  for (int p = 0; p < P; ++p) {
+    const int a = pair_clouds[2 * p], b = pair_clouds[2 * p + 1];
+    if (a < 0 || a >= n_clouds || b < 0 || b >= n_clouds || !similarity_ok(init[p])) return TZR_ERR_INVALID_ARG;
+  }
+  std::vector<VoxCloud> vt0((size_t)n_clouds);
+  VoxPlan vplan;
+  if (voxel_plan(n_clouds, n, vt0.data(), &vplan) != TZR_OK) {
+    ctx->last_error = "the clouds' points do not fit 32-bit indices";
+    return TZR_ERR_TOO_LARGE;
+  }
+  std::vector<int> vox((size_t)S, -1);  // the voxel output slot of every scale, -1: the clouds as given
+  int SV = 0;
+  for (int s = 0; s < S; ++s)
+    if (scales[s].voxel_size > 0) vox[s] = SV++;
+  // the bounds: every scale planned at the dense sizes
+  const size_t N = (size_t)vplan.N, C = (size_t)n_clouds;
+  const bool want_info = information || info_counts;  // either output alone runs the information pass
+  size_t work = al256(vplan.scratch_bytes) + N * 4, max_chunks = 0;
+  IcpScalePlan sp;
+  for (int s = 0; s < S; ++s) {
+    if (icp_scale_plan(ctx, scales[s], method, epsilon, lambda_geometric, kernel, n_clouds, n, P, pair_clouds, &sp) !=
+        TZR_OK) {
+      ctx->last_error = "the clouds' points or grids do not fit 32-bit indices";
+      return TZR_ERR_TOO_LARGE;
+    }
+    work = std::max(work, icp_scale_work(sp, method, N, want_info));
+    max_chunks = std::max(max_chunks, sp.chunks.size());
+  }
+  // one scale's tables: [problems | ICP cloud table | chunks | normals cloud table | gradient cloud table | pair_of |
+  // prob_of]
+  const size_t t_icl = al256((size_t)P * sizeof(IcpProb)), t_chk = t_icl + al256(C * sizeof(FpfhCloud)),
+               t_ncl = t_chk + al256(max_chunks * 4), t_gcl = t_ncl + al256(C * sizeof(FpfhCloud)),
+               t_pair = t_gcl + al256(C * sizeof(FpfhCloud)), t_prob = t_pair + al256((size_t)P * 4),
+               tab = al256(t_prob + (size_t)P * 4);
+  const size_t o_col = al256(N * 12), o_vtab = o_col + al256(colored ? N * 12 : 0),
+               o_pose = o_vtab + al256((size_t)SV * C * sizeof(VoxCloud)),
+               in_bytes = o_pose + (size_t)P * sizeof(tzr_similarity), o_vout = al256(in_bytes),
+               o_vcol = o_vout + al256((size_t)SV * N * 12), o_tab = o_vcol + al256(colored ? (size_t)SV * N * 12 : 0),
+               o_rec = o_tab + (size_t)S * tab, o_ovf = o_rec + al256((size_t)P * S * sizeof(tzr_icp_result)),
+               out_bytes = o_ovf + (size_t)S * C * 4 - o_rec, o_work = al256(o_rec + out_bytes);
+  // pinned: [upload | tables], host writes that may overlap the copies in flight; then [records | overflow flags |
+  // information | counts], read back once every copy before them has run
+  const size_t h_tab = al256(in_bytes), h_info = al256(out_bytes), h_cnt = h_info + al256((size_t)P * 36 * 8),
+               pin = std::max(h_tab + (size_t)S * tab, h_cnt + (size_t)P * 4);
+  int rc;
+  cudaSetDevice(ctx->device);
+  cudaStream_t st = ctx->stream;
+  if ((rc = ensure(ctx, ctx->icp, o_work + work)) != TZR_OK) return rc;
+  if ((rc = ensure_pinned(ctx, pin)) != TZR_OK) return rc;
+  char* h = (char*)ctx->h_pin;
+  char* d = (char*)ctx->icp.p;
+  std::vector<CopySpan> spans;
+  for (int c = 0; c < n_clouds; ++c) {
+    spans.push_back(CopySpan{h + (size_t)vt0[c].lo * 12, pts[c], (size_t)n[c] * 12});
+    if (colored) spans.push_back(CopySpan{h + o_col + (size_t)vt0[c].lo * 12, colors[c], (size_t)n[c] * 12});
+  }
+  for (int v = 0; v < SV; ++v)
+    spans.push_back(CopySpan{h + o_vtab + (size_t)v * C * sizeof(VoxCloud), vt0.data(), C * sizeof(VoxCloud)});
+  spans.push_back(CopySpan{h + o_pose, init, (size_t)P * sizeof(tzr_similarity)});
+  CK(stage_in(spans, h, d, o_vtab, in_bytes, false, st));
+  const float* d_pts = (const float*)d;
+  const float* d_col = colored ? (const float*)(d + o_col) : nullptr;
+  VoxCloud* d_vtab = (VoxCloud*)(d + o_vtab);
+  tzr_similarity* d_pose = (tzr_similarity*)(d + o_pose);
+  char* d_work = d + o_work;
+  for (int s = 0; s < S; ++s)
+    if (vox[s] >= 0)
+      ctx->launches += launch_voxel(vplan, scales[s].voxel_size, d_pts, d_vtab + (size_t)vox[s] * C, d_work,
+                                    (float*)(d + o_vout) + (size_t)vox[s] * N * 3, (int*)(d_work + al256(vplan.scratch_bytes)),
+                                    st, d_col, colored ? (float*)(d + o_vcol) + (size_t)vox[s] * N * 3 : nullptr);
+  if ((rc = check_launch(ctx, "multi-scale voxel launch")) != TZR_OK) return rc;
+  // synchronisation 1 (with a voxel scale): every scale's cloud sizes
+  std::vector<VoxCloud> vt((size_t)SV * C);
+  if (SV > 0) {
+    CK(cudaMemcpyAsync(vt.data(), d_vtab, vt.size() * sizeof(VoxCloud), cudaMemcpyDeviceToHost, st));
+    CK(cudaStreamSynchronize(st));
+  }
+  std::vector<int32_t> nd(C * S);  // cloud-major, as n_down
+  bool grid_too_large = false;
+  for (int c = 0; c < n_clouds; ++c)
+    for (int s = 0; s < S; ++s) {
+      const VoxCloud* v = vox[s] >= 0 ? &vt[(size_t)vox[s] * C + c] : nullptr;
+      nd[(size_t)c * S + s] = v ? v->n_out : n[c];
+      if (n_down) n_down[(size_t)c * S + s] = nd[(size_t)c * S + s];
+      if (status) status[(size_t)c * S + s] = v ? v->status : TZR_OK;
+      grid_too_large |= v && v->status != TZR_OK;
+    }
+  if (grid_too_large) {
+    memset(results, 0, (size_t)P * S * sizeof(tzr_icp_result));
+    if (information) memset(information, 0, (size_t)P * 36 * 8);
+    if (info_counts) memset(info_counts, 0, (size_t)P * 4);
+    ctx->last_error = "a cloud's voxel grid is too large for a scale's voxel size (Open3D's INT_MAX check or 2^62 cells)";
+    return TZR_ERR_TOO_LARGE;
+  }
+  // every scale planned from its sizes, its tables staged in one upload
+  std::vector<IcpScalePlan> plans((size_t)S);
+  std::vector<int32_t> nds((size_t)n_clouds);
+  for (int s = 0; s < S; ++s) {
+    for (int c = 0; c < n_clouds; ++c) nds[c] = nd[(size_t)c * S + s];
+    IcpScalePlan& q = plans[s];
+    if (icp_scale_plan(ctx, scales[s], method, epsilon, lambda_geometric, kernel, n_clouds, nds.data(), P,
+                       pair_clouds, &q) != TZR_OK ||
+        q.chunks.size() > max_chunks || icp_scale_work(q, method, N, want_info) > work) {
+      ctx->last_error = "a scale's plan exceeds the workspace sized from the clouds as given";
+      return TZR_ERR_TOO_LARGE;
+    }
+    char* t = h + h_tab + (size_t)s * tab;
+    memcpy(t, q.probs.data(), q.probs.size() * sizeof(IcpProb));
+    if (!q.pair_of.empty()) memcpy(t + t_icl, q.icl.data(), C * sizeof(FpfhCloud));
+    memcpy(t + t_chk, q.chunks.data(), q.chunks.size() * 4);
+    if (normals) memcpy(t + t_ncl, q.ncl.data(), C * sizeof(FpfhCloud));
+    if (!q.gcl.empty()) memcpy(t + t_gcl, q.gcl.data(), C * sizeof(FpfhCloud));
+    memcpy(t + t_pair, q.pair_of.data(), q.pair_of.size() * 4);
+    memcpy(t + t_prob, q.prob_of.data(), (size_t)P * 4);
+  }
+  CK(cudaMemcpyAsync(d + o_tab, h + h_tab, (size_t)S * tab, cudaMemcpyHostToDevice, st));
+  // every scale enqueued: normals, pose load, ICP (with the gradient pass), pose store; the information at the end
+  float4* d_nrm = (float4*)d_work;
+  char* d_scr = d_work + (normals ? al256(N * 16) : 0);
+  tzr_icp_result* d_rec = (tzr_icp_result*)(d + o_rec);
+  IcpBuffers last{};
+  for (int s = 0; s < S; ++s) {
+    const IcpScalePlan& q = plans[s];
+    char* t = d + o_tab + (size_t)s * tab;
+    const float* sp_pts = vox[s] >= 0 ? (const float*)(d + o_vout) + (size_t)vox[s] * N * 3 : d_pts;
+    const float* sp_col = !colored ? nullptr : vox[s] >= 0 ? (const float*)(d + o_vcol) + (size_t)vox[s] * N * 3 : d_col;
+    if (normals && q.nplan.N > 0)
+      ctx->launches += launch_fpfh(q.nplan, sp_pts, (FpfhCloud*)(t + t_ncl), scales[s].normal_search_radius,
+                                   scales[s].normal_search_radius, d_nrm, nullptr, nullptr,
+                                   (int*)(d + o_ovf) + (size_t)s * C, q.nplan.grid_bytes ? d_scr : nullptr, st);
+    const int B = (int)q.pair_of.size();
+    const bool info_here = want_info && s == S - 1 && B > 0;
+    IcpBuffers buf{};
+    IcpGrid grid{nullptr, nullptr, nullptr};
+    if (B > 0) {
+      buf = icp_buffers(d_scr, icp_layout(q.ip, 0, info_here));
+      buf.probs = (IcpProb*)t;
+      buf.clouds = (FpfhCloud*)(t + t_icl);
+      buf.chunk_prob = (const int*)(t + t_chk);
+      buf.src = buf.dst = sp_pts;
+      if (normals) buf.src_normals = buf.dst_normals = d_nrm;
+      if (colored) {
+        buf.src_colors = buf.dst_colors = sp_col;
+        buf.gclouds = (FpfhCloud*)(t + t_gcl);
+      }
+      ctx->launches += launch_icp_pose_load(buf.probs, B, (const int*)(t + t_pair), d_pose, st);
+      ctx->launches += launch_icp(q.ip, buf, st, &grid);
+    }
+    ctx->launches += launch_icp_pose_store(B > 0 ? buf.probs : nullptr, P, (const int*)(t + t_prob), d_pose, d_rec + s,
+                                           S, st);
+    if (info_here) {
+      ctx->launches += launch_icp_information(q.ip, buf, true, st, &grid);
+      last = buf;
+    }
+    if ((rc = check_launch(ctx, "multi-scale icp launch")) != TZR_OK) return rc;
+  }
+  // synchronisation 2: the records, the overflow flags and the information matrices
+  const IcpScalePlan& ql = plans[S - 1];
+  const int BL = (int)ql.pair_of.size();
+  CK(cudaMemcpyAsync(h, d + o_rec, out_bytes, cudaMemcpyDeviceToHost, st));
+  if (last.info) {
+    CK(cudaMemcpyAsync(h + h_info, last.info, (size_t)BL * 36 * 8, cudaMemcpyDeviceToHost, st));
+    CK(cudaMemcpyAsync(h + h_cnt, last.counts, (size_t)BL * 4, cudaMemcpyDeviceToHost, st));
+  }
+  CK(cudaStreamSynchronize(st));
+  memcpy(results, h, (size_t)P * S * sizeof(tzr_icp_result));
+  const int* ovf = (const int*)(h + (o_ovf - o_rec));
+  std::vector<int> first_bad((size_t)n_clouds, S);  // the first scale at which the cloud's normals overflowed
+  bool overflow = false;
+  for (int s = 0; s < S; ++s) {
+    if (!normals || plans[s].nplan.N == 0) continue;
+    for (int c = 0; c < n_clouds; ++c)
+      if (ovf[(size_t)s * C + c]) {
+        if (status) status[(size_t)c * S + s] = TZR_ERR_TOO_LARGE;
+        first_bad[c] = std::min(first_bad[c], s);
+        overflow = true;
+      }
+  }
+  if (information) memset(information, 0, (size_t)P * 36 * 8);
+  if (info_counts) memset(info_counts, 0, (size_t)P * 4);
+  for (int p = 0; p < P; ++p) {
+    const int s0 = std::min(first_bad[pair_clouds[2 * p]], first_bad[pair_clouds[2 * p + 1]]);
+    for (int s = s0; s < S; ++s) memset(&results[(size_t)p * S + s], 0, sizeof(tzr_icp_result));
+    const int k = ql.prob_of[p];
+    if (!last.info || k < 0 || s0 < S) continue;
+    if (information) memcpy(information + (size_t)p * 36, h + h_info + (size_t)k * 36 * 8, 36 * 8);
+    if (info_counts) info_counts[p] = ((const int*)(h + h_cnt))[k];
+  }
+  if (overflow) {
+    ctx->last_error = "a cloud has a point with more than 4096 neighbours inside a scale's normal radius";
+    return TZR_ERR_TOO_LARGE;
+  }
+  return TZR_OK;
+}
+
 void tzr_pose_graph_params_default(tzr_pose_graph_params* p) {
   if (!p) return;
   memset(p, 0, sizeof(*p));

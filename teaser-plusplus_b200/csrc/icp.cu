@@ -791,7 +791,59 @@ __global__ void icp_info_seed_kernel(IcpProb* probs, int B) {
   if (b < B) probs[b].active = probs[b].seeded;
 }
 
+// ---- multi-scale schedule (DESIGN.md §3.19) ---------------------------------------------------------------------------
+// Problem b of a scale starts from the pose of its pair pair_of[b]: the seed, or the pair's transform after the previous
+// scale.  Sets active = seeded = 1.
+__global__ void icp_pose_load_kernel(IcpProb* probs, int B, const int* __restrict__ pair_of,
+                                     const tzr_similarity* __restrict__ pose) {
+  const int b = blockIdx.x * blockDim.x + threadIdx.x;
+  if (b >= B) return;
+  const tzr_similarity& x = pose[pair_of[b]];
+  IcpProb& pr = probs[b];
+  pr.active = pr.seeded = 1;
+  pr.s = x.scale;
+  for (int k = 0; k < 9; ++k) pr.R[k] = x.rotation[k];
+  for (int k = 0; k < 3; ++k) pr.t[k] = x.translation[k];
+}
+
+// Pair p's record of a scale at rec[p * stride]: a refined pair (prob_of[p] >= 0) gets its problem's result, whose
+// transform also becomes the pair's pose; any other pair carries its pose with every other field 0
+__global__ void icp_pose_store_kernel(const IcpProb* __restrict__ probs, int P, const int* __restrict__ prob_of,
+                                      tzr_similarity* __restrict__ pose, tzr_icp_result* __restrict__ rec, int stride) {
+  const int p = blockIdx.x * blockDim.x + threadIdx.x;
+  if (p >= P) return;
+  tzr_similarity& x = pose[p];
+  tzr_icp_result r;
+  r.fitness = r.inlier_rmse = 0.0;
+  r.iterations = r.n_correspondences = r.converged = r.reserved = 0;
+  const int k = prob_of[p];
+  if (k >= 0) {
+    const IcpProb& pr = probs[k];
+    x.scale = pr.s;
+    for (int q = 0; q < 9; ++q) x.rotation[q] = pr.R[q];
+    for (int q = 0; q < 3; ++q) x.translation[q] = pr.t[q];
+    r.fitness = pr.fitness;
+    r.inlier_rmse = pr.rmse;
+    r.iterations = pr.iterations;
+    r.n_correspondences = pr.count;
+    r.converged = pr.converged;
+  }
+  r.transform = x;
+  rec[(size_t)p * stride] = r;
+}
+
 }  // namespace
+
+int launch_icp_pose_load(IcpProb* probs, int B, const int* pair_of, const tzr_similarity* pose, cudaStream_t st) {
+  icp_pose_load_kernel<<<(B + 127) / 128, 128, 0, st>>>(probs, B, pair_of, pose);
+  return 1;
+}
+
+int launch_icp_pose_store(const IcpProb* probs, int P, const int* prob_of, tzr_similarity* pose, tzr_icp_result* rec,
+                          int stride, cudaStream_t st) {
+  icp_pose_store_kernel<<<(P + 127) / 128, 128, 0, st>>>(probs, P, prob_of, pose, rec, stride);
+  return 1;
+}
 
 int icp_plan(int B, const int32_t* ns, const int32_t* s_lo, const int32_t* tc, int T, const int32_t* nt, double r,
              int route, const tzr_similarity* init, IcpPlan* plan, std::vector<FpfhCloud>* clouds,

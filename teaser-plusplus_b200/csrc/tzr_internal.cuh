@@ -617,6 +617,13 @@ int launch_icp_seed(IcpProb* probs, int B, const tzr_solution* sol, cudaStream_t
 // grid is nullptr.
 int launch_icp_information(const IcpPlan& plan, const IcpBuffers& buf, bool reseed, cudaStream_t st,
                            const IcpGrid* grid = nullptr);
+// The multi-scale schedule (tzr_icp_multiscale_batch, DESIGN.md §3.19), around launch_icp at every scale.  Load: problem
+// b of B takes the pose of pair pair_of[b] (P poses, device) and becomes active and seeded.  Store: for each of the P
+// pairs, prob_of[p] >= 0 writes that problem's result to rec[p * stride] and its transform to pose[p]; -1 writes the
+// pose with every other field 0 (probs may then be nullptr when no pair is refined).  One launch each.
+int launch_icp_pose_load(IcpProb* probs, int B, const int* pair_of, const tzr_similarity* pose, cudaStream_t st);
+int launch_icp_pose_store(const IcpProb* probs, int P, const int* prob_of, tzr_similarity* pose, tzr_icp_result* rec,
+                          int stride, cudaStream_t st);
 
 // pose_graph.cu (tzr_pose_graph_optimize, DESIGN.md §3.16): one graph of K nodes and E edges, device-resident
 struct PgEdge {         // one per edge; the host fills it, the kernels read it

@@ -12,10 +12,10 @@ from . import _teaserpp as _ext
 
 # ---- re-exports -----------------------------------------------------------------------------------------------------
 _PUBLIC = ("OMP_MAX_THREADS", "CertificationResult", "ColoredICP", "DRSCertifier", "EigSolverType", "GeneralizedICP",
-           "InlierGraphFormulation", "InlierSelectionMode", "PointToPlaneICP", "PointToPointICP", "PoseGraph",
+           "InlierGraphFormulation", "InlierSelectionMode", "MultiScaleICP", "PointToPlaneICP", "PointToPointICP", "PoseGraph",
            "RegistrationSolution", "RobustKernel", "RobustRegistrationSolver", "RotationEstimationAlgorithm",
            "estimate_color_gradients", "estimate_color_gradients_batch", "estimate_normals",
-           "estimate_normals_batch", "information_matrix", "information_matrix_batch", "voxel_down_sample",
+           "estimate_normals_batch", "information_matrix", "information_matrix_batch", "multiscale_icp", "voxel_down_sample",
            "voxel_down_sample_batch")
 globals().update({name: getattr(_ext, name) for name in _PUBLIC})
 

@@ -139,6 +139,77 @@ py::array_t<double> square_to_numpy(const Eigen::Matrix<double, N, N>& M) {
 }
 using SqArr = py::array_t<double, py::array::c_style | py::array::forcecast>;
 
+// MultiScaleICP's scales from Python: (voxel_size, max_correspondence_distance, max_iteration[, normal_search_radius[,
+// relative_fitness[, relative_rmse]]]) tuples or dicts with those keys; the normal radius defaults to 2 voxel_size
+std::vector<teaser::ICPScale> scales_of(const py::list& scales) {
+  static const char* keys[] = {"voxel_size", "max_correspondence_distance", "max_iteration", "normal_search_radius",
+                               "relative_fitness", "relative_rmse"};
+  std::vector<teaser::ICPScale> out;
+  for (const py::handle& h : scales) {
+    std::vector<py::object> v(6);
+    if (py::isinstance<py::dict>(h)) {
+      const py::dict d = py::reinterpret_borrow<py::dict>(h);
+      for (auto kv : d) {
+        const std::string k = py::str(kv.first);
+        int i = 0;
+        while (i < 6 && k != keys[i]) ++i;
+        if (i == 6) throw std::invalid_argument("MultiScaleICP: unknown scale field " + k);
+        v[i] = py::reinterpret_borrow<py::object>(kv.second);
+      }
+    } else {
+      const py::sequence q = py::reinterpret_borrow<py::sequence>(h);
+      if (q.size() > 6) throw std::invalid_argument("MultiScaleICP: a scale tuple has at most 6 entries");
+      for (size_t i = 0; i < q.size(); ++i) v[i] = q[i];
+    }
+    for (int i = 0; i < 3; ++i)
+      if (!v[i]) throw std::invalid_argument(std::string("MultiScaleICP: a scale needs ") + keys[i]);
+    teaser::ICPScale sc(v[0].cast<double>(), v[1].cast<double>(), v[2].cast<int>());
+    if (v[3]) sc.normal_search_radius = v[3].cast<double>();
+    if (v[4]) sc.relative_fitness = v[4].cast<double>();
+    if (v[5]) sc.relative_rmse = v[5].cast<double>();
+    out.push_back(sc);
+  }
+  return out;
+}
+
+teaser::MultiScaleICP::Method method_of(const std::string& m) {
+  if (m == "point_to_point") return teaser::MultiScaleICP::kPointToPoint;
+  if (m == "point_to_plane") return teaser::MultiScaleICP::kPointToPlane;
+  if (m == "generalized") return teaser::MultiScaleICP::kGeneralized;
+  if (m == "colored") return teaser::MultiScaleICP::kColored;
+  throw std::invalid_argument("MultiScaleICP: unknown method " + m);
+}
+
+py::dict multiscale_dict(const teaser::MultiScaleICP::Result& r) {
+  py::list records, info;
+  for (const auto& pr : r.records) {
+    py::list row;
+    for (const auto& x : pr) row.append(icp_dict(x));
+    records.append(row);
+  }
+  for (const auto& M : r.information) info.append(square_to_numpy<6>(M));
+  return py::dict(py::arg("records") = records, py::arg("n_down") = r.n_down, py::arg("status") = r.status,
+                  py::arg("too_large") = r.too_large, py::arg("information") = info,
+                  py::arg("info_counts") = r.info_counts);
+}
+
+py::dict multiscale_run(const teaser::MultiScaleICP& icp, const std::vector<CloudArray>& clouds,
+                        const std::vector<std::pair<int, int>>& pairs,
+                        const std::vector<teaser::RegistrationSolution>& init, const py::object& colors,
+                        bool information) {
+  std::vector<teaser::PointCloud> pcs;
+  std::vector<teaser::ColorCloud> ccs;
+  for (const auto& a : clouds) pcs.push_back(cloud_of(a));
+  if (!colors.is_none())
+    for (const auto& a : colors.cast<std::vector<CloudArray>>()) ccs.push_back(colors_of(a));
+  teaser::MultiScaleICP::Result r;
+  {
+    py::gil_scoped_release release;
+    r = icp.refineBatch(pcs, ccs, pairs, init, information);
+  }
+  return multiscale_dict(r);
+}
+
 }  // namespace
 
 PYBIND11_MODULE(_teaserpp, m) {
@@ -464,6 +535,41 @@ PYBIND11_MODULE(_teaserpp, m) {
            },
            py::arg("src"), py::arg("dst"), py::arg("dst_normals"), py::arg("src_colors"), py::arg("dst_colors"),
            py::arg("init"));
+
+  // GPU extra: multi-scale ICP (teaser::MultiScaleICP) over a cloud table; refine_batch returns a dict: records
+  // (per pair, per scale, icp dicts without correspondences), n_down and status (per cloud, per scale), too_large, and
+  // with information the last scale's information matrices and counts
+  py::class_<teaser::MultiScaleICP>(m, "MultiScaleICP")
+      .def(py::init([](const py::list& scales, const std::string& method, double lambda_geometric, double epsilon,
+                       const teaser::RobustKernel& kernel) {
+             teaser::MultiScaleICP::Params p;
+             p.scales = scales_of(scales);
+             p.method = method_of(method);
+             p.lambda_geometric = lambda_geometric;
+             p.epsilon = epsilon;
+             p.kernel = kernel;
+             return teaser::MultiScaleICP(p);
+           }),
+           py::arg("scales"), py::arg("method") = "point_to_plane", py::arg("lambda_geometric") = 0.968,
+           py::arg("epsilon") = 1e-3, py::arg("kernel") = teaser::RobustKernel())
+      .def("refine_batch", &multiscale_run, py::arg("clouds"), py::arg("pairs"), py::arg("init"),
+           py::arg("colors") = py::none(), py::arg("information") = false);
+  m.def(
+      "multiscale_icp",
+      [](const std::vector<CloudArray>& clouds, const std::vector<std::pair<int, int>>& pairs, const py::list& scales,
+         const std::vector<teaser::RegistrationSolution>& init, const std::string& method, const py::object& colors,
+         double lambda_geometric, double epsilon, const teaser::RobustKernel& kernel, bool information) {
+        teaser::MultiScaleICP::Params p;
+        p.scales = scales_of(scales);
+        p.method = method_of(method);
+        p.lambda_geometric = lambda_geometric;
+        p.epsilon = epsilon;
+        p.kernel = kernel;
+        return multiscale_run(teaser::MultiScaleICP(p), clouds, pairs, init, colors, information);
+      },
+      py::arg("clouds"), py::arg("pairs"), py::arg("scales"), py::arg("init"), py::arg("method") = "point_to_plane",
+      py::arg("colors") = py::none(), py::arg("lambda_geometric") = 0.968, py::arg("epsilon") = 1e-3,
+      py::arg("kernel") = teaser::RobustKernel(), py::arg("information") = false);
 
   // GPU extra: coloured ICP's colour gradients (teaser::estimateColorGradients), as (n,3) float64
   m.def("estimate_color_gradients",

@@ -227,4 +227,79 @@ std::vector<ColoredICP::Result> ColoredICP::refineBatch(const std::vector<PointC
   return out;
 }
 
+MultiScaleICP::Result MultiScaleICP::refineBatch(const std::vector<PointCloud>& clouds,
+                                                 const std::vector<ColorCloud>& colors,
+                                                 const std::vector<std::pair<int, int>>& pairs,
+                                                 const std::vector<RegistrationSolution>& init,
+                                                 bool information) const {
+  const size_t K = clouds.size(), P = pairs.size(), S = params_.scales.size();
+  const bool colored = params_.method == kColored;
+  if (init.size() != P) throw std::invalid_argument("MultiScaleICP: one seed per pair");
+  if (colored && colors.size() != K) throw std::invalid_argument("MultiScaleICP: one colour cloud per cloud");
+  static_assert(sizeof(ColorRGB) == 3 * sizeof(float), "ColorRGB must be three packed floats");
+  std::vector<int32_t> n(K), pc(2 * P);
+  std::vector<const float*> pts(K), cols(colored ? K : 0);
+  for (size_t c = 0; c < K; ++c) {
+    if (clouds[c].empty()) throw std::invalid_argument("MultiScaleICP: clouds must be non-empty");
+    if (colored && colors[c].size() != clouds[c].size())
+      throw std::invalid_argument("MultiScaleICP: one colour per point");
+    n[c] = static_cast<int32_t>(clouds[c].size());
+    pts[c] = &clouds[c][0].x;
+    if (colored) cols[c] = &colors[c][0].r;
+  }
+  std::vector<tzr_similarity> seeds(P);
+  for (size_t p = 0; p < P; ++p) {
+    pc[2 * p] = pairs[p].first;
+    pc[2 * p + 1] = pairs[p].second;
+    seeds[p] = to_c(init[p]);
+  }
+  std::vector<tzr_icp_scale> sc(S);
+  for (size_t s = 0; s < S; ++s) {
+    const ICPScale& x = params_.scales[s];
+    sc[s] = tzr_icp_scale{x.voxel_size, x.max_correspondence_distance, x.normal_search_radius, x.relative_fitness,
+                          x.relative_rmse, x.max_iteration, 0};
+  }
+  tzr_robust_kernel k;
+  std::memset(&k, 0, sizeof(k));
+  k.type = static_cast<int32_t>(params_.kernel.type);
+  k.k = params_.kernel.k;
+  const tzr_robust_kernel* kp = params_.kernel.type == RobustKernel::kL2 ? nullptr : &k;
+  std::vector<tzr_icp_result> res(P * S);
+  std::vector<int32_t> nd(K * S), st(K * S), cnt(information ? P : 0);
+  std::vector<double> info(information ? 36 * P : 0);
+  tzr_ctx* ctx = b200_context();
+  const int rc = tzr_icp_multiscale_batch(
+      ctx, static_cast<int>(params_.method), static_cast<int>(S), sc.data(), static_cast<int>(K), n.data(),
+      pts.data(), colored ? cols.data() : nullptr, static_cast<int>(P), pc.data(), seeds.data(), params_.epsilon,
+      params_.lambda_geometric, kp, res.data(), nd.data(), st.data(), information ? info.data() : nullptr,
+      information ? cnt.data() : nullptr);
+  if (rc != TZR_OK && rc != TZR_ERR_TOO_LARGE)
+    throw std::runtime_error(std::string("MultiScaleICP: ") + tzr_status_string(rc) + " (" + tzr_last_error(ctx) +
+                             ")");
+  Result out;
+  out.too_large = rc == TZR_ERR_TOO_LARGE;
+  out.records.assign(P, std::vector<PointToPointICPResult>(S));
+  for (size_t p = 0; p < P; ++p)
+    for (size_t s = 0; s < S; ++s) {
+      const tzr_icp_result& r = res[p * S + s];
+      icp_result_from_c(r, nullptr, &out.records[p][s]);
+      out.records[p][s].solution.valid = r.transform.scale != 0;
+    }
+  out.n_down.assign(K, std::vector<int>(S));
+  out.status.assign(K, std::vector<int>(S));
+  for (size_t c = 0; c < K; ++c)
+    for (size_t s = 0; s < S; ++s) {
+      out.n_down[c][s] = nd[c * S + s];
+      out.status[c][s] = st[c * S + s];
+    }
+  if (information) {
+    out.information.resize(P);
+    for (size_t p = 0; p < P; ++p)
+      for (int r = 0; r < 6; ++r)
+        for (int c = 0; c < 6; ++c) out.information[p](r, c) = info[36 * p + 6 * r + c];
+    out.info_counts.assign(cnt.begin(), cnt.end());
+  }
+  return out;
+}
+
 }  // namespace teaser
