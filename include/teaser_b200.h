@@ -979,6 +979,88 @@ int tzr_icp_multiscale_batch(tzr_ctx* ctx, int method, int S, const tzr_icp_scal
                              double lambda_geometric, const tzr_robust_kernel* kernel, tzr_icp_result* results,
                              int32_t* n_down, int32_t* status, double* information, int32_t* info_counts);
 
+/* ---- global registration: Fast Global Registration ----------------------------------------------------------------
+ * Zhou, Park and Koltun's FGR (ECCV 2016) as Open3D's registration_fgr_based_on_correspondence runs it, for many problems
+ * at once, defined here as follows (DESIGN.md §3.20).  Every expression is IEEE float64 with no FMA contraction.
+ *   - Inputs: source x (ns float xyz), target y (nd float xyz), both read exactly as float64, and K correspondences
+ *     (i_k, j_k) (source index, target index).  Duplicated rows are kept and count once each.  A point is finite when its
+ *     three coordinates are.
+ *   - Normalisation (Open3D's NormalizePointCloud): mu_s, mu_t the means of the finite points of each whole cloud, each
+ *     component the sum over the cloud divided by the count; sigma the largest ||x - mu_s|| or ||y - mu_t|| over the
+ *     finite points of both clouds, ||d|| = sqrt((d0 d0 + d1 d1) + d2 d2).  use_absolute_scale = 0: scale_global =
+ *     sigma (1 when sigma = 0, every finite point at its mean) and mu_start = 1; = 1: scale_global = 1 and mu_start =
+ *     sigma.  The optimiser sees p = (x_i - mu_s) / scale_global and q = (y_j - mu_t) / scale_global, per component.  A
+ *     correspondence with a non-finite end is dropped (Open3D would carry the NaN through everything); the remaining
+ *     K' keep their input order.  Sums run in one fixed order that depends only on the cloud: thread l of 256 sums points
+ *     l, l + 256, ... in ascending order, then a butterfly inside each warp of 32 and the 8 warp sums in warp order.
+ *   - Optimiser (Open3D's OptimizePairwise): T = (R, t) = I, mu = mu_start.  For itr in [0, iteration_number): when
+ *     decrease_mu is set, itr % 4 == 0 and mu > maximum_correspondence_distance, mu = mu / division_factor (Open3D
+ *     compares mu with a distance; kept).  Each correspondence k takes q' = R q + t from the original q and the current
+ *     T, row r ((R(r,0) q0 + R(r,1) q1) + R(r,2) q2) + t(r), r = p - q', w = mu / (((r0 r0 + r1 r1) + r2 r2) + mu), w =
+ *     w w, and adds three rows with weight w (the robust point-to-plane rows' terms: (w J_a) J_b to the 21 entries of the
+ *     upper triangle of A, row by row, and (w J_a) r_row to g):
+ *       x: J = (0, -q'2, q'1, -1, 0, 0), r0;  y: J = (q'2, 0, -q'0, 0, -1, 0), r1;  z: J = (-q'1, q'0, 0, 0, 0, -1), r2.
+ *     The sums run in the order of the normalisation's, over the K' rows (thread l of 256 takes rows l, l + 256, ...,
+ *     each row's x, y, z terms in that order).  xi solves A xi = -g by tzr_icp_point_to_plane's 6 x 6 solve.  Delta R =
+ *     Rz(xi2) Ry(xi1) Rx(xi0), written out as tzr_icp_point_to_plane's R_u; R <- Delta R R, t <- Delta R t + (xi3, xi4,
+ *     xi5), each entry as ((a b + c d) + e f) (+ xi).  A step whose xi has a non-finite component leaves T unchanged.
+ *   - Back to the input frame (Open3D's GetTransformationOriginalScale, then its inverse): T maps the normalised target
+ *     onto the normalised source; in the input frame it is R and t' = (-(R mu_t) + scale_global t) + mu_s.  The result
+ *     maps the source onto the target: rotation R^T and translation -(R^T t'), the exact rigid inverse (Open3D takes a
+ *     general 4 x 4 inverse).
+ *   - Fallback: K' < 10, or iteration_number = 0: the result is the identity, iterations = 0 and converged = 0 (this
+ *     project's choice; Open3D is not matched there).
+ *   - Evaluation (Open3D's evaluate_registration): fitness, inlier_rmse, n_correspondences and eval_corr are bit for bit
+ *     tzr_icp_batch's with max_iteration = 0 and max_correspondence_distance = maximum_correspondence_distance, seeded
+ *     with the result.  Open3D uses the one distance both as the mu stop (normalised units) and here (input units); kept.
+ * Result (tzr_icp_result, which seeds tzr_icp_batch directly): transform (scale 1, R, t), the evaluation, iterations
+ * (iteration_number, or 0 for the fallback) and converged (1 when the optimiser ran, 0 for the fallback).
+ * Launches: 4 (the normalisation, the optimiser, the evaluation's search and its combination), + 4 for the evaluation's
+ * grid build when some target has 1024 points or more, whatever iteration_number and B.  Each problem's iterations
+ * run inside one CTA of one launch.  No limit on K: the sums of the batch's points and of its correspondences must each
+ * stay below 2^31 (TZR_ERR_TOO_LARGE otherwise); TZR_ERR_ALLOC when the workspace does not fit the device
+ * (tzr_last_error names the size).  Not a solve entry: FGR's tables have a workspace of their own and the evaluation
+ * uses tzr_icp's, so a retained solve stays retained. */
+typedef struct tzr_fgr_params {
+  double division_factor;                 /* 1.4; <= 0 or non-finite is TZR_ERR_INVALID_ARG */
+  int32_t use_absolute_scale;             /* 0 */
+  int32_t decrease_mu;                    /* 1 */
+  double maximum_correspondence_distance; /* 0.025; <= 0 or non-finite is TZR_ERR_INVALID_ARG */
+  int32_t iteration_number;               /* 64; < 0 is TZR_ERR_INVALID_ARG */
+  int32_t reserved;
+} tzr_fgr_params;
+
+/* Open3D's FastGlobalRegistrationOption defaults (the tuple test's parameters stay in tzr_frontend_params). */
+void tzr_fgr_params_default(tzr_fgr_params* p);
+
+/* B ragged problems: problem b has ns[b] >= 1 source points at src[b], nd[b] >= 1 target points at dst[b] and n_corr[b]
+ * >= 0 correspondences at corr[b] (n_corr[b] x 2 int32; may be NULL when n_corr[b] = 0).  results: B entries.
+ * eval_corr (may be NULL, or hold NULL entries; capacity ns[b] x 2 int32): the evaluation's correspondences, as
+ * tzr_icp_batch's corr.  A negative count, an index outside its cloud or a refused parameter is TZR_ERR_INVALID_ARG
+ * before any device work.  Per problem, every output is bit-identical to the same problem solved alone. */
+int tzr_fgr_batch(tzr_ctx* ctx, const tzr_fgr_params* params, int B, const int32_t* ns, const float* const* src,
+                  const int32_t* nd, const float* const* dst, const int32_t* n_corr, const int32_t* const* corr,
+                  tzr_icp_result* results, int32_t* const* eval_corr);
+
+/* One problem: tzr_fgr_batch with B = 1. */
+int tzr_fgr(tzr_ctx* ctx, const tzr_fgr_params* params, const float* src, int ns, const float* dst, int nd,
+            int n_corr, const int32_t* corr, tzr_icp_result* result, int32_t* eval_corr);
+
+/* Open3D's registration_fgr_based_on_feature_matching over a table of clouds: tzr_register_cloud_pairs' front end
+ * (FPFH of every cloud, matching of every pair; the same arguments, status rules, n_corr, corr and global_scale), then
+ * FGR of every pair with status TZR_OK on its matched rows, with no robust solve.  results: P entries, zeroed for a pair
+ * that was not registered (TZR_ERR_TOO_LARGE: a radius overflow; TZR_ERR_INVALID_ARG: no correspondence).  Each record
+ * is bit-identical to tzr_compute_fpfh_batch, then tzr_match_correspondences_batch with the same seeds, then
+ * tzr_fgr_batch on the matched rows.  The correspondences are the matcher's sorted unique rows; Open3D keeps its tuples
+ * in trial order with duplicates, caps them at maximum_tuple_count and draws them from another generator, so matched
+ * correspondences never equal Open3D's.  Two host synchronisations (the counts after matching, the results at the end).
+ * Launches: the front end's (tzr_register_cloud_pairs' without the solve), the index gather when some pair has
+ * correspondences, and tzr_fgr_batch's over the registered pairs.  Not a solve entry: a retained solve stays retained. */
+int tzr_register_cloud_pairs_fgr(tzr_ctx* ctx, const tzr_frontend_params* fparams, const tzr_fgr_params* fgr,
+                                 int n_clouds, const int32_t* n, const float* const* pts, int P,
+                                 const int32_t* pair_clouds, const uint64_t* tuple_seeds, int32_t* status,
+                                 int64_t* n_corr, int32_t* const* corr, float* global_scale, tzr_icp_result* results);
+
 /* ---- multiway registration: robust pose graph ------------------------------------------------------------------
  * The global step of Open3D's multiway registration (global_optimization over a PoseGraph), with GNC-TLS pruning the
  * uncertain edges instead of Open3D's line process.  One graph per call, defined here as follows (DESIGN.md §3.16):

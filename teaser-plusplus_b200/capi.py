@@ -163,6 +163,13 @@ class RobustKernel(C.Structure):
     _fields_ = [("type", C.c_int32), ("reserved", C.c_int32), ("k", C.c_double)]
 
 
+class FgrParams(C.Structure):
+    """tzr_fgr_params: Fast Global Registration's options (Open3D's FastGlobalRegistrationOption)."""
+    _fields_ = [("division_factor", C.c_double), ("use_absolute_scale", C.c_int32), ("decrease_mu", C.c_int32),
+                ("maximum_correspondence_distance", C.c_double), ("iteration_number", C.c_int32),
+                ("reserved", C.c_int32)]
+
+
 class PoseGraphParams(C.Structure):
     """tzr_pose_graph_params: the GNC-TLS pose graph's distance c, schedule and reference node."""
     _fields_ = [("max_correspondence_distance", C.c_double), ("gnc_factor", C.c_double),
@@ -181,6 +188,7 @@ assert C.sizeof(IcpParams) == 32, C.sizeof(IcpParams)
 assert C.sizeof(PoseGraphParams) == 40 and PoseGraphParams.reference_node.offset == 32, C.sizeof(PoseGraphParams)
 assert C.sizeof(PoseGraphSummary) == 16 and PoseGraphSummary.cost.offset == 8, C.sizeof(PoseGraphSummary)
 assert C.sizeof(IcpScale) == 48 and IcpScale.max_iteration.offset == 40, C.sizeof(IcpScale)
+assert C.sizeof(FgrParams) == 32 and FgrParams.maximum_correspondence_distance.offset == 16, C.sizeof(FgrParams)
 assert C.sizeof(RobustKernel) == 16 and RobustKernel.k.offset == 8, C.sizeof(RobustKernel)
 assert SIMILARITY_DTYPE.itemsize == C.sizeof(Similarity) == 104, C.sizeof(Similarity)
 assert ICP_RESULT_DTYPE.itemsize == C.sizeof(IcpResult) == 136, (ICP_RESULT_DTYPE.itemsize, C.sizeof(IcpResult))
@@ -208,6 +216,7 @@ _SYMBOLS = [
     "tzr_register_cloud_pairs_multiway", "tzr_estimate_color_gradients", "tzr_estimate_color_gradients_batch",
     "tzr_icp_colored", "tzr_icp_colored_batch", "tzr_voxel_downsample_colors", "tzr_voxel_downsample_colors_batch",
     "tzr_register_cloud_pairs_icp_colored", "tzr_register_cloud_pairs_multiway_colored", "tzr_icp_multiscale_batch",
+    "tzr_fgr_params_default", "tzr_fgr", "tzr_fgr_batch", "tzr_register_cloud_pairs_fgr",
 ]
 
 # status codes (tzr_status)
@@ -390,6 +399,14 @@ def lib():
     L.tzr_icp_multiscale_batch.argtypes = [vp, C.c_int, C.c_int, C.POINTER(IcpScale), C.c_int, i32p, fpp, fpp,
                                            C.c_int, i32p, C.POINTER(Similarity), C.c_double, C.c_double,
                                            C.POINTER(RobustKernel), C.POINTER(IcpResult), i32p, i32p, dp, i32p]
+    L.tzr_fgr_params_default.argtypes = [C.POINTER(FgrParams)]
+    L.tzr_fgr_params_default.restype = None
+    L.tzr_fgr.argtypes = [vp, C.POINTER(FgrParams), fp, C.c_int, fp, C.c_int, C.c_int, i32p, C.POINTER(IcpResult), i32p]
+    L.tzr_fgr_batch.argtypes = [vp, C.POINTER(FgrParams), C.c_int, i32p, fpp, i32p, fpp, i32p, C.POINTER(i32p),
+                                C.POINTER(IcpResult), C.POINTER(i32p)]
+    L.tzr_register_cloud_pairs_fgr.argtypes = [vp, C.POINTER(FrontendParams), C.POINTER(FgrParams), C.c_int, i32p, fpp,
+                                               C.c_int, i32p, u64p, i32p, i64p, C.POINTER(i32p), fp,
+                                               C.POINTER(IcpResult)]
     for s in _SYMBOLS:
         getattr(L, s)  # raises AttributeError if the header and the library disagree
     _lib = L
@@ -428,6 +445,32 @@ def pose_graph_params(max_correspondence_distance: float, **kw) -> PoseGraphPara
             raise AttributeError(k)
         setattr(p, k, v)
     return p
+
+
+def fgr_params(**kw) -> FgrParams:
+    """tzr_fgr_params_default (Open3D's FastGlobalRegistrationOption defaults) with any field in kw set; the library
+    checks the values."""
+    p = FgrParams()
+    lib().tzr_fgr_params_default(C.byref(p))
+    for k, v in kw.items():
+        if not hasattr(p, k):
+            raise AttributeError(k)
+        setattr(p, k, v)
+    return p
+
+
+def corr_rows(corr, what="fgr"):
+    """One problem's correspondences as a (K,2) int32 C-contiguous array of (source index, target index) rows: any
+    (K,2) integer array or sequence of pairs, K = 0 included.  Values outside int32 are refused here; the library checks
+    each index against its cloud."""
+    a = np.asarray(corr)
+    if a.size == 0:
+        return np.zeros((0, 2), dtype=np.int32)
+    if a.ndim != 2 or a.shape[1] != 2 or not np.issubdtype(a.dtype, np.integer):
+        raise TzrError(f"{what}: correspondences must be a (K,2) integer array")
+    if a.min() < np.iinfo(np.int32).min or a.max() > np.iinfo(np.int32).max:
+        raise TzrError(f"{what}: a correspondence index does not fit int32")
+    return np.ascontiguousarray(a, dtype=np.int32)
 
 
 def _poses(sims):
@@ -1350,6 +1393,47 @@ class Context:
             return out + (icp_res, mw)
         return out if icp is None else out + (icp_res,)
 
+    def register_cloud_pairs_fgr(self, clouds, pairs, normal_search_radius=0.03, fpfh_search_radius=0.05,
+                                 use_absolute_scale=True, use_crosscheck=True, use_tuple_test=True, tuple_scale=0.0,
+                                 tuple_seeds=None, fgr=None):
+        """tzr_register_cloud_pairs_fgr: register_cloud_pairs' front end (FPFH of every (n,3) float32 cloud, matching of
+        every (source cloud, target cloud) pair), then Fast Global Registration of every pair with correspondences on
+        its matched rows, with no robust solve.  fgr: an FgrParams (None: fgr_params()).  Returns (status (P,) int32,
+        correspondences (list of (m_p,2) int32), global scales (list of floats), FGR records (structured array (P,) of
+        ICP_RESULT_DTYPE, zeroed for a pair that was not registered)).  The call raises only for errors of the whole
+        call; TZR_ERR_TOO_LARGE of some pairs is reported in status."""
+        cl = [np.ascontiguousarray(c, dtype=np.float32) for c in clouds]
+        if not cl or any(c.ndim != 2 or c.shape[1] != 3 or c.shape[0] == 0 for c in cl):
+            raise TzrError("register_cloud_pairs_fgr: a non-empty list of non-empty (n,3) clouds is required")
+        pc = np.ascontiguousarray(pairs, dtype=np.int32).reshape(-1, 2)
+        P = pc.shape[0]
+        if P == 0:
+            raise TzrError("register_cloud_pairs_fgr: at least one pair is required")
+        if pc.min() < 0 or pc.max() >= len(cl):
+            raise TzrError("register_cloud_pairs_fgr: a pair names a cloud that is not in the list")
+        seeds = np.zeros(P, dtype=np.uint64) if tuple_seeds is None else \
+            np.ascontiguousarray([int(s) for s in tuple_seeds], dtype=np.uint64)
+        if seeds.shape != (P,):
+            raise TzrError("register_cloud_pairs_fgr: tuple_seeds needs one entry per pair")
+        fgr = fgr_params() if fgr is None else fgr
+        n = np.array([c.shape[0] for c in cl], dtype=np.int32)
+        fpar = FrontendParams(float(normal_search_radius), float(fpfh_search_radius), int(bool(use_absolute_scale)),
+                              int(bool(use_crosscheck)), int(bool(use_tuple_test)), float(tuple_scale))
+        corr = [np.zeros((int(n[a]) + int(n[b]), 2), dtype=np.int32) for a, b in pc]
+        status = np.zeros(P, dtype=np.int32)
+        cnt = np.zeros(P, dtype=np.int64)
+        g = np.zeros(P, dtype=np.float32)
+        res = np.zeros(P, dtype=ICP_RESULT_DTYPE)
+        fp, i32p = C.POINTER(C.c_float), C.POINTER(C.c_int32)
+        rc = lib().tzr_register_cloud_pairs_fgr(self._h, C.byref(fpar), C.byref(fgr), len(cl), _p(n, C.c_int32),
+                                                (fp * len(cl))(*[_p(c, C.c_float) for c in cl]), P,
+                                                _p(pc, C.c_int32), _p(seeds, C.c_uint64), _p(status, C.c_int32),
+                                                _p(cnt, C.c_int64), (i32p * P)(*[_p(c, C.c_int32) for c in corr]),
+                                                _p(g, C.c_float), res.ctypes.data_as(C.POINTER(IcpResult)))
+        if rc not in (0, TZR_ERR_TOO_LARGE):
+            self._ck(rc)
+        return status, [c[:k].copy() for c, k in zip(corr, cnt)], [float(x) for x in g], res
+
     def register_multiway(self, clouds, pairs, params: Params, max_correspondence_distance, uncertain=None,
                           normal_search_radius=0.03, fpfh_search_radius=0.05, use_absolute_scale=True,
                           use_crosscheck=True, use_tuple_test=True, tuple_scale=0.0, tuple_seeds=None, max_iteration=30,
@@ -1444,6 +1528,44 @@ class Context:
                                    max_iteration=max_iteration, relative_fitness=relative_fitness,
                                    relative_rmse=relative_rmse, single=True)
         return icp_result_dict(res[0]), corr[0]
+
+    def fgr(self, src, dst, corr, fgr=None):
+        """tzr_fgr: Fast Global Registration of the (ns,3) source onto the (nd,3) target (float32) on the (K,2)
+        correspondences corr (source index, target index).  fgr: an FgrParams (None: fgr_params()).  Returns (result
+        dict as icp_result_dict, the evaluation's correspondences (m,2) int32 ascending by source)."""
+        res, ev = self.fgr_batch([src], [dst], [corr], fgr=fgr, single=True)
+        return icp_result_dict(res[0]), ev[0]
+
+    def fgr_batch(self, srcs, dsts, corrs, fgr=None, single=False):
+        """tzr_fgr_batch over B (source, target, correspondences) problems; corrs: one (K_b,2) integer array per
+        problem (K_b = 0 allowed).  Returns (results structured array (B,) of ICP_RESULT_DTYPE, list of B evaluation
+        correspondence arrays).  single=True goes through tzr_fgr (B must be 1)."""
+        S = [_cloud32(a, "fgr") for a in srcs]
+        D = [_cloud32(a, "fgr") for a in dsts]
+        B = len(S)
+        if B == 0 or len(D) != B or len(corrs) != B:
+            raise TzrError("fgr_batch: one target and one correspondence array per source cloud are required")
+        K = [corr_rows(c, "fgr_batch") for c in corrs]
+        fgr = fgr_params() if fgr is None else fgr
+        res = np.zeros(B, dtype=ICP_RESULT_DTYPE)
+        out = res.ctypes.data_as(C.POINTER(IcpResult))
+        ev = [np.zeros((a.shape[0], 2), dtype=np.int32) for a in S]
+        fp, i32p = C.POINTER(C.c_float), C.POINTER(C.c_int32)
+        if single:
+            assert B == 1
+            rc = lib().tzr_fgr(self._h, C.byref(fgr), _p(S[0], C.c_float), S[0].shape[0], _p(D[0], C.c_float),
+                               D[0].shape[0], K[0].shape[0], _p(K[0], C.c_int32), out, _p(ev[0], C.c_int32))
+        else:
+            ns = np.array([a.shape[0] for a in S], dtype=np.int32)
+            nd = np.array([a.shape[0] for a in D], dtype=np.int32)
+            nc = np.array([k.shape[0] for k in K], dtype=np.int32)
+            rc = lib().tzr_fgr_batch(self._h, C.byref(fgr), B, _p(ns, C.c_int32),
+                                     (fp * B)(*[_p(a, C.c_float) for a in S]), _p(nd, C.c_int32),
+                                     (fp * B)(*[_p(a, C.c_float) for a in D]), _p(nc, C.c_int32),
+                                     (i32p * B)(*[_p(k, C.c_int32) for k in K]), out,
+                                     (i32p * B)(*[_p(e, C.c_int32) for e in ev]))
+        self._ck(rc)
+        return res, [e[:int(r["n_correspondences"])].copy() for e, r in zip(ev, res)]
 
     def icp_point_to_plane(self, src, dst, dst_normals, max_correspondence_distance, init=None, max_iteration=30,
                            relative_fitness=1e-6, relative_rmse=1e-6, kernel=None):

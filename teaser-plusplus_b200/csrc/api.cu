@@ -136,6 +136,8 @@ struct tzr_ctx {
   DevBuf vox;
   // tzr_pose_graph_optimize: its own workspace, for the same reason
   DevBuf pg;
+  // tzr_fgr(_batch) and tzr_register_cloud_pairs_fgr: FGR's tables and normalised rows (its evaluation uses icp)
+  DevBuf fgr;
   int last_strip_blocks = 0;  // strip length of the most recent graph kernel launch (tzr_ctx_last_strip_blocks)
   int max_n = kMaxN;  // per-problem size limit of this context (tzr_ctx_set_max_n: kMaxN ... kMaxNLarge)
   // pinned host staging
@@ -2405,6 +2407,34 @@ struct MultiwayOut {
   int32_t* pg_status;
 };
 
+// FGR (DESIGN.md §3.20): Open3D's FastGlobalRegistrationOption ranges
+static bool fgr_params_ok(const tzr_fgr_params* p) {
+  return p && std::isfinite(p->division_factor) && p->division_factor > 0 &&
+         std::isfinite(p->maximum_correspondence_distance) && p->maximum_correspondence_distance > 0 &&
+         p->iteration_number >= 0;
+}
+
+// the ICP settings of FGR's evaluation: tzr_icp_batch with max_iteration = 0 at FGR's distance
+static void fgr_eval_settings(IcpPlan* plan, const tzr_fgr_params& p) {
+  tzr_icp_params ip;
+  tzr_icp_params_default(&ip);
+  ip.max_correspondence_distance = p.maximum_correspondence_distance;
+  ip.max_iteration = 0;
+  icp_iteration_settings(plan, ip, kIcpPointToPoint, 0.0, nullptr);
+}
+
+// the final correspondences of a problem (rows (source, target), ascending by source) from the per-point matches
+static void icp_corr_rows(const IcpProb& pr, const int32_t* match, int32_t* rows) {
+  long long k = 0;
+  for (int i = 0; i < pr.ns; ++i) {
+    const int j = match[(size_t)pr.m_lo + i];
+    if (j < 0) continue;
+    rows[2 * k] = i;
+    rows[2 * k + 1] = j;
+    ++k;
+  }
+}
+
 static void icp_result_of(const IcpProb& pr, tzr_icp_result* out) {
   memset(out, 0, sizeof(*out));
   if (!pr.seeded) return;
@@ -2418,6 +2448,25 @@ static void icp_result_of(const IcpProb& pr, tzr_icp_result* out) {
   out->converged = pr.converged;
 }
 
+// FGR's record of a problem: the evaluation's fields from its ICP problem, the optimiser's from its FGR problem
+static void fgr_result_of(const IcpProb& pr, const FgrProb& fp, tzr_icp_result* out) {
+  icp_result_of(pr, out);
+  out->iterations = fp.iterations;
+  out->converged = fp.converged;
+}
+
+// [problems | normalised rows (K x 6 doubles)] of ctx->fgr, and (corr_bytes > 0) the correspondences between them
+struct FgrLayout {
+  size_t corr, pq, end;
+};
+static FgrLayout fgr_layout(int B, long long K, bool own_corr) {
+  FgrLayout L;
+  L.corr = al256((size_t)B * sizeof(FgrProb));
+  L.pq = L.corr + (own_corr ? al256((size_t)K * 8) : 0);
+  L.end = L.pq + (size_t)K * 48;
+  return L;
+}
+
 // FPFH over the clouds, matching over the pairs, the ragged solve over the pairs that can be solved (DESIGN.md §3.10).
 // Workspace: m_in holds the clouds and every table, m_scratch the FPFH scratch and then the matcher's, m_out the stages'
 // outputs (descriptors alive while matching runs) and the solve's inputs and outputs.  All of it is sized before any work.
@@ -2427,6 +2476,9 @@ static void icp_result_of(const IcpProb& pr, tzr_icp_result* out) {
 // icp_kernel: the robust kernel of the point-to-plane, generalized and coloured modes (checked by the caller; NULL = L2).
 // colors, lambda_geometric: the coloured mode's (n_clouds entries aligned with pts; lambda already checked and mapped
 // into [0, 1] by the caller).
+// fgr (may be NULL; then params and solutions are not used and may be NULL): no solve; FGR of every pair with
+// correspondences on its matched rows (still in m_out) and its two clouds (in m_in), evaluated as tzr_fgr_batch
+// evaluates it; fgr_results (P entries) then receives the records, zeroed for a pair that was not registered.
 static int register_pairs_run(tzr_ctx* ctx, const tzr_frontend_params* fp, const tzr_params* params, int n_clouds,
                               const int32_t* n, const float* const* pts, int P, const int32_t* pair_clouds,
                               const uint64_t* tuple_seeds, tzr_solution* solutions, int32_t* status,
@@ -2434,12 +2486,14 @@ static int register_pairs_run(tzr_ctx* ctx, const tzr_frontend_params* fp, const
                               float* global_scale, const tzr_icp_params* icp, tzr_icp_result* icp_results,
                               int icp_mode = kIcpPointToPoint, double icp_epsilon = 0,
                               const tzr_robust_kernel* icp_kernel = nullptr, const MultiwayOut* mw = nullptr,
-                              const float* const* colors = nullptr, double lambda_geometric = 0) {
+                              const float* const* colors = nullptr, double lambda_geometric = 0,
+                              const tzr_fgr_params* fgr = nullptr, tzr_icp_result* fgr_results = nullptr) {
   const bool colored = icp && icp_mode == kIcpColored;
-  if (!ctx || !fp || !params || n_clouds < 1 || !n || !pts || P < 1 || !pair_clouds || !solutions || !status ||
-      !n_corr || !(fp->normal_search_radius > 0) || !(fp->fpfh_search_radius > 0))
+  if (!ctx || !fp || (!params && !fgr) || n_clouds < 1 || !n || !pts || P < 1 || !pair_clouds ||
+      (!solutions && !fgr) || !status || !n_corr || !(fp->normal_search_radius > 0) || !(fp->fpfh_search_radius > 0))
     return TZR_ERR_INVALID_ARG;
   if (icp && (!icp_params_ok(icp) || !icp_results)) return TZR_ERR_INVALID_ARG;
+  if (fgr && (icp || !fgr_params_ok(fgr) || !fgr_results)) return TZR_ERR_INVALID_ARG;
   if (mw && (!icp || params->estimate_scaling || !mw->uncertain || !pg_params_ok(mw->pg) || !mw->information ||
              !mw->info_counts || !mw->edge_weights || !mw->edge_mask || !mw->poses || !mw->pg_status))
     return TZR_ERR_INVALID_ARG;
@@ -2503,6 +2557,8 @@ static int register_pairs_run(tzr_ctx* ctx, const tzr_frontend_params* fp, const
   // depend on which pairs are solved, so it is planned once, here, and staged with the clouds and their colours; the
   // layout's own slot for it in ctx->icp stays unused.
   IcpPlan iplan;
+  if (fgr) fgr_eval_settings(&iplan, *fgr);  // FGR's evaluation: the same planning over the registered pairs
+  const double icp_r = icp ? icp->max_correspondence_distance : fgr ? fgr->maximum_correspondence_distance : 0.0;
   std::vector<FpfhCloud> iclouds, gclouds;
   std::vector<IcpProb> iprobs;
   std::vector<int> ichunks;
@@ -2513,15 +2569,15 @@ static int register_pairs_run(tzr_ctx* ctx, const tzr_frontend_params* fp, const
       i_slo.push_back(clouds[pair_clouds[2 * p]].lo);
       i_tc.push_back(pair_clouds[2 * p + 1]);
     }
-    return icp_plan((int)pairs.size(), i_ns.data(), i_slo.data(), i_tc.data(), n_clouds, n,
-                    icp->max_correspondence_distance, search_route(ctx->flags, kFlagIcpBrute, kFlagIcpGrid), nullptr,
-                    &iplan, &iclouds, &iprobs, &ichunks);
+    return icp_plan((int)pairs.size(), i_ns.data(), i_slo.data(), i_tc.data(), n_clouds, n, icp_r,
+                    search_route(ctx->flags, kFlagIcpBrute, kFlagIcpGrid), nullptr, &iplan, &iclouds, &iprobs,
+                    &ichunks);
   };
   IcpLayout il{};
-  if (icp) {
+  if (icp || fgr) {
     std::vector<int> every(P);
     for (int p = 0; p < P; ++p) every[p] = p;
-    icp_iteration_settings(&iplan, *icp, icp_mode, icp_epsilon, icp_kernel);
+    if (icp) icp_iteration_settings(&iplan, *icp, icp_mode, icp_epsilon, icp_kernel);
     iplan.lambda_geometric = lambda_geometric;
     if (colored) {
       iplan.grad_r = 2.0 * icp->max_correspondence_distance;
@@ -2537,14 +2593,22 @@ static int register_pairs_run(tzr_ctx* ctx, const tzr_frontend_params* fp, const
     }
     il = icp_layout(iplan, 0, mw != nullptr);
   }
+  // FGR: its problem table (staged in, read back) after the ICP tables
   const size_t hi_tab = al256(pin_base), hi_info = al256(hi_tab + il.match),
-               hi_icnt = hi_info + al256((size_t)P * 36 * 8),
-               pin_bytes = mw ? hi_icnt + (size_t)P * 4 : icp ? hi_tab + il.match : pin_base;
+               hi_icnt = hi_info + al256((size_t)P * 36 * 8), hi_fgr = hi_info,
+               pin_bytes = mw    ? hi_icnt + (size_t)P * 4
+                           : fgr ? hi_fgr + (size_t)P * sizeof(FgrProb)
+                           : icp ? hi_tab + il.match
+                                 : pin_base;
   int rc;
   if ((rc = ensure(ctx, ctx->m_in, in_bytes)) != TZR_OK) return rc;
   if ((rc = ensure(ctx, ctx->m_scratch, scratch_bytes)) != TZR_OK) return rc;
   if ((rc = ensure(ctx, ctx->m_out, out_bytes)) != TZR_OK) return rc;
   if ((rc = ensure_pinned(ctx, pin_bytes)) != TZR_OK) return rc;
+  if (fgr) {  // FGR's evaluation over every pair and its rows, at most C of them (the registered pairs fit both)
+    if ((rc = ensure(ctx, ctx->icp, il.end)) != TZR_OK) return rc;
+    if ((rc = ensure(ctx, ctx->fgr, fgr_layout(P, (long long)C, false).end)) != TZR_OK) return rc;
+  }
   char* h = (char*)ctx->h_pin;
   char* d_in = (char*)ctx->m_in.p;
   char* d_out = (char*)ctx->m_out.p;
@@ -2587,6 +2651,7 @@ static int register_pairs_run(tzr_ctx* ctx, const tzr_frontend_params* fp, const
   PairGather* table = (PairGather*)(h + h_g);
   std::vector<int32_t> solved_n;
   std::vector<int> solved;  // pair of every retained problem
+  std::vector<int> registered;  // FGR: pair of every registered problem
   std::vector<long long> corr_row(P, -1);
   int n_table = 0, max_count = 0;
   long long corr_rows = 0, solve_rows = 0;
@@ -2594,7 +2659,7 @@ static int register_pairs_run(tzr_ctx* ctx, const tzr_frontend_params* fp, const
   for (int p = 0; p < P; ++p) {
     if (global_scale) global_scale[p] = gs[p];
     if (problem_index) problem_index[p] = -1;
-    memset(&solutions[p], 0, sizeof(tzr_solution));
+    if (solutions) memset(&solutions[p], 0, sizeof(tzr_solution));
     if (overflow[pair_clouds[2 * p]] || overflow[pair_clouds[2 * p + 1]]) {
       status[p] = TZR_ERR_TOO_LARGE;
       n_corr[p] = 0;
@@ -2605,6 +2670,21 @@ static int register_pairs_run(tzr_ctx* ctx, const tzr_frontend_params* fp, const
     n_corr[p] = cnt;
     if (cnt == 0) {
       status[p] = TZR_ERR_INVALID_ARG;
+      continue;
+    }
+    if (fgr) {  // every pair with correspondences is registered on its gathered index rows
+      status[p] = TZR_OK;
+      PairGather& g = table[n_table++];
+      g.src_lo = cloud_lo[p].x;
+      g.dst_lo = cloud_lo[p].y;
+      g.slot = MP[p].s_off + MP[p].d_off;
+      g.count = cnt;
+      g.corr_row = corr_rows;
+      g.solve_row = -1;
+      max_count = std::max(max_count, cnt);
+      corr_row[p] = corr_rows;
+      corr_rows += cnt;
+      registered.push_back(p);
       continue;
     }
     const bool solve = cnt <= ctx->max_n && !(params->estimate_scaling && !scale_scratch_bytes(1, cnt, ctx->flags));
@@ -2648,8 +2728,36 @@ static int register_pairs_run(tzr_ctx* ctx, const tzr_frontend_params* fp, const
   if (S > 0) {
     rc = solve_ragged_dev(ctx, *params, S, solved_n.data(), d_src, d_dst, d_sol, want_clq ? d_clq : nullptr);
     if (rc) return rc;
-  } else {  // nothing solved: no solve is retained
+  } else if (!fgr) {  // nothing solved: no solve is retained (FGR is not a solve entry and leaves it as it is)
     forget_retained(ctx);
+  }
+  // FGR of the registered pairs on their gathered rows and their clouds in place, then its evaluation (DESIGN.md §3.20)
+  const int R = (int)registered.size();
+  FgrProb* hf = (FgrProb*)(h + hi_fgr);
+  if (fgr && R > 0) {
+    plan_icp(registered);  // a subset of the pairs planned above: it fits
+    il = icp_layout(iplan, 0, false);
+    const FgrLayout fl = fgr_layout(R, corr_rows, false);  // both buffers were sized before any work
+    char* hi = h + hi_tab;
+    memcpy(hi + il.probs, iprobs.data(), (size_t)R * sizeof(IcpProb));
+    memcpy(hi + il.clouds, iclouds.data(), (size_t)n_clouds * sizeof(FpfhCloud));
+    memcpy(hi + il.chunks, ichunks.data(), ichunks.size() * 4);
+    for (int k = 0; k < R; ++k) {
+      hf[k] = FgrProb{};
+      hf[k].c_lo = corr_row[registered[k]];
+      hf[k].K = (int)n_corr[registered[k]];
+    }
+    char* di = (char*)ctx->icp.p;
+    char* df = (char*)ctx->fgr.p;
+    CK(cudaMemcpyAsync(di, hi, il.match, cudaMemcpyHostToDevice, st));
+    CK(cudaMemcpyAsync(df, hf, (size_t)R * sizeof(FgrProb), cudaMemcpyHostToDevice, st));
+    IcpBuffers buf = icp_buffers(di, il);
+    buf.src = buf.dst = d_pts;
+    ctx->launches += launch_fgr(*fgr, R, (FgrProb*)df, buf.probs, d_pts, d_pts, d_corr, (double*)(df + fl.pq), st);
+    ctx->launches += launch_icp(iplan, buf, st);
+    if ((rc = check_launch(ctx, "fgr launch")) != TZR_OK) return rc;
+    CK(cudaMemcpyAsync(hi + il.probs, buf.probs, (size_t)R * sizeof(IcpProb), cudaMemcpyDeviceToHost, st));
+    CK(cudaMemcpyAsync(hf, df, (size_t)R * sizeof(FgrProb), cudaMemcpyDeviceToHost, st));
   }
   // the refinement of the solved pairs, seeded on the device from their records (no synchronisation, no upload of points)
   char* hi = h + hi_tab;
@@ -2687,13 +2795,19 @@ static int register_pairs_run(tzr_ctx* ctx, const tzr_frontend_params* fp, const
   }
   // synchronisation 2: the records, and the index pairs and cliques that were asked for
   if (S > 0) CK(cudaMemcpyAsync(h + h_sol, d_sol, (size_t)S * sizeof(tzr_solution), cudaMemcpyDeviceToHost, st));
-  if (corr_rows > 0) CK(cudaMemcpyAsync(h + h_corr, d_corr, (size_t)corr_rows * 8, cudaMemcpyDeviceToHost, st));
+  bool read_corr = corr_rows > 0;
+  if (fgr) {  // FGR gathers every registered pair's rows: read back only when some were asked for
+    read_corr = false;
+    for (int p : registered) read_corr |= corr && corr[p];
+  }
+  if (read_corr) CK(cudaMemcpyAsync(h + h_corr, d_corr, (size_t)corr_rows * 8, cudaMemcpyDeviceToHost, st));
   if (want_clq) CK(cudaMemcpyAsync(h + h_clq, d_clq, (size_t)solve_rows * 4, cudaMemcpyDeviceToHost, st));
   CK(cudaStreamSynchronize(st));
   const tzr_solution* sol = (const tzr_solution*)(h + h_sol);
   spans.clear();
   for (int p = 0; p < P; ++p)
-    if (corr_row[p] >= 0) spans.push_back(CopySpan{corr[p], h + h_corr + (size_t)corr_row[p] * 8, (size_t)n_corr[p] * 8});
+    if (corr_row[p] >= 0 && corr && corr[p])
+      spans.push_back(CopySpan{corr[p], h + h_corr + (size_t)corr_row[p] * 8, (size_t)n_corr[p] * 8});
   bool no_room = false;
   long long row = 0;
   for (int k = 0; k < S; ++k) {
@@ -2708,6 +2822,10 @@ static int register_pairs_run(tzr_ctx* ctx, const tzr_frontend_params* fp, const
   if (icp) {
     for (int p = 0; p < P; ++p) memset(&icp_results[p], 0, sizeof(tzr_icp_result));
     for (int k = 0; k < S; ++k) icp_result_of(hi_probs[k], &icp_results[solved[k]]);
+  }
+  if (fgr) {
+    for (int p = 0; p < P; ++p) memset(&fgr_results[p], 0, sizeof(tzr_icp_result));
+    for (int k = 0; k < R; ++k) fgr_result_of(hi_probs[k], hf[k], &fgr_results[registered[k]]);
   }
   if (mw) {  // the pose graph over the refined pairs, in pair order
     memset(mw->information, 0, (size_t)P * 36 * 8);
@@ -2841,6 +2959,16 @@ int tzr_register_cloud_pairs_icp_colored(tzr_ctx* ctx, const tzr_frontend_params
                             kernel, nullptr, colors, lambda_geometric);
 }
 
+int tzr_register_cloud_pairs_fgr(tzr_ctx* ctx, const tzr_frontend_params* fp, const tzr_fgr_params* fgr,
+                                 int n_clouds, const int32_t* n, const float* const* pts, int P,
+                                 const int32_t* pair_clouds, const uint64_t* tuple_seeds, int32_t* status,
+                                 int64_t* n_corr, int32_t* const* corr, float* global_scale, tzr_icp_result* results) {
+  if (!fgr) return TZR_ERR_INVALID_ARG;
+  return register_pairs_run(ctx, fp, nullptr, n_clouds, n, pts, P, pair_clouds, tuple_seeds, nullptr, status, nullptr,
+                            n_corr, corr, nullptr, global_scale, nullptr, nullptr, kIcpPointToPoint, 0, nullptr,
+                            nullptr, nullptr, 0, fgr, results);
+}
+
 void tzr_icp_params_default(tzr_icp_params* p) {
   if (!p) return;
   memset(p, 0, sizeof(*p));
@@ -2957,19 +3085,88 @@ static int icp_batch_run(tzr_ctx* ctx, const tzr_icp_params* params, int mode, i
   for (int b = 0; b < B; ++b) {
     const IcpProb& pr = probs[b];
     icp_result_of(pr, &results[b]);
-    if (corr && corr[b]) {
-      int32_t* rows = corr[b];
-      long long k = 0;
-      for (int i = 0; i < pr.ns; ++i) {
-        const int j = match[(size_t)pr.m_lo + i];
-        if (j < 0) continue;
-        rows[2 * k] = i;
-        rows[2 * k + 1] = j;
-        ++k;
-      }
-    }
+    if (corr && corr[b]) icp_corr_rows(pr, match.data(), corr[b]);
   }
   return TZR_OK;
+}
+
+// ---- Fast Global Registration (DESIGN.md §3.20) ------------------------------------------------------------------------
+int tzr_fgr_batch(tzr_ctx* ctx, const tzr_fgr_params* params, int B, const int32_t* ns, const float* const* src,
+                  const int32_t* nd, const float* const* dst, const int32_t* n_corr, const int32_t* const* corr,
+                  tzr_icp_result* results, int32_t* const* eval_corr) {
+  if (!ctx || !fgr_params_ok(params) || B < 1 || !ns || !nd || !n_corr || !results) return TZR_ERR_INVALID_ARG;
+  long long K = 0;
+  for (int b = 0; b < B; ++b) {
+    if (ns[b] < 1 || nd[b] < 1 || n_corr[b] < 0 || (n_corr[b] > 0 && (!corr || !corr[b]))) return TZR_ERR_INVALID_ARG;
+    for (int k = 0; k < n_corr[b]; ++k) {
+      const int32_t i = corr[b][2 * k], j = corr[b][2 * k + 1];
+      if (i < 0 || i >= ns[b] || j < 0 || j >= nd[b]) return TZR_ERR_INVALID_ARG;
+    }
+    K += n_corr[b];
+  }
+  if (K > 0x7fffffffll) {
+    ctx->last_error = "the batch's " + std::to_string(K) + " correspondences do not fit 32-bit indices";
+    return TZR_ERR_TOO_LARGE;
+  }
+  IcpPlan plan;
+  fgr_eval_settings(&plan, *params);
+  tzr_similarity id;
+  memset(&id, 0, sizeof(id));
+  id.scale = 1.0;
+  id.rotation[0] = id.rotation[4] = id.rotation[8] = 1.0;
+  const std::vector<tzr_similarity> init((size_t)B, id);  // placeholders: fgr_kernel writes every seed
+  std::vector<IcpProb> probs;
+  IcpBuffers buf;
+  int rc = icp_batch_stage(ctx, &plan, B, ns, src, nullptr, nd, dst, nullptr, init.data(),
+                           params->maximum_correspondence_distance, false, &probs, &buf);
+  if (rc != TZR_OK) return rc;
+  const FgrLayout L = fgr_layout(B, K, true);
+  if ((rc = ensure(ctx, ctx->fgr, L.end)) != TZR_OK) return rc;
+  std::vector<char> h(L.pq);
+  FgrProb* fp = (FgrProb*)h.data();
+  long long c_lo = 0;
+  for (int b = 0; b < B; ++b) {
+    fp[b] = FgrProb{};
+    fp[b].c_lo = c_lo;
+    fp[b].K = n_corr[b];
+    if (n_corr[b] > 0) memcpy(h.data() + L.corr + (size_t)c_lo * 8, corr[b], (size_t)n_corr[b] * 8);
+    c_lo += n_corr[b];
+  }
+  cudaStream_t st = ctx->stream;
+  char* d = (char*)ctx->fgr.p;
+  CK(cudaMemcpyAsync(d, h.data(), L.pq, cudaMemcpyHostToDevice, st));
+  ctx->launches += launch_fgr(*params, B, (FgrProb*)d, buf.probs, buf.src, buf.dst, (const int2*)(d + L.corr),
+                              (double*)(d + L.pq), st);
+  ctx->launches += launch_icp(plan, buf, st);
+  if ((rc = check_launch(ctx, "fgr launch")) != TZR_OK) return rc;
+  CK(cudaMemcpyAsync(probs.data(), buf.probs, (size_t)B * sizeof(IcpProb), cudaMemcpyDeviceToHost, st));
+  CK(cudaMemcpyAsync(fp, d, (size_t)B * sizeof(FgrProb), cudaMemcpyDeviceToHost, st));
+  bool want_corr = false;
+  for (int b = 0; b < B && eval_corr; ++b) want_corr |= eval_corr[b] != nullptr;
+  std::vector<int32_t> match(want_corr ? (size_t)plan.NS : 0);
+  if (want_corr) CK(cudaMemcpyAsync(match.data(), buf.match, (size_t)plan.NS * 4, cudaMemcpyDeviceToHost, st));
+  CK(cudaStreamSynchronize(st));
+  for (int b = 0; b < B; ++b) {
+    fgr_result_of(probs[b], fp[b], &results[b]);
+    if (eval_corr && eval_corr[b]) icp_corr_rows(probs[b], match.data(), eval_corr[b]);
+  }
+  return TZR_OK;
+}
+
+int tzr_fgr(tzr_ctx* ctx, const tzr_fgr_params* params, const float* src, int ns, const float* dst, int nd,
+            int n_corr, const int32_t* corr, tzr_icp_result* result, int32_t* eval_corr) {
+  int32_t* const ec[1] = {eval_corr};
+  return tzr_fgr_batch(ctx, params, 1, &ns, &src, &nd, &dst, &n_corr, &corr, result, eval_corr ? ec : nullptr);
+}
+
+void tzr_fgr_params_default(tzr_fgr_params* p) {
+  if (!p) return;
+  memset(p, 0, sizeof(*p));
+  p->division_factor = 1.4;
+  p->use_absolute_scale = 0;
+  p->decrease_mu = 1;
+  p->maximum_correspondence_distance = 0.025;
+  p->iteration_number = 64;
 }
 
 int tzr_icp_batch(tzr_ctx* ctx, const tzr_icp_params* params, int B, const int32_t* ns, const float* const* src,

@@ -63,25 +63,6 @@ __device__ __forceinline__ void icp_keep(double d2, int j, double* best, int* bj
   }
 }
 
-// Fixed-order sum over a CTA of kIcpThreads threads: butterfly inside each warp (every lane ends with the same bits),
-// then the warp sums in warp order by one thread.  Result in s_out[0..K).
-template <int K>
-__device__ void icp_block_sum(double (&v)[K], double* s_buf /* (kIcpThreads/32) * K */, double* s_out) {
-  const int w = threadIdx.x >> 5, lane = threadIdx.x & 31;
-#pragma unroll
-  for (int k = 0; k < K; ++k)
-    for (int o = 16; o; o >>= 1) v[k] += __shfl_xor_sync(0xffffffffu, v[k], o);
-  if (lane == 0)
-#pragma unroll
-    for (int k = 0; k < K; ++k) s_buf[w * K + k] = v[k];
-  __syncthreads();
-  if (threadIdx.x < K) {
-    double s = 0.0;
-    for (int q = 0; q < kIcpThreads / 32; ++q) s += s_buf[q * K + threadIdx.x];
-    s_out[threadIdx.x] = s;
-  }
-}
-
 // Fixed-order sum of the problem's nc chunk partials (K of the S doubles each: S = 9 for the nearest-neighbour sums and
 // the covariance, 27 for the point-to-plane system) over one warp: lane l takes chunks l, l + 32, ..., then a
 // butterfly; every lane returns the same bits.
@@ -585,27 +566,6 @@ __global__ void __launch_bounds__(kIcpThreads) icp_gicp_system_kernel(IcpArgs a,
 }
 
 // ---- coloured ICP (DESIGN.md §3.17) ---------------------------------------------------------------------------------
-// The terms of one row (J, r) with weight w (kRobust) into v: (w J_a) J_b (21) and (w J_a) r (6); without kRobust J_a J_b
-// and J_a r, point-to-plane's unweighted products.  add: v += the terms, else v = the terms.
-template <bool kRobust>
-__device__ __forceinline__ void icp_row_terms(const double J[6], double r, double w, bool add,
-                                              double (&v)[kIcpPlaneSums]) {
-  double wJ[6];
-#pragma unroll
-  for (int row = 0; row < 6; ++row) wJ[row] = kRobust ? w * J[row] : J[row];
-  int k = 0;
-#pragma unroll
-  for (int row = 0; row < 6; ++row)
-#pragma unroll
-    for (int col = row; col < 6; ++col) {
-      const double t = wJ[row] * J[col];
-      v[k] = add ? v[k] + t : t;
-      ++k;
-    }
-#pragma unroll
-  for (int row = 0; row < 6; ++row) v[21 + row] = add ? v[21 + row] + wJ[row] * r : wJ[row] * r;
-}
-
 // One CTA per chunk: each correspondence (i, j) whose target normal n has three finite components adds a geometric row
 // J_G = sqrt(lambda) (u x n, n), r_G = sqrt(lambda) r (r: point-to-plane's residual) and then a photometric row
 // J_I = sqrt(1 - lambda) (u x m, m), r_I = sqrt(1 - lambda) (i_s - i_hat) with m = -(I - n n^T) g, g the target's

@@ -545,6 +545,45 @@ struct IcpPlan {
   double grad_r = 0;
   FpfhPlan ggrid;
 };
+// Fixed-order sum over a CTA of kIcpChunk threads: butterfly inside each warp (every lane ends with the same bits),
+// then the warp sums in warp order by one thread.  Result in s_out[0..K).  ICP's chunk sums and FGR's (fgr.cu).
+template <int K>
+__device__ void icp_block_sum(double (&v)[K], double* s_buf /* (kIcpChunk/32) * K */, double* s_out) {
+  const int w = threadIdx.x >> 5, lane = threadIdx.x & 31;
+#pragma unroll
+  for (int k = 0; k < K; ++k)
+    for (int o = 16; o; o >>= 1) v[k] += __shfl_xor_sync(0xffffffffu, v[k], o);
+  if (lane == 0)
+#pragma unroll
+    for (int k = 0; k < K; ++k) s_buf[w * K + k] = v[k];
+  __syncthreads();
+  if (threadIdx.x < K) {
+    double s = 0.0;
+    for (int q = 0; q < kIcpChunk / 32; ++q) s += s_buf[q * K + threadIdx.x];
+    s_out[threadIdx.x] = s;
+  }
+}
+// The terms of one row (J, r) with weight w (kRobust) into v: (w J_a) J_b (21) and (w J_a) r (6); without kRobust J_a J_b
+// and J_a r, point-to-plane's unweighted products.  add: v += the terms, else v = the terms.  Coloured ICP's rows
+// (icp.cu) and FGR's (fgr.cu).
+template <bool kRobust>
+__device__ __forceinline__ void icp_row_terms(const double J[6], double r, double w, bool add,
+                                              double (&v)[kIcpPlaneSums]) {
+  double wJ[6];
+#pragma unroll
+  for (int row = 0; row < 6; ++row) wJ[row] = kRobust ? w * J[row] : J[row];
+  int k = 0;
+#pragma unroll
+  for (int row = 0; row < 6; ++row)
+#pragma unroll
+    for (int col = row; col < 6; ++col) {
+      const double t = wJ[row] * J[col];
+      v[k] = add ? v[k] + t : t;
+      ++k;
+    }
+#pragma unroll
+  for (int row = 0; row < 6; ++row) v[21 + row] = add ? v[21 + row] + wJ[row] * r : wJ[row] * r;
+}
 constexpr int kIcpInfoSums = 21;  // doubles per chunk of launch_icp_information's partial buffer
 // The tables of B problems against T target clouds of nt[0..T) points, back to back in the flat target array: problem
 // b refines ns[b] sources from flat point s_lo[b] (s_lo nullptr: the sources back to back) onto target cloud tc[b]
@@ -624,6 +663,24 @@ int launch_icp_information(const IcpPlan& plan, const IcpBuffers& buf, bool rese
 int launch_icp_pose_load(IcpProb* probs, int B, const int* pair_of, const tzr_similarity* pose, cudaStream_t st);
 int launch_icp_pose_store(const IcpProb* probs, int P, const int* prob_of, tzr_similarity* pose, tzr_icp_result* rec,
                           int stride, cudaStream_t st);
+
+// fgr.cu (Fast Global Registration, tzr_fgr_batch, DESIGN.md §3.20): B problems whose clouds are those of B ICP problems
+// (IcpProb s_lo, ns, d_lo, nd into the ICP buffers' src and dst), so that the evaluation is launch_icp's
+constexpr int kFgrMinCorr = 10;  // fewer usable correspondences than this: the identity (the fallback)
+struct FgrProb {        // one per problem; the host fills c_lo and K, the kernels the rest
+  long long c_lo;       // first row of the problem's correspondences (int2 (i, j)) and of its normalised rows (6 doubles)
+  int K;                // its correspondences
+  int Kv;               // the usable ones (both ends finite), compacted in input order
+  int iterations, converged;
+  double scale_global, mu0;  // the normalisation's divisor and the first mu
+  double mean_s[3], mean_t[3], sigma;
+  double R[9], t[3];    // the result, mapping the source onto the target (column-major R)
+};
+// Two launches: fgr_prep_kernel (the normalisation and the compaction) and fgr_kernel (every iteration of every problem
+// and the result, which it also writes into icp[b] as a seed: s = 1, R, t, active = seeded = 1).  corr: the problems'
+// rows; pq: sum K x 6 doubles of scratch.
+int launch_fgr(const tzr_fgr_params& prm, int B, FgrProb* probs, IcpProb* icp, const float* src, const float* dst,
+               const int2* corr, double* pq, cudaStream_t st);
 
 // pose_graph.cu (tzr_pose_graph_optimize, DESIGN.md §3.16): one graph of K nodes and E edges, device-resident
 struct PgEdge {         // one per edge; the host fills it, the kernels read it

@@ -13,6 +13,7 @@
 #include <sstream>
 
 #include "teaser/certification.h"
+#include "teaser/fgr.h"
 #include "teaser/icp.h"
 #include "teaser/pose_graph.h"
 #include "teaser/normals.h"
@@ -119,6 +120,56 @@ py::dict icp_dict(const teaser::PointToPointICPResult& r) {
   return py::dict(py::arg("solution") = r.solution, py::arg("fitness") = r.fitness,
                   py::arg("inlier_rmse") = r.inlier_rmse, py::arg("iterations") = r.iterations,
                   py::arg("converged") = r.converged, py::arg("correspondences") = r.correspondences);
+}
+
+// (K,2) integer rows -> (source index, target index) pairs
+std::vector<std::pair<int, int>> corr_of(const py::array_t<int32_t, py::array::c_style | py::array::forcecast>& a) {
+  if (a.size() == 0) return {};
+  if (a.ndim() != 2 || a.shape(1) != 2) throw std::invalid_argument("correspondences must be (K,2) integer arrays");
+  std::vector<std::pair<int, int>> out(static_cast<size_t>(a.shape(0)));
+  const int32_t* d = a.data();
+  for (size_t k = 0; k < out.size(); ++k) out[k] = {d[2 * k], d[2 * k + 1]};
+  return out;
+}
+
+teaser::FastGlobalRegistration fgr_of(double maximum_correspondence_distance, int iteration_number,
+                                      double division_factor, bool use_absolute_scale, bool decrease_mu) {
+  teaser::FastGlobalRegistration::Params p;
+  p.maximum_correspondence_distance = maximum_correspondence_distance;
+  p.iteration_number = iteration_number;
+  p.division_factor = division_factor;
+  p.use_absolute_scale = use_absolute_scale;
+  p.decrease_mu = decrease_mu;
+  return teaser::FastGlobalRegistration(p);
+}
+
+// registerCloudPairs as a list of dicts: status, correspondences, global_scale, registered and fgr (an icp dict, None
+// for a pair that was not registered)
+py::list fgr_pairs_run(const teaser::FastGlobalRegistration& fgr, const std::vector<CloudArray>& clouds,
+                       const std::vector<std::pair<int, int>>& pairs, double normal_search_radius,
+                       double fpfh_search_radius, bool use_absolute_scale, bool use_crosscheck, bool use_tuple_test,
+                       float tuple_scale, uint64_t tuple_seed) {
+  std::vector<teaser::PointCloud> pcs;
+  for (const auto& a : clouds) pcs.push_back(cloud_of(a));
+  teaser::FastGlobalRegistration::CloudPairParams cp;
+  cp.normal_search_radius = normal_search_radius;
+  cp.fpfh_search_radius = fpfh_search_radius;
+  cp.use_absolute_scale = use_absolute_scale;
+  cp.use_crosscheck = use_crosscheck;
+  cp.use_tuple_test = use_tuple_test;
+  cp.tuple_scale = tuple_scale;
+  cp.tuple_seed = tuple_seed;
+  std::vector<teaser::FastGlobalRegistration::CloudPairResult> res;
+  {
+    py::gil_scoped_release release;
+    res = fgr.registerCloudPairs(pcs, pairs, cp);
+  }
+  py::list out;
+  for (const auto& r : res)
+    out.append(py::dict(py::arg("status") = r.status, py::arg("correspondences") = r.correspondences,
+                        py::arg("global_scale") = r.global_scale, py::arg("registered") = r.registered,
+                        py::arg("fgr") = r.registered ? py::object(icp_dict(r.fgr)) : py::object(py::none())));
+  return out;
 }
 
 // (4,4) float64 matrices <-> Eigen::Matrix4d, (6,6) <-> teaser::Matrix6d
@@ -570,6 +621,64 @@ PYBIND11_MODULE(_teaserpp, m) {
       py::arg("clouds"), py::arg("pairs"), py::arg("scales"), py::arg("init"), py::arg("method") = "point_to_plane",
       py::arg("colors") = py::none(), py::arg("lambda_geometric") = 0.968, py::arg("epsilon") = 1e-3,
       py::arg("kernel") = teaser::RobustKernel(), py::arg("information") = false);
+
+  // GPU extra: Fast Global Registration (teaser::FastGlobalRegistration) on given correspondences ((K,2) integer
+  // arrays) or, over a cloud table, on matched ones; records are icp dicts whose correspondences are the evaluation's
+  py::class_<teaser::FastGlobalRegistration>(m, "FastGlobalRegistration")
+      .def(py::init(&fgr_of), py::arg("maximum_correspondence_distance") = 0.025, py::arg("iteration_number") = 64,
+           py::arg("division_factor") = 1.4, py::arg("use_absolute_scale") = false, py::arg("decrease_mu") = true)
+      .def("register",
+           [](const teaser::FastGlobalRegistration& fgr, const CloudArray& src, const CloudArray& dst,
+              const py::array_t<int32_t, py::array::c_style | py::array::forcecast>& corr) {
+             const teaser::PointCloud s = cloud_of(src), d = cloud_of(dst);
+             const auto c = corr_of(corr);
+             teaser::FastGlobalRegistration::Result r;
+             {
+               py::gil_scoped_release release;
+               r = fgr.registerPair(s, d, c);
+             }
+             return icp_dict(r);
+           },
+           py::arg("src"), py::arg("dst"), py::arg("corr"))
+      .def("register_batch",
+           [](const teaser::FastGlobalRegistration& fgr, const std::vector<CloudArray>& src,
+              const std::vector<CloudArray>& dst,
+              const std::vector<py::array_t<int32_t, py::array::c_style | py::array::forcecast>>& corr) {
+             std::vector<teaser::PointCloud> s, d;
+             std::vector<std::vector<std::pair<int, int>>> c;
+             for (const auto& a : src) s.push_back(cloud_of(a));
+             for (const auto& a : dst) d.push_back(cloud_of(a));
+             for (const auto& a : corr) c.push_back(corr_of(a));
+             std::vector<teaser::FastGlobalRegistration::Result> res;
+             {
+               py::gil_scoped_release release;
+               res = fgr.registerBatch(s, d, c);
+             }
+             py::list out;
+             for (const auto& r : res) out.append(icp_dict(r));
+             return out;
+           },
+           py::arg("src"), py::arg("dst"), py::arg("corr"))
+      .def("register_cloud_pairs", &fgr_pairs_run, py::arg("clouds"), py::arg("pairs"),
+           py::arg("normal_search_radius") = 0.03, py::arg("fpfh_search_radius") = 0.05,
+           py::arg("use_absolute_scale") = true, py::arg("use_crosscheck") = true, py::arg("use_tuple_test") = true,
+           py::arg("tuple_scale") = 0.0f, py::arg("tuple_seed") = 0x7ea5e2ull);
+  m.def(
+      "register_cloud_pairs_fgr",
+      [](const std::vector<CloudArray>& clouds, const std::vector<std::pair<int, int>>& pairs,
+         double normal_search_radius, double fpfh_search_radius, bool use_absolute_scale, bool use_crosscheck,
+         bool use_tuple_test, float tuple_scale, uint64_t tuple_seed, double maximum_correspondence_distance,
+         int iteration_number, double division_factor, bool fgr_absolute_scale, bool decrease_mu) {
+        return fgr_pairs_run(fgr_of(maximum_correspondence_distance, iteration_number, division_factor,
+                                    fgr_absolute_scale, decrease_mu),
+                             clouds, pairs, normal_search_radius, fpfh_search_radius, use_absolute_scale,
+                             use_crosscheck, use_tuple_test, tuple_scale, tuple_seed);
+      },
+      py::arg("clouds"), py::arg("pairs"), py::arg("normal_search_radius") = 0.03,
+      py::arg("fpfh_search_radius") = 0.05, py::arg("use_absolute_scale") = true, py::arg("use_crosscheck") = true,
+      py::arg("use_tuple_test") = true, py::arg("tuple_scale") = 0.0f, py::arg("tuple_seed") = 0x7ea5e2ull,
+      py::arg("maximum_correspondence_distance") = 0.025, py::arg("iteration_number") = 64,
+      py::arg("division_factor") = 1.4, py::arg("fgr_absolute_scale") = false, py::arg("decrease_mu") = true);
 
   // GPU extra: coloured ICP's colour gradients (teaser::estimateColorGradients), as (n,3) float64
   m.def("estimate_color_gradients",
