@@ -1061,6 +1061,125 @@ int tzr_register_cloud_pairs_fgr(tzr_ctx* ctx, const tzr_frontend_params* fparam
                                  const int32_t* pair_clouds, const uint64_t* tuple_seeds, int32_t* status,
                                  int64_t* n_corr, int32_t* const* corr, float* global_scale, tzr_icp_result* results);
 
+/* ---- global registration: RANSAC ---------------------------------------------------------------------------------
+ * Correspondence RANSAC in the shape of Open3D's registration_ransac_based_on_correspondence, for many problems at once,
+ * defined here as follows (DESIGN.md §3.21).  It is this project's own definition: the generator, the estimate, the
+ * summation order, the exit bound's edge cases and the fallback differ from Open3D's, so results never equal Open3D's
+ * bit for bit.  Every expression is IEEE float64 with no FMA contraction.
+ *   - Inputs: source x (ns >= 1 float xyz), target y (nd >= 1 float xyz), both read exactly as float64, K >= 0
+ *     correspondences (i_k, j_k) (source index, target index), a 64-bit seed, and for the normal checker the normals of
+ *     both clouds (n x 4 floats, the library's normals layout; the fourth float is ignored).  A row with a non-finite
+ *     end is dropped; the remaining K' rows keep their input order and are the only ones drawn and scored.
+ *   - Hypothesis itr (0, 1, ...): ransac_n rows drawn with replacement, draw j the row mulhi64(splitmix64(seed +
+ *     ransac_n itr + j), K') (unsigned 64-bit arithmetic, mulhi64 the high word of the 128-bit product, splitmix64 the
+ *     tuple test's mixer of tzr_frontend_params).  The estimate is point-to-point Kabsch: mu_p, mu_q the means of the
+ *     drawn rows (sums in draw order from 0, divided by ransac_n), H(r, c) = sum over the draws in order, from 0, of
+ *     (p - mu_p)(r) (q - mu_q)(c), R = tzr_icp's rotation of H (the rotation stage's SVD with its reflection fix),
+ *     t(r) = mu_q(r) - ((R(r,0) mu_p0 + R(r,1) mu_p1) + R(r,2) mu_p2), scale 1.
+ *   - Checkers (Open3D's CorrespondenceChecker*, each off unless enabled; a hypothesis passes when every enabled one
+ *     does; they only filter, so their order does not change the result):
+ *       edge length: fails when d_x < d_y s or d_y < d_x s for some draws i < j, d_x = ||x_i - x_j||, d_y = ||y_i - y_j||,
+ *         ||d|| = sqrt((d0 d0 + d1 d1) + d2 d2), s = edge_length_similarity (strict: d_x = d_y s passes);
+ *       distance: fails when ||T x - y|| > distance_threshold for some draw (strict: equality passes), T x as below;
+ *       normal: fails when (n_y0 m0 + n_y1 m1) + n_y2 m2 < cos(normal_angle_threshold) for some draw, m = R n_x (rows as
+ *         T x without t; strict: equality passes; a non-finite normal never fails, as in Open3D), cos the host libm's.
+ *   - Score of a passing hypothesis: row k is an inlier when d2 = ||T x - y||^2 < r^2 (strict), r =
+ *     max_correspondence_distance, each component (R(r,0) x0 + R(r,1) x1) + R(r,2) x2 + t(r) minus y(r), d2 = (e0 e0 +
+ *     e1 e1) + e2 e2 (tzr_icp's transform at s = 1).  fitness = count / K' and rmse = sqrt(sum d2 / count) (both 0
+ *     without an inlier).  sum d2 runs over segments of 512 rows: each segment's inliers summed in ascending row order
+ *     from 0, the segment sums added in ascending segment order from 0.
+ *   - The loop, one sequential run of:
+ *       best = none (fitness 0, rmse 0), exit = max_iteration
+ *       for itr = 0, 1, ... while itr < max_iteration and itr < exit:
+ *         draw, estimate and check hypothesis itr; if it passes, score it
+ *         if it passes and is better than best: best = it, exit = min(exit, bound(fitness))
+ *     "better": a higher fitness, or the same fitness and a smaller rmse (so an earlier hypothesis wins a tie, and a
+ *     hypothesis without an inlier never wins).  bound(f) = ceil(log(1 - confidence) / log(1 - f^ransac_n)), f^n the
+ *     product ((f f) f) ... in order (Open3D calls pow), log the device's; when that is NaN or -inf (confidence 1 with
+ *     f = 1, or 1 - f^n rounding to 1, where Open3D's cast to int is undefined) it is +inf: exit is not lowered.  A
+ *     bound of 0 (confidence 0, or f = 1) stops the loop after the hypothesis that set it.
+ *   - Fallback: K' < ransac_n, max_iteration = 0, or no hypothesis better than none: the identity.
+ *   - Evaluation (Open3D's evaluate_registration): fitness, inlier_rmse, n_correspondences and eval_corr are bit for bit
+ *     tzr_icp_batch's with max_iteration = 0 and max_correspondence_distance, seeded with the result.
+ * Result (tzr_icp_result, which seeds tzr_icp_batch directly): transform (scale 1, the winner's R, t), the evaluation,
+ * iterations = the hypotheses drawn (0 for K' < ransac_n; otherwise max(winner + 1, min(max_iteration, exit))) and
+ * converged (1 when the bound stopped the loop before max_iteration).  The hypotheses run in rounds of up to 65536 per
+ * problem, all of a round at once; the results do not depend on the rounds.
+ * Launches: 4 + 3 per round (the compaction, each round's hypotheses, scores and selection, the seed, the evaluation's
+ * search and combination), + 4 for the evaluation's grid build when some target has 1024 points or more.  The rounds
+ * span 256, 512, 1024, ... hypotheses up to a cap, until max_iteration is covered; the cap is 65536, halved while cap x
+ * ceil(K_max / 512) > 65536 (not below 256), K_max the batch's largest correspondence count.  So the launch count
+ * depends on max_iteration and K_max, not on B or the data.  The sums of the batch's points and of its correspondences
+ * must each stay below 2^31 (TZR_ERR_TOO_LARGE); TZR_ERR_ALLOC when the workspace does not fit the device
+ * (tzr_last_error names the size).  The workspace is sized for the largest round run, whatever the bound does: per
+ * problem, 104 B per hypothesis of that round (6.8 MB at the defaults with K_max <= 512, 0.4 MB at K_max = 5000), at
+ * most 1 MiB of partial sums, and 24 B per correspondence (48 B with the normal checker), beside the evaluation's
+ * tzr_icp_batch workspace.  Not a solve entry: a retained solve stays retained. */
+typedef struct tzr_ransac_params {
+  double max_correspondence_distance; /* no default (0: the caller must set it); <= 0 or non-finite is refused */
+  int32_t ransac_n;                   /* 3; 3 ... 16 */
+  int32_t max_iteration;              /* 100000; >= 0 */
+  double confidence;                  /* 0.999; in [0, 1] */
+  int32_t check_edge_length;          /* 0: off, 1: on */
+  int32_t check_distance;             /* 0: off, 1: on */
+  double edge_length_similarity;      /* 0.9 (Open3D's tutorial); finite when checked */
+  double distance_threshold;          /* 0; finite when checked */
+  int32_t check_normal;               /* 0: off, 1: on (both normals arrays required) */
+  int32_t reserved;
+  double normal_angle_threshold;      /* radians, 0.52359878 (30 degrees); finite when checked */
+} tzr_ransac_params;
+
+/* Open3D's defaults: ransac_n 3, RANSACConvergenceCriteria(100000, 0.999), no checkers. */
+void tzr_ransac_params_default(tzr_ransac_params* p);
+
+/* Per problem, optional. */
+typedef struct tzr_ransac_info {
+  int32_t drawn;   /* hypotheses drawn (the record's iterations) */
+  int32_t passed;  /* of them, those that passed every enabled checker */
+  int32_t winner;  /* the winning hypothesis's index, -1: none (the identity) */
+  int32_t inliers; /* its inliers among the usable rows (its score's count) */
+  int32_t usable;  /* K', the usable rows */
+  int32_t reserved;
+  double rmse;     /* its score's rmse (0 without a winner) */
+} tzr_ransac_info;
+
+/* B ragged problems: problem b has ns[b] >= 1 source points at src[b], nd[b] >= 1 target points at dst[b], n_corr[b]
+ * >= 0 correspondences at corr[b] (n_corr[b] x 2 int32; may be NULL when n_corr[b] = 0) and seeds[b] (seeds may be
+ * NULL: 0 for every problem).  src_normals, dst_normals (B entries, ns[b] / nd[b] x 4 floats): required, with every
+ * entry, when the normal checker is on, not read otherwise.  results: B entries; info (may be NULL): B entries.
+ * eval_corr (may be NULL, or hold NULL entries; capacity ns[b] x 2 int32): the evaluation's correspondences, as
+ * tzr_icp_batch's corr.  A negative count, an index outside its cloud, a missing array or a refused parameter is
+ * TZR_ERR_INVALID_ARG before any device work.  Per problem, every output is bit-identical to the same problem alone. */
+int tzr_ransac_batch(tzr_ctx* ctx, const tzr_ransac_params* params, int B, const int32_t* ns, const float* const* src,
+                     const int32_t* nd, const float* const* dst, const int32_t* n_corr, const int32_t* const* corr,
+                     const uint64_t* seeds, const float* const* src_normals, const float* const* dst_normals,
+                     tzr_icp_result* results, tzr_ransac_info* info, int32_t* const* eval_corr);
+
+/* One problem: tzr_ransac_batch with B = 1 (normals: ns x 4 and nd x 4 floats, or NULL without the normal checker). */
+int tzr_ransac(tzr_ctx* ctx, const tzr_ransac_params* params, const float* src, int ns, const float* dst, int nd,
+               int n_corr, const int32_t* corr, uint64_t seed, const float* src_normals, const float* dst_normals,
+               tzr_icp_result* result, tzr_ransac_info* info, int32_t* eval_corr);
+
+/* Open3D's registration_ransac_based_on_feature_matching over a table of clouds: tzr_register_cloud_pairs' front end
+ * (FPFH of every cloud, matching of every pair; the same arguments, status rules, n_corr, corr and global_scale), then
+ * RANSAC of every pair with status TZR_OK on its matched rows with seed ransac_seeds[p] (ransac_seeds may be NULL: 0),
+ * with no robust solve.  The normal checker reads the FPFH stage's normals (PCL radius normals at
+ * normal_search_radius, flipped towards the origin): it depends on their sign, which Open3D's normals need not share.
+ * results: P entries, zeroed for a pair that was not registered (TZR_ERR_TOO_LARGE: a radius overflow;
+ * TZR_ERR_INVALID_ARG: no correspondence); info (may be NULL): P entries, zeroed likewise.  Each record is
+ * bit-identical to tzr_compute_fpfh_batch, then tzr_match_correspondences_batch with the same seeds, then
+ * tzr_ransac_batch on the matched rows with the FPFH normals.  The correspondences are the matcher's sorted unique rows,
+ * not Open3D's 1-nearest-neighbour (optionally mutual) feature matches, so they never equal Open3D's.  Two host
+ * synchronisations (the counts after matching, the results at the end).  Launches: the front end's
+ * (tzr_register_cloud_pairs' without the solve), the index gather when some pair has correspondences, and
+ * tzr_ransac_batch's over the registered pairs.  Not a solve entry: a retained solve stays retained. */
+int tzr_register_cloud_pairs_ransac(tzr_ctx* ctx, const tzr_frontend_params* fparams, const tzr_ransac_params* ransac,
+                                    int n_clouds, const int32_t* n, const float* const* pts, int P,
+                                    const int32_t* pair_clouds, const uint64_t* tuple_seeds,
+                                    const uint64_t* ransac_seeds, int32_t* status, int64_t* n_corr,
+                                    int32_t* const* corr, float* global_scale, tzr_icp_result* results,
+                                    tzr_ransac_info* info);
+
 /* ---- multiway registration: robust pose graph ------------------------------------------------------------------
  * The global step of Open3D's multiway registration (global_optimization over a PoseGraph), with GNC-TLS pruning the
  * uncertain edges instead of Open3D's line process.  One graph per call, defined here as follows (DESIGN.md §3.16):

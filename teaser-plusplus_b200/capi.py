@@ -170,6 +170,25 @@ class FgrParams(C.Structure):
                 ("reserved", C.c_int32)]
 
 
+class RansacParams(C.Structure):
+    """tzr_ransac_params: correspondence RANSAC's options (Open3D's ransac_n, RANSACConvergenceCriteria and its three
+    correspondence checkers, each with an enable flag)."""
+    _fields_ = [("max_correspondence_distance", C.c_double), ("ransac_n", C.c_int32), ("max_iteration", C.c_int32),
+                ("confidence", C.c_double), ("check_edge_length", C.c_int32), ("check_distance", C.c_int32),
+                ("edge_length_similarity", C.c_double), ("distance_threshold", C.c_double),
+                ("check_normal", C.c_int32), ("reserved", C.c_int32), ("normal_angle_threshold", C.c_double)]
+
+
+class RansacInfo(C.Structure):
+    """tzr_ransac_info: one problem's loop summary."""
+    _fields_ = [("drawn", C.c_int32), ("passed", C.c_int32), ("winner", C.c_int32), ("inliers", C.c_int32),
+                ("usable", C.c_int32), ("reserved", C.c_int32), ("rmse", C.c_double)]
+
+
+RANSAC_INFO_DTYPE = np.dtype([("drawn", np.int32), ("passed", np.int32), ("winner", np.int32), ("inliers", np.int32),
+                              ("usable", np.int32), ("reserved", np.int32), ("rmse", np.float64)])
+
+
 class PoseGraphParams(C.Structure):
     """tzr_pose_graph_params: the GNC-TLS pose graph's distance c, schedule and reference node."""
     _fields_ = [("max_correspondence_distance", C.c_double), ("gnc_factor", C.c_double),
@@ -189,6 +208,8 @@ assert C.sizeof(PoseGraphParams) == 40 and PoseGraphParams.reference_node.offset
 assert C.sizeof(PoseGraphSummary) == 16 and PoseGraphSummary.cost.offset == 8, C.sizeof(PoseGraphSummary)
 assert C.sizeof(IcpScale) == 48 and IcpScale.max_iteration.offset == 40, C.sizeof(IcpScale)
 assert C.sizeof(FgrParams) == 32 and FgrParams.maximum_correspondence_distance.offset == 16, C.sizeof(FgrParams)
+assert C.sizeof(RansacParams) == 64 and RansacParams.normal_angle_threshold.offset == 56, C.sizeof(RansacParams)
+assert RANSAC_INFO_DTYPE.itemsize == C.sizeof(RansacInfo) == 32, C.sizeof(RansacInfo)
 assert C.sizeof(RobustKernel) == 16 and RobustKernel.k.offset == 8, C.sizeof(RobustKernel)
 assert SIMILARITY_DTYPE.itemsize == C.sizeof(Similarity) == 104, C.sizeof(Similarity)
 assert ICP_RESULT_DTYPE.itemsize == C.sizeof(IcpResult) == 136, (ICP_RESULT_DTYPE.itemsize, C.sizeof(IcpResult))
@@ -217,6 +238,7 @@ _SYMBOLS = [
     "tzr_icp_colored", "tzr_icp_colored_batch", "tzr_voxel_downsample_colors", "tzr_voxel_downsample_colors_batch",
     "tzr_register_cloud_pairs_icp_colored", "tzr_register_cloud_pairs_multiway_colored", "tzr_icp_multiscale_batch",
     "tzr_fgr_params_default", "tzr_fgr", "tzr_fgr_batch", "tzr_register_cloud_pairs_fgr",
+    "tzr_ransac_params_default", "tzr_ransac", "tzr_ransac_batch", "tzr_register_cloud_pairs_ransac",
 ]
 
 # status codes (tzr_status)
@@ -407,6 +429,15 @@ def lib():
     L.tzr_register_cloud_pairs_fgr.argtypes = [vp, C.POINTER(FrontendParams), C.POINTER(FgrParams), C.c_int, i32p, fpp,
                                                C.c_int, i32p, u64p, i32p, i64p, C.POINTER(i32p), fp,
                                                C.POINTER(IcpResult)]
+    L.tzr_ransac_params_default.argtypes = [C.POINTER(RansacParams)]
+    L.tzr_ransac_params_default.restype = None
+    L.tzr_ransac.argtypes = [vp, C.POINTER(RansacParams), fp, C.c_int, fp, C.c_int, C.c_int, i32p, C.c_uint64, fp, fp,
+                             C.POINTER(IcpResult), C.POINTER(RansacInfo), i32p]
+    L.tzr_ransac_batch.argtypes = [vp, C.POINTER(RansacParams), C.c_int, i32p, fpp, i32p, fpp, i32p, C.POINTER(i32p),
+                                   u64p, fpp, fpp, C.POINTER(IcpResult), C.POINTER(RansacInfo), C.POINTER(i32p)]
+    L.tzr_register_cloud_pairs_ransac.argtypes = [vp, C.POINTER(FrontendParams), C.POINTER(RansacParams), C.c_int,
+                                                  i32p, fpp, C.c_int, i32p, u64p, u64p, i32p, i64p, C.POINTER(i32p),
+                                                  fp, C.POINTER(IcpResult), C.POINTER(RansacInfo)]
     for s in _SYMBOLS:
         getattr(L, s)  # raises AttributeError if the header and the library disagree
     _lib = L
@@ -457,6 +488,29 @@ def fgr_params(**kw) -> FgrParams:
             raise AttributeError(k)
         setattr(p, k, v)
     return p
+
+
+def ransac_params(max_correspondence_distance, **kw) -> RansacParams:
+    """tzr_ransac_params_default (Open3D's defaults: ransac_n 3, 100000 iterations, confidence 0.999, no checkers) at
+    max_correspondence_distance, with any field in kw set; the library checks the values."""
+    p = RansacParams()
+    lib().tzr_ransac_params_default(C.byref(p))
+    p.max_correspondence_distance = float(max_correspondence_distance)
+    for k, v in kw.items():
+        if not hasattr(p, k):
+            raise AttributeError(k)
+        setattr(p, k, v)
+    return p
+
+
+def _seeds64(seeds, n, what):
+    """n 64-bit seeds as a uint64 array (None: zeros); Python integers taken modulo 2^64."""
+    if seeds is None:
+        return np.zeros(n, dtype=np.uint64)
+    a = np.array([int(x) % (1 << 64) for x in seeds], dtype=np.uint64)
+    if a.shape != (n,):
+        raise TzrError(f"{what}: one seed per problem is required")
+    return a
 
 
 def corr_rows(corr, what="fgr"):
@@ -1434,6 +1488,48 @@ class Context:
             self._ck(rc)
         return status, [c[:k].copy() for c, k in zip(corr, cnt)], [float(x) for x in g], res
 
+    def register_cloud_pairs_ransac(self, clouds, pairs, ransac: RansacParams, normal_search_radius=0.03,
+                                    fpfh_search_radius=0.05, use_absolute_scale=True, use_crosscheck=True,
+                                    use_tuple_test=True, tuple_scale=0.0, tuple_seeds=None, ransac_seeds=None):
+        """tzr_register_cloud_pairs_ransac: register_cloud_pairs' front end (FPFH of every (n,3) float32 cloud,
+        matching of every (source cloud, target cloud) pair), then RANSAC of every pair with correspondences on its
+        matched rows (seed ransac_seeds[p], None: 0; the normal checker reads the FPFH stage's normals), with no robust
+        solve.  Returns (status (P,) int32, correspondences (list of (m_p,2) int32), global scales (list of floats),
+        RANSAC records (structured array (P,) of ICP_RESULT_DTYPE), infos (structured array (P,) of
+        RANSAC_INFO_DTYPE)), both zeroed for a pair that was not registered.  The call raises only for errors of the
+        whole call; TZR_ERR_TOO_LARGE of some pairs is reported in status."""
+        cl = [np.ascontiguousarray(c, dtype=np.float32) for c in clouds]
+        if not cl or any(c.ndim != 2 or c.shape[1] != 3 or c.shape[0] == 0 for c in cl):
+            raise TzrError("register_cloud_pairs_ransac: a non-empty list of non-empty (n,3) clouds is required")
+        pc = np.ascontiguousarray(pairs, dtype=np.int32).reshape(-1, 2)
+        P = pc.shape[0]
+        if P == 0:
+            raise TzrError("register_cloud_pairs_ransac: at least one pair is required")
+        if pc.min() < 0 or pc.max() >= len(cl):
+            raise TzrError("register_cloud_pairs_ransac: a pair names a cloud that is not in the list")
+        seeds = _seeds64(tuple_seeds, P, "register_cloud_pairs_ransac")
+        rseeds = _seeds64(ransac_seeds, P, "register_cloud_pairs_ransac")
+        n = np.array([c.shape[0] for c in cl], dtype=np.int32)
+        fpar = FrontendParams(float(normal_search_radius), float(fpfh_search_radius), int(bool(use_absolute_scale)),
+                              int(bool(use_crosscheck)), int(bool(use_tuple_test)), float(tuple_scale))
+        corr = [np.zeros((int(n[a]) + int(n[b]), 2), dtype=np.int32) for a, b in pc]
+        status = np.zeros(P, dtype=np.int32)
+        cnt = np.zeros(P, dtype=np.int64)
+        g = np.zeros(P, dtype=np.float32)
+        res = np.zeros(P, dtype=ICP_RESULT_DTYPE)
+        info = np.zeros(P, dtype=RANSAC_INFO_DTYPE)
+        fp, i32p = C.POINTER(C.c_float), C.POINTER(C.c_int32)
+        rc = lib().tzr_register_cloud_pairs_ransac(self._h, C.byref(fpar), C.byref(ransac), len(cl),
+                                                   _p(n, C.c_int32), (fp * len(cl))(*[_p(c, C.c_float) for c in cl]),
+                                                   P, _p(pc, C.c_int32), _p(seeds, C.c_uint64),
+                                                   _p(rseeds, C.c_uint64), _p(status, C.c_int32),
+                                                   _p(cnt, C.c_int64), (i32p * P)(*[_p(c, C.c_int32) for c in corr]),
+                                                   _p(g, C.c_float), res.ctypes.data_as(C.POINTER(IcpResult)),
+                                                   info.ctypes.data_as(C.POINTER(RansacInfo)))
+        if rc not in (0, TZR_ERR_TOO_LARGE):
+            self._ck(rc)
+        return status, [c[:k].copy() for c, k in zip(corr, cnt)], [float(x) for x in g], res, info
+
     def register_multiway(self, clouds, pairs, params: Params, max_correspondence_distance, uncertain=None,
                           normal_search_radius=0.03, fpfh_search_radius=0.05, use_absolute_scale=True,
                           use_crosscheck=True, use_tuple_test=True, tuple_scale=0.0, tuple_seeds=None, max_iteration=30,
@@ -1566,6 +1662,59 @@ class Context:
                                      (i32p * B)(*[_p(e, C.c_int32) for e in ev]))
         self._ck(rc)
         return res, [e[:int(r["n_correspondences"])].copy() for e, r in zip(ev, res)]
+
+    def ransac(self, src, dst, corr, ransac: RansacParams, seed=0, src_normals=None, dst_normals=None):
+        """tzr_ransac: correspondence RANSAC of the (ns,3) source onto the (nd,3) target (float32) on the (K,2)
+        correspondences corr (source index, target index), with a 64-bit seed; the normals ((n,3) or (n,4)) are
+        needed by the normal checker only.  Returns (result dict as icp_result_dict, info dict (RANSAC_INFO_DTYPE's
+        fields), the evaluation's correspondences (m,2) int32 ascending by source)."""
+        res, info, ev = self.ransac_batch([src], [dst], [corr], ransac, seeds=[seed],
+                                          src_normals=None if src_normals is None else [src_normals],
+                                          dst_normals=None if dst_normals is None else [dst_normals], single=True)
+        return icp_result_dict(res[0]), {k: info[0][k].item() for k in RANSAC_INFO_DTYPE.names}, ev[0]
+
+    def ransac_batch(self, srcs, dsts, corrs, ransac: RansacParams, seeds=None, src_normals=None, dst_normals=None,
+                     single=False):
+        """tzr_ransac_batch over B (source, target, correspondences) problems; corrs: one (K_b,2) integer array per
+        problem (K_b = 0 allowed); seeds: B 64-bit seeds (None: 0); src_normals, dst_normals: B arrays each, or None.
+        Returns (results structured array (B,) of ICP_RESULT_DTYPE, infos structured array (B,) of RANSAC_INFO_DTYPE,
+        list of B evaluation correspondence arrays).  single=True goes through tzr_ransac (B must be 1)."""
+        S = [_cloud32(a, "ransac") for a in srcs]
+        D = [_cloud32(a, "ransac") for a in dsts]
+        B = len(S)
+        if B == 0 or len(D) != B or len(corrs) != B:
+            raise TzrError("ransac_batch: one target and one correspondence array per source cloud are required")
+        K = [corr_rows(c, "ransac_batch") for c in corrs]
+        sd = _seeds64(seeds, B, "ransac_batch")
+        SN = None if src_normals is None else [_normals32(a, s.shape[0], "ransac") for a, s in zip(src_normals, S)]
+        DN = None if dst_normals is None else [_normals32(a, d.shape[0], "ransac") for a, d in zip(dst_normals, D)]
+        if (SN is not None and len(SN) != B) or (DN is not None and len(DN) != B):
+            raise TzrError("ransac_batch: one normals array per problem is required")
+        res = np.zeros(B, dtype=ICP_RESULT_DTYPE)
+        info = np.zeros(B, dtype=RANSAC_INFO_DTYPE)
+        out = res.ctypes.data_as(C.POINTER(IcpResult))
+        iout = info.ctypes.data_as(C.POINTER(RansacInfo))
+        ev = [np.zeros((a.shape[0], 2), dtype=np.int32) for a in S]
+        fp, i32p = C.POINTER(C.c_float), C.POINTER(C.c_int32)
+        if single:
+            assert B == 1
+            rc = lib().tzr_ransac(self._h, C.byref(ransac), _p(S[0], C.c_float), S[0].shape[0], _p(D[0], C.c_float),
+                                  D[0].shape[0], K[0].shape[0], _p(K[0], C.c_int32), int(sd[0]),
+                                  None if SN is None else _p(SN[0], C.c_float),
+                                  None if DN is None else _p(DN[0], C.c_float), out, iout, _p(ev[0], C.c_int32))
+        else:
+            ns = np.array([a.shape[0] for a in S], dtype=np.int32)
+            nd = np.array([a.shape[0] for a in D], dtype=np.int32)
+            nc = np.array([k.shape[0] for k in K], dtype=np.int32)
+            rc = lib().tzr_ransac_batch(self._h, C.byref(ransac), B, _p(ns, C.c_int32),
+                                        (fp * B)(*[_p(a, C.c_float) for a in S]), _p(nd, C.c_int32),
+                                        (fp * B)(*[_p(a, C.c_float) for a in D]), _p(nc, C.c_int32),
+                                        (i32p * B)(*[_p(k, C.c_int32) for k in K]), _p(sd, C.c_uint64),
+                                        None if SN is None else (fp * B)(*[_p(a, C.c_float) for a in SN]),
+                                        None if DN is None else (fp * B)(*[_p(a, C.c_float) for a in DN]), out, iout,
+                                        (i32p * B)(*[_p(e, C.c_int32) for e in ev]))
+        self._ck(rc)
+        return res, info, [e[:int(r["n_correspondences"])].copy() for e, r in zip(ev, res)]
 
     def icp_point_to_plane(self, src, dst, dst_normals, max_correspondence_distance, init=None, max_iteration=30,
                            relative_fitness=1e-6, relative_rmse=1e-6, kernel=None):

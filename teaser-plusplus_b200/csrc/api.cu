@@ -138,6 +138,8 @@ struct tzr_ctx {
   DevBuf pg;
   // tzr_fgr(_batch) and tzr_register_cloud_pairs_fgr: FGR's tables and normalised rows (its evaluation uses icp)
   DevBuf fgr;
+  // tzr_ransac(_batch) and tzr_register_cloud_pairs_ransac: RANSAC's tables, rows, hypotheses and partial sums
+  DevBuf ransac;
   int last_strip_blocks = 0;  // strip length of the most recent graph kernel launch (tzr_ctx_last_strip_blocks)
   int max_n = kMaxN;  // per-problem size limit of this context (tzr_ctx_set_max_n: kMaxN ... kMaxNLarge)
   // pinned host staging
@@ -2455,6 +2457,86 @@ static void fgr_result_of(const IcpProb& pr, const FgrProb& fp, tzr_icp_result* 
   out->converged = fp.converged;
 }
 
+// RANSAC (DESIGN.md §3.21): the header's ranges
+static bool ransac_params_ok(const tzr_ransac_params* p) {
+  auto flag = [](int32_t f) { return f == 0 || f == 1; };
+  return p && std::isfinite(p->max_correspondence_distance) && p->max_correspondence_distance > 0 &&
+         p->ransac_n >= 3 && p->ransac_n <= kRansacMaxN && p->max_iteration >= 0 && p->confidence >= 0 &&
+         p->confidence <= 1 && flag(p->check_edge_length) && flag(p->check_distance) && flag(p->check_normal) &&
+         (!p->check_edge_length || std::isfinite(p->edge_length_similarity)) &&
+         (!p->check_distance || std::isfinite(p->distance_threshold)) &&
+         (!p->check_normal || std::isfinite(p->normal_angle_threshold));
+}
+
+// the ICP settings of RANSAC's evaluation: tzr_icp_batch with max_iteration = 0 at RANSAC's distance
+static void ransac_eval_settings(IcpPlan* plan, const tzr_ransac_params& p) {
+  tzr_icp_params ip;
+  tzr_icp_params_default(&ip);
+  ip.max_correspondence_distance = p.max_correspondence_distance;
+  ip.max_iteration = 0;
+  icp_iteration_settings(plan, ip, kIcpPointToPoint, 0.0, nullptr);
+}
+
+// RANSAC's record of a problem: the evaluation's fields from its ICP problem, the loop's from its RANSAC problem
+static void ransac_result_of(const IcpProb& pr, const RansacProb& rp, tzr_icp_result* out, tzr_ransac_info* info) {
+  icp_result_of(pr, out);
+  out->iterations = rp.drawn;
+  out->converged = rp.converged;
+  if (!info) return;
+  memset(info, 0, sizeof(*info));
+  info->drawn = rp.drawn;
+  info->passed = rp.passed;
+  info->winner = rp.best;
+  info->inliers = rp.best >= 0 ? rp.best_count : 0;
+  info->usable = rp.Kv;
+  info->rmse = rp.best >= 0 ? rp.best_rmse : 0.0;
+}
+
+// ctx->ransac: [problems | (own_corr) correspondences | (staged normals: NS, ND x float4) | usable rows (K x 6 floats) |
+// (normal checker) their normals | hypotheses (B x cap) | tile counts | partial sums (B x nseg x cap double2)]
+struct RansacLayout {
+  size_t corr, snrm, dnrm, rows, nrows, hyps, cnt, partial, end;
+};
+static RansacLayout ransac_layout(int B, long long K, bool own_corr, size_t NS, size_t ND, bool normals, int cap,
+                                  int nseg) {
+  RansacLayout L;
+  L.corr = al256((size_t)B * sizeof(RansacProb));
+  L.snrm = L.corr + (own_corr ? al256((size_t)K * 8) : 0);
+  L.dnrm = L.snrm + al256(NS * 16);
+  L.rows = L.dnrm + al256(ND * 16);
+  L.nrows = L.rows + al256((size_t)K * 24);
+  L.hyps = L.nrows + al256(normals ? (size_t)K * 24 : 0);
+  L.cnt = L.hyps + al256((size_t)B * cap * sizeof(RansacHyp));
+  L.partial = L.cnt + al256((size_t)B * (cap / kRansacThreads) * 4);
+  L.end = L.partial + (size_t)B * nseg * cap * sizeof(double2);
+  return L;
+}
+
+// the kernels' arguments over the workspace at d (the problems, clouds, correspondences and normals are set by the
+// caller)
+static RansacArgs ransac_args(const tzr_ransac_params& p, const RansacLayout& L, char* d, int cap, int nseg) {
+  RansacArgs a{};
+  a.probs = (RansacProb*)d;
+  a.rows = (float*)(d + L.rows);
+  a.nrows = (float*)(d + L.nrows);
+  a.hyps = (RansacHyp*)(d + L.hyps);
+  a.tile_cnt = (int*)(d + L.cnt);
+  a.partial = (double2*)(d + L.partial);
+  a.cap = cap;
+  a.nseg = nseg;
+  a.n = p.ransac_n;
+  a.max_iteration = p.max_iteration;
+  a.check_edge = p.check_edge_length;
+  a.check_dist = p.check_distance;
+  a.check_normal = p.check_normal;
+  a.r2 = p.max_correspondence_distance * p.max_correspondence_distance;
+  a.edge_sim = p.edge_length_similarity;
+  a.dist_thr = p.distance_threshold;
+  a.cos_normal = p.check_normal ? std::cos(p.normal_angle_threshold) : 0.0;
+  a.log1mc = std::log(1.0 - p.confidence);
+  return a;
+}
+
 // [problems | normalised rows (K x 6 doubles)] of ctx->fgr, and (corr_bytes > 0) the correspondences between them
 struct FgrLayout {
   size_t corr, pq, end;
@@ -2479,6 +2561,9 @@ static FgrLayout fgr_layout(int B, long long K, bool own_corr) {
 // fgr (may be NULL; then params and solutions are not used and may be NULL): no solve; FGR of every pair with
 // correspondences on its matched rows (still in m_out) and its two clouds (in m_in), evaluated as tzr_fgr_batch
 // evaluates it; fgr_results (P entries) then receives the records, zeroed for a pair that was not registered.
+// ransac (may be NULL; as fgr, and not with it): RANSAC of every pair with correspondences instead, with seed
+// ransac_seeds[p] (NULL: 0) and the FPFH stage's normals, evaluated as tzr_ransac_batch evaluates it; the records go to
+// fgr_results and the per-pair summaries to ransac_info (may be NULL), zeroed for a pair that was not registered.
 static int register_pairs_run(tzr_ctx* ctx, const tzr_frontend_params* fp, const tzr_params* params, int n_clouds,
                               const int32_t* n, const float* const* pts, int P, const int32_t* pair_clouds,
                               const uint64_t* tuple_seeds, tzr_solution* solutions, int32_t* status,
@@ -2487,13 +2572,18 @@ static int register_pairs_run(tzr_ctx* ctx, const tzr_frontend_params* fp, const
                               int icp_mode = kIcpPointToPoint, double icp_epsilon = 0,
                               const tzr_robust_kernel* icp_kernel = nullptr, const MultiwayOut* mw = nullptr,
                               const float* const* colors = nullptr, double lambda_geometric = 0,
-                              const tzr_fgr_params* fgr = nullptr, tzr_icp_result* fgr_results = nullptr) {
+                              const tzr_fgr_params* fgr = nullptr, tzr_icp_result* fgr_results = nullptr,
+                              const tzr_ransac_params* ransac = nullptr, const uint64_t* ransac_seeds = nullptr,
+                              tzr_ransac_info* ransac_info = nullptr) {
   const bool colored = icp && icp_mode == kIcpColored;
-  if (!ctx || !fp || (!params && !fgr) || n_clouds < 1 || !n || !pts || P < 1 || !pair_clouds ||
-      (!solutions && !fgr) || !status || !n_corr || !(fp->normal_search_radius > 0) || !(fp->fpfh_search_radius > 0))
+  const bool global = fgr || ransac;  // a global registration of every pair with correspondences instead of the solve
+  if (!ctx || !fp || (!params && !global) || n_clouds < 1 || !n || !pts || P < 1 || !pair_clouds ||
+      (!solutions && !global) || !status || !n_corr || !(fp->normal_search_radius > 0) ||
+      !(fp->fpfh_search_radius > 0))
     return TZR_ERR_INVALID_ARG;
   if (icp && (!icp_params_ok(icp) || !icp_results)) return TZR_ERR_INVALID_ARG;
   if (fgr && (icp || !fgr_params_ok(fgr) || !fgr_results)) return TZR_ERR_INVALID_ARG;
+  if (ransac && (icp || fgr || !ransac_params_ok(ransac) || !fgr_results)) return TZR_ERR_INVALID_ARG;
   if (mw && (!icp || params->estimate_scaling || !mw->uncertain || !pg_params_ok(mw->pg) || !mw->information ||
              !mw->info_counts || !mw->edge_weights || !mw->edge_mask || !mw->poses || !mw->pg_status))
     return TZR_ERR_INVALID_ARG;
@@ -2558,7 +2648,11 @@ static int register_pairs_run(tzr_ctx* ctx, const tzr_frontend_params* fp, const
   // layout's own slot for it in ctx->icp stays unused.
   IcpPlan iplan;
   if (fgr) fgr_eval_settings(&iplan, *fgr);  // FGR's evaluation: the same planning over the registered pairs
-  const double icp_r = icp ? icp->max_correspondence_distance : fgr ? fgr->maximum_correspondence_distance : 0.0;
+  if (ransac) ransac_eval_settings(&iplan, *ransac);  // RANSAC's, likewise
+  const double icp_r = icp      ? icp->max_correspondence_distance
+                       : fgr    ? fgr->maximum_correspondence_distance
+                       : ransac ? ransac->max_correspondence_distance
+                                : 0.0;
   std::vector<FpfhCloud> iclouds, gclouds;
   std::vector<IcpProb> iprobs;
   std::vector<int> ichunks;
@@ -2574,7 +2668,7 @@ static int register_pairs_run(tzr_ctx* ctx, const tzr_frontend_params* fp, const
                     &ichunks);
   };
   IcpLayout il{};
-  if (icp || fgr) {
+  if (icp || global) {
     std::vector<int> every(P);
     for (int p = 0; p < P; ++p) every[p] = p;
     if (icp) icp_iteration_settings(&iplan, *icp, icp_mode, icp_epsilon, icp_kernel);
@@ -2593,13 +2687,14 @@ static int register_pairs_run(tzr_ctx* ctx, const tzr_frontend_params* fp, const
     }
     il = icp_layout(iplan, 0, mw != nullptr);
   }
-  // FGR: its problem table (staged in, read back) after the ICP tables
+  // FGR and RANSAC: their problem table (staged in, read back) after the ICP tables
   const size_t hi_tab = al256(pin_base), hi_info = al256(hi_tab + il.match),
                hi_icnt = hi_info + al256((size_t)P * 36 * 8), hi_fgr = hi_info,
-               pin_bytes = mw    ? hi_icnt + (size_t)P * 4
-                           : fgr ? hi_fgr + (size_t)P * sizeof(FgrProb)
-                           : icp ? hi_tab + il.match
-                                 : pin_base;
+               pin_bytes = mw       ? hi_icnt + (size_t)P * 4
+                           : fgr    ? hi_fgr + (size_t)P * sizeof(FgrProb)
+                           : ransac ? hi_fgr + (size_t)P * sizeof(RansacProb)
+                           : icp    ? hi_tab + il.match
+                                    : pin_base;
   int rc;
   if ((rc = ensure(ctx, ctx->m_in, in_bytes)) != TZR_OK) return rc;
   if ((rc = ensure(ctx, ctx->m_scratch, scratch_bytes)) != TZR_OK) return rc;
@@ -2609,6 +2704,9 @@ static int register_pairs_run(tzr_ctx* ctx, const tzr_frontend_params* fp, const
     if ((rc = ensure(ctx, ctx->icp, il.end)) != TZR_OK) return rc;
     if ((rc = ensure(ctx, ctx->fgr, fgr_layout(P, (long long)C, false).end)) != TZR_OK) return rc;
   }
+  // RANSAC's evaluation likewise; its own workspace depends on the largest matched count and is sized once the counts
+  // are known, before its first launch
+  if (ransac && (rc = ensure(ctx, ctx->icp, il.end)) != TZR_OK) return rc;
   char* h = (char*)ctx->h_pin;
   char* d_in = (char*)ctx->m_in.p;
   char* d_out = (char*)ctx->m_out.p;
@@ -2672,7 +2770,7 @@ static int register_pairs_run(tzr_ctx* ctx, const tzr_frontend_params* fp, const
       status[p] = TZR_ERR_INVALID_ARG;
       continue;
     }
-    if (fgr) {  // every pair with correspondences is registered on its gathered index rows
+    if (global) {  // every pair with correspondences is registered on its gathered index rows
       status[p] = TZR_OK;
       PairGather& g = table[n_table++];
       g.src_lo = cloud_lo[p].x;
@@ -2728,7 +2826,7 @@ static int register_pairs_run(tzr_ctx* ctx, const tzr_frontend_params* fp, const
   if (S > 0) {
     rc = solve_ragged_dev(ctx, *params, S, solved_n.data(), d_src, d_dst, d_sol, want_clq ? d_clq : nullptr);
     if (rc) return rc;
-  } else if (!fgr) {  // nothing solved: no solve is retained (FGR is not a solve entry and leaves it as it is)
+  } else if (!global) {  // nothing solved: no solve is retained (FGR and RANSAC are not solve entries)
     forget_retained(ctx);
   }
   // FGR of the registered pairs on their gathered rows and their clouds in place, then its evaluation (DESIGN.md §3.20)
@@ -2758,6 +2856,46 @@ static int register_pairs_run(tzr_ctx* ctx, const tzr_frontend_params* fp, const
     if ((rc = check_launch(ctx, "fgr launch")) != TZR_OK) return rc;
     CK(cudaMemcpyAsync(hi + il.probs, buf.probs, (size_t)R * sizeof(IcpProb), cudaMemcpyDeviceToHost, st));
     CK(cudaMemcpyAsync(hf, df, (size_t)R * sizeof(FgrProb), cudaMemcpyDeviceToHost, st));
+  }
+  // RANSAC of the registered pairs on their gathered rows, their clouds and the FPFH stage's normals in place (still in
+  // m_out, indexed like the cloud table), then its evaluation (DESIGN.md §3.21)
+  RansacProb* hr = (RansacProb*)(h + hi_fgr);
+  if (ransac && R > 0) {
+    plan_icp(registered);  // a subset of the pairs planned above: it fits
+    il = icp_layout(iplan, 0, false);
+    long long k_max = 0;
+    for (int p : registered) k_max = std::max(k_max, (long long)n_corr[p]);
+    std::vector<int> spans;
+    int cap, nseg;
+    ransac_schedule(ransac->max_iteration, k_max, &spans, &cap, &nseg);
+    const RansacLayout rl = ransac_layout(R, corr_rows, false, 0, 0, ransac->check_normal != 0, cap, nseg);
+    if ((rc = ensure(ctx, ctx->ransac, rl.end)) != TZR_OK) return rc;
+    char* hi = h + hi_tab;
+    memcpy(hi + il.probs, iprobs.data(), (size_t)R * sizeof(IcpProb));
+    memcpy(hi + il.clouds, iclouds.data(), (size_t)n_clouds * sizeof(FpfhCloud));
+    memcpy(hi + il.chunks, ichunks.data(), ichunks.size() * 4);
+    for (int k = 0; k < R; ++k) {
+      hr[k] = RansacProb{};
+      hr[k].c_lo = corr_row[registered[k]];
+      hr[k].K = (int)n_corr[registered[k]];
+      hr[k].seed = ransac_seeds ? ransac_seeds[registered[k]] : 0;
+    }
+    char* di = (char*)ctx->icp.p;
+    char* dr = (char*)ctx->ransac.p;
+    CK(cudaMemcpyAsync(di, hi, il.match, cudaMemcpyHostToDevice, st));
+    CK(cudaMemcpyAsync(dr, hr, (size_t)R * sizeof(RansacProb), cudaMemcpyHostToDevice, st));
+    IcpBuffers buf = icp_buffers(di, il);
+    buf.src = buf.dst = d_pts;
+    RansacArgs a = ransac_args(*ransac, rl, dr, cap, nseg);
+    a.icp = buf.probs;
+    a.src = a.dst = d_pts;
+    a.corr = d_corr;
+    if (ransac->check_normal) a.src_normals = a.dst_normals = (const float4*)(d_out + o_nrm);
+    ctx->launches += launch_ransac(a, R, spans, st);
+    ctx->launches += launch_icp(iplan, buf, st);
+    if ((rc = check_launch(ctx, "ransac launch")) != TZR_OK) return rc;
+    CK(cudaMemcpyAsync(hi + il.probs, buf.probs, (size_t)R * sizeof(IcpProb), cudaMemcpyDeviceToHost, st));
+    CK(cudaMemcpyAsync(hr, dr, (size_t)R * sizeof(RansacProb), cudaMemcpyDeviceToHost, st));
   }
   // the refinement of the solved pairs, seeded on the device from their records (no synchronisation, no upload of points)
   char* hi = h + hi_tab;
@@ -2796,7 +2934,7 @@ static int register_pairs_run(tzr_ctx* ctx, const tzr_frontend_params* fp, const
   // synchronisation 2: the records, and the index pairs and cliques that were asked for
   if (S > 0) CK(cudaMemcpyAsync(h + h_sol, d_sol, (size_t)S * sizeof(tzr_solution), cudaMemcpyDeviceToHost, st));
   bool read_corr = corr_rows > 0;
-  if (fgr) {  // FGR gathers every registered pair's rows: read back only when some were asked for
+  if (global) {  // FGR and RANSAC gather every registered pair's rows: read back only when some were asked for
     read_corr = false;
     for (int p : registered) read_corr |= corr && corr[p];
   }
@@ -2826,6 +2964,13 @@ static int register_pairs_run(tzr_ctx* ctx, const tzr_frontend_params* fp, const
   if (fgr) {
     for (int p = 0; p < P; ++p) memset(&fgr_results[p], 0, sizeof(tzr_icp_result));
     for (int k = 0; k < R; ++k) fgr_result_of(hi_probs[k], hf[k], &fgr_results[registered[k]]);
+  }
+  if (ransac) {
+    for (int p = 0; p < P; ++p) memset(&fgr_results[p], 0, sizeof(tzr_icp_result));
+    if (ransac_info) memset(ransac_info, 0, (size_t)P * sizeof(tzr_ransac_info));
+    for (int k = 0; k < R; ++k)
+      ransac_result_of(hi_probs[k], hr[k], &fgr_results[registered[k]],
+                       ransac_info ? &ransac_info[registered[k]] : nullptr);
   }
   if (mw) {  // the pose graph over the refined pairs, in pair order
     memset(mw->information, 0, (size_t)P * 36 * 8);
@@ -2957,6 +3102,18 @@ int tzr_register_cloud_pairs_icp_colored(tzr_ctx* ctx, const tzr_frontend_params
   return register_pairs_run(ctx, fp, params, n_clouds, n, pts, P, pair_clouds, tuple_seeds, solutions, status,
                             problem_index, n_corr, corr, cliques, global_scale, icp, icp_results, kIcpColored, 0,
                             kernel, nullptr, colors, lambda_geometric);
+}
+
+int tzr_register_cloud_pairs_ransac(tzr_ctx* ctx, const tzr_frontend_params* fp, const tzr_ransac_params* ransac,
+                                    int n_clouds, const int32_t* n, const float* const* pts, int P,
+                                    const int32_t* pair_clouds, const uint64_t* tuple_seeds,
+                                    const uint64_t* ransac_seeds, int32_t* status, int64_t* n_corr,
+                                    int32_t* const* corr, float* global_scale, tzr_icp_result* results,
+                                    tzr_ransac_info* info) {
+  if (!ransac) return TZR_ERR_INVALID_ARG;
+  return register_pairs_run(ctx, fp, nullptr, n_clouds, n, pts, P, pair_clouds, tuple_seeds, nullptr, status, nullptr,
+                            n_corr, corr, nullptr, global_scale, nullptr, nullptr, kIcpPointToPoint, 0, nullptr,
+                            nullptr, nullptr, 0, nullptr, results, ransac, ransac_seeds, info);
 }
 
 int tzr_register_cloud_pairs_fgr(tzr_ctx* ctx, const tzr_frontend_params* fp, const tzr_fgr_params* fgr,
@@ -3167,6 +3324,111 @@ void tzr_fgr_params_default(tzr_fgr_params* p) {
   p->decrease_mu = 1;
   p->maximum_correspondence_distance = 0.025;
   p->iteration_number = 64;
+}
+
+// ---- RANSAC (DESIGN.md §3.21) ----------------------------------------------------------------------------------------
+int tzr_ransac_batch(tzr_ctx* ctx, const tzr_ransac_params* params, int B, const int32_t* ns, const float* const* src,
+                     const int32_t* nd, const float* const* dst, const int32_t* n_corr, const int32_t* const* corr,
+                     const uint64_t* seeds, const float* const* src_normals, const float* const* dst_normals,
+                     tzr_icp_result* results, tzr_ransac_info* info, int32_t* const* eval_corr) {
+  if (!ctx || !ransac_params_ok(params) || B < 1 || !ns || !nd || !n_corr || !results) return TZR_ERR_INVALID_ARG;
+  const bool nrm = params->check_normal != 0;
+  if (nrm && (!src_normals || !dst_normals)) return TZR_ERR_INVALID_ARG;
+  long long K = 0, k_max = 0;
+  for (int b = 0; b < B; ++b) {
+    if (ns[b] < 1 || nd[b] < 1 || n_corr[b] < 0 || (n_corr[b] > 0 && (!corr || !corr[b]))) return TZR_ERR_INVALID_ARG;
+    if (nrm && (!src_normals[b] || !dst_normals[b])) return TZR_ERR_INVALID_ARG;
+    for (int k = 0; k < n_corr[b]; ++k) {
+      const int32_t i = corr[b][2 * k], j = corr[b][2 * k + 1];
+      if (i < 0 || i >= ns[b] || j < 0 || j >= nd[b]) return TZR_ERR_INVALID_ARG;
+    }
+    K += n_corr[b];
+    k_max = std::max(k_max, (long long)n_corr[b]);
+  }
+  if (K > 0x7fffffffll) {
+    ctx->last_error = "the batch's " + std::to_string(K) + " correspondences do not fit 32-bit indices";
+    return TZR_ERR_TOO_LARGE;
+  }
+  IcpPlan plan;
+  ransac_eval_settings(&plan, *params);
+  tzr_similarity id;
+  memset(&id, 0, sizeof(id));
+  id.scale = 1.0;
+  id.rotation[0] = id.rotation[4] = id.rotation[8] = 1.0;
+  const std::vector<tzr_similarity> init((size_t)B, id);  // placeholders: ransac_seed_kernel writes every seed
+  std::vector<IcpProb> probs;
+  IcpBuffers buf;
+  int rc = icp_batch_stage(ctx, &plan, B, ns, src, nullptr, nd, dst, nullptr, init.data(),
+                           params->max_correspondence_distance, false, &probs, &buf);
+  if (rc != TZR_OK) return rc;
+  std::vector<int> spans;
+  int cap, nseg;
+  ransac_schedule(params->max_iteration, k_max, &spans, &cap, &nseg);
+  const size_t NS = nrm ? (size_t)plan.NS : 0, ND = nrm ? (size_t)plan.ND : 0;
+  const RansacLayout L = ransac_layout(B, K, true, NS, ND, nrm, cap, nseg);
+  if ((rc = ensure(ctx, ctx->ransac, L.end)) != TZR_OK) return rc;
+  std::vector<char> h(L.rows);
+  RansacProb* rp = (RansacProb*)h.data();
+  long long c_lo = 0;
+  for (int b = 0; b < B; ++b) {
+    rp[b] = RansacProb{};
+    rp[b].c_lo = c_lo;
+    rp[b].K = n_corr[b];
+    rp[b].seed = seeds ? seeds[b] : 0;
+    if (n_corr[b] > 0) memcpy(h.data() + L.corr + (size_t)c_lo * 8, corr[b], (size_t)n_corr[b] * 8);
+    if (nrm) {  // the normals at their points' rows of the staged clouds
+      memcpy(h.data() + L.snrm + (size_t)probs[b].s_lo * 16, src_normals[b], (size_t)ns[b] * 16);
+      memcpy(h.data() + L.dnrm + (size_t)probs[b].d_lo * 16, dst_normals[b], (size_t)nd[b] * 16);
+    }
+    c_lo += n_corr[b];
+  }
+  cudaStream_t st = ctx->stream;
+  char* d = (char*)ctx->ransac.p;
+  CK(cudaMemcpyAsync(d, h.data(), L.rows, cudaMemcpyHostToDevice, st));
+  RansacArgs a = ransac_args(*params, L, d, cap, nseg);
+  a.icp = buf.probs;
+  a.src = buf.src;
+  a.dst = buf.dst;
+  a.corr = (const int2*)(d + L.corr);
+  if (nrm) {
+    a.src_normals = (const float4*)(d + L.snrm);
+    a.dst_normals = (const float4*)(d + L.dnrm);
+  }
+  ctx->launches += launch_ransac(a, B, spans, st);
+  ctx->launches += launch_icp(plan, buf, st);
+  if ((rc = check_launch(ctx, "ransac launch")) != TZR_OK) return rc;
+  CK(cudaMemcpyAsync(probs.data(), buf.probs, (size_t)B * sizeof(IcpProb), cudaMemcpyDeviceToHost, st));
+  CK(cudaMemcpyAsync(rp, d, (size_t)B * sizeof(RansacProb), cudaMemcpyDeviceToHost, st));
+  bool want_corr = false;
+  for (int b = 0; b < B && eval_corr; ++b) want_corr |= eval_corr[b] != nullptr;
+  std::vector<int32_t> match(want_corr ? (size_t)plan.NS : 0);
+  if (want_corr) CK(cudaMemcpyAsync(match.data(), buf.match, (size_t)plan.NS * 4, cudaMemcpyDeviceToHost, st));
+  CK(cudaStreamSynchronize(st));
+  for (int b = 0; b < B; ++b) {
+    ransac_result_of(probs[b], rp[b], &results[b], info ? &info[b] : nullptr);
+    if (eval_corr && eval_corr[b]) icp_corr_rows(probs[b], match.data(), eval_corr[b]);
+  }
+  return TZR_OK;
+}
+
+int tzr_ransac(tzr_ctx* ctx, const tzr_ransac_params* params, const float* src, int ns, const float* dst, int nd,
+               int n_corr, const int32_t* corr, uint64_t seed, const float* src_normals, const float* dst_normals,
+               tzr_icp_result* result, tzr_ransac_info* info, int32_t* eval_corr) {
+  int32_t* const ec[1] = {eval_corr};
+  const float* const sn[1] = {src_normals};
+  const float* const dn[1] = {dst_normals};
+  return tzr_ransac_batch(ctx, params, 1, &ns, &src, &nd, &dst, &n_corr, &corr, &seed, sn, dn, result, info,
+                          eval_corr ? ec : nullptr);
+}
+
+void tzr_ransac_params_default(tzr_ransac_params* p) {
+  if (!p) return;
+  memset(p, 0, sizeof(*p));
+  p->ransac_n = 3;
+  p->max_iteration = 100000;
+  p->confidence = 0.999;
+  p->edge_length_similarity = 0.9;
+  p->normal_angle_threshold = 0.52359877559829882;
 }
 
 int tzr_icp_batch(tzr_ctx* ctx, const tzr_icp_params* params, int B, const int32_t* ns, const float* const* src,

@@ -316,13 +316,6 @@ __global__ void __launch_bounds__(1024) corres_kernel(const MatchPair* __restric
   if (threadIdx.x == 0) ncorr[blockIdx.x] = base;
 }
 
-__device__ __forceinline__ uint64_t splitmix64(uint64_t x) {
-  x += 0x9E3779B97F4A7C15ull;
-  x = (x ^ (x >> 30)) * 0xBF58476D1CE4E5B9ull;
-  x = (x ^ (x >> 27)) * 0x94D049BB133111EBull;
-  return x ^ (x >> 31);
-}
-
 __device__ __forceinline__ float dist3(const float* a, const float* b) {
   const float x = __fsub_rn(a[0], b[0]), y = __fsub_rn(a[1], b[1]), z = __fsub_rn(a[2], b[2]);
   return __fsqrt_rn(__fadd_rn(__fadd_rn(__fmul_rn(x, x), __fmul_rn(y, y)), __fmul_rn(z, z)));

@@ -484,6 +484,14 @@ int launch_match(const MatchPlan& plan, const MatchPair* pairs, const NnWork* wo
                  int use_crosscheck, int use_tuple_test, float tuple_scale, void* scratch, int32_t* out_pairs,
                  int* counts, float* gscale, int num_sms, cudaStream_t st);
 
+// SplitMix64's output function: the tuple test's trial draws (matcher.cu) and RANSAC's sample draws (ransac.cu)
+__device__ __forceinline__ uint64_t splitmix64(uint64_t x) {
+  x += 0x9E3779B97F4A7C15ull;
+  x = (x ^ (x >> 30)) * 0xBF58476D1CE4E5B9ull;
+  x = (x ^ (x >> 27)) * 0x94D049BB133111EBull;
+  return x ^ (x >> 31);
+}
+
 // register_pairs.cu (tzr_register_cloud_pairs, DESIGN.md §3.10): the handoffs FPFH -> matcher -> ragged solve
 struct PairGather {     // one per pair whose matcher rows go on, built on the host from the read-back counts
   int src_lo, dst_lo;   // first point of the pair's source / target cloud in the flat cloud array
@@ -681,6 +689,59 @@ struct FgrProb {        // one per problem; the host fills c_lo and K, the kerne
 // rows; pq: sum K x 6 doubles of scratch.
 int launch_fgr(const tzr_fgr_params& prm, int B, FgrProb* probs, IcpProb* icp, const float* src, const float* dst,
                const int2* corr, double* pq, cudaStream_t st);
+
+// ransac.cu (RANSAC on correspondences, tzr_ransac_batch, DESIGN.md §3.21): B problems whose clouds are those of B ICP
+// problems, as FGR's.  The hypotheses run in rounds; round i draws hypotheses [start, start + span) of every problem that
+// is still running, and each of its kernels returns at once for a finished problem.
+constexpr int kRansacThreads = 256;   // hypotheses per tile: one CTA of the hypothesis and the score kernels
+constexpr int kRansacSeg = 512;       // rows per score segment (the contract's S)
+constexpr int kRansacMaxN = 16;       // largest ransac_n
+constexpr int kRansacMinRound = 256;  // the first round's span; each later one doubles up to the cap
+constexpr int kRansacMaxRound = 65536;
+constexpr long long kRansacPartialBudget = 1ll << 16;  // cap * segments per problem (the partial sums' entries)
+struct RansacProb {     // one per problem; the host fills c_lo, K and seed, the kernels the rest
+  long long c_lo;       // first row of the problem's correspondences (int2 (i, j)) and of its usable rows
+  unsigned long long seed;
+  int K;                // its correspondences
+  int Kv;               // the usable ones (both ends finite), compacted in input order
+  int done;             // 1: the loop has stopped
+  int passed;           // hypotheses drawn so far that passed every checker
+  int best;             // the winner so far, -1: none
+  int best_count;       // its inliers
+  int drawn, converged; // the seed kernel's summary
+  double exit;          // the confidence bound so far (max_iteration at first)
+  double best_fit, best_rmse;
+  double R[9], t[3];    // the winner's transform (column-major R)
+};
+struct RansacHyp {      // a hypothesis that passed every checker, in its tile's list
+  double R[9], t[3];
+  int itr, pad;
+};
+struct RansacArgs {
+  RansacProb* probs;
+  IcpProb* icp;
+  const float* src;
+  const float* dst;
+  const float4* src_normals;  // NULL unless the normal checker is on (indexed like src, dst)
+  const float4* dst_normals;
+  const int2* corr;
+  float* rows;          // sum K x 6 floats: the usable rows (x, y), compacted
+  float* nrows;         // sum K x 6 floats: their normals (normal checker only)
+  RansacHyp* hyps;      // B x cap
+  int* tile_cnt;        // B x cap / kRansacThreads
+  double2* partial;     // B x nseg x cap: (count, sum d^2) per passing hypothesis and segment
+  int cap, nseg;        // the largest round, and segments of the batch's largest problem
+  int n, max_iteration;
+  int check_edge, check_dist, check_normal;
+  double r2, edge_sim, dist_thr, cos_normal, log1mc;
+};
+// The round schedule: the span of every round (kRansacMinRound, doubling, capped at cap) until max_iteration is covered;
+// cap: kRansacMaxRound halved while cap * nseg > kRansacPartialBudget (not below kRansacMinRound), nseg from the
+// batch's largest K.  Depends on max_iteration and K_max only.
+void ransac_schedule(int max_iteration, long long k_max, std::vector<int>* spans, int* cap, int* nseg);
+// 1 (prep) + 3 per round + 1 (seed) launches; the seed writes every winner into icp[b] (s = 1, active = seeded = 1)
+// for launch_icp to evaluate.
+int launch_ransac(const RansacArgs& a, int B, const std::vector<int>& spans, cudaStream_t st);
 
 // pose_graph.cu (tzr_pose_graph_optimize, DESIGN.md §3.16): one graph of K nodes and E edges, device-resident
 struct PgEdge {         // one per edge; the host fills it, the kernels read it

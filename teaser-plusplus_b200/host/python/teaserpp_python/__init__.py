@@ -13,11 +13,11 @@ from . import _teaserpp as _ext
 # ---- re-exports -----------------------------------------------------------------------------------------------------
 _PUBLIC = ("OMP_MAX_THREADS", "CertificationResult", "ColoredICP", "DRSCertifier", "EigSolverType",
            "FastGlobalRegistration", "GeneralizedICP", "InlierGraphFormulation", "InlierSelectionMode", "MultiScaleICP",
-           "PointToPlaneICP", "PointToPointICP", "PoseGraph", "RegistrationSolution", "RobustKernel",
-           "RobustRegistrationSolver", "RotationEstimationAlgorithm", "estimate_color_gradients",
+           "PointToPlaneICP", "PointToPointICP", "PoseGraph", "RANSACRegistration", "RegistrationSolution",
+           "RobustKernel", "RobustRegistrationSolver", "RotationEstimationAlgorithm", "estimate_color_gradients",
            "estimate_color_gradients_batch", "estimate_normals", "estimate_normals_batch", "information_matrix",
-           "information_matrix_batch", "multiscale_icp", "register_cloud_pairs_fgr", "voxel_down_sample",
-           "voxel_down_sample_batch")
+           "information_matrix_batch", "multiscale_icp", "register_cloud_pairs_fgr", "register_cloud_pairs_ransac",
+           "voxel_down_sample", "voxel_down_sample_batch")
 globals().update({name: getattr(_ext, name) for name in _PUBLIC})
 
 # ---- v1.0 spellings of the enums, kept as class attributes ----------------------------------------------------------

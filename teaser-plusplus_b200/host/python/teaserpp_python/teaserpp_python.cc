@@ -14,6 +14,7 @@
 
 #include "teaser/certification.h"
 #include "teaser/fgr.h"
+#include "teaser/ransac.h"
 #include "teaser/icp.h"
 #include "teaser/pose_graph.h"
 #include "teaser/normals.h"
@@ -169,6 +170,67 @@ py::list fgr_pairs_run(const teaser::FastGlobalRegistration& fgr, const std::vec
     out.append(py::dict(py::arg("status") = r.status, py::arg("correspondences") = r.correspondences,
                         py::arg("global_scale") = r.global_scale, py::arg("registered") = r.registered,
                         py::arg("fgr") = r.registered ? py::object(icp_dict(r.fgr)) : py::object(py::none())));
+  return out;
+}
+
+teaser::RANSACRegistration ransac_of(double max_correspondence_distance, int ransac_n, int max_iteration,
+                                     double confidence, bool check_edge_length, double edge_length_similarity,
+                                     bool check_distance, double distance_threshold, bool check_normal,
+                                     double normal_angle_threshold) {
+  teaser::RANSACRegistration::Params p;
+  p.max_correspondence_distance = max_correspondence_distance;
+  p.ransac_n = ransac_n;
+  p.max_iteration = max_iteration;
+  p.confidence = confidence;
+  p.check_edge_length = check_edge_length;
+  p.edge_length_similarity = edge_length_similarity;
+  p.check_distance = check_distance;
+  p.distance_threshold = distance_threshold;
+  p.check_normal = check_normal;
+  p.normal_angle_threshold = normal_angle_threshold;
+  return teaser::RANSACRegistration(p);
+}
+
+py::dict ransac_info_dict(const teaser::RANSACInfo& i) {
+  return py::dict(py::arg("drawn") = i.drawn, py::arg("passed") = i.passed, py::arg("winner") = i.winner,
+                  py::arg("inliers") = i.inliers, py::arg("usable") = i.usable, py::arg("rmse") = i.rmse);
+}
+
+// an icp dict with the loop's summary under "info"
+py::dict ransac_dict(const teaser::PointToPointICPResult& r, const teaser::RANSACInfo& i) {
+  py::dict d = icp_dict(r);
+  d["info"] = ransac_info_dict(i);
+  return d;
+}
+
+// registerCloudPairs as a list of dicts: status, correspondences, global_scale, registered and ransac (an icp dict
+// with "info", None for a pair that was not registered)
+py::list ransac_pairs_run(const teaser::RANSACRegistration& rs, const std::vector<CloudArray>& clouds,
+                          const std::vector<std::pair<int, int>>& pairs, double normal_search_radius,
+                          double fpfh_search_radius, bool use_absolute_scale, bool use_crosscheck,
+                          bool use_tuple_test, float tuple_scale, uint64_t tuple_seed,
+                          const std::vector<uint64_t>& ransac_seeds) {
+  std::vector<teaser::PointCloud> pcs;
+  for (const auto& a : clouds) pcs.push_back(cloud_of(a));
+  teaser::RANSACRegistration::CloudPairParams cp;
+  cp.normal_search_radius = normal_search_radius;
+  cp.fpfh_search_radius = fpfh_search_radius;
+  cp.use_absolute_scale = use_absolute_scale;
+  cp.use_crosscheck = use_crosscheck;
+  cp.use_tuple_test = use_tuple_test;
+  cp.tuple_scale = tuple_scale;
+  cp.tuple_seed = tuple_seed;
+  std::vector<teaser::RANSACRegistration::CloudPairResult> res;
+  {
+    py::gil_scoped_release release;
+    res = rs.registerCloudPairs(pcs, pairs, cp, ransac_seeds);
+  }
+  py::list out;
+  for (const auto& r : res)
+    out.append(py::dict(py::arg("status") = r.status, py::arg("correspondences") = r.correspondences,
+                        py::arg("global_scale") = r.global_scale, py::arg("registered") = r.registered,
+                        py::arg("ransac") = r.registered ? py::object(ransac_dict(r.ransac, r.info))
+                                                         : py::object(py::none())));
   return out;
 }
 
@@ -679,6 +741,89 @@ PYBIND11_MODULE(_teaserpp, m) {
       py::arg("use_tuple_test") = true, py::arg("tuple_scale") = 0.0f, py::arg("tuple_seed") = 0x7ea5e2ull,
       py::arg("maximum_correspondence_distance") = 0.025, py::arg("iteration_number") = 64,
       py::arg("division_factor") = 1.4, py::arg("fgr_absolute_scale") = false, py::arg("decrease_mu") = true);
+
+  // GPU extra: correspondence RANSAC (teaser::RANSACRegistration) on given correspondences ((K,2) integer arrays) or,
+  // over a cloud table, on matched ones; records are icp dicts (correspondences: the evaluation's) with the loop's
+  // summary under "info"
+  py::class_<teaser::RANSACRegistration>(m, "RANSACRegistration")
+      .def(py::init(&ransac_of), py::arg("max_correspondence_distance"), py::arg("ransac_n") = 3,
+           py::arg("max_iteration") = 100000, py::arg("confidence") = 0.999, py::arg("check_edge_length") = false,
+           py::arg("edge_length_similarity") = 0.9, py::arg("check_distance") = false,
+           py::arg("distance_threshold") = 0.0, py::arg("check_normal") = false,
+           py::arg("normal_angle_threshold") = 0.52359877559829882)
+      .def("register",
+           [](const teaser::RANSACRegistration& rs, const CloudArray& src, const CloudArray& dst,
+              const py::array_t<int32_t, py::array::c_style | py::array::forcecast>& corr, uint64_t seed,
+              const py::object& src_normals, const py::object& dst_normals) {
+             const teaser::PointCloud s = cloud_of(src), d = cloud_of(dst);
+             const auto c = corr_of(corr);
+             teaser::NormalCloud sn, dn;
+             if (!src_normals.is_none()) sn = normals_of(src_normals.cast<CloudArray>());
+             if (!dst_normals.is_none()) dn = normals_of(dst_normals.cast<CloudArray>());
+             teaser::RANSACRegistration::Result r;
+             teaser::RANSACInfo info;
+             {
+               py::gil_scoped_release release;
+               r = rs.registerPair(s, d, c, seed, src_normals.is_none() ? nullptr : &sn,
+                                   dst_normals.is_none() ? nullptr : &dn, &info);
+             }
+             return ransac_dict(r, info);
+           },
+           py::arg("src"), py::arg("dst"), py::arg("corr"), py::arg("seed") = 0, py::arg("src_normals") = py::none(),
+           py::arg("dst_normals") = py::none())
+      .def("register_batch",
+           [](const teaser::RANSACRegistration& rs, const std::vector<CloudArray>& src,
+              const std::vector<CloudArray>& dst,
+              const std::vector<py::array_t<int32_t, py::array::c_style | py::array::forcecast>>& corr,
+              const std::vector<uint64_t>& seeds, const std::vector<CloudArray>& src_normals,
+              const std::vector<CloudArray>& dst_normals) {
+             std::vector<teaser::PointCloud> s, d;
+             std::vector<std::vector<std::pair<int, int>>> c;
+             std::vector<teaser::NormalCloud> sn, dn;
+             for (const auto& a : src) s.push_back(cloud_of(a));
+             for (const auto& a : dst) d.push_back(cloud_of(a));
+             for (const auto& a : corr) c.push_back(corr_of(a));
+             for (const auto& a : src_normals) sn.push_back(normals_of(a));
+             for (const auto& a : dst_normals) dn.push_back(normals_of(a));
+             std::vector<teaser::RANSACRegistration::Result> res;
+             std::vector<teaser::RANSACInfo> info;
+             {
+               py::gil_scoped_release release;
+               res = rs.registerBatch(s, d, c, seeds, sn, dn, &info);
+             }
+             py::list out;
+             for (size_t b = 0; b < res.size(); ++b) out.append(ransac_dict(res[b], info[b]));
+             return out;
+           },
+           py::arg("src"), py::arg("dst"), py::arg("corr"), py::arg("seeds") = std::vector<uint64_t>(),
+           py::arg("src_normals") = std::vector<CloudArray>(), py::arg("dst_normals") = std::vector<CloudArray>())
+      .def("register_cloud_pairs", &ransac_pairs_run, py::arg("clouds"), py::arg("pairs"),
+           py::arg("normal_search_radius") = 0.03, py::arg("fpfh_search_radius") = 0.05,
+           py::arg("use_absolute_scale") = true, py::arg("use_crosscheck") = true, py::arg("use_tuple_test") = true,
+           py::arg("tuple_scale") = 0.0f, py::arg("tuple_seed") = 0x7ea5e2ull,
+           py::arg("ransac_seeds") = std::vector<uint64_t>());
+  m.def(
+      "register_cloud_pairs_ransac",
+      [](const std::vector<CloudArray>& clouds, const std::vector<std::pair<int, int>>& pairs,
+         double max_correspondence_distance, double normal_search_radius, double fpfh_search_radius,
+         bool use_absolute_scale, bool use_crosscheck, bool use_tuple_test, float tuple_scale, uint64_t tuple_seed,
+         const std::vector<uint64_t>& ransac_seeds, int ransac_n, int max_iteration, double confidence,
+         bool check_edge_length, double edge_length_similarity, bool check_distance, double distance_threshold,
+         bool check_normal, double normal_angle_threshold) {
+        return ransac_pairs_run(ransac_of(max_correspondence_distance, ransac_n, max_iteration, confidence,
+                                          check_edge_length, edge_length_similarity, check_distance,
+                                          distance_threshold, check_normal, normal_angle_threshold),
+                                clouds, pairs, normal_search_radius, fpfh_search_radius, use_absolute_scale,
+                                use_crosscheck, use_tuple_test, tuple_scale, tuple_seed, ransac_seeds);
+      },
+      py::arg("clouds"), py::arg("pairs"), py::arg("max_correspondence_distance"),
+      py::arg("normal_search_radius") = 0.03, py::arg("fpfh_search_radius") = 0.05,
+      py::arg("use_absolute_scale") = true, py::arg("use_crosscheck") = true, py::arg("use_tuple_test") = true,
+      py::arg("tuple_scale") = 0.0f, py::arg("tuple_seed") = 0x7ea5e2ull,
+      py::arg("ransac_seeds") = std::vector<uint64_t>(), py::arg("ransac_n") = 3, py::arg("max_iteration") = 100000,
+      py::arg("confidence") = 0.999, py::arg("check_edge_length") = false, py::arg("edge_length_similarity") = 0.9,
+      py::arg("check_distance") = false, py::arg("distance_threshold") = 0.0, py::arg("check_normal") = false,
+      py::arg("normal_angle_threshold") = 0.52359877559829882);
 
   // GPU extra: coloured ICP's colour gradients (teaser::estimateColorGradients), as (n,3) float64
   m.def("estimate_color_gradients",
