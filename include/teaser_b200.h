@@ -1289,6 +1289,123 @@ int tzr_register_cloud_pairs_multiway_colored(
     const tzr_pose_graph_params* pg, double* information, int32_t* info_counts, double* edge_weights,
     uint8_t* edge_mask, tzr_similarity* poses, tzr_pose_graph_summary* pg_summary, int32_t* pg_status);
 
+/* ---- multiway registration: Open3D's line process ---------------------------------------------------------------
+ * A second pose-graph optimiser beside the GNC-TLS one above: Open3D's global_optimization with
+ * GlobalOptimizationLevenbergMarquardt (Choi, Zhou and Koltun 2015, the line process), written from Open3D's
+ * GlobalOptimization.cpp.  Open3D cannot be run beside this library's tests, so this text is the contract and
+ * tests/line_process_reference.py is its executable form; where the two differ from Open3D, DESIGN.md §3.22 says so.
+ * One graph per call (DESIGN.md §3.22):
+ *   - Graph: nodes T_k (cloud k -> world), 2 <= K <= 1024 (K > 1024 is TZR_ERR_TOO_LARGE); edges (s, d, X = T_sd,
+ *     Lambda, uncertain) with p_d ~ X p_s, validated exactly as tzr_pose_graph_optimize validates them (rigid to 1e-6,
+ *     finite, Lambda(5,5) >= 0, the edges with s != d and Lambda(5,5) > 0 connecting every node, else
+ *     TZR_ERR_INVALID_ARG).  Initial poses: initial_poses, or NULL: tzr_pose_graph_optimize's breadth-first start from
+ *     reference_node (node 0 when reference_node = -1).  Every confidence l_e starts at 1.
+ *   - Misalignment: M_e = X^-1 T_d^-1 T_s, zeta_e = lin(M_e) = ((M21 - M12) / 2, (M02 - M20) / 2, (M10 - M01) / 2, M03,
+ *     M13, M23).  Jacobians: G_0, G_1, G_2 the skew generators about x, y, z, G_3, G_4, G_5 the unit translations;
+ *     J_s[:, i] = lin(X^-1 T_d^-1 G_i T_s), J_d = -J_s.  They are the exact derivatives of zeta under the update.
+ *   - Update: every node is free (no fixed node); T_k <- V(delta_k) T_k, V(d) = [R_z(d2) R_y(d1) R_x(d0) | (d3, d4, d5)]
+ *     (Open3D's TransformVector6dToMatrix4d).  x stacks Open3D's TransformMatrix4dToVector6d of every T_k: with
+ *     sy = sqrt(R00^2 + R10^2), (atan2(R21, R22), atan2(-R20, sy), atan2(R10, R00)), or (atan2(-R12, R11),
+ *     atan2(-R20, sy), 0) when sy < 1e-6; then t_k.
+ *   - Linear system over all 6 K unknowns (gauge included): H = sum_e l_e [J_s^T Lambda J_s, J_s^T Lambda J_d;
+ *     J_d^T Lambda J_s, J_d^T Lambda J_d], b = -sum_e l_e (J_s, J_d)^T Lambda zeta_e, assembled per 6 x 6 block in
+ *     ascending edge index over the edges with s != d and Lambda(5,5) > 0.
+ *   - Line process: mu = preference_loop_closure c^2 mean_e Lambda_e(5,5) over the pass's edges (c =
+ *     max_correspondence_distance; mu = 0 for a pass with no edge); F = sum_e [l_e zeta_e^T Lambda_e zeta_e +
+ *     mu (sqrt(l_e) - 1)^2]; the update l_e = (mu / (mu + zeta_e^T Lambda_e zeta_e))^2 for uncertain edges (the minimiser
+ *     of the edge's term), 1 for certain ones.
+ *   - One pass: F is computed with the incoming confidences, then the confidences are updated and H and b built;
+ *     lambda = 1e-5 max diag(H), nu = 2; stop (TZR_LP_STOP_RIGHT_TERM) if max(b) < min_right_term.  Outer iterations
+ *     while iter < max_iteration, each running trials until one has rho > 0 or the pass stops:
+ *       1. solve (H + lambda I) delta = b (Cholesky; a failed factorisation or a non-finite delta is a rejection, 6);
+ *       2. stop (TZR_LP_STOP_REL_INCREMENT) if |delta| < min_relative_increment (|x| + min_relative_increment);
+ *       3. F' at the candidate poses with the old confidences; rho = (F - F') / (delta . (lambda delta + b) + 1e-3);
+ *       4. rho > 0 and F - F' < min_relative_residual_increment F: stop (TZR_LP_STOP_REL_RESIDUAL), the candidate
+ *          discarded (Open3D leaves its trial loop before applying it);
+ *       5. rho > 0 otherwise: accept; lambda <- lambda max(lower_scale_factor, min(upper_scale_factor,
+ *          1 - (2 rho - 1)^3)), nu <- 2, F <- F'; update the confidences, rebuild H and b, and stop
+ *          (TZR_LP_STOP_RIGHT_TERM) if max(b) < min_right_term;
+ *       6. rho <= 0 (or NaN): reject; lambda <- lambda nu, nu <- 2 nu;
+ *       7. once the outer iteration has run max_iteration_lm trials (Open3D's lm_count >= max_iteration_lm after
+ *          each trial, whatever its outcome; an accepted last trial is kept), stop
+ *          (TZR_LP_STOP_LM_TRIALS).
+ *     After an outer iteration ended by an accepted trial: stop (TZR_LP_STOP_MIN_RESIDUAL) if F < min_residual, then
+ *     (TZR_LP_STOP_MAX_ITERATION) if max_iteration outer iterations have run.
+ *   - Two passes: pass 1 on the whole graph; every uncertain edge with l_e <= edge_prune_threshold is pruned; pass 2
+ *     on the kept edges (in index order) from pass 1's poses and the kept edges' pass-1 confidences, mu recomputed
+ *     over the kept edges.  Pass 2 does not re-check connectivity.
+ *   - Compensation: if 0 <= reference_node < K, every pose T_k <- C T_k with C = T0_ref (T_ref)^-1, T0_ref the
+ *     reference node's starting pose (given, or the breadth-first identity); reference_node = -1 (Open3D's own default)
+ *     skips it.
+ * Reductions: F, |delta|, |x|, delta . (lambda delta + b), max(b) and max diag(H) each run in one fixed order, so the
+ * call is deterministic.  Outputs: poses (K, scale 1); per edge (each may be NULL): confidence (pass 2's for a kept edge,
+ * pass 1's for a pruned one), kept (1 byte) and zeta^T Lambda zeta at the returned poses; summary (may be NULL).  Host
+ * pointers, synchronous.  All control flow runs on the device: the host enqueues trials in chunks of 1, 2, 4, then 8
+ * and reads the state back once per chunk, once between the passes and once at the end; kernels of a stopped pass
+ * return at once, but the chunk's cuSOLVER calls still run.  Launches: per pass 4 + 7 T, with T the trials enqueued:
+ * the first of the chunk ends 1, 3, 7, 15, 23, 31, ... that is >= max(1, trials), at most max_iteration
+ * max_iteration_lm; plus 2 cuSOLVER calls per trial enqueued; then 1 (+ 1 with compensation).
+ * Workspace: ctx's pose-graph workspace (2 (6 K)^2 doubles: about 604 MB at K = 1024), so a retained solve stays
+ * retained.  TZR_ERR_UNSUPPORTED when cuSOLVER cannot be loaded. */
+#define TZR_LP_STOP_RIGHT_TERM 1
+#define TZR_LP_STOP_REL_INCREMENT 2
+#define TZR_LP_STOP_REL_RESIDUAL 3
+#define TZR_LP_STOP_LM_TRIALS 4
+#define TZR_LP_STOP_MIN_RESIDUAL 5
+#define TZR_LP_STOP_MAX_ITERATION 6
+
+typedef struct tzr_line_process_params {
+  double max_correspondence_distance;     /* c: no default; finite and > 0 */
+  double edge_prune_threshold;            /* 0.25; in [0, 1] */
+  double preference_loop_closure;         /* 1.0; finite and > 0 */
+  double min_relative_increment;          /* 1e-6; finite and >= 0 */
+  double min_relative_residual_increment; /* 1e-6; finite and >= 0 */
+  double min_right_term;                  /* 1e-6; finite and >= 0 */
+  double min_residual;                    /* 1e-6; finite and >= 0 */
+  double upper_scale_factor;              /* 2/3; finite, >= lower_scale_factor */
+  double lower_scale_factor;              /* 1/3; finite and > 0 */
+  int32_t reference_node;                 /* 0 (Open3D's tutorial); -1 or a node */
+  int32_t max_iteration;                  /* 100; >= 1 */
+  int32_t max_iteration_lm;               /* 20; >= 1 */
+  int32_t reserved;
+} tzr_line_process_params;
+
+typedef struct tzr_line_process_summary {
+  int32_t iterations[2];   /* outer iterations begun, per pass */
+  int32_t trials[2];       /* trials (linear solves), per pass */
+  int32_t stop_reason[2];  /* TZR_LP_STOP_* per pass */
+  int32_t pruned;          /* uncertain edges pruned after pass 1 */
+  int32_t reserved;
+  double residual;         /* F at the end of pass 2 */
+  double mu[2];            /* mu per pass */
+} tzr_line_process_summary;
+
+/* max_correspondence_distance 0 (the caller must set it) and Open3D's defaults otherwise, reference_node 0. */
+void tzr_line_process_params_default(tzr_line_process_params* p);
+
+/* Arguments as tzr_pose_graph_optimize's; confidence (E doubles), kept (E bytes) and residuals (E doubles) may be NULL. */
+int tzr_pose_graph_optimize_line_process(tzr_ctx* ctx, const tzr_line_process_params* params, int K, int E,
+                                         const int32_t* edges, const tzr_similarity* edge_transforms,
+                                         const double* information, const int32_t* uncertain,
+                                         const tzr_similarity* initial_poses, tzr_similarity* poses,
+                                         double* confidence, uint8_t* kept, double* residuals,
+                                         tzr_line_process_summary* summary);
+
+/* tzr_register_cloud_pairs_multiway_colored's arguments with tzr_line_process_params in place of the GNC-TLS ones:
+ * colors NULL refines by point-to-plane ICP (tzr_register_cloud_pairs_icp_point_to_plane; a non-NULL kernel is then
+ * TZR_ERR_INVALID_ARG), otherwise by coloured ICP; then the information matrices as in tzr_register_cloud_pairs_multiway,
+ * then tzr_pose_graph_optimize_line_process over the refined pairs in pair order.  edge_confidence (P doubles) and
+ * edge_kept (P bytes) take the place of edge_weights and edge_mask, 0 for a pair that is not an edge; lp_status as
+ * pg_status.  Every output equals that chain of public calls bit for bit.  A solve entry. */
+int tzr_register_cloud_pairs_multiway_line_process(
+    tzr_ctx* ctx, const tzr_frontend_params* fparams, const tzr_params* params, int n_clouds, const int32_t* n,
+    const float* const* pts, int P, const int32_t* pair_clouds, const uint64_t* tuple_seeds, tzr_solution* solutions,
+    int32_t* status, int32_t* problem_index, int64_t* n_corr, int32_t* const* corr, int32_t* const* cliques,
+    float* global_scale, const tzr_icp_params* icp, const float* const* colors, double lambda_geometric,
+    const tzr_robust_kernel* kernel, tzr_icp_result* icp_results, const int32_t* uncertain,
+    const tzr_line_process_params* lp, double* information, int32_t* info_counts, double* edge_confidence,
+    uint8_t* edge_kept, tzr_similarity* poses, tzr_line_process_summary* lp_summary, int32_t* lp_status);
+
 /* ---- downsampling point clouds: voxel-grid averaging ----------------------------------------------------------
  * The first step of the reference's FPFH + TEASER++ + ICP tutorial (voxel_down_sample on both raw scans), for many
  * clouds at once.  Open3D's PointCloud::VoxelDownSample, points only, with a defined order.  Per cloud, all arithmetic

@@ -201,11 +201,33 @@ class PoseGraphSummary(C.Structure):
     _fields_ = [("iterations", C.c_int32), ("inner_iterations", C.c_int32), ("cost", C.c_double)]
 
 
+class LineProcessParams(C.Structure):
+    """tzr_line_process_params: Open3D's GlobalOptimizationOption and ConvergenceCriteria for the line process."""
+    _fields_ = [("max_correspondence_distance", C.c_double), ("edge_prune_threshold", C.c_double),
+                ("preference_loop_closure", C.c_double), ("min_relative_increment", C.c_double),
+                ("min_relative_residual_increment", C.c_double), ("min_right_term", C.c_double),
+                ("min_residual", C.c_double), ("upper_scale_factor", C.c_double), ("lower_scale_factor", C.c_double),
+                ("reference_node", C.c_int32), ("max_iteration", C.c_int32), ("max_iteration_lm", C.c_int32),
+                ("reserved", C.c_int32)]
+
+
+class LineProcessSummary(C.Structure):
+    """tzr_line_process_summary: per pass (iterations, trials, stop reason, mu), the pruned count and the final F."""
+    _fields_ = [("iterations", C.c_int32 * 2), ("trials", C.c_int32 * 2), ("stop_reason", C.c_int32 * 2),
+                ("pruned", C.c_int32), ("reserved", C.c_int32), ("residual", C.c_double), ("mu", C.c_double * 2)]
+
+
+# TZR_LP_STOP_*: the rule that stopped a line-process pass
+LP_STOP = {1: "right_term", 2: "relative_increment", 3: "relative_residual", 4: "lm_trials", 5: "min_residual",
+           6: "max_iteration"}
+
 # robust kernel types (TZR_LOSS_*), by the names robust_kernel() accepts
 LOSS_TYPES = {"l2": 0, "l1": 1, "huber": 2, "cauchy": 3, "gm": 4, "tukey": 5}
 assert C.sizeof(IcpParams) == 32, C.sizeof(IcpParams)
 assert C.sizeof(PoseGraphParams) == 40 and PoseGraphParams.reference_node.offset == 32, C.sizeof(PoseGraphParams)
 assert C.sizeof(PoseGraphSummary) == 16 and PoseGraphSummary.cost.offset == 8, C.sizeof(PoseGraphSummary)
+assert C.sizeof(LineProcessParams) == 88 and LineProcessParams.reference_node.offset == 72, C.sizeof(LineProcessParams)
+assert C.sizeof(LineProcessSummary) == 56 and LineProcessSummary.residual.offset == 32, C.sizeof(LineProcessSummary)
 assert C.sizeof(IcpScale) == 48 and IcpScale.max_iteration.offset == 40, C.sizeof(IcpScale)
 assert C.sizeof(FgrParams) == 32 and FgrParams.maximum_correspondence_distance.offset == 16, C.sizeof(FgrParams)
 assert C.sizeof(RansacParams) == 64 and RansacParams.normal_angle_threshold.offset == 56, C.sizeof(RansacParams)
@@ -239,6 +261,8 @@ _SYMBOLS = [
     "tzr_register_cloud_pairs_icp_colored", "tzr_register_cloud_pairs_multiway_colored", "tzr_icp_multiscale_batch",
     "tzr_fgr_params_default", "tzr_fgr", "tzr_fgr_batch", "tzr_register_cloud_pairs_fgr",
     "tzr_ransac_params_default", "tzr_ransac", "tzr_ransac_batch", "tzr_register_cloud_pairs_ransac",
+    "tzr_line_process_params_default", "tzr_pose_graph_optimize_line_process",
+    "tzr_register_cloud_pairs_multiway_line_process",
 ]
 
 # status codes (tzr_status)
@@ -438,6 +462,13 @@ def lib():
     L.tzr_register_cloud_pairs_ransac.argtypes = [vp, C.POINTER(FrontendParams), C.POINTER(RansacParams), C.c_int,
                                                   i32p, fpp, C.c_int, i32p, u64p, u64p, i32p, i64p, C.POINTER(i32p),
                                                   fp, C.POINTER(IcpResult), C.POINTER(RansacInfo)]
+    L.tzr_line_process_params_default.argtypes = [C.POINTER(LineProcessParams)]
+    L.tzr_line_process_params_default.restype = None
+    L.tzr_pose_graph_optimize_line_process.argtypes = [vp, C.POINTER(LineProcessParams)] + \
+        L.tzr_pose_graph_optimize.argtypes[2:-1] + [C.POINTER(LineProcessSummary)]
+    L.tzr_register_cloud_pairs_multiway_line_process.argtypes = L.tzr_register_cloud_pairs_icp_colored.argtypes + [
+        i32p, C.POINTER(LineProcessParams), dp, i32p, dp, u8p, C.POINTER(Similarity), C.POINTER(LineProcessSummary),
+        i32p]
     for s in _SYMBOLS:
         getattr(L, s)  # raises AttributeError if the header and the library disagree
     _lib = L
@@ -464,6 +495,23 @@ def icp_params(max_correspondence_distance: float, **kw) -> IcpParams:
             raise AttributeError(k)
         setattr(p, k, v)
     return p
+
+
+def line_process_params(max_correspondence_distance: float, **kw) -> LineProcessParams:
+    """tzr_line_process_params_default with max_correspondence_distance and any field in kw set."""
+    p = LineProcessParams()
+    lib().tzr_line_process_params_default(C.byref(p))
+    p.max_correspondence_distance = float(max_correspondence_distance)
+    for k, v in kw.items():
+        if not hasattr(p, k):
+            raise AttributeError(k)
+        setattr(p, k, v)
+    return p
+
+
+def _line_process_summary(summ):
+    return dict(iterations=list(summ.iterations), trials=list(summ.trials), stop_reason=list(summ.stop_reason),
+                pruned=int(summ.pruned), residual=float(summ.residual), mu=list(summ.mu))
 
 
 def pose_graph_params(max_correspondence_distance: float, **kw) -> PoseGraphParams:
@@ -1406,6 +1454,7 @@ class Context:
             out_res = icp_res.ctypes.data_as(C.POINTER(IcpResult))
             if multiway is not None:
                 unc, pg = multiway
+                lp = isinstance(pg, LineProcessParams)
                 unc = np.ascontiguousarray(unc, dtype=np.int32)
                 if unc.shape != (P,):
                     raise TzrError("register_multiway: uncertain needs one entry per pair")
@@ -1414,18 +1463,26 @@ class Context:
                 ew = np.zeros(P)
                 em = np.zeros(P, dtype=np.uint8)
                 poses = (Similarity * len(cl))()
-                summ = PoseGraphSummary()
+                summ = LineProcessSummary() if lp else PoseGraphSummary()
                 pg_status = C.c_int32(0)
                 mw_out = (_p(unc, C.c_int32), C.byref(pg), _p(info, C.c_double), _p(icnt, C.c_int32),
                           _p(ew, C.c_double), _p(em, C.c_uint8), poses, C.byref(summ), C.byref(pg_status))
-                if colored is not None:
+                if lp:
+                    cargs = col_args if colored is not None else (None, 0.0, None)
+                    rc = lib().tzr_register_cloud_pairs_multiway_line_process(*args, C.byref(icp), *cargs, out_res,
+                                                                              *mw_out)
+                elif colored is not None:
                     rc = lib().tzr_register_cloud_pairs_multiway_colored(*args, C.byref(icp), *col_args, out_res,
                                                                          *mw_out)
                 else:
                     rc = lib().tzr_register_cloud_pairs_multiway(*args, C.byref(icp), out_res, *mw_out)
-                mw = dict(information=info, counts=icnt, weights=ew, mask=em.astype(bool), poses=_poses(poses),
-                          status=int(pg_status.value), iterations=int(summ.iterations),
-                          inner_iterations=int(summ.inner_iterations), cost=float(summ.cost))
+                if lp:
+                    mw = dict(information=info, counts=icnt, confidence=ew, kept=em.astype(bool), poses=_poses(poses),
+                              status=int(pg_status.value), **_line_process_summary(summ))
+                else:
+                    mw = dict(information=info, counts=icnt, weights=ew, mask=em.astype(bool), poses=_poses(poses),
+                              status=int(pg_status.value), iterations=int(summ.iterations),
+                              inner_iterations=int(summ.inner_iterations), cost=float(summ.cost))
             elif colored is not None:
                 rc = lib().tzr_register_cloud_pairs_icp_colored(*args, C.byref(icp), *col_args, out_res)
             elif kernel is not None:
@@ -1534,7 +1591,7 @@ class Context:
                           normal_search_radius=0.03, fpfh_search_radius=0.05, use_absolute_scale=True,
                           use_crosscheck=True, use_tuple_test=True, tuple_scale=0.0, tuple_seeds=None, max_iteration=30,
                           relative_fitness=1e-6, relative_rmse=1e-6, pose_graph=None, colors=None,
-                          lambda_geometric=0.968, kernel=None):
+                          lambda_geometric=0.968, kernel=None, optimizer="gnc_tls", line_process=None):
         """tzr_register_cloud_pairs_multiway: register_cloud_pairs_icp(method="point_to_plane"), the information
         matrix of every refined pair and the GNC-TLS pose graph over the clouds, in one call.  uncertain: one flag per
         pair (None: Open3D's tutorial rule, pair (k, k + 1) certain and every other pair uncertain).  pose_graph: a
@@ -1542,14 +1599,26 @@ class Context:
         seven results plus a dict: information (P,6,6), counts (P,), weights (P,), mask (P,) bool, poses (n_clouds,4,4),
         status (the pose graph's TZR status), iterations, inner_iterations, cost.  colors (one (n,3) array per cloud)
         refines by coloured ICP instead (tzr_register_cloud_pairs_multiway_colored) with lambda_geometric and kernel
-        (None: L2); a kernel without colours is refused."""
+        (None: L2); a kernel without colours is refused.  optimizer="line_process" runs Open3D's line process instead of
+        GNC-TLS (tzr_register_cloud_pairs_multiway_line_process) with line_process (a LineProcessParams, None: the
+        defaults with c = max_correspondence_distance); its dict has confidence (P,) and kept (P,) bool in place of
+        weights and mask, and global_optimization()'s summary keys in place of iterations, inner_iterations and cost."""
+        if optimizer not in ("gnc_tls", "line_process"):
+            raise TzrError(f"register_multiway: unknown optimizer {optimizer!r}")
+        if (optimizer == "line_process" and pose_graph is not None) or (optimizer == "gnc_tls" and
+                                                                        line_process is not None):
+            raise TzrError(f"register_multiway: optimizer={optimizer!r} takes "
+                           f"{'line_process' if optimizer == 'line_process' else 'pose_graph'}, not the other's parameters")
         kernel = robust_kernel(kernel)
         if kernel is not None and colors is None:
             raise TzrError("register_multiway: a robust kernel needs colors (coloured ICP)")
         pc = np.ascontiguousarray(pairs, dtype=np.int32).reshape(-1, 2)
         if uncertain is None:
             uncertain = [0 if b == a + 1 else 1 for a, b in pc]
-        pg = pose_graph if pose_graph is not None else pose_graph_params(max_correspondence_distance)
+        if optimizer == "line_process":
+            pg = line_process if line_process is not None else line_process_params(max_correspondence_distance)
+        else:
+            pg = pose_graph if pose_graph is not None else pose_graph_params(max_correspondence_distance)
         icp = icp_params(max_correspondence_distance, max_iteration=int(max_iteration),
                          relative_fitness=float(relative_fitness), relative_rmse=float(relative_rmse))
         return self._register_pairs(clouds, pc, params, normal_search_radius, fpfh_search_radius, use_absolute_scale,
@@ -1614,6 +1683,33 @@ class Context:
                                                C.byref(summ)))
         return dict(poses=_poses(poses), weights=w[:E], mask=m[:E].astype(bool), residuals=r[:E],
                     iterations=int(summ.iterations), inner_iterations=int(summ.inner_iterations), cost=float(summ.cost))
+
+    def global_optimization(self, K, edges, transforms, information, max_correspondence_distance, uncertain=None,
+                            initial_poses=None, **params):
+        """tzr_pose_graph_optimize_line_process: Open3D's global_optimization with the Levenberg-Marquardt line process.
+        Arguments as optimize_pose_graph's; params: any LineProcessParams field.  Returns a dict: poses (K,4,4),
+        confidence (E,), kept (E,) bool, residuals (E,) zeta^T Lambda zeta, and per pass iterations, trials,
+        stop_reason (TZR_LP_STOP_*, see LP_STOP) and mu (2-lists), pruned, residual (the final F)."""
+        ed = np.ascontiguousarray(edges, dtype=np.int32).reshape(-1, 2)
+        E = ed.shape[0]
+        info = np.ascontiguousarray(information, dtype=np.float64).reshape(E, 36)
+        if len(transforms) != E:
+            raise TzrError("global_optimization: one transform per edge is required")
+        tr = (Similarity * E)(*[similarity(x) for x in transforms])
+        unc = None if uncertain is None else np.ascontiguousarray(uncertain, dtype=np.int32)
+        if unc is not None and unc.shape != (E,):
+            raise TzrError("global_optimization: uncertain needs one entry per edge")
+        init = None if initial_poses is None else (Similarity * int(K))(*[similarity(x) for x in initial_poses])
+        lp = line_process_params(max_correspondence_distance, **params)
+        poses = (Similarity * max(1, int(K)))()
+        l, m, r = np.zeros(max(1, E)), np.zeros(max(1, E), dtype=np.uint8), np.zeros(max(1, E))
+        summ = LineProcessSummary()
+        self._ck(lib().tzr_pose_graph_optimize_line_process(
+            self._h, C.byref(lp), int(K), E, _p(ed, C.c_int32), tr, _p(info, C.c_double),
+            None if unc is None else _p(unc, C.c_int32), init, poses, _p(l, C.c_double), _p(m, C.c_uint8),
+            _p(r, C.c_double), C.byref(summ)))
+        return dict(poses=_poses(poses), confidence=l[:E], kept=m[:E].astype(bool), residuals=r[:E],
+                    **_line_process_summary(summ))
 
     def icp(self, src, dst, max_correspondence_distance, init=None, max_iteration=30, relative_fitness=1e-6,
             relative_rmse=1e-6):

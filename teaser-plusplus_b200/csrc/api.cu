@@ -2219,25 +2219,15 @@ static bool pg_bfs(int K, int E, const int32_t* ends, const tzr_similarity* T, c
   return (int)order.size() == K;
 }
 
-static int pose_graph_run(tzr_ctx* ctx, const tzr_pose_graph_params* prm, int K, int E, const int32_t* ends,
-                          const tzr_similarity* T, const double* info, const int32_t* uncertain,
-                          const tzr_similarity* init, tzr_similarity* poses, double* weights, uint8_t* inlier_mask,
-                          double* residuals, tzr_pose_graph_summary* summary) {
-  if (!ctx || !pg_params_ok(prm) || K < 2 || E < 1 || !ends || !T || !info || !poses) {
-    if (ctx) ctx->last_error = "pose graph: invalid arguments (K >= 2, E >= 1 and the parameters' ranges)";
-    return TZR_ERR_INVALID_ARG;
-  }
-  if (K > 1024) {
-    ctx->last_error = "pose graph: more than 1024 nodes";
-    return TZR_ERR_TOO_LARGE;
-  }
-  const int ref = prm->reference_node;
-  if (ref < 0 || ref >= K) {
-    ctx->last_error = "pose graph: reference_node " + std::to_string(ref) + " is not a node";
-    return TZR_ERR_INVALID_ARG;
-  }
-  std::vector<char> live((size_t)E);
-  double info_sum = 0.0;
+// The checks and the start shared by both pose-graph optimisers (include/teaser_b200.h): every edge in range, rigid,
+// with finite information and Lambda(5,5) >= 0; rigid initial poses; the breadth-first start from `root` (or the given
+// poses), which must reach every node.  live[e]: s != d and Lambda(5,5) > 0; info_sum: sum of Lambda(5,5).
+static int pg_start(tzr_ctx* ctx, int K, int E, const int32_t* ends, const tzr_similarity* T, const double* info,
+                    const int32_t* uncertain, const tzr_similarity* init, int root, std::vector<char>* live_out,
+                    double* info_sum, std::vector<double>* pose_out) {
+  std::vector<char>& live = *live_out;
+  live.assign((size_t)E, 0);
+  *info_sum = 0.0;
   for (int e = 0; e < E; ++e) {
     const int s = ends[2 * e], d = ends[2 * e + 1];
     if (s < 0 || s >= K || d < 0 || d >= K || !rigid_ok(T[e])) {
@@ -2255,7 +2245,7 @@ static int pose_graph_run(tzr_ctx* ctx, const tzr_pose_graph_params* prm, int K,
       return TZR_ERR_INVALID_ARG;
     }
     live[e] = s != d && l55 > 0;
-    info_sum += l55;
+    *info_sum += l55;
   }
   if (init)
     for (int k = 0; k < K; ++k)
@@ -2263,27 +2253,41 @@ static int pose_graph_run(tzr_ctx* ctx, const tzr_pose_graph_params* prm, int K,
         ctx->last_error = "pose graph: initial pose " + std::to_string(k) + " is not rigid and finite";
         return TZR_ERR_INVALID_ARG;
       }
-  std::vector<double> pose((size_t)K * 12);
+  std::vector<double>& pose = *pose_out;
+  pose.assign((size_t)K * 12, 0.0);
   if (init)
     for (int k = 0; k < K; ++k) {
       memcpy(&pose[12 * (size_t)k], init[k].rotation, 72);
       memcpy(&pose[12 * (size_t)k + 9], init[k].translation, 24);
     }
-  if (!pg_bfs(K, E, ends, T, live, uncertain, ref, init != nullptr, &pose)) {
+  if (!pg_bfs(K, E, ends, T, live, uncertain, root, init != nullptr, &pose)) {
     ctx->last_error = "pose graph: the edges do not connect every node to the reference node";
     return TZR_ERR_INVALID_ARG;
   }
-  const double c = prm->max_correspondence_distance;
-  // edge table; the plan of H's lower blocks and of the right-hand side, each block's terms in ascending edge index
-  std::vector<PgEdge> ed((size_t)E);
+  return TZR_OK;
+}
+
+// The edge table and the plan of H's lower blocks and of the right-hand side, each block's terms in ascending edge
+// index.  ref >= 0: the GNC-TLS graph, whose free nodes skip the reference node; ref < 0: every node is free (the line
+// process).
+static void pg_edge_table(int E, const int32_t* ends, const tzr_similarity* T, const double* info,
+                          const int32_t* uncertain, const std::vector<char>& live, int ref, double c,
+                          std::vector<PgEdge>* ed_out, std::vector<PgBlock>* blocks, std::vector<PgTerm>* terms) {
+  std::vector<PgEdge>& ed = *ed_out;
+  ed.assign((size_t)E, PgEdge{});
   std::map<std::pair<int, int>, std::vector<PgTerm>> plan_map;
   for (int e = 0; e < E; ++e) {
     PgEdge& x = ed[e];
     x = PgEdge{};
     x.s = ends[2 * e];
     x.d = ends[2 * e + 1];
-    x.fs = x.s == ref ? -1 : x.s < ref ? x.s : x.s - 1;
-    x.fd = x.d == ref ? -1 : x.d < ref ? x.d : x.d - 1;
+    if (ref < 0) {
+      x.fs = x.s;
+      x.fd = x.d;
+    } else {
+      x.fs = x.s == ref ? -1 : x.s < ref ? x.s : x.s - 1;
+      x.fd = x.d == ref ? -1 : x.d < ref ? x.d : x.d - 1;
+    }
     x.uncertain = uncertain && uncertain[e] ? 1 : 0;
     memcpy(x.R, T[e].rotation, 72);
     memcpy(x.t, T[e].translation, 24);
@@ -2303,13 +2307,42 @@ static int pose_graph_run(tzr_ctx* ctx, const tzr_pose_graph_params* prm, int K,
     }
     if (x.fs >= 0 && x.fd >= 0) plan_map[{std::max(x.fs, x.fd), std::min(x.fs, x.fd)}].push_back(PgTerm{e, -1});
   }
+  blocks->clear();
+  terms->clear();
+  for (const auto& kv : plan_map) {
+    blocks->push_back(PgBlock{kv.first.first, kv.first.second, (int)terms->size(), 0});
+    terms->insert(terms->end(), kv.second.begin(), kv.second.end());
+    blocks->back().hi = (int)terms->size();
+  }
+}
+
+static int pose_graph_run(tzr_ctx* ctx, const tzr_pose_graph_params* prm, int K, int E, const int32_t* ends,
+                          const tzr_similarity* T, const double* info, const int32_t* uncertain,
+                          const tzr_similarity* init, tzr_similarity* poses, double* weights, uint8_t* inlier_mask,
+                          double* residuals, tzr_pose_graph_summary* summary) {
+  if (!ctx || !pg_params_ok(prm) || K < 2 || E < 1 || !ends || !T || !info || !poses) {
+    if (ctx) ctx->last_error = "pose graph: invalid arguments (K >= 2, E >= 1 and the parameters' ranges)";
+    return TZR_ERR_INVALID_ARG;
+  }
+  if (K > 1024) {
+    ctx->last_error = "pose graph: more than 1024 nodes";
+    return TZR_ERR_TOO_LARGE;
+  }
+  const int ref = prm->reference_node;
+  if (ref < 0 || ref >= K) {
+    ctx->last_error = "pose graph: reference_node " + std::to_string(ref) + " is not a node";
+    return TZR_ERR_INVALID_ARG;
+  }
+  std::vector<char> live;
+  double info_sum = 0.0;
+  std::vector<double> pose;
+  int rc = pg_start(ctx, K, E, ends, T, info, uncertain, init, ref, &live, &info_sum, &pose);
+  if (rc != TZR_OK) return rc;
+  const double c = prm->max_correspondence_distance;
+  std::vector<PgEdge> ed;
   std::vector<PgBlock> blocks;
   std::vector<PgTerm> terms;
-  for (const auto& kv : plan_map) {
-    blocks.push_back(PgBlock{kv.first.first, kv.first.second, (int)terms.size(), 0});
-    terms.insert(terms.end(), kv.second.begin(), kv.second.end());
-    blocks.back().hi = (int)terms.size();
-  }
+  pg_edge_table(E, ends, T, info, uncertain, live, ref, c, &ed, &blocks, &terms);
   PgPlan plan;
   plan.K = K;
   plan.E = E;
@@ -2329,7 +2362,6 @@ static int pose_graph_run(tzr_ctx* ctx, const tzr_pose_graph_params* prm, int K,
                o_g = o_H + al256(n * n * 8), o_work = o_g + al256(n * 8);
   cudaSetDevice(ctx->device);
   cudaStream_t st = ctx->stream;
-  int rc;
   if ((rc = ensure(ctx, ctx->pg, o_work + 256)) != TZR_OK) return rc;
   int lwork = 0;
   if ((rc = dense_cholesky_setup(&ctx->solver_handle, (int)n, (double*)((char*)ctx->pg.p + o_H), &lwork, st,
@@ -2396,6 +2428,216 @@ static int pose_graph_run(tzr_ctx* ctx, const tzr_pose_graph_params* prm, int K,
   return TZR_OK;
 }
 
+// ---- multiway registration: Open3D's line process (DESIGN.md §3.22) ---------------------------------------------------
+static bool lp_params_ok(const tzr_line_process_params* p) {
+  auto fin0 = [](double v) { return std::isfinite(v) && v >= 0; };
+  return p && std::isfinite(p->max_correspondence_distance) && p->max_correspondence_distance > 0 &&
+         p->edge_prune_threshold >= 0 && p->edge_prune_threshold <= 1 && std::isfinite(p->preference_loop_closure) &&
+         p->preference_loop_closure > 0 && fin0(p->min_relative_increment) &&
+         fin0(p->min_relative_residual_increment) && fin0(p->min_right_term) && fin0(p->min_residual) &&
+         std::isfinite(p->lower_scale_factor) && p->lower_scale_factor > 0 && std::isfinite(p->upper_scale_factor) &&
+         p->upper_scale_factor >= p->lower_scale_factor && p->max_iteration >= 1 && p->max_iteration_lm >= 1;
+}
+
+// trials enqueued per state read-back: 1, 2, 4, then 8 per chunk, so that a pass that stops within its first few trials
+// (the usual case) enqueues few idle ones, and a long pass still reads its state back once per 8 trials
+constexpr int kLpChunkMax = 8;
+
+// mu of a pass: preference_loop_closure c^2 mean Lambda(5,5) over its edges, the sum in edge order
+static double lp_mu(const tzr_line_process_params* p, const double* info, const std::vector<int>& idx) {
+  if (idx.empty()) return 0.0;
+  double a = 0.0;
+  for (int e : idx) a = a + info[36 * (size_t)e + 35];
+  const double c = p->max_correspondence_distance;
+  return p->preference_loop_closure * (c * c) * (a / (double)idx.size());
+}
+
+static int line_process_run(tzr_ctx* ctx, const tzr_line_process_params* prm, int K, int E, const int32_t* ends,
+                            const tzr_similarity* T, const double* info, const int32_t* uncertain,
+                            const tzr_similarity* init, tzr_similarity* poses, double* confidence, uint8_t* kept,
+                            double* residuals, tzr_line_process_summary* summary) {
+  if (!ctx || !lp_params_ok(prm) || K < 2 || E < 1 || !ends || !T || !info || !poses) {
+    if (ctx) ctx->last_error = "line process: invalid arguments (K >= 2, E >= 1 and the parameters' ranges)";
+    return TZR_ERR_INVALID_ARG;
+  }
+  if (K > 1024) {
+    ctx->last_error = "line process: more than 1024 nodes";
+    return TZR_ERR_TOO_LARGE;
+  }
+  const int ref = prm->reference_node;
+  if (ref < -1 || ref >= K) {
+    ctx->last_error = "line process: reference_node " + std::to_string(ref) + " is neither -1 nor a node";
+    return TZR_ERR_INVALID_ARG;
+  }
+  std::vector<char> live;
+  double info_sum = 0.0;
+  std::vector<double> pose;
+  int rc = pg_start(ctx, K, E, ends, T, info, uncertain, init, ref < 0 ? 0 : ref, &live, &info_sum, &pose);
+  if (rc != TZR_OK) return rc;
+  const double c = prm->max_correspondence_distance;
+  std::vector<PgEdge> ed;
+  std::vector<PgBlock> blocks;
+  std::vector<PgTerm> terms;
+  pg_edge_table(E, ends, T, info, uncertain, live, -1, c, &ed, &blocks, &terms);
+  std::vector<int> all(E);
+  for (int e = 0; e < E; ++e) all[e] = e;
+  LpPlan plan;
+  plan.K = K;
+  plan.E = E;
+  plan.n = 6 * K;
+  plan.blocks = (int)blocks.size();
+  plan.mu = lp_mu(prm, info, all);
+  plan.min_rel_inc = prm->min_relative_increment;
+  plan.min_rel_res_inc = prm->min_relative_residual_increment;
+  plan.min_right_term = prm->min_right_term;
+  plan.min_residual = prm->min_residual;
+  plan.upper = prm->upper_scale_factor;
+  plan.lower = prm->lower_scale_factor;
+  plan.max_iteration = prm->max_iteration;
+  plan.max_lm = prm->max_iteration_lm;
+  const size_t n = (size_t)plan.n;
+  // workspace: [edges of pass 1 | edges of pass 2 | blocks | terms | poses (2 buffers) | confidences | state] (pass 1's
+  // staged in one copy; pass 2's edges, blocks, terms and confidences overwrite theirs between the passes), then the
+  // edge terms, H, the factor A, b, delta and the factorisation's workspace.  Pass 2's plan is never larger.
+  const size_t o_ed2 = al256((size_t)E * sizeof(PgEdge)), o_blk = o_ed2 + al256((size_t)E * sizeof(PgEdge)),
+               o_trm = o_blk + al256(blocks.size() * sizeof(PgBlock)),
+               o_pose = o_trm + al256(terms.size() * sizeof(PgTerm)), o_l = o_pose + al256((size_t)K * 24 * 8),
+               o_st = o_l + al256((size_t)E * 8), in_bytes = o_st + sizeof(LpState), o_term = al256(in_bytes),
+               o_H = o_term + al256((size_t)E * 2 * kPgTermStride * 8), o_A = o_H + al256(n * n * 8),
+               o_b = o_A + al256(n * n * 8), o_dx = o_b + al256(n * 8), o_work = o_dx + al256(n * 8);
+  cudaSetDevice(ctx->device);
+  cudaStream_t st = ctx->stream;
+  if ((rc = ensure(ctx, ctx->pg, o_work + 256)) != TZR_OK) return rc;
+  int lwork = 0;
+  if ((rc = dense_cholesky_setup(&ctx->solver_handle, (int)n, (double*)((char*)ctx->pg.p + o_A), &lwork, st,
+                                 &ctx->last_error)) != TZR_OK)
+    return rc;
+  if ((rc = ensure(ctx, ctx->pg, o_work + (size_t)std::max(lwork, 1) * 8)) != TZR_OK) return rc;
+  char* d = (char*)ctx->pg.p;
+  std::vector<char> h(in_bytes, 0);
+  memcpy(h.data(), ed.data(), (size_t)E * sizeof(PgEdge));
+  memcpy(h.data() + o_blk, blocks.data(), blocks.size() * sizeof(PgBlock));
+  memcpy(h.data() + o_trm, terms.data(), terms.size() * sizeof(PgTerm));
+  memcpy(h.data() + o_pose, pose.data(), (size_t)K * 12 * 8);
+  for (int e = 0; e < E; ++e) ((double*)(h.data() + o_l))[e] = 1.0;
+  LpState s0{};
+  memcpy(h.data() + o_st, &s0, sizeof(s0));
+  CK(cudaMemcpyAsync(d, h.data(), in_bytes, cudaMemcpyHostToDevice, st));
+  LpDev dv{(const PgEdge*)d, (const PgBlock*)(d + o_blk), (const PgTerm*)(d + o_trm), (double*)(d + o_pose),
+           (double*)(d + o_term), (double*)(d + o_l), (double*)(d + o_H), (double*)(d + o_A), (double*)(d + o_b),
+           (double*)(d + o_dx), (LpState*)(d + o_st)};
+  const long long cap = (long long)prm->max_iteration * prm->max_iteration_lm;
+  LpState hs{};
+  // one pass: H and b cleared (the blocks a pass never lists stay 0), the start, then chunks of trials until the state
+  // read back says the pass has stopped
+  auto pass = [&](const LpPlan& pl, const LpDev& v) -> int {
+    CK(cudaMemsetAsync(v.H, 0, n * n * 8, st));
+    CK(cudaMemsetAsync(v.b, 0, n * 8, st));
+    ctx->launches += launch_line_process_begin(pl, v, st);
+    long long enq = 0, next = 1;
+    do {
+      const long long chunk = std::min(next, cap - enq);
+      next = std::min<long long>(2 * next, kLpChunkMax);
+      for (long long j = 0; j < chunk; ++j) {
+        ctx->launches += launch_line_process_damp(pl, v, st);
+        int r2;
+        if ((r2 = dense_cholesky_solve(ctx->solver_handle, (int)n, v.A, v.delta, (double*)(d + o_work), lwork,
+                                       v.state->info, &ctx->last_error)) != TZR_OK)
+          return r2;
+        ctx->launches += launch_line_process_trial(pl, v, st);
+      }
+      enq += chunk;
+      int r2;
+      if ((r2 = check_launch(ctx, "line process launch")) != TZR_OK) return r2;
+      CK(cudaMemcpyAsync(&hs, v.state, sizeof(hs), cudaMemcpyDeviceToHost, st));
+      CK(cudaStreamSynchronize(st));
+    } while (!hs.done && enq < cap);
+    return TZR_OK;
+  };
+  tzr_line_process_summary sm{};
+  sm.mu[0] = plan.mu;
+  if ((rc = pass(plan, dv)) != TZR_OK) return rc;
+  sm.iterations[0] = hs.iter;
+  sm.trials[0] = hs.trials;
+  sm.stop_reason[0] = hs.reason;
+  // between the passes: pass 1's confidences, the pruned edge list and its plan
+  std::vector<double> l1((size_t)E);
+  CK(cudaMemcpyAsync(l1.data(), dv.conf, (size_t)E * 8, cudaMemcpyDeviceToHost, st));
+  CK(cudaStreamSynchronize(st));
+  std::vector<int> keep;
+  for (int e = 0; e < E; ++e)
+    if (!ed[e].uncertain || l1[e] > prm->edge_prune_threshold) keep.push_back(e);
+  const int E2 = (int)keep.size();
+  sm.pruned = E - E2;
+  {
+    std::vector<int32_t> ends2((size_t)std::max(E2, 1) * 2), unc2(std::max(E2, 1));
+    std::vector<tzr_similarity> T2(std::max(E2, 1));
+    std::vector<double> info2((size_t)std::max(E2, 1) * 36), l2(std::max(E2, 1));
+    std::vector<char> live2(E2);
+    for (int j = 0; j < E2; ++j) {
+      const int e = keep[j];
+      ends2[2 * j] = ends[2 * e];
+      ends2[2 * j + 1] = ends[2 * e + 1];
+      unc2[j] = ed[e].uncertain;
+      T2[j] = T[e];
+      memcpy(&info2[36 * (size_t)j], info + 36 * (size_t)e, 36 * 8);
+      live2[j] = live[e];
+      l2[j] = l1[e];
+    }
+    std::vector<PgEdge> ed2;
+    pg_edge_table(E2, ends2.data(), T2.data(), info2.data(), unc2.data(), live2, -1, c, &ed2, &blocks, &terms);
+    LpPlan plan2 = plan;
+    plan2.E = E2;
+    plan2.blocks = (int)blocks.size();
+    plan2.mu = lp_mu(prm, info, keep);
+    sm.mu[1] = plan2.mu;
+    if (E2 > 0) {
+      CK(cudaMemcpyAsync(d + o_ed2, ed2.data(), (size_t)E2 * sizeof(PgEdge), cudaMemcpyHostToDevice, st));
+      CK(cudaMemcpyAsync(d + o_l, l2.data(), (size_t)E2 * 8, cudaMemcpyHostToDevice, st));
+    }
+    if (!blocks.empty()) {
+      CK(cudaMemcpyAsync(d + o_blk, blocks.data(), blocks.size() * sizeof(PgBlock), cudaMemcpyHostToDevice, st));
+      CK(cudaMemcpyAsync(d + o_trm, terms.data(), terms.size() * sizeof(PgTerm), cudaMemcpyHostToDevice, st));
+    }
+    LpDev dv2 = dv;
+    dv2.edges = (const PgEdge*)(d + o_ed2);
+    if ((rc = pass(plan2, dv2)) != TZR_OK) return rc;
+    sm.iterations[1] = hs.iter;
+    sm.trials[1] = hs.trials;
+    sm.stop_reason[1] = hs.reason;
+    sm.residual = hs.F;
+    std::vector<double> l2out((size_t)std::max(E2, 1));
+    CK(cudaMemcpyAsync(l2out.data(), dv.conf, (size_t)E2 * 8, cudaMemcpyDeviceToHost, st));
+    // the end: compensation, and every edge's terms at the returned poses (pass 1's edge table)
+    const double* T0 = pose.data() + 12 * (size_t)(ref < 0 ? 0 : ref);
+    ctx->launches += launch_line_process_finish(plan, dv, ref, T0, st);
+    if ((rc = check_launch(ctx, "line process launch")) != TZR_OK) return rc;
+    const int buf = ref >= 0 ? 1 - hs.cur : hs.cur;
+    std::vector<double> terms_out((size_t)E * kPgTermStride);
+    CK(cudaMemcpyAsync(pose.data(), dv.poses + (size_t)buf * K * 12, (size_t)K * 12 * 8, cudaMemcpyDeviceToHost, st));
+    CK(cudaMemcpyAsync(terms_out.data(), dv.eterm + (size_t)buf * E * kPgTermStride, (size_t)E * kPgTermStride * 8,
+                       cudaMemcpyDeviceToHost, st));
+    CK(cudaStreamSynchronize(st));
+    std::vector<double> lf = l1;
+    for (int j = 0; j < E2; ++j) lf[keep[j]] = l2out[j];
+    std::vector<uint8_t> km((size_t)E, 0);
+    for (int j = 0; j < E2; ++j) km[keep[j]] = 1;
+    for (int k = 0; k < K; ++k) {
+      memset(&poses[k], 0, sizeof(tzr_similarity));
+      poses[k].scale = 1.0;
+      memcpy(poses[k].rotation, &pose[12 * (size_t)k], 72);
+      memcpy(poses[k].translation, &pose[12 * (size_t)k + 9], 24);
+    }
+    for (int e = 0; e < E; ++e) {
+      if (confidence) confidence[e] = lf[e];
+      if (kept) kept[e] = km[e];
+      if (residuals) residuals[e] = terms_out[(size_t)e * kPgTermStride + 42];
+    }
+  }
+  if (summary) *summary = sm;
+  return TZR_OK;
+}
+
 // what tzr_register_cloud_pairs_multiway adds to register_pairs_run (include/teaser_b200.h)
 struct MultiwayOut {
   const int32_t* uncertain;
@@ -2407,6 +2649,10 @@ struct MultiwayOut {
   tzr_similarity* poses;
   tzr_pose_graph_summary* summary;
   int32_t* pg_status;
+  // Open3D's line process in place of GNC-TLS (pg is then NULL; edge_weights and edge_mask take the confidences and
+  // the kept mask)
+  const tzr_line_process_params* lp = nullptr;
+  tzr_line_process_summary* lp_summary = nullptr;
 };
 
 // FGR (DESIGN.md §3.20): Open3D's FastGlobalRegistrationOption ranges
@@ -2584,7 +2830,8 @@ static int register_pairs_run(tzr_ctx* ctx, const tzr_frontend_params* fp, const
   if (icp && (!icp_params_ok(icp) || !icp_results)) return TZR_ERR_INVALID_ARG;
   if (fgr && (icp || !fgr_params_ok(fgr) || !fgr_results)) return TZR_ERR_INVALID_ARG;
   if (ransac && (icp || fgr || !ransac_params_ok(ransac) || !fgr_results)) return TZR_ERR_INVALID_ARG;
-  if (mw && (!icp || params->estimate_scaling || !mw->uncertain || !pg_params_ok(mw->pg) || !mw->information ||
+  if (mw && (!icp || params->estimate_scaling || !mw->uncertain ||
+             (mw->lp ? !lp_params_ok(mw->lp) : !pg_params_ok(mw->pg)) || !mw->information ||
              !mw->info_counts || !mw->edge_weights || !mw->edge_mask || !mw->poses || !mw->pg_status))
     return TZR_ERR_INVALID_ARG;
   if (icp && icp_mode == kIcpGeneralized && !icp_epsilon_ok(icp_epsilon)) return TZR_ERR_INVALID_ARG;
@@ -2997,8 +3244,11 @@ static int register_pairs_run(tzr_ctx* ctx, const tzr_frontend_params* fp, const
     std::vector<uint8_t> m(std::max(E, 1));
     for (int e = 0; e < E; ++e) memcpy(&L[(size_t)e * 36], mw->information + (size_t)edge_pair[e] * 36, 36 * 8);
     const std::string reg_error = ctx->last_error;
-    *mw->pg_status = pose_graph_run(ctx, mw->pg, n_clouds, E, ends.data(), Tsd.data(), L.data(), unc.data(), nullptr,
-                                    mw->poses, w.data(), m.data(), nullptr, mw->summary);
+    *mw->pg_status =
+        mw->lp ? line_process_run(ctx, mw->lp, n_clouds, E, ends.data(), Tsd.data(), L.data(), unc.data(), nullptr,
+                                  mw->poses, w.data(), m.data(), nullptr, mw->lp_summary)
+               : pose_graph_run(ctx, mw->pg, n_clouds, E, ends.data(), Tsd.data(), L.data(), unc.data(), nullptr,
+                                mw->poses, w.data(), m.data(), nullptr, mw->summary);
     if (*mw->pg_status == TZR_OK) {
       for (int e = 0; e < E; ++e) {
         mw->edge_weights[edge_pair[e]] = w[e];
@@ -3007,6 +3257,7 @@ static int register_pairs_run(tzr_ctx* ctx, const tzr_frontend_params* fp, const
     } else {
       memset(mw->poses, 0, (size_t)n_clouds * sizeof(tzr_similarity));
       if (mw->summary) memset(mw->summary, 0, sizeof(*mw->summary));
+      if (mw->lp_summary) memset(mw->lp_summary, 0, sizeof(*mw->lp_summary));
       if (*mw->pg_status == TZR_ERR_CUDA) return TZR_ERR_CUDA;
     }
     if (no_room || too_large) ctx->last_error = reg_error;
@@ -3894,6 +4145,55 @@ int tzr_register_cloud_pairs_multiway_colored(
     uint8_t* edge_mask, tzr_similarity* poses, tzr_pose_graph_summary* pg_summary, int32_t* pg_status) {
   if (!icp || !colors || colored_args(&lambda_geometric, kernel) != TZR_OK) return TZR_ERR_INVALID_ARG;
   const MultiwayOut mw{uncertain, pg, information, info_counts, edge_weights, edge_mask, poses, pg_summary, pg_status};
+  return register_pairs_run(ctx, fp, params, n_clouds, n, pts, P, pair_clouds, tuple_seeds, solutions, status,
+                            problem_index, n_corr, corr, cliques, global_scale, icp, icp_results, kIcpColored, 0,
+                            kernel, &mw, colors, lambda_geometric);
+}
+
+void tzr_line_process_params_default(tzr_line_process_params* p) {
+  if (!p) return;
+  memset(p, 0, sizeof(*p));
+  p->max_correspondence_distance = 0;  // no default (the caller's ICP distance)
+  p->edge_prune_threshold = 0.25;
+  p->preference_loop_closure = 1.0;
+  p->min_relative_increment = 1e-6;
+  p->min_relative_residual_increment = 1e-6;
+  p->min_right_term = 1e-6;
+  p->min_residual = 1e-6;
+  p->upper_scale_factor = 2.0 / 3.0;
+  p->lower_scale_factor = 1.0 / 3.0;
+  p->reference_node = 0;
+  p->max_iteration = 100;
+  p->max_iteration_lm = 20;
+}
+
+int tzr_pose_graph_optimize_line_process(tzr_ctx* ctx, const tzr_line_process_params* params, int K, int E,
+                                         const int32_t* edges, const tzr_similarity* edge_transforms,
+                                         const double* information, const int32_t* uncertain,
+                                         const tzr_similarity* initial_poses, tzr_similarity* poses,
+                                         double* confidence, uint8_t* kept, double* residuals,
+                                         tzr_line_process_summary* summary) {
+  return line_process_run(ctx, params, K, E, edges, edge_transforms, information, uncertain, initial_poses, poses,
+                          confidence, kept, residuals, summary);
+}
+
+int tzr_register_cloud_pairs_multiway_line_process(
+    tzr_ctx* ctx, const tzr_frontend_params* fp, const tzr_params* params, int n_clouds, const int32_t* n,
+    const float* const* pts, int P, const int32_t* pair_clouds, const uint64_t* tuple_seeds, tzr_solution* solutions,
+    int32_t* status, int32_t* problem_index, int64_t* n_corr, int32_t* const* corr, int32_t* const* cliques,
+    float* global_scale, const tzr_icp_params* icp, const float* const* colors, double lambda_geometric,
+    const tzr_robust_kernel* kernel, tzr_icp_result* icp_results, const int32_t* uncertain,
+    const tzr_line_process_params* lp, double* information, int32_t* info_counts, double* edge_confidence,
+    uint8_t* edge_kept, tzr_similarity* poses, tzr_line_process_summary* lp_summary, int32_t* lp_status) {
+  if (!icp || (!colors && kernel)) return TZR_ERR_INVALID_ARG;
+  if (colors && colored_args(&lambda_geometric, kernel) != TZR_OK) return TZR_ERR_INVALID_ARG;
+  MultiwayOut mw{uncertain, nullptr, information, info_counts, edge_confidence, edge_kept, poses, nullptr, lp_status};
+  mw.lp = lp;
+  mw.lp_summary = lp_summary;
+  if (!colors)
+    return register_pairs_run(ctx, fp, params, n_clouds, n, pts, P, pair_clouds, tuple_seeds, solutions, status,
+                              problem_index, n_corr, corr, cliques, global_scale, icp, icp_results, kIcpPointToPlane, 0,
+                              nullptr, &mw);
   return register_pairs_run(ctx, fp, params, n_clouds, n, pts, P, pair_clouds, tuple_seeds, solutions, status,
                             problem_index, n_corr, corr, cliques, global_scale, icp, icp_results, kIcpColored, 0,
                             kernel, &mw, colors, lambda_geometric);

@@ -409,4 +409,448 @@ int launch_pose_graph_gnc(const PgPlan& plan, const PgDev& dv, int iter, cudaStr
   return 1;
 }
 
+// ---- Open3D's line process (tzr_pose_graph_optimize_line_process, DESIGN.md §3.22) -------------------------------------
+//   lp_edge_kernel      one thread per edge: M = X^-1 T_d^-1 T_s, zeta = lin(M), J_s from the generator products,
+//                       J_s^T Lambda J_s, J_s^T Lambda zeta and zeta^T Lambda zeta at the current, candidate or returned
+//                       poses.
+//   lp_begin_kernel     one block: F with the incoming confidences, then the confidence update; starts the pass.
+//   lp_assemble_kernel  one warp per listed block: H (undamped) and b = -sum sign l_e v_e, as pg_assemble_kernel.
+//   lp_stats_kernel     one block: max(b), |x|; at the start lambda = 1e-5 max diag(H); after an accepted trial the
+//                       end of the outer iteration (min_right_term, min_residual, max_iteration).
+//   lp_damp_kernel      H + lambda I (lower triangle) and b into the factor buffer, which potrf overwrites.
+//   (cuSOLVER)          cusolverDnDpotrf + cusolverDnDpotrs on the 6 K rows.
+//   lp_step_kernel      one block: |delta|, delta . (lambda delta + b) and the min_relative_increment rule.
+//   lp_update_kernel    one thread per node: the candidate V(delta_k) T_k.
+//   lp_decide_kernel    one block: F' with the old confidences, rho, accept / reject, the lambda / nu schedule and the
+//                       trial rules; an accepted candidate updates the confidences.
+// Every kernel returns at once when the pass has stopped.  Reductions run in one block in a fixed order: thread t adds
+// the entries t, t + blockDim, ... in turn, then a shared-memory tree (tests/line_process_reference.py: block_sum).
+namespace {
+
+constexpr int kLpSmall = 256;   // threads of the edge-sum kernels (begin, decide)
+constexpr int kLpLarge = 1024;  // threads of the kernels that reduce over 6 K entries or K nodes (step, stats)
+
+struct Pose12 {
+  double v[12];
+};
+
+__device__ __forceinline__ double* lp_pose(const LpDev& dv, int K, int buf, int k) {
+  return dv.poses + 12 * ((size_t)buf * K + k);
+}
+__device__ __forceinline__ double* lp_terms(const LpDev& dv, int E, int buf, int e) {
+  return dv.eterm + kPgTermStride * ((size_t)buf * E + e);
+}
+
+// the block's fixed-order sum / max of one value per thread (blockDim a power of two)
+__device__ double lp_block_sum(double a, double* sh) {
+  const int t = threadIdx.x;
+  sh[t] = a;
+  __syncthreads();
+  for (int s = blockDim.x >> 1; s; s >>= 1) {
+    if (t < s) sh[t] = sh[t] + sh[t + s];
+    __syncthreads();
+  }
+  const double r = sh[0];
+  __syncthreads();
+  return r;
+}
+__device__ double lp_block_max(double a, double* sh) {
+  const int t = threadIdx.x;
+  sh[t] = a;
+  __syncthreads();
+  for (int s = blockDim.x >> 1; s; s >>= 1) {
+    if (t < s) sh[t] = fmax(sh[t], sh[t + s]);
+    __syncthreads();
+  }
+  const double r = sh[0];
+  __syncthreads();
+  return r;
+}
+
+// F = sum_e l_e c_e + mu (sqrt(l_e) - 1)^2 over edge-term buffer buf
+__device__ double lp_residual(const LpDev& dv, int E, int buf, double mu, double* sh) {
+  double a = 0.0;
+  for (int e = threadIdx.x; e < E; e += blockDim.x) {
+    const double l = dv.conf[e], q = sqrt(l) - 1.0;
+    a = a + (l * lp_terms(dv, E, buf, e)[42] + mu * (q * q));
+  }
+  return lp_block_sum(a, sh);
+}
+
+// the confidence update of the uncertain edges from edge-term buffer buf: l = (mu / (mu + c))^2
+__device__ void lp_confidences(const LpDev& dv, int E, int buf, double mu) {
+  for (int e = threadIdx.x; e < E; e += blockDim.x)
+    if (dv.edges[e].uncertain) {
+      const double q = mu / (mu + lp_terms(dv, E, buf, e)[42]);
+      dv.conf[e] = q * q;
+    }
+}
+
+// lin(N) of the top 3 x 4 of a 4 x 4 matrix: N column-major 3 x 3 and its translation column
+__device__ __forceinline__ void lp_lin(const double* N, const double* t, double* z) {
+  z[0] = 0.5 * (N[5] - N[7]);
+  z[1] = 0.5 * (N[6] - N[2]);
+  z[2] = 0.5 * (N[1] - N[3]);
+  z[3] = t[0];
+  z[4] = t[1];
+  z[5] = t[2];
+}
+
+// which = 0: the current poses into the current terms; 1: the candidate poses (the other buffer), skipped once the pass
+// has stopped or the trial formed no candidate; 2: the other buffer, always (the compensated poses)
+__global__ void lp_edge_kernel(LpDev dv, int K, int E, int which) {
+  const int e = blockIdx.x * blockDim.x + threadIdx.x;
+  if (e >= E) return;
+  const LpState& st = *dv.state;
+  if (which == 1 && (st.done || st.skip)) return;
+  const int buf = which == 0 ? st.cur : 1 - st.cur;
+  const PgEdge& ed = dv.edges[e];
+  const double* Ts = lp_pose(dv, K, buf, ed.s);
+  const double* Td = lp_pose(dv, K, buf, ed.d);
+  // P = X^-1 T_d^-1: R_P = (R_d R_X)^T, t_P = -R_X^T (R_d^T t_d + t_X); M = P T_s
+  double RdX[9], RP[9], u[3], tP[3], RM[9], tM[3];
+  m33(Td, ed.R, RdX);
+#pragma unroll
+  for (int k = 0; k < 3; ++k)
+#pragma unroll
+    for (int r = 0; r < 3; ++r) RP[3 * k + r] = RdX[3 * r + k];
+  mtv3(Td, Td + 9, u);
+#pragma unroll
+  for (int r = 0; r < 3; ++r) u[r] = u[r] + ed.t[r];
+  mtv3(ed.R, u, tP);
+#pragma unroll
+  for (int r = 0; r < 3; ++r) tP[r] = -tP[r];
+  m33(RP, Ts, RM);
+  mv3(RP, Ts + 9, tM);
+#pragma unroll
+  for (int r = 0; r < 3; ++r) tM[r] = tM[r] + tP[r];
+  double z[6];
+  lp_lin(RM, tM, z);
+  // J_s[:, i] = lin(P G_i T_s): G_0..2 the skew generators, G_3..5 the unit translations
+  double J[6][6];  // J[row][col]
+#pragma unroll
+  for (int i = 0; i < 3; ++i) {
+    double G[9] = {0.0, 0.0, 0.0, 0.0, 0.0, 0.0, 0.0, 0.0, 0.0};
+    // skew(e_i), column-major: (i=0) (2,1) = 1, (1,2) = -1; (i=1) (0,2) = 1, (2,0) = -1; (i=2) (1,0) = 1, (0,1) = -1
+    const int j = (i + 1) % 3, k = (i + 2) % 3;
+    G[3 * j + k] = 1.0;
+    G[3 * k + j] = -1.0;
+    double Q[9], N[9], tN[3], col[6];
+    m33(RP, G, Q);
+    m33(Q, Ts, N);
+    mv3(Q, Ts + 9, tN);
+    lp_lin(N, tN, col);
+#pragma unroll
+    for (int r = 0; r < 6; ++r) J[r][i] = col[r];
+  }
+#pragma unroll
+  for (int i = 0; i < 3; ++i) {
+#pragma unroll
+    for (int r = 0; r < 3; ++r) J[r][3 + i] = 0.0;
+#pragma unroll
+    for (int r = 0; r < 3; ++r) J[3 + r][3 + i] = RP[3 * i + r];
+  }
+  // Lz = Lambda zeta, c = zeta^T Lambda zeta
+  double Lz[6];
+#pragma unroll
+  for (int r = 0; r < 6; ++r) {
+    double a = 0.0;
+#pragma unroll
+    for (int k = 0; k < 6; ++k) a = a + ed.L[6 * r + k] * z[k];
+    Lz[r] = a;
+  }
+  double c = 0.0;
+#pragma unroll
+  for (int k = 0; k < 6; ++k) c = c + z[k] * Lz[k];
+  double LJ[6][6];
+#pragma unroll
+  for (int r = 0; r < 6; ++r)
+#pragma unroll
+    for (int k = 0; k < 6; ++k) {
+      double a = 0.0;
+#pragma unroll
+      for (int q = 0; q < 6; ++q) a = a + ed.L[6 * r + q] * J[q][k];
+      LJ[r][k] = a;
+    }
+  double* out = lp_terms(dv, E, buf, e);
+#pragma unroll
+  for (int r = 0; r < 6; ++r) {
+#pragma unroll
+    for (int k = 0; k < 6; ++k) {
+      double a = 0.0;
+#pragma unroll
+      for (int q = 0; q < 6; ++q) a = a + J[q][r] * LJ[q][k];
+      out[6 * r + k] = a;
+    }
+    double a = 0.0;
+#pragma unroll
+    for (int q = 0; q < 6; ++q) a = a + J[q][r] * Lz[q];
+    out[36 + r] = a;
+  }
+  out[42] = c;
+}
+
+// The start of a pass: F with the incoming confidences, then their update; H and b follow
+__global__ void lp_begin_kernel(LpDev dv, LpPlan p) {
+  __shared__ double sh[kLpSmall];
+  LpState& st = *dv.state;
+  const double F = lp_residual(dv, p.E, st.cur, p.mu, sh);
+  lp_confidences(dv, p.E, st.cur, p.mu);
+  if (threadIdx.x != 0) return;
+  st.F = F;
+  st.Fc = 0.0;
+  st.nu = 2.0;
+  st.done = st.reason = st.skip = 0;
+  st.accepted = 1;
+  st.iter = st.lm = st.trials = 0;
+}
+
+// One warp per listed block: H block (bi, bj), bi >= bj: sum of sign * (l_e A_e(r, k)) in the listed order (column-major
+// n x n, lower blocks only); b block bi (bj = -1): -(sum of sign * (l_e v_e(r))).  Only after the start or an accepted
+// trial.
+__global__ void lp_assemble_kernel(LpDev dv, int E, int n, int nblocks) {
+  const int bk = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
+  const int lane = threadIdx.x & 31;
+  if (bk >= nblocks) return;
+  const LpState& st = *dv.state;
+  if (st.done || !st.accepted) return;
+  const PgBlock bl = dv.blocks[bk];
+  const int cur = st.cur;
+  if (bl.bj < 0) {
+    if (lane >= 6) return;
+    double a = 0.0;
+    for (int q = bl.lo; q < bl.hi; ++q) {
+      const PgTerm tm = dv.terms[q];
+      a = a + (double)tm.sign * (dv.conf[tm.e] * lp_terms(dv, E, cur, tm.e)[36 + lane]);
+    }
+    dv.b[6 * bl.bi + lane] = -a;
+    return;
+  }
+  for (int l = lane; l < 36; l += 32) {
+    const int r = l / 6, k = l % 6;
+    double a = 0.0;
+    for (int q = bl.lo; q < bl.hi; ++q) {
+      const PgTerm tm = dv.terms[q];
+      a = a + (double)tm.sign * (dv.conf[tm.e] * lp_terms(dv, E, cur, tm.e)[6 * r + k]);
+    }
+    dv.H[(size_t)(6 * bl.bi + r) + (size_t)(6 * bl.bj + k) * (size_t)n] = a;
+  }
+}
+
+// Open3D's TransformMatrix4dToVector6d of a pose (R column-major): ZYX Euler angles, then t; its squared norm in order
+__device__ double lp_euler_sq(const double* T) {
+  const double sy = sqrt(T[0] * T[0] + T[1] * T[1]);
+  double x, y, z;
+  if (!(sy < 1e-6)) {
+    x = atan2(T[5], T[8]);
+    y = atan2(-T[2], sy);
+    z = atan2(T[1], T[0]);
+  } else {
+    x = atan2(-T[7], T[4]);
+    y = atan2(-T[2], sy);
+    z = 0.0;
+  }
+  return ((((x * x + y * y) + z * z) + T[9] * T[9]) + T[10] * T[10]) + T[11] * T[11];
+}
+
+// mode 0: the start of a pass (lambda = 1e-5 max diag H, nu = 2); mode 1: after an accepted trial, the end of the outer
+// iteration.  Both: max(b) against min_right_term and |x| of the current poses.
+__global__ void lp_stats_kernel(LpDev dv, LpPlan p, int mode) {
+  __shared__ double sh[kLpLarge];
+  LpState& st = *dv.state;
+  if (st.done || !st.accepted) return;
+  double bm = -INFINITY, hm = -INFINITY;
+  for (int i = threadIdx.x; i < p.n; i += blockDim.x) {
+    bm = fmax(bm, dv.b[i]);
+    if (mode == 0) hm = fmax(hm, dv.H[(size_t)i * p.n + i]);
+  }
+  bm = lp_block_max(bm, sh);
+  if (mode == 0) hm = lp_block_max(hm, sh);
+  double xs = 0.0;
+  for (int k = threadIdx.x; k < p.K; k += blockDim.x) xs = xs + lp_euler_sq(lp_pose(dv, p.K, st.cur, k));
+  xs = lp_block_sum(xs, sh);
+  if (threadIdx.x != 0) return;
+  st.xnorm = sqrt(xs);
+  if (mode == 0) st.lambda = 1e-5 * hm;
+  if (bm < p.min_right_term) {
+    st.done = 1;
+    st.reason = TZR_LP_STOP_RIGHT_TERM;
+  }
+  if (mode == 0) return;
+  st.lm = 0;
+  if (!st.done && st.F < p.min_residual) {
+    st.done = 1;
+    st.reason = TZR_LP_STOP_MIN_RESIDUAL;
+  }
+  if (!st.done && st.iter >= p.max_iteration) {
+    st.done = 1;
+    st.reason = TZR_LP_STOP_MAX_ITERATION;
+  }
+}
+
+// H + lambda I (lower triangle; A's upper triangle is not read) into A and b into delta.  Grid (ceil(n / 256), n): one
+// thread per row of column blockIdx.y.
+__global__ void lp_damp_kernel(LpDev dv, int n) {
+  const LpState& st = *dv.state;
+  if (st.done) return;
+  const int i = blockIdx.x * blockDim.x + threadIdx.x, j = blockIdx.y;
+  if (i >= n) return;
+  if (j == 0) dv.delta[i] = dv.b[i];
+  if (i < j) return;
+  const size_t o = (size_t)i + (size_t)j * n;
+  dv.A[o] = i == j ? dv.H[o] + st.lambda : dv.H[o];
+}
+
+// |delta|, delta . (lambda delta + b) and the trial's outcome before any candidate: skip 2 when the factorisation failed
+// or delta is not finite, 1 when |delta| < min_relative_increment (|x| + min_relative_increment)
+__global__ void lp_step_kernel(LpDev dv, LpPlan p) {
+  __shared__ double sh[kLpLarge];
+  LpState& st = *dv.state;
+  if (st.done) return;
+  const double lam = st.lambda;
+  double s2 = 0.0, pd = 0.0;
+  for (int i = threadIdx.x; i < p.n; i += blockDim.x) {
+    const double d = dv.delta[i];
+    s2 = s2 + d * d;
+    pd = pd + d * (lam * d + dv.b[i]);
+  }
+  s2 = lp_block_sum(s2, sh);
+  pd = lp_block_sum(pd, sh);
+  if (threadIdx.x != 0) return;
+  const double dn = sqrt(s2);
+  st.dnorm = dn;
+  st.pred = pd;
+  if (st.info[0] != 0 || st.info[1] != 0 || !isfinite(s2) || !isfinite(pd))
+    st.skip = 2;
+  else if (dn < p.min_rel_inc * (st.xnorm + p.min_rel_inc))
+    st.skip = 1;
+  else
+    st.skip = 0;
+}
+
+// One thread per node: the candidate V(delta_k) T_k, V(d) = [R_z(d_2) R_y(d_1) R_x(d_0) | (d_3, d_4, d_5)]
+__global__ void lp_update_kernel(LpDev dv, int K) {
+  const int k = blockIdx.x * blockDim.x + threadIdx.x;
+  if (k >= K) return;
+  const LpState& st = *dv.state;
+  if (st.done || st.skip) return;
+  const double* T = lp_pose(dv, K, st.cur, k);
+  double* Tn = lp_pose(dv, K, 1 - st.cur, k);
+  const double* d = dv.delta + 6 * (size_t)k;
+  const double cx = cos(d[0]), sx = sin(d[0]), cy = cos(d[1]), sy = sin(d[1]), cz = cos(d[2]), sz = sin(d[2]);
+  const double Rz[9] = {cz, sz, 0.0, -sz, cz, 0.0, 0.0, 0.0, 1.0};
+  const double Ry[9] = {cy, 0.0, -sy, 0.0, 1.0, 0.0, sy, 0.0, cy};
+  const double Rx[9] = {1.0, 0.0, 0.0, 0.0, cx, sx, 0.0, -sx, cx};
+  double Rzy[9], V[9], u[3];
+  m33(Rz, Ry, Rzy);
+  m33(Rzy, Rx, V);
+  m33(V, T, Tn);
+  mv3(V, T + 9, u);
+#pragma unroll
+  for (int r = 0; r < 3; ++r) Tn[9 + r] = u[r] + d[3 + r];
+}
+
+// The trial's decision (include/teaser_b200.h states the rules in order)
+__global__ void lp_decide_kernel(LpDev dv, LpPlan p) {
+  __shared__ double sh[kLpSmall];
+  __shared__ int acc;
+  LpState& st = *dv.state;
+  if (st.done) return;
+  const int skip = st.skip;
+  const double Fc = skip ? 0.0 : lp_residual(dv, p.E, 1 - st.cur, p.mu, sh);
+  if (threadIdx.x == 0) {
+    if (st.lm == 0) st.iter += 1;
+    st.lm += 1;
+    st.trials += 1;
+    st.Fc = Fc;
+    int a = 0;
+    if (skip == 1) {
+      st.done = 1;
+      st.reason = TZR_LP_STOP_REL_INCREMENT;
+    } else {
+      const double dF = st.F - Fc;
+      const double rho = skip ? -1.0 : dF / (st.pred + 1e-3);
+      if (rho > 0.0 && dF < p.min_rel_res_inc * st.F) {
+        st.done = 1;
+        st.reason = TZR_LP_STOP_REL_RESIDUAL;
+      } else if (rho > 0.0) {
+        const double q = 2.0 * rho - 1.0;
+        st.lambda = st.lambda * fmax(p.lower, fmin(p.upper, 1.0 - (q * q) * q));
+        st.nu = 2.0;
+        st.F = Fc;
+        st.cur = 1 - st.cur;
+        a = 1;
+      } else {
+        st.lambda = st.lambda * st.nu;
+        st.nu = 2.0 * st.nu;
+      }
+    }
+    if (!st.done && st.lm >= p.max_lm) {
+      st.done = 1;
+      st.reason = TZR_LP_STOP_LM_TRIALS;
+    }
+    st.accepted = a;
+    acc = a;
+  }
+  __syncthreads();
+  if (acc) lp_confidences(dv, p.E, st.cur, p.mu);
+}
+
+// The compensation T_k <- C T_k with C = T0 (T_ref)^-1 into the other buffer (each thread forms C in the same order)
+__global__ void lp_compensate_kernel(LpDev dv, int K, int ref, Pose12 T0) {
+  const int k = blockIdx.x * blockDim.x + threadIdx.x;
+  if (k >= K) return;
+  const LpState& st = *dv.state;
+  const double* Tr = lp_pose(dv, K, st.cur, ref);
+  // C: R_C = R0 R_ref^T, t_C = t0 - R_C t_ref
+  double RC[9], tC[3], u[3];
+  m33_nt(T0.v, Tr, RC);
+  mv3(RC, Tr + 9, u);
+#pragma unroll
+  for (int r = 0; r < 3; ++r) tC[r] = T0.v[9 + r] - u[r];
+  const double* T = lp_pose(dv, K, st.cur, k);
+  double* Tn = lp_pose(dv, K, 1 - st.cur, k);
+  m33(RC, T, Tn);
+  mv3(RC, T + 9, u);
+#pragma unroll
+  for (int r = 0; r < 3; ++r) Tn[9 + r] = u[r] + tC[r];
+}
+
+}  // namespace
+
+int launch_line_process_begin(const LpPlan& plan, const LpDev& dv, cudaStream_t st) {
+  lp_edge_kernel<<<(std::max(plan.E, 1) + 127) / 128, 128, 0, st>>>(dv, plan.K, plan.E, 0);
+  lp_begin_kernel<<<1, kLpSmall, 0, st>>>(dv, plan);
+  lp_assemble_kernel<<<(std::max(plan.blocks, 1) + 3) / 4, 128, 0, st>>>(dv, plan.E, plan.n, plan.blocks);
+  lp_stats_kernel<<<1, kLpLarge, 0, st>>>(dv, plan, 0);
+  return 4;
+}
+
+int launch_line_process_damp(const LpPlan& plan, const LpDev& dv, cudaStream_t st) {
+  lp_damp_kernel<<<dim3((plan.n + 255) / 256, plan.n), 256, 0, st>>>(dv, plan.n);
+  return 1;
+}
+
+int launch_line_process_trial(const LpPlan& plan, const LpDev& dv, cudaStream_t st) {
+  lp_step_kernel<<<1, kLpLarge, 0, st>>>(dv, plan);
+  lp_update_kernel<<<(plan.K + 127) / 128, 128, 0, st>>>(dv, plan.K);
+  lp_edge_kernel<<<(std::max(plan.E, 1) + 127) / 128, 128, 0, st>>>(dv, plan.K, plan.E, 1);
+  lp_decide_kernel<<<1, kLpSmall, 0, st>>>(dv, plan);
+  lp_assemble_kernel<<<(std::max(plan.blocks, 1) + 3) / 4, 128, 0, st>>>(dv, plan.E, plan.n, plan.blocks);
+  lp_stats_kernel<<<1, kLpLarge, 0, st>>>(dv, plan, 1);
+  return 6;
+}
+
+int launch_line_process_finish(const LpPlan& plan, const LpDev& dv, int ref, const double* T0, cudaStream_t st) {
+  int n = 0;
+  if (ref >= 0) {
+    Pose12 t0;
+    for (int q = 0; q < 12; ++q) t0.v[q] = T0[q];
+    lp_compensate_kernel<<<(plan.K + 127) / 128, 128, 0, st>>>(dv, plan.K, ref, t0);
+    ++n;
+  }
+  lp_edge_kernel<<<(std::max(plan.E, 1) + 127) / 128, 128, 0, st>>>(dv, plan.K, plan.E, ref >= 0 ? 2 : 0);
+  return n + 1;
+}
+
 }  // namespace tzr

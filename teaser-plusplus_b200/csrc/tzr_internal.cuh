@@ -801,6 +801,57 @@ int launch_pose_graph_assemble(const PgPlan& plan, const PgDev& dv, cudaStream_t
 int launch_pose_graph_step(const PgPlan& plan, const PgDev& dv, int ref, double cost_floor, cudaStream_t st);
 // GNC-TLS weight update after GNC iteration `iter`.  Returns the launches (1).
 int launch_pose_graph_gnc(const PgPlan& plan, const PgDev& dv, int iter, cudaStream_t st);
+
+// pose_graph.cu, Open3D's line process (tzr_pose_graph_optimize_line_process, DESIGN.md §3.22): one pass of the
+// Levenberg-Marquardt loop over the edge table of PgEdge (fs = s, fd = d: every node free), with the per-block term plan
+// of the GNC-TLS graph built in its keep-every-node mode.  Edge terms use kPgTermStride: J_s^T Lambda J_s (36),
+// J_s^T Lambda zeta (6), zeta^T Lambda zeta.
+struct LpState {        // one pass's device-side state, read back once per chunk of trials
+  double lambda, nu;    // the damping and its rejection factor
+  double F, Fc;         // the residual at the current poses and at the latest candidate
+  double xnorm;         // |x| of the current poses (their Euler vectors)
+  double dnorm, pred;   // |delta| and delta . (lambda delta + b) of the latest trial
+  int cur;              // which pose / edge-term buffer holds the current poses
+  int done;             // 1: the pass has stopped
+  int reason;           // its TZR_LP_STOP_* rule
+  int skip;             // the latest trial formed no candidate: 1 the step was too small, 2 the factorisation failed
+  int accepted;         // the latest trial was accepted (H and b are rebuilt)
+  int iter, lm, trials; // outer iterations begun, trials of the current one, trials of the pass
+  int info[2];          // potrf / potrs status of the latest trial
+};
+struct LpPlan {
+  int K = 0, E = 0, n = 0, blocks = 0;  // nodes, this pass's edges, 6 K, listed blocks of H and b
+  double mu = 0;                        // preference_loop_closure c^2 mean Lambda(5,5) over this pass's edges
+  double min_rel_inc = 0, min_rel_res_inc = 0, min_right_term = 0, min_residual = 0;
+  double upper = 0, lower = 0;
+  int max_iteration = 0, max_lm = 0;
+};
+// poses: 2 x K x 12; eterm: 2 x E x kPgTermStride; conf: E; H: n x n (lower blocks as assembled); A: n x n (the
+// factor); b, delta: n; state: one LpState.
+struct LpDev {
+  const PgEdge* edges;
+  const PgBlock* blocks;
+  const PgTerm* terms;
+  double* poses;
+  double* eterm;
+  double* conf;
+  double* H;
+  double* A;
+  double* b;
+  double* delta;
+  LpState* state;
+};
+// The start of a pass: edge terms, F with the incoming confidences, the confidence update, H and b, lambda and the
+// max(b) test.  Returns the launches (4); the caller clears H first.
+int launch_line_process_begin(const LpPlan& plan, const LpDev& dv, cudaStream_t st);
+// One trial before the factorisation: H + lambda I and b into A and delta.  Returns the launches (1).
+int launch_line_process_damp(const LpPlan& plan, const LpDev& dv, cudaStream_t st);
+// One trial after the factorisation: the stop rule on |delta|, the candidate poses and terms, the decision, and after
+// an accepted candidate the rebuilt H and b.  Returns the launches (6).
+int launch_line_process_trial(const LpPlan& plan, const LpDev& dv, cudaStream_t st);
+// The end of the call: compensation by T0_ref (T_ref)^-1 into the other pose buffer when ref >= 0 (T0: 12 doubles), then
+// every edge's terms at the returned poses (which buffer: 1 - cur with compensation, cur without).  Returns the launches.
+int launch_line_process_finish(const LpPlan& plan, const LpDev& dv, int ref, const double* T0, cudaStream_t st);
 // dense Cholesky through the lazily loaded cuSOLVER (certify.cu): handle and workspace size of an n x n lower factor;
 // TZR_ERR_UNSUPPORTED when cuSOLVER cannot be loaded
 int dense_cholesky_setup(void** solver_handle, int n, double* A, int* lwork, cudaStream_t st, std::string* err);

@@ -2,7 +2,9 @@
 // get_information_matrix_from_point_clouds (teaser::informationMatrix, informationMatrixBatch: tzr_information_matrix,
 // tzr_information_matrix_batch) and a pose graph with GNC-TLS on its uncertain edges (teaser::PoseGraph:
 // tzr_pose_graph_optimize).  RobustRegistrationSolver::solveMultiway (teaser/registration.h) chains both after the
-// cloud-pair call.  No CPU implementation: without a CUDA device the first call throws std::runtime_error.
+// cloud-pair call.  teaser::GlobalOptimization is Open3D's global_optimization with the line process
+// (tzr_pose_graph_optimize_line_process, DESIGN.md §3.22), and solveMultiway has overloads that take its Params.  No CPU
+// implementation: without a CUDA device the first call throws std::runtime_error.
 #pragma once
 
 #include <vector>
@@ -49,6 +51,36 @@ class PoseGraph {
   // tzr_pose_graph_optimize over num_nodes nodes on this thread's context.  initial_poses (null: breadth-first from
   // the reference node) holds num_nodes rigid matrices.  Throws std::runtime_error with the library's message on an
   // invalid graph (disconnected, more than 1024 nodes, a non-rigid edge).
+  Result optimize(int num_nodes, const std::vector<Edge>& edges,
+                  const std::vector<Eigen::Matrix4d>* initial_poses = nullptr) const;
+
+  const Params& getParams() const { return params_; }
+  void setParams(const Params& params) { params_ = params; }
+
+ private:
+  Params params_;
+};
+
+// Open3D's global_optimization with GlobalOptimizationLevenbergMarquardt: the line process, pruning of the uncertain
+// edges whose confidence is at most edge_prune_threshold, a second pass on the kept edges, then the compensation that
+// returns the reference node to its starting pose.
+class GlobalOptimization {
+ public:
+  using Params = LineProcessParams;
+  using Edge = PoseGraph::Edge;
+  struct Result {
+    std::vector<Eigen::Matrix4d> poses;  // node k into the world frame
+    std::vector<double> confidence;      // per edge: pass 2's for a kept edge, pass 1's for a pruned one
+    std::vector<bool> kept;
+    std::vector<double> residuals;       // zeta^T Lambda zeta at the returned poses
+    LineProcessSummary summary;
+  };
+
+  GlobalOptimization() = default;
+  explicit GlobalOptimization(const Params& params) : params_(params) {}
+
+  // tzr_pose_graph_optimize_line_process over num_nodes nodes on this thread's context; initial_poses as
+  // PoseGraph::optimize's.  Throws std::runtime_error with the library's message on an invalid graph or parameters.
   Result optimize(int num_nodes, const std::vector<Edge>& edges,
                   const std::vector<Eigen::Matrix4d>* initial_poses = nullptr) const;
 

@@ -85,6 +85,31 @@ struct PoseGraphParams {
   int max_inner_iterations = 10;
   int reference_node = 0;
 };
+// Open3D's line-process pose graph (teaser/pose_graph.h: GlobalOptimization, tzr_pose_graph_optimize_line_process):
+// Open3D's GlobalOptimizationOption and ConvergenceCriteria, with its defaults.
+struct LineProcessParams {
+  double max_correspondence_distance = 0;  // no default: must be set (> 0), normally the ICP distance
+  double edge_prune_threshold = 0.25;
+  double preference_loop_closure = 1.0;
+  int reference_node = 0;                  // -1: no compensation (Open3D's own default)
+  int max_iteration = 100;
+  double min_relative_increment = 1e-6;
+  double min_relative_residual_increment = 1e-6;
+  double min_right_term = 1e-6;
+  double min_residual = 1e-6;
+  int max_iteration_lm = 20;
+  double upper_scale_factor = 2.0 / 3.0;
+  double lower_scale_factor = 1.0 / 3.0;
+};
+// tzr_line_process_summary: per pass (pass 1 on every edge, pass 2 on the kept ones)
+struct LineProcessSummary {
+  int iterations[2] = {0, 0};   // outer iterations begun
+  int trials[2] = {0, 0};       // linear solves
+  int stop_reason[2] = {0, 0};  // TZR_LP_STOP_*
+  int pruned = 0;               // uncertain edges pruned after pass 1
+  double residual = 0;          // F at the end of pass 2
+  double mu[2] = {0, 0};
+};
 struct PointToPointICPResult {
   RegistrationSolution solution;  // the refined transform; scale is the seed's, held fixed
   double fitness = 0;
@@ -417,6 +442,7 @@ class RobustRegistrationSolver {
     int iterations = 0;
     int inner_iterations = 0;
     double cost = 0;
+    LineProcessSummary line_process;  // the line-process overloads: their summary (iterations and cost stay 0)
   };
   MultiwayResult solveMultiway(const std::vector<PointCloud>& clouds, const std::vector<std::pair<int, int>>& pairs,
                                const CloudPairParams& params, const PointToPointICPParams& icp,
@@ -433,6 +459,23 @@ class RobustRegistrationSolver {
   MultiwayResult solveMultiway(const std::vector<PointCloud>& clouds, const std::vector<ColorCloud>& colors,
                                const std::vector<std::pair<int, int>>& pairs, const CloudPairParams& params,
                                const ColoredICPParams& icp, const PoseGraphParams& pose_graph,
+                               const std::vector<bool>& uncertain, const RobustKernel& kernel = RobustKernel());
+  // The four overloads above with Open3D's line process in place of GNC-TLS
+  // (tzr_register_cloud_pairs_multiway_line_process): edge_weights receive the confidences, edge_inliers the kept mask,
+  // pose_graph_status the optimiser's status and line_process its summary.
+  MultiwayResult solveMultiway(const std::vector<PointCloud>& clouds, const std::vector<std::pair<int, int>>& pairs,
+                               const CloudPairParams& params, const PointToPointICPParams& icp,
+                               const LineProcessParams& global_optimization);
+  MultiwayResult solveMultiway(const std::vector<PointCloud>& clouds, const std::vector<std::pair<int, int>>& pairs,
+                               const CloudPairParams& params, const PointToPointICPParams& icp,
+                               const LineProcessParams& global_optimization, const std::vector<bool>& uncertain);
+  MultiwayResult solveMultiway(const std::vector<PointCloud>& clouds, const std::vector<ColorCloud>& colors,
+                               const std::vector<std::pair<int, int>>& pairs, const CloudPairParams& params,
+                               const ColoredICPParams& icp, const LineProcessParams& global_optimization,
+                               const RobustKernel& kernel = RobustKernel());
+  MultiwayResult solveMultiway(const std::vector<PointCloud>& clouds, const std::vector<ColorCloud>& colors,
+                               const std::vector<std::pair<int, int>>& pairs, const CloudPairParams& params,
+                               const ColoredICPParams& icp, const LineProcessParams& global_optimization,
                                const std::vector<bool>& uncertain, const RobustKernel& kernel = RobustKernel());
   bool isMaxCliqueProvenOptimal() const { return clique_proven_; }
   long long getNumInlierGraphEdges() const { return n_edges_; }

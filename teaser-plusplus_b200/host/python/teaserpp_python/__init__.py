@@ -12,7 +12,7 @@ from . import _teaserpp as _ext
 
 # ---- re-exports -----------------------------------------------------------------------------------------------------
 _PUBLIC = ("OMP_MAX_THREADS", "CertificationResult", "ColoredICP", "DRSCertifier", "EigSolverType",
-           "FastGlobalRegistration", "GeneralizedICP", "InlierGraphFormulation", "InlierSelectionMode", "MultiScaleICP",
+           "FastGlobalRegistration", "GeneralizedICP", "GlobalOptimization", "InlierGraphFormulation", "InlierSelectionMode", "MultiScaleICP",
            "PointToPlaneICP", "PointToPointICP", "PoseGraph", "RANSACRegistration", "RegistrationSolution",
            "RobustKernel", "RobustRegistrationSolver", "RotationEstimationAlgorithm", "estimate_color_gradients",
            "estimate_color_gradients_batch", "estimate_normals", "estimate_normals_batch", "information_matrix",

@@ -117,6 +117,15 @@ py::array_t<double> gradients_to_numpy(const std::vector<std::array<double, 3>>&
   return out;
 }
 
+// tzr_line_process_summary as global_optimization's keys (lists of the two passes)
+py::dict line_process_dict(const teaser::LineProcessSummary& s) {
+  return py::dict(py::arg("iterations") = std::vector<int>(s.iterations, s.iterations + 2),
+                  py::arg("trials") = std::vector<int>(s.trials, s.trials + 2),
+                  py::arg("stop_reason") = std::vector<int>(s.stop_reason, s.stop_reason + 2),
+                  py::arg("pruned") = s.pruned, py::arg("residual") = s.residual,
+                  py::arg("mu") = std::vector<double>(s.mu, s.mu + 2));
+}
+
 py::dict icp_dict(const teaser::PointToPointICPResult& r) {
   return py::dict(py::arg("solution") = r.solution, py::arg("fitness") = r.fitness,
                   py::arg("inlier_rmse") = r.inlier_rmse, py::arg("iterations") = r.iterations,
@@ -495,6 +504,69 @@ PYBIND11_MODULE(_teaserpp, m) {
             return py::dict(py::arg("poses") = poses, py::arg("weights") = r.weights, py::arg("inliers") = r.inliers,
                             py::arg("residuals") = r.residuals, py::arg("iterations") = r.iterations,
                             py::arg("inner_iterations") = r.inner_iterations, py::arg("cost") = r.cost);
+          },
+          py::arg("num_nodes"), py::arg("edges"), py::arg("transforms"), py::arg("information"),
+          py::arg("uncertain") = std::vector<bool>(), py::arg("initial_poses") = py::none());
+
+  // GPU extra: Open3D's line-process pose graph (teaser::GlobalOptimization)
+  py::class_<teaser::GlobalOptimization>(m, "GlobalOptimization")
+      .def(py::init([](double max_correspondence_distance, double edge_prune_threshold,
+                       double preference_loop_closure, int reference_node, int max_iteration,
+                       double min_relative_increment, double min_relative_residual_increment, double min_right_term,
+                       double min_residual, int max_iteration_lm, double upper_scale_factor,
+                       double lower_scale_factor) {
+             teaser::GlobalOptimization::Params p;
+             p.max_correspondence_distance = max_correspondence_distance;
+             p.edge_prune_threshold = edge_prune_threshold;
+             p.preference_loop_closure = preference_loop_closure;
+             p.reference_node = reference_node;
+             p.max_iteration = max_iteration;
+             p.min_relative_increment = min_relative_increment;
+             p.min_relative_residual_increment = min_relative_residual_increment;
+             p.min_right_term = min_right_term;
+             p.min_residual = min_residual;
+             p.max_iteration_lm = max_iteration_lm;
+             p.upper_scale_factor = upper_scale_factor;
+             p.lower_scale_factor = lower_scale_factor;
+             return teaser::GlobalOptimization(p);
+           }),
+           py::arg("max_correspondence_distance"), py::arg("edge_prune_threshold") = 0.25,
+           py::arg("preference_loop_closure") = 1.0, py::arg("reference_node") = 0, py::arg("max_iteration") = 100,
+           py::arg("min_relative_increment") = 1e-6, py::arg("min_relative_residual_increment") = 1e-6,
+           py::arg("min_right_term") = 1e-6, py::arg("min_residual") = 1e-6, py::arg("max_iteration_lm") = 20,
+           py::arg("upper_scale_factor") = 2.0 / 3.0, py::arg("lower_scale_factor") = 1.0 / 3.0)
+      .def(
+          "optimize",
+          [](const teaser::GlobalOptimization& g, int num_nodes, const std::vector<std::pair<int, int>>& edges,
+             const std::vector<SqArr>& transforms, const std::vector<SqArr>& information,
+             const std::vector<bool>& uncertain, const py::object& initial_poses) {
+            if (transforms.size() != edges.size() || information.size() != edges.size() ||
+                (!uncertain.empty() && uncertain.size() != edges.size()))
+              throw std::invalid_argument("one transform, information matrix (and uncertain flag) per edge");
+            std::vector<teaser::GlobalOptimization::Edge> E(edges.size());
+            for (size_t e = 0; e < edges.size(); ++e) {
+              E[e].source = edges[e].first;
+              E[e].target = edges[e].second;
+              E[e].transform = square_of<4>(transforms[e]);
+              E[e].information = square_of<6>(information[e]);
+              E[e].uncertain = !uncertain.empty() && uncertain[e];
+            }
+            std::vector<Eigen::Matrix4d> init;
+            if (!initial_poses.is_none())
+              for (const auto& a : initial_poses.cast<std::vector<SqArr>>()) init.push_back(square_of<4>(a));
+            teaser::GlobalOptimization::Result r;
+            {
+              py::gil_scoped_release release;
+              r = g.optimize(num_nodes, E, initial_poses.is_none() ? nullptr : &init);
+            }
+            py::list poses;
+            for (const auto& T : r.poses) poses.append(square_to_numpy<4>(T));
+            py::dict out = line_process_dict(r.summary);
+            out["poses"] = poses;
+            out["confidence"] = r.confidence;
+            out["kept"] = r.kept;
+            out["residuals"] = r.residuals;
+            return out;
           },
           py::arg("num_nodes"), py::arg("edges"), py::arg("transforms"), py::arg("information"),
           py::arg("uncertain") = std::vector<bool>(), py::arg("initial_poses") = py::none());
@@ -1119,10 +1191,13 @@ PYBIND11_MODULE(_teaserpp, m) {
              bool use_absolute_scale, bool use_crosscheck, bool use_tuple_test, float tuple_scale,
              uint64_t tuple_seed, double gnc_factor, double cost_threshold, int max_iterations,
              int max_inner_iterations, int reference_node, const py::object& colors, double lambda_geometric,
-             const py::object& kernel) {
+             const py::object& kernel, const py::object& global_optimization) {
             // GPU extra: solve_cloud_pairs_icp(method="point_to_plane"), information matrices and the GNC-TLS pose
             // graph in one call (solveMultiway); uncertain None: pair (k, k + 1) certain, every other pair uncertain.
-            // colors (one (n,3) array per cloud): method="colored" instead, with lambda_geometric and kernel (None: L2)
+            // colors (one (n,3) array per cloud): method="colored" instead, with lambda_geometric and kernel (None: L2).
+            // global_optimization (a GlobalOptimization): Open3D's line process in place of GNC-TLS, whose keyword
+            // arguments must then stay at their defaults; edge_weights / edge_inliers hold the confidences and the
+            // kept mask, and the summary keys of GlobalOptimization.optimize are added.
             if (!kernel.is_none() && colors.is_none())
               throw std::invalid_argument("a robust kernel needs colors (coloured ICP)");
             const teaser::RobustKernel rk = kernel.is_none() ? teaser::RobustKernel() : kernel.cast<teaser::RobustKernel>();
@@ -1153,10 +1228,25 @@ PYBIND11_MODULE(_teaserpp, m) {
             pg.reference_node = reference_node;
             const bool given = !uncertain.is_none();
             const std::vector<bool> unc = given ? uncertain.cast<std::vector<bool>>() : std::vector<bool>();
+            const bool lp = !global_optimization.is_none();
+            if (lp && (gnc_factor != 1.4 || cost_threshold != 1e-6 || max_iterations != 100 ||
+                       max_inner_iterations != 10 || reference_node != 0))
+              throw std::invalid_argument("the GNC-TLS arguments do not apply with global_optimization");
+            const teaser::LineProcessParams lpp =
+                lp ? global_optimization.cast<const teaser::GlobalOptimization&>().getParams()
+                   : teaser::LineProcessParams();
             Solver::MultiwayResult r;
             {
               py::gil_scoped_release release;
-              if (!colors.is_none()) {
+              if (lp && !colors.is_none()) {
+                teaser::ColoredICPParams cip;
+                static_cast<teaser::PointToPointICPParams&>(cip) = ip;
+                cip.lambda_geometric = lambda_geometric;
+                r = given ? s.solveMultiway(pcs, ccs, pairs, cp, cip, lpp, unc, rk)
+                          : s.solveMultiway(pcs, ccs, pairs, cp, cip, lpp, rk);
+              } else if (lp) {
+                r = given ? s.solveMultiway(pcs, pairs, cp, ip, lpp, unc) : s.solveMultiway(pcs, pairs, cp, ip, lpp);
+              } else if (!colors.is_none()) {
                 teaser::ColoredICPParams cip;
                 static_cast<teaser::PointToPointICPParams&>(cip) = ip;
                 cip.lambda_geometric = lambda_geometric;
@@ -1173,12 +1263,14 @@ PYBIND11_MODULE(_teaserpp, m) {
                                        py::arg("icp") = q.refined ? py::object(icp_dict(q.icp)) : py::object(py::none())));
             for (const auto& M : r.information) info.append(square_to_numpy<6>(M));
             for (const auto& T : r.poses) poses.append(square_to_numpy<4>(T));
-            return py::dict(py::arg("pairs") = pair_out, py::arg("information") = info,
-                            py::arg("information_counts") = r.information_counts,
-                            py::arg("edge_weights") = r.edge_weights, py::arg("edge_inliers") = r.edge_inliers,
-                            py::arg("poses") = poses, py::arg("pose_graph_status") = r.pose_graph_status,
-                            py::arg("iterations") = r.iterations, py::arg("inner_iterations") = r.inner_iterations,
-                            py::arg("cost") = r.cost);
+            py::dict out(py::arg("pairs") = pair_out, py::arg("information") = info,
+                         py::arg("information_counts") = r.information_counts,
+                         py::arg("edge_weights") = r.edge_weights, py::arg("edge_inliers") = r.edge_inliers,
+                         py::arg("poses") = poses, py::arg("pose_graph_status") = r.pose_graph_status,
+                         py::arg("iterations") = r.iterations, py::arg("inner_iterations") = r.inner_iterations,
+                         py::arg("cost") = r.cost);
+            if (lp) out["line_process"] = line_process_dict(r.line_process);
+            return out;
           },
           py::arg("clouds"), py::arg("pairs"), py::arg("max_correspondence_distance"), py::arg("uncertain") = py::none(),
           py::arg("max_iteration") = 30, py::arg("relative_fitness") = 1e-6, py::arg("relative_rmse") = 1e-6,
@@ -1187,7 +1279,7 @@ PYBIND11_MODULE(_teaserpp, m) {
           py::arg("tuple_scale") = 0.0f, py::arg("tuple_seed") = 0x7ea5e2ull, py::arg("gnc_factor") = 1.4,
           py::arg("cost_threshold") = 1e-6, py::arg("max_iterations") = 100, py::arg("max_inner_iterations") = 10,
           py::arg("reference_node") = 0, py::arg("colors") = py::none(), py::arg("lambda_geometric") = 0.968,
-          py::arg("kernel") = py::none())
+          py::arg("kernel") = py::none(), py::arg("global_optimization") = py::none())
       .def_property_readonly("solution", &Solver::getSolution)
       .def("getSolution", &Solver::getSolution)
       .def_property_readonly("gnc_rotation_cost_at_termination", &Solver::getGNCRotationCostAtTermination)

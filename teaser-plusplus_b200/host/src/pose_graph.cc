@@ -53,7 +53,43 @@ Matrix6d matrix6_of(const double* L) {
   return M;
 }
 
+// the edge arrays of both optimisers' C calls
+void edges_c(const std::vector<PoseGraph::Edge>& edges, std::vector<int32_t>* ends, std::vector<int32_t>* unc,
+             std::vector<tzr_similarity>* tr, std::vector<double>* L) {
+  const size_t E = edges.size();
+  ends->resize(2 * E);
+  unc->resize(E);
+  tr->resize(E);
+  L->resize(36 * E);
+  for (size_t e = 0; e < E; ++e) {
+    (*ends)[2 * e] = edges[e].source;
+    (*ends)[2 * e + 1] = edges[e].target;
+    (*unc)[e] = edges[e].uncertain ? 1 : 0;
+    (*tr)[e] = sim_of(edges[e].transform);
+    for (int r = 0; r < 6; ++r)
+      for (int c = 0; c < 6; ++c) (*L)[36 * e + 6 * r + c] = edges[e].information(r, c);
+  }
+}
+
 }  // namespace
+
+tzr_line_process_params line_process_c(const LineProcessParams& q) {
+  tzr_line_process_params p;
+  tzr_line_process_params_default(&p);
+  p.max_correspondence_distance = q.max_correspondence_distance;
+  p.edge_prune_threshold = q.edge_prune_threshold;
+  p.preference_loop_closure = q.preference_loop_closure;
+  p.reference_node = q.reference_node;
+  p.max_iteration = q.max_iteration;
+  p.min_relative_increment = q.min_relative_increment;
+  p.min_relative_residual_increment = q.min_relative_residual_increment;
+  p.min_right_term = q.min_right_term;
+  p.min_residual = q.min_residual;
+  p.max_iteration_lm = q.max_iteration_lm;
+  p.upper_scale_factor = q.upper_scale_factor;
+  p.lower_scale_factor = q.lower_scale_factor;
+  return p;
+}
 
 std::vector<Matrix6d> informationMatrixBatch(const std::vector<PointCloud>& src, const std::vector<PointCloud>& dst,
                                              const std::vector<RegistrationSolution>& T,
@@ -116,17 +152,10 @@ PoseGraph::Result PoseGraph::optimize(int num_nodes, const std::vector<Edge>& ed
   p.max_iterations = params_.max_iterations;
   p.max_inner_iterations = params_.max_inner_iterations;
   p.reference_node = params_.reference_node;
-  std::vector<int32_t> ends(2 * E), unc(E);
-  std::vector<tzr_similarity> tr(E);
-  std::vector<double> L(36 * E);
-  for (size_t e = 0; e < E; ++e) {
-    ends[2 * e] = edges[e].source;
-    ends[2 * e + 1] = edges[e].target;
-    unc[e] = edges[e].uncertain ? 1 : 0;
-    tr[e] = sim_of(edges[e].transform);
-    for (int r = 0; r < 6; ++r)
-      for (int c = 0; c < 6; ++c) L[36 * e + 6 * r + c] = edges[e].information(r, c);
-  }
+  std::vector<int32_t> ends, unc;
+  std::vector<tzr_similarity> tr;
+  std::vector<double> L;
+  edges_c(edges, &ends, &unc, &tr, &L);
   std::vector<tzr_similarity> init;
   if (initial_poses)
     for (const Eigen::Matrix4d& T : *initial_poses) init.push_back(sim_of(T));
@@ -147,6 +176,45 @@ PoseGraph::Result PoseGraph::optimize(int num_nodes, const std::vector<Edge>& ed
   out.iterations = summary.iterations;
   out.inner_iterations = summary.inner_iterations;
   out.cost = summary.cost;
+  return out;
+}
+
+GlobalOptimization::Result GlobalOptimization::optimize(int num_nodes, const std::vector<Edge>& edges,
+                                                        const std::vector<Eigen::Matrix4d>* initial_poses) const {
+  const size_t E = edges.size();
+  if (initial_poses && initial_poses->size() != static_cast<size_t>(num_nodes))
+    throw std::invalid_argument("teaser::GlobalOptimization::optimize: one initial pose per node");
+  const tzr_line_process_params p = line_process_c(params_);
+  std::vector<int32_t> ends, unc;
+  std::vector<tzr_similarity> tr;
+  std::vector<double> L;
+  edges_c(edges, &ends, &unc, &tr, &L);
+  std::vector<tzr_similarity> init;
+  if (initial_poses)
+    for (const Eigen::Matrix4d& T : *initial_poses) init.push_back(sim_of(T));
+  std::vector<tzr_similarity> poses(num_nodes > 0 ? num_nodes : 1);
+  std::vector<double> l(E ? E : 1), res(E ? E : 1);
+  std::vector<uint8_t> kept(E ? E : 1);
+  tzr_line_process_summary s{};
+  tzr_ctx* ctx = b200_context();
+  const int rc = tzr_pose_graph_optimize_line_process(ctx, &p, num_nodes, static_cast<int>(E), ends.data(),
+                                                      tr.data(), L.data(), unc.data(),
+                                                      initial_poses ? init.data() : nullptr, poses.data(), l.data(),
+                                                      kept.data(), res.data(), &s);
+  if (rc != TZR_OK) fail("teaser::GlobalOptimization::optimize", rc, ctx);
+  Result out;
+  for (int k = 0; k < num_nodes; ++k) out.poses.push_back(matrix_of(poses[k]));
+  out.confidence.assign(l.begin(), l.begin() + E);
+  for (size_t e = 0; e < E; ++e) out.kept.push_back(kept[e] != 0);
+  out.residuals.assign(res.begin(), res.begin() + E);
+  for (int q = 0; q < 2; ++q) {
+    out.summary.iterations[q] = s.iterations[q];
+    out.summary.trials[q] = s.trials[q];
+    out.summary.stop_reason[q] = s.stop_reason[q];
+    out.summary.mu[q] = s.mu[q];
+  }
+  out.summary.pruned = s.pruned;
+  out.summary.residual = s.residual;
   return out;
 }
 

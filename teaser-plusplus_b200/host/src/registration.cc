@@ -628,6 +628,7 @@ std::vector<RobustRegistrationSolver::SolveCertifyResult> RobustRegistrationSolv
 }
 
 void icp_result_from_c(const tzr_icp_result& r, const int32_t* corr, PointToPointICPResult* out);  // icp.cc
+tzr_line_process_params line_process_c(const LineProcessParams& p);                                  // pose_graph.cc
 
 namespace {
 
@@ -645,6 +646,8 @@ struct MultiwayCall {
   tzr_similarity* poses;
   tzr_pose_graph_summary* summary;
   int32_t* pg_status;
+  const tzr_line_process_params* lp = nullptr;  // the line process in place of GNC-TLS (pg unused)
+  tzr_line_process_summary* lp_summary = nullptr;
 };
 std::vector<RobustRegistrationSolver::CloudPairResult> run_cloud_pairs(
     const tzr_params& p, const std::vector<PointCloud>& clouds, const std::vector<std::pair<int, int>>& pairs,
@@ -714,7 +717,15 @@ std::vector<RobustRegistrationSolver::CloudPairResult> run_cloud_pairs(
       k.type = static_cast<int32_t>(kernel->type);
       k.k = kernel->k;
     }
-    if (mw && method == IcpMethod::kColored) {
+    if (mw && mw->lp) {
+      const bool colored = method == IcpMethod::kColored;
+      rc = tzr_register_cloud_pairs_multiway_line_process(
+          ctx, &f, &p, K, n.data(), pts.data(), P, pc.data(), seeds.data(), sols.data(), status.data(), index.data(),
+          n_corr.data(), corr_p.data(), clq_p.data(), scales.data(), icp, colored ? col.data() : nullptr,
+          colored ? lambda_geometric : 0.0, colored && kernel ? &k : nullptr, icp_res->data(), mw->uncertain, mw->lp,
+          mw->information, mw->info_counts, mw->edge_weights, mw->edge_mask, mw->poses, mw->lp_summary,
+          mw->pg_status);
+    } else if (mw && method == IcpMethod::kColored) {
       rc = tzr_register_cloud_pairs_multiway_colored(
           ctx, &f, &p, K, n.data(), pts.data(), P, pc.data(), seeds.data(), sols.data(), status.data(), index.data(),
           n_corr.data(), corr_p.data(), clq_p.data(), scales.data(), icp, col.data(), lambda_geometric,
@@ -811,7 +822,7 @@ static RobustRegistrationSolver::MultiwayResult run_multiway(
     const RobustRegistrationSolver::CloudPairParams& cp, const PointToPointICPParams& icp,
     const PoseGraphParams& pose_graph, const std::vector<bool>& uncertain,
     const std::vector<ColorCloud>* colors = nullptr, double lambda_geometric = 0,
-    const RobustKernel* kernel = nullptr) {
+    const RobustKernel* kernel = nullptr, const LineProcessParams* line_process = nullptr) {
   using CloudPairResult = RobustRegistrationSolver::CloudPairResult;
   const size_t P = pairs.size(), K = clouds.size();
   if (uncertain.size() != P) throw std::invalid_argument("teaser: solveMultiway: one uncertain flag per pair");
@@ -836,8 +847,15 @@ static RobustRegistrationSolver::MultiwayResult run_multiway(
   std::vector<tzr_similarity> poses(K);
   tzr_pose_graph_summary summary{};
   int32_t pg_status = 0;
-  const MultiwayCall mw{unc.data(), &pg, info.data(), counts.data(), w.data(), mask.data(), poses.data(), &summary,
-                        &pg_status};
+  MultiwayCall mw{unc.data(), &pg, info.data(), counts.data(), w.data(), mask.data(), poses.data(), &summary,
+                  &pg_status};
+  tzr_line_process_params lp;
+  tzr_line_process_summary lp_summary{};
+  if (line_process) {
+    lp = line_process_c(*line_process);
+    mw.lp = &lp;
+    mw.lp_summary = &lp_summary;
+  }
   std::vector<tzr_icp_result> res;
   std::vector<CloudPairResult> base =
       run_cloud_pairs(p, clouds, pairs, cp, &ip, &res, colors ? IcpMethod::kColored : IcpMethod::kPointToPlane, 0,
@@ -870,7 +888,44 @@ static RobustRegistrationSolver::MultiwayResult run_multiway(
   out.iterations = summary.iterations;
   out.inner_iterations = summary.inner_iterations;
   out.cost = summary.cost;
+  for (int q = 0; q < 2; ++q) {
+    out.line_process.iterations[q] = lp_summary.iterations[q];
+    out.line_process.trials[q] = lp_summary.trials[q];
+    out.line_process.stop_reason[q] = lp_summary.stop_reason[q];
+    out.line_process.mu[q] = lp_summary.mu[q];
+  }
+  out.line_process.pruned = lp_summary.pruned;
+  out.line_process.residual = lp_summary.residual;
   return out;
+}
+
+RobustRegistrationSolver::MultiwayResult RobustRegistrationSolver::solveMultiway(
+    const std::vector<PointCloud>& clouds, const std::vector<std::pair<int, int>>& pairs, const CloudPairParams& cp,
+    const PointToPointICPParams& icp, const LineProcessParams& global_optimization) {
+  return solveMultiway(clouds, pairs, cp, icp, global_optimization, tutorial_uncertain(pairs));
+}
+
+RobustRegistrationSolver::MultiwayResult RobustRegistrationSolver::solveMultiway(
+    const std::vector<PointCloud>& clouds, const std::vector<std::pair<int, int>>& pairs, const CloudPairParams& cp,
+    const PointToPointICPParams& icp, const LineProcessParams& global_optimization,
+    const std::vector<bool>& uncertain) {
+  return run_multiway(to_c(params_), clouds, pairs, cp, icp, PoseGraphParams(), uncertain, nullptr, 0, nullptr,
+                      &global_optimization);
+}
+
+RobustRegistrationSolver::MultiwayResult RobustRegistrationSolver::solveMultiway(
+    const std::vector<PointCloud>& clouds, const std::vector<ColorCloud>& colors,
+    const std::vector<std::pair<int, int>>& pairs, const CloudPairParams& cp, const ColoredICPParams& icp,
+    const LineProcessParams& global_optimization, const RobustKernel& kernel) {
+  return solveMultiway(clouds, colors, pairs, cp, icp, global_optimization, tutorial_uncertain(pairs), kernel);
+}
+
+RobustRegistrationSolver::MultiwayResult RobustRegistrationSolver::solveMultiway(
+    const std::vector<PointCloud>& clouds, const std::vector<ColorCloud>& colors,
+    const std::vector<std::pair<int, int>>& pairs, const CloudPairParams& cp, const ColoredICPParams& icp,
+    const LineProcessParams& global_optimization, const std::vector<bool>& uncertain, const RobustKernel& kernel) {
+  return run_multiway(to_c(params_), clouds, pairs, cp, icp, PoseGraphParams(), uncertain, &colors,
+                      icp.lambda_geometric, &kernel, &global_optimization);
 }
 
 RobustRegistrationSolver::MultiwayResult RobustRegistrationSolver::solveMultiway(
