@@ -392,6 +392,11 @@ int tzr_solve_batch_ragged_dev(tzr_ctx* ctx, const tzr_params* params, int B, co
  * problem b (caller's order) has its own n[b] rows of tzr_words_per_row(n[b]) words and n[b] degrees, equal to its
  * single-solve graph. */
 int tzr_last_graph(tzr_ctx* ctx, int b, uint64_t* adj_bits, int32_t* degree);
+/* The graph filter's constants of problem b of the most recent solve (diagnostics: how its graph was built).  centres6:
+ * the source and destination box centres subtracted before the float conversion; gram7: the two-slope Gram test's
+ * m_hi, c_hi, m_lo, c_lo and the single-slope test's c_u, c_v, dl (0 when the problem does not run it); paths2: 1 if
+ * every pair takes the exact FP64 test, 1 if the conditioning guard admits the Gram test.  Any pointer may be NULL. */
+int tzr_last_filter_consts(tzr_ctx* ctx, int b, double* centres6, float* gram7, int32_t* paths2);
 /* What tzr_last_graph would return: batch size and n of the retained solve (0, 0 if none; the largest n after a ragged
  * batch), whether a graph was
  * built (0 after inlier selection NONE: the reference never populates the graph, registration.cc:607-650, and

@@ -241,7 +241,7 @@ _SYMBOLS = [
     "tzr_abi_version", "tzr_status_string", "tzr_last_error", "tzr_params_default", "tzr_ctx_create",
     "tzr_ctx_destroy", "tzr_ctx_set_stream", "tzr_ctx_synchronize", "tzr_ctx_kernel_launches", "tzr_words_per_row",
     "tzr_graph_build", "tzr_max_clique", "tzr_max_clique_batch", "tzr_gnc_tls_rotation", "tzr_rotation_solve", "tzr_tls_translation", "tzr_scalar_tls",
-    "tzr_solve", "tzr_solve_batch", "tzr_solve_batch_dev", "tzr_solve_batch_ragged_dev", "tzr_last_graph", "tzr_last_stage_ms",
+    "tzr_solve", "tzr_solve_batch", "tzr_solve_batch_dev", "tzr_solve_batch_ragged_dev", "tzr_last_graph", "tzr_last_filter_consts", "tzr_last_stage_ms",
     "tzr_ctx_set_flags", "tzr_ctx_filter_mismatches", "tzr_ctx_filter_rechecks", "tzr_ctx_debug_counters",
     "tzr_match_correspondences", "tzr_feature_nn", "tzr_compute_fpfh", "tzr_certifier_params_default", "tzr_certify",
     "tzr_certifier_initial_matrix", "tzr_certifier_dual_projection", "tzr_last_graph_info", "tzr_ctx_stage_log",
@@ -347,6 +347,7 @@ def lib():
     L.tzr_solve_batch_dev.argtypes = [vp, C.POINTER(Params), C.c_int, C.c_int, vp, vp, vp, vp]
     L.tzr_solve_batch_ragged_dev.argtypes = [vp, C.POINTER(Params), C.c_int, i32p, vp, vp, vp, vp]
     L.tzr_last_graph.argtypes = [vp, C.c_int, u64p, i32p]
+    L.tzr_last_filter_consts.argtypes = [vp, C.c_int, dp, C.POINTER(C.c_float), i32p]
     L.tzr_last_stage_ms.argtypes = [vp, dp, dp, dp, dp]
     L.tzr_last_graph_info.argtypes = [vp, i32p, i32p, i32p, u64p]
     L.tzr_ctx_stage_log.argtypes = [vp, C.c_int]
@@ -2047,6 +2048,16 @@ class Context:
         deg = np.zeros(n, dtype=np.int32)
         self._ck(lib().tzr_last_graph(self._h, b, _p(bits, C.c_uint64), _p(deg, C.c_int32)))
         return bits, deg
+
+    def last_filter_consts(self, b: int):
+        """Graph filter constants of problem b of the most recent solve: box centres, the Gram tests' constants (float32)
+        and which paths the problem takes."""
+        cen = np.zeros(6, dtype=np.float64)
+        g = np.zeros(7, dtype=np.float32)
+        paths = np.zeros(2, dtype=np.int32)
+        self._ck(lib().tzr_last_filter_consts(self._h, b, _p(cen, C.c_double), _p(g, C.c_float), _p(paths, C.c_int32)))
+        return dict(cs=cen[:3], cd=cen[3:], mhi=g[0], chi=g[1], mlo=g[2], clo=g[3], cu=g[4], cv=g[5], dl=g[6],
+                    use_fp64=bool(paths[0]), use_gram=bool(paths[1]))
 
 
 def rotation_from_solution_record(rec) -> np.ndarray:

@@ -679,7 +679,7 @@ int run_pipeline(tzr_ctx* ctx, Batch& bt, const tzr_params& p, cudaEvent_t* ev, 
   ctx->launches += 1;
   // before prep: the FP32 filter copies are pre-scaled by the estimate
   if (bt.scale_mode) ctx->launches += launch_scale_estimation(bt, ctx->flags, ctx->sc.p, sg);
-  launch_prep(bt, sg);
+  CK(launch_prep(bt, sg));
   ctx->launches += 1;
   cudaEventRecord(ev[1], sg);
   int nl = 0;
@@ -1362,7 +1362,7 @@ int tzr_graph_build(tzr_ctx* ctx, const double* src, const double* dst, int n, d
   CK(cudaMemcpyAsync((void*)bt.src, src, (size_t)n * 3 * sizeof(double), cudaMemcpyHostToDevice, st));
   CK(cudaMemcpyAsync((void*)bt.dst, dst, (size_t)n * 3 * sizeof(double), cudaMemcpyHostToDevice, st));
   if (ctx->flags & 6u) cudaMemsetAsync((void*)ctx->dbg.p, 0, 16 * sizeof(unsigned long long), st);
-  launch_prep(bt, st);
+  CK(launch_prep(bt, st));
   ctx->launches += 2 + launch_graph(bt, st, ctx->num_sms, &ctx->last_strip_blocks);
   launch_degree(bt, st);
   rc = check_launch(ctx, "graph build");
@@ -1795,6 +1795,29 @@ int tzr_last_graph(tzr_ctx* ctx, int b, uint64_t* adj_bits, int32_t* degree) {
                          cudaMemcpyDeviceToHost, st));
   if (degree) CK(cudaMemcpyAsync(degree, v.deg, (size_t)n * 4, cudaMemcpyDeviceToHost, st));
   CK(cudaStreamSynchronize(st));
+  return TZR_OK;
+}
+
+int tzr_last_filter_consts(tzr_ctx* ctx, int b, double* centres6, float* gram7, int32_t* paths2) {
+  if (!ctx || b < 0 || b >= (int)ctx->last.at.size()) return TZR_ERR_INVALID_ARG;
+  cudaSetDevice(ctx->device);
+  const Batch v = retained_problem(ctx, b);
+  GraphConsts gc;
+  CK(cudaMemcpyAsync(&gc, v.gc, sizeof(gc), cudaMemcpyDeviceToHost, ctx->stream));
+  CK(cudaStreamSynchronize(ctx->stream));
+  if (centres6)
+    for (int k = 0; k < 3; ++k) {
+      centres6[k] = gc.cs[k];
+      centres6[3 + k] = gc.cd[k];
+    }
+  if (gram7) {
+    const float g[7] = {gc.g_mhi, gc.g_chi, gc.g_mlo, gc.g_clo, gc.g_cu, gc.g_cv, gc.g_dl};
+    for (int k = 0; k < 7; ++k) gram7[k] = g[k];
+  }
+  if (paths2) {
+    paths2[0] = gc.use_fp64;
+    paths2[1] = gc.use_gram;
+  }
   return TZR_OK;
 }
 

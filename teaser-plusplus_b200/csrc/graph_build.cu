@@ -25,7 +25,11 @@
 namespace tzr {
 
 // ------------------------------------------------------------------------------------------------
-// prep: bounding boxes, centred float copies, filter constants.  One CTA per problem.
+// prep: bounding boxes, centred float copies, filter constants.  One thread-block cluster of up to kPrepCtas CTAs per
+// problem (prep_ctas): each CTA reduces the bounding boxes of its slice of the points, the cluster exchanges the partial boxes
+// through distributed shared memory, and each CTA then writes the float copies of its slice.  The problem's constants
+// are computed by CTA 0 alone, with the interval / v7, tensor-core and Gram groups on three warps; the other CTAs need
+// only the centres and the Gram scale, which they derive from the same boxes by the same operations.
 // ------------------------------------------------------------------------------------------------
 __device__ __forceinline__ double warp_min(double v) {
   for (int o = 16; o; o >>= 1) v = fmin(v, __shfl_xor_sync(0xffffffffu, v, o));
@@ -47,22 +51,256 @@ __host__ __device__ __forceinline__ bool tc_path_active(uint32_t flags) {
   return (flags & 1024u) && !(flags & (8u | 16u | 32u | 64u | 128u | 256u | 512u));
 }
 
-__global__ void __launch_bounds__(256) prep_kernel(Batch bt) {
-  const int b = blockIdx.x;
+constexpr int kPrepCtas = 8;  // most CTAs per problem: one cluster (the portable maximum)
+// points per CTA the cluster size aims at (prep_ctas).  Smaller clusters for small problems: a cluster is only placed
+// where all its CTAs fit at once, and CTA 0 stays resident through the serial constants
+constexpr int kPrepPoints = 640;
+constexpr int kPrepThreads = 256;
+constexpr double kU32 = 5.9604644775390625e-08;            // 2^-24
+constexpr double kUp = 1.0 + 9.5367431640625e-07, kDn = 1.0 - 9.5367431640625e-07;  // 1 +- 2^-20
+
+// What every constant group starts from: the boxes' centres and half extents, the scale, the exact-path decision and
+// the Gram test's conditioning guard.
+struct PrepBase {
+  double cs[3], cd[3], Ms, Md, beta, s_hat;
+  double Ds2, Dd2, b2, b4, lam, Dmin, gE;
+  int use64, use_gram;
+};
+
+__device__ PrepBase prep_base(const Batch& bt, int b, const double* mn, const double* mx, int anybad) {
+  PrepBase q;
+  double Ms = 0, Md = 0;
+  for (int k = 0; k < 3; ++k) {
+    q.cs[k] = 0.5 * (mn[k] + mx[k]);
+    q.cd[k] = 0.5 * (mn[3 + k] + mx[3 + k]);
+    Ms = fmax(Ms, 0.5 * (mx[k] - mn[k]));
+    Md = fmax(Md, 0.5 * (mx[3 + k] - mn[3 + k]));
+  }
+  const double beta = bt.beta;
+  q.beta = beta;
+  // Unknown scale: |d2/d1 - s| <= beta/d1  <=>  |d2 - s*d1| <= beta (d1 > 0), i.e. the fixed-scale test on a
+  // source cloud scaled by s: the float copies are pre-scaled, the exact re-check keeps the reference's
+  // division-based sequence (its rounding differs from the real-number predicate by ~1e-16 relative, far
+  // inside delta).
+  double s_hat = 1.0;
+  if (bt.scale_mode) {
+    s_hat = bt.sol[b].scale;
+    if (!(s_hat > 1e-6) || !(s_hat < 1e6)) {
+      s_hat = 1.0;
+      anybad = 1;  // degenerate estimate: exact path for every pair
+    }
+    Ms *= s_hat;
+  }
+  q.s_hat = s_hat;
+  q.Ms = Ms;
+  q.Md = Md;
+  // delta: bound on the FP32 error of |D1 - D2| (DESIGN.md: <= ~70 u32 (Ms+Md)); 256 u32 (...) used.
+  const double delta = 256.0 * kU32 * (Ms + Md + beta);
+  const double gam2 = beta + delta;
+  q.use64 = anybad || !(Ms < 1e8) || !(Md < 1e8) || !(gam2 > 1e-8) || !isfinite(beta) || (bt.flags_dbg & 1u);
+  double Ds2 = 0, Dd2 = 0;  // largest possible squared distance inside each (scaled) cloud
+  for (int k = 0; k < 3; ++k) {
+    const double es = (mx[k] - mn[k]) * s_hat, ed = mx[3 + k] - mn[3 + k];
+    Ds2 += es * es;
+    Dd2 += ed * ed;
+  }
+  q.Ds2 = Ds2;
+  q.Dd2 = Dd2;
+  q.b2 = beta * beta;
+  q.b4 = q.b2 * q.b2;
+  q.lam = 0.75 * beta * sqrt(0.5 * (Ds2 + Dd2));
+  q.Dmin = sqrt(fmin(Ds2, Dd2));
+  q.gE = 7.0 * kU32 * (Ds2 + Dd2);
+  // conditioning guard of the Gram test (same form as use_tc's): beta <= D/8 keeps pairs with s <= beta^2 rare, 64 E <=
+  // 0.75 D beta keeps the band narrow against beta (and k <= 1/64).  C1 (outliers moved 5-10 extents away, beta/D ~ 1e-4)
+  // fails it.
+  q.use_gram = (!q.use64 && (bt.flags_dbg & 512u) == 0 && Ds2 > 0 && Dd2 > 0 && Ds2 < 1e8 && Dd2 < 1e8 && q.b4 > 1e-30 &&
+                isfinite(q.gE) && 8.0 * beta <= q.Dmin && 64.0 * q.gE <= 0.75 * q.Dmin * beta) ? 1 : 0;
+  return q;
+}
+
+// 1 / (2 beta) for the problems whose graph is built by the single-slope Gram test (their gq copies), 0 otherwise
+__device__ __forceinline__ double prep_sig(const Batch& bt, const PrepBase& q) {
+  return (q.use_gram && !(bt.flags_dbg & kFlagTwoSlope)) ? 0.5 / q.beta : 0.0;
+}
+
+// interval test (graph_strip2_kernel's fallback) and v7 constants (graph_strip3_kernel)
+__device__ void prep_interval_v7(const PrepBase& q, GraphConsts& gc) {
+  const double beta = q.beta, Ms = q.Ms, Md = q.Md;
+  const int use64 = q.use64;
+  for (int k = 0; k < 3; ++k) {
+    gc.cs[k] = q.cs[k];
+    gc.cd[k] = q.cd[k];
+  }
+  gc.beta = beta;
+  const double delta = 256.0 * kU32 * (Ms + Md + beta);
+  const double gam1 = beta - delta, gam2 = beta + delta;
+  // sure edge: x <= b1; sure non-edge: x > b2.  Exact path for everything: b1 = -1 (x >= 0), b2 = +inf.
+  gc.b1 = (use64 || !(gam1 > 0)) ? -1.0f : (float)(gam1 * kDn);
+  gc.b2 = use64 ? __int_as_float(0x7f800000) : (float)(gam2 * kUp);
+  gc.use_fp64 = use64;
+  gc.pad = 0;
+  gc.s_hat = q.s_hat;
+  // ---- v7 strip kernel (graph_strip3_kernel): d_hi = t^2 - (beta^2 - K) w < 0 proves an edge, d_lo = t^2 -
+  // (beta^2 + K) w >= 0 proves a non-edge, K = dt (2 beta + dt) + 32 u beta^2 relative to w = (sqrt a + sqrt b)^2.
+  // dt bounds |g' - g|: float conversion of the centred coordinates (<= u M each), the differences, squares and sums
+  // give |sqrt a' - sqrt a| <= ~15 u M per cloud; 64 u (Ms + Md) is used, plus the bias eps of the squared norms.
+  const double d3 = 64.0 * kU32 * (Ms + Md);
+  const double eps = fmax((d3 / 16.0) * (d3 / 16.0), 1e-36);
+  const double dt = 1.125 * d3;
+  const double K = dt * (2.0 * beta + dt) + 32.0 * kU32 * beta * beta;
+  const double b2v = beta * beta;
+  gc.f3_eps = (float)eps;
+  if (use64) {  // exact path for every pair (the kernel also overrides the words: NaN inputs have no sign)
+    gc.f3_nlo = -__int_as_float(0x7f800000);
+    gc.f3_nhi = __int_as_float(0x7f800000);
+  } else {
+    gc.f3_nlo = (float)(-(b2v + K) * kUp);
+    gc.f3_nhi = (b2v - K > 0) ? (float)(-(b2v - K) * kDn) : (float)((K - b2v) * kUp + 1e-37);
+  }
+  gc.pad2 = 0;
+}
+
+// ---- tensor-core filter constants (graph_tc.cu; derivation in DESIGN.md §3.1).  a' = |ds|^2 and b' = |dd|^2 come
+// out of the tensor core with |a' - a| <= ea, |b' - b| <= eb (E = ea + eb).  With t = a - b, s = a + b,
+//   f(a, b) = t^2 - 2 beta^2 s + beta^4 = (g^2 - beta^2)(w - beta^2),  g = |sqrt a - sqrt b|,  w = (sqrt a + sqrt b)^2 >= s
+// so   edge  <=>  s <= beta^2  or  f <= 0   — a polynomial, no square root, no division:
+//   |f(a', b') - f(a, b)| <= 2 E |t'| + E^2 + 2 beta^2 E                      (tensor-core error)
+//   |d^ - f(a', b')|      <= 8 u (t'^2 + 2 beta^2 s' + beta^4)                 (FP32 evaluation of d^: 4 roundings + 2 constants)
+// and for s <= beta^2 (where the sign of f says nothing)  f <= (beta^2 - s)^2 <= beta^4.  The kernel decides by the
+// signs of d^ +- band, band = kap (t'^2 + beta^4) + c0 with 2 E |t'| <= (E/lam) t'^2 + E lam (lam = the typical |t| at the
+// threshold, 0.75 beta D): kap = E/lam + 8 u, c0 = E lam + E^2 + 2 beta^2 E + 16 u beta^2 Smax + 8 u beta^4 + beta^4.
+// (8 u t'^2 needs no case split: it is part of kap.)  d^ + band < 0 proves f < 0 (an edge whatever s is); d^ - band >= 0
+// proves f > beta^4, hence s > beta^2 and a non-edge; everything else goes to the exact FP64 re-check.
+__device__ void prep_tc(const Batch& bt, const PrepBase& q, GraphConsts& gc) {
+  const double beta = q.beta, Ds2 = q.Ds2, Dd2 = q.Dd2, b2 = q.b2, b4 = q.b4, lam = q.lam;
+  const double kappa = bt.tc_kappa > 0 ? bt.tc_kappa : kTcKappa;
+  const double ea = kappa * kU32 * Ds2, eb = kappa * kU32 * Dd2, E = ea + eb;
+  const double Smax = Ds2 + Dd2 + E;
+  const double kap = E / lam + 8.0 * kU32;
+  const double c0 = E * lam + E * E + 2.0 * b2 * E + 16.0 * kU32 * b2 * Smax + 8.0 * kU32 * b4 + b4;
+  // When is the filter worth it (correctness never depends on this)?  beta <= D/8: the beta^4 floor of the band stays
+  // below ~1e-3 of the pairs; E / (0.75 D) <= beta / 64: the band in g = |sqrt a - sqrt b| is a small fraction of the
+  // threshold (fails when the noise bound is tiny against the extent of a cloud: beta/D below ~3e-4); b4 a normal float.
+  const double Dmin = q.Dmin;
+  const bool ok = !q.use64 && (bt.flags_dbg & 1024u) != 0 && (bt.flags_dbg & 512u) == 0 && Ds2 > 0 && Dd2 > 0 &&
+                  Ds2 < 1e8 && Dd2 < 1e8 && b4 > 1e-30 && isfinite(E) && isfinite(kap) && 8.0 * beta <= Dmin &&
+                  64.0 * E <= 0.75 * Dmin * beta;
+  gc.use_tc = ok ? 1 : 0;
+  gc.tc_c2 = (float)(2.0 * b2);
+  gc.tc_b4 = (float)b4;
+  gc.tc_kap = (float)(kap * kUp);
+  gc.tc_c0 = (float)(c0 * kUp);
+  gc.tc_pad = 0.f;
+  if (ok && bt.rechecks) atomicAdd(bt.mismatches + 7, 1ull);  // debug counter 7: problems on the tensor-core path
+}
+
+// ---- Gram-form test of graph_strip2_kernel (derivation in DESIGN.md §3.1).  a' = fl(N_i + N_j - 2 q_i.q_j) from the
+// float copies q (|q| <= R, R^2 <= Ds2 / 4 about the box centre) is within 8 u R^2 (conversion) + 2 u R^2 (rounded
+// norms) + 14 u R^2 (one FADD and three FMA roundings on partial sums of at most 2 R^2 and 4 R^2) of a; 28 u R^2 is
+// used, the rest covers second-order terms and the reference's own FP64 rounding.  With E = ea + eb, k = E / lam,
+// C = E lam + E^2 + 2 beta^2 E and 4 u (t^2 + |m| S + |c|) the FP32 evaluation error of fma(t, t, fma(s, m, c)):
+//   t^2 + mhi s + chi <= 0  =>  (1 + k) t^2 - 2 beta^2 s + beta^4 + C <= 0  =>  f(a, b) <= 0           (edge)
+//   t^2 + mlo s + clo >= 0  =>  (1 - k) t^2 - 2 beta^2 s - C > 0            =>  f(a, b) > beta^4      (s > beta^2: not)
+__device__ void prep_gram(const Batch& bt, const PrepBase& q, GraphConsts& gc) {
+  const double beta = q.beta, Ds2 = q.Ds2, Dd2 = q.Dd2, b2 = q.b2, b4 = q.b4, lam = q.lam;
+  const double gE = q.gE, gk = gE / lam, gS = Ds2 + Dd2 + gE;
+  const double gC = gE * lam + gE * gE + 2.0 * b2 * gE;
+  gc.g_mhi = (float)(-2.0 * b2 * (1.0 - 4.0 * kU32) / (1.0 + gk) * kDn);
+  gc.g_chi = (float)(((b4 + gC) / (1.0 + gk) + 8.0 * kU32 * b2 * gS) * kUp);
+  gc.g_mlo = (float)(-2.0 * b2 * (1.0 + 4.0 * kU32) / (1.0 - gk) * kUp);
+  gc.g_clo = (float)(-(gC + 9.0 * kU32 * b2 * gS) / (1.0 - gk) * kUp * kUp);
+  gc.use_gram = q.use_gram;
+  // ---- single-slope form of the Gram test (default; derivation in DESIGN.md §3.1).  Lengths in units of 2 beta
+  // (sig = 1 / (2 beta), so beta^2 -> 1/4):  f = (A - B + 1/4)^2 - A,  edge <= f <= 0,  non-edge <= f > 1/16.  The kernel
+  // computes u = c_u - A', v = c_v - B' (A', B' within Eu, Ev of A, B; c_v = c_u + 1/4 exactly), T = fl(v - u),
+  // dh = fma(T, T, u) and dl = fl(dh + dl_c):
+  //   dh < 0   =>  T^2 < A - c_u + Eu  =>  f <= -c_u + Eu + 5u As + 2 E1 |T| (1 + 2u) + E1^2 <= 0         (edge)
+  //   dl >= 0  =>  T^2 >= A + K, K = |dl_c| (1 - u) - c_u - Eu  =>  f >= K (1 - 2u) - 2u As - 2 E1 sqrt(As + K) > 1/16
+  // with E1 = Eu + Ev, |T| <= sqrt(As + Eu) and A <= As (the scaled source diagonal squared).  Eu = 25 u R^2 + 5 u c_u
+  // to first order (conversion 8, norms 2, the row constant 1, the FADD 2, three FMAs 12; R^2 = As / 4); 28 and 6 are
+  // used.  c_u appears on both sides with a slope far below 1, so the fixed point is reached from below by iteration.
+  if (gc.use_gram && !(bt.flags_dbg & kFlagTwoSlope)) {
+    const double sig = 0.5 / beta, As = sig * sig * Ds2, Ad = sig * sig * Dd2;
+    auto eu = [&](double c) { return kU32 * (7.0 * As + 6.0 * c); };
+    auto ev = [&](double c) { return kU32 * (7.0 * Ad + 6.0 * (c + 0.25)); };
+    double cu = 0.0;
+    for (int it = 0; it < 8; ++it) {
+      const double Eu = eu(cu), E1 = Eu + ev(cu);
+      cu = Eu + 5.0 * kU32 * (As + Eu) + 2.0 * (1.0 + 2.0 * kU32) * E1 * sqrt(As + Eu) + E1 * E1;
+    }
+    const float cv_f = __double2float_ru((double)__double2float_ru(cu * (1.0 + 1.52587890625e-05)) + 0.25);
+    const double cu_f = (double)cv_f - 0.25;  // exact: c_v - c_u = 1/4 in the kernel's floats
+    const double Eu = eu(cu_f), E1 = Eu + ev(cu_f);
+    double K = 0.0;
+    for (int it = 0; it < 8; ++it) K = (0.0625 + 2.0 * kU32 * As + 2.0 * E1 * sqrt(As + K)) / (1.0 - 2.0 * kU32);
+    K *= 1.0 + 1.52587890625e-05;  // 1 + 2^-16 over the iterate (the iteration converges from below)
+    gc.g_cu = (float)cu_f;
+    gc.g_cv = cv_f;
+    gc.g_dl = -__double2float_ru((K + cu_f + Eu) / (1.0 - kU32));
+  } else {
+    gc.g_cu = gc.g_cv = gc.g_dl = 0.f;
+  }
+}
+
+__device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
+__device__ __forceinline__ uint32_t cluster_nctarank() {
+  uint32_t r;
+  asm volatile("mov.u32 %0, %%cluster_nctarank;" : "=r"(r));
+  return r;
+}
+__device__ __forceinline__ uint32_t cluster_ctarank() {
+  uint32_t r;
+  asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
+  return r;
+}
+__device__ __forceinline__ void cluster_sync_all() {
+  asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
+}
+__device__ __forceinline__ void cluster_arrive() { asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory"); }
+__device__ __forceinline__ void cluster_wait() { asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory"); }
+// 8 bytes of CTA `rank`'s shared memory at the address of `p` in this CTA (distributed shared memory)
+__device__ __forceinline__ double ld_dsmem_f64(const void* p, uint32_t rank) {
+  uint32_t a;
+  asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(a) : "r"(smem_u32(p)), "r"(rank));
+  double v;
+  asm volatile("ld.shared::cluster.f64 %0, [%1];" : "=d"(v) : "r"(a) : "memory");
+  return v;
+}
+
+// Slice of problem points [i0, i1) handled by CTA `rank` of the cluster: whole 128-point blocks of the padded length
+// (so that the pair-interleaved copy stays inside one CTA).
+__device__ __forceinline__ void prep_slice(int npad, uint32_t rank, uint32_t nct, int& i0, int& i1) {
+  const int blocks = npad / 128, per = (blocks + (int)nct - 1) / (int)nct;
+  i0 = min((int)rank * per, blocks) * 128;
+  i1 = min(((int)rank + 1) * per, blocks) * 128;
+}
+
+__global__ void __launch_bounds__(kPrepThreads) prep_kernel(Batch bt) {
+  const uint32_t rank = cluster_ctarank(), nct = cluster_nctarank();
+  const int b = blockIdx.x / nct;
   const int n = bt.n;
   const int nv = bt.nb ? bt.nb[b] : n;  // the problem's own points (ragged class: the rest of the slot is padding)
   const double* src = bt.src + (size_t)b * n * 3;
   const double* dst = bt.dst + (size_t)b * n * 3;
-  __shared__ double s_red[8][12];
-  __shared__ int s_bad[8];
-  __shared__ double s_c[8];
+  const int npad = npad128(n);
+  int i0, i1;
+  prep_slice(npad, rank, nct, i0, i1);
+  constexpr int kWarps = kPrepThreads / 32;
+  __shared__ double s_red[kWarps][13];
+  __shared__ double s_box[13];  // this CTA's box: min[6], max[6], non-finite flag (read by the whole cluster)
+  __shared__ GraphConsts s_gc;
+  __shared__ double s_c[8];     // cs[3], cd[3], s_hat, sig
+  // ---- this slice's bounding boxes
   double mn[6], mx[6];
   for (int k = 0; k < 6; ++k) {
     mn[k] = 1.0 / 0.0;
     mx[k] = -1.0 / 0.0;
   }
   int bad = 0;
-  for (int i = threadIdx.x; i < nv; i += blockDim.x) {
+  const int e1 = min(i1, nv);
+#pragma unroll 2
+  for (int i = i0 + threadIdx.x; i < e1; i += kPrepThreads) {
     for (int k = 0; k < 3; ++k) {
       const double a = src[3 * i + k], c = dst[3 * i + k];
       bad |= !isfinite(a) | !isfinite(c);
@@ -83,181 +321,67 @@ __global__ void __launch_bounds__(256) prep_kernel(Batch bt) {
       s_red[w][k] = mn[k];
       s_red[w][6 + k] = mx[k];
     }
-    s_bad[w] = bad;
+    s_red[w][12] = bad ? 1.0 : 0.0;
   }
   __syncthreads();
-  if (threadIdx.x == 0) {
-    int anybad = 0;
-    for (int k = 0; k < 6; ++k) {
-      double a = s_red[0][k], c = s_red[0][6 + k];
-      for (int q = 1; q < 8; ++q) {
-        a = fmin(a, s_red[q][k]);
-        c = fmax(c, s_red[q][6 + k]);
+  if (threadIdx.x < 13) {
+    const int k = threadIdx.x;
+    double v = s_red[0][k];
+    for (int q = 1; q < kWarps; ++q) v = k < 6 ? fmin(v, s_red[q][k]) : fmax(v, s_red[q][k]);
+    s_box[k] = v;
+  }
+  cluster_sync_all();
+  // ---- the problem's boxes: every CTA reduces the cluster's partial boxes (min / max: the order does not matter)
+  if (w < 3) {
+    for (int k = 0; k < 12; ++k) {
+      double v = lane < (int)nct ? ld_dsmem_f64(&s_box[k], (uint32_t)lane) : (k < 6 ? 1.0 / 0.0 : -1.0 / 0.0);
+      v = k < 6 ? warp_min(v) : warp_max(v);
+      if (k < 6)
+        mn[k] = v;
+      else
+        mx[k - 6] = v;
+    }
+    double f = lane < (int)nct ? ld_dsmem_f64(&s_box[12], (uint32_t)lane) : 0.0;
+    bad = warp_max(f) != 0.0;
+  }
+  cluster_arrive();  // this CTA's s_box may be released once every CTA has read it (the wait is at the end)
+  if (w < 3) {
+    const PrepBase q = prep_base(bt, b, mn, mx, bad);
+    if (rank == 0) {
+      if (lane == 0) {  // the three constant groups run concurrently, one warp each
+        if (w == 0) prep_interval_v7(q, s_gc);
+        if (w == 1) prep_tc(bt, q, s_gc);
+        if (w == 2) prep_gram(bt, q, s_gc);
       }
-      mn[k] = a;
-      mx[k] = c;
     }
-    for (int q = 0; q < 8; ++q) anybad |= s_bad[q];
-    double Ms = 0, Md = 0;
-    GraphConsts gc;
-    for (int k = 0; k < 3; ++k) {
-      gc.cs[k] = 0.5 * (mn[k] + mx[k]);
-      gc.cd[k] = 0.5 * (mn[3 + k] + mx[3 + k]);
-      Ms = fmax(Ms, 0.5 * (mx[k] - mn[k]));
-      Md = fmax(Md, 0.5 * (mx[3 + k] - mn[3 + k]));
-      s_c[k] = gc.cs[k];
-      s_c[3 + k] = gc.cd[k];
-    }
-    const double beta = bt.beta;
-    gc.beta = beta;
-    // Unknown scale: |d2/d1 - s| <= beta/d1  <=>  |d2 - s*d1| <= beta (d1 > 0), i.e. the fixed-scale test on a
-    // source cloud scaled by s: the float copies are pre-scaled, the exact re-check keeps the reference's
-    // division-based sequence (its rounding differs from the real-number predicate by ~1e-16 relative, far
-    // inside delta).
-    double s_hat = 1.0;
-    if (bt.scale_mode) {
-      s_hat = bt.sol[b].scale;
-      if (!(s_hat > 1e-6) || !(s_hat < 1e6)) {
-        s_hat = 1.0;
-        anybad = 1;  // degenerate estimate: exact path for every pair
-      }
-      Ms *= s_hat;
-    }
-    s_c[6] = s_hat;
-    // delta: bound on the FP32 error of |D1 - D2| (DESIGN.md: <= ~70 u32 (Ms+Md)); 256 u32 (...) used.
-    const double u32 = 5.9604644775390625e-08;  // 2^-24
-    const double delta = 256.0 * u32 * (Ms + Md + beta);
-    const double gam1 = beta - delta, gam2 = beta + delta;
-    const double up = 1.0 + 9.5367431640625e-07, dn = 1.0 - 9.5367431640625e-07;  // 1 +- 2^-20
-    int use64 = anybad || !(Ms < 1e8) || !(Md < 1e8) || !(gam2 > 1e-8) || !isfinite(beta) || (bt.flags_dbg & 1u);
-    // sure edge: x <= b1; sure non-edge: x > b2.  Exact path for everything: b1 = -1 (x >= 0), b2 = +inf.
-    gc.b1 = (use64 || !(gam1 > 0)) ? -1.0f : (float)(gam1 * dn);
-    gc.b2 = use64 ? __int_as_float(0x7f800000) : (float)(gam2 * up);
-    gc.use_fp64 = use64;
-    gc.s_hat = s_hat;
-    // ---- v7 strip kernel (graph_strip3_kernel): d_hi = t^2 - (beta^2 - K) w < 0 proves an edge, d_lo = t^2 -
-    // (beta^2 + K) w >= 0 proves a non-edge, K = dt (2 beta + dt) + 32 u beta^2 relative to w = (sqrt a + sqrt b)^2.
-    // dt bounds |g' - g|: float conversion of the centred coordinates (<= u M each), the differences, squares and sums
-    // give |sqrt a' - sqrt a| <= ~15 u M per cloud; 64 u (Ms + Md) is used, plus the bias eps of the squared norms.
-    {
-      const double d3 = 64.0 * u32 * (Ms + Md);
-      const double eps = fmax((d3 / 16.0) * (d3 / 16.0), 1e-36);
-      const double dt = 1.125 * d3;
-      const double K = dt * (2.0 * beta + dt) + 32.0 * u32 * beta * beta;
-      const double b2v = beta * beta;
-      gc.f3_eps = (float)eps;
-      if (use64) {  // exact path for every pair (the kernel also overrides the words: NaN inputs have no sign)
-        gc.f3_nlo = -__int_as_float(0x7f800000);
-        gc.f3_nhi = __int_as_float(0x7f800000);
-      } else {
-        gc.f3_nlo = (float)(-(b2v + K) * up);
-        gc.f3_nhi = (b2v - K > 0) ? (float)(-(b2v - K) * dn) : (float)((K - b2v) * up + 1e-37);
-      }
-      gc.pad2 = 0;
-    }
-    // ---- tensor-core filter constants (graph_tc.cu; derivation in DESIGN.md §3.1).  a' = |ds|^2 and b' = |dd|^2 come
-    // out of the tensor core with |a' - a| <= ea, |b' - b| <= eb (E = ea + eb).  With t = a - b, s = a + b,
-    //   f(a, b) = t^2 - 2 beta^2 s + beta^4 = (g^2 - beta^2)(w - beta^2),  g = |sqrt a - sqrt b|,  w = (sqrt a + sqrt b)^2 >= s
-    // so   edge  <=>  s <= beta^2  or  f <= 0   — a polynomial, no square root, no division:
-    //   |f(a', b') - f(a, b)| <= 2 E |t'| + E^2 + 2 beta^2 E                      (tensor-core error)
-    //   |d^ - f(a', b')|      <= 8 u (t'^2 + 2 beta^2 s' + beta^4)                 (FP32 evaluation of d^: 4 roundings + 2 constants)
-    // and for s <= beta^2 (where the sign of f says nothing)  f <= (beta^2 - s)^2 <= beta^4.  The kernel decides by the
-    // signs of d^ +- band, band = kap (t'^2 + beta^4) + c0 with 2 E |t'| <= (E/lam) t'^2 + E lam (lam = the typical |t| at the
-    // threshold, 0.75 beta D): kap = E/lam + 8 u, c0 = E lam + E^2 + 2 beta^2 E + 16 u beta^2 Smax + 8 u beta^4 + beta^4.
-    // (8 u t'^2 needs no case split: it is part of kap.)  d^ + band < 0 proves f < 0 (an edge whatever s is); d^ - band >= 0
-    // proves f > beta^4, hence s > beta^2 and a non-edge; everything else goes to the exact FP64 re-check.
-    {
-      double Ds2 = 0, Dd2 = 0;  // largest possible squared distance inside each (scaled) cloud
+    if (w == 0 && lane == 0) {
       for (int k = 0; k < 3; ++k) {
-        const double es = (mx[k] - mn[k]) * s_hat, ed = mx[3 + k] - mn[3 + k];
-        Ds2 += es * es;
-        Dd2 += ed * ed;
+        s_c[k] = q.cs[k];
+        s_c[3 + k] = q.cd[k];
       }
-      const double kappa = bt.tc_kappa > 0 ? bt.tc_kappa : kTcKappa;
-      const double ea = kappa * u32 * Ds2, eb = kappa * u32 * Dd2, E = ea + eb;
-      const double b2 = beta * beta, b4 = b2 * b2;
-      const double lam = 0.75 * beta * sqrt(0.5 * (Ds2 + Dd2));
-      const double Smax = Ds2 + Dd2 + E;
-      const double kap = E / lam + 8.0 * u32;
-      const double c0 = E * lam + E * E + 2.0 * b2 * E + 16.0 * u32 * b2 * Smax + 8.0 * u32 * b4 + b4;
-      // When is the filter worth it (correctness never depends on this)?  beta <= D/8: the beta^4 floor of the band stays
-      // below ~1e-3 of the pairs; E / (0.75 D) <= beta / 64: the band in g = |sqrt a - sqrt b| is a small fraction of the
-      // threshold (fails when the noise bound is tiny against the extent of a cloud: beta/D below ~3e-4); b4 a normal float.
-      const double Dmin = sqrt(fmin(Ds2, Dd2));
-      const bool ok = !use64 && (bt.flags_dbg & 1024u) != 0 && (bt.flags_dbg & 512u) == 0 && Ds2 > 0 && Dd2 > 0 && Ds2 < 1e8 && Dd2 < 1e8 &&
-                      b4 > 1e-30 && isfinite(E) && isfinite(kap) && 8.0 * beta <= Dmin && 64.0 * E <= 0.75 * Dmin * beta;
-      gc.use_tc = ok ? 1 : 0;
-      gc.tc_c2 = (float)(2.0 * b2);
-      gc.tc_b4 = (float)b4;
-      gc.tc_kap = (float)(kap * up);
-      gc.tc_c0 = (float)(c0 * up);
-      gc.tc_pad = 0.f;
-      if (ok && bt.rechecks) atomicAdd(bt.mismatches + 7, 1ull);  // debug counter 7: problems on the tensor-core path
-      // ---- Gram-form test of graph_strip2_kernel (derivation in DESIGN.md §3.1).  a' = fl(N_i + N_j - 2 q_i.q_j) from the
-      // float copies q (|q| <= R, R^2 <= Ds2 / 4 about the box centre) is within 8 u R^2 (conversion) + 2 u R^2 (rounded
-      // norms) + 14 u R^2 (one FADD and three FMA roundings on partial sums of at most 2 R^2 and 4 R^2) of a; 28 u R^2 is
-      // used, the rest covers second-order terms and the reference's own FP64 rounding.  With E = ea + eb, k = E / lam,
-      // C = E lam + E^2 + 2 beta^2 E and 4 u (t^2 + |m| S + |c|) the FP32 evaluation error of fma(t, t, fma(s, m, c)):
-      //   t^2 + mhi s + chi <= 0  =>  (1 + k) t^2 - 2 beta^2 s + beta^4 + C <= 0  =>  f(a, b) <= 0           (edge)
-      //   t^2 + mlo s + clo >= 0  =>  (1 - k) t^2 - 2 beta^2 s - C > 0            =>  f(a, b) > beta^4      (s > beta^2: not)
-      const double gE = 7.0 * u32 * (Ds2 + Dd2), gk = gE / lam, gS = Ds2 + Dd2 + gE;
-      const double gC = gE * lam + gE * gE + 2.0 * b2 * gE;
-      gc.g_mhi = (float)(-2.0 * b2 * (1.0 - 4.0 * u32) / (1.0 + gk) * dn);
-      gc.g_chi = (float)(((b4 + gC) / (1.0 + gk) + 8.0 * u32 * b2 * gS) * up);
-      gc.g_mlo = (float)(-2.0 * b2 * (1.0 + 4.0 * u32) / (1.0 - gk) * up);
-      gc.g_clo = (float)(-(gC + 9.0 * u32 * b2 * gS) / (1.0 - gk) * up * up);
-      // conditioning guard (same form as use_tc's): beta <= D/8 keeps pairs with s <= beta^2 rare, 64 E <= 0.75 D beta keeps
-      // the band narrow against beta (and k <= 1/64).  C1 (outliers moved 5-10 extents away, beta/D ~ 1e-4) fails it.
-      gc.use_gram = (!use64 && (bt.flags_dbg & 512u) == 0 && Ds2 > 0 && Dd2 > 0 && Ds2 < 1e8 && Dd2 < 1e8 && b4 > 1e-30 &&
-                     isfinite(gE) && 8.0 * beta <= Dmin && 64.0 * gE <= 0.75 * Dmin * beta) ? 1 : 0;
-      // ---- single-slope form of the Gram test (default; derivation in DESIGN.md §3.1).  Lengths in units of 2 beta
-      // (sig = 1 / (2 beta), so beta^2 -> 1/4):  f = (A - B + 1/4)^2 - A,  edge <= f <= 0,  non-edge <= f > 1/16.  The kernel
-      // computes u = c_u - A', v = c_v - B' (A', B' within Eu, Ev of A, B; c_v = c_u + 1/4 exactly), T = fl(v - u),
-      // dh = fma(T, T, u) and dl = fl(dh + dl_c):
-      //   dh < 0   =>  T^2 < A - c_u + Eu  =>  f <= -c_u + Eu + 5u As + 2 E1 |T| (1 + 2u) + E1^2 <= 0         (edge)
-      //   dl >= 0  =>  T^2 >= A + K, K = |dl_c| (1 - u) - c_u - Eu  =>  f >= K (1 - 2u) - 2u As - 2 E1 sqrt(As + K) > 1/16
-      // with E1 = Eu + Ev, |T| <= sqrt(As + Eu) and A <= As (the scaled source diagonal squared).  Eu = 25 u R^2 + 5 u c_u
-      // to first order (conversion 8, norms 2, the row constant 1, the FADD 2, three FMAs 12; R^2 = As / 4); 28 and 6 are
-      // used.  c_u appears on both sides with a slope far below 1, so the fixed point is reached from below by iteration.
-      if (gc.use_gram && !(bt.flags_dbg & kFlagTwoSlope)) {
-        const double sig = 0.5 / beta, As = sig * sig * Ds2, Ad = sig * sig * Dd2;
-        auto eu = [&](double c) { return u32 * (7.0 * As + 6.0 * c); };
-        auto ev = [&](double c) { return u32 * (7.0 * Ad + 6.0 * (c + 0.25)); };
-        double cu = 0.0;
-        for (int it = 0; it < 8; ++it) {
-          const double Eu = eu(cu), E1 = Eu + ev(cu);
-          cu = Eu + 5.0 * u32 * (As + Eu) + 2.0 * (1.0 + 2.0 * u32) * E1 * sqrt(As + Eu) + E1 * E1;
-        }
-        const float cv_f = __double2float_ru((double)__double2float_ru(cu * (1.0 + 1.52587890625e-05)) + 0.25);
-        const double cu_f = (double)cv_f - 0.25;  // exact: c_v - c_u = 1/4 in the kernel's floats
-        const double Eu = eu(cu_f), E1 = Eu + ev(cu_f);
-        double K = 0.0;
-        for (int it = 0; it < 8; ++it) K = (0.0625 + 2.0 * u32 * As + 2.0 * E1 * sqrt(As + K)) / (1.0 - 2.0 * u32);
-        K *= 1.0 + 1.52587890625e-05;  // 1 + 2^-16 over the iterate (the iteration converges from below)
-        gc.g_cu = (float)cu_f;
-        gc.g_cv = cv_f;
-        gc.g_dl = -__double2float_ru((K + cu_f + Eu) / (1.0 - u32));
-        s_c[7] = sig;
-      } else {
-        gc.g_cu = gc.g_cv = gc.g_dl = 0.f;
-        s_c[7] = 0.0;
-      }
-      // debug counter 15: problems graph_strip2_kernel builds with the Gram test (not those graph_tc_kernel or
-      // graph_strip3_kernel builds; launch_graph makes the same choice)
-      if (gc.use_gram && bt.rechecks && !(ok && tc_path_active(bt.flags_dbg)) && !(bt.flags_dbg & 2048u))
-        atomicAdd(bt.mismatches + 15, 1ull);
+      s_c[6] = q.s_hat;
+      s_c[7] = prep_sig(bt, q);
     }
+  }
+  __syncthreads();
+  if (rank == 0 && threadIdx.x == 0) {
+    const GraphConsts gc = s_gc;
+    // debug counter 15: problems graph_strip2_kernel builds with the Gram test (not those graph_tc_kernel or
+    // graph_strip3_kernel builds; launch_graph makes the same choice)
+    if (gc.use_gram && bt.rechecks && !(gc.use_tc && tc_path_active(bt.flags_dbg)) && !(bt.flags_dbg & 2048u))
+      atomicAdd(bt.mismatches + 15, 1ull);
     bt.gc[b] = gc;
     bt.n_edges2[b] = 0ull;
   }
-  __syncthreads();
+  // ---- this slice's float copies
   float4* sf = bt.sf + (size_t)b * n;
   float4* df = bt.df + (size_t)b * n;
   // the single-slope Gram test's operands (problems that run it): the same centred points in units of 2 beta, rounded
   // once from FP64
   float4* gq = s_c[7] > 0.0 ? bt.gq + (size_t)b * n * 2 : nullptr;
   const double ss = s_c[6] * s_c[7], sd = s_c[7];
-  for (int i = threadIdx.x; i < n; i += blockDim.x) {
+  const int e2 = min(i1, n);
+  for (int i = i0 + threadIdx.x; i < e2; i += kPrepThreads) {
     const double vs[3] = {src[3 * i + 0] - s_c[0], src[3 * i + 1] - s_c[1], src[3 * i + 2] - s_c[2]};
     const double vd[3] = {dst[3 * i + 0] - s_c[3], dst[3 * i + 1] - s_c[4], dst[3 * i + 2] - s_c[5]};
     float4 a, c;
@@ -282,9 +406,8 @@ __global__ void __launch_bounds__(256) prep_kernel(Batch bt) {
     }
   }
   // pair-interleaved copy for the packed kernel: (point o, point o+32) of every 64-column half block adjacent
-  const int npad = npad128(n);
   float* pk = bt.pk + (size_t)b * 6 * npad;
-  for (int j = threadIdx.x; j < npad; j += blockDim.x) {
+  for (int j = i0 + threadIdx.x; j < i1; j += kPrepThreads) {
     const int o = j & 127, pos = (j & ~127) + (o >> 6) * 64 + (o & 31) * 2 + ((o >> 5) & 1);
     float v[6] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
     if (j < nv) {
@@ -298,6 +421,7 @@ __global__ void __launch_bounds__(256) prep_kernel(Batch bt) {
 #pragma unroll
     for (int q = 0; q < 6; ++q) pk[(size_t)q * npad + pos] = v[q];
   }
+  cluster_wait();
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -1549,7 +1673,28 @@ __global__ void __launch_bounds__(256) degree_kernel(Batch bt) {
   }
 }
 
-void launch_prep(const Batch& bt, cudaStream_t st) { prep_kernel<<<bt.B, 256, 0, st>>>(bt); }
+// CTAs per problem of prep_kernel: about kPrepPoints points each, at most kPrepCtas
+static int prep_ctas(int n) { return std::max(1, std::min(kPrepCtas, (npad128(n) + kPrepPoints - 1) / kPrepPoints)); }
+
+// Returns the launch's own status (a cluster that cannot be placed fails here, before any kernel of the pipeline runs),
+// cleared from the runtime's last error so that it is reported once, by the caller.
+cudaError_t launch_prep(const Batch& bt, cudaStream_t st) {
+  const unsigned ctas = (unsigned)prep_ctas(bt.n);
+  cudaLaunchConfig_t cfg = {};
+  cfg.gridDim = dim3((unsigned)bt.B * ctas);
+  cfg.blockDim = dim3(kPrepThreads);
+  cfg.stream = st;
+  cudaLaunchAttribute attr;
+  attr.id = cudaLaunchAttributeClusterDimension;
+  attr.val.clusterDim.x = ctas;
+  attr.val.clusterDim.y = 1;
+  attr.val.clusterDim.z = 1;
+  cfg.attrs = &attr;
+  cfg.numAttrs = 1;
+  const cudaError_t e = cudaLaunchKernelEx(&cfg, prep_kernel, bt);
+  if (e != cudaSuccess) cudaGetLastError();
+  return e;
+}
 
 int launch_graph(const Batch& bt0, cudaStream_t st, int num_sms, int* strip_blocks) {
   Batch bt = bt0;

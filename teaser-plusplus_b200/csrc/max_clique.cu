@@ -36,6 +36,11 @@ namespace {
 
 constexpr int kHeurThreads = 512;
 constexpr int kPeelThreads = 1024;
+// Smaller CTAs of the small route's heuristic and peel kernels for batches that fill the GPU with them (launch_clique):
+// their loops walk a few hundred candidates and rows of a few hundred words between block-wide barriers, so more
+// problems resident per SM hide more of the row-read latency than more threads per problem do.
+constexpr int kHeurThreadsBig = 256;
+constexpr int kPeelThreadsBig = 256;
 constexpr int kExactThreads = 256;
 #ifndef TZR_EXACT_MIN_BLOCKS
 #define TZR_EXACT_MIN_BLOCKS 3  // CTAs per SM the exact kernel is compiled for (80 registers; 2 -> 128)
@@ -276,7 +281,8 @@ __device__ __forceinline__ void heur_body(const Batch& bt, int r, int b, uint32_
 
 }  // namespace
 
-__global__ void __launch_bounds__(kHeurThreads) clique_heur_kernel(Batch bt) {
+template <int kThreads>
+__global__ void __launch_bounds__(kThreads) clique_heur_kernel(Batch bt) {
   const int r = blockIdx.x, b = blockIdx.y;
   const int n = bt.n, W = pitch32(n);
   extern __shared__ __align__(16) unsigned char smem_raw[];
@@ -382,7 +388,8 @@ __device__ void peel_to_core(const Batch& bt, int b, uint32_t* S, uint32_t* Sn, 
 
 }  // namespace
 
-__global__ void __launch_bounds__(kPeelThreads) clique_peel_kernel(Batch bt, int mode) {
+template <int kThreads>
+__global__ void __launch_bounds__(kThreads) clique_peel_kernel(Batch bt, int mode) {
   const int b = blockIdx.x;
   const int n = bt.n, W = pitch32(n);
   extern __shared__ __align__(16) unsigned char smem_raw[];
@@ -1864,6 +1871,8 @@ __global__ void __launch_bounds__(256) core_map_back_kernel(Batch bt, Batch cb, 
 }
 
 namespace {
+int sms_dev[64] = {};  // SMs per device (clique_set_attrs)
+
 void clique_set_attrs() {
   // per device: a process may hold contexts on several GPUs
   static bool attr_done_dev[64] = {};
@@ -1871,8 +1880,11 @@ void clique_set_attrs() {
   cudaGetDevice(&dev);
   bool& attr_done = attr_done_dev[dev & 63];
   if (!attr_done) {
-    cudaFuncSetAttribute(clique_heur_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
-    cudaFuncSetAttribute(clique_peel_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
+    cudaFuncSetAttribute(clique_heur_kernel<kHeurThreads>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
+    cudaFuncSetAttribute(clique_heur_kernel<kHeurThreadsBig>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
+    cudaFuncSetAttribute(clique_peel_kernel<kPeelThreads>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
+    cudaFuncSetAttribute(clique_peel_kernel<kPeelThreadsBig>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
+    cudaDeviceGetAttribute(&sms_dev[dev & 63], cudaDevAttrMultiProcessorCount, dev);
     cudaFuncSetAttribute(clique_exact_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
     cudaFuncSetAttribute(clique_kcore_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
     attr_done = true;
@@ -1934,8 +1946,19 @@ void launch_clique(const Batch& bt, const tzr_params& p, int mode, cudaStream_t 
     b2.kcore_final = nullptr;
   }
   dim3 g1(kHeurRoots, (unsigned)bt.B);
-  clique_heur_kernel<<<g1, kHeurThreads, clique_heur_smem(n), st>>>(b2);
-  clique_peel_kernel<<<bt.B, kPeelThreads, clique_peel_smem(n), st>>>(b2, mode == 0 ? 0 : 1);
+  // small CTAs when the batch gives every SM at least four heuristic CTAs / two peel CTAs of them; the candidate list
+  // is then enumerated in one scan while a row has at most kHeurThreadsBig words
+  int dev = 0;
+  cudaGetDevice(&dev);
+  const int sms = std::max(sms_dev[dev & 63], 1);
+  if (bt.B * kHeurRoots >= 4 * sms && pitch32(n) <= kHeurThreadsBig)
+    clique_heur_kernel<kHeurThreadsBig><<<g1, kHeurThreadsBig, clique_heur_smem(n), st>>>(b2);
+  else
+    clique_heur_kernel<kHeurThreads><<<g1, kHeurThreads, clique_heur_smem(n), st>>>(b2);
+  if (bt.B >= 2 * sms)
+    clique_peel_kernel<kPeelThreadsBig><<<bt.B, kPeelThreadsBig, clique_peel_smem(n), st>>>(b2, mode == 0 ? 0 : 1);
+  else
+    clique_peel_kernel<kPeelThreads><<<bt.B, kPeelThreads, clique_peel_smem(n), st>>>(b2, mode == 0 ? 0 : 1);
   launches += 2;
   if (mode == 0) launches += launch_exact_passes(b2, st);
   if (n_launches) *n_launches += launches;
@@ -1956,7 +1979,7 @@ void launch_clique_large_front(const Batch& bt, const tzr_params& p, int mode, u
   dim3 g1(kHeurRoots, (unsigned)bt.B);
   clique_heur_large_kernel<<<g1, kHeurThreads, clique_heur_large_smem(n), st>>>(b2, lists);
   // mode 1: selects the best heuristic clique into clq / L / best_bits and stops (no peel, no search)
-  clique_peel_kernel<<<bt.B, kPeelThreads, clique_peel_smem(n), st>>>(b2, 1);
+  clique_peel_kernel<kPeelThreads><<<bt.B, kPeelThreads, clique_peel_smem(n), st>>>(b2, 1);
   launches += 2;
   if (n_launches) *n_launches += launches;
 }
@@ -1992,7 +2015,7 @@ void launch_clique_search(const Batch& cb, cudaStream_t st, int* n_launches) {
   clique_set_attrs();
   Batch b2 = cb;
   b2.kcore_final = nullptr;
-  clique_peel_kernel<<<cb.B, kPeelThreads, clique_peel_smem(cb.n), st>>>(b2, 0);
+  clique_peel_kernel<kPeelThreads><<<cb.B, kPeelThreads, clique_peel_smem(cb.n), st>>>(b2, 0);
   const int launches = 1 + launch_exact_passes(b2, st);
   if (n_launches) *n_launches += launches;
 }

@@ -20,7 +20,13 @@ namespace tzr {
 
 namespace {
 
-constexpr int kRTWarps = kRTThreads / 32;  // kRTThreads (tzr_internal.cuh): 128 regs x 128 threads, 4 CTAs/SM
+constexpr int kRTWarps = kRTThreads / 32;  // kRTThreads (tzr_internal.cuh)
+// CTAs per SM of rot_trans_kernel's build for large batches (64 registers, with spills).  Each GNC iteration is
+// latency-bound: a block reduction, then the 3x3 SVD on one thread while the block waits.  Once a batch needs more
+// than one wave of the spill-free build (150 registers: three CTAs per SM), eight resident problems per SM hide more of
+// that than the spills cost, and 1024 problems fit one wave.  Smaller batches take rot_trans_kernel<0>, built without
+// a minimum (the same 150-register code as a plain __launch_bounds__(kRTThreads)).
+constexpr int kRTMinBlocksBig = 8;
 
 // ---- 3x3 helpers: M3, svd3, normalise_scale, rotation_from_H (rot3.cuh) ------------------------------------
 
@@ -275,7 +281,8 @@ __device__ int tls_translation(const double* __restrict__ raw, int m, double bet
 // =================================================================================================
 // batch kernel: clique finalisation + chain TIMs + GNC-TLS + TLS translation
 // =================================================================================================
-__global__ void __launch_bounds__(kRTThreads) rot_trans_kernel(Batch bt, tzr_params p, int use_clique, int exact_mode) {
+template <int kMinBlocks>
+__global__ void __launch_bounds__(kRTThreads, kMinBlocks) rot_trans_kernel(Batch bt, tzr_params p, int use_clique, int exact_mode) {
   const int b = blockIdx.x;
   const int n = bt.n;
   const int tid = threadIdx.x;
@@ -456,16 +463,23 @@ __global__ void __launch_bounds__(kRTThreads) rot_trans_kernel(Batch bt, tzr_par
 
 void launch_rot_trans(const Batch& bt, const tzr_params& p, int use_clique, cudaStream_t st) {
   static bool attr_done_dev[64] = {};  // per device: a process may hold contexts on several GPUs
+  static int sms_dev[64] = {};
   int dev = 0;
   cudaGetDevice(&dev);
   if (!attr_done_dev[dev & 63]) {
-    cudaFuncSetAttribute(rot_trans_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 64 * 1024);
+    cudaFuncSetAttribute(rot_trans_kernel<0>, cudaFuncAttributeMaxDynamicSharedMemorySize, 64 * 1024);
+    cudaFuncSetAttribute(rot_trans_kernel<kRTMinBlocksBig>, cudaFuncAttributeMaxDynamicSharedMemorySize, 64 * 1024);
+    cudaDeviceGetAttribute(&sms_dev[dev & 63], cudaDevAttrMultiProcessorCount, dev);
     attr_done_dev[dev & 63] = true;
   }
   int mode = p.inlier_selection_mode;
   if (!p.use_max_clique) mode = 3;
   if (!p.max_clique_exact_solution) mode = 1;
-  rot_trans_kernel<<<bt.B, kRTThreads, (size_t)pitch32(bt.n) * 4 + 16, st>>>(bt, p, use_clique, mode == 0 ? 1 : 0);
+  const size_t smem = (size_t)pitch32(bt.n) * 4 + 16;
+  if (bt.B > 3 * sms_dev[dev & 63])
+    rot_trans_kernel<kRTMinBlocksBig><<<bt.B, kRTThreads, smem, st>>>(bt, p, use_clique, mode == 0 ? 1 : 0);
+  else
+    rot_trans_kernel<0><<<bt.B, kRTThreads, smem, st>>>(bt, p, use_clique, mode == 0 ? 1 : 0);
 }
 
 // =================================================================================================

@@ -153,7 +153,7 @@ struct Batch {
 };
 
 // ---- rotation TIM sets (shared by rot_trans_kernel and the certifier's gather of a retained solve) ----------------------
-constexpr int kRTThreads = 128;  // threads of the CTAs that walk a TIM set (rot_trans.cu: 128 regs x 128 threads, 4 CTAs/SM)
+constexpr int kRTThreads = 128;  // threads of the CTAs that walk a TIM set (rot_trans.cu: 3 CTAs/SM, or 8 for large batches)
 
 // CHAIN (registration.cc:657-680): m TIMs materialised in ps/pd (pd already de-scaled, :697).
 // COMPLETE (registration.cc:681-694): all m(m-1)/2 differences of the clique points, in computeTIMs order
@@ -273,7 +273,7 @@ __device__ void ldlt_solve(const double* __restrict__ Aup, const double* __restr
 }
 
 // kernels (defined in the .cu files) -------------------------------------------------------------
-void launch_prep(const Batch& bt, cudaStream_t st);
+cudaError_t launch_prep(const Batch& bt, cudaStream_t st);
 // returns the number of kernels launched; strip_blocks (may be NULL): graph_strip2_kernel's strip length, 0 if it did not run
 int launch_graph(const Batch& bt, cudaStream_t st, int num_sms, int* strip_blocks = nullptr);
 // graph_strip2_kernel's strip order on the host: the (I, J0) of strips 0 ... strips_below(nt, L) - 1 (either may be
