@@ -1396,6 +1396,41 @@ int tzr_pose_graph_optimize_line_process(tzr_ctx* ctx, const tzr_line_process_pa
                                          double* confidence, uint8_t* kept, double* residuals,
                                          tzr_line_process_summary* summary);
 
+/* Many independent graphs in one call, one set of params (DESIGN.md §3.23).  Per graph g the contract is
+ * tzr_pose_graph_optimize_line_process's, with these differences:
+ *   - Arguments: G >= 1 graphs; K[g], E[g]; edges[g] (E x 2 int32), edge_transforms[g] (E), information[g] (E x 36);
+ *     uncertain and initial_poses may be NULL or hold NULL entries, each with the single entry's meaning.  Outputs:
+ *     poses[g] (K); confidence, kept and residuals may be NULL or hold NULL entries; summaries (G entries) may be NULL;
+ *     status (G entries) is required.
+ *   - Refusals: a NULL ctx, parameters the single entry refuses, G < 1 or a NULL K, E, edges, edge_transforms,
+ *     information, poses or status is TZR_ERR_INVALID_ARG before any device work, with nothing written.  Otherwise the
+ *     call returns TZR_OK, and status[g] is what tzr_pose_graph_optimize_line_process returns on graph g alone (K < 2,
+ *     E < 1, K > 1024, a non-rigid or non-finite edge or start pose, an endpoint out of range, a disconnected graph,
+ *     reference_node not a node of g, ...).  A graph that is refused gets zeroed outputs (poses, confidence, kept,
+ *     residuals, summary); the other graphs are solved.  TZR_ERR_ALLOC or TZR_ERR_CUDA when the batched route's
+ *     workspace does not fit or a launch fails (tzr_last_error names the size or the failure); tzr_last_error otherwise
+ *     holds the last refusal's message.
+ *   - Routes: a graph with K <= 128 runs on the batched route: one CTA per graph runs each pass's whole
+ *     Levenberg-Marquardt loop (every outer iteration and trial) with its own dense Cholesky of the 6 K x 6 K system,
+ *     so no cuSOLVER call.  It has exactly the single entry's decisions (iterations, trials, stop reasons, pruned, the
+ *     kept set, both mu bit for bit); its poses, confidences, F and residuals may differ from the single entry's in the
+ *     last bits, because the factorisation is not cuSOLVER's.  A graph with 128 < K <= 1024 runs through
+ *     tzr_pose_graph_optimize_line_process after the batched route, one graph at a time, and its result is that
+ *     entry's bit for bit.
+ *   - Independence: each graph's outputs are bit-identical whatever the batch around it (its position, the other
+ *     graphs, G), and two calls are bit-identical: every reduction runs in one fixed shape within the graph's CTA.
+ *   - Launches and synchronisations on the batched route: exactly 2 kernel launches (one per pass) and 2 host
+ *     synchronisations (one read-back of every graph's pass-1 state and confidences, from which the host plans pass 2,
+ *     and one at the end), whatever G, K, E or the trials run; the K > 128 graphs add the single entry's counts.
+ *   - Workspace: ctx's pose-graph workspace (so a retained solve stays retained), the batched graphs back to back:
+ *     H and its factor as two (6 K)^2 doubles per graph (9.4 MB at K = 128) plus the edge tables and terms. */
+int tzr_pose_graph_optimize_line_process_batch(
+    tzr_ctx* ctx, const tzr_line_process_params* params, int G, const int32_t* K, const int32_t* E,
+    const int32_t* const* edges, const tzr_similarity* const* edge_transforms, const double* const* information,
+    const int32_t* const* uncertain, const tzr_similarity* const* initial_poses, tzr_similarity* const* poses,
+    double* const* confidence, uint8_t* const* kept, double* const* residuals, tzr_line_process_summary* summaries,
+    int32_t* status);
+
 /* tzr_register_cloud_pairs_multiway_colored's arguments with tzr_line_process_params in place of the GNC-TLS ones:
  * colors NULL refines by point-to-plane ICP (tzr_register_cloud_pairs_icp_point_to_plane; a non-NULL kernel is then
  * TZR_ERR_INVALID_ARG), otherwise by coloured ICP; then the information matrices as in tzr_register_cloud_pairs_multiway,

@@ -182,5 +182,16 @@ except capi.TzrError as e:
 sols, cl = capi.solve_batch_multi([p["src"] for p in prs[:5]], [p["dst"] for p in prs[:5]],
                                   capi.default_params(**dict(kw, noise_bound=prs[0]["noise_bound"])))
 print("multi", int(sols["valid"].sum()), "/ 5")
+# the batched line process: two fragment-shaped graphs on the batched route (the Cholesky's shared-memory tiles) and
+# one refused graph
+sys.path.insert(0, os.path.join(ROOT, "tests"))
+from line_process_fragments import fragment  # noqa: E402
+lpg = []
+for seed, K in ((1, 40), (2, 75)):
+    gt_, e_, T_, L_, u_ = fragment(seed, K, n_wrong=1)
+    lpg.append(dict(K=K, edges=e_, transforms=T_, information=L_, uncertain=u_))
+lpg.append(dict(lpg[0], K=41))
+lpr = ctx.global_optimization_batch(lpg, 0.05)
+print("line process batch", [r["status"] for r in lpr], [r["trials"] for r in lpr])
 ctx.close()
 print("DONE")

@@ -262,6 +262,7 @@ _SYMBOLS = [
     "tzr_fgr_params_default", "tzr_fgr", "tzr_fgr_batch", "tzr_register_cloud_pairs_fgr",
     "tzr_ransac_params_default", "tzr_ransac", "tzr_ransac_batch", "tzr_register_cloud_pairs_ransac",
     "tzr_line_process_params_default", "tzr_pose_graph_optimize_line_process",
+    "tzr_pose_graph_optimize_line_process_batch",
     "tzr_register_cloud_pairs_multiway_line_process",
 ]
 
@@ -467,6 +468,10 @@ def lib():
     L.tzr_line_process_params_default.restype = None
     L.tzr_pose_graph_optimize_line_process.argtypes = [vp, C.POINTER(LineProcessParams)] + \
         L.tzr_pose_graph_optimize.argtypes[2:-1] + [C.POINTER(LineProcessSummary)]
+    L.tzr_pose_graph_optimize_line_process_batch.argtypes = [
+        vp, C.POINTER(LineProcessParams), C.c_int, i32p, i32p, C.POINTER(i32p), C.POINTER(C.POINTER(Similarity)),
+        C.POINTER(dp), C.POINTER(i32p), C.POINTER(C.POINTER(Similarity)), C.POINTER(C.POINTER(Similarity)),
+        C.POINTER(dp), C.POINTER(u8p), C.POINTER(dp), C.POINTER(LineProcessSummary), i32p]
     L.tzr_register_cloud_pairs_multiway_line_process.argtypes = L.tzr_register_cloud_pairs_icp_colored.argtypes + [
         i32p, C.POINTER(LineProcessParams), dp, i32p, dp, u8p, C.POINTER(Similarity), C.POINTER(LineProcessSummary),
         i32p]
@@ -1711,6 +1716,64 @@ class Context:
             _p(r, C.c_double), C.byref(summ)))
         return dict(poses=_poses(poses), confidence=l[:E], kept=m[:E].astype(bool), residuals=r[:E],
                     **_line_process_summary(summ))
+
+    def global_optimization_batch(self, graphs, max_correspondence_distance, **params):
+        """tzr_pose_graph_optimize_line_process_batch: many graphs, one LineProcessParams (params: any of its fields).
+        graphs: dicts with K, edges, transforms, information and optionally uncertain and initial_poses (None or absent:
+        the single entry's default).  Returns one dict per graph as global_optimization returns, plus status (the single
+        entry's return on that graph; a refused graph's outputs are zero).  Raises only on call-level refusals."""
+        lp = line_process_params(max_correspondence_distance, **params)
+        G = len(graphs)
+        keep = []  # the arrays the pointers refer to
+
+        def ptr(a, t):
+            keep.append(a)
+            return C.cast(a.ctypes.data, C.POINTER(t))
+
+        Ks, Es = np.zeros(max(1, G), dtype=np.int32), np.zeros(max(1, G), dtype=np.int32)
+        P = max(1, G)
+        i32p = C.POINTER(C.c_int32)
+        ed_p, tr_p, info_p = (i32p * P)(), (C.POINTER(Similarity) * P)(), (C.POINTER(C.c_double) * P)()
+        unc_p, init_p, pose_p = (i32p * P)(), (C.POINTER(Similarity) * P)(), (C.POINTER(Similarity) * P)()
+        l_p, m_p, r_p = (C.POINTER(C.c_double) * P)(), (C.POINTER(C.c_uint8) * P)(), (C.POINTER(C.c_double) * P)()
+        outs = []
+        for g, gr in enumerate(graphs):
+            K = int(gr["K"])
+            ed = np.ascontiguousarray(gr["edges"], dtype=np.int32).reshape(-1, 2)
+            E = ed.shape[0]
+            info = np.ascontiguousarray(gr["information"], dtype=np.float64).reshape(E, 36)
+            if len(gr["transforms"]) != E:
+                raise TzrError("global_optimization_batch: one transform per edge is required")
+            tr = (Similarity * max(1, E))(*[similarity(x) for x in gr["transforms"]])
+            keep.append(tr)
+            Ks[g], Es[g] = K, E
+            ed_p[g], info_p[g] = ptr(ed, C.c_int32), ptr(info, C.c_double)
+            tr_p[g] = C.cast(tr, C.POINTER(Similarity))
+            if gr.get("uncertain") is not None:
+                unc = np.ascontiguousarray(gr["uncertain"], dtype=np.int32)
+                if unc.shape != (E,):
+                    raise TzrError("global_optimization_batch: uncertain needs one entry per edge")
+                unc_p[g] = ptr(unc, C.c_int32)
+            if gr.get("initial_poses") is not None:
+                init = (Similarity * max(1, K))(*[similarity(x) for x in gr["initial_poses"]])
+                keep.append(init)
+                init_p[g] = C.cast(init, C.POINTER(Similarity))
+            poses = (Similarity * max(1, K))()
+            l, m, r = np.zeros(max(1, E)), np.zeros(max(1, E), dtype=np.uint8), np.zeros(max(1, E))
+            keep.append(poses)
+            pose_p[g] = C.cast(poses, C.POINTER(Similarity))
+            l_p[g], m_p[g], r_p[g] = ptr(l, C.c_double), ptr(m, C.c_uint8), ptr(r, C.c_double)
+            outs.append((K, E, poses, l, m, r))
+        summ = (LineProcessSummary * P)()
+        status = np.zeros(P, dtype=np.int32)
+        self._ck(lib().tzr_pose_graph_optimize_line_process_batch(
+            self._h, C.byref(lp), G, _p(Ks, C.c_int32), _p(Es, C.c_int32), ed_p, tr_p, info_p, unc_p, init_p, pose_p,
+            l_p, m_p, r_p, summ, _p(status, C.c_int32)))
+        res = []
+        for g, (K, E, poses, l, m, r) in enumerate(outs):
+            res.append(dict(poses=_poses(poses)[:K], confidence=l[:E], kept=m[:E].astype(bool), residuals=r[:E],
+                            status=int(status[g]), **_line_process_summary(summ[g])))
+        return res
 
     def icp(self, src, dst, max_correspondence_distance, init=None, max_iteration=30, relative_fitness=1e-6,
             relative_rmse=1e-6):

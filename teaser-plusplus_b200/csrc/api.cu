@@ -2475,10 +2475,18 @@ static double lp_mu(const tzr_line_process_params* p, const double* info, const 
   return p->preference_loop_closure * (c * c) * (a / (double)idx.size());
 }
 
-static int line_process_run(tzr_ctx* ctx, const tzr_line_process_params* prm, int K, int E, const int32_t* ends,
-                            const tzr_similarity* T, const double* info, const int32_t* uncertain,
-                            const tzr_similarity* init, tzr_similarity* poses, double* confidence, uint8_t* kept,
-                            double* residuals, tzr_line_process_summary* summary) {
+// One graph's checks, start and pass-1 plan, in the single entry's order of refusals (include/teaser_b200.h)
+struct LpGraphPrep {
+  std::vector<char> live;
+  std::vector<double> pose;  // K x 12 starting poses
+  std::vector<PgEdge> ed;
+  std::vector<PgBlock> blocks;
+  std::vector<PgTerm> terms;
+  LpPlan plan;
+};
+static int lp_prepare(tzr_ctx* ctx, const tzr_line_process_params* prm, int K, int E, const int32_t* ends,
+                      const tzr_similarity* T, const double* info, const int32_t* uncertain,
+                      const tzr_similarity* init, const tzr_similarity* poses, LpGraphPrep* g) {
   if (!ctx || !lp_params_ok(prm) || K < 2 || E < 1 || !ends || !T || !info || !poses) {
     if (ctx) ctx->last_error = "line process: invalid arguments (K >= 2, E >= 1 and the parameters' ranges)";
     return TZR_ERR_INVALID_ARG;
@@ -2492,23 +2500,18 @@ static int line_process_run(tzr_ctx* ctx, const tzr_line_process_params* prm, in
     ctx->last_error = "line process: reference_node " + std::to_string(ref) + " is neither -1 nor a node";
     return TZR_ERR_INVALID_ARG;
   }
-  std::vector<char> live;
   double info_sum = 0.0;
-  std::vector<double> pose;
-  int rc = pg_start(ctx, K, E, ends, T, info, uncertain, init, ref < 0 ? 0 : ref, &live, &info_sum, &pose);
+  int rc = pg_start(ctx, K, E, ends, T, info, uncertain, init, ref < 0 ? 0 : ref, &g->live, &info_sum, &g->pose);
   if (rc != TZR_OK) return rc;
-  const double c = prm->max_correspondence_distance;
-  std::vector<PgEdge> ed;
-  std::vector<PgBlock> blocks;
-  std::vector<PgTerm> terms;
-  pg_edge_table(E, ends, T, info, uncertain, live, -1, c, &ed, &blocks, &terms);
+  pg_edge_table(E, ends, T, info, uncertain, g->live, -1, prm->max_correspondence_distance, &g->ed, &g->blocks,
+                &g->terms);
   std::vector<int> all(E);
   for (int e = 0; e < E; ++e) all[e] = e;
-  LpPlan plan;
+  LpPlan& plan = g->plan;
   plan.K = K;
   plan.E = E;
   plan.n = 6 * K;
-  plan.blocks = (int)blocks.size();
+  plan.blocks = (int)g->blocks.size();
   plan.mu = lp_mu(prm, info, all);
   plan.min_rel_inc = prm->min_relative_increment;
   plan.min_rel_res_inc = prm->min_relative_residual_increment;
@@ -2518,6 +2521,76 @@ static int line_process_run(tzr_ctx* ctx, const tzr_line_process_params* prm, in
   plan.lower = prm->lower_scale_factor;
   plan.max_iteration = prm->max_iteration;
   plan.max_lm = prm->max_iteration_lm;
+  return TZR_OK;
+}
+
+// Between the passes: the kept edges (every certain edge, and the uncertain ones with l1 > edge_prune_threshold) in
+// index order, their edge table and block plan, their pass-1 confidences l2 and pass 2's mu
+static void lp_second_pass(const tzr_line_process_params* prm, int E, const int32_t* ends, const tzr_similarity* T,
+                           const double* info, const LpGraphPrep& g, const std::vector<double>& l1,
+                           std::vector<int>* keep_out, std::vector<PgEdge>* ed2, std::vector<PgBlock>* blocks,
+                           std::vector<PgTerm>* terms, std::vector<double>* l2, double* mu2) {
+  std::vector<int>& keep = *keep_out;
+  keep.clear();
+  for (int e = 0; e < E; ++e)
+    if (!g.ed[e].uncertain || l1[e] > prm->edge_prune_threshold) keep.push_back(e);
+  const int E2 = (int)keep.size();
+  std::vector<int32_t> ends2((size_t)std::max(E2, 1) * 2), unc2(std::max(E2, 1));
+  std::vector<tzr_similarity> T2(std::max(E2, 1));
+  std::vector<double> info2((size_t)std::max(E2, 1) * 36);
+  l2->assign(std::max(E2, 1), 0.0);
+  std::vector<char> live2(E2);
+  for (int j = 0; j < E2; ++j) {
+    const int e = keep[j];
+    ends2[2 * j] = ends[2 * e];
+    ends2[2 * j + 1] = ends[2 * e + 1];
+    unc2[j] = g.ed[e].uncertain;
+    T2[j] = T[e];
+    memcpy(&info2[36 * (size_t)j], info + 36 * (size_t)e, 36 * 8);
+    live2[j] = g.live[e];
+    (*l2)[j] = l1[e];
+  }
+  pg_edge_table(E2, ends2.data(), T2.data(), info2.data(), unc2.data(), live2, -1, prm->max_correspondence_distance,
+                ed2, blocks, terms);
+  *mu2 = lp_mu(prm, info, keep);
+}
+
+// One graph's outputs: the final poses (K x 12), the confidences (pass 2's l2out[j] for kept edge keep[j], pass 1's l1
+// for a pruned one), the kept mask and the residuals res[e * res_stride]
+static void lp_write_outputs(int K, int E, const std::vector<int>& keep, const std::vector<double>& l1,
+                             const double* l2out, const double* pose, const double* res, size_t res_stride,
+                             tzr_similarity* poses, double* confidence, uint8_t* kept, double* residuals) {
+  const int E2 = (int)keep.size();
+  std::vector<double> lf = l1;
+  for (int j = 0; j < E2; ++j) lf[keep[j]] = l2out[j];
+  std::vector<uint8_t> km((size_t)E, 0);
+  for (int j = 0; j < E2; ++j) km[keep[j]] = 1;
+  for (int k = 0; k < K; ++k) {
+    memset(&poses[k], 0, sizeof(tzr_similarity));
+    poses[k].scale = 1.0;
+    memcpy(poses[k].rotation, &pose[12 * (size_t)k], 72);
+    memcpy(poses[k].translation, &pose[12 * (size_t)k + 9], 24);
+  }
+  for (int e = 0; e < E; ++e) {
+    if (confidence) confidence[e] = lf[e];
+    if (kept) kept[e] = km[e];
+    if (residuals) residuals[e] = res[(size_t)e * res_stride];
+  }
+}
+
+static int line_process_run(tzr_ctx* ctx, const tzr_line_process_params* prm, int K, int E, const int32_t* ends,
+                            const tzr_similarity* T, const double* info, const int32_t* uncertain,
+                            const tzr_similarity* init, tzr_similarity* poses, double* confidence, uint8_t* kept,
+                            double* residuals, tzr_line_process_summary* summary) {
+  LpGraphPrep g;
+  int rc = lp_prepare(ctx, prm, K, E, ends, T, info, uncertain, init, poses, &g);
+  if (rc != TZR_OK) return rc;
+  const int ref = prm->reference_node;
+  std::vector<double>& pose = g.pose;
+  std::vector<PgEdge>& ed = g.ed;
+  std::vector<PgBlock>& blocks = g.blocks;
+  std::vector<PgTerm>& terms = g.terms;
+  const LpPlan& plan = g.plan;
   const size_t n = (size_t)plan.n;
   // workspace: [edges of pass 1 | edges of pass 2 | blocks | terms | poses (2 buffers) | confidences | state] (pass 1's
   // staged in one copy; pass 2's edges, blocks, terms and confidences overwrite theirs between the passes), then the
@@ -2588,31 +2661,17 @@ static int line_process_run(tzr_ctx* ctx, const tzr_line_process_params* prm, in
   CK(cudaMemcpyAsync(l1.data(), dv.conf, (size_t)E * 8, cudaMemcpyDeviceToHost, st));
   CK(cudaStreamSynchronize(st));
   std::vector<int> keep;
-  for (int e = 0; e < E; ++e)
-    if (!ed[e].uncertain || l1[e] > prm->edge_prune_threshold) keep.push_back(e);
+  std::vector<PgEdge> ed2;
+  std::vector<double> l2;
+  double mu2 = 0.0;
+  lp_second_pass(prm, E, ends, T, info, g, l1, &keep, &ed2, &blocks, &terms, &l2, &mu2);
   const int E2 = (int)keep.size();
   sm.pruned = E - E2;
   {
-    std::vector<int32_t> ends2((size_t)std::max(E2, 1) * 2), unc2(std::max(E2, 1));
-    std::vector<tzr_similarity> T2(std::max(E2, 1));
-    std::vector<double> info2((size_t)std::max(E2, 1) * 36), l2(std::max(E2, 1));
-    std::vector<char> live2(E2);
-    for (int j = 0; j < E2; ++j) {
-      const int e = keep[j];
-      ends2[2 * j] = ends[2 * e];
-      ends2[2 * j + 1] = ends[2 * e + 1];
-      unc2[j] = ed[e].uncertain;
-      T2[j] = T[e];
-      memcpy(&info2[36 * (size_t)j], info + 36 * (size_t)e, 36 * 8);
-      live2[j] = live[e];
-      l2[j] = l1[e];
-    }
-    std::vector<PgEdge> ed2;
-    pg_edge_table(E2, ends2.data(), T2.data(), info2.data(), unc2.data(), live2, -1, c, &ed2, &blocks, &terms);
     LpPlan plan2 = plan;
     plan2.E = E2;
     plan2.blocks = (int)blocks.size();
-    plan2.mu = lp_mu(prm, info, keep);
+    plan2.mu = mu2;
     sm.mu[1] = plan2.mu;
     if (E2 > 0) {
       CK(cudaMemcpyAsync(d + o_ed2, ed2.data(), (size_t)E2 * sizeof(PgEdge), cudaMemcpyHostToDevice, st));
@@ -2641,23 +2700,223 @@ static int line_process_run(tzr_ctx* ctx, const tzr_line_process_params* prm, in
     CK(cudaMemcpyAsync(terms_out.data(), dv.eterm + (size_t)buf * E * kPgTermStride, (size_t)E * kPgTermStride * 8,
                        cudaMemcpyDeviceToHost, st));
     CK(cudaStreamSynchronize(st));
-    std::vector<double> lf = l1;
-    for (int j = 0; j < E2; ++j) lf[keep[j]] = l2out[j];
-    std::vector<uint8_t> km((size_t)E, 0);
-    for (int j = 0; j < E2; ++j) km[keep[j]] = 1;
-    for (int k = 0; k < K; ++k) {
-      memset(&poses[k], 0, sizeof(tzr_similarity));
-      poses[k].scale = 1.0;
-      memcpy(poses[k].rotation, &pose[12 * (size_t)k], 72);
-      memcpy(poses[k].translation, &pose[12 * (size_t)k + 9], 24);
-    }
-    for (int e = 0; e < E; ++e) {
-      if (confidence) confidence[e] = lf[e];
-      if (kept) kept[e] = km[e];
-      if (residuals) residuals[e] = terms_out[(size_t)e * kPgTermStride + 42];
-    }
+    lp_write_outputs(K, E, keep, l1, l2out.data(), pose.data(), terms_out.data() + 42, kPgTermStride, poses, confidence,
+                     kept, residuals);
   }
   if (summary) *summary = sm;
+  return TZR_OK;
+}
+
+// ---- many graphs in one call (tzr_pose_graph_optimize_line_process_batch, DESIGN.md §3.23) ---------------------------
+// The largest K of the batched route: kLpBatchMaxK, or TZR_LP_BATCH_MAX_K for measurements of the crossover, capped at
+// the largest K whose lp_batch_kernel fits the device's shared memory.
+static int lp_batch_max_k(tzr_ctx* ctx) {
+  int optin = 0;
+  cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, ctx->device);
+  int cap = 1024;
+  while (cap > 2 && line_process_batch_smem(6 * cap) > (size_t)optin) --cap;
+  const char* e = std::getenv("TZR_LP_BATCH_MAX_K");
+  const int k = e ? std::atoi(e) : 0;
+  return std::min(k >= 1 ? k : kLpBatchMaxK, cap);
+}
+
+static void lp_zero_outputs(int K, int E, tzr_similarity* poses, double* confidence, uint8_t* kept, double* residuals,
+                            tzr_line_process_summary* summary) {
+  if (poses && K > 0) memset(poses, 0, (size_t)K * sizeof(tzr_similarity));
+  if (E > 0) {
+    if (confidence) memset(confidence, 0, (size_t)E * 8);
+    if (kept) memset(kept, 0, (size_t)E);
+    if (residuals) memset(residuals, 0, (size_t)E * 8);
+  }
+  if (summary) memset(summary, 0, sizeof(*summary));
+}
+
+static int line_process_batch_run(tzr_ctx* ctx, const tzr_line_process_params* prm, int G, const int32_t* K,
+                                  const int32_t* E, const int32_t* const* edges, const tzr_similarity* const* T,
+                                  const double* const* info, const int32_t* const* uncertain,
+                                  const tzr_similarity* const* init, tzr_similarity* const* poses,
+                                  double* const* confidence, uint8_t* const* kept, double* const* residuals,
+                                  tzr_line_process_summary* summaries, int32_t* status) {
+  auto opt = [](auto arr, int g) { return arr ? arr[g] : nullptr; };
+  const int kmax = lp_batch_max_k(ctx);
+  // validate, start and plan every graph of the batched route; the others run through the single entry afterwards
+  std::vector<int> small, large;
+  std::vector<LpGraphPrep> prep(G);
+  for (int g = 0; g < G; ++g) {
+    status[g] = TZR_OK;
+    if (K[g] > kmax) {
+      large.push_back(g);
+      continue;
+    }
+    const int rc = lp_prepare(ctx, prm, K[g], E[g], edges[g], T[g], info[g], opt(uncertain, g), opt(init, g),
+                              poses[g], &prep[g]);
+    if (rc != TZR_OK) {
+      status[g] = rc;
+      lp_zero_outputs(K[g], E[g], poses[g], opt(confidence, g), opt(kept, g), opt(residuals, g),
+                      summaries ? summaries + g : nullptr);
+      continue;
+    }
+    small.push_back(g);
+  }
+  const std::string refusal = ctx->last_error;
+  if (!small.empty()) {
+    // workspace, graphs back to back: [descriptors | per graph: this pass's edges, blocks, terms, confidences (staged
+    // per pass) | per graph: pass 1's edges, starting poses (staged with pass 1)] then the outputs [per graph: state,
+    // confidences, poses, residuals] (read back after each pass) and the working buffers [per graph: poses, edge terms,
+    // H, A, b]
+    const int S = (int)small.size();
+    struct Off { size_t ed, blk, trm, l, ed1, init, st, out, pose, term, H, A, b; };
+    std::vector<Off> off(S);
+    int n_max = 0;
+    size_t o = al256((size_t)S * sizeof(LpBatchGraph));
+    for (int j = 0; j < S; ++j) {
+      const LpGraphPrep& g = prep[small[j]];
+      const size_t e = (size_t)g.plan.E;
+      off[j].ed = o;
+      off[j].blk = off[j].ed + al256(e * sizeof(PgEdge));
+      off[j].trm = off[j].blk + al256(g.blocks.size() * sizeof(PgBlock));
+      off[j].l = off[j].trm + al256(g.terms.size() * sizeof(PgTerm));
+      o = off[j].l + al256(e * 8);
+    }
+    const size_t in2_end = o;
+    for (int j = 0; j < S; ++j) {
+      const LpGraphPrep& g = prep[small[j]];
+      off[j].ed1 = o;
+      off[j].init = off[j].ed1 + al256((size_t)g.plan.E * sizeof(PgEdge));
+      o = off[j].init + al256((size_t)g.plan.K * 12 * 8);
+    }
+    const size_t in_end = o, out_lo = o;
+    for (int j = 0; j < S; ++j) {
+      const LpGraphPrep& g = prep[small[j]];
+      off[j].st = o;
+      off[j].out = off[j].st + al256(sizeof(LpState));
+      o = off[j].out + al256(((size_t)2 * g.plan.E + (size_t)12 * g.plan.K) * 8);
+    }
+    const size_t out_hi = o;
+    for (int j = 0; j < S; ++j) {
+      const LpGraphPrep& g = prep[small[j]];
+      const size_t n = (size_t)g.plan.n;
+      n_max = std::max(n_max, g.plan.n);
+      off[j].pose = o;
+      off[j].term = off[j].pose + al256((size_t)g.plan.K * 24 * 8);
+      off[j].H = off[j].term + al256((size_t)g.plan.E * 2 * kPgTermStride * 8);
+      off[j].A = off[j].H + al256(n * n * 8);
+      off[j].b = off[j].A + al256(n * n * 8);
+      o = off[j].b + al256(n * 8);
+    }
+    cudaSetDevice(ctx->device);
+    cudaStream_t st = ctx->stream;
+    int rc;
+    if ((rc = ensure(ctx, ctx->pg, o)) != TZR_OK) return rc;
+    char* d = (char*)ctx->pg.p;
+    std::vector<LpBatchGraph> desc(S);
+    for (int j = 0; j < S; ++j) {
+      const LpGraphPrep& g = prep[small[j]];
+      const Off& f = off[j];
+      LpBatchGraph& x = desc[j];
+      x.dv = LpDev{(const PgEdge*)(d + f.ed), (const PgBlock*)(d + f.blk), (const PgTerm*)(d + f.trm),
+                   (double*)(d + f.pose), (double*)(d + f.term), (double*)(d + f.l), (double*)(d + f.H),
+                   (double*)(d + f.A), (double*)(d + f.b), nullptr, (LpState*)(d + f.st)};
+      x.plan = g.plan;
+      x.edges1 = (const PgEdge*)(d + f.ed1);
+      x.init = (const double*)(d + f.init);
+      x.out = (double*)(d + f.out);
+      x.E1 = g.plan.E;
+      x.ref = prm->reference_node;
+      memcpy(x.T0, g.pose.data() + 12 * (size_t)(x.ref < 0 ? 0 : x.ref), 12 * 8);
+    }
+    // pass 1: everything staged in one copy
+    std::vector<char> h(in_end, 0);
+    memcpy(h.data(), desc.data(), (size_t)S * sizeof(LpBatchGraph));
+    for (int j = 0; j < S; ++j) {
+      const LpGraphPrep& g = prep[small[j]];
+      const Off& f = off[j];
+      const size_t e = (size_t)g.plan.E;
+      memcpy(h.data() + f.ed, g.ed.data(), e * sizeof(PgEdge));
+      memcpy(h.data() + f.blk, g.blocks.data(), g.blocks.size() * sizeof(PgBlock));
+      memcpy(h.data() + f.trm, g.terms.data(), g.terms.size() * sizeof(PgTerm));
+      for (size_t q = 0; q < e; ++q) ((double*)(h.data() + f.l))[q] = 1.0;
+      memcpy(h.data() + f.ed1, g.ed.data(), e * sizeof(PgEdge));
+      memcpy(h.data() + f.init, g.pose.data(), (size_t)g.plan.K * 12 * 8);
+    }
+    const LpBatchGraph* gd = (const LpBatchGraph*)d;
+    CK(cudaMemcpyAsync(d, h.data(), in_end, cudaMemcpyHostToDevice, st));
+    ctx->launches += launch_line_process_batch(gd, S, n_max, 0, st);
+    if ((rc = check_launch(ctx, "line process batch launch")) != TZR_OK) return rc;
+    std::vector<char> out(out_hi - out_lo);
+    CK(cudaMemcpyAsync(out.data(), d + out_lo, out.size(), cudaMemcpyDeviceToHost, st));
+    CK(cudaStreamSynchronize(st));
+    // between the passes: every graph's pruned edge list and pass-2 plan, staged in one copy
+    std::vector<tzr_line_process_summary> sm(S);
+    std::vector<std::vector<double>> l1(S);
+    std::vector<std::vector<int>> keep(S);
+    std::fill(h.begin(), h.begin() + in2_end, 0);
+    for (int j = 0; j < S; ++j) {
+      const int gi = small[j];
+      const LpGraphPrep& g = prep[gi];
+      const Off& f = off[j];
+      const int Eg = g.plan.E;
+      LpState s1;
+      memcpy(&s1, out.data() + (f.st - out_lo), sizeof(s1));
+      sm[j] = tzr_line_process_summary{};
+      sm[j].mu[0] = g.plan.mu;
+      sm[j].iterations[0] = s1.iter;
+      sm[j].trials[0] = s1.trials;
+      sm[j].stop_reason[0] = s1.reason;
+      const double* lo = (const double*)(out.data() + (f.out - out_lo));
+      l1[j].assign(lo, lo + Eg);
+      std::vector<PgEdge> ed2;
+      std::vector<PgBlock> blocks;
+      std::vector<PgTerm> terms;
+      std::vector<double> l2;
+      double mu2 = 0.0;
+      lp_second_pass(prm, Eg, edges[gi], T[gi], info[gi], g, l1[j], &keep[j], &ed2, &blocks, &terms, &l2, &mu2);
+      const int E2 = (int)keep[j].size();
+      sm[j].pruned = Eg - E2;
+      sm[j].mu[1] = mu2;
+      desc[j].plan.E = E2;
+      desc[j].plan.blocks = (int)blocks.size();
+      desc[j].plan.mu = mu2;
+      memcpy(h.data() + f.ed, ed2.data(), (size_t)E2 * sizeof(PgEdge));
+      memcpy(h.data() + f.blk, blocks.data(), blocks.size() * sizeof(PgBlock));
+      memcpy(h.data() + f.trm, terms.data(), terms.size() * sizeof(PgTerm));
+      memcpy(h.data() + f.l, l2.data(), (size_t)E2 * 8);
+    }
+    memcpy(h.data(), desc.data(), (size_t)S * sizeof(LpBatchGraph));
+    CK(cudaMemcpyAsync(d, h.data(), in2_end, cudaMemcpyHostToDevice, st));
+    ctx->launches += launch_line_process_batch(gd, S, n_max, 1, st);
+    if ((rc = check_launch(ctx, "line process batch launch")) != TZR_OK) return rc;
+    CK(cudaMemcpyAsync(out.data(), d + out_lo, out.size(), cudaMemcpyDeviceToHost, st));
+    CK(cudaStreamSynchronize(st));
+    for (int j = 0; j < S; ++j) {
+      const int gi = small[j];
+      const Off& f = off[j];
+      const int Kg = K[gi], Eg = E[gi];
+      LpState s2;
+      memcpy(&s2, out.data() + (f.st - out_lo), sizeof(s2));
+      sm[j].iterations[1] = s2.iter;
+      sm[j].trials[1] = s2.trials;
+      sm[j].stop_reason[1] = s2.reason;
+      sm[j].residual = s2.F;
+      const double* lo = (const double*)(out.data() + (f.out - out_lo));
+      lp_write_outputs(Kg, Eg, keep[j], l1[j], lo, lo + Eg, lo + Eg + 12 * (size_t)Kg, 1, poses[gi],
+                       opt(confidence, gi), opt(kept, gi), opt(residuals, gi));
+      if (summaries) summaries[gi] = sm[j];
+    }
+  }
+  // the graphs above the batched route's size, one by one through the single entry
+  std::string last = refusal;
+  for (int g : large) {
+    status[g] = line_process_run(ctx, prm, K[g], E[g], edges[g], T[g], info[g], opt(uncertain, g), opt(init, g),
+                                 poses[g], opt(confidence, g), opt(kept, g), opt(residuals, g),
+                                 summaries ? summaries + g : nullptr);
+    if (status[g] != TZR_OK) {
+      last = ctx->last_error;
+      lp_zero_outputs(K[g], E[g], poses[g], opt(confidence, g), opt(kept, g), opt(residuals, g),
+                      summaries ? summaries + g : nullptr);
+    }
+  }
+  ctx->last_error = last;
   return TZR_OK;
 }
 
@@ -4198,6 +4457,21 @@ int tzr_pose_graph_optimize_line_process(tzr_ctx* ctx, const tzr_line_process_pa
                                          tzr_line_process_summary* summary) {
   return line_process_run(ctx, params, K, E, edges, edge_transforms, information, uncertain, initial_poses, poses,
                           confidence, kept, residuals, summary);
+}
+
+int tzr_pose_graph_optimize_line_process_batch(
+    tzr_ctx* ctx, const tzr_line_process_params* params, int G, const int32_t* K, const int32_t* E,
+    const int32_t* const* edges, const tzr_similarity* const* edge_transforms, const double* const* information,
+    const int32_t* const* uncertain, const tzr_similarity* const* initial_poses, tzr_similarity* const* poses,
+    double* const* confidence, uint8_t* const* kept, double* const* residuals, tzr_line_process_summary* summaries,
+    int32_t* status) {
+  if (!ctx) return TZR_ERR_INVALID_ARG;
+  if (!lp_params_ok(params) || G < 1 || !K || !E || !edges || !edge_transforms || !information || !poses || !status) {
+    ctx->last_error = "line process batch: invalid arguments (the parameters' ranges, G >= 1 and the required arrays)";
+    return TZR_ERR_INVALID_ARG;
+  }
+  return line_process_batch_run(ctx, params, G, K, E, edges, edge_transforms, information, uncertain, initial_poses,
+                                poses, confidence, kept, residuals, summaries, status);
 }
 
 int tzr_register_cloud_pairs_multiway_line_process(

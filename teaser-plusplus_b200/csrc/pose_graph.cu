@@ -496,17 +496,8 @@ __device__ __forceinline__ void lp_lin(const double* N, const double* t, double*
   z[5] = t[2];
 }
 
-// which = 0: the current poses into the current terms; 1: the candidate poses (the other buffer), skipped once the pass
-// has stopped or the trial formed no candidate; 2: the other buffer, always (the compensated poses)
-__global__ void lp_edge_kernel(LpDev dv, int K, int E, int which) {
-  const int e = blockIdx.x * blockDim.x + threadIdx.x;
-  if (e >= E) return;
-  const LpState& st = *dv.state;
-  if (which == 1 && (st.done || st.skip)) return;
-  const int buf = which == 0 ? st.cur : 1 - st.cur;
-  const PgEdge& ed = dv.edges[e];
-  const double* Ts = lp_pose(dv, K, buf, ed.s);
-  const double* Td = lp_pose(dv, K, buf, ed.d);
+// One edge's terms at poses Ts, Td into out (kPgTermStride doubles; lp_edge_kernel and the batched pass share it)
+__device__ __forceinline__ void lp_edge_terms(const PgEdge& ed, const double* Ts, const double* Td, double* out) {
   // P = X^-1 T_d^-1: R_P = (R_d R_X)^T, t_P = -R_X^T (R_d^T t_d + t_X); M = P T_s
   double RdX[9], RP[9], u[3], tP[3], RM[9], tM[3];
   m33(Td, ed.R, RdX);
@@ -572,7 +563,6 @@ __global__ void lp_edge_kernel(LpDev dv, int K, int E, int which) {
       for (int q = 0; q < 6; ++q) a = a + ed.L[6 * r + q] * J[q][k];
       LJ[r][k] = a;
     }
-  double* out = lp_terms(dv, E, buf, e);
 #pragma unroll
   for (int r = 0; r < 6; ++r) {
 #pragma unroll
@@ -588,6 +578,18 @@ __global__ void lp_edge_kernel(LpDev dv, int K, int E, int which) {
     out[36 + r] = a;
   }
   out[42] = c;
+}
+
+// which = 0: the current poses into the current terms; 1: the candidate poses (the other buffer), skipped once the pass
+// has stopped or the trial formed no candidate; 2: the other buffer, always (the compensated poses)
+__global__ void lp_edge_kernel(LpDev dv, int K, int E, int which) {
+  const int e = blockIdx.x * blockDim.x + threadIdx.x;
+  if (e >= E) return;
+  const LpState& st = *dv.state;
+  if (which == 1 && (st.done || st.skip)) return;
+  const int buf = which == 0 ? st.cur : 1 - st.cur;
+  const PgEdge& ed = dv.edges[e];
+  lp_edge_terms(ed, lp_pose(dv, K, buf, ed.s), lp_pose(dv, K, buf, ed.d), lp_terms(dv, E, buf, e));
 }
 
 // The start of a pass: F with the incoming confidences, then their update; H and b follow
@@ -608,6 +610,17 @@ __global__ void lp_begin_kernel(LpDev dv, LpPlan p) {
 // One warp per listed block: H block (bi, bj), bi >= bj: sum of sign * (l_e A_e(r, k)) in the listed order (column-major
 // n x n, lower blocks only); b block bi (bj = -1): -(sum of sign * (l_e v_e(r))).  Only after the start or an accepted
 // trial.
+// Entry j of a block: sum of sign * (l_e term_e[j]) over its terms in the listed order, as lp_assemble_kernel sums it
+// (that kernel keeps its own loop, whose machine code this helper would move)
+__device__ __forceinline__ double lp_block_entry(const LpDev& dv, int E, int cur, const PgBlock& bl, int j) {
+  double a = 0.0;
+  for (int q = bl.lo; q < bl.hi; ++q) {
+    const PgTerm tm = dv.terms[q];
+    a = a + (double)tm.sign * (dv.conf[tm.e] * lp_terms(dv, E, cur, tm.e)[j]);
+  }
+  return a;
+}
+
 __global__ void lp_assemble_kernel(LpDev dv, int E, int n, int nblocks) {
   const int bk = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
   const int lane = threadIdx.x & 31;
@@ -651,6 +664,27 @@ __device__ double lp_euler_sq(const double* T) {
     z = 0.0;
   }
   return ((((x * x + y * y) + z * z) + T[9] * T[9]) + T[10] * T[10]) + T[11] * T[11];
+}
+
+// The rules of lp_stats_kernel once max(b) = bm, max diag(H) = hm (mode 0) and |x|^2 = xs are known, for the batched
+// pass (lp_stats_kernel keeps its own copy, whose machine code calling this helper would move)
+__device__ __forceinline__ void lp_stats_rule(LpState& st, const LpPlan& p, int mode, double bm, double hm, double xs) {
+  st.xnorm = sqrt(xs);
+  if (mode == 0) st.lambda = 1e-5 * hm;
+  if (bm < p.min_right_term) {
+    st.done = 1;
+    st.reason = TZR_LP_STOP_RIGHT_TERM;
+  }
+  if (mode == 0) return;
+  st.lm = 0;
+  if (!st.done && st.F < p.min_residual) {
+    st.done = 1;
+    st.reason = TZR_LP_STOP_MIN_RESIDUAL;
+  }
+  if (!st.done && st.iter >= p.max_iteration) {
+    st.done = 1;
+    st.reason = TZR_LP_STOP_MAX_ITERATION;
+  }
 }
 
 // mode 0: the start of a pass (lambda = 1e-5 max diag H, nu = 2); mode 1: after an accepted trial, the end of the outer
@@ -701,6 +735,19 @@ __global__ void lp_damp_kernel(LpDev dv, int n) {
   dv.A[o] = i == j ? dv.H[o] + st.lambda : dv.H[o];
 }
 
+// The trial's outcome before any candidate from |delta|^2 = s2 and pd = delta . (lambda delta + b)
+__device__ __forceinline__ void lp_step_rule(LpState& st, const LpPlan& p, double s2, double pd) {
+  const double dn = sqrt(s2);
+  st.dnorm = dn;
+  st.pred = pd;
+  if (st.info[0] != 0 || st.info[1] != 0 || !isfinite(s2) || !isfinite(pd))
+    st.skip = 2;
+  else if (dn < p.min_rel_inc * (st.xnorm + p.min_rel_inc))
+    st.skip = 1;
+  else
+    st.skip = 0;
+}
+
 // |delta|, delta . (lambda delta + b) and the trial's outcome before any candidate: skip 2 when the factorisation failed
 // or delta is not finite, 1 when |delta| < min_relative_increment (|x| + min_relative_increment)
 __global__ void lp_step_kernel(LpDev dv, LpPlan p) {
@@ -717,26 +764,11 @@ __global__ void lp_step_kernel(LpDev dv, LpPlan p) {
   s2 = lp_block_sum(s2, sh);
   pd = lp_block_sum(pd, sh);
   if (threadIdx.x != 0) return;
-  const double dn = sqrt(s2);
-  st.dnorm = dn;
-  st.pred = pd;
-  if (st.info[0] != 0 || st.info[1] != 0 || !isfinite(s2) || !isfinite(pd))
-    st.skip = 2;
-  else if (dn < p.min_rel_inc * (st.xnorm + p.min_rel_inc))
-    st.skip = 1;
-  else
-    st.skip = 0;
+  lp_step_rule(st, p, s2, pd);
 }
 
-// One thread per node: the candidate V(delta_k) T_k, V(d) = [R_z(d_2) R_y(d_1) R_x(d_0) | (d_3, d_4, d_5)]
-__global__ void lp_update_kernel(LpDev dv, int K) {
-  const int k = blockIdx.x * blockDim.x + threadIdx.x;
-  if (k >= K) return;
-  const LpState& st = *dv.state;
-  if (st.done || st.skip) return;
-  const double* T = lp_pose(dv, K, st.cur, k);
-  double* Tn = lp_pose(dv, K, 1 - st.cur, k);
-  const double* d = dv.delta + 6 * (size_t)k;
+// The candidate Tn = V(d) T, V(d) = [R_z(d_2) R_y(d_1) R_x(d_0) | (d_3, d_4, d_5)]
+__device__ __forceinline__ void lp_candidate(const double* T, const double* d, double* Tn) {
   const double cx = cos(d[0]), sx = sin(d[0]), cy = cos(d[1]), sy = sin(d[1]), cz = cos(d[2]), sz = sin(d[2]);
   const double Rz[9] = {cz, sz, 0.0, -sz, cz, 0.0, 0.0, 0.0, 1.0};
   const double Ry[9] = {cy, 0.0, -sy, 0.0, 1.0, 0.0, sy, 0.0, cy};
@@ -750,7 +782,53 @@ __global__ void lp_update_kernel(LpDev dv, int K) {
   for (int r = 0; r < 3; ++r) Tn[9 + r] = u[r] + d[3 + r];
 }
 
-// The trial's decision (include/teaser_b200.h states the rules in order)
+// One thread per node: the candidate V(delta_k) T_k
+__global__ void lp_update_kernel(LpDev dv, int K) {
+  const int k = blockIdx.x * blockDim.x + threadIdx.x;
+  if (k >= K) return;
+  const LpState& st = *dv.state;
+  if (st.done || st.skip) return;
+  lp_candidate(lp_pose(dv, K, st.cur, k), dv.delta + 6 * (size_t)k, lp_pose(dv, K, 1 - st.cur, k));
+}
+
+// The trial's decision from F' = Fc (include/teaser_b200.h states the rules in order); returns 1 when the candidate
+// is accepted
+__device__ __forceinline__ int lp_decide_rule(LpState& st, const LpPlan& p, int skip, double Fc) {
+  if (st.lm == 0) st.iter += 1;
+  st.lm += 1;
+  st.trials += 1;
+  st.Fc = Fc;
+  int a = 0;
+  if (skip == 1) {
+    st.done = 1;
+    st.reason = TZR_LP_STOP_REL_INCREMENT;
+  } else {
+    const double dF = st.F - Fc;
+    const double rho = skip ? -1.0 : dF / (st.pred + 1e-3);
+    if (rho > 0.0 && dF < p.min_rel_res_inc * st.F) {
+      st.done = 1;
+      st.reason = TZR_LP_STOP_REL_RESIDUAL;
+    } else if (rho > 0.0) {
+      const double q = 2.0 * rho - 1.0;
+      st.lambda = st.lambda * fmax(p.lower, fmin(p.upper, 1.0 - (q * q) * q));
+      st.nu = 2.0;
+      st.F = Fc;
+      st.cur = 1 - st.cur;
+      a = 1;
+    } else {
+      st.lambda = st.lambda * st.nu;
+      st.nu = 2.0 * st.nu;
+    }
+  }
+  if (!st.done && st.lm >= p.max_lm) {
+    st.done = 1;
+    st.reason = TZR_LP_STOP_LM_TRIALS;
+  }
+  st.accepted = a;
+  return a;
+}
+
+// The trial's decision
 __global__ void lp_decide_kernel(LpDev dv, LpPlan p) {
   __shared__ double sh[kLpSmall];
   __shared__ int acc;
@@ -758,62 +836,326 @@ __global__ void lp_decide_kernel(LpDev dv, LpPlan p) {
   if (st.done) return;
   const int skip = st.skip;
   const double Fc = skip ? 0.0 : lp_residual(dv, p.E, 1 - st.cur, p.mu, sh);
-  if (threadIdx.x == 0) {
-    if (st.lm == 0) st.iter += 1;
-    st.lm += 1;
-    st.trials += 1;
-    st.Fc = Fc;
-    int a = 0;
-    if (skip == 1) {
-      st.done = 1;
-      st.reason = TZR_LP_STOP_REL_INCREMENT;
-    } else {
-      const double dF = st.F - Fc;
-      const double rho = skip ? -1.0 : dF / (st.pred + 1e-3);
-      if (rho > 0.0 && dF < p.min_rel_res_inc * st.F) {
-        st.done = 1;
-        st.reason = TZR_LP_STOP_REL_RESIDUAL;
-      } else if (rho > 0.0) {
-        const double q = 2.0 * rho - 1.0;
-        st.lambda = st.lambda * fmax(p.lower, fmin(p.upper, 1.0 - (q * q) * q));
-        st.nu = 2.0;
-        st.F = Fc;
-        st.cur = 1 - st.cur;
-        a = 1;
-      } else {
-        st.lambda = st.lambda * st.nu;
-        st.nu = 2.0 * st.nu;
-      }
-    }
-    if (!st.done && st.lm >= p.max_lm) {
-      st.done = 1;
-      st.reason = TZR_LP_STOP_LM_TRIALS;
-    }
-    st.accepted = a;
-    acc = a;
-  }
+  if (threadIdx.x == 0) acc = lp_decide_rule(st, p, skip, Fc);
   __syncthreads();
   if (acc) lp_confidences(dv, p.E, st.cur, p.mu);
 }
 
-// The compensation T_k <- C T_k with C = T0 (T_ref)^-1 into the other buffer (each thread forms C in the same order)
-__global__ void lp_compensate_kernel(LpDev dv, int K, int ref, Pose12 T0) {
-  const int k = blockIdx.x * blockDim.x + threadIdx.x;
-  if (k >= K) return;
-  const LpState& st = *dv.state;
-  const double* Tr = lp_pose(dv, K, st.cur, ref);
+// Tn = C T with C = T0 (T_ref)^-1 (each caller forms C in the same order)
+__device__ __forceinline__ void lp_compensate_pose(const double* T0, const double* Tr, const double* T, double* Tn) {
   // C: R_C = R0 R_ref^T, t_C = t0 - R_C t_ref
   double RC[9], tC[3], u[3];
-  m33_nt(T0.v, Tr, RC);
+  m33_nt(T0, Tr, RC);
   mv3(RC, Tr + 9, u);
 #pragma unroll
-  for (int r = 0; r < 3; ++r) tC[r] = T0.v[9 + r] - u[r];
-  const double* T = lp_pose(dv, K, st.cur, k);
-  double* Tn = lp_pose(dv, K, 1 - st.cur, k);
+  for (int r = 0; r < 3; ++r) tC[r] = T0[9 + r] - u[r];
   m33(RC, T, Tn);
   mv3(RC, T + 9, u);
 #pragma unroll
   for (int r = 0; r < 3; ++r) Tn[9 + r] = u[r] + tC[r];
+}
+
+// The compensation T_k <- C T_k with C = T0 (T_ref)^-1 into the other buffer
+__global__ void lp_compensate_kernel(LpDev dv, int K, int ref, Pose12 T0) {
+  const int k = blockIdx.x * blockDim.x + threadIdx.x;
+  if (k >= K) return;
+  const LpState& st = *dv.state;
+  lp_compensate_pose(T0.v, lp_pose(dv, K, st.cur, ref), lp_pose(dv, K, st.cur, k), lp_pose(dv, K, 1 - st.cur, k));
+}
+
+// ---- many graphs in one call (tzr_pose_graph_optimize_line_process_batch, DESIGN.md §3.23) ----------------------------
+// lp_batch_kernel: one CTA of kLbThreads per graph runs a whole pass of the line process: the edge terms, F and the
+// confidence update, H and b over the host's block plan, the start's statistics, then every trial (H + lambda I, a dense
+// Cholesky of the 6 K rows, the two substitutions, |delta| and delta . (lambda delta + b), the candidate and its edge
+// terms, the decision, and after an accepted trial the rebuilt H and b) until the pass stops, with the pass's state in
+// shared memory.  The rules are the single entry's helpers above (lp_edge_terms, lp_candidate, lp_step_rule,
+// lp_decide_rule, lp_stats_rule, lp_block_entry, lp_residual, lp_confidences, lp_compensate_pose).  Every reduction is
+// a fixed-shape block reduction over kLbThreads, so a graph's result depends on nothing but the graph.
+constexpr int kLbThreads = 256;  // threads per graph
+constexpr int kLbNb = 32;        // Cholesky panel width
+constexpr int kLbDt = 33;        // row stride of the diagonal tile in shared memory
+
+// Dense Cholesky A = L L^T of the lower triangle of the column-major n x n A, in place, right-looking in panels of 32
+// columns: the diagonal tile is factored in shared memory (Dt), the rows below it are solved against it one thread per
+// row and kept in shared memory (Ps: column k of the panel at Ps + k ldp), then the trailing lower triangle is updated
+// in 64 x 64 tiles, 4 x 4 entries per thread, by FP64 FMAs in ascending k.  The strict upper triangle is neither read
+// nor written.  Returns 0, or 1 + the first column whose pivot is not > 0 (NaN included); every thread returns the same.
+__device__ int lb_cholesky(double* A, int n, double* Ps, int ldp, double* Dt) {
+  const int t = threadIdx.x;
+  for (int j0 = 0; j0 < n; j0 += kLbNb) {
+    const int nb = min(kLbNb, n - j0), p = j0 + nb, m = n - p;
+    for (int w = t; w < nb * nb; w += kLbThreads) {
+      const int r = w % nb, c = w / nb;
+      if (r >= c) Dt[r * kLbDt + c] = A[(size_t)(j0 + r) + (size_t)(j0 + c) * n];
+    }
+    __syncthreads();
+    for (int k = 0; k < nb; ++k) {
+      const double piv = Dt[k * kLbDt + k];
+      if (!(piv > 0.0)) return j0 + k + 1;
+      const double lkk = sqrt(piv);
+      if (t > k && t < nb) Dt[t * kLbDt + k] = Dt[t * kLbDt + k] / lkk;
+      __syncthreads();
+      if (t == 0) Dt[k * kLbDt + k] = lkk;
+      const int q = nb - 1 - k;
+      for (int w = t; w < q * q; w += kLbThreads) {
+        const int r = k + 1 + w % q, c = k + 1 + w / q;
+        if (r >= c) Dt[r * kLbDt + c] = Dt[r * kLbDt + c] - Dt[r * kLbDt + k] * Dt[c * kLbDt + k];
+      }
+      __syncthreads();
+    }
+    for (int w = t; w < nb * nb; w += kLbThreads) {
+      const int r = w % nb, c = w / nb;
+      if (r >= c) A[(size_t)(j0 + r) + (size_t)(j0 + c) * n] = Dt[r * kLbDt + c];
+    }
+    if (m == 0) break;  // the last panel; any panel with rows below it is 32 wide
+    // L21 = A21 L11^-T: row i solves x L11^T = a by forward substitution
+    for (int i = p + t; i < n; i += kLbThreads) {
+      double x[kLbNb];
+#pragma unroll
+      for (int k = 0; k < kLbNb; ++k) {
+        double s = A[(size_t)i + (size_t)(j0 + k) * n];
+#pragma unroll
+        for (int q = 0; q < k; ++q) s = fma(-x[q], Dt[k * kLbDt + q], s);
+        x[k] = s / Dt[k * kLbDt + k];
+        A[(size_t)i + (size_t)(j0 + k) * n] = x[k];
+        Ps[k * ldp + (i - p)] = x[k];
+      }
+    }
+    __syncthreads();
+    // A22 -= L21 L21^T on the lower 64 x 64 tiles; thread (tr, tc) owns rows tr + 16 a and columns tc + 16 c of a tile
+    const int T = (m + 63) / 64, tr = t & 15, tc = t >> 4;
+    for (int ti = 0; ti < T; ++ti)
+      for (int tj = 0; tj <= ti; ++tj) {
+        int ri[4], cj[4];
+#pragma unroll
+        for (int a = 0; a < 4; ++a) {
+          ri[a] = 64 * ti + tr + 16 * a;
+          cj[a] = 64 * tj + tc + 16 * a;
+        }
+        double acc[4][4];
+#pragma unroll
+        for (int a = 0; a < 4; ++a)
+#pragma unroll
+          for (int c = 0; c < 4; ++c) acc[a][c] = 0.0;
+#pragma unroll 4
+        for (int k = 0; k < kLbNb; ++k) {
+          const double* col = Ps + k * ldp;
+          double u[4], v[4];
+#pragma unroll
+          for (int a = 0; a < 4; ++a) {
+            u[a] = col[min(ri[a], m - 1)];
+            v[a] = col[min(cj[a], m - 1)];
+          }
+#pragma unroll
+          for (int a = 0; a < 4; ++a)
+#pragma unroll
+            for (int c = 0; c < 4; ++c) acc[a][c] = fma(u[a], v[c], acc[a][c]);
+        }
+#pragma unroll
+        for (int a = 0; a < 4; ++a)
+#pragma unroll
+          for (int c = 0; c < 4; ++c)
+            if (ri[a] < m && ri[a] >= cj[c]) {
+              double* e = A + (size_t)(p + ri[a]) + (size_t)(p + cj[c]) * n;
+              *e = *e - acc[a][c];
+            }
+      }
+    __syncthreads();
+  }
+  return 0;
+}
+
+// x <- (L L^T)^-1 x with the factor of lb_cholesky (x in shared memory).  Each 32-row block's triangle is solved by
+// warp 0 (one row per lane, the solved entry broadcast by a shuffle); the forward sweep then updates the rows below one
+// thread per row, and the backward sweep first forms each block's sum over the rows below it, one warp per column, the
+// lanes' partial sums added by a butterfly.
+__device__ void lb_solve(const double* A, int n, double* x, double* tmp) {
+  const int t = threadIdx.x, lane = t & 31, warp = t >> 5;
+  for (int j0 = 0; j0 < n; j0 += kLbNb) {
+    const int nb = min(kLbNb, n - j0);
+    if (warp == 0) {
+      double v = lane < nb ? x[j0 + lane] : 0.0;
+      for (int k = 0; k < nb; ++k) {
+        if (lane == k) v = v / A[(size_t)(j0 + k) * (n + 1)];
+        const double yk = __shfl_sync(0xffffffffu, v, k);
+        if (lane > k && lane < nb) v = v - A[(size_t)(j0 + lane) + (size_t)(j0 + k) * n] * yk;
+      }
+      if (lane < nb) x[j0 + lane] = v;
+    }
+    __syncthreads();
+    for (int i = j0 + nb + t; i < n; i += kLbThreads) {
+      double s = x[i];
+      for (int k = 0; k < nb; ++k) s = s - A[(size_t)i + (size_t)(j0 + k) * n] * x[j0 + k];
+      x[i] = s;
+    }
+    __syncthreads();
+  }
+  for (int j0 = ((n - 1) / kLbNb) * kLbNb; j0 >= 0; j0 -= kLbNb) {
+    const int nb = min(kLbNb, n - j0), p = j0 + nb;
+    for (int c = warp; c < nb; c += kLbThreads / 32) {
+      double s = 0.0;
+      for (int i = p + lane; i < n; i += 32) s = s + A[(size_t)i + (size_t)(j0 + c) * n] * x[i];
+      for (int o = 16; o; o >>= 1) s = s + __shfl_xor_sync(0xffffffffu, s, o);
+      if (lane == 0) tmp[c] = s;
+    }
+    __syncthreads();
+    if (warp == 0) {
+      double v = lane < nb ? x[j0 + lane] - tmp[lane] : 0.0;
+      for (int k = nb - 1; k >= 0; --k) {
+        if (lane == k) v = v / A[(size_t)(j0 + k) * (n + 1)];
+        const double xk = __shfl_sync(0xffffffffu, v, k);
+        if (lane < k) v = v - A[(size_t)(j0 + k) + (size_t)(j0 + lane) * n] * xk;
+      }
+      if (lane < nb) x[j0 + lane] = v;
+    }
+    __syncthreads();
+  }
+}
+
+// H (listed lower blocks) and b from the terms in buffer cur, one thread per block entry
+__device__ void lb_assemble(const LpDev& dv, const LpPlan& p, int cur) {
+  for (int w = threadIdx.x; w < p.blocks * 36; w += kLbThreads) {
+    const PgBlock bl = dv.blocks[w / 36];
+    const int j = w % 36;
+    if (bl.bj < 0) {
+      if (j < 6) dv.b[6 * bl.bi + j] = -lp_block_entry(dv, p.E, cur, bl, 36 + j);
+    } else {
+      dv.H[(size_t)(6 * bl.bi + j / 6) + (size_t)(6 * bl.bj + j % 6) * (size_t)p.n] = lp_block_entry(dv, p.E, cur, bl, j);
+    }
+  }
+  __syncthreads();
+}
+
+// max(b), max diag(H) (mode 0) and |x| of the current poses, then lp_stats_rule
+__device__ void lb_stats(const LpDev& dv, const LpPlan& p, int mode, LpState& st, double* red) {
+  double bm = -INFINITY, hm = -INFINITY;
+  for (int i = threadIdx.x; i < p.n; i += kLbThreads) {
+    bm = fmax(bm, dv.b[i]);
+    if (mode == 0) hm = fmax(hm, dv.H[(size_t)i * p.n + i]);
+  }
+  bm = lp_block_max(bm, red);
+  if (mode == 0) hm = lp_block_max(hm, red);
+  double xs = 0.0;
+  for (int k = threadIdx.x; k < p.K; k += kLbThreads) xs = xs + lp_euler_sq(lp_pose(dv, p.K, st.cur, k));
+  xs = lp_block_sum(xs, red);
+  if (threadIdx.x == 0) lp_stats_rule(st, p, mode, bm, hm, xs);
+  __syncthreads();
+}
+
+// the terms of every edge at the poses in buffer buf
+__device__ void lb_edges(const LpDev& dv, int K, int E, int buf) {
+  for (int e = threadIdx.x; e < E; e += kLbThreads) {
+    const PgEdge& ed = dv.edges[e];
+    lp_edge_terms(ed, lp_pose(dv, K, buf, ed.s), lp_pose(dv, K, buf, ed.d), lp_terms(dv, E, buf, e));
+  }
+  __syncthreads();
+}
+
+// One pass of graph blockIdx.x.  pass 0 starts from the graph's starting poses; pass 1 continues from the poses pass 0
+// left (its state's cur), then compensates and evaluates every edge of pass 1's table at the returned poses.  Both
+// write the state and the confidences to the graph's output slice, pass 1 also the poses and the residuals.
+__global__ void __launch_bounds__(kLbThreads) lp_batch_kernel(const LpBatchGraph* graphs, int pass, int ldp) {
+  extern __shared__ double smem[];
+  double* Ps = smem;                   // kLbNb x ldp: the Cholesky panel
+  double* Dt = Ps + kLbNb * ldp;       // kLbNb x kLbDt: its diagonal tile
+  double* x = Dt + kLbNb * kLbDt;      // ldp: b, then delta
+  double* red = x + ldp;               // kLbThreads: block reductions
+  double* tmp = red + kLbThreads;      // kLbNb: the backward sweep's sums
+  __shared__ LpState st;
+  const LpBatchGraph& g = graphs[blockIdx.x];
+  const LpDev dv = g.dv;
+  const LpPlan p = g.plan;
+  const int K = p.K, E = p.E, n = p.n, t = threadIdx.x;
+  if (pass == 0)
+    for (int w = t; w < 12 * K; w += kLbThreads) dv.poses[w] = g.init[w];
+  if (t == 0) st.cur = pass == 0 ? 0 : dv.state->cur;
+  for (size_t w = t; w < (size_t)n * n; w += kLbThreads) dv.H[w] = 0.0;
+  for (int i = t; i < n; i += kLbThreads) dv.b[i] = 0.0;
+  __syncthreads();
+  // the start (lp_begin_kernel, lp_assemble_kernel, lp_stats_kernel mode 0)
+  lb_edges(dv, K, E, st.cur);
+  const double F = lp_residual(dv, E, st.cur, p.mu, red);
+  lp_confidences(dv, E, st.cur, p.mu);
+  if (t == 0) {
+    st.F = F;
+    st.Fc = 0.0;
+    st.nu = 2.0;
+    st.done = st.reason = st.skip = 0;
+    st.accepted = 1;
+    st.iter = st.lm = st.trials = 0;
+    st.info[0] = st.info[1] = 0;
+  }
+  __syncthreads();
+  lb_assemble(dv, p, st.cur);
+  lb_stats(dv, p, 0, st, red);
+  while (!st.done) {
+    // H + lambda I and b (lp_damp_kernel), the factorisation and the solve
+    const double lam = st.lambda;
+    for (int j = 0; j < n; ++j)
+      for (int i = j + t; i < n; i += kLbThreads) {
+        const size_t o = (size_t)i + (size_t)j * n;
+        dv.A[o] = i == j ? dv.H[o] + lam : dv.H[o];
+      }
+    for (int i = t; i < n; i += kLbThreads) x[i] = dv.b[i];
+    __syncthreads();
+    const int bad = lb_cholesky(dv.A, n, Ps, ldp, Dt);
+    __syncthreads();
+    if (!bad) lb_solve(dv.A, n, x, tmp);
+    // lp_step_kernel
+    double s2 = 0.0, pd = 0.0;
+    for (int i = t; i < n; i += kLbThreads) {
+      const double d = x[i];
+      s2 = s2 + d * d;
+      pd = pd + d * (lam * d + dv.b[i]);
+    }
+    s2 = lp_block_sum(s2, red);
+    pd = lp_block_sum(pd, red);
+    if (t == 0) {
+      st.info[0] = bad;
+      lp_step_rule(st, p, s2, pd);
+    }
+    __syncthreads();
+    // the candidate and its terms (lp_update_kernel, lp_edge_kernel), then lp_decide_kernel
+    const int skip = st.skip, cur = st.cur;
+    double Fc = 0.0;
+    if (!skip) {
+      for (int k = t; k < K; k += kLbThreads) lp_candidate(lp_pose(dv, K, cur, k), x + 6 * k, lp_pose(dv, K, 1 - cur, k));
+      __syncthreads();
+      lb_edges(dv, K, E, 1 - cur);
+      Fc = lp_residual(dv, E, 1 - cur, p.mu, red);
+    }
+    if (t == 0) lp_decide_rule(st, p, skip, Fc);
+    __syncthreads();
+    if (st.accepted) {
+      lp_confidences(dv, E, st.cur, p.mu);
+      __syncthreads();
+      if (!st.done) {
+        lb_assemble(dv, p, st.cur);
+        lb_stats(dv, p, 1, st, red);
+      }
+    }
+  }
+  for (int e = t; e < E; e += kLbThreads) g.out[e] = dv.conf[e];
+  if (pass == 1) {
+    // lp_compensate_kernel, then every edge of pass 1's table at the returned poses (lp_edge_kernel's last launch)
+    int buf = st.cur;
+    if (g.ref >= 0) {
+      for (int k = t; k < K; k += kLbThreads)
+        lp_compensate_pose(g.T0, lp_pose(dv, K, buf, g.ref), lp_pose(dv, K, buf, k), lp_pose(dv, K, 1 - buf, k));
+      buf = 1 - buf;
+      __syncthreads();
+    }
+    double* out_pose = g.out + g.E1;
+    double* out_res = out_pose + 12 * K;
+    for (int w = t; w < 12 * K; w += kLbThreads) out_pose[w] = dv.poses[(size_t)buf * 12 * K + w];
+    for (int e = t; e < g.E1; e += kLbThreads) {
+      const PgEdge& ed = g.edges1[e];
+      double term[kPgTermStride];
+      lp_edge_terms(ed, lp_pose(dv, K, buf, ed.s), lp_pose(dv, K, buf, ed.d), term);
+      out_res[e] = term[42];
+    }
+  }
+  if (t == 0) *dv.state = st;
 }
 
 }  // namespace
@@ -851,6 +1193,17 @@ int launch_line_process_finish(const LpPlan& plan, const LpDev& dv, int ref, con
   }
   lp_edge_kernel<<<(std::max(plan.E, 1) + 127) / 128, 128, 0, st>>>(dv, plan.K, plan.E, ref >= 0 ? 2 : 0);
   return n + 1;
+}
+
+size_t line_process_batch_smem(int n_max) {
+  return sizeof(double) * ((size_t)(kLbNb + 1) * n_max + kLbNb * kLbDt + kLbThreads + kLbNb);
+}
+
+int launch_line_process_batch(const LpBatchGraph* graphs, int G, int n_max, int pass, cudaStream_t st) {
+  const size_t smem = line_process_batch_smem(n_max);
+  cudaFuncSetAttribute(lp_batch_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+  lp_batch_kernel<<<G, kLbThreads, smem, st>>>(graphs, pass, n_max);
+  return 1;
 }
 
 }  // namespace tzr

@@ -852,6 +852,24 @@ int launch_line_process_trial(const LpPlan& plan, const LpDev& dv, cudaStream_t 
 // The end of the call: compensation by T0_ref (T_ref)^-1 into the other pose buffer when ref >= 0 (T0: 12 doubles), then
 // every edge's terms at the returned poses (which buffer: 1 - cur with compensation, cur without).  Returns the launches.
 int launch_line_process_finish(const LpPlan& plan, const LpDev& dv, int ref, const double* T0, cudaStream_t st);
+// Many graphs in one call (tzr_pose_graph_optimize_line_process_batch, DESIGN.md §3.23): graphs of at most
+// kLpBatchMaxK nodes run a whole pass in one CTA each.  One entry per graph and pass, in device memory.
+constexpr int kLpBatchMaxK = 128;
+struct LpBatchGraph {
+  LpDev dv;              // this pass's edges, blocks, terms and confidences; the graph's poses (2 x K x 12), edge terms
+                         // (2 x E1 x kPgTermStride), H and A (n x n each), b (n); state: the graph's LpState
+  LpPlan plan;           // this pass's plan
+  const PgEdge* edges1;  // pass 1's edge table: the returned residuals
+  const double* init;    // K x 12: the starting poses
+  double* out;           // [confidences (E1) | poses (K x 12) | residuals (E1)]
+  int E1, ref;           // pass 1's edge count, reference_node
+  double T0[12];         // the reference node's starting pose (node 0's when ref = -1)
+};
+// Dynamic shared memory of lp_batch_kernel for graphs of at most n_max = 6 K rows.
+size_t line_process_batch_smem(int n_max);
+// One pass of every graph: pass 0 from the starting poses, pass 1 from pass 0's and to the outputs.  Returns the
+// launches (1).
+int launch_line_process_batch(const LpBatchGraph* graphs, int G, int n_max, int pass, cudaStream_t st);
 // dense Cholesky through the lazily loaded cuSOLVER (certify.cu): handle and workspace size of an n x n lower factor;
 // TZR_ERR_UNSUPPORTED when cuSOLVER cannot be loaded
 int dense_cholesky_setup(void** solver_handle, int n, double* A, int* lwork, cudaStream_t st, std::string* err);

@@ -76,6 +76,13 @@ class GlobalOptimization {
     LineProcessSummary summary;
   };
 
+  // One graph of a batch: initial_poses empty means the breadth-first start from the reference node.
+  struct Graph {
+    int num_nodes = 0;
+    std::vector<Edge> edges;
+    std::vector<Eigen::Matrix4d> initial_poses;
+  };
+
   GlobalOptimization() = default;
   explicit GlobalOptimization(const Params& params) : params_(params) {}
 
@@ -83,6 +90,12 @@ class GlobalOptimization {
   // PoseGraph::optimize's.  Throws std::runtime_error with the library's message on an invalid graph or parameters.
   Result optimize(int num_nodes, const std::vector<Edge>& edges,
                   const std::vector<Eigen::Matrix4d>* initial_poses = nullptr) const;
+
+  // tzr_pose_graph_optimize_line_process_batch: every graph in one call.  Entry g equals optimize() on graphs[g] for
+  // a graph of more than 128 nodes, and has its decisions for a smaller one (DESIGN.md §3.23).  A graph the single
+  // call would refuse gets an empty Result (no poses) and its status in *status (may be null; TZR_OK = 0 otherwise).
+  // Throws std::runtime_error only on call-level errors (invalid parameters, an empty batch, the workspace).
+  std::vector<Result> optimizeBatch(const std::vector<Graph>& graphs, std::vector<int>* status = nullptr) const;
 
   const Params& getParams() const { return params_; }
   void setParams(const Params& params) { params_ = params; }

@@ -569,7 +569,59 @@ PYBIND11_MODULE(_teaserpp, m) {
             return out;
           },
           py::arg("num_nodes"), py::arg("edges"), py::arg("transforms"), py::arg("information"),
-          py::arg("uncertain") = std::vector<bool>(), py::arg("initial_poses") = py::none());
+          py::arg("uncertain") = std::vector<bool>(), py::arg("initial_poses") = py::none())
+      .def(
+          "optimize_batch",
+          // graphs: dicts with optimize's keys (num_nodes, edges, transforms, information, and optionally uncertain
+          // and initial_poses); one dict per graph as optimize returns, plus status (a refused graph: no poses)
+          [](const teaser::GlobalOptimization& g, const py::list& graphs) {
+            std::vector<teaser::GlobalOptimization::Graph> gs(graphs.size());
+            for (size_t j = 0; j < gs.size(); ++j) {
+              const py::dict d = graphs[j].cast<py::dict>();
+              const auto edges = d["edges"].cast<std::vector<std::pair<int, int>>>();
+              const auto transforms = d["transforms"].cast<std::vector<SqArr>>();
+              const auto information = d["information"].cast<std::vector<SqArr>>();
+              const auto uncertain =
+                  d.contains("uncertain") && !d["uncertain"].is_none() ? d["uncertain"].cast<std::vector<bool>>()
+                                                                       : std::vector<bool>();
+              if (transforms.size() != edges.size() || information.size() != edges.size() ||
+                  (!uncertain.empty() && uncertain.size() != edges.size()))
+                throw std::invalid_argument("one transform, information matrix (and uncertain flag) per edge");
+              gs[j].num_nodes = d["num_nodes"].cast<int>();
+              gs[j].edges.resize(edges.size());
+              for (size_t e = 0; e < edges.size(); ++e) {
+                gs[j].edges[e].source = edges[e].first;
+                gs[j].edges[e].target = edges[e].second;
+                gs[j].edges[e].transform = square_of<4>(transforms[e]);
+                gs[j].edges[e].information = square_of<6>(information[e]);
+                gs[j].edges[e].uncertain = !uncertain.empty() && uncertain[e];
+              }
+              if (d.contains("initial_poses") && !d["initial_poses"].is_none())
+                for (const auto& a : d["initial_poses"].cast<std::vector<SqArr>>())
+                  gs[j].initial_poses.push_back(square_of<4>(a));
+            }
+            std::vector<teaser::GlobalOptimization::Result> rs;
+            std::vector<int> status;
+            {
+              py::gil_scoped_release release;
+              rs = g.optimizeBatch(gs, &status);
+            }
+            py::list out;
+            for (size_t j = 0; j < rs.size(); ++j) {
+              const auto& r = rs[j];
+              py::list poses;
+              for (const auto& T : r.poses) poses.append(square_to_numpy<4>(T));
+              py::dict o = line_process_dict(r.summary);
+              o["poses"] = poses;
+              o["confidence"] = r.confidence;
+              o["kept"] = r.kept;
+              o["residuals"] = r.residuals;
+              o["status"] = status[j];
+              out.append(o);
+            }
+            return out;
+          },
+          py::arg("graphs"));
 
   // GPU extra: point-to-plane ICP (teaser::PointToPlaneICP), given the target normals
   py::class_<teaser::PointToPlaneICP>(m, "PointToPlaneICP")

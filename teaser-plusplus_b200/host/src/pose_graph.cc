@@ -218,4 +218,71 @@ GlobalOptimization::Result GlobalOptimization::optimize(int num_nodes, const std
   return out;
 }
 
+std::vector<GlobalOptimization::Result> GlobalOptimization::optimizeBatch(const std::vector<Graph>& graphs,
+                                                                          std::vector<int>* status) const {
+  const size_t G = graphs.size();
+  const tzr_line_process_params p = line_process_c(params_);
+  std::vector<int32_t> K(G ? G : 1), E(G ? G : 1), st(G ? G : 1);
+  std::vector<std::vector<int32_t>> ends(G), unc(G);
+  std::vector<std::vector<tzr_similarity>> tr(G), init(G), poses(G);
+  std::vector<std::vector<double>> L(G), l(G), res(G);
+  std::vector<std::vector<uint8_t>> kept(G);
+  std::vector<const int32_t*> ep(G ? G : 1), up(G ? G : 1);
+  std::vector<const tzr_similarity*> tp(G ? G : 1), ip(G ? G : 1);
+  std::vector<const double*> Lp(G ? G : 1);
+  std::vector<tzr_similarity*> pp(G ? G : 1);
+  std::vector<double*> lp(G ? G : 1), rp(G ? G : 1);
+  std::vector<uint8_t*> kp(G ? G : 1);
+  for (size_t g = 0; g < G; ++g) {
+    const Graph& gr = graphs[g];
+    const size_t Eg = gr.edges.size();
+    if (!gr.initial_poses.empty() && gr.initial_poses.size() != static_cast<size_t>(gr.num_nodes))
+      throw std::invalid_argument("teaser::GlobalOptimization::optimizeBatch: one initial pose per node");
+    edges_c(gr.edges, &ends[g], &unc[g], &tr[g], &L[g]);
+    for (const Eigen::Matrix4d& T : gr.initial_poses) init[g].push_back(sim_of(T));
+    K[g] = gr.num_nodes;
+    E[g] = static_cast<int32_t>(Eg);
+    poses[g].resize(gr.num_nodes > 0 ? gr.num_nodes : 1);
+    l[g].resize(Eg ? Eg : 1);
+    res[g].resize(Eg ? Eg : 1);
+    kept[g].resize(Eg ? Eg : 1);
+    ep[g] = ends[g].data();
+    up[g] = unc[g].data();
+    tp[g] = tr[g].data();
+    Lp[g] = L[g].data();
+    ip[g] = gr.initial_poses.empty() ? nullptr : init[g].data();
+    pp[g] = poses[g].data();
+    lp[g] = l[g].data();
+    rp[g] = res[g].data();
+    kp[g] = kept[g].data();
+  }
+  std::vector<tzr_line_process_summary> s(G ? G : 1);
+  tzr_ctx* ctx = b200_context();
+  const int rc = tzr_pose_graph_optimize_line_process_batch(ctx, &p, static_cast<int>(G), K.data(), E.data(),
+                                                            ep.data(), tp.data(), Lp.data(), up.data(), ip.data(),
+                                                            pp.data(), lp.data(), kp.data(), rp.data(), s.data(),
+                                                            st.data());
+  if (rc != TZR_OK) fail("teaser::GlobalOptimization::optimizeBatch", rc, ctx);
+  std::vector<Result> out(G);
+  if (status) status->assign(st.begin(), st.begin() + G);
+  for (size_t g = 0; g < G; ++g) {
+    if (st[g] != TZR_OK) continue;
+    Result& r = out[g];
+    const size_t Eg = graphs[g].edges.size();
+    for (int k = 0; k < K[g]; ++k) r.poses.push_back(matrix_of(poses[g][k]));
+    r.confidence.assign(l[g].begin(), l[g].begin() + Eg);
+    for (size_t e = 0; e < Eg; ++e) r.kept.push_back(kept[g][e] != 0);
+    r.residuals.assign(res[g].begin(), res[g].begin() + Eg);
+    for (int q = 0; q < 2; ++q) {
+      r.summary.iterations[q] = s[g].iterations[q];
+      r.summary.trials[q] = s[g].trials[q];
+      r.summary.stop_reason[q] = s[g].stop_reason[q];
+      r.summary.mu[q] = s[g].mu[q];
+    }
+    r.summary.pruned = s[g].pruned;
+    r.summary.residual = s[g].residual;
+  }
+  return out;
+}
+
 }  // namespace teaser
