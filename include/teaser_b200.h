@@ -1255,6 +1255,43 @@ int tzr_pose_graph_optimize(tzr_ctx* ctx, const tzr_pose_graph_params* params, i
                             const tzr_similarity* initial_poses, tzr_similarity* poses, double* weights,
                             uint8_t* inlier_mask, double* residuals, tzr_pose_graph_summary* summary);
 
+/* Many independent graphs in one call, one set of params (DESIGN.md §3.24).  Per graph g the contract is
+ * tzr_pose_graph_optimize's, with these differences:
+ *   - Arguments: G >= 1 graphs; K[g], E[g]; edges[g] (E x 2 int32), edge_transforms[g] (E), information[g] (E x 36);
+ *     uncertain and initial_poses may be NULL or hold NULL entries, each with the single entry's meaning.  Outputs:
+ *     poses[g] (K); weights, inlier_mask and residuals may be NULL or hold NULL entries; summaries (G entries) may be
+ *     NULL; status (G entries) is required.
+ *   - Refusals: a NULL ctx, parameters the single entry refuses, G < 1 or a NULL K, E, edges, edge_transforms,
+ *     information, poses or status is TZR_ERR_INVALID_ARG before any device work, with nothing written.  Otherwise the
+ *     call returns TZR_OK, and status[g] is what tzr_pose_graph_optimize returns on graph g alone (K < 2, E < 1,
+ *     K > 1024, a non-rigid or non-finite edge or start pose, an endpoint out of range, a disconnected graph,
+ *     reference_node not a node of g, ...).  A graph that is refused gets zeroed outputs (poses, weights, inlier_mask,
+ *     residuals, summary); the other graphs are solved.  TZR_ERR_ALLOC or TZR_ERR_CUDA when the batched route's
+ *     workspace does not fit or the launch fails (tzr_last_error names the size or the failure); tzr_last_error
+ *     otherwise holds the last refusal's message.
+ *   - Routes: a graph with K <= 128 runs on the batched route: one CTA per graph runs the whole GNC-TLS solve (every
+ *     GNC iteration and every inner iteration, which may stop once the inner solve has stopped) with its own dense
+ *     Cholesky of the 6 (K - 1) x 6 (K - 1) system, so no cuSOLVER call.  A factorisation that meets a pivot that is not
+ *     > 0 is a rejection, as a non-zero potrf status is.  The costs, the weight updates and mu are computed in the
+ *     single entry's order, so the only source of difference is the factorisation: the iterations, inner iterations
+ *     and inlier mask are the single entry's unless a comparison lies within rounding of its threshold (DESIGN.md
+ *     §3.24); poses, weights, residuals and cost may differ from the single entry's in the last bits.  A graph with
+ *     128 < K <= 1024 runs through tzr_pose_graph_optimize after the batched route, one graph at a time, and its
+ *     result is that entry's bit for bit.
+ *   - Independence: each graph's outputs are bit-identical whatever the batch around it (its position, the other
+ *     graphs, G), and two calls are bit-identical: every reduction runs in one fixed shape within the graph's CTA.
+ *   - Launches and synchronisations on the batched route: exactly 1 kernel launch and 1 host synchronisation (one
+ *     read-back of every graph's outputs), whatever G, K, E or the iterations run; the K > 128 graphs add the single
+ *     entry's counts.
+ *   - Workspace: ctx's pose-graph workspace (so a retained solve stays retained), the batched graphs back to back: H
+ *     as (6 (K - 1))^2 doubles per graph (4.6 MB at K = 128) plus the edge tables and terms. */
+int tzr_pose_graph_optimize_batch(tzr_ctx* ctx, const tzr_pose_graph_params* params, int G, const int32_t* K,
+                                  const int32_t* E, const int32_t* const* edges,
+                                  const tzr_similarity* const* edge_transforms, const double* const* information,
+                                  const int32_t* const* uncertain, const tzr_similarity* const* initial_poses,
+                                  tzr_similarity* const* poses, double* const* weights, uint8_t* const* inlier_mask,
+                                  double* const* residuals, tzr_pose_graph_summary* summaries, int32_t* status);
+
 /* tzr_register_cloud_pairs_icp_point_to_plane (same arguments, same outputs bit for bit), then the information matrix
  * of every refined pair (solved, valid and finite record) at its ICP transform and the ICP's
  * max_correspondence_distance, from the clouds and transforms already on the device (no upload), then

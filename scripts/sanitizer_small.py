@@ -193,5 +193,8 @@ for seed, K in ((1, 40), (2, 75)):
 lpg.append(dict(lpg[0], K=41))
 lpr = ctx.global_optimization_batch(lpg, 0.05)
 print("line process batch", [r["status"] for r in lpr], [r["trials"] for r in lpr])
+# the batched GNC-TLS pose graph on the same graphs (one refused)
+pgr = ctx.optimize_pose_graph_batch(lpg, 0.05)
+print("pose graph batch", [r["status"] for r in pgr], [r["inner_iterations"] for r in pgr])
 ctx.close()
 print("DONE")

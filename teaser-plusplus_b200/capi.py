@@ -256,6 +256,7 @@ _SYMBOLS = [
     "tzr_register_cloud_pairs_icp_generalized", "tzr_icp_point_to_plane_robust_batch", "tzr_icp_generalized_robust_batch",
     "tzr_register_cloud_pairs_icp_robust", "tzr_ctx_last_strip_blocks", "tzr_graph_strip_schedule",
     "tzr_information_matrix", "tzr_information_matrix_batch", "tzr_pose_graph_params_default", "tzr_pose_graph_optimize",
+    "tzr_pose_graph_optimize_batch",
     "tzr_register_cloud_pairs_multiway", "tzr_estimate_color_gradients", "tzr_estimate_color_gradients_batch",
     "tzr_icp_colored", "tzr_icp_colored_batch", "tzr_voxel_downsample_colors", "tzr_voxel_downsample_colors_batch",
     "tzr_register_cloud_pairs_icp_colored", "tzr_register_cloud_pairs_multiway_colored", "tzr_icp_multiscale_batch",
@@ -429,6 +430,10 @@ def lib():
     L.tzr_pose_graph_optimize.argtypes = [vp, C.POINTER(PoseGraphParams), C.c_int, C.c_int, i32p,
                                           C.POINTER(Similarity), dp, i32p, C.POINTER(Similarity),
                                           C.POINTER(Similarity), dp, u8p, dp, C.POINTER(PoseGraphSummary)]
+    L.tzr_pose_graph_optimize_batch.argtypes = [
+        vp, C.POINTER(PoseGraphParams), C.c_int, i32p, i32p, C.POINTER(i32p), C.POINTER(C.POINTER(Similarity)),
+        C.POINTER(dp), C.POINTER(i32p), C.POINTER(C.POINTER(Similarity)), C.POINTER(C.POINTER(Similarity)),
+        C.POINTER(dp), C.POINTER(u8p), C.POINTER(dp), C.POINTER(PoseGraphSummary), i32p]
     L.tzr_register_cloud_pairs_multiway.argtypes = L.tzr_register_cloud_pairs_icp.argtypes + [
         i32p, C.POINTER(PoseGraphParams), dp, i32p, dp, u8p, C.POINTER(Similarity), C.POINTER(PoseGraphSummary), i32p]
     L.tzr_estimate_color_gradients.argtypes = [vp, fp, C.c_int, fp, fp, C.c_double, dp]
@@ -668,6 +673,64 @@ def _pts(a):
 
 def _p(a, t):
     return a.ctypes.data_as(C.POINTER(t))
+
+
+class _GraphBatch:
+    """The pointer-per-graph arrays of the batched pose-graph calls: G, K, E, edges, transforms, information,
+    uncertain, initial_poses (NULL entries where a graph has none) and, per graph, the outputs poses (K), a double (E), a
+    byte (E) and a double (E) array.  outs[g] = (K, E, poses, double, byte, double); status (G int32) and status_p."""
+
+    def __init__(self, graphs, who):
+        G = len(graphs)
+        self.G, self.P = G, max(1, G)
+        P = self.P
+        self.keep = []  # the arrays the pointers refer to
+        i32p, dp = C.POINTER(C.c_int32), C.POINTER(C.c_double)
+        simp = C.POINTER(Similarity)
+        self.Ks, self.Es = np.zeros(P, dtype=np.int32), np.zeros(P, dtype=np.int32)
+        self.ed_p, self.tr_p, self.info_p = (i32p * P)(), (simp * P)(), (dp * P)()
+        self.unc_p, self.init_p, self.pose_p = (i32p * P)(), (simp * P)(), (simp * P)()
+        self.d1_p, self.u8_p, self.d2_p = (dp * P)(), (C.POINTER(C.c_uint8) * P)(), (dp * P)()
+        self.outs = []
+        for g, gr in enumerate(graphs):
+            K = int(gr["K"])
+            ed = np.ascontiguousarray(gr["edges"], dtype=np.int32).reshape(-1, 2)
+            E = ed.shape[0]
+            info = np.ascontiguousarray(gr["information"], dtype=np.float64).reshape(E, 36)
+            if len(gr["transforms"]) != E:
+                raise TzrError(f"{who}: one transform per edge is required")
+            tr = (Similarity * max(1, E))(*[similarity(x) for x in gr["transforms"]])
+            self.keep.append(tr)
+            self.Ks[g], self.Es[g] = K, E
+            self.ed_p[g], self.info_p[g] = self._ptr(ed, C.c_int32), self._ptr(info, C.c_double)
+            self.tr_p[g] = C.cast(tr, simp)
+            if gr.get("uncertain") is not None:
+                unc = np.ascontiguousarray(gr["uncertain"], dtype=np.int32)
+                if unc.shape != (E,):
+                    raise TzrError(f"{who}: uncertain needs one entry per edge")
+                self.unc_p[g] = self._ptr(unc, C.c_int32)
+            if gr.get("initial_poses") is not None:
+                init = (Similarity * max(1, K))(*[similarity(x) for x in gr["initial_poses"]])
+                self.keep.append(init)
+                self.init_p[g] = C.cast(init, simp)
+            poses = (Similarity * max(1, K))()
+            d1, u8, d2 = np.zeros(max(1, E)), np.zeros(max(1, E), dtype=np.uint8), np.zeros(max(1, E))
+            self.keep.append(poses)
+            self.pose_p[g] = C.cast(poses, simp)
+            self.d1_p[g], self.u8_p[g], self.d2_p[g] = (self._ptr(d1, C.c_double), self._ptr(u8, C.c_uint8),
+                                                        self._ptr(d2, C.c_double))
+            self.outs.append((K, E, poses, d1, u8, d2))
+        self.status = np.zeros(P, dtype=np.int32)
+        self.status_p = _p(self.status, C.c_int32)
+
+    def _ptr(self, a, t):
+        self.keep.append(a)
+        return C.cast(a.ctypes.data, C.POINTER(t))
+
+    def args(self):
+        """G through the per-graph output arrays, in the batched calls' order."""
+        return (self.G, _p(self.Ks, C.c_int32), _p(self.Es, C.c_int32), self.ed_p, self.tr_p, self.info_p, self.unc_p,
+                self.init_p, self.pose_p, self.d1_p, self.u8_p, self.d2_p)
 
 
 class Context:
@@ -1717,63 +1780,32 @@ class Context:
         return dict(poses=_poses(poses), confidence=l[:E], kept=m[:E].astype(bool), residuals=r[:E],
                     **_line_process_summary(summ))
 
+    def optimize_pose_graph_batch(self, graphs, max_correspondence_distance, **params):
+        """tzr_pose_graph_optimize_batch: many GNC-TLS graphs, one PoseGraphParams (params: any of its fields).  graphs
+        as global_optimization_batch's.  Returns one dict per graph as optimize_pose_graph returns, plus status (the
+        single entry's return on that graph; a refused graph's outputs are zero).  Raises only on call-level
+        refusals."""
+        pg = pose_graph_params(max_correspondence_distance, **params)
+        a = _GraphBatch(graphs, "optimize_pose_graph_batch")
+        summ = (PoseGraphSummary * a.P)()
+        self._ck(lib().tzr_pose_graph_optimize_batch(self._h, C.byref(pg), *a.args(), summ, a.status_p))
+        return [dict(poses=_poses(poses)[:K], weights=w[:E], mask=m[:E].astype(bool), residuals=r[:E],
+                     status=int(a.status[g]), iterations=int(summ[g].iterations),
+                     inner_iterations=int(summ[g].inner_iterations), cost=float(summ[g].cost))
+                for g, (K, E, poses, w, m, r) in enumerate(a.outs)]
+
     def global_optimization_batch(self, graphs, max_correspondence_distance, **params):
         """tzr_pose_graph_optimize_line_process_batch: many graphs, one LineProcessParams (params: any of its fields).
         graphs: dicts with K, edges, transforms, information and optionally uncertain and initial_poses (None or absent:
         the single entry's default).  Returns one dict per graph as global_optimization returns, plus status (the single
         entry's return on that graph; a refused graph's outputs are zero).  Raises only on call-level refusals."""
         lp = line_process_params(max_correspondence_distance, **params)
-        G = len(graphs)
-        keep = []  # the arrays the pointers refer to
-
-        def ptr(a, t):
-            keep.append(a)
-            return C.cast(a.ctypes.data, C.POINTER(t))
-
-        Ks, Es = np.zeros(max(1, G), dtype=np.int32), np.zeros(max(1, G), dtype=np.int32)
-        P = max(1, G)
-        i32p = C.POINTER(C.c_int32)
-        ed_p, tr_p, info_p = (i32p * P)(), (C.POINTER(Similarity) * P)(), (C.POINTER(C.c_double) * P)()
-        unc_p, init_p, pose_p = (i32p * P)(), (C.POINTER(Similarity) * P)(), (C.POINTER(Similarity) * P)()
-        l_p, m_p, r_p = (C.POINTER(C.c_double) * P)(), (C.POINTER(C.c_uint8) * P)(), (C.POINTER(C.c_double) * P)()
-        outs = []
-        for g, gr in enumerate(graphs):
-            K = int(gr["K"])
-            ed = np.ascontiguousarray(gr["edges"], dtype=np.int32).reshape(-1, 2)
-            E = ed.shape[0]
-            info = np.ascontiguousarray(gr["information"], dtype=np.float64).reshape(E, 36)
-            if len(gr["transforms"]) != E:
-                raise TzrError("global_optimization_batch: one transform per edge is required")
-            tr = (Similarity * max(1, E))(*[similarity(x) for x in gr["transforms"]])
-            keep.append(tr)
-            Ks[g], Es[g] = K, E
-            ed_p[g], info_p[g] = ptr(ed, C.c_int32), ptr(info, C.c_double)
-            tr_p[g] = C.cast(tr, C.POINTER(Similarity))
-            if gr.get("uncertain") is not None:
-                unc = np.ascontiguousarray(gr["uncertain"], dtype=np.int32)
-                if unc.shape != (E,):
-                    raise TzrError("global_optimization_batch: uncertain needs one entry per edge")
-                unc_p[g] = ptr(unc, C.c_int32)
-            if gr.get("initial_poses") is not None:
-                init = (Similarity * max(1, K))(*[similarity(x) for x in gr["initial_poses"]])
-                keep.append(init)
-                init_p[g] = C.cast(init, C.POINTER(Similarity))
-            poses = (Similarity * max(1, K))()
-            l, m, r = np.zeros(max(1, E)), np.zeros(max(1, E), dtype=np.uint8), np.zeros(max(1, E))
-            keep.append(poses)
-            pose_p[g] = C.cast(poses, C.POINTER(Similarity))
-            l_p[g], m_p[g], r_p[g] = ptr(l, C.c_double), ptr(m, C.c_uint8), ptr(r, C.c_double)
-            outs.append((K, E, poses, l, m, r))
-        summ = (LineProcessSummary * P)()
-        status = np.zeros(P, dtype=np.int32)
-        self._ck(lib().tzr_pose_graph_optimize_line_process_batch(
-            self._h, C.byref(lp), G, _p(Ks, C.c_int32), _p(Es, C.c_int32), ed_p, tr_p, info_p, unc_p, init_p, pose_p,
-            l_p, m_p, r_p, summ, _p(status, C.c_int32)))
-        res = []
-        for g, (K, E, poses, l, m, r) in enumerate(outs):
-            res.append(dict(poses=_poses(poses)[:K], confidence=l[:E], kept=m[:E].astype(bool), residuals=r[:E],
-                            status=int(status[g]), **_line_process_summary(summ[g])))
-        return res
+        a = _GraphBatch(graphs, "global_optimization_batch")
+        summ = (LineProcessSummary * a.P)()
+        self._ck(lib().tzr_pose_graph_optimize_line_process_batch(self._h, C.byref(lp), *a.args(), summ, a.status_p))
+        return [dict(poses=_poses(poses)[:K], confidence=l[:E], kept=m[:E].astype(bool), residuals=r[:E],
+                     status=int(a.status[g]), **_line_process_summary(summ[g]))
+                for g, (K, E, poses, l, m, r) in enumerate(a.outs)]
 
     def icp(self, src, dst, max_correspondence_distance, init=None, max_iteration=30, relative_fitness=1e-6,
             relative_rmse=1e-6):

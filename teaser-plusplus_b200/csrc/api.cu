@@ -2339,10 +2339,18 @@ static void pg_edge_table(int E, const int32_t* ends, const tzr_similarity* T, c
   }
 }
 
-static int pose_graph_run(tzr_ctx* ctx, const tzr_pose_graph_params* prm, int K, int E, const int32_t* ends,
-                          const tzr_similarity* T, const double* info, const int32_t* uncertain,
-                          const tzr_similarity* init, tzr_similarity* poses, double* weights, uint8_t* inlier_mask,
-                          double* residuals, tzr_pose_graph_summary* summary) {
+// One graph's checks, start and plan, in the single entry's order of refusals (include/teaser_b200.h)
+struct PgGraphPrep {
+  std::vector<double> pose;  // K x 12 starting poses
+  std::vector<PgEdge> ed;
+  std::vector<PgBlock> blocks;
+  std::vector<PgTerm> terms;
+  PgPlan plan;
+  double cost_floor = 0;     // 1e-24 c^2 sum Lambda(5,5)
+};
+static int pg_prepare(tzr_ctx* ctx, const tzr_pose_graph_params* prm, int K, int E, const int32_t* ends,
+                      const tzr_similarity* T, const double* info, const int32_t* uncertain,
+                      const tzr_similarity* init, const tzr_similarity* poses, PgGraphPrep* g) {
   if (!ctx || !pg_params_ok(prm) || K < 2 || E < 1 || !ends || !T || !info || !poses) {
     if (ctx) ctx->last_error = "pose graph: invalid arguments (K >= 2, E >= 1 and the parameters' ranges)";
     return TZR_ERR_INVALID_ARG;
@@ -2358,23 +2366,53 @@ static int pose_graph_run(tzr_ctx* ctx, const tzr_pose_graph_params* prm, int K,
   }
   std::vector<char> live;
   double info_sum = 0.0;
-  std::vector<double> pose;
-  int rc = pg_start(ctx, K, E, ends, T, info, uncertain, init, ref, &live, &info_sum, &pose);
+  int rc = pg_start(ctx, K, E, ends, T, info, uncertain, init, ref, &live, &info_sum, &g->pose);
   if (rc != TZR_OK) return rc;
   const double c = prm->max_correspondence_distance;
-  std::vector<PgEdge> ed;
-  std::vector<PgBlock> blocks;
-  std::vector<PgTerm> terms;
-  pg_edge_table(E, ends, T, info, uncertain, live, ref, c, &ed, &blocks, &terms);
-  PgPlan plan;
+  pg_edge_table(E, ends, T, info, uncertain, live, ref, c, &g->ed, &g->blocks, &g->terms);
+  PgPlan& plan = g->plan;
   plan.K = K;
   plan.E = E;
   plan.n = 6 * (K - 1);
-  plan.blocks = (int)blocks.size();
+  plan.blocks = (int)g->blocks.size();
   plan.max_inner = prm->max_inner_iterations;
   plan.gnc_factor = prm->gnc_factor;
   plan.cost_threshold = prm->cost_threshold;
-  const double cost_floor = 1e-24 * (c * c) * info_sum;
+  g->cost_floor = 1e-24 * (c * c) * info_sum;
+  return TZR_OK;
+}
+
+// One graph's outputs: the final poses (K x 12), and per edge the weight w[e], its inlier flag and r-bar
+// res[e * res_stride]
+static void pg_write_outputs(int K, int E, const double* pose, const double* w, const double* res, size_t res_stride,
+                             tzr_similarity* poses, double* weights, uint8_t* inlier_mask, double* residuals) {
+  for (int k = 0; k < K; ++k) {
+    memset(&poses[k], 0, sizeof(tzr_similarity));
+    poses[k].scale = 1.0;
+    memcpy(poses[k].rotation, &pose[12 * (size_t)k], 72);
+    memcpy(poses[k].translation, &pose[12 * (size_t)k + 9], 24);
+  }
+  for (int e = 0; e < E; ++e) {
+    if (weights) weights[e] = w[e];
+    if (inlier_mask) inlier_mask[e] = w[e] >= 0.5 ? 1 : 0;
+    if (residuals) residuals[e] = res[(size_t)e * res_stride];
+  }
+}
+
+static int pose_graph_run(tzr_ctx* ctx, const tzr_pose_graph_params* prm, int K, int E, const int32_t* ends,
+                          const tzr_similarity* T, const double* info, const int32_t* uncertain,
+                          const tzr_similarity* init, tzr_similarity* poses, double* weights, uint8_t* inlier_mask,
+                          double* residuals, tzr_pose_graph_summary* summary) {
+  PgGraphPrep gp;
+  int rc = pg_prepare(ctx, prm, K, E, ends, T, info, uncertain, init, poses, &gp);
+  if (rc != TZR_OK) return rc;
+  const int ref = prm->reference_node;
+  std::vector<double>& pose = gp.pose;
+  const std::vector<PgEdge>& ed = gp.ed;
+  const std::vector<PgBlock>& blocks = gp.blocks;
+  const std::vector<PgTerm>& terms = gp.terms;
+  const PgPlan& plan = gp.plan;
+  const double cost_floor = gp.cost_floor;
   const size_t n = (size_t)plan.n;
   // workspace: [edges | blocks | terms | poses (2 buffers) | weights | state] staged in one copy, then the edge terms,
   // H, g and the factorisation's workspace
@@ -2432,17 +2470,8 @@ static int pose_graph_run(tzr_ctx* ctx, const tzr_pose_graph_params* prm, int K,
   CK(cudaMemcpyAsync(terms_out.data(), dv.eterm + (size_t)hs.cur * E * kPgTermStride, (size_t)E * kPgTermStride * 8,
                      cudaMemcpyDeviceToHost, st));
   CK(cudaStreamSynchronize(st));
-  for (int k = 0; k < K; ++k) {
-    memset(&poses[k], 0, sizeof(tzr_similarity));
-    poses[k].scale = 1.0;
-    memcpy(poses[k].rotation, &pose[12 * (size_t)k], 72);
-    memcpy(poses[k].translation, &pose[12 * (size_t)k + 9], 24);
-  }
-  for (int e = 0; e < E; ++e) {
-    if (weights) weights[e] = w[e];
-    if (inlier_mask) inlier_mask[e] = w[e] >= 0.5 ? 1 : 0;
-    if (residuals) residuals[e] = terms_out[(size_t)e * kPgTermStride + 43];
-  }
+  pg_write_outputs(K, E, pose.data(), w.data(), terms_out.data() + 43, kPgTermStride, poses, weights, inlier_mask,
+                   residuals);
   if (summary) {
     summary->iterations = outer;
     summary->inner_iterations = (int32_t)inner_total;
@@ -2708,9 +2737,10 @@ static int line_process_run(tzr_ctx* ctx, const tzr_line_process_params* prm, in
 }
 
 // ---- many graphs in one call (tzr_pose_graph_optimize_line_process_batch, DESIGN.md §3.23) ---------------------------
-// The largest K of the batched route: kLpBatchMaxK, or TZR_LP_BATCH_MAX_K for measurements of the crossover, capped at
-// the largest K whose lp_batch_kernel fits the device's shared memory.
-static int lp_batch_max_k(tzr_ctx* ctx) {
+// The largest K of both optimisers' batched routes (DESIGN.md §3.23, §3.24): kLpBatchMaxK, or TZR_LP_BATCH_MAX_K for
+// measurements of the crossover, capped at the largest K whose lp_batch_kernel fits the device's shared memory (the
+// GNC-TLS kernel's 6 (K - 1) rows need less).  A graph's route depends on its own K alone.
+static int pose_graph_batch_max_k(tzr_ctx* ctx) {
   int optin = 0;
   cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, ctx->device);
   int cap = 1024;
@@ -2720,15 +2750,21 @@ static int lp_batch_max_k(tzr_ctx* ctx) {
   return std::min(k >= 1 ? k : kLpBatchMaxK, cap);
 }
 
-static void lp_zero_outputs(int K, int E, tzr_similarity* poses, double* confidence, uint8_t* kept, double* residuals,
-                            tzr_line_process_summary* summary) {
+// A refused graph's outputs of either optimiser's batch: its poses, its three per-edge arrays (the weights or
+// confidences, the inlier or kept mask, the residuals) and its summary, zeroed (a template, so C++ linkage inside this
+// file's extern "C" block)
+extern "C++" {
+template <class Summary>
+static void zero_graph_outputs(int K, int E, tzr_similarity* poses, double* per_edge, uint8_t* mask, double* residuals,
+                               Summary* summary) {
   if (poses && K > 0) memset(poses, 0, (size_t)K * sizeof(tzr_similarity));
   if (E > 0) {
-    if (confidence) memset(confidence, 0, (size_t)E * 8);
-    if (kept) memset(kept, 0, (size_t)E);
+    if (per_edge) memset(per_edge, 0, (size_t)E * 8);
+    if (mask) memset(mask, 0, (size_t)E);
     if (residuals) memset(residuals, 0, (size_t)E * 8);
   }
   if (summary) memset(summary, 0, sizeof(*summary));
+}
 }
 
 static int line_process_batch_run(tzr_ctx* ctx, const tzr_line_process_params* prm, int G, const int32_t* K,
@@ -2738,7 +2774,7 @@ static int line_process_batch_run(tzr_ctx* ctx, const tzr_line_process_params* p
                                   double* const* confidence, uint8_t* const* kept, double* const* residuals,
                                   tzr_line_process_summary* summaries, int32_t* status) {
   auto opt = [](auto arr, int g) { return arr ? arr[g] : nullptr; };
-  const int kmax = lp_batch_max_k(ctx);
+  const int kmax = pose_graph_batch_max_k(ctx);
   // validate, start and plan every graph of the batched route; the others run through the single entry afterwards
   std::vector<int> small, large;
   std::vector<LpGraphPrep> prep(G);
@@ -2752,8 +2788,8 @@ static int line_process_batch_run(tzr_ctx* ctx, const tzr_line_process_params* p
                               poses[g], &prep[g]);
     if (rc != TZR_OK) {
       status[g] = rc;
-      lp_zero_outputs(K[g], E[g], poses[g], opt(confidence, g), opt(kept, g), opt(residuals, g),
-                      summaries ? summaries + g : nullptr);
+      zero_graph_outputs(K[g], E[g], poses[g], opt(confidence, g), opt(kept, g), opt(residuals, g),
+                         summaries ? summaries + g : nullptr);
       continue;
     }
     small.push_back(g);
@@ -2912,8 +2948,137 @@ static int line_process_batch_run(tzr_ctx* ctx, const tzr_line_process_params* p
                                  summaries ? summaries + g : nullptr);
     if (status[g] != TZR_OK) {
       last = ctx->last_error;
-      lp_zero_outputs(K[g], E[g], poses[g], opt(confidence, g), opt(kept, g), opt(residuals, g),
-                      summaries ? summaries + g : nullptr);
+      zero_graph_outputs(K[g], E[g], poses[g], opt(confidence, g), opt(kept, g), opt(residuals, g),
+                         summaries ? summaries + g : nullptr);
+    }
+  }
+  ctx->last_error = last;
+  return TZR_OK;
+}
+
+// ---- many GNC-TLS graphs in one call (tzr_pose_graph_optimize_batch, DESIGN.md §3.24) --------------------------------
+static int pose_graph_batch_run(tzr_ctx* ctx, const tzr_pose_graph_params* prm, int G, const int32_t* K,
+                                const int32_t* E, const int32_t* const* edges, const tzr_similarity* const* T,
+                                const double* const* info, const int32_t* const* uncertain,
+                                const tzr_similarity* const* init, tzr_similarity* const* poses,
+                                double* const* weights, uint8_t* const* inlier_mask, double* const* residuals,
+                                tzr_pose_graph_summary* summaries, int32_t* status) {
+  auto opt = [](auto arr, int g) { return arr ? arr[g] : nullptr; };
+  const int kmax = pose_graph_batch_max_k(ctx);
+  // validate, start and plan every graph of the batched route; the others run through the single entry afterwards
+  std::vector<int> small, large;
+  std::vector<PgGraphPrep> prep(G);
+  for (int g = 0; g < G; ++g) {
+    status[g] = TZR_OK;
+    if (K[g] > kmax) {
+      large.push_back(g);
+      continue;
+    }
+    const int rc = pg_prepare(ctx, prm, K[g], E[g], edges[g], T[g], info[g], opt(uncertain, g), opt(init, g),
+                              poses[g], &prep[g]);
+    if (rc != TZR_OK) {
+      status[g] = rc;
+      zero_graph_outputs(K[g], E[g], poses[g], opt(weights, g), opt(inlier_mask, g), opt(residuals, g),
+                         summaries ? summaries + g : nullptr);
+      continue;
+    }
+    small.push_back(g);
+  }
+  const std::string refusal = ctx->last_error;
+  if (!small.empty()) {
+    // workspace, graphs back to back: [descriptors | per graph: edges, blocks, terms, starting poses, weights, state]
+    // (staged in one copy) then [per graph: summary and outputs (poses, weights, r-bar)] (read back in one copy) and
+    // the working buffers [per graph: poses, edge terms, H]
+    const int S = (int)small.size();
+    struct Off { size_t ed, blk, trm, init, w, st, sum, out, pose, term, H; };
+    std::vector<Off> off(S);
+    int n_max = 0;
+    size_t o = al256((size_t)S * sizeof(PgBatchGraph));
+    for (int j = 0; j < S; ++j) {
+      const PgGraphPrep& g = prep[small[j]];
+      const size_t e = (size_t)g.plan.E;
+      off[j].ed = o;
+      off[j].blk = off[j].ed + al256(e * sizeof(PgEdge));
+      off[j].trm = off[j].blk + al256(g.blocks.size() * sizeof(PgBlock));
+      off[j].init = off[j].trm + al256(g.terms.size() * sizeof(PgTerm));
+      off[j].w = off[j].init + al256((size_t)g.plan.K * 12 * 8);
+      off[j].st = off[j].w + al256(e * 8);
+      o = off[j].st + al256(sizeof(PgState));
+    }
+    const size_t in_end = o, out_lo = o;
+    for (int j = 0; j < S; ++j) {
+      const PgGraphPrep& g = prep[small[j]];
+      off[j].sum = o;
+      off[j].out = off[j].sum + al256(sizeof(tzr_pose_graph_summary));
+      o = off[j].out + al256(((size_t)12 * g.plan.K + (size_t)2 * g.plan.E) * 8);
+    }
+    const size_t out_hi = o;
+    for (int j = 0; j < S; ++j) {
+      const PgGraphPrep& g = prep[small[j]];
+      const size_t n = (size_t)g.plan.n;
+      n_max = std::max(n_max, g.plan.n);
+      off[j].pose = o;
+      off[j].term = off[j].pose + al256((size_t)g.plan.K * 24 * 8);
+      off[j].H = off[j].term + al256((size_t)g.plan.E * 2 * kPgTermStride * 8);
+      o = off[j].H + al256(n * n * 8);
+    }
+    cudaSetDevice(ctx->device);
+    cudaStream_t st = ctx->stream;
+    int rc;
+    if ((rc = ensure(ctx, ctx->pg, o)) != TZR_OK) return rc;
+    char* d = (char*)ctx->pg.p;
+    std::vector<char> h(in_end, 0);
+    for (int j = 0; j < S; ++j) {
+      const PgGraphPrep& g = prep[small[j]];
+      const Off& f = off[j];
+      PgBatchGraph x{};
+      x.dv = PgDev{(const PgEdge*)(d + f.ed), (const PgBlock*)(d + f.blk), (const PgTerm*)(d + f.trm),
+                   (double*)(d + f.pose), (double*)(d + f.term), (double*)(d + f.w), (double*)(d + f.H), nullptr,
+                   (PgState*)(d + f.st)};
+      x.plan = g.plan;
+      x.init = (const double*)(d + f.init);
+      x.out = (double*)(d + f.out);
+      x.summary = (tzr_pose_graph_summary*)(d + f.sum);
+      x.ref = prm->reference_node;
+      x.max_iterations = prm->max_iterations;
+      x.cost_floor = g.cost_floor;
+      memcpy(h.data() + (size_t)j * sizeof(PgBatchGraph), &x, sizeof(x));
+      const size_t e = (size_t)g.plan.E;
+      memcpy(h.data() + f.ed, g.ed.data(), e * sizeof(PgEdge));
+      memcpy(h.data() + f.blk, g.blocks.data(), g.blocks.size() * sizeof(PgBlock));
+      memcpy(h.data() + f.trm, g.terms.data(), g.terms.size() * sizeof(PgTerm));
+      memcpy(h.data() + f.init, g.pose.data(), (size_t)g.plan.K * 12 * 8);
+      for (size_t q = 0; q < e; ++q) ((double*)(h.data() + f.w))[q] = 1.0;
+      PgState s0{};  // as the single entry stages it
+      s0.gnc_cost = INFINITY;
+      memcpy(h.data() + f.st, &s0, sizeof(s0));
+    }
+    CK(cudaMemcpyAsync(d, h.data(), in_end, cudaMemcpyHostToDevice, st));
+    ctx->launches += launch_pose_graph_batch((const PgBatchGraph*)d, S, n_max, st);
+    if ((rc = check_launch(ctx, "pose graph batch launch")) != TZR_OK) return rc;
+    std::vector<char> out(out_hi - out_lo);
+    CK(cudaMemcpyAsync(out.data(), d + out_lo, out.size(), cudaMemcpyDeviceToHost, st));
+    CK(cudaStreamSynchronize(st));
+    for (int j = 0; j < S; ++j) {
+      const int gi = small[j];
+      const Off& f = off[j];
+      const int Kg = K[gi], Eg = E[gi];
+      const double* lo = (const double*)(out.data() + (f.out - out_lo));
+      pg_write_outputs(Kg, Eg, lo, lo + 12 * (size_t)Kg, lo + 12 * (size_t)Kg + Eg, 1, poses[gi], opt(weights, gi),
+                       opt(inlier_mask, gi), opt(residuals, gi));
+      if (summaries) memcpy(summaries + gi, out.data() + (f.sum - out_lo), sizeof(tzr_pose_graph_summary));
+    }
+  }
+  // the graphs above the batched route's size, one by one through the single entry
+  std::string last = refusal;
+  for (int g : large) {
+    status[g] = pose_graph_run(ctx, prm, K[g], E[g], edges[g], T[g], info[g], opt(uncertain, g), opt(init, g),
+                               poses[g], opt(weights, g), opt(inlier_mask, g), opt(residuals, g),
+                               summaries ? summaries + g : nullptr);
+    if (status[g] != TZR_OK) {
+      last = ctx->last_error;
+      zero_graph_outputs(K[g], E[g], poses[g], opt(weights, g), opt(inlier_mask, g), opt(residuals, g),
+                         summaries ? summaries + g : nullptr);
     }
   }
   ctx->last_error = last;
@@ -4399,6 +4564,21 @@ int tzr_pose_graph_optimize(tzr_ctx* ctx, const tzr_pose_graph_params* params, i
                             uint8_t* inlier_mask, double* residuals, tzr_pose_graph_summary* summary) {
   return pose_graph_run(ctx, params, K, E, edges, edge_transforms, information, uncertain, initial_poses, poses,
                         weights, inlier_mask, residuals, summary);
+}
+
+int tzr_pose_graph_optimize_batch(tzr_ctx* ctx, const tzr_pose_graph_params* params, int G, const int32_t* K,
+                                  const int32_t* E, const int32_t* const* edges,
+                                  const tzr_similarity* const* edge_transforms, const double* const* information,
+                                  const int32_t* const* uncertain, const tzr_similarity* const* initial_poses,
+                                  tzr_similarity* const* poses, double* const* weights, uint8_t* const* inlier_mask,
+                                  double* const* residuals, tzr_pose_graph_summary* summaries, int32_t* status) {
+  if (!ctx) return TZR_ERR_INVALID_ARG;
+  if (!pg_params_ok(params) || G < 1 || !K || !E || !edges || !edge_transforms || !information || !poses || !status) {
+    ctx->last_error = "pose graph batch: invalid arguments (the parameters' ranges, G >= 1 and the required arrays)";
+    return TZR_ERR_INVALID_ARG;
+  }
+  return pose_graph_batch_run(ctx, params, G, K, E, edges, edge_transforms, information, uncertain, initial_poses,
+                              poses, weights, inlier_mask, residuals, summaries, status);
 }
 
 int tzr_register_cloud_pairs_multiway(tzr_ctx* ctx, const tzr_frontend_params* fp, const tzr_params* params,

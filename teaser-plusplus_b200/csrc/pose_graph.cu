@@ -138,14 +138,8 @@ __device__ __forceinline__ double* term_at(const PgDev& dv, int E, int buf, int 
   return dv.eterm + kPgTermStride * ((size_t)buf * E + e);
 }
 
-// which = 0: the current poses into the current terms; 1: the candidate poses (the other buffer), skipped once the
-// inner solve has stopped
-__global__ void pg_edge_kernel(PgDev dv, int K, int E, int which) {
-  const int e = blockIdx.x * blockDim.x + threadIdx.x;
-  if (e >= E) return;
-  const PgState& st = *dv.state;
-  if (which == 1 && st.done) return;
-  const int buf = which == 0 ? st.cur : 1 - st.cur;
+// Edge e's terms at the poses in buffer buf into that buffer's terms (pg_edge_kernel and the batched solve share it)
+__device__ __forceinline__ void pg_edge_terms(const PgDev& dv, int K, int E, int buf, int e) {
   const PgEdge& ed = dv.edges[e];
   const double* Ts = pose_at(dv, K, buf, ed.s);
   const double* Td = pose_at(dv, K, buf, ed.d);
@@ -226,6 +220,16 @@ __global__ void pg_edge_kernel(PgDev dv, int K, int E, int which) {
   out[43] = c * ed.inv_norm;
 }
 
+// which = 0: the current poses into the current terms; 1: the candidate poses (the other buffer), skipped once the
+// inner solve has stopped
+__global__ void pg_edge_kernel(PgDev dv, int K, int E, int which) {
+  const int e = blockIdx.x * blockDim.x + threadIdx.x;
+  if (e >= E) return;
+  const PgState& st = *dv.state;
+  if (which == 1 && st.done) return;
+  pg_edge_terms(dv, K, E, which == 0 ? st.cur : 1 - st.cur, e);
+}
+
 // The fixed-order weighted sum over one warp: lane l adds w_e x_e for e = l, l + 32, ... in turn, then a butterfly
 __device__ double pg_warp_sum(const PgDev& dv, int E, int buf) {
   double a = 0.0;
@@ -234,19 +238,18 @@ __device__ double pg_warp_sum(const PgDev& dv, int E, int buf) {
   return a;
 }
 
-// mode 0: start the inner solve at the current poses; mode 1: decide on the candidate (include/teaser_b200.h states
-// the rule)
-__global__ void pg_cost_kernel(PgDev dv, int E, int mode, double cost_floor) {
-  PgState& st = *dv.state;
-  if (mode == 0) {
-    const double cost = pg_warp_sum(dv, E, st.cur);
-    if (threadIdx.x != 0) return;
-    st.cost = cost;
-    st.lambda = kPgLambda0;
-    st.done = 0;
-    st.inner = 0;
-    return;
-  }
+// pg_cost_kernel's two modes on the state st, run by one warp.  Start: the inner solve at the current poses' cost.
+__device__ __forceinline__ void pg_cost_start(const PgDev& dv, PgState& st, int E) {
+  const double cost = pg_warp_sum(dv, E, st.cur);
+  if (threadIdx.x != 0) return;
+  st.cost = cost;
+  st.lambda = kPgLambda0;
+  st.done = 0;
+  st.inner = 0;
+}
+
+// Step: the decision on the candidate poses' cost (include/teaser_b200.h states the rule)
+__device__ __forceinline__ void pg_cost_step(const PgDev& dv, PgState& st, int E, double cost_floor) {
   if (st.done) return;
   const double cand = pg_warp_sum(dv, E, 1 - st.cur);
   if (threadIdx.x != 0) return;
@@ -269,18 +272,21 @@ __global__ void pg_cost_kernel(PgDev dv, int E, int mode, double cost_floor) {
   }
 }
 
-// One warp per listed block.  H block (bi, bj), bi >= bj: entry (r, k) = sum over its terms of sign * (w_e M_e(r, k))
-// in the listed order, then on a diagonal block's diagonal a + lambda (a + 1): the additive part keeps the damped system
-// positive definite when a node's every edge has weight 0 (its block of H is then 0); H is column-major n x n and
-// only its lower triangle is read.  Right-hand-side block bi (bj = -1): -(sum of sign * (w_e v_e(r))).
-__global__ void pg_assemble_kernel(PgDev dv, int E, int n, int nblocks) {
-  const int b = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
-  const int lane = threadIdx.x & 31;
-  if (b >= nblocks) return;
-  const PgState& st = *dv.state;
-  if (st.done) return;
-  const PgBlock bl = dv.blocks[b];
-  const int cur = st.cur;
+// mode 0: start the inner solve at the current poses; mode 1: decide on the candidate
+__global__ void pg_cost_kernel(PgDev dv, int E, int mode, double cost_floor) {
+  PgState& st = *dv.state;
+  if (mode == 0) {
+    pg_cost_start(dv, st, E);
+    return;
+  }
+  pg_cost_step(dv, st, E, cost_floor);
+}
+
+// One warp's share of pg_assemble_kernel: listed block bl of H (lower triangle; entry (r, k) = sum of sign * (w_e
+// M_e(r, k)) in the listed order, then on a diagonal block's diagonal a + lambda (a + 1)) or the right-hand side block
+// -(sum of sign * (w_e v_e(r))) into g
+__device__ __forceinline__ void pg_assemble_block(const PgDev& dv, const PgState& st, int E, int n, int cur,
+                                                  const PgBlock bl, int lane, double* g) {
   if (bl.bj < 0) {
     if (lane >= 6) return;
     double a = 0.0;
@@ -288,7 +294,7 @@ __global__ void pg_assemble_kernel(PgDev dv, int E, int n, int nblocks) {
       const PgTerm tm = dv.terms[q];
       a = a + (double)tm.sign * (dv.weight[tm.e] * term_at(dv, E, cur, tm.e)[36 + lane]);
     }
-    dv.g[6 * bl.bi + lane] = -a;
+    g[6 * bl.bi + lane] = -a;
     return;
   }
   for (int l = lane; l < 36; l += 32) {
@@ -303,8 +309,30 @@ __global__ void pg_assemble_kernel(PgDev dv, int E, int n, int nblocks) {
   }
 }
 
-// One thread per node: the candidate T_k' = Exp(delta_k) T_k (R' = R_x R, t' = R_x t + t_x); the reference node keeps
-// its pose
+// One warp per listed block.  H block (bi, bj), bi >= bj: entry (r, k) = sum over its terms of sign * (w_e M_e(r, k))
+// in the listed order, then on a diagonal block's diagonal a + lambda (a + 1): the additive part keeps the damped system
+// positive definite when a node's every edge has weight 0 (its block of H is then 0); H is column-major n x n and
+// only its lower triangle is read.  Right-hand-side block bi (bj = -1): -(sum of sign * (w_e v_e(r))).
+__global__ void pg_assemble_kernel(PgDev dv, int E, int n, int nblocks) {
+  const int b = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
+  const int lane = threadIdx.x & 31;
+  if (b >= nblocks) return;
+  const PgState& st = *dv.state;
+  if (st.done) return;
+  pg_assemble_block(dv, st, E, n, st.cur, dv.blocks[b], lane, dv.g);
+}
+
+// The candidate Tn = Exp(x) T (R' = R_x R, t' = R_x t + t_x) from the node's 6 entries x of the step
+__device__ __forceinline__ void pg_candidate(const double* T, const double* x, double* Tn) {
+  double Rx[9], tx[3], u[3];
+  se3_exp(x, x + 3, Rx, tx);
+  m33(Rx, T, Tn);
+  mv3(Rx, T + 9, u);
+#pragma unroll
+  for (int r = 0; r < 3; ++r) Tn[9 + r] = u[r] + tx[r];
+}
+
+// One thread per node: the candidate T_k' = Exp(delta_k) T_k; the reference node keeps its pose
 __global__ void pg_update_kernel(PgDev dv, int K, int ref) {
   const int k = blockIdx.x * blockDim.x + threadIdx.x;
   if (k >= K) return;
@@ -316,20 +344,15 @@ __global__ void pg_update_kernel(PgDev dv, int K, int ref) {
     for (int q = 0; q < 12; ++q) Tn[q] = T[q];
     return;
   }
-  const double* x = dv.g + 6 * (k < ref ? k : k - 1);
-  double Rx[9], tx[3], u[3];
-  se3_exp(x, x + 3, Rx, tx);
-  m33(Rx, T, Tn);
-  mv3(Rx, T + 9, u);
-#pragma unroll
-  for (int r = 0; r < 3; ++r) Tn[9 + r] = u[r] + tx[r];
+  pg_candidate(T, dv.g + 6 * (k < ref ? k : k - 1), Tn);
 }
 
-// GNC-TLS after GNC iteration `iter` (the rotation stage's schedule on r-bar, include/teaser_b200.h).  The weight
-// formula is a copy of gnc_tls_block's (rot_trans.cu), not a shared function: sharing it would move the rotation
-// kernels' code, which must stay as it is, and this one reads a normalised residual (noise bound 1) from one warp.
-__global__ void pg_gnc_kernel(PgDev dv, int E, int iter, double gnc_factor, double cost_threshold) {
-  PgState& st = *dv.state;
+// GNC-TLS after GNC iteration `iter` (the rotation stage's schedule on r-bar, include/teaser_b200.h), run by one warp
+// (lane = threadIdx.x) on the state st.  The weight formula is a copy of gnc_tls_block's (rot_trans.cu), not a shared
+// function: sharing it would move the rotation kernels' code, which must stay as it is, and this one reads a
+// normalised residual (noise bound 1) from one warp.
+__device__ __forceinline__ void pg_gnc_rule(const PgDev& dv, PgState& st, int E, int iter, double gnc_factor,
+                                            double cost_threshold) {
   const int lane = threadIdx.x;
   const int cur = st.cur;
   int n_unc = 0;
@@ -382,6 +405,10 @@ __global__ void pg_gnc_kernel(PgDev dv, int E, int iter, double gnc_factor, doub
   st.mu = mu * gnc_factor;
   st.gnc_cost = c;
   if (diff < cost_threshold) st.stop = 1;
+}
+
+__global__ void pg_gnc_kernel(PgDev dv, int E, int iter, double gnc_factor, double cost_threshold) {
+  pg_gnc_rule(dv, *dv.state, E, iter, gnc_factor, cost_threshold);
 }
 
 }  // namespace
@@ -1158,6 +1185,104 @@ __global__ void __launch_bounds__(kLbThreads) lp_batch_kernel(const LpBatchGraph
   if (t == 0) *dv.state = st;
 }
 
+// ---- many GNC-TLS graphs in one call (tzr_pose_graph_optimize_batch, DESIGN.md §3.24) ---------------------------------
+// pg_batch_kernel: one CTA of kLbThreads per graph runs the whole GNC-TLS solve with its state in shared memory: per
+// GNC iteration the edge terms and the cost (pg_edge_kernel, pg_cost_kernel mode 0), then per inner iteration H
+// cleared, assembled and damped (pg_assemble_kernel), lb_cholesky and lb_solve in place of potrf / potrs, the candidate
+// and its terms and the decision (pg_update_kernel, pg_edge_kernel, pg_cost_kernel mode 1), then the weight update
+// (pg_gnc_kernel).  The rules are the single entry's helpers, and warp 0 runs the cost sums and the weight update as
+// the single entry's one-warp kernels do, so with the same edge terms the costs, mu and the weights are the same bits.
+
+// the terms of every edge at the poses in buffer buf
+__device__ void pb_edges(const PgDev& dv, int K, int E, int buf) {
+  for (int e = threadIdx.x; e < E; e += kLbThreads) pg_edge_terms(dv, K, E, buf, e);
+  __syncthreads();
+}
+
+__global__ void __launch_bounds__(kLbThreads) pg_batch_kernel(const PgBatchGraph* graphs, int ldp) {
+  extern __shared__ double smem[];
+  double* Ps = smem;                   // kLbNb x ldp: the Cholesky panel
+  double* Dt = Ps + kLbNb * ldp;       // kLbNb x kLbDt: its diagonal tile
+  double* x = Dt + kLbNb * kLbDt;      // ldp: -g, then the step
+  // x + ldp: kLbThreads doubles that only lp_batch_kernel uses (its reductions; the two share
+  // line_process_batch_smem's layout)
+  double* tmp = x + ldp + kLbThreads;  // kLbNb: the backward sweep's sums
+  __shared__ PgState st;
+  const PgBatchGraph& g = graphs[blockIdx.x];
+  const PgDev dv = g.dv;
+  const PgPlan p = g.plan;
+  const int K = p.K, E = p.E, n = p.n, ref = g.ref, t = threadIdx.x;
+  for (int w = t; w < 12 * K; w += kLbThreads) dv.poses[w] = g.init[w];
+  if (t == 0) st = *dv.state;
+  __syncthreads();
+  // the terms of the buffer that holds no candidate yet are zeroed, so that the cost sum after a failed factorisation
+  // (pg_cost_step sums the candidate buffer whatever its status) reads defined values
+  double* cand_terms = dv.eterm + (size_t)(1 - st.cur) * E * kPgTermStride;
+  for (int w = t; w < E * kPgTermStride; w += kLbThreads) cand_terms[w] = 0.0;
+  int outer = 0, inner_total = 0;
+  for (int it = 0; it < g.max_iterations; ++it) {
+    pb_edges(dv, K, E, st.cur);
+    if (t < 32) pg_cost_start(dv, st, E);
+    __syncthreads();
+    // the single entry enqueues max_inner iterations, and every one after the stop is a no-op
+    for (int j = 0; j < p.max_inner && !st.done; ++j) {
+      // H's lower triangle cleared (the factor of the previous iteration fills blocks the plan does not list), then
+      // the listed blocks with the damping, one warp per block as pg_assemble_kernel, and -g into x
+      for (int w = t; w < n * n; w += kLbThreads)
+        if (w % n >= w / n) dv.H[w] = 0.0;
+      __syncthreads();
+      const int cur = st.cur;
+      for (int b = t >> 5; b < p.blocks; b += kLbThreads / 32)
+        pg_assemble_block(dv, st, E, n, cur, dv.blocks[b], t & 31, x);
+      __syncthreads();
+      const int bad = lb_cholesky(dv.H, n, Ps, ldp, Dt);
+      __syncthreads();
+      if (!bad) {
+        lb_solve(dv.H, n, x, tmp);
+        for (int k = t; k < K; k += kLbThreads) {
+          const double* T = pose_at(dv, K, cur, k);
+          double* Tn = pose_at(dv, K, 1 - cur, k);
+          if (k == ref)
+            for (int q = 0; q < 12; ++q) Tn[q] = T[q];
+          else
+            pg_candidate(T, x + 6 * (k < ref ? k : k - 1), Tn);
+        }
+        __syncthreads();
+        pb_edges(dv, K, E, 1 - cur);
+      }
+      // a failed factorisation is a rejection, as a non-zero potrf status is; pg_cost_step then sums the candidate
+      // buffer's terms from an earlier candidate (or the zeros written above) and discards the sum
+      if (t == 0) {
+        st.info[0] = bad;
+        st.info[1] = 0;
+      }
+      if (t < 32) pg_cost_step(dv, st, E, g.cost_floor);
+      __syncthreads();
+    }
+    outer = it + 1;
+    inner_total += st.inner;
+    if (t < 32) pg_gnc_rule(dv, st, E, it, p.gnc_factor, p.cost_threshold);
+    __syncthreads();
+    if (st.stop) break;
+  }
+  // the outputs: poses and r-bar at the current buffer, the weights, the summary
+  const int cur = st.cur;
+  double* out_pose = g.out;
+  double* out_w = out_pose + 12 * K;
+  double* out_res = out_w + E;
+  for (int w = t; w < 12 * K; w += kLbThreads) out_pose[w] = dv.poses[(size_t)cur * 12 * K + w];
+  for (int e = t; e < E; e += kLbThreads) {
+    out_w[e] = dv.weight[e];
+    out_res[e] = term_at(dv, E, cur, e)[43];
+  }
+  if (t == 0) {
+    g.summary->iterations = outer;
+    g.summary->inner_iterations = inner_total;
+    g.summary->cost = st.cost;
+    *dv.state = st;
+  }
+}
+
 }  // namespace
 
 int launch_line_process_begin(const LpPlan& plan, const LpDev& dv, cudaStream_t st) {
@@ -1203,6 +1328,13 @@ int launch_line_process_batch(const LpBatchGraph* graphs, int G, int n_max, int 
   const size_t smem = line_process_batch_smem(n_max);
   cudaFuncSetAttribute(lp_batch_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
   lp_batch_kernel<<<G, kLbThreads, smem, st>>>(graphs, pass, n_max);
+  return 1;
+}
+
+int launch_pose_graph_batch(const PgBatchGraph* graphs, int G, int n_max, cudaStream_t st) {
+  const size_t smem = line_process_batch_smem(n_max);
+  cudaFuncSetAttribute(pg_batch_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+  pg_batch_kernel<<<G, kLbThreads, smem, st>>>(graphs, n_max);
   return 1;
 }
 

@@ -870,6 +870,22 @@ size_t line_process_batch_smem(int n_max);
 // One pass of every graph: pass 0 from the starting poses, pass 1 from pass 0's and to the outputs.  Returns the
 // launches (1).
 int launch_line_process_batch(const LpBatchGraph* graphs, int G, int n_max, int pass, cudaStream_t st);
+// Many GNC-TLS graphs in one call (tzr_pose_graph_optimize_batch, DESIGN.md §3.24): graphs of at most kLpBatchMaxK
+// nodes run their whole solve in one CTA each.  One entry per graph, in device memory.
+struct PgBatchGraph {
+  PgDev dv;                        // the graph's edges, blocks, terms, weights (staged at 1) and state (staged as the
+                                   // single entry stages it); its poses (2 x K x 12), edge terms (2 x E x
+                                   // kPgTermStride) and H (n x n, factored in place); g is not used
+  PgPlan plan;
+  const double* init;              // K x 12: the starting poses
+  double* out;                     // [poses (K x 12) | weights (E) | r-bar (E)]
+  tzr_pose_graph_summary* summary;
+  int ref, max_iterations;
+  double cost_floor;               // the inner solve's stopping floor, 1e-24 c^2 sum Lambda(5,5)
+};
+// The whole solve of every graph (dynamic shared memory line_process_batch_smem(n_max), n_max = the largest
+// 6 (K - 1)).  Returns the launches (1).
+int launch_pose_graph_batch(const PgBatchGraph* graphs, int G, int n_max, cudaStream_t st);
 // dense Cholesky through the lazily loaded cuSOLVER (certify.cu): handle and workspace size of an n x n lower factor;
 // TZR_ERR_UNSUPPORTED when cuSOLVER cannot be loaded
 int dense_cholesky_setup(void** solver_handle, int n, double* A, int* lwork, cudaStream_t st, std::string* err);

@@ -1,7 +1,8 @@
 // Multiway registration on the GPU through the C-ABI (include/teaser_b200.h, DESIGN.md §3.16): Open3D's
 // get_information_matrix_from_point_clouds (teaser::informationMatrix, informationMatrixBatch: tzr_information_matrix,
 // tzr_information_matrix_batch) and a pose graph with GNC-TLS on its uncertain edges (teaser::PoseGraph:
-// tzr_pose_graph_optimize).  RobustRegistrationSolver::solveMultiway (teaser/registration.h) chains both after the
+// tzr_pose_graph_optimize; PoseGraph::optimizeBatch: tzr_pose_graph_optimize_batch, DESIGN.md §3.24).
+// RobustRegistrationSolver::solveMultiway (teaser/registration.h) chains both after the
 // cloud-pair call.  teaser::GlobalOptimization is Open3D's global_optimization with the line process
 // (tzr_pose_graph_optimize_line_process, DESIGN.md §3.22), and solveMultiway has overloads that take its Params.  No CPU
 // implementation: without a CUDA device the first call throws std::runtime_error.
@@ -44,6 +45,13 @@ class PoseGraph {
     int inner_iterations = 0;            // Levenberg-Marquardt iterations, summed
     double cost = 0;
   };
+  // One graph of a batch (both optimisers' optimizeBatch): initial_poses empty means the breadth-first start from the
+  // reference node.
+  struct Graph {
+    int num_nodes = 0;
+    std::vector<Edge> edges;
+    std::vector<Eigen::Matrix4d> initial_poses;
+  };
 
   PoseGraph() = default;
   explicit PoseGraph(const Params& params) : params_(params) {}
@@ -53,6 +61,12 @@ class PoseGraph {
   // invalid graph (disconnected, more than 1024 nodes, a non-rigid edge).
   Result optimize(int num_nodes, const std::vector<Edge>& edges,
                   const std::vector<Eigen::Matrix4d>* initial_poses = nullptr) const;
+
+  // tzr_pose_graph_optimize_batch: every graph in one call.  Entry g equals optimize() on graphs[g] for a graph of
+  // more than 128 nodes, and has its decisions for a smaller one (DESIGN.md §3.24).  A graph the single call would
+  // refuse gets an empty Result (no poses) and its status in *status (may be null; TZR_OK = 0 otherwise).  Throws
+  // std::runtime_error only on call-level errors (invalid parameters, an empty batch, the workspace).
+  std::vector<Result> optimizeBatch(const std::vector<Graph>& graphs, std::vector<int>* status = nullptr) const;
 
   const Params& getParams() const { return params_; }
   void setParams(const Params& params) { params_ = params; }
@@ -68,19 +82,13 @@ class GlobalOptimization {
  public:
   using Params = LineProcessParams;
   using Edge = PoseGraph::Edge;
+  using Graph = PoseGraph::Graph;
   struct Result {
     std::vector<Eigen::Matrix4d> poses;  // node k into the world frame
     std::vector<double> confidence;      // per edge: pass 2's for a kept edge, pass 1's for a pruned one
     std::vector<bool> kept;
     std::vector<double> residuals;       // zeta^T Lambda zeta at the returned poses
     LineProcessSummary summary;
-  };
-
-  // One graph of a batch: initial_poses empty means the breadth-first start from the reference node.
-  struct Graph {
-    int num_nodes = 0;
-    std::vector<Edge> edges;
-    std::vector<Eigen::Matrix4d> initial_poses;
   };
 
   GlobalOptimization() = default;

@@ -261,6 +261,37 @@ py::array_t<double> square_to_numpy(const Eigen::Matrix<double, N, N>& M) {
 }
 using SqArr = py::array_t<double, py::array::c_style | py::array::forcecast>;
 
+// The graphs of both optimisers' optimize_batch: dicts with optimize's keys (num_nodes, edges, transforms,
+// information, and optionally uncertain and initial_poses)
+std::vector<teaser::PoseGraph::Graph> graphs_of(const py::list& graphs) {
+  std::vector<teaser::PoseGraph::Graph> gs(graphs.size());
+  for (size_t j = 0; j < gs.size(); ++j) {
+    const py::dict d = graphs[j].cast<py::dict>();
+    const auto edges = d["edges"].cast<std::vector<std::pair<int, int>>>();
+    const auto transforms = d["transforms"].cast<std::vector<SqArr>>();
+    const auto information = d["information"].cast<std::vector<SqArr>>();
+    const auto uncertain =
+        d.contains("uncertain") && !d["uncertain"].is_none() ? d["uncertain"].cast<std::vector<bool>>()
+                                                             : std::vector<bool>();
+    if (transforms.size() != edges.size() || information.size() != edges.size() ||
+        (!uncertain.empty() && uncertain.size() != edges.size()))
+      throw std::invalid_argument("one transform, information matrix (and uncertain flag) per edge");
+    gs[j].num_nodes = d["num_nodes"].cast<int>();
+    gs[j].edges.resize(edges.size());
+    for (size_t e = 0; e < edges.size(); ++e) {
+      gs[j].edges[e].source = edges[e].first;
+      gs[j].edges[e].target = edges[e].second;
+      gs[j].edges[e].transform = square_of<4>(transforms[e]);
+      gs[j].edges[e].information = square_of<6>(information[e]);
+      gs[j].edges[e].uncertain = !uncertain.empty() && uncertain[e];
+    }
+    if (d.contains("initial_poses") && !d["initial_poses"].is_none())
+      for (const auto& a : d["initial_poses"].cast<std::vector<SqArr>>())
+        gs[j].initial_poses.push_back(square_of<4>(a));
+  }
+  return gs;
+}
+
 // MultiScaleICP's scales from Python: (voxel_size, max_correspondence_distance, max_iteration[, normal_search_radius[,
 // relative_fitness[, relative_rmse]]]) tuples or dicts with those keys; the normal radius defaults to 2 voxel_size
 std::vector<teaser::ICPScale> scales_of(const py::list& scales) {
@@ -506,7 +537,32 @@ PYBIND11_MODULE(_teaserpp, m) {
                             py::arg("inner_iterations") = r.inner_iterations, py::arg("cost") = r.cost);
           },
           py::arg("num_nodes"), py::arg("edges"), py::arg("transforms"), py::arg("information"),
-          py::arg("uncertain") = std::vector<bool>(), py::arg("initial_poses") = py::none());
+          py::arg("uncertain") = std::vector<bool>(), py::arg("initial_poses") = py::none())
+      .def(
+          "optimize_batch",
+          // graphs: dicts with optimize's keys; one dict per graph as optimize returns, plus status (a refused graph:
+          // no poses)
+          [](const teaser::PoseGraph& g, const py::list& graphs) {
+            const std::vector<teaser::PoseGraph::Graph> gs = graphs_of(graphs);
+            std::vector<teaser::PoseGraph::Result> rs;
+            std::vector<int> status;
+            {
+              py::gil_scoped_release release;
+              rs = g.optimizeBatch(gs, &status);
+            }
+            py::list out;
+            for (size_t j = 0; j < rs.size(); ++j) {
+              const auto& r = rs[j];
+              py::list poses;
+              for (const auto& T : r.poses) poses.append(square_to_numpy<4>(T));
+              out.append(py::dict(py::arg("poses") = poses, py::arg("weights") = r.weights,
+                                  py::arg("inliers") = r.inliers, py::arg("residuals") = r.residuals,
+                                  py::arg("iterations") = r.iterations, py::arg("inner_iterations") = r.inner_iterations,
+                                  py::arg("cost") = r.cost, py::arg("status") = status[j]));
+            }
+            return out;
+          },
+          py::arg("graphs"));
 
   // GPU extra: Open3D's line-process pose graph (teaser::GlobalOptimization)
   py::class_<teaser::GlobalOptimization>(m, "GlobalOptimization")
@@ -572,34 +628,10 @@ PYBIND11_MODULE(_teaserpp, m) {
           py::arg("uncertain") = std::vector<bool>(), py::arg("initial_poses") = py::none())
       .def(
           "optimize_batch",
-          // graphs: dicts with optimize's keys (num_nodes, edges, transforms, information, and optionally uncertain
-          // and initial_poses); one dict per graph as optimize returns, plus status (a refused graph: no poses)
+          // graphs: dicts with optimize's keys; one dict per graph as optimize returns, plus status (a refused graph:
+          // no poses)
           [](const teaser::GlobalOptimization& g, const py::list& graphs) {
-            std::vector<teaser::GlobalOptimization::Graph> gs(graphs.size());
-            for (size_t j = 0; j < gs.size(); ++j) {
-              const py::dict d = graphs[j].cast<py::dict>();
-              const auto edges = d["edges"].cast<std::vector<std::pair<int, int>>>();
-              const auto transforms = d["transforms"].cast<std::vector<SqArr>>();
-              const auto information = d["information"].cast<std::vector<SqArr>>();
-              const auto uncertain =
-                  d.contains("uncertain") && !d["uncertain"].is_none() ? d["uncertain"].cast<std::vector<bool>>()
-                                                                       : std::vector<bool>();
-              if (transforms.size() != edges.size() || information.size() != edges.size() ||
-                  (!uncertain.empty() && uncertain.size() != edges.size()))
-                throw std::invalid_argument("one transform, information matrix (and uncertain flag) per edge");
-              gs[j].num_nodes = d["num_nodes"].cast<int>();
-              gs[j].edges.resize(edges.size());
-              for (size_t e = 0; e < edges.size(); ++e) {
-                gs[j].edges[e].source = edges[e].first;
-                gs[j].edges[e].target = edges[e].second;
-                gs[j].edges[e].transform = square_of<4>(transforms[e]);
-                gs[j].edges[e].information = square_of<6>(information[e]);
-                gs[j].edges[e].uncertain = !uncertain.empty() && uncertain[e];
-              }
-              if (d.contains("initial_poses") && !d["initial_poses"].is_none())
-                for (const auto& a : d["initial_poses"].cast<std::vector<SqArr>>())
-                  gs[j].initial_poses.push_back(square_of<4>(a));
-            }
+            const std::vector<teaser::PoseGraph::Graph> gs = graphs_of(graphs);
             std::vector<teaser::GlobalOptimization::Result> rs;
             std::vector<int> status;
             {

@@ -71,7 +71,83 @@ void edges_c(const std::vector<PoseGraph::Edge>& edges, std::vector<int32_t>* en
   }
 }
 
+// The pointer-per-graph arrays of both optimisers' batched C calls, and per graph the outputs: poses (K), a double
+// (E), a byte (E) and a double (E) array
+struct GraphArrays {
+  std::vector<int32_t> K, E, status;
+  std::vector<std::vector<int32_t>> ends, unc;
+  std::vector<std::vector<tzr_similarity>> tr, init, poses;
+  std::vector<std::vector<double>> L, d1, d2;
+  std::vector<std::vector<uint8_t>> u8;
+  std::vector<const int32_t*> ep, up;
+  std::vector<const tzr_similarity*> tp, ip;
+  std::vector<const double*> Lp;
+  std::vector<tzr_similarity*> pp;
+  std::vector<double*> d1p, d2p;
+  std::vector<uint8_t*> u8p;
+
+  GraphArrays(const std::vector<PoseGraph::Graph>& graphs, const char* who) {
+    const size_t G = graphs.size(), P = G ? G : 1;
+    K.resize(P);
+    E.resize(P);
+    status.resize(P);
+    ends.resize(G);
+    unc.resize(G);
+    tr.resize(G);
+    init.resize(G);
+    poses.resize(G);
+    L.resize(G);
+    d1.resize(G);
+    d2.resize(G);
+    u8.resize(G);
+    ep.resize(P);
+    up.resize(P);
+    tp.resize(P);
+    ip.resize(P);
+    Lp.resize(P);
+    pp.resize(P);
+    d1p.resize(P);
+    d2p.resize(P);
+    u8p.resize(P);
+    for (size_t g = 0; g < G; ++g) {
+      const PoseGraph::Graph& gr = graphs[g];
+      const size_t Eg = gr.edges.size();
+      if (!gr.initial_poses.empty() && gr.initial_poses.size() != static_cast<size_t>(gr.num_nodes))
+        throw std::invalid_argument(std::string(who) + ": one initial pose per node");
+      edges_c(gr.edges, &ends[g], &unc[g], &tr[g], &L[g]);
+      for (const Eigen::Matrix4d& T : gr.initial_poses) init[g].push_back(sim_of(T));
+      K[g] = gr.num_nodes;
+      E[g] = static_cast<int32_t>(Eg);
+      poses[g].resize(gr.num_nodes > 0 ? gr.num_nodes : 1);
+      d1[g].resize(Eg ? Eg : 1);
+      d2[g].resize(Eg ? Eg : 1);
+      u8[g].resize(Eg ? Eg : 1);
+      ep[g] = ends[g].data();
+      up[g] = unc[g].data();
+      tp[g] = tr[g].data();
+      Lp[g] = L[g].data();
+      ip[g] = gr.initial_poses.empty() ? nullptr : init[g].data();
+      pp[g] = poses[g].data();
+      d1p[g] = d1[g].data();
+      d2p[g] = d2[g].data();
+      u8p[g] = u8[g].data();
+    }
+  }
+};
+
 }  // namespace
+
+tzr_pose_graph_params pose_graph_c(const PoseGraphParams& q) {
+  tzr_pose_graph_params p;
+  tzr_pose_graph_params_default(&p);
+  p.max_correspondence_distance = q.max_correspondence_distance;
+  p.gnc_factor = q.gnc_factor;
+  p.cost_threshold = q.cost_threshold;
+  p.max_iterations = q.max_iterations;
+  p.max_inner_iterations = q.max_inner_iterations;
+  p.reference_node = q.reference_node;
+  return p;
+}
 
 tzr_line_process_params line_process_c(const LineProcessParams& q) {
   tzr_line_process_params p;
@@ -144,14 +220,7 @@ PoseGraph::Result PoseGraph::optimize(int num_nodes, const std::vector<Edge>& ed
   const size_t E = edges.size();
   if (initial_poses && initial_poses->size() != static_cast<size_t>(num_nodes))
     throw std::invalid_argument("teaser::PoseGraph::optimize: one initial pose per node");
-  tzr_pose_graph_params p;
-  tzr_pose_graph_params_default(&p);
-  p.max_correspondence_distance = params_.max_correspondence_distance;
-  p.gnc_factor = params_.gnc_factor;
-  p.cost_threshold = params_.cost_threshold;
-  p.max_iterations = params_.max_iterations;
-  p.max_inner_iterations = params_.max_inner_iterations;
-  p.reference_node = params_.reference_node;
+  const tzr_pose_graph_params p = pose_graph_c(params_);
   std::vector<int32_t> ends, unc;
   std::vector<tzr_similarity> tr;
   std::vector<double> L;
@@ -218,61 +287,56 @@ GlobalOptimization::Result GlobalOptimization::optimize(int num_nodes, const std
   return out;
 }
 
+std::vector<PoseGraph::Result> PoseGraph::optimizeBatch(const std::vector<Graph>& graphs,
+                                                        std::vector<int>* status) const {
+  const size_t G = graphs.size();
+  const tzr_pose_graph_params p = pose_graph_c(params_);
+  GraphArrays a(graphs, "teaser::PoseGraph::optimizeBatch");
+  std::vector<tzr_pose_graph_summary> s(G ? G : 1);
+  tzr_ctx* ctx = b200_context();
+  const int rc = tzr_pose_graph_optimize_batch(ctx, &p, static_cast<int>(G), a.K.data(), a.E.data(), a.ep.data(),
+                                               a.tp.data(), a.Lp.data(), a.up.data(), a.ip.data(), a.pp.data(),
+                                               a.d1p.data(), a.u8p.data(), a.d2p.data(), s.data(), a.status.data());
+  if (rc != TZR_OK) fail("teaser::PoseGraph::optimizeBatch", rc, ctx);
+  std::vector<Result> out(G);
+  if (status) status->assign(a.status.begin(), a.status.begin() + G);
+  for (size_t g = 0; g < G; ++g) {
+    if (a.status[g] != TZR_OK) continue;
+    Result& r = out[g];
+    const size_t Eg = graphs[g].edges.size();
+    for (int k = 0; k < a.K[g]; ++k) r.poses.push_back(matrix_of(a.poses[g][k]));
+    r.weights.assign(a.d1[g].begin(), a.d1[g].begin() + Eg);
+    for (size_t e = 0; e < Eg; ++e) r.inliers.push_back(a.u8[g][e] != 0);
+    r.residuals.assign(a.d2[g].begin(), a.d2[g].begin() + Eg);
+    r.iterations = s[g].iterations;
+    r.inner_iterations = s[g].inner_iterations;
+    r.cost = s[g].cost;
+  }
+  return out;
+}
+
 std::vector<GlobalOptimization::Result> GlobalOptimization::optimizeBatch(const std::vector<Graph>& graphs,
                                                                           std::vector<int>* status) const {
   const size_t G = graphs.size();
   const tzr_line_process_params p = line_process_c(params_);
-  std::vector<int32_t> K(G ? G : 1), E(G ? G : 1), st(G ? G : 1);
-  std::vector<std::vector<int32_t>> ends(G), unc(G);
-  std::vector<std::vector<tzr_similarity>> tr(G), init(G), poses(G);
-  std::vector<std::vector<double>> L(G), l(G), res(G);
-  std::vector<std::vector<uint8_t>> kept(G);
-  std::vector<const int32_t*> ep(G ? G : 1), up(G ? G : 1);
-  std::vector<const tzr_similarity*> tp(G ? G : 1), ip(G ? G : 1);
-  std::vector<const double*> Lp(G ? G : 1);
-  std::vector<tzr_similarity*> pp(G ? G : 1);
-  std::vector<double*> lp(G ? G : 1), rp(G ? G : 1);
-  std::vector<uint8_t*> kp(G ? G : 1);
-  for (size_t g = 0; g < G; ++g) {
-    const Graph& gr = graphs[g];
-    const size_t Eg = gr.edges.size();
-    if (!gr.initial_poses.empty() && gr.initial_poses.size() != static_cast<size_t>(gr.num_nodes))
-      throw std::invalid_argument("teaser::GlobalOptimization::optimizeBatch: one initial pose per node");
-    edges_c(gr.edges, &ends[g], &unc[g], &tr[g], &L[g]);
-    for (const Eigen::Matrix4d& T : gr.initial_poses) init[g].push_back(sim_of(T));
-    K[g] = gr.num_nodes;
-    E[g] = static_cast<int32_t>(Eg);
-    poses[g].resize(gr.num_nodes > 0 ? gr.num_nodes : 1);
-    l[g].resize(Eg ? Eg : 1);
-    res[g].resize(Eg ? Eg : 1);
-    kept[g].resize(Eg ? Eg : 1);
-    ep[g] = ends[g].data();
-    up[g] = unc[g].data();
-    tp[g] = tr[g].data();
-    Lp[g] = L[g].data();
-    ip[g] = gr.initial_poses.empty() ? nullptr : init[g].data();
-    pp[g] = poses[g].data();
-    lp[g] = l[g].data();
-    rp[g] = res[g].data();
-    kp[g] = kept[g].data();
-  }
+  GraphArrays a(graphs, "teaser::GlobalOptimization::optimizeBatch");
   std::vector<tzr_line_process_summary> s(G ? G : 1);
   tzr_ctx* ctx = b200_context();
-  const int rc = tzr_pose_graph_optimize_line_process_batch(ctx, &p, static_cast<int>(G), K.data(), E.data(),
-                                                            ep.data(), tp.data(), Lp.data(), up.data(), ip.data(),
-                                                            pp.data(), lp.data(), kp.data(), rp.data(), s.data(),
-                                                            st.data());
+  const int rc = tzr_pose_graph_optimize_line_process_batch(ctx, &p, static_cast<int>(G), a.K.data(), a.E.data(),
+                                                            a.ep.data(), a.tp.data(), a.Lp.data(), a.up.data(),
+                                                            a.ip.data(), a.pp.data(), a.d1p.data(), a.u8p.data(),
+                                                            a.d2p.data(), s.data(), a.status.data());
   if (rc != TZR_OK) fail("teaser::GlobalOptimization::optimizeBatch", rc, ctx);
   std::vector<Result> out(G);
-  if (status) status->assign(st.begin(), st.begin() + G);
+  if (status) status->assign(a.status.begin(), a.status.begin() + G);
   for (size_t g = 0; g < G; ++g) {
-    if (st[g] != TZR_OK) continue;
+    if (a.status[g] != TZR_OK) continue;
     Result& r = out[g];
     const size_t Eg = graphs[g].edges.size();
-    for (int k = 0; k < K[g]; ++k) r.poses.push_back(matrix_of(poses[g][k]));
-    r.confidence.assign(l[g].begin(), l[g].begin() + Eg);
-    for (size_t e = 0; e < Eg; ++e) r.kept.push_back(kept[g][e] != 0);
-    r.residuals.assign(res[g].begin(), res[g].begin() + Eg);
+    for (int k = 0; k < a.K[g]; ++k) r.poses.push_back(matrix_of(a.poses[g][k]));
+    r.confidence.assign(a.d1[g].begin(), a.d1[g].begin() + Eg);
+    for (size_t e = 0; e < Eg; ++e) r.kept.push_back(a.u8[g][e] != 0);
+    r.residuals.assign(a.d2[g].begin(), a.d2[g].begin() + Eg);
     for (int q = 0; q < 2; ++q) {
       r.summary.iterations[q] = s[g].iterations[q];
       r.summary.trials[q] = s[g].trials[q];

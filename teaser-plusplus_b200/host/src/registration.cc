@@ -629,6 +629,7 @@ std::vector<RobustRegistrationSolver::SolveCertifyResult> RobustRegistrationSolv
 
 void icp_result_from_c(const tzr_icp_result& r, const int32_t* corr, PointToPointICPResult* out);  // icp.cc
 tzr_line_process_params line_process_c(const LineProcessParams& p);                                  // pose_graph.cc
+tzr_pose_graph_params pose_graph_c(const PoseGraphParams& p);                                        // pose_graph.cc
 
 namespace {
 
@@ -832,14 +833,7 @@ static RobustRegistrationSolver::MultiwayResult run_multiway(
   ip.max_iteration = icp.max_iteration;
   ip.relative_fitness = icp.relative_fitness;
   ip.relative_rmse = icp.relative_rmse;
-  tzr_pose_graph_params pg;
-  tzr_pose_graph_params_default(&pg);
-  pg.max_correspondence_distance = pose_graph.max_correspondence_distance;
-  pg.gnc_factor = pose_graph.gnc_factor;
-  pg.cost_threshold = pose_graph.cost_threshold;
-  pg.max_iterations = pose_graph.max_iterations;
-  pg.max_inner_iterations = pose_graph.max_inner_iterations;
-  pg.reference_node = pose_graph.reference_node;
+  tzr_pose_graph_params pg = pose_graph_c(pose_graph);
   std::vector<int32_t> unc(P), counts(P);
   for (size_t q = 0; q < P; ++q) unc[q] = uncertain[q] ? 1 : 0;
   std::vector<double> info(P * 36), w(P);
