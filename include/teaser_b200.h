@@ -1483,6 +1483,68 @@ int tzr_register_cloud_pairs_multiway_line_process(
     const tzr_line_process_params* lp, double* information, int32_t* info_counts, double* edge_confidence,
     uint8_t* edge_kept, tzr_similarity* poses, tzr_line_process_summary* lp_summary, int32_t* lp_status);
 
+/* ---- multiway registration of many scan sequences in one call (DESIGN.md §3.25) ------------------------------------
+ * tzr_register_cloud_pairs_multiway_line_process's arguments (colors may be NULL: point-to-plane ICP, and kernel must
+ * then be NULL; otherwise coloured ICP) over the clouds of G sequences, plus:
+ *   - G >= 1 and graph_offsets (G + 1 int32): graph g owns clouds [off[g], off[g+1]), its node k is cloud off[g] + k.
+ *     Pairs of different graphs may interleave in pair_clouds, but a pair's two clouds must lie in one graph.
+ *   - Per graph: pg_status (G entries, required), the summaries (G entries, may be NULL).  poses (n_clouds entries):
+ *     each cloud's pose in its own graph's frame.  edge_weights / edge_mask (or the confidences / kept mask) and the
+ *     information matrices per pair, as in the single entries.
+ *   - The fused map: map_voxel_size 0 makes none (map_points, map_counts and map_colors may then be NULL); > 0 (finite)
+ *     makes one per graph whose pose graph returned TZR_OK: every point p of the graph's clouds transformed by its
+ *     cloud's pose in float64 with p read exactly, in the order ((R00 x + R01 y) + R02 z) + t0 (likewise y, z), rounded
+ *     once to float, concatenated in cloud order and inside a cloud in point order, then voxel-downsampled exactly as
+ *     tzr_voxel_downsample(_colors)_batch downsamples that concatenation (with colours, the colours averaged as it
+ *     averages them).  map_points[g] needs room for the graph's total point count x 3 floats (map_colors[g] likewise;
+ *     map_colors is required with colours and ignored without them); map_counts[g] receives the map's rows, 0 for a
+ *     graph that was refused by its pose graph or whose grid is too large (TZR_ERR_TOO_LARGE, as the voxel batch).
+ *     Deviation from Open3D's tutorial: Open3D keeps the transformed points in double; here they are rounded to float,
+ *     like every other cloud in this library.  The map reads the clouds already on the device (no second upload).
+ * Contract:
+ *   - Every per-pair output equals the whole table through tzr_register_cloud_pairs_icp_point_to_plane (without
+ *     colours) or tzr_register_cloud_pairs_icp_colored (with them) bit for bit; the information matrices equal
+ *     tzr_information_matrix_batch over the refined pairs in pair order.
+ *   - Graph g's edges are its refined pairs in ascending pair index, end points shifted by -off[g], uncertain flags
+ *     uncertain[p].  Poses, weights or confidences, masks or kept sets, summaries and statuses equal
+ *     tzr_pose_graph_optimize_batch (or tzr_pose_graph_optimize_line_process_batch) over those G graphs bit for bit,
+ *     with its routing (K <= 128 on the one-CTA kernel, larger graphs through the single entry).  A graph refused by
+ *     the pose graph (no refined pair, disconnected, K < 2, ...) gets zeroed poses, weights and masks and map count 0;
+ *     the other graphs are still solved.
+ *   - Independence: graph g's outputs equal a call on sequence g alone (its clouds, its pairs in the same relative
+ *     order, the same tuple_seeds) bit for bit: every stage (FPFH, matching, the solve, ICP, the information matrices,
+ *     the pose graph and the map) computes each cloud, pair and graph independently of the rest of the batch.
+ *   - Refusals: TZR_ERR_INVALID_ARG before any device work, with nothing written, for everything the single entries
+ *     refuse (params->estimate_scaling = 1 included) and for G < 1, off[0] != 0, decreasing offsets,
+ *     off[G] != n_clouds, a pair across two graphs, a NULL pg_status, or a map voxel size that is negative or not
+ *     finite, or positive with a NULL map_points, map_counts, map_points[g] or (with colours) map_colors(g).
+ *   - Returns what the registration returns, as the single entries; TZR_ERR_CUDA or TZR_ERR_ALLOC from the pose-graph
+ *     batch is passed through; otherwise TZR_ERR_TOO_LARGE when a map's grid is too large.  A solve entry:
+ *     tzr_last_inliers and tzr_certify_last_solve see its solve (the pose graph and the map use workspaces of their
+ *     own).
+ *   - Launches: the chain's own, plus 1 (GNC-TLS) or 2 (line process) for the pose graphs of K <= 128, plus 11 for the
+ *     map (one transform launch and the voxel pipeline's 10) when it is made. */
+int tzr_register_cloud_pairs_multiway_batch(
+    tzr_ctx* ctx, const tzr_frontend_params* fparams, const tzr_params* params, int n_clouds, const int32_t* n,
+    const float* const* pts, int P, const int32_t* pair_clouds, const uint64_t* tuple_seeds, tzr_solution* solutions,
+    int32_t* status, int32_t* problem_index, int64_t* n_corr, int32_t* const* corr, int32_t* const* cliques,
+    float* global_scale, const tzr_icp_params* icp, const float* const* colors, double lambda_geometric,
+    const tzr_robust_kernel* kernel, tzr_icp_result* icp_results, const int32_t* uncertain,
+    const tzr_pose_graph_params* pg, double* information, int32_t* info_counts, double* edge_weights,
+    uint8_t* edge_mask, tzr_similarity* poses, tzr_pose_graph_summary* pg_summaries, int32_t* pg_status, int G,
+    const int32_t* graph_offsets, double map_voxel_size, float* const* map_points, int32_t* map_counts,
+    float* const* map_colors);
+int tzr_register_cloud_pairs_multiway_line_process_batch(
+    tzr_ctx* ctx, const tzr_frontend_params* fparams, const tzr_params* params, int n_clouds, const int32_t* n,
+    const float* const* pts, int P, const int32_t* pair_clouds, const uint64_t* tuple_seeds, tzr_solution* solutions,
+    int32_t* status, int32_t* problem_index, int64_t* n_corr, int32_t* const* corr, int32_t* const* cliques,
+    float* global_scale, const tzr_icp_params* icp, const float* const* colors, double lambda_geometric,
+    const tzr_robust_kernel* kernel, tzr_icp_result* icp_results, const int32_t* uncertain,
+    const tzr_line_process_params* lp, double* information, int32_t* info_counts, double* edge_confidence,
+    uint8_t* edge_kept, tzr_similarity* poses, tzr_line_process_summary* lp_summaries, int32_t* lp_status, int G,
+    const int32_t* graph_offsets, double map_voxel_size, float* const* map_points, int32_t* map_counts,
+    float* const* map_colors);
+
 /* ---- downsampling point clouds: voxel-grid averaging ----------------------------------------------------------
  * The first step of the reference's FPFH + TEASER++ + ICP tutorial (voxel_down_sample on both raw scans), for many
  * clouds at once.  Open3D's PointCloud::VoxelDownSample, points only, with a defined order.  Per cloud, all arithmetic

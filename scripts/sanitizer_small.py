@@ -196,5 +196,13 @@ print("line process batch", [r["status"] for r in lpr], [r["trials"] for r in lp
 # the batched GNC-TLS pose graph on the same graphs (one refused)
 pgr = ctx.optimize_pose_graph_batch(lpg, 0.05)
 print("pose graph batch", [r["status"] for r in pgr], [r["inner_iterations"] for r in pgr])
+# many scan sequences in one multiway call with fused maps: two small sequences and one refused (an unsolvable pair)
+mw_seqs = [[ic_src, ic_dst, ic_src[1:]], [ic_dst, ic_src], [ic_src, ic_dst[:2]]]
+for opt in ("gnc_tls", "line_process"):
+    mwr = ctx.register_multiway_batch(mw_seqs, [[(0, 1), (1, 2)], [(0, 1)], [(0, 1)]],
+                                      capi.default_params(noise_bound=0.01, estimate_scaling=0), 0.05,
+                                      normal_search_radius=0.05, fpfh_search_radius=0.1, max_iteration=3,
+                                      optimizer=opt, map_voxel_size=0.05)
+    print("multiway batch", opt, [r[7]["status"] for r in mwr], [len(r[7]["map"]) for r in mwr])
 ctx.close()
 print("DONE")

@@ -265,6 +265,7 @@ _SYMBOLS = [
     "tzr_line_process_params_default", "tzr_pose_graph_optimize_line_process",
     "tzr_pose_graph_optimize_line_process_batch",
     "tzr_register_cloud_pairs_multiway_line_process",
+    "tzr_register_cloud_pairs_multiway_batch", "tzr_register_cloud_pairs_multiway_line_process_batch",
 ]
 
 # status codes (tzr_status)
@@ -480,6 +481,11 @@ def lib():
     L.tzr_register_cloud_pairs_multiway_line_process.argtypes = L.tzr_register_cloud_pairs_icp_colored.argtypes + [
         i32p, C.POINTER(LineProcessParams), dp, i32p, dp, u8p, C.POINTER(Similarity), C.POINTER(LineProcessSummary),
         i32p]
+    mw_batch = [C.c_int, i32p, C.c_double, fpp, i32p, fpp]  # G, graph_offsets and the fused map
+    L.tzr_register_cloud_pairs_multiway_batch.argtypes = L.tzr_register_cloud_pairs_icp_colored.argtypes + \
+        L.tzr_register_cloud_pairs_multiway.argtypes[len(L.tzr_register_cloud_pairs_icp.argtypes):] + mw_batch
+    L.tzr_register_cloud_pairs_multiway_line_process_batch.argtypes = \
+        L.tzr_register_cloud_pairs_multiway_line_process.argtypes + mw_batch
     for s in _SYMBOLS:
         getattr(L, s)  # raises AttributeError if the header and the library disagree
     _lib = L
@@ -731,6 +737,57 @@ class _GraphBatch:
         """G through the per-graph output arrays, in the batched calls' order."""
         return (self.G, _p(self.Ks, C.c_int32), _p(self.Es, C.c_int32), self.ed_p, self.tr_p, self.info_p, self.unc_p,
                 self.init_p, self.pose_p, self.d1_p, self.u8_p, self.d2_p)
+
+
+def multiway_batch_table(sequences, pairs, uncertain=None, tuple_seeds=None, colors=None):
+    """The flat table of register_multiway_batch: clouds, colours, pairs (global cloud indices), uncertain flags and
+    tuple seeds of every sequence back to back, with offsets (the graph offsets, G + 1) and pair_offsets (each
+    sequence's first pair, G + 1)."""
+    G = len(sequences)
+    if G == 0 or len(pairs) != G:
+        raise TzrError("register_multiway_batch: one list of pairs per sequence is required")
+    for name, arg in (("uncertain", uncertain), ("tuple_seeds", tuple_seeds), ("colors", colors)):
+        if arg is not None and len(arg) != G:
+            raise TzrError(f"register_multiway_batch: {name} needs one entry per sequence")
+    clouds, cols, flat, unc, seeds, off, poff = [], [], [], [], [], [0], [0]
+    for g, seq in enumerate(sequences):
+        pc = np.asarray(pairs[g], dtype=np.int64).reshape(-1, 2)
+        if pc.size and (pc.min() < 0 or pc.max() >= len(seq)):
+            raise TzrError(f"register_multiway_batch: a pair of sequence {g} names a cloud that is not in it")
+        u = [0 if b == a + 1 else 1 for a, b in pc] if uncertain is None or uncertain[g] is None else list(uncertain[g])
+        t = [0] * len(pc) if tuple_seeds is None or tuple_seeds[g] is None else [int(x) for x in tuple_seeds[g]]
+        if len(u) != len(pc) or len(t) != len(pc):
+            raise TzrError(f"register_multiway_batch: sequence {g} needs one uncertain flag and tuple seed per pair")
+        if colors is not None and len(colors[g]) != len(seq):
+            raise TzrError(f"register_multiway_batch: sequence {g} needs one colour array per cloud")
+        flat += [(off[-1] + int(a), off[-1] + int(b)) for a, b in pc]
+        unc += u
+        seeds += t
+        clouds += list(seq)
+        cols += [] if colors is None else list(colors[g])
+        off.append(off[-1] + len(seq))
+        poff.append(len(flat))
+    return dict(clouds=clouds, colors=None if colors is None else cols, pairs=np.array(flat, dtype=np.int32).reshape(-1, 2),
+                uncertain=np.array(unc, dtype=np.int32), tuple_seeds=seeds, offsets=np.array(off, dtype=np.int32),
+                pair_offsets=poff)
+
+
+def split_multiway_batch(out, pair_offsets, offsets):
+    """register_multiway_batch's per-sequence results from _register_pairs' output over the flat table: each
+    sequence's slice of every per-pair output, its problem indices counted within the sequence, and its dict (its
+    pairs' rows of the per-pair arrays, its poses, its graph's status, summary and map)."""
+    sols, status, index, corr, clq, gs, icp_res, mw = out
+    res = []
+    for g in range(len(pair_offsets) - 1):
+        a, b = pair_offsets[g], pair_offsets[g + 1]
+        idx = index[a:b].copy()
+        solved = idx >= 0
+        idx[solved] = np.arange(int(solved.sum()), dtype=idx.dtype)
+        d = {k: v[a:b] for k, v in mw.items() if k not in ("poses", "graphs")}
+        d["poses"] = mw["poses"][offsets[g]:offsets[g + 1]]
+        d.update(mw["graphs"][g])
+        res.append((sols[a:b], status[a:b], idx, corr[a:b], clq[a:b], gs[a:b], icp_res[a:b], d))
+    return res
 
 
 class Context:
@@ -1521,7 +1578,10 @@ class Context:
         else:
             icp_res = np.zeros(P, dtype=ICP_RESULT_DTYPE)
             out_res = icp_res.ctypes.data_as(C.POINTER(IcpResult))
-            if multiway is not None:
+            if multiway is not None and len(multiway) == 4:  # (uncertain, params, graph offsets, map voxel size)
+                rc, mw = self._multiway_batch(args, icp, out_res, n, *multiway,
+                                              col_args if colored is not None else None)
+            elif multiway is not None:
                 unc, pg = multiway
                 lp = isinstance(pg, LineProcessParams)
                 unc = np.ascontiguousarray(unc, dtype=np.int32)
@@ -1572,6 +1632,44 @@ class Context:
         if multiway is not None:
             return out + (icp_res, mw)
         return out if icp is None else out + (icp_res,)
+
+    def _multiway_batch(self, args, icp, out_res, n, unc, pg, off, map_voxel_size, col_args):
+        """The many-sequence entries' call over the flat table in args (_register_pairs' arguments) with the graphs at
+        graph offsets off; returns (the entry's return, a dict of the per-pair outputs, poses (n_clouds,4,4) and one
+        dict per graph: status, the summary's keys, and map / map_colors when map_voxel_size > 0)."""
+        P, lp = len(unc), isinstance(pg, LineProcessParams)
+        unc = np.ascontiguousarray(unc, dtype=np.int32)
+        off = np.ascontiguousarray(off, dtype=np.int32)
+        G, vox = len(off) - 1, float(map_voxel_size)
+        info, icnt, ew, em = np.zeros((P, 6, 6)), np.zeros(P, dtype=np.int32), np.zeros(P), np.zeros(P, dtype=np.uint8)
+        poses = (Similarity * len(n))()
+        summ = ((LineProcessSummary if lp else PoseGraphSummary) * max(G, 1))()
+        status, mcnt = np.zeros(max(G, 1), dtype=np.int32), np.zeros(max(G, 1), dtype=np.int32)
+        tot = [int(n[off[g]:off[g + 1]].sum()) for g in range(G)] if vox > 0 and G >= 1 else []
+        maps = [np.zeros((max(t, 1), 3), dtype=np.float32) for t in tot]
+        mcols = [np.zeros((max(t, 1), 3), dtype=np.float32) for t in tot] if col_args is not None else []
+        fp = C.POINTER(C.c_float)
+        entry = lib().tzr_register_cloud_pairs_multiway_line_process_batch if lp else \
+            lib().tzr_register_cloud_pairs_multiway_batch
+        rc = entry(*args, C.byref(icp), *(col_args if col_args is not None else (None, 0.0, None)), out_res,
+                   _p(unc, C.c_int32), C.byref(pg), _p(info, C.c_double), _p(icnt, C.c_int32), _p(ew, C.c_double),
+                   _p(em, C.c_uint8), poses, summ, _p(status, C.c_int32), G, _p(off, C.c_int32), vox,
+                   (fp * len(maps))(*[_p(m, C.c_float) for m in maps]) if maps else None, _p(mcnt, C.c_int32),
+                   (fp * len(mcols))(*[_p(m, C.c_float) for m in mcols]) if mcols else None)
+        graphs = []
+        for g in range(G):
+            d = dict(status=int(status[g]))
+            d.update(_line_process_summary(summ[g]) if lp else
+                     dict(iterations=int(summ[g].iterations), inner_iterations=int(summ[g].inner_iterations),
+                          cost=float(summ[g].cost)))
+            if vox > 0:
+                d["map"] = maps[g][:mcnt[g]].copy()
+                if col_args is not None:
+                    d["map_colors"] = mcols[g][:mcnt[g]].copy()
+            graphs.append(d)
+        mw = dict(information=info, counts=icnt, poses=_poses(poses), graphs=graphs)
+        mw.update(dict(confidence=ew, kept=em.astype(bool)) if lp else dict(weights=ew, mask=em.astype(bool)))
+        return rc, mw
 
     def register_cloud_pairs_fgr(self, clouds, pairs, normal_search_radius=0.03, fpfh_search_radius=0.05,
                                  use_absolute_scale=True, use_crosscheck=True, use_tuple_test=True, tuple_scale=0.0,
@@ -1694,6 +1792,44 @@ class Context:
                                     use_crosscheck, use_tuple_test, tuple_scale, tuple_seeds, icp, plane=True,
                                     kernel=kernel, multiway=(uncertain, pg),
                                     colored=None if colors is None else (colors, float(lambda_geometric)))
+
+    def register_multiway_batch(self, sequences, pairs, params: Params, max_correspondence_distance, uncertain=None,
+                                normal_search_radius=0.03, fpfh_search_radius=0.05, use_absolute_scale=True,
+                                use_crosscheck=True, use_tuple_test=True, tuple_scale=0.0, tuple_seeds=None,
+                                max_iteration=30, relative_fitness=1e-6, relative_rmse=1e-6, pose_graph=None,
+                                colors=None, lambda_geometric=0.968, kernel=None, optimizer="gnc_tls",
+                                line_process=None, map_voxel_size=0.0):
+        """tzr_register_cloud_pairs_multiway(_line_process)_batch: register_multiway over many scan sequences in one
+        call, every sequence's pose graph in the batched pose-graph kernels.  sequences: one list of (n,3) clouds per
+        sequence; pairs: one list of local (s, d) pairs per sequence; uncertain, tuple_seeds and colors: None or one
+        list per sequence (uncertain None: register_multiway's rule per sequence).  The other arguments as
+        register_multiway's.  map_voxel_size > 0 also fuses each solved sequence's clouds into one map (every cloud
+        by its pose, concatenated, voxel-downsampled).  Returns one result per sequence, shaped like
+        register_multiway's: its pairs' seven registration results (problem_index counted within the sequence) plus
+        a dict with its pairs' information, counts, weights and mask (or confidence and kept), its poses, status and
+        summary keys, and map / map_colors when a map was asked for (empty for a refused sequence)."""
+        flat = multiway_batch_table(sequences, pairs, uncertain, tuple_seeds, colors)
+        if optimizer not in ("gnc_tls", "line_process"):
+            raise TzrError(f"register_multiway_batch: unknown optimizer {optimizer!r}")
+        if (optimizer == "line_process" and pose_graph is not None) or (optimizer == "gnc_tls" and
+                                                                        line_process is not None):
+            raise TzrError(f"register_multiway_batch: optimizer={optimizer!r} takes "
+                           f"{'line_process' if optimizer == 'line_process' else 'pose_graph'}, not the other's parameters")
+        kernel = robust_kernel(kernel)
+        if kernel is not None and colors is None:
+            raise TzrError("register_multiway_batch: a robust kernel needs colors (coloured ICP)")
+        if optimizer == "line_process":
+            pg = line_process if line_process is not None else line_process_params(max_correspondence_distance)
+        else:
+            pg = pose_graph if pose_graph is not None else pose_graph_params(max_correspondence_distance)
+        icp = icp_params(max_correspondence_distance, max_iteration=int(max_iteration),
+                         relative_fitness=float(relative_fitness), relative_rmse=float(relative_rmse))
+        out = self._register_pairs(flat["clouds"], flat["pairs"], params, normal_search_radius, fpfh_search_radius,
+                                   use_absolute_scale, use_crosscheck, use_tuple_test, tuple_scale, flat["tuple_seeds"],
+                                   icp, plane=True, kernel=kernel,
+                                   multiway=(flat["uncertain"], pg, flat["offsets"], float(map_voxel_size)),
+                                   colored=None if colors is None else (flat["colors"], float(lambda_geometric)))
+        return split_multiway_batch(out, flat["pair_offsets"], flat["offsets"])
 
     def information_matrix(self, src, dst, transform, max_correspondence_distance):
         """tzr_information_matrix: (Lambda (6,6) float64, count) of the (ns,3) source at transform (see similarity())

@@ -3100,7 +3100,185 @@ struct MultiwayOut {
   // the kept mask)
   const tzr_line_process_params* lp = nullptr;
   tzr_line_process_summary* lp_summary = nullptr;
+  // many sequences in one call (G > 0, checked by multiway_batch_args): the clouds split into graphs at graph_offsets,
+  // pg_status and the summaries G entries each, and the fused map of every solved graph when map_voxel_size > 0
+  int G = 0;
+  const int32_t* graph_offsets = nullptr;
+  double map_voxel_size = 0;
+  float* const* map_points = nullptr;
+  int32_t* map_counts = nullptr;
+  float* const* map_colors = nullptr;
 };
+
+// The call-level checks of the many-sequence entries beyond the single ones', before any device work
+static bool multiway_batch_args(const MultiwayOut& mw, int n_clouds, int P, const int32_t* pair_clouds,
+                                bool with_colors) {
+  const int G = mw.G;
+  const int32_t* off = mw.graph_offsets;
+  if (G < 1 || !off || off[0] != 0 || off[G] != n_clouds || !pair_clouds || P < 1) return false;
+  for (int g = 0; g < G; ++g)
+    if (off[g + 1] < off[g]) return false;
+  auto graph_of = [&](int c) { return (int)(std::upper_bound(off, off + G + 1, c) - off) - 1; };
+  for (int p = 0; p < P; ++p) {
+    const int a = pair_clouds[2 * p], b = pair_clouds[2 * p + 1];
+    if (a < 0 || a >= n_clouds || b < 0 || b >= n_clouds || graph_of(a) != graph_of(b)) return false;
+  }
+  const double v = mw.map_voxel_size;
+  if (!std::isfinite(v) || v < 0) return false;
+  if (v > 0) {
+    if (!mw.map_points || !mw.map_counts || (with_colors && !mw.map_colors)) return false;
+    for (int g = 0; g < G; ++g)
+      if (!mw.map_points[g] || (with_colors && !mw.map_colors[g])) return false;
+  }
+  return true;
+}
+
+// The fused maps of the many-sequence entries (DESIGN.md §3.25): every cloud of every graph with pg_status TZR_OK,
+// transformed by its pose from its points in place (d_pts, d_col: the chain's clouds and colours, cloud c from row
+// clouds[c].lo), concatenated graph by graph and downsampled by launch_voxel with one batch entry per graph.
+// Workspace ctx->vox (so a retained solve stays retained): [points | colours | voxel cloud table | map cloud table |
+// voxels | colour means | voxel_of | scratch]; the pinned area mirrors it up to the colour means.  Returns TZR_OK,
+// TZR_ERR_TOO_LARGE when a graph's grid is too large (its count 0, the others written), or an allocation or CUDA error.
+static int multiway_maps_run(tzr_ctx* ctx, const MultiwayOut& mw, const int32_t* n, const std::vector<FpfhCloud>& clouds,
+                             const float* d_pts, const float* d_col) {
+  const int32_t* off = mw.graph_offsets;
+  std::vector<int> graphs;
+  std::vector<int32_t> gn;
+  std::vector<MapCloud> mc;
+  int rows = 0;  // every map point fits 32-bit indices: they are the chain's own points
+  for (int g = 0; g < mw.G; ++g) {
+    mw.map_counts[g] = 0;
+    if (mw.pg_status[g] != TZR_OK) continue;
+    graphs.push_back(g);
+    gn.push_back(0);
+    for (int c = off[g]; c < off[g + 1]; ++c) {
+      MapCloud m{clouds[c].lo, rows, n[c], 0, {}};
+      const tzr_similarity& x = mw.poses[c];
+      for (int r = 0; r < 3; ++r) {
+        for (int k = 0; k < 3; ++k) m.T[3 * r + k] = x.rotation[3 * k + r];  // column-major rotation
+        m.T[9 + r] = x.translation[r];
+      }
+      mc.push_back(m);
+      rows += n[c];
+      gn.back() += n[c];
+    }
+  }
+  const int B = (int)graphs.size();
+  if (B == 0) return TZR_OK;
+  std::vector<VoxCloud> vc((size_t)B);
+  VoxPlan plan;
+  if (voxel_plan(B, gn.data(), vc.data(), &plan) != TZR_OK) {
+    ctx->last_error = "the maps' points do not fit 32-bit indices";
+    return TZR_ERR_TOO_LARGE;
+  }
+  const size_t N = (size_t)plan.N, pb = N * 12, cb = d_col ? pb : 0, tb = (size_t)B * sizeof(VoxCloud),
+               mb = mc.size() * sizeof(MapCloud);
+  const size_t o_col = al256(pb), o_tab = o_col + al256(cb), o_map = o_tab + al256(tb), o_out = al256(o_map + mb),
+               o_cout = o_out + al256(pb), o_vo = o_cout + al256(cb), o_scr = o_vo + al256(N * 4),
+               total = o_scr + plan.scratch_bytes;
+  cudaStream_t st = ctx->stream;
+  int rc;
+  if ((rc = ensure(ctx, ctx->vox, total)) != TZR_OK) return rc;
+  if ((rc = ensure_pinned(ctx, o_vo)) != TZR_OK) return rc;
+  char* h = (char*)ctx->h_pin;
+  char* d = (char*)ctx->vox.p;
+  memcpy(h + o_tab, vc.data(), tb);
+  memcpy(h + o_map, mc.data(), mb);
+  CK(cudaMemcpyAsync(d + o_tab, h + o_tab, o_map + mb - o_tab, cudaMemcpyHostToDevice, st));
+  float* d_cin = d_col ? (float*)(d + o_col) : nullptr;
+  ctx->launches += launch_map_transform((const MapCloud*)(d + o_map), (int)mc.size(), d_pts, d_col, (float*)d, d_cin,
+                                        st);
+  ctx->launches += launch_voxel(plan, mw.map_voxel_size, (const float*)d, (VoxCloud*)(d + o_tab), d + o_scr,
+                                (float*)(d + o_out), (int*)(d + o_vo), st, d_cin,
+                                d_col ? (float*)(d + o_cout) : nullptr);
+  if ((rc = check_launch(ctx, "map launch")) != TZR_OK) return rc;
+  CK(cudaMemcpyAsync(vc.data(), d + o_tab, tb, cudaMemcpyDeviceToHost, st));
+  CK(cudaStreamSynchronize(st));
+  const size_t out_rows = (size_t)vc[B - 1].out_lo + (size_t)vc[B - 1].n_out;
+  if (out_rows) CK(cudaMemcpyAsync(h + o_out, d + o_out, out_rows * 12, cudaMemcpyDeviceToHost, st));
+  if (out_rows && d_col) CK(cudaMemcpyAsync(h + o_cout, d + o_cout, out_rows * 12, cudaMemcpyDeviceToHost, st));
+  CK(cudaStreamSynchronize(st));
+  std::vector<CopySpan> spans;
+  bool too_large = false;
+  for (int b = 0; b < B; ++b) {
+    const VoxCloud& c = vc[b];
+    const int g = graphs[b];
+    spans.push_back(CopySpan{mw.map_points[g], h + o_out + (size_t)c.out_lo * 12, (size_t)c.n_out * 12});
+    if (d_col) spans.push_back(CopySpan{mw.map_colors[g], h + o_cout + (size_t)c.out_lo * 12, (size_t)c.n_out * 12});
+    mw.map_counts[g] = c.n_out;
+    too_large |= c.status != TZR_OK;
+  }
+  parallel_copy(spans);
+  if (too_large) {
+    ctx->last_error = "a map's voxel grid is too large for the voxel size (Open3D's INT_MAX check or 2^62 cells)";
+    return TZR_ERR_TOO_LARGE;
+  }
+  return TZR_OK;
+}
+
+// The many-sequence tail of register_pairs_run (DESIGN.md §3.25): graph g's edges are the refined pairs among its
+// clouds, in pair order with end points shifted by -off[g], through the pose-graph batch of mw's optimiser; then the
+// weights or confidences and masks scattered back to their pairs, and the fused maps.  The edge list (ends, unc, Tsd,
+// L) is the single tail's, edge e being pair edge_pair[e].  Returns TZR_OK, the pose-graph batch's TZR_ERR_CUDA or
+// TZR_ERR_ALLOC, or the map step's return.
+static int multiway_graphs_run(tzr_ctx* ctx, const MultiwayOut& mw, const int32_t* n,
+                               const std::vector<FpfhCloud>& clouds, const std::vector<int>& edge_pair,
+                               const std::vector<int32_t>& ends, const std::vector<int32_t>& unc,
+                               const std::vector<tzr_similarity>& Tsd, const std::vector<double>& L,
+                               const float* d_pts, const float* d_col) {
+  const int G = mw.G;
+  const int32_t* off = mw.graph_offsets;
+  std::vector<std::vector<int>> eg((size_t)G);  // every graph's edges, ascending
+  for (size_t e = 0; e < edge_pair.size(); ++e)
+    eg[std::upper_bound(off, off + G + 1, ends[2 * e]) - off - 1].push_back((int)e);
+  std::vector<int32_t> K(G), E(G);
+  std::vector<std::vector<int32_t>> ge(G), gu(G);
+  std::vector<std::vector<tzr_similarity>> gT(G);
+  std::vector<std::vector<double>> gL(G), gw(G);
+  std::vector<std::vector<uint8_t>> gm(G);
+  std::vector<const int32_t*> pe(G), pu(G);
+  std::vector<const tzr_similarity*> pT(G);
+  std::vector<const double*> pL(G);
+  std::vector<tzr_similarity*> pose(G);
+  std::vector<double*> pw(G);
+  std::vector<uint8_t*> pm(G);
+  for (int g = 0; g < G; ++g) {
+    K[g] = off[g + 1] - off[g];
+    E[g] = (int)eg[g].size();
+    for (int e : eg[g]) {
+      ge[g].push_back(ends[2 * e] - off[g]);
+      ge[g].push_back(ends[2 * e + 1] - off[g]);
+      gu[g].push_back(unc[e]);
+      gT[g].push_back(Tsd[e]);
+      gL[g].insert(gL[g].end(), L.begin() + (size_t)e * 36, L.begin() + (size_t)(e + 1) * 36);
+    }
+    gw[g].assign(std::max(E[g], 1), 0.0);
+    gm[g].assign(std::max(E[g], 1), 0);
+    pe[g] = ge[g].data();
+    pu[g] = gu[g].data();
+    pT[g] = gT[g].data();
+    pL[g] = gL[g].data();
+    pose[g] = mw.poses + off[g];
+    pw[g] = gw[g].data();
+    pm[g] = gm[g].data();
+  }
+  const int rc = mw.lp ? line_process_batch_run(ctx, mw.lp, G, K.data(), E.data(), pe.data(), pT.data(), pL.data(),
+                                                pu.data(), nullptr, pose.data(), pw.data(), pm.data(), nullptr,
+                                                mw.lp_summary, mw.pg_status)
+                       : pose_graph_batch_run(ctx, mw.pg, G, K.data(), E.data(), pe.data(), pT.data(), pL.data(),
+                                              pu.data(), nullptr, pose.data(), pw.data(), pm.data(), nullptr,
+                                              mw.summary, mw.pg_status);
+  if (rc != TZR_OK) return rc;
+  for (int g = 0; g < G; ++g) {
+    if (mw.pg_status[g] != TZR_OK) continue;
+    for (int j = 0; j < E[g]; ++j) {
+      mw.edge_weights[edge_pair[eg[g][j]]] = gw[g][j];
+      mw.edge_mask[edge_pair[eg[g][j]]] = gm[g][j];
+    }
+  }
+  if (!(mw.map_voxel_size > 0)) return TZR_OK;
+  return multiway_maps_run(ctx, mw, n, clouds, d_pts, d_col);
+}
 
 // FGR (DESIGN.md §3.20): Open3D's FastGlobalRegistrationOption ranges
 static bool fgr_params_ok(const tzr_fgr_params* p) {
@@ -3666,6 +3844,7 @@ static int register_pairs_run(tzr_ctx* ctx, const tzr_frontend_params* fp, const
       ransac_result_of(hi_probs[k], hr[k], &fgr_results[registered[k]],
                        ransac_info ? &ransac_info[registered[k]] : nullptr);
   }
+  bool map_too_large = false;  // the many-sequence entries: a map's grid was too large (tzr_last_error says so)
   if (mw) {  // the pose graph over the refined pairs, in pair order
     memset(mw->information, 0, (size_t)P * 36 * 8);
     memset(mw->info_counts, 0, (size_t)P * 4);
@@ -3691,21 +3870,28 @@ static int register_pairs_run(tzr_ctx* ctx, const tzr_frontend_params* fp, const
     std::vector<uint8_t> m(std::max(E, 1));
     for (int e = 0; e < E; ++e) memcpy(&L[(size_t)e * 36], mw->information + (size_t)edge_pair[e] * 36, 36 * 8);
     const std::string reg_error = ctx->last_error;
-    *mw->pg_status =
-        mw->lp ? line_process_run(ctx, mw->lp, n_clouds, E, ends.data(), Tsd.data(), L.data(), unc.data(), nullptr,
-                                  mw->poses, w.data(), m.data(), nullptr, mw->lp_summary)
-               : pose_graph_run(ctx, mw->pg, n_clouds, E, ends.data(), Tsd.data(), L.data(), unc.data(), nullptr,
-                                mw->poses, w.data(), m.data(), nullptr, mw->summary);
-    if (*mw->pg_status == TZR_OK) {
-      for (int e = 0; e < E; ++e) {
-        mw->edge_weights[edge_pair[e]] = w[e];
-        mw->edge_mask[edge_pair[e]] = m[e];
-      }
+    if (mw->G > 0) {  // many sequences: the pose-graph batch over every graph, then the maps
+      const int mrc = multiway_graphs_run(ctx, *mw, n, clouds, edge_pair, ends, unc, Tsd, L, d_pts,
+                                          colored ? (const float*)(d_in + o_col) : nullptr);
+      if (mrc != TZR_OK && mrc != TZR_ERR_TOO_LARGE) return mrc;
+      map_too_large = mrc == TZR_ERR_TOO_LARGE;
     } else {
-      memset(mw->poses, 0, (size_t)n_clouds * sizeof(tzr_similarity));
-      if (mw->summary) memset(mw->summary, 0, sizeof(*mw->summary));
-      if (mw->lp_summary) memset(mw->lp_summary, 0, sizeof(*mw->lp_summary));
-      if (*mw->pg_status == TZR_ERR_CUDA) return TZR_ERR_CUDA;
+      *mw->pg_status =
+          mw->lp ? line_process_run(ctx, mw->lp, n_clouds, E, ends.data(), Tsd.data(), L.data(), unc.data(), nullptr,
+                                    mw->poses, w.data(), m.data(), nullptr, mw->lp_summary)
+                 : pose_graph_run(ctx, mw->pg, n_clouds, E, ends.data(), Tsd.data(), L.data(), unc.data(), nullptr,
+                                  mw->poses, w.data(), m.data(), nullptr, mw->summary);
+      if (*mw->pg_status == TZR_OK) {
+        for (int e = 0; e < E; ++e) {
+          mw->edge_weights[edge_pair[e]] = w[e];
+          mw->edge_mask[edge_pair[e]] = m[e];
+        }
+      } else {
+        memset(mw->poses, 0, (size_t)n_clouds * sizeof(tzr_similarity));
+        if (mw->summary) memset(mw->summary, 0, sizeof(*mw->summary));
+        if (mw->lp_summary) memset(mw->lp_summary, 0, sizeof(*mw->lp_summary));
+        if (*mw->pg_status == TZR_ERR_CUDA) return TZR_ERR_CUDA;
+      }
     }
     if (no_room || too_large) ctx->last_error = reg_error;
   }
@@ -3718,7 +3904,7 @@ static int register_pairs_run(tzr_ctx* ctx, const tzr_frontend_params* fp, const
                       "exceed the solve's size limit";
     return TZR_ERR_TOO_LARGE;
   }
-  return TZR_OK;
+  return map_too_large ? TZR_ERR_TOO_LARGE : TZR_OK;
 }
 
 int tzr_register_cloud_pairs(tzr_ctx* ctx, const tzr_frontend_params* fp, const tzr_params* params, int n_clouds,
@@ -4674,6 +4860,77 @@ int tzr_register_cloud_pairs_multiway_line_process(
   return register_pairs_run(ctx, fp, params, n_clouds, n, pts, P, pair_clouds, tuple_seeds, solutions, status,
                             problem_index, n_corr, corr, cliques, global_scale, icp, icp_results, kIcpColored, 0,
                             kernel, &mw, colors, lambda_geometric);
+}
+
+// Both many-sequence entries (DESIGN.md §3.25): point-to-plane ICP without colours, coloured ICP with them
+static int multiway_batch_entry(tzr_ctx* ctx, const tzr_frontend_params* fp, const tzr_params* params, int n_clouds,
+                                const int32_t* n, const float* const* pts, int P, const int32_t* pair_clouds,
+                                const uint64_t* tuple_seeds, tzr_solution* solutions, int32_t* status,
+                                int32_t* problem_index, int64_t* n_corr, int32_t* const* corr,
+                                int32_t* const* cliques, float* global_scale, const tzr_icp_params* icp,
+                                const float* const* colors, double lambda_geometric, const tzr_robust_kernel* kernel,
+                                tzr_icp_result* icp_results, const MultiwayOut& mw) {
+  if (!icp || (!colors && kernel)) return TZR_ERR_INVALID_ARG;
+  if (colors && colored_args(&lambda_geometric, kernel) != TZR_OK) return TZR_ERR_INVALID_ARG;
+  if (!multiway_batch_args(mw, n_clouds, P, pair_clouds, colors != nullptr)) {
+    if (ctx)
+      ctx->last_error = "multiway batch: invalid arguments (G >= 1, graph offsets from 0 to n_clouds and not "
+                        "decreasing, every pair inside one graph, the map's voxel size and buffers)";
+    return TZR_ERR_INVALID_ARG;
+  }
+  if (!colors)
+    return register_pairs_run(ctx, fp, params, n_clouds, n, pts, P, pair_clouds, tuple_seeds, solutions, status,
+                              problem_index, n_corr, corr, cliques, global_scale, icp, icp_results, kIcpPointToPlane, 0,
+                              nullptr, &mw);
+  return register_pairs_run(ctx, fp, params, n_clouds, n, pts, P, pair_clouds, tuple_seeds, solutions, status,
+                            problem_index, n_corr, corr, cliques, global_scale, icp, icp_results, kIcpColored, 0,
+                            kernel, &mw, colors, lambda_geometric);
+}
+
+int tzr_register_cloud_pairs_multiway_batch(
+    tzr_ctx* ctx, const tzr_frontend_params* fp, const tzr_params* params, int n_clouds, const int32_t* n,
+    const float* const* pts, int P, const int32_t* pair_clouds, const uint64_t* tuple_seeds, tzr_solution* solutions,
+    int32_t* status, int32_t* problem_index, int64_t* n_corr, int32_t* const* corr, int32_t* const* cliques,
+    float* global_scale, const tzr_icp_params* icp, const float* const* colors, double lambda_geometric,
+    const tzr_robust_kernel* kernel, tzr_icp_result* icp_results, const int32_t* uncertain,
+    const tzr_pose_graph_params* pg, double* information, int32_t* info_counts, double* edge_weights,
+    uint8_t* edge_mask, tzr_similarity* poses, tzr_pose_graph_summary* pg_summaries, int32_t* pg_status, int G,
+    const int32_t* graph_offsets, double map_voxel_size, float* const* map_points, int32_t* map_counts,
+    float* const* map_colors) {
+  MultiwayOut mw{uncertain, pg, information, info_counts, edge_weights, edge_mask, poses, pg_summaries, pg_status};
+  mw.G = G;
+  mw.graph_offsets = graph_offsets;
+  mw.map_voxel_size = map_voxel_size;
+  mw.map_points = map_points;
+  mw.map_counts = map_counts;
+  mw.map_colors = map_colors;
+  return multiway_batch_entry(ctx, fp, params, n_clouds, n, pts, P, pair_clouds, tuple_seeds, solutions, status,
+                              problem_index, n_corr, corr, cliques, global_scale, icp, colors, lambda_geometric, kernel,
+                              icp_results, mw);
+}
+
+int tzr_register_cloud_pairs_multiway_line_process_batch(
+    tzr_ctx* ctx, const tzr_frontend_params* fp, const tzr_params* params, int n_clouds, const int32_t* n,
+    const float* const* pts, int P, const int32_t* pair_clouds, const uint64_t* tuple_seeds, tzr_solution* solutions,
+    int32_t* status, int32_t* problem_index, int64_t* n_corr, int32_t* const* corr, int32_t* const* cliques,
+    float* global_scale, const tzr_icp_params* icp, const float* const* colors, double lambda_geometric,
+    const tzr_robust_kernel* kernel, tzr_icp_result* icp_results, const int32_t* uncertain,
+    const tzr_line_process_params* lp, double* information, int32_t* info_counts, double* edge_confidence,
+    uint8_t* edge_kept, tzr_similarity* poses, tzr_line_process_summary* lp_summaries, int32_t* lp_status, int G,
+    const int32_t* graph_offsets, double map_voxel_size, float* const* map_points, int32_t* map_counts,
+    float* const* map_colors) {
+  MultiwayOut mw{uncertain, nullptr, information, info_counts, edge_confidence, edge_kept, poses, nullptr, lp_status};
+  mw.lp = lp;
+  mw.lp_summary = lp_summaries;
+  mw.G = G;
+  mw.graph_offsets = graph_offsets;
+  mw.map_voxel_size = map_voxel_size;
+  mw.map_points = map_points;
+  mw.map_counts = map_counts;
+  mw.map_colors = map_colors;
+  return multiway_batch_entry(ctx, fp, params, n_clouds, n, pts, P, pair_clouds, tuple_seeds, solutions, status,
+                              problem_index, n_corr, corr, cliques, global_scale, icp, colors, lambda_geometric, kernel,
+                              icp_results, mw);
 }
 
 // tzr_voxel_downsample(_batch): the clouds staged back to back (one H2D copy), the batch's launches (launch_voxel), a

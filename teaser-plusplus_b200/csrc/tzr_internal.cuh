@@ -918,6 +918,16 @@ int voxel_plan(int B, const int32_t* n, VoxCloud* clouds, VoxPlan* plan);
 // each voxel's colour mean, summed like its point.  Returns the launches (10).
 int launch_voxel(const VoxPlan& plan, double voxel_size, const float* pts, VoxCloud* clouds, void* scratch, float* out,
                  int* voxel_of, cudaStream_t st, const float* colors = nullptr, float* colors_out = nullptr);
+// The fused map of many-sequence multiway registration (DESIGN.md §3.25): cloud j's n points at src_lo of pts (and of
+// colors) go to rows dst_lo... of out (and colors_out), each point float(R p + t) in float64 in the order
+// ((R00 x + R01 y) + R02 z) + t0.  T: the pose's rotation (row-major) then its translation.
+struct MapCloud {
+  int src_lo, dst_lo, n, pad;
+  double T[12];
+};
+// One CTA per cloud (clouds: device table); colors and colors_out may be nullptr.  Returns the launches (1).
+int launch_map_transform(const MapCloud* clouds, int n_clouds, const float* pts, const float* colors, float* out,
+                         float* colors_out, cudaStream_t st);
 
 
 }  // namespace tzr

@@ -303,4 +303,33 @@ int launch_voxel(const VoxPlan& plan, double voxel_size, const float* pts, VoxCl
   return 10;
 }
 
+// One CTA per cloud: its points through its pose in float64 (each product and sum rounded on its own, so the result
+// does not depend on contraction), rounded once to float; its colours copied alongside.
+__global__ void __launch_bounds__(256) map_transform_kernel(const MapCloud* __restrict__ clouds,
+                                                            const float* __restrict__ pts,
+                                                            const float* __restrict__ colors, float* __restrict__ out,
+                                                            float* __restrict__ colors_out) {
+  const MapCloud c = clouds[blockIdx.x];
+  for (int i = threadIdx.x; i < c.n; i += blockDim.x) {
+    const size_t s = 3 * ((size_t)c.src_lo + i), d = 3 * ((size_t)c.dst_lo + i);
+    const double x = pts[s], y = pts[s + 1], z = pts[s + 2];
+#pragma unroll
+    for (int r = 0; r < 3; ++r)
+      out[d + r] = (float)__dadd_rn(
+          __dadd_rn(__dadd_rn(__dmul_rn(c.T[3 * r], x), __dmul_rn(c.T[3 * r + 1], y)), __dmul_rn(c.T[3 * r + 2], z)),
+          c.T[9 + r]);
+    if (colors) {
+      colors_out[d] = colors[s];
+      colors_out[d + 1] = colors[s + 1];
+      colors_out[d + 2] = colors[s + 2];
+    }
+  }
+}
+
+int launch_map_transform(const MapCloud* clouds, int n_clouds, const float* pts, const float* colors, float* out,
+                         float* colors_out, cudaStream_t st) {
+  map_transform_kernel<<<n_clouds, 256, 0, st>>>(clouds, pts, colors, out, colors_out);
+  return 1;
+}
+
 }  // namespace tzr

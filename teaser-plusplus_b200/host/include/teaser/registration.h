@@ -443,6 +443,10 @@ class RobustRegistrationSolver {
     int inner_iterations = 0;
     double cost = 0;
     LineProcessSummary line_process;  // the line-process overloads: their summary (iterations and cost stay 0)
+    // solveMultiwayBatch with map_voxel_size > 0: the fused map (every cloud by its pose, concatenated and
+    // voxel-downsampled) and, with colours, its colours; empty for a sequence whose pose graph was refused
+    PointCloud map;
+    ColorCloud map_colors;
   };
   MultiwayResult solveMultiway(const std::vector<PointCloud>& clouds, const std::vector<std::pair<int, int>>& pairs,
                                const CloudPairParams& params, const PointToPointICPParams& icp,
@@ -477,6 +481,30 @@ class RobustRegistrationSolver {
                                const std::vector<std::pair<int, int>>& pairs, const CloudPairParams& params,
                                const ColoredICPParams& icp, const LineProcessParams& global_optimization,
                                const std::vector<bool>& uncertain, const RobustKernel& kernel = RobustKernel());
+  // Many scan sequences in one call (tzr_register_cloud_pairs_multiway(_line_process)_batch, DESIGN.md §3.25): every
+  // sequence's pairs in one cloud-pair pass, every pose graph in the batched pose-graph kernels and, with
+  // map_voxel_size > 0, each solved sequence's fused map.  A sequence holds its clouds, their colours (empty: point-to-
+  // plane ICP; either every sequence of a call has colours, refined by coloured ICP with icp.lambda_geometric and
+  // kernel, or none has and kernel must be L2), its pairs (indices into its own clouds) and their uncertain flags
+  // (empty: Open3D's tutorial rule).  Pair j of a sequence gets the tuple seed params.tuple_seed + 0x9E3779B97F4A7C15 j,
+  // as in solveMultiway on that sequence alone.  Returns one MultiwayResult per sequence, its poses in its own frame;
+  // every output equals solveMultiway on the sequence alone except that the pose graph of at most 128 nodes runs on
+  // the batched kernels (the same decisions; poses within rounding).
+  struct MultiwaySequence {
+    std::vector<PointCloud> clouds;
+    std::vector<ColorCloud> colors;
+    std::vector<std::pair<int, int>> pairs;
+    std::vector<bool> uncertain;
+  };
+  std::vector<MultiwayResult> solveMultiwayBatch(const std::vector<MultiwaySequence>& sequences,
+                                                 const CloudPairParams& params, const ColoredICPParams& icp,
+                                                 const PoseGraphParams& pose_graph, double map_voxel_size = 0,
+                                                 const RobustKernel& kernel = RobustKernel());
+  std::vector<MultiwayResult> solveMultiwayBatch(const std::vector<MultiwaySequence>& sequences,
+                                                 const CloudPairParams& params, const ColoredICPParams& icp,
+                                                 const LineProcessParams& global_optimization,
+                                                 double map_voxel_size = 0,
+                                                 const RobustKernel& kernel = RobustKernel());
   bool isMaxCliqueProvenOptimal() const { return clique_proven_; }
   long long getNumInlierGraphEdges() const { return n_edges_; }
   int getGNCRotationIterations() const { return gnc_iterations_; }

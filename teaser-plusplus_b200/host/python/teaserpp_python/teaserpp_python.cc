@@ -363,6 +363,24 @@ py::dict multiscale_run(const teaser::MultiScaleICP& icp, const std::vector<Clou
   return multiscale_dict(r);
 }
 
+// solve_multiway's result dict, and each of solve_multiway_batch's (lp: the line process's summary is added)
+py::dict multiway_dict(const teaser::RobustRegistrationSolver::MultiwayResult& r, bool lp) {
+  py::list pair_out, info, poses;
+  for (const auto& q : r.pairs)
+    pair_out.append(py::dict(py::arg("status") = q.status, py::arg("solution") = q.solution,
+                             py::arg("refined") = q.refined,
+                             py::arg("icp") = q.refined ? py::object(icp_dict(q.icp)) : py::object(py::none())));
+  for (const auto& M : r.information) info.append(square_to_numpy<6>(M));
+  for (const auto& T : r.poses) poses.append(square_to_numpy<4>(T));
+  py::dict out(py::arg("pairs") = pair_out, py::arg("information") = info,
+               py::arg("information_counts") = r.information_counts, py::arg("edge_weights") = r.edge_weights,
+               py::arg("edge_inliers") = r.edge_inliers, py::arg("poses") = poses,
+               py::arg("pose_graph_status") = r.pose_graph_status, py::arg("iterations") = r.iterations,
+               py::arg("inner_iterations") = r.inner_iterations, py::arg("cost") = r.cost);
+  if (lp) out["line_process"] = line_process_dict(r.line_process);
+  return out;
+}
+
 }  // namespace
 
 PYBIND11_MODULE(_teaserpp, m) {
@@ -1340,21 +1358,7 @@ PYBIND11_MODULE(_teaserpp, m) {
                 r = given ? s.solveMultiway(pcs, pairs, cp, ip, pg, unc) : s.solveMultiway(pcs, pairs, cp, ip, pg);
               }
             }
-            py::list pair_out, info, poses;
-            for (const auto& q : r.pairs)
-              pair_out.append(py::dict(py::arg("status") = q.status, py::arg("solution") = q.solution,
-                                       py::arg("refined") = q.refined,
-                                       py::arg("icp") = q.refined ? py::object(icp_dict(q.icp)) : py::object(py::none())));
-            for (const auto& M : r.information) info.append(square_to_numpy<6>(M));
-            for (const auto& T : r.poses) poses.append(square_to_numpy<4>(T));
-            py::dict out(py::arg("pairs") = pair_out, py::arg("information") = info,
-                         py::arg("information_counts") = r.information_counts,
-                         py::arg("edge_weights") = r.edge_weights, py::arg("edge_inliers") = r.edge_inliers,
-                         py::arg("poses") = poses, py::arg("pose_graph_status") = r.pose_graph_status,
-                         py::arg("iterations") = r.iterations, py::arg("inner_iterations") = r.inner_iterations,
-                         py::arg("cost") = r.cost);
-            if (lp) out["line_process"] = line_process_dict(r.line_process);
-            return out;
+            return multiway_dict(r, lp);
           },
           py::arg("clouds"), py::arg("pairs"), py::arg("max_correspondence_distance"), py::arg("uncertain") = py::none(),
           py::arg("max_iteration") = 30, py::arg("relative_fitness") = 1e-6, py::arg("relative_rmse") = 1e-6,
@@ -1364,6 +1368,106 @@ PYBIND11_MODULE(_teaserpp, m) {
           py::arg("cost_threshold") = 1e-6, py::arg("max_iterations") = 100, py::arg("max_inner_iterations") = 10,
           py::arg("reference_node") = 0, py::arg("colors") = py::none(), py::arg("lambda_geometric") = 0.968,
           py::arg("kernel") = py::none(), py::arg("global_optimization") = py::none())
+      .def(
+          "solve_multiway_batch",
+          [](Solver& s, const std::vector<std::vector<CloudArray>>& sequences,
+             const std::vector<std::vector<std::pair<int, int>>>& pairs, double max_correspondence_distance,
+             const py::object& uncertain, int max_iteration, double relative_fitness, double relative_rmse,
+             double normal_search_radius, double fpfh_search_radius, bool use_absolute_scale, bool use_crosscheck,
+             bool use_tuple_test, float tuple_scale, uint64_t tuple_seed, double gnc_factor, double cost_threshold,
+             int max_iterations, int max_inner_iterations, int reference_node, const py::object& colors,
+             double lambda_geometric, const py::object& kernel, const py::object& global_optimization,
+             double map_voxel_size) {
+            // GPU extra: solve_multiway over many scan sequences in one call (solveMultiwayBatch).  sequences: one
+            // list of (n,3) clouds per sequence; pairs, uncertain (None or one list or None per sequence) and colors
+            // (None, or one list of (n,3) arrays per sequence) likewise.  Returns one solve_multiway dict per
+            // sequence, plus map (and map_colors with colours) when map_voxel_size > 0.
+            if (pairs.size() != sequences.size())
+              throw std::invalid_argument("one list of pairs per sequence is required");
+            if (!kernel.is_none() && colors.is_none())
+              throw std::invalid_argument("a robust kernel needs colors (coloured ICP)");
+            const teaser::RobustKernel rk = kernel.is_none() ? teaser::RobustKernel() : kernel.cast<teaser::RobustKernel>();
+            const auto unc = uncertain.is_none() ? py::list() : uncertain.cast<py::list>();
+            const auto cols = colors.is_none() ? std::vector<std::vector<CloudArray>>()
+                                               : colors.cast<std::vector<std::vector<CloudArray>>>();
+            if ((!uncertain.is_none() && unc.size() != sequences.size()) ||
+                (!colors.is_none() && cols.size() != sequences.size()))
+              throw std::invalid_argument("uncertain and colors need one entry per sequence");
+            std::vector<Solver::MultiwaySequence> seqs(sequences.size());
+            for (size_t g = 0; g < seqs.size(); ++g) {
+              for (const auto& a : sequences[g]) seqs[g].clouds.push_back(cloud_of(a));
+              if (!colors.is_none())
+                for (const auto& a : cols[g]) seqs[g].colors.push_back(colors_of(a));
+              seqs[g].pairs = pairs[g];
+              if (!uncertain.is_none() && !unc[g].is_none()) seqs[g].uncertain = unc[g].cast<std::vector<bool>>();
+            }
+            Solver::CloudPairParams cp;
+            cp.normal_search_radius = normal_search_radius;
+            cp.fpfh_search_radius = fpfh_search_radius;
+            cp.use_absolute_scale = use_absolute_scale;
+            cp.use_crosscheck = use_crosscheck;
+            cp.use_tuple_test = use_tuple_test;
+            cp.tuple_scale = tuple_scale;
+            cp.tuple_seed = tuple_seed;
+            teaser::ColoredICPParams cip;
+            cip.max_correspondence_distance = max_correspondence_distance;
+            cip.max_iteration = max_iteration;
+            cip.relative_fitness = relative_fitness;
+            cip.relative_rmse = relative_rmse;
+            cip.lambda_geometric = lambda_geometric;
+            teaser::PoseGraphParams pg;
+            pg.max_correspondence_distance = max_correspondence_distance;
+            pg.gnc_factor = gnc_factor;
+            pg.cost_threshold = cost_threshold;
+            pg.max_iterations = max_iterations;
+            pg.max_inner_iterations = max_inner_iterations;
+            pg.reference_node = reference_node;
+            const bool lp = !global_optimization.is_none();
+            if (lp && (gnc_factor != 1.4 || cost_threshold != 1e-6 || max_iterations != 100 ||
+                       max_inner_iterations != 10 || reference_node != 0))
+              throw std::invalid_argument("the GNC-TLS arguments do not apply with global_optimization");
+            std::vector<Solver::MultiwayResult> rs;
+            {
+              py::gil_scoped_release release;
+              rs = lp ? s.solveMultiwayBatch(
+                            seqs, cp, cip, global_optimization.cast<const teaser::GlobalOptimization&>().getParams(),
+                            map_voxel_size, rk)
+                      : s.solveMultiwayBatch(seqs, cp, cip, pg, map_voxel_size, rk);
+            }
+            py::list out;
+            for (const auto& r : rs) {
+              py::dict d = multiway_dict(r, lp);
+              if (map_voxel_size > 0) {
+                py::array_t<float> mp({static_cast<py::ssize_t>(r.map.size()), static_cast<py::ssize_t>(3)});
+                for (size_t i = 0; i < r.map.size(); ++i) {
+                  mp.mutable_at(i, 0) = r.map[i].x;
+                  mp.mutable_at(i, 1) = r.map[i].y;
+                  mp.mutable_at(i, 2) = r.map[i].z;
+                }
+                d["map"] = mp;
+                if (!colors.is_none()) {
+                  py::array_t<float> mc({static_cast<py::ssize_t>(r.map_colors.size()), static_cast<py::ssize_t>(3)});
+                  for (size_t i = 0; i < r.map_colors.size(); ++i) {
+                    mc.mutable_at(i, 0) = r.map_colors[i].r;
+                    mc.mutable_at(i, 1) = r.map_colors[i].g;
+                    mc.mutable_at(i, 2) = r.map_colors[i].b;
+                  }
+                  d["map_colors"] = mc;
+                }
+              }
+              out.append(d);
+            }
+            return out;
+          },
+          py::arg("sequences"), py::arg("pairs"), py::arg("max_correspondence_distance"),
+          py::arg("uncertain") = py::none(), py::arg("max_iteration") = 30, py::arg("relative_fitness") = 1e-6,
+          py::arg("relative_rmse") = 1e-6, py::arg("normal_search_radius") = 0.03,
+          py::arg("fpfh_search_radius") = 0.05, py::arg("use_absolute_scale") = true,
+          py::arg("use_crosscheck") = true, py::arg("use_tuple_test") = true, py::arg("tuple_scale") = 0.0f,
+          py::arg("tuple_seed") = 0x7ea5e2ull, py::arg("gnc_factor") = 1.4, py::arg("cost_threshold") = 1e-6,
+          py::arg("max_iterations") = 100, py::arg("max_inner_iterations") = 10, py::arg("reference_node") = 0,
+          py::arg("colors") = py::none(), py::arg("lambda_geometric") = 0.968, py::arg("kernel") = py::none(),
+          py::arg("global_optimization") = py::none(), py::arg("map_voxel_size") = 0.0)
       .def_property_readonly("solution", &Solver::getSolution)
       .def("getSolution", &Solver::getSolution)
       .def_property_readonly("gnc_rotation_cost_at_termination", &Solver::getGNCRotationCostAtTermination)

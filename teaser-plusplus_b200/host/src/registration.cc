@@ -649,13 +649,22 @@ struct MultiwayCall {
   int32_t* pg_status;
   const tzr_line_process_params* lp = nullptr;  // the line process in place of GNC-TLS (pg unused)
   tzr_line_process_summary* lp_summary = nullptr;
+  // solveMultiwayBatch (tzr_register_cloud_pairs_multiway(_line_process)_batch): G > 0 graphs at graph_offsets, the
+  // summaries and pg_status G entries each, and the fused maps
+  int G = 0;
+  const int32_t* graph_offsets = nullptr;
+  double map_voxel_size = 0;
+  float* const* map_points = nullptr;
+  int32_t* map_counts = nullptr;
+  float* const* map_colors = nullptr;
 };
 std::vector<RobustRegistrationSolver::CloudPairResult> run_cloud_pairs(
     const tzr_params& p, const std::vector<PointCloud>& clouds, const std::vector<std::pair<int, int>>& pairs,
     const RobustRegistrationSolver::CloudPairParams& cp, const tzr_icp_params* icp,
     std::vector<tzr_icp_result>* icp_res, IcpMethod method = IcpMethod::kPointToPoint, double epsilon = 0,
     const RobustKernel* kernel = nullptr, const MultiwayCall* mw = nullptr,
-    const std::vector<ColorCloud>* colors = nullptr, double lambda_geometric = 0) {
+    const std::vector<ColorCloud>* colors = nullptr, double lambda_geometric = 0,
+    const std::vector<uint64_t>* tuple_seeds = nullptr) {
   using CloudPairResult = RobustRegistrationSolver::CloudPairResult;
   const int K = static_cast<int>(clouds.size()), P = static_cast<int>(pairs.size());
   std::vector<CloudPairResult> out(P);
@@ -686,7 +695,7 @@ std::vector<RobustRegistrationSolver::CloudPairResult> run_cloud_pairs(
     if (a < 0 || a >= K || b < 0 || b >= K) throw std::invalid_argument("teaser: solveCloudPairs: no such cloud");
     pc[2 * p] = a;
     pc[2 * p + 1] = b;
-    seeds[p] = cp.tuple_seed + 0x9E3779B97F4A7C15ull * static_cast<uint64_t>(p);
+    seeds[p] = tuple_seeds ? (*tuple_seeds)[p] : cp.tuple_seed + 0x9E3779B97F4A7C15ull * static_cast<uint64_t>(p);
     const size_t cap = static_cast<size_t>(n[a]) + n[b];
     corr[p].resize(2 * cap);
     clq[p].resize(cap);
@@ -718,7 +727,24 @@ std::vector<RobustRegistrationSolver::CloudPairResult> run_cloud_pairs(
       k.type = static_cast<int32_t>(kernel->type);
       k.k = kernel->k;
     }
-    if (mw && mw->lp) {
+    if (mw && mw->G > 0) {
+      const bool colored = method == IcpMethod::kColored;
+      const float* const* cl = colored ? col.data() : nullptr;
+      const double lam = colored ? lambda_geometric : 0.0;
+      const tzr_robust_kernel* kp = colored && kernel ? &k : nullptr;
+      rc = mw->lp ? tzr_register_cloud_pairs_multiway_line_process_batch(
+                        ctx, &f, &p, K, n.data(), pts.data(), P, pc.data(), seeds.data(), sols.data(), status.data(),
+                        index.data(), n_corr.data(), corr_p.data(), clq_p.data(), scales.data(), icp, cl, lam, kp,
+                        icp_res->data(), mw->uncertain, mw->lp, mw->information, mw->info_counts, mw->edge_weights,
+                        mw->edge_mask, mw->poses, mw->lp_summary, mw->pg_status, mw->G, mw->graph_offsets,
+                        mw->map_voxel_size, mw->map_points, mw->map_counts, mw->map_colors)
+                  : tzr_register_cloud_pairs_multiway_batch(
+                        ctx, &f, &p, K, n.data(), pts.data(), P, pc.data(), seeds.data(), sols.data(), status.data(),
+                        index.data(), n_corr.data(), corr_p.data(), clq_p.data(), scales.data(), icp, cl, lam, kp,
+                        icp_res->data(), mw->uncertain, mw->pg, mw->information, mw->info_counts, mw->edge_weights,
+                        mw->edge_mask, mw->poses, mw->summary, mw->pg_status, mw->G, mw->graph_offsets,
+                        mw->map_voxel_size, mw->map_points, mw->map_counts, mw->map_colors);
+    } else if (mw && mw->lp) {
       const bool colored = method == IcpMethod::kColored;
       rc = tzr_register_cloud_pairs_multiway_line_process(
           ctx, &f, &p, K, n.data(), pts.data(), P, pc.data(), seeds.data(), sols.data(), status.data(), index.data(),
@@ -817,6 +843,54 @@ static std::vector<bool> tutorial_uncertain(const std::vector<std::pair<int, int
   return uncertain;
 }
 
+// One sequence's MultiwayResult from the multiway outputs: its P pairs from pair q0 of base, res and the per-pair
+// arrays, its K poses from poses, its status and summaries
+static RobustRegistrationSolver::MultiwayResult multiway_result(
+    std::vector<RobustRegistrationSolver::CloudPairResult>& base, const std::vector<tzr_icp_result>& res,
+    const double* info, const int32_t* counts, const double* w, const uint8_t* mask, size_t q0, size_t P,
+    const tzr_similarity* poses, size_t K, int32_t pg_status, const tzr_pose_graph_summary& summary,
+    const tzr_line_process_summary& lp_summary) {
+  using CloudPairResult = RobustRegistrationSolver::CloudPairResult;
+  RobustRegistrationSolver::MultiwayResult out;
+  out.pairs.resize(P);
+  out.information.resize(P);
+  out.information_counts.assign(counts + q0, counts + q0 + P);
+  out.edge_weights.assign(w + q0, w + q0 + P);
+  out.edge_inliers.resize(P);
+  for (size_t j = 0; j < P; ++j) {
+    const size_t q = q0 + j;
+    static_cast<CloudPairResult&>(out.pairs[j]) = std::move(base[q]);
+    out.pairs[j].refined = out.pairs[j].status == TZR_OK && out.pairs[j].solution.valid && res[q].transform.scale > 0;
+    if (out.pairs[j].refined) icp_result_from_c(res[q], nullptr, &out.pairs[j].icp);
+    for (int r = 0; r < 6; ++r)
+      for (int c = 0; c < 6; ++c) out.information[j](r, c) = info[36 * q + 6 * r + c];
+    out.edge_inliers[j] = mask[q] != 0;
+  }
+  out.poses.resize(K);
+  for (size_t k = 0; k < K; ++k) {
+    Eigen::Matrix4d T = Eigen::Matrix4d::Zero();
+    for (int r = 0; r < 3; ++r) {
+      for (int c = 0; c < 3; ++c) T(r, c) = poses[k].rotation[3 * c + r];
+      T(r, 3) = poses[k].translation[r];
+    }
+    T(3, 3) = 1.0;
+    out.poses[k] = T;
+  }
+  out.pose_graph_status = pg_status;
+  out.iterations = summary.iterations;
+  out.inner_iterations = summary.inner_iterations;
+  out.cost = summary.cost;
+  for (int q = 0; q < 2; ++q) {
+    out.line_process.iterations[q] = lp_summary.iterations[q];
+    out.line_process.trials[q] = lp_summary.trials[q];
+    out.line_process.stop_reason[q] = lp_summary.stop_reason[q];
+    out.line_process.mu[q] = lp_summary.mu[q];
+  }
+  out.line_process.pruned = lp_summary.pruned;
+  out.line_process.residual = lp_summary.residual;
+  return out;
+}
+
 // every solveMultiway overload: point-to-plane without colours, coloured ICP with them
 static RobustRegistrationSolver::MultiwayResult run_multiway(
     const tzr_params& p, const std::vector<PointCloud>& clouds, const std::vector<std::pair<int, int>>& pairs,
@@ -854,43 +928,117 @@ static RobustRegistrationSolver::MultiwayResult run_multiway(
   std::vector<CloudPairResult> base =
       run_cloud_pairs(p, clouds, pairs, cp, &ip, &res, colors ? IcpMethod::kColored : IcpMethod::kPointToPlane, 0,
                       kernel, &mw, colors, lambda_geometric);
-  RobustRegistrationSolver::MultiwayResult out;
-  out.pairs.resize(P);
-  out.information.resize(P);
-  out.information_counts.assign(counts.begin(), counts.end());
-  out.edge_weights = w;
-  out.edge_inliers.resize(P);
-  for (size_t q = 0; q < P; ++q) {
-    static_cast<CloudPairResult&>(out.pairs[q]) = std::move(base[q]);
-    out.pairs[q].refined = out.pairs[q].status == TZR_OK && out.pairs[q].solution.valid && res[q].transform.scale > 0;
-    if (out.pairs[q].refined) icp_result_from_c(res[q], nullptr, &out.pairs[q].icp);
-    for (int r = 0; r < 6; ++r)
-      for (int c = 0; c < 6; ++c) out.information[q](r, c) = info[36 * q + 6 * r + c];
-    out.edge_inliers[q] = mask[q] != 0;
-  }
-  out.poses.resize(K);
-  for (size_t k = 0; k < K; ++k) {
-    Eigen::Matrix4d T = Eigen::Matrix4d::Zero();
-    for (int r = 0; r < 3; ++r) {
-      for (int c = 0; c < 3; ++c) T(r, c) = poses[k].rotation[3 * c + r];
-      T(r, 3) = poses[k].translation[r];
+  return multiway_result(base, res, info.data(), counts.data(), w.data(), mask.data(), 0, P, poses.data(), K, pg_status,
+                         summary, lp_summary);
+}
+
+// both solveMultiwayBatch overloads: the sequences flattened into one table (pair j of a sequence keeps its solo tuple
+// seed), one call, the outputs split back per sequence
+static std::vector<RobustRegistrationSolver::MultiwayResult> run_multiway_batch(
+    const tzr_params& p, const std::vector<RobustRegistrationSolver::MultiwaySequence>& seqs,
+    const RobustRegistrationSolver::CloudPairParams& cp, const ColoredICPParams& icp, const PoseGraphParams& pose_graph,
+    const LineProcessParams* line_process, double map_voxel_size, const RobustKernel& kernel) {
+  using CloudPairResult = RobustRegistrationSolver::CloudPairResult;
+  const size_t G = seqs.size();
+  if (G == 0) throw std::invalid_argument("teaser: solveMultiwayBatch: at least one sequence is required");
+  const bool colored = !seqs[0].colors.empty();
+  if (!colored && kernel.type != RobustKernel::kL2)
+    throw std::invalid_argument("teaser: solveMultiwayBatch: a robust kernel needs colours (coloured ICP)");
+  std::vector<PointCloud> clouds;
+  std::vector<ColorCloud> colors;
+  std::vector<std::pair<int, int>> pairs;
+  std::vector<int32_t> unc, off{0};
+  std::vector<uint64_t> seeds;
+  std::vector<size_t> pair_off{0}, points(G, 0);
+  for (size_t g = 0; g < G; ++g) {
+    const auto& s = seqs[g];
+    if (s.colors.empty() == colored)
+      throw std::invalid_argument("teaser: solveMultiwayBatch: every sequence has colours, or none has");
+    if (!s.uncertain.empty() && s.uncertain.size() != s.pairs.size())
+      throw std::invalid_argument("teaser: solveMultiwayBatch: one uncertain flag per pair");
+    const int K = static_cast<int>(s.clouds.size());
+    for (size_t j = 0; j < s.pairs.size(); ++j) {
+      const auto& q = s.pairs[j];
+      if (q.first < 0 || q.first >= K || q.second < 0 || q.second >= K)
+        throw std::invalid_argument("teaser: solveMultiwayBatch: a pair names a cloud outside its sequence");
+      pairs.emplace_back(off.back() + q.first, off.back() + q.second);
+      unc.push_back(s.uncertain.empty() ? (q.second != q.first + 1) : s.uncertain[j]);
+      seeds.push_back(cp.tuple_seed + 0x9E3779B97F4A7C15ull * static_cast<uint64_t>(j));
     }
-    T(3, 3) = 1.0;
-    out.poses[k] = T;
+    for (const auto& c : s.clouds) points[g] += c.size();
+    clouds.insert(clouds.end(), s.clouds.begin(), s.clouds.end());
+    colors.insert(colors.end(), s.colors.begin(), s.colors.end());
+    off.push_back(off.back() + K);
+    pair_off.push_back(pairs.size());
   }
-  out.pose_graph_status = pg_status;
-  out.iterations = summary.iterations;
-  out.inner_iterations = summary.inner_iterations;
-  out.cost = summary.cost;
-  for (int q = 0; q < 2; ++q) {
-    out.line_process.iterations[q] = lp_summary.iterations[q];
-    out.line_process.trials[q] = lp_summary.trials[q];
-    out.line_process.stop_reason[q] = lp_summary.stop_reason[q];
-    out.line_process.mu[q] = lp_summary.mu[q];
+  const size_t P = pairs.size(), K = clouds.size();
+  tzr_icp_params ip;
+  tzr_icp_params_default(&ip);
+  ip.max_correspondence_distance = icp.max_correspondence_distance;
+  ip.max_iteration = icp.max_iteration;
+  ip.relative_fitness = icp.relative_fitness;
+  ip.relative_rmse = icp.relative_rmse;
+  tzr_pose_graph_params pg = pose_graph_c(pose_graph);
+  std::vector<int32_t> counts(P), status(G), map_counts(G);
+  std::vector<double> info(P * 36), w(P);
+  std::vector<uint8_t> mask(P);
+  std::vector<tzr_similarity> poses(K);
+  std::vector<tzr_pose_graph_summary> summary(G);
+  std::vector<tzr_line_process_summary> lp_summary(G);
+  std::vector<std::vector<float>> maps(G), map_cols(G);
+  std::vector<float*> map_p(G), map_c(G);
+  const bool with_map = map_voxel_size > 0;
+  for (size_t g = 0; g < G && with_map; ++g) {
+    maps[g].resize(3 * std::max<size_t>(points[g], 1));
+    map_p[g] = maps[g].data();
+    if (colored) {
+      map_cols[g].resize(maps[g].size());
+      map_c[g] = map_cols[g].data();
+    }
   }
-  out.line_process.pruned = lp_summary.pruned;
-  out.line_process.residual = lp_summary.residual;
+  MultiwayCall mw{unc.data(), &pg, info.data(), counts.data(), w.data(), mask.data(), poses.data(), summary.data(),
+                  status.data()};
+  tzr_line_process_params lp;
+  if (line_process) {
+    lp = line_process_c(*line_process);
+    mw.lp = &lp;
+    mw.lp_summary = lp_summary.data();
+  }
+  mw.G = static_cast<int>(G);
+  mw.graph_offsets = off.data();
+  mw.map_voxel_size = map_voxel_size;
+  mw.map_points = with_map ? map_p.data() : nullptr;
+  mw.map_counts = with_map ? map_counts.data() : nullptr;
+  mw.map_colors = with_map && colored ? map_c.data() : nullptr;
+  std::vector<tzr_icp_result> res;
+  std::vector<CloudPairResult> base =
+      run_cloud_pairs(p, clouds, pairs, cp, &ip, &res, colored ? IcpMethod::kColored : IcpMethod::kPointToPlane, 0,
+                      colored ? &kernel : nullptr, &mw, colored ? &colors : nullptr, icp.lambda_geometric, &seeds);
+  std::vector<RobustRegistrationSolver::MultiwayResult> out;
+  for (size_t g = 0; g < G; ++g) {
+    out.push_back(multiway_result(base, res, info.data(), counts.data(), w.data(), mask.data(), pair_off[g],
+                                  pair_off[g + 1] - pair_off[g], poses.data() + off[g], off[g + 1] - off[g], status[g],
+                                  summary[g], lp_summary[g]));
+    for (int32_t r = 0; with_map && r < map_counts[g]; ++r) {
+      out.back().map.push_back(PointXYZ{maps[g][3 * r], maps[g][3 * r + 1], maps[g][3 * r + 2]});
+      if (colored) out.back().map_colors.push_back(ColorRGB{map_cols[g][3 * r], map_cols[g][3 * r + 1],
+                                                            map_cols[g][3 * r + 2]});
+    }
+  }
   return out;
+}
+
+std::vector<RobustRegistrationSolver::MultiwayResult> RobustRegistrationSolver::solveMultiwayBatch(
+    const std::vector<MultiwaySequence>& sequences, const CloudPairParams& cp, const ColoredICPParams& icp,
+    const PoseGraphParams& pose_graph, double map_voxel_size, const RobustKernel& kernel) {
+  return run_multiway_batch(to_c(params_), sequences, cp, icp, pose_graph, nullptr, map_voxel_size, kernel);
+}
+
+std::vector<RobustRegistrationSolver::MultiwayResult> RobustRegistrationSolver::solveMultiwayBatch(
+    const std::vector<MultiwaySequence>& sequences, const CloudPairParams& cp, const ColoredICPParams& icp,
+    const LineProcessParams& global_optimization, double map_voxel_size, const RobustKernel& kernel) {
+  return run_multiway_batch(to_c(params_), sequences, cp, icp, PoseGraphParams(), &global_optimization,
+                            map_voxel_size, kernel);
 }
 
 RobustRegistrationSolver::MultiwayResult RobustRegistrationSolver::solveMultiway(
