@@ -1468,6 +1468,23 @@ int tzr_pose_graph_optimize_line_process_batch(
     double* const* confidence, uint8_t* const* kept, double* const* residuals, tzr_line_process_summary* summaries,
     int32_t* status);
 
+/* The factorisation and solve of both batched pose-graph routes (tzr_pose_graph_optimize_batch,
+ * tzr_pose_graph_optimize_line_process_batch) on given matrices, for tests and diagnostics (DESIGN.md §3.23).  G >= 1
+ * matrices; A[g] is n[g] x n[g] column-major (only its lower triangle is read), b[g] has n[g] entries.  One kernel
+ * launch runs every matrix in one CTA, with those kernels' shared memory and panel stride (the largest n of the call):
+ * the right-looking Cholesky A = L L^T in panels of 32 columns, then, when it succeeds, x = (L L^T)^-1 b.
+ *   - Outputs: A_out[g] receives the whole n x n array: L in the lower triangle, the strict upper triangle as given.
+ *     info[g] is 0, or 1 + the first column whose pivot is not > 0 (NaN included); then the columns of the 32-column
+ *     panels before that column's panel hold their final L, the rest of the lower triangle is partly updated, and
+ *     x_out[g] is left untouched.  Otherwise x_out[g] receives x.
+ *   - Refusals, with nothing written: a NULL ctx, G < 1, a NULL array (n, A, b, A_out, x_out, info, or an entry of a
+ *     matrix with n[g] > 0) or n[g] < 0 is TZR_ERR_INVALID_ARG; n[g] above 6 x the batched routes' largest K on this
+ *     device (the largest K whose line-process kernel fits the opt-in shared memory: 139 with 227 KB, n = 834) is
+ *     TZR_ERR_TOO_LARGE.
+ *   - Workspace: ctx's pose-graph workspace (so a retained solve stays retained).  Host pointers, synchronous. */
+int tzr_dense_cholesky_batch(tzr_ctx* ctx, int G, const int32_t* n, const double* const* A, const double* const* b,
+                             double* const* A_out, double* const* x_out, int32_t* info);
+
 /* tzr_register_cloud_pairs_multiway_colored's arguments with tzr_line_process_params in place of the GNC-TLS ones:
  * colors NULL refines by point-to-plane ICP (tzr_register_cloud_pairs_icp_point_to_plane; a non-NULL kernel is then
  * TZR_ERR_INVALID_ARG), otherwise by coloured ICP; then the information matrices as in tzr_register_cloud_pairs_multiway,

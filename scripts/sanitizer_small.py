@@ -204,5 +204,10 @@ for opt in ("gnc_tls", "line_process"):
                                       normal_search_radius=0.05, fpfh_search_radius=0.1, max_iteration=3,
                                       optimizer=opt, map_voxel_size=0.05)
     print("multiway batch", opt, [r[7]["status"] for r in mwr], [len(r[7]["map"]) for r in mwr])
+# the batched routes' Cholesky on given matrices: mixed sizes (panel stride 70), one that fails at column 40
+dc_A = [np.eye(n) * 4.0 + np.tril(np.full((n, n), 0.01), -1) for n in (0, 5, 33, 70)]
+dc_A[3][40, 40] = -1.0
+_, _, dc_info = ctx.dense_cholesky_batch(dc_A, [np.ones(len(a)) for a in dc_A])
+print("dense cholesky batch", dc_info.tolist())
 ctx.close()
 print("DONE")

@@ -263,7 +263,7 @@ _SYMBOLS = [
     "tzr_fgr_params_default", "tzr_fgr", "tzr_fgr_batch", "tzr_register_cloud_pairs_fgr",
     "tzr_ransac_params_default", "tzr_ransac", "tzr_ransac_batch", "tzr_register_cloud_pairs_ransac",
     "tzr_line_process_params_default", "tzr_pose_graph_optimize_line_process",
-    "tzr_pose_graph_optimize_line_process_batch",
+    "tzr_pose_graph_optimize_line_process_batch", "tzr_dense_cholesky_batch",
     "tzr_register_cloud_pairs_multiway_line_process",
     "tzr_register_cloud_pairs_multiway_batch", "tzr_register_cloud_pairs_multiway_line_process_batch",
 ]
@@ -478,6 +478,8 @@ def lib():
         vp, C.POINTER(LineProcessParams), C.c_int, i32p, i32p, C.POINTER(i32p), C.POINTER(C.POINTER(Similarity)),
         C.POINTER(dp), C.POINTER(i32p), C.POINTER(C.POINTER(Similarity)), C.POINTER(C.POINTER(Similarity)),
         C.POINTER(dp), C.POINTER(u8p), C.POINTER(dp), C.POINTER(LineProcessSummary), i32p]
+    L.tzr_dense_cholesky_batch.argtypes = [vp, C.c_int, i32p, C.POINTER(dp), C.POINTER(dp), C.POINTER(dp),
+                                           C.POINTER(dp), i32p]
     L.tzr_register_cloud_pairs_multiway_line_process.argtypes = L.tzr_register_cloud_pairs_icp_colored.argtypes + [
         i32p, C.POINTER(LineProcessParams), dp, i32p, dp, u8p, C.POINTER(Similarity), C.POINTER(LineProcessSummary),
         i32p]
@@ -1942,6 +1944,32 @@ class Context:
         return [dict(poses=_poses(poses)[:K], confidence=l[:E], kept=m[:E].astype(bool), residuals=r[:E],
                      status=int(a.status[g]), **_line_process_summary(summ[g]))
                 for g, (K, E, poses, l, m, r) in enumerate(a.outs)]
+
+    def dense_cholesky_batch(self, A, b, x_out=None):
+        """tzr_dense_cholesky_batch: the batched pose-graph routes' Cholesky factorisation and solve on given matrices.
+        A: G square float64 arrays (only the lower triangle is factored), b: G vectors.  x_out: G contiguous float64
+        vectors the solutions are written into (None: NaN-filled ones); a matrix whose factorisation fails leaves its
+        vector untouched.  Returns (factors, x, info): factors[g] the whole returned array (L in the lower triangle, the
+        strict upper triangle as given), x the x_out vectors, info (G,) int32: 0 or 1 + the failed column."""
+        G = len(A)
+        if len(b) != G or (x_out is not None and len(x_out) != G):
+            raise TzrError("dense_cholesky_batch: one b (and one x_out) per matrix is required")
+        mats = [np.asfortranarray(a, dtype=np.float64) for a in A]  # column-major
+        ns = np.array([m.shape[0] for m in mats], dtype=np.int32)
+        if any(m.ndim != 2 or m.shape[0] != m.shape[1] for m in mats):
+            raise TzrError("dense_cholesky_batch: every matrix must be square")
+        bs = [np.ascontiguousarray(v, dtype=np.float64).reshape(int(k)) for v, k in zip(b, ns)]
+        xs = [np.full(int(k), np.nan) for k in ns] if x_out is None else list(x_out)
+        if any(x.dtype != np.float64 or not x.flags.c_contiguous or x.shape != (k,) for x, k in zip(xs, ns)):
+            raise TzrError("dense_cholesky_batch: x_out needs one contiguous float64 vector of n entries per matrix")
+        out = [np.empty((k, k), order="F") for k in ns]
+        info = np.zeros(max(1, G), dtype=np.int32)
+        dpp = C.POINTER(C.c_double) * max(1, G)
+        self._ck(lib().tzr_dense_cholesky_batch(self._h, G, _p(ns, C.c_int32), dpp(*[_p(m, C.c_double) for m in mats]),
+                                                dpp(*[_p(v, C.c_double) for v in bs]),
+                                                dpp(*[_p(m, C.c_double) for m in out]),
+                                                dpp(*[_p(x, C.c_double) for x in xs]), _p(info, C.c_int32)))
+        return out, xs, info[:G]
 
     def icp(self, src, dst, max_correspondence_distance, init=None, max_iteration=30, relative_fitness=1e-6,
             relative_rmse=1e-6):

@@ -2737,14 +2737,21 @@ static int line_process_run(tzr_ctx* ctx, const tzr_line_process_params* prm, in
 }
 
 // ---- many graphs in one call (tzr_pose_graph_optimize_line_process_batch, DESIGN.md §3.23) ---------------------------
-// The largest K of both optimisers' batched routes (DESIGN.md §3.23, §3.24): kLpBatchMaxK, or TZR_LP_BATCH_MAX_K for
-// measurements of the crossover, capped at the largest K whose lp_batch_kernel fits the device's shared memory (the
-// GNC-TLS kernel's 6 (K - 1) rows need less).  A graph's route depends on its own K alone.
-static int pose_graph_batch_max_k(tzr_ctx* ctx) {
+// The largest K whose lp_batch_kernel (6 K rows) fits the device's opt-in shared memory: the batched routes' hard cap,
+// and 6 x it the largest n of tzr_dense_cholesky_batch
+static int pose_graph_batch_cap(tzr_ctx* ctx) {
   int optin = 0;
   cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, ctx->device);
   int cap = 1024;
   while (cap > 2 && line_process_batch_smem(6 * cap) > (size_t)optin) --cap;
+  return cap;
+}
+
+// The largest K of both optimisers' batched routes (DESIGN.md §3.23, §3.24): kLpBatchMaxK, or TZR_LP_BATCH_MAX_K for
+// measurements of the crossover, capped by pose_graph_batch_cap (the GNC-TLS kernel's 6 (K - 1) rows need less).  A
+// graph's route depends on its own K alone.
+static int pose_graph_batch_max_k(tzr_ctx* ctx) {
+  const int cap = pose_graph_batch_cap(ctx);
   const char* e = std::getenv("TZR_LP_BATCH_MAX_K");
   const int k = e ? std::atoi(e) : 0;
   return std::min(k >= 1 ? k : kLpBatchMaxK, cap);
@@ -4838,6 +4845,61 @@ int tzr_pose_graph_optimize_line_process_batch(
   }
   return line_process_batch_run(ctx, params, G, K, E, edges, edge_transforms, information, uncertain, initial_poses,
                                 poses, confidence, kept, residuals, summaries, status);
+}
+
+int tzr_dense_cholesky_batch(tzr_ctx* ctx, int G, const int32_t* n, const double* const* A, const double* const* b,
+                             double* const* A_out, double* const* x_out, int32_t* info) {
+  if (!ctx) return TZR_ERR_INVALID_ARG;
+  bool ok = G >= 1 && n && A && b && A_out && x_out && info;
+  for (int g = 0; ok && g < G; ++g)
+    ok = n[g] >= 0 && (n[g] == 0 || (A[g] && b[g] && A_out[g] && x_out[g]));
+  if (!ok) {
+    ctx->last_error = "dense cholesky batch: invalid arguments (G >= 1, every array, n >= 0)";
+    return TZR_ERR_INVALID_ARG;
+  }
+  int n_max = 0;
+  for (int g = 0; g < G; ++g) n_max = std::max(n_max, (int)n[g]);
+  const int n_cap = 6 * pose_graph_batch_cap(ctx);
+  if (n_max > n_cap) {
+    ctx->last_error = "dense cholesky batch: n = " + std::to_string(n_max) + " above " + std::to_string(n_cap) +
+                      ", the batched pose-graph kernels' shared-memory limit on this device";
+    return TZR_ERR_TOO_LARGE;
+  }
+  // workspace: [descriptors | info (G) | per matrix: A (n x n), x (n)]
+  const size_t o_info = al256((size_t)G * sizeof(DcMatrix));
+  std::vector<size_t> o_A(G), o_x(G);
+  size_t o = o_info + al256((size_t)G * 4);
+  for (int g = 0; g < G; ++g) {
+    o_A[g] = o;
+    o_x[g] = o_A[g] + al256((size_t)n[g] * n[g] * 8);
+    o = o_x[g] + al256((size_t)n[g] * 8);
+  }
+  cudaSetDevice(ctx->device);
+  cudaStream_t st = ctx->stream;
+  int rc;
+  if ((rc = ensure(ctx, ctx->pg, o)) != TZR_OK) return rc;
+  char* d = (char*)ctx->pg.p;
+  std::vector<DcMatrix> desc(G);
+  for (int g = 0; g < G; ++g) {
+    desc[g] = DcMatrix{(double*)(d + o_A[g]), (double*)(d + o_x[g]), (int32_t*)(d + o_info) + g, (int)n[g]};
+    if (n[g] == 0) continue;
+    CK(cudaMemcpyAsync(d + o_A[g], A[g], (size_t)n[g] * n[g] * 8, cudaMemcpyHostToDevice, st));
+    CK(cudaMemcpyAsync(d + o_x[g], b[g], (size_t)n[g] * 8, cudaMemcpyHostToDevice, st));
+  }
+  CK(cudaMemcpyAsync(d, desc.data(), (size_t)G * sizeof(DcMatrix), cudaMemcpyHostToDevice, st));
+  ctx->launches += launch_dense_cholesky_batch((const DcMatrix*)d, G, n_max, st);
+  if ((rc = check_launch(ctx, "dense cholesky batch launch")) != TZR_OK) return rc;
+  std::vector<int32_t> h_info(G);
+  CK(cudaMemcpyAsync(h_info.data(), d + o_info, (size_t)G * 4, cudaMemcpyDeviceToHost, st));
+  CK(cudaStreamSynchronize(st));
+  for (int g = 0; g < G; ++g) {
+    if (n[g] == 0) continue;
+    CK(cudaMemcpyAsync(A_out[g], d + o_A[g], (size_t)n[g] * n[g] * 8, cudaMemcpyDeviceToHost, st));
+    if (h_info[g] == 0) CK(cudaMemcpyAsync(x_out[g], d + o_x[g], (size_t)n[g] * 8, cudaMemcpyDeviceToHost, st));
+  }
+  CK(cudaStreamSynchronize(st));
+  memcpy(info, h_info.data(), (size_t)G * 4);
+  return TZR_OK;
 }
 
 int tzr_register_cloud_pairs_multiway_line_process(

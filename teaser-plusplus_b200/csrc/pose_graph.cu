@@ -1283,6 +1283,29 @@ __global__ void __launch_bounds__(kLbThreads) pg_batch_kernel(const PgBatchGraph
   }
 }
 
+// ---- the batch kernels' factorisation on given matrices (tzr_dense_cholesky_batch, DESIGN.md §3.23) ------------------
+// dc_batch_kernel: one CTA of kLbThreads per matrix, with the two batch kernels' shared-memory layout and panel stride
+// ldp = n_max: lb_cholesky on the matrix in place, then, when it succeeds, lb_solve on x = b in the slot where those
+// kernels keep their right-hand side.
+__global__ void __launch_bounds__(kLbThreads) dc_batch_kernel(const DcMatrix* mats, int ldp) {
+  extern __shared__ double smem[];
+  double* Ps = smem;                   // kLbNb x ldp: the Cholesky panel
+  double* Dt = Ps + kLbNb * ldp;       // kLbNb x kLbDt: its diagonal tile
+  double* x = Dt + kLbNb * kLbDt;      // ldp: b, then the solution
+  double* tmp = x + ldp + kLbThreads;  // kLbNb: the backward sweep's sums
+  const DcMatrix m = mats[blockIdx.x];
+  const int n = m.n, t = threadIdx.x;
+  for (int i = t; i < n; i += kLbThreads) x[i] = m.x[i];
+  __syncthreads();
+  const int bad = lb_cholesky(m.A, n, Ps, ldp, Dt);
+  __syncthreads();
+  if (!bad) {
+    lb_solve(m.A, n, x, tmp);
+    for (int i = t; i < n; i += kLbThreads) m.x[i] = x[i];
+  }
+  if (t == 0) *m.info = bad;
+}
+
 }  // namespace
 
 int launch_line_process_begin(const LpPlan& plan, const LpDev& dv, cudaStream_t st) {
@@ -1335,6 +1358,13 @@ int launch_pose_graph_batch(const PgBatchGraph* graphs, int G, int n_max, cudaSt
   const size_t smem = line_process_batch_smem(n_max);
   cudaFuncSetAttribute(pg_batch_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
   pg_batch_kernel<<<G, kLbThreads, smem, st>>>(graphs, n_max);
+  return 1;
+}
+
+int launch_dense_cholesky_batch(const DcMatrix* mats, int G, int n_max, cudaStream_t st) {
+  const size_t smem = line_process_batch_smem(n_max);
+  cudaFuncSetAttribute(dc_batch_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+  dc_batch_kernel<<<G, kLbThreads, smem, st>>>(mats, n_max);
   return 1;
 }
 

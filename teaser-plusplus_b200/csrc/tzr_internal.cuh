@@ -886,6 +886,17 @@ struct PgBatchGraph {
 // The whole solve of every graph (dynamic shared memory line_process_batch_smem(n_max), n_max = the largest
 // 6 (K - 1)).  Returns the launches (1).
 int launch_pose_graph_batch(const PgBatchGraph* graphs, int G, int n_max, cudaStream_t st);
+// The factorisation of both batch kernels on given matrices (tzr_dense_cholesky_batch, DESIGN.md §3.23).  One entry
+// per matrix, in device memory.
+struct DcMatrix {
+  double* A;      // n x n column-major: factored in place (L in the lower triangle, the upper triangle untouched)
+  double* x;      // n: b, replaced by the solution when the factorisation succeeds
+  int32_t* info;  // 0, or 1 + the first column whose pivot is not > 0
+  int n;
+};
+// Every matrix in one CTA each, with the batch kernels' shared memory line_process_batch_smem(n_max) and panel stride
+// n_max (n_max = the largest n).  Returns the launches (1).
+int launch_dense_cholesky_batch(const DcMatrix* mats, int G, int n_max, cudaStream_t st);
 // dense Cholesky through the lazily loaded cuSOLVER (certify.cu): handle and workspace size of an n x n lower factor;
 // TZR_ERR_UNSUPPORTED when cuSOLVER cannot be loaded
 int dense_cholesky_setup(void** solver_handle, int n, double* A, int* lwork, cudaStream_t st, std::string* err);
