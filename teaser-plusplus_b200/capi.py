@@ -740,6 +740,25 @@ class _GraphBatch:
         return (self.G, _p(self.Ks, C.c_int32), _p(self.Es, C.c_int32), self.ed_p, self.tr_p, self.info_p, self.unc_p,
                 self.init_p, self.pose_p, self.d1_p, self.u8_p, self.d2_p)
 
+    def one(self):
+        """The single calls' K through the output arrays: graph 0's entries of args()."""
+        return (int(self.Ks[0]), int(self.Es[0]), self.ed_p[0], self.tr_p[0], self.info_p[0], self.unc_p[0],
+                self.init_p[0], self.pose_p[0], self.d1_p[0], self.u8_p[0], self.d2_p[0])
+
+
+def _pose_graph_result(out, summ):
+    """One graph's dict of optimize_pose_graph(_batch) from its _GraphBatch outputs and summary."""
+    K, E, poses, w, m, r = out
+    return dict(poses=_poses(poses)[:K], weights=w[:E], mask=m[:E].astype(bool), residuals=r[:E],
+                iterations=int(summ.iterations), inner_iterations=int(summ.inner_iterations), cost=float(summ.cost))
+
+
+def _line_process_result(out, summ):
+    """One graph's dict of global_optimization(_batch) from its _GraphBatch outputs and summary."""
+    K, E, poses, l, m, r = out
+    return dict(poses=_poses(poses)[:K], confidence=l[:E], kept=m[:E].astype(bool), residuals=r[:E],
+                **_line_process_summary(summ))
+
 
 def multiway_batch_table(sequences, pairs, uncertain=None, tuple_seeds=None, colors=None):
     """The flat table of register_multiway_batch: clouds, colours, pairs (global cloud indices), uncertain flags and
@@ -1870,26 +1889,12 @@ class Context:
         similarity() takes), information (E,6,6), uncertain (E flags, None: every edge certain), initial_poses (K, None:
         breadth-first from the reference node); params: any PoseGraphParams field.  Returns a dict: poses (K,4,4),
         weights (E,), mask (E,) bool, residuals (E,) r-bar, iterations, inner_iterations, cost."""
-        ed = np.ascontiguousarray(edges, dtype=np.int32).reshape(-1, 2)
-        E = ed.shape[0]
-        info = np.ascontiguousarray(information, dtype=np.float64).reshape(E, 36)
-        if len(transforms) != E:
-            raise TzrError("optimize_pose_graph: one transform per edge is required")
-        tr = (Similarity * E)(*[similarity(x) for x in transforms])
-        unc = None if uncertain is None else np.ascontiguousarray(uncertain, dtype=np.int32)
-        if unc is not None and unc.shape != (E,):
-            raise TzrError("optimize_pose_graph: uncertain needs one entry per edge")
-        init = None if initial_poses is None else (Similarity * int(K))(*[similarity(x) for x in initial_poses])
+        a = _GraphBatch([dict(K=K, edges=edges, transforms=transforms, information=information, uncertain=uncertain,
+                              initial_poses=initial_poses)], "optimize_pose_graph")
         pg = pose_graph_params(max_correspondence_distance, **params)
-        poses = (Similarity * max(1, int(K)))()
-        w, m, r = np.zeros(max(1, E)), np.zeros(max(1, E), dtype=np.uint8), np.zeros(max(1, E))
         summ = PoseGraphSummary()
-        self._ck(lib().tzr_pose_graph_optimize(self._h, C.byref(pg), int(K), E, _p(ed, C.c_int32), tr,
-                                               _p(info, C.c_double), None if unc is None else _p(unc, C.c_int32), init,
-                                               poses, _p(w, C.c_double), _p(m, C.c_uint8), _p(r, C.c_double),
-                                               C.byref(summ)))
-        return dict(poses=_poses(poses), weights=w[:E], mask=m[:E].astype(bool), residuals=r[:E],
-                    iterations=int(summ.iterations), inner_iterations=int(summ.inner_iterations), cost=float(summ.cost))
+        self._ck(lib().tzr_pose_graph_optimize(self._h, C.byref(pg), *a.one(), C.byref(summ)))
+        return _pose_graph_result(a.outs[0], summ)
 
     def global_optimization(self, K, edges, transforms, information, max_correspondence_distance, uncertain=None,
                             initial_poses=None, **params):
@@ -1897,26 +1902,12 @@ class Context:
         Arguments as optimize_pose_graph's; params: any LineProcessParams field.  Returns a dict: poses (K,4,4),
         confidence (E,), kept (E,) bool, residuals (E,) zeta^T Lambda zeta, and per pass iterations, trials,
         stop_reason (TZR_LP_STOP_*, see LP_STOP) and mu (2-lists), pruned, residual (the final F)."""
-        ed = np.ascontiguousarray(edges, dtype=np.int32).reshape(-1, 2)
-        E = ed.shape[0]
-        info = np.ascontiguousarray(information, dtype=np.float64).reshape(E, 36)
-        if len(transforms) != E:
-            raise TzrError("global_optimization: one transform per edge is required")
-        tr = (Similarity * E)(*[similarity(x) for x in transforms])
-        unc = None if uncertain is None else np.ascontiguousarray(uncertain, dtype=np.int32)
-        if unc is not None and unc.shape != (E,):
-            raise TzrError("global_optimization: uncertain needs one entry per edge")
-        init = None if initial_poses is None else (Similarity * int(K))(*[similarity(x) for x in initial_poses])
+        a = _GraphBatch([dict(K=K, edges=edges, transforms=transforms, information=information, uncertain=uncertain,
+                              initial_poses=initial_poses)], "global_optimization")
         lp = line_process_params(max_correspondence_distance, **params)
-        poses = (Similarity * max(1, int(K)))()
-        l, m, r = np.zeros(max(1, E)), np.zeros(max(1, E), dtype=np.uint8), np.zeros(max(1, E))
         summ = LineProcessSummary()
-        self._ck(lib().tzr_pose_graph_optimize_line_process(
-            self._h, C.byref(lp), int(K), E, _p(ed, C.c_int32), tr, _p(info, C.c_double),
-            None if unc is None else _p(unc, C.c_int32), init, poses, _p(l, C.c_double), _p(m, C.c_uint8),
-            _p(r, C.c_double), C.byref(summ)))
-        return dict(poses=_poses(poses), confidence=l[:E], kept=m[:E].astype(bool), residuals=r[:E],
-                    **_line_process_summary(summ))
+        self._ck(lib().tzr_pose_graph_optimize_line_process(self._h, C.byref(lp), *a.one(), C.byref(summ)))
+        return _line_process_result(a.outs[0], summ)
 
     def optimize_pose_graph_batch(self, graphs, max_correspondence_distance, **params):
         """tzr_pose_graph_optimize_batch: many GNC-TLS graphs, one PoseGraphParams (params: any of its fields).  graphs
@@ -1927,10 +1918,7 @@ class Context:
         a = _GraphBatch(graphs, "optimize_pose_graph_batch")
         summ = (PoseGraphSummary * a.P)()
         self._ck(lib().tzr_pose_graph_optimize_batch(self._h, C.byref(pg), *a.args(), summ, a.status_p))
-        return [dict(poses=_poses(poses)[:K], weights=w[:E], mask=m[:E].astype(bool), residuals=r[:E],
-                     status=int(a.status[g]), iterations=int(summ[g].iterations),
-                     inner_iterations=int(summ[g].inner_iterations), cost=float(summ[g].cost))
-                for g, (K, E, poses, w, m, r) in enumerate(a.outs)]
+        return [dict(_pose_graph_result(out, summ[g]), status=int(a.status[g])) for g, out in enumerate(a.outs)]
 
     def global_optimization_batch(self, graphs, max_correspondence_distance, **params):
         """tzr_pose_graph_optimize_line_process_batch: many graphs, one LineProcessParams (params: any of its fields).
@@ -1941,9 +1929,7 @@ class Context:
         a = _GraphBatch(graphs, "global_optimization_batch")
         summ = (LineProcessSummary * a.P)()
         self._ck(lib().tzr_pose_graph_optimize_line_process_batch(self._h, C.byref(lp), *a.args(), summ, a.status_p))
-        return [dict(poses=_poses(poses)[:K], confidence=l[:E], kept=m[:E].astype(bool), residuals=r[:E],
-                     status=int(a.status[g]), **_line_process_summary(summ[g]))
-                for g, (K, E, poses, l, m, r) in enumerate(a.outs)]
+        return [dict(_line_process_result(out, summ[g]), status=int(a.status[g])) for g, out in enumerate(a.outs)]
 
     def dense_cholesky_batch(self, A, b, x_out=None):
         """tzr_dense_cholesky_batch: the batched pose-graph routes' Cholesky factorisation and solve on given matrices.

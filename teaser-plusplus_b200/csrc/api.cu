@@ -2339,53 +2339,79 @@ static void pg_edge_table(int E, const int32_t* ends, const tzr_similarity* T, c
   }
 }
 
-// One graph's checks, start and plan, in the single entry's order of refusals (include/teaser_b200.h)
-struct PgGraphPrep {
+// One graph's checks, start and edge table, the same for both optimisers
+struct GraphPrep {
+  std::vector<char> live;
   std::vector<double> pose;  // K x 12 starting poses
   std::vector<PgEdge> ed;
   std::vector<PgBlock> blocks;
   std::vector<PgTerm> terms;
-  PgPlan plan;
-  double cost_floor = 0;     // 1e-24 c^2 sum Lambda(5,5)
+  double info_sum = 0;       // sum of Lambda(5,5)
 };
-static int pg_prepare(tzr_ctx* ctx, const tzr_pose_graph_params* prm, int K, int E, const int32_t* ends,
-                      const tzr_similarity* T, const double* info, const int32_t* uncertain,
-                      const tzr_similarity* init, const tzr_similarity* poses, PgGraphPrep* g) {
-  if (!ctx || !pg_params_ok(prm) || K < 2 || E < 1 || !ends || !T || !info || !poses) {
-    if (ctx) ctx->last_error = "pose graph: invalid arguments (K >= 2, E >= 1 and the parameters' ranges)";
+
+// A graph's GraphPrep for either optimiser, in the single entries' order of refusals (include/teaser_b200.h): who
+// prefixes the messages, params_ok is the optimiser's own parameter check, free_ref allows reference_node ref = -1,
+// and fixed_ref holds the reference node fixed (GNC-TLS) where otherwise every node is free (the line process).  The
+// breadth-first start is from the reference node, node 0 for -1; c: max_correspondence_distance.  ref and c are only
+// read once params_ok holds.
+static int graph_prepare(tzr_ctx* ctx, const char* who, bool params_ok, bool free_ref, bool fixed_ref, int ref,
+                         double c, int K, int E, const int32_t* ends, const tzr_similarity* T, const double* info,
+                         const int32_t* uncertain, const tzr_similarity* init, const tzr_similarity* poses,
+                         GraphPrep* g) {
+  if (!ctx || !params_ok || K < 2 || E < 1 || !ends || !T || !info || !poses) {
+    if (ctx) ctx->last_error = std::string(who) + ": invalid arguments (K >= 2, E >= 1 and the parameters' ranges)";
     return TZR_ERR_INVALID_ARG;
   }
   if (K > 1024) {
-    ctx->last_error = "pose graph: more than 1024 nodes";
+    ctx->last_error = std::string(who) + ": more than 1024 nodes";
     return TZR_ERR_TOO_LARGE;
   }
-  const int ref = prm->reference_node;
-  if (ref < 0 || ref >= K) {
-    ctx->last_error = "pose graph: reference_node " + std::to_string(ref) + " is not a node";
+  if (ref < (free_ref ? -1 : 0) || ref >= K) {
+    ctx->last_error = std::string(who) + ": reference_node " + std::to_string(ref) +
+                      (free_ref ? " is neither -1 nor a node" : " is not a node");
     return TZR_ERR_INVALID_ARG;
   }
-  std::vector<char> live;
-  double info_sum = 0.0;
-  int rc = pg_start(ctx, K, E, ends, T, info, uncertain, init, ref, &live, &info_sum, &g->pose);
+  const int rc = pg_start(ctx, K, E, ends, T, info, uncertain, init, ref < 0 ? 0 : ref, &g->live, &g->info_sum,
+                          &g->pose);
   if (rc != TZR_OK) return rc;
-  const double c = prm->max_correspondence_distance;
-  pg_edge_table(E, ends, T, info, uncertain, live, ref, c, &g->ed, &g->blocks, &g->terms);
-  PgPlan& plan = g->plan;
-  plan.K = K;
-  plan.E = E;
-  plan.n = 6 * (K - 1);
-  plan.blocks = (int)g->blocks.size();
-  plan.max_inner = prm->max_inner_iterations;
-  plan.gnc_factor = prm->gnc_factor;
-  plan.cost_threshold = prm->cost_threshold;
-  g->cost_floor = 1e-24 * (c * c) * info_sum;
+  pg_edge_table(E, ends, T, info, uncertain, g->live, fixed_ref ? ref : -1, c, &g->ed, &g->blocks, &g->terms);
   return TZR_OK;
 }
 
-// One graph's outputs: the final poses (K x 12), and per edge the weight w[e], its inlier flag and r-bar
-// res[e * res_stride]
-static void pg_write_outputs(int K, int E, const double* pose, const double* w, const double* res, size_t res_stride,
-                             tzr_similarity* poses, double* weights, uint8_t* inlier_mask, double* residuals) {
+static int pg_prepare(tzr_ctx* ctx, const tzr_pose_graph_params* prm, int K, int E, const int32_t* ends,
+                      const tzr_similarity* T, const double* info, const int32_t* uncertain,
+                      const tzr_similarity* init, const tzr_similarity* poses, GraphPrep* g) {
+  return graph_prepare(ctx, "pose graph", pg_params_ok(prm), false, true, prm ? prm->reference_node : 0,
+                       prm ? prm->max_correspondence_distance : 0, K, E, ends, T, info, uncertain, init, poses, g);
+}
+
+// GNC-TLS's plan of a prepared graph, and its cost floor 1e-24 c^2 sum Lambda(5,5)
+static PgPlan pg_plan(const tzr_pose_graph_params* prm, int K, int E, const GraphPrep& g, double* cost_floor) {
+  PgPlan plan;
+  plan.K = K;
+  plan.E = E;
+  plan.n = 6 * (K - 1);
+  plan.blocks = (int)g.blocks.size();
+  plan.max_inner = prm->max_inner_iterations;
+  plan.gnc_factor = prm->gnc_factor;
+  plan.cost_threshold = prm->cost_threshold;
+  const double c = prm->max_correspondence_distance;
+  *cost_floor = 1e-24 * (c * c) * g.info_sum;
+  return plan;
+}
+
+// GNC-TLS's inlier mask: w[e] >= 0.5
+static std::vector<uint8_t> pg_inliers(int E, const double* w) {
+  std::vector<uint8_t> m((size_t)E);
+  for (int e = 0; e < E; ++e) m[e] = w[e] >= 0.5 ? 1 : 0;
+  return m;
+}
+
+// One graph's outputs, for either optimiser: the final poses (K x 12), and per edge its weight or confidence w[e], its
+// inlier or kept flag m[e] and its residual res[e * res_stride]
+static void graph_write_outputs(int K, int E, const double* pose, const double* w, const uint8_t* m,
+                                const double* res, size_t res_stride, tzr_similarity* poses, double* per_edge,
+                                uint8_t* mask, double* residuals) {
   for (int k = 0; k < K; ++k) {
     memset(&poses[k], 0, sizeof(tzr_similarity));
     poses[k].scale = 1.0;
@@ -2393,8 +2419,8 @@ static void pg_write_outputs(int K, int E, const double* pose, const double* w, 
     memcpy(poses[k].translation, &pose[12 * (size_t)k + 9], 24);
   }
   for (int e = 0; e < E; ++e) {
-    if (weights) weights[e] = w[e];
-    if (inlier_mask) inlier_mask[e] = w[e] >= 0.5 ? 1 : 0;
+    if (per_edge) per_edge[e] = w[e];
+    if (mask) mask[e] = m[e];
     if (residuals) residuals[e] = res[(size_t)e * res_stride];
   }
 }
@@ -2403,7 +2429,7 @@ static int pose_graph_run(tzr_ctx* ctx, const tzr_pose_graph_params* prm, int K,
                           const tzr_similarity* T, const double* info, const int32_t* uncertain,
                           const tzr_similarity* init, tzr_similarity* poses, double* weights, uint8_t* inlier_mask,
                           double* residuals, tzr_pose_graph_summary* summary) {
-  PgGraphPrep gp;
+  GraphPrep gp;
   int rc = pg_prepare(ctx, prm, K, E, ends, T, info, uncertain, init, poses, &gp);
   if (rc != TZR_OK) return rc;
   const int ref = prm->reference_node;
@@ -2411,8 +2437,8 @@ static int pose_graph_run(tzr_ctx* ctx, const tzr_pose_graph_params* prm, int K,
   const std::vector<PgEdge>& ed = gp.ed;
   const std::vector<PgBlock>& blocks = gp.blocks;
   const std::vector<PgTerm>& terms = gp.terms;
-  const PgPlan& plan = gp.plan;
-  const double cost_floor = gp.cost_floor;
+  double cost_floor;
+  const PgPlan plan = pg_plan(prm, K, E, gp, &cost_floor);
   const size_t n = (size_t)plan.n;
   // workspace: [edges | blocks | terms | poses (2 buffers) | weights | state] staged in one copy, then the edge terms,
   // H, g and the factorisation's workspace
@@ -2470,8 +2496,8 @@ static int pose_graph_run(tzr_ctx* ctx, const tzr_pose_graph_params* prm, int K,
   CK(cudaMemcpyAsync(terms_out.data(), dv.eterm + (size_t)hs.cur * E * kPgTermStride, (size_t)E * kPgTermStride * 8,
                      cudaMemcpyDeviceToHost, st));
   CK(cudaStreamSynchronize(st));
-  pg_write_outputs(K, E, pose.data(), w.data(), terms_out.data() + 43, kPgTermStride, poses, weights, inlier_mask,
-                   residuals);
+  graph_write_outputs(K, E, pose.data(), w.data(), pg_inliers(E, w.data()).data(), terms_out.data() + 43, kPgTermStride,
+                      poses, weights, inlier_mask, residuals);
   if (summary) {
     summary->iterations = outer;
     summary->inner_iterations = (int32_t)inner_total;
@@ -2504,43 +2530,22 @@ static double lp_mu(const tzr_line_process_params* p, const double* info, const 
   return p->preference_loop_closure * (c * c) * (a / (double)idx.size());
 }
 
-// One graph's checks, start and pass-1 plan, in the single entry's order of refusals (include/teaser_b200.h)
-struct LpGraphPrep {
-  std::vector<char> live;
-  std::vector<double> pose;  // K x 12 starting poses
-  std::vector<PgEdge> ed;
-  std::vector<PgBlock> blocks;
-  std::vector<PgTerm> terms;
-  LpPlan plan;
-};
 static int lp_prepare(tzr_ctx* ctx, const tzr_line_process_params* prm, int K, int E, const int32_t* ends,
                       const tzr_similarity* T, const double* info, const int32_t* uncertain,
-                      const tzr_similarity* init, const tzr_similarity* poses, LpGraphPrep* g) {
-  if (!ctx || !lp_params_ok(prm) || K < 2 || E < 1 || !ends || !T || !info || !poses) {
-    if (ctx) ctx->last_error = "line process: invalid arguments (K >= 2, E >= 1 and the parameters' ranges)";
-    return TZR_ERR_INVALID_ARG;
-  }
-  if (K > 1024) {
-    ctx->last_error = "line process: more than 1024 nodes";
-    return TZR_ERR_TOO_LARGE;
-  }
-  const int ref = prm->reference_node;
-  if (ref < -1 || ref >= K) {
-    ctx->last_error = "line process: reference_node " + std::to_string(ref) + " is neither -1 nor a node";
-    return TZR_ERR_INVALID_ARG;
-  }
-  double info_sum = 0.0;
-  int rc = pg_start(ctx, K, E, ends, T, info, uncertain, init, ref < 0 ? 0 : ref, &g->live, &info_sum, &g->pose);
-  if (rc != TZR_OK) return rc;
-  pg_edge_table(E, ends, T, info, uncertain, g->live, -1, prm->max_correspondence_distance, &g->ed, &g->blocks,
-                &g->terms);
+                      const tzr_similarity* init, const tzr_similarity* poses, GraphPrep* g) {
+  return graph_prepare(ctx, "line process", lp_params_ok(prm), true, false, prm ? prm->reference_node : 0,
+                       prm ? prm->max_correspondence_distance : 0, K, E, ends, T, info, uncertain, init, poses, g);
+}
+
+// The line process's pass-1 plan of a prepared graph
+static LpPlan lp_plan(const tzr_line_process_params* prm, int K, int E, const double* info, const GraphPrep& g) {
   std::vector<int> all(E);
   for (int e = 0; e < E; ++e) all[e] = e;
-  LpPlan& plan = g->plan;
+  LpPlan plan;
   plan.K = K;
   plan.E = E;
   plan.n = 6 * K;
-  plan.blocks = (int)g->blocks.size();
+  plan.blocks = (int)g.blocks.size();
   plan.mu = lp_mu(prm, info, all);
   plan.min_rel_inc = prm->min_relative_increment;
   plan.min_rel_res_inc = prm->min_relative_residual_increment;
@@ -2550,13 +2555,13 @@ static int lp_prepare(tzr_ctx* ctx, const tzr_line_process_params* prm, int K, i
   plan.lower = prm->lower_scale_factor;
   plan.max_iteration = prm->max_iteration;
   plan.max_lm = prm->max_iteration_lm;
-  return TZR_OK;
+  return plan;
 }
 
 // Between the passes: the kept edges (every certain edge, and the uncertain ones with l1 > edge_prune_threshold) in
 // index order, their edge table and block plan, their pass-1 confidences l2 and pass 2's mu
 static void lp_second_pass(const tzr_line_process_params* prm, int E, const int32_t* ends, const tzr_similarity* T,
-                           const double* info, const LpGraphPrep& g, const std::vector<double>& l1,
+                           const double* info, const GraphPrep& g, const std::vector<double>& l1,
                            std::vector<int>* keep_out, std::vector<PgEdge>* ed2, std::vector<PgBlock>* blocks,
                            std::vector<PgTerm>* terms, std::vector<double>* l2, double* mu2) {
   std::vector<int>& keep = *keep_out;
@@ -2584,26 +2589,15 @@ static void lp_second_pass(const tzr_line_process_params* prm, int E, const int3
   *mu2 = lp_mu(prm, info, keep);
 }
 
-// One graph's outputs: the final poses (K x 12), the confidences (pass 2's l2out[j] for kept edge keep[j], pass 1's l1
-// for a pruned one), the kept mask and the residuals res[e * res_stride]
-static void lp_write_outputs(int K, int E, const std::vector<int>& keep, const std::vector<double>& l1,
-                             const double* l2out, const double* pose, const double* res, size_t res_stride,
-                             tzr_similarity* poses, double* confidence, uint8_t* kept, double* residuals) {
-  const int E2 = (int)keep.size();
-  std::vector<double> lf = l1;
-  for (int j = 0; j < E2; ++j) lf[keep[j]] = l2out[j];
-  std::vector<uint8_t> km((size_t)E, 0);
-  for (int j = 0; j < E2; ++j) km[keep[j]] = 1;
-  for (int k = 0; k < K; ++k) {
-    memset(&poses[k], 0, sizeof(tzr_similarity));
-    poses[k].scale = 1.0;
-    memcpy(poses[k].rotation, &pose[12 * (size_t)k], 72);
-    memcpy(poses[k].translation, &pose[12 * (size_t)k + 9], 24);
-  }
-  for (int e = 0; e < E; ++e) {
-    if (confidence) confidence[e] = lf[e];
-    if (kept) kept[e] = km[e];
-    if (residuals) residuals[e] = res[(size_t)e * res_stride];
+// The line process's per-edge outputs: the confidences (pass 2's l2out[j] for kept edge keep[j], pass 1's l1 for a
+// pruned one) and the kept mask
+static void lp_confidences(int E, const std::vector<int>& keep, const std::vector<double>& l1, const double* l2out,
+                           std::vector<double>* lf, std::vector<uint8_t>* km) {
+  *lf = l1;
+  km->assign((size_t)E, 0);
+  for (size_t j = 0; j < keep.size(); ++j) {
+    (*lf)[keep[j]] = l2out[j];
+    (*km)[keep[j]] = 1;
   }
 }
 
@@ -2611,7 +2605,7 @@ static int line_process_run(tzr_ctx* ctx, const tzr_line_process_params* prm, in
                             const tzr_similarity* T, const double* info, const int32_t* uncertain,
                             const tzr_similarity* init, tzr_similarity* poses, double* confidence, uint8_t* kept,
                             double* residuals, tzr_line_process_summary* summary) {
-  LpGraphPrep g;
+  GraphPrep g;
   int rc = lp_prepare(ctx, prm, K, E, ends, T, info, uncertain, init, poses, &g);
   if (rc != TZR_OK) return rc;
   const int ref = prm->reference_node;
@@ -2619,7 +2613,7 @@ static int line_process_run(tzr_ctx* ctx, const tzr_line_process_params* prm, in
   std::vector<PgEdge>& ed = g.ed;
   std::vector<PgBlock>& blocks = g.blocks;
   std::vector<PgTerm>& terms = g.terms;
-  const LpPlan& plan = g.plan;
+  const LpPlan plan = lp_plan(prm, K, E, info, g);
   const size_t n = (size_t)plan.n;
   // workspace: [edges of pass 1 | edges of pass 2 | blocks | terms | poses (2 buffers) | confidences | state] (pass 1's
   // staged in one copy; pass 2's edges, blocks, terms and confidences overwrite theirs between the passes), then the
@@ -2729,8 +2723,11 @@ static int line_process_run(tzr_ctx* ctx, const tzr_line_process_params* prm, in
     CK(cudaMemcpyAsync(terms_out.data(), dv.eterm + (size_t)buf * E * kPgTermStride, (size_t)E * kPgTermStride * 8,
                        cudaMemcpyDeviceToHost, st));
     CK(cudaStreamSynchronize(st));
-    lp_write_outputs(K, E, keep, l1, l2out.data(), pose.data(), terms_out.data() + 42, kPgTermStride, poses, confidence,
-                     kept, residuals);
+    std::vector<double> lf;
+    std::vector<uint8_t> km;
+    lp_confidences(E, keep, l1, l2out.data(), &lf, &km);
+    graph_write_outputs(K, E, pose.data(), lf.data(), km.data(), terms_out.data() + 42, kPgTermStride, poses,
+                        confidence, kept, residuals);
   }
   if (summary) *summary = sm;
   return TZR_OK;
@@ -2757,10 +2754,16 @@ static int pose_graph_batch_max_k(tzr_ctx* ctx) {
   return std::min(k >= 1 ? k : kLpBatchMaxK, cap);
 }
 
-// A refused graph's outputs of either optimiser's batch: its poses, its three per-edge arrays (the weights or
-// confidences, the inlier or kept mask, the residuals) and its summary, zeroed (a template, so C++ linkage inside this
-// file's extern "C" block)
+// Templates below, so C++ linkage inside this file's extern "C" block.
 extern "C++" {
+// entry g of a per-graph pointer array that may be NULL
+template <class T>
+static T* opt_at(T* const* arr, int g) {
+  return arr ? arr[g] : nullptr;
+}
+
+// A refused graph's outputs of either optimiser's batch: its poses, its three per-edge arrays (the weights or
+// confidences, the inlier or kept mask, the residuals) and its summary, zeroed
 template <class Summary>
 static void zero_graph_outputs(int K, int E, tzr_similarity* poses, double* per_edge, uint8_t* mask, double* residuals,
                                Summary* summary) {
@@ -2772,6 +2775,56 @@ static void zero_graph_outputs(int K, int E, tzr_similarity* poses, double* per_
   }
   if (summary) memset(summary, 0, sizeof(*summary));
 }
+
+// What both optimisers' batch drivers share around their own device layout and launches (DESIGN.md §3.23, §3.24):
+// every graph of at most pose_graph_batch_max_k nodes is checked and started by `prepare`, and those it accepts run
+// together in batched(small, prep); the larger graphs then run one by one through `single`, the optimiser's single
+// driver.  status[g] is the graph's return, a refused graph's outputs are zeroed, and tzr_last_error is the last
+// refusal's message.
+template <class Params, class Summary, class Prepare, class Single, class Batched>
+static int graph_batch_run(tzr_ctx* ctx, const Params* prm, int G, const int32_t* K, const int32_t* E,
+                           const int32_t* const* edges, const tzr_similarity* const* T, const double* const* info,
+                           const int32_t* const* uncertain, const tzr_similarity* const* init,
+                           tzr_similarity* const* poses, double* const* per_edge, uint8_t* const* mask,
+                           double* const* residuals, Summary* summaries, int32_t* status, Prepare prepare,
+                           Single single, Batched batched) {
+  auto refuse = [&](int g) {
+    zero_graph_outputs(K[g], E[g], poses[g], opt_at(per_edge, g), opt_at(mask, g), opt_at(residuals, g),
+                       summaries ? summaries + g : nullptr);
+  };
+  const int kmax = pose_graph_batch_max_k(ctx);
+  std::vector<int> small, large;
+  std::vector<GraphPrep> prep(G);
+  for (int g = 0; g < G; ++g) {
+    status[g] = TZR_OK;
+    if (K[g] > kmax) {
+      large.push_back(g);
+      continue;
+    }
+    status[g] = prepare(ctx, prm, K[g], E[g], edges[g], T[g], info[g], opt_at(uncertain, g), opt_at(init, g),
+                        poses[g], &prep[g]);
+    if (status[g] != TZR_OK)
+      refuse(g);
+    else
+      small.push_back(g);
+  }
+  const std::string refusal = ctx->last_error;
+  if (!small.empty()) {
+    const int rc = batched(small, prep);
+    if (rc != TZR_OK) return rc;
+  }
+  std::string last = refusal;
+  for (int g : large) {
+    status[g] = single(ctx, prm, K[g], E[g], edges[g], T[g], info[g], opt_at(uncertain, g), opt_at(init, g), poses[g],
+                       opt_at(per_edge, g), opt_at(mask, g), opt_at(residuals, g), summaries ? summaries + g : nullptr);
+    if (status[g] != TZR_OK) {
+      last = ctx->last_error;
+      refuse(g);
+    }
+  }
+  ctx->last_error = last;
+  return TZR_OK;
+}
 }
 
 static int line_process_batch_run(tzr_ctx* ctx, const tzr_line_process_params* prm, int G, const int32_t* K,
@@ -2780,41 +2833,21 @@ static int line_process_batch_run(tzr_ctx* ctx, const tzr_line_process_params* p
                                   const tzr_similarity* const* init, tzr_similarity* const* poses,
                                   double* const* confidence, uint8_t* const* kept, double* const* residuals,
                                   tzr_line_process_summary* summaries, int32_t* status) {
-  auto opt = [](auto arr, int g) { return arr ? arr[g] : nullptr; };
-  const int kmax = pose_graph_batch_max_k(ctx);
-  // validate, start and plan every graph of the batched route; the others run through the single entry afterwards
-  std::vector<int> small, large;
-  std::vector<LpGraphPrep> prep(G);
-  for (int g = 0; g < G; ++g) {
-    status[g] = TZR_OK;
-    if (K[g] > kmax) {
-      large.push_back(g);
-      continue;
-    }
-    const int rc = lp_prepare(ctx, prm, K[g], E[g], edges[g], T[g], info[g], opt(uncertain, g), opt(init, g),
-                              poses[g], &prep[g]);
-    if (rc != TZR_OK) {
-      status[g] = rc;
-      zero_graph_outputs(K[g], E[g], poses[g], opt(confidence, g), opt(kept, g), opt(residuals, g),
-                         summaries ? summaries + g : nullptr);
-      continue;
-    }
-    small.push_back(g);
-  }
-  const std::string refusal = ctx->last_error;
-  if (!small.empty()) {
+  auto batched = [&](const std::vector<int>& small, const std::vector<GraphPrep>& prep) -> int {
     // workspace, graphs back to back: [descriptors | per graph: this pass's edges, blocks, terms, confidences (staged
     // per pass) | per graph: pass 1's edges, starting poses (staged with pass 1)] then the outputs [per graph: state,
     // confidences, poses, residuals] (read back after each pass) and the working buffers [per graph: poses, edge terms,
     // H, A, b]
     const int S = (int)small.size();
+    std::vector<LpPlan> plan(S);
+    for (int j = 0; j < S; ++j) plan[j] = lp_plan(prm, K[small[j]], E[small[j]], info[small[j]], prep[small[j]]);
     struct Off { size_t ed, blk, trm, l, ed1, init, st, out, pose, term, H, A, b; };
     std::vector<Off> off(S);
     int n_max = 0;
     size_t o = al256((size_t)S * sizeof(LpBatchGraph));
     for (int j = 0; j < S; ++j) {
-      const LpGraphPrep& g = prep[small[j]];
-      const size_t e = (size_t)g.plan.E;
+      const GraphPrep& g = prep[small[j]];
+      const size_t e = (size_t)plan[j].E;
       off[j].ed = o;
       off[j].blk = off[j].ed + al256(e * sizeof(PgEdge));
       off[j].trm = off[j].blk + al256(g.blocks.size() * sizeof(PgBlock));
@@ -2823,26 +2856,23 @@ static int line_process_batch_run(tzr_ctx* ctx, const tzr_line_process_params* p
     }
     const size_t in2_end = o;
     for (int j = 0; j < S; ++j) {
-      const LpGraphPrep& g = prep[small[j]];
       off[j].ed1 = o;
-      off[j].init = off[j].ed1 + al256((size_t)g.plan.E * sizeof(PgEdge));
-      o = off[j].init + al256((size_t)g.plan.K * 12 * 8);
+      off[j].init = off[j].ed1 + al256((size_t)plan[j].E * sizeof(PgEdge));
+      o = off[j].init + al256((size_t)plan[j].K * 12 * 8);
     }
     const size_t in_end = o, out_lo = o;
     for (int j = 0; j < S; ++j) {
-      const LpGraphPrep& g = prep[small[j]];
       off[j].st = o;
       off[j].out = off[j].st + al256(sizeof(LpState));
-      o = off[j].out + al256(((size_t)2 * g.plan.E + (size_t)12 * g.plan.K) * 8);
+      o = off[j].out + al256(((size_t)2 * plan[j].E + (size_t)12 * plan[j].K) * 8);
     }
     const size_t out_hi = o;
     for (int j = 0; j < S; ++j) {
-      const LpGraphPrep& g = prep[small[j]];
-      const size_t n = (size_t)g.plan.n;
-      n_max = std::max(n_max, g.plan.n);
+      const size_t n = (size_t)plan[j].n;
+      n_max = std::max(n_max, plan[j].n);
       off[j].pose = o;
-      off[j].term = off[j].pose + al256((size_t)g.plan.K * 24 * 8);
-      off[j].H = off[j].term + al256((size_t)g.plan.E * 2 * kPgTermStride * 8);
+      off[j].term = off[j].pose + al256((size_t)plan[j].K * 24 * 8);
+      off[j].H = off[j].term + al256((size_t)plan[j].E * 2 * kPgTermStride * 8);
       off[j].A = off[j].H + al256(n * n * 8);
       off[j].b = off[j].A + al256(n * n * 8);
       o = off[j].b + al256(n * 8);
@@ -2854,17 +2884,17 @@ static int line_process_batch_run(tzr_ctx* ctx, const tzr_line_process_params* p
     char* d = (char*)ctx->pg.p;
     std::vector<LpBatchGraph> desc(S);
     for (int j = 0; j < S; ++j) {
-      const LpGraphPrep& g = prep[small[j]];
+      const GraphPrep& g = prep[small[j]];
       const Off& f = off[j];
       LpBatchGraph& x = desc[j];
       x.dv = LpDev{(const PgEdge*)(d + f.ed), (const PgBlock*)(d + f.blk), (const PgTerm*)(d + f.trm),
                    (double*)(d + f.pose), (double*)(d + f.term), (double*)(d + f.l), (double*)(d + f.H),
                    (double*)(d + f.A), (double*)(d + f.b), nullptr, (LpState*)(d + f.st)};
-      x.plan = g.plan;
+      x.plan = plan[j];
       x.edges1 = (const PgEdge*)(d + f.ed1);
       x.init = (const double*)(d + f.init);
       x.out = (double*)(d + f.out);
-      x.E1 = g.plan.E;
+      x.E1 = plan[j].E;
       x.ref = prm->reference_node;
       memcpy(x.T0, g.pose.data() + 12 * (size_t)(x.ref < 0 ? 0 : x.ref), 12 * 8);
     }
@@ -2872,15 +2902,15 @@ static int line_process_batch_run(tzr_ctx* ctx, const tzr_line_process_params* p
     std::vector<char> h(in_end, 0);
     memcpy(h.data(), desc.data(), (size_t)S * sizeof(LpBatchGraph));
     for (int j = 0; j < S; ++j) {
-      const LpGraphPrep& g = prep[small[j]];
+      const GraphPrep& g = prep[small[j]];
       const Off& f = off[j];
-      const size_t e = (size_t)g.plan.E;
+      const size_t e = (size_t)plan[j].E;
       memcpy(h.data() + f.ed, g.ed.data(), e * sizeof(PgEdge));
       memcpy(h.data() + f.blk, g.blocks.data(), g.blocks.size() * sizeof(PgBlock));
       memcpy(h.data() + f.trm, g.terms.data(), g.terms.size() * sizeof(PgTerm));
       for (size_t q = 0; q < e; ++q) ((double*)(h.data() + f.l))[q] = 1.0;
       memcpy(h.data() + f.ed1, g.ed.data(), e * sizeof(PgEdge));
-      memcpy(h.data() + f.init, g.pose.data(), (size_t)g.plan.K * 12 * 8);
+      memcpy(h.data() + f.init, g.pose.data(), (size_t)plan[j].K * 12 * 8);
     }
     const LpBatchGraph* gd = (const LpBatchGraph*)d;
     CK(cudaMemcpyAsync(d, h.data(), in_end, cudaMemcpyHostToDevice, st));
@@ -2896,13 +2926,13 @@ static int line_process_batch_run(tzr_ctx* ctx, const tzr_line_process_params* p
     std::fill(h.begin(), h.begin() + in2_end, 0);
     for (int j = 0; j < S; ++j) {
       const int gi = small[j];
-      const LpGraphPrep& g = prep[gi];
+      const GraphPrep& g = prep[gi];
       const Off& f = off[j];
-      const int Eg = g.plan.E;
+      const int Eg = plan[j].E;
       LpState s1;
       memcpy(&s1, out.data() + (f.st - out_lo), sizeof(s1));
       sm[j] = tzr_line_process_summary{};
-      sm[j].mu[0] = g.plan.mu;
+      sm[j].mu[0] = plan[j].mu;
       sm[j].iterations[0] = s1.iter;
       sm[j].trials[0] = s1.trials;
       sm[j].stop_reason[0] = s1.reason;
@@ -2942,25 +2972,17 @@ static int line_process_batch_run(tzr_ctx* ctx, const tzr_line_process_params* p
       sm[j].stop_reason[1] = s2.reason;
       sm[j].residual = s2.F;
       const double* lo = (const double*)(out.data() + (f.out - out_lo));
-      lp_write_outputs(Kg, Eg, keep[j], l1[j], lo, lo + Eg, lo + Eg + 12 * (size_t)Kg, 1, poses[gi],
-                       opt(confidence, gi), opt(kept, gi), opt(residuals, gi));
+      std::vector<double> lf;
+      std::vector<uint8_t> km;
+      lp_confidences(Eg, keep[j], l1[j], lo, &lf, &km);
+      graph_write_outputs(Kg, Eg, lo + Eg, lf.data(), km.data(), lo + Eg + 12 * (size_t)Kg, 1, poses[gi],
+                          opt_at(confidence, gi), opt_at(kept, gi), opt_at(residuals, gi));
       if (summaries) summaries[gi] = sm[j];
     }
-  }
-  // the graphs above the batched route's size, one by one through the single entry
-  std::string last = refusal;
-  for (int g : large) {
-    status[g] = line_process_run(ctx, prm, K[g], E[g], edges[g], T[g], info[g], opt(uncertain, g), opt(init, g),
-                                 poses[g], opt(confidence, g), opt(kept, g), opt(residuals, g),
-                                 summaries ? summaries + g : nullptr);
-    if (status[g] != TZR_OK) {
-      last = ctx->last_error;
-      zero_graph_outputs(K[g], E[g], poses[g], opt(confidence, g), opt(kept, g), opt(residuals, g),
-                         summaries ? summaries + g : nullptr);
-    }
-  }
-  ctx->last_error = last;
-  return TZR_OK;
+    return TZR_OK;
+  };
+  return graph_batch_run(ctx, prm, G, K, E, edges, T, info, uncertain, init, poses, confidence, kept, residuals,
+                         summaries, status, lp_prepare, line_process_run, batched);
 }
 
 // ---- many GNC-TLS graphs in one call (tzr_pose_graph_optimize_batch, DESIGN.md §3.24) --------------------------------
@@ -2970,63 +2992,42 @@ static int pose_graph_batch_run(tzr_ctx* ctx, const tzr_pose_graph_params* prm, 
                                 const tzr_similarity* const* init, tzr_similarity* const* poses,
                                 double* const* weights, uint8_t* const* inlier_mask, double* const* residuals,
                                 tzr_pose_graph_summary* summaries, int32_t* status) {
-  auto opt = [](auto arr, int g) { return arr ? arr[g] : nullptr; };
-  const int kmax = pose_graph_batch_max_k(ctx);
-  // validate, start and plan every graph of the batched route; the others run through the single entry afterwards
-  std::vector<int> small, large;
-  std::vector<PgGraphPrep> prep(G);
-  for (int g = 0; g < G; ++g) {
-    status[g] = TZR_OK;
-    if (K[g] > kmax) {
-      large.push_back(g);
-      continue;
-    }
-    const int rc = pg_prepare(ctx, prm, K[g], E[g], edges[g], T[g], info[g], opt(uncertain, g), opt(init, g),
-                              poses[g], &prep[g]);
-    if (rc != TZR_OK) {
-      status[g] = rc;
-      zero_graph_outputs(K[g], E[g], poses[g], opt(weights, g), opt(inlier_mask, g), opt(residuals, g),
-                         summaries ? summaries + g : nullptr);
-      continue;
-    }
-    small.push_back(g);
-  }
-  const std::string refusal = ctx->last_error;
-  if (!small.empty()) {
+  auto batched = [&](const std::vector<int>& small, const std::vector<GraphPrep>& prep) -> int {
     // workspace, graphs back to back: [descriptors | per graph: edges, blocks, terms, starting poses, weights, state]
     // (staged in one copy) then [per graph: summary and outputs (poses, weights, r-bar)] (read back in one copy) and
     // the working buffers [per graph: poses, edge terms, H]
     const int S = (int)small.size();
+    std::vector<PgPlan> plan(S);
+    std::vector<double> cost_floor(S);
+    for (int j = 0; j < S; ++j) plan[j] = pg_plan(prm, K[small[j]], E[small[j]], prep[small[j]], &cost_floor[j]);
     struct Off { size_t ed, blk, trm, init, w, st, sum, out, pose, term, H; };
     std::vector<Off> off(S);
     int n_max = 0;
     size_t o = al256((size_t)S * sizeof(PgBatchGraph));
     for (int j = 0; j < S; ++j) {
-      const PgGraphPrep& g = prep[small[j]];
-      const size_t e = (size_t)g.plan.E;
+      const GraphPrep& g = prep[small[j]];
+      const size_t e = (size_t)plan[j].E;
       off[j].ed = o;
       off[j].blk = off[j].ed + al256(e * sizeof(PgEdge));
       off[j].trm = off[j].blk + al256(g.blocks.size() * sizeof(PgBlock));
       off[j].init = off[j].trm + al256(g.terms.size() * sizeof(PgTerm));
-      off[j].w = off[j].init + al256((size_t)g.plan.K * 12 * 8);
+      off[j].w = off[j].init + al256((size_t)plan[j].K * 12 * 8);
       off[j].st = off[j].w + al256(e * 8);
       o = off[j].st + al256(sizeof(PgState));
     }
     const size_t in_end = o, out_lo = o;
     for (int j = 0; j < S; ++j) {
-      const PgGraphPrep& g = prep[small[j]];
       off[j].sum = o;
       off[j].out = off[j].sum + al256(sizeof(tzr_pose_graph_summary));
-      o = off[j].out + al256(((size_t)12 * g.plan.K + (size_t)2 * g.plan.E) * 8);
+      o = off[j].out + al256(((size_t)12 * plan[j].K + (size_t)2 * plan[j].E) * 8);
     }
     const size_t out_hi = o;
     for (int j = 0; j < S; ++j) {
-      const PgGraphPrep& g = prep[small[j]];
-      const size_t n = (size_t)g.plan.n;
-      n_max = std::max(n_max, g.plan.n);
+      const size_t n = (size_t)plan[j].n;
+      n_max = std::max(n_max, plan[j].n);
       off[j].pose = o;
-      off[j].term = off[j].pose + al256((size_t)g.plan.K * 24 * 8);
-      off[j].H = off[j].term + al256((size_t)g.plan.E * 2 * kPgTermStride * 8);
+      off[j].term = off[j].pose + al256((size_t)plan[j].K * 24 * 8);
+      off[j].H = off[j].term + al256((size_t)plan[j].E * 2 * kPgTermStride * 8);
       o = off[j].H + al256(n * n * 8);
     }
     cudaSetDevice(ctx->device);
@@ -3036,25 +3037,25 @@ static int pose_graph_batch_run(tzr_ctx* ctx, const tzr_pose_graph_params* prm, 
     char* d = (char*)ctx->pg.p;
     std::vector<char> h(in_end, 0);
     for (int j = 0; j < S; ++j) {
-      const PgGraphPrep& g = prep[small[j]];
+      const GraphPrep& g = prep[small[j]];
       const Off& f = off[j];
       PgBatchGraph x{};
       x.dv = PgDev{(const PgEdge*)(d + f.ed), (const PgBlock*)(d + f.blk), (const PgTerm*)(d + f.trm),
                    (double*)(d + f.pose), (double*)(d + f.term), (double*)(d + f.w), (double*)(d + f.H), nullptr,
                    (PgState*)(d + f.st)};
-      x.plan = g.plan;
+      x.plan = plan[j];
       x.init = (const double*)(d + f.init);
       x.out = (double*)(d + f.out);
       x.summary = (tzr_pose_graph_summary*)(d + f.sum);
       x.ref = prm->reference_node;
       x.max_iterations = prm->max_iterations;
-      x.cost_floor = g.cost_floor;
+      x.cost_floor = cost_floor[j];
       memcpy(h.data() + (size_t)j * sizeof(PgBatchGraph), &x, sizeof(x));
-      const size_t e = (size_t)g.plan.E;
+      const size_t e = (size_t)plan[j].E;
       memcpy(h.data() + f.ed, g.ed.data(), e * sizeof(PgEdge));
       memcpy(h.data() + f.blk, g.blocks.data(), g.blocks.size() * sizeof(PgBlock));
       memcpy(h.data() + f.trm, g.terms.data(), g.terms.size() * sizeof(PgTerm));
-      memcpy(h.data() + f.init, g.pose.data(), (size_t)g.plan.K * 12 * 8);
+      memcpy(h.data() + f.init, g.pose.data(), (size_t)plan[j].K * 12 * 8);
       for (size_t q = 0; q < e; ++q) ((double*)(h.data() + f.w))[q] = 1.0;
       PgState s0{};  // as the single entry stages it
       s0.gnc_cost = INFINITY;
@@ -3071,25 +3072,15 @@ static int pose_graph_batch_run(tzr_ctx* ctx, const tzr_pose_graph_params* prm, 
       const Off& f = off[j];
       const int Kg = K[gi], Eg = E[gi];
       const double* lo = (const double*)(out.data() + (f.out - out_lo));
-      pg_write_outputs(Kg, Eg, lo, lo + 12 * (size_t)Kg, lo + 12 * (size_t)Kg + Eg, 1, poses[gi], opt(weights, gi),
-                       opt(inlier_mask, gi), opt(residuals, gi));
+      const double* w = lo + 12 * (size_t)Kg;
+      graph_write_outputs(Kg, Eg, lo, w, pg_inliers(Eg, w).data(), w + Eg, 1, poses[gi], opt_at(weights, gi),
+                          opt_at(inlier_mask, gi), opt_at(residuals, gi));
       if (summaries) memcpy(summaries + gi, out.data() + (f.sum - out_lo), sizeof(tzr_pose_graph_summary));
     }
-  }
-  // the graphs above the batched route's size, one by one through the single entry
-  std::string last = refusal;
-  for (int g : large) {
-    status[g] = pose_graph_run(ctx, prm, K[g], E[g], edges[g], T[g], info[g], opt(uncertain, g), opt(init, g),
-                               poses[g], opt(weights, g), opt(inlier_mask, g), opt(residuals, g),
-                               summaries ? summaries + g : nullptr);
-    if (status[g] != TZR_OK) {
-      last = ctx->last_error;
-      zero_graph_outputs(K[g], E[g], poses[g], opt(weights, g), opt(inlier_mask, g), opt(residuals, g),
-                         summaries ? summaries + g : nullptr);
-    }
-  }
-  ctx->last_error = last;
-  return TZR_OK;
+    return TZR_OK;
+  };
+  return graph_batch_run(ctx, prm, G, K, E, edges, T, info, uncertain, init, poses, weights, inlier_mask, residuals,
+                         summaries, status, pg_prepare, pose_graph_run, batched);
 }
 
 // what tzr_register_cloud_pairs_multiway adds to register_pairs_run (include/teaser_b200.h)
@@ -3223,6 +3214,15 @@ static int multiway_maps_run(tzr_ctx* ctx, const MultiwayOut& mw, const int32_t*
   return TZR_OK;
 }
 
+// A solved graph's weights or confidences w and mask m, scattered back to the pairs: its edge j is pair pair_of[j]
+static void scatter_to_pairs(const MultiwayOut& mw, const std::vector<int>& pair_of, const double* w,
+                             const uint8_t* m) {
+  for (size_t j = 0; j < pair_of.size(); ++j) {
+    mw.edge_weights[pair_of[j]] = w[j];
+    mw.edge_mask[pair_of[j]] = m[j];
+  }
+}
+
 // The many-sequence tail of register_pairs_run (DESIGN.md §3.25): graph g's edges are the refined pairs among its
 // clouds, in pair order with end points shifted by -off[g], through the pose-graph batch of mw's optimiser; then the
 // weights or confidences and masks scattered back to their pairs, and the fused maps.  The edge list (ends, unc, Tsd,
@@ -3235,9 +3235,12 @@ static int multiway_graphs_run(tzr_ctx* ctx, const MultiwayOut& mw, const int32_
                                const float* d_pts, const float* d_col) {
   const int G = mw.G;
   const int32_t* off = mw.graph_offsets;
-  std::vector<std::vector<int>> eg((size_t)G);  // every graph's edges, ascending
-  for (size_t e = 0; e < edge_pair.size(); ++e)
-    eg[std::upper_bound(off, off + G + 1, ends[2 * e]) - off - 1].push_back((int)e);
+  std::vector<std::vector<int>> eg((size_t)G), gp((size_t)G);  // every graph's edges, ascending, and their pairs
+  for (size_t e = 0; e < edge_pair.size(); ++e) {
+    const size_t g = std::upper_bound(off, off + G + 1, ends[2 * e]) - off - 1;
+    eg[g].push_back((int)e);
+    gp[g].push_back(edge_pair[e]);
+  }
   std::vector<int32_t> K(G), E(G);
   std::vector<std::vector<int32_t>> ge(G), gu(G);
   std::vector<std::vector<tzr_similarity>> gT(G);
@@ -3276,13 +3279,8 @@ static int multiway_graphs_run(tzr_ctx* ctx, const MultiwayOut& mw, const int32_
                                               pu.data(), nullptr, pose.data(), pw.data(), pm.data(), nullptr,
                                               mw.summary, mw.pg_status);
   if (rc != TZR_OK) return rc;
-  for (int g = 0; g < G; ++g) {
-    if (mw.pg_status[g] != TZR_OK) continue;
-    for (int j = 0; j < E[g]; ++j) {
-      mw.edge_weights[edge_pair[eg[g][j]]] = gw[g][j];
-      mw.edge_mask[edge_pair[eg[g][j]]] = gm[g][j];
-    }
-  }
+  for (int g = 0; g < G; ++g)
+    if (mw.pg_status[g] == TZR_OK) scatter_to_pairs(mw, gp[g], gw[g].data(), gm[g].data());
   if (!(mw.map_voxel_size > 0)) return TZR_OK;
   return multiway_maps_run(ctx, mw, n, clouds, d_pts, d_col);
 }
@@ -3889,14 +3887,12 @@ static int register_pairs_run(tzr_ctx* ctx, const tzr_frontend_params* fp, const
                  : pose_graph_run(ctx, mw->pg, n_clouds, E, ends.data(), Tsd.data(), L.data(), unc.data(), nullptr,
                                   mw->poses, w.data(), m.data(), nullptr, mw->summary);
       if (*mw->pg_status == TZR_OK) {
-        for (int e = 0; e < E; ++e) {
-          mw->edge_weights[edge_pair[e]] = w[e];
-          mw->edge_mask[edge_pair[e]] = m[e];
-        }
+        scatter_to_pairs(*mw, edge_pair, w.data(), m.data());
       } else {
-        memset(mw->poses, 0, (size_t)n_clouds * sizeof(tzr_similarity));
-        if (mw->summary) memset(mw->summary, 0, sizeof(*mw->summary));
-        if (mw->lp_summary) memset(mw->lp_summary, 0, sizeof(*mw->lp_summary));
+        if (mw->lp)
+          zero_graph_outputs(n_clouds, 0, mw->poses, nullptr, nullptr, nullptr, mw->lp_summary);
+        else
+          zero_graph_outputs(n_clouds, 0, mw->poses, nullptr, nullptr, nullptr, mw->summary);
         if (*mw->pg_status == TZR_ERR_CUDA) return TZR_ERR_CUDA;
       }
     }

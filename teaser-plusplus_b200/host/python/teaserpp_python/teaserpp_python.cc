@@ -261,6 +261,33 @@ py::array_t<double> square_to_numpy(const Eigen::Matrix<double, N, N>& M) {
 }
 using SqArr = py::array_t<double, py::array::c_style | py::array::forcecast>;
 
+// The edges of both optimisers' optimize and optimize_batch
+std::vector<teaser::PoseGraph::Edge> edges_of(const std::vector<std::pair<int, int>>& edges,
+                                              const std::vector<SqArr>& transforms,
+                                              const std::vector<SqArr>& information,
+                                              const std::vector<bool>& uncertain) {
+  if (transforms.size() != edges.size() || information.size() != edges.size() ||
+      (!uncertain.empty() && uncertain.size() != edges.size()))
+    throw std::invalid_argument("one transform, information matrix (and uncertain flag) per edge");
+  std::vector<teaser::PoseGraph::Edge> E(edges.size());
+  for (size_t e = 0; e < edges.size(); ++e) {
+    E[e].source = edges[e].first;
+    E[e].target = edges[e].second;
+    E[e].transform = square_of<4>(transforms[e]);
+    E[e].information = square_of<6>(information[e]);
+    E[e].uncertain = !uncertain.empty() && uncertain[e];
+  }
+  return E;
+}
+
+// (4,4) matrices from a list of them, none for None
+std::vector<Eigen::Matrix4d> matrices_of(const py::object& a) {
+  std::vector<Eigen::Matrix4d> out;
+  if (!a.is_none())
+    for (const auto& m : a.cast<std::vector<SqArr>>()) out.push_back(square_of<4>(m));
+  return out;
+}
+
 // The graphs of both optimisers' optimize_batch: dicts with optimize's keys (num_nodes, edges, transforms,
 // information, and optionally uncertain and initial_poses)
 std::vector<teaser::PoseGraph::Graph> graphs_of(const py::list& graphs) {
@@ -273,23 +300,30 @@ std::vector<teaser::PoseGraph::Graph> graphs_of(const py::list& graphs) {
     const auto uncertain =
         d.contains("uncertain") && !d["uncertain"].is_none() ? d["uncertain"].cast<std::vector<bool>>()
                                                              : std::vector<bool>();
-    if (transforms.size() != edges.size() || information.size() != edges.size() ||
-        (!uncertain.empty() && uncertain.size() != edges.size()))
-      throw std::invalid_argument("one transform, information matrix (and uncertain flag) per edge");
+    gs[j].edges = edges_of(edges, transforms, information, uncertain);
     gs[j].num_nodes = d["num_nodes"].cast<int>();
-    gs[j].edges.resize(edges.size());
-    for (size_t e = 0; e < edges.size(); ++e) {
-      gs[j].edges[e].source = edges[e].first;
-      gs[j].edges[e].target = edges[e].second;
-      gs[j].edges[e].transform = square_of<4>(transforms[e]);
-      gs[j].edges[e].information = square_of<6>(information[e]);
-      gs[j].edges[e].uncertain = !uncertain.empty() && uncertain[e];
-    }
-    if (d.contains("initial_poses") && !d["initial_poses"].is_none())
-      for (const auto& a : d["initial_poses"].cast<std::vector<SqArr>>())
-        gs[j].initial_poses.push_back(square_of<4>(a));
+    if (d.contains("initial_poses")) gs[j].initial_poses = matrices_of(d["initial_poses"]);
   }
   return gs;
+}
+
+// A result of each optimiser as optimize returns it (and optimize_batch, which adds status)
+py::dict pose_graph_dict(const teaser::PoseGraph::Result& r) {
+  py::list poses;
+  for (const auto& T : r.poses) poses.append(square_to_numpy<4>(T));
+  return py::dict(py::arg("poses") = poses, py::arg("weights") = r.weights, py::arg("inliers") = r.inliers,
+                  py::arg("residuals") = r.residuals, py::arg("iterations") = r.iterations,
+                  py::arg("inner_iterations") = r.inner_iterations, py::arg("cost") = r.cost);
+}
+py::dict global_optimization_dict(const teaser::GlobalOptimization::Result& r) {
+  py::list poses;
+  for (const auto& T : r.poses) poses.append(square_to_numpy<4>(T));
+  py::dict out = line_process_dict(r.summary);
+  out["poses"] = poses;
+  out["confidence"] = r.confidence;
+  out["kept"] = r.kept;
+  out["residuals"] = r.residuals;
+  return out;
 }
 
 // MultiScaleICP's scales from Python: (voxel_size, max_correspondence_distance, max_iteration[, normal_search_radius[,
@@ -529,30 +563,14 @@ PYBIND11_MODULE(_teaserpp, m) {
           [](const teaser::PoseGraph& g, int num_nodes, const std::vector<std::pair<int, int>>& edges,
              const std::vector<SqArr>& transforms, const std::vector<SqArr>& information,
              const std::vector<bool>& uncertain, const py::object& initial_poses) {
-            if (transforms.size() != edges.size() || information.size() != edges.size() ||
-                (!uncertain.empty() && uncertain.size() != edges.size()))
-              throw std::invalid_argument("one transform, information matrix (and uncertain flag) per edge");
-            std::vector<teaser::PoseGraph::Edge> E(edges.size());
-            for (size_t e = 0; e < edges.size(); ++e) {
-              E[e].source = edges[e].first;
-              E[e].target = edges[e].second;
-              E[e].transform = square_of<4>(transforms[e]);
-              E[e].information = square_of<6>(information[e]);
-              E[e].uncertain = !uncertain.empty() && uncertain[e];
-            }
-            std::vector<Eigen::Matrix4d> init;
-            if (!initial_poses.is_none())
-              for (const auto& a : initial_poses.cast<std::vector<SqArr>>()) init.push_back(square_of<4>(a));
+            const auto E = edges_of(edges, transforms, information, uncertain);
+            const auto init = matrices_of(initial_poses);
             teaser::PoseGraph::Result r;
             {
               py::gil_scoped_release release;
               r = g.optimize(num_nodes, E, initial_poses.is_none() ? nullptr : &init);
             }
-            py::list poses;
-            for (const auto& T : r.poses) poses.append(square_to_numpy<4>(T));
-            return py::dict(py::arg("poses") = poses, py::arg("weights") = r.weights, py::arg("inliers") = r.inliers,
-                            py::arg("residuals") = r.residuals, py::arg("iterations") = r.iterations,
-                            py::arg("inner_iterations") = r.inner_iterations, py::arg("cost") = r.cost);
+            return pose_graph_dict(r);
           },
           py::arg("num_nodes"), py::arg("edges"), py::arg("transforms"), py::arg("information"),
           py::arg("uncertain") = std::vector<bool>(), py::arg("initial_poses") = py::none())
@@ -570,13 +588,9 @@ PYBIND11_MODULE(_teaserpp, m) {
             }
             py::list out;
             for (size_t j = 0; j < rs.size(); ++j) {
-              const auto& r = rs[j];
-              py::list poses;
-              for (const auto& T : r.poses) poses.append(square_to_numpy<4>(T));
-              out.append(py::dict(py::arg("poses") = poses, py::arg("weights") = r.weights,
-                                  py::arg("inliers") = r.inliers, py::arg("residuals") = r.residuals,
-                                  py::arg("iterations") = r.iterations, py::arg("inner_iterations") = r.inner_iterations,
-                                  py::arg("cost") = r.cost, py::arg("status") = status[j]));
+              py::dict o = pose_graph_dict(rs[j]);
+              o["status"] = status[j];
+              out.append(o);
             }
             return out;
           },
@@ -614,33 +628,14 @@ PYBIND11_MODULE(_teaserpp, m) {
           [](const teaser::GlobalOptimization& g, int num_nodes, const std::vector<std::pair<int, int>>& edges,
              const std::vector<SqArr>& transforms, const std::vector<SqArr>& information,
              const std::vector<bool>& uncertain, const py::object& initial_poses) {
-            if (transforms.size() != edges.size() || information.size() != edges.size() ||
-                (!uncertain.empty() && uncertain.size() != edges.size()))
-              throw std::invalid_argument("one transform, information matrix (and uncertain flag) per edge");
-            std::vector<teaser::GlobalOptimization::Edge> E(edges.size());
-            for (size_t e = 0; e < edges.size(); ++e) {
-              E[e].source = edges[e].first;
-              E[e].target = edges[e].second;
-              E[e].transform = square_of<4>(transforms[e]);
-              E[e].information = square_of<6>(information[e]);
-              E[e].uncertain = !uncertain.empty() && uncertain[e];
-            }
-            std::vector<Eigen::Matrix4d> init;
-            if (!initial_poses.is_none())
-              for (const auto& a : initial_poses.cast<std::vector<SqArr>>()) init.push_back(square_of<4>(a));
+            const auto E = edges_of(edges, transforms, information, uncertain);
+            const auto init = matrices_of(initial_poses);
             teaser::GlobalOptimization::Result r;
             {
               py::gil_scoped_release release;
               r = g.optimize(num_nodes, E, initial_poses.is_none() ? nullptr : &init);
             }
-            py::list poses;
-            for (const auto& T : r.poses) poses.append(square_to_numpy<4>(T));
-            py::dict out = line_process_dict(r.summary);
-            out["poses"] = poses;
-            out["confidence"] = r.confidence;
-            out["kept"] = r.kept;
-            out["residuals"] = r.residuals;
-            return out;
+            return global_optimization_dict(r);
           },
           py::arg("num_nodes"), py::arg("edges"), py::arg("transforms"), py::arg("information"),
           py::arg("uncertain") = std::vector<bool>(), py::arg("initial_poses") = py::none())
@@ -658,14 +653,7 @@ PYBIND11_MODULE(_teaserpp, m) {
             }
             py::list out;
             for (size_t j = 0; j < rs.size(); ++j) {
-              const auto& r = rs[j];
-              py::list poses;
-              for (const auto& T : r.poses) poses.append(square_to_numpy<4>(T));
-              py::dict o = line_process_dict(r.summary);
-              o["poses"] = poses;
-              o["confidence"] = r.confidence;
-              o["kept"] = r.kept;
-              o["residuals"] = r.residuals;
+              py::dict o = global_optimization_dict(rs[j]);
               o["status"] = status[j];
               out.append(o);
             }

@@ -53,26 +53,8 @@ Matrix6d matrix6_of(const double* L) {
   return M;
 }
 
-// the edge arrays of both optimisers' C calls
-void edges_c(const std::vector<PoseGraph::Edge>& edges, std::vector<int32_t>* ends, std::vector<int32_t>* unc,
-             std::vector<tzr_similarity>* tr, std::vector<double>* L) {
-  const size_t E = edges.size();
-  ends->resize(2 * E);
-  unc->resize(E);
-  tr->resize(E);
-  L->resize(36 * E);
-  for (size_t e = 0; e < E; ++e) {
-    (*ends)[2 * e] = edges[e].source;
-    (*ends)[2 * e + 1] = edges[e].target;
-    (*unc)[e] = edges[e].uncertain ? 1 : 0;
-    (*tr)[e] = sim_of(edges[e].transform);
-    for (int r = 0; r < 6; ++r)
-      for (int c = 0; c < 6; ++c) (*L)[36 * e + 6 * r + c] = edges[e].information(r, c);
-  }
-}
-
-// The pointer-per-graph arrays of both optimisers' batched C calls, and per graph the outputs: poses (K), a double
-// (E), a byte (E) and a double (E) array
+// The pointer-per-graph arrays of both optimisers' C calls (a single call's graph is a batch of one), and per graph the
+// outputs: poses (K), a double (E), a byte (E) and a double (E) array
 struct GraphArrays {
   std::vector<int32_t> K, E, status;
   std::vector<std::vector<int32_t>> ends, unc;
@@ -114,7 +96,14 @@ struct GraphArrays {
       const size_t Eg = gr.edges.size();
       if (!gr.initial_poses.empty() && gr.initial_poses.size() != static_cast<size_t>(gr.num_nodes))
         throw std::invalid_argument(std::string(who) + ": one initial pose per node");
-      edges_c(gr.edges, &ends[g], &unc[g], &tr[g], &L[g]);
+      for (const PoseGraph::Edge& e : gr.edges) {
+        ends[g].push_back(e.source);
+        ends[g].push_back(e.target);
+        unc[g].push_back(e.uncertain ? 1 : 0);
+        tr[g].push_back(sim_of(e.transform));
+        for (int r = 0; r < 6; ++r)
+          for (int c = 0; c < 6; ++c) L[g].push_back(e.information(r, c));
+      }
       for (const Eigen::Matrix4d& T : gr.initial_poses) init[g].push_back(sim_of(T));
       K[g] = gr.num_nodes;
       E[g] = static_cast<int32_t>(Eg);
@@ -134,6 +123,51 @@ struct GraphArrays {
     }
   }
 };
+
+// The single calls' graph as a batch of one.  A non-null initial_poses must hold num_nodes poses, even none:
+// GraphArrays reads an empty list as the breadth-first start.
+std::vector<PoseGraph::Graph> one_graph(int num_nodes, const std::vector<PoseGraph::Edge>& edges,
+                                        const std::vector<Eigen::Matrix4d>* initial_poses, const char* who) {
+  if (initial_poses && initial_poses->size() != static_cast<size_t>(num_nodes))
+    throw std::invalid_argument(std::string(who) + ": one initial pose per node");
+  std::vector<PoseGraph::Graph> gs(1);
+  gs[0].num_nodes = num_nodes;
+  gs[0].edges = edges;
+  if (initial_poses) gs[0].initial_poses = *initial_poses;
+  return gs;
+}
+
+// Graph g's results, of either call of each optimiser
+PoseGraph::Result pose_graph_result(const GraphArrays& a, size_t g, const tzr_pose_graph_summary& s) {
+  PoseGraph::Result r;
+  const size_t E = a.E[g];
+  for (int k = 0; k < a.K[g]; ++k) r.poses.push_back(matrix_of(a.poses[g][k]));
+  r.weights.assign(a.d1[g].begin(), a.d1[g].begin() + E);
+  for (size_t e = 0; e < E; ++e) r.inliers.push_back(a.u8[g][e] != 0);
+  r.residuals.assign(a.d2[g].begin(), a.d2[g].begin() + E);
+  r.iterations = s.iterations;
+  r.inner_iterations = s.inner_iterations;
+  r.cost = s.cost;
+  return r;
+}
+
+GlobalOptimization::Result line_process_result(const GraphArrays& a, size_t g, const tzr_line_process_summary& s) {
+  GlobalOptimization::Result r;
+  const size_t E = a.E[g];
+  for (int k = 0; k < a.K[g]; ++k) r.poses.push_back(matrix_of(a.poses[g][k]));
+  r.confidence.assign(a.d1[g].begin(), a.d1[g].begin() + E);
+  for (size_t e = 0; e < E; ++e) r.kept.push_back(a.u8[g][e] != 0);
+  r.residuals.assign(a.d2[g].begin(), a.d2[g].begin() + E);
+  for (int q = 0; q < 2; ++q) {
+    r.summary.iterations[q] = s.iterations[q];
+    r.summary.trials[q] = s.trials[q];
+    r.summary.stop_reason[q] = s.stop_reason[q];
+    r.summary.mu[q] = s.mu[q];
+  }
+  r.summary.pruned = s.pruned;
+  r.summary.residual = s.residual;
+  return r;
+}
 
 }  // namespace
 
@@ -217,74 +251,28 @@ Matrix6d informationMatrix(const PointCloud& src, const PointCloud& dst, const R
 
 PoseGraph::Result PoseGraph::optimize(int num_nodes, const std::vector<Edge>& edges,
                                       const std::vector<Eigen::Matrix4d>* initial_poses) const {
-  const size_t E = edges.size();
-  if (initial_poses && initial_poses->size() != static_cast<size_t>(num_nodes))
-    throw std::invalid_argument("teaser::PoseGraph::optimize: one initial pose per node");
   const tzr_pose_graph_params p = pose_graph_c(params_);
-  std::vector<int32_t> ends, unc;
-  std::vector<tzr_similarity> tr;
-  std::vector<double> L;
-  edges_c(edges, &ends, &unc, &tr, &L);
-  std::vector<tzr_similarity> init;
-  if (initial_poses)
-    for (const Eigen::Matrix4d& T : *initial_poses) init.push_back(sim_of(T));
-  std::vector<tzr_similarity> poses(num_nodes > 0 ? num_nodes : 1);
-  std::vector<double> w(E ? E : 1), res(E ? E : 1);
-  std::vector<uint8_t> mask(E ? E : 1);
-  tzr_pose_graph_summary summary{};
+  const char* who = "teaser::PoseGraph::optimize";
+  const GraphArrays a(one_graph(num_nodes, edges, initial_poses, who), who);
+  tzr_pose_graph_summary s{};
   tzr_ctx* ctx = b200_context();
-  const int rc = tzr_pose_graph_optimize(ctx, &p, num_nodes, static_cast<int>(E), ends.data(), tr.data(), L.data(),
-                                         unc.data(), initial_poses ? init.data() : nullptr, poses.data(), w.data(),
-                                         mask.data(), res.data(), &summary);
-  if (rc != TZR_OK) fail("teaser::PoseGraph::optimize", rc, ctx);
-  Result out;
-  for (int k = 0; k < num_nodes; ++k) out.poses.push_back(matrix_of(poses[k]));
-  out.weights.assign(w.begin(), w.begin() + E);
-  for (size_t e = 0; e < E; ++e) out.inliers.push_back(mask[e] != 0);
-  out.residuals.assign(res.begin(), res.begin() + E);
-  out.iterations = summary.iterations;
-  out.inner_iterations = summary.inner_iterations;
-  out.cost = summary.cost;
-  return out;
+  const int rc = tzr_pose_graph_optimize(ctx, &p, a.K[0], a.E[0], a.ep[0], a.tp[0], a.Lp[0], a.up[0], a.ip[0],
+                                         a.pp[0], a.d1p[0], a.u8p[0], a.d2p[0], &s);
+  if (rc != TZR_OK) fail(who, rc, ctx);
+  return pose_graph_result(a, 0, s);
 }
 
 GlobalOptimization::Result GlobalOptimization::optimize(int num_nodes, const std::vector<Edge>& edges,
                                                         const std::vector<Eigen::Matrix4d>* initial_poses) const {
-  const size_t E = edges.size();
-  if (initial_poses && initial_poses->size() != static_cast<size_t>(num_nodes))
-    throw std::invalid_argument("teaser::GlobalOptimization::optimize: one initial pose per node");
   const tzr_line_process_params p = line_process_c(params_);
-  std::vector<int32_t> ends, unc;
-  std::vector<tzr_similarity> tr;
-  std::vector<double> L;
-  edges_c(edges, &ends, &unc, &tr, &L);
-  std::vector<tzr_similarity> init;
-  if (initial_poses)
-    for (const Eigen::Matrix4d& T : *initial_poses) init.push_back(sim_of(T));
-  std::vector<tzr_similarity> poses(num_nodes > 0 ? num_nodes : 1);
-  std::vector<double> l(E ? E : 1), res(E ? E : 1);
-  std::vector<uint8_t> kept(E ? E : 1);
+  const char* who = "teaser::GlobalOptimization::optimize";
+  const GraphArrays a(one_graph(num_nodes, edges, initial_poses, who), who);
   tzr_line_process_summary s{};
   tzr_ctx* ctx = b200_context();
-  const int rc = tzr_pose_graph_optimize_line_process(ctx, &p, num_nodes, static_cast<int>(E), ends.data(),
-                                                      tr.data(), L.data(), unc.data(),
-                                                      initial_poses ? init.data() : nullptr, poses.data(), l.data(),
-                                                      kept.data(), res.data(), &s);
-  if (rc != TZR_OK) fail("teaser::GlobalOptimization::optimize", rc, ctx);
-  Result out;
-  for (int k = 0; k < num_nodes; ++k) out.poses.push_back(matrix_of(poses[k]));
-  out.confidence.assign(l.begin(), l.begin() + E);
-  for (size_t e = 0; e < E; ++e) out.kept.push_back(kept[e] != 0);
-  out.residuals.assign(res.begin(), res.begin() + E);
-  for (int q = 0; q < 2; ++q) {
-    out.summary.iterations[q] = s.iterations[q];
-    out.summary.trials[q] = s.trials[q];
-    out.summary.stop_reason[q] = s.stop_reason[q];
-    out.summary.mu[q] = s.mu[q];
-  }
-  out.summary.pruned = s.pruned;
-  out.summary.residual = s.residual;
-  return out;
+  const int rc = tzr_pose_graph_optimize_line_process(ctx, &p, a.K[0], a.E[0], a.ep[0], a.tp[0], a.Lp[0], a.up[0],
+                                                      a.ip[0], a.pp[0], a.d1p[0], a.u8p[0], a.d2p[0], &s);
+  if (rc != TZR_OK) fail(who, rc, ctx);
+  return line_process_result(a, 0, s);
 }
 
 std::vector<PoseGraph::Result> PoseGraph::optimizeBatch(const std::vector<Graph>& graphs,
@@ -300,18 +288,8 @@ std::vector<PoseGraph::Result> PoseGraph::optimizeBatch(const std::vector<Graph>
   if (rc != TZR_OK) fail("teaser::PoseGraph::optimizeBatch", rc, ctx);
   std::vector<Result> out(G);
   if (status) status->assign(a.status.begin(), a.status.begin() + G);
-  for (size_t g = 0; g < G; ++g) {
-    if (a.status[g] != TZR_OK) continue;
-    Result& r = out[g];
-    const size_t Eg = graphs[g].edges.size();
-    for (int k = 0; k < a.K[g]; ++k) r.poses.push_back(matrix_of(a.poses[g][k]));
-    r.weights.assign(a.d1[g].begin(), a.d1[g].begin() + Eg);
-    for (size_t e = 0; e < Eg; ++e) r.inliers.push_back(a.u8[g][e] != 0);
-    r.residuals.assign(a.d2[g].begin(), a.d2[g].begin() + Eg);
-    r.iterations = s[g].iterations;
-    r.inner_iterations = s[g].inner_iterations;
-    r.cost = s[g].cost;
-  }
+  for (size_t g = 0; g < G; ++g)
+    if (a.status[g] == TZR_OK) out[g] = pose_graph_result(a, g, s[g]);
   return out;
 }
 
@@ -329,23 +307,8 @@ std::vector<GlobalOptimization::Result> GlobalOptimization::optimizeBatch(const 
   if (rc != TZR_OK) fail("teaser::GlobalOptimization::optimizeBatch", rc, ctx);
   std::vector<Result> out(G);
   if (status) status->assign(a.status.begin(), a.status.begin() + G);
-  for (size_t g = 0; g < G; ++g) {
-    if (a.status[g] != TZR_OK) continue;
-    Result& r = out[g];
-    const size_t Eg = graphs[g].edges.size();
-    for (int k = 0; k < a.K[g]; ++k) r.poses.push_back(matrix_of(a.poses[g][k]));
-    r.confidence.assign(a.d1[g].begin(), a.d1[g].begin() + Eg);
-    for (size_t e = 0; e < Eg; ++e) r.kept.push_back(a.u8[g][e] != 0);
-    r.residuals.assign(a.d2[g].begin(), a.d2[g].begin() + Eg);
-    for (int q = 0; q < 2; ++q) {
-      r.summary.iterations[q] = s[g].iterations[q];
-      r.summary.trials[q] = s[g].trials[q];
-      r.summary.stop_reason[q] = s[g].stop_reason[q];
-      r.summary.mu[q] = s[g].mu[q];
-    }
-    r.summary.pruned = s[g].pruned;
-    r.summary.residual = s[g].residual;
-  }
+  for (size_t g = 0; g < G; ++g)
+    if (a.status[g] == TZR_OK) out[g] = line_process_result(a, g, s[g]);
   return out;
 }
 

@@ -64,6 +64,17 @@ def test_no_cpu_fallback(tp):
         s.solve(np.zeros((3, 10)), np.ones((3, 10)))
 
 
+@pytest.mark.parametrize("cls", ["PoseGraph", "GlobalOptimization"])
+@pytest.mark.parametrize("n_init", [0, 1, 3])
+def test_single_optimize_needs_one_initial_pose_per_node(tp, cls, n_init):
+    # a given initial-pose list must hold num_nodes poses, an empty one included (not read as the breadth-first
+    # start); refused before any device work, so with or without a GPU
+    import numpy as np
+    g = getattr(tp, cls)(0.05)
+    with pytest.raises(ValueError, match=f"teaser::{cls}::optimize: one initial pose per node"):
+        g.optimize(2, [(0, 1)], [np.eye(4)], [np.eye(6)], initial_poses=[np.eye(4)] * n_init)
+
+
 def test_mex_shim_compiles_against_stub():
     """matlab/teaser_mex.cc (MATLAB absent here): syntax/type check against a stub of the MEX API."""
     mex = os.path.join(HOST, "matlab")
