@@ -146,9 +146,10 @@ int tzr_ctx_clique_info(tzr_ctx* ctx, int32_t* geometry3, int32_t* heuristic_bes
  * the full graph, the (L-1)-core of the graph on the device, and the small route's exact search on that core compacted
  * to at most 32768 vertices (the relabelling keeps the index order, so the canonical tie-break is unchanged).  A graph
  * whose core keeps more than 32768 vertices (a dense graph, e.g. most vertices in one large inlier set) is not
- * searched: it returns its heuristic clique, a valid clique with clique_proven_optimal = 0.  estimate_scaling = 1 needs
- * the unknown-scale stage's scratch (tens of GB at these sizes) and is TZR_ERR_TOO_LARGE from n = 46341 (2K end points
- * exceed 2^31).  A buffer that does not fit the device is TZR_ERR_ALLOC (tzr_last_error names the size). */
+ * searched: it returns its heuristic clique, a valid clique with clique_proven_optimal = 0.  estimate_scaling = 1 works
+ * at every n up to max_n: the unknown-scale stage regenerates the TIM ratios in chunks of end points above 8192 points and
+ * keeps its scratch under 3.5 GiB at any size (tzr_ctx_set_scale_chunk).  A buffer that does not fit the device is
+ * TZR_ERR_ALLOC (tzr_last_error names the size). */
 int tzr_ctx_set_max_n(tzr_ctx* ctx, int max_n);
 /* Clique route of each problem of the most recent clique stage on this context (a solve or a max-clique call; B
  * entries; TZR_ERR_INVALID_ARG once another call has reused the workspace): 0 = small route; k > 0 = large route with
@@ -462,8 +463,8 @@ void tzr_frontend_params_default(tzr_frontend_params* p);
  * capacity) the sorted max clique, as rows of corr[p]; global_scale (P floats, may be NULL) Matcher::global_scale_;
  * problem_index (P int32, may be NULL) p's index in the retained solve, -1 when p was not solved.
  * status[p]: TZR_OK solved; TZR_ERR_TOO_LARGE when a point of one of its clouds has more than 4096 neighbours inside a
- * radius (nothing matched, n_corr = 0), or its correspondences exceed the context's max_n, or with estimate_scaling
- * reach 46341 (correspondences written, not solved); TZR_ERR_INVALID_ARG no correspondence.  An unsolved pair gets a
+ * radius (nothing matched, n_corr = 0), or its correspondences exceed the context's max_n (correspondences written,
+ * not solved); TZR_ERR_INVALID_ARG no correspondence.  An unsolved pair gets a
  * zeroed record (valid = 0).  Returns TZR_ERR_TOO_LARGE when some pair was too large (every other pair is complete),
  * TZR_ERR_ALLOC when the batch's buffers do not fit the device (tzr_last_error names the size).
  * For every solved pair the outputs are bit-identical (the record except stage_ms, the clique, the correspondences and
@@ -1677,6 +1678,17 @@ int tzr_ctx_set_flags(tzr_ctx* ctx, uint32_t flags);
  * class or sub-chunk of a batch); 0 before any graph build, or when that build ran another kernel (debug bits 3 to 7
  * and 11). */
 int tzr_ctx_last_strip_blocks(const tzr_ctx* ctx);
+/* Chunk capacity of the unknown-scale stage's regenerating route (DESIGN.md 3.4), in interval end points (2 per TIM).
+ * Above 8192 points the stage regenerates each TIM's ratio and range from the points, cuts the 2K end points, in sorted
+ * order, into chunks of at most this many, and sorts and sweeps one chunk at a time; from 257 to 8192 points it sorts
+ * stored ratios and ranges at once.  Both give the same estimate, at every capacity.  0 (the default) = automatic:
+ * 2^27 end points.  k >= 2048 = the regenerating route for every problem above 256 points, in chunks of at most
+ * min(k, 2^27) end points, raised to 2K / 4096 (rounded up) when more than 4096 chunks would be needed, so that tests
+ * reach many chunks at small n.  Any other value is TZR_ERR_INVALID_ARG. */
+int tzr_ctx_set_scale_chunk(tzr_ctx* ctx, long long max_end_points);
+/* Largest chunk count of one problem in the most recent unknown-scale stage on this context (1: the problem's end
+ * points were sorted at once); 0 before any, or when every problem of it took the bitonic path (n <= 256). */
+int tzr_ctx_last_scale_chunks(const tzr_ctx* ctx);
 /* The default graph kernel's strip order over nt row blocks of 128 points, as the device decodes it, for strips of L
  * blocks: I[p] (row block) and J0[p] (first column block) of strip p = 0 ... count - 1, strips numbered from row block 0
  * down, each row block's strips left to right.  Host-only, needs no device; I and J0 may be NULL.  Returns the count,

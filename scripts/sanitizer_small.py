@@ -27,6 +27,12 @@ print("scale small", g["scale"])
 q = synth.make_problem(1600, 0.5, 5, "ball")
 g = ctx.solve(q["src"], q["dst"] * 2.0, capi.default_params(noise_bound=2 * q["noise_bound"], estimate_scaling=1))
 print("scale large", g["scale"], len(g["clique"]))
+# the unknown-scale stage in forced chunks of 2048 end points at n = 300 on a lattice (tie groups split across chunks)
+lat = np.stack(np.meshgrid(*[np.arange(7.0)] * 3, indexing="ij"), -1).reshape(-1, 3)[:300]
+ctx.set_scale_chunk(2048)
+g = ctx.solve(lat, lat * 2.0, capi.default_params(noise_bound=0.01, estimate_scaling=1))
+print("scale chunks", ctx.last_scale_chunks(), g["scale"])
+ctx.set_scale_chunk(0)
 g = ctx.solve(pr["src"], pr["dst"], capi.default_params(inlier_selection_mode=3, **kw))
 print("none mode", len(g["clique"]))
 prs = [synth.config_problem("C4", b, n=257) for b in range(70)]

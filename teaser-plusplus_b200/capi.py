@@ -255,6 +255,7 @@ _SYMBOLS = [
     "tzr_register_cloud_pairs_icp_point_to_plane", "tzr_icp_generalized", "tzr_icp_generalized_batch",
     "tzr_register_cloud_pairs_icp_generalized", "tzr_icp_point_to_plane_robust_batch", "tzr_icp_generalized_robust_batch",
     "tzr_register_cloud_pairs_icp_robust", "tzr_ctx_last_strip_blocks", "tzr_graph_strip_schedule",
+    "tzr_ctx_set_scale_chunk", "tzr_ctx_last_scale_chunks",
     "tzr_information_matrix", "tzr_information_matrix_batch", "tzr_pose_graph_params_default", "tzr_pose_graph_optimize",
     "tzr_pose_graph_optimize_batch",
     "tzr_register_cloud_pairs_multiway", "tzr_estimate_color_gradients", "tzr_estimate_color_gradients_batch",
@@ -364,6 +365,8 @@ def lib():
     L.tzr_ctx_filter_rechecks.restype = C.c_int64
     L.tzr_ctx_debug_counters.argtypes = [vp, i64p]
     L.tzr_ctx_last_strip_blocks.argtypes = [vp]
+    L.tzr_ctx_set_scale_chunk.argtypes = [vp, C.c_longlong]
+    L.tzr_ctx_last_scale_chunks.argtypes = [vp]
     L.tzr_graph_strip_schedule.argtypes = [C.c_int, C.c_int, i32p, i32p]
     L.tzr_ctx_clique_info.argtypes = [vp, i32p, i32p]
     L.tzr_ctx_set_max_n.argtypes = [vp, C.c_int]
@@ -869,6 +872,17 @@ class Context:
     def last_strip_blocks(self) -> int:
         """Strip length of the default graph kernel's most recent launch (0: none, or another kernel built the graph)."""
         return int(lib().tzr_ctx_last_strip_blocks(self._h))
+
+    def set_scale_chunk(self, max_end_points: int):
+        """Chunk capacity of the unknown-scale stage's regenerating route, in end points (2 per TIM): 0 automatic
+        (2^27, the route above 8192 points), k >= 2048 that route above 256 points in chunks of at most k end points
+        (raised when more than 4096 chunks would be needed).  Every capacity gives the same estimate."""
+        self._ck(lib().tzr_ctx_set_scale_chunk(self._h, int(max_end_points)))
+
+    def last_scale_chunks(self) -> int:
+        """Largest chunk count of one problem in the most recent unknown-scale stage (1: sorted at once; 0: none, or
+        the bitonic path)."""
+        return int(lib().tzr_ctx_last_scale_chunks(self._h))
 
     def clique_info(self, B: int):
         """Geometry of the most recent max_clique(_batch) call and each problem's root-heuristic clique size."""

@@ -142,6 +142,8 @@ struct tzr_ctx {
   DevBuf ransac;
   int last_strip_blocks = 0;  // strip length of the most recent graph kernel launch (tzr_ctx_last_strip_blocks)
   int max_n = kMaxN;  // per-problem size limit of this context (tzr_ctx_set_max_n: kMaxN ... kMaxNLarge)
+  long long scale_chunk = 0;  // unknown-scale chunk capacity in end points (tzr_ctx_set_scale_chunk; 0: automatic)
+  int last_scale_chunks = 0;  // largest chunk count of the most recent unknown-scale stage (tzr_ctx_last_scale_chunks)
   // pinned host staging
   void* h_pin = nullptr;
   size_t h_pin_cap = 0;
@@ -666,19 +668,15 @@ int run_pipeline(tzr_ctx* ctx, Batch& bt, const tzr_params& p, cudaEvent_t* ev, 
   // unknown scale (Params default): TLS over the K TIM ratios first (registration.cc:603 -> :410-425)
   bt.scale_mode = p.estimate_scaling ? 1 : 0;
   if (bt.scale_mode) {
-    const size_t bytes = scale_scratch_bytes(bt.B, bt.n, ctx->flags);
-    if (!bytes) {
-      ctx->last_error = "estimate_scaling: 2K end points exceed 2^31";
-      return TZR_ERR_TOO_LARGE;
-    }
-    const int rc = ensure(ctx, ctx->sc, bytes);
+    const int rc = ensure(ctx, ctx->sc, scale_scratch_bytes(bt.B, bt.n, ctx->flags, ctx->scale_chunk));
     if (rc != TZR_OK) return rc;
   }
   cudaEventRecord(ev[0], sg);
   init_solutions_kernel<<<(bt.B + 127) / 128, 128, 0, sg>>>(bt.sol, bt.B);
   ctx->launches += 1;
   // before prep: the FP32 filter copies are pre-scaled by the estimate
-  if (bt.scale_mode) ctx->launches += launch_scale_estimation(bt, ctx->flags, ctx->sc.p, sg);
+  if (bt.scale_mode)
+    ctx->launches += launch_scale_estimation(bt, ctx->flags, ctx->scale_chunk, ctx->sc.p, &ctx->last_scale_chunks, sg);
   CK(launch_prep(bt, sg));
   ctx->launches += 1;
   cudaEventRecord(ev[1], sg);
@@ -741,6 +739,7 @@ int run_chunks(tzr_ctx* ctx, std::vector<Batch>& chunks, const std::vector<int>&
   }
   const bool lanes = n_chunks > 1 && ctx->gstream && ctx->hstream && lanes_ok;
   route.assign((size_t)bounds.back(), 0);
+  if (p.estimate_scaling) ctx->last_scale_chunks = 0;
   // debug counters cover the whole call: zeroed once, ahead of every chunk on either lane (not per chunk, which would
   // keep only the last chunk's counts)
   if (ctx->flags & 6u) CK(cudaMemsetAsync((void*)ctx->dbg.p, 0, 16 * sizeof(unsigned long long), ctx->stream));
@@ -953,12 +952,7 @@ int solve_ragged_dev(tzr_ctx* ctx, const tzr_params& p, int B, const int32_t* n,
       bounds.push_back(lo[c] + cb[k + 1]);
       if (p.estimate_scaling) {
         // sized here for every chunk at once: run_pipeline must not re-allocate it under an earlier chunk's kernels
-        const size_t bytes = scale_scratch_bytes(Bc, ns[c], ctx->flags);
-        if (!bytes) {
-          ctx->last_error = "estimate_scaling: 2K end points exceed 2^31";
-          return TZR_ERR_TOO_LARGE;
-        }
-        sc_bytes = std::max(sc_bytes, bytes);
+        sc_bytes = std::max(sc_bytes, scale_scratch_bytes(Bc, ns[c], ctx->flags, ctx->scale_chunk));
       }
     }
   }
@@ -1333,6 +1327,14 @@ int tzr_ctx_debug_counters(tzr_ctx* ctx, int64_t* out16) {
 }
 
 int tzr_ctx_last_strip_blocks(const tzr_ctx* ctx) { return ctx ? ctx->last_strip_blocks : 0; }
+
+int tzr_ctx_set_scale_chunk(tzr_ctx* ctx, long long max_end_points) {
+  if (!ctx || (max_end_points != 0 && max_end_points < 2048)) return TZR_ERR_INVALID_ARG;
+  ctx->scale_chunk = max_end_points;
+  return TZR_OK;
+}
+
+int tzr_ctx_last_scale_chunks(const tzr_ctx* ctx) { return ctx ? ctx->last_scale_chunks : 0; }
 
 int tzr_graph_strip_schedule(int nt, int L, int32_t* I, int32_t* J0) {
   if (nt < 1 || nt > kMaxNLarge / kTile || L < 1 || L > 15) return TZR_ERR_INVALID_ARG;
@@ -3662,7 +3664,7 @@ static int register_pairs_run(tzr_ctx* ctx, const tzr_frontend_params* fp, const
       registered.push_back(p);
       continue;
     }
-    const bool solve = cnt <= ctx->max_n && !(params->estimate_scaling && !scale_scratch_bytes(1, cnt, ctx->flags));
+    const bool solve = cnt <= ctx->max_n;
     status[p] = solve ? TZR_OK : TZR_ERR_TOO_LARGE;
     too_large |= !solve;
     const bool want_corr = corr && corr[p];

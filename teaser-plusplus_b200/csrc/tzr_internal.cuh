@@ -294,12 +294,15 @@ void launch_clique(const Batch& bt, const tzr_params& p, int mode, cudaStream_t 
 size_t tls_scratch_bytes(long long m, int count, bool large);
 int launch_scalar_tls(const double* x, const double* ranges, long long m, bool large, void* scratch, double* out_est,
                       uint8_t* inliers, cudaStream_t st);
-// Unknown-scale stage: TIM ratios, ranges and sort scratch of a batch (0: too large), and its launches.
-size_t scale_scratch_bytes(int B, int n, uint32_t flags);
+// Unknown-scale stage: scratch of a batch (bounded at every n <= kMaxNLarge), and its launches.  chunk: the context's
+// chunk capacity (tzr_ctx_set_scale_chunk; 0 automatic).  *chunks: raised to the largest chunk count of a problem on
+// the regenerating route.
+size_t scale_scratch_bytes(int B, int n, uint32_t flags, long long chunk);
 // Which of the two scale paths a problem of n correspondences takes (the large one above 256, or under debug flag 262144).
 // The paths differ in the last bits of the estimate, so a ragged size class never mixes them.
 bool scale_large(int n, uint32_t flags);
-int launch_scale_estimation(const Batch& bt, uint32_t flags, void* scratch, cudaStream_t st);
+int launch_scale_estimation(const Batch& bt, uint32_t flags, long long chunk, void* scratch, int* chunks,
+                            cudaStream_t st);
 void launch_rot_trans(const Batch& bt, const tzr_params& p, int use_clique, cudaStream_t st);
 // Large route (n > kMaxN or debug flag 524288; DESIGN.md §3.2).  lists: B * kHeurRoots * 2n u16 of heuristic scratch;
 // chg: B * kCoreSlots change counters (slot 0: peel this problem in the next block of rounds; slot r + 1: removals in

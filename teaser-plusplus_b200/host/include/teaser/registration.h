@@ -361,8 +361,8 @@ class RobustRegistrationSolver {
     uint64_t tuple_seed = 0x7ea5e2ull;
   };
   // One pair of solveCloudPairs.  status: 0 (TZR_OK) solved; TZR_ERR_TOO_LARGE (-6) a cloud with a point of more than
-  // 4096 neighbours (no correspondences), or more correspondences than one solve takes (65536, or 46340 with
-  // estimate_scaling; correspondences given, not solved); TZR_ERR_INVALID_ARG (-1) no correspondence.  An unsolved
+  // 4096 neighbours (no correspondences), or more correspondences than one solve takes (65536; correspondences
+  // given, not solved); TZR_ERR_INVALID_ARG (-1) no correspondence.  An unsolved
   // pair has an invalid solution and an empty clique.
   struct CloudPairResult {
     int status = 0;
